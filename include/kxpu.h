@@ -244,7 +244,11 @@ typedef struct kxpu_shard {
 } kxpu_shard;
 /* kxpu_pciids_join_sharded for all ranks of the group from ONE host thread: the kernels of every
  * rank are enqueued phase by phase, then all streams are awaited once.  tables_out[i] belongs to
- * kxpu_multi_ctx(m, i).  nq_total = 0: load only. */
+ * kxpu_multi_ctx(m, i).  nq_total = 0: load only.
+ * Limit: the ranks of a group exchange their winner rows through fixed peer slabs of 65 536 rows
+ * and 2 MiB of names per rank.  A text whose shard holds more winners (or more name bytes)
+ * fails with KXPU_E_CAPACITY ("winner rows outgrow the peer slab"); the group stays usable for
+ * smaller texts.  Load such a text with one context (kxpu_pciids_load_device) instead. */
 int32_t kxpu_multi_pciids_join(kxpu_multi *m, const kxpu_shard *shards /* [size] */, size_t nq_total,
                                kxpu_table **tables_out /* [size] */);
 

@@ -302,7 +302,8 @@ class Kxpu:
     def lookup_device(self, table, d_keys, n, d_rows):
         self._chk(self.L.kxpu_lookup_device(self.ctx, table.handle, d_keys, n, d_rows))
 
-    def names(self, table, rows):
+    def names_blob(self, table, rows):
+        """kxpu_names as it comes: (blob bytes, offs uint32[n+1]), name i = blob[offs[i]:offs[i+1]]."""
         rows = np.ascontiguousarray(rows, dtype=np.int32)
         offs = np.empty(len(rows) + 1, np.uint32)
         need = C.c_size_t(0)
@@ -312,8 +313,11 @@ class Kxpu:
         out = np.empty(max(need.value, 1), np.uint8)
         self._chk(self.L.kxpu_names(self.ctx, table.handle, _ptr(rows), len(rows), _ptr(out), need.value, _ptr(offs),
                                     C.byref(need)))
-        blob = out[:need.value].tobytes()
-        return [blob[offs[i]:offs[i + 1]] for i in range(len(rows))], blob, offs
+        return out[:need.value].tobytes(), offs
+
+    def names(self, table, rows):
+        blob, offs = self.names_blob(table, rows)
+        return [blob[offs[i]:offs[i + 1]] for i in range(len(offs) - 1)], blob, offs
 
     # -- the rest of the pci.ids model
     def full_load_device(self, d_text, n, table):

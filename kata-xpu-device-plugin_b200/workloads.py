@@ -20,7 +20,7 @@ def load_pci_ids() -> bytes:
 
 def make_queries(present_keys, n, seed, hit_frac=0.75):
     """cfg2/cfg4 key mix: hit_frac hits drawn uniformly from the present pairs, the rest
-    misses -- half with a present vendor and an absent device, half with an absent vendor."""
+    misses -- half with a present vendor and an absent device, half with an absent vendor (when one exists)."""
     rng = np.random.default_rng(seed)
     present_keys = np.asarray(present_keys, dtype=np.uint32)
     pset = set(int(k) for k in present_keys)
@@ -29,6 +29,8 @@ def make_queries(present_keys, n, seed, hit_frac=0.75):
     n_hit = int(round(n * hit_frac))
     n_m1 = (n - n_hit) // 2
     n_m2 = n - n_hit - n_m1
+    if len(vset) == 65536:  # every vendor id is present (a text of all 65 536 vendors): every miss has an absent device
+        n_m1, n_m2 = n - n_hit, 0
     hits = present_keys[rng.integers(0, len(present_keys), n_hit)]
     m1 = np.empty(n_m1, np.uint32)
     i = 0

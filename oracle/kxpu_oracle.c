@@ -232,6 +232,31 @@ size_t kxo_line_rest(const uint8_t *text, size_t n, uint64_t line_off, size_t *r
     return le - ls - 5;
 }
 
+/* Sanitised names of many rows at once: name i (the line at line_offs[i], as kxo_line_rest and
+ * kxo_sanitise give it) is blob[offs[i] .. offs[i+1]).  Returns the bytes all names need; names
+ * that do not fit in cap are not written, and offs (count + 1 entries) is always complete. */
+size_t kxo_names_bulk(const uint8_t *text, size_t n, const uint64_t *line_offs, size_t count, uint8_t *blob, size_t cap,
+                      uint32_t *offs) {
+    size_t total = 0, tmp_cap = 0;
+    uint8_t *tmp = NULL;
+    for (size_t i = 0; i < count; i++) {
+        offs[i] = (uint32_t)total;
+        size_t ro = 0;
+        const size_t rl = kxo_line_rest(text, n, line_offs[i], &ro);
+        if (rl + 1 > tmp_cap) {
+            free(tmp);
+            tmp_cap = rl + 1 > 4096 ? rl + 1 : 4096;
+            tmp = (uint8_t *)malloc(tmp_cap);
+        }
+        const size_t m = kxo_sanitise(text + ro, rl, tmp);
+        if (blob && total + m <= cap) memcpy(blob + total, tmp, m);
+        total += m;
+    }
+    offs[count] = (uint32_t)total;
+    free(tmp);
+    return total;
+}
+
 /* ------------------------------------------------------------------------- */
 /* createIommuDeviceMap (device_plugin.go:126-180) over a flat record table,   */
 /* + device-list build of createDevicePlugins (:91-98).                        */

@@ -62,6 +62,8 @@ def lib():
         L.kxo_table_build.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
         L.kxo_line_rest.restype = C.c_size_t
         L.kxo_line_rest.argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, C.POINTER(C.c_size_t)]
+        L.kxo_names_bulk.restype = C.c_size_t
+        L.kxo_names_bulk.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
         L.kxo_classify.restype = C.c_int32
         L.kxo_classify.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(ClassifyOut)]
         L.kxo_is_base60.restype = C.c_int
@@ -146,6 +148,23 @@ def row_name(text, line_off: int) -> bytes:
     ro = C.c_size_t(0)
     rl = lib().kxo_line_rest(p, n, line_off, C.byref(ro))
     return sanitise(bytes(keep[ro.value:ro.value + rl]))
+
+
+def names_bulk(text, line_offs):
+    """row_name of every line in line_offs, in one call: (blob bytes, offs uint32[count+1]) with
+    name i = blob[offs[i]:offs[i+1]] -- the layout kxpu_names returns."""
+    p, n, keep = _buf(text)
+    lo = np.ascontiguousarray(line_offs, dtype=np.uint64)
+    offs = np.empty(len(lo) + 1, np.uint32)
+    # a sanitised name is never longer than its line, so the text length bounds the names of distinct lines
+    cap = n
+    blob = np.empty(max(cap, 1), np.uint8)
+    need = lib().kxo_names_bulk(p, n, lo.ctypes.data, lo.size, blob.ctypes.data, cap, offs.ctypes.data)
+    if need > cap:
+        blob = np.empty(need, np.uint8)
+        lib().kxo_names_bulk(p, n, lo.ctypes.data, lo.size, blob.ctypes.data, need, offs.ctypes.data)
+    assert need < (1 << 32), "names of more than 4 GiB do not fit uint32 offsets"
+    return blob[:need].tobytes(), offs
 
 
 def classify(recs: np.ndarray):

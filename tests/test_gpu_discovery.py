@@ -71,6 +71,20 @@ def test_classify_sizes_and_degenerate(kx, oracle, workloads, oracle_rows):
     assert_classify_equal(kx.classify(recs), oracle.classify(recs))
     recs["iommu_group"] = np.arange(20000, dtype=np.uint32)[::-1]
     assert_classify_equal(kx.classify(recs), oracle.classify(recs))
+    # distinct 5-digit device ids, every record its own group: 200 000 ids cannot fit the 2^17 slots of the
+    # first device-id table (the run is repeated with a full-size one); 100 000 may or may not need the retry
+    for n in (200000, 100000):
+        recs = np.zeros(n, dtype=base.dtype)
+        recs["bdf"] = workloads.enumerate_bdfs(n).view("S16").reshape(n)
+        recs["vendor_txt"] = np.frombuffer(b"0x10de\n\0", np.uint8)
+        recs["device_txt"] = np.frombuffer(b"".join(b"0x%05x\n" % i for i in range(n)), np.uint8).reshape(n, 8)
+        recs["vendor_len"], recs["device_len"] = 7, 8
+        recs["driver"] = b"vfio-pci"
+        recs["iommu_group"] = np.arange(n, dtype=np.uint32)
+        res = kx.classify(recs)
+        assert res["n_devids"] == res["n_groups"] == n
+        assert_classify_equal(res, oracle.classify(recs))
+    assert 200000 > (1 << 17)
 
 
 def test_cfg3_one_million_devices(kx, oracle, workloads, oracle_rows):

@@ -36,7 +36,7 @@ def test_real_pci_ids_full_model(kx, oracle, pci_text):
     check_full(kx, oracle, pci_text)
 
 
-def test_full_model_first_occurrence_and_edges(kx, oracle, pci_text):
+def test_full_model_first_occurrence_and_edges(kx, oracle, pci_text, workloads):
     cut = pci_text.find(b"\n", 1400000) + 1
     check_full(kx, oracle, pci_text * 2)                         # every block twice: the first copy wins at every level
     check_full(kx, oracle, pci_text[700000:cut] + pci_text)      # later vendors first, class section twice
@@ -51,6 +51,16 @@ def test_full_model_first_occurrence_and_edges(kx, oracle, pci_text):
     big = b"abcd  Vendor\n\t0001  dev\n" + b"".join(b"\t\t%04x %04x  subsystem number %d\n" % (i >> 8, i & 0xffff, i) for i in range(9000))
     big += b"C ff  class\n\t01  sub\n" + b"".join(b"\t\t%02x  prog-if %d\n" % (i & 0xff, i) for i in range(400))
     check_full(kx, oracle, big)
+    # more subsystem rows than the first subsystem hash table (2^17 slots) and more prog-if rows than the first
+    # prog-if table (2^12 slots) hold: both are grown x4 and built again
+    text = workloads.synthetic_pci_ids(512, 64, subs_per_dev=8).tobytes()
+    classes = b"".join(b"C %02x  Class %d\n\t%02x  Subclass\n" % (c, c, c) + b"".join(b"\t\t%02x  Prog-if %d\n" % (p, p) for p in range(256))
+                       for c in range(20))
+    text += classes
+    assert len(oracle.full_build(text, 1)) == 262144 > (1 << 17)
+    progifs = oracle.full_build(text, 2)
+    assert int(((progifs["key"] >> np.uint64(24)) == 3).sum()) == 5120 > (1 << 12)
+    check_full(kx, oracle, text)
 
 
 def test_full_model_fuzz(kx, oracle):

@@ -357,10 +357,24 @@ def test_every_range_length(rch, oracle, pci_text, monkeypatch):
         k.close()
 
 
-def test_name_lengths_around_the_finalize_windows(kx, oracle):
+@pytest.mark.parametrize("scan_w", ["auto", "8", "16", "32"])
+def test_name_lengths_around_the_finalize_windows(scan_w, kx, oracle, monkeypatch):
     """The finalize looks at a 128-byte window per row (fast path), stages up to ~1 KB for longer lines
     (warp path) and reads even longer ones serially: names of every length around those limits, at
-    every 16-byte phase of the line start, with trailing CR / blanks / non-ASCII bytes."""
+    every 16-byte phase of the line start, with trailing CR / blanks / non-ASCII bytes.  Also with every
+    number of table slots a finalize warp scans per step (KXPU_SCAN_W, fresh context)."""
+    if scan_w != "auto":
+        import kxpu_b200 as K
+        monkeypatch.setenv("KXPU_SCAN_W", scan_w)
+        kx = K.Kxpu(0)
+    try:
+        _check_name_lengths(kx, oracle)
+    finally:
+        if scan_w != "auto":
+            kx.close()
+
+
+def _check_name_lengths(kx, oracle):
     rng = np.random.default_rng(3)
     alphabet = np.frombuffer(b"abcXYZ019 /._-[]()\t", np.uint8)
     parts, keys = [b"1234  Vendor\n"], []
@@ -447,11 +461,15 @@ def test_zero_copy_join_from_pinned_host_buffers(kx, oracle, pci_text, oracle_ro
                 kx.pinned_free(p)
 
 
-def test_small_texts_through_the_big_text_kernels(oracle, pci_text, monkeypatch):
+@pytest.mark.parametrize("scan_w", ["auto", "8", "16", "32"])
+def test_small_texts_through_the_big_text_kernels(scan_w, oracle, pci_text, monkeypatch):
     """Small texts normally take the cooperative one-launch kernel; KXPU_NO_SMALL=1 sends them through
-    parse_kernel_v5 + resolve + select_finalize, which must agree (ragged sizes, edge texts, real file)."""
+    parse_kernel_v5 + resolve + select_finalize, which must agree (ragged sizes, edge texts, real file),
+    with every number of table slots a finalize warp scans per step (KXPU_SCAN_W)."""
     import kxpu_b200 as K
     monkeypatch.setenv("KXPU_NO_SMALL", "1")
+    if scan_w != "auto":
+        monkeypatch.setenv("KXPU_SCAN_W", scan_w)
     k = K.Kxpu(0)
     try:
         check_text(k, oracle, pci_text)

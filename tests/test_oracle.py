@@ -40,6 +40,29 @@ def test_spot_values(oracle, pci_text, golden):
     assert oracle.device_name(pci_text, 0x10de2901) == (-1, None)
 
 
+def test_names_bulk_equals_row_name(oracle, pci_text, oracle_rows):
+    """names_bulk (one call for all rows, the checker of the large-table GPU tests) == row_name for every
+    row of the real file, and == the Python sanitiser on a sample; edge lines too."""
+    offs_in = oracle_rows["line_off"]
+    blob, offs = oracle.names_bulk(pci_text, offs_in)
+    assert len(offs) == len(offs_in) + 1 and offs[0] == 0 and offs[-1] == len(blob)
+    for i, o in enumerate(offs_in.tolist()):
+        assert blob[offs[i]:offs[i + 1]] == oracle.row_name(pci_text, o), i
+    rng = np.random.default_rng(5)
+    for i in rng.choice(len(offs_in), 300, replace=False).tolist():
+        o = int(offs_in[i])
+        line = pci_text[o:pci_text.index(b"\n", o)].removesuffix(b"\r")
+        assert blob[offs[i]:offs[i + 1]] == pyref.sanitise(line[5:])
+    # short, empty, CRLF and unterminated lines; the same line twice; no lines at all
+    text = b"10de  V\n\t0001\n\t0002  a b\r\n\t00\n\t0003  \xc4\xb1x/y"
+    lo = np.array([8, 14, 26, 8, 30, 14], np.uint64)
+    blob, offs = oracle.names_bulk(text, lo)
+    assert [blob[offs[i]:offs[i + 1]] for i in range(len(lo))] == [oracle.row_name(text, int(o)) for o in lo]
+    assert [blob[offs[i]:offs[i + 1]] for i in range(len(lo))] == [b"", b"A_B", b"", b"", b"IX_Y", b"A_B"]
+    blob, offs = oracle.names_bulk(text, np.empty(0, np.uint64))
+    assert blob == b"" and offs.tolist() == [0]
+
+
 def test_literal_scan_equals_single_pass_table(oracle, pci_text, oracle_rows):
     """Every key of the one-pass table resolves, by the literal getDeviceName scan, to the
     same line; sampled (the literal scan is O(file) per key)."""

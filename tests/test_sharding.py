@@ -132,11 +132,15 @@ def _aligned_upload(kx, data):
     return d
 
 
-def _check_multi(oracle, text, nranks, q=None, ordinals=None):
-    """Sharded load (+ join) of `text` over `nranks` contexts of one process == oracle on the whole text."""
+def _check_multi(oracle, text, nranks, q=None, ordinals=None, m=None):
+    """Sharded load (+ join) of `text` over `nranks` contexts of one process == oracle on the whole text.
+    With `m`, the load runs on that existing group, which stays open."""
     import kxpu_b200 as K
     want = oracle.table_build(text)
-    m = K.KxpuMulti(ordinals or [0] * nranks)
+    own = m is None
+    if own:
+        m = K.KxpuMulti(ordinals or [0] * nranks)
+    assert len(m) == nranks
     bufs = []
     try:
         for rep in range(3):  # both exchange buffers and their clearing one epoch ahead
@@ -187,7 +191,10 @@ def _check_multi(oracle, text, nranks, q=None, ordinals=None):
                 kx.dev_free(d)
             bufs = []
     finally:
-        m.close()
+        for kx, d in bufs:
+            kx.dev_free(d)
+        if own:
+            m.close()
 
 
 @pytest.mark.gpu
@@ -207,10 +214,15 @@ def test_sharded_load_and_join_on_one_gpu(nranks, oracle, pci_text, workloads, o
     _check_multi(oracle, b"\tonly\n\tdevice lines\n", nranks)
 
 
+def _short_name_text(n_vendors, devs):
+    return b"".join(b"%04x  V\n" % v + b"".join(b"\t%04x  d\n" % d for d in range(devs)) for v in range(0x100, 0x100 + n_vendors))
+
+
 @pytest.mark.gpu
-def test_sharded_too_long_line_and_growth(oracle):
+def test_sharded_too_long_line_and_growth(oracle, pci_text, workloads, oracle_rows):
     """A >= 64 KiB line in one shard cuts every later shard off (bufio.ErrTooLong, global minimum of
-    the shards' cut-offs); a text with more keys than the default table grows on every rank alike."""
+    the shards' cut-offs); a text with more keys than the default table grows on every rank alike, up to
+    the limit of the peer slabs."""
     head = b"1111  one\n\t0001  a\n2222  two\n\t0002  b\n"
     long_line = b"3333  " + b"x" * 70000 + b"\n\t0003  hidden\n"
     tail = b"4444  four\n\t0004  also hidden\n" * 50
@@ -219,6 +231,34 @@ def test_sharded_too_long_line_and_growth(oracle):
         _check_multi(oracle, head * 200 + long_line + tail, nr, q)
     big = b"".join(b"%04x  V\n" % v + b"".join(b"\t%04x  d%d\n" % (d, d) for d in range(0, 2500, 7)) for v in range(0x100, 0x100 + 140))
     _check_multi(oracle, big, 3, np.array([0x01000000, 0x01010007, 0x018b09bd, 0x01000001], np.uint32))
+    # 4 ranks with ~60 k winners each (under the 65 536 rows / 2 MiB names of a rank's peer slab): the merged
+    # table needs >= 2^19 slots.  A text with ~80 k winners per rank outgrows the slab: KXPU_E_CAPACITY.  The
+    # same group loads pci.ids correctly after each (its table size only ever grows)
+    import kxpu_b200 as K
+    from kxpu_b200.binding import E_CAPACITY
+    def winners_per_rank(text):
+        lines = oracle.table_build(text)["line_off"]
+        return [int(((lines >= a) & (lines < b)).sum()) for a, b in K.plan_shards(text, 4)]
+
+    m = K.KxpuMulti([0] * 4)
+    try:
+        text = _short_name_text(1200, 200)
+        want = oracle.table_build(text)
+        assert len(want) == 240000 > (1 << 18) - (1 << 15)  # a merged table of 2^18 slots takes 7/8 of them
+        per_rank = winners_per_rank(text)
+        assert max(per_rank) < 65536 and min(per_rank) > 50000, per_rank
+        _check_multi(oracle, text, 4, workloads.make_queries(want["key"], 20000, 23), m=m)
+        q = workloads.make_queries(oracle_rows["key"], 5000, 29)
+        _check_multi(oracle, pci_text, 4, q, m=m)
+        over = _short_name_text(1600, 200)
+        per_rank = winners_per_rank(over)
+        assert min(per_rank) > 65536, per_rank
+        with pytest.raises(K.KxpuError) as e:
+            _check_multi(oracle, over, 4, m=m)
+        assert e.value.status == E_CAPACITY and "winner rows outgrow the peer slab" in str(e.value)
+        _check_multi(oracle, pci_text, 4, q, m=m)
+    finally:
+        m.close()
 
 
 @pytest.mark.gpu
