@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 2
+#define KXPU_ABI_VERSION 3
 
 /* status codes */
 #define KXPU_OK             0
@@ -299,6 +299,36 @@ typedef struct kxpu_classify_out {
  * createDevicePlugins (device_plugin.go:91-98) over a flat record table. */
 int32_t kxpu_classify(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out);
 
+/* One accepted (vendor, driver) pair of kxpu_classify_rules.  32 bytes. */
+typedef struct kxpu_xpu_rule {
+    char     vendor[8];    /* vendor id exactly as readIDFromFile returns it (data[2:], '\n' trimmed), e.g. "1002"; NUL padded */
+    char     driver[16];   /* basename of the driver link, e.g. "vfio-pci"; NUL padded */
+    uint32_t reserved[2];
+} kxpu_xpu_rule;
+#define KXPU_MAX_RULES 16
+
+/* kxpu_classify for accelerators of any configured vendor (the reference's README TODO "To support other
+ * GPUs", README.md:34-39).  The walk is createIommuDeviceMap's (device_plugin.go:126-180) with the two
+ * NVIDIA constants replaced by a rule list:
+ *   - a record is a candidate iff the conditions of :137-161 hold for some rule r, where the `10de` test
+ *     of :149 reads "read_id(vendor) equals rules[r].vendor byte for byte, length included" and the
+ *     `vfio-pci` test of :156 reads "driver equals rules[r].driver".  Rules are pairwise distinct, so at
+ *     most one rule matches a record;
+ *   - ONE walk and ONE busIndex counter (:130, :171-175) over all rules: accept_index, group_ids,
+ *     group_off and group_members mean what they mean for kxpu_classify;
+ *   - a group belongs to its FIRST member (:162-170) and to that member's rule; the members of one group
+ *     may match different rules;
+ *   - the key of a deviceMap entry (:169) is (rule of the group's first member, device id): one device
+ *     id under two vendors gives two entries.  dev_ids keeps its meaning, dev_rule[d] (caller array of
+ *     n entries, may be NULL) receives the rule index of entry d.
+ * Invalid rule lists return KXPU_E_INVALID: n_rules is 0 or more than KXPU_MAX_RULES; a vendor is empty,
+ * longer than 6 bytes (the longest id a record can carry after data[2:]), contains '\n' or has a
+ * non-NUL byte after its first NUL; a driver is empty, 16 bytes or longer, contains '/' or has a non-NUL
+ * byte after its first NUL; two rules are the same (vendor, driver) pair.
+ * With rules = {{"10de", "vfio-pci"}} every array equals kxpu_classify's and dev_rule is all 0. */
+int32_t kxpu_classify_rules(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs,
+                            size_t n, kxpu_classify_out *out, uint8_t *dev_rule /* [n] */);
+
 /* ------------------------------------------------------- S3: CDI spec emit */
 
 /* One accepted device as generateCDISpec sees it (device_plugin.go:59-76). 32 bytes. */
@@ -318,12 +348,34 @@ typedef struct kxpu_cdidev {
 int32_t kxpu_cdi_emit(kxpu_ctx *ctx, int32_t format, const kxpu_cdidev *devs, size_t n,
                       uint8_t *out, size_t cap, size_t *len);
 
+/* kxpu_cdi_emit with the CDI kind as an argument: `kind` replaces "nvidia.com/gpu" (CdiVendorClass,
+ * generic_device_plugin.go:31) in the `kind:` field (device_plugin.go:78), in the cdi.k8s.io/vfio<g>
+ * annotation value (:66) and, for kind = "nvidia.com/gpu", the bytes equal kxpu_cdi_emit's.
+ * Supported domain (else KXPU_E_UNSUPPORTED): a NUL-terminated "vendor/class" of at most 63 bytes;
+ * vendor = a letter, then [A-Za-z0-9_.-], ending in a letter or digit; class = a letter, then
+ * [A-Za-z0-9_-], ending in a letter or digit.  This is a subset of what the CDI v0.8.0 pkg/parser
+ * vendor / class rules accept.  Inside it the kind is always written as it is:
+ *   - YAML: it starts with a letter and contains '/', so yaml.v3's resolve cannot read it as an int,
+ *     float, bool, null or timestamp, and neither isBase60Float nor isOldBool matches it (both need a
+ *     leading digit / sign or a whole-word boolean); no character of it is an indicator that forces
+ *     quoting in a plain scalar.  "kind=<index>" stays plain for the same reasons.
+ *   - JSON: it holds no '"', '\\', control byte, '<', '>' or '&', so encoding/json escapes nothing.
+ * Kinds up to 22 bytes run on the same kernel configuration as kxpu_cdi_emit; longer ones on a variant
+ * with a larger per-device fragment bound (fewer CTAs per SM, DESIGN.md K6). */
+int32_t kxpu_cdi_emit_kind(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_cdidev *devs, size_t n,
+                           uint8_t *out, size_t cap, size_t *len);
+
 /* ------------------------------------------------------ S5: Allocate names */
 
 /* updateResponseForCDI / QualifiedName (generic_device_plugin.go:274-299,
  * cdi/cdi-utils.go:9): name i = "nvidia.com/gpu=" + decimal(idx[i]). */
 int32_t kxpu_alloc_names(kxpu_ctx *ctx, const uint64_t *idx, size_t n, uint8_t *out,
                          size_t cap, uint32_t *offsets, size_t *need);
+/* The same with the CDI kind as an argument (QualifiedName(vendor, class, idx), cdi-utils.go:9):
+ * name i = kind + "=" + decimal(idx[i]).  `kind` has kxpu_cdi_emit_kind's domain (else
+ * KXPU_E_UNSUPPORTED); kind = "nvidia.com/gpu" gives kxpu_alloc_names' bytes. */
+int32_t kxpu_alloc_names_kind(kxpu_ctx *ctx, const char *kind, const uint64_t *idx, size_t n, uint8_t *out,
+                              size_t cap, uint32_t *offsets, size_t *need);
 
 /* ListAndWatchResponse wire bytes for a device list (generic_device_plugin.go:224):
  * repeated field 1 { string ID = 1 (decimal group); string health = 2 }.

@@ -179,3 +179,92 @@ func (k *kxpu) allocNames(idx []uint64) ([]string, error) {
 	}
 	return out, err
 }
+
+// ---- accelerators of any configured vendor (README TODO "To support other GPUs")
+
+// xpuClass is one accelerator class the plugin serves: the constants nvidiaVendorID (device_plugin.go:19),
+// "vfio-pci" (:156), DevicePluginNamespace / CdiVendorClass (generic_device_plugin.go:26,31) and the CDI file
+// stem (device_plugin.go:79) become fields.  The default list is {"10de", "vfio-pci", "nvidia.com",
+// "nvidia.com/gpu", "cdi-vfio-xxxx"}.
+type xpuClass struct {
+	Vendor, Driver, Namespace, Kind, FileStem string
+}
+
+// S1 with a class list: one rule per class (rule index == class index).  devRule[d] is the class of deviceMap
+// entry d; the same device id can appear under two classes.
+func (k *kxpu) classifyRules(classes []xpuClass, recs []C.kxpu_devrec) (accept, gids, goff, gmem []uint32, dids []uint64,
+	doff, dgrp []uint32, devRule []uint8, err error) {
+	n := len(recs)
+	accept, gids, goff, gmem = make([]uint32, n), make([]uint32, n), make([]uint32, n+1), make([]uint32, n)
+	dids, doff, dgrp, devRule = make([]uint64, n), make([]uint32, n+1), make([]uint32, n), make([]uint8, n)
+	if n == 0 {
+		return
+	}
+	rules := make([]C.kxpu_xpu_rule, len(classes))
+	for i, c := range classes {
+		for j := 0; j < len(c.Vendor) && j < len(rules[i].vendor); j++ {
+			rules[i].vendor[j] = C.char(c.Vendor[j])
+		}
+		for j := 0; j < len(c.Driver) && j < len(rules[i].driver); j++ {
+			rules[i].driver[j] = C.char(c.Driver[j])
+		}
+	}
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, p := range []*uint32{&accept[0], &gids[0], &goff[0], &gmem[0], &doff[0], &dgrp[0]} {
+		pin.Pin(p)
+	}
+	pin.Pin(&dids[0])
+	var out C.kxpu_classify_out
+	out.accept_index = (*C.uint32_t)(unsafe.Pointer(&accept[0]))
+	out.group_ids = (*C.uint32_t)(unsafe.Pointer(&gids[0]))
+	out.group_off = (*C.uint32_t)(unsafe.Pointer(&goff[0]))
+	out.group_members = (*C.uint32_t)(unsafe.Pointer(&gmem[0]))
+	out.dev_ids = (*C.uint64_t)(unsafe.Pointer(&dids[0]))
+	out.dev_off = (*C.uint32_t)(unsafe.Pointer(&doff[0]))
+	out.dev_groups = (*C.uint32_t)(unsafe.Pointer(&dgrp[0]))
+	var rp *C.kxpu_xpu_rule
+	if len(rules) > 0 {
+		rp = &rules[0]
+	}
+	err = kxCheck(k.ctx, "kxpu_classify_rules", C.kxpu_classify_rules(k.ctx, rp, C.size_t(len(rules)), &recs[0], C.size_t(n), &out,
+		(*C.uint8_t)(unsafe.Pointer(&devRule[0]))))
+	gids, goff, gmem = gids[:out.n_groups], goff[:out.n_groups+1], gmem[:out.n_accepted]
+	dids, doff, dgrp, devRule = dids[:out.n_devids], doff[:out.n_devids+1], dgrp[:out.n_groups], devRule[:out.n_devids]
+	return
+}
+
+// S3 for one class: the CDI document of that class's devices with its kind.
+func (k *kxpu) cdiEmitKind(format int, kind string, devs []C.kxpu_cdidev) ([]byte, error) {
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	var p *C.kxpu_cdidev
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	var n C.size_t
+	C.kxpu_cdi_emit_kind(k.ctx, C.int32_t(format), ck, p, C.size_t(len(devs)), nil, 0, &n) // sizing call
+	buf := make([]byte, n+1)
+	err := kxCheck(k.ctx, "kxpu_cdi_emit_kind", C.kxpu_cdi_emit_kind(k.ctx, C.int32_t(format), ck, p, C.size_t(len(devs)),
+		(*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n))
+	return buf[:n], err
+}
+
+// S5 for one class: "<kind>=<index>" names of an Allocate response.
+func (k *kxpu) allocNamesKind(kind string, idx []uint64) ([]string, error) {
+	if len(idx) == 0 {
+		return nil, nil
+	}
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	offs := make([]C.uint32_t, len(idx)+1)
+	buf := make([]byte, (len(kind)+22)*len(idx))
+	var need C.size_t
+	err := kxCheck(k.ctx, "kxpu_alloc_names_kind", C.kxpu_alloc_names_kind(k.ctx, ck, (*C.uint64_t)(unsafe.Pointer(&idx[0])),
+		C.size_t(len(idx)), (*C.uint8_t)(unsafe.Pointer(&buf[0])), C.size_t(len(buf)), &offs[0], &need))
+	out := make([]string, len(idx))
+	for i := range idx {
+		out[i] = string(buf[offs[i]:offs[i+1]])
+	}
+	return out, err
+}

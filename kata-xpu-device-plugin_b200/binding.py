@@ -25,7 +25,9 @@ DEVREC_DTYPE = np.dtype([("bdf", "S16"), ("vendor_txt", "u1", (8,)), ("device_tx
                          ("device_len", "u1"), ("flags", "u1"), ("reserved0", "u1"),
                          ("reserved1", "<u4", (2,))])
 CDIDEV_DTYPE = np.dtype([("bdf", "S16"), ("iommu_group", "<u4"), ("reserved", "<u4"), ("index", "<u8")])
-assert DEVREC_DTYPE.itemsize == 64 and CDIDEV_DTYPE.itemsize == 32
+RULE_DTYPE = np.dtype([("vendor", "S8"), ("driver", "S16"), ("reserved", "<u4", (2,))])  # kxpu_xpu_rule
+assert DEVREC_DTYPE.itemsize == 64 and CDIDEV_DTYPE.itemsize == 32 and RULE_DTYPE.itemsize == 32
+MAX_RULES = 16
 
 # every symbol include/kxpu.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -36,7 +38,8 @@ ABI_SYMBOLS = [
     "kxpu_lookup_device", "kxpu_pciids_join_device", "kxpu_pciids_join", "kxpu_names", "kxpu_comm_unique_id", "kxpu_comm_init", "kxpu_comm_destroy",
     "kxpu_pciids_load_sharded", "kxpu_pciids_join_sharded", "kxpu_plan_shards", "kxpu_ctx_create_multi", "kxpu_multi_destroy",
     "kxpu_multi_size", "kxpu_multi_ctx", "kxpu_multi_pciids_join", "kxpu_classify", "kxpu_cdi_emit", "kxpu_alloc_names",
-    "kxpu_lw_encode", "kxpu_pciids_full_load_device", "kxpu_full_free", "kxpu_full_export", "kxpu_full_lookup",
+    "kxpu_lw_encode", "kxpu_classify_rules", "kxpu_cdi_emit_kind", "kxpu_alloc_names_kind",
+    "kxpu_pciids_full_load_device", "kxpu_full_free", "kxpu_full_export", "kxpu_full_lookup",
 ]
 
 
@@ -117,6 +120,9 @@ def load_library():
         "kxpu_classify": (i32, [vp, vp, sz, C.POINTER(ClassifyOut)]),
         "kxpu_cdi_emit": (i32, [vp, i32, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_alloc_names": (i32, [vp, vp, sz, vp, sz, vp, C.POINTER(sz)]),
+        "kxpu_classify_rules": (i32, [vp, vp, sz, vp, sz, C.POINTER(ClassifyOut), vp]),
+        "kxpu_cdi_emit_kind": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_alloc_names_kind": (i32, [vp, C.c_char_p, vp, sz, vp, sz, vp, C.POINTER(sz)]),
         "kxpu_lw_encode": (i32, [vp, vp, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_pciids_full_load_device": (i32, [vp, vp, sz, vp, C.POINTER(vp)]),
         "kxpu_full_free": (i32, [vp, vp]),
@@ -132,6 +138,21 @@ def load_library():
 
 def _ptr(a):
     return None if a is None else a.ctypes.data
+
+
+def _kind(kind):
+    return kind.encode() if isinstance(kind, str) else kind
+
+
+def rules_array(rules):
+    """[(vendor, driver)] (bytes or str) -> RULE_DTYPE array for kxpu_classify_rules; an array passes through."""
+    if isinstance(rules, np.ndarray):
+        assert rules.dtype == RULE_DTYPE
+        return np.ascontiguousarray(rules)
+    a = np.zeros(len(rules), RULE_DTYPE)
+    for i, (v, d) in enumerate(rules):
+        a[i]["vendor"], a[i]["driver"] = _kind(v), _kind(d)
+    return a
 
 
 class Table:
@@ -373,34 +394,71 @@ class Kxpu:
                     group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
                     dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g])
 
-    def cdi_emit(self, fmt, devs):
+    def classify_rules(self, rules, recs):
+        """kxpu_classify_rules: rules is a RULE_DTYPE array or [(vendor bytes, driver bytes)]; classify's dict plus
+        dev_rule (rule index of every device-map entry)."""
+        ra = rules_array(rules)
+        recs = np.ascontiguousarray(recs)
+        assert recs.dtype == DEVREC_DTYPE
+        n = len(recs)
+        arrs = dict(accept_index=np.empty(n, np.uint32), group_ids=np.empty(n, np.uint32),
+                    group_off=np.empty(n + 1, np.uint32), group_members=np.empty(n, np.uint32),
+                    dev_ids=np.empty(n, np.uint64), dev_off=np.empty(n + 1, np.uint32),
+                    dev_groups=np.empty(n, np.uint32))
+        dev_rule = np.empty(max(n, 1), np.uint8)
+        out = ClassifyOut(**{k: v.ctypes.data for k, v in arrs.items()})
+        self._chk(self.L.kxpu_classify_rules(self.ctx, _ptr(ra) if len(ra) else None, len(ra), _ptr(recs) if n else None, n,
+                                             C.byref(out), _ptr(dev_rule)))
+        g, d, a = out.n_groups, out.n_devids, out.n_accepted
+        return dict(accept_index=arrs["accept_index"], n_accepted=a, n_groups=g, n_devids=d,
+                    group_ids=arrs["group_ids"][:g], group_off=arrs["group_off"][:g + 1],
+                    group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
+                    dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g], dev_rule=dev_rule[:d])
+
+    def cdi_emit(self, fmt, devs, kind=None):
+        """kind=None: kxpu_cdi_emit (kind nvidia.com/gpu); else kxpu_cdi_emit_kind with that CDI kind (bytes or str)."""
         devs = np.ascontiguousarray(devs)
         assert devs.dtype == CDIDEV_DTYPE
-        # one call with a buffer no document can outgrow (<= 384 B per device); the two-call sizing
-        # protocol (out = NULL -> *len) remains available and is exercised by the tests
-        cap = 400 * len(devs) + 1024
+        # one call with a buffer no document can outgrow (<= 384 B per device, plus the kind's bytes beyond 14); the
+        # two-call sizing protocol (out = NULL -> *len) remains available and is exercised by the tests
+        kb = _kind(kind)
+        cap = (400 + (len(kb) if kb else 0)) * len(devs) + 1024
         out = np.empty(cap, np.uint8)
         got = C.c_size_t(0)
-        self._chk(self.L.kxpu_cdi_emit(self.ctx, fmt, _ptr(devs) if len(devs) else None, len(devs), _ptr(out), cap,
-                                       C.byref(got)))
+        dp = _ptr(devs) if len(devs) else None
+        if kb is None:
+            self._chk(self.L.kxpu_cdi_emit(self.ctx, fmt, dp, len(devs), _ptr(out), cap, C.byref(got)))
+        else:
+            self._chk(self.L.kxpu_cdi_emit_kind(self.ctx, fmt, kb, dp, len(devs), _ptr(out), cap, C.byref(got)))
         return out[:got.value].tobytes()
 
-    def cdi_emit_len(self, fmt, devs):
+    def cdi_emit_len(self, fmt, devs, kind=None):
         """Sizing call of the two-call protocol: out = NULL, returns the required length."""
         devs = np.ascontiguousarray(devs)
         need = C.c_size_t(0)
-        rc = self.L.kxpu_cdi_emit(self.ctx, fmt, _ptr(devs) if len(devs) else None, len(devs), None, 0, C.byref(need))
+        kb = _kind(kind)
+        dp = _ptr(devs) if len(devs) else None
+        if kb is None:
+            rc = self.L.kxpu_cdi_emit(self.ctx, fmt, dp, len(devs), None, 0, C.byref(need))
+        else:
+            rc = self.L.kxpu_cdi_emit_kind(self.ctx, fmt, kb, dp, len(devs), None, 0, C.byref(need))
         if rc not in (KXPU_OK, E_NOSPACE):
             self._chk(rc)
         return need.value
 
-    def alloc_names(self, idx):
+    def alloc_names(self, idx, kind=None):
+        """kind=None: kxpu_alloc_names ("nvidia.com/gpu=<idx>"); else kxpu_alloc_names_kind ("<kind>=<idx>")."""
         idx = np.ascontiguousarray(idx, dtype=np.uint64)
         offs = np.empty(len(idx) + 1, np.uint32)
         need = C.c_size_t(0)
-        cap = 36 * len(idx) + 16
+        kb = _kind(kind)
+        cap = (22 + (len(kb) if kb else 14)) * len(idx) + 16
         out = np.empty(cap, np.uint8)
-        self._chk(self.L.kxpu_alloc_names(self.ctx, _ptr(idx), len(idx), _ptr(out), cap, _ptr(offs), C.byref(need)))
+        if kb is None:
+            self._chk(self.L.kxpu_alloc_names(self.ctx, _ptr(idx), len(idx), _ptr(out), cap, _ptr(offs), C.byref(need)))
+        else:
+            self._chk(self.L.kxpu_alloc_names_kind(self.ctx, kb, _ptr(idx), len(idx), _ptr(out), cap, _ptr(offs),
+                                                   C.byref(need)))
         return out[:need.value].tobytes(), offs
 
     def lw_encode(self, groups, healthy=None):

@@ -4,6 +4,8 @@
 // :91-98 (per-device-id group lists).  The sequential walk is restated as data-parallel
 // primitives whose results equal the walk's:
 //   candidate(i)  = !dir && vendor=="10de" && driver=="vfio-pci" && links readable   (:137-161)
+//                   (kxpu_classify_rules: (vendor, driver) equals the pair of some rule r; the device-id key
+//                   below becomes (rule of the group's first member, device id))
 //   gfirst[g]     = min{ i : candidate(i), group(i)=g, device file readable }        (:162-170:
 //                   a group only comes into existence at a record whose device read works)
 //   accept(i)     = candidate(i) && gfirst[group(i)] <= i                            (:171-175)
@@ -52,7 +54,19 @@ struct Work {
     // outputs (device)
     uint32_t *accept_index, *group_ids, *group_off, *dev_off;
     unsigned long long *dev_ids;
+    // kxpu_classify_rules only (NULL otherwise): rule of record i, rule of device-map entry d
+    uint8_t *rrule, *dev_rule;
 };
+
+// The rule list of kxpu_classify_rules as k_candidates compares it: per rule the vendor id bytes with the id
+// length in bits 56-63 (the same packing as read_id's result), and the driver as two 64-bit words with
+// masks that cover its bytes and the NUL behind it (strncmp over the 16-byte field).
+struct RuleTable {
+    unsigned long long vend[KXPU_MAX_RULES], d0[KXPU_MAX_RULES], d1[KXPU_MAX_RULES], m0[KXPU_MAX_RULES], m1[KXPU_MAX_RULES];
+    uint32_t n;
+};
+// the device-id key carries the rule in bits 48-63: an id is at most 6 bytes after data[2:]
+constexpr unsigned long long DEVID_MASK = 0x0000FFFFFFFFFFFFull;
 
 // readIDFromFileFunc (device_plugin.go:183-191): data[2:] with '\n' trimmed at both ends.
 // Returns false when the file is shorter than 2 bytes (the reference would panic) or longer
@@ -104,8 +118,10 @@ __device__ __forceinline__ uint32_t dinsert(const Work &W, unsigned long long ke
     return 0u;
 }
 
-// pass 1: candidates, group table, gfirst
-__global__ void __launch_bounds__(256) k_candidates(const Work W) {
+// pass 1: candidates, group table, gfirst.  RULES: the (vendor, driver) pair is matched against the rule list of
+// kxpu_classify_rules and the matching rule is stored per record for k_groups; otherwise the NVIDIA constants.
+template <bool RULES>
+__device__ __forceinline__ void candidates(const Work &W, const RuleTable &R) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= W.n) return;
     // one 64-byte record per thread: three 16-byte vector loads (the bdf is not needed to classify)
@@ -120,9 +136,24 @@ __global__ void __launch_bounds__(256) k_candidates(const Work W) {
     unsigned long long vid, did;
     uint32_t vl, dl;
     bool vok = read_id(vtxt, vlen, vid, vl);
-    bool cand = !(fl & KXPU_REC_IS_DIR) && !(fl & KXPU_REC_VENDOR_ERR) && vok && vl == 4u &&
-                vid == 0x65643031ull /* "10de" */ && !(fl & KXPU_REC_DRIVER_ERR) &&
-                drv0 == 0x6963702d6f696676ull /* "vfio-pci" */ && drv8 == 0u && !(fl & KXPU_REC_IOMMU_ERR);
+    bool match;
+    uint32_t rule = 0;
+    if (RULES) {
+        const unsigned long long vkey = vid | ((unsigned long long)vl << 56);
+        const unsigned long long drv1 = ((unsigned long long)q2.w << 32) | q2.z;  // driver[8..16)
+        match = false;
+#pragma unroll
+        for (uint32_t r = 0; r < KXPU_MAX_RULES; r++) {  // constant indices: the table stays in the parameter bank
+            if (r < R.n && vkey == R.vend[r] && (drv0 & R.m0[r]) == R.d0[r] && (drv1 & R.m1[r]) == R.d1[r]) {
+                match = true;
+                rule = r;
+            }
+        }
+    } else {
+        match = vl == 4u && vid == 0x65643031ull /* "10de" */ && drv0 == 0x6963702d6f696676ull /* "vfio-pci" */ && drv8 == 0u;
+    }
+    bool cand = !(fl & KXPU_REC_IS_DIR) && !(fl & KXPU_REC_VENDOR_ERR) && vok && match && !(fl & KXPU_REC_DRIVER_ERR) &&
+                !(fl & KXPU_REC_IOMMU_ERR);
     bool dok = !(fl & KXPU_REC_DEVICE_ERR) && read_id(dtxt, dlen, did, dl);
     if (!(fl & (KXPU_REC_IS_DIR | KXPU_REC_VENDOR_ERR)) && vlen > 8u) atomicOr(&W.totals[3], 1u);
     if (cand && (group == EMPTY32 || (dok && did == EMPTY64) || (!(fl & KXPU_REC_DEVICE_ERR) && dlen > 8u)))
@@ -133,6 +164,11 @@ __global__ void __launch_bounds__(256) k_candidates(const Work W) {
         if (dok && i < __ldcg(&W.gtab[slot].first)) atomicMin(&W.gtab[slot].first, i);
     }
     W.gslot[i] = slot;
+    if (RULES) W.rrule[i] = (uint8_t)rule;
+}
+__global__ void __launch_bounds__(256) k_candidates(const Work W) { candidates<false>(W, RuleTable{}); }
+__global__ void __launch_bounds__(256) k_candidates_rules(const Work W, const __grid_constant__ RuleTable R) {
+    candidates<true>(W, R);
 }
 
 // pass 2: accept / group-first flags of a 2048-record tile, both exclusive scans in the same kernel
@@ -214,6 +250,8 @@ __global__ void __launch_bounds__(C_THREADS) k_accept_scan(const Work W) {
 // attributed to the device id of its FIRST member, device_plugin.go:162-170) -> device-id table, first-seen minimum.
 // Kept out of k_accept_scan: there the chain record read -> table insert -> minimum ran serially per record in a
 // divergent loop (6 % issue utilisation); here every group is an independent thread.
+// RULES: the device-id key is (rule of the first member) << 48 | device id.
+template <bool RULES>
 __global__ void __launch_bounds__(256) k_groups(const Work W) {
     const uint32_t o = blockIdx.x * blockDim.x + threadIdx.x;
     if (o >= W.totals[1]) return;
@@ -225,6 +263,7 @@ __global__ void __launch_bounds__(256) k_groups(const Work W) {
     unsigned long long did;
     uint32_t dl;
     read_id(reinterpret_cast<const uint8_t *>(&dq), dlen, did, dl);
+    if (RULES) did |= (unsigned long long)W.rrule[i] << 48;
     const uint32_t ds = dinsert(W, did);
     // a few hot device ids own most groups: same-address atomics run at ~1 per ns, so only a group that can
     // still lower the minimum issues one
@@ -259,7 +298,8 @@ __global__ void __launch_bounds__(C_THREADS) k_devfirst_scan(const Work W) {
         if ((dfm >> k) & 1u) {
             DSlot &d = W.dtab[W.grp_dslot[base + k]];
             d.ord = run;
-            W.dev_ids[run] = d.key;
+            W.dev_ids[run] = d.key & DEVID_MASK;
+            if (W.dev_rule) W.dev_rule[run] = (uint8_t)(d.key >> 48);
             run++;
         }
     }
@@ -437,21 +477,72 @@ static uint32_t bits_for(uint32_t n) {
     return b;
 }
 
-static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out, bool small_dtab, bool *retry);
+// R == nullptr: kxpu_classify (the NVIDIA constants); else the rule list of kxpu_classify_rules
+static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
+                             uint8_t *dev_rule, bool small_dtab, bool *retry);
 
-extern "C" int32_t kxpu_classify(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out) {
-    if (!ctx || !out || (n && !recs)) return KXPU_E_INVALID;
-    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+static int32_t classify_run(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
+                            uint8_t *dev_rule) {
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
     bool retry = false;
-    int32_t rc = classify_once(ctx, recs, n, out, true, &retry);
-    if (retry) rc = classify_once(ctx, recs, n, out, false, &retry);  // more distinct device ids than the small table holds
+    int32_t rc = classify_once(ctx, recs, n, out, R, dev_rule, true, &retry);
+    if (retry) rc = classify_once(ctx, recs, n, out, R, dev_rule, false, &retry);  // more distinct device ids than the small table holds
     return rc;
 }
 
-static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out, bool small_dtab, bool *retry) {
+extern "C" int32_t kxpu_classify(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out) {
+    if (!ctx || !out || (n && !recs)) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    return classify_run(ctx, recs, n, out, nullptr, nullptr);
+}
+
+// a NUL-padded field: length of the text before the first NUL, -1 when a non-NUL byte follows that NUL
+static int field_len(const char *f, int cap) {
+    int l = 0;
+    while (l < cap && f[l]) l++;
+    for (int k = l; k < cap; k++)
+        if (f[k]) return -1;
+    return l;
+}
+
+extern "C" int32_t kxpu_classify_rules(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs,
+                                       size_t n, kxpu_classify_out *out, uint8_t *dev_rule) {
+    if (!ctx || !out || (n && !recs) || !rules || n_rules == 0 || n_rules > KXPU_MAX_RULES) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    RuleTable R;
+    memset(&R, 0, sizeof R);
+    R.n = (uint32_t)n_rules;
+    for (size_t r = 0; r < n_rules; r++) {
+        const kxpu_xpu_rule &u = rules[r];
+        const int vl = field_len(u.vendor, (int)sizeof u.vendor), dl = field_len(u.driver, (int)sizeof u.driver);
+        if (vl < 1 || vl > 6 || memchr(u.vendor, '\n', (size_t)vl)) {
+            KX_SET_ERR(ctx, "classify_rules: rule %zu: vendor must be 1-6 bytes without '\\n', NUL padded", r);
+            return KXPU_E_INVALID;
+        }
+        if (dl < 1 || dl > 15 || memchr(u.driver, '/', (size_t)dl)) {
+            KX_SET_ERR(ctx, "classify_rules: rule %zu: driver must be 1-15 bytes without '/', NUL padded", r);
+            return KXPU_E_INVALID;
+        }
+        for (size_t q = 0; q < r; q++) {
+            if (memcmp(rules[q].vendor, u.vendor, sizeof u.vendor) == 0 && memcmp(rules[q].driver, u.driver, sizeof u.driver) == 0) {
+                KX_SET_ERR(ctx, "classify_rules: rules %zu and %zu are the same (vendor, driver) pair", q, r);
+                return KXPU_E_INVALID;
+            }
+        }
+        unsigned long long v = 0, d[2] = {0, 0}, m[2] = {0, 0};
+        memcpy(&v, u.vendor, (size_t)vl);
+        R.vend[r] = v | ((unsigned long long)vl << 56);
+        memcpy(d, u.driver, sizeof u.driver);
+        for (int k = 0; k <= dl; k++) m[k >> 3] |= 0xffull << (8 * (k & 7));  // the driver's bytes and its NUL
+        R.d0[r] = d[0]; R.d1[r] = d[1]; R.m0[r] = m[0]; R.m1[r] = m[1];
+    }
+    return classify_run(ctx, recs, n, out, &R, dev_rule);
+}
+
+static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
+                             uint8_t *dev_rule, bool small_dtab, bool *retry) {
     *retry = false;
     out->n_accepted = out->n_groups = out->n_devids = 0;
     if (n == 0) {
@@ -488,6 +579,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, k
     const size_t o_bk = take(n * 4), o_bv = take(n * 4), o_bk2 = take(n * 4), o_bv2 = take(n * 4);
     const size_t o_acc_idx = take(n * 4 + 64), o_gids = take(n * 4), o_goff = take((n + 1) * 4);
     const size_t o_dids = take(n * 8), o_doff = take((n + 1) * 4);
+    const size_t o_rrule = R ? take(n) : 0, o_drule = R ? take(n) : 0;
     KxScratch sc(ctx);
     uint8_t *b = nullptr;
     KX_CUDA(ctx, sc.alloc((void **)&b, off));
@@ -507,6 +599,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, k
     W.ak = (uint32_t *)(b + o_ak); W.av = (uint32_t *)(b + o_av); W.bk = (uint32_t *)(b + o_bk); W.bv = (uint32_t *)(b + o_bv);
     W.accept_index = (uint32_t *)(b + o_acc_idx); W.group_ids = (uint32_t *)(b + o_gids);
     W.group_off = (uint32_t *)(b + o_goff); W.dev_ids = (unsigned long long *)(b + o_dids); W.dev_off = (uint32_t *)(b + o_doff);
+    if (R) { W.rrule = b + o_rrule; W.dev_rule = b + o_drule; }
 
     cudaMemcpyAsync(b + o_recs, recs, n * sizeof(kxpu_devrec), cudaMemcpyHostToDevice, ctx->stream);
     const unsigned g = (N + 255) / 256;
@@ -516,9 +609,11 @@ static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, k
         KxTimer tm(ctx, KXPU_T_CLASSIFY);
         k_reset<<<std::min<unsigned>((unsigned)((ff_bytes / 16 + 255) / 256), 8u * ctx->sm_count), 256, 0, ctx->stream>>>(
             (uint4 *)b, ff_bytes / 16, W.totals, (uint32_t)zero_words);
-        k_candidates<<<g, 256, 0, ctx->stream>>>(W);
+        if (R) k_candidates_rules<<<g, 256, 0, ctx->stream>>>(W, *R);
+        else k_candidates<<<g, 256, 0, ctx->stream>>>(W);
         k_accept_scan<<<c_tiles, C_THREADS, 0, ctx->stream>>>(W);
-        k_groups<<<g, 256, 0, ctx->stream>>>(W);
+        if (R) k_groups<true><<<g, 256, 0, ctx->stream>>>(W);
+        else k_groups<false><<<g, 256, 0, ctx->stream>>>(W);
         k_devfirst_scan<<<c_tiles, C_THREADS, 0, ctx->stream>>>(W);
         k_pairs<<<std::min<unsigned>(g, 4u * ctx->sm_count), 256, 0, ctx->stream>>>(W, passes);
         ctx->launches += 6;
@@ -557,6 +652,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, k
         cudaMemcpyAsync(out->dev_ids, W.dev_ids, (size_t)nd * 8, cudaMemcpyDeviceToHost, ctx->stream);
         cudaMemcpyAsync(out->dev_off, W.dev_off, ((size_t)nd + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream);
         cudaMemcpyAsync(out->dev_groups, bv, (size_t)ng * 4, cudaMemcpyDeviceToHost, ctx->stream);
+        if (dev_rule && nd) cudaMemcpyAsync(dev_rule, W.dev_rule, nd, cudaMemcpyDeviceToHost, ctx->stream);
         e = cudaStreamSynchronize(ctx->stream);
         if (e != cudaSuccess) { KX_SET_ERR(ctx, "classify D2H failed: %s", cudaGetErrorString(e)); rc = KXPU_E_CUDA; }
         if (ng == 0) out->group_off[0] = 0;

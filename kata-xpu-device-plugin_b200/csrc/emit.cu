@@ -14,6 +14,8 @@
 // shared -> global) plus at most 15 head / tail bytes.  Document header and tail belong to the first
 // and the last tile.  Allocate names and ListAndWatch bytes (<= 24 B per item) are length -> single-
 // pass scan -> thread-per-item write.
+#include <cstring>
+#include <string>
 #include <vector>
 
 #include "common.cuh"
@@ -23,38 +25,75 @@ namespace kxemit {
 
 constexpr int TILE = 128;      // devices per CTA
 constexpr int EMIT_THREADS = 256;
-constexpr int MAX_FRAG = 368;  // upper bound of one fragment: literals (<= 284) + 2 x 20 + 2 x 10 + 15 + 2 + slack; with the rest of
-                               // TileSmem this keeps a CTA under 56.7 KB: four CTAs per SM, the 512 tiles of cfg5 are ONE wave
+constexpr int MAX_FRAG = 368;  // upper bound of one fragment: literals (<= 267 + kind) + 2 x 20 + 2 x 10 + 15 + 2 + slack; with the
+                               // rest of TileSmem this keeps a CTA under 56.7 KB: four CTAs per SM, the 512 tiles of cfg5 are ONE
+                               // wave.  Holds every kind up to 22 bytes.
+constexpr int MAX_FRAG_LONG = 416;  // kinds of 23..63 bytes: 62.7 KB per CTA, three CTAs per SM
 constexpr int POOL_MAX = 640;
+constexpr int KIND_MAX = 63;
 
 // ------------------------------------------------------------------ templates
 // YAML (yaml.v3, indent 2) and JSON (MarshalIndent "  ") literals between the variable
-// fields: see SURVEY.md 8a-fmt for the derivation.
+// fields: see SURVEY.md 8a-fmt for the derivation.  The CDI kind (CdiVendorClass, "nvidia.com/gpu" in the
+// reference, generic_device_plugin.go:31) is a runtime argument: literal 3 and the document head are
+// <before> kind <after>, assembled on the host into the pool the kernel receives as a parameter.
+// KX_*A / KX_*B: the text before / after the kind
 #define KX_Y0 "  - name: \""
 #define KX_Y1 "\"\n    annotations:\n      attach-pci: \"true\"\n      bdf: "
 #define KX_Y2 "\n      cdi.k8s.io/vfio"
-#define KX_Y3 ": nvidia.com/gpu="
+#define KX_Y3A ": "
+#define KX_Y3B "="
 #define KX_Y4 "\n    containerEdits:\n      deviceNodes:\n        - path: /dev/vfio/"
 #define KX_Y5 "\n"
-#define KX_YH "cdiVersion: 0.6.0\nkind: nvidia.com/gpu\ndevices:\n"
+#define KX_YHA "cdiVersion: 0.6.0\nkind: "
+#define KX_YHB "\ndevices:\n"
 #define KX_YT ""
+#define KX_YEB "\ndevices: []\n"
 #define KX_J0 "    {\n      \"name\": \""
 #define KX_J1 "\",\n      \"annotations\": {\n        \"attach-pci\": \"true\",\n        \"bdf\": \""
 #define KX_J2 "\",\n        \"cdi.k8s.io/vfio"
-#define KX_J3 "\": \"nvidia.com/gpu="
+#define KX_J3A "\": \""
+#define KX_J3B "="
 #define KX_J4 "\"\n      },\n      \"containerEdits\": {\n        \"deviceNodes\": [\n          {\n            \"path\": \"/dev/vfio/"
 #define KX_J5 "\"\n          }\n        ]\n      }\n    }"
-#define KX_JH "{\n  \"cdiVersion\": \"0.6.0\",\n  \"kind\": \"nvidia.com/gpu\",\n  \"devices\": [\n"
+#define KX_JHA "{\n  \"cdiVersion\": \"0.6.0\",\n  \"kind\": \""
+#define KX_JHB "\",\n  \"devices\": [\n"
 #define KX_JT "  ],\n  \"containerEdits\": {}\n}"
-// pool = six literals | document head | document tail
-__constant__ char c_yaml_pool[] = KX_Y0 KX_Y1 KX_Y2 KX_Y3 KX_Y4 KX_Y5 KX_YH KX_YT;
-__constant__ char c_json_pool[] = KX_J0 KX_J1 KX_J2 KX_J3 KX_J4 KX_J5 KX_JH KX_JT;
-static const char *h_yaml_parts[8] = {KX_Y0, KX_Y1, KX_Y2, KX_Y3, KX_Y4, KX_Y5, KX_YH, KX_YT};
-static const char *h_json_parts[8] = {KX_J0, KX_J1, KX_J2, KX_J3, KX_J4, KX_J5, KX_JH, KX_JT};
+#define KX_JEB "\",\n  \"devices\": null,\n  \"containerEdits\": {}\n}"
+// part k = before[k] (+ kind + after[k] when after[k] != NULL); parts 0-5 are the literals, 6 the document head,
+// 7 the tail, 8 the whole document for zero devices (Devices stays nil, cdi/spec.go:42-49)
+struct Parts { const char *before[9], *after[9]; };
+static const Parts h_yaml_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_Y4, KX_Y5, KX_YHA, KX_YT, KX_YHA},
+                                   {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB}};
+static const Parts h_json_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_J4, KX_J5, KX_JHA, KX_JT, KX_JHA},
+                                   {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB}};
+static const char *kDefaultKind = "nvidia.com/gpu";  // CdiVendorClass, generic_device_plugin.go:31
 
-static const char h_yaml_empty[] = "cdiVersion: 0.6.0\nkind: nvidia.com/gpu\ndevices: []\n";
-static const char h_json_empty[] =
-    "{\n  \"cdiVersion\": \"0.6.0\",\n  \"kind\": \"nvidia.com/gpu\",\n  \"devices\": null,\n  \"containerEdits\": {}\n}";
+// The supported kind domain (include/kxpu.h): "vendor/class", <= 63 bytes; vendor = letter [A-Za-z0-9_.-]*
+// alnum, class = letter [A-Za-z0-9_-]* alnum (a subset of CDI v0.8.0 pkg/parser's vendor / class rules).
+static bool kind_ok(const char *kind) {
+    if (!kind) return false;
+    const size_t len = strnlen(kind, KIND_MAX + 1);
+    if (len > (size_t)KIND_MAX) return false;
+    const char *slash = (const char *)memchr(kind, '/', len);
+    if (!slash) return false;
+    auto alpha = [](char c) { return (c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z'); };
+    auto alnum = [&](char c) { return alpha(c) || (c >= '0' && c <= '9'); };
+    auto part = [&](const char *s, size_t l, bool dots) {
+        if (l == 0 || !alpha(s[0]) || !alnum(s[l - 1])) return false;
+        for (size_t k = 0; k < l; k++)
+            if (!(alnum(s[k]) || s[k] == '_' || s[k] == '-' || (dots && s[k] == '.'))) return false;
+        return true;
+    };
+    const size_t vl = (size_t)(slash - kind);
+    return part(kind, vl, true) && part(slash + 1, len - vl - 1, false);
+}
+
+static std::string part_text(const Parts &P, int k, const char *kind) {
+    std::string s = P.before[k];
+    if (P.after[k]) { s += kind; s += P.after[k]; }
+    return s;
+}
 
 __device__ __forceinline__ uint32_t dec_len(unsigned long long v) {
     uint32_t l = 1;
@@ -111,10 +150,12 @@ struct EmitParams {
     uint32_t epoch;
     unsigned long long *total_out;
     uint32_t *flags;
+    uint8_t pool[POOL_MAX];   // literals | head | tail, built on the host for the call's kind
 };
 
+template <int MAXF>
 struct TileSmem {
-    alignas(16) uint8_t stage[TILE * MAX_FRAG + 512];
+    alignas(16) uint8_t stage[TILE * MAXF + 512];
     uint8_t pool[POOL_MAX];
     uint8_t idx[TILE][20], grp[TILE][12], bdf[TILE][16];
     uint32_t meta[TILE];    // il | gl << 8 | bl << 16 | quoted << 24
@@ -124,15 +165,14 @@ struct TileSmem {
     uint32_t tile_total;
 };
 
-template <int FMT>
-__global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const EmitParams E) {
+template <int FMT, int MAXF>
+__global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constant__ EmitParams E) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
-    TileSmem &S = *reinterpret_cast<TileSmem *>(smem_raw);
+    TileSmem<MAXF> &S = *reinterpret_cast<TileSmem<MAXF> *>(smem_raw);
     const uint32_t tid = threadIdx.x, lane = tid & 31u, w = tid >> 5;
     const uint32_t tile = blockIdx.x, i0 = tile * TILE;
     const bool first_tile = tile == 0, last_tile = tile == gridDim.x - 1;
-    const char *cpool = FMT == KXPU_FMT_YAML ? c_yaml_pool : c_json_pool;
-    for (uint32_t k = tid; k < E.pool_len; k += EMIT_THREADS) S.pool[k] = (uint8_t)cpool[k];
+    for (uint32_t k = tid; k < E.pool_len; k += EMIT_THREADS) S.pool[k] = E.pool[k];
 
     // ---- fragment lengths and variable fields: one thread per device
     uint32_t flen = 0;
@@ -229,22 +269,26 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const EmitParams E) 
 }
 
 // ------------------------------------------------------------------ Allocate names
+// name i = prefix + decimal(idx[i]), prefix = kind + "=" (<= 64 bytes)
+struct NamePrefix {
+    uint8_t b[KIND_MAX + 1];
+    uint32_t len;
+};
 __global__ void __launch_bounds__(256) k_alloc_len(const unsigned long long *__restrict__ idx, uint32_t n,
-                                                   uint32_t *__restrict__ lens) {
+                                                   uint32_t *__restrict__ lens, uint32_t prefix_len) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i > n) return;
-    lens[i] = i < n ? 15u + dec_len(idx[i]) : 0u;  // len("nvidia.com/gpu=") == 15
+    lens[i] = i < n ? prefix_len + dec_len(idx[i]) : 0u;
 }
 __global__ void __launch_bounds__(256) k_alloc_write(const unsigned long long *__restrict__ idx, uint32_t n,
-                                                     const uint32_t *__restrict__ offs, uint8_t *__restrict__ out) {
+                                                     const uint32_t *__restrict__ offs, uint8_t *__restrict__ out,
+                                                     const __grid_constant__ NamePrefix P) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const char pre[16] = "nvidia.com/gpu=";
     uint8_t *dst = out + offs[i];
-#pragma unroll
-    for (int k = 0; k < 15; k++) dst[k] = (uint8_t)pre[k];
+    for (uint32_t k = 0; k < P.len; k++) dst[k] = P.b[k];
     unsigned long long v = idx[i];
-    dec_write(v, dec_len(v), dst + 15);
+    dec_write(v, dec_len(v), dst + P.len);
 }
 
 // ------------------------------------------------------------------ ListAndWatchResponse
@@ -277,41 +321,54 @@ __global__ void __launch_bounds__(256) k_lw_write(const uint32_t *__restrict__ g
 
 using namespace kxemit;
 
-extern "C" int32_t kxpu_cdi_emit(kxpu_ctx *ctx, int32_t format, const kxpu_cdidev *devs, size_t n, uint8_t *out,
-                                 size_t cap, size_t *len) {
-    if (!ctx || !len || (n && !devs) || (format != KXPU_FMT_YAML && format != KXPU_FMT_JSON)) return KXPU_E_INVALID;
-    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+template <int FMT, int MAXF>
+static void emit_launch(kxpu_ctx *ctx, uint32_t tiles, const EmitParams &E) {
+    k_cdi_fused<FMT, MAXF><<<tiles, EMIT_THREADS, sizeof(TileSmem<MAXF>), ctx->stream>>>(E);
+}
+
+static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_cdidev *devs, size_t n, uint8_t *out,
+                        size_t cap, size_t *len) {
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
+    const Parts &parts = format == KXPU_FMT_YAML ? h_yaml_parts : h_json_parts;
     if (n == 0) {  // Devices stays nil: yaml "devices: []", json "devices": null (cdi/spec.go:42-49)
-        const char *doc = format == KXPU_FMT_YAML ? h_yaml_empty : h_json_empty;
-        *len = strlen(doc);
+        const std::string doc = part_text(parts, 8, kind);
+        *len = doc.size();
         if (cap < *len || !out) return KXPU_E_NOSPACE;
-        memcpy(out, doc, *len);
+        memcpy(out, doc.data(), *len);
         return KXPU_OK;
     }
     static bool attr_done = false;
     if (!attr_done) {
-        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem));
-        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_JSON>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem));
+        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAX_FRAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem<MAX_FRAG>));
+        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_JSON, MAX_FRAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem<MAX_FRAG>));
+        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAX_FRAG_LONG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)sizeof(TileSmem<MAX_FRAG_LONG>));
+        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_JSON, MAX_FRAG_LONG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)sizeof(TileSmem<MAX_FRAG_LONG>));
         attr_done = true;
     }
-    const char **parts = format == KXPU_FMT_YAML ? h_yaml_parts : h_json_parts;
     EmitParams E;
     memset(&E, 0, sizeof E);
     uint32_t acc = 0;
     for (int k = 0; k < 8; k++) {
+        const std::string s = part_text(parts, k, kind);
+        if (acc + s.size() > (size_t)POOL_MAX) return KXPU_E_INVALID;  // the literals grew: POOL_MAX must follow
+        memcpy(E.pool + acc, s.data(), s.size());
         E.off[k] = (uint16_t)acc;
-        E.len[k] = (uint16_t)strlen(parts[k]);
+        E.len[k] = (uint16_t)s.size();
         acc += E.len[k];
         if (k < 6) E.lit_total += E.len[k];
     }
     E.pool_len = acc;
     const uint32_t N = (uint32_t)n;
     const uint32_t tiles = (N + TILE - 1) / TILE;
-    const size_t bound = (size_t)n * (E.lit_total + 2 * 20 + 2 * 10 + 15 + 2 + 2) + E.len[6] + E.len[7] + 64;  // no fragment is longer
-    if (E.lit_total + 2 * 20 + 2 * 10 + 15 + 2 + 2 > (uint32_t)MAX_FRAG) return KXPU_E_INVALID;  // the literals grew: MAX_FRAG must follow
+    const uint32_t frag = E.lit_total + 2 * 20 + 2 * 10 + 15 + 2 + 2;  // no fragment is longer
+    const size_t bound = (size_t)n * frag + E.len[6] + E.len[7] + 64;
+    // kinds up to 22 bytes fit the four-CTAs-per-SM tile, longer ones take the MAX_FRAG_LONG instantiation
+    const bool long_frag = frag > (uint32_t)MAX_FRAG;
+    if (frag > (uint32_t)MAX_FRAG_LONG) return KXPU_E_INVALID;  // the literals grew: MAX_FRAG_LONG must follow
     KxScratch sc(ctx);
     kxpu_cdidev *d_devs = nullptr;
     uint8_t *d_out = nullptr;
@@ -327,8 +384,13 @@ extern "C" int32_t kxpu_cdi_emit(kxpu_ctx *ctx, int32_t format, const kxpu_cdide
     E.epoch = kx_next_epoch(ctx);
     {
         KxTimer tm(ctx, KXPU_T_EMIT);
-        if (format == KXPU_FMT_YAML) k_cdi_fused<KXPU_FMT_YAML><<<tiles, EMIT_THREADS, sizeof(TileSmem), ctx->stream>>>(E);
-        else k_cdi_fused<KXPU_FMT_JSON><<<tiles, EMIT_THREADS, sizeof(TileSmem), ctx->stream>>>(E);
+        if (format == KXPU_FMT_YAML) {
+            if (long_frag) emit_launch<KXPU_FMT_YAML, MAX_FRAG_LONG>(ctx, tiles, E);
+            else emit_launch<KXPU_FMT_YAML, MAX_FRAG>(ctx, tiles, E);
+        } else {
+            if (long_frag) emit_launch<KXPU_FMT_JSON, MAX_FRAG_LONG>(ctx, tiles, E);
+            else emit_launch<KXPU_FMT_JSON, MAX_FRAG>(ctx, tiles, E);
+        }
         KX_LAUNCHED(ctx);
     }
     unsigned long long h[2] = {0, 0};
@@ -343,6 +405,21 @@ extern "C" int32_t kxpu_cdi_emit(kxpu_ctx *ctx, int32_t format, const kxpu_cdide
     e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) { KX_SET_ERR(ctx, "cdi_emit D2H failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
     return KXPU_OK;
+}
+
+extern "C" int32_t kxpu_cdi_emit(kxpu_ctx *ctx, int32_t format, const kxpu_cdidev *devs, size_t n, uint8_t *out,
+                                 size_t cap, size_t *len) {
+    if (!ctx || !len || (n && !devs) || (format != KXPU_FMT_YAML && format != KXPU_FMT_JSON)) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    return cdi_emit(ctx, format, kDefaultKind, devs, n, out, cap, len);
+}
+
+extern "C" int32_t kxpu_cdi_emit_kind(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_cdidev *devs, size_t n,
+                                      uint8_t *out, size_t cap, size_t *len) {
+    if (!ctx || !len || !kind || (n && !devs) || (format != KXPU_FMT_YAML && format != KXPU_FMT_JSON)) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    if (!kind_ok(kind)) { KX_SET_ERR(ctx, "cdi_emit_kind: kind is not a CDI vendor/class of at most 63 bytes"); return KXPU_E_UNSUPPORTED; }
+    return cdi_emit(ctx, format, kind, devs, n, out, cap, len);
 }
 
 // shared driver of the two "thread per item" emitters
@@ -386,23 +463,41 @@ static int32_t emit_items(kxpu_ctx *ctx, size_t n, size_t in_bytes, const void *
     return rc;
 }
 
-extern "C" int32_t kxpu_alloc_names(kxpu_ctx *ctx, const uint64_t *idx, size_t n, uint8_t *out, size_t cap,
-                                    uint32_t *offsets, size_t *need) {
-    if (!ctx || !offsets || (n && !idx)) return KXPU_E_INVALID;
-    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+static int32_t alloc_names(kxpu_ctx *ctx, const char *kind, const uint64_t *idx, size_t n, uint8_t *out, size_t cap,
+                           uint32_t *offsets, size_t *need) {
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
     if (n == 0) { offsets[0] = 0; if (need) *need = 0; return KXPU_OK; }
+    NamePrefix P;
+    memset(&P, 0, sizeof P);
+    P.len = (uint32_t)strlen(kind) + 1u;  // kind_ok: <= 63 bytes
+    memcpy(P.b, kind, P.len - 1u);
+    P.b[P.len - 1u] = (uint8_t)'=';
     cudaStream_t st = ctx->stream;
     return emit_items(
         ctx, n, n * 8, idx, nullptr, out, cap, offsets, need,
-        [st](const uint8_t *in, const uint8_t *, uint32_t N, uint32_t *lens) {
-            k_alloc_len<<<(N + 1 + 255) / 256, 256, 0, st>>>((const unsigned long long *)in, N, lens);
+        [st, &P](const uint8_t *in, const uint8_t *, uint32_t N, uint32_t *lens) {
+            k_alloc_len<<<(N + 1 + 255) / 256, 256, 0, st>>>((const unsigned long long *)in, N, lens, P.len);
         },
-        [st](const uint8_t *in, const uint8_t *, uint32_t N, const uint32_t *offs, uint8_t *o) {
-            k_alloc_write<<<(N + 255) / 256, 256, 0, st>>>((const unsigned long long *)in, N, offs, o);
+        [st, &P](const uint8_t *in, const uint8_t *, uint32_t N, const uint32_t *offs, uint8_t *o) {
+            k_alloc_write<<<(N + 255) / 256, 256, 0, st>>>((const unsigned long long *)in, N, offs, o, P);
         });
+}
+
+extern "C" int32_t kxpu_alloc_names(kxpu_ctx *ctx, const uint64_t *idx, size_t n, uint8_t *out, size_t cap,
+                                    uint32_t *offsets, size_t *need) {
+    if (!ctx || !offsets || (n && !idx)) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    return alloc_names(ctx, kDefaultKind, idx, n, out, cap, offsets, need);
+}
+
+extern "C" int32_t kxpu_alloc_names_kind(kxpu_ctx *ctx, const char *kind, const uint64_t *idx, size_t n, uint8_t *out,
+                                         size_t cap, uint32_t *offsets, size_t *need) {
+    if (!ctx || !offsets || !kind || (n && !idx)) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    if (!kind_ok(kind)) { KX_SET_ERR(ctx, "alloc_names_kind: kind is not a CDI vendor/class of at most 63 bytes"); return KXPU_E_UNSUPPORTED; }
+    return alloc_names(ctx, kind, idx, n, out, cap, offsets, need);
 }
 
 extern "C" int32_t kxpu_lw_encode(kxpu_ctx *ctx, const uint32_t *group_ids, const uint8_t *healthy, size_t n,

@@ -27,6 +27,15 @@ static const char *kUnhealthy = "Unhealthy";                                 // 
 static const char *kK8SCDIVendorClass = "KUBERNETES_CDI_VENDOR_CLASS";       // generic_device_plugin.go:29
 static const char *kCdiVendorClass = "nvidia.com/gpu";                       // generic_device_plugin.go:30
 
+XpuClass defaultXpuClass() { return XpuClass{"10de", "vfio-pci", "nvidia.com", kCdiVendorClass, "cdi-vfio-xxxx"}; }
+
+bool Plugin::defaultClasses() const {
+    if (xpuClasses.size() != 1) return false;
+    const XpuClass &c = xpuClasses[0], d = defaultXpuClass();
+    return c.vendor == d.vendor && c.driver == d.driver && c.resourceNamespace == d.resourceNamespace && c.cdiKind == d.cdiKind &&
+           c.cdiFileStem == d.cdiFileStem;
+}
+
 static Error fail(const std::string &m) { Error e; e.failed = true; e.message = m; return e; }
 static Error kxfail(kxpu_ctx *ctx, const char *what, int32_t rc) {
     return fail(std::string(what) + ": " + kxpu_strerror(rc) + " (" + kxpu_last_error(ctx) + ")");
@@ -160,12 +169,14 @@ static bool packID(const std::string &raw, uint8_t txt[8], uint8_t &len) {
 
 // The body of the walk callback for one non-directory entry (device_plugin.go:141-175, the reads
 // only, in the reference's order and as lazily as the reference: nothing is read behind a vendor
-// that is not 10de or a driver that is not vfio-pci): raw bytes of `vendor` / `device`, basenames
+// that no class has -- 10de by default -- or a driver that is not that vendor's class driver --
+// vfio-pci by default): raw bytes of `vendor` / `device`, basenames
 // of the `driver` / `iommu_group` links.  An entry the record cannot carry (address longer than 15
 // bytes, group that is not a canonical decimal below 2^32-1, id longer than the field) is logged and
 // skipped like a read error -- and only if the reference would have accepted it; it never stops the walk.
 template <typename ReadID, typename ReadLnk>
-static Error leafRecord(const std::string &name, ReadID readID, ReadLnk readLnk, kxpu_devrec &r) {
+static Error leafRecord(const std::string &name, const std::vector<XpuClass> &classes, ReadID readID, ReadLnk readLnk,
+                        kxpu_devrec &r) {
     memset(&r, 0, sizeof r);
     strncpy(r.bdf, name.c_str(), sizeof r.bdf - 1);
     std::string s;
@@ -173,19 +184,23 @@ static Error leafRecord(const std::string &name, ReadID readID, ReadLnk readLnk,
         r.flags |= KXPU_REC_VENDOR_ERR;  // "Could not get vendor ID for device" -> skipped (:143-146)
         return Error();
     }
-    const bool nvidia = trimID(s) == "10de";  // :149
+    const std::string vendor = trimID(s);
+    bool known = false;  // :149 -- the vendor of some class
+    for (const XpuClass &c : classes) known = known || vendor == c.vendor;
     if (!packID(s, r.vendor_txt, r.vendor_len)) {  // an id of six or more characters is not 10de
         memcpy(r.vendor_txt, s.data(), 8);
         r.vendor_len = 8;
         r.flags |= KXPU_REC_VENDOR_ERR;
     }
-    if (!nvidia) return Error();
+    if (!known) return Error();
     if (!readLnk("driver", s)) {
         r.flags |= KXPU_REC_DRIVER_ERR;  // :152-155
         return Error();
     }
     memcpy(r.driver, s.data(), std::min<size_t>(s.size(), sizeof r.driver - 1));
-    if (s != "vfio-pci") return Error();  // :156
+    bool bound = false;  // :156 -- the driver of that vendor's class
+    for (const XpuClass &c : classes) bound = bound || (vendor == c.vendor && s == c.driver);
+    if (!bound) return Error();
     if (name.size() > sizeof r.bdf - 1) {
         fprintf(stderr, "PCI address longer than 15 bytes, device skipped: %s\n", name.c_str());
         r.flags |= KXPU_REC_IOMMU_ERR;
@@ -243,7 +258,7 @@ static Error walkDir(Plugin &p, const std::string &path, const std::string &name
     // one raw record per non-directory entry; every read goes through the seams and is keyed by
     // info.Name() under basePath exactly like :142,:151,:157,:164
     kxpu_devrec r;
-    Error e = leafRecord(name,
+    Error e = leafRecord(name, p.xpuClasses,
                          [&](const char *prop, std::string &out) { return p.readIDFromFile(p.basePath, name, prop, out); },
                          [&](const char *link, std::string &out) { return p.readLink(p.basePath, name, link, out); }, r);
     if (e) return e;
@@ -331,7 +346,7 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
         for (size_t i = lo; i < hi; i++) {
             if (ents[i].dir) continue;
             const std::string &name = ents[i].name;
-            errs[i] = leafRecord(name, [&](const char *prop, std::string &out) { return readID(name, prop, out); },
+            errs[i] = leafRecord(name, xpuClasses, [&](const char *prop, std::string &out) { return readID(name, prop, out); },
                                  [&](const char *link, std::string &out) { return readLnk(name, link, out); }, flat[i]);
         }
     };
@@ -369,6 +384,8 @@ static std::string devIdString(uint64_t packed) {
 Error Plugin::createIommuDeviceMap() {
     iommuMap.clear();   // :127
     deviceMap.clear();  // :128
+    iommuClass.clear();
+    deviceClass.clear();
     // the generation is read BEFORE the walk: an event during the walk makes the snapshot stale, never fresh
     haveSnapshotGen_ = snapshotValidation && bindGeneration && bindGeneration(snapshotGen_);
     std::vector<kxpu_devrec> recs;
@@ -381,22 +398,54 @@ Error Plugin::createIommuDeviceMap() {
     memset(&out, 0, sizeof out);
     out.accept_index = accept.data(); out.group_ids = gids.data(); out.group_off = goff.data();
     out.group_members = gmem.data(); out.dev_ids = dids.data(); out.dev_off = doff.data(); out.dev_groups = dgrp.data();
-    int32_t rc = kxpu_classify(ctx_, recs.data(), n, &out);
-    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify", rc);  // fatal: there is no CPU path
+    const bool dflt = defaultClasses();
+    std::vector<uint8_t> drule(n ? n : 1, 0);
+    int32_t rc;
+    if (dflt) {
+        rc = kxpu_classify(ctx_, recs.data(), n, &out);
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify", rc);  // fatal: there is no CPU path
+    } else {
+        // one rule per class: rule index == class index
+        std::vector<kxpu_xpu_rule> rules(xpuClasses.size());
+        for (size_t c = 0; c < xpuClasses.size(); c++) {
+            memset(&rules[c], 0, sizeof rules[c]);
+            strncpy(rules[c].vendor, xpuClasses[c].vendor.c_str(), sizeof rules[c].vendor);
+            strncpy(rules[c].driver, xpuClasses[c].driver.c_str(), sizeof rules[c].driver);
+        }
+        rc = kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data());
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify_rules", rc);
+    }
+    // class of a group = the rule of its first member, which the device-map entry listing it carries
+    std::map<uint32_t, size_t> groupClass;
+    for (uint32_t d = 0; d < out.n_devids; d++)
+        for (uint32_t k = doff[d]; k < doff[d + 1]; k++) groupClass[dgrp[k]] = drule[d];
     for (uint32_t g = 0; g < out.n_groups; g++) {
         std::vector<NvidiaGpuDevice> devs;
         for (uint32_t k = goff[g]; k < goff[g + 1]; k++) {
             uint32_t i = gmem[k];
             devs.push_back(NvidiaGpuDevice{std::string(recs[i].bdf), accept[i]});  // :171-174
+            if (!dflt) {  // the class this function itself matched (a group may hold functions of several classes)
+                const std::string vendor = trimID(std::string((const char *)recs[i].vendor_txt, recs[i].vendor_len));
+                for (size_t c = 0; c < xpuClasses.size(); c++)
+                    if (xpuClasses[c].vendor == vendor && xpuClasses[c].driver == recs[i].driver) devs.back().xpuClass = c;
+            }
         }
         iommuMap.emplace_back(std::to_string(gids[g]), std::move(devs));
+        iommuClass.push_back(groupClass[gids[g]]);
     }
     for (uint32_t d = 0; d < out.n_devids; d++) {
         std::vector<std::string> groups;
         for (uint32_t k = doff[d]; k < doff[d + 1]; k++) groups.push_back(std::to_string(dgrp[k]));  // :169
         deviceMap.emplace_back(devIdString(dids[d]), std::move(groups));
+        deviceClass.push_back(drule[d]);
     }
     return Error();
+}
+
+size_t Plugin::classOfGroup(const std::string &group) const {
+    for (size_t g = 0; g < iommuMap.size() && g < iommuClass.size(); g++)
+        if (iommuMap[g].first == group) return iommuClass[g];
+    return 0;
 }
 
 // The pci.ids file into page-locked memory the GPU can address (kxpu_pinned_alloc): with text, keys and rows in
@@ -466,13 +515,16 @@ static bool parseHex4(const std::string &s, uint32_t &v) {
 // getDeviceName, device_plugin.go:208-259, for a whole batch of device ids: ONE join and ONE name
 // gather through the ABI (cgo calls stay coarse, SURVEY H7).  "" means "not found" exactly like the
 // reference; sysfs ids are four lowercase hex digits, anything else is treated as not found.
-std::vector<std::string> Plugin::getDeviceNames(const std::vector<std::string> &deviceIDs) {
+// With `vendors` the key of id i is (vendors[i] << 16) | id; a vendor that is not four lowercase hex digits
+// never names anything, so that device falls back to its raw id like a miss (:100-103).
+std::vector<std::string> Plugin::getDeviceNames(const std::vector<std::string> &deviceIDs, const std::vector<std::string> *vendors) {
     std::vector<std::string> out(deviceIDs.size());
     std::vector<uint32_t> keys;
     std::vector<size_t> where;
     for (size_t i = 0; i < deviceIDs.size(); i++) {
-        uint32_t d;
-        if (parseHex4(deviceIDs[i], d)) { keys.push_back((0x10deu << 16) | d); where.push_back(i); }  // nvidiaVendorID, :19
+        uint32_t d, v = 0x10deu;  // nvidiaVendorID, :19
+        if (vendors && !parseHex4((*vendors)[i], v)) continue;
+        if (parseHex4(deviceIDs[i], d)) { keys.push_back((v << 16) | d); where.push_back(i); }
     }
     std::vector<int32_t> rows(keys.size(), KXPU_ROW_MISS);
     if (!table_) {
@@ -492,7 +544,8 @@ std::vector<std::string> Plugin::getDeviceNames(const std::vector<std::string> &
     if (need && kxpu_names(ctx_, table_, rows.data(), rows.size(), blob.data(), need, offs.data(), &need) != KXPU_OK) return out;
     for (size_t k = 0; k < keys.size(); k++) {
         if (rows[k] == KXPU_ROW_MISS) {
-            fprintf(stderr, "Could not find NVIDIA device with id: %s\n", deviceIDs[where[k]].c_str());  // :234
+            if (vendors) fprintf(stderr, "Could not find device %s:%s\n", (*vendors)[where[k]].c_str(), deviceIDs[where[k]].c_str());
+            else fprintf(stderr, "Could not find NVIDIA device with id: %s\n", deviceIDs[where[k]].c_str());  // :234
             continue;
         }
         out[where[k]].assign((const char *)blob.data() + offs[k], offs[k + 1] - offs[k]);
@@ -502,8 +555,59 @@ std::vector<std::string> Plugin::getDeviceNames(const std::vector<std::string> &
 
 std::string Plugin::getDeviceName(const std::string &deviceID) { return getDeviceNames({deviceID})[0]; }
 
+static Error writeSpecFile(const std::string &file_path, const std::vector<uint8_t> &doc, size_t len, bool &written) {
+    written = false;
+    FILE *f = fopen(file_path.c_str(), "wb");  // os.Create
+    if (!f) {
+        printf("Error creating file: %s\n", strerror(errno));  // spec.go:95: printed and swallowed
+        return Error();
+    }
+    size_t w = fwrite(doc.data(), 1, len, f);
+    fclose(f);
+    if (w != len) { printf("Error writing to file\n"); return Error(); }
+    written = true;
+    printf("Data successfully written to file\n");  // spec.go:126
+    return Error();
+}
+
+// generateCDISpec for a class list: one file per class, <stem>.yaml|.json, with that class's kind and only the devices
+// of its groups in ascending index; a class without devices gets the empty document (the reference writes one for
+// zero devices too).
+Error Plugin::generateCDISpecClasses(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, int32_t fmt) {
+    std::vector<std::vector<kxpu_cdidev>> per(xpuClasses.size());
+    for (const auto &kv : m) {
+        const size_t c = classOfGroup(kv.first);
+        for (const NvidiaGpuDevice &dev : kv.second) {
+            kxpu_cdidev d;
+            memset(&d, 0, sizeof d);
+            strncpy(d.bdf, dev.addr.c_str(), sizeof d.bdf - 1);
+            d.iommu_group = (uint32_t)strtoul(kv.first.c_str(), nullptr, 10);
+            d.index = dev.index;
+            per[c].push_back(d);
+        }
+    }
+    for (size_t c = 0; c < xpuClasses.size(); c++) {
+        std::vector<kxpu_cdidev> &devs = per[c];
+        std::sort(devs.begin(), devs.end(), [](const kxpu_cdidev &a, const kxpu_cdidev &b) { return a.index < b.index; });
+        const char *kind = xpuClasses[c].cdiKind.c_str();
+        size_t len = 0;
+        int32_t rc = kxpu_cdi_emit_kind(ctx_, fmt, kind, devs.data(), devs.size(), nullptr, 0, &len);
+        if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, "kxpu_cdi_emit_kind", rc);
+        std::vector<uint8_t> doc(len ? len : 1);
+        rc = kxpu_cdi_emit_kind(ctx_, fmt, kind, devs.data(), devs.size(), doc.data(), len, &len);
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_cdi_emit_kind", rc);
+        const std::string file_path = cdiConfigPath + xpuClasses[c].cdiFileStem + (fmt == KXPU_FMT_YAML ? ".yaml" : ".json");
+        bool written = false;
+        writeSpecFile(file_path, doc, len, written);
+        if (written) { cdiFiles.push_back(file_path); lastCdiFile = file_path; }
+    }
+    return Error();
+}
+
 // generateCDISpec, device_plugin.go:55-80 + CdiSpec.Save, cdi/spec.go:85-127
 Error Plugin::generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, const std::string &format) {
+    cdiFiles.clear();
+    if (!defaultClasses()) return generateCDISpecClasses(m, format == "YAML" ? KXPU_FMT_YAML : KXPU_FMT_JSON);
     std::vector<kxpu_cdidev> devs;
     for (const auto &kv : m) {
         for (const NvidiaGpuDevice &dev : kv.second) {
@@ -534,6 +638,7 @@ Error Plugin::generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m,
     fclose(f);
     if (w != len) { printf("Error writing to file\n"); return Error(); }
     lastCdiFile = file_path;
+    cdiFiles.push_back(file_path);
     printf("Data successfully written to file\n");  // spec.go:126
     return Error();
 }
@@ -541,12 +646,18 @@ Error Plugin::generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m,
 // createDevicePlugins, device_plugin.go:83-112 (nothing is started: no gRPC here)
 Error Plugin::createDevicePlugins() {
     devicePlugins.clear();
-    std::vector<std::string> ids;
-    for (const auto &kv : deviceMap) ids.push_back(kv.first);
-    const std::vector<std::string> names = getDeviceNames(ids);  // :99 for every device id at once
+    std::vector<std::string> ids, vendors;
+    for (size_t d = 0; d < deviceMap.size(); d++) {
+        ids.push_back(deviceMap[d].first);
+        vendors.push_back(xpuClasses[d < deviceClass.size() ? deviceClass[d] : 0].vendor);
+    }
+    const bool dflt = defaultClasses();
+    const std::vector<std::string> names = getDeviceNames(ids, dflt ? nullptr : &vendors);  // :99 for every device id at once
     size_t at = 0;
     for (const auto &kv : deviceMap) {  // :91
         GenericDevicePlugin dp;
+        dp.xpuClass = at < deviceClass.size() ? deviceClass[at] : 0;
+        dp.resourceNamespace = xpuClasses[dp.xpuClass].resourceNamespace;
         for (const std::string &dev : kv.second) dp.devs.push_back(Device{dev, kHealthy});  // :93-98
         std::string devpluginName = names[at++];
         if (devpluginName.empty()) {
@@ -581,10 +692,19 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
         uint64_t now = 0;
         fromSnapshot = bindGeneration(now) && now == snapshotGen_;
     }
+    const bool dflt = defaultClasses();
+    bool haveClass = false;
+    size_t reqClass = 0;  // the class of the request's groups: one plugin serves one class
     for (const std::string &iommuId : devicesIDs) {  // :324
         const std::vector<NvidiaGpuDevice> *nvDevs = nullptr;
         for (const auto &kv : returnedMap) if (kv.first == iommuId) { nvDevs = &kv.second; break; }
         if (!nvDevs) continue;  // unknown group id: empty nvDevs, no error (:327)
+        if (!dflt) {
+            const size_t c = classOfGroup(iommuId);
+            if (haveClass && c != reqClass) return fail("invalid allocation request: devices of more than one class");
+            haveClass = true;
+            reqClass = c;
+        }
         for (const NvidiaGpuDevice &dev : *nvDevs) {
             if (fromSnapshot) {
                 snapshotValidations++;
@@ -595,7 +715,8 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
             std::string iommuGroup, vendor;
             if (!readLink(basePath, dev.addr, "iommu_group", iommuGroup) || iommuGroup != iommuId)  // :329-333
                 return fail("invalid allocation request: unknown device: " + dev.addr);
-            if (!readIDFromFile(basePath, dev.addr, "vendor", vendor) || trimID(vendor) != "10de")  // :334-338
+            const std::string &want = dflt ? std::string("10de") : xpuClasses[dev.xpuClass].vendor;  // the device's class
+            if (!readIDFromFile(basePath, dev.addr, "vendor", vendor) || trimID(vendor) != want)  // :334-338
                 return fail("invalid allocation request: unknown device: " + dev.addr);
             devIndexes.push_back(dev.index);  // :340
         }
@@ -603,15 +724,23 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
     resp.CDIDevices.clear();
     if (!devIndexes.empty()) {  // updateResponseForCDI :274-299; strategy cdi-cri is on (:61)
         std::vector<uint32_t> offs(devIndexes.size() + 1);
-        std::vector<uint8_t> buf(36 * devIndexes.size());
         size_t need = 0;
-        int32_t rc = kxpu_alloc_names(ctx_, devIndexes.data(), devIndexes.size(), buf.data(), buf.size(), offs.data(), &need);
+        int32_t rc;
+        std::vector<uint8_t> buf;
+        if (dflt) {
+            buf.resize(36 * devIndexes.size());
+            rc = kxpu_alloc_names(ctx_, devIndexes.data(), devIndexes.size(), buf.data(), buf.size(), offs.data(), &need);
+        } else {
+            const std::string &kind = xpuClasses[reqClass].cdiKind;
+            buf.resize((kind.size() + 22) * devIndexes.size());
+            rc = kxpu_alloc_names_kind(ctx_, kind.c_str(), devIndexes.data(), devIndexes.size(), buf.data(), buf.size(), offs.data(), &need);
+        }
         if (rc != KXPU_OK) return fail("failed to get allocate response: " + std::string(kxpu_strerror(rc)));
         for (size_t i = 0; i < devIndexes.size(); i++)
             resp.CDIDevices.emplace_back((const char *)buf.data() + offs[i], offs[i + 1] - offs[i]);
     }
     resp.Envs.clear();
-    resp.Envs[kK8SCDIVendorClass] = kCdiVendorClass;  // :348-350 overwrites Envs
+    resp.Envs[kK8SCDIVendorClass] = dflt ? std::string(kCdiVendorClass) : xpuClasses[reqClass].cdiKind;  // :348-350 overwrites Envs
     return Error();
 }
 
@@ -758,6 +887,51 @@ int kxh_gather_fast(const char *base_path, unsigned threads, kxpu_devrec *out, s
     return 0;
 }
 
+// "vendor,driver,namespace,kind,stem;..." -> class list; false on a malformed spec
+static bool parseClasses(const char *spec, std::vector<device_plugin::XpuClass> &out) {
+    out.clear();
+    std::string all(spec), item;
+    size_t pos = 0;
+    while (pos <= all.size()) {
+        size_t semi = all.find(';', pos);
+        if (semi == std::string::npos) semi = all.size();
+        item = all.substr(pos, semi - pos);
+        pos = semi + 1;
+        if (item.empty()) continue;
+        std::vector<std::string> f;
+        size_t a = 0;
+        for (;;) {
+            size_t c = item.find(',', a);
+            f.push_back(item.substr(a, c == std::string::npos ? std::string::npos : c - a));
+            if (c == std::string::npos) break;
+            a = c + 1;
+        }
+        if (f.size() != 5) return false;
+        out.push_back(device_plugin::XpuClass{f[0], f[1], f[2], f[3], f[4]});
+    }
+    return !out.empty();
+}
+
+// CPU only: the raw gather under a class list (fast = the batched / threaded variant)
+int kxh_gather_classes(const char *base_path, const char *classes, int fast, unsigned threads, kxpu_devrec *out, size_t cap,
+                       size_t *n, char *err, size_t errcap) {
+    Plugin p(nullptr);
+    p.basePath = base_path;
+    if (!parseClasses(classes, p.xpuClasses)) { copy_out("malformed class list", err, errcap); return -1; }
+    std::vector<kxpu_devrec> recs;
+    device_plugin::Error e = fast ? p.gatherRecordsFast(recs, threads) : p.gatherRecords(recs);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    *n = recs.size();
+    if (recs.size() > cap) return -2;
+    memcpy(out, recs.data(), recs.size() * sizeof(kxpu_devrec));
+    return 0;
+}
+
+// the class list of a plugin (xpuClasses seam)
+int kxh_set_classes(void *h, const char *classes) {
+    return parseClasses(classes, ((Plugin *)h)->xpuClasses) ? 0 : -1;
+}
+
 void *kxh_new(kxpu_ctx *ctx, const char *base_path, const char *pciids_path, const char *cdi_dir) {
     Plugin *p = new Plugin(ctx);
     p->basePath = base_path;
@@ -801,16 +975,23 @@ int kxh_init(void *h, const char *format, char *json, size_t cap) {
         if (!first) o += ',';
         first = false;
         o += "{\"name\":"; jstr(o, dp.devpluginName);
-        o += ",\"resource\":"; jstr(o, "nvidia.com/" + dp.devpluginName);
+        o += ",\"resource\":"; jstr(o, dp.resourceNamespace + "/" + dp.devpluginName);
         o += ",\"socket\":"; jstr(o, dp.socketPath);
         o += ",\"devs\":[";
         for (size_t i = 0; i < dp.devs.size(); i++) {
             if (i) o += ',';
             o += '['; jstr(o, dp.devs[i].ID); o += ','; jstr(o, dp.devs[i].Health); o += ']';
         }
-        o += "]}";
+        o += "],\"class\":" + std::to_string(dp.xpuClass) + "}";
     }
-    o += "],\"cdiFile\":"; jstr(o, p->lastCdiFile); o += '}';
+    o += "],\"cdiFile\":"; jstr(o, p->lastCdiFile);
+    o += ",\"iommuClass\":[";
+    for (size_t i = 0; i < p->iommuClass.size(); i++) o += (i ? "," : "") + std::to_string(p->iommuClass[i]);
+    o += "],\"deviceClass\":[";
+    for (size_t i = 0; i < p->deviceClass.size(); i++) o += (i ? "," : "") + std::to_string(p->deviceClass[i]);
+    o += "],\"cdiFiles\":[";
+    for (size_t i = 0; i < p->cdiFiles.size(); i++) { if (i) o += ','; jstr(o, p->cdiFiles[i]); }
+    o += "]}";
     return copy_out(o, json, cap);
 }
 

@@ -26,8 +26,9 @@ namespace device_plugin {
 
 // pkg/device_plugin/device_plugin.go:24-28
 struct NvidiaGpuDevice {
-    std::string addr;  // PCI address of device
-    uint64_t index;    // PCI device index on PCI bus
+    std::string addr;    // PCI address of device
+    uint64_t index;      // PCI device index on PCI bus
+    size_t xpuClass = 0; // index into Plugin::xpuClasses of the class this function matched
 };
 
 // Go maps iterate in random order; the canonical order used here (and by the oracle) is
@@ -41,7 +42,9 @@ struct Device {  // pluginapi.Device
     std::string Health;
 };
 struct GenericDevicePlugin {
-    std::string devpluginName;   // resource name suffix: "nvidia.com/<devpluginName>" (:211)
+    std::string devpluginName;   // resource name suffix: "<resourceNamespace>/<devpluginName>" (:211)
+    std::string resourceNamespace = "nvidia.com";  // DevicePluginNamespace (:26), per class (XpuClass)
+    size_t xpuClass = 0;         // index into Plugin::xpuClasses
     std::string socketPath;      // DevicePluginPath + "kata-xpu-<name>.sock" (:76)
     std::string devicePath;      // "/dev/vfio/" (device_plugin.go:105)
     std::vector<Device> devs;
@@ -114,6 +117,18 @@ class BindWatcher {
     uint64_t gen_ = 0;
 };
 
+// One kind of accelerator the plugin serves (the reference hard-codes the NVIDIA one: nvidiaVendorID
+// device_plugin.go:19, the vfio-pci check :156, DevicePluginNamespace / CdiVendorClass
+// generic_device_plugin.go:26,31, the CDI file name device_plugin.go:79).
+struct XpuClass {
+    std::string vendor;             // vendor id as readIDFromFile returns it, e.g. "1002"
+    std::string driver;             // basename of the driver link, e.g. "vfio-pci"
+    std::string resourceNamespace;  // resource = <resourceNamespace>/<device name>
+    std::string cdiKind;            // CDI kind of this class's spec file and Allocate names
+    std::string cdiFileStem;        // <cdiConfigPath><cdiFileStem>.yaml|.json
+};
+XpuClass defaultXpuClass();  // {"10de", "vfio-pci", "nvidia.com", "nvidia.com/gpu", "cdi-vfio-xxxx"}
+
 class Plugin {
   public:
     // ---- seams (device_plugin.go:36-39, generic_device_plugin.go:34)
@@ -129,6 +144,12 @@ class Plugin {
     // unhealthy watcher) falls back to the live reads for that request.  bindGeneration is a seam: by
     // default it asks the BindWatcher (started on first use), tests replace it.
     bool snapshotValidation = false;
+    // The accelerator classes served.  The default (one NVIDIA class) runs exactly the reference's code paths;
+    // any other list goes through kxpu_classify_rules / kxpu_cdi_emit_kind / kxpu_alloc_names_kind.  Classes must
+    // be distinct (vendor, driver) pairs, at most KXPU_MAX_RULES.  Socket names stay kata-xpu-<name>.sock, so two
+    // classes whose devices get the same name collide like two NVIDIA device ids with the same name do in the
+    // reference (generic_device_plugin.go:76); nothing resolves that.
+    std::vector<XpuClass> xpuClasses{defaultXpuClass()};
     std::function<bool(uint64_t &generation)> bindGeneration;
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
 
@@ -137,6 +158,9 @@ class Plugin {
     OrderedMap<std::vector<std::string>> deviceMap;     // device id -> iommu groups
     std::vector<GenericDevicePlugin> devicePlugins;
     std::string lastCdiFile;
+    // class of every iommuMap / deviceMap entry (same positions); all 0 with the default class list
+    std::vector<size_t> iommuClass, deviceClass;
+    std::vector<std::string> cdiFiles;  // files the last generateCDISpec wrote, one per class
 
     explicit Plugin(kxpu_ctx *ctx);
     ~Plugin();
@@ -148,7 +172,9 @@ class Plugin {
     // device_plugin.go:208-259: parse-once table + batched lookup + sanitiser on the GPU (S2)
     std::string getDeviceName(const std::string &deviceID);
     // the same for a batch of ids: one kxpu_lookup + one kxpu_names (device_plugin.go:99 for every id of deviceMap)
-    std::vector<std::string> getDeviceNames(const std::vector<std::string> &deviceIDs);
+    // vendors == nullptr: every id is an NVIDIA device id (the reference); else vendors[i] is the vendor id of deviceIDs[i]
+    std::vector<std::string> getDeviceNames(const std::vector<std::string> &deviceIDs,
+                                            const std::vector<std::string> *vendors = nullptr);
     // device_plugin.go:55-80 + cdi/spec.go:85-127: emit on the GPU, host writes the file (S3)
     Error generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, const std::string &format = "YAML");
     // device_plugin.go:83-112: per device id device lists + plugin objects (S4); nothing is started
@@ -168,6 +194,9 @@ class Plugin {
     kxpu_ctx *ctx_;
     kxpu_table *table_ = nullptr;
     Error ensureTable();
+    bool defaultClasses() const;
+    size_t classOfGroup(const std::string &group) const;
+    Error generateCDISpecClasses(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, int32_t fmt);
     // first use: kxpu_pciids_join on pinned buffers = file -> table -> row handles of `keys` in one call
     Error loadAndJoin(const std::vector<uint32_t> &keys, std::vector<int32_t> &rows);
     BindWatcher bindWatcher_;

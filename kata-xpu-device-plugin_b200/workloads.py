@@ -123,6 +123,46 @@ def cfg3_records(present_keys, n=1 << 20, seed=1):
     return recs
 
 
+XPU_VENDORS = (0x10de, 0x1002, 0x8086, 0x15b3, 0x1d0f)
+
+
+def xpu_records(present_keys, n=1 << 20, seed=4):
+    """cfg3's shape for a node with accelerators of several vendors: vendor uniform over XPU_VENDORS, each drawing
+    device ids from its own pci.ids rows; 2% of the records of 10de and 1002 take a device id that both vendors
+    list (the same id string under two vendors); driver 60% vfio-pci, 10% nvidia, 10% amdgpu, 20% unbound
+    (unreadable link); iommu group = bdf>>3, so one group can hold functions of different vendors."""
+    rng = np.random.default_rng(seed)
+    present_keys = np.asarray(present_keys, dtype=np.uint32)
+    recs = np.zeros(n, dtype=DEVREC_DTYPE)
+    recs["bdf"] = enumerate_bdfs(n).view("S16").reshape(n)
+    vendors = np.array(XPU_VENDORS, dtype=np.int64)
+    vendor = vendors[rng.integers(0, len(vendors), n)]
+    dev = np.zeros(n, np.int64)
+    ids = {}
+    for v in XPU_VENDORS:
+        ids[v] = (present_keys[(present_keys >> 16) == v] & 0xFFFF).astype(np.int64)
+        sel = vendor == v
+        dev[sel] = ids[v][rng.integers(0, len(ids[v]), int(sel.sum()))]
+    shared = np.intersect1d(ids[0x10de], ids[0x1002])
+    assert len(shared), "pci.ids lists no device id under both 10de and 1002"
+    both = ((vendor == 0x10de) | (vendor == 0x1002)) & (rng.random(n) < 0.02)
+    dev[both] = shared[0]
+    recs["vendor_txt"] = _id_text(vendor)
+    recs["device_txt"] = _id_text(dev)
+    recs["vendor_len"] = 7
+    recs["device_len"] = 7
+    r = rng.random(n)
+    drv = np.where(r < 0.6, b"vfio-pci", np.where(r < 0.7, b"nvidia", np.where(r < 0.8, b"amdgpu", b""))).astype("S16")
+    recs["driver"] = drv
+    recs["flags"] = np.where(r >= 0.8, REC_DRIVER_ERR, 0).astype(np.uint8)
+    recs["iommu_group"] = (np.arange(n, dtype=np.int64) >> 3).astype(np.uint32)
+    return recs
+
+
+XPU_RULES = [(b"10de", b"vfio-pci"), (b"1002", b"vfio-pci"), (b"8086", b"vfio-pci"), (b"15b3", b"vfio-pci"),
+             (b"1d0f", b"vfio-pci")]
+
+
 def cfg1_record():
     """One mocked VFIO NVIDIA GPU (SURVEY.md 8(d) cfg1)."""
     recs = np.zeros(1, dtype=DEVREC_DTYPE)
