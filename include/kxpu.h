@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 3
+#define KXPU_ABI_VERSION 4
 
 /* status codes */
 #define KXPU_OK             0
@@ -329,6 +329,66 @@ typedef struct kxpu_xpu_rule {
 int32_t kxpu_classify_rules(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs,
                             size_t n, kxpu_classify_out *out, uint8_t *dev_rule /* [n] */);
 
+/* ------------------------------------------------- S1/S4 for mediated vGPUs */
+
+/* One entry under /sys/bus/mdev/devices (the reference's README TODO "To support vGPUs", README.md:34-39), raw
+ * bytes as the host gathered them with the reference's read semantics (readIDFromFile = data[2:] with '\n'
+ * trimmed, readLink = basename), entries in lexical order (the order filepath.Walk gives the PCI walk,
+ * device_plugin.go:132).  Each entry <uuid> is a symlink into its parent PCI device's directory.  128 bytes, a
+ * multiple of 16: the classify kernel reads a record with eight 16-byte vector loads. */
+typedef struct kxpu_mdevrec {
+    char     uuid[36];             /* entry name; anything but a 36-byte name is stored as 36 NUL bytes     */
+    char     parent[16];           /* basename of the parent directory (its PCI address), NUL padded        */
+    uint8_t  parent_vendor_txt[8]; /* first 8 bytes of <uuid>/../vendor                                     */
+    char     driver[16];           /* basename of the mdev's `driver` link, NUL padded                      */
+    uint8_t  type_name[40];        /* first 40 bytes of <uuid>/mdev_type/name                               */
+    uint32_t iommu_group;          /* basename of the mdev's `iommu_group` link, decimal                    */
+    uint8_t  vendor_len;           /* length of the parent's vendor file (a file over 8 bytes: a failed read) */
+    uint8_t  name_len;             /* length of the type name file (0..40)                                  */
+    uint8_t  flags;                /* KXPU_REC_VENDOR_ERR / _DRIVER_ERR / _IOMMU_ERR / _IS_DIR / _NAME_ERR  */
+    uint8_t  reserved0;
+    uint32_t reserved1;
+} kxpu_mdevrec;
+#define KXPU_REC_NAME_ERR 0x20u /* reading mdev_type/name failed (kxpu_mdevrec only)                       */
+
+/* kxpu_classify for mediated devices (vGPUs).  The semantics follow the shape of kubevirt-gpu-device-plugin, the
+ * model the reference names, and keep the rest of this plugin's model: device ID = IOMMU group, one busIndex per
+ * walk, CDI names <kind>=<index>.
+ *   - a record is a CANDIDATE for rule r when it is not a directory, its uuid is a canonical lowercase UUID
+ *     (8-4-4-4-12 hex digits [0-9a-f] with '-' between), read_id(parent_vendor_txt) equals rules[r].vendor, driver
+ *     equals rules[r].driver (the matching of kxpu_classify_rules, "vendor" meaning the parent's vendor) and the
+ *     vendor, driver and iommu_group reads succeeded;
+ *   - the TYPE KEY of a record plays the part of the PCI `device` file: type_name[0..name_len) with the bytes
+ *     "\t\n\v\f\r " trimmed from both ends, every ' ' replaced by '_', then every byte outside [A-Za-z0-9_.-]
+ *     deleted.  It is at most 40 bytes and is the resource-name suffix (kubevirt: "GRID T4-1Q" -> GRID_T4-1Q);
+ *   - a group comes into existence only at a candidate whose name read succeeded and whose type key is non-empty
+ *     (the "device read works" rule of device_plugin.go:162-170); later members of an existing group are
+ *     accepted without it;
+ *   - grouping and indexing are kxpu_classify_rules': a group belongs to its first good record and that record's
+ *     rule, busIndex counts accepted records over all rules in one walk, the iommuMap is a CSR in walk order;
+ *   - a deviceMap entry is keyed by (rule of the group's first member, type key), entries in first-seen order.
+ *     Two raw names with the same type key share one entry (one resource).
+ * Domain restrictions; a record outside them is skipped like the corresponding read error, so this call never
+ * returns KXPU_E_UNSUPPORTED:
+ *   - name_len > 40 (a longer name file) counts as KXPU_REC_NAME_ERR;
+ *   - vendor_len > 8 counts as KXPU_REC_VENDOR_ERR;
+ *   - iommu_group must be the canonical decimal basename of the link and below 4294967295 (the host marks
+ *     anything else KXPU_REC_IOMMU_ERR; iommu_group = 0xFFFFFFFF counts as that error here too);
+ *   - parent is at most 15 bytes over [0-9a-f:.] (the host marks anything else KXPU_REC_VENDOR_ERR: the parent
+ *     cannot be named in a CDI spec).
+ * Outputs: `out` is filled with kxpu_classify_rules' meaning, EXCEPT dev_ids: here dev_ids[d] is the index of the
+ * first record (lowest index) that is a candidate of any rule and carries entry d's type key, so the host reads
+ * the type name (kxpu_mdev_names) and the UUID from its own records.  dev_rule as in kxpu_classify_rules.
+ * Invalid rule lists return KXPU_E_INVALID, as in kxpu_classify_rules. */
+int32_t kxpu_classify_mdev(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_mdevrec *recs,
+                           size_t n, kxpu_classify_out *out, uint8_t *dev_rule /* [n] */);
+
+/* The type keys (see kxpu_classify_mdev) of records recs[rec_idx[j]], j < k, with kxpu_names' two-call sizing:
+ * key j occupies out[offsets[j] .. offsets[j+1]), *need receives the total.  A record whose name read failed
+ * (KXPU_REC_NAME_ERR or name_len > 40) yields an empty key.  rec_idx[j] >= n is KXPU_E_INVALID. */
+int32_t kxpu_mdev_names(kxpu_ctx *ctx, const kxpu_mdevrec *recs, size_t n, const uint32_t *rec_idx, size_t k,
+                        uint8_t *out, size_t cap, uint32_t *offsets /* [k+1] */, size_t *need);
+
 /* ------------------------------------------------------- S3: CDI spec emit */
 
 /* One accepted device as generateCDISpec sees it (device_plugin.go:59-76). 32 bytes. */
@@ -363,6 +423,38 @@ int32_t kxpu_cdi_emit(kxpu_ctx *ctx, int32_t format, const kxpu_cdidev *devs, si
  * Kinds up to 22 bytes run on the same kernel configuration as kxpu_cdi_emit; longer ones on a variant
  * with a larger per-device fragment bound (fewer CTAs per SM, DESIGN.md K6). */
 int32_t kxpu_cdi_emit_kind(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_cdidev *devs, size_t n,
+                           uint8_t *out, size_t cap, size_t *len);
+
+/* One accepted vGPU as its CDI spec names it.  64 bytes. */
+typedef struct kxpu_mdevcdi {
+    char     uuid[36];      /* the mdev's UUID, canonical lowercase form                     */
+    uint32_t iommu_group;   /* the mdev's own IOMMU group: /dev/vfio/<g>                      */
+    char     parent[16];    /* PCI address of the parent device, NUL padded                   */
+    uint64_t index;         /* busIndex                                                       */
+} kxpu_mdevcdi;
+
+/* The CDI spec of a vGPU class: kxpu_cdi_emit_kind's document (same head, tail, device order, zero-device form
+ * and kind domain, KXPU_E_UNSUPPORTED outside it) with one annotation more per device.  The annotations, in
+ * sorted key order for both encoders (yaml.v3 and encoding/json sort map keys; these four sort the same either
+ * way):
+ *   attach-pci: "true"
+ *   bdf: <parent address>             (yaml.v3's isBase60Float quoting, as for kxpu_cdi_emit)
+ *   cdi.k8s.io/vfio<g>: <kind>=<index>
+ *   mdev: <uuid>
+ * and the device node is /dev/vfio/<g> with g = iommu_group.  A uuid outside the canonical lowercase form
+ * (8-4-4-4-12 over [0-9a-f], '-' between) or a parent that is empty or holds a byte outside [0-9a-f:.] is
+ * KXPU_E_UNSUPPORTED.
+ * A canonical UUID is always written as it is:
+ *   - YAML: it has exactly four '-' and 32 hex digits.  yaml.v3's resolve reads a plain scalar as int / float
+ *     only when it is [-+]?digits (with an optional 0x / 0o / 0b prefix, '_' separators) or a float of the form
+ *     [-+]?(\.[0-9]+|[0-9]+(\.[0-9]*)?)([eE][-+]?[0-9]+)? -- none has a '-' after the first byte; as a
+ *     timestamp only in the forms 2006-01-02 ... which need a 4-digit group first (the UUID has 8 before its first
+ *     '-'); never as bool / null (whole words: true, false, yes, no, on, off, y, n, null, ~) and never as base 60
+ *     (that needs ':').  Its first byte is a hex digit, not an indicator, and it holds no ':', '#', space or
+ *     quote, so the encoder emits it plain (a UUID of only decimal digits and '-', e.g.
+ *     12345678-1234-1234-1234-123456789012, stays plain too).
+ *   - JSON: it holds no '"', '\\', control byte, '<', '>' or '&', so encoding/json escapes nothing. */
+int32_t kxpu_cdi_emit_mdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_mdevcdi *devs, size_t n,
                            uint8_t *out, size_t cap, size_t *len);
 
 /* ------------------------------------------------------ S5: Allocate names */

@@ -268,3 +268,84 @@ func (k *kxpu) allocNamesKind(kind string, idx []uint64) ([]string, error) {
 	}
 	return out, err
 }
+
+// vGPUs (mediated devices): a vGPU class is an xpuClass whose Vendor is the parent PCI device's vendor and whose
+// Driver is the mdev's driver.  The walk of /sys/bus/mdev/devices fills one C.kxpu_mdevrec per entry.
+
+// S1 for the mdev walk: classifyRules' outputs, except that dids[d] is the index of the first record carrying
+// entry d's type key; typeKeys returns the keys themselves.
+func (k *kxpu) classifyMdev(classes []xpuClass, recs []C.kxpu_mdevrec) (accept, gids, goff, gmem []uint32, dids []uint64,
+	doff, dgrp []uint32, devRule []uint8, err error) {
+	n := len(recs)
+	accept, gids, goff, gmem = make([]uint32, n), make([]uint32, n), make([]uint32, n+1), make([]uint32, n)
+	dids, doff, dgrp, devRule = make([]uint64, n), make([]uint32, n+1), make([]uint32, n), make([]uint8, n)
+	if n == 0 {
+		return
+	}
+	rules := make([]C.kxpu_xpu_rule, len(classes))
+	for i, c := range classes {
+		for j := 0; j < len(c.Vendor) && j < len(rules[i].vendor); j++ {
+			rules[i].vendor[j] = C.char(c.Vendor[j])
+		}
+		for j := 0; j < len(c.Driver) && j < len(rules[i].driver); j++ {
+			rules[i].driver[j] = C.char(c.Driver[j])
+		}
+	}
+	var pin runtime.Pinner
+	defer pin.Unpin()
+	for _, p := range []*uint32{&accept[0], &gids[0], &goff[0], &gmem[0], &doff[0], &dgrp[0]} {
+		pin.Pin(p)
+	}
+	pin.Pin(&dids[0])
+	var out C.kxpu_classify_out
+	out.accept_index = (*C.uint32_t)(unsafe.Pointer(&accept[0]))
+	out.group_ids = (*C.uint32_t)(unsafe.Pointer(&gids[0]))
+	out.group_off = (*C.uint32_t)(unsafe.Pointer(&goff[0]))
+	out.group_members = (*C.uint32_t)(unsafe.Pointer(&gmem[0]))
+	out.dev_ids = (*C.uint64_t)(unsafe.Pointer(&dids[0]))
+	out.dev_off = (*C.uint32_t)(unsafe.Pointer(&doff[0]))
+	out.dev_groups = (*C.uint32_t)(unsafe.Pointer(&dgrp[0]))
+	var rp *C.kxpu_xpu_rule
+	if len(rules) > 0 {
+		rp = &rules[0]
+	}
+	err = kxCheck(k.ctx, "kxpu_classify_mdev", C.kxpu_classify_mdev(k.ctx, rp, C.size_t(len(rules)), &recs[0], C.size_t(n), &out,
+		(*C.uint8_t)(unsafe.Pointer(&devRule[0]))))
+	gids, goff, gmem = gids[:out.n_groups], goff[:out.n_groups+1], gmem[:out.n_accepted]
+	dids, doff, dgrp, devRule = dids[:out.n_devids], doff[:out.n_devids+1], dgrp[:out.n_groups], devRule[:out.n_devids]
+	return
+}
+
+// The type keys (resource-name suffixes) of recs[idx[j]].
+func (k *kxpu) typeKeys(recs []C.kxpu_mdevrec, idx []uint32) ([]string, error) {
+	if len(idx) == 0 || len(recs) == 0 {
+		return nil, nil
+	}
+	offs := make([]C.uint32_t, len(idx)+1)
+	buf := make([]byte, 40*len(idx)+1)
+	var need C.size_t
+	err := kxCheck(k.ctx, "kxpu_mdev_names", C.kxpu_mdev_names(k.ctx, &recs[0], C.size_t(len(recs)),
+		(*C.uint32_t)(unsafe.Pointer(&idx[0])), C.size_t(len(idx)), (*C.uint8_t)(unsafe.Pointer(&buf[0])), C.size_t(len(buf)),
+		&offs[0], &need))
+	out := make([]string, len(idx))
+	for j := range idx {
+		out[j] = string(buf[offs[j]:offs[j+1]])
+	}
+	return out, err
+}
+
+// S3 for one vGPU class: the CDI document with the mdev annotation per device.
+func (k *kxpu) cdiEmitMdev(format int, kind string, devs []C.kxpu_mdevcdi) ([]byte, error) {
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	var p *C.kxpu_mdevcdi
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	var n C.size_t
+	C.kxpu_cdi_emit_mdev(k.ctx, C.int32_t(format), ck, p, C.size_t(len(devs)), nil, 0, &n) // sizing call
+	buf := make([]byte, n+1)
+	err := kxCheck(k.ctx, "kxpu_cdi_emit_mdev", C.kxpu_cdi_emit_mdev(k.ctx, C.int32_t(format), ck, p, C.size_t(len(devs)),
+		(*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n))
+	return buf[:n], err
+}

@@ -18,7 +18,7 @@ FMT_YAML, FMT_JSON = 0, 1
 T_PARSE, T_FINALIZE, T_LOOKUP, T_NAMES, T_CLASSIFY, T_EMIT, T_MERGE, T_RESOLVE, T_COUNT = 0, 1, 2, 3, 4, 5, 6, 7, 8
 COMM_ID_BYTES = 128
 
-REC_VENDOR_ERR, REC_DRIVER_ERR, REC_IOMMU_ERR, REC_DEVICE_ERR, REC_IS_DIR = 1, 2, 4, 8, 16
+REC_VENDOR_ERR, REC_DRIVER_ERR, REC_IOMMU_ERR, REC_DEVICE_ERR, REC_IS_DIR, REC_NAME_ERR = 1, 2, 4, 8, 16, 32
 
 DEVREC_DTYPE = np.dtype([("bdf", "S16"), ("vendor_txt", "u1", (8,)), ("device_txt", "u1", (8,)),
                          ("driver", "S16"), ("iommu_group", "<u4"), ("vendor_len", "u1"),
@@ -28,6 +28,12 @@ CDIDEV_DTYPE = np.dtype([("bdf", "S16"), ("iommu_group", "<u4"), ("reserved", "<
 RULE_DTYPE = np.dtype([("vendor", "S8"), ("driver", "S16"), ("reserved", "<u4", (2,))])  # kxpu_xpu_rule
 assert DEVREC_DTYPE.itemsize == 64 and CDIDEV_DTYPE.itemsize == 32 and RULE_DTYPE.itemsize == 32
 MAX_RULES = 16
+# kxpu_mdevrec / kxpu_mdevcdi (vGPUs on the mdev bus)
+MDEVREC_DTYPE = np.dtype([("uuid", "S36"), ("parent", "S16"), ("parent_vendor_txt", "u1", (8,)), ("driver", "S16"),
+                          ("type_name", "u1", (40,)), ("iommu_group", "<u4"), ("vendor_len", "u1"), ("name_len", "u1"),
+                          ("flags", "u1"), ("reserved0", "u1"), ("reserved1", "<u4")])
+MDEVCDI_DTYPE = np.dtype([("uuid", "S36"), ("iommu_group", "<u4"), ("parent", "S16"), ("index", "<u8")])
+assert MDEVREC_DTYPE.itemsize == 128 and MDEVCDI_DTYPE.itemsize == 64
 
 # every symbol include/kxpu.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -39,6 +45,7 @@ ABI_SYMBOLS = [
     "kxpu_pciids_load_sharded", "kxpu_pciids_join_sharded", "kxpu_plan_shards", "kxpu_ctx_create_multi", "kxpu_multi_destroy",
     "kxpu_multi_size", "kxpu_multi_ctx", "kxpu_multi_pciids_join", "kxpu_classify", "kxpu_cdi_emit", "kxpu_alloc_names",
     "kxpu_lw_encode", "kxpu_classify_rules", "kxpu_cdi_emit_kind", "kxpu_alloc_names_kind",
+    "kxpu_classify_mdev", "kxpu_mdev_names", "kxpu_cdi_emit_mdev",
     "kxpu_pciids_full_load_device", "kxpu_full_free", "kxpu_full_export", "kxpu_full_lookup",
 ]
 
@@ -124,6 +131,9 @@ def load_library():
         "kxpu_cdi_emit_kind": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_alloc_names_kind": (i32, [vp, C.c_char_p, vp, sz, vp, sz, vp, C.POINTER(sz)]),
         "kxpu_lw_encode": (i32, [vp, vp, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_classify_mdev": (i32, [vp, vp, sz, vp, sz, C.POINTER(ClassifyOut), vp]),
+        "kxpu_mdev_names": (i32, [vp, vp, sz, vp, sz, vp, sz, vp, C.POINTER(sz)]),
+        "kxpu_cdi_emit_mdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_pciids_full_load_device": (i32, [vp, vp, sz, vp, C.POINTER(vp)]),
         "kxpu_full_free": (i32, [vp, vp]),
         "kxpu_full_export": (i32, [vp, vp, i32, vp, vp, sz, C.POINTER(C.c_uint32)]),
@@ -414,6 +424,58 @@ class Kxpu:
                     group_ids=arrs["group_ids"][:g], group_off=arrs["group_off"][:g + 1],
                     group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
                     dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g], dev_rule=dev_rule[:d])
+
+    def classify_mdev(self, rules, recs):
+        """kxpu_classify_mdev over MDEVREC_DTYPE records: classify_rules' dict, except that dev_ids[d] is the index
+        of the first candidate record carrying entry d's type key."""
+        ra = rules_array(rules)
+        recs = np.ascontiguousarray(recs)
+        assert recs.dtype == MDEVREC_DTYPE
+        n = len(recs)
+        arrs = dict(accept_index=np.empty(n, np.uint32), group_ids=np.empty(n, np.uint32),
+                    group_off=np.empty(n + 1, np.uint32), group_members=np.empty(n, np.uint32),
+                    dev_ids=np.empty(n, np.uint64), dev_off=np.empty(n + 1, np.uint32),
+                    dev_groups=np.empty(n, np.uint32))
+        dev_rule = np.empty(max(n, 1), np.uint8)
+        out = ClassifyOut(**{k: v.ctypes.data for k, v in arrs.items()})
+        self._chk(self.L.kxpu_classify_mdev(self.ctx, _ptr(ra) if len(ra) else None, len(ra), _ptr(recs) if n else None, n,
+                                            C.byref(out), _ptr(dev_rule)))
+        g, d, a = out.n_groups, out.n_devids, out.n_accepted
+        return dict(accept_index=arrs["accept_index"], n_accepted=a, n_groups=g, n_devids=d,
+                    group_ids=arrs["group_ids"][:g], group_off=arrs["group_off"][:g + 1],
+                    group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
+                    dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g], dev_rule=dev_rule[:d])
+
+    def mdev_names(self, recs, idx):
+        """kxpu_mdev_names: (blob, offsets) of the type keys of recs[idx], with the two-call sizing."""
+        recs = np.ascontiguousarray(recs)
+        assert recs.dtype == MDEVREC_DTYPE
+        idx = np.ascontiguousarray(idx, dtype=np.uint32)
+        offs = np.empty(len(idx) + 1, np.uint32)
+        need = C.c_size_t(0)
+        rp = _ptr(recs) if len(recs) else None
+        rc = self.L.kxpu_mdev_names(self.ctx, rp, len(recs), _ptr(idx), len(idx), None, 0, _ptr(offs), C.byref(need))
+        if rc not in (KXPU_OK, E_NOSPACE):
+            self._chk(rc)
+        out = np.empty(max(need.value, 1), np.uint8)
+        self._chk(self.L.kxpu_mdev_names(self.ctx, rp, len(recs), _ptr(idx), len(idx), _ptr(out), need.value, _ptr(offs),
+                                         C.byref(need)))
+        return out[:need.value].tobytes(), offs
+
+    def cdi_emit_mdev(self, fmt, devs, kind):
+        """kxpu_cdi_emit_mdev: the CDI spec of a vGPU class (MDEVCDI_DTYPE devices, kind bytes or str)."""
+        devs = np.ascontiguousarray(devs)
+        assert devs.dtype == MDEVCDI_DTYPE
+        kb = _kind(kind)
+        need = C.c_size_t(0)
+        dp = _ptr(devs) if len(devs) else None
+        rc = self.L.kxpu_cdi_emit_mdev(self.ctx, fmt, kb, dp, len(devs), None, 0, C.byref(need))
+        if rc not in (KXPU_OK, E_NOSPACE):
+            self._chk(rc)
+        out = np.empty(max(need.value, 1), np.uint8)
+        got = C.c_size_t(0)
+        self._chk(self.L.kxpu_cdi_emit_mdev(self.ctx, fmt, kb, dp, len(devs), _ptr(out), need.value, C.byref(got)))
+        return out[:got.value].tobytes()
 
     def cdi_emit(self, fmt, devs, kind=None):
         """kind=None: kxpu_cdi_emit (kind nvidia.com/gpu); else kxpu_cdi_emit_kind with that CDI kind (bytes or str)."""

@@ -14,6 +14,9 @@
 //   iommuMap CSR  = accepted records stably sorted by group ordinal -> LSD radix sort
 //   deviceMap     = groups keyed by the device id of their first member, ids ordered by
 //                   first appearance; CSR by a second stable sort.
+// kxpu_classify_mdev: the candidate kernel reads 128-byte mdev records and writes each candidate's type key; a
+// name-intern pass maps every key to the first candidate carrying it (hash table, keys compared byte for byte);
+// the device-id key becomes (rule << 48 | that record's index).  Everything from k_accept_scan on is shared.
 // Launches: reset | candidates | accept + both scans (single pass, decoupled look-back) | per-group device ids | device-id
 // first-seen scan over the groups | sort pairs + all digit histograms | <= 4 radix passes, each ONE
 // kernel for both sorts (per-tile ranking + per-digit look-back, "onesweep") | CSR boundaries.
@@ -21,6 +24,7 @@
 #include <utility>
 
 #include "common.cuh"
+#include "mdev.cuh"
 #include "scan.cuh"
 
 namespace kxclass {
@@ -30,6 +34,7 @@ constexpr unsigned long long EMPTY64 = 0xFFFFFFFFFFFFFFFFull;
 
 struct __align__(16) GSlot { uint32_t key, first, ord, pad; };                // iommu group -> first good record, ordinal
 struct __align__(16) DSlot { unsigned long long key; uint32_t first, ord; };  // device id string -> first group-first record, ordinal
+struct __align__(16) ISlot { unsigned long long tag; uint32_t first, pad; };   // type key: hash << 32 | some record with it; first such record
 
 constexpr int C_THREADS = 256;
 constexpr int C_ITEMS = 8;
@@ -56,7 +61,15 @@ struct Work {
     unsigned long long *dev_ids;
     // kxpu_classify_rules only (NULL otherwise): rule of record i, rule of device-map entry d
     uint8_t *rrule, *dev_rule;
+    // kxpu_classify_mdev only: the records, per-record type keys (48 bytes: 40 key bytes, zero padded, length in
+    // byte 47), intern slot of each record (EMPTY32: no key to intern) and the intern table
+    const kxpu_mdevrec *mrecs;
+    uint4 *keybuf;
+    uint32_t *islot;
+    ISlot *itab;
+    uint32_t icap, ishift;
 };
+enum { MODE_NV = 0, MODE_RULES = 1, MODE_MDEV = 2 };
 
 // The rule list of kxpu_classify_rules as k_candidates compares it: per rule the vendor id bytes with the id
 // length in bits 56-63 (the same packing as read_id's result), and the driver as two 64-bit words with
@@ -171,6 +184,97 @@ __global__ void __launch_bounds__(256) k_candidates_rules(const Work W, const __
     candidates<true>(W, R);
 }
 
+// pass 1 of kxpu_classify_mdev: candidates, group table, gfirst (a group starts at a candidate with a non-empty type
+// key), and the type key of every such candidate into keybuf for k_intern.  One 128-byte record per thread, eight
+// vector loads; the key is assembled in this thread's 48-byte row of shared memory.
+__global__ void __launch_bounds__(256) k_candidates_mdev(const Work W, const __grid_constant__ RuleTable R) {
+    __shared__ __align__(16) uint8_t skey[256][48];
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= W.n) return;
+    const uint4 *rp = reinterpret_cast<const uint4 *>(W.mrecs + i);
+    uint4 q[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) q[k] = rp[k];
+    const uint32_t uw[9] = {q[0].x, q[0].y, q[0].z, q[0].w, q[1].x, q[1].y, q[1].z, q[1].w, q[2].x};  // uuid[36]
+    const uint2 vtxt = make_uint2(q[3].y, q[3].z);                                 // parent_vendor_txt @52
+    const unsigned long long drv0 = ((unsigned long long)q[4].x << 32) | q[3].w;   // driver @60
+    const unsigned long long drv1 = ((unsigned long long)q[4].z << 32) | q[4].y;
+    const uint32_t nw[10] = {q[4].w, q[5].x, q[5].y, q[5].z, q[5].w, q[6].x, q[6].y, q[6].z, q[6].w, q[7].x};  // type_name @76
+    const uint32_t group = q[7].y;
+    const uint32_t vlen = q[7].z & 0xffu, nlen = (q[7].z >> 8) & 0xffu, fl = (q[7].z >> 16) & 0xffu;
+    unsigned long long vid;
+    uint32_t vl;
+    const bool vok = read_id(reinterpret_cast<const uint8_t *>(&vtxt), vlen, vid, vl);
+    const unsigned long long vkey = vid | ((unsigned long long)vl << 56);
+    bool match = false;
+    uint32_t rule = 0;
+#pragma unroll
+    for (uint32_t r = 0; r < KXPU_MAX_RULES; r++) {
+        if (r < R.n && vkey == R.vend[r] && (drv0 & R.m0[r]) == R.d0[r] && (drv1 & R.m1[r]) == R.d1[r]) {
+            match = true;
+            rule = r;
+        }
+    }
+    const bool cand = !(fl & (KXPU_REC_IS_DIR | KXPU_REC_VENDOR_ERR | KXPU_REC_DRIVER_ERR | KXPU_REC_IOMMU_ERR)) && vok && match &&
+                      group != EMPTY32 && kxmdev::uuid_ok(uw);
+    uint8_t *row = skey[threadIdx.x];
+    uint4 *row4 = reinterpret_cast<uint4 *>(row);
+    row4[0] = row4[1] = row4[2] = make_uint4(0u, 0u, 0u, 0u);
+    const bool nread = !(fl & KXPU_REC_NAME_ERR) && nlen <= kxmdev::NAME_MAX_BYTES;
+    const uint32_t klen = nread ? kxmdev::type_key(nw, nlen, [&](uint32_t p, uint8_t c) { row[p] = c; }) : 0u;
+    const bool nok = klen != 0u;
+    uint32_t slot = EMPTY32;
+    if (cand) {
+        slot = ginsert(W, group);
+        if (nok && i < __ldcg(&W.gtab[slot].first)) atomicMin(&W.gtab[slot].first, i);
+    }
+    W.gslot[i] = slot;
+    W.rrule[i] = (uint8_t)rule;
+    W.islot[i] = cand && nok ? 0u : EMPTY32;
+    if (cand && nok) {
+        row[47] = (uint8_t)klen;
+        uint4 *kb = W.keybuf + 3 * (size_t)i;
+        kb[0] = row4[0]; kb[1] = row4[1]; kb[2] = row4[2];
+    }
+}
+
+__device__ __forceinline__ bool key_eq(const uint4 &a, const uint4 &b) { return a.x == b.x && a.y == b.y && a.z == b.z && a.w == b.w; }
+
+// pass 1b of kxpu_classify_mdev: intern the type keys.  A slot holds (hash << 32 | some record with the key), claimed by
+// CAS; a hash hit compares the 48 key bytes with that record's.  The slot's `first` is the lowest record with the key
+// (atomicMin).  Like the device-id table the intern table starts small: a probe run of 512 flags it (totals[3] bit 2)
+// and the host runs again with both tables at full size.
+__global__ void __launch_bounds__(256) k_intern(const Work W) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= W.n || W.islot[i] == EMPTY32) return;
+    const uint4 *kp = W.keybuf + 3 * (size_t)i;
+    const uint4 k0 = kp[0], k1 = kp[1], k2 = kp[2];
+    unsigned long long hv = 0x9E3779B97F4A7C15ull;
+    const uint32_t kw[12] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z, k1.w, k2.x, k2.y, k2.z, k2.w};
+#pragma unroll
+    for (int k = 0; k < 12; k++) { hv = (hv ^ kw[k]) * 0xff51afd7ed558ccdull; hv ^= hv >> 29; }
+    const uint32_t h = (uint32_t)(hv >> 32);
+    const unsigned long long tag = ((unsigned long long)h << 32) | i;
+    uint32_t slot = h >> W.ishift;
+    for (uint32_t step = 0; step < 512u; step++) {
+        unsigned long long t = __ldcg(&W.itab[slot].tag);
+        if (t == EMPTY64) {
+            t = atomicCAS(&W.itab[slot].tag, EMPTY64, tag);
+            if (t == EMPTY64) t = tag;
+        }
+        if ((uint32_t)(t >> 32) == h) {
+            const uint4 *op = W.keybuf + 3 * (size_t)(uint32_t)t;
+            if (key_eq(op[0], k0) && key_eq(op[1], k1) && key_eq(op[2], k2)) {
+                if (i < __ldcg(&W.itab[slot].first)) atomicMin(&W.itab[slot].first, i);
+                W.islot[i] = slot;
+                return;
+            }
+        }
+        slot = (slot + 1) & (W.icap - 1);
+    }
+    atomicOr(&W.totals[3], 4u);
+}
+
 // pass 2: accept / group-first flags of a 2048-record tile, both exclusive scans in the same kernel
 // (two look-backs, warp 0 and warp 1), busIndex out, group ordinals out, device-id table insert.
 __global__ void __launch_bounds__(C_THREADS) k_accept_scan(const Work W) {
@@ -250,12 +354,21 @@ __global__ void __launch_bounds__(C_THREADS) k_accept_scan(const Work W) {
 // attributed to the device id of its FIRST member, device_plugin.go:162-170) -> device-id table, first-seen minimum.
 // Kept out of k_accept_scan: there the chain record read -> table insert -> minimum ran serially per record in a
 // divergent loop (6 % issue utilisation); here every group is an independent thread.
-// RULES: the device-id key is (rule of the first member) << 48 | device id.
-template <bool RULES>
+// MODE_RULES: the device-id key is (rule of the first member) << 48 | device id; MODE_MDEV: (rule of the first member)
+// << 48 | first record with its type key.
+template <int MODE>
 __global__ void __launch_bounds__(256) k_groups(const Work W) {
     const uint32_t o = blockIdx.x * blockDim.x + threadIdx.x;
     if (o >= W.totals[1]) return;
     const uint32_t i = W.grp_rec[o];
+    if (MODE == MODE_MDEV) {
+        W.group_ids[o] = reinterpret_cast<const uint32_t *>(W.mrecs + i)[29];  // iommu_group @116
+        const unsigned long long key = ((unsigned long long)W.rrule[i] << 48) | W.itab[W.islot[i]].first;
+        const uint32_t ds = dinsert(W, key);
+        if (i < __ldcg(&W.dtab[ds].first)) atomicMin(&W.dtab[ds].first, i);
+        W.grp_dslot[o] = ds;
+        return;
+    }
     const uint32_t *rw = reinterpret_cast<const uint32_t *>(W.recs + i);
     const uint2 dq = make_uint2(rw[6], rw[7]);  // device_txt
     const uint32_t dlen = (rw[13] >> 8) & 0xffu;
@@ -263,7 +376,7 @@ __global__ void __launch_bounds__(256) k_groups(const Work W) {
     unsigned long long did;
     uint32_t dl;
     read_id(reinterpret_cast<const uint8_t *>(&dq), dlen, did, dl);
-    if (RULES) did |= (unsigned long long)W.rrule[i] << 48;
+    if (MODE == MODE_RULES) did |= (unsigned long long)W.rrule[i] << 48;
     const uint32_t ds = dinsert(W, did);
     // a few hot device ids own most groups: same-address atomics run at ~1 per ns, so only a group that can
     // still lower the minimum issues one
@@ -477,25 +590,27 @@ static uint32_t bits_for(uint32_t n) {
     return b;
 }
 
-// R == nullptr: kxpu_classify (the NVIDIA constants); else the rule list of kxpu_classify_rules
-static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
-                             uint8_t *dev_rule, bool small_dtab, bool *retry);
+// R == nullptr: kxpu_classify (the NVIDIA constants); else the rule list of kxpu_classify_rules, or with mdev of
+// kxpu_classify_mdev (recs then points at kxpu_mdevrec records)
+static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
+                             bool mdev, uint8_t *dev_rule, bool small_dtab, bool *retry);
 
-static int32_t classify_run(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
+static int32_t classify_run(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R, bool mdev,
                             uint8_t *dev_rule) {
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
     bool retry = false;
-    int32_t rc = classify_once(ctx, recs, n, out, R, dev_rule, true, &retry);
-    if (retry) rc = classify_once(ctx, recs, n, out, R, dev_rule, false, &retry);  // more distinct device ids than the small table holds
+    int32_t rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, true, &retry);
+    // more distinct device ids (or type keys) than the small tables hold
+    if (retry) rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, false, &retry);
     return rc;
 }
 
 extern "C" int32_t kxpu_classify(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out) {
     if (!ctx || !out || (n && !recs)) return KXPU_E_INVALID;
     if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
-    return classify_run(ctx, recs, n, out, nullptr, nullptr);
+    return classify_run(ctx, recs, n, out, nullptr, false, nullptr);
 }
 
 // a NUL-padded field: length of the text before the first NUL, -1 when a non-NUL byte follows that NUL
@@ -507,11 +622,8 @@ static int field_len(const char *f, int cap) {
     return l;
 }
 
-extern "C" int32_t kxpu_classify_rules(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs,
-                                       size_t n, kxpu_classify_out *out, uint8_t *dev_rule) {
-    if (!ctx || !out || (n && !recs) || !rules || n_rules == 0 || n_rules > KXPU_MAX_RULES) return KXPU_E_INVALID;
-    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
-    RuleTable R;
+// the rule list of kxpu_classify_rules / kxpu_classify_mdev -> R; KXPU_E_INVALID with a message when it is invalid
+static int32_t rule_table(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, RuleTable &R) {
     memset(&R, 0, sizeof R);
     R.n = (uint32_t)n_rules;
     for (size_t r = 0; r < n_rules; r++) {
@@ -538,11 +650,32 @@ extern "C" int32_t kxpu_classify_rules(kxpu_ctx *ctx, const kxpu_xpu_rule *rules
         for (int k = 0; k <= dl; k++) m[k >> 3] |= 0xffull << (8 * (k & 7));  // the driver's bytes and its NUL
         R.d0[r] = d[0]; R.d1[r] = d[1]; R.m0[r] = m[0]; R.m1[r] = m[1];
     }
-    return classify_run(ctx, recs, n, out, &R, dev_rule);
+    return KXPU_OK;
 }
 
-static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
-                             uint8_t *dev_rule, bool small_dtab, bool *retry) {
+extern "C" int32_t kxpu_classify_rules(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs,
+                                       size_t n, kxpu_classify_out *out, uint8_t *dev_rule) {
+    if (!ctx || !out || (n && !recs) || !rules || n_rules == 0 || n_rules > KXPU_MAX_RULES) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    RuleTable R;
+    const int32_t rc = rule_table(ctx, rules, n_rules, R);
+    if (rc != KXPU_OK) return rc;
+    return classify_run(ctx, recs, n, out, &R, false, dev_rule);
+}
+
+extern "C" int32_t kxpu_classify_mdev(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_mdevrec *recs,
+                                      size_t n, kxpu_classify_out *out, uint8_t *dev_rule) {
+    static_assert(sizeof(kxpu_mdevrec) == 128 && offsetof(kxpu_mdevrec, iommu_group) == 116, "kxpu_mdevrec layout");
+    if (!ctx || !out || (n && !recs) || !rules || n_rules == 0 || n_rules > KXPU_MAX_RULES) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    RuleTable R;
+    const int32_t rc = rule_table(ctx, rules, n_rules, R);
+    if (rc != KXPU_OK) return rc;
+    return classify_run(ctx, recs, n, out, &R, true, dev_rule);
+}
+
+static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
+                             bool mdev, uint8_t *dev_rule, bool small_dtab, bool *retry) {
     *retry = false;
     out->n_accepted = out->n_groups = out->n_devids = 0;
     if (n == 0) {
@@ -569,17 +702,21 @@ static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, k
     // one arena; [ff-region | zero-region | rest]
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
+    const uint32_t icap = mdev ? dcap : 0u;  // the intern table grows with the device-id table
     const size_t o_gtab = take((size_t)gcap * sizeof(GSlot)), o_dtab = take((size_t)dcap * sizeof(DSlot));
+    const size_t o_itab = mdev ? take((size_t)icap * sizeof(ISlot)) : 0;
     const size_t ff_bytes = off;
     const size_t o_totals = take(16), o_ghist = take(2 * 4 * 256 * 4);
     const size_t zero_words = (off - ff_bytes) / 4;
-    const size_t o_recs = take(n * sizeof(kxpu_devrec));
+    const size_t rec_bytes = mdev ? sizeof(kxpu_mdevrec) : sizeof(kxpu_devrec);
+    const size_t o_recs = take(n * rec_bytes);
     const size_t o_gslot = take(n * 4 + 64), o_grec = take(n * 4), o_gds = take(n * 4);
     const size_t o_ak = take(n * 4), o_av = take(n * 4), o_ak2 = take(n * 4), o_av2 = take(n * 4);
     const size_t o_bk = take(n * 4), o_bv = take(n * 4), o_bk2 = take(n * 4), o_bv2 = take(n * 4);
     const size_t o_acc_idx = take(n * 4 + 64), o_gids = take(n * 4), o_goff = take((n + 1) * 4);
     const size_t o_dids = take(n * 8), o_doff = take((n + 1) * 4);
     const size_t o_rrule = R ? take(n) : 0, o_drule = R ? take(n) : 0;
+    const size_t o_keys = mdev ? take(n * 48) : 0, o_islot = mdev ? take(n * 4) : 0;
     KxScratch sc(ctx);
     uint8_t *b = nullptr;
     KX_CUDA(ctx, sc.alloc((void **)&b, off));
@@ -600,8 +737,13 @@ static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, k
     W.accept_index = (uint32_t *)(b + o_acc_idx); W.group_ids = (uint32_t *)(b + o_gids);
     W.group_off = (uint32_t *)(b + o_goff); W.dev_ids = (unsigned long long *)(b + o_dids); W.dev_off = (uint32_t *)(b + o_doff);
     if (R) { W.rrule = b + o_rrule; W.dev_rule = b + o_drule; }
+    if (mdev) {
+        W.mrecs = (const kxpu_mdevrec *)(b + o_recs);
+        W.keybuf = (uint4 *)(b + o_keys); W.islot = (uint32_t *)(b + o_islot);
+        W.itab = (ISlot *)(b + o_itab); W.icap = icap; W.ishift = 32 - dlg;
+    }
 
-    cudaMemcpyAsync(b + o_recs, recs, n * sizeof(kxpu_devrec), cudaMemcpyHostToDevice, ctx->stream);
+    cudaMemcpyAsync(b + o_recs, recs, n * rec_bytes, cudaMemcpyHostToDevice, ctx->stream);
     const unsigned g = (N + 255) / 256;
     uint32_t *ak = W.ak, *av = W.av, *ak2 = (uint32_t *)(b + o_ak2), *av2 = (uint32_t *)(b + o_av2);
     uint32_t *bk = W.bk, *bv = W.bv, *bk2 = (uint32_t *)(b + o_bk2), *bv2 = (uint32_t *)(b + o_bv2);
@@ -609,11 +751,16 @@ static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, k
         KxTimer tm(ctx, KXPU_T_CLASSIFY);
         k_reset<<<std::min<unsigned>((unsigned)((ff_bytes / 16 + 255) / 256), 8u * ctx->sm_count), 256, 0, ctx->stream>>>(
             (uint4 *)b, ff_bytes / 16, W.totals, (uint32_t)zero_words);
-        if (R) k_candidates_rules<<<g, 256, 0, ctx->stream>>>(W, *R);
+        if (mdev) {
+            k_candidates_mdev<<<g, 256, 0, ctx->stream>>>(W, *R);
+            k_intern<<<g, 256, 0, ctx->stream>>>(W);
+            ctx->launches++;
+        } else if (R) k_candidates_rules<<<g, 256, 0, ctx->stream>>>(W, *R);
         else k_candidates<<<g, 256, 0, ctx->stream>>>(W);
         k_accept_scan<<<c_tiles, C_THREADS, 0, ctx->stream>>>(W);
-        if (R) k_groups<true><<<g, 256, 0, ctx->stream>>>(W);
-        else k_groups<false><<<g, 256, 0, ctx->stream>>>(W);
+        if (mdev) k_groups<MODE_MDEV><<<g, 256, 0, ctx->stream>>>(W);
+        else if (R) k_groups<MODE_RULES><<<g, 256, 0, ctx->stream>>>(W);
+        else k_groups<MODE_NV><<<g, 256, 0, ctx->stream>>>(W);
         k_devfirst_scan<<<c_tiles, C_THREADS, 0, ctx->stream>>>(W);
         k_pairs<<<std::min<unsigned>(g, 4u * ctx->sm_count), 256, 0, ctx->stream>>>(W, passes);
         ctx->launches += 6;
@@ -639,9 +786,9 @@ static int32_t classify_once(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n, k
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
     int32_t rc = KXPU_OK;
     if (e != cudaSuccess) { KX_SET_ERR(ctx, "classify failed: %s", cudaGetErrorString(e)); rc = KXPU_E_CUDA; }
-    else if ((h[3] & 2u) && small_dtab) { *retry = true; return KXPU_E_CAPACITY; }
+    else if ((h[3] & 6u) && small_dtab) { *retry = true; return KXPU_E_CAPACITY; }
     else if (h[3] & 1u) { KX_SET_ERR(ctx, "classify: record outside the supported domain (group 0xffffffff or id file > 8 bytes)"); rc = KXPU_E_UNSUPPORTED; }
-    else if (h[3] & 2u) { KX_SET_ERR(ctx, "classify: device-id table overflow"); rc = KXPU_E_CAPACITY; }
+    else if (h[3] & 6u) { KX_SET_ERR(ctx, "classify: device-id or type-key table overflow"); rc = KXPU_E_CAPACITY; }
     if (rc == KXPU_OK) {
         const uint32_t na = h[0], ng = h[1], nd = h[2];
         out->n_accepted = na; out->n_groups = ng; out->n_devids = nd;

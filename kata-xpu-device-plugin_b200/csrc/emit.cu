@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "mdev.cuh"
 #include "scan.cuh"
 
 namespace kxemit {
@@ -29,6 +30,9 @@ constexpr int MAX_FRAG = 368;  // upper bound of one fragment: literals (<= 267 
                                // rest of TileSmem this keeps a CTA under 56.7 KB: four CTAs per SM, the 512 tiles of cfg5 are ONE
                                // wave.  Holds every kind up to 22 bytes.
 constexpr int MAX_FRAG_LONG = 416;  // kinds of 23..63 bytes: 62.7 KB per CTA, three CTAs per SM
+constexpr int MAX_FRAG_MDEV = 480;  // kxpu_cdi_emit_mdev, every kind: the PCI bound + the mdev annotation (<= 20 + 36 bytes);
+                                    // 69.8 KB per CTA, three CTAs per SM
+constexpr int LAYOUT_PCI = 0, LAYOUT_MDEV = 1;  // kxpu_cdidev / kxpu_mdevcdi
 constexpr int POOL_MAX = 640;
 constexpr int KIND_MAX = 63;
 
@@ -60,13 +64,22 @@ constexpr int KIND_MAX = 63;
 #define KX_JHB "\",\n  \"devices\": [\n"
 #define KX_JT "  ],\n  \"containerEdits\": {}\n}"
 #define KX_JEB "\",\n  \"devices\": null,\n  \"containerEdits\": {}\n}"
+// kxpu_cdi_emit_mdev: after "kind=<index>" comes the mdev annotation (literal 4 below, then the uuid) and literal 9,
+// which is the PCI literal 4
+#define KX_YM "\n      mdev: "
+#define KX_JM "\",\n        \"mdev\": \""
 // part k = before[k] (+ kind + after[k] when after[k] != NULL); parts 0-5 are the literals, 6 the document head,
-// 7 the tail, 8 the whole document for zero devices (Devices stays nil, cdi/spec.go:42-49)
-struct Parts { const char *before[9], *after[9]; };
-static const Parts h_yaml_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_Y4, KX_Y5, KX_YHA, KX_YT, KX_YHA},
-                                   {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB}};
-static const Parts h_json_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_J4, KX_J5, KX_JHA, KX_JT, KX_JHA},
-                                   {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB}};
+// 7 the tail, 8 the whole document for zero devices (Devices stays nil, cdi/spec.go:42-49), 9 the literal after the
+// mdev uuid (NULL: none)
+struct Parts { const char *before[10], *after[10]; };
+static const Parts h_yaml_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_Y4, KX_Y5, KX_YHA, KX_YT, KX_YHA, nullptr},
+                                   {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB, nullptr}};
+static const Parts h_json_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_J4, KX_J5, KX_JHA, KX_JT, KX_JHA, nullptr},
+                                   {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB, nullptr}};
+static const Parts h_yaml_mdev_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_YM, KX_Y5, KX_YHA, KX_YT, KX_YHA, KX_Y4},
+                                        {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB, nullptr}};
+static const Parts h_json_mdev_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_JM, KX_J5, KX_JHA, KX_JT, KX_JHA, KX_J4},
+                                        {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB, nullptr}};
 static const char *kDefaultKind = "nvidia.com/gpu";  // CdiVendorClass, generic_device_plugin.go:31
 
 // The supported kind domain (include/kxpu.h): "vendor/class", <= 63 bytes; vendor = letter [A-Za-z0-9_.-]*
@@ -90,7 +103,7 @@ static bool kind_ok(const char *kind) {
 }
 
 static std::string part_text(const Parts &P, int k, const char *kind) {
-    std::string s = P.before[k];
+    std::string s = P.before[k] ? P.before[k] : "";
     if (P.after[k]) { s += kind; s += P.after[k]; }
     return s;
 }
@@ -141,15 +154,15 @@ __device__ __forceinline__ bool bdf_charset_ok(const uint8_t *s, uint32_t len) {
 }
 
 struct EmitParams {
-    const kxpu_cdidev *devs;
+    const void *devs;         // kxpu_cdidev[n] or kxpu_mdevcdi[n]
     uint32_t n;
-    uint16_t off[8], len[8];  // literal k / head (6) / tail (7) inside the pool
+    uint16_t off[9], len[9];  // literal k / head (6) / tail (7) / the literal after the mdev uuid (8) inside the pool
     uint32_t pool_len, lit_total;
     uint8_t *out;
     unsigned long long *state;  // tile status words (scan.cuh look-back)
     uint32_t epoch;
     unsigned long long *total_out;
-    uint32_t *flags;
+    uint32_t *flags;          // [0]: a bdf outside [0-9a-f:.], [1]: a uuid outside the canonical form
     uint8_t pool[POOL_MAX];   // literals | head | tail, built on the host for the call's kind
 };
 
@@ -165,7 +178,7 @@ struct TileSmem {
     uint32_t tile_total;
 };
 
-template <int FMT, int MAXF>
+template <int FMT, int MAXF, int LAYOUT>
 __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constant__ EmitParams E) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
     TileSmem<MAXF> &S = *reinterpret_cast<TileSmem<MAXF> *>(smem_raw);
@@ -177,19 +190,33 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
     // ---- fragment lengths and variable fields: one thread per device
     uint32_t flen = 0;
     if (tid < TILE && i0 + tid < E.n) {
-        const uint4 *p = reinterpret_cast<const uint4 *>(E.devs + i0 + tid);
-        const uint4 q0 = p[0], q1 = p[1];
-        const uint8_t *bdf = reinterpret_cast<const uint8_t *>(&q0);
-        const uint32_t group = q1.x;
-        const unsigned long long index = ((unsigned long long)q1.w << 32) | q1.z;
+        uint4 bq;  // the bdf / parent address
+        uint32_t group;
+        unsigned long long index;
+        if (LAYOUT == LAYOUT_PCI) {
+            const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const kxpu_cdidev *>(E.devs) + i0 + tid);
+            const uint4 q0 = p[0], q1 = p[1];
+            bq = q0;
+            group = q1.x;
+            index = ((unsigned long long)q1.w << 32) | q1.z;
+        } else {  // uuid[36] | iommu_group | parent[16] | index
+            const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const kxpu_mdevcdi *>(E.devs) + i0 + tid);
+            const uint4 q0 = p[0], q1 = p[1], q2 = p[2], q3 = p[3];
+            const uint32_t uw[9] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x};
+            if (!kxmdev::uuid_ok(uw)) E.flags[1] = 1u;
+            bq = make_uint4(q2.z, q2.w, q3.x, q3.y);
+            group = q2.y;
+            index = ((unsigned long long)q3.w << 32) | q3.z;
+        }
+        const uint8_t *bdf = reinterpret_cast<const uint8_t *>(&bq);
         const uint32_t bl = bdf_len16(bdf), il = dec_len(index), gl = dec_len(group);
         if (!bdf_charset_ok(bdf, bl)) E.flags[0] = 1u;
         const bool quoted = FMT == KXPU_FMT_YAML && is_base60(bdf, bl);
         dec_write(index, il, S.idx[tid]);
         dec_write(group, gl, S.grp[tid]);
-        *reinterpret_cast<uint4 *>(S.bdf[tid]) = q0;
+        *reinterpret_cast<uint4 *>(S.bdf[tid]) = bq;
         S.meta[tid] = il | (gl << 8) | (bl << 16) | ((quoted ? 1u : 0u) << 24);
-        flen = E.lit_total + 2u * il + 2u * gl + bl + (quoted ? 2u : 0u);
+        flen = E.lit_total + 2u * il + 2u * gl + bl + (quoted ? 2u : 0u) + (LAYOUT == LAYOUT_MDEV ? 36u : 0u);
         if (FMT == KXPU_FMT_JSON) flen += (i0 + tid + 1u < E.n) ? 2u : 1u;  // ",\n" between devices, "\n" after the last
     }
     // ---- scan of the 128 lengths (threads >= TILE contribute 0)
@@ -242,7 +269,14 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
             if (FMT == KXPU_FMT_YAML && quoted) { if (lane == 0) dst[o] = (uint8_t)'"'; o += 1u; }
         };
         lit(0); var(S.idx[d], il); lit(1); quote(); var(S.bdf[d], bl); quote(); lit(2); var(S.grp[d], gl);
-        lit(3); var(S.idx[d], il); lit(4); var(S.grp[d], gl); lit(5);
+        lit(3); var(S.idx[d], il); lit(4);
+        if (LAYOUT == LAYOUT_MDEV) {  // the uuid straight from the device array (L2), then the PCI literal 4
+            const uint8_t *u = static_cast<const uint8_t *>(E.devs) + (size_t)(i0 + d) * sizeof(kxpu_mdevcdi);
+            for (uint32_t l = lane; l < 36u; l += 32u) dst[o + l] = u[l];
+            o += 36u;
+            lit(8);
+        }
+        var(S.grp[d], gl); lit(5);
         if (FMT == KXPU_FMT_JSON) {
             const bool more = i0 + d + 1u < E.n;
             if (lane == 0) { if (more) { dst[o] = (uint8_t)','; dst[o + 1] = (uint8_t)'\n'; } else dst[o] = (uint8_t)'\n'; }
@@ -291,6 +325,28 @@ __global__ void __launch_bounds__(256) k_alloc_write(const unsigned long long *_
     dec_write(v, dec_len(v), dst + P.len);
 }
 
+// ------------------------------------------------------------------ vGPU type keys (kxpu_mdev_names)
+// one gathered 128-byte record per thread: the key length, then the key bytes at their offset
+__device__ __forceinline__ uint32_t mdev_key(const kxpu_mdevrec *rec, uint8_t *dst) {
+    const uint4 *rp = reinterpret_cast<const uint4 *>(rec);
+    const uint4 q4 = rp[4], q5 = rp[5], q6 = rp[6], q7 = rp[7];
+    const uint32_t nw[10] = {q4.w, q5.x, q5.y, q5.z, q5.w, q6.x, q6.y, q6.z, q6.w, q7.x};  // type_name @76
+    const uint32_t nlen = (q7.z >> 8) & 0xffu, fl = (q7.z >> 16) & 0xffu;
+    if ((fl & KXPU_REC_NAME_ERR) || nlen > kxmdev::NAME_MAX_BYTES) return 0u;
+    return kxmdev::type_key(nw, nlen, [&](uint32_t p, uint8_t c) { if (dst) dst[p] = c; });
+}
+__global__ void __launch_bounds__(256) k_mdev_name_len(const kxpu_mdevrec *__restrict__ recs, uint32_t n, uint32_t *__restrict__ lens) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > n) return;
+    lens[i] = i < n ? mdev_key(recs + i, nullptr) : 0u;
+}
+__global__ void __launch_bounds__(256) k_mdev_name_write(const kxpu_mdevrec *__restrict__ recs, uint32_t n,
+                                                         const uint32_t *__restrict__ offs, uint8_t *__restrict__ out) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    mdev_key(recs + i, out + offs[i]);
+}
+
 // ------------------------------------------------------------------ ListAndWatchResponse
 // repeated Device devices = 1; Device { string ID = 1; string health = 2; }
 __global__ void __launch_bounds__(256) k_lw_len(const uint32_t *__restrict__ groups, const uint8_t *__restrict__ healthy,
@@ -321,17 +377,19 @@ __global__ void __launch_bounds__(256) k_lw_write(const uint32_t *__restrict__ g
 
 using namespace kxemit;
 
-template <int FMT, int MAXF>
+template <int FMT, int MAXF, int LAYOUT>
 static void emit_launch(kxpu_ctx *ctx, uint32_t tiles, const EmitParams &E) {
-    k_cdi_fused<FMT, MAXF><<<tiles, EMIT_THREADS, sizeof(TileSmem<MAXF>), ctx->stream>>>(E);
+    k_cdi_fused<FMT, MAXF, LAYOUT><<<tiles, EMIT_THREADS, sizeof(TileSmem<MAXF>), ctx->stream>>>(E);
 }
 
-static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_cdidev *devs, size_t n, uint8_t *out,
-                        size_t cap, size_t *len) {
+// mdev: devs is kxpu_mdevcdi[n], else kxpu_cdidev[n]
+static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const void *devs, size_t n, uint8_t *out,
+                        size_t cap, size_t *len, bool mdev = false) {
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
-    const Parts &parts = format == KXPU_FMT_YAML ? h_yaml_parts : h_json_parts;
+    const Parts &parts = mdev ? (format == KXPU_FMT_YAML ? h_yaml_mdev_parts : h_json_mdev_parts)
+                              : (format == KXPU_FMT_YAML ? h_yaml_parts : h_json_parts);
     if (n == 0) {  // Devices stays nil: yaml "devices: []", json "devices": null (cdi/spec.go:42-49)
         const std::string doc = part_text(parts, 8, kind);
         *len = doc.size();
@@ -341,42 +399,50 @@ static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const k
     }
     static bool attr_done = false;
     if (!attr_done) {
-        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAX_FRAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem<MAX_FRAG>));
-        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_JSON, MAX_FRAG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem<MAX_FRAG>));
-        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAX_FRAG_LONG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAX_FRAG, LAYOUT_PCI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)sizeof(TileSmem<MAX_FRAG>));
+        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_JSON, MAX_FRAG, LAYOUT_PCI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)sizeof(TileSmem<MAX_FRAG>));
+        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAX_FRAG_LONG, LAYOUT_PCI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)sizeof(TileSmem<MAX_FRAG_LONG>));
-        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_JSON, MAX_FRAG_LONG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_JSON, MAX_FRAG_LONG, LAYOUT_PCI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)sizeof(TileSmem<MAX_FRAG_LONG>));
+        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAX_FRAG_MDEV, LAYOUT_MDEV>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)sizeof(TileSmem<MAX_FRAG_MDEV>));
+        cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_JSON, MAX_FRAG_MDEV, LAYOUT_MDEV>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)sizeof(TileSmem<MAX_FRAG_MDEV>));
         attr_done = true;
     }
     EmitParams E;
     memset(&E, 0, sizeof E);
     uint32_t acc = 0;
-    for (int k = 0; k < 8; k++) {
-        const std::string s = part_text(parts, k, kind);
+    for (int k = 0; k < 9; k++) {
+        const std::string s = part_text(parts, k < 8 ? k : 9, kind);  // slot 8 <- part 9 (part 8 is the zero-device document)
         if (acc + s.size() > (size_t)POOL_MAX) return KXPU_E_INVALID;  // the literals grew: POOL_MAX must follow
         memcpy(E.pool + acc, s.data(), s.size());
         E.off[k] = (uint16_t)acc;
         E.len[k] = (uint16_t)s.size();
         acc += E.len[k];
-        if (k < 6) E.lit_total += E.len[k];
+        if (k < 6 || k == 8) E.lit_total += E.len[k];
     }
     E.pool_len = acc;
     const uint32_t N = (uint32_t)n;
     const uint32_t tiles = (N + TILE - 1) / TILE;
-    const uint32_t frag = E.lit_total + 2 * 20 + 2 * 10 + 15 + 2 + 2;  // no fragment is longer
+    const uint32_t frag = E.lit_total + 2 * 20 + 2 * 10 + 15 + 2 + 2 + (mdev ? 36 : 0);  // no fragment is longer
     const size_t bound = (size_t)n * frag + E.len[6] + E.len[7] + 64;
-    // kinds up to 22 bytes fit the four-CTAs-per-SM tile, longer ones take the MAX_FRAG_LONG instantiation
+    // kinds up to 22 bytes fit the four-CTAs-per-SM tile, longer ones take the MAX_FRAG_LONG instantiation; every
+    // mdev kind the MAX_FRAG_MDEV one
     const bool long_frag = frag > (uint32_t)MAX_FRAG;
-    if (frag > (uint32_t)MAX_FRAG_LONG) return KXPU_E_INVALID;  // the literals grew: MAX_FRAG_LONG must follow
+    if (frag > (uint32_t)(mdev ? MAX_FRAG_MDEV : MAX_FRAG_LONG)) return KXPU_E_INVALID;  // the literals grew: the bound must follow
+    const size_t dev_bytes = mdev ? sizeof(kxpu_mdevcdi) : sizeof(kxpu_cdidev);
     KxScratch sc(ctx);
-    kxpu_cdidev *d_devs = nullptr;
+    void *d_devs = nullptr;
     uint8_t *d_out = nullptr;
     unsigned long long *d_total = nullptr;
-    KX_CUDA(ctx, sc.alloc((void **)&d_devs, n * sizeof(kxpu_cdidev)));
+    KX_CUDA(ctx, sc.alloc((void **)&d_devs, n * dev_bytes));
     KX_CUDA(ctx, sc.alloc((void **)&d_out, bound));
     KX_CUDA(ctx, sc.alloc((void **)&d_total, 16));
-    cudaMemcpyAsync(d_devs, devs, n * sizeof(kxpu_cdidev), cudaMemcpyHostToDevice, ctx->stream);
+    cudaMemcpyAsync(d_devs, devs, n * dev_bytes, cudaMemcpyHostToDevice, ctx->stream);
     cudaMemsetAsync(d_total, 0, 16, ctx->stream);
     E.devs = d_devs; E.n = N; E.out = d_out; E.total_out = d_total; E.flags = (uint32_t *)(d_total + 1);
     E.state = kx_scan_state(ctx, tiles);
@@ -384,12 +450,15 @@ static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const k
     E.epoch = kx_next_epoch(ctx);
     {
         KxTimer tm(ctx, KXPU_T_EMIT);
-        if (format == KXPU_FMT_YAML) {
-            if (long_frag) emit_launch<KXPU_FMT_YAML, MAX_FRAG_LONG>(ctx, tiles, E);
-            else emit_launch<KXPU_FMT_YAML, MAX_FRAG>(ctx, tiles, E);
+        if (mdev) {
+            if (format == KXPU_FMT_YAML) emit_launch<KXPU_FMT_YAML, MAX_FRAG_MDEV, LAYOUT_MDEV>(ctx, tiles, E);
+            else emit_launch<KXPU_FMT_JSON, MAX_FRAG_MDEV, LAYOUT_MDEV>(ctx, tiles, E);
+        } else if (format == KXPU_FMT_YAML) {
+            if (long_frag) emit_launch<KXPU_FMT_YAML, MAX_FRAG_LONG, LAYOUT_PCI>(ctx, tiles, E);
+            else emit_launch<KXPU_FMT_YAML, MAX_FRAG, LAYOUT_PCI>(ctx, tiles, E);
         } else {
-            if (long_frag) emit_launch<KXPU_FMT_JSON, MAX_FRAG_LONG>(ctx, tiles, E);
-            else emit_launch<KXPU_FMT_JSON, MAX_FRAG>(ctx, tiles, E);
+            if (long_frag) emit_launch<KXPU_FMT_JSON, MAX_FRAG_LONG, LAYOUT_PCI>(ctx, tiles, E);
+            else emit_launch<KXPU_FMT_JSON, MAX_FRAG, LAYOUT_PCI>(ctx, tiles, E);
         }
         KX_LAUNCHED(ctx);
     }
@@ -398,6 +467,7 @@ static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const k
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) { KX_SET_ERR(ctx, "cdi_emit failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
     if ((uint32_t)h[1]) { KX_SET_ERR(ctx, "cdi_emit: bdf outside [0-9a-f:.]"); return KXPU_E_UNSUPPORTED; }
+    if ((uint32_t)(h[1] >> 32)) { KX_SET_ERR(ctx, "cdi_emit_mdev: uuid outside the canonical lowercase form"); return KXPU_E_UNSUPPORTED; }
     const size_t total = (size_t)h[0];
     *len = total;
     if (cap < total || !out) return KXPU_E_NOSPACE;
@@ -420,6 +490,15 @@ extern "C" int32_t kxpu_cdi_emit_kind(kxpu_ctx *ctx, int32_t format, const char 
     if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
     if (!kind_ok(kind)) { KX_SET_ERR(ctx, "cdi_emit_kind: kind is not a CDI vendor/class of at most 63 bytes"); return KXPU_E_UNSUPPORTED; }
     return cdi_emit(ctx, format, kind, devs, n, out, cap, len);
+}
+
+extern "C" int32_t kxpu_cdi_emit_mdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_mdevcdi *devs, size_t n,
+                                      uint8_t *out, size_t cap, size_t *len) {
+    static_assert(sizeof(kxpu_mdevcdi) == 64 && offsetof(kxpu_mdevcdi, parent) == 40, "kxpu_mdevcdi layout");
+    if (!ctx || !len || !kind || (n && !devs) || (format != KXPU_FMT_YAML && format != KXPU_FMT_JSON)) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    if (!kind_ok(kind)) { KX_SET_ERR(ctx, "cdi_emit_mdev: kind is not a CDI vendor/class of at most 63 bytes"); return KXPU_E_UNSUPPORTED; }
+    return cdi_emit(ctx, format, kind, devs, n, out, cap, len, true);
 }
 
 // shared driver of the two "thread per item" emitters
@@ -498,6 +577,30 @@ extern "C" int32_t kxpu_alloc_names_kind(kxpu_ctx *ctx, const char *kind, const 
     if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
     if (!kind_ok(kind)) { KX_SET_ERR(ctx, "alloc_names_kind: kind is not a CDI vendor/class of at most 63 bytes"); return KXPU_E_UNSUPPORTED; }
     return alloc_names(ctx, kind, idx, n, out, cap, offsets, need);
+}
+
+extern "C" int32_t kxpu_mdev_names(kxpu_ctx *ctx, const kxpu_mdevrec *recs, size_t n, const uint32_t *rec_idx, size_t k,
+                                   uint8_t *out, size_t cap, uint32_t *offsets, size_t *need) {
+    if (!ctx || !offsets || (k && (!recs || !rec_idx))) return KXPU_E_INVALID;
+    if (k >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    std::vector<kxpu_mdevrec> pick(k);  // only the k records travel to the device
+    for (size_t j = 0; j < k; j++) {
+        if (rec_idx[j] >= n) { KX_SET_ERR(ctx, "mdev_names: rec_idx[%zu] = %u is not below n = %zu", j, rec_idx[j], n); return KXPU_E_INVALID; }
+        pick[j] = recs[rec_idx[j]];
+    }
+    std::lock_guard<std::mutex> guard(ctx->mu);
+    cudaSetDevice(ctx->device);
+    kx_clear_timings(ctx);
+    if (k == 0) { offsets[0] = 0; if (need) *need = 0; return KXPU_OK; }
+    cudaStream_t st = ctx->stream;
+    return emit_items(
+        ctx, k, k * sizeof(kxpu_mdevrec), pick.data(), nullptr, out, cap, offsets, need,
+        [st](const uint8_t *in, const uint8_t *, uint32_t N, uint32_t *lens) {
+            k_mdev_name_len<<<(N + 1 + 255) / 256, 256, 0, st>>>((const kxpu_mdevrec *)in, N, lens);
+        },
+        [st](const uint8_t *in, const uint8_t *, uint32_t N, const uint32_t *offs, uint8_t *o) {
+            k_mdev_name_write<<<(N + 255) / 256, 256, 0, st>>>((const kxpu_mdevrec *)in, N, offs, o);
+        });
 }
 
 extern "C" int32_t kxpu_lw_encode(kxpu_ctx *ctx, const uint32_t *group_ids, const uint8_t *healthy, size_t n,

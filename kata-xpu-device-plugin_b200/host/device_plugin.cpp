@@ -12,6 +12,8 @@
 
 #include <fcntl.h>
 
+#include <climits>
+
 #include <algorithm>
 #include <cerrno>
 #include <cstdio>
@@ -78,6 +80,7 @@ Plugin::Plugin(kxpu_ctx *ctx) : ctx_(ctx) {
     readLink = readLinkFunc;
     readIDFromFile = readIDFromFileFunc;
     returnIommuMap = [this]() -> const OrderedMap<std::vector<NvidiaGpuDevice>> & { return iommuMap; };
+    returnMdevMap = [this]() -> const OrderedMap<std::vector<MdevDevice>> & { return mdevMap; };
     bindGeneration = [this](uint64_t &generation) {
         if (!bindWatcher_.healthy() && bindWatcher_.start()) return false;
         generation = bindWatcher_.generation();
@@ -442,6 +445,157 @@ Error Plugin::createIommuDeviceMap() {
     return Error();
 }
 
+// ---------------------------------------------------------------------------- vGPUs (mediated devices)
+// canonical decimal below 2^32-1 (the domain of kxpu_mdevrec.iommu_group)
+static bool parseGroup(const std::string &s, uint32_t &v) {
+    if (s.empty() || s.size() > 10 || (s.size() > 1 && s[0] == '0')) return false;
+    unsigned long long x = 0;
+    for (char c : s) {
+        if (c < '0' || c > '9') return false;
+        x = x * 10 + (unsigned)(c - '0');
+    }
+    if (x >= 0xFFFFFFFFull) return false;
+    v = (uint32_t)x;
+    return true;
+}
+
+// One entry of mdevBasePath, read with the reference's read semantics through the seams: the parent's vendor
+// (<uuid>/../vendor), the parent's PCI address (the basename of <uuid>/.. resolved), the `driver` and `iommu_group`
+// links, and mdev_type/name.  A failed read sets its flag and ends the record, like the PCI leaf; a value outside the
+// record's domain counts as that read failing (include/kxpu.h, kxpu_classify_mdev).
+static void mdevRecord(Plugin &p, const std::string &name, bool isDir, kxpu_mdevrec &r) {
+    memset(&r, 0, sizeof r);
+    if (name.size() == sizeof r.uuid) memcpy(r.uuid, name.data(), sizeof r.uuid);  // else 36 NUL bytes: not a candidate
+    if (isDir) { r.flags |= KXPU_REC_IS_DIR; return; }
+    if (name.size() != sizeof r.uuid) return;
+    std::string s;
+    char real[PATH_MAX];
+    const std::string up = p.mdevBasePath + "/" + name + "/..";
+    if (!realpath(up.c_str(), real)) { r.flags |= KXPU_REC_VENDOR_ERR; return; }
+    std::string parent(real);
+    parent = parent.substr(parent.find_last_of('/') + 1);
+    bool pok = !parent.empty() && parent.size() < sizeof r.parent;
+    for (char c : parent) pok = pok && ((c >= '0' && c <= '9') || (c >= 'a' && c <= 'f') || c == ':' || c == '.');
+    if (!pok) {
+        fprintf(stderr, "parent of mdev %s is not a PCI address of at most 15 bytes, mdev skipped: %s\n", name.c_str(), parent.c_str());
+        r.flags |= KXPU_REC_VENDOR_ERR;
+        return;
+    }
+    memcpy(r.parent, parent.data(), parent.size());
+    if (!p.readIDFromFile(p.mdevBasePath, name, "../vendor", s) || !packID(s, r.parent_vendor_txt, r.vendor_len)) {
+        r.flags |= KXPU_REC_VENDOR_ERR;
+        return;
+    }
+    if (!p.readLink(p.mdevBasePath, name, "driver", s)) { r.flags |= KXPU_REC_DRIVER_ERR; return; }
+    memcpy(r.driver, s.data(), std::min<size_t>(s.size(), sizeof r.driver - 1));
+    uint32_t g = 0;
+    if (!p.readLink(p.mdevBasePath, name, "iommu_group", s) || !parseGroup(s, g)) { r.flags |= KXPU_REC_IOMMU_ERR; return; }
+    r.iommu_group = g;
+    if (!p.readIDFromFile(p.mdevBasePath, name, "mdev_type/name", s) || s.size() > sizeof r.type_name) {
+        r.flags |= KXPU_REC_NAME_ERR;
+        return;
+    }
+    memcpy(r.type_name, s.data(), s.size());
+    r.name_len = (uint8_t)s.size();
+}
+
+// The entries of mdevBasePath in lexical order (filepath.Walk's order for the PCI walk).  The mdev bus directory only
+// holds one level of links, so a directory inside it is recorded as such and not descended into.
+Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs) {
+    recs.clear();
+    DIR *d = opendir(mdevBasePath.c_str());
+    if (!d) return fail("Error accessing file path \"" + mdevBasePath + "\": " + strerror(errno));
+    std::vector<std::string> names;
+    while (struct dirent *de = readdir(d)) {
+        if (strcmp(de->d_name, ".") == 0 || strcmp(de->d_name, "..") == 0) continue;
+        names.push_back(de->d_name);
+    }
+    closedir(d);
+    std::sort(names.begin(), names.end());
+    for (const std::string &n : names) {
+        struct stat sb;
+        const bool isDir = lstat((mdevBasePath + "/" + n).c_str(), &sb) == 0 && S_ISDIR(sb.st_mode);
+        kxpu_mdevrec r;
+        mdevRecord(*this, n, isDir, r);
+        recs.push_back(r);
+    }
+    return Error();
+}
+
+Error Plugin::checkVgpuClasses() const {
+    std::vector<const XpuClass *> all;
+    for (const XpuClass &c : xpuClasses) all.push_back(&c);
+    for (const XpuClass &c : vgpuClasses) all.push_back(&c);
+    for (size_t v = xpuClasses.size(); v < all.size(); v++)
+        for (size_t o = 0; o < all.size(); o++)
+            if (o != v && (all[o]->cdiKind == all[v]->cdiKind || all[o]->cdiFileStem == all[v]->cdiFileStem))
+                return fail("vGPU class " + all[v]->vendor + "/" + all[v]->driver + ": CDI kind and file stem must differ from every other class's");
+    if (vgpuClasses.size() > KXPU_MAX_RULES) return fail("more vGPU classes than KXPU_MAX_RULES");
+    return Error();
+}
+
+Error Plugin::createMdevMap() {
+    mdevMap.clear();
+    typeMap.clear();
+    mdevClass.clear();
+    typeClass.clear();
+    if (vgpuClasses.empty()) return Error();  // nothing under mdevBasePath is read
+    Error e = checkVgpuClasses();
+    if (e) return e;
+    std::vector<kxpu_mdevrec> recs;
+    e = gatherMdevRecords(recs);
+    if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // like the PCI walk: an unreadable bus is an empty one
+    const size_t n = recs.size();
+    std::vector<uint32_t> accept(n), gids(n), goff(n + 1), gmem(n), doff(n + 1), dgrp(n);
+    std::vector<uint64_t> dids(n);
+    std::vector<uint8_t> drule(n ? n : 1, 0);
+    kxpu_classify_out out;
+    memset(&out, 0, sizeof out);
+    out.accept_index = accept.data(); out.group_ids = gids.data(); out.group_off = goff.data();
+    out.group_members = gmem.data(); out.dev_ids = dids.data(); out.dev_off = doff.data(); out.dev_groups = dgrp.data();
+    std::vector<kxpu_xpu_rule> rules(vgpuClasses.size());  // one rule per class: rule index == class index
+    for (size_t c = 0; c < vgpuClasses.size(); c++) {
+        memset(&rules[c], 0, sizeof rules[c]);
+        strncpy(rules[c].vendor, vgpuClasses[c].vendor.c_str(), sizeof rules[c].vendor);
+        strncpy(rules[c].driver, vgpuClasses[c].driver.c_str(), sizeof rules[c].driver);
+    }
+    int32_t rc = kxpu_classify_mdev(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data());
+    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify_mdev", rc);
+    std::vector<uint32_t> first(out.n_devids);
+    for (uint32_t d = 0; d < out.n_devids; d++) first[d] = (uint32_t)dids[d];
+    std::vector<uint32_t> koff(first.size() + 1);
+    size_t need = 0;
+    rc = kxpu_mdev_names(ctx_, recs.data(), n, first.data(), first.size(), nullptr, 0, koff.data(), &need);
+    if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, "kxpu_mdev_names", rc);
+    std::vector<uint8_t> keys(need ? need : 1);
+    rc = kxpu_mdev_names(ctx_, recs.data(), n, first.data(), first.size(), keys.data(), need, koff.data(), &need);
+    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_mdev_names", rc);
+    std::map<uint32_t, size_t> groupClass;  // class of a group = the rule of its first member
+    for (uint32_t d = 0; d < out.n_devids; d++)
+        for (uint32_t k = doff[d]; k < doff[d + 1]; k++) groupClass[dgrp[k]] = drule[d];
+    for (uint32_t g = 0; g < out.n_groups; g++) {
+        std::vector<MdevDevice> devs;
+        for (uint32_t k = goff[g]; k < goff[g + 1]; k++) {
+            const kxpu_mdevrec &r = recs[gmem[k]];
+            MdevDevice m{std::string(r.uuid, sizeof r.uuid), std::string(r.parent, strnlen(r.parent, sizeof r.parent)), accept[gmem[k]], 0};
+            const std::string vendor = trimID(std::string((const char *)r.parent_vendor_txt, r.vendor_len));
+            for (size_t c = 0; c < vgpuClasses.size(); c++)
+                if (vgpuClasses[c].vendor == vendor && vgpuClasses[c].driver == std::string(r.driver, strnlen(r.driver, sizeof r.driver)))
+                    m.vgpuClass = c;
+            devs.push_back(std::move(m));
+        }
+        mdevMap.emplace_back(std::to_string(gids[g]), std::move(devs));
+        mdevClass.push_back(groupClass[gids[g]]);
+    }
+    for (uint32_t d = 0; d < out.n_devids; d++) {
+        std::vector<std::string> groups;
+        for (uint32_t k = doff[d]; k < doff[d + 1]; k++) groups.push_back(std::to_string(dgrp[k]));
+        typeMap.emplace_back(std::string((const char *)keys.data() + koff[d], koff[d + 1] - koff[d]), std::move(groups));
+        typeClass.push_back(drule[d]);
+    }
+    return Error();
+}
+
 size_t Plugin::classOfGroup(const std::string &group) const {
     for (size_t g = 0; g < iommuMap.size() && g < iommuClass.size(); g++)
         if (iommuMap[g].first == group) return iommuClass[g];
@@ -643,6 +797,42 @@ Error Plugin::generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m,
     return Error();
 }
 
+// One CDI spec per vGPU class: the mdevs of the class's groups in ascending index; a class without mdevs gets the empty
+// document, like an accelerator class without devices.
+Error Plugin::generateMdevCDISpec(const std::string &format) {
+    mdevCdiFiles.clear();
+    if (vgpuClasses.empty()) return Error();
+    const int32_t fmt = format == "YAML" ? KXPU_FMT_YAML : KXPU_FMT_JSON;
+    std::vector<std::vector<kxpu_mdevcdi>> per(vgpuClasses.size());
+    for (size_t g = 0; g < mdevMap.size(); g++) {
+        for (const MdevDevice &m : mdevMap[g].second) {
+            kxpu_mdevcdi d;
+            memset(&d, 0, sizeof d);
+            memcpy(d.uuid, m.uuid.data(), std::min(m.uuid.size(), sizeof d.uuid));
+            strncpy(d.parent, m.parent.c_str(), sizeof d.parent - 1);
+            d.iommu_group = (uint32_t)strtoul(mdevMap[g].first.c_str(), nullptr, 10);
+            d.index = m.index;
+            per[mdevClass[g]].push_back(d);
+        }
+    }
+    for (size_t c = 0; c < vgpuClasses.size(); c++) {
+        std::vector<kxpu_mdevcdi> &devs = per[c];
+        std::sort(devs.begin(), devs.end(), [](const kxpu_mdevcdi &a, const kxpu_mdevcdi &b) { return a.index < b.index; });
+        const char *kind = vgpuClasses[c].cdiKind.c_str();
+        size_t len = 0;
+        int32_t rc = kxpu_cdi_emit_mdev(ctx_, fmt, kind, devs.data(), devs.size(), nullptr, 0, &len);
+        if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, "kxpu_cdi_emit_mdev", rc);
+        std::vector<uint8_t> doc(len ? len : 1);
+        rc = kxpu_cdi_emit_mdev(ctx_, fmt, kind, devs.data(), devs.size(), doc.data(), len, &len);
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_cdi_emit_mdev", rc);
+        const std::string file_path = cdiConfigPath + vgpuClasses[c].cdiFileStem + (fmt == KXPU_FMT_YAML ? ".yaml" : ".json");
+        bool written = false;
+        writeSpecFile(file_path, doc, len, written);
+        if (written) mdevCdiFiles.push_back(file_path);
+    }
+    return Error();
+}
+
 // createDevicePlugins, device_plugin.go:83-112 (nothing is started: no gRPC here)
 Error Plugin::createDevicePlugins() {
     devicePlugins.clear();
@@ -669,13 +859,28 @@ Error Plugin::createDevicePlugins() {
         dp.socketPath = std::string(kDevicePluginPath) + "kata-xpu-" + devpluginName + ".sock";  // generic:76
         devicePlugins.push_back(std::move(dp));
     }
+    for (size_t t = 0; t < typeMap.size(); t++) {  // one plugin per (vGPU class, type key)
+        GenericDevicePlugin dp;
+        dp.vgpu = true;
+        dp.xpuClass = typeClass[t];
+        dp.resourceNamespace = vgpuClasses[dp.xpuClass].resourceNamespace;
+        for (const std::string &g : typeMap[t].second) dp.devs.push_back(Device{g, kHealthy});
+        dp.devpluginName = typeMap[t].first;
+        dp.devicePath = "/dev/vfio/";  // an mdev has its own IOMMU group and /dev/vfio/<group>
+        dp.socketPath = std::string(kDevicePluginPath) + "kata-xpu-" + dp.devpluginName + ".sock";
+        devicePlugins.push_back(std::move(dp));
+    }
     return Error();
 }
 
 Error Plugin::InitiateDevicePlugin() {
     Error e = createIommuDeviceMap();  // :46
     if (e) return e;
+    e = createMdevMap();
+    if (e) return e;
     e = generateCDISpec(iommuMap);  // :49
+    if (e) return e;
+    e = generateMdevCDISpec();
     if (e) return e;
     return createDevicePlugins();  // :52
 }
@@ -695,10 +900,33 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
     const bool dflt = defaultClasses();
     bool haveClass = false;
     size_t reqClass = 0;  // the class of the request's groups: one plugin serves one class
+    const auto &mdevs = returnMdevMap();
+    bool havePci = false, haveVgpu = false;
+    size_t vgpuClass = 0;
     for (const std::string &iommuId : devicesIDs) {  // :324
+        const std::vector<MdevDevice> *mDevs = nullptr;
+        size_t mg = 0;
+        for (; mg < mdevs.size(); mg++) if (mdevs[mg].first == iommuId) { mDevs = &mdevs[mg].second; break; }
+        if (mDevs) {  // a vGPU group: always live reads (the uevent snapshot only follows PCI binds)
+            const size_t c = mg < mdevClass.size() ? mdevClass[mg] : 0;
+            if (havePci || (haveVgpu && c != vgpuClass)) return fail("invalid allocation request: devices of more than one class");
+            haveVgpu = true;
+            vgpuClass = c;
+            for (const MdevDevice &m : *mDevs) {
+                liveValidations++;
+                std::string iommuGroup, vendor;
+                if (!readLink(mdevBasePath, m.uuid, "iommu_group", iommuGroup) || iommuGroup != iommuId ||
+                    !readIDFromFile(mdevBasePath, m.uuid, "../vendor", vendor) || trimID(vendor) != vgpuClasses[m.vgpuClass].vendor)
+                    return fail("invalid allocation request: unknown device: " + m.uuid);
+                devIndexes.push_back(m.index);
+            }
+            continue;
+        }
         const std::vector<NvidiaGpuDevice> *nvDevs = nullptr;
         for (const auto &kv : returnedMap) if (kv.first == iommuId) { nvDevs = &kv.second; break; }
         if (!nvDevs) continue;  // unknown group id: empty nvDevs, no error (:327)
+        if (haveVgpu) return fail("invalid allocation request: devices of more than one class");
+        havePci = true;
         if (!dflt) {
             const size_t c = classOfGroup(iommuId);
             if (haveClass && c != reqClass) return fail("invalid allocation request: devices of more than one class");
@@ -727,7 +955,11 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
         size_t need = 0;
         int32_t rc;
         std::vector<uint8_t> buf;
-        if (dflt) {
+        if (haveVgpu) {
+            const std::string &kind = vgpuClasses[vgpuClass].cdiKind;
+            buf.resize((kind.size() + 22) * devIndexes.size());
+            rc = kxpu_alloc_names_kind(ctx_, kind.c_str(), devIndexes.data(), devIndexes.size(), buf.data(), buf.size(), offs.data(), &need);
+        } else if (dflt) {
             buf.resize(36 * devIndexes.size());
             rc = kxpu_alloc_names(ctx_, devIndexes.data(), devIndexes.size(), buf.data(), buf.size(), offs.data(), &need);
         } else {
@@ -740,7 +972,9 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
             resp.CDIDevices.emplace_back((const char *)buf.data() + offs[i], offs[i + 1] - offs[i]);
     }
     resp.Envs.clear();
-    resp.Envs[kK8SCDIVendorClass] = dflt ? std::string(kCdiVendorClass) : xpuClasses[reqClass].cdiKind;  // :348-350 overwrites Envs
+    resp.Envs[kK8SCDIVendorClass] = haveVgpu ? vgpuClasses[vgpuClass].cdiKind
+                                    : dflt   ? std::string(kCdiVendorClass)
+                                             : xpuClasses[reqClass].cdiKind;  // :348-350 overwrites Envs
     return Error();
 }
 
@@ -941,11 +1175,42 @@ void *kxh_new(kxpu_ctx *ctx, const char *base_path, const char *pciids_path, con
 }
 void kxh_free(void *h) { delete (Plugin *)h; }
 
+// the vGPU classes of a plugin (vgpuClasses seam), same spec format; "" clears them
+int kxh_set_vgpu_classes(void *h, const char *classes) {
+    Plugin *p = (Plugin *)h;
+    if (!classes[0]) { p->vgpuClasses.clear(); return 0; }
+    return parseClasses(classes, p->vgpuClasses) ? 0 : -1;
+}
+void kxh_set_mdev_base(void *h, const char *path) { ((Plugin *)h)->mdevBasePath = path; }
+// the device path a plugin's health watcher watches (tests point it at a fake /dev/vfio)
+int kxh_set_device_path(void *h, int plugin_index, const char *path) {
+    Plugin *p = (Plugin *)h;
+    if (plugin_index < 0 || (size_t)plugin_index >= p->devicePlugins.size()) return -1;
+    p->devicePlugins[(size_t)plugin_index].devicePath = path;
+    return 0;
+}
+
+// CPU only: the raw mdev gather under a vGPU class list
+int kxh_gather_mdev(const char *mdev_base, const char *classes, kxpu_mdevrec *out, size_t cap, size_t *n, char *err, size_t errcap) {
+    Plugin p(nullptr);
+    p.mdevBasePath = mdev_base;
+    if (!parseClasses(classes, p.vgpuClasses)) { copy_out("malformed class list", err, errcap); return -1; }
+    std::vector<kxpu_mdevrec> recs;
+    device_plugin::Error e = p.gatherMdevRecords(recs);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    *n = recs.size();
+    if (recs.size() > cap) return -2;
+    memcpy(out, recs.data(), recs.size() * sizeof(kxpu_mdevrec));
+    return 0;
+}
+
 // InitiateDevicePlugin + a JSON dump of the resulting state
 int kxh_init(void *h, const char *format, char *json, size_t cap) {
     Plugin *p = (Plugin *)h;
     device_plugin::Error e = p->createIommuDeviceMap();
+    if (!e) e = p->createMdevMap();
     if (!e) e = p->generateCDISpec(p->iommuMap, format);
+    if (!e) e = p->generateMdevCDISpec(format);
     if (!e) e = p->createDevicePlugins();
     if (e) { copy_out(e.message, json, cap); return -1; }
     std::string o = "{\"iommuMap\":[";
@@ -982,7 +1247,7 @@ int kxh_init(void *h, const char *format, char *json, size_t cap) {
             if (i) o += ',';
             o += '['; jstr(o, dp.devs[i].ID); o += ','; jstr(o, dp.devs[i].Health); o += ']';
         }
-        o += "],\"class\":" + std::to_string(dp.xpuClass) + "}";
+        o += "],\"class\":" + std::to_string(dp.xpuClass) + ",\"vgpu\":" + (dp.vgpu ? "true" : "false") + "}";
     }
     o += "],\"cdiFile\":"; jstr(o, p->lastCdiFile);
     o += ",\"iommuClass\":[";
@@ -991,6 +1256,31 @@ int kxh_init(void *h, const char *format, char *json, size_t cap) {
     for (size_t i = 0; i < p->deviceClass.size(); i++) o += (i ? "," : "") + std::to_string(p->deviceClass[i]);
     o += "],\"cdiFiles\":[";
     for (size_t i = 0; i < p->cdiFiles.size(); i++) { if (i) o += ','; jstr(o, p->cdiFiles[i]); }
+    o += "],\"mdevMap\":[";
+    for (size_t g = 0; g < p->mdevMap.size(); g++) {
+        if (g) o += ',';
+        o += '['; jstr(o, p->mdevMap[g].first); o += ",[";
+        for (size_t i = 0; i < p->mdevMap[g].second.size(); i++) {
+            const device_plugin::MdevDevice &m = p->mdevMap[g].second[i];
+            if (i) o += ',';
+            o += '['; jstr(o, m.uuid); o += ','; jstr(o, m.parent);
+            o += ',' + std::to_string(m.index) + ',' + std::to_string(m.vgpuClass) + ']';
+        }
+        o += "]]";
+    }
+    o += "],\"mdevClass\":[";
+    for (size_t i = 0; i < p->mdevClass.size(); i++) o += (i ? "," : "") + std::to_string(p->mdevClass[i]);
+    o += "],\"typeMap\":[";
+    for (size_t t = 0; t < p->typeMap.size(); t++) {
+        if (t) o += ',';
+        o += '['; jstr(o, p->typeMap[t].first); o += ",[";
+        for (size_t i = 0; i < p->typeMap[t].second.size(); i++) { if (i) o += ','; jstr(o, p->typeMap[t].second[i]); }
+        o += "]]";
+    }
+    o += "],\"typeClass\":[";
+    for (size_t i = 0; i < p->typeClass.size(); i++) o += (i ? "," : "") + std::to_string(p->typeClass[i]);
+    o += "],\"mdevCdiFiles\":[";
+    for (size_t i = 0; i < p->mdevCdiFiles.size(); i++) { if (i) o += ','; jstr(o, p->mdevCdiFiles[i]); }
     o += "]}";
     return copy_out(o, json, cap);
 }

@@ -31,6 +31,14 @@ struct NvidiaGpuDevice {
     size_t xpuClass = 0; // index into Plugin::xpuClasses of the class this function matched
 };
 
+// One mediated device (vGPU) of the mdev walk: the mdevMap counterpart of NvidiaGpuDevice
+struct MdevDevice {
+    std::string uuid;      // entry name under mdevBasePath
+    std::string parent;    // PCI address of the parent device
+    uint64_t index;        // busIndex of the mdev walk
+    size_t vgpuClass = 0;  // index into Plugin::vgpuClasses of the class this mdev matched
+};
+
 // Go maps iterate in random order; the canonical order used here (and by the oracle) is
 // first-seen walk order, which is one of the orders the reference can produce.
 template <typename V>
@@ -44,7 +52,8 @@ struct Device {  // pluginapi.Device
 struct GenericDevicePlugin {
     std::string devpluginName;   // resource name suffix: "<resourceNamespace>/<devpluginName>" (:211)
     std::string resourceNamespace = "nvidia.com";  // DevicePluginNamespace (:26), per class (XpuClass)
-    size_t xpuClass = 0;         // index into Plugin::xpuClasses
+    size_t xpuClass = 0;         // index into Plugin::xpuClasses (Plugin::vgpuClasses when vgpu)
+    bool vgpu = false;           // serves one vGPU type (devs are mdev IOMMU groups)
     std::string socketPath;      // DevicePluginPath + "kata-xpu-<name>.sock" (:76)
     std::string devicePath;      // "/dev/vfio/" (device_plugin.go:105)
     std::vector<Device> devs;
@@ -150,6 +159,13 @@ class Plugin {
     // classes whose devices get the same name collide like two NVIDIA device ids with the same name do in the
     // reference (generic_device_plugin.go:76); nothing resolves that.
     std::vector<XpuClass> xpuClasses{defaultXpuClass()};
+    // vGPU classes: mediated devices under mdevBasePath, one resource <resourceNamespace>/<type key> per (class, type
+    // key).  vendor = the parent PCI device's vendor id, driver = the mdev's driver.  Empty (default): nothing under
+    // mdevBasePath is read and every flow is the one above.  A class's cdiKind and cdiFileStem must differ from those
+    // of every other class (xpuClasses and vgpuClasses), else InitiateDevicePlugin fails.
+    std::vector<XpuClass> vgpuClasses;
+    std::string mdevBasePath = "/sys/bus/mdev/devices";
+    std::function<const OrderedMap<std::vector<MdevDevice>> &()> returnMdevMap;
     std::function<bool(uint64_t &generation)> bindGeneration;
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
 
@@ -161,6 +177,11 @@ class Plugin {
     // class of every iommuMap / deviceMap entry (same positions); all 0 with the default class list
     std::vector<size_t> iommuClass, deviceClass;
     std::vector<std::string> cdiFiles;  // files the last generateCDISpec wrote, one per class
+    // the mdev walk: IOMMU group -> mdevs, type key -> groups, and the vGPU class of every entry (same positions)
+    OrderedMap<std::vector<MdevDevice>> mdevMap;
+    OrderedMap<std::vector<std::string>> typeMap;
+    std::vector<size_t> mdevClass, typeClass;
+    std::vector<std::string> mdevCdiFiles;  // files the last generateMdevCDISpec wrote, one per vGPU class
 
     explicit Plugin(kxpu_ctx *ctx);
     ~Plugin();
@@ -177,7 +198,12 @@ class Plugin {
                                             const std::vector<std::string> *vendors = nullptr);
     // device_plugin.go:55-80 + cdi/spec.go:85-127: emit on the GPU, host writes the file (S3)
     Error generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, const std::string &format = "YAML");
-    // device_plugin.go:83-112: per device id device lists + plugin objects (S4); nothing is started
+    // the mdev walk (single-threaded, lexical order) + kxpu_classify_mdev; reads nothing when vgpuClasses is empty
+    Error createMdevMap();
+    // one CDI spec per vGPU class (kxpu_cdi_emit_mdev), <stem>.yaml|.json; nothing when vgpuClasses is empty
+    Error generateMdevCDISpec(const std::string &format = "YAML");
+    // device_plugin.go:83-112: per device id device lists + plugin objects (S4), then one plugin per (vGPU class, type
+    // key); nothing is started
     Error createDevicePlugins();
     // generic_device_plugin.go:320-355 for one container request (S5)
     Error Allocate(const std::vector<std::string> &devicesIDs, ContainerAllocateResponse &resp);
@@ -189,6 +215,8 @@ class Plugin {
     // the same records, read with openat / readlinkat relative to basePath by several threads
     // (SURVEY 8(f) row 2); falls back to gatherRecords when a seam was replaced.  threads = 0: automatic
     Error gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads = 0);
+    // raw gather of mdevBasePath under vgpuClasses (no GPU): one record per entry, lexical order
+    Error gatherMdevRecords(std::vector<kxpu_mdevrec> &recs);
 
   private:
     kxpu_ctx *ctx_;
@@ -196,6 +224,7 @@ class Plugin {
     Error ensureTable();
     bool defaultClasses() const;
     size_t classOfGroup(const std::string &group) const;
+    Error checkVgpuClasses() const;
     Error generateCDISpecClasses(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, int32_t fmt);
     // first use: kxpu_pciids_join on pinned buffers = file -> table -> row handles of `keys` in one call
     Error loadAndJoin(const std::vector<uint32_t> &keys, std::vector<int32_t> &rows);

@@ -5,7 +5,8 @@ import os
 
 import numpy as np
 
-from .binding import CDIDEV_DTYPE, DEVREC_DTYPE, REC_DRIVER_ERR
+from .binding import (CDIDEV_DTYPE, DEVREC_DTYPE, MDEVREC_DTYPE, REC_DRIVER_ERR, REC_IOMMU_ERR, REC_NAME_ERR,
+                      REC_VENDOR_ERR)
 
 _REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PCI_IDS_GZ = os.path.join(_REPO, "tests", "golden", "pci.ids.gz")
@@ -231,3 +232,71 @@ def synthetic_pci_ids(n_vendors, devs_per_vendor, subs_per_dev=1, seed=7, copies
         put_dec(body, o + 29, d_ids, 5)
     flat = out.reshape(-1)
     return np.tile(flat, copies) if copies > 1 else flat
+
+
+MDEV_RULES = [(b"10de", b"nvidia-vgpu"), (b"10de", b"vfio_mdev"), (b"8086", b"vfio_mdev"), (b"1002", b"vfio_mdev")]
+MDEV_TYPE_NAMES = [b"GRID T4-1Q\n", b"GRID T4-2B\n", b"GRID V100-8Q", b"NVIDIA A100-4C\n", b"NVIDIA  A100-4C",
+                   b"GRID A40-24Q (x)\n", b"i915-GVTg_V5_4", b"  GRID\tT4-1Q \n\n", b"\n", b"MxGPU+/vf 2"]
+
+
+def uuids(n, seed=0):
+    """n distinct random canonical lowercase UUIDs in lexical order, as an (n, 36) uint8 array."""
+    rng = np.random.default_rng(seed)
+    raw = rng.integers(0, 16, (n, 32), dtype=np.uint8)
+    raw[:, 0] = (np.arange(n, dtype=np.int64) * 16 // max(n, 1)).astype(np.uint8)  # spread, then sort
+    hexd = np.frombuffer(b"0123456789abcdef", np.uint8)
+    out = np.full((n, 36), ord("-"), np.uint8)
+    cols = [c for c in range(36) if c not in (8, 13, 18, 23)]
+    out[:, cols] = hexd[raw]
+    s = np.unique(out.view("S36").reshape(n))  # sorted, distinct
+    if len(s) < n:  # astronomically unlikely; keep n rows
+        s = np.concatenate([s, s[:n - len(s)]])
+    return s.view(np.uint8).reshape(n, 36)
+
+
+def mdev_records(n=1 << 20, seed=5):
+    """n synthetic /sys/bus/mdev/devices records (kxpu_mdevrec), entries in lexical UUID order.  Parent vendors
+    10de (60 %), 8086, 1002 and 1af4; mdev drivers nvidia-vgpu, vfio_mdev and others; type names from a few
+    realistic ones (inner runs of spaces, trailing newlines, bytes the type key deletes, a name that is only white
+    space) plus about 6 000 generated ones; groups shared by two mdevs each; 10 % read errors over the vendor,
+    driver, iommu_group and name reads.  Every rule of MDEV_RULES matches part of the records."""
+    rng = np.random.default_rng(seed)
+    recs = np.zeros(n, dtype=MDEVREC_DTYPE)
+    recs["uuid"] = uuids(n, seed).view("S36").reshape(n)
+    recs["parent"] = enumerate_bdfs(n >> 4 or 1)[np.arange(n) >> 4].view("S16").reshape(n)
+    vend = np.array([0x10de, 0x8086, 0x1002, 0x1af4], np.int64)[np.searchsorted([0.6, 0.75, 0.9], rng.random(n), side="right")]
+    recs["parent_vendor_txt"] = _id_text(vend)
+    recs["vendor_len"] = 7
+    r = rng.random(n)
+    recs["driver"] = np.where(r < 0.5, b"nvidia-vgpu", np.where(r < 0.9, b"vfio_mdev", b"i915")).astype("S16")
+    gen = [b"NVIDIA L40S-%dQ%s" % (k, b"\n" if k & 1 else b"") for k in range(6000)]
+    pool = MDEV_TYPE_NAMES + gen
+    pa = np.zeros((len(pool), 40), np.uint8)
+    pl = np.zeros(len(pool), np.uint8)
+    for i, nm in enumerate(pool):
+        pa[i, :len(nm)] = np.frombuffer(nm, np.uint8)
+        pl[i] = len(nm)
+    pick = np.where(rng.random(n) < 0.7, rng.integers(0, len(MDEV_TYPE_NAMES), n), rng.integers(0, len(pool), n))
+    recs["type_name"] = pa[pick]
+    recs["name_len"] = pl[pick]
+    recs["iommu_group"] = (np.arange(n, dtype=np.int64) >> 1).astype(np.uint32) + 100
+    e = rng.random(n)
+    flags = np.zeros(n, np.uint8)
+    flags[e < 0.025] = REC_VENDOR_ERR
+    flags[(e >= 0.025) & (e < 0.05)] = REC_DRIVER_ERR
+    flags[(e >= 0.05) & (e < 0.075)] = REC_IOMMU_ERR
+    flags[(e >= 0.075) & (e < 0.1)] = REC_NAME_ERR
+    recs["flags"] = flags
+    return recs
+
+
+def mdev_devices(n=65536, seed=6):
+    """n kxpu_mdevcdi entries: index 0..n-1, one group each, parents enumerated as in cfg3 (quoted and plain YAML
+    forms both occur)."""
+    from .binding import MDEVCDI_DTYPE
+    devs = np.zeros(n, dtype=MDEVCDI_DTYPE)
+    devs["uuid"] = uuids(n, seed).view("S36").reshape(n)
+    devs["parent"] = enumerate_bdfs(n).view("S16").reshape(n)
+    devs["iommu_group"] = (2000 + np.arange(n)).astype(np.uint32)
+    devs["index"] = np.arange(n, dtype=np.uint64)
+    return devs
