@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 4
+#define KXPU_ABI_VERSION 5
 
 /* status codes */
 #define KXPU_OK             0
@@ -266,7 +266,7 @@ typedef struct kxpu_devrec {
     uint8_t  vendor_len;     /* length of the vendor file (0..8; longer => set flag)    */
     uint8_t  device_len;
     uint8_t  flags;          /* KXPU_REC_* */
-    uint8_t  reserved0;
+    uint8_t  numa_node;      /* NUMA node of the function (0..63), valid only with KXPU_REC_NUMA (ABI v5) */
     uint32_t reserved1[2];
 } kxpu_devrec;
 
@@ -275,6 +275,18 @@ typedef struct kxpu_devrec {
 #define KXPU_REC_IOMMU_ERR  0x04u /* readLink(iommu_group) failed   (device_plugin.go:158) */
 #define KXPU_REC_DEVICE_ERR 0x08u /* readIDFromFile(device) failed  (device_plugin.go:165) */
 #define KXPU_REC_IS_DIR     0x10u /* info.IsDir()                   (device_plugin.go:137) */
+/* numa_node holds a known NUMA node (kxpu_devrec and kxpu_mdevrec).  Without it the record's node is unknown,
+ * so a zero-filled record -- every record built before ABI v5 -- means "no topology".
+ *
+ * NUMA node of a record: the host reads <entry>/numa_node (/sys/bus/pci/devices/<bdf>/numa_node for a PCI
+ * function, <uuid>/../numa_node -- the parent's -- for an mdev), strips ONE trailing '\n', and sets the flag
+ * only when what is left is a canonical decimal 0..63 (no sign, no leading zero except "0" itself).  Anything
+ * else -- "-1" (no node), a failed read, 64 and above, "01", an empty file, junk -- leaves the node unknown and
+ * is never an error.  The read changes nothing else: whether a record is accepted, its busIndex, its group and
+ * every other output of kxpu_classify / _rules / _mdev and kxpu_mdev_names ignore numa_node and this flag.
+ * A record whose flag is set with numa_node >= 64 counts as unknown. */
+#define KXPU_REC_NUMA       0x40u
+#define KXPU_MAX_NUMA_NODES 64
 
 /* Caller-allocated outputs of kxpu_classify; every array has room for n entries
  * (group_off / dev_off: n+1). */
@@ -345,8 +357,8 @@ typedef struct kxpu_mdevrec {
     uint32_t iommu_group;          /* basename of the mdev's `iommu_group` link, decimal                    */
     uint8_t  vendor_len;           /* length of the parent's vendor file (a file over 8 bytes: a failed read) */
     uint8_t  name_len;             /* length of the type name file (0..40)                                  */
-    uint8_t  flags;                /* KXPU_REC_VENDOR_ERR / _DRIVER_ERR / _IOMMU_ERR / _IS_DIR / _NAME_ERR  */
-    uint8_t  reserved0;
+    uint8_t  flags;                /* KXPU_REC_VENDOR_ERR / _DRIVER_ERR / _IOMMU_ERR / _IS_DIR / _NAME_ERR / _NUMA */
+    uint8_t  numa_node;            /* the parent's NUMA node, valid only with KXPU_REC_NUMA (ABI v5)        */
     uint32_t reserved1;
 } kxpu_mdevrec;
 #define KXPU_REC_NAME_ERR 0x20u /* reading mdev_type/name failed (kxpu_mdevrec only)                       */
@@ -388,6 +400,48 @@ int32_t kxpu_classify_mdev(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_r
  * (KXPU_REC_NAME_ERR or name_len > 40) yields an empty key.  rec_idx[j] >= n is KXPU_E_INVALID. */
 int32_t kxpu_mdev_names(kxpu_ctx *ctx, const kxpu_mdevrec *recs, size_t n, const uint32_t *rec_idx, size_t k,
                         uint8_t *out, size_t cap, uint32_t *offsets /* [k+1] */, size_t *need);
+
+/* ------------------------------------------------------- NUMA topology of the groups */
+
+/* kxpu_classify_rules / kxpu_classify_mdev plus the NUMA nodes of every group.  group_numa (caller array of n
+ * entries) receives, for group ordinal g < n_groups:
+ *   group_numa[g] = OR of (1 << numa_node) over the ACCEPTED members of group g that carry KXPU_REC_NUMA with
+ *                   numa_node < 64;
+ * 0 means "no topology" (no member's node is known).  Every other output is bitwise what kxpu_classify_rules /
+ * kxpu_classify_mdev return for the same arguments (with rules = {{"10de", "vfio-pci"}}: what kxpu_classify
+ * returns), and the calls run the same launches: the mask is folded into the pass that already visits every
+ * accepted record with its group ordinal. */
+int32_t kxpu_classify_topo(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs, size_t n,
+                           kxpu_classify_out *out, uint8_t *dev_rule /* [n] */, uint64_t *group_numa /* [n] */);
+int32_t kxpu_classify_mdev_topo(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_mdevrec *recs,
+                                size_t n, kxpu_classify_out *out, uint8_t *dev_rule /* [n] */,
+                                uint64_t *group_numa /* [n] */);
+
+/* GetPreferredAllocation (the reference returns nil, nil: generic_device_plugin.go:378-386), batched over the
+ * container requests of one PreferredAllocationRequest.  dev_numa[d] is the NUMA mask of the plugin's device d (the
+ * group_numa of its group); positions are indices into that device list.  Request q:
+ *   available      = avail[avail_off[q] .. avail_off[q+1])
+ *   must-include   = must[must_off[q] .. must_off[q+1])
+ *   size           = size[q]
+ * Let home(d) = lowest set bit of dev_numa[d], or 64 when the mask is 0; U = the home nodes below 64 of the
+ * must-include devices; candidates = available minus must-include; c[k] = the number of candidates with home k;
+ * r = size - |must|.  The bins are ordered
+ *   1. bins k in U with c[k] > 0, by c[k] descending, then k ascending;
+ *   2. the other bins k < 64 with c[k] > 0, in the same order;
+ *   3. bin 64 (unknown node) last.
+ * The answer of request q, out[out_off[q] .. out_off[q+1]) with out_off[q+1] - out_off[q] = size[q], is the
+ * must-include positions in request order followed by the first r candidates taken bin by bin, ascending position
+ * inside a bin (position order is walk order: adjacent addresses stay together).  out_off is computed by the call.
+ * KXPU_E_INVALID (and no output) when any request has a position >= n_devs, a duplicate inside available or inside
+ * must-include, a must-include position that is not available, size < |must| or size > |available|.
+ * Requests of up to 256 available positions run one warp each in a single launch; a larger request runs a
+ * histogram pass, then a stable per-bin rank and scatter over the device positions with a decoupled look-back.
+ * Limits (else KXPU_E_UNSUPPORTED): n_devs, n_req and the total of avail / must below 2^31. */
+int32_t kxpu_preferred_allocation(kxpu_ctx *ctx, const uint64_t *dev_numa, size_t n_devs,
+                                  const uint32_t *avail_off /* [n_req+1] */, const uint32_t *avail,
+                                  const uint32_t *must_off /* [n_req+1] */, const uint32_t *must,
+                                  const uint32_t *size /* [n_req] */, size_t n_req,
+                                  uint32_t *out /* [sum of size] */, uint32_t *out_off /* [n_req+1] */);
 
 /* ------------------------------------------------------- S3: CDI spec emit */
 
@@ -474,6 +528,17 @@ int32_t kxpu_alloc_names_kind(kxpu_ctx *ctx, const char *kind, const uint64_t *i
  * healthy[i] != 0 -> "Healthy" else "Unhealthy"; healthy == NULL -> all healthy. */
 int32_t kxpu_lw_encode(kxpu_ctx *ctx, const uint32_t *group_ids, const uint8_t *healthy,
                        size_t n, uint8_t *out, size_t cap, size_t *len);
+
+/* kxpu_lw_encode with the NUMA topology of every device (v1beta1 Device.topology, what the kubelet Topology
+ * Manager aligns on).  Device i, fields in number order as kubelet v0.30's gogo-generated api.pb.go marshals them:
+ *   string ID = 1; string health = 2;
+ *   when numa_mask[i] != 0: TopologyInfo topology = 3 { repeated NUMANode nodes = 1 { int64 ID = 1 } },
+ *   one node per set bit, ascending.
+ * proto3 omits a zero int64, so node 0 is an empty NUMANode (0a 00).  A topology of many nodes makes a Device longer
+ * than 127 bytes: both lengths are varints.  numa_mask == NULL or all masks 0 gives kxpu_lw_encode's bytes.
+ * Limit (else KXPU_E_UNSUPPORTED): n below 2^32 / 283 (the longest Device is 283 bytes). */
+int32_t kxpu_lw_encode_topo(kxpu_ctx *ctx, const uint32_t *group_ids, const uint8_t *healthy, const uint64_t *numa_mask,
+                            size_t n, uint8_t *out, size_t cap, size_t *len);
 
 #ifdef __cplusplus
 }

@@ -18,6 +18,8 @@ import (
 	"os"
 	"runtime"
 	"unsafe"
+
+	pluginapi "k8s.io/kubelet/pkg/apis/deviceplugin/v1beta1"
 )
 
 type kxpu struct {
@@ -348,4 +350,90 @@ func (k *kxpu) cdiEmitMdev(format int, kind string, devs []C.kxpu_mdevcdi) ([]by
 	err := kxCheck(k.ctx, "kxpu_cdi_emit_mdev", C.kxpu_cdi_emit_mdev(k.ctx, C.int32_t(format), ck, p, C.size_t(len(devs)),
 		(*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n))
 	return buf[:n], err
+}
+
+// NUMA topology (ABI v5).  With topology on, the walks fill numa_node / KXPU_REC_NUMA from <entry>/numa_node (an mdev:
+// <uuid>/../numa_node), classify returns one NUMA mask per group, and the Go call sites use the masks:
+//   - createDevicePlugins: pluginapi.Device{ID, Health, Topology: topologyInfo(mask)} for every group;
+//   - Register: pluginapi.DevicePluginOptions{GetPreferredAllocationAvailable: true};
+//   - GetDevicePluginOptions returns the same options; GetPreferredAllocation calls preferredAllocation once per
+//     PreferredAllocationRequest with the positions of the request's IDs in dpi.devs.
+
+// classifyRules / classifyMdev plus the NUMA mask of every group (mdev selects kxpu_classify_mdev_topo; recs is then a
+// []C.kxpu_mdevrec passed as its first element's address and n).
+func (k *kxpu) groupNuma(out *C.kxpu_classify_out, rules []C.kxpu_xpu_rule, recs unsafe.Pointer, n int, mdev bool,
+	devRule []uint8) ([]uint64, error) {
+	gnuma := make([]uint64, n)
+	if n == 0 {
+		return gnuma, nil
+	}
+	var rp *C.kxpu_xpu_rule
+	if len(rules) > 0 {
+		rp = &rules[0]
+	}
+	var rc C.int32_t
+	if mdev {
+		rc = C.kxpu_classify_mdev_topo(k.ctx, rp, C.size_t(len(rules)), (*C.kxpu_mdevrec)(recs), C.size_t(n), out,
+			(*C.uint8_t)(unsafe.Pointer(&devRule[0])), (*C.uint64_t)(unsafe.Pointer(&gnuma[0])))
+	} else {
+		rc = C.kxpu_classify_topo(k.ctx, rp, C.size_t(len(rules)), (*C.kxpu_devrec)(recs), C.size_t(n), out,
+			(*C.uint8_t)(unsafe.Pointer(&devRule[0])), (*C.uint64_t)(unsafe.Pointer(&gnuma[0])))
+	}
+	return gnuma[:out.n_groups], kxCheck(k.ctx, "kxpu_classify_topo", rc)
+}
+
+// pluginapi.TopologyInfo of a mask: one NUMANode per set bit, ascending; nil for 0 (no topology)
+func topologyInfo(mask uint64) *pluginapi.TopologyInfo {
+	if mask == 0 {
+		return nil
+	}
+	t := &pluginapi.TopologyInfo{}
+	for n := 0; n < 64; n++ {
+		if mask>>n&1 == 1 {
+			t.Nodes = append(t.Nodes, &pluginapi.NUMANode{ID: int64(n)})
+		}
+	}
+	return t
+}
+
+// ListAndWatchResponse bytes with Device.topology (what proto.Marshal of the response gives).
+func (k *kxpu) lwEncodeTopo(groups []uint32, healthy []uint8, masks []uint64) ([]byte, error) {
+	if len(groups) == 0 {
+		return nil, nil
+	}
+	g, h, m := (*C.uint32_t)(unsafe.Pointer(&groups[0])), (*C.uint8_t)(unsafe.Pointer(&healthy[0])), (*C.uint64_t)(unsafe.Pointer(&masks[0]))
+	var n C.size_t
+	C.kxpu_lw_encode_topo(k.ctx, g, h, m, C.size_t(len(groups)), nil, 0, &n) // sizing call
+	buf := make([]byte, n+1)
+	err := kxCheck(k.ctx, "kxpu_lw_encode_topo", C.kxpu_lw_encode_topo(k.ctx, g, h, m, C.size_t(len(groups)),
+		(*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n))
+	return buf[:n], err
+}
+
+// GetPreferredAllocation for all container requests of one PreferredAllocationRequest: avail / must hold positions in
+// dpi.devs, masks[d] is dpi.devs[d]'s NUMA mask.  Returns the positions of each request's answer.
+func (k *kxpu) preferredAllocation(masks []uint64, avail, must [][]uint32, size []uint32) ([][]uint32, error) {
+	nreq := len(size)
+	aoff, moff := make([]uint32, nreq+1), make([]uint32, nreq+1)
+	var a, m []uint32
+	total := 0
+	for q := 0; q < nreq; q++ {
+		a, m = append(a, avail[q]...), append(m, must[q]...)
+		aoff[q+1], moff[q+1] = uint32(len(a)), uint32(len(m))
+		total += int(size[q])
+	}
+	a, m = append(a, 0), append(m, 0) // valid pointers for empty lists
+	masks = append(masks, 0)
+	sz := append(size, 0)
+	out, ooff := make([]uint32, total+1), make([]uint32, nreq+1)
+	err := kxCheck(k.ctx, "kxpu_preferred_allocation", C.kxpu_preferred_allocation(k.ctx,
+		(*C.uint64_t)(unsafe.Pointer(&masks[0])), C.size_t(len(masks)-1), (*C.uint32_t)(unsafe.Pointer(&aoff[0])),
+		(*C.uint32_t)(unsafe.Pointer(&a[0])), (*C.uint32_t)(unsafe.Pointer(&moff[0])), (*C.uint32_t)(unsafe.Pointer(&m[0])),
+		(*C.uint32_t)(unsafe.Pointer(&sz[0])), C.size_t(nreq), (*C.uint32_t)(unsafe.Pointer(&out[0])),
+		(*C.uint32_t)(unsafe.Pointer(&ooff[0]))))
+	res := make([][]uint32, nreq)
+	for q := 0; err == nil && q < nreq; q++ {
+		res[q] = out[ooff[q]:ooff[q+1]]
+	}
+	return res, err
 }

@@ -20,6 +20,8 @@ import (
 	"path/filepath"
 	"strings"
 	"testing"
+
+	pluginapi "k8s.io/kubelet/pkg/apis/deviceplugin/v1beta1"
 )
 
 type kxGolden struct {
@@ -149,5 +151,31 @@ func TestKxpuCfg1(t *testing.T) {
 	want, _ := os.ReadFile(filepath.Join(kxRepo(t), "tests", "golden", "cfg1.yaml"))
 	if !bytes.Equal(got, want) {
 		t.Fatalf("CDI YAML differs from the oracle's:\n%s\n--- want\n%s", got, want)
+	}
+}
+
+// kxpu_lw_encode_topo: the ListAndWatchResponse with Device.topology that gogo's Marshal (kubelet v0.30 api.pb.go:
+// fields in number order, a zero int64 skipped) produces, against the oracle's bytes for the same list.
+func TestKxpuListAndWatchTopology(t *testing.T) {
+	node := func(ids ...int64) *pluginapi.TopologyInfo {
+		ti := &pluginapi.TopologyInfo{}
+		for _, id := range ids {
+			ti.Nodes = append(ti.Nodes, &pluginapi.NUMANode{ID: id})
+		}
+		return ti
+	}
+	resp := &pluginapi.ListAndWatchResponse{Devices: []*pluginapi.Device{
+		{ID: "214", Health: pluginapi.Healthy, Topology: node(0, 1)},
+		{ID: "7", Health: pluginapi.Unhealthy},
+		{ID: "30", Health: pluginapi.Healthy, Topology: node(63)},
+	}}
+	got, err := resp.Marshal()
+	if err != nil {
+		t.Fatal(err)
+	}
+	// oracle/kxpu_topo_oracle.c: kxo_lw_encode_topo([214, 7, 30], [1, 0, 1], [0b11, 0, 1 << 63])
+	want := "0a160a0332313412074865616c7468791a060a000a0208010a0e0a01371209556e6865616c7468790a130a02333012074865616c7468791a040a02083f"
+	if hex.EncodeToString(got) != want {
+		t.Fatalf("topology wire bytes differ:\n got %x\nwant %s", got, want)
 	}
 }

@@ -19,6 +19,11 @@ T_PARSE, T_FINALIZE, T_LOOKUP, T_NAMES, T_CLASSIFY, T_EMIT, T_MERGE, T_RESOLVE, 
 COMM_ID_BYTES = 128
 
 REC_VENDOR_ERR, REC_DRIVER_ERR, REC_IOMMU_ERR, REC_DEVICE_ERR, REC_IS_DIR, REC_NAME_ERR = 1, 2, 4, 8, 16, 32
+REC_NUMA = 64  # the record's numa_node byte is valid (ABI v5)
+MAX_NUMA_NODES = 64
+# The numa_node byte of kxpu_devrec / kxpu_mdevrec (ABI v5) keeps its pre-v5 numpy field name "reserved0": the
+# dtypes below must stay equal to the checkers' (oracle/*.py), which compare dtypes field name by field name.
+NUMA_FIELD = "reserved0"
 
 DEVREC_DTYPE = np.dtype([("bdf", "S16"), ("vendor_txt", "u1", (8,)), ("device_txt", "u1", (8,)),
                          ("driver", "S16"), ("iommu_group", "<u4"), ("vendor_len", "u1"),
@@ -47,6 +52,7 @@ ABI_SYMBOLS = [
     "kxpu_lw_encode", "kxpu_classify_rules", "kxpu_cdi_emit_kind", "kxpu_alloc_names_kind",
     "kxpu_classify_mdev", "kxpu_mdev_names", "kxpu_cdi_emit_mdev",
     "kxpu_pciids_full_load_device", "kxpu_full_free", "kxpu_full_export", "kxpu_full_lookup",
+    "kxpu_classify_topo", "kxpu_classify_mdev_topo", "kxpu_lw_encode_topo", "kxpu_preferred_allocation",
 ]
 
 
@@ -138,6 +144,10 @@ def load_library():
         "kxpu_full_free": (i32, [vp, vp]),
         "kxpu_full_export": (i32, [vp, vp, i32, vp, vp, sz, C.POINTER(C.c_uint32)]),
         "kxpu_full_lookup": (i32, [vp, vp, i32, vp, sz, vp]),
+        "kxpu_classify_topo": (i32, [vp, vp, sz, vp, sz, C.POINTER(ClassifyOut), vp, vp]),
+        "kxpu_classify_mdev_topo": (i32, [vp, vp, sz, vp, sz, C.POINTER(ClassifyOut), vp, vp]),
+        "kxpu_lw_encode_topo": (i32, [vp, vp, vp, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_preferred_allocation": (i32, [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp, vp]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -446,6 +456,64 @@ class Kxpu:
                     group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
                     dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g], dev_rule=dev_rule[:d])
 
+    def classify_topo(self, rules, recs, mdev=False):
+        """kxpu_classify_topo (DEVREC_DTYPE records) or kxpu_classify_mdev_topo (mdev=True, MDEVREC_DTYPE): the dict of
+        classify_rules / classify_mdev plus group_numa, the NUMA mask of every group ordinal."""
+        ra = rules_array(rules)
+        recs = np.ascontiguousarray(recs)
+        assert recs.dtype == (MDEVREC_DTYPE if mdev else DEVREC_DTYPE)
+        n = len(recs)
+        arrs = dict(accept_index=np.empty(n, np.uint32), group_ids=np.empty(n, np.uint32),
+                    group_off=np.empty(n + 1, np.uint32), group_members=np.empty(n, np.uint32),
+                    dev_ids=np.empty(n, np.uint64), dev_off=np.empty(n + 1, np.uint32),
+                    dev_groups=np.empty(n, np.uint32))
+        dev_rule = np.empty(max(n, 1), np.uint8)
+        gnuma = np.empty(max(n, 1), np.uint64)
+        out = ClassifyOut(**{k: v.ctypes.data for k, v in arrs.items()})
+        fn = self.L.kxpu_classify_mdev_topo if mdev else self.L.kxpu_classify_topo
+        self._chk(fn(self.ctx, _ptr(ra) if len(ra) else None, len(ra), _ptr(recs) if n else None, n, C.byref(out),
+                     _ptr(dev_rule), _ptr(gnuma)))
+        g, d, a = out.n_groups, out.n_devids, out.n_accepted
+        return dict(accept_index=arrs["accept_index"], n_accepted=a, n_groups=g, n_devids=d,
+                    group_ids=arrs["group_ids"][:g], group_off=arrs["group_off"][:g + 1],
+                    group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
+                    dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g], dev_rule=dev_rule[:d],
+                    group_numa=gnuma[:g])
+
+    def lw_encode_topo(self, groups, healthy=None, masks=None):
+        """kxpu_lw_encode_topo: ListAndWatchResponse bytes with Device.topology from the NUMA masks."""
+        groups = np.ascontiguousarray(groups, dtype=np.uint32)
+        if healthy is not None:
+            healthy = np.ascontiguousarray(healthy, dtype=np.uint8)
+        if masks is not None:
+            masks = np.ascontiguousarray(masks, dtype=np.uint64)
+        need = C.c_size_t(0)
+        rc = self.L.kxpu_lw_encode_topo(self.ctx, _ptr(groups), _ptr(healthy), _ptr(masks), len(groups), None, 0, C.byref(need))
+        if rc not in (KXPU_OK, E_NOSPACE):
+            self._chk(rc)
+        out = np.empty(max(need.value, 1), np.uint8)
+        got = C.c_size_t(0)
+        self._chk(self.L.kxpu_lw_encode_topo(self.ctx, _ptr(groups), _ptr(healthy), _ptr(masks), len(groups), _ptr(out),
+                                             need.value, C.byref(got)))
+        return out[:got.value].tobytes()
+
+    def preferred_allocation(self, dev_numa, requests):
+        """kxpu_preferred_allocation.  requests: [(available positions, must-include positions, size)]; returns one
+        position list per request."""
+        a = pref_requests(requests)
+        out = np.empty(max(int(a["size"].sum()), 1), np.uint32)
+        out_off = np.empty(len(requests) + 1, np.uint32)
+        self.preferred_allocation_raw(dev_numa, a, out, out_off)
+        return [out[out_off[q]:out_off[q + 1]].tolist() for q in range(len(requests))]
+
+    def preferred_allocation_raw(self, dev_numa, a, out, out_off):
+        """The bare call on a pref_requests() dict and caller buffers (timing loops)."""
+        dev_numa = np.ascontiguousarray(dev_numa, dtype=np.uint64)
+        self._chk(self.L.kxpu_preferred_allocation(self.ctx, _ptr(dev_numa) if len(dev_numa) else None, len(dev_numa),
+                                                   _ptr(a["avail_off"]), _ptr(a["avail"]), _ptr(a["must_off"]),
+                                                   _ptr(a["must"]), _ptr(a["size"]), len(a["size"]), _ptr(out),
+                                                   _ptr(out_off)))
+
     def mdev_names(self, recs, idx):
         """kxpu_mdev_names: (blob, offsets) of the type keys of recs[idx], with the two-call sizing."""
         recs = np.ascontiguousarray(recs)
@@ -536,6 +604,24 @@ class Kxpu:
         self._chk(self.L.kxpu_lw_encode(self.ctx, _ptr(groups), _ptr(healthy), len(groups), _ptr(out), need.value,
                                         C.byref(got)))
         return out[:got.value].tobytes()
+
+
+def pref_requests(requests):
+    """[(available, must-include, size)] -> the CSR arrays of kxpu_preferred_allocation (a one-element array stands in
+    for an empty list, so that every pointer is valid)."""
+    na = [len(r[0]) for r in requests]
+    nm = [len(r[1]) for r in requests]
+    avail_off = np.zeros(len(requests) + 1, np.uint32)
+    must_off = np.zeros(len(requests) + 1, np.uint32)
+    avail_off[1:] = np.cumsum(na, dtype=np.int64)
+    must_off[1:] = np.cumsum(nm, dtype=np.int64)
+    avail = np.zeros(max(int(avail_off[-1]), 1), np.uint32)
+    must = np.zeros(max(int(must_off[-1]), 1), np.uint32)
+    for q, (av, mu, _) in enumerate(requests):
+        avail[avail_off[q]:avail_off[q + 1]] = av
+        must[must_off[q]:must_off[q + 1]] = mu
+    return dict(avail_off=avail_off, avail=avail, must_off=must_off, must=must,
+                size=np.array([r[2] for r in requests], np.uint32).reshape(-1))
 
 
 def plan_shards(text, nranks):

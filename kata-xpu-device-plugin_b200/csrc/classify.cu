@@ -17,6 +17,8 @@
 // kxpu_classify_mdev: the candidate kernel reads 128-byte mdev records and writes each candidate's type key; a
 // name-intern pass maps every key to the first candidate carrying it (hash table, keys compared byte for byte);
 // the device-id key becomes (rule << 48 | that record's index).  Everything from k_accept_scan on is shared.
+// kxpu_classify_topo / _mdev_topo: k_pairs<true> also ORs each accepted record's NUMA node into its group ordinal's mask
+// (zeroed by k_reset with the totals); same launches as the non-topology call.
 // Launches: reset | candidates | accept + both scans (single pass, decoupled look-back) | per-group device ids | device-id
 // first-seen scan over the groups | sort pairs + all digit histograms | <= 4 radix passes, each ONE
 // kernel for both sorts (per-tile ranking + per-digit look-back, "onesweep") | CSR boundaries.
@@ -68,6 +70,8 @@ struct Work {
     uint32_t *islot;
     ISlot *itab;
     uint32_t icap, ishift;
+    // kxpu_classify_topo / _mdev_topo only: [n] NUMA mask per group ordinal (zeroed by k_reset)
+    unsigned long long *group_numa;
 };
 enum { MODE_NV = 0, MODE_RULES = 1, MODE_MDEV = 2 };
 
@@ -420,6 +424,10 @@ __global__ void __launch_bounds__(C_THREADS) k_devfirst_scan(const Work W) {
 
 // pass 4: sort inputs -- members (group ordinal, record) at busIndex, groups (device ordinal, group id)
 // at group ordinal -- and the digit histograms of all radix passes of both sorts.
+// TOPO (kxpu_classify_topo / _mdev_topo): this pass already holds every accepted record with its group ordinal, so it
+// also ORs the record's NUMA node into group_numa[ordinal]: one more 4-byte load (the flags / numa_node word) and one
+// 64-bit atomicOr per accepted record that carries a node.
+template <bool TOPO>
 __global__ void __launch_bounds__(256) k_pairs(const Work W, uint32_t passes) {
     __shared__ uint32_t h[2 * 4 * 256];
     for (uint32_t k = threadIdx.x; k < 2 * 4 * 256; k += 256) h[k] = 0u;
@@ -432,6 +440,13 @@ __global__ void __launch_bounds__(256) k_pairs(const Work W, uint32_t passes) {
             const uint32_t key = W.gtab[W.gslot[i]].ord;
             W.ak[b] = key;
             W.av[b] = i;
+            if (TOPO) {
+                // kxpu_devrec word 13 / kxpu_mdevrec word 30: [.., .., flags, numa_node]
+                const uint32_t fw = W.mrecs ? reinterpret_cast<const uint32_t *>(W.mrecs + i)[30]
+                                            : reinterpret_cast<const uint32_t *>(W.recs + i)[13];
+                const uint32_t node = fw >> 24;
+                if ((fw & (KXPU_REC_NUMA << 16)) && node < KXPU_MAX_NUMA_NODES) atomicOr(&W.group_numa[key], 1ull << node);
+            }
             for (uint32_t p = 0; p < passes; p++) atomicAdd(&h[(0 * 4 + p) * 256 + ((key >> (8 * p)) & 255u)], 1u);
         }
         if (i < ng) {
@@ -592,18 +607,19 @@ static uint32_t bits_for(uint32_t n) {
 
 // R == nullptr: kxpu_classify (the NVIDIA constants); else the rule list of kxpu_classify_rules, or with mdev of
 // kxpu_classify_mdev (recs then points at kxpu_mdevrec records)
+// group_numa != nullptr: the _topo calls (NUMA mask per group)
 static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
-                             bool mdev, uint8_t *dev_rule, bool small_dtab, bool *retry);
+                             bool mdev, uint8_t *dev_rule, uint64_t *group_numa, bool small_dtab, bool *retry);
 
 static int32_t classify_run(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R, bool mdev,
-                            uint8_t *dev_rule) {
+                            uint8_t *dev_rule, uint64_t *group_numa = nullptr) {
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
     bool retry = false;
-    int32_t rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, true, &retry);
+    int32_t rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, true, &retry);
     // more distinct device ids (or type keys) than the small tables hold
-    if (retry) rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, false, &retry);
+    if (retry) rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, false, &retry);
     return rc;
 }
 
@@ -674,8 +690,28 @@ extern "C" int32_t kxpu_classify_mdev(kxpu_ctx *ctx, const kxpu_xpu_rule *rules,
     return classify_run(ctx, recs, n, out, &R, true, dev_rule);
 }
 
+extern "C" int32_t kxpu_classify_topo(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs,
+                                      size_t n, kxpu_classify_out *out, uint8_t *dev_rule, uint64_t *group_numa) {
+    if (!ctx || !out || (n && (!recs || !group_numa)) || !rules || n_rules == 0 || n_rules > KXPU_MAX_RULES) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    RuleTable R;
+    const int32_t rc = rule_table(ctx, rules, n_rules, R);
+    if (rc != KXPU_OK) return rc;
+    return classify_run(ctx, recs, n, out, &R, false, dev_rule, group_numa);
+}
+
+extern "C" int32_t kxpu_classify_mdev_topo(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_mdevrec *recs,
+                                           size_t n, kxpu_classify_out *out, uint8_t *dev_rule, uint64_t *group_numa) {
+    if (!ctx || !out || (n && (!recs || !group_numa)) || !rules || n_rules == 0 || n_rules > KXPU_MAX_RULES) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    RuleTable R;
+    const int32_t rc = rule_table(ctx, rules, n_rules, R);
+    if (rc != KXPU_OK) return rc;
+    return classify_run(ctx, recs, n, out, &R, true, dev_rule, group_numa);
+}
+
 static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
-                             bool mdev, uint8_t *dev_rule, bool small_dtab, bool *retry) {
+                             bool mdev, uint8_t *dev_rule, uint64_t *group_numa, bool small_dtab, bool *retry) {
     *retry = false;
     out->n_accepted = out->n_groups = out->n_devids = 0;
     if (n == 0) {
@@ -707,6 +743,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
     const size_t o_itab = mdev ? take((size_t)icap * sizeof(ISlot)) : 0;
     const size_t ff_bytes = off;
     const size_t o_totals = take(16), o_ghist = take(2 * 4 * 256 * 4);
+    const size_t o_gnuma = group_numa ? take(n * 8) : 0;  // zeroed with the totals: one reset launch either way
     const size_t zero_words = (off - ff_bytes) / 4;
     const size_t rec_bytes = mdev ? sizeof(kxpu_mdevrec) : sizeof(kxpu_devrec);
     const size_t o_recs = take(n * rec_bytes);
@@ -737,6 +774,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
     W.accept_index = (uint32_t *)(b + o_acc_idx); W.group_ids = (uint32_t *)(b + o_gids);
     W.group_off = (uint32_t *)(b + o_goff); W.dev_ids = (unsigned long long *)(b + o_dids); W.dev_off = (uint32_t *)(b + o_doff);
     if (R) { W.rrule = b + o_rrule; W.dev_rule = b + o_drule; }
+    if (group_numa) W.group_numa = (unsigned long long *)(b + o_gnuma);
     if (mdev) {
         W.mrecs = (const kxpu_mdevrec *)(b + o_recs);
         W.keybuf = (uint4 *)(b + o_keys); W.islot = (uint32_t *)(b + o_islot);
@@ -762,7 +800,8 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
         else if (R) k_groups<MODE_RULES><<<g, 256, 0, ctx->stream>>>(W);
         else k_groups<MODE_NV><<<g, 256, 0, ctx->stream>>>(W);
         k_devfirst_scan<<<c_tiles, C_THREADS, 0, ctx->stream>>>(W);
-        k_pairs<<<std::min<unsigned>(g, 4u * ctx->sm_count), 256, 0, ctx->stream>>>(W, passes);
+        if (group_numa) k_pairs<true><<<std::min<unsigned>(g, 4u * ctx->sm_count), 256, 0, ctx->stream>>>(W, passes);
+        else k_pairs<false><<<std::min<unsigned>(g, 4u * ctx->sm_count), 256, 0, ctx->stream>>>(W, passes);
         ctx->launches += 6;
         for (uint32_t p = 0; p < passes; p++) {
             SweepParams S;
@@ -800,6 +839,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
         cudaMemcpyAsync(out->dev_off, W.dev_off, ((size_t)nd + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream);
         cudaMemcpyAsync(out->dev_groups, bv, (size_t)ng * 4, cudaMemcpyDeviceToHost, ctx->stream);
         if (dev_rule && nd) cudaMemcpyAsync(dev_rule, W.dev_rule, nd, cudaMemcpyDeviceToHost, ctx->stream);
+        if (group_numa && ng) cudaMemcpyAsync(group_numa, W.group_numa, (size_t)ng * 8, cudaMemcpyDeviceToHost, ctx->stream);
         e = cudaStreamSynchronize(ctx->stream);
         if (e != cudaSuccess) { KX_SET_ERR(ctx, "classify D2H failed: %s", cudaGetErrorString(e)); rc = KXPU_E_CUDA; }
         if (ng == 0) out->group_off[0] = 0;

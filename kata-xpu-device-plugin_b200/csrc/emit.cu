@@ -348,29 +348,65 @@ __global__ void __launch_bounds__(256) k_mdev_name_write(const kxpu_mdevrec *__r
 }
 
 // ------------------------------------------------------------------ ListAndWatchResponse
-// repeated Device devices = 1; Device { string ID = 1; string health = 2; }
+// repeated Device devices = 1; Device { string ID = 1; string health = 2; TopologyInfo topology = 3; }
+// TOPO = false: kxpu_lw_encode (no topology, every length fits one byte).  TOPO = true: kxpu_lw_encode_topo, field 3
+// when the device's mask is non-zero: TopologyInfo { repeated NUMANode nodes = 1 { int64 ID = 1 } }, nodes ascending.
+// A NUMANode of node k > 0 is 0a 02 08 k (4 bytes, k < 128 is one varint byte); node 0 is 0a 00 (proto3 drops the zero
+// ID).  Up to 64 nodes make the topology 254 bytes and the Device 280: both lengths become two-byte varints.
+__device__ __forceinline__ uint32_t topo_len(unsigned long long mask) {  // TopologyInfo body
+    return 4u * (uint32_t)__popcll(mask) - 2u * (uint32_t)(mask & 1ull);
+}
+__device__ __forceinline__ uint32_t varint_len(uint32_t v) { return v < 128u ? 1u : 2u; }  // v < 2^14 here
+__device__ __forceinline__ uint8_t *varint_write(uint32_t v, uint8_t *d) {
+    if (v < 128u) { d[0] = (uint8_t)v; return d + 1; }
+    d[0] = (uint8_t)(0x80u | (v & 0x7fu)); d[1] = (uint8_t)(v >> 7); return d + 2;
+}
+// the Device body length of device i
+template <bool TOPO>
+__device__ __forceinline__ uint32_t lw_body(uint32_t group, bool ok, unsigned long long mask) {
+    uint32_t l = 2u + dec_len(group) + 2u + (ok ? 7u : 9u);
+    if (TOPO && mask) { const uint32_t t = topo_len(mask); l += 1u + varint_len(t) + t; }
+    return l;
+}
+template <bool TOPO>
 __global__ void __launch_bounds__(256) k_lw_len(const uint32_t *__restrict__ groups, const uint8_t *__restrict__ healthy,
-                                                uint32_t n, uint32_t *__restrict__ lens) {
+                                                const unsigned long long *__restrict__ masks, uint32_t n, uint32_t *__restrict__ lens) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i > n) return;
     if (i == n) { lens[i] = 0; return; }
-    uint32_t hl = (!healthy || healthy[i]) ? 7u : 9u;
-    lens[i] = 2u + 2u + dec_len(groups[i]) + 2u + hl;
+    const uint32_t body = lw_body<TOPO>(groups[i], !healthy || healthy[i], TOPO && masks ? masks[i] : 0ull);
+    lens[i] = 1u + (TOPO ? varint_len(body) : 1u) + body;
 }
+template <bool TOPO>
 __global__ void __launch_bounds__(256) k_lw_write(const uint32_t *__restrict__ groups, const uint8_t *__restrict__ healthy,
-                                                  uint32_t n, const uint32_t *__restrict__ offs, uint8_t *__restrict__ out) {
+                                                  const unsigned long long *__restrict__ masks, uint32_t n,
+                                                  const uint32_t *__restrict__ offs, uint8_t *__restrict__ out) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const bool ok = !healthy || healthy[i];
     const char hs[10] = "Unhealthy";
+    const unsigned long long mask = TOPO && masks ? masks[i] : 0ull;
     const uint32_t hl = ok ? 7u : 9u, gl = dec_len(groups[i]);
     uint8_t *d = out + offs[i];
-    d[0] = 0x0a; d[1] = (uint8_t)(2u + gl + 2u + hl);
+    d[0] = 0x0a;
+    if (TOPO) d = varint_write(lw_body<TOPO>(groups[i], ok, mask), d + 1) - 2;  // d + 2 = start of the body
+    else d[1] = (uint8_t)(2u + gl + 2u + hl);
     d[2] = 0x0a; d[3] = (uint8_t)gl;
     dec_write(groups[i], gl, d + 4);
     d[4 + gl] = 0x12; d[5 + gl] = (uint8_t)hl;
     for (uint32_t k = 0; k < hl; k++) d[6 + gl + k] = (uint8_t)hs[ok ? k + 2 : k];  // "Healthy" = "Unhealthy"+2 with 'h'->'H'
     if (ok) d[6 + gl] = (uint8_t)'H';
+    if (TOPO && mask) {
+        uint8_t *t = d + 6 + gl + hl;
+        *t++ = 0x1a;
+        t = varint_write(topo_len(mask), t);
+        for (unsigned long long m = mask; m; m &= m - 1ull) {
+            const uint32_t k = (uint32_t)__ffsll((long long)m) - 1u;
+            t[0] = 0x0a;
+            if (k == 0u) { t[1] = 0x00; t += 2; }
+            else { t[1] = 0x02; t[2] = 0x08; t[3] = (uint8_t)k; t += 4; }
+        }
+    }
 }
 
 }  // namespace kxemit
@@ -501,19 +537,26 @@ extern "C" int32_t kxpu_cdi_emit_mdev(kxpu_ctx *ctx, int32_t format, const char 
     return cdi_emit(ctx, format, kind, devs, n, out, cap, len, true);
 }
 
-// shared driver of the two "thread per item" emitters
+// shared driver of the "thread per item" emitters.  h_in3 (optional, in3_bytes): one more input, uploaded like the
+// others; its device address is stored to *d_in3 before the kernels are enqueued (the lambdas read it from there).
 template <typename LenK, typename WriteK>
 static int32_t emit_items(kxpu_ctx *ctx, size_t n, size_t in_bytes, const void *h_in, const uint8_t *h_in2, uint8_t *out,
-                          size_t cap, uint32_t *offsets, size_t *need, LenK lenk, WriteK writek) {
+                          size_t cap, uint32_t *offsets, size_t *need, LenK lenk, WriteK writek, const void *h_in3 = nullptr,
+                          size_t in3_bytes = 0, const uint8_t **d_in3 = nullptr) {
     const uint32_t N = (uint32_t)n;
     uint8_t *b = nullptr;
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
     size_t o_in = take(in_bytes), o_in2 = take(h_in2 ? n : 16), o_lens = take((n + 1) * 4), o_offs = take((n + 1) * 4);
+    const size_t o_in3 = h_in3 ? take(in3_bytes) : 0;
     KxScratch sc(ctx);
     KX_CUDA(ctx, sc.alloc((void **)&b, off));
     cudaMemcpyAsync(b + o_in, h_in, in_bytes, cudaMemcpyHostToDevice, ctx->stream);
     if (h_in2) cudaMemcpyAsync(b + o_in2, h_in2, n, cudaMemcpyHostToDevice, ctx->stream);
+    if (h_in3) {
+        cudaMemcpyAsync(b + o_in3, h_in3, in3_bytes, cudaMemcpyHostToDevice, ctx->stream);
+        *d_in3 = b + o_in3;
+    }
     uint32_t *d_lens = (uint32_t *)(b + o_lens), *d_offs = (uint32_t *)(b + o_offs);
     lenk(b + o_in, h_in2 ? b + o_in2 : nullptr, N, d_lens);
     ctx->launches++;
@@ -615,9 +658,31 @@ extern "C" int32_t kxpu_lw_encode(kxpu_ctx *ctx, const uint32_t *group_ids, cons
     return emit_items(
         ctx, n, n * 4, group_ids, healthy, out, cap, nullptr, len,
         [st](const uint8_t *in, const uint8_t *in2, uint32_t N, uint32_t *lens) {
-            k_lw_len<<<(N + 1 + 255) / 256, 256, 0, st>>>((const uint32_t *)in, in2, N, lens);
+            k_lw_len<false><<<(N + 1 + 255) / 256, 256, 0, st>>>((const uint32_t *)in, in2, nullptr, N, lens);
         },
         [st](const uint8_t *in, const uint8_t *in2, uint32_t N, const uint32_t *offs, uint8_t *o) {
-            k_lw_write<<<(N + 255) / 256, 256, 0, st>>>((const uint32_t *)in, in2, N, offs, o);
+            k_lw_write<false><<<(N + 255) / 256, 256, 0, st>>>((const uint32_t *)in, in2, nullptr, N, offs, o);
         });
+}
+
+extern "C" int32_t kxpu_lw_encode_topo(kxpu_ctx *ctx, const uint32_t *group_ids, const uint8_t *healthy, const uint64_t *numa_mask,
+                                       size_t n, uint8_t *out, size_t cap, size_t *len) {
+    if (!ctx || !len || (n && !group_ids)) return KXPU_E_INVALID;
+    if (n >= 0xFFFFFFFFull / 283u) return KXPU_E_UNSUPPORTED;  // the uint32 offsets of the longest Devices
+    std::lock_guard<std::mutex> guard(ctx->mu);
+    cudaSetDevice(ctx->device);
+    kx_clear_timings(ctx);
+    if (n == 0) { *len = 0; return KXPU_OK; }
+    cudaStream_t st = ctx->stream;
+    const uint8_t *d_masks = nullptr;  // the masks' device copy (emit_items), NULL without masks
+    return emit_items(
+        ctx, n, n * 4, group_ids, healthy, out, cap, nullptr, len,
+        [st, &d_masks](const uint8_t *in, const uint8_t *in2, uint32_t N, uint32_t *lens) {
+            k_lw_len<true><<<(N + 1 + 255) / 256, 256, 0, st>>>((const uint32_t *)in, in2, (const unsigned long long *)d_masks, N, lens);
+        },
+        [st, &d_masks](const uint8_t *in, const uint8_t *in2, uint32_t N, const uint32_t *offs, uint8_t *o) {
+            k_lw_write<true><<<(N + 255) / 256, 256, 0, st>>>((const uint32_t *)in, in2, (const unsigned long long *)d_masks, N,
+                                                             offs, o);
+        },
+        numa_mask, n * 8, &d_masks);
 }

@@ -76,7 +76,46 @@ static bool readLinkFunc(const std::string &base, const std::string &addr, const
     return true;
 }
 
+// <base>/<entry>/numa_node, raw bytes.  Quiet: a missing file only means "node unknown".
+static bool readNumaNodeFunc(const std::string &base, const std::string &entry, std::string &out) {
+    const std::string path = base + "/" + entry + "/numa_node";
+    FILE *f = fopen(path.c_str(), "rb");
+    if (!f) return false;
+    char buf[64];
+    size_t n = fread(buf, 1, sizeof buf, f);
+    bool err = ferror(f) != 0;
+    fclose(f);
+    if (err) return false;
+    out.assign(buf, n);
+    return true;
+}
+
+// the numa_node rule of include/kxpu.h: one trailing '\n' stripped, then a canonical decimal 0..63
+static bool parseNumaNode(const std::string &raw, uint8_t &node) {
+    std::string s = raw;
+    if (!s.empty() && s.back() == '\n') s.pop_back();
+    if (s.empty() || s.size() > 2 || (s.size() > 1 && s[0] == '0')) return false;
+    unsigned v = 0;
+    for (char c : s) {
+        if (c < '0' || c > '9') return false;
+        v = v * 10 + (unsigned)(c - '0');
+    }
+    if (v >= KXPU_MAX_NUMA_NODES) return false;
+    node = (uint8_t)v;
+    return true;
+}
+template <typename ReadNuma>
+static void numaRecord(ReadNuma readNuma, uint8_t &flags, uint8_t &node) {
+    std::string s;
+    uint8_t k = 0;
+    if (readNuma(s) && parseNumaNode(s, k)) {
+        node = k;
+        flags |= KXPU_REC_NUMA;
+    }
+}
+
 Plugin::Plugin(kxpu_ctx *ctx) : ctx_(ctx) {
+    readNumaNode = readNumaNodeFunc;
     readLink = readLinkFunc;
     readIDFromFile = readIDFromFileFunc;
     returnIommuMap = [this]() -> const OrderedMap<std::vector<NvidiaGpuDevice>> & { return iommuMap; };
@@ -177,9 +216,11 @@ static bool packID(const std::string &raw, uint8_t txt[8], uint8_t &len) {
 // of the `driver` / `iommu_group` links.  An entry the record cannot carry (address longer than 15
 // bytes, group that is not a canonical decimal below 2^32-1, id longer than the field) is logged and
 // skipped like a read error -- and only if the reference would have accepted it; it never stops the walk.
-template <typename ReadID, typename ReadLnk>
+// readNuma == nullptr: numa_node is not read (Plugin::topologyAware false).  It is read last, only for a record that
+// got as far as its device read, and changes nothing but numa_node / KXPU_REC_NUMA.
+template <typename ReadID, typename ReadLnk, typename ReadNuma>
 static Error leafRecord(const std::string &name, const std::vector<XpuClass> &classes, ReadID readID, ReadLnk readLnk,
-                        kxpu_devrec &r) {
+                        const ReadNuma *readNuma, kxpu_devrec &r) {
     memset(&r, 0, sizeof r);
     strncpy(r.bdf, name.c_str(), sizeof r.bdf - 1);
     std::string s;
@@ -233,6 +274,7 @@ static Error leafRecord(const std::string &name, const std::vector<XpuClass> &cl
     } else {
         r.flags |= KXPU_REC_DEVICE_ERR;  // :165-168
     }
+    if (readNuma) numaRecord(*readNuma, r.flags, r.numa_node);
     return Error();
 }
 
@@ -261,9 +303,11 @@ static Error walkDir(Plugin &p, const std::string &path, const std::string &name
     // one raw record per non-directory entry; every read goes through the seams and is keyed by
     // info.Name() under basePath exactly like :142,:151,:157,:164
     kxpu_devrec r;
+    auto readNuma = [&](std::string &out) { return p.readNumaNode(p.basePath, name, out); };
     Error e = leafRecord(name, p.xpuClasses,
                          [&](const char *prop, std::string &out) { return p.readIDFromFile(p.basePath, name, prop, out); },
-                         [&](const char *link, std::string &out) { return p.readLink(p.basePath, name, link, out); }, r);
+                         [&](const char *link, std::string &out) { return p.readLink(p.basePath, name, link, out); },
+                         p.topologyAware ? &readNuma : nullptr, r);
     if (e) return e;
     recs.push_back(r);
     return Error();
@@ -289,7 +333,10 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
     // the fast reads bypass the seams: only when nobody replaced them (tests do, device_plugin.go:38-39)
     using SeamFn = bool (*)(const std::string &, const std::string &, const std::string &, std::string &);
     SeamFn const *rl = readLink.target<SeamFn>(), *ri = readIDFromFile.target<SeamFn>();
-    const bool defaultSeams = rl && *rl == readLinkFunc && ri && *ri == readIDFromFileFunc;
+    using NumaFn = bool (*)(const std::string &, const std::string &, std::string &);
+    NumaFn const *rn = readNumaNode.target<NumaFn>();
+    const bool defaultSeams = rl && *rl == readLinkFunc && ri && *ri == readIDFromFileFunc &&
+                              (!topologyAware || (rn && *rn == readNumaNodeFunc));
     if (!S_ISDIR(sb.st_mode) || !defaultSeams) return gatherRecords(recs);
     int basefd = open(basePath.c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
     if (basefd < 0) return fail("Error accessing file path \"" + basePath + "\": " + strerror(errno));
@@ -349,8 +396,20 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
         for (size_t i = lo; i < hi; i++) {
             if (ents[i].dir) continue;
             const std::string &name = ents[i].name;
+            // numa_node on the same directory descriptor; quiet like readNumaNodeFunc
+            auto readNuma = [&](std::string &out) {
+                int fd = openat(basefd, (name + "/numa_node").c_str(), O_RDONLY | O_CLOEXEC);
+                if (fd < 0) return false;
+                char buf[64];
+                ssize_t k = read(fd, buf, sizeof buf);
+                close(fd);
+                if (k < 0) return false;
+                out.assign(buf, (size_t)k);
+                return true;
+            };
             errs[i] = leafRecord(name, xpuClasses, [&](const char *prop, std::string &out) { return readID(name, prop, out); },
-                                 [&](const char *link, std::string &out) { return readLnk(name, link, out); }, flat[i]);
+                                 [&](const char *link, std::string &out) { return readLnk(name, link, out); },
+                                 topologyAware ? &readNuma : nullptr, flat[i]);
         }
     };
     if (threads == 0) threads = std::min(8u, std::max(1u, std::thread::hardware_concurrency()));
@@ -389,6 +448,7 @@ Error Plugin::createIommuDeviceMap() {
     deviceMap.clear();  // :128
     iommuClass.clear();
     deviceClass.clear();
+    iommuNuma.clear();
     // the generation is read BEFORE the walk: an event during the walk makes the snapshot stale, never fresh
     haveSnapshotGen_ = snapshotValidation && bindGeneration && bindGeneration(snapshotGen_);
     std::vector<kxpu_devrec> recs;
@@ -403,8 +463,9 @@ Error Plugin::createIommuDeviceMap() {
     out.group_members = gmem.data(); out.dev_ids = dids.data(); out.dev_off = doff.data(); out.dev_groups = dgrp.data();
     const bool dflt = defaultClasses();
     std::vector<uint8_t> drule(n ? n : 1, 0);
+    std::vector<uint64_t> gnuma(n ? n : 1, 0);
     int32_t rc;
-    if (dflt) {
+    if (dflt && !topologyAware) {
         rc = kxpu_classify(ctx_, recs.data(), n, &out);
         if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify", rc);  // fatal: there is no CPU path
     } else {
@@ -415,8 +476,13 @@ Error Plugin::createIommuDeviceMap() {
             strncpy(rules[c].vendor, xpuClasses[c].vendor.c_str(), sizeof rules[c].vendor);
             strncpy(rules[c].driver, xpuClasses[c].driver.c_str(), sizeof rules[c].driver);
         }
-        rc = kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data());
-        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify_rules", rc);
+        if (topologyAware) {  // with the default class list: rule {10de, vfio-pci}, kxpu_classify's outputs
+            rc = kxpu_classify_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data(), gnuma.data());
+            if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify_topo", rc);
+        } else {
+            rc = kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data());
+            if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify_rules", rc);
+        }
     }
     // class of a group = the rule of its first member, which the device-map entry listing it carries
     std::map<uint32_t, size_t> groupClass;
@@ -435,6 +501,7 @@ Error Plugin::createIommuDeviceMap() {
         }
         iommuMap.emplace_back(std::to_string(gids[g]), std::move(devs));
         iommuClass.push_back(groupClass[gids[g]]);
+        if (topologyAware) iommuNuma.push_back(gnuma[g]);
     }
     for (uint32_t d = 0; d < out.n_devids; d++) {
         std::vector<std::string> groups;
@@ -491,6 +558,8 @@ static void mdevRecord(Plugin &p, const std::string &name, bool isDir, kxpu_mdev
     uint32_t g = 0;
     if (!p.readLink(p.mdevBasePath, name, "iommu_group", s) || !parseGroup(s, g)) { r.flags |= KXPU_REC_IOMMU_ERR; return; }
     r.iommu_group = g;
+    // the parent's node; read before the name, since a record without a name can still join an existing group
+    if (p.topologyAware) numaRecord([&](std::string &out) { return p.readNumaNode(p.mdevBasePath, name + "/..", out); }, r.flags, r.numa_node);
     if (!p.readIDFromFile(p.mdevBasePath, name, "mdev_type/name", s) || s.size() > sizeof r.type_name) {
         r.flags |= KXPU_REC_NAME_ERR;
         return;
@@ -539,6 +608,7 @@ Error Plugin::createMdevMap() {
     typeMap.clear();
     mdevClass.clear();
     typeClass.clear();
+    mdevNuma.clear();
     if (vgpuClasses.empty()) return Error();  // nothing under mdevBasePath is read
     Error e = checkVgpuClasses();
     if (e) return e;
@@ -559,8 +629,10 @@ Error Plugin::createMdevMap() {
         strncpy(rules[c].vendor, vgpuClasses[c].vendor.c_str(), sizeof rules[c].vendor);
         strncpy(rules[c].driver, vgpuClasses[c].driver.c_str(), sizeof rules[c].driver);
     }
-    int32_t rc = kxpu_classify_mdev(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data());
-    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify_mdev", rc);
+    std::vector<uint64_t> gnuma(n ? n : 1, 0);
+    int32_t rc = topologyAware ? kxpu_classify_mdev_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data(), gnuma.data())
+                               : kxpu_classify_mdev(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data());
+    if (rc != KXPU_OK) return kxfail(ctx_, topologyAware ? "kxpu_classify_mdev_topo" : "kxpu_classify_mdev", rc);
     std::vector<uint32_t> first(out.n_devids);
     for (uint32_t d = 0; d < out.n_devids; d++) first[d] = (uint32_t)dids[d];
     std::vector<uint32_t> koff(first.size() + 1);
@@ -586,6 +658,7 @@ Error Plugin::createMdevMap() {
         }
         mdevMap.emplace_back(std::to_string(gids[g]), std::move(devs));
         mdevClass.push_back(groupClass[gids[g]]);
+        if (topologyAware) mdevNuma.push_back(gnuma[g]);
     }
     for (uint32_t d = 0; d < out.n_devids; d++) {
         std::vector<std::string> groups;
@@ -843,12 +916,19 @@ Error Plugin::createDevicePlugins() {
     }
     const bool dflt = defaultClasses();
     const std::vector<std::string> names = getDeviceNames(ids, dflt ? nullptr : &vendors);  // :99 for every device id at once
+    std::map<std::string, uint64_t> numaOf, mdevNumaOf;  // group id -> NUMA mask (topologyAware)
+    for (size_t g = 0; g < iommuNuma.size() && g < iommuMap.size(); g++) numaOf[iommuMap[g].first] = iommuNuma[g];
+    for (size_t g = 0; g < mdevNuma.size() && g < mdevMap.size(); g++) mdevNumaOf[mdevMap[g].first] = mdevNuma[g];
+    auto maskOf = [](const std::map<std::string, uint64_t> &m, const std::string &g) {
+        auto it = m.find(g);
+        return it == m.end() ? uint64_t(0) : it->second;
+    };
     size_t at = 0;
     for (const auto &kv : deviceMap) {  // :91
         GenericDevicePlugin dp;
         dp.xpuClass = at < deviceClass.size() ? deviceClass[at] : 0;
         dp.resourceNamespace = xpuClasses[dp.xpuClass].resourceNamespace;
-        for (const std::string &dev : kv.second) dp.devs.push_back(Device{dev, kHealthy});  // :93-98
+        for (const std::string &dev : kv.second) dp.devs.push_back(Device{dev, kHealthy, maskOf(numaOf, dev)});  // :93-98
         std::string devpluginName = names[at++];
         if (devpluginName.empty()) {
             fprintf(stderr, "Error: Could not find device name for device id: %s\n", kv.first.c_str());
@@ -864,7 +944,7 @@ Error Plugin::createDevicePlugins() {
         dp.vgpu = true;
         dp.xpuClass = typeClass[t];
         dp.resourceNamespace = vgpuClasses[dp.xpuClass].resourceNamespace;
-        for (const std::string &g : typeMap[t].second) dp.devs.push_back(Device{g, kHealthy});
+        for (const std::string &g : typeMap[t].second) dp.devs.push_back(Device{g, kHealthy, maskOf(mdevNumaOf, g)});
         dp.devpluginName = typeMap[t].first;
         dp.devicePath = "/dev/vfio/";  // an mdev has its own IOMMU group and /dev/vfio/<group>
         dp.socketPath = std::string(kDevicePluginPath) + "kata-xpu-" + dp.devpluginName + ".sock";
@@ -981,17 +1061,73 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
 Error Plugin::ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8_t> &out) {
     std::vector<uint32_t> groups;
     std::vector<uint8_t> healthy;
+    std::vector<uint64_t> masks;
     for (const Device &d : dp.devs) {
         groups.push_back((uint32_t)strtoul(d.ID.c_str(), nullptr, 10));
         healthy.push_back(d.Health == kHealthy);
+        masks.push_back(d.numa);
     }
+    // topologyAware: Device.topology from each device's mask (the HealthWatcher's re-sends come through here too)
+    const char *what = topologyAware ? "kxpu_lw_encode_topo" : "kxpu_lw_encode";
+    auto encode = [&](uint8_t *o, size_t cap, size_t *len) {
+        return topologyAware ? kxpu_lw_encode_topo(ctx_, groups.data(), healthy.data(), masks.data(), groups.size(), o, cap, len)
+                             : kxpu_lw_encode(ctx_, groups.data(), healthy.data(), groups.size(), o, cap, len);
+    };
     size_t len = 0;
-    int32_t rc = kxpu_lw_encode(ctx_, groups.data(), healthy.data(), groups.size(), nullptr, 0, &len);
-    if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, "kxpu_lw_encode", rc);
+    int32_t rc = encode(nullptr, 0, &len);
+    if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, what, rc);
     out.resize(len);
     if (len == 0) return Error();
-    rc = kxpu_lw_encode(ctx_, groups.data(), healthy.data(), groups.size(), out.data(), len, &len);
-    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_lw_encode", rc);
+    rc = encode(out.data(), len, &len);
+    if (rc != KXPU_OK) return kxfail(ctx_, what, rc);
+    return Error();
+}
+
+DevicePluginOptions Plugin::GetDevicePluginOptions() const {
+    DevicePluginOptions o;  // PreStartRequired: false (generic_device_plugin.go:255)
+    o.GetPreferredAllocationAvailable = topologyAware;
+    return o;
+}
+
+Error Plugin::GetPreferredAllocation(const GenericDevicePlugin &dp, const std::vector<ContainerPreferredAllocationRequest> &requests,
+                                     std::vector<ContainerPreferredAllocationResponse> &responses) {
+    responses.clear();
+    if (!topologyAware) return Error();  // the reference's empty response (generic_device_plugin.go:378-386)
+    std::map<std::string, uint32_t> posOf;
+    std::vector<uint64_t> numa(dp.devs.size());
+    for (size_t d = 0; d < dp.devs.size(); d++) {
+        posOf.emplace(dp.devs[d].ID, (uint32_t)d);
+        numa[d] = dp.devs[d].numa;
+    }
+    std::vector<uint32_t> availOff{0}, mustOff{0}, avail, must, size;
+    auto positions = [&](const std::vector<std::string> &ids, std::vector<uint32_t> &to) {
+        for (const std::string &id : ids) {
+            auto it = posOf.find(id);
+            if (it == posOf.end()) return fail("invalid preferred allocation request: unknown device: " + id);
+            to.push_back(it->second);
+        }
+        return Error();
+    };
+    for (const ContainerPreferredAllocationRequest &r : requests) {
+        Error e = positions(r.AvailableDeviceIDs, avail);
+        if (!e) e = positions(r.MustIncludeDeviceIDs, must);
+        if (e) return e;
+        if (r.AllocationSize < 0) return fail("invalid preferred allocation request: negative allocation size");
+        availOff.push_back((uint32_t)avail.size());
+        mustOff.push_back((uint32_t)must.size());
+        size.push_back((uint32_t)r.AllocationSize);
+    }
+    size_t total = 0;
+    for (uint32_t s : size) total += s;
+    std::vector<uint32_t> out(total ? total : 1), outOff(requests.size() + 1);
+    int32_t rc = kxpu_preferred_allocation(ctx_, numa.data(), numa.size(), availOff.data(), avail.data(), mustOff.data(),
+                                           must.data(), size.data(), requests.size(), out.data(), outOff.data());
+    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_preferred_allocation", rc);
+    for (size_t q = 0; q < requests.size(); q++) {
+        ContainerPreferredAllocationResponse resp;
+        for (uint32_t k = outOff[q]; k < outOff[q + 1]; k++) resp.DeviceIDs.push_back(dp.devs[out[k]].ID);
+        responses.push_back(std::move(resp));
+    }
     return Error();
 }
 
@@ -1381,6 +1517,113 @@ int kxh_list_and_watch(void *h, int plugin_index, uint8_t *out, size_t cap) {
     if (b.size() > cap) return -2;
     memcpy(out, b.data(), b.size());
     return (int)b.size();
+}
+
+// ---- NUMA topology (tests)
+void kxh_set_topology(void *h, int on) { ((Plugin *)h)->topologyAware = on != 0; }
+void kxh_options(void *h, int *pre_start_required, int *preferred_allocation_available) {
+    const device_plugin::DevicePluginOptions o = ((Plugin *)h)->GetDevicePluginOptions();
+    *pre_start_required = o.PreStartRequired;
+    *preferred_allocation_available = o.GetPreferredAllocationAvailable;
+}
+
+// counting_seam != 0: readNumaNode is replaced by a wrapper of the default read that counts its calls into *numa_reads
+static void numaSeam(Plugin &p, int counting_seam, uint64_t *numa_reads) {
+    if (!counting_seam) return;
+    auto dflt = p.readNumaNode;
+    p.readNumaNode = [dflt, numa_reads](const std::string &base, const std::string &entry, std::string &out) {
+        (*numa_reads)++;
+        return dflt(base, entry, out);
+    };
+}
+
+// CPU only: the raw PCI gather with topologyAware = topo; fast = the batched / threaded variant
+int kxh_gather_topo(const char *base_path, int topo, int fast, unsigned threads, int counting_seam, kxpu_devrec *out, size_t cap,
+                    size_t *n, uint64_t *numa_reads, char *err, size_t errcap) {
+    Plugin p(nullptr);
+    p.basePath = base_path;
+    p.topologyAware = topo != 0;
+    *numa_reads = 0;
+    numaSeam(p, counting_seam, numa_reads);
+    std::vector<kxpu_devrec> recs;
+    device_plugin::Error e = fast ? p.gatherRecordsFast(recs, threads) : p.gatherRecords(recs);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    *n = recs.size();
+    if (recs.size() > cap) return -2;
+    memcpy(out, recs.data(), recs.size() * sizeof(kxpu_devrec));
+    return 0;
+}
+
+// CPU only: the raw mdev gather under a vGPU class list with topologyAware = topo
+int kxh_gather_mdev_topo(const char *mdev_base, const char *classes, int topo, int counting_seam, kxpu_mdevrec *out, size_t cap,
+                         size_t *n, uint64_t *numa_reads, char *err, size_t errcap) {
+    Plugin p(nullptr);
+    p.mdevBasePath = mdev_base;
+    p.topologyAware = topo != 0;
+    *numa_reads = 0;
+    numaSeam(p, counting_seam, numa_reads);
+    if (!parseClasses(classes, p.vgpuClasses)) { copy_out("malformed class list", err, errcap); return -1; }
+    std::vector<kxpu_mdevrec> recs;
+    device_plugin::Error e = p.gatherMdevRecords(recs);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    *n = recs.size();
+    if (recs.size() > cap) return -2;
+    memcpy(out, recs.data(), recs.size() * sizeof(kxpu_mdevrec));
+    return 0;
+}
+
+// GetPreferredAllocation for plugin plugin_index.  spec: container requests separated by ';', each
+// "<available ids csv>|<must-include ids csv>|<size>".  json: [[ids of request 0], ...]
+int kxh_preferred_allocation(void *h, int plugin_index, const char *spec, char *json, size_t cap) {
+    Plugin *p = (Plugin *)h;
+    if (plugin_index < 0 || (size_t)plugin_index >= p->devicePlugins.size()) return -1;
+    auto split = [](const std::string &s, char sep) {
+        std::vector<std::string> v;
+        size_t a = 0;
+        for (;;) {
+            size_t c = s.find(sep, a);
+            v.push_back(s.substr(a, c == std::string::npos ? std::string::npos : c - a));
+            if (c == std::string::npos) break;
+            a = c + 1;
+        }
+        return v;
+    };
+    std::vector<device_plugin::ContainerPreferredAllocationRequest> reqs;
+    if (spec[0]) {
+        for (const std::string &item : split(spec, ';')) {
+            std::vector<std::string> f = split(item, '|');
+            if (f.size() != 3) { copy_out("malformed request", json, cap); return -1; }
+            device_plugin::ContainerPreferredAllocationRequest r;
+            if (!f[0].empty()) r.AvailableDeviceIDs = split(f[0], ',');
+            if (!f[1].empty()) r.MustIncludeDeviceIDs = split(f[1], ',');
+            r.AllocationSize = atoi(f[2].c_str());
+            reqs.push_back(std::move(r));
+        }
+    }
+    std::vector<device_plugin::ContainerPreferredAllocationResponse> resps;
+    device_plugin::Error e = p->GetPreferredAllocation(p->devicePlugins[(size_t)plugin_index], reqs, resps);
+    if (e) { copy_out(e.message, json, cap); return -1; }
+    std::string o = "[";
+    for (size_t q = 0; q < resps.size(); q++) {
+        if (q) o += ',';
+        o += '[';
+        for (size_t i = 0; i < resps[q].DeviceIDs.size(); i++) { if (i) o += ','; jstr(o, resps[q].DeviceIDs[i]); }
+        o += ']';
+    }
+    o += ']';
+    return copy_out(o, json, cap);
+}
+
+// "id=mask,..." of one plugin's devices (the NUMA mask each Device carries)
+int kxh_devs_numa(void *h, int plugin_index, char *out, size_t cap) {
+    Plugin *p = (Plugin *)h;
+    if (plugin_index < 0 || (size_t)plugin_index >= p->devicePlugins.size()) return -1;
+    std::string o;
+    for (const auto &d : p->devicePlugins[(size_t)plugin_index].devs) {
+        if (!o.empty()) o += ',';
+        o += d.ID + "=" + std::to_string(d.numa);
+    }
+    return copy_out(o, out, cap);
 }
 
 }  // extern "C"

@@ -48,6 +48,21 @@ using OrderedMap = std::vector<std::pair<std::string, V>>;
 struct Device {  // pluginapi.Device
     std::string ID;
     std::string Health;
+    uint64_t numa = 0;  // Device.Topology: bit k = NUMA node k (the group's mask); 0 = no topology
+};
+// pluginapi.DevicePluginOptions (GetDevicePluginOptions, generic_device_plugin.go:253-258)
+struct DevicePluginOptions {
+    bool PreStartRequired = false;
+    bool GetPreferredAllocationAvailable = false;
+};
+// pluginapi.ContainerPreferredAllocationRequest / ContainerPreferredAllocationResponse
+struct ContainerPreferredAllocationRequest {
+    std::vector<std::string> AvailableDeviceIDs;
+    std::vector<std::string> MustIncludeDeviceIDs;
+    int32_t AllocationSize = 0;
+};
+struct ContainerPreferredAllocationResponse {
+    std::vector<std::string> DeviceIDs;
 };
 struct GenericDevicePlugin {
     std::string devpluginName;   // resource name suffix: "<resourceNamespace>/<devpluginName>" (:211)
@@ -167,6 +182,13 @@ class Plugin {
     std::string mdevBasePath = "/sys/bus/mdev/devices";
     std::function<const OrderedMap<std::vector<MdevDevice>> &()> returnMdevMap;
     std::function<bool(uint64_t &generation)> bindGeneration;
+    // NUMA topology (include/kxpu.h, ABI v5).  false (default): nothing named numa_node is opened, the records, the
+    // ListAndWatch bytes and the options are the reference's, GetPreferredAllocation answers nothing.  true: the gathers
+    // read <entry>/numa_node through readNumaNode (an mdev: its parent's, entry "<uuid>/.."), classify returns a NUMA
+    // mask per group, every Device carries its group's mask (ListAndWatch sends Device.topology), and
+    // GetPreferredAllocation keeps an allocation on as few nodes as it can (kxpu_preferred_allocation).
+    bool topologyAware = false;
+    std::function<bool(const std::string &base, const std::string &entry, std::string &out)> readNumaNode;
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
 
     // ---- state (device_plugin.go:31,34)
@@ -176,6 +198,7 @@ class Plugin {
     std::string lastCdiFile;
     // class of every iommuMap / deviceMap entry (same positions); all 0 with the default class list
     std::vector<size_t> iommuClass, deviceClass;
+    std::vector<uint64_t> iommuNuma, mdevNuma;  // NUMA mask of every iommuMap / mdevMap entry (topologyAware only)
     std::vector<std::string> cdiFiles;  // files the last generateCDISpec wrote, one per class
     // the mdev walk: IOMMU group -> mdevs, type key -> groups, and the vGPU class of every entry (same positions)
     OrderedMap<std::vector<MdevDevice>> mdevMap;
@@ -209,6 +232,12 @@ class Plugin {
     Error Allocate(const std::vector<std::string> &devicesIDs, ContainerAllocateResponse &resp);
     // generic_device_plugin.go:224: the bytes of ListAndWatchResponse{Devices: dpi.devs}
     Error ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8_t> &out);
+    // generic_device_plugin.go:253-258: GetPreferredAllocationAvailable = topologyAware
+    DevicePluginOptions GetDevicePluginOptions() const;
+    // generic_device_plugin.go:378-386 (the reference: nil, nil).  topologyAware: one kxpu_preferred_allocation call for
+    // all container requests, device IDs mapped to positions in dp.devs; an ID not in dp.devs is an error naming it.
+    Error GetPreferredAllocation(const GenericDevicePlugin &dp, const std::vector<ContainerPreferredAllocationRequest> &requests,
+                                 std::vector<ContainerPreferredAllocationResponse> &responses);
 
     // raw gather only (no GPU): exposed for CPU tests of the walk
     Error gatherRecords(std::vector<kxpu_devrec> &recs);

@@ -300,3 +300,58 @@ def mdev_devices(n=65536, seed=6):
     devs["iommu_group"] = (2000 + np.arange(n)).astype(np.uint32)
     devs["index"] = np.arange(n, dtype=np.uint64)
     return devs
+
+
+# ---------------------------------------------------------------- NUMA topology (ABI v5)
+def _numa_assign(recs, bus, nodes, rng):
+    """numa_node / KXPU_REC_NUMA by bus range over `nodes` nodes, 3 % unknown (no flag), and about 1 % of the records
+    moved to another node (some groups then span two nodes)."""
+    from .binding import NUMA_FIELD, REC_NUMA
+    n = len(recs)
+    node = bus * nodes // (int(bus.max()) + 1 if n else 1)  # contiguous bus ranges, one per node
+    moved = rng.random(n) < 0.01
+    node = np.where(moved, (node + 1 + rng.integers(0, max(nodes - 1, 1), n)) % nodes, node)
+    known = rng.random(n) >= 0.03
+    recs[NUMA_FIELD] = np.where(known, node, 0).astype(np.uint8)
+    recs["flags"] = recs["flags"] | np.where(known, REC_NUMA, 0).astype(np.uint8)
+    return recs
+
+
+def topo_records(present_keys, n=1 << 20, nodes=2, seed=1):
+    """cfg3_records(present_keys, n, seed) plus a NUMA assignment by PCI bus range over `nodes` nodes (2 or 4):
+    3 % unknown nodes and a few functions on another node than the rest of their slot (multi-node groups)."""
+    recs = cfg3_records(present_keys, n, seed)
+    bus = np.arange(n, dtype=np.int64) >> 8  # domain:bus of the walk position
+    return _numa_assign(recs, bus, nodes, np.random.default_rng(seed + 100))
+
+
+def topo_mdev_records(n=1 << 20, nodes=2, seed=5):
+    """mdev_records(n, seed) with the parents' NUMA nodes assigned like topo_records (by the parent's bus)."""
+    recs = mdev_records(n, seed)
+    bus = (np.arange(n, dtype=np.int64) >> 4) >> 8  # domain:bus of the parent
+    return _numa_assign(recs, bus, nodes, np.random.default_rng(seed + 100))
+
+
+def topo_requests(dev_numa, n_req=4096, avail=16, size=8, must_max=2, seed=9):
+    """n_req GetPreferredAllocation container requests over a device list with masks dev_numa: each offers `avail`
+    distinct random positions, must-include 0..must_max of them, and asks for `size`.  avail = len(dev_numa) with
+    n_req = 1 is the one-request-over-everything case."""
+    rng = np.random.default_rng(seed)
+    n = len(dev_numa)
+    reqs = []
+    for _ in range(n_req):
+        av = rng.permutation(n)[:avail] if avail < n else rng.permutation(n)
+        nm = int(rng.integers(0, must_max + 1))
+        mu = av[rng.permutation(len(av))[:nm]]
+        reqs.append((av.astype(np.uint32), mu.astype(np.uint32), size))
+    return reqs
+
+
+def topo_dev_numa(n, nodes=4, seed=11):
+    """NUMA masks of n devices: by position range over `nodes` nodes, 5 % unknown (0), 2 % on two nodes."""
+    rng = np.random.default_rng(seed)
+    node = (np.arange(n, dtype=np.int64) * nodes // max(n, 1))
+    m = (np.uint64(1) << node.astype(np.uint64))
+    two = rng.random(n) < 0.02
+    m = np.where(two, m | (np.uint64(1) << ((node + 1) % nodes).astype(np.uint64)), m)
+    return np.where(rng.random(n) < 0.05, np.uint64(0), m).astype(np.uint64)

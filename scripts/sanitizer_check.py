@@ -17,6 +17,13 @@ res = kx.classify(recs)
 devs = W.cfg5_devices(3000)
 print("classify", res["n_accepted"], "json", len(kx.cdi_emit(1, devs)), "yaml", len(kx.cdi_emit(0, devs)))
 print("alloc", len(kx.alloc_names(devs["index"])[0]), "lw", len(kx.lw_encode(res["group_ids"][:100])))
+# NUMA topology: classify masks (PCI and mdev), topology wire bytes, both preferred-allocation shapes
+tres = kx.classify_topo([(b"10de", b"vfio-pci")], W.topo_records(keys, n=20000, nodes=4))
+mres = kx.classify_topo(W.MDEV_RULES, W.topo_mdev_records(n=20000), mdev=True)
+dn = W.topo_dev_numa(20000)
+print("topo groups", tres["n_groups"], mres["n_groups"], "lw", len(kx.lw_encode_topo(tres["group_ids"], None, tres["group_numa"])),
+      "pref", len(kx.preferred_allocation(dn, W.topo_requests(dn, n_req=300))),
+      len(kx.preferred_allocation(dn, W.topo_requests(dn, n_req=1, avail=20000, size=5000, must_max=3))[0]))
 tab.free()
 # zero-copy join: text, keys and rows in mapped pinned host memory
 h_t, p1 = kx.pinned(len(text)); h_t[:] = np.frombuffer(text, np.uint8)
