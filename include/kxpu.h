@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 5
+#define KXPU_ABI_VERSION 6
 
 /* status codes */
 #define KXPU_OK             0
@@ -71,7 +71,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_FINALIZE 1
 #define KXPU_T_LOOKUP   2
 #define KXPU_T_NAMES    3
-#define KXPU_T_CLASSIFY 4
+#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's kernels: the slot holds the kernels of the most recent of the two */
 #define KXPU_T_EMIT     5
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
@@ -442,6 +442,53 @@ int32_t kxpu_preferred_allocation(kxpu_ctx *ctx, const uint64_t *dev_numa, size_
                                   const uint32_t *must_off /* [n_req+1] */, const uint32_t *must,
                                   const uint32_t *size /* [n_req] */, size_t n_req,
                                   uint32_t *out /* [sum of size] */, uint32_t *out_off /* [n_req+1] */);
+
+/* ------------------------------------------------- runtime rediscovery (ABI v6) */
+
+/* One accepted entry of a walk, as a rediscovery compares two walks.  64 bytes. */
+typedef struct kxpu_snaprec {
+    char     key[40];       /* PCI address (PCI walk) or UUID (mdev walk), NUL padded, 1..39 bytes          */
+    uint32_t iommu_group;
+    uint32_t klass;         /* index of the class (xpuClasses / vgpuClasses) the entry itself matched       */
+    uint64_t tag;           /* opaque identity word, compared for equality only                             */
+    uint64_t index;         /* prev: its index; cur: ignored                                                */
+} kxpu_snaprec;
+
+#define KXPU_RC_KEPT    0u  /* same key, group, klass and tag in both walks: keeps its index           */
+#define KXPU_RC_NEW     1u  /* cur only: the key is absent from prev                                   */
+#define KXPU_RC_CHANGED 2u  /* the key is in both walks, but its group, klass or tag differs           */
+#define KXPU_RC_RETIRED 3u  /* prev only: the key is absent from cur                                   */
+
+typedef struct kxpu_reconcile_counts {
+    uint64_t n_kept, n_new, n_changed, n_retired;  /* n_changed counts pairs: one cur and one prev entry each */
+    uint64_t next_index_out;                       /* next_index + n_new + n_changed                          */
+} kxpu_reconcile_counts;
+
+/* Index reconciliation of a rediscovery: which entries of the new walk `cur` are the entries of the previous
+ * snapshot `prev`, and which CDI index each gets.  Allocate hands out <kind>=<index> and the container runtime
+ * resolves that name against the spec file later, so an index must never name two different devices while the
+ * process lives:
+ *   - cur[i] is KEPT iff some prev[j] has the same 40 key bytes, iommu_group, klass and tag; then
+ *     index_out[i] = prev[j].index and prev_state[j] = KXPU_RC_KEPT;
+ *   - every other cur[i] gets index_out[i] = next_index + (number of non-kept cur entries before i): fresh
+ *     indices in walk order, never one handed out before (every prev index is below next_index);
+ *   - cur_state[i]: KXPU_RC_KEPT, KXPU_RC_NEW (no prev entry has its key) or KXPU_RC_CHANGED (one has, with
+ *     another group, klass or tag: the entry gets a fresh index);
+ *   - prev_state[j]: KXPU_RC_KEPT, KXPU_RC_RETIRED (no cur entry has its key) or KXPU_RC_CHANGED;
+ *   - counts: the four counts and next_index_out = next_index + (number of non-kept cur entries).
+ * KXPU_E_INVALID, and nothing is written to any output, when: a key occurs twice within prev or within cur; a key is
+ * empty (first byte NUL) or has a non-NUL byte after its first NUL; some prev[j].index >= next_index;
+ * next_index + n_cur overflows 64 bits.
+ * Two identities tie the call to the walk: n_prev = 0 with next_index = 0 gives index_out[i] = i (kxpu_classify's
+ * busIndex when cur is the accepted records in walk order), and prev = the output of a call over the same cur (index
+ * = index_out) gives all KEPT, the same indices and next_index_out = next_index.
+ * The join is a hash table of at least 2 * (n_prev + n_cur) 16-byte slots (keys compared byte for byte on a hash
+ * hit), one probe per cur entry, and the fresh indices come from the single-pass scan of the classify kernels.
+ * Limit (else KXPU_E_UNSUPPORTED): n_prev + n_cur <= 2^30.  cur_state / prev_state / counts may be NULL. */
+int32_t kxpu_reconcile(kxpu_ctx *ctx, const kxpu_snaprec *prev, size_t n_prev, uint64_t next_index,
+                       const kxpu_snaprec *cur, size_t n_cur, uint64_t *index_out /* [n_cur] */,
+                       uint8_t *cur_state /* [n_cur] */, uint8_t *prev_state /* [n_prev] */,
+                       kxpu_reconcile_counts *counts);
 
 /* ------------------------------------------------------- S3: CDI spec emit */
 

@@ -437,3 +437,32 @@ func (k *kxpu) preferredAllocation(masks []uint64, avail, must [][]uint32, size 
 	}
 	return res, err
 }
+
+// Runtime rediscovery (ABI v6).  After the walk and classify of a rediscovery, build one C.kxpu_snaprec per accepted
+// function (key = PCI address, tag = the packed device id text) or mdev (key = UUID, tag = FNV-1a 64 of the type key),
+// in walk order, and reconcile it against the previous snapshot: survivors keep their CDI index, everything else gets
+// a fresh one from nextIndex on.  The returned snapshot (cur with the new indices) and next index are the input of the
+// next rediscovery.  prev may be empty (nextIndex = 0 numbers by walk order, the start-up busIndex).
+func (k *kxpu) reconcile(prev []C.kxpu_snaprec, nextIndex uint64, cur []C.kxpu_snaprec) (snap []C.kxpu_snaprec,
+	curState, prevState []uint8, counts C.kxpu_reconcile_counts, err error) {
+	idx := make([]uint64, len(cur)+1)
+	curState, prevState = make([]uint8, len(cur)+1), make([]uint8, len(prev)+1)
+	var pp, cp unsafe.Pointer
+	if len(prev) > 0 {
+		pp = unsafe.Pointer(&prev[0])
+	}
+	if len(cur) > 0 {
+		cp = unsafe.Pointer(&cur[0])
+	}
+	err = kxCheck(k.ctx, "kxpu_reconcile", C.kxpu_reconcile(k.ctx, (*C.kxpu_snaprec)(pp), C.size_t(len(prev)),
+		C.uint64_t(nextIndex), (*C.kxpu_snaprec)(cp), C.size_t(len(cur)), (*C.uint64_t)(unsafe.Pointer(&idx[0])),
+		(*C.uint8_t)(unsafe.Pointer(&curState[0])), (*C.uint8_t)(unsafe.Pointer(&prevState[0])), &counts))
+	if err != nil {
+		return nil, nil, nil, counts, err
+	}
+	snap = append([]C.kxpu_snaprec(nil), cur...)
+	for i := range snap {
+		snap[i].index = C.uint64_t(idx[i])
+	}
+	return snap, curState[:len(cur)], prevState[:len(prev)], counts, nil
+}

@@ -39,6 +39,12 @@ MDEVREC_DTYPE = np.dtype([("uuid", "S36"), ("parent", "S16"), ("parent_vendor_tx
                           ("flags", "u1"), ("reserved0", "u1"), ("reserved1", "<u4")])
 MDEVCDI_DTYPE = np.dtype([("uuid", "S36"), ("iommu_group", "<u4"), ("parent", "S16"), ("index", "<u8")])
 assert MDEVREC_DTYPE.itemsize == 128 and MDEVCDI_DTYPE.itemsize == 64
+# kxpu_snaprec / kxpu_reconcile_counts (runtime rediscovery, ABI v6)
+SNAPREC_DTYPE = np.dtype([("key", "S40"), ("iommu_group", "<u4"), ("klass", "<u4"), ("tag", "<u8"), ("index", "<u8")])
+RC_COUNTS_DTYPE = np.dtype([("n_kept", "<u8"), ("n_new", "<u8"), ("n_changed", "<u8"), ("n_retired", "<u8"),
+                            ("next_index_out", "<u8")])
+assert SNAPREC_DTYPE.itemsize == 64 and RC_COUNTS_DTYPE.itemsize == 40
+RC_KEPT, RC_NEW, RC_CHANGED, RC_RETIRED = 0, 1, 2, 3
 
 # every symbol include/kxpu.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -53,6 +59,7 @@ ABI_SYMBOLS = [
     "kxpu_classify_mdev", "kxpu_mdev_names", "kxpu_cdi_emit_mdev",
     "kxpu_pciids_full_load_device", "kxpu_full_free", "kxpu_full_export", "kxpu_full_lookup",
     "kxpu_classify_topo", "kxpu_classify_mdev_topo", "kxpu_lw_encode_topo", "kxpu_preferred_allocation",
+    "kxpu_reconcile",
 ]
 
 
@@ -148,6 +155,7 @@ def load_library():
         "kxpu_classify_mdev_topo": (i32, [vp, vp, sz, vp, sz, C.POINTER(ClassifyOut), vp, vp]),
         "kxpu_lw_encode_topo": (i32, [vp, vp, vp, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_preferred_allocation": (i32, [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp, vp]),
+        "kxpu_reconcile": (i32, [vp, vp, sz, u64, vp, sz, vp, vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -514,6 +522,21 @@ class Kxpu:
                                                    _ptr(a["must"]), _ptr(a["size"]), len(a["size"]), _ptr(out),
                                                    _ptr(out_off)))
 
+    def reconcile(self, prev, cur, next_index):
+        """kxpu_reconcile: prev / cur are SNAPREC_DTYPE arrays.  Returns dict(index, cur_state, prev_state, counts),
+        counts a dict of the five kxpu_reconcile_counts fields."""
+        prev, cur = np.ascontiguousarray(prev), np.ascontiguousarray(cur)
+        assert prev.dtype == SNAPREC_DTYPE and cur.dtype == SNAPREC_DTYPE
+        out = reconcile_outputs(len(prev), len(cur))
+        self.reconcile_raw(prev, cur, next_index, out)
+        return reconcile_result(out)
+
+    def reconcile_raw(self, prev, cur, next_index, out):
+        """The bare call into the buffers of reconcile_outputs() (timing loops, untouched-output checks)."""
+        self._chk(self.L.kxpu_reconcile(self.ctx, _ptr(prev) if len(prev) else None, len(prev), next_index,
+                                        _ptr(cur) if len(cur) else None, len(cur), _ptr(out["index"]),
+                                        _ptr(out["cur_state"]), _ptr(out["prev_state"]), _ptr(out["counts"])))
+
     def mdev_names(self, recs, idx):
         """kxpu_mdev_names: (blob, offsets) of the type keys of recs[idx], with the two-call sizing."""
         recs = np.ascontiguousarray(recs)
@@ -604,6 +627,20 @@ class Kxpu:
         self._chk(self.L.kxpu_lw_encode(self.ctx, _ptr(groups), _ptr(healthy), len(groups), _ptr(out), need.value,
                                         C.byref(got)))
         return out[:got.value].tobytes()
+
+
+def reconcile_outputs(n_prev, n_cur, fill=0):
+    """Caller buffers of kxpu_reconcile (one spare element each, so that every pointer is valid), filled with `fill`."""
+    return dict(index=np.full(max(n_cur, 1), fill, np.uint64), cur_state=np.full(max(n_cur, 1), fill & 0xFF, np.uint8),
+                prev_state=np.full(max(n_prev, 1), fill & 0xFF, np.uint8), counts=np.zeros(1, RC_COUNTS_DTYPE),
+                n_prev=n_prev, n_cur=n_cur)
+
+
+def reconcile_result(out):
+    c = out["counts"][0]
+    return dict(index=out["index"][:out["n_cur"]].copy(), cur_state=out["cur_state"][:out["n_cur"]].copy(),
+                prev_state=out["prev_state"][:out["n_prev"]].copy(),
+                counts={k: int(c[k]) for k in RC_COUNTS_DTYPE.names})
 
 
 def pref_requests(requests):

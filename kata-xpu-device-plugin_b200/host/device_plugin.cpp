@@ -13,6 +13,7 @@
 #include <fcntl.h>
 
 #include <climits>
+#include <mutex>
 
 #include <algorithm>
 #include <cerrno>
@@ -125,6 +126,11 @@ Plugin::Plugin(kxpu_ctx *ctx) : ctx_(ctx) {
         generation = bindWatcher_.generation();
         return bindWatcher_.healthy();
     };
+    mdevGeneration = [this](uint64_t &generation) {
+        if (!bindWatcher_.healthy() && bindWatcher_.start()) return false;
+        generation = bindWatcher_.mdevGeneration();
+        return bindWatcher_.healthy();
+    };
 }
 
 // ---------------------------------------------------------------------------- bind / unbind uevents
@@ -159,7 +165,9 @@ void BindWatcher::feed(const char *msg, size_t len) {
         else if (strncmp(p, "SUBSYSTEM=", 10) == 0) subsystem = p + 10;
         if (memchr(p, 0, (size_t)(end - p)) == nullptr) break;  // unterminated tail
     }
-    if (subsystem == "pci" && (action == "bind" || action == "unbind" || action == "add" || action == "remove")) gen_++;
+    const bool moved = action == "bind" || action == "unbind" || action == "add" || action == "remove";
+    if (subsystem == "pci" && moved) gen_++;
+    else if (subsystem == "mdev" && moved) mdevGen_++;
 }
 
 uint64_t BindWatcher::generation() {
@@ -173,10 +181,15 @@ uint64_t BindWatcher::generation() {
             continue;
         }
         if (k < 0 && errno == EINTR) continue;
-        if (k < 0 && errno == ENOBUFS) { lost_ = true; gen_ += 1ull << 32; }  // messages were dropped
+        if (k < 0 && errno == ENOBUFS) { lost_ = true; gen_ += 1ull << 32; mdevGen_ += 1ull << 32; }  // messages were dropped
         break;
     }
     return gen_;
+}
+
+uint64_t BindWatcher::mdevGeneration() {
+    generation();  // drains the socket: both counters are fed from the same messages
+    return mdevGen_;
 }
 
 Plugin::~Plugin() {
@@ -450,20 +463,33 @@ Error Plugin::createIommuDeviceMap() {
     deviceClass.clear();
     iommuNuma.clear();
     // the generation is read BEFORE the walk: an event during the walk makes the snapshot stale, never fresh
-    haveSnapshotGen_ = snapshotValidation && bindGeneration && bindGeneration(snapshotGen_);
-    std::vector<kxpu_devrec> recs;
-    Error e = gatherRecordsFast(recs);  // same records as gatherRecords (falls back to it when a seam was replaced)
+    haveWalkGen_ = bindGeneration && bindGeneration(walkGen_);
+    haveSnapshotGen_ = snapshotValidation && haveWalkGen_;
+    snapshotGen_ = walkGen_;
+    PciWalk w;
+    Error e = classifyPci(w);
+    if (e) return e;
+    buildIommuMaps(w, nullptr);
+    pciSnap_ = snapshotOf(w, nullptr);  // host bookkeeping for a later rediscovery: no GPU call
+    pciNext_ = pciSnap_.size();
+    return Error();
+}
+
+// the walk and classify of createIommuDeviceMap
+Error Plugin::classifyPci(PciWalk &w) {
+    Error e = gatherRecordsFast(w.recs);  // same records as gatherRecords (falls back to it when a seam was replaced)
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // Walk's error is ignored by the reference (:132)
+    const std::vector<kxpu_devrec> &recs = w.recs;
     const size_t n = recs.size();
-    std::vector<uint32_t> accept(n), gids(n), goff(n + 1), gmem(n), doff(n + 1), dgrp(n);
-    std::vector<uint64_t> dids(n);
+    w.accept.assign(n, 0); w.gids.assign(n, 0); w.goff.assign(n + 1, 0); w.gmem.assign(n, 0); w.doff.assign(n + 1, 0);
+    w.dgrp.assign(n, 0); w.dids.assign(n, 0);
     kxpu_classify_out out;
     memset(&out, 0, sizeof out);
-    out.accept_index = accept.data(); out.group_ids = gids.data(); out.group_off = goff.data();
-    out.group_members = gmem.data(); out.dev_ids = dids.data(); out.dev_off = doff.data(); out.dev_groups = dgrp.data();
+    out.accept_index = w.accept.data(); out.group_ids = w.gids.data(); out.group_off = w.goff.data();
+    out.group_members = w.gmem.data(); out.dev_ids = w.dids.data(); out.dev_off = w.doff.data(); out.dev_groups = w.dgrp.data();
     const bool dflt = defaultClasses();
-    std::vector<uint8_t> drule(n ? n : 1, 0);
-    std::vector<uint64_t> gnuma(n ? n : 1, 0);
+    w.drule.assign(n ? n : 1, 0);
+    w.gnuma.assign(n ? n : 1, 0);
     int32_t rc;
     if (dflt && !topologyAware) {
         rc = kxpu_classify(ctx_, recs.data(), n, &out);
@@ -477,39 +503,77 @@ Error Plugin::createIommuDeviceMap() {
             strncpy(rules[c].driver, xpuClasses[c].driver.c_str(), sizeof rules[c].driver);
         }
         if (topologyAware) {  // with the default class list: rule {10de, vfio-pci}, kxpu_classify's outputs
-            rc = kxpu_classify_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data(), gnuma.data());
+            rc = kxpu_classify_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, w.drule.data(), w.gnuma.data());
             if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify_topo", rc);
         } else {
-            rc = kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data());
+            rc = kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, w.drule.data());
             if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify_rules", rc);
         }
     }
+    w.nGroups = out.n_groups;
+    w.nDevids = out.n_devids;
+    return Error();
+}
+
+// the class an accepted function itself matched (a group may hold functions of several classes)
+static size_t recordClass(const std::vector<XpuClass> &classes, bool dflt, const kxpu_devrec &r) {
+    if (dflt) return 0;
+    const std::string vendor = trimID(std::string((const char *)r.vendor_txt, r.vendor_len));
+    size_t cls = 0;
+    for (size_t c = 0; c < classes.size(); c++)
+        if (classes[c].vendor == vendor && classes[c].driver == r.driver) cls = c;
+    return cls;
+}
+
+void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
+    iommuMap.clear();
+    deviceMap.clear();
+    iommuClass.clear();
+    deviceClass.clear();
+    iommuNuma.clear();
+    const bool dflt = defaultClasses();
     // class of a group = the rule of its first member, which the device-map entry listing it carries
     std::map<uint32_t, size_t> groupClass;
-    for (uint32_t d = 0; d < out.n_devids; d++)
-        for (uint32_t k = doff[d]; k < doff[d + 1]; k++) groupClass[dgrp[k]] = drule[d];
-    for (uint32_t g = 0; g < out.n_groups; g++) {
+    for (uint32_t d = 0; d < w.nDevids; d++)
+        for (uint32_t k = w.doff[d]; k < w.doff[d + 1]; k++) groupClass[w.dgrp[k]] = w.drule[d];
+    for (uint32_t g = 0; g < w.nGroups; g++) {
         std::vector<NvidiaGpuDevice> devs;
-        for (uint32_t k = goff[g]; k < goff[g + 1]; k++) {
-            uint32_t i = gmem[k];
-            devs.push_back(NvidiaGpuDevice{std::string(recs[i].bdf), accept[i]});  // :171-174
-            if (!dflt) {  // the class this function itself matched (a group may hold functions of several classes)
-                const std::string vendor = trimID(std::string((const char *)recs[i].vendor_txt, recs[i].vendor_len));
-                for (size_t c = 0; c < xpuClasses.size(); c++)
-                    if (xpuClasses[c].vendor == vendor && xpuClasses[c].driver == recs[i].driver) devs.back().xpuClass = c;
-            }
+        for (uint32_t k = w.goff[g]; k < w.goff[g + 1]; k++) {
+            const uint32_t i = w.gmem[k];
+            const uint64_t idx = index ? (*index)[w.accept[i]] : w.accept[i];
+            devs.push_back(NvidiaGpuDevice{std::string(w.recs[i].bdf), idx});  // :171-174
+            devs.back().xpuClass = recordClass(xpuClasses, dflt, w.recs[i]);
         }
-        iommuMap.emplace_back(std::to_string(gids[g]), std::move(devs));
-        iommuClass.push_back(groupClass[gids[g]]);
-        if (topologyAware) iommuNuma.push_back(gnuma[g]);
+        iommuMap.emplace_back(std::to_string(w.gids[g]), std::move(devs));
+        iommuClass.push_back(groupClass[w.gids[g]]);
+        if (topologyAware) iommuNuma.push_back(w.gnuma[g]);
     }
-    for (uint32_t d = 0; d < out.n_devids; d++) {
+    for (uint32_t d = 0; d < w.nDevids; d++) {
         std::vector<std::string> groups;
-        for (uint32_t k = doff[d]; k < doff[d + 1]; k++) groups.push_back(std::to_string(dgrp[k]));  // :169
-        deviceMap.emplace_back(devIdString(dids[d]), std::move(groups));
-        deviceClass.push_back(drule[d]);
+        for (uint32_t k = w.doff[d]; k < w.doff[d + 1]; k++) groups.push_back(std::to_string(w.dgrp[k]));  // :169
+        deviceMap.emplace_back(devIdString(w.dids[d]), std::move(groups));
+        deviceClass.push_back(w.drule[d]);
     }
-    return Error();
+}
+
+// one entry per accepted function in walk order: key = PCI address, tag = its device id text packed as dev_ids packs it
+std::vector<kxpu_snaprec> Plugin::snapshotOf(const PciWalk &w, const std::vector<uint64_t> *index) const {
+    std::vector<kxpu_snaprec> snap;
+    const bool dflt = defaultClasses();
+    for (size_t i = 0; i < w.recs.size(); i++) {
+        if (w.accept[i] == KXPU_REJECTED) continue;
+        const kxpu_devrec &r = w.recs[i];
+        kxpu_snaprec s;
+        memset(&s, 0, sizeof s);
+        memcpy(s.key, r.bdf, strnlen(r.bdf, sizeof r.bdf));
+        s.iommu_group = r.iommu_group;
+        s.klass = (uint32_t)recordClass(xpuClasses, dflt, r);
+        const std::string id = trimID(std::string((const char *)r.device_txt, std::min<size_t>(r.device_len, sizeof r.device_txt)));
+        memcpy(&s.tag, id.data(), std::min<size_t>(id.size(), 8));
+        s.index = index ? (*index)[w.accept[i]] : w.accept[i];
+        snap.push_back(s);
+    }
+    return snap;
 }
 
 // ---------------------------------------------------------------------------- vGPUs (mediated devices)
@@ -609,64 +673,123 @@ Error Plugin::createMdevMap() {
     mdevClass.clear();
     typeClass.clear();
     mdevNuma.clear();
+    mdevSnap_.clear();
+    mdevNext_ = 0;
     if (vgpuClasses.empty()) return Error();  // nothing under mdevBasePath is read
     Error e = checkVgpuClasses();
     if (e) return e;
-    std::vector<kxpu_mdevrec> recs;
-    e = gatherMdevRecords(recs);
+    haveWalkMdevGen_ = mdevGeneration && mdevGeneration(walkMdevGen_);
+    MdevWalk w;
+    e = classifyMdev(w);
+    if (e) return e;
+    buildMdevMaps(w, nullptr);
+    mdevSnap_ = snapshotOf(w, nullptr);
+    mdevNext_ = mdevSnap_.size();
+    return Error();
+}
+
+Error Plugin::classifyMdev(MdevWalk &w) {
+    Error e = gatherMdevRecords(w.recs);
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // like the PCI walk: an unreadable bus is an empty one
+    const std::vector<kxpu_mdevrec> &recs = w.recs;
     const size_t n = recs.size();
-    std::vector<uint32_t> accept(n), gids(n), goff(n + 1), gmem(n), doff(n + 1), dgrp(n);
-    std::vector<uint64_t> dids(n);
-    std::vector<uint8_t> drule(n ? n : 1, 0);
+    w.accept.assign(n, 0); w.gids.assign(n, 0); w.goff.assign(n + 1, 0); w.gmem.assign(n, 0); w.doff.assign(n + 1, 0);
+    w.dgrp.assign(n, 0); w.dids.assign(n, 0);
+    w.drule.assign(n ? n : 1, 0);
     kxpu_classify_out out;
     memset(&out, 0, sizeof out);
-    out.accept_index = accept.data(); out.group_ids = gids.data(); out.group_off = goff.data();
-    out.group_members = gmem.data(); out.dev_ids = dids.data(); out.dev_off = doff.data(); out.dev_groups = dgrp.data();
+    out.accept_index = w.accept.data(); out.group_ids = w.gids.data(); out.group_off = w.goff.data();
+    out.group_members = w.gmem.data(); out.dev_ids = w.dids.data(); out.dev_off = w.doff.data(); out.dev_groups = w.dgrp.data();
     std::vector<kxpu_xpu_rule> rules(vgpuClasses.size());  // one rule per class: rule index == class index
     for (size_t c = 0; c < vgpuClasses.size(); c++) {
         memset(&rules[c], 0, sizeof rules[c]);
         strncpy(rules[c].vendor, vgpuClasses[c].vendor.c_str(), sizeof rules[c].vendor);
         strncpy(rules[c].driver, vgpuClasses[c].driver.c_str(), sizeof rules[c].driver);
     }
-    std::vector<uint64_t> gnuma(n ? n : 1, 0);
-    int32_t rc = topologyAware ? kxpu_classify_mdev_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data(), gnuma.data())
-                               : kxpu_classify_mdev(ctx_, rules.data(), rules.size(), recs.data(), n, &out, drule.data());
+    w.gnuma.assign(n ? n : 1, 0);
+    int32_t rc = topologyAware ? kxpu_classify_mdev_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, w.drule.data(), w.gnuma.data())
+                               : kxpu_classify_mdev(ctx_, rules.data(), rules.size(), recs.data(), n, &out, w.drule.data());
     if (rc != KXPU_OK) return kxfail(ctx_, topologyAware ? "kxpu_classify_mdev_topo" : "kxpu_classify_mdev", rc);
+    w.nGroups = out.n_groups;
+    w.nDevids = out.n_devids;
     std::vector<uint32_t> first(out.n_devids);
-    for (uint32_t d = 0; d < out.n_devids; d++) first[d] = (uint32_t)dids[d];
-    std::vector<uint32_t> koff(first.size() + 1);
+    for (uint32_t d = 0; d < out.n_devids; d++) first[d] = (uint32_t)w.dids[d];
+    w.koff.assign(first.size() + 1, 0);
     size_t need = 0;
-    rc = kxpu_mdev_names(ctx_, recs.data(), n, first.data(), first.size(), nullptr, 0, koff.data(), &need);
+    rc = kxpu_mdev_names(ctx_, recs.data(), n, first.data(), first.size(), nullptr, 0, w.koff.data(), &need);
     if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, "kxpu_mdev_names", rc);
-    std::vector<uint8_t> keys(need ? need : 1);
-    rc = kxpu_mdev_names(ctx_, recs.data(), n, first.data(), first.size(), keys.data(), need, koff.data(), &need);
+    w.keys.assign(need ? need : 1, 0);
+    rc = kxpu_mdev_names(ctx_, recs.data(), n, first.data(), first.size(), w.keys.data(), need, w.koff.data(), &need);
     if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_mdev_names", rc);
+    return Error();
+}
+
+static size_t mdevRecordClass(const std::vector<XpuClass> &classes, const kxpu_mdevrec &r) {
+    const std::string vendor = trimID(std::string((const char *)r.parent_vendor_txt, r.vendor_len));
+    size_t cls = 0;
+    for (size_t c = 0; c < classes.size(); c++)
+        if (classes[c].vendor == vendor && classes[c].driver == std::string(r.driver, strnlen(r.driver, sizeof r.driver))) cls = c;
+    return cls;
+}
+
+void Plugin::buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
+    mdevMap.clear();
+    typeMap.clear();
+    mdevClass.clear();
+    typeClass.clear();
+    mdevNuma.clear();
     std::map<uint32_t, size_t> groupClass;  // class of a group = the rule of its first member
-    for (uint32_t d = 0; d < out.n_devids; d++)
-        for (uint32_t k = doff[d]; k < doff[d + 1]; k++) groupClass[dgrp[k]] = drule[d];
-    for (uint32_t g = 0; g < out.n_groups; g++) {
+    for (uint32_t d = 0; d < w.nDevids; d++)
+        for (uint32_t k = w.doff[d]; k < w.doff[d + 1]; k++) groupClass[w.dgrp[k]] = w.drule[d];
+    for (uint32_t g = 0; g < w.nGroups; g++) {
         std::vector<MdevDevice> devs;
-        for (uint32_t k = goff[g]; k < goff[g + 1]; k++) {
-            const kxpu_mdevrec &r = recs[gmem[k]];
-            MdevDevice m{std::string(r.uuid, sizeof r.uuid), std::string(r.parent, strnlen(r.parent, sizeof r.parent)), accept[gmem[k]], 0};
-            const std::string vendor = trimID(std::string((const char *)r.parent_vendor_txt, r.vendor_len));
-            for (size_t c = 0; c < vgpuClasses.size(); c++)
-                if (vgpuClasses[c].vendor == vendor && vgpuClasses[c].driver == std::string(r.driver, strnlen(r.driver, sizeof r.driver)))
-                    m.vgpuClass = c;
+        for (uint32_t k = w.goff[g]; k < w.goff[g + 1]; k++) {
+            const kxpu_mdevrec &r = w.recs[w.gmem[k]];
+            const uint64_t idx = index ? (*index)[w.accept[w.gmem[k]]] : w.accept[w.gmem[k]];
+            MdevDevice m{std::string(r.uuid, sizeof r.uuid), std::string(r.parent, strnlen(r.parent, sizeof r.parent)), idx, 0};
+            m.vgpuClass = mdevRecordClass(vgpuClasses, r);
             devs.push_back(std::move(m));
         }
-        mdevMap.emplace_back(std::to_string(gids[g]), std::move(devs));
-        mdevClass.push_back(groupClass[gids[g]]);
-        if (topologyAware) mdevNuma.push_back(gnuma[g]);
+        mdevMap.emplace_back(std::to_string(w.gids[g]), std::move(devs));
+        mdevClass.push_back(groupClass[w.gids[g]]);
+        if (topologyAware) mdevNuma.push_back(w.gnuma[g]);
     }
-    for (uint32_t d = 0; d < out.n_devids; d++) {
+    for (uint32_t d = 0; d < w.nDevids; d++) {
         std::vector<std::string> groups;
-        for (uint32_t k = doff[d]; k < doff[d + 1]; k++) groups.push_back(std::to_string(dgrp[k]));
-        typeMap.emplace_back(std::string((const char *)keys.data() + koff[d], koff[d + 1] - koff[d]), std::move(groups));
-        typeClass.push_back(drule[d]);
+        for (uint32_t k = w.doff[d]; k < w.doff[d + 1]; k++) groups.push_back(std::to_string(w.dgrp[k]));
+        typeMap.emplace_back(std::string((const char *)w.keys.data() + w.koff[d], w.koff[d + 1] - w.koff[d]), std::move(groups));
+        typeClass.push_back(w.drule[d]);
     }
-    return Error();
+}
+
+static uint64_t fnv1a64(const std::string &s) {
+    uint64_t h = 0xCBF29CE484222325ull;
+    for (unsigned char c : s) h = (h ^ c) * 0x100000001B3ull;
+    return h;
+}
+
+// one entry per accepted mdev in walk order: key = UUID, tag = FNV-1a 64 of the type key of the resource its group is
+// served under (the type key of the group's device-map entry: known on the host without another GPU call)
+std::vector<kxpu_snaprec> Plugin::snapshotOf(const MdevWalk &w, const std::vector<uint64_t> *index) const {
+    std::map<uint32_t, uint64_t> groupTag;
+    for (uint32_t d = 0; d < w.nDevids; d++) {
+        const uint64_t t = fnv1a64(std::string((const char *)w.keys.data() + w.koff[d], w.koff[d + 1] - w.koff[d]));
+        for (uint32_t k = w.doff[d]; k < w.doff[d + 1]; k++) groupTag[w.dgrp[k]] = t;
+    }
+    std::vector<kxpu_snaprec> snap;
+    for (size_t i = 0; i < w.recs.size(); i++) {
+        if (w.accept[i] == KXPU_REJECTED) continue;
+        const kxpu_mdevrec &r = w.recs[i];
+        kxpu_snaprec s;
+        memset(&s, 0, sizeof s);
+        memcpy(s.key, r.uuid, sizeof r.uuid);
+        s.iommu_group = r.iommu_group;
+        s.klass = (uint32_t)mdevRecordClass(vgpuClasses, r);
+        s.tag = groupTag[r.iommu_group];
+        s.index = index ? (*index)[w.accept[i]] : w.accept[i];
+        snap.push_back(s);
+    }
+    return snap;
 }
 
 size_t Plugin::classOfGroup(const std::string &group) const {
@@ -797,6 +920,52 @@ static Error writeSpecFile(const std::string &file_path, const std::vector<uint8
     return Error();
 }
 
+// The rediscovery writer: nothing when the file already holds these bytes; else <dir>/.<name>.tmp, fsync, rename, so
+// that a reader sees the old document or the new one, never a partial one (a reader that opened the old file keeps
+// reading the old bytes).  The CDI cache only loads *.json / *.yaml, so it ignores the .tmp file.
+static Error writeSpecFileAtomic(const std::string &file_path, const uint8_t *doc, size_t len, bool &written) {
+    written = false;
+    if (FILE *f = fopen(file_path.c_str(), "rb")) {
+        std::vector<uint8_t> old(len + 1);
+        const size_t got = fread(old.data(), 1, len + 1, f);
+        fclose(f);
+        if (got == len && memcmp(old.data(), doc, len) == 0) return Error();
+    }
+    const size_t slash = file_path.find_last_of('/');
+    const std::string dir = slash == std::string::npos ? std::string(".") : file_path.substr(0, slash);
+    const std::string name = slash == std::string::npos ? file_path : file_path.substr(slash + 1);
+    const std::string tmp = dir + "/." + name + ".tmp";
+    int fd = open(tmp.c_str(), O_WRONLY | O_CREAT | O_TRUNC | O_CLOEXEC, 0644);
+    if (fd < 0) return fail("Error creating file " + tmp + ": " + strerror(errno));
+    size_t off = 0;
+    while (off < len) {
+        ssize_t k = write(fd, doc + off, len - off);
+        if (k < 0 && errno == EINTR) continue;
+        if (k <= 0) break;
+        off += (size_t)k;
+    }
+    const bool ok = off == len && fsync(fd) == 0;
+    close(fd);
+    if (!ok || rename(tmp.c_str(), file_path.c_str()) != 0) {
+        const std::string err = strerror(errno);
+        unlink(tmp.c_str());
+        return fail("Error writing file " + file_path + ": " + err);
+    }
+    written = true;
+    return Error();
+}
+
+Error writeSpecFileAtomicForTests(const std::string &file_path, const uint8_t *doc, size_t len, bool &written) {
+    return writeSpecFileAtomic(file_path, doc, len, written);
+}
+
+Error Plugin::writeSpec(const std::string &path, const std::vector<uint8_t> &doc, size_t len, bool &written) {
+    if (!atomicSpecs_) return writeSpecFile(path, doc, len, written);  // start-up: the reference's os.Create path
+    Error e = writeSpecFileAtomic(path, doc.data(), len, written);
+    if (written) specsWritten_.push_back(path);
+    return e;
+}
+
 // generateCDISpec for a class list: one file per class, <stem>.yaml|.json, with that class's kind and only the devices
 // of its groups in ascending index; a class without devices gets the empty document (the reference writes one for
 // zero devices too).
@@ -825,8 +994,9 @@ Error Plugin::generateCDISpecClasses(const OrderedMap<std::vector<NvidiaGpuDevic
         if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_cdi_emit_kind", rc);
         const std::string file_path = cdiConfigPath + xpuClasses[c].cdiFileStem + (fmt == KXPU_FMT_YAML ? ".yaml" : ".json");
         bool written = false;
-        writeSpecFile(file_path, doc, len, written);
-        if (written) { cdiFiles.push_back(file_path); lastCdiFile = file_path; }
+        Error e = writeSpec(file_path, doc, len, written);
+        if (e) return e;
+        if (written || atomicSpecs_) { cdiFiles.push_back(file_path); lastCdiFile = file_path; }
     }
     return Error();
 }
@@ -856,17 +1026,10 @@ Error Plugin::generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m,
     rc = kxpu_cdi_emit(ctx_, fmt, devs.data(), devs.size(), doc.data(), len, &len);
     if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_cdi_emit", rc);
     const std::string file_path = cdiConfigPath + "cdi-vfio-xxxx" + (fmt == KXPU_FMT_YAML ? ".yaml" : ".json");  // :79, spec.go:92
-    FILE *f = fopen(file_path.c_str(), "wb");  // os.Create
-    if (!f) {
-        printf("Error creating file: %s\n", strerror(errno));  // spec.go:95: printed and swallowed
-        return Error();
-    }
-    size_t w = fwrite(doc.data(), 1, len, f);
-    fclose(f);
-    if (w != len) { printf("Error writing to file\n"); return Error(); }
-    lastCdiFile = file_path;
-    cdiFiles.push_back(file_path);
-    printf("Data successfully written to file\n");  // spec.go:126
+    bool written = false;
+    Error e = writeSpec(file_path, doc, len, written);  // os.Create at start-up (spec.go:93-126)
+    if (e) return e;
+    if (written || atomicSpecs_) { lastCdiFile = file_path; cdiFiles.push_back(file_path); }
     return Error();
 }
 
@@ -900,14 +1063,23 @@ Error Plugin::generateMdevCDISpec(const std::string &format) {
         if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_cdi_emit_mdev", rc);
         const std::string file_path = cdiConfigPath + vgpuClasses[c].cdiFileStem + (fmt == KXPU_FMT_YAML ? ".yaml" : ".json");
         bool written = false;
-        writeSpecFile(file_path, doc, len, written);
-        if (written) mdevCdiFiles.push_back(file_path);
+        Error e = writeSpec(file_path, doc, len, written);
+        if (e) return e;
+        if (written || atomicSpecs_) mdevCdiFiles.push_back(file_path);
     }
     return Error();
 }
 
 // createDevicePlugins, device_plugin.go:83-112 (nothing is started: no gRPC here)
 Error Plugin::createDevicePlugins() {
+    std::vector<GenericDevicePlugin> dps;
+    Error e = buildPlugins(dps);
+    devicePlugins.assign(std::make_move_iterator(dps.begin()), std::make_move_iterator(dps.end()));
+    return e;
+}
+
+// the plugin list of the current maps, every device Healthy
+Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
     devicePlugins.clear();
     std::vector<std::string> ids, vendors;
     for (size_t d = 0; d < deviceMap.size(); d++) {
@@ -937,6 +1109,7 @@ Error Plugin::createDevicePlugins() {
         dp.devpluginName = devpluginName;
         dp.devicePath = "/dev/vfio/";                                                          // :105
         dp.socketPath = std::string(kDevicePluginPath) + "kata-xpu-" + devpluginName + ".sock";  // generic:76
+        dp.deviceKey = kv.first;
         devicePlugins.push_back(std::move(dp));
     }
     for (size_t t = 0; t < typeMap.size(); t++) {  // one plugin per (vGPU class, type key)
@@ -948,6 +1121,7 @@ Error Plugin::createDevicePlugins() {
         dp.devpluginName = typeMap[t].first;
         dp.devicePath = "/dev/vfio/";  // an mdev has its own IOMMU group and /dev/vfio/<group>
         dp.socketPath = std::string(kDevicePluginPath) + "kata-xpu-" + dp.devpluginName + ".sock";
+        dp.deviceKey = typeMap[t].first;
         devicePlugins.push_back(std::move(dp));
     }
     return Error();
@@ -965,8 +1139,117 @@ Error Plugin::InitiateDevicePlugin() {
     return createDevicePlugins();  // :52
 }
 
+bool Plugin::discoveryStale() {
+    uint64_t g = 0;
+    bool fresh = haveWalkGen_ && bindGeneration && bindGeneration(g) && g == walkGen_;
+    if (fresh && !vgpuClasses.empty()) fresh = haveWalkMdevGen_ && mdevGeneration && mdevGeneration(g) && g == walkMdevGen_;
+    return !fresh;
+}
+
+// walk, classify and reconcile one kind of walk against its snapshot; the maps get the reconciled indices
+template <typename Walk>
+static Error reconcileWalk(kxpu_ctx *ctx, const Walk &w, const std::vector<kxpu_snaprec> &cur, std::vector<kxpu_snaprec> &snap,
+                           uint64_t &next, kxpu_reconcile_counts &counts, std::vector<uint64_t> &index) {
+    index.assign(cur.size() + 1, 0);
+    const int32_t rc = kxpu_reconcile(ctx, snap.data(), snap.size(), next, cur.data(), cur.size(), index.data(), nullptr,
+                                      nullptr, &counts);
+    if (rc != KXPU_OK) return kxfail(ctx, "kxpu_reconcile", rc);
+    index.resize(cur.size());
+    snap = cur;
+    for (size_t i = 0; i < snap.size(); i++) snap[i].index = index[i];
+    next = counts.next_index_out;
+    (void)w;
+    return Error();
+}
+
+Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
+    std::unique_lock<std::shared_mutex> lock(mu_);
+    report = RediscoverReport();
+    report.pci.next_index_out = pciNext_;
+    report.mdev.next_index_out = mdevNext_;
+    // 1. the generations BEFORE the walks (an event during a walk makes the result stale, never fresh)
+    uint64_t gen = 0, mgen = 0;
+    const bool haveGen = bindGeneration && bindGeneration(gen);
+    const bool haveMgen = !vgpuClasses.empty() && mdevGeneration && mdevGeneration(mgen);
+    // 2.-3. the same walks and classify variants as start-up, reconciled against the snapshots
+    PciWalk pw;
+    Error e = classifyPci(pw);
+    if (e) return e;
+    std::vector<uint64_t> pidx;
+    e = reconcileWalk(ctx_, pw, snapshotOf(pw, nullptr), pciSnap_, pciNext_, report.pci, pidx);
+    if (e) return e;
+    buildIommuMaps(pw, &pidx);
+    if (!vgpuClasses.empty()) {
+        MdevWalk mw;
+        e = classifyMdev(mw);
+        if (e) return e;
+        std::vector<uint64_t> midx;
+        e = reconcileWalk(ctx_, mw, snapshotOf(mw, nullptr), mdevSnap_, mdevNext_, report.mdev, midx);
+        if (e) return e;
+        buildMdevMaps(mw, &midx);
+    }
+    // 4. the CDI specs: a file is rewritten only when its bytes changed, atomically
+    atomicSpecs_ = true;
+    specsWritten_.clear();
+    e = generateCDISpec(iommuMap, format);
+    if (!e) e = generateMdevCDISpec(format);
+    atomicSpecs_ = false;
+    report.cdiFilesWritten = specsWritten_;
+    if (e) return e;
+    // 5. devicePlugins in place: health carried per group, new groups Healthy, new plugins appended
+    std::vector<GenericDevicePlugin> want;
+    e = buildPlugins(want);
+    if (e) return e;
+    std::map<std::string, std::string> healthOf;
+    for (const GenericDevicePlugin &dp : devicePlugins)
+        for (const Device &d : dp.devs) healthOf[d.ID] = d.Health;
+    std::vector<bool> seen(devicePlugins.size(), false);
+    for (GenericDevicePlugin &w : want) {
+        for (Device &d : w.devs) {
+            auto it = healthOf.find(d.ID);
+            if (it != healthOf.end()) d.Health = it->second;
+        }
+        size_t at = devicePlugins.size();
+        for (size_t k = 0; k < devicePlugins.size(); k++) {
+            const GenericDevicePlugin &o = devicePlugins[k];
+            if (!seen[k] && o.vgpu == w.vgpu && o.xpuClass == w.xpuClass && o.deviceKey == w.deviceKey) { at = k; break; }
+        }
+        if (at == devicePlugins.size()) {
+            devicePlugins.push_back(std::move(w));
+            seen.push_back(true);
+            report.addedPlugins.push_back(at);
+            report.changedPlugins.push_back(at);
+            continue;
+        }
+        seen[at] = true;
+        std::vector<Device> &cur = devicePlugins[at].devs;
+        bool same = cur.size() == w.devs.size();
+        for (size_t i = 0; same && i < cur.size(); i++)
+            same = cur[i].ID == w.devs[i].ID && cur[i].Health == w.devs[i].Health && cur[i].numa == w.devs[i].numa;
+        if (!same) {
+            cur = std::move(w.devs);
+            report.changedPlugins.push_back(at);
+        }
+    }
+    for (size_t k = 0; k < seen.size(); k++) {
+        if (seen[k] || devicePlugins[k].devs.empty()) continue;
+        devicePlugins[k].devs.clear();  // every device left: the resource stays, with an empty list
+        report.changedPlugins.push_back(k);
+    }
+    std::sort(report.changedPlugins.begin(), report.changedPlugins.end());
+    // 6. a fresh snapshot generation: Allocate answers from the snapshot again
+    haveWalkGen_ = haveGen;
+    walkGen_ = gen;
+    haveWalkMdevGen_ = haveMgen;
+    walkMdevGen_ = mgen;
+    haveSnapshotGen_ = snapshotValidation && haveGen;
+    snapshotGen_ = gen;
+    return Error();
+}
+
 // Allocate, generic_device_plugin.go:320-355, for one ContainerAllocateRequest
 Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllocateResponse &resp) {
+    std::shared_lock<std::shared_mutex> lock(mu_);  // a rediscovery rebuilds the maps under the exclusive lock
     std::vector<uint64_t> devIndexes;
     const auto &returnedMap = returnIommuMap();
     // snapshot validation (off by default): every device of returnedMap was NVIDIA, bound to vfio-pci and in
@@ -1059,6 +1342,7 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
 }
 
 Error Plugin::ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8_t> &out) {
+    std::shared_lock<std::shared_mutex> lock(mu_);
     std::vector<uint32_t> groups;
     std::vector<uint8_t> healthy;
     std::vector<uint64_t> masks;
@@ -1091,6 +1375,7 @@ DevicePluginOptions Plugin::GetDevicePluginOptions() const {
 
 Error Plugin::GetPreferredAllocation(const GenericDevicePlugin &dp, const std::vector<ContainerPreferredAllocationRequest> &requests,
                                      std::vector<ContainerPreferredAllocationResponse> &responses) {
+    std::shared_lock<std::shared_mutex> lock(mu_);
     responses.clear();
     if (!topologyAware) return Error();  // the reference's empty response (generic_device_plugin.go:378-386)
     std::map<std::string, uint32_t> posOf;
@@ -1160,6 +1445,32 @@ Error HealthWatcher::start() {
         if (dirWd_ < 0) return fail("Unable to add device directory to fsnotify watcher: " + dp_.devicePath + ": " + strerror(errno));
     }
     return Error();
+}
+
+Error HealthWatcher::resync() {
+    if (fd_ < 0) return fail("health watcher not started");
+    std::map<std::string, bool> want;
+    for (const Device &dev : dp_.devs) want[dev.ID] = true;
+    std::map<std::string, bool> have;
+    for (auto it = wdToId_.begin(); it != wdToId_.end();) {
+        if (!want.count(it->second)) {
+            inotify_rm_watch(fd_, it->first);  // the IN_IGNORED that follows finds no entry
+            it = wdToId_.erase(it);
+        } else {
+            have[it->second] = true;
+            ++it;
+        }
+    }
+    Error err;
+    const uint32_t mask = IN_DELETE_SELF | IN_MOVE_SELF | IN_ATTRIB | IN_MODIFY;
+    for (const auto &kv : want) {
+        if (have.count(kv.first)) continue;
+        const std::string devicePath = joinPath(dp_.devicePath, kv.first);
+        int wd = inotify_add_watch(fd_, devicePath.c_str(), mask);
+        if (wd < 0) { err = fail("Unable to add device path to fsnotify watcher: " + devicePath + ": " + strerror(errno)); continue; }
+        wdToId_[wd] = kv.first;
+    }
+    return err;
 }
 
 // ListAndWatch's loops over dpi.devs (:230-234, :239-243): every dev with that ID
@@ -1340,6 +1651,8 @@ int kxh_gather_mdev(const char *mdev_base, const char *classes, kxpu_mdevrec *ou
     return 0;
 }
 
+static std::string dumpState(Plugin *p);
+
 // InitiateDevicePlugin + a JSON dump of the resulting state
 int kxh_init(void *h, const char *format, char *json, size_t cap) {
     Plugin *p = (Plugin *)h;
@@ -1349,6 +1662,22 @@ int kxh_init(void *h, const char *format, char *json, size_t cap) {
     if (!e) e = p->generateMdevCDISpec(format);
     if (!e) e = p->createDevicePlugins();
     if (e) { copy_out(e.message, json, cap); return -1; }
+    return copy_out(dumpState(p) + "}", json, cap);
+}
+
+static void jsnap(std::string &o, const std::vector<kxpu_snaprec> &snap) {
+    o += '[';
+    for (size_t i = 0; i < snap.size(); i++) {
+        if (i) o += ',';
+        o += '['; jstr(o, std::string(snap[i].key, strnlen(snap[i].key, sizeof snap[i].key)));
+        o += ',' + std::to_string(snap[i].iommu_group) + ',' + std::to_string(snap[i].klass) + ',' + std::to_string(snap[i].tag) +
+             ',' + std::to_string(snap[i].index) + ']';
+    }
+    o += ']';
+}
+
+// the state kxh_init reports, without the closing brace
+static std::string dumpState(Plugin *p) {
     std::string o = "{\"iommuMap\":[";
     bool first = true;
     for (const auto &kv : p->iommuMap) {
@@ -1417,8 +1746,45 @@ int kxh_init(void *h, const char *format, char *json, size_t cap) {
     for (size_t i = 0; i < p->typeClass.size(); i++) o += (i ? "," : "") + std::to_string(p->typeClass[i]);
     o += "],\"mdevCdiFiles\":[";
     for (size_t i = 0; i < p->mdevCdiFiles.size(); i++) { if (i) o += ','; jstr(o, p->mdevCdiFiles[i]); }
-    o += "]}";
+    o += "],\"pciSnapshot\":";
+    jsnap(o, p->pciSnapshot());
+    o += ",\"mdevSnapshot\":";
+    jsnap(o, p->mdevSnapshot());
+    o += ",\"pciNext\":" + std::to_string(p->pciNextIndex()) + ",\"mdevNext\":" + std::to_string(p->mdevNextIndex());
+    return o;
+}
+
+// rediscover + kxh_init's state + the report
+int kxh_rediscover(void *h, const char *format, char *json, size_t cap) {
+    Plugin *p = (Plugin *)h;
+    device_plugin::RediscoverReport r;
+    device_plugin::Error e = p->rediscover(r, format);
+    if (e) { copy_out(e.message, json, cap); return -1; }
+    std::string o = dumpState(p) + ",\"report\":{\"changed\":[";
+    for (size_t i = 0; i < r.changedPlugins.size(); i++) o += (i ? "," : "") + std::to_string(r.changedPlugins[i]);
+    o += "],\"added\":[";
+    for (size_t i = 0; i < r.addedPlugins.size(); i++) o += (i ? "," : "") + std::to_string(r.addedPlugins[i]);
+    o += "],\"written\":[";
+    for (size_t i = 0; i < r.cdiFilesWritten.size(); i++) { if (i) o += ','; jstr(o, r.cdiFilesWritten[i]); }
+    o += "]";
+    for (const auto &c : {std::make_pair("pci", &r.pci), std::make_pair("mdev", &r.mdev)}) {
+        o += ",\"" + std::string(c.first) + "\":{\"n_kept\":" + std::to_string(c.second->n_kept) +
+             ",\"n_new\":" + std::to_string(c.second->n_new) + ",\"n_changed\":" + std::to_string(c.second->n_changed) +
+             ",\"n_retired\":" + std::to_string(c.second->n_retired) +
+             ",\"next_index_out\":" + std::to_string(c.second->next_index_out) + "}";
+    }
+    o += "}}";
     return copy_out(o, json, cap);
+}
+int kxh_discovery_stale(void *h) { return ((Plugin *)h)->discoveryStale() ? 1 : 0; }
+// the mdev generation through a seam (tests), like kxh_snapshot_enable's PCI one
+void kxh_mdev_generation_seam(void *h, const uint64_t *generation) {
+    ((Plugin *)h)->mdevGeneration = [generation](uint64_t &g) { g = *generation; return true; };
+}
+int kxh_health_resync(void *w, char *err, size_t errcap) {
+    device_plugin::Error e = ((device_plugin::HealthWatcher *)w)->resync();
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    return 0;
 }
 
 // Allocate for one container request; ids = comma separated IOMMU group ids
@@ -1458,7 +1824,16 @@ uint64_t kxh_uevent_feed(void **w, const char *msg, size_t len) {
     if (msg) bw->feed(msg, len);
     return bw->generation();
 }
+// the mdev counter of the same watcher (kxh_uevent_feed creates it)
+uint64_t kxh_uevent_mdev_generation(void *w) { return ((device_plugin::BindWatcher *)w)->mdevGeneration(); }
 void kxh_uevent_free(void *w) { delete (device_plugin::BindWatcher *)w; }
+// the rediscovery spec writer (CPU tests): 1 = written, 0 = the file already held these bytes, -1 = error
+int kxh_write_spec_atomic(const char *path, const uint8_t *doc, size_t len) {
+    bool written = false;
+    device_plugin::Error e = device_plugin::writeSpecFileAtomicForTests(path, doc, len, written);
+    if (e) return -1;
+    return written ? 1 : 0;
+}
 // the real socket: 0 = opened (and healthy), < 0 = this box does not allow it
 int kxh_uevent_socket_ok() {
     device_plugin::BindWatcher bw;

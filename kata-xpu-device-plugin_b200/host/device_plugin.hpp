@@ -14,8 +14,10 @@
 // cgo shim that replaces this file in production is shown in INTEGRATION.md.
 #pragma once
 #include <cstdint>
+#include <deque>
 #include <functional>
 #include <map>
+#include <shared_mutex>
 #include <string>
 #include <utility>
 #include <vector>
@@ -72,6 +74,7 @@ struct GenericDevicePlugin {
     std::string socketPath;      // DevicePluginPath + "kata-xpu-<name>.sock" (:76)
     std::string devicePath;      // "/dev/vfio/" (device_plugin.go:105)
     std::vector<Device> devs;
+    std::string deviceKey;       // the device id (passthrough) or type key (vgpu) the plugin serves; matches it on rediscovery
 };
 
 // pluginapi.ContainerAllocateResponse as Allocate fills it (generic_device_plugin.go:304-350)
@@ -102,6 +105,8 @@ class HealthWatcher {
     HealthWatcher(const HealthWatcher &) = delete;
     HealthWatcher &operator=(const HealthWatcher &) = delete;
     Error start();             // watcher.Add(devicePath/ID) for every dev (:421-430)
+    // after a rediscovery changed the plugin's device list: watch the IDs that are new, drop the watches of IDs that left
+    Error resync();
     int poll(int timeout_ms);  // #devs whose Health changed in this batch; 0 = none; -1 = error
     uint64_t events() const { return events_; }
 
@@ -132,13 +137,17 @@ class BindWatcher {
     // drains the socket; the generation grows by one per pci bind / unbind / add / remove event and jumps
     // when the kernel reports lost messages (ENOBUFS): then nothing can be said about what was missed
     uint64_t generation();
+    // a separate counter for the mdev bus: grows by one per mdev add / remove / bind / unbind event (a vGPU created or
+    // destroyed), and jumps with generation() on lost messages.  generation() never counts mdev events, so the PCI
+    // snapshot of Allocate stays valid while vGPUs come and go.  Drains the socket like generation().
+    uint64_t mdevGeneration();
     // feeds one raw uevent message (tests; also what generation() calls per datagram)
     void feed(const char *msg, size_t len);
 
   private:
     int fd_ = -1;
     bool lost_ = false;
-    uint64_t gen_ = 0;
+    uint64_t gen_ = 0, mdevGen_ = 0;
 };
 
 // One kind of accelerator the plugin serves (the reference hard-codes the NVIDIA one: nvidiaVendorID
@@ -152,6 +161,33 @@ struct XpuClass {
     std::string cdiFileStem;        // <cdiConfigPath><cdiFileStem>.yaml|.json
 };
 XpuClass defaultXpuClass();  // {"10de", "vfio-pci", "nvidia.com", "nvidia.com/gpu", "cdi-vfio-xxxx"}
+
+// What Plugin::rediscover changed.  Positions are indices into Plugin::devicePlugins.
+struct RediscoverReport {
+    std::vector<size_t> changedPlugins;  // device list changed: re-send ListAndWatch, resync the health watcher
+    std::vector<size_t> addedPlugins;    // new resources: Start and Register them (then they count as changed too)
+    kxpu_reconcile_counts pci{}, mdev{}; // kept / new / changed / retired of each walk, and its next index
+    std::vector<std::string> cdiFilesWritten;  // spec files whose bytes changed (rewritten atomically)
+};
+
+// the atomic spec writer of Plugin::rediscover (exposed for CPU tests)
+Error writeSpecFileAtomicForTests(const std::string &file_path, const uint8_t *doc, size_t len, bool &written);
+
+// One walk's classify result, kept so that the maps can be rebuilt with reconciled indices (host bookkeeping).
+struct PciWalk {
+    std::vector<kxpu_devrec> recs;
+    std::vector<uint32_t> accept, gids, goff, gmem, doff, dgrp;
+    std::vector<uint64_t> dids, gnuma;
+    std::vector<uint8_t> drule;
+    uint32_t nGroups = 0, nDevids = 0;
+};
+struct MdevWalk {
+    std::vector<kxpu_mdevrec> recs;
+    std::vector<uint32_t> accept, gids, goff, gmem, doff, dgrp, koff;
+    std::vector<uint64_t> dids, gnuma;
+    std::vector<uint8_t> drule, keys;
+    uint32_t nGroups = 0, nDevids = 0;
+};
 
 class Plugin {
   public:
@@ -182,6 +218,8 @@ class Plugin {
     std::string mdevBasePath = "/sys/bus/mdev/devices";
     std::function<const OrderedMap<std::vector<MdevDevice>> &()> returnMdevMap;
     std::function<bool(uint64_t &generation)> bindGeneration;
+    // the mdev counterpart (BindWatcher::mdevGeneration by default); read before each mdev walk
+    std::function<bool(uint64_t &generation)> mdevGeneration;
     // NUMA topology (include/kxpu.h, ABI v5).  false (default): nothing named numa_node is opened, the records, the
     // ListAndWatch bytes and the options are the reference's, GetPreferredAllocation answers nothing.  true: the gathers
     // read <entry>/numa_node through readNumaNode (an mdev: its parent's, entry "<uuid>/.."), classify returns a NUMA
@@ -194,7 +232,8 @@ class Plugin {
     // ---- state (device_plugin.go:31,34)
     OrderedMap<std::vector<NvidiaGpuDevice>> iommuMap;  // group id -> devices
     OrderedMap<std::vector<std::string>> deviceMap;     // device id -> iommu groups
-    std::vector<GenericDevicePlugin> devicePlugins;
+    // a deque: a rediscovery appends plugins without moving the others (HealthWatcher holds a reference)
+    std::deque<GenericDevicePlugin> devicePlugins;
     std::string lastCdiFile;
     // class of every iommuMap / deviceMap entry (same positions); all 0 with the default class list
     std::vector<size_t> iommuClass, deviceClass;
@@ -239,6 +278,22 @@ class Plugin {
     Error GetPreferredAllocation(const GenericDevicePlugin &dp, const std::vector<ContainerPreferredAllocationRequest> &requests,
                                  std::vector<ContainerPreferredAllocationResponse> &responses);
 
+    // Runtime rediscovery (include/kxpu.h, kxpu_reconcile).  Under an exclusive lock (Allocate, ListAndWatchBytes and
+    // GetPreferredAllocation take it shared): read the uevent generations, walk and classify as at start-up, reconcile
+    // each walk against its snapshot (a surviving function or mdev keeps its CDI index, every other one gets an index
+    // never handed out before), rebuild the maps, rewrite each CDI spec whose bytes changed (atomically), update
+    // devicePlugins in place (matched by vgpu, class and device key; health carried per group, new groups Healthy, new
+    // plugins appended, a plugin whose devices all left keeps an empty list) and take a fresh snapshot generation.
+    // A restart numbers by walk order again: the index high-water mark is not persisted.
+    Error rediscover(RediscoverReport &report, const std::string &format = "YAML");
+    // has a pci (or, with vGPU classes, an mdev) uevent generation moved since the last walk?  true when it cannot tell
+    bool discoveryStale();
+    // the snapshot of the last walks (kxpu_snaprec per accepted function / mdev in walk order) and their next index
+    const std::vector<kxpu_snaprec> &pciSnapshot() const { return pciSnap_; }
+    const std::vector<kxpu_snaprec> &mdevSnapshot() const { return mdevSnap_; }
+    uint64_t pciNextIndex() const { return pciNext_; }
+    uint64_t mdevNextIndex() const { return mdevNext_; }
+
     // raw gather only (no GPU): exposed for CPU tests of the walk
     Error gatherRecords(std::vector<kxpu_devrec> &recs);
     // the same records, read with openat / readlinkat relative to basePath by several threads
@@ -257,6 +312,22 @@ class Plugin {
     Error generateCDISpecClasses(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, int32_t fmt);
     // first use: kxpu_pciids_join on pinned buffers = file -> table -> row handles of `keys` in one call
     Error loadAndJoin(const std::vector<uint32_t> &keys, std::vector<int32_t> &rows);
+    Error classifyPci(PciWalk &w);
+    Error classifyMdev(MdevWalk &w);
+    // iommuMap / deviceMap (mdevMap / typeMap) of a walk; index == nullptr: busIndex, else index[busIndex]
+    void buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index);
+    void buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index);
+    std::vector<kxpu_snaprec> snapshotOf(const PciWalk &w, const std::vector<uint64_t> *index) const;
+    std::vector<kxpu_snaprec> snapshotOf(const MdevWalk &w, const std::vector<uint64_t> *index) const;
+    Error buildPlugins(std::vector<GenericDevicePlugin> &out);
+    bool atomicSpecs_ = false;  // rediscover: specs are written only when changed, through .tmp + fsync + rename
+    std::vector<std::string> specsWritten_;
+    Error writeSpec(const std::string &path, const std::vector<uint8_t> &doc, size_t len, bool &written);
+    mutable std::shared_mutex mu_;
+    std::vector<kxpu_snaprec> pciSnap_, mdevSnap_;
+    uint64_t pciNext_ = 0, mdevNext_ = 0;
+    bool haveWalkGen_ = false, haveWalkMdevGen_ = false;
+    uint64_t walkGen_ = 0, walkMdevGen_ = 0;
     BindWatcher bindWatcher_;
     bool haveSnapshotGen_ = false;
     uint64_t snapshotGen_ = 0;

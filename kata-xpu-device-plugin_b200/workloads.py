@@ -355,3 +355,77 @@ def topo_dev_numa(n, nodes=4, seed=11):
     two = rng.random(n) < 0.02
     m = np.where(two, m | (np.uint64(1) << ((node + 1) % nodes).astype(np.uint64)), m)
     return np.where(rng.random(n) < 0.05, np.uint64(0), m).astype(np.uint64)
+
+
+# ---------------------------------------------------------------- runtime rediscovery (ABI v6)
+def fnv1a64(data: bytes) -> int:
+    """64-bit FNV-1a: the snapshot tag of an mdev (over its type key)."""
+    h = 0xCBF29CE484222325
+    for c in data:
+        h = ((h ^ c) * 0x100000001B3) & 0xFFFFFFFFFFFFFFFF
+    return h
+
+
+def pack_id_text(txt: bytes) -> int:
+    """An id string (e.g. b"2330") packed little-endian into a u64, NUL padded: what kxpu_classify's dev_ids holds and
+    the snapshot tag of a PCI function."""
+    return int.from_bytes(txt[:8].ljust(8, b"\0"), "little")
+
+
+def snapshot_of_records(recs, accept_index):
+    """The snapshot (SNAPREC_DTYPE) of a PCI walk: one entry per accepted record in walk order, key = bdf, group,
+    klass 0, tag = the packed device id text, index = busIndex."""
+    from .binding import SNAPREC_DTYPE
+    acc = np.nonzero(np.asarray(accept_index) != 0xFFFFFFFF)[0]
+    snap = np.zeros(len(acc), SNAPREC_DTYPE)
+    snap["key"] = recs["bdf"][acc]
+    snap["iommu_group"] = recs["iommu_group"][acc]
+    dl = recs["device_len"][acc].astype(np.int64)
+    txt = recs["device_txt"][acc].copy()
+    txt[:, :6] = txt[:, 2:8]  # readIDFromFile: data[2:], '\n' trimmed
+    txt[:, 6:] = 0
+    pos = np.arange(8)[None, :]
+    keep = pos < np.maximum(dl - 2, 0)[:, None]
+    keep &= np.cumsum(txt == ord("\n"), axis=1) == 0
+    snap["tag"] = np.where(keep, txt, 0).astype(np.uint8).view("<u8").reshape(-1)
+    snap["index"] = np.asarray(accept_index)[acc]
+    return snap
+
+
+def reconcile_pair(seed=3, n=1 << 20, mdev=False):
+    """(prev, cur, next_index) of a rediscovery.  prev: an n-entry accepted snapshot (PCI addresses, or UUIDs with
+    mdev=True) in lexical walk order, indices 0..n-1, next_index = n.  cur: the next walk, with 5 % of prev removed,
+    5 % new keys interleaved in lexical order, and 1 % each with a changed group, a changed class and a changed tag.
+    Tags: packed device id texts (PCI) or FNV-1a 64 of type keys (mdev), a few distinct values."""
+    from .binding import SNAPREC_DTYPE
+    rng = np.random.default_rng(seed)
+    m = n + n // 20
+    if mdev:
+        keys = uuids(m, seed).view("S36").reshape(m)
+        tags = np.array([fnv1a64(b"GRID_T4-%dQ" % k) for k in (1, 2, 4, 8, 16)], np.uint64)
+    else:
+        keys = enumerate_bdfs(m).view("S16").reshape(m)
+        tags = np.array([pack_id_text(b"%04x" % d) for d in (0x2330, 0x2331, 0x20b5, 0x26b9, 0x1db6)], np.uint64)
+    is_new = np.zeros(m, bool)
+    is_new[rng.permutation(m)[:m - n]] = True
+    group = (np.arange(m, dtype=np.int64) >> 1).astype(np.uint32) + 7
+    klass = rng.integers(0, 3, m).astype(np.uint32)
+    tag = tags[rng.integers(0, len(tags), m)]
+    prev = np.zeros(n, SNAPREC_DTYPE)
+    pi = np.nonzero(~is_new)[0]
+    prev["key"], prev["iommu_group"], prev["klass"], prev["tag"] = keys[pi], group[pi], klass[pi], tag[pi]
+    prev["index"] = np.arange(n, dtype=np.uint64)
+    removed = np.zeros(m, bool)
+    removed[pi[rng.permutation(n)[:n // 20]]] = True
+    ci = np.nonzero(~removed)[0]
+    cur = np.zeros(len(ci), SNAPREC_DTYPE)
+    cur["key"], cur["iommu_group"], cur["klass"], cur["tag"] = keys[ci], group[ci], klass[ci], tag[ci]
+    cur["index"] = rng.integers(0, 1 << 62, len(ci), dtype=np.uint64)  # ignored by the call
+    survivors = np.nonzero(~is_new[ci])[0]
+    pick = rng.permutation(len(survivors))[:3 * (n // 100)]
+    g_, k_, t_ = np.array_split(survivors[pick], 3)
+    cur["iommu_group"][g_] += np.uint32(1 << 20)
+    cur["klass"][k_] = (cur["klass"][k_] + 1) % 3
+    tag_pos = {int(v): i for i, v in enumerate(tags)}
+    cur["tag"][t_] = tags[[(tag_pos[int(v)] + 1) % len(tags) for v in cur["tag"][t_]]]
+    return prev, cur, n

@@ -24,6 +24,10 @@ dn = W.topo_dev_numa(20000)
 print("topo groups", tres["n_groups"], mres["n_groups"], "lw", len(kx.lw_encode_topo(tres["group_ids"], None, tres["group_numa"])),
       "pref", len(kx.preferred_allocation(dn, W.topo_requests(dn, n_req=300))),
       len(kx.preferred_allocation(dn, W.topo_requests(dn, n_req=1, avail=20000, size=5000, must_max=3))[0]))
+# rediscovery: index reconciliation over PCI and UUID keys
+for mdev in (False, True):
+    prev, cur, ni = W.reconcile_pair(3, 20000, mdev=mdev)
+    print("reconcile", kx.reconcile(prev, cur, ni)["counts"])
 tab.free()
 # zero-copy join: text, keys and rows in mapped pinned host memory
 h_t, p1 = kx.pinned(len(text)); h_t[:] = np.frombuffer(text, np.uint8)
