@@ -75,6 +75,11 @@ int32_t kx_ctx_create_on(int32_t ordinal, kxpu_ctx **out) {
     c->no_small = getenv("KXPU_NO_SMALL") != nullptr;
     c->no_zero_copy = getenv("KXPU_NO_ZERO_COPY") != nullptr;
     if (const char *sw = getenv("KXPU_SCAN_W")) { const int v = atoi(sw); c->force_scan_w = (v == 8 || v == 16 || v == 32) ? v : 0; }
+    if (const char *el = getenv("KXPU_SCAN_EPOCH_LIMIT")) {  // 2 .. 2^24 in decimal; anything else keeps the default
+        char *end = nullptr;
+        const unsigned long long v = (el[0] >= '0' && el[0] <= '9') ? strtoull(el, &end, 10) : 0;
+        if (end && !*end && v >= 2 && v <= (1ull << 24)) c->scan_epoch_limit = (uint32_t)v;
+    }
     *out = c;
     return KXPU_OK;
 }
@@ -197,7 +202,10 @@ unsigned long long *kx_scan_state(kxpu_ctx *ctx, size_t words) {
     while (want < words) want <<= 1;
     unsigned long long *p = nullptr;
     cudaStreamSynchronize(ctx->stream);  // kernels in flight may still use the old words
-    if (cudaMalloc((void **)&p, want * 8) != cudaSuccess || cudaMemset(p, 0, want * 8) != cudaSuccess) {
+    // Zeroed on the ctx stream, in front of the look-back that asked for the words.  A cudaMemset would run on
+    // the legacy stream, which the non-blocking ctx stream does not wait for; the new memory can hold a destroyed
+    // context's words with the very epochs this context's first calls use.
+    if (cudaMalloc((void **)&p, want * 8) != cudaSuccess || cudaMemsetAsync(p, 0, want * 8, ctx->stream) != cudaSuccess) {
         cudaGetLastError();
         if (p) cudaFree(p);
         KX_SET_ERR(ctx, "cudaMalloc(%zu) for the look-back state failed", want * 8);
@@ -210,7 +218,7 @@ unsigned long long *kx_scan_state(kxpu_ctx *ctx, size_t words) {
 }
 
 uint32_t kx_next_epoch(kxpu_ctx *ctx) {
-    if (++ctx->scan_epoch >= (1u << 24)) {  // 24-bit tag wraps: forget every old word
+    if (++ctx->scan_epoch >= ctx->scan_epoch_limit) {  // the tag wraps: forget every old word
         if (ctx->scan_state) cudaMemsetAsync(ctx->scan_state, 0, ctx->scan_state_words * 8, ctx->stream);
         ctx->scan_epoch = 1;
     }
@@ -825,8 +833,9 @@ extern "C" int32_t kxpu_names(kxpu_ctx *ctx, kxpu_table *t, const int32_t *rows,
                                                                                        t->n_rows, d_lens);
         KX_LAUNCHED(ctx);
         // scanning n+1 items makes offsets[n] the total
-        kxscan::exclusive_scan<uint32_t>(ctx, d_lens, n + 1, d_offs, nullptr);
+        rc = kxscan::exclusive_scan<uint32_t>(ctx, d_lens, n + 1, d_offs, nullptr);
     }
+    if (rc != KXPU_OK) return rc;  // no offsets were computed: nothing to copy or size
     cudaMemcpyAsync(offsets, d_offs, (n + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream);
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) { KX_SET_ERR(ctx, "names failed: %s", cudaGetErrorString(e)); rc = KXPU_E_CUDA; }

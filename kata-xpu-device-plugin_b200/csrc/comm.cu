@@ -392,8 +392,12 @@ static int32_t stage_reserve(kxpu_ctx *ctx, KxExchange *x, const XCaps &want) {
     cudaStreamSynchronize(ctx->stream);
     if (x->stage) { cudaFree(x->stage); x->stage = nullptr; }
     if (x->send_slab) { cudaFree(x->send_slab); x->send_slab = nullptr; }
-    if (!x->scratch && (cudaMalloc((void **)&x->scratch, 256) != cudaSuccess || cudaMemset(x->scratch, 0, 256) != cudaSuccess)) {
+    // zeroed on the ctx stream: the stream is non-blocking, so a legacy-stream cudaMemset would not be ordered
+    // in front of the kernels that read these counters
+    if (!x->scratch && (cudaMalloc((void **)&x->scratch, 256) != cudaSuccess ||
+                        cudaMemsetAsync(x->scratch, 0, 256, ctx->stream) != cudaSuccess)) {
         cudaGetLastError();
+        if (x->scratch) { cudaFree(x->scratch); x->scratch = nullptr; }
         return KXPU_E_NOMEM;
     }
     x->scaps = want;

@@ -45,10 +45,14 @@ struct kxpu_ctx {
     std::vector<KxArena> pool;
     uint32_t cap_hint = 1u << 16;       // table capacity the next load starts with (follows the last text)
     uint32_t blob_hint = 0;             // name blob capacity of the last load (0 = derive from the text size)
-    // tile status words of the single-pass scans / look-backs (scan.cuh): zeroed once, epoch-tagged
+    // tile status words of the single-pass scans / look-backs (scan.cuh): zeroed on the ctx stream when
+    // (re)allocated and when the epoch wraps, epoch-tagged
     unsigned long long *scan_state = nullptr;
     size_t scan_state_words = 0;
     uint32_t scan_epoch = 0;
+    // KXPU_SCAN_EPOCH_LIMIT (2 .. 2^24, else 2^24): epochs run 1 .. limit-1, then the words are zeroed and the
+    // count starts again at 1.  A small limit makes that wrap frequent without changing any result, for tests
+    uint32_t scan_epoch_limit = 1u << 24;
     // host staging of kxpu_pciids_load / kxpu_lookup (grown on demand, kept)
     void *d_stage = nullptr;
     size_t d_stage_bytes = 0;

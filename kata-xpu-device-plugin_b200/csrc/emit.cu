@@ -560,13 +560,13 @@ static int32_t emit_items(kxpu_ctx *ctx, size_t n, size_t in_bytes, const void *
     uint32_t *d_lens = (uint32_t *)(b + o_lens), *d_offs = (uint32_t *)(b + o_offs);
     lenk(b + o_in, h_in2 ? b + o_in2 : nullptr, N, d_lens);
     ctx->launches++;
-    kxscan::exclusive_scan<uint32_t>(ctx, d_lens, n + 1, d_offs, nullptr);
+    int32_t rc = kxscan::exclusive_scan<uint32_t>(ctx, d_lens, n + 1, d_offs, nullptr);
+    if (rc != KXPU_OK) return rc;  // no offsets were computed: nothing to copy or size
     std::vector<uint32_t> tmp;
     uint32_t *h_offs = offsets;
     if (!h_offs) { tmp.resize(n + 1); h_offs = tmp.data(); }
     cudaMemcpyAsync(h_offs, d_offs, (n + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream);
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    int32_t rc = KXPU_OK;
     if (e != cudaSuccess) { KX_SET_ERR(ctx, "emit sizing failed: %s", cudaGetErrorString(e)); rc = KXPU_E_CUDA; }
     const size_t total = rc == KXPU_OK ? h_offs[n] : 0;
     if (need) *need = total;

@@ -3,11 +3,14 @@
 // data dependent (name gather, Allocate names, ListAndWatch bytes, busIndex, radix-sort digit bases).
 //
 // Tile status word (u64): [63:40] call epoch, [39:38] 1 = aggregate / 2 = inclusive prefix,
-// [37:0] value.  The words live in a per-ctx buffer that is zeroed once (kx_scan_state, api.cu) and
-// then only written by these look-backs with increasing epochs: a word whose epoch is not the
-// current call's counts as "not published yet", so nothing is cleared between calls (the buffer is
-// zeroed again when the 24-bit epoch wraps).  Tiles are taken in blockIdx order, which the hardware
-// dispatches in order (the same assumption CUB's scan makes).
+// [37:0] value.  The words live in a per-ctx buffer that is zeroed when it is allocated or grown
+// (kx_scan_state, api.cu) and then only written by these look-backs with increasing epochs: a word
+// whose epoch is not the current call's counts as "not published yet", so nothing is cleared between
+// calls.  When the 24-bit epoch wraps (kx_next_epoch), the whole buffer is zeroed again.  Both zeroings
+// are cudaMemsetAsync on the ctx stream, so they land before the next look-back on that stream reads a
+// word.  KXPU_SCAN_EPOCH_LIMIT (2 .. 2^24, read at context creation) moves the wrap down to that limit,
+// so that tests can run it often; results do not depend on it.  Tiles are taken in blockIdx order,
+// which the hardware dispatches in order (the same assumption CUB's scan makes).
 #pragma once
 #include "common.cuh"
 
@@ -136,15 +139,18 @@ __global__ void __launch_bounds__(SCAN_THREADS) scan_kernel(const uint32_t *__re
     }
 }
 
-// d_total: optional u64 (device)
+// d_total: optional u64 (device).  KXPU_E_NOMEM (ctx->err set, nothing enqueued, d_out untouched) when
+// the status words could not be allocated; kx_scan_state has already cleared the CUDA error, so a later
+// stream sync does not report it: the caller must return this status.
 template <typename OutT>
-static inline void exclusive_scan(kxpu_ctx *ctx, const uint32_t *d_in, size_t n, OutT *d_out, unsigned long long *d_total) {
+static inline int32_t exclusive_scan(kxpu_ctx *ctx, const uint32_t *d_in, size_t n, OutT *d_out, unsigned long long *d_total) {
     size_t nb = (n + SCAN_TILE - 1) / SCAN_TILE;
     if (nb == 0) nb = 1;
     unsigned long long *state = kx_scan_state(ctx, nb);
-    if (!state) return;  // allocation failure: the caller's stream sync reports the CUDA error state; outputs stay untouched
+    if (!state) return KXPU_E_NOMEM;
     scan_kernel<OutT><<<(unsigned)nb, SCAN_THREADS, 0, ctx->stream>>>(d_in, n, d_out, state, kx_next_epoch(ctx), d_total);
     ctx->launches += 1;
+    return KXPU_OK;
 }
 
 }  // namespace kxscan

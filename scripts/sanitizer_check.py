@@ -28,6 +28,43 @@ print("topo groups", tres["n_groups"], mres["n_groups"], "lw", len(kx.lw_encode_
 for mdev in (False, True):
     prev, cur, ni = W.reconcile_pair(3, 20000, mdev=mdev)
     print("reconcile", kx.reconcile(prev, cur, ni)["counts"])
+
+
+# look-back state across epoch wraps (tests/test_gpu_lookback_state.py at reduced sizes): every user of the status
+# words with at least two tiles, on a context whose epoch wraps every two epochs, against the default context
+def lookback_pass(k, t):
+    xr, mr = W.xpu_records(keys, n=4097, seed=7), W.mdev_records(n=4112, seed=7)
+    dn = W.topo_dev_numa(2 * 4096 + 1)
+    big = W.topo_requests(dn, n_req=3, avail=len(dn), size=700, must_max=3, seed=7)
+    small = W.topo_requests(dn, n_req=4, avail=100, size=10, seed=8)
+    prev, cur, ni = W.reconcile_pair(7, 1500)
+    return [k.classify(W.cfg3_records(keys, n=70000, seed=7)), k.classify_rules(W.XPU_RULES, xr),
+            k.classify_mdev(W.MDEV_RULES, mr), k.classify_topo(W.MDEV_RULES, W.topo_mdev_records(n=4112), mdev=True),
+            k.names_blob(t, k.table_export(t)[2][:5000]), k.alloc_names(np.arange(5000, dtype=np.uint64), "amd.com/gpu"),
+            k.mdev_names(mr, np.arange(4100, dtype=np.uint32)), k.lw_encode_topo(xr["iommu_group"], None, np.ones(4097, np.uint64)),
+            k.cdi_emit(0, W.cfg5_devices(300), "amd.com/gpu"), k.cdi_emit_mdev(1, W.mdev_devices(300), "nvidia.com/vgpu"),
+            k.reconcile(prev, cur, ni), k.preferred_allocation(dn, big[:1] + small + big[1:])]
+
+
+def equal(a, b):
+    if isinstance(a, dict):
+        return a.keys() == b.keys() and all(equal(a[x], b[x]) for x in a)
+    if isinstance(a, (list, tuple)):
+        return len(a) == len(b) and all(equal(x, y) for x, y in zip(a, b))
+    if isinstance(a, np.ndarray):
+        return np.array_equal(a, b)
+    return a == b
+
+
+os.environ["KXPU_SCAN_EPOCH_LIMIT"] = "3"
+kw = K.Kxpu(0)
+del os.environ["KXPU_SCAN_EPOCH_LIMIT"]
+tw = kw.pciids_load(text * copies)
+diff = [i for i, (a, b) in enumerate(zip(lookback_pass(kw, tw), lookback_pass(kx, tab))) if not equal(a, b)]
+assert not diff, "calls %s differ across epoch wraps" % diff
+print("look-back pass across epoch wraps: equal")
+tw.free()
+kw.close()
 tab.free()
 # zero-copy join: text, keys and rows in mapped pinned host memory
 h_t, p1 = kx.pinned(len(text)); h_t[:] = np.frombuffer(text, np.uint8)
