@@ -34,6 +34,8 @@ constexpr unsigned long long OFF_MASK = (1ull << 44) - 1;
 // top word:  [63] present, [62:61] 1 vendor (4 hex) / 2 class ("C " + 2 hex) / 0 other, [59:44] id, [43:0] offset
 // tab1 word: [63] present, [62] four hex digits follow the tab, [61] at least two do, [59:44] the four-digit value (or the
 //            two-digit value << 8): parsed without looking at the governing line, which a lane may not know yet; [43:0] offset
+// empty-slot key.  It is also a legal subsystem key (\t\tffff ffff under device ffff of vendor ffff): that key lives
+// in the dedicated slot [cap] behind the probed ones, as key 0xffffffff does in the (vendor,device) table
 constexpr unsigned long long KEY_EMPTY = ~0ull;
 
 struct HSlot { unsigned long long key, line; };
@@ -45,7 +47,7 @@ struct Params {
     unsigned long long *top_state, *tab_state;  // [num_chunks] chunk summaries
     unsigned long long *class_first;            // [256]
     unsigned long long *sub_line;               // [65536] winning subclass line of (class << 8 | subclass)
-    HSlot *hs, *hp;                             // subsystem rows / prog-if rows (first occurrence: atomicMin of the line)
+    HSlot *hs, *hp;                             // subsystem rows [hcap + 1] / prog-if rows [pcap + 1] (first occurrence: atomicMin of the line)
     uint32_t hcap, hshift, pcap, pshift;
     uint32_t *flags;                            // [0] subsystem table overflow, [1] prog-if table overflow
     KxTableDev tab;                             // the finished (vendor,device) table of the same text
@@ -138,6 +140,7 @@ __global__ void __launch_bounds__(WARPS * 32) k_summary(const Params P) {
 }
 
 __device__ __forceinline__ void hash_min(HSlot *hs, uint32_t cap, uint32_t shift, uint32_t *overflow, unsigned long long key, unsigned long long line) {
+    if (key == KEY_EMPTY) { atomicMin(&hs[cap].line, line); return; }
     uint32_t slot = (uint32_t)((key * 0x9E3779B97F4A7C15ull) >> shift);
     for (uint32_t step = 0; step < 2048u && step < cap; step++) {
         const unsigned long long k = __ldcg(&hs[slot].key);
@@ -151,6 +154,7 @@ __device__ __forceinline__ void hash_min(HSlot *hs, uint32_t cap, uint32_t shift
     *overflow = 1u;
 }
 __device__ __forceinline__ unsigned long long hash_get(const HSlot *hs, uint32_t cap, uint32_t shift, unsigned long long key) {
+    if (key == KEY_EMPTY) return hs[cap].line;
     uint32_t slot = (uint32_t)((key * 0x9E3779B97F4A7C15ull) >> shift);
     for (uint32_t step = 0; step < cap; step++) {
         const unsigned long long k = hs[slot].key;
@@ -304,7 +308,7 @@ extern "C" int32_t kxpu_pciids_full_load_device(kxpu_ctx *ctx, const void *d_tex
         while ((1u << plg) < pcap) plg++;
         size_t off = 0;
         auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
-        const size_t o_cf = take(256 * 8), o_sl = take(65536 * 8), o_hs = take((size_t)hcap * sizeof(HSlot)), o_hp = take((size_t)pcap * sizeof(HSlot));
+        const size_t o_cf = take(256 * 8), o_sl = take(65536 * 8), o_hs = take((size_t)(hcap + 1) * sizeof(HSlot)), o_hp = take((size_t)(pcap + 1) * sizeof(HSlot));
         const size_t ff_words = off / 8;
         const size_t o_fl = take(64), o_ts = take((size_t)(num_chunks + 1) * 8), o_ds = take((size_t)(num_chunks + 1) * 8);
         if (cudaMalloc((void **)&f->arena, off) != cudaSuccess) {
@@ -380,11 +384,11 @@ extern "C" int32_t kxpu_full_export(kxpu_ctx *ctx, kxpu_full *f, int32_t kind, u
     if (kind == 1 || kind == 2) {
         const HSlot *d = kind == 1 ? f->P.hs : f->P.hp;
         const uint32_t cnt = kind == 1 ? f->P.hcap : f->P.pcap;
-        std::vector<HSlot> h(cnt);
-        KX_CUDA(ctx, cudaMemcpyAsync(h.data(), d, (size_t)cnt * sizeof(HSlot), cudaMemcpyDeviceToHost, ctx->stream));
+        std::vector<HSlot> h((size_t)cnt + 1);  // + the dedicated slot [cnt], whose key reads KEY_EMPTY
+        KX_CUDA(ctx, cudaMemcpyAsync(h.data(), d, ((size_t)cnt + 1) * sizeof(HSlot), cudaMemcpyDeviceToHost, ctx->stream));
         KX_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-        for (const HSlot &s : h)
-            if (s.key != KEY_EMPTY && s.line != KX_NO_OFF && s.line < tr) rows.emplace_back(s.line, s.key);
+        for (size_t i = 0; i <= cnt; i++)
+            if ((h[i].key != KEY_EMPTY || i == cnt) && h[i].line != KX_NO_OFF && h[i].line < tr) rows.emplace_back(h[i].line, h[i].key);
     }
     std::sort(rows.begin(), rows.end());  // file order
     *n_rows = (uint32_t)rows.size();

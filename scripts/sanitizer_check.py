@@ -66,6 +66,18 @@ print("look-back pass across epoch wraps: equal")
 tw.free()
 kw.close()
 tab.free()
+# full pci.ids model: build, export and lookup of every kind on the real file behind a block with the all-ones
+# subsystem key (ffff ffff under device ffff of vendor ffff); the length is not a multiple of the 2 KiB chunk
+ftext = b"ffff  Illegal\n\tffff  all\n\t\tffff ffff  ones\n\t\tffff fffe  x\n\t\t0000 0000  z\n" + text
+assert len(ftext) % 2048
+d_f = kx.dev_alloc(len(ftext)); kx.upload(d_f, np.frombuffer(ftext, np.uint8))
+t_f = kx.pciids_load_device(d_f, len(ftext))
+full = kx.full_load_device(d_f, len(ftext), t_f)
+for kind in (0, 1, 2):
+    fk, fo = kx.full_export(full, kind)
+    fl = kx.full_lookup(full, kind, np.concatenate([fk, fk ^ np.uint64(32), np.array([(1 << 64) - 1], np.uint64)]))
+    print("full kind", kind, "rows", len(fk), "hits", int((fl >= 0).sum()))
+kx.full_free(full); t_f.free(); kx.dev_free(d_f)
 # zero-copy join: text, keys and rows in mapped pinned host memory
 h_t, p1 = kx.pinned(len(text)); h_t[:] = np.frombuffer(text, np.uint8)
 qq = W.cfg2_queries(keys)

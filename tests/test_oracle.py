@@ -1,5 +1,5 @@
 """CPU tests: the oracle against its pins (golden.json), the format goldens of SURVEY.md
-8a-fmt and an independent Python restatement (pyref.py)."""
+8a-fmt and independent Python restatements (pyref.py, pyref_full.py)."""
 import hashlib
 import json
 import os
@@ -9,8 +9,11 @@ import pytest
 import yaml
 from hypothesis import given, settings, strategies as st
 
+import full_texts
 import pyref
+import pyref_full
 from conftest import GOLDEN
+from pyref import MAX_TOKEN
 
 
 def test_pci_ids_fixture_pinned(pci_text, golden):
@@ -153,6 +156,87 @@ def test_sanitise_property(oracle, s):
     if b"\n" in b:
         return
     assert oracle.sanitise(b) == pyref.sanitise(b)
+
+
+def full_rows_equal(oracle, text):
+    for kind in (0, 1, 2):
+        want = oracle.full_build(text, kind)
+        assert list(zip(want["key"].tolist(), want["line_off"].tolist())) == pyref_full.full_build(text, kind), kind
+
+
+def test_full_model_real_file_vs_python(oracle, pci_text):
+    """kxo_full_build == pyref_full on the real file: every vendor, subsystem and class-section row."""
+    assert [len(pyref_full.full_build(pci_text, k)) for k in (0, 1, 2)] == [2388, 16297, 210]
+    full_rows_equal(oracle, pci_text)
+    full_rows_equal(oracle, pci_text[700000:pci_text.find(b"\n", 1400000) + 1] + pci_text)
+
+
+def test_full_model_edge_texts_vs_python(oracle):
+    texts = full_texts.EDGE_TEXTS + [full_texts.ALL_ONES, full_texts.all_ones_first(), full_texts.seam_text()]
+    texts += full_texts.lookback_texts() + full_texts.length_texts()
+    for t in texts:
+        full_rows_equal(oracle, t)
+    want = oracle.full_build(full_texts.ALL_ONES, 1)
+    assert want["key"].tolist() == full_texts.ALL_ONES_KEYS and want["line_off"].tolist() == full_texts.ALL_ONES_OFFS
+
+
+def test_full_model_cutoff_vs_python(oracle):
+    """A line of 64 KiB or more (a trailing '\\r' counts) ends the scan: no row of any kind at or behind it."""
+    for text, uncut, kept in full_texts.cutoff_texts():
+        full_rows_equal(oracle, text)
+        full_rows_equal(oracle, uncut)
+        at = text.index(b"x" * 1000) - 1
+        got = [oracle.full_build(text, k) for k in (0, 1, 2)]
+        allr = [oracle.full_build(uncut, k) for k in (0, 1, 2)]
+        if kept:
+            assert [len(g) for g in got] == [len(a) for a in allr]
+        else:
+            assert all((g["line_off"] < at).all() for g in got)
+            assert sum(len(g) for g in got) < sum(len(a) for a in allr)
+
+
+FULL_IDS = [b"0000", b"0001", b"00ff", b"abcd", b"fffe", b"ffff", b"00FF", b"ABCD", b"FFFE", b"FFFF"]
+FULL_IDS2 = [b"00", b"01", b"ff", b"FF", b"0g", b"a"]
+
+
+@st.composite
+def full_model_text(draw):
+    """blocks of a top-level line and the lines that follow it, drawn from every line kind of both sections, their
+    malformed forms (uppercase, invalid or too few digits, three tabs), comments, blank lines and CRLF endings"""
+    i4, i2 = st.sampled_from(FULL_IDS), st.sampled_from(FULL_IDS2)
+    top = st.one_of(
+        st.tuples(i4).map(lambda t: t[0] + b"  V"),
+        st.tuples(i2).map(lambda t: b"C " + t[0] + b"  K"),
+        st.tuples(i2, st.sampled_from([b"c ", b"C\t", b"C  ", b"C"])).map(lambda t: t[1] + t[0]),
+        st.sampled_from([b"C ", b"C 0", b"ffff", b"fff", b"", b"zz"]),
+    )
+    body = st.one_of(
+        st.tuples(i4).map(lambda t: b"\t" + t[0] + b"  D"),
+        st.tuples(i4, i4).map(lambda t: b"\t\t" + t[0] + b" " + t[1] + b"  S"),
+        st.tuples(i4, i4).map(lambda t: b"\t\t" + t[0] + b" " + t[1]),
+        st.tuples(i2).map(lambda t: b"\t" + t[0] + b"  SC"),
+        st.tuples(i2).map(lambda t: b"\t\t" + t[0] + b"  PI"),
+        st.tuples(i4, st.integers(0, 3)).map(lambda t: b"\t" + t[0][:t[1]]),
+        st.tuples(i4, i4, st.integers(0, 3)).map(lambda t: b"\t\t" + t[0] + b" " + t[1][:t[2]]),
+        st.tuples(i4, st.integers(0, 3)).map(lambda t: b"\t\t" + t[0][:t[1]]),
+        st.tuples(i4, i4, st.sampled_from([b"", b"\t", b"x"])).map(lambda t: b"\t\t" + t[0] + t[2] + t[1]),
+        st.tuples(i4, i4, st.sampled_from([b"\t\t\t", b"\t\t\t\t"])).map(lambda t: t[2] + t[0] + b" " + t[1]),
+        st.sampled_from([b"\t", b"\t\t", b"# c", b"#", b"#\tffff ffff"]),
+    )
+    blocks = draw(st.lists(st.tuples(top, st.lists(body, max_size=12)), max_size=10))
+    endings = st.sampled_from([b"\n", b"\n", b"\r\n"])
+    lines = [(l, draw(endings)) for t, b in blocks for l in [t] + b]
+    if lines and draw(st.integers(0, 7)) == 0:  # now and then one line of 64 KiB - 1 (kept) or 64 KiB (the scan stops)
+        long = draw(st.sampled_from([b"#" + b"x" * (MAX_TOKEN - 2), b"#" + b"x" * (MAX_TOKEN - 1), b"ffff" + b"x" * (MAX_TOKEN - 4)]))
+        lines.insert(draw(st.integers(0, len(lines))), (long, draw(st.sampled_from([b"\n", b"\r\n"]))))
+    text = b"".join(l + e for l, e in lines)
+    return text[:-1] if draw(st.booleans()) and text else text
+
+
+@settings(max_examples=400, deadline=None)
+@given(full_model_text())
+def test_full_model_property_vs_python(oracle, text):
+    full_rows_equal(oracle, text)
 
 
 def test_cdi_goldens_cfg1(oracle, workloads):
