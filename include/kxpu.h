@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 6
+#define KXPU_ABI_VERSION 7
 
 /* status codes */
 #define KXPU_OK             0
@@ -71,7 +71,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_FINALIZE 1
 #define KXPU_T_LOOKUP   2
 #define KXPU_T_NAMES    3
-#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's kernels: the slot holds the kernels of the most recent of the two */
+#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's and kxpu_pcie_tree's kernels: the slot holds the most recent call's */
 #define KXPU_T_EMIT     5
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
@@ -442,6 +442,75 @@ int32_t kxpu_preferred_allocation(kxpu_ctx *ctx, const uint64_t *dev_numa, size_
                                   const uint32_t *must_off /* [n_req+1] */, const uint32_t *must,
                                   const uint32_t *size /* [n_req] */, size_t n_req,
                                   uint32_t *out /* [sum of size] */, uint32_t *out_off /* [n_req+1] */);
+
+/* ------------------------------------------------- PCIe topology of the groups (ABI v7) */
+
+/* The PCIe path of one kxpu_devrec, a side record at the same index.  128 bytes.  len == 0 means "unknown", so a
+ * zero-filled record is unknown.
+ * Host side: readlink(<basePath>/<bdf>) (on real sysfs e.g.
+ * "../../../devices/pci0000:00/0000:00:01.0/0000:01:00.0/0000:02:00.0/0000:03:00.0"); path holds the target from its
+ * first path component whose name begins with "pci" to the end, len its length.  No such component, a target longer
+ * than 120 bytes from there, or a failed readlink store len = 0; none of these is an error.
+ * Grammar (anything else makes the path unknown, never an error, like numa_node): components separated by a single
+ * '/', no empty component, no trailing '/'; hex digits lowercase;
+ *   host bridge  "pci" <domain> ":" <bus>
+ *   function     <domain> ":" <bus> ":" <dev> "." <fn>
+ * domain = exactly 4 digits, or 5..8 digits with a non-zero first digit (VMD domains such as 10000); bus = 2 digits;
+ * dev = 2 digits, at most 1f; fn = one digit 0..7.  The first component is a host bridge; each later one is a
+ * function or a host bridge (VMD puts pci10000:e0 below an endpoint); the last equals recs[i].bdf byte for byte
+ * (up to its first NUL).  The components before the last are the record's CHAIN, 1..KXPU_PCIE_MAX_DEPTH long; the
+ * depth of a component is its index in the chain.  Node key of a component:
+ *   function     domain << 16 | bus << 8 | dev << 3 | fn
+ *   host bridge  1 << 63 | domain << 16 | bus << 8 */
+typedef struct kxpu_pcipath {
+    char    path[120];
+    uint8_t len;            /* 0..120; 0 = unknown; above 120 counts as unknown */
+    uint8_t reserved[7];
+} kxpu_pcipath;
+#define KXPU_PCIE_MAX_DEPTH 8
+#define KXPU_PCIE_NO_NODE   0xFFFFFFFFu
+
+/* The PCIe forest of a walk.  recs / paths: the n records and paths the classify call saw; group_off [n_groups+1] /
+ * group_members: its iommuMap CSR (kxpu_classify_out).
+ *   - chain of group g = the longest common prefix, key by key, of the chains of its members whose path is known; a
+ *     group none of whose members has a known path has no node;
+ *   - a NODE is a distinct chain prefix (the whole prefix, not its last key), numbered in first-seen order: groups in
+ *     ordinal order, each chain root to leaf, so parent[v] < v;
+ *   - group_node[g] = the last node of g's chain, or KXPU_PCIE_NO_NODE;
+ *   - key[v], parent[v] (KXPU_PCIE_NO_NODE for a root), depth[v] for v < *n_nodes.  key / parent / depth hold
+ *     KXPU_PCIE_MAX_DEPTH * n_groups entries, which bounds the node count.
+ * KXPU_E_INVALID (nothing written) when group_off decreases or a member index is >= n.
+ * GPU: a parse of each path by 16 lanes (vector loads), one longest-common-prefix pass per group, a hash table of
+ * the prefixes (keys compared prefix by prefix on a hit) with an atomic min of the first group, and the ordinals
+ * from the single-pass scan.  Limit (else KXPU_E_UNSUPPORTED): n and n_groups below 2^28. */
+int32_t kxpu_pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
+                       const uint32_t *group_off /* [n_groups+1] */, const uint32_t *group_members, size_t n_groups,
+                       uint32_t *group_node /* [n_groups] */, uint64_t *key, uint32_t *parent, uint8_t *depth,
+                       uint32_t *n_nodes);
+
+/* kxpu_preferred_allocation that keeps an allocation under as few PCIe switches as it can.  dev_node[d] is the node
+ * of device d's group (kxpu_pcie_tree's group_node) or KXPU_PCIE_NO_NODE; parent / depth (n_nodes entries) are the
+ * forest.  Device d lies in node v when v is on the path from dev_node[d] to its root.  Per request, with M the
+ * must-include set, C the candidates (available minus M) and r = size - |M| as in kxpu_preferred_allocation:
+ *   1. avail(v) = the available devices in v, mustin(v) = the must-include devices in v.  v qualifies when
+ *      mustin(v) = |M| and avail(v) >= size.  X is the qualifying node with the smallest key
+ *        (avail(v), -depth(v), avail(parent(v)), avail(grandparent(v)), ..., avail(root), lowest available position in v)
+ *      -- a best fit at every level -- or all devices when no node qualifies.
+ *   2. The candidates in X are ranked by lca, deepest first, then by NUMA bin (kxpu_preferred_allocation's order,
+ *      c[k] counted over the candidates in X), then by position.  lca(c) = the greatest depth of a node holding c and
+ *      at least one must-include device; "none" (every candidate when M is empty) ranks after depth 0.
+ *   3. The answer is M in request order followed by the first r candidates of X in that order.
+ * KXPU_E_INVALID (and no output): every case of kxpu_preferred_allocation; dev_node[d] >= n_nodes other than
+ * KXPU_PCIE_NO_NODE; parent[v] >= v other than KXPU_PCIE_NO_NODE; depth[v] != depth[parent[v]] + 1, or != 0 for a
+ * root; depth[v] >= KXPU_PCIE_MAX_DEPTH.
+ * dev_node == NULL, or every entry KXPU_PCIE_NO_NODE, gives kxpu_preferred_allocation's answer byte for byte.
+ * Shapes, limits and out_off as kxpu_preferred_allocation; n_nodes below 2^31. */
+int32_t kxpu_preferred_allocation_pcie(kxpu_ctx *ctx, const uint64_t *dev_numa, const uint32_t *dev_node, size_t n_devs,
+                                       const uint32_t *parent, const uint8_t *depth, size_t n_nodes,
+                                       const uint32_t *avail_off /* [n_req+1] */, const uint32_t *avail,
+                                       const uint32_t *must_off /* [n_req+1] */, const uint32_t *must,
+                                       const uint32_t *size /* [n_req] */, size_t n_req,
+                                       uint32_t *out /* [sum of size] */, uint32_t *out_off /* [n_req+1] */);
 
 /* ------------------------------------------------- runtime rediscovery (ABI v6) */
 

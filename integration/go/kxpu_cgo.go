@@ -17,6 +17,7 @@ import (
 	"fmt"
 	"os"
 	"runtime"
+	"strings"
 	"unsafe"
 
 	pluginapi "k8s.io/kubelet/pkg/apis/deviceplugin/v1beta1"
@@ -431,6 +432,96 @@ func (k *kxpu) preferredAllocation(masks []uint64, avail, must [][]uint32, size 
 		(*C.uint32_t)(unsafe.Pointer(&a[0])), (*C.uint32_t)(unsafe.Pointer(&moff[0])), (*C.uint32_t)(unsafe.Pointer(&m[0])),
 		(*C.uint32_t)(unsafe.Pointer(&sz[0])), C.size_t(nreq), (*C.uint32_t)(unsafe.Pointer(&out[0])),
 		(*C.uint32_t)(unsafe.Pointer(&ooff[0]))))
+	res := make([][]uint32, nreq)
+	for q := 0; err == nil && q < nreq; q++ {
+		res[q] = out[ooff[q]:ooff[q+1]]
+	}
+	return res, err
+}
+
+// PCIe topology (ABI v7).  With pcieTopology on, the PCI walk also runs os.Readlink(<basePath>/<entry>) per entry and
+// keeps the target from its first component that begins with "pci" (pciPath); after classify, pcieTree builds the walk's
+// forest, every passthrough pluginapi.Device keeps its group's node beside it, GetDevicePluginOptions reports
+// GetPreferredAllocationAvailable, and GetPreferredAllocation of a passthrough plugin calls
+// preferredAllocationPcie with the forest shared by all plugins of the walk (vGPU plugins keep preferredAllocation).
+
+// the kxpu_pcipath of one link target: unknown (len 0) without a "pci" component or past 120 bytes
+func pciPath(target string) C.kxpu_pcipath {
+	var p C.kxpu_pcipath
+	for at := 0; at < len(target); {
+		if strings.HasPrefix(target[at:], "pci") {
+			if rest := target[at:]; len(rest) <= len(p.path) {
+				for i := 0; i < len(rest); i++ {
+					p.path[i] = C.char(rest[i])
+				}
+				p.len = C.uint8_t(len(rest))
+			}
+			return p
+		}
+		slash := strings.IndexByte(target[at:], '/')
+		if slash < 0 {
+			break
+		}
+		at += slash + 1
+	}
+	return p
+}
+
+// the forest of a walk: recs / paths at the same indices, goff / gmem the classify CSR of nGroups groups
+func (k *kxpu) pcieTree(recs []C.kxpu_devrec, paths []C.kxpu_pcipath, goff, gmem []uint32, nGroups int) (gnode, parent []uint32,
+	depth []uint8, err error) {
+	capN := 8*nGroups + 1
+	gnode, parent, depth = make([]uint32, nGroups+1), make([]uint32, capN), make([]uint8, capN)
+	key := make([]uint64, capN)
+	var nn C.uint32_t
+	var r unsafe.Pointer
+	var pp *C.kxpu_pcipath
+	if len(recs) > 0 {
+		r, pp = unsafe.Pointer(&recs[0]), &paths[0]
+	}
+	gm := append(gmem, 0) // a valid pointer for an empty walk
+	err = kxCheck(k.ctx, "kxpu_pcie_tree", C.kxpu_pcie_tree(k.ctx, (*C.kxpu_devrec)(r), pp, C.size_t(len(recs)),
+		(*C.uint32_t)(unsafe.Pointer(&goff[0])), (*C.uint32_t)(unsafe.Pointer(&gm[0])), C.size_t(nGroups),
+		(*C.uint32_t)(unsafe.Pointer(&gnode[0])), (*C.uint64_t)(unsafe.Pointer(&key[0])),
+		(*C.uint32_t)(unsafe.Pointer(&parent[0])), (*C.uint8_t)(unsafe.Pointer(&depth[0])), &nn))
+	return gnode[:nGroups], parent[:nn], depth[:nn], err
+}
+
+// pcieTree over records that carry only their address, one per link target (walk order): what pcieTree sees of a walk
+func (k *kxpu) pcieTreeOfLinks(bdfs, targets []string, goff, gmem []uint32) (gnode, parent []uint32, depth []uint8, err error) {
+	recs, paths := make([]C.kxpu_devrec, len(bdfs)), make([]C.kxpu_pcipath, len(bdfs))
+	for i, b := range bdfs {
+		for j := 0; j < len(b) && j < len(recs[i].bdf)-1; j++ {
+			recs[i].bdf[j] = C.char(b[j])
+		}
+		paths[i] = pciPath(targets[i])
+	}
+	return k.pcieTree(recs, paths, goff, gmem, len(goff)-1)
+}
+
+// preferredAllocation with each device's PCIe node (nodes[d] of dpi.devs[d]) and the walk's forest
+func (k *kxpu) preferredAllocationPcie(masks []uint64, nodes, parent []uint32, depth []uint8, avail, must [][]uint32,
+	size []uint32) ([][]uint32, error) {
+	nreq := len(size)
+	aoff, moff := make([]uint32, nreq+1), make([]uint32, nreq+1)
+	var a, m []uint32
+	total := 0
+	for q := 0; q < nreq; q++ {
+		a, m = append(a, avail[q]...), append(m, must[q]...)
+		aoff[q+1], moff[q+1] = uint32(len(a)), uint32(len(m))
+		total += int(size[q])
+	}
+	a, m = append(a, 0), append(m, 0) // valid pointers for empty lists
+	masks, nodes = append(masks, 0), append(nodes, 0xFFFFFFFF)
+	par, dep := append(parent, 0), append(depth, 0)
+	sz := append(size, 0)
+	out, ooff := make([]uint32, total+1), make([]uint32, nreq+1)
+	err := kxCheck(k.ctx, "kxpu_preferred_allocation_pcie", C.kxpu_preferred_allocation_pcie(k.ctx,
+		(*C.uint64_t)(unsafe.Pointer(&masks[0])), (*C.uint32_t)(unsafe.Pointer(&nodes[0])), C.size_t(len(masks)-1),
+		(*C.uint32_t)(unsafe.Pointer(&par[0])), (*C.uint8_t)(unsafe.Pointer(&dep[0])), C.size_t(len(parent)),
+		(*C.uint32_t)(unsafe.Pointer(&aoff[0])), (*C.uint32_t)(unsafe.Pointer(&a[0])), (*C.uint32_t)(unsafe.Pointer(&moff[0])),
+		(*C.uint32_t)(unsafe.Pointer(&m[0])), (*C.uint32_t)(unsafe.Pointer(&sz[0])), C.size_t(nreq),
+		(*C.uint32_t)(unsafe.Pointer(&out[0])), (*C.uint32_t)(unsafe.Pointer(&ooff[0]))))
 	res := make([][]uint32, nreq)
 	for q := 0; err == nil && q < nreq; q++ {
 		res[q] = out[ooff[q]:ooff[q+1]]

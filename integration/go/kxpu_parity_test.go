@@ -179,3 +179,52 @@ func TestKxpuListAndWatchTopology(t *testing.T) {
 		t.Fatalf("topology wire bytes differ:\n got %x\nwant %s", got, want)
 	}
 }
+
+// kxpu_preferred_allocation_pcie on the worked example of include/kxpu.h (tests/pcie_example.py): two sockets, a host
+// bridge each with two root ports, a switch under each root port and two GPUs under each switch; groups 10-13 on NUMA
+// node 0, 20-23 on node 1, positions 0..7.  The answers are the C oracle's (oracle/kxpu_pcie_oracle.c).
+func TestKxpuPreferredAllocationPcie(t *testing.T) {
+	k, err := newKxpu(0)
+	if err != nil {
+		t.Skip(err)
+	}
+	var bdfs, targets []string
+	for _, hb := range []int{0x00, 0x80} {
+		// root port, switch, down port, GPU (bus offsets from the host bridge's bus)
+		ports := [][4]string{{"%02x:01.0", "%02x:00.0", "%02x:00.0", "%02x:00.0"}, {"%02x:01.0", "%02x:00.0", "%02x:01.0", "%02x:00.0"},
+			{"%02x:02.0", "%02x:00.0", "%02x:00.0", "%02x:00.0"}, {"%02x:02.0", "%02x:00.0", "%02x:01.0", "%02x:00.0"}}
+		buses := [][4]int{{0, 1, 2, 3}, {0, 1, 2, 4}, {0, 5, 6, 7}, {0, 5, 6, 8}}
+		for i, r := range ports {
+			var c [4]string
+			for j := range r {
+				c[j] = fmt.Sprintf(r[j], hb+buses[i][j])
+			}
+			bdf := "0000:" + c[3]
+			bdfs = append(bdfs, bdf)
+			targets = append(targets, fmt.Sprintf("../../../devices/pci0000:%02x/0000:%s/0000:%s/0000:%s/%s", hb, c[0], c[1], c[2], bdf))
+		}
+	}
+	nodes, parent, depth, err := k.pcieTreeOfLinks(bdfs, targets, []uint32{0, 1, 2, 3, 4, 5, 6, 7, 8}, []uint32{0, 1, 2, 3, 4, 5, 6, 7})
+	if err != nil || len(parent) != 18 {
+		t.Fatalf("pcieTree: %v, %d nodes", err, len(parent))
+	}
+	masks := []uint64{1, 1, 1, 1, 2, 2, 2, 2}
+	all := []uint32{0, 1, 2, 3, 4, 5, 6, 7}
+	but := func(x uint32) []uint32 {
+		var r []uint32
+		for _, p := range all {
+			if p != x {
+				r = append(r, p)
+			}
+		}
+		return r
+	}
+	avail := [][]uint32{all, but(0), but(0), but(2), all, all}
+	must := [][]uint32{nil, nil, nil, nil, {2}, nil}
+	size := []uint32{2, 2, 1, 1, 3, 5}
+	want := [][]uint32{{0, 1}, {2, 3}, {1}, {3}, {2, 3, 0}, {0, 1, 2, 3, 4}}
+	got, err := k.preferredAllocationPcie(masks, nodes, parent, depth, avail, must, size)
+	if err != nil || fmt.Sprint(got) != fmt.Sprint(want) {
+		t.Fatalf("preferredAllocationPcie: %v %v, want %v", got, err, want)
+	}
+}

@@ -45,6 +45,11 @@ RC_COUNTS_DTYPE = np.dtype([("n_kept", "<u8"), ("n_new", "<u8"), ("n_changed", "
                             ("next_index_out", "<u8")])
 assert SNAPREC_DTYPE.itemsize == 64 and RC_COUNTS_DTYPE.itemsize == 40
 RC_KEPT, RC_NEW, RC_CHANGED, RC_RETIRED = 0, 1, 2, 3
+# kxpu_pcipath (PCIe topology, ABI v7): one per kxpu_devrec, at the same index
+PCIPATH_DTYPE = np.dtype([("path", "S120"), ("len", "u1"), ("reserved", "u1", (7,))])
+assert PCIPATH_DTYPE.itemsize == 128
+PCIE_MAX_DEPTH = 8
+PCIE_NO_NODE = 0xFFFFFFFF
 
 # every symbol include/kxpu.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -59,7 +64,7 @@ ABI_SYMBOLS = [
     "kxpu_classify_mdev", "kxpu_mdev_names", "kxpu_cdi_emit_mdev",
     "kxpu_pciids_full_load_device", "kxpu_full_free", "kxpu_full_export", "kxpu_full_lookup",
     "kxpu_classify_topo", "kxpu_classify_mdev_topo", "kxpu_lw_encode_topo", "kxpu_preferred_allocation",
-    "kxpu_reconcile",
+    "kxpu_reconcile", "kxpu_pcie_tree", "kxpu_preferred_allocation_pcie",
 ]
 
 
@@ -156,6 +161,8 @@ def load_library():
         "kxpu_lw_encode_topo": (i32, [vp, vp, vp, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_preferred_allocation": (i32, [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp, vp]),
         "kxpu_reconcile": (i32, [vp, vp, sz, u64, vp, sz, vp, vp, vp, vp]),
+        "kxpu_pcie_tree": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32)]),
+        "kxpu_preferred_allocation_pcie": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp, sz, vp, vp]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -521,6 +528,49 @@ class Kxpu:
                                                    _ptr(a["avail_off"]), _ptr(a["avail"]), _ptr(a["must_off"]),
                                                    _ptr(a["must"]), _ptr(a["size"]), len(a["size"]), _ptr(out),
                                                    _ptr(out_off)))
+
+    def pcie_tree(self, recs, paths, group_off, group_members):
+        """kxpu_pcie_tree: recs (DEVREC_DTYPE) and paths (PCIPATH_DTYPE) at the same indices, the group CSR of a classify
+        call.  Returns dict(group_node, key, parent, depth), the forest trimmed to its node count."""
+        recs, paths = np.ascontiguousarray(recs), np.ascontiguousarray(paths)
+        assert recs.dtype == DEVREC_DTYPE and paths.dtype == PCIPATH_DTYPE and len(recs) == len(paths)
+        group_off = np.ascontiguousarray(group_off, dtype=np.uint32)
+        group_members = np.ascontiguousarray(group_members, dtype=np.uint32)
+        G = len(group_off) - 1
+        cap = max(PCIE_MAX_DEPTH * G, 1)
+        gnode = np.empty(max(G, 1), np.uint32)
+        key, parent, depth = np.empty(cap, np.uint64), np.empty(cap, np.uint32), np.empty(cap, np.uint8)
+        nn = C.c_uint32(0)
+        n = len(recs)
+        self._chk(self.L.kxpu_pcie_tree(self.ctx, _ptr(recs) if n else None, _ptr(paths) if n else None, n,
+                                        _ptr(group_off), _ptr(group_members) if len(group_members) else None, G,
+                                        _ptr(gnode), _ptr(key), _ptr(parent), _ptr(depth), C.byref(nn)))
+        m = nn.value
+        return dict(group_node=gnode[:G], key=key[:m], parent=parent[:m], depth=depth[:m])
+
+    def preferred_allocation_pcie(self, dev_numa, dev_node, parent, depth, requests):
+        """kxpu_preferred_allocation_pcie: kxpu_preferred_allocation's requests and answers, with each device's PCIe
+        node (dev_node, None: no PCIe information) and the forest (parent, depth)."""
+        a = pref_requests(requests)
+        out = np.empty(max(int(a["size"].sum()), 1), np.uint32)
+        out_off = np.empty(len(requests) + 1, np.uint32)
+        self.preferred_allocation_pcie_raw(dev_numa, dev_node, parent, depth, a, out, out_off)
+        return [out[out_off[q]:out_off[q + 1]].tolist() for q in range(len(requests))]
+
+    def preferred_allocation_pcie_raw(self, dev_numa, dev_node, parent, depth, a, out, out_off):
+        """The bare call on a pref_requests() dict and caller buffers (timing loops, untouched-output checks)."""
+        dev_numa = np.ascontiguousarray(dev_numa, dtype=np.uint64)
+        if dev_node is not None:
+            dev_node = np.ascontiguousarray(dev_node, dtype=np.uint32)
+            assert len(dev_node) == len(dev_numa)
+        parent = np.ascontiguousarray(parent, dtype=np.uint32)
+        depth = np.ascontiguousarray(depth, dtype=np.uint8)
+        n = len(dev_numa)
+        self._chk(self.L.kxpu_preferred_allocation_pcie(
+            self.ctx, _ptr(dev_numa) if n else None, _ptr(dev_node) if dev_node is not None and n else None, n,
+            _ptr(parent) if len(parent) else None, _ptr(depth) if len(depth) else None, len(parent),
+            _ptr(a["avail_off"]), _ptr(a["avail"]), _ptr(a["must_off"]), _ptr(a["must"]), _ptr(a["size"]),
+            len(a["size"]), _ptr(out), _ptr(out_off)))
 
     def reconcile(self, prev, cur, next_index):
         """kxpu_reconcile: prev / cur are SNAPREC_DTYPE arrays.  Returns dict(index, cur_state, prev_state, counts),

@@ -1,0 +1,317 @@
+// pcie.cu -- K10: the PCIe forest of a walk (kxpu_pcie_tree).  include/kxpu.h states the path grammar and the tree.
+//
+// Five kernels and one scan:
+//   - k_parse: 16 lanes per 128-byte kxpu_pcipath (two records per warp).  Eight lanes load the record with one 16-byte
+//     vector load each; lane j then finds and parses component j of the path (at most 9 components: 8 of chain, the
+//     function itself), a ballot over the 16 lanes decides "known", and lane j stores key j of the record's chain.
+//   - k_lcp: one thread per group: the longest common prefix of its members' chains (member indices checked).
+//   - k_insert: one thread per group inserts each prefix of its chain into an open-addressing table of u64 slots
+//     (group << 3 | depth).  A slot is claimed by CAS; a hit compares the two prefixes key by key through the groups'
+//     chains and then takes the atomic min, so every slot ends up naming the FIRST group with that prefix.  A slot's
+//     group only ever changes to another group with the same prefix, so the comparison stays valid throughout.
+//   - k_count: a group's prefixes whose first group is itself are its new nodes: always a suffix of its chain.
+//   - the single-pass scan (scan.cuh) of the new-node counts gives each group's first ordinal; the total is n_nodes.
+//   - k_emit: ordinal of prefix (g, t) = base[f] + t - (len(f) - new(f)), f its first group; a group writes key,
+//     parent and depth of its own new nodes and its group_node.
+#include <algorithm>
+
+#include "common.cuh"
+#include "scan.cuh"
+
+namespace kxpcie {
+
+constexpr uint32_t NO_NODE = KXPU_PCIE_NO_NODE;
+constexpr int MAXD = KXPU_PCIE_MAX_DEPTH;
+constexpr int PATH_LANES = 16;
+constexpr int PARSE_THREADS = 256;
+constexpr int PARSE_RECS = PARSE_THREADS / PATH_LANES;
+constexpr unsigned long long HOST_BRIDGE = 1ull << 63;
+constexpr unsigned long long EMPTY = ~0ull;
+
+__device__ __forceinline__ int hexv(char c) {
+    return (c >= '0' && c <= '9') ? c - '0' : (c >= 'a' && c <= 'f') ? c - 'a' + 10 : -1;
+}
+
+// component t[s, e): 0 = not a component, 1 = function, 2 = host bridge; *key its node key
+__device__ int parse_comp(const char *t, int s, int e, unsigned long long *key) {
+    bool hb = false;
+    if (e - s >= 3 && t[s] == 'p' && t[s + 1] == 'c' && t[s + 2] == 'i') { hb = true; s += 3; }
+    int c = s;
+    unsigned long long dom = 0;
+    while (c < e && c - s < 9 && t[c] != ':') {
+        const int v = hexv(t[c]);
+        if (v < 0) return 0;
+        dom = dom << 4 | (unsigned)v;
+        c++;
+    }
+    const int dl = c - s;
+    if (!(dl == 4 || (dl >= 5 && dl <= 8 && t[s] != '0'))) return 0;
+    if (c >= e || t[c] != ':' || e - c < 3) return 0;
+    const int b0 = hexv(t[c + 1]), b1 = hexv(t[c + 2]);
+    if (b0 < 0 || b1 < 0) return 0;
+    const unsigned long long bus = (unsigned)(b0 << 4 | b1);
+    c += 3;
+    if (hb) {
+        if (c != e) return 0;
+        *key = HOST_BRIDGE | dom << 16 | bus << 8;
+        return 2;
+    }
+    if (e - c != 5 || t[c] != ':' || t[c + 3] != '.') return 0;
+    const int d0 = hexv(t[c + 1]), d1 = hexv(t[c + 2]), f = t[c + 4] - '0';
+    if (d0 < 0 || d1 < 0 || f < 0 || f > 7 || (d0 << 4 | d1) > 0x1f) return 0;
+    *key = dom << 16 | bus << 8 | (unsigned long long)(d0 << 4 | d1) << 3 | (unsigned)f;
+    return 1;
+}
+
+// chain[i * MAXD + t] = key of component t of record i, clen[i] = chain length (0: unknown path)
+__global__ void __launch_bounds__(PARSE_THREADS) k_parse(const kxpu_devrec *__restrict__ recs, const kxpu_pcipath *__restrict__ paths,
+                                                         uint32_t n, unsigned long long *__restrict__ chain, uint8_t *__restrict__ clen) {
+    __shared__ __align__(16) char txt[PARSE_RECS][128];
+    const uint32_t lane = threadIdx.x & (PATH_LANES - 1), slot = threadIdx.x / PATH_LANES;
+    const uint32_t i = blockIdx.x * PARSE_RECS + slot;
+    const bool have = i < n;
+    if (have && lane < 8) reinterpret_cast<uint4 *>(txt[slot])[lane] = reinterpret_cast<const uint4 *>(paths + i)[lane];
+    __syncwarp();
+    const char *t = txt[slot];
+    const int len = have ? (uint8_t)t[120] : 0;
+    bool ok = len > 0 && len <= 120;
+    // component `lane`: [s, e); n_comp = slashes + 1
+    int s = 0, e = len, slashes = 0;
+    if (ok) {
+        for (int c = 0; c < len; c++) {
+            if (t[c] != '/') continue;
+            if (slashes == (int)lane - 1) s = c + 1;
+            if (slashes == (int)lane) e = c;
+            slashes++;
+        }
+    }
+    const int ncomp = slashes + 1;
+    ok = ok && ncomp >= 2 && ncomp <= MAXD + 1;
+    bool mine = true;
+    unsigned long long key = 0;
+    if (ok && (int)lane < ncomp) {
+        const int kind = parse_comp(t, s, e, &key);
+        if (lane == 0) mine = kind == 2;
+        else mine = kind != 0;
+        if ((int)lane == ncomp - 1 && mine) {  // the function itself: equals the record's bdf
+            const char *b = recs[i].bdf;
+            int bl = 0;
+            while (bl < 16 && b[bl]) bl++;
+            mine = e - s == bl;
+            for (int k = 0; mine && k < bl; k++) mine = t[s + k] == b[k];
+        }
+    }
+    const uint32_t half = (threadIdx.x & 31u) & ~(uint32_t)(PATH_LANES - 1);
+    const uint32_t bad = (__ballot_sync(0xffffffffu, !mine) >> half) & 0xffffu;
+    ok = ok && bad == 0;
+    if (!have) return;
+    if (ok && (int)lane < ncomp - 1) chain[(size_t)i * MAXD + lane] = key;
+    if (lane == 0) clen[i] = ok ? (uint8_t)(ncomp - 1) : 0;
+}
+
+struct Tree {
+    const uint32_t *goff, *gmem;
+    uint32_t n, G;
+    const unsigned long long *chain;
+    const uint8_t *clen;
+    unsigned long long *gchain;  // [G * MAXD]
+    uint8_t *glen;               // [G]
+    unsigned long long *slots;   // [mask + 1]
+    uint32_t mask;
+    uint32_t *first;             // [G * MAXD] first group of prefix (g, t)
+    uint32_t *cnt, *base;        // [G] new nodes of g, their first ordinal
+    uint32_t *group_node, *parent;
+    unsigned long long *key;
+    uint8_t *depth;
+    uint32_t *err;               // [0] = 1: a member index >= n
+};
+
+__global__ void __launch_bounds__(256) k_lcp(const Tree T) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= T.G) return;
+    unsigned long long k[MAXD];
+    int L = -1;
+    bool bad = false;
+    for (uint32_t m = T.goff[g]; m < T.goff[g + 1]; m++) {
+        const uint32_t i = T.gmem[m];
+        if (i >= T.n) { bad = true; continue; }
+        const int l = T.clen[i];
+        if (!l) continue;
+        const unsigned long long *c = T.chain + (size_t)i * MAXD;
+        int nl = L < 0 ? l : min(L, l);
+#pragma unroll
+        for (int t = 0; t < MAXD; t++) {
+            if (t >= nl) continue;
+            const unsigned long long x = c[t];
+            if (L < 0) k[t] = x;
+            else if (x != k[t]) nl = min(nl, t);
+        }
+        L = nl;
+    }
+    if (bad) atomicOr(T.err, 1u);
+    L = max(L, 0);
+#pragma unroll
+    for (int t = 0; t < MAXD; t++)
+        if (t < L) T.gchain[(size_t)g * MAXD + t] = k[t];
+    T.glen[g] = (uint8_t)L;
+}
+
+__device__ __forceinline__ unsigned long long mix(unsigned long long h, unsigned long long x) {
+    h = (h ^ x) * 0x9E3779B97F4A7C15ull;
+    return h ^ (h >> 29);
+}
+
+// slot of prefix (g, t) (the prefix has been inserted when insert = false).  The table has at least two slots per
+// prefix, so a probe sequence always ends; the bound only guarantees that it does (err[1] set, ~0u returned).
+__device__ __forceinline__ uint32_t find_slot(const Tree &T, uint32_t g, int t, unsigned long long h, bool insert) {
+    const unsigned long long *mine = T.gchain + (size_t)g * MAXD;
+    const unsigned long long me = (unsigned long long)g << 3 | (unsigned)t;
+    uint32_t s = (uint32_t)h & T.mask;
+    for (uint32_t probes = 0; probes <= T.mask; probes++, s = (s + 1) & T.mask) {
+        unsigned long long v = *reinterpret_cast<volatile unsigned long long *>(T.slots + s);
+        if (v == EMPTY) {
+            if (!insert) break;
+            v = atomicCAS(T.slots + s, EMPTY, me);
+            if (v == EMPTY) return s;
+        }
+        if ((int)(v & 7u) != t) continue;
+        const unsigned long long *other = T.gchain + (size_t)(v >> 3) * MAXD;
+        bool same = true;
+        for (int u = t; u >= 0 && same; u--) same = other[u] == mine[u];
+        if (!same) continue;
+        if (insert) atomicMin(T.slots + s, me);
+        return s;
+    }
+    atomicOr(T.err + 1, 1u);
+    return ~0u;
+}
+
+__global__ void __launch_bounds__(256) k_insert(const Tree T) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= T.G) return;
+    unsigned long long h = 0x243F6A8885A308D3ull;
+    for (int t = 0; t < T.glen[g]; t++) {
+        h = mix(h, T.gchain[(size_t)g * MAXD + t]);
+        find_slot(T, g, t, h, true);
+    }
+}
+
+__global__ void __launch_bounds__(256) k_count(const Tree T) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= T.G) return;
+    unsigned long long h = 0x243F6A8885A308D3ull;
+    uint32_t fresh = 0;
+    for (int t = 0; t < T.glen[g]; t++) {
+        h = mix(h, T.gchain[(size_t)g * MAXD + t]);
+        const uint32_t s = find_slot(T, g, t, h, false);
+        const uint32_t f = s == ~0u ? g : (uint32_t)(T.slots[s] >> 3);
+        T.first[(size_t)g * MAXD + t] = f;
+        fresh += f == g;
+    }
+    T.cnt[g] = fresh;
+}
+
+__global__ void __launch_bounds__(256) k_emit(const Tree T) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= T.G) return;
+    const int L = T.glen[g];
+    uint32_t prev = NO_NODE;
+    for (int t = 0; t < L; t++) {
+        const uint32_t f = T.first[(size_t)g * MAXD + t];
+        const uint32_t v = T.base[f] + (uint32_t)t - ((uint32_t)T.glen[f] - T.cnt[f]);
+        if (f == g) {
+            T.key[v] = T.gchain[(size_t)g * MAXD + t];
+            T.parent[v] = prev;
+            T.depth[v] = (uint8_t)t;
+        }
+        prev = v;
+    }
+    T.group_node[g] = prev;
+}
+
+}  // namespace kxpcie
+
+using namespace kxpcie;
+
+extern "C" int32_t kxpu_pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
+                                  const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
+                                  uint32_t *group_node, uint64_t *key, uint32_t *parent, uint8_t *depth, uint32_t *n_nodes) {
+    static_assert(sizeof(kxpu_pcipath) == 128 && offsetof(kxpu_pcipath, len) == 120, "kxpu_pcipath layout");
+    if (!ctx || !n_nodes || (n && (!recs || !paths)) || !group_off) return KXPU_E_INVALID;
+    if (n >= (1ull << 28) || n_groups >= (1ull << 28)) return KXPU_E_UNSUPPORTED;
+    *n_nodes = 0;
+    for (size_t g = 0; g < n_groups; g++)
+        if (group_off[g + 1] < group_off[g]) { KX_SET_ERR(ctx, "pcie_tree: group %zu: offsets decrease", g); return KXPU_E_INVALID; }
+    const size_t nm = group_off[n_groups];
+    if ((nm && !group_members) || (n_groups && (!group_node || !key || !parent || !depth))) return KXPU_E_INVALID;
+    if (n_groups == 0) return KXPU_OK;
+    if (nm >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+
+    std::lock_guard<std::mutex> guard(ctx->mu);
+    cudaSetDevice(ctx->device);
+    kx_clear_timings(ctx);
+    const size_t G = n_groups, GD = G * MAXD;
+    uint32_t slots = 1;
+    while (slots < 2 * GD) slots <<= 1;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
+    const size_t o_recs = take(n * sizeof(kxpu_devrec)), o_paths = take(n * sizeof(kxpu_pcipath));
+    const size_t o_goff = take((G + 1) * 4), o_gmem = take(nm * 4), o_chain = take(n * MAXD * 8), o_clen = take(n);
+    const size_t o_gchain = take(GD * 8), o_glen = take(G), o_slots = take((size_t)slots * 8), o_first = take(GD * 4);
+    const size_t o_cnt = take(G * 4), o_base = take(G * 4), o_gnode = take(G * 4), o_parent = take(GD * 4);
+    const size_t o_key = take(GD * 8), o_depth = take(GD), o_err = take(8 + 8);
+    KxScratch sc(ctx);
+    uint8_t *b = nullptr;
+    KX_CUDA(ctx, sc.alloc((void **)&b, off));
+    cudaStream_t st = ctx->stream;
+    auto up = [&](size_t o, const void *h, size_t bytes) { if (bytes) cudaMemcpyAsync(b + o, h, bytes, cudaMemcpyHostToDevice, st); };
+    up(o_recs, recs, n * sizeof(kxpu_devrec)); up(o_paths, paths, n * sizeof(kxpu_pcipath));
+    up(o_goff, group_off, (G + 1) * 4); up(o_gmem, group_members, nm * 4);
+    cudaMemsetAsync(b + o_slots, 0xFF, (size_t)slots * 8, st);
+    cudaMemsetAsync(b + o_err, 0, 16, st);
+    Tree T;
+    T.goff = (const uint32_t *)(b + o_goff); T.gmem = (const uint32_t *)(b + o_gmem);
+    T.n = (uint32_t)n; T.G = (uint32_t)G;
+    T.chain = (const unsigned long long *)(b + o_chain); T.clen = (const uint8_t *)(b + o_clen);
+    T.gchain = (unsigned long long *)(b + o_gchain); T.glen = b + o_glen;
+    T.slots = (unsigned long long *)(b + o_slots); T.mask = slots - 1;
+    T.first = (uint32_t *)(b + o_first); T.cnt = (uint32_t *)(b + o_cnt); T.base = (uint32_t *)(b + o_base);
+    T.group_node = (uint32_t *)(b + o_gnode); T.parent = (uint32_t *)(b + o_parent);
+    T.key = (unsigned long long *)(b + o_key); T.depth = b + o_depth; T.err = (uint32_t *)(b + o_err);
+    unsigned long long *d_total = (unsigned long long *)(b + o_err + 8);
+    {
+        KxTimer tm(ctx, KXPU_T_CLASSIFY);
+        if (n) {
+            k_parse<<<(unsigned)((n + PARSE_RECS - 1) / PARSE_RECS), PARSE_THREADS, 0, st>>>(
+                (const kxpu_devrec *)(b + o_recs), (const kxpu_pcipath *)(b + o_paths), (uint32_t)n,
+                (unsigned long long *)(b + o_chain), b + o_clen);
+            ctx->launches++;
+        }
+        const unsigned gb = (unsigned)((G + 255) / 256);
+        k_lcp<<<gb, 256, 0, st>>>(T);
+        k_insert<<<gb, 256, 0, st>>>(T);
+        k_count<<<gb, 256, 0, st>>>(T);
+        ctx->launches += 3;
+        const int32_t rc = kxscan::exclusive_scan(ctx, T.cnt, G, T.base, d_total);
+        if (rc != KXPU_OK) return rc;
+        k_emit<<<gb, 256, 0, st>>>(T);
+        ctx->launches++;
+    }
+    uint32_t *h = ctx->h_ctl;
+    cudaMemcpyAsync(h, T.err, 16, cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "pcie_tree failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    if (h[0]) { KX_SET_ERR(ctx, "pcie_tree: a group member index is >= n"); return KXPU_E_INVALID; }
+    if (h[1]) { KX_SET_ERR(ctx, "pcie_tree: prefix table overflow"); return KXPU_E_CAPACITY; }
+    const uint32_t nn = h[2];
+    cudaMemcpyAsync(group_node, T.group_node, G * 4, cudaMemcpyDeviceToHost, st);
+    if (nn) {
+        cudaMemcpyAsync(key, T.key, (size_t)nn * 8, cudaMemcpyDeviceToHost, st);
+        cudaMemcpyAsync(parent, T.parent, (size_t)nn * 4, cudaMemcpyDeviceToHost, st);
+        cudaMemcpyAsync(depth, T.depth, nn, cudaMemcpyDeviceToHost, st);
+    }
+    e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "pcie_tree D2H failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    *n_nodes = nn;
+    return KXPU_OK;
+}

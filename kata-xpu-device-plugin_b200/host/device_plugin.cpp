@@ -105,6 +105,34 @@ static bool parseNumaNode(const std::string &raw, uint8_t &node) {
     node = (uint8_t)v;
     return true;
 }
+// readlink(<base>/<entry>): the whole target.  Quiet: a failed read only means "path unknown".
+static bool readPciPathFunc(const std::string &base, const std::string &entry, std::string &out) {
+    char buf[4096];
+    ssize_t k = readlink((base + "/" + entry).c_str(), buf, sizeof buf);
+    if (k < 0 || k == (ssize_t)sizeof buf) return false;
+    out.assign(buf, (size_t)k);
+    return true;
+}
+
+// the host rule of kxpu_pcipath: the target from its first component that begins with "pci"; none, or more than 120
+// bytes from there, leaves the path unknown (len 0)
+static void pciPathRecord(const std::string &target, kxpu_pcipath &p) {
+    memset(&p, 0, sizeof p);
+    for (size_t at = 0; at < target.size();) {
+        if (target.compare(at, 3, "pci") == 0) {
+            const size_t len = target.size() - at;
+            if (len <= sizeof p.path) {
+                memcpy(p.path, target.data() + at, len);
+                p.len = (uint8_t)len;
+            }
+            return;
+        }
+        const size_t slash = target.find('/', at);
+        if (slash == std::string::npos) return;
+        at = slash + 1;
+    }
+}
+
 template <typename ReadNuma>
 static void numaRecord(ReadNuma readNuma, uint8_t &flags, uint8_t &node) {
     std::string s;
@@ -117,6 +145,7 @@ static void numaRecord(ReadNuma readNuma, uint8_t &flags, uint8_t &node) {
 
 Plugin::Plugin(kxpu_ctx *ctx) : ctx_(ctx) {
     readNumaNode = readNumaNodeFunc;
+    readPciPath = readPciPathFunc;
     readLink = readLinkFunc;
     readIDFromFile = readIDFromFileFunc;
     returnIommuMap = [this]() -> const OrderedMap<std::vector<NvidiaGpuDevice>> & { return iommuMap; };
@@ -294,7 +323,8 @@ static Error leafRecord(const std::string &name, const std::vector<XpuClass> &cl
 // filepath.Walk(basePath, ...) (device_plugin.go:132): lexical order, os.Lstat (symlinks are not
 // followed, so a real sysfs entry is "not a directory"), directories are descended into and
 // reported as "Not a device" (:137-140).
-static Error walkDir(Plugin &p, const std::string &path, const std::string &name, std::vector<kxpu_devrec> &recs) {
+static Error walkDir(Plugin &p, const std::string &path, const std::string &name, std::vector<kxpu_devrec> &recs,
+                     std::vector<kxpu_pcipath> *paths) {
     struct stat sb;
     if (lstat(path.c_str(), &sb) != 0) return fail("Error accessing file path \"" + path + "\": " + strerror(errno));  // :133-136
     if (S_ISDIR(sb.st_mode)) {
@@ -308,7 +338,7 @@ static Error walkDir(Plugin &p, const std::string &path, const std::string &name
         closedir(d);
         std::sort(names.begin(), names.end());
         for (const std::string &n : names) {
-            Error e = walkDir(p, path + "/" + n, n, recs);
+            Error e = walkDir(p, path + "/" + n, n, recs, paths);
             if (e) return e;
         }
         return Error();
@@ -323,13 +353,22 @@ static Error walkDir(Plugin &p, const std::string &path, const std::string &name
                          p.topologyAware ? &readNuma : nullptr, r);
     if (e) return e;
     recs.push_back(r);
+    if (paths) {  // pcieTopologyAware: the entry's link, one readlink
+        kxpu_pcipath pp;
+        std::string target;
+        if (p.readPciPath(p.basePath, name, target)) pciPathRecord(target, pp);
+        else memset(&pp, 0, sizeof pp);
+        paths->push_back(pp);
+    }
     return Error();
 }
 
-Error Plugin::gatherRecords(std::vector<kxpu_devrec> &recs) {
+Error Plugin::gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pcipath> *paths) {
     recs.clear();
+    if (paths) paths->clear();
     size_t slash = basePath.find_last_of('/');
-    return walkDir(*this, basePath, slash == std::string::npos ? basePath : basePath.substr(slash + 1), recs);
+    return walkDir(*this, basePath, slash == std::string::npos ? basePath : basePath.substr(slash + 1), recs,
+                   pcieTopologyAware ? paths : nullptr);
 }
 
 // ---------------------------------------------------------------------------- SURVEY 8(f) row 2
@@ -339,8 +378,10 @@ Error Plugin::gatherRecords(std::vector<kxpu_devrec> &recs) {
 // buffering) and by several threads, each filling its own slice of the record table, so that S1 ends
 // in one contiguous table ready for a single H2D copy.  Only with the default seams; real directories
 // under basePath (never on sysfs) go through the generic walk at their position.
-Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads) {
+Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads, std::vector<kxpu_pcipath> *paths) {
     recs.clear();
+    if (paths) paths->clear();
+    if (!pcieTopologyAware) paths = nullptr;
     struct stat sb;
     if (lstat(basePath.c_str(), &sb) != 0) return fail("Error accessing file path \"" + basePath + "\": " + strerror(errno));
     // the fast reads bypass the seams: only when nobody replaced them (tests do, device_plugin.go:38-39)
@@ -348,9 +389,11 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
     SeamFn const *rl = readLink.target<SeamFn>(), *ri = readIDFromFile.target<SeamFn>();
     using NumaFn = bool (*)(const std::string &, const std::string &, std::string &);
     NumaFn const *rn = readNumaNode.target<NumaFn>();
+    NumaFn const *rp = readPciPath.target<NumaFn>();
     const bool defaultSeams = rl && *rl == readLinkFunc && ri && *ri == readIDFromFileFunc &&
-                              (!topologyAware || (rn && *rn == readNumaNodeFunc));
-    if (!S_ISDIR(sb.st_mode) || !defaultSeams) return gatherRecords(recs);
+                              (!topologyAware || (rn && *rn == readNumaNodeFunc)) &&
+                              (!paths || (rp && *rp == readPciPathFunc));
+    if (!S_ISDIR(sb.st_mode) || !defaultSeams) return gatherRecords(recs, paths);
     int basefd = open(basePath.c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
     if (basefd < 0) return fail("Error accessing file path \"" + basePath + "\": " + strerror(errno));
     DIR *d = fdopendir(dup(basefd));
@@ -371,6 +414,7 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
 
     const size_t N = ents.size();
     std::vector<kxpu_devrec> flat(N);
+    std::vector<kxpu_pcipath> flatPaths(paths ? N : 0);
     std::vector<Error> errs(N);
     auto readID = [&](const std::string &name, const char *prop, std::string &out) {
         const std::string rel = name + "/" + prop;
@@ -423,6 +467,12 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
             errs[i] = leafRecord(name, xpuClasses, [&](const char *prop, std::string &out) { return readID(name, prop, out); },
                                  [&](const char *link, std::string &out) { return readLnk(name, link, out); },
                                  topologyAware ? &readNuma : nullptr, flat[i]);
+            if (paths && !errs[i]) {  // the entry's own link on the same directory descriptor
+                char buf[4096];
+                const ssize_t k = readlinkat(basefd, name.c_str(), buf, sizeof buf);
+                if (k >= 0 && k < (ssize_t)sizeof buf) pciPathRecord(std::string(buf, (size_t)k), flatPaths[i]);
+                else memset(&flatPaths[i], 0, sizeof flatPaths[i]);
+            }
         }
     };
     if (threads == 0) threads = std::min(8u, std::max(1u, std::thread::hardware_concurrency()));
@@ -438,11 +488,12 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
     // assemble in walk order; the first error in walk order wins, like the sequential walk
     for (size_t i = 0; i < N; i++) {
         if (ents[i].dir) {
-            Error e = walkDir(*this, basePath + "/" + ents[i].name, ents[i].name, recs);
+            Error e = walkDir(*this, basePath + "/" + ents[i].name, ents[i].name, recs, paths);
             if (e) return e;
         } else {
             if (errs[i]) return errs[i];
             recs.push_back(flat[i]);
+            if (paths) paths->push_back(flatPaths[i]);
         }
     }
     return Error();
@@ -477,7 +528,7 @@ Error Plugin::createIommuDeviceMap() {
 
 // the walk and classify of createIommuDeviceMap
 Error Plugin::classifyPci(PciWalk &w) {
-    Error e = gatherRecordsFast(w.recs);  // same records as gatherRecords (falls back to it when a seam was replaced)
+    Error e = gatherRecordsFast(w.recs, 0, &w.paths);  // same records as gatherRecords (falls back to it when a seam was replaced)
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // Walk's error is ignored by the reference (:132)
     const std::vector<kxpu_devrec> &recs = w.recs;
     const size_t n = recs.size();
@@ -512,6 +563,14 @@ Error Plugin::classifyPci(PciWalk &w) {
     }
     w.nGroups = out.n_groups;
     w.nDevids = out.n_devids;
+    if (pcieTopologyAware) {  // the forest of the walk, one node per group
+        const size_t cap = (size_t)KXPU_PCIE_MAX_DEPTH * w.nGroups + 1;
+        w.gnode.assign(w.nGroups + 1, KXPU_PCIE_NO_NODE);
+        w.nodeKey.assign(cap, 0); w.nodeParent.assign(cap, 0); w.nodeDepth.assign(cap, 0);
+        rc = kxpu_pcie_tree(ctx_, recs.data(), w.paths.data(), n, w.goff.data(), w.gmem.data(), w.nGroups, w.gnode.data(),
+                            w.nodeKey.data(), w.nodeParent.data(), w.nodeDepth.data(), &w.nNodes);
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_pcie_tree", rc);
+    }
     return Error();
 }
 
@@ -531,6 +590,7 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
     iommuClass.clear();
     deviceClass.clear();
     iommuNuma.clear();
+    iommuPcieNode.clear();
     const bool dflt = defaultClasses();
     // class of a group = the rule of its first member, which the device-map entry listing it carries
     std::map<uint32_t, size_t> groupClass;
@@ -547,6 +607,11 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
         iommuMap.emplace_back(std::to_string(w.gids[g]), std::move(devs));
         iommuClass.push_back(groupClass[w.gids[g]]);
         if (topologyAware) iommuNuma.push_back(w.gnuma[g]);
+        if (pcieTopologyAware) iommuPcieNode.push_back(w.gnode[g]);
+    }
+    if (pcieTopologyAware) {
+        pcieParent.assign(w.nodeParent.begin(), w.nodeParent.begin() + w.nNodes);
+        pcieDepth.assign(w.nodeDepth.begin(), w.nodeDepth.begin() + w.nNodes);
     }
     for (uint32_t d = 0; d < w.nDevids; d++) {
         std::vector<std::string> groups;
@@ -1095,12 +1160,18 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         auto it = m.find(g);
         return it == m.end() ? uint64_t(0) : it->second;
     };
+    std::map<std::string, uint32_t> nodeOf;  // group id -> PCIe node (pcieTopologyAware)
+    for (size_t g = 0; g < iommuPcieNode.size() && g < iommuMap.size(); g++) nodeOf[iommuMap[g].first] = iommuPcieNode[g];
+    auto pcieNodeOf = [&](const std::string &g) {
+        auto it = nodeOf.find(g);
+        return it == nodeOf.end() ? KXPU_PCIE_NO_NODE : it->second;
+    };
     size_t at = 0;
     for (const auto &kv : deviceMap) {  // :91
         GenericDevicePlugin dp;
         dp.xpuClass = at < deviceClass.size() ? deviceClass[at] : 0;
         dp.resourceNamespace = xpuClasses[dp.xpuClass].resourceNamespace;
-        for (const std::string &dev : kv.second) dp.devs.push_back(Device{dev, kHealthy, maskOf(numaOf, dev)});  // :93-98
+        for (const std::string &dev : kv.second) dp.devs.push_back(Device{dev, kHealthy, maskOf(numaOf, dev), pcieNodeOf(dev)});  // :93-98
         std::string devpluginName = names[at++];
         if (devpluginName.empty()) {
             fprintf(stderr, "Error: Could not find device name for device id: %s\n", kv.first.c_str());
@@ -1225,7 +1296,8 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         std::vector<Device> &cur = devicePlugins[at].devs;
         bool same = cur.size() == w.devs.size();
         for (size_t i = 0; same && i < cur.size(); i++)
-            same = cur[i].ID == w.devs[i].ID && cur[i].Health == w.devs[i].Health && cur[i].numa == w.devs[i].numa;
+            same = cur[i].ID == w.devs[i].ID && cur[i].Health == w.devs[i].Health && cur[i].numa == w.devs[i].numa &&
+                   cur[i].pcieNode == w.devs[i].pcieNode;
         if (!same) {
             cur = std::move(w.devs);
             report.changedPlugins.push_back(at);
@@ -1369,7 +1441,7 @@ Error Plugin::ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8
 
 DevicePluginOptions Plugin::GetDevicePluginOptions() const {
     DevicePluginOptions o;  // PreStartRequired: false (generic_device_plugin.go:255)
-    o.GetPreferredAllocationAvailable = topologyAware;
+    o.GetPreferredAllocationAvailable = topologyAware || pcieTopologyAware;
     return o;
 }
 
@@ -1377,12 +1449,14 @@ Error Plugin::GetPreferredAllocation(const GenericDevicePlugin &dp, const std::v
                                      std::vector<ContainerPreferredAllocationResponse> &responses) {
     std::shared_lock<std::shared_mutex> lock(mu_);
     responses.clear();
-    if (!topologyAware) return Error();  // the reference's empty response (generic_device_plugin.go:378-386)
+    if (!topologyAware && !pcieTopologyAware) return Error();  // the reference's empty response (generic_device_plugin.go:378-386)
     std::map<std::string, uint32_t> posOf;
     std::vector<uint64_t> numa(dp.devs.size());
+    std::vector<uint32_t> node(dp.devs.size());
     for (size_t d = 0; d < dp.devs.size(); d++) {
         posOf.emplace(dp.devs[d].ID, (uint32_t)d);
         numa[d] = dp.devs[d].numa;
+        node[d] = dp.devs[d].pcieNode;
     }
     std::vector<uint32_t> availOff{0}, mustOff{0}, avail, must, size;
     auto positions = [&](const std::vector<std::string> &ids, std::vector<uint32_t> &to) {
@@ -1405,9 +1479,14 @@ Error Plugin::GetPreferredAllocation(const GenericDevicePlugin &dp, const std::v
     size_t total = 0;
     for (uint32_t s : size) total += s;
     std::vector<uint32_t> out(total ? total : 1), outOff(requests.size() + 1);
-    int32_t rc = kxpu_preferred_allocation(ctx_, numa.data(), numa.size(), availOff.data(), avail.data(), mustOff.data(),
-                                           must.data(), size.data(), requests.size(), out.data(), outOff.data());
-    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_preferred_allocation", rc);
+    const bool pcie = pcieTopologyAware && !dp.vgpu;  // one forest for all passthrough plugins of the walk
+    int32_t rc = pcie ? kxpu_preferred_allocation_pcie(ctx_, numa.data(), node.data(), numa.size(), pcieParent.data(),
+                                                       pcieDepth.data(), pcieParent.size(), availOff.data(), avail.data(),
+                                                       mustOff.data(), must.data(), size.data(), requests.size(), out.data(),
+                                                       outOff.data())
+                      : kxpu_preferred_allocation(ctx_, numa.data(), numa.size(), availOff.data(), avail.data(), mustOff.data(),
+                                                  must.data(), size.data(), requests.size(), out.data(), outOff.data());
+    if (rc != KXPU_OK) return kxfail(ctx_, pcie ? "kxpu_preferred_allocation_pcie" : "kxpu_preferred_allocation", rc);
     for (size_t q = 0; q < requests.size(); q++) {
         ContainerPreferredAllocationResponse resp;
         for (uint32_t k = outOff[q]; k < outOff[q + 1]; k++) resp.DeviceIDs.push_back(dp.devs[out[k]].ID);
@@ -1945,6 +2024,49 @@ int kxh_gather_mdev_topo(const char *mdev_base, const char *classes, int topo, i
     if (recs.size() > cap) return -2;
     memcpy(out, recs.data(), recs.size() * sizeof(kxpu_mdevrec));
     return 0;
+}
+
+// ---- PCIe topology (tests)
+void kxh_set_pcie_topology(void *h, int on) { ((Plugin *)h)->pcieTopologyAware = on != 0; }
+
+// CPU only: the raw PCI gather with pcieTopologyAware = pcie; counting_seam != 0 wraps readPciPath in a counter of its
+// calls (*path_reads), which also sends the fast gather down the walk
+int kxh_gather_pcie(const char *base_path, int pcie, int fast, unsigned threads, int counting_seam, kxpu_devrec *out,
+                    kxpu_pcipath *paths_out, size_t cap, size_t *n, size_t *n_paths, uint64_t *path_reads, char *err,
+                    size_t errcap) {
+    Plugin p(nullptr);
+    p.basePath = base_path;
+    p.pcieTopologyAware = pcie != 0;
+    *path_reads = 0;
+    if (counting_seam) {
+        auto dflt = p.readPciPath;
+        p.readPciPath = [dflt, path_reads](const std::string &base, const std::string &entry, std::string &target) {
+            (*path_reads)++;
+            return dflt(base, entry, target);
+        };
+    }
+    std::vector<kxpu_devrec> recs;
+    std::vector<kxpu_pcipath> paths;
+    device_plugin::Error e = fast ? p.gatherRecordsFast(recs, threads, &paths) : p.gatherRecords(recs, &paths);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    *n = recs.size();
+    *n_paths = paths.size();
+    if (recs.size() > cap) return -2;
+    memcpy(out, recs.data(), recs.size() * sizeof(kxpu_devrec));
+    memcpy(paths_out, paths.data(), paths.size() * sizeof(kxpu_pcipath));
+    return 0;
+}
+
+// "id=node,..." of one plugin's devices (the PCIe node each Device carries)
+int kxh_devs_pcie(void *h, int plugin_index, char *out, size_t cap) {
+    Plugin *p = (Plugin *)h;
+    if (plugin_index < 0 || (size_t)plugin_index >= p->devicePlugins.size()) return -1;
+    std::string o;
+    for (const auto &d : p->devicePlugins[(size_t)plugin_index].devs) {
+        if (!o.empty()) o += ',';
+        o += d.ID + "=" + std::to_string(d.pcieNode);
+    }
+    return copy_out(o, out, cap);
 }
 
 // GetPreferredAllocation for plugin plugin_index.  spec: container requests separated by ';', each

@@ -51,6 +51,7 @@ struct Device {  // pluginapi.Device
     std::string ID;
     std::string Health;
     uint64_t numa = 0;  // Device.Topology: bit k = NUMA node k (the group's mask); 0 = no topology
+    uint32_t pcieNode = KXPU_PCIE_NO_NODE;  // the group's node in Plugin::pcieParent / pcieDepth (pcieTopologyAware)
 };
 // pluginapi.DevicePluginOptions (GetDevicePluginOptions, generic_device_plugin.go:253-258)
 struct DevicePluginOptions {
@@ -180,6 +181,12 @@ struct PciWalk {
     std::vector<uint64_t> dids, gnuma;
     std::vector<uint8_t> drule;
     uint32_t nGroups = 0, nDevids = 0;
+    // pcieTopologyAware: the path of every record and the walk's PCIe forest (kxpu_pcie_tree)
+    std::vector<kxpu_pcipath> paths;
+    std::vector<uint32_t> gnode, nodeParent;
+    std::vector<uint64_t> nodeKey;
+    std::vector<uint8_t> nodeDepth;
+    uint32_t nNodes = 0;
 };
 struct MdevWalk {
     std::vector<kxpu_mdevrec> recs;
@@ -227,6 +234,13 @@ class Plugin {
     // GetPreferredAllocation keeps an allocation on as few nodes as it can (kxpu_preferred_allocation).
     bool topologyAware = false;
     std::function<bool(const std::string &base, const std::string &entry, std::string &out)> readNumaNode;
+    // PCIe topology (include/kxpu.h, ABI v7).  false (default): nothing more is read and every output is as above.  true:
+    // the PCI gathers read the link <basePath>/<entry> through readPciPath (the whole target), each record keeps its path
+    // from the first component that begins with "pci", kxpu_pcie_tree builds the walk's forest, every passthrough Device
+    // carries its group's node, and GetPreferredAllocation keeps an allocation under as few PCIe switches as it can
+    // (kxpu_preferred_allocation_pcie; vGPU plugins keep the NUMA answer).  Both settings may be on together.
+    bool pcieTopologyAware = false;
+    std::function<bool(const std::string &base, const std::string &entry, std::string &target)> readPciPath;
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
 
     // ---- state (device_plugin.go:31,34)
@@ -238,6 +252,10 @@ class Plugin {
     // class of every iommuMap / deviceMap entry (same positions); all 0 with the default class list
     std::vector<size_t> iommuClass, deviceClass;
     std::vector<uint64_t> iommuNuma, mdevNuma;  // NUMA mask of every iommuMap / mdevMap entry (topologyAware only)
+    // pcieTopologyAware only: the PCIe node of every iommuMap entry and the forest of the last PCI walk, shared by all
+    // passthrough plugins
+    std::vector<uint32_t> iommuPcieNode, pcieParent;
+    std::vector<uint8_t> pcieDepth;
     std::vector<std::string> cdiFiles;  // files the last generateCDISpec wrote, one per class
     // the mdev walk: IOMMU group -> mdevs, type key -> groups, and the vGPU class of every entry (same positions)
     OrderedMap<std::vector<MdevDevice>> mdevMap;
@@ -271,7 +289,7 @@ class Plugin {
     Error Allocate(const std::vector<std::string> &devicesIDs, ContainerAllocateResponse &resp);
     // generic_device_plugin.go:224: the bytes of ListAndWatchResponse{Devices: dpi.devs}
     Error ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8_t> &out);
-    // generic_device_plugin.go:253-258: GetPreferredAllocationAvailable = topologyAware
+    // generic_device_plugin.go:253-258: GetPreferredAllocationAvailable = topologyAware || pcieTopologyAware
     DevicePluginOptions GetDevicePluginOptions() const;
     // generic_device_plugin.go:378-386 (the reference: nil, nil).  topologyAware: one kxpu_preferred_allocation call for
     // all container requests, device IDs mapped to positions in dp.devs; an ID not in dp.devs is an error naming it.
@@ -294,11 +312,12 @@ class Plugin {
     uint64_t pciNextIndex() const { return pciNext_; }
     uint64_t mdevNextIndex() const { return mdevNext_; }
 
-    // raw gather only (no GPU): exposed for CPU tests of the walk
-    Error gatherRecords(std::vector<kxpu_devrec> &recs);
+    // raw gather only (no GPU): exposed for CPU tests of the walk.  paths (pcieTopologyAware only, else left empty):
+    // one kxpu_pcipath per record, same index
+    Error gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pcipath> *paths = nullptr);
     // the same records, read with openat / readlinkat relative to basePath by several threads
     // (SURVEY 8(f) row 2); falls back to gatherRecords when a seam was replaced.  threads = 0: automatic
-    Error gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads = 0);
+    Error gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads = 0, std::vector<kxpu_pcipath> *paths = nullptr);
     // raw gather of mdevBasePath under vgpuClasses (no GPU): one record per entry, lexical order
     Error gatherMdevRecords(std::vector<kxpu_mdevrec> &recs);
 

@@ -357,6 +357,75 @@ def topo_dev_numa(n, nodes=4, seed=11):
     return np.where(rng.random(n) < 0.05, np.uint64(0), m).astype(np.uint64)
 
 
+# ---------------------------------------------------------------- PCIe topology (ABI v7)
+def _pcie_prefix(dom, bus, dev, kind):
+    """Components above the function at dom:bus:dev.  An HGX-like board: a host bridge per 64 buses, 8 root ports
+    under it, a switch per bus, a down port per slot.  kind 1: a VMD domain between the root port and the switch;
+    2: 4 more bridge levels (a chain of exactly 8); 3: 5 more (9: unknown); 4: upper-case hex (unknown)."""
+    hb = bus & 0xC0
+    comps = ["pci%04x:%02x" % (dom, hb), "%04x:%02x:%02x.0" % (dom, hb, ((bus >> 3) & 7) + 1)]
+    if kind == 1:
+        comps += ["%04x:%02x:00.5" % (dom, hb), "pci10000:e0", "10000:e0:%02x.0" % (bus & 0x1F)]
+    if kind in (2, 3):
+        comps += ["%04x:%02x:%02x.0" % (dom, (bus + 1 + k) & 0xFF, k) for k in range(4 if kind == 2 else 5)]
+    comps += ["%04x:%02x:00.0" % (dom, bus), "%04x:%02x:%02x.0" % (dom, bus, dev)]
+    if kind == 4:
+        comps[1] = comps[1].upper().replace("X", "x")
+    return "/".join(comps) + "/"
+
+
+def pcie_walk(n=1 << 20, seed=21, group_max=4):
+    """n records (DEVREC_DTYPE, bdfs in walk order) with their kxpu_pcipath side records and a group CSR over them
+    (groups of 1..group_max consecutive records, 4 % of the records in no group).  Per bus: 2 % behind a VMD domain,
+    1 % with a chain of exactly 8, 1 % with 9 (unknown), 1 % with upper-case hex (unknown); per record: 3 % unknown
+    (len 0), 0.5 % with a trailing '/'.  A group may straddle two slots or buses, so its chain is the common prefix.
+    Returns (recs, paths, group_off, group_members)."""
+    from .binding import PCIPATH_DTYPE
+    rng = np.random.default_rng(seed)
+    recs = np.zeros(n, dtype=DEVREC_DTYPE)
+    bdfs = enumerate_bdfs(n)
+    recs["bdf"] = bdfs.view("S16").reshape(n)
+    recs["driver"] = b"vfio-pci"
+    recs["vendor_txt"] = _id_text(np.full(n, 0x10DE))
+    recs["device_txt"] = _id_text(np.full(n, 0x2330))
+    recs["vendor_len"] = recs["device_len"] = 7
+    i = np.arange(n, dtype=np.int64)
+    dom, bus, dev = i >> 16, (i >> 8) & 255, (i >> 3) & 31
+    n_bus = int((n + 255) >> 8)
+    bus_kind = rng.choice(5, size=n_bus, p=[0.95, 0.02, 0.01, 0.01, 0.01])
+    texts = []
+    cache = {}
+    for k in range(n):
+        slot = int(k >> 3)
+        pre = cache.get(slot)
+        if pre is None:
+            pre = cache[slot] = _pcie_prefix(int(dom[k]), int(bus[k]), int(dev[k]), int(bus_kind[k >> 8]))
+        texts.append(pre + bytes(bdfs[k][:12]).decode())
+    paths = np.zeros(n, dtype=PCIPATH_DTYPE)
+    paths["path"] = np.array([t.encode() for t in texts], dtype="S120")
+    paths["len"] = np.array([len(t) for t in texts], np.uint8)
+    r = rng.random(n)
+    paths["len"][r < 0.03] = 0
+    trail = (r >= 0.03) & (r < 0.035)
+    for k in np.nonzero(trail)[0]:
+        t = texts[k] + "/"
+        paths["path"][k], paths["len"][k] = t.encode(), len(t)
+    sizes = rng.integers(1, group_max + 1, n)
+    starts = np.cumsum(sizes) - sizes
+    starts = starts[starts < n]
+    keep = rng.random(n) >= 0.04
+    members, off = [], [0]
+    for g, s in enumerate(starts):
+        e = min(int(s) + int(sizes[g]), n)
+        m = [x for x in range(int(s), e) if keep[x]]
+        if not m:
+            continue
+        members.extend(m)
+        off.append(len(members))
+    recs["iommu_group"] = np.repeat(np.arange(len(starts), dtype=np.uint32), np.diff(np.append(starts, n)))
+    return recs, paths, np.array(off, np.uint32), np.array(members, np.uint32)
+
+
 # ---------------------------------------------------------------- runtime rediscovery (ABI v6)
 def fnv1a64(data: bytes) -> int:
     """64-bit FNV-1a: the snapshot tag of an mdev (over its type key)."""

@@ -24,6 +24,15 @@ dn = W.topo_dev_numa(20000)
 print("topo groups", tres["n_groups"], mres["n_groups"], "lw", len(kx.lw_encode_topo(tres["group_ids"], None, tres["group_numa"])),
       "pref", len(kx.preferred_allocation(dn, W.topo_requests(dn, n_req=300))),
       len(kx.preferred_allocation(dn, W.topo_requests(dn, n_req=1, avail=20000, size=5000, must_max=3))[0]))
+# PCIe topology: the forest of a walk, both preferred-allocation shapes over it
+precs, ppaths, poff, pmem = W.pcie_walk(20000, group_max=1)
+ptree = kx.pcie_tree(precs, ppaths, poff, pmem)
+pnode = ptree["group_node"][:15000].copy()
+pdn = W.topo_dev_numa(len(pnode))
+print("pcie nodes", len(ptree["key"]), "pref",
+      len(kx.preferred_allocation_pcie(pdn, pnode, ptree["parent"], ptree["depth"], W.topo_requests(pdn, n_req=300))),
+      len(kx.preferred_allocation_pcie(pdn, pnode, ptree["parent"], ptree["depth"],
+                                       W.topo_requests(pdn, n_req=1, avail=len(pnode), size=5000, must_max=3))[0]))
 # rediscovery: index reconciliation over PCI and UUID keys
 for mdev in (False, True):
     prev, cur, ni = W.reconcile_pair(3, 20000, mdev=mdev)
