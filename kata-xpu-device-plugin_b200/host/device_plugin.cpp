@@ -32,13 +32,6 @@ static const char *kCdiVendorClass = "nvidia.com/gpu";                       // 
 
 XpuClass defaultXpuClass() { return XpuClass{"10de", "vfio-pci", "nvidia.com", kCdiVendorClass, "cdi-vfio-xxxx"}; }
 
-bool Plugin::defaultClasses() const {
-    if (xpuClasses.size() != 1) return false;
-    const XpuClass &c = xpuClasses[0], d = defaultXpuClass();
-    return c.vendor == d.vendor && c.driver == d.driver && c.resourceNamespace == d.resourceNamespace && c.cdiKind == d.cdiKind &&
-           c.cdiFileStem == d.cdiFileStem;
-}
-
 static Error fail(const std::string &m) { Error e; e.failed = true; e.message = m; return e; }
 static Error kxfail(kxpu_ctx *ctx, const char *what, int32_t rc) {
     return fail(std::string(what) + ": " + kxpu_strerror(rc) + " (" + kxpu_last_error(ctx) + ")");
@@ -526,62 +519,75 @@ Error Plugin::createIommuDeviceMap() {
     return Error();
 }
 
+// one rule per class: rule index == class index
+static std::vector<kxpu_xpu_rule> classRules(const std::vector<XpuClass> &classes) {
+    std::vector<kxpu_xpu_rule> rules(classes.size());
+    for (size_t c = 0; c < classes.size(); c++) {
+        kxpu_xpu_rule &r = rules[c];
+        const char *vendor = classes[c].vendor.c_str(), *driver = classes[c].driver.c_str();
+        memset(&r, 0, sizeof r);  // NUL padded; a field filled to its end is left for kxpu_classify_rules to reject
+        memcpy(r.vendor, vendor, strnlen(vendor, sizeof r.vendor));
+        memcpy(r.driver, driver, strnlen(driver, sizeof r.driver));
+    }
+    return rules;
+}
+
+kxpu_classify_out ClassifyResult::wire(size_t n) {
+    accept.assign(n, 0); gids.assign(n, 0); goff.assign(n + 1, 0); gmem.assign(n, 0); doff.assign(n + 1, 0);
+    dgrp.assign(n, 0); dids.assign(n, 0);
+    drule.assign(n ? n : 1, 0);
+    gnuma.assign(n ? n : 1, 0);
+    kxpu_classify_out out;
+    memset(&out, 0, sizeof out);
+    out.accept_index = accept.data(); out.group_ids = gids.data(); out.group_off = goff.data();
+    out.group_members = gmem.data(); out.dev_ids = dids.data(); out.dev_off = doff.data(); out.dev_groups = dgrp.data();
+    return out;
+}
+
+// class of a group = the rule of its first member, which the device-map entry listing it carries
+static std::map<uint32_t, size_t> groupClasses(const ClassifyResult &r) {
+    std::map<uint32_t, size_t> groupClass;
+    for (uint32_t d = 0; d < r.nDevids; d++)
+        for (uint32_t k = r.doff[d]; k < r.doff[d + 1]; k++) groupClass[r.dgrp[k]] = r.drule[d];
+    return groupClass;
+}
+
+// the class an accepted record itself matched (a group may hold records of several classes): the class of its
+// (vendor, driver) pair
+static size_t recordClass(const std::vector<XpuClass> &classes, const uint8_t *vendorTxt, uint8_t vendorLen, const char *driver,
+                          size_t driverCap) {
+    const std::string vendor = trimID(std::string((const char *)vendorTxt, vendorLen));
+    const std::string drv(driver, strnlen(driver, driverCap));
+    size_t cls = 0;
+    for (size_t c = 0; c < classes.size(); c++)
+        if (classes[c].vendor == vendor && classes[c].driver == drv) cls = c;
+    return cls;
+}
+
 // the walk and classify of createIommuDeviceMap
 Error Plugin::classifyPci(PciWalk &w) {
     Error e = gatherRecordsFast(w.recs, 0, &w.paths);  // same records as gatherRecords (falls back to it when a seam was replaced)
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // Walk's error is ignored by the reference (:132)
     const std::vector<kxpu_devrec> &recs = w.recs;
     const size_t n = recs.size();
-    w.accept.assign(n, 0); w.gids.assign(n, 0); w.goff.assign(n + 1, 0); w.gmem.assign(n, 0); w.doff.assign(n + 1, 0);
-    w.dgrp.assign(n, 0); w.dids.assign(n, 0);
-    kxpu_classify_out out;
-    memset(&out, 0, sizeof out);
-    out.accept_index = w.accept.data(); out.group_ids = w.gids.data(); out.group_off = w.goff.data();
-    out.group_members = w.gmem.data(); out.dev_ids = w.dids.data(); out.dev_off = w.doff.data(); out.dev_groups = w.dgrp.data();
-    const bool dflt = defaultClasses();
-    w.drule.assign(n ? n : 1, 0);
-    w.gnuma.assign(n ? n : 1, 0);
-    int32_t rc;
-    if (dflt && !topologyAware) {
-        rc = kxpu_classify(ctx_, recs.data(), n, &out);
-        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify", rc);  // fatal: there is no CPU path
-    } else {
-        // one rule per class: rule index == class index
-        std::vector<kxpu_xpu_rule> rules(xpuClasses.size());
-        for (size_t c = 0; c < xpuClasses.size(); c++) {
-            memset(&rules[c], 0, sizeof rules[c]);
-            strncpy(rules[c].vendor, xpuClasses[c].vendor.c_str(), sizeof rules[c].vendor);
-            strncpy(rules[c].driver, xpuClasses[c].driver.c_str(), sizeof rules[c].driver);
-        }
-        if (topologyAware) {  // with the default class list: rule {10de, vfio-pci}, kxpu_classify's outputs
-            rc = kxpu_classify_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, w.drule.data(), w.gnuma.data());
-            if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify_topo", rc);
-        } else {
-            rc = kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, w.drule.data());
-            if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_classify_rules", rc);
-        }
-    }
-    w.nGroups = out.n_groups;
-    w.nDevids = out.n_devids;
+    ClassifyResult &c = w.out;
+    kxpu_classify_out out = c.wire(n);
+    const std::vector<kxpu_xpu_rule> rules = classRules(xpuClasses);
+    // fatal on failure: there is no CPU path
+    int32_t rc = topologyAware ? kxpu_classify_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(), c.gnuma.data())
+                               : kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data());
+    if (rc != KXPU_OK) return kxfail(ctx_, topologyAware ? "kxpu_classify_topo" : "kxpu_classify_rules", rc);
+    c.nGroups = out.n_groups;
+    c.nDevids = out.n_devids;
     if (pcieTopologyAware) {  // the forest of the walk, one node per group
-        const size_t cap = (size_t)KXPU_PCIE_MAX_DEPTH * w.nGroups + 1;
-        w.gnode.assign(w.nGroups + 1, KXPU_PCIE_NO_NODE);
+        const size_t cap = (size_t)KXPU_PCIE_MAX_DEPTH * c.nGroups + 1;
+        w.gnode.assign(c.nGroups + 1, KXPU_PCIE_NO_NODE);
         w.nodeKey.assign(cap, 0); w.nodeParent.assign(cap, 0); w.nodeDepth.assign(cap, 0);
-        rc = kxpu_pcie_tree(ctx_, recs.data(), w.paths.data(), n, w.goff.data(), w.gmem.data(), w.nGroups, w.gnode.data(),
+        rc = kxpu_pcie_tree(ctx_, recs.data(), w.paths.data(), n, c.goff.data(), c.gmem.data(), c.nGroups, w.gnode.data(),
                             w.nodeKey.data(), w.nodeParent.data(), w.nodeDepth.data(), &w.nNodes);
         if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_pcie_tree", rc);
     }
     return Error();
-}
-
-// the class an accepted function itself matched (a group may hold functions of several classes)
-static size_t recordClass(const std::vector<XpuClass> &classes, bool dflt, const kxpu_devrec &r) {
-    if (dflt) return 0;
-    const std::string vendor = trimID(std::string((const char *)r.vendor_txt, r.vendor_len));
-    size_t cls = 0;
-    for (size_t c = 0; c < classes.size(); c++)
-        if (classes[c].vendor == vendor && classes[c].driver == r.driver) cls = c;
-    return cls;
 }
 
 void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
@@ -591,51 +597,47 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
     deviceClass.clear();
     iommuNuma.clear();
     iommuPcieNode.clear();
-    const bool dflt = defaultClasses();
-    // class of a group = the rule of its first member, which the device-map entry listing it carries
-    std::map<uint32_t, size_t> groupClass;
-    for (uint32_t d = 0; d < w.nDevids; d++)
-        for (uint32_t k = w.doff[d]; k < w.doff[d + 1]; k++) groupClass[w.dgrp[k]] = w.drule[d];
-    for (uint32_t g = 0; g < w.nGroups; g++) {
+    const ClassifyResult &c = w.out;
+    std::map<uint32_t, size_t> groupClass = groupClasses(c);
+    for (uint32_t g = 0; g < c.nGroups; g++) {
         std::vector<NvidiaGpuDevice> devs;
-        for (uint32_t k = w.goff[g]; k < w.goff[g + 1]; k++) {
-            const uint32_t i = w.gmem[k];
-            const uint64_t idx = index ? (*index)[w.accept[i]] : w.accept[i];
-            devs.push_back(NvidiaGpuDevice{std::string(w.recs[i].bdf), idx});  // :171-174
-            devs.back().xpuClass = recordClass(xpuClasses, dflt, w.recs[i]);
+        for (uint32_t k = c.goff[g]; k < c.goff[g + 1]; k++) {
+            const kxpu_devrec &r = w.recs[c.gmem[k]];
+            const uint64_t idx = index ? (*index)[c.accept[c.gmem[k]]] : c.accept[c.gmem[k]];
+            devs.push_back(NvidiaGpuDevice{std::string(r.bdf), idx});  // :171-174
+            devs.back().xpuClass = recordClass(xpuClasses, r.vendor_txt, r.vendor_len, r.driver, sizeof r.driver);
         }
-        iommuMap.emplace_back(std::to_string(w.gids[g]), std::move(devs));
-        iommuClass.push_back(groupClass[w.gids[g]]);
-        if (topologyAware) iommuNuma.push_back(w.gnuma[g]);
+        iommuMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
+        iommuClass.push_back(groupClass[c.gids[g]]);
+        if (topologyAware) iommuNuma.push_back(c.gnuma[g]);
         if (pcieTopologyAware) iommuPcieNode.push_back(w.gnode[g]);
     }
     if (pcieTopologyAware) {
         pcieParent.assign(w.nodeParent.begin(), w.nodeParent.begin() + w.nNodes);
         pcieDepth.assign(w.nodeDepth.begin(), w.nodeDepth.begin() + w.nNodes);
     }
-    for (uint32_t d = 0; d < w.nDevids; d++) {
+    for (uint32_t d = 0; d < c.nDevids; d++) {
         std::vector<std::string> groups;
-        for (uint32_t k = w.doff[d]; k < w.doff[d + 1]; k++) groups.push_back(std::to_string(w.dgrp[k]));  // :169
-        deviceMap.emplace_back(devIdString(w.dids[d]), std::move(groups));
-        deviceClass.push_back(w.drule[d]);
+        for (uint32_t k = c.doff[d]; k < c.doff[d + 1]; k++) groups.push_back(std::to_string(c.dgrp[k]));  // :169
+        deviceMap.emplace_back(devIdString(c.dids[d]), std::move(groups));
+        deviceClass.push_back(c.drule[d]);
     }
 }
 
 // one entry per accepted function in walk order: key = PCI address, tag = its device id text packed as dev_ids packs it
 std::vector<kxpu_snaprec> Plugin::snapshotOf(const PciWalk &w, const std::vector<uint64_t> *index) const {
     std::vector<kxpu_snaprec> snap;
-    const bool dflt = defaultClasses();
     for (size_t i = 0; i < w.recs.size(); i++) {
-        if (w.accept[i] == KXPU_REJECTED) continue;
+        if (w.out.accept[i] == KXPU_REJECTED) continue;
         const kxpu_devrec &r = w.recs[i];
         kxpu_snaprec s;
         memset(&s, 0, sizeof s);
         memcpy(s.key, r.bdf, strnlen(r.bdf, sizeof r.bdf));
         s.iommu_group = r.iommu_group;
-        s.klass = (uint32_t)recordClass(xpuClasses, dflt, r);
+        s.klass = (uint32_t)recordClass(xpuClasses, r.vendor_txt, r.vendor_len, r.driver, sizeof r.driver);
         const std::string id = trimID(std::string((const char *)r.device_txt, std::min<size_t>(r.device_len, sizeof r.device_txt)));
         memcpy(&s.tag, id.data(), std::min<size_t>(id.size(), 8));
-        s.index = index ? (*index)[w.accept[i]] : w.accept[i];
+        s.index = index ? (*index)[w.out.accept[i]] : w.out.accept[i];
         snap.push_back(s);
     }
     return snap;
@@ -758,27 +760,16 @@ Error Plugin::classifyMdev(MdevWalk &w) {
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // like the PCI walk: an unreadable bus is an empty one
     const std::vector<kxpu_mdevrec> &recs = w.recs;
     const size_t n = recs.size();
-    w.accept.assign(n, 0); w.gids.assign(n, 0); w.goff.assign(n + 1, 0); w.gmem.assign(n, 0); w.doff.assign(n + 1, 0);
-    w.dgrp.assign(n, 0); w.dids.assign(n, 0);
-    w.drule.assign(n ? n : 1, 0);
-    kxpu_classify_out out;
-    memset(&out, 0, sizeof out);
-    out.accept_index = w.accept.data(); out.group_ids = w.gids.data(); out.group_off = w.goff.data();
-    out.group_members = w.gmem.data(); out.dev_ids = w.dids.data(); out.dev_off = w.doff.data(); out.dev_groups = w.dgrp.data();
-    std::vector<kxpu_xpu_rule> rules(vgpuClasses.size());  // one rule per class: rule index == class index
-    for (size_t c = 0; c < vgpuClasses.size(); c++) {
-        memset(&rules[c], 0, sizeof rules[c]);
-        strncpy(rules[c].vendor, vgpuClasses[c].vendor.c_str(), sizeof rules[c].vendor);
-        strncpy(rules[c].driver, vgpuClasses[c].driver.c_str(), sizeof rules[c].driver);
-    }
-    w.gnuma.assign(n ? n : 1, 0);
-    int32_t rc = topologyAware ? kxpu_classify_mdev_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, w.drule.data(), w.gnuma.data())
-                               : kxpu_classify_mdev(ctx_, rules.data(), rules.size(), recs.data(), n, &out, w.drule.data());
+    ClassifyResult &c = w.out;
+    kxpu_classify_out out = c.wire(n);
+    const std::vector<kxpu_xpu_rule> rules = classRules(vgpuClasses);
+    int32_t rc = topologyAware ? kxpu_classify_mdev_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(), c.gnuma.data())
+                               : kxpu_classify_mdev(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data());
     if (rc != KXPU_OK) return kxfail(ctx_, topologyAware ? "kxpu_classify_mdev_topo" : "kxpu_classify_mdev", rc);
-    w.nGroups = out.n_groups;
-    w.nDevids = out.n_devids;
+    c.nGroups = out.n_groups;
+    c.nDevids = out.n_devids;
     std::vector<uint32_t> first(out.n_devids);
-    for (uint32_t d = 0; d < out.n_devids; d++) first[d] = (uint32_t)w.dids[d];
+    for (uint32_t d = 0; d < out.n_devids; d++) first[d] = (uint32_t)c.dids[d];
     w.koff.assign(first.size() + 1, 0);
     size_t need = 0;
     rc = kxpu_mdev_names(ctx_, recs.data(), n, first.data(), first.size(), nullptr, 0, w.koff.data(), &need);
@@ -789,41 +780,32 @@ Error Plugin::classifyMdev(MdevWalk &w) {
     return Error();
 }
 
-static size_t mdevRecordClass(const std::vector<XpuClass> &classes, const kxpu_mdevrec &r) {
-    const std::string vendor = trimID(std::string((const char *)r.parent_vendor_txt, r.vendor_len));
-    size_t cls = 0;
-    for (size_t c = 0; c < classes.size(); c++)
-        if (classes[c].vendor == vendor && classes[c].driver == std::string(r.driver, strnlen(r.driver, sizeof r.driver))) cls = c;
-    return cls;
-}
-
 void Plugin::buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
     mdevMap.clear();
     typeMap.clear();
     mdevClass.clear();
     typeClass.clear();
     mdevNuma.clear();
-    std::map<uint32_t, size_t> groupClass;  // class of a group = the rule of its first member
-    for (uint32_t d = 0; d < w.nDevids; d++)
-        for (uint32_t k = w.doff[d]; k < w.doff[d + 1]; k++) groupClass[w.dgrp[k]] = w.drule[d];
-    for (uint32_t g = 0; g < w.nGroups; g++) {
+    const ClassifyResult &c = w.out;
+    std::map<uint32_t, size_t> groupClass = groupClasses(c);
+    for (uint32_t g = 0; g < c.nGroups; g++) {
         std::vector<MdevDevice> devs;
-        for (uint32_t k = w.goff[g]; k < w.goff[g + 1]; k++) {
-            const kxpu_mdevrec &r = w.recs[w.gmem[k]];
-            const uint64_t idx = index ? (*index)[w.accept[w.gmem[k]]] : w.accept[w.gmem[k]];
+        for (uint32_t k = c.goff[g]; k < c.goff[g + 1]; k++) {
+            const kxpu_mdevrec &r = w.recs[c.gmem[k]];
+            const uint64_t idx = index ? (*index)[c.accept[c.gmem[k]]] : c.accept[c.gmem[k]];
             MdevDevice m{std::string(r.uuid, sizeof r.uuid), std::string(r.parent, strnlen(r.parent, sizeof r.parent)), idx, 0};
-            m.vgpuClass = mdevRecordClass(vgpuClasses, r);
+            m.vgpuClass = recordClass(vgpuClasses, r.parent_vendor_txt, r.vendor_len, r.driver, sizeof r.driver);
             devs.push_back(std::move(m));
         }
-        mdevMap.emplace_back(std::to_string(w.gids[g]), std::move(devs));
-        mdevClass.push_back(groupClass[w.gids[g]]);
-        if (topologyAware) mdevNuma.push_back(w.gnuma[g]);
+        mdevMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
+        mdevClass.push_back(groupClass[c.gids[g]]);
+        if (topologyAware) mdevNuma.push_back(c.gnuma[g]);
     }
-    for (uint32_t d = 0; d < w.nDevids; d++) {
+    for (uint32_t d = 0; d < c.nDevids; d++) {
         std::vector<std::string> groups;
-        for (uint32_t k = w.doff[d]; k < w.doff[d + 1]; k++) groups.push_back(std::to_string(w.dgrp[k]));
+        for (uint32_t k = c.doff[d]; k < c.doff[d + 1]; k++) groups.push_back(std::to_string(c.dgrp[k]));
         typeMap.emplace_back(std::string((const char *)w.keys.data() + w.koff[d], w.koff[d + 1] - w.koff[d]), std::move(groups));
-        typeClass.push_back(w.drule[d]);
+        typeClass.push_back(c.drule[d]);
     }
 }
 
@@ -836,22 +818,23 @@ static uint64_t fnv1a64(const std::string &s) {
 // one entry per accepted mdev in walk order: key = UUID, tag = FNV-1a 64 of the type key of the resource its group is
 // served under (the type key of the group's device-map entry: known on the host without another GPU call)
 std::vector<kxpu_snaprec> Plugin::snapshotOf(const MdevWalk &w, const std::vector<uint64_t> *index) const {
+    const ClassifyResult &c = w.out;
     std::map<uint32_t, uint64_t> groupTag;
-    for (uint32_t d = 0; d < w.nDevids; d++) {
+    for (uint32_t d = 0; d < c.nDevids; d++) {
         const uint64_t t = fnv1a64(std::string((const char *)w.keys.data() + w.koff[d], w.koff[d + 1] - w.koff[d]));
-        for (uint32_t k = w.doff[d]; k < w.doff[d + 1]; k++) groupTag[w.dgrp[k]] = t;
+        for (uint32_t k = c.doff[d]; k < c.doff[d + 1]; k++) groupTag[c.dgrp[k]] = t;
     }
     std::vector<kxpu_snaprec> snap;
     for (size_t i = 0; i < w.recs.size(); i++) {
-        if (w.accept[i] == KXPU_REJECTED) continue;
+        if (c.accept[i] == KXPU_REJECTED) continue;
         const kxpu_mdevrec &r = w.recs[i];
         kxpu_snaprec s;
         memset(&s, 0, sizeof s);
         memcpy(s.key, r.uuid, sizeof r.uuid);
         s.iommu_group = r.iommu_group;
-        s.klass = (uint32_t)mdevRecordClass(vgpuClasses, r);
+        s.klass = (uint32_t)recordClass(vgpuClasses, r.parent_vendor_txt, r.vendor_len, r.driver, sizeof r.driver);
         s.tag = groupTag[r.iommu_group];
-        s.index = index ? (*index)[w.accept[i]] : w.accept[i];
+        s.index = index ? (*index)[c.accept[i]] : c.accept[i];
         snap.push_back(s);
     }
     return snap;
@@ -930,16 +913,15 @@ static bool parseHex4(const std::string &s, uint32_t &v) {
 // getDeviceName, device_plugin.go:208-259, for a whole batch of device ids: ONE join and ONE name
 // gather through the ABI (cgo calls stay coarse, SURVEY H7).  "" means "not found" exactly like the
 // reference; sysfs ids are four lowercase hex digits, anything else is treated as not found.
-// With `vendors` the key of id i is (vendors[i] << 16) | id; a vendor that is not four lowercase hex digits
+// The key of id i is (vendors[i] << 16) | id; a vendor that is not four lowercase hex digits
 // never names anything, so that device falls back to its raw id like a miss (:100-103).
-std::vector<std::string> Plugin::getDeviceNames(const std::vector<std::string> &deviceIDs, const std::vector<std::string> *vendors) {
+std::vector<std::string> Plugin::getDeviceNames(const std::vector<std::string> &deviceIDs, const std::vector<std::string> &vendors) {
     std::vector<std::string> out(deviceIDs.size());
     std::vector<uint32_t> keys;
     std::vector<size_t> where;
     for (size_t i = 0; i < deviceIDs.size(); i++) {
-        uint32_t d, v = 0x10deu;  // nvidiaVendorID, :19
-        if (vendors && !parseHex4((*vendors)[i], v)) continue;
-        if (parseHex4(deviceIDs[i], d)) { keys.push_back((v << 16) | d); where.push_back(i); }
+        uint32_t d, v;
+        if (parseHex4(vendors[i], v) && parseHex4(deviceIDs[i], d)) { keys.push_back((v << 16) | d); where.push_back(i); }
     }
     std::vector<int32_t> rows(keys.size(), KXPU_ROW_MISS);
     if (!table_) {
@@ -959,8 +941,9 @@ std::vector<std::string> Plugin::getDeviceNames(const std::vector<std::string> &
     if (need && kxpu_names(ctx_, table_, rows.data(), rows.size(), blob.data(), need, offs.data(), &need) != KXPU_OK) return out;
     for (size_t k = 0; k < keys.size(); k++) {
         if (rows[k] == KXPU_ROW_MISS) {
-            if (vendors) fprintf(stderr, "Could not find device %s:%s\n", (*vendors)[where[k]].c_str(), deviceIDs[where[k]].c_str());
-            else fprintf(stderr, "Could not find NVIDIA device with id: %s\n", deviceIDs[where[k]].c_str());  // :234
+            const std::string &vendor = vendors[where[k]], &id = deviceIDs[where[k]];
+            if (vendor == "10de") fprintf(stderr, "Could not find NVIDIA device with id: %s\n", id.c_str());  // :234
+            else fprintf(stderr, "Could not find device %s:%s\n", vendor.c_str(), id.c_str());
             continue;
         }
         out[where[k]].assign((const char *)blob.data() + offs[k], offs[k + 1] - offs[k]);
@@ -968,7 +951,7 @@ std::vector<std::string> Plugin::getDeviceNames(const std::vector<std::string> &
     return out;
 }
 
-std::string Plugin::getDeviceName(const std::string &deviceID) { return getDeviceNames({deviceID})[0]; }
+std::string Plugin::getDeviceName(const std::string &deviceID) { return getDeviceNames({deviceID}, {defaultXpuClass().vendor})[0]; }
 
 static Error writeSpecFile(const std::string &file_path, const std::vector<uint8_t> &doc, size_t len, bool &written) {
     written = false;
@@ -1031,71 +1014,69 @@ Error Plugin::writeSpec(const std::string &path, const std::vector<uint8_t> &doc
     return e;
 }
 
-// generateCDISpec for a class list: one file per class, <stem>.yaml|.json, with that class's kind and only the devices
-// of its groups in ascending index; a class without devices gets the empty document (the reference writes one for
-// zero devices too).
-Error Plugin::generateCDISpecClasses(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, int32_t fmt) {
-    std::vector<std::vector<kxpu_cdidev>> per(xpuClasses.size());
-    for (const auto &kv : m) {
-        const size_t c = classOfGroup(kv.first);
-        for (const NvidiaGpuDevice &dev : kv.second) {
-            kxpu_cdidev d;
-            memset(&d, 0, sizeof d);
-            strncpy(d.bdf, dev.addr.c_str(), sizeof d.bdf - 1);
-            d.iommu_group = (uint32_t)strtoul(kv.first.c_str(), nullptr, 10);
-            d.index = dev.index;
-            per[c].push_back(d);
-        }
-    }
-    for (size_t c = 0; c < xpuClasses.size(); c++) {
-        std::vector<kxpu_cdidev> &devs = per[c];
-        std::sort(devs.begin(), devs.end(), [](const kxpu_cdidev &a, const kxpu_cdidev &b) { return a.index < b.index; });
-        const char *kind = xpuClasses[c].cdiKind.c_str();
+// the CDI record of one device of group `group`
+static kxpu_cdidev cdiRecord(const std::string &group, const NvidiaGpuDevice &dev) {
+    kxpu_cdidev d;
+    memset(&d, 0, sizeof d);
+    strncpy(d.bdf, dev.addr.c_str(), sizeof d.bdf - 1);
+    d.iommu_group = (uint32_t)strtoul(group.c_str(), nullptr, 10);
+    d.index = dev.index;
+    return d;
+}
+static kxpu_mdevcdi cdiRecord(const std::string &group, const MdevDevice &m) {
+    kxpu_mdevcdi d;
+    memset(&d, 0, sizeof d);
+    memcpy(d.uuid, m.uuid.data(), std::min(m.uuid.size(), sizeof d.uuid));
+    strncpy(d.parent, m.parent.c_str(), sizeof d.parent - 1);
+    d.iommu_group = (uint32_t)strtoul(group.c_str(), nullptr, 10);
+    d.index = m.index;
+    return d;
+}
+
+// One file per class, <stem>.yaml|.json, with that class's kind and only the devices of its entries in ascending index
+// (Go ranges over the map in random order, device_plugin.go:59); a class without devices gets the empty document (the
+// reference writes one for zero devices too).  The files written go to `files`.
+template <typename Dev, typename Rec>
+Error Plugin::generateClassSpecs(const std::vector<XpuClass> &classes, const OrderedMap<std::vector<Dev>> &m,
+                                 const std::vector<size_t> &entryClass, int32_t fmt, const char *what,
+                                 int32_t (*emit)(kxpu_ctx *, int32_t, const char *, const Rec *, size_t, uint8_t *, size_t, size_t *),
+                                 std::vector<std::string> &files) {
+    std::vector<std::vector<Rec>> per(classes.size());
+    for (size_t g = 0; g < m.size(); g++)
+        for (const Dev &dev : m[g].second) per[entryClass[g]].push_back(cdiRecord(m[g].first, dev));
+    for (size_t c = 0; c < classes.size(); c++) {
+        std::vector<Rec> &devs = per[c];
+        std::sort(devs.begin(), devs.end(), [](const Rec &a, const Rec &b) { return a.index < b.index; });
+        const char *kind = classes[c].cdiKind.c_str();
         size_t len = 0;
-        int32_t rc = kxpu_cdi_emit_kind(ctx_, fmt, kind, devs.data(), devs.size(), nullptr, 0, &len);
-        if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, "kxpu_cdi_emit_kind", rc);
+        int32_t rc = emit(ctx_, fmt, kind, devs.data(), devs.size(), nullptr, 0, &len);
+        if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, what, rc);
         std::vector<uint8_t> doc(len ? len : 1);
-        rc = kxpu_cdi_emit_kind(ctx_, fmt, kind, devs.data(), devs.size(), doc.data(), len, &len);
-        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_cdi_emit_kind", rc);
-        const std::string file_path = cdiConfigPath + xpuClasses[c].cdiFileStem + (fmt == KXPU_FMT_YAML ? ".yaml" : ".json");
+        rc = emit(ctx_, fmt, kind, devs.data(), devs.size(), doc.data(), len, &len);
+        if (rc != KXPU_OK) return kxfail(ctx_, what, rc);
+        const std::string file_path = cdiConfigPath + classes[c].cdiFileStem + (fmt == KXPU_FMT_YAML ? ".yaml" : ".json");  // spec.go:92
         bool written = false;
-        Error e = writeSpec(file_path, doc, len, written);
+        Error e = writeSpec(file_path, doc, len, written);  // os.Create at start-up (spec.go:93-126)
         if (e) return e;
-        if (written || atomicSpecs_) { cdiFiles.push_back(file_path); lastCdiFile = file_path; }
+        if (written || atomicSpecs_) files.push_back(file_path);
     }
     return Error();
 }
 
-// generateCDISpec, device_plugin.go:55-80 + CdiSpec.Save, cdi/spec.go:85-127
+// generateCDISpec, device_plugin.go:55-80 + CdiSpec.Save, cdi/spec.go:85-127, one file per class
 Error Plugin::generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, const std::string &format) {
     cdiFiles.clear();
-    if (!defaultClasses()) return generateCDISpecClasses(m, format == "YAML" ? KXPU_FMT_YAML : KXPU_FMT_JSON);
-    std::vector<kxpu_cdidev> devs;
+    std::map<std::string, size_t> classOf;  // group -> class, from the maps of the last walk
+    for (size_t g = 0; g < iommuMap.size() && g < iommuClass.size(); g++) classOf.emplace(iommuMap[g].first, iommuClass[g]);
+    std::vector<size_t> entryClass;
     for (const auto &kv : m) {
-        for (const NvidiaGpuDevice &dev : kv.second) {
-            kxpu_cdidev c;
-            memset(&c, 0, sizeof c);
-            strncpy(c.bdf, dev.addr.c_str(), sizeof c.bdf - 1);
-            c.iommu_group = (uint32_t)strtoul(kv.first.c_str(), nullptr, 10);
-            c.index = dev.index;
-            devs.push_back(c);
-        }
+        auto it = classOf.find(kv.first);
+        entryClass.push_back(it == classOf.end() ? 0 : it->second);
     }
-    // Go ranges over the map in random order (:59); canonical order = ascending index
-    std::sort(devs.begin(), devs.end(), [](const kxpu_cdidev &a, const kxpu_cdidev &b) { return a.index < b.index; });
     const int32_t fmt = format == "YAML" ? KXPU_FMT_YAML : KXPU_FMT_JSON;  // spec.go:86-89,102-114
-    size_t len = 0;
-    int32_t rc = kxpu_cdi_emit(ctx_, fmt, devs.data(), devs.size(), nullptr, 0, &len);
-    if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, "kxpu_cdi_emit", rc);
-    std::vector<uint8_t> doc(len ? len : 1);
-    rc = kxpu_cdi_emit(ctx_, fmt, devs.data(), devs.size(), doc.data(), len, &len);
-    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_cdi_emit", rc);
-    const std::string file_path = cdiConfigPath + "cdi-vfio-xxxx" + (fmt == KXPU_FMT_YAML ? ".yaml" : ".json");  // :79, spec.go:92
-    bool written = false;
-    Error e = writeSpec(file_path, doc, len, written);  // os.Create at start-up (spec.go:93-126)
-    if (e) return e;
-    if (written || atomicSpecs_) { lastCdiFile = file_path; cdiFiles.push_back(file_path); }
-    return Error();
+    Error e = generateClassSpecs(xpuClasses, m, entryClass, fmt, "kxpu_cdi_emit_kind", kxpu_cdi_emit_kind, cdiFiles);
+    if (!cdiFiles.empty()) lastCdiFile = cdiFiles.back();
+    return e;
 }
 
 // One CDI spec per vGPU class: the mdevs of the class's groups in ascending index; a class without mdevs gets the empty
@@ -1104,35 +1085,7 @@ Error Plugin::generateMdevCDISpec(const std::string &format) {
     mdevCdiFiles.clear();
     if (vgpuClasses.empty()) return Error();
     const int32_t fmt = format == "YAML" ? KXPU_FMT_YAML : KXPU_FMT_JSON;
-    std::vector<std::vector<kxpu_mdevcdi>> per(vgpuClasses.size());
-    for (size_t g = 0; g < mdevMap.size(); g++) {
-        for (const MdevDevice &m : mdevMap[g].second) {
-            kxpu_mdevcdi d;
-            memset(&d, 0, sizeof d);
-            memcpy(d.uuid, m.uuid.data(), std::min(m.uuid.size(), sizeof d.uuid));
-            strncpy(d.parent, m.parent.c_str(), sizeof d.parent - 1);
-            d.iommu_group = (uint32_t)strtoul(mdevMap[g].first.c_str(), nullptr, 10);
-            d.index = m.index;
-            per[mdevClass[g]].push_back(d);
-        }
-    }
-    for (size_t c = 0; c < vgpuClasses.size(); c++) {
-        std::vector<kxpu_mdevcdi> &devs = per[c];
-        std::sort(devs.begin(), devs.end(), [](const kxpu_mdevcdi &a, const kxpu_mdevcdi &b) { return a.index < b.index; });
-        const char *kind = vgpuClasses[c].cdiKind.c_str();
-        size_t len = 0;
-        int32_t rc = kxpu_cdi_emit_mdev(ctx_, fmt, kind, devs.data(), devs.size(), nullptr, 0, &len);
-        if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, "kxpu_cdi_emit_mdev", rc);
-        std::vector<uint8_t> doc(len ? len : 1);
-        rc = kxpu_cdi_emit_mdev(ctx_, fmt, kind, devs.data(), devs.size(), doc.data(), len, &len);
-        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_cdi_emit_mdev", rc);
-        const std::string file_path = cdiConfigPath + vgpuClasses[c].cdiFileStem + (fmt == KXPU_FMT_YAML ? ".yaml" : ".json");
-        bool written = false;
-        Error e = writeSpec(file_path, doc, len, written);
-        if (e) return e;
-        if (written || atomicSpecs_) mdevCdiFiles.push_back(file_path);
-    }
-    return Error();
+    return generateClassSpecs(vgpuClasses, mdevMap, mdevClass, fmt, "kxpu_cdi_emit_mdev", kxpu_cdi_emit_mdev, mdevCdiFiles);
 }
 
 // createDevicePlugins, device_plugin.go:83-112 (nothing is started: no gRPC here)
@@ -1151,8 +1104,7 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         ids.push_back(deviceMap[d].first);
         vendors.push_back(xpuClasses[d < deviceClass.size() ? deviceClass[d] : 0].vendor);
     }
-    const bool dflt = defaultClasses();
-    const std::vector<std::string> names = getDeviceNames(ids, dflt ? nullptr : &vendors);  // :99 for every device id at once
+    const std::vector<std::string> names = getDeviceNames(ids, vendors);  // :99 for every device id at once
     std::map<std::string, uint64_t> numaOf, mdevNumaOf;  // group id -> NUMA mask (topologyAware)
     for (size_t g = 0; g < iommuNuma.size() && g < iommuMap.size(); g++) numaOf[iommuMap[g].first] = iommuNuma[g];
     for (size_t g = 0; g < mdevNuma.size() && g < mdevMap.size(); g++) mdevNumaOf[mdevMap[g].first] = mdevNuma[g];
@@ -1332,8 +1284,6 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
         uint64_t now = 0;
         fromSnapshot = bindGeneration(now) && now == snapshotGen_;
     }
-    const bool dflt = defaultClasses();
-    bool haveClass = false;
     size_t reqClass = 0;  // the class of the request's groups: one plugin serves one class
     const auto &mdevs = returnMdevMap();
     bool havePci = false, haveVgpu = false;
@@ -1360,14 +1310,10 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
         const std::vector<NvidiaGpuDevice> *nvDevs = nullptr;
         for (const auto &kv : returnedMap) if (kv.first == iommuId) { nvDevs = &kv.second; break; }
         if (!nvDevs) continue;  // unknown group id: empty nvDevs, no error (:327)
-        if (haveVgpu) return fail("invalid allocation request: devices of more than one class");
+        const size_t c = classOfGroup(iommuId);
+        if (haveVgpu || (havePci && c != reqClass)) return fail("invalid allocation request: devices of more than one class");
         havePci = true;
-        if (!dflt) {
-            const size_t c = classOfGroup(iommuId);
-            if (haveClass && c != reqClass) return fail("invalid allocation request: devices of more than one class");
-            haveClass = true;
-            reqClass = c;
-        }
+        reqClass = c;
         for (const NvidiaGpuDevice &dev : *nvDevs) {
             if (fromSnapshot) {
                 snapshotValidations++;
@@ -1378,38 +1324,26 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
             std::string iommuGroup, vendor;
             if (!readLink(basePath, dev.addr, "iommu_group", iommuGroup) || iommuGroup != iommuId)  // :329-333
                 return fail("invalid allocation request: unknown device: " + dev.addr);
-            const std::string &want = dflt ? std::string("10de") : xpuClasses[dev.xpuClass].vendor;  // the device's class
+            const std::string &want = xpuClasses[dev.xpuClass].vendor;  // the device's class
             if (!readIDFromFile(basePath, dev.addr, "vendor", vendor) || trimID(vendor) != want)  // :334-338
                 return fail("invalid allocation request: unknown device: " + dev.addr);
             devIndexes.push_back(dev.index);  // :340
         }
     }
+    const std::string &kind = haveVgpu ? vgpuClasses[vgpuClass].cdiKind : xpuClasses[reqClass].cdiKind;
     resp.CDIDevices.clear();
     if (!devIndexes.empty()) {  // updateResponseForCDI :274-299; strategy cdi-cri is on (:61)
         std::vector<uint32_t> offs(devIndexes.size() + 1);
         size_t need = 0;
-        int32_t rc;
-        std::vector<uint8_t> buf;
-        if (haveVgpu) {
-            const std::string &kind = vgpuClasses[vgpuClass].cdiKind;
-            buf.resize((kind.size() + 22) * devIndexes.size());
-            rc = kxpu_alloc_names_kind(ctx_, kind.c_str(), devIndexes.data(), devIndexes.size(), buf.data(), buf.size(), offs.data(), &need);
-        } else if (dflt) {
-            buf.resize(36 * devIndexes.size());
-            rc = kxpu_alloc_names(ctx_, devIndexes.data(), devIndexes.size(), buf.data(), buf.size(), offs.data(), &need);
-        } else {
-            const std::string &kind = xpuClasses[reqClass].cdiKind;
-            buf.resize((kind.size() + 22) * devIndexes.size());
-            rc = kxpu_alloc_names_kind(ctx_, kind.c_str(), devIndexes.data(), devIndexes.size(), buf.data(), buf.size(), offs.data(), &need);
-        }
+        std::vector<uint8_t> buf((kind.size() + 22) * devIndexes.size());
+        const int32_t rc =
+            kxpu_alloc_names_kind(ctx_, kind.c_str(), devIndexes.data(), devIndexes.size(), buf.data(), buf.size(), offs.data(), &need);
         if (rc != KXPU_OK) return fail("failed to get allocate response: " + std::string(kxpu_strerror(rc)));
         for (size_t i = 0; i < devIndexes.size(); i++)
             resp.CDIDevices.emplace_back((const char *)buf.data() + offs[i], offs[i + 1] - offs[i]);
     }
     resp.Envs.clear();
-    resp.Envs[kK8SCDIVendorClass] = haveVgpu ? vgpuClasses[vgpuClass].cdiKind
-                                    : dflt   ? std::string(kCdiVendorClass)
-                                             : xpuClasses[reqClass].cdiKind;  // :348-350 overwrites Envs
+    resp.Envs[kK8SCDIVendorClass] = kind;  // :348-350 overwrites Envs
     return Error();
 }
 

@@ -174,13 +174,20 @@ struct RediscoverReport {
 // the atomic spec writer of Plugin::rediscover (exposed for CPU tests)
 Error writeSpecFileAtomicForTests(const std::string &file_path, const uint8_t *doc, size_t len, bool &written);
 
-// One walk's classify result, kept so that the maps can be rebuilt with reconciled indices (host bookkeeping).
-struct PciWalk {
-    std::vector<kxpu_devrec> recs;
+// The output arrays of one classify call (kxpu_classify_out + dev_rule + group_numa) and their counts.
+struct ClassifyResult {
     std::vector<uint32_t> accept, gids, goff, gmem, doff, dgrp;
     std::vector<uint64_t> dids, gnuma;
     std::vector<uint8_t> drule;
     uint32_t nGroups = 0, nDevids = 0;
+    // sizes the arrays for n records and points a kxpu_classify_out at them
+    kxpu_classify_out wire(size_t n);
+};
+
+// One walk's classify result, kept so that the maps can be rebuilt with reconciled indices (host bookkeeping).
+struct PciWalk {
+    std::vector<kxpu_devrec> recs;
+    ClassifyResult out;
     // pcieTopologyAware: the path of every record and the walk's PCIe forest (kxpu_pcie_tree)
     std::vector<kxpu_pcipath> paths;
     std::vector<uint32_t> gnode, nodeParent;
@@ -190,10 +197,9 @@ struct PciWalk {
 };
 struct MdevWalk {
     std::vector<kxpu_mdevrec> recs;
-    std::vector<uint32_t> accept, gids, goff, gmem, doff, dgrp, koff;
-    std::vector<uint64_t> dids, gnuma;
-    std::vector<uint8_t> drule, keys;
-    uint32_t nGroups = 0, nDevids = 0;
+    ClassifyResult out;
+    std::vector<uint32_t> koff;
+    std::vector<uint8_t> keys;
 };
 
 class Plugin {
@@ -211,11 +217,12 @@ class Plugin {
     // unhealthy watcher) falls back to the live reads for that request.  bindGeneration is a seam: by
     // default it asks the BindWatcher (started on first use), tests replace it.
     bool snapshotValidation = false;
-    // The accelerator classes served.  The default (one NVIDIA class) runs exactly the reference's code paths;
-    // any other list goes through kxpu_classify_rules / kxpu_cdi_emit_kind / kxpu_alloc_names_kind.  Classes must
-    // be distinct (vendor, driver) pairs, at most KXPU_MAX_RULES.  Socket names stay kata-xpu-<name>.sock, so two
-    // classes whose devices get the same name collide like two NVIDIA device ids with the same name do in the
-    // reference (generic_device_plugin.go:76); nothing resolves that.
+    // The accelerator classes served.  Every list, the default (one NVIDIA class) included, goes through
+    // kxpu_classify_rules / kxpu_cdi_emit_kind / kxpu_alloc_names_kind; with the default list these return the bytes
+    // of the reference's NVIDIA-only calls (include/kxpu.h).  Classes must be distinct (vendor, driver) pairs, at most
+    // KXPU_MAX_RULES.  Socket names stay kata-xpu-<name>.sock, so two classes whose devices get the same name collide
+    // like two NVIDIA device ids with the same name do in the reference (generic_device_plugin.go:76); nothing
+    // resolves that.
     std::vector<XpuClass> xpuClasses{defaultXpuClass()};
     // vGPU classes: mediated devices under mdevBasePath, one resource <resourceNamespace>/<type key> per (class, type
     // key).  vendor = the parent PCI device's vendor id, driver = the mdev's driver.  Empty (default): nothing under
@@ -272,10 +279,9 @@ class Plugin {
     Error createIommuDeviceMap();
     // device_plugin.go:208-259: parse-once table + batched lookup + sanitiser on the GPU (S2)
     std::string getDeviceName(const std::string &deviceID);
-    // the same for a batch of ids: one kxpu_lookup + one kxpu_names (device_plugin.go:99 for every id of deviceMap)
-    // vendors == nullptr: every id is an NVIDIA device id (the reference); else vendors[i] is the vendor id of deviceIDs[i]
-    std::vector<std::string> getDeviceNames(const std::vector<std::string> &deviceIDs,
-                                            const std::vector<std::string> *vendors = nullptr);
+    // the same for a batch of ids: one kxpu_lookup + one kxpu_names (device_plugin.go:99 for every id of deviceMap);
+    // vendors[i] is the vendor id of deviceIDs[i]
+    std::vector<std::string> getDeviceNames(const std::vector<std::string> &deviceIDs, const std::vector<std::string> &vendors);
     // device_plugin.go:55-80 + cdi/spec.go:85-127: emit on the GPU, host writes the file (S3)
     Error generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, const std::string &format = "YAML");
     // the mdev walk (single-threaded, lexical order) + kxpu_classify_mdev; reads nothing when vgpuClasses is empty
@@ -325,10 +331,14 @@ class Plugin {
     kxpu_ctx *ctx_;
     kxpu_table *table_ = nullptr;
     Error ensureTable();
-    bool defaultClasses() const;
     size_t classOfGroup(const std::string &group) const;
     Error checkVgpuClasses() const;
-    Error generateCDISpecClasses(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, int32_t fmt);
+    // one CDI spec per class: the devices of m whose entry has that class (entryClass, same positions as m)
+    template <typename Dev, typename Rec>
+    Error generateClassSpecs(const std::vector<XpuClass> &classes, const OrderedMap<std::vector<Dev>> &m,
+                             const std::vector<size_t> &entryClass, int32_t fmt, const char *what,
+                             int32_t (*emit)(kxpu_ctx *, int32_t, const char *, const Rec *, size_t, uint8_t *, size_t, size_t *),
+                             std::vector<std::string> &files);
     // first use: kxpu_pciids_join on pinned buffers = file -> table -> row handles of `keys` in one call
     Error loadAndJoin(const std::vector<uint32_t> &keys, std::vector<int32_t> &rows);
     Error classifyPci(PciWalk &w);
