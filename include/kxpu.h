@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 7
+#define KXPU_ABI_VERSION 8
 
 /* status codes */
 #define KXPU_OK             0
@@ -287,6 +287,9 @@ typedef struct kxpu_devrec {
  * A record whose flag is set with numa_node >= 64 counts as unknown. */
 #define KXPU_REC_NUMA       0x40u
 #define KXPU_MAX_NUMA_NODES 64
+/* The entry is bound to a driver outside the caller's viability list, and iommu_group holds its group (ABI v8; see
+ * kxpu_classify_viable).  Only kxpu_classify_viable reads it: every other call ignores the flag. */
+#define KXPU_REC_BLOCKS     0x80u
 
 /* Caller-allocated outputs of kxpu_classify; every array has room for n entries
  * (group_off / dev_off: n+1). */
@@ -416,6 +419,34 @@ int32_t kxpu_classify_topo(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_r
 int32_t kxpu_classify_mdev_topo(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_mdevrec *recs,
                                 size_t n, kxpu_classify_out *out, uint8_t *dev_rule /* [n] */,
                                 uint64_t *group_numa /* [n] */);
+
+/* ------------------------------------------------- IOMMU group viability (ABI v8) */
+
+/* Whether VFIO can open each group.  The kernel lets VFIO take a group only when every PCI function in it is unbound
+ * or bound to a driver that leaves DMA to its owner (vfio-pci and its variant drivers, pci-stub, pcieport); a group
+ * that breaks this is offered to the kubelet, allocated, and then fails in QEMU with "group is not viable".
+ * Host side: for a non-directory entry that is not a class candidate, the host reads its `driver` link; when that
+ * driver is bound and not in the caller's viability list (the class drivers always count as allowed), it reads
+ * `iommu_group`, and when that is a canonical decimal below 4294967295 it stores the group and the driver (first 15
+ * bytes) and sets KXPU_REC_BLOCKS.
+ *   - a record is a BLOCKER when it carries KXPU_REC_BLOCKS, is not KXPU_REC_IS_DIR and is not a candidate of any rule
+ *     (a candidate ignores the flag: a class driver is always allowed);
+ *   - group_blocker[o], for each group ordinal o < n_groups, is min{ i : record i is a blocker and
+ *     iommu_group(i) == group_ids[o] }, or KXPU_VIABLE when there is none.  The minimum is walk order, so the host
+ *     names the first blocking function.  A blocker may come before or after the group's first accepted record;
+ *     blockers of groups that never come into existence (no candidate, or none whose device read works) produce
+ *     nothing;
+ *   - a blocker with iommu_group = 0xFFFFFFFF is outside the domain: KXPU_E_UNSUPPORTED, as for a candidate.
+ * group_numa == NULL: every other output equals kxpu_classify_rules'; otherwise kxpu_classify_topo's (group_numa then
+ * receives the masks).  KXPU_REC_BLOCKS changes nothing else, in this call or in any other.  Argument checks are
+ * kxpu_classify_topo's, with group_blocker required instead of group_numa.
+ * GPU: the candidate pass inserts a blocker's group into the same group table and lowers a spare word of its slot
+ * with an atomic min; the per-group pass reads that word.  Same launches as kxpu_classify_rules / _topo.
+ * vGPUs are out of scope: an mdev's IOMMU group is its own. */
+#define KXPU_VIABLE 0xFFFFFFFFu
+int32_t kxpu_classify_viable(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs,
+                             size_t n, kxpu_classify_out *out, uint8_t *dev_rule /* [n] */,
+                             uint64_t *group_numa /* [n] or NULL */, uint32_t *group_blocker /* [n] */);
 
 /* GetPreferredAllocation (the reference returns nil, nil: generic_device_plugin.go:378-386), batched over the
  * container requests of one PreferredAllocationRequest.  dev_numa[d] is the NUMA mask of the plugin's device d (the

@@ -383,6 +383,42 @@ func (k *kxpu) groupNuma(out *C.kxpu_classify_out, rules []C.kxpu_xpu_rule, recs
 	return gnuma[:out.n_groups], kxCheck(k.ctx, "kxpu_classify_topo", rc)
 }
 
+// IOMMU group viability (ABI v8).  With it on, the PCI walk sets KXPU_REC_BLOCKS, the group and the driver on every
+// function that is not a class candidate and is bound to a driver outside the viability list, and the Go call sites use
+// the first blocker of each group:
+//   - createIommuDeviceMap: classifyViable in place of classifyRules / groupNuma, one "<bdf> is bound to <driver>" per
+//     group with a blocker;
+//   - createDevicePlugins / ListAndWatch: such a group's Device is sent Unhealthy whatever its health watch says;
+//   - Allocate: a request naming such a group fails before any read.
+
+// classifyRules plus the first blocking record of every group (KXPU_VIABLE: none); topo also fills the NUMA masks
+// (kxpu_classify_topo's), else gnuma is nil.  out must be wired and pinned as for classifyRules.
+func (k *kxpu) classifyViable(out *C.kxpu_classify_out, rules []C.kxpu_xpu_rule, recs []C.kxpu_devrec, devRule []uint8,
+	topo bool) (blockers []uint32, gnuma []uint64, err error) {
+	n := len(recs)
+	blockers = make([]uint32, n)
+	if topo {
+		gnuma = make([]uint64, n)
+	}
+	if n == 0 {
+		return blockers, gnuma, nil
+	}
+	var rp *C.kxpu_xpu_rule
+	if len(rules) > 0 {
+		rp = &rules[0]
+	}
+	var np *C.uint64_t
+	if topo {
+		np = (*C.uint64_t)(unsafe.Pointer(&gnuma[0]))
+	}
+	rc := C.kxpu_classify_viable(k.ctx, rp, C.size_t(len(rules)), &recs[0], C.size_t(n), out,
+		(*C.uint8_t)(unsafe.Pointer(&devRule[0])), np, (*C.uint32_t)(unsafe.Pointer(&blockers[0])))
+	if topo {
+		gnuma = gnuma[:out.n_groups]
+	}
+	return blockers[:out.n_groups], gnuma, kxCheck(k.ctx, "kxpu_classify_viable", rc)
+}
+
 // pluginapi.TopologyInfo of a mask: one NUMANode per set bit, ascending; nil for 0 (no topology)
 func topologyInfo(mask uint64) *pluginapi.TopologyInfo {
 	if mask == 0 {

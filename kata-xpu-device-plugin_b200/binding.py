@@ -21,6 +21,8 @@ COMM_ID_BYTES = 128
 REC_VENDOR_ERR, REC_DRIVER_ERR, REC_IOMMU_ERR, REC_DEVICE_ERR, REC_IS_DIR, REC_NAME_ERR = 1, 2, 4, 8, 16, 32
 REC_NUMA = 64  # the record's numa_node byte is valid (ABI v5)
 MAX_NUMA_NODES = 64
+REC_BLOCKS = 0x80  # bound to a driver outside the viability list; iommu_group holds its group (ABI v8)
+VIABLE = 0xFFFFFFFF  # kxpu_classify_viable: the group has no blocker
 # The numa_node byte of kxpu_devrec / kxpu_mdevrec (ABI v5) keeps its pre-v5 numpy field name "reserved0": the
 # dtypes below must stay equal to the checkers' (oracle/*.py), which compare dtypes field name by field name.
 NUMA_FIELD = "reserved0"
@@ -64,7 +66,7 @@ ABI_SYMBOLS = [
     "kxpu_classify_mdev", "kxpu_mdev_names", "kxpu_cdi_emit_mdev",
     "kxpu_pciids_full_load_device", "kxpu_full_free", "kxpu_full_export", "kxpu_full_lookup",
     "kxpu_classify_topo", "kxpu_classify_mdev_topo", "kxpu_lw_encode_topo", "kxpu_preferred_allocation",
-    "kxpu_reconcile", "kxpu_pcie_tree", "kxpu_preferred_allocation_pcie",
+    "kxpu_reconcile", "kxpu_pcie_tree", "kxpu_preferred_allocation_pcie", "kxpu_classify_viable",
 ]
 
 
@@ -163,6 +165,7 @@ def load_library():
         "kxpu_reconcile": (i32, [vp, vp, sz, u64, vp, sz, vp, vp, vp, vp]),
         "kxpu_pcie_tree": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32)]),
         "kxpu_preferred_allocation_pcie": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp, sz, vp, vp]),
+        "kxpu_classify_viable": (i32, [vp, vp, sz, vp, sz, C.POINTER(ClassifyOut), vp, vp, vp]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -494,6 +497,33 @@ class Kxpu:
                     group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
                     dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g], dev_rule=dev_rule[:d],
                     group_numa=gnuma[:g])
+
+    def classify_viable(self, rules, recs, topo=False):
+        """kxpu_classify_viable (DEVREC_DTYPE records): the dict of classify_rules (topo=False) or classify_topo
+        (topo=True) plus group_blocker, the first blocking record of every group ordinal or VIABLE."""
+        ra = rules_array(rules)
+        recs = np.ascontiguousarray(recs)
+        assert recs.dtype == DEVREC_DTYPE
+        n = len(recs)
+        arrs = dict(accept_index=np.empty(n, np.uint32), group_ids=np.empty(n, np.uint32),
+                    group_off=np.empty(n + 1, np.uint32), group_members=np.empty(n, np.uint32),
+                    dev_ids=np.empty(n, np.uint64), dev_off=np.empty(n + 1, np.uint32),
+                    dev_groups=np.empty(n, np.uint32))
+        dev_rule = np.empty(max(n, 1), np.uint8)
+        gnuma = np.empty(max(n, 1), np.uint64) if topo else None
+        gblk = np.empty(max(n, 1), np.uint32)
+        out = ClassifyOut(**{k: v.ctypes.data for k, v in arrs.items()})
+        self._chk(self.L.kxpu_classify_viable(self.ctx, _ptr(ra) if len(ra) else None, len(ra), _ptr(recs) if n else None,
+                                              n, C.byref(out), _ptr(dev_rule), _ptr(gnuma), _ptr(gblk)))
+        g, d, a = out.n_groups, out.n_devids, out.n_accepted
+        res = dict(accept_index=arrs["accept_index"], n_accepted=a, n_groups=g, n_devids=d,
+                   group_ids=arrs["group_ids"][:g], group_off=arrs["group_off"][:g + 1],
+                   group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
+                   dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g], dev_rule=dev_rule[:d],
+                   group_blocker=gblk[:g])
+        if topo:
+            res["group_numa"] = gnuma[:g]
+        return res
 
     def lw_encode_topo(self, groups, healthy=None, masks=None):
         """kxpu_lw_encode_topo: ListAndWatchResponse bytes with Device.topology from the NUMA masks."""

@@ -17,6 +17,8 @@
 // kxpu_classify_mdev: the candidate kernel reads 128-byte mdev records and writes each candidate's type key; a
 // name-intern pass maps every key to the first candidate carrying it (hash table, keys compared byte for byte);
 // the device-id key becomes (rule << 48 | that record's index).  Everything from k_accept_scan on is shared.
+// kxpu_classify_viable: k_candidates_viable also folds the first blocker of every group into the group table's spare
+// word, k_groups<MODE_VIAB> copies it out per ordinal (both on kxpu_classify_rules' launches).
 // kxpu_classify_topo / _mdev_topo: k_pairs<true> also ORs each accepted record's NUMA node into its group ordinal's mask
 // (zeroed by k_reset with the totals); same launches as the non-topology call.
 // Launches: reset | candidates | accept + both scans (single pass, decoupled look-back) | per-group device ids | device-id
@@ -34,7 +36,8 @@ namespace kxclass {
 constexpr uint32_t EMPTY32 = 0xFFFFFFFFu;
 constexpr unsigned long long EMPTY64 = 0xFFFFFFFFFFFFFFFFull;
 
-struct __align__(16) GSlot { uint32_t key, first, ord, pad; };                // iommu group -> first good record, ordinal
+// iommu group -> first good record, ordinal; pad: first blocker of the group (kxpu_classify_viable only)
+struct __align__(16) GSlot { uint32_t key, first, ord, pad; };
 struct __align__(16) DSlot { unsigned long long key; uint32_t first, ord; };  // device id string -> first group-first record, ordinal
 struct __align__(16) ISlot { unsigned long long tag; uint32_t first, pad; };   // type key: hash << 32 | some record with it; first such record
 
@@ -67,13 +70,16 @@ struct Work {
     // byte 47), intern slot of each record (EMPTY32: no key to intern) and the intern table
     const kxpu_mdevrec *mrecs;
     uint4 *keybuf;
-    uint32_t *islot;
+    union {
+        uint32_t *islot;
+        uint32_t *group_blocker;  // kxpu_classify_viable only (never mdev): [n] first blocker per group ordinal
+    };
     ISlot *itab;
     uint32_t icap, ishift;
     // kxpu_classify_topo / _mdev_topo only: [n] NUMA mask per group ordinal (zeroed by k_reset)
     unsigned long long *group_numa;
 };
-enum { MODE_NV = 0, MODE_RULES = 1, MODE_MDEV = 2 };
+enum { MODE_NV = 0, MODE_RULES = 1, MODE_MDEV = 2, MODE_VIAB = 3 };
 
 // The rule list of kxpu_classify_rules as k_candidates compares it: per rule the vendor id bytes with the id
 // length in bits 56-63 (the same packing as read_id's result), and the driver as two 64-bit words with
@@ -137,7 +143,10 @@ __device__ __forceinline__ uint32_t dinsert(const Work &W, unsigned long long ke
 
 // pass 1: candidates, group table, gfirst.  RULES: the (vendor, driver) pair is matched against the rule list of
 // kxpu_classify_rules and the matching rule is stored per record for k_groups; otherwise the NVIDIA constants.
-template <bool RULES>
+// VIAB (kxpu_classify_viable): a blocker -- KXPU_REC_BLOCKS, not a directory, not a candidate -- inserts its group too
+// and lowers the slot's pad word (all ones from k_reset) to its index.  Its slot never gets an ordinal: the scans
+// read gslot[i], which stays EMPTY32 for a non-candidate.  Each record inserts at most one group, so gcap >= 2n holds.
+template <bool RULES, bool VIAB = false>
 __device__ __forceinline__ void candidates(const Work &W, const RuleTable &R) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= W.n) return;
@@ -180,12 +189,23 @@ __device__ __forceinline__ void candidates(const Work &W, const RuleTable &R) {
         slot = ginsert(W, group);
         if (dok && i < __ldcg(&W.gtab[slot].first)) atomicMin(&W.gtab[slot].first, i);
     }
+    if (VIAB && !cand && (fl & (KXPU_REC_BLOCKS | KXPU_REC_IS_DIR)) == KXPU_REC_BLOCKS) {
+        if (group == EMPTY32) {
+            atomicOr(&W.totals[3], 1u);  // outside the supported domain, as for a candidate
+        } else {
+            const uint32_t bs = ginsert(W, group);
+            if (i < __ldcg(&W.gtab[bs].pad)) atomicMin(&W.gtab[bs].pad, i);
+        }
+    }
     W.gslot[i] = slot;
     if (RULES) W.rrule[i] = (uint8_t)rule;
 }
 __global__ void __launch_bounds__(256) k_candidates(const Work W) { candidates<false>(W, RuleTable{}); }
 __global__ void __launch_bounds__(256) k_candidates_rules(const Work W, const __grid_constant__ RuleTable R) {
     candidates<true>(W, R);
+}
+__global__ void __launch_bounds__(256) k_candidates_viable(const Work W, const __grid_constant__ RuleTable R) {
+    candidates<true, true>(W, R);
 }
 
 // pass 1 of kxpu_classify_mdev: candidates, group table, gfirst (a group starts at a candidate with a non-empty type
@@ -359,7 +379,7 @@ __global__ void __launch_bounds__(C_THREADS) k_accept_scan(const Work W) {
 // Kept out of k_accept_scan: there the chain record read -> table insert -> minimum ran serially per record in a
 // divergent loop (6 % issue utilisation); here every group is an independent thread.
 // MODE_RULES: the device-id key is (rule of the first member) << 48 | device id; MODE_MDEV: (rule of the first member)
-// << 48 | first record with its type key.
+// << 48 | first record with its type key.  MODE_VIAB: MODE_RULES plus the group's first blocker from its slot.
 template <int MODE>
 __global__ void __launch_bounds__(256) k_groups(const Work W) {
     const uint32_t o = blockIdx.x * blockDim.x + threadIdx.x;
@@ -380,7 +400,8 @@ __global__ void __launch_bounds__(256) k_groups(const Work W) {
     unsigned long long did;
     uint32_t dl;
     read_id(reinterpret_cast<const uint8_t *>(&dq), dlen, did, dl);
-    if (MODE == MODE_RULES) did |= (unsigned long long)W.rrule[i] << 48;
+    if (MODE == MODE_RULES || MODE == MODE_VIAB) did |= (unsigned long long)W.rrule[i] << 48;
+    if (MODE == MODE_VIAB) W.group_blocker[o] = W.gtab[W.gslot[i]].pad;
     const uint32_t ds = dinsert(W, did);
     // a few hot device ids own most groups: same-address atomics run at ~1 per ns, so only a group that can
     // still lower the minimum issues one
@@ -607,19 +628,20 @@ static uint32_t bits_for(uint32_t n) {
 
 // R == nullptr: kxpu_classify (the NVIDIA constants); else the rule list of kxpu_classify_rules, or with mdev of
 // kxpu_classify_mdev (recs then points at kxpu_mdevrec records)
-// group_numa != nullptr: the _topo calls (NUMA mask per group)
+// group_numa != nullptr: the _topo calls (NUMA mask per group); group_blocker != nullptr: kxpu_classify_viable
 static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
-                             bool mdev, uint8_t *dev_rule, uint64_t *group_numa, bool small_dtab, bool *retry);
+                             bool mdev, uint8_t *dev_rule, uint64_t *group_numa, uint32_t *group_blocker, bool small_dtab,
+                             bool *retry);
 
 static int32_t classify_run(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R, bool mdev,
-                            uint8_t *dev_rule, uint64_t *group_numa = nullptr) {
+                            uint8_t *dev_rule, uint64_t *group_numa = nullptr, uint32_t *group_blocker = nullptr) {
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
     bool retry = false;
-    int32_t rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, true, &retry);
-    // more distinct device ids (or type keys) than the small tables hold
-    if (retry) rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, false, &retry);
+    int32_t rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, group_blocker, true, &retry);
+    // more distinct device ids (or type keys) than the small tables hold; the rerun resets every table, blockers included
+    if (retry) rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, group_blocker, false, &retry);
     return rc;
 }
 
@@ -710,8 +732,21 @@ extern "C" int32_t kxpu_classify_mdev_topo(kxpu_ctx *ctx, const kxpu_xpu_rule *r
     return classify_run(ctx, recs, n, out, &R, true, dev_rule, group_numa);
 }
 
+extern "C" int32_t kxpu_classify_viable(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs,
+                                        size_t n, kxpu_classify_out *out, uint8_t *dev_rule, uint64_t *group_numa,
+                                        uint32_t *group_blocker) {
+    if (!ctx || !out || (n && (!recs || !group_blocker)) || !rules || n_rules == 0 || n_rules > KXPU_MAX_RULES)
+        return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    RuleTable R;
+    const int32_t rc = rule_table(ctx, rules, n_rules, R);
+    if (rc != KXPU_OK) return rc;
+    return classify_run(ctx, recs, n, out, &R, false, dev_rule, group_numa, group_blocker);
+}
+
 static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
-                             bool mdev, uint8_t *dev_rule, uint64_t *group_numa, bool small_dtab, bool *retry) {
+                             bool mdev, uint8_t *dev_rule, uint64_t *group_numa, uint32_t *group_blocker, bool small_dtab,
+                             bool *retry) {
     *retry = false;
     out->n_accepted = out->n_groups = out->n_devids = 0;
     if (n == 0) {
@@ -754,6 +789,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
     const size_t o_dids = take(n * 8), o_doff = take((n + 1) * 4);
     const size_t o_rrule = R ? take(n) : 0, o_drule = R ? take(n) : 0;
     const size_t o_keys = mdev ? take(n * 48) : 0, o_islot = mdev ? take(n * 4) : 0;
+    const size_t o_gblk = group_blocker ? take(n * 4) : 0;  // every ordinal is written by k_groups: no reset
     KxScratch sc(ctx);
     uint8_t *b = nullptr;
     KX_CUDA(ctx, sc.alloc((void **)&b, off));
@@ -775,6 +811,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
     W.group_off = (uint32_t *)(b + o_goff); W.dev_ids = (unsigned long long *)(b + o_dids); W.dev_off = (uint32_t *)(b + o_doff);
     if (R) { W.rrule = b + o_rrule; W.dev_rule = b + o_drule; }
     if (group_numa) W.group_numa = (unsigned long long *)(b + o_gnuma);
+    if (group_blocker) W.group_blocker = (uint32_t *)(b + o_gblk);
     if (mdev) {
         W.mrecs = (const kxpu_mdevrec *)(b + o_recs);
         W.keybuf = (uint4 *)(b + o_keys); W.islot = (uint32_t *)(b + o_islot);
@@ -793,10 +830,12 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
             k_candidates_mdev<<<g, 256, 0, ctx->stream>>>(W, *R);
             k_intern<<<g, 256, 0, ctx->stream>>>(W);
             ctx->launches++;
-        } else if (R) k_candidates_rules<<<g, 256, 0, ctx->stream>>>(W, *R);
+        } else if (group_blocker) k_candidates_viable<<<g, 256, 0, ctx->stream>>>(W, *R);
+        else if (R) k_candidates_rules<<<g, 256, 0, ctx->stream>>>(W, *R);
         else k_candidates<<<g, 256, 0, ctx->stream>>>(W);
         k_accept_scan<<<c_tiles, C_THREADS, 0, ctx->stream>>>(W);
         if (mdev) k_groups<MODE_MDEV><<<g, 256, 0, ctx->stream>>>(W);
+        else if (group_blocker) k_groups<MODE_VIAB><<<g, 256, 0, ctx->stream>>>(W);
         else if (R) k_groups<MODE_RULES><<<g, 256, 0, ctx->stream>>>(W);
         else k_groups<MODE_NV><<<g, 256, 0, ctx->stream>>>(W);
         k_devfirst_scan<<<c_tiles, C_THREADS, 0, ctx->stream>>>(W);
@@ -840,6 +879,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
         cudaMemcpyAsync(out->dev_groups, bv, (size_t)ng * 4, cudaMemcpyDeviceToHost, ctx->stream);
         if (dev_rule && nd) cudaMemcpyAsync(dev_rule, W.dev_rule, nd, cudaMemcpyDeviceToHost, ctx->stream);
         if (group_numa && ng) cudaMemcpyAsync(group_numa, W.group_numa, (size_t)ng * 8, cudaMemcpyDeviceToHost, ctx->stream);
+        if (group_blocker && ng) cudaMemcpyAsync(group_blocker, W.group_blocker, (size_t)ng * 4, cudaMemcpyDeviceToHost, ctx->stream);
         e = cudaStreamSynchronize(ctx->stream);
         if (e != cudaSuccess) { KX_SET_ERR(ctx, "classify D2H failed: %s", cudaGetErrorString(e)); rc = KXPU_E_CUDA; }
         if (ng == 0) out->group_off[0] = 0;

@@ -253,15 +253,39 @@ static bool packID(const std::string &raw, uint8_t txt[8], uint8_t &len) {
 // skipped like a read error -- and only if the reference would have accepted it; it never stops the walk.
 // readNuma == nullptr: numa_node is not read (Plugin::topologyAware false).  It is read last, only for a record that
 // got as far as its device read, and changes nothing but numa_node / KXPU_REC_NUMA.
+// allowed == nullptr: Plugin::groupViability false.  Otherwise an entry the class test rejected is a blocker when its
+// driver (the `driver` link, read here if the class test did not read it) is bound and not in *allowed: the record then
+// carries its `iommu_group` and driver and KXPU_REC_BLOCKS.  An unbound entry (failed read) is not a blocker; a group
+// link outside the record's domain is logged and leaves the record as it is.
+static bool parseGroup(const std::string &s, uint32_t &v);
 template <typename ReadID, typename ReadLnk, typename ReadNuma>
 static Error leafRecord(const std::string &name, const std::vector<XpuClass> &classes, ReadID readID, ReadLnk readLnk,
-                        const ReadNuma *readNuma, kxpu_devrec &r) {
+                        const ReadNuma *readNuma, const std::vector<std::string> *allowed, kxpu_devrec &r) {
     memset(&r, 0, sizeof r);
     strncpy(r.bdf, name.c_str(), sizeof r.bdf - 1);
     std::string s;
+    // drv: the driver's basename when the class test read it already
+    auto viability = [&](const std::string *drv) {
+        if (!allowed) return Error();
+        std::string d, g;
+        if (drv) d = *drv;
+        else if (!readLnk("driver", d)) return Error();
+        if (std::find(allowed->begin(), allowed->end(), d) != allowed->end()) return Error();
+        uint32_t v = 0;
+        if (!readLnk("iommu_group", g) || !parseGroup(g, v)) {
+            fprintf(stderr, "%s is bound to %s but its iommu_group is not a canonical decimal below 2^32-1: viability unknown\n",
+                    name.c_str(), d.c_str());
+            return Error();
+        }
+        r.iommu_group = v;
+        memset(r.driver, 0, sizeof r.driver);
+        memcpy(r.driver, d.data(), std::min<size_t>(d.size(), sizeof r.driver - 1));
+        r.flags |= KXPU_REC_BLOCKS;
+        return Error();
+    };
     if (!readID("vendor", s)) {
         r.flags |= KXPU_REC_VENDOR_ERR;  // "Could not get vendor ID for device" -> skipped (:143-146)
-        return Error();
+        return viability(nullptr);
     }
     const std::string vendor = trimID(s);
     bool known = false;  // :149 -- the vendor of some class
@@ -271,7 +295,7 @@ static Error leafRecord(const std::string &name, const std::vector<XpuClass> &cl
         r.vendor_len = 8;
         r.flags |= KXPU_REC_VENDOR_ERR;
     }
-    if (!known) return Error();
+    if (!known) return viability(nullptr);
     if (!readLnk("driver", s)) {
         r.flags |= KXPU_REC_DRIVER_ERR;  // :152-155
         return Error();
@@ -279,7 +303,7 @@ static Error leafRecord(const std::string &name, const std::vector<XpuClass> &cl
     memcpy(r.driver, s.data(), std::min<size_t>(s.size(), sizeof r.driver - 1));
     bool bound = false;  // :156 -- the driver of that vendor's class
     for (const XpuClass &c : classes) bound = bound || (vendor == c.vendor && s == c.driver);
-    if (!bound) return Error();
+    if (!bound) return viability(&s);
     if (name.size() > sizeof r.bdf - 1) {
         fprintf(stderr, "PCI address longer than 15 bytes, device skipped: %s\n", name.c_str());
         r.flags |= KXPU_REC_IOMMU_ERR;
@@ -313,6 +337,14 @@ static Error leafRecord(const std::string &name, const std::vector<XpuClass> &cl
     return Error();
 }
 
+// groupViability: the drivers that leave a group viable (viabilityDrivers and every class driver); nullptr when off
+static const std::vector<std::string> *allowedDrivers(const Plugin &p, std::vector<std::string> &buf) {
+    if (!p.groupViability) return nullptr;
+    buf = p.viabilityDrivers;
+    for (const XpuClass &c : p.xpuClasses) buf.push_back(c.driver);
+    return &buf;
+}
+
 // filepath.Walk(basePath, ...) (device_plugin.go:132): lexical order, os.Lstat (symlinks are not
 // followed, so a real sysfs entry is "not a directory"), directories are descended into and
 // reported as "Not a device" (:137-140).
@@ -340,10 +372,11 @@ static Error walkDir(Plugin &p, const std::string &path, const std::string &name
     // info.Name() under basePath exactly like :142,:151,:157,:164
     kxpu_devrec r;
     auto readNuma = [&](std::string &out) { return p.readNumaNode(p.basePath, name, out); };
+    std::vector<std::string> allowed;
     Error e = leafRecord(name, p.xpuClasses,
                          [&](const char *prop, std::string &out) { return p.readIDFromFile(p.basePath, name, prop, out); },
                          [&](const char *link, std::string &out) { return p.readLink(p.basePath, name, link, out); },
-                         p.topologyAware ? &readNuma : nullptr, r);
+                         p.topologyAware ? &readNuma : nullptr, allowedDrivers(p, allowed), r);
     if (e) return e;
     recs.push_back(r);
     if (paths) {  // pcieTopologyAware: the entry's link, one readlink
@@ -409,6 +442,8 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
     std::vector<kxpu_devrec> flat(N);
     std::vector<kxpu_pcipath> flatPaths(paths ? N : 0);
     std::vector<Error> errs(N);
+    std::vector<std::string> allowedBuf;
+    const std::vector<std::string> *allowed = allowedDrivers(*this, allowedBuf);
     auto readID = [&](const std::string &name, const char *prop, std::string &out) {
         const std::string rel = name + "/" + prop;
         int fd = openat(basefd, rel.c_str(), O_RDONLY | O_CLOEXEC);
@@ -459,7 +494,7 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
             };
             errs[i] = leafRecord(name, xpuClasses, [&](const char *prop, std::string &out) { return readID(name, prop, out); },
                                  [&](const char *link, std::string &out) { return readLnk(name, link, out); },
-                                 topologyAware ? &readNuma : nullptr, flat[i]);
+                                 topologyAware ? &readNuma : nullptr, allowed, flat[i]);
             if (paths && !errs[i]) {  // the entry's own link on the same directory descriptor
                 char buf[4096];
                 const ssize_t k = readlinkat(basefd, name.c_str(), buf, sizeof buf);
@@ -564,6 +599,11 @@ static size_t recordClass(const std::vector<XpuClass> &classes, const uint8_t *v
     return cls;
 }
 
+// "<bdf> is bound to <driver>" of a blocking record
+static std::string blockerOf(const kxpu_devrec &r) {
+    return std::string(r.bdf, strnlen(r.bdf, sizeof r.bdf)) + " is bound to " + std::string(r.driver, strnlen(r.driver, sizeof r.driver));
+}
+
 // the walk and classify of createIommuDeviceMap
 Error Plugin::classifyPci(PciWalk &w) {
     Error e = gatherRecordsFast(w.recs, 0, &w.paths);  // same records as gatherRecords (falls back to it when a seam was replaced)
@@ -574,11 +614,25 @@ Error Plugin::classifyPci(PciWalk &w) {
     kxpu_classify_out out = c.wire(n);
     const std::vector<kxpu_xpu_rule> rules = classRules(xpuClasses);
     // fatal on failure: there is no CPU path
-    int32_t rc = topologyAware ? kxpu_classify_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(), c.gnuma.data())
-                               : kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data());
-    if (rc != KXPU_OK) return kxfail(ctx_, topologyAware ? "kxpu_classify_topo" : "kxpu_classify_rules", rc);
+    int32_t rc;
+    const char *what;
+    if (groupViability) {
+        c.gblk.assign(n ? n : 1, KXPU_VIABLE);
+        rc = kxpu_classify_viable(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(),
+                                  topologyAware ? c.gnuma.data() : nullptr, c.gblk.data());
+        what = "kxpu_classify_viable";
+    } else {
+        rc = topologyAware ? kxpu_classify_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(), c.gnuma.data())
+                           : kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data());
+        what = topologyAware ? "kxpu_classify_topo" : "kxpu_classify_rules";
+    }
+    if (rc != KXPU_OK) return kxfail(ctx_, what, rc);
     c.nGroups = out.n_groups;
     c.nDevids = out.n_devids;
+    if (groupViability)
+        for (uint32_t g = 0; g < c.nGroups; g++)
+            if (c.gblk[g] != KXPU_VIABLE)
+                fprintf(stderr, "IOMMU group %u is not viable: %s\n", c.gids[g], blockerOf(recs[c.gblk[g]]).c_str());
     if (pcieTopologyAware) {  // the forest of the walk, one node per group
         const size_t cap = (size_t)KXPU_PCIE_MAX_DEPTH * c.nGroups + 1;
         w.gnode.assign(c.nGroups + 1, KXPU_PCIE_NO_NODE);
@@ -597,6 +651,7 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
     deviceClass.clear();
     iommuNuma.clear();
     iommuPcieNode.clear();
+    iommuBlocker.clear();
     const ClassifyResult &c = w.out;
     std::map<uint32_t, size_t> groupClass = groupClasses(c);
     for (uint32_t g = 0; g < c.nGroups; g++) {
@@ -611,6 +666,7 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
         iommuClass.push_back(groupClass[c.gids[g]]);
         if (topologyAware) iommuNuma.push_back(c.gnuma[g]);
         if (pcieTopologyAware) iommuPcieNode.push_back(w.gnode[g]);
+        if (groupViability) iommuBlocker.push_back(c.gblk[g] == KXPU_VIABLE ? std::string() : blockerOf(w.recs[c.gblk[g]]));
     }
     if (pcieTopologyAware) {
         pcieParent.assign(w.nodeParent.begin(), w.nodeParent.begin() + w.nNodes);
@@ -1118,12 +1174,18 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         auto it = nodeOf.find(g);
         return it == nodeOf.end() ? KXPU_PCIE_NO_NODE : it->second;
     };
+    std::map<std::string, std::string> blockerOfGroup;  // group id -> its first blocker (groupViability)
+    for (size_t g = 0; g < iommuBlocker.size() && g < iommuMap.size(); g++)
+        if (!iommuBlocker[g].empty()) blockerOfGroup[iommuMap[g].first] = iommuBlocker[g];
     size_t at = 0;
     for (const auto &kv : deviceMap) {  // :91
         GenericDevicePlugin dp;
         dp.xpuClass = at < deviceClass.size() ? deviceClass[at] : 0;
         dp.resourceNamespace = xpuClasses[dp.xpuClass].resourceNamespace;
-        for (const std::string &dev : kv.second) dp.devs.push_back(Device{dev, kHealthy, maskOf(numaOf, dev), pcieNodeOf(dev)});  // :93-98
+        for (const std::string &dev : kv.second) {  // :93-98
+            auto it = blockerOfGroup.find(dev);
+            dp.devs.push_back(Device{dev, kHealthy, maskOf(numaOf, dev), pcieNodeOf(dev), it == blockerOfGroup.end() ? std::string() : it->second});
+        }
         std::string devpluginName = names[at++];
         if (devpluginName.empty()) {
             fprintf(stderr, "Error: Could not find device name for device id: %s\n", kv.first.c_str());
@@ -1249,7 +1311,7 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         bool same = cur.size() == w.devs.size();
         for (size_t i = 0; same && i < cur.size(); i++)
             same = cur[i].ID == w.devs[i].ID && cur[i].Health == w.devs[i].Health && cur[i].numa == w.devs[i].numa &&
-                   cur[i].pcieNode == w.devs[i].pcieNode;
+                   cur[i].pcieNode == w.devs[i].pcieNode && cur[i].blocker == w.devs[i].blocker;
         if (!same) {
             cur = std::move(w.devs);
             report.changedPlugins.push_back(at);
@@ -1310,6 +1372,9 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
         const std::vector<NvidiaGpuDevice> *nvDevs = nullptr;
         for (const auto &kv : returnedMap) if (kv.first == iommuId) { nvDevs = &kv.second; break; }
         if (!nvDevs) continue;  // unknown group id: empty nvDevs, no error (:327)
+        for (size_t g = 0; g < iommuBlocker.size() && g < iommuMap.size(); g++)  // the verdict of the last walk, before any read
+            if (iommuMap[g].first == iommuId && !iommuBlocker[g].empty())
+                return fail("invalid allocation request: IOMMU group " + iommuId + " is not viable: " + iommuBlocker[g]);
         const size_t c = classOfGroup(iommuId);
         if (haveVgpu || (havePci && c != reqClass)) return fail("invalid allocation request: devices of more than one class");
         havePci = true;
@@ -1354,7 +1419,7 @@ Error Plugin::ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8
     std::vector<uint64_t> masks;
     for (const Device &d : dp.devs) {
         groups.push_back((uint32_t)strtoul(d.ID.c_str(), nullptr, 10));
-        healthy.push_back(d.Health == kHealthy);
+        healthy.push_back(d.Health == kHealthy && d.blocker.empty());  // a group VFIO cannot open is never offered
         masks.push_back(d.numa);
     }
     // topologyAware: Device.topology from each device's mask (the HealthWatcher's re-sends come through here too)
@@ -1885,7 +1950,7 @@ void *kxh_health_start(void *h, int plugin_index, int watch_creates, char *err, 
 int kxh_health_poll(void *w, int timeout_ms) { return ((device_plugin::HealthWatcher *)w)->poll(timeout_ms); }
 void kxh_health_stop(void *w) { delete (device_plugin::HealthWatcher *)w; }
 
-// "id=Health,id=Health,..." of one plugin
+// "id=Health,id=Health,..." of one plugin; a device of a group that is not viable shows "id=Health/<blocker>"
 int kxh_devs(void *h, int plugin_index, char *out, size_t cap) {
     Plugin *p = (Plugin *)h;
     if (plugin_index < 0 || (size_t)plugin_index >= p->devicePlugins.size()) return -1;
@@ -1893,6 +1958,7 @@ int kxh_devs(void *h, int plugin_index, char *out, size_t cap) {
     for (const auto &d : p->devicePlugins[(size_t)plugin_index].devs) {
         if (!o.empty()) o += ',';
         o += d.ID + "=" + d.Health;
+        if (!d.blocker.empty()) o += "/" + d.blocker;
     }
     return copy_out(o, out, cap);
 }
@@ -2055,6 +2121,61 @@ int kxh_devs_numa(void *h, int plugin_index, char *out, size_t cap) {
         o += d.ID + "=" + std::to_string(d.numa);
     }
     return copy_out(o, out, cap);
+}
+
+// ---- IOMMU group viability (tests)
+// on != 0: groupViability; drivers_csv != NULL replaces viabilityDrivers ("" = none)
+void kxh_set_viability(void *h, int on, const char *drivers_csv) {
+    Plugin *p = (Plugin *)h;
+    p->groupViability = on != 0;
+    if (!drivers_csv) return;
+    p->viabilityDrivers.clear();
+    std::string cur;
+    for (const char *c = drivers_csv;; c++) {
+        if (*c == ',' || *c == 0) {
+            if (!cur.empty()) p->viabilityDrivers.push_back(cur);
+            cur.clear();
+            if (*c == 0) break;
+        } else {
+            cur += *c;
+        }
+    }
+}
+
+// CPU only: the raw PCI gather under a class list with groupViability = on (drivers_csv as kxh_set_viability); fast = the
+// batched / threaded variant.  counting_seam != 0 wraps readLink in a counter of the `driver` and `iommu_group` reads of
+// entries whose vendor no class has (*foreign_reads), which also sends the fast gather down the walk
+int kxh_gather_viab(const char *base_path, const char *classes, int on, const char *drivers_csv, int fast, unsigned threads,
+                    int counting_seam, kxpu_devrec *out, size_t cap, size_t *n, uint64_t *foreign_reads, char *err, size_t errcap) {
+    Plugin p(nullptr);
+    p.basePath = base_path;
+    if (!parseClasses(classes, p.xpuClasses)) { copy_out("malformed class list", err, errcap); return -1; }
+    kxh_set_viability(&p, on, drivers_csv);
+    *foreign_reads = 0;
+    if (counting_seam) {
+        auto dflt = p.readLink;
+        auto readID = p.readIDFromFile;
+        const std::vector<device_plugin::XpuClass> classList = p.xpuClasses;
+        p.readLink = [dflt, readID, classList, foreign_reads](const std::string &base, const std::string &addr,
+                                                               const std::string &link, std::string &o) {
+            std::string v;
+            bool known = false;
+            if (readID(base, addr, "vendor", v) && v.size() > 2) {
+                std::string id = v.substr(2);
+                while (!id.empty() && id.back() == '\n') id.pop_back();
+                for (const auto &c : classList) known = known || c.vendor == id;
+            }
+            if (!known) (*foreign_reads)++;
+            return dflt(base, addr, link, o);
+        };
+    }
+    std::vector<kxpu_devrec> recs;
+    device_plugin::Error e = fast ? p.gatherRecordsFast(recs, threads) : p.gatherRecords(recs);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    *n = recs.size();
+    if (recs.size() > cap) return -2;
+    memcpy(out, recs.data(), recs.size() * sizeof(kxpu_devrec));
+    return 0;
 }
 
 }  // extern "C"

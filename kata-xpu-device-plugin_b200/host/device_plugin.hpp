@@ -52,6 +52,9 @@ struct Device {  // pluginapi.Device
     std::string Health;
     uint64_t numa = 0;  // Device.Topology: bit k = NUMA node k (the group's mask); 0 = no topology
     uint32_t pcieNode = KXPU_PCIE_NO_NODE;  // the group's node in Plugin::pcieParent / pcieDepth (pcieTopologyAware)
+    // groupViability: why VFIO cannot open the group ("<bdf> is bound to <driver>"), from the last walk; empty = viable.
+    // Separate from Health, which the HealthWatcher flips: the device is sent Unhealthy when either says so.
+    std::string blocker{};
 };
 // pluginapi.DevicePluginOptions (GetDevicePluginOptions, generic_device_plugin.go:253-258)
 struct DevicePluginOptions {
@@ -178,6 +181,7 @@ Error writeSpecFileAtomicForTests(const std::string &file_path, const uint8_t *d
 struct ClassifyResult {
     std::vector<uint32_t> accept, gids, goff, gmem, doff, dgrp;
     std::vector<uint64_t> dids, gnuma;
+    std::vector<uint32_t> gblk;  // groupViability: first blocking record per group ordinal, or KXPU_VIABLE
     std::vector<uint8_t> drule;
     uint32_t nGroups = 0, nDevids = 0;
     // sizes the arrays for n records and points a kxpu_classify_out at them
@@ -248,6 +252,14 @@ class Plugin {
     // (kxpu_preferred_allocation_pcie; vGPU plugins keep the NUMA answer).  Both settings may be on together.
     bool pcieTopologyAware = false;
     std::function<bool(const std::string &base, const std::string &entry, std::string &target)> readPciPath;
+    // IOMMU group viability (include/kxpu.h, ABI v8).  false (default): nothing more is read and every output is as
+    // above.  true: for every non-directory entry that is not a class candidate the gathers read its `driver` link (when
+    // not read yet); a bound driver that is neither in viabilityDrivers nor the driver of a class makes the entry a
+    // blocker of the group its `iommu_group` link names (KXPU_REC_BLOCKS).  Classify runs kxpu_classify_viable; every
+    // device of a group with a blocker is sent Unhealthy and Allocate refuses it, naming the blocking function.  CDI specs
+    // and vGPU plugins do not change.
+    bool groupViability = false;
+    std::vector<std::string> viabilityDrivers{"vfio-pci", "pci-stub", "pcieport"};
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
 
     // ---- state (device_plugin.go:31,34)
@@ -263,6 +275,8 @@ class Plugin {
     // passthrough plugins
     std::vector<uint32_t> iommuPcieNode, pcieParent;
     std::vector<uint8_t> pcieDepth;
+    // groupViability only: "<bdf> is bound to <driver>" of the first blocker of every iommuMap entry; empty = viable
+    std::vector<std::string> iommuBlocker;
     std::vector<std::string> cdiFiles;  // files the last generateCDISpec wrote, one per class
     // the mdev walk: IOMMU group -> mdevs, type key -> groups, and the vGPU class of every entry (same positions)
     OrderedMap<std::vector<MdevDevice>> mdevMap;
@@ -291,7 +305,8 @@ class Plugin {
     // device_plugin.go:83-112: per device id device lists + plugin objects (S4), then one plugin per (vGPU class, type
     // key); nothing is started
     Error createDevicePlugins();
-    // generic_device_plugin.go:320-355 for one container request (S5)
+    // generic_device_plugin.go:320-355 for one container request (S5).  groupViability: a group the last walk found not
+    // viable fails the request before any read
     Error Allocate(const std::vector<std::string> &devicesIDs, ContainerAllocateResponse &resp);
     // generic_device_plugin.go:224: the bytes of ListAndWatchResponse{Devices: dpi.devs}
     Error ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8_t> &out);

@@ -498,3 +498,71 @@ def reconcile_pair(seed=3, n=1 << 20, mdev=False):
     tag_pos = {int(v): i for i, v in enumerate(tags)}
     cur["tag"][t_] = tags[[(tag_pos[int(v)] + 1) % len(tags) for v in cur["tag"][t_]]]
     return prev, cur, n
+
+
+# ---------------------------------------------------------------- IOMMU group viability (ABI v8)
+VIAB_RULES = [(b"10de", b"vfio-pci")]
+
+
+def viab_records(n=1 << 20, seed=31):
+    """n records in HGX-like IOMMU groups for kxpu_classify_viable, one 8-function slot per group.  Slot kinds:
+      - 55 % GPU: a 10de:2330 GPU on vfio-pci and its 10de:22a3 HD-audio function behind it (40 % on snd_hda_intel, a
+        blocker; 40 % on vfio-pci, a member; 20 % unbound).  In a fifth of these slots function 0 is a NIC on ixgbe (a
+        blocker in front of the GPU) and the GPU moves to function 1.  The other functions: 30 % switch ports on
+        pcieport, 10 % on a host driver (blockers behind the members), the rest unbound;
+      - 15 % switch: every function on pcieport;
+      - 15 % host: NVMe drives and NICs on their host drivers, every one a blocker (blocker-only groups);
+      - 15 % empty: every function unbound.
+    A tenth of the slots share the group of the slot before them (no ACS between them), so some groups hold several
+    blockers and a blocker may sit far behind the group's first member.  Blockers carry KXPU_REC_BLOCKS and their
+    group, as the host stores them; unbound functions carry KXPU_REC_DRIVER_ERR."""
+    from .binding import REC_BLOCKS
+    rng = np.random.default_rng(seed)
+    i = np.arange(n, dtype=np.int64)
+    slot, fn = i >> 3, i & 7
+    n_slots = int(slot[-1]) + 1 if n else 0
+    kind = rng.choice(4, n_slots, p=[0.55, 0.15, 0.15, 0.15])[slot]
+    shift = (rng.random(n_slots) < 0.2)[slot]  # GPU slots: a blocker in front of the GPU
+    audio = rng.choice(3, n_slots, p=[0.4, 0.4, 0.2])[slot]
+    merged = rng.random(n_slots) < 0.1
+    merged[:1] = False
+    group = np.arange(n_slots, dtype=np.int64)
+    for s in np.flatnonzero(merged):
+        group[s] = group[s - 1]
+    r = rng.random(n)
+    vendor = np.full(n, 0x8086, np.int64)
+    dev = np.full(n, 0x1533, np.int64)
+    drv = np.full(n, b"", "S16")
+    blocks = np.zeros(n, bool)
+    gpu_fn = np.where(shift, 1, 0)
+    is_gpu = (kind == 0) & (fn == gpu_fn)
+    is_audio = (kind == 0) & (fn == gpu_fn + 1)
+    front = (kind == 0) & shift & (fn == 0)
+    rest = (kind == 0) & ~is_gpu & ~is_audio & ~front
+    vendor[is_gpu | is_audio] = 0x10de
+    dev[is_gpu] = 0x2330
+    dev[is_audio] = 0x22a3
+    drv[is_gpu] = b"vfio-pci"
+    drv[is_audio & (audio == 0)] = b"snd_hda_intel"
+    drv[is_audio & (audio == 1)] = b"vfio-pci"
+    blocks |= is_audio & (audio == 0)
+    drv[front] = b"ixgbe"
+    blocks |= front
+    port = (rest & (r < 0.3)) | (kind == 1)
+    vendor[port], dev[port], drv[port] = 0x10b5, 0xc010, b"pcieport"
+    host = (rest & (r >= 0.3) & (r < 0.4)) | (kind == 2)
+    hsel = rng.integers(0, 3, n)
+    vendor[host] = np.array([0x144d, 0x15b3, 0x8086])[hsel[host]]
+    dev[host] = np.array([0xa80a, 0x1021, 0x10fb])[hsel[host]]
+    drv[host] = np.array([b"nvme", b"mlx5_core", b"ixgbe"], "S16")[hsel[host]]
+    blocks |= host
+    recs = np.zeros(n, dtype=DEVREC_DTYPE)
+    recs["bdf"] = enumerate_bdfs(n).view("S16").reshape(n)
+    recs["vendor_txt"] = _id_text(vendor)
+    recs["device_txt"] = _id_text(dev)
+    recs["vendor_len"] = 7
+    recs["device_len"] = 7
+    recs["driver"] = drv
+    recs["flags"] = np.where(drv == b"", REC_DRIVER_ERR, 0).astype(np.uint8) | np.where(blocks, REC_BLOCKS, 0).astype(np.uint8)
+    recs["iommu_group"] = group[slot].astype(np.uint32)
+    return recs

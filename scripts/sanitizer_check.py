@@ -3,7 +3,7 @@ import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import kxpu_b200 as K
-from kxpu_b200 import workloads as W
+from kxpu_b200 import binding as B, workloads as W
 kx = K.Kxpu(0)
 text = W.load_pci_ids()
 copies = int(os.environ.get("COPIES", "3"))
@@ -37,6 +37,11 @@ print("pcie nodes", len(ptree["key"]), "pref",
 for mdev in (False, True):
     prev, cur, ni = W.reconcile_pair(3, 20000, mdev=mdev)
     print("reconcile", kx.reconcile(prev, cur, ni)["counts"])
+# IOMMU group viability: the blocker pass with and without NUMA masks
+vrecs = W.viab_records(20000)
+for topo in (False, True):
+    vres = kx.classify_viable(W.VIAB_RULES, vrecs, topo=topo)
+    print("viable groups", vres["n_groups"], "blocked", int((vres["group_blocker"] != B.VIABLE).sum()))
 
 
 # look-back state across epoch wraps (tests/test_gpu_lookback_state.py at reduced sizes): every user of the status
