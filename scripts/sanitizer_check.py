@@ -121,4 +121,42 @@ for rep in range(3):
         t.free()
 for k2, d, dq, dr in bufs:
     k2.dev_free(d); k2.dev_free(dq); k2.dev_free(dr)
+bufs = []
+# the same group at the peer slab's edges (tests/test_gpu_sharded.py): rank 1 with exactly 65 536 winner rows, rank 2
+# with exactly 2 MiB of names, every offset past 2^32; parts of one length (comment lines behind the vendor line) so
+# that the cuts fall between them
+rng = np.random.default_rng(1)
+alnum = np.frombuffer(b"ABCDEFGHIJKLMNOPQRSTUVWXYZ0123456789", np.uint8)
+parts = []
+for v, n_dev, name_len in ((0x1000, 1, 8), (0x1001, 65536, 1), (0x1002, 32768, 64)):
+    nm = alnum[rng.integers(0, len(alnum), n_dev * name_len)].tobytes()
+    parts.append([b"%04x  V\n" % v, b"".join(b"\t%04x  " % d + nm[d * name_len:(d + 1) * name_len] + b"\n" for d in range(n_dev))])
+plen = max(len(h) + len(b) for h, b in parts) + 2
+edge = b""
+for h, b in parts:
+    pad = plen - len(h) - len(b)
+    edge += h + b"".join(b"#" + b"p" * 998 + b"\n" for _ in range((pad - 2) // 1000)) + b"#" + b"p" * ((pad - 2) % 1000) + b"\n" + b
+assert K.plan_shards(edge, 3) == [(0, plen), (plen, 2 * plen), (2 * plen, 3 * plen)]
+shift = (1 << 32) - 1000
+qe = np.concatenate([q, np.array([0x10010000, 0x1002ffff], np.uint32)])  # 770 keys: slices of 256, 256 and 258
+shards = []
+for r, (a, b) in enumerate(K.plan_shards(edge, 3)):
+    k2 = m.ctxs[r]
+    lo, hi = 256 * r, (770 if r == 2 else 256 * r + 256)
+    d = k2.dev_alloc(b - a); k2.upload(d, np.frombuffer(edge[a:b], np.uint8))
+    dq, dr = k2.dev_alloc((hi - lo) * 4), k2.dev_alloc(770 * 4)
+    k2.upload(dq, qe[lo:hi])
+    shards.append(dict(d_text=d, n=b - a, global_base=a + shift, d_keys=dq, nq=hi - lo, key_offset=lo, d_rows_all=dr))
+    bufs.append((k2, d, dq, dr))
+tabs = m.pciids_join(shards, 770)
+_, eoffs, erows = m.ctxs[1].table_export(tabs[1])
+got = m.ctxs[1].download(shards[1]["d_rows_all"], 770 * 4, np.int32)
+names = m.ctxs[2].names_blob(tabs[2], erows)[0]
+assert [t.rows for t in tabs] == [1 + 65536 + 32768] * 3 and int(eoffs.min()) >= shift and got[768] >= 0 and got[769] == -1
+assert len(names) == 8 + 65536 + (2 << 20)
+print("sharded slab edges rows", tabs[0].rows, "name bytes", len(names))
+for t in tabs:
+    t.free()
+for k2, d, dq, dr in bufs:
+    k2.dev_free(d); k2.dev_free(dq); k2.dev_free(dr)
 m.close()

@@ -131,15 +131,23 @@ def test_too_long_line(kx, oracle):
     check_text(kx, oracle, text, extra_keys=[0x10de0001, 0x10de0002])
 
 
+UNICODE_CRLF_TEXT = (b"10de  NV\r\n\t0001  Wi-Fi\xc2\xae 5 \xc2\xa0\r\n\t0002  d\xc4\xb1g \xc5\xbf\n\t0003   \n\t0004\n"
+                     b"\t0005  a\tb \x0b c \n\t0006  \xe2\x80\x83em\xe3\x80\x80\n\t0007  \xff\xfe ok\n")
+
+
 def test_unicode_and_crlf_names(kx, oracle):
-    text = (b"10de  NV\r\n\t0001  Wi-Fi\xc2\xae 5 \xc2\xa0\r\n\t0002  d\xc4\xb1g \xc5\xbf\n\t0003   \n\t0004\n"
-            b"\t0005  a\tb \x0b c \n\t0006  \xe2\x80\x83em\xe3\x80\x80\n\t0007  \xff\xfe ok\n")
-    check_text(kx, oracle, text, extra_keys=[0x10de0000 + i for i in range(1, 9)])
+    check_text(kx, oracle, UNICODE_CRLF_TEXT, extra_keys=[0x10de0000 + i for i in range(1, 9)])
 
 
 def test_random_pciids_shaped_texts(kx, oracle):
     """Seeded random texts with the pci.ids grammar plus noise (blank lines, class section,
     duplicate vendors, upper-case hex, short lines)."""
+    for text, keys in random_pciids_texts():
+        check_text(kx, oracle, text, extra_keys=keys)
+
+
+def random_pciids_texts():
+    """(text, keys) of test_random_pciids_shaped_texts: twelve seeded texts and 40 keys each."""
     rng = np.random.default_rng(2024)
     for trial in range(12):
         lines = []
@@ -168,7 +176,7 @@ def test_random_pciids_shaped_texts(kx, oracle):
         if trial % 3 == 0:
             text = text.rstrip(b"\n")
         keys = [(int(rng.integers(0, 40)) * 0x0101 << 16) | int(rng.integers(0, 60)) for _ in range(40)]
-        check_text(kx, oracle, text, extra_keys=keys)
+        yield text, keys
 
 
 def test_x1000_first_occurrence_wins(kx, oracle, pci_text, oracle_rows, workloads):
@@ -295,6 +303,12 @@ def test_block_boundaries_at_range_edges(kx, oracle):
 def test_structural_byte_fuzz(kx, oracle):
     """Random byte soup weighted towards the bytes the parser branches on (newline, tab, '#', hex
     digits, CR, VT, NUL, high bytes): every window / chunk / range code path sees odd neighbours."""
+    for body, keys in structural_fuzz_texts():
+        check_text(kx, oracle, body, extra_keys=keys)
+
+
+def structural_fuzz_texts():
+    """(text, keys) of test_structural_byte_fuzz: sixty seeded byte soups and 16 keys each."""
     rng = np.random.default_rng(99)
     alphabet = np.frombuffer(b"\n\n\n\n\t\t\t##0123456789abcdefABCDEF  \r\x0b\x00\xff\x80xyz", dtype=np.uint8)
     for trial in range(60):
@@ -305,7 +319,7 @@ def test_structural_byte_fuzz(kx, oracle):
             pieces = [body[i:i + 257] for i in range(0, len(body), 257)]
             body = b"".join(p + b"\n%04x  V\n\t%04x  D\n" % (int(rng.integers(0, 6)), int(rng.integers(0, 6))) for p in pieces)
         keys = [(int(rng.integers(0, 6)) << 16) | int(rng.integers(0, 6)) for _ in range(16)]
-        check_text(kx, oracle, body, extra_keys=keys)
+        yield body, keys
 
 
 def test_join_device_equals_load_then_lookup(kx, pci_text, oracle_rows, workloads):
@@ -375,19 +389,7 @@ def test_name_lengths_around_the_finalize_windows(scan_w, kx, oracle, monkeypatc
 
 
 def _check_name_lengths(kx, oracle):
-    rng = np.random.default_rng(3)
-    alphabet = np.frombuffer(b"abcXYZ019 /._-[]()\t", np.uint8)
-    parts, keys = [b"1234  Vendor\n"], []
-    d = 0
-    for ln in list(range(0, 20)) + list(range(100, 135)) + list(range(980, 1040)) + [2000, 5000]:
-        for pad in (0, 3, 7, 13):
-            name = alphabet[rng.integers(0, len(alphabet), ln)].tobytes()
-            tail = [b"", b"\r", b"  ", b" \xc2\xa0"][(ln + pad) % 4]
-            parts.append(b"#" + b"x" * pad + b"\n")  # shifts the 16-byte phase of the next line
-            parts.append(b"\t%04x  " % d + name + tail + b"\n")
-            keys.append(0x12340000 | d)
-            d += 1
-    text = b"".join(parts)
+    text, keys = name_length_text()
     tab = kx.pciids_load(text)
     try:
         r = kx.lookup(tab, np.array(keys, np.uint32))
@@ -397,6 +399,25 @@ def _check_name_lengths(kx, oracle):
             assert nm == (oracle.device_name(text, k)[1] or b""), hex(k)
     finally:
         tab.free()
+
+
+def name_length_text(vendor=0x1234):
+    """One vendor block of names of every length around the finalize's 128-byte window and ~1 KB staging
+    area and beyond, at four 16-byte phases of the line start, with trailing CR / blanks / non-ASCII bytes.
+    Returns (text, keys of its device lines)."""
+    rng = np.random.default_rng(3)
+    alphabet = np.frombuffer(b"abcXYZ019 /._-[]()\t", np.uint8)
+    parts, keys = [b"%04x  Vendor\n" % vendor], []
+    d = 0
+    for ln in list(range(0, 20)) + list(range(100, 135)) + list(range(980, 1040)) + [2000, 5000]:
+        for pad in (0, 3, 7, 13):
+            name = alphabet[rng.integers(0, len(alphabet), ln)].tobytes()
+            tail = [b"", b"\r", b"  ", b" \xc2\xa0"][(ln + pad) % 4]
+            parts.append(b"#" + b"x" * pad + b"\n")  # shifts the 16-byte phase of the next line
+            parts.append(b"\t%04x  " % d + name + tail + b"\n")
+            keys.append(vendor << 16 | d)
+            d += 1
+    return b"".join(parts), keys
 
 
 def test_host_join_one_round_trip(kx, oracle, pci_text, oracle_rows, workloads):
