@@ -69,7 +69,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
  * lookup, ...).  Index with KXPU_T_*.  Measured with CUDA events on the ctx stream. */
 #define KXPU_T_PARSE    0
 #define KXPU_T_FINALIZE 1
-#define KXPU_T_LOOKUP   2
+#define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
 #define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's and kxpu_pcie_tree's kernels: the slot holds the most recent call's */
 #define KXPU_T_EMIT     5

@@ -234,7 +234,7 @@ static inline size_t range_words_bytes(uint32_t num_chunks) { return ((size_t)nu
 
 struct ArenaLayout {
     size_t o_slots, o_vfirst, o_trunc, ff_bytes, o_counters, o_range, o_row_key, o_row_line, o_row_anchor, o_row_noff, o_row_nlen,
-        o_sel, o_blob, total;
+        o_blob, total;
 };
 static ArenaLayout arena_layout(uint32_t cap, uint32_t blob_cap, size_t range_bytes) {
     ArenaLayout L;
@@ -251,7 +251,6 @@ static ArenaLayout arena_layout(uint32_t cap, uint32_t blob_cap, size_t range_by
     L.o_row_anchor = off;  off = align_up(off + slots * 8, 256);
     L.o_row_noff = off;    off = align_up(off + slots * 4, 256);
     L.o_row_nlen = off;    off = align_up(off + slots * 4, 256);
-    L.o_sel = off;         off = align_up(off + slots * 4, 256);
     L.o_blob = off;        off = align_up(off + (size_t)blob_cap + 16, 256);
     L.total = off;
     return L;
@@ -323,7 +322,6 @@ int32_t kx_table_acquire(kxpu_ctx *ctx, uint32_t cap, uint32_t blob_cap, uint32_
     t->row_anchor = (unsigned long long *)(b + L.o_row_anchor);
     t->row_name_off = (uint32_t *)(b + L.o_row_noff);
     t->row_name_len = (uint32_t *)(b + L.o_row_nlen);
-    t->sel = (uint32_t *)(b + L.o_sel);
     t->blob = b + L.o_blob;
     t->blob_cap = blob_cap;
     t->rows_cap = cap + 1;
@@ -462,13 +460,40 @@ int32_t kx_launch_finalize(kxpu_ctx *ctx, kxpu_table *t, const uint8_t *d_text, 
     return KXPU_OK;
 }
 
+// CTAs of a join over n keys: one key per thread, at most 32 CTAs per SM (the rest by grid stride)
+static unsigned join_ctas(kxpu_ctx *ctx, size_t n) { return (unsigned)std::min<size_t>((n + 255) / 256, (size_t)ctx->sm_count * 32); }
+
 int32_t kx_launch_lookup(kxpu_ctx *ctx, kxpu_table *t, const uint32_t *d_keys, size_t n, int32_t *d_rows) {
     if (n == 0) return KXPU_OK;
     KxTimer tm(ctx, KXPU_T_LOOKUP);
-    size_t blocks = (n + 255) / 256;
-    size_t maxb = (size_t)ctx->sm_count * 32;
-    if (blocks > maxb) blocks = maxb;
-    kxparse::lookup_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(d_keys, n, t->dev.slots, t->cap, t->shift, d_rows);
+    kxparse::lookup_kernel<<<join_ctas(ctx, n), 256, 0, ctx->stream>>>(d_keys, n, t->dev.slots, t->cap, t->shift, d_rows);
+    KX_LAUNCHED(ctx);
+    KX_CUDA(ctx, cudaGetLastError());
+    return KXPU_OK;
+}
+
+// Single-text load behind the parse: validity + row handles (one lane per slot), then the names of the rows and the
+// join of d_keys[0..nq) side by side in one launch (nq = 0: names only).  Both go under KXPU_T_FINALIZE.
+static int32_t kx_launch_rows_names_join(kxpu_ctx *ctx, kxpu_table *t, const uint8_t *d_text, size_t n, const uint32_t *d_keys,
+                                         size_t nq, int32_t *d_rows) {
+    using namespace kxparse;
+    FinalizeParams F;
+    memset(&F, 0, sizeof F);
+    F.text = d_text; F.n = n; F.base = 0; F.tab = t->dev;
+    F.mv.a = t->dev.vendor_first; F.mv.stride = 0; F.mv.n = 1; F.mv.trunc1 = t->dev.trunc;
+    F.row_key = t->row_key; F.row_line = t->row_line; F.row_anchor = t->row_anchor;
+    F.row_name_off = t->row_name_off; F.row_name_len = t->row_name_len;
+    F.blob = t->blob; F.blob_cap = t->blob_cap;
+    KxTimer tm(ctx, KXPU_T_FINALIZE);
+    select_rows_kernel<<<(t->cap + SF_WARPS * 32) / (SF_WARPS * 32), SF_WARPS * 32, 0, ctx->stream>>>(F);
+    KX_LAUNCHED(ctx);
+    // The row count is only known on the device, but a table with more than cap / 2 keys is grown, so there are at
+    // most cap / 2 rows: enough name CTAs for one step each (a step costs ~8 us, the join of 2^20 keys ~15 us on an
+    // H100; CTAs without rows leave at once), at most one resident wave of them for big tables.
+    const uint32_t want = (t->cap / 2 + SF_CTA_ROWS - 1) / SF_CTA_ROWS;
+    const unsigned name_ctas = std::max<unsigned>(1u, std::min<unsigned>(want, 8u * ctx->sm_count));
+    const unsigned grid = name_ctas + (nq ? join_ctas(ctx, nq) : 0u);
+    names_join_kernel<<<grid, SF_WARPS * 32, 0, ctx->stream>>>(F, name_ctas, d_keys, nq, d_rows);
     KX_LAUNCHED(ctx);
     KX_CUDA(ctx, cudaGetLastError());
     return KXPU_OK;
@@ -621,10 +646,11 @@ static int32_t kx_build_table_join(kxpu_ctx *ctx, const uint8_t *d_text, size_t 
             // a text with a >= 2 KiB stretch without a newline was seen on an earlier attempt: the exact
             // bufio.ErrTooLong cut-off is computed before the finalize
             if (rc == KXPU_OK && have_trunc) rc = kx_launch_trunc(ctx, t, d_text, n, 0);
-            if (rc == KXPU_OK) rc = kx_launch_finalize(ctx, t, d_text, n, 0, nullptr, nullptr, nullptr);
-            // the join does not need anything from the host: enqueue it before the round trip below
-            // (it is simply run again if the table has to be rebuilt)
-            if (rc == KXPU_OK && join) rc = kx_launch_lookup(ctx, t, join->d_keys, join->n, join->d_rows);
+            // the join does not need anything from the host: it runs beside the names, before the round trip below
+            // (and is simply run again if the table has to be rebuilt)
+            if (rc == KXPU_OK)
+                rc = join ? kx_launch_rows_names_join(ctx, t, d_text, n, join->d_keys, join->n, join->d_rows)
+                          : kx_launch_rows_names_join(ctx, t, d_text, n, nullptr, 0, nullptr);
         }
         if (rc != KXPU_OK) { kx_table_release(ctx, t); return rc; }
         const bool zero_copy = small_path && join && join->src_text;  // the kernel wrote rows and counters to host memory itself

@@ -15,7 +15,6 @@ struct kxpu_table {
     unsigned long long *row_anchor = nullptr;
     uint32_t *row_name_off = nullptr;
     uint32_t *row_name_len = nullptr;
-    uint32_t *sel = nullptr;
     uint8_t *blob = nullptr;
     uint32_t blob_cap = 0;
     uint32_t rows_cap = 0;  // entries of the row arrays
