@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 8
+#define KXPU_ABI_VERSION 9
 
 /* status codes */
 #define KXPU_OK             0
@@ -686,6 +686,84 @@ int32_t kxpu_lw_encode(kxpu_ctx *ctx, const uint32_t *group_ids, const uint8_t *
  * Limit (else KXPU_E_UNSUPPORTED): n below 2^32 / 283 (the longest Device is 283 bytes). */
 int32_t kxpu_lw_encode_topo(kxpu_ctx *ctx, const uint32_t *group_ids, const uint8_t *healthy, const uint64_t *numa_mask,
                             size_t n, uint8_t *out, size_t cap, size_t *len);
+
+/* ------------------------------------------- DRA ResourceSlices (ABI v9) */
+
+/* Kubernetes Dynamic Resource Allocation publishes devices as ResourceSlice objects (resource.k8s.io/v1).  Facts about
+ * that API are stated from memory of the upstream Go types, not checked against k8s.io/api; each is marked [assumed]:
+ *   [assumed] resource.k8s.io/v1 is GA since Kubernetes 1.34;
+ *   [assumed] the v1 ResourceSlice field order is kind, apiVersion, metadata, spec; ResourceSliceSpec is driver, pool,
+ *             nodeName, ..., devices; ResourcePool is name, generation, resourceSliceCount; Device is name, attributes;
+ *             DeviceAttribute holds exactly one of int, bool, string, version;
+ *   [assumed] a slice lists at most 128 devices; a device has at most 32 attributes; an attribute name is a C
+ *             identifier of at most 32 bytes, optionally qualified by a DNS subdomain; a string value is at most 64
+ *             bytes; a device name is a DNS label;
+ *   [assumed] the driver name is a lowercase DNS subdomain of at most 63 bytes; pool and node names are lowercase DNS
+ *             subdomains of at most 253 bytes;
+ *   [assumed] resource.kubernetes.io/pcieRoot is the standard attribute that aligns devices of different drivers
+ *             under one PCIe root complex;
+ *   [assumed] v1 has no per-device health: a published device is schedulable. */
+
+/* One published device (one IOMMU group of one class).  128 bytes: the kernel reads it with eight 16-byte loads. */
+typedef struct kxpu_dradev {
+    uint8_t  product[64];   /* productName bytes, NUL padded                                                 */
+    char     bdf[16];       /* PCI address of the group's first accepted member                              */
+    char     pcie_root[16]; /* "pci<domain>:<bus>", the first component of that member's path; "" = unknown */
+    char     vendor[8];     /* read_id(vendor) of that member, NUL padded                                    */
+    char     device[8];     /* read_id(device)                                                               */
+    uint64_t numa_mask;     /* the group's NUMA mask (kxpu_classify_topo)                                    */
+    uint32_t iommu_group;
+    uint8_t  product_len;   /* 0..64                                                                         */
+    uint8_t  reserved[3];
+} kxpu_dradev;
+#define KXPU_DRA_SLICE_DEVICES 128       /* devices per slice: the v1 limit [assumed]                          */
+#define KXPU_DRA_MAX_DEVICES   (1u << 24) /* n must be below this                                               */
+
+/* The ResourceSlices of one pool: S = max(1, ceil(n / 128)) slices, slice s holding devs[128 s .. min(n, 128 s + 128))
+ * in array order.  out receives S compact JSON objects (no spaces), each followed by one '\n' (a JSON Lines file);
+ * object s is out[slice_off[s] .. slice_off[s+1] - 1) and its '\n' is the byte before slice_off[s+1].  With out == NULL
+ * or cap < *len the call stores *len and *n_slices and returns KXPU_E_NOSPACE, as kxpu_cdi_emit does.  slice_off (may be
+ * NULL) has S + 1 entries and is written only on KXPU_OK.
+ *
+ * Every object is
+ *   {"kind":"ResourceSlice","apiVersion":"resource.k8s.io/v1","metadata":{"generateName":"<node>-<driver>-"},
+ *    "spec":{"driver":"<driver>","pool":{"name":"<pool>","generation":<generation>,"resourceSliceCount":<S>},
+ *    "nodeName":"<node>","devices":[<device>,<device>,...]}}
+ * (one line; fields in the declaration order of the Go v1 types [assumed]).  A device is
+ *   {"name":"vfio<g>","attributes":{<attributes>}}
+ * with g = iommu_group in decimal: a DNS label that mirrors the cdi.k8s.io/vfio<g> annotation of the CDI spec.  The
+ * attributes, keys sorted bytewise as encoding/json sorts map keys:
+ *   "deviceID":{"string":"<device>"}                                  always
+ *   "iommuGroup":{"int":<g>}                                          always
+ *   "numaNode":{"int":<k>}                                            only when numa_mask has exactly one bit k set
+ *   "pciAddress":{"string":"<bdf>"}                                   always; a driver-local name on purpose
+ *   "productName":{"string":"<product[0..product_len)>"}              only when product_len > 0
+ *   "resource.kubernetes.io/pcieRoot":{"string":"<pcie_root>"}        only when pcie_root is not empty
+ *   "vendorID":{"string":"<vendor>"}                                  always
+ * n = 0 gives one slice with "devices":[]: a pool without devices still tells the scheduler the node has none.
+ * These bytes are this project's canonical form (the checker pins them); they are not claimed to equal Go's, which
+ * would also write "creationTimestamp":null.
+ *
+ * KXPU_E_INVALID, nothing written (not even *len): ctx, len or n_slices NULL, devs NULL with n > 0; driver not a
+ * lowercase DNS subdomain (labels of [a-z0-9-] that start and end with [a-z0-9], joined by '.', each at most 63 bytes)
+ * of at most 63 bytes; pool or node not such a subdomain of at most 253 bytes; generation >= 2^63.  These checks mean
+ * that no string needs JSON escaping.
+ * KXPU_E_UNSUPPORTED, with *len, the output and slice_off untouched: n >= KXPU_DRA_MAX_DEVICES, or a record outside
+ * the domain:
+ *   - product[0..product_len) over [A-Za-z0-9_.-] (the resource-name sanitiser's output and a raw hex id both fit);
+ *     bytes past product_len are ignored; product_len <= 64;
+ *   - bdf: the bytes before its first NUL (all 16 when there is none), 1..16 of them, over [0-9a-f:.];
+ *   - pcie_root: empty (first byte NUL), or "pci" followed by 1..13 bytes over [0-9a-f:] before its first NUL;
+ *   - vendor, device: 1..6 bytes over [0-9a-f] before the first NUL;
+ *   - iommu_group below 4294967295.
+ * GPU: one CTA per slice.  One thread per device computes its fragment length, a block scan places the devices in
+ * the slice, the slice's offset is the exclusive prefix of a decoupled look-back over the slice totals (which is
+ * slice_off[s]), and the slice is staged in shared memory at its destination's 16-byte phase and written with one
+ * bulk store.  The header and tail, the same for every slice, are built on the host once per call.  Timed under
+ * KXPU_T_EMIT. */
+int32_t kxpu_dra_slices(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                        const kxpu_dradev *devs, size_t n, uint8_t *out, size_t cap, size_t *len,
+                        uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
 
 #ifdef __cplusplus
 }

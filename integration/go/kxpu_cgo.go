@@ -593,3 +593,33 @@ func (k *kxpu) reconcile(prev []C.kxpu_snaprec, nextIndex uint64, cur []C.kxpu_s
 	}
 	return snap, curState[:len(cur)], prevState[:len(prev)], counts, nil
 }
+
+// DRA ResourceSlices (ABI v9).  One pool per class with a DRA driver, named after the node (NODE_NAME): devs holds one
+// kxpu_dradev per published IOMMU group in walk order (groups with a viability blocker left out).  Returns the slices
+// as JSON Lines, one object per line; the caller POSTs each line to /apis/resource.k8s.io/v1/resourceslices and then
+// deletes the slices of its driver and node with an older spec.pool.generation.
+func (k *kxpu) draSlices(driver, node string, generation uint64, devs []C.kxpu_dradev) ([]string, error) {
+	cd, cn := C.CString(driver), C.CString(node)
+	defer C.free(unsafe.Pointer(cd))
+	defer C.free(unsafe.Pointer(cn))
+	var p *C.kxpu_dradev
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	var n, ns C.size_t
+	rc := C.kxpu_dra_slices(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), nil, 0, &n, nil, &ns) // sizing call
+	if rc != C.KXPU_E_NOSPACE {
+		return nil, kxCheck(k.ctx, "kxpu_dra_slices", rc)
+	}
+	buf := make([]byte, n)
+	off := make([]uint64, ns+1)
+	if err := kxCheck(k.ctx, "kxpu_dra_slices", C.kxpu_dra_slices(k.ctx, cd, cn, cn, C.uint64_t(generation), p,
+		C.size_t(len(devs)), (*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n, (*C.uint64_t)(unsafe.Pointer(&off[0])), &ns)); err != nil {
+		return nil, err
+	}
+	lines := make([]string, ns)
+	for s := range lines {
+		lines[s] = string(buf[off[s] : off[s+1]-1]) // without the '\n'
+	}
+	return lines, nil
+}

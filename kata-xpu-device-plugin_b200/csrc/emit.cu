@@ -153,6 +153,29 @@ __device__ __forceinline__ bool bdf_charset_ok(const uint8_t *s, uint32_t len) {
     return true;
 }
 
+// The store epilogue of a staged tile: stg[0, total) sits in shared memory at g's 16-byte phase and goes to g with one
+// bulk store for the 16-byte aligned body and byte stores for the ragged ends.  Called by every thread of a CTA of at
+// least 80 threads, after the staging writes.
+__device__ __forceinline__ void tile_store(uint8_t *g, const uint8_t *stg, uint32_t total) {
+    const uint32_t tid = threadIdx.x;
+    // generic-proxy writes to shared memory must be visible to the async proxy (TMA) that reads them
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(g) & 15u);
+    const uint32_t lead = total < 16u ? total : ((16u - mis) & 15u);
+    const uint32_t body = (total - lead) & ~15u;
+    if (tid == 0 && body) {
+        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(g + lead),
+                     "r"((uint32_t)__cvta_generic_to_shared(stg + lead)), "r"(body)
+                     : "memory");
+        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    }
+    if (tid >= 32 && tid < 32 + lead) g[tid - 32] = stg[tid - 32];
+    const uint32_t rest = total - lead - body;
+    if (tid >= 64 && tid < 64 + rest) g[lead + body + tid - 64] = stg[lead + body + tid - 64];
+    if (tid == 0 && body) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // smem must outlive the read
+}
+
 struct EmitParams {
     const void *devs;         // kxpu_cdidev[n] or kxpu_mdevcdi[n]
     uint32_t n;
@@ -282,24 +305,173 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
             if (lane == 0) { if (more) { dst[o] = (uint8_t)','; dst[o + 1] = (uint8_t)'\n'; } else dst[o] = (uint8_t)'\n'; }
         }
     }
-    // generic-proxy writes to shared memory must be visible to the async proxy (TMA) that reads them
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    // ---- one bulk store for the 16-byte aligned body, byte stores for the ragged ends
-    const uint32_t total = head_len + tile_total + tail_len;
-    uint8_t *g = E.out + base;
-    const uint32_t lead = total < 16u ? total : ((16u - mis) & 15u);
-    const uint32_t body = (total - lead) & ~15u;
-    if (tid == 0 && body) {
-        asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(g + lead),
-                     "r"((uint32_t)__cvta_generic_to_shared(stg + lead)), "r"(body)
-                     : "memory");
-        asm volatile("cp.async.bulk.commit_group;" ::: "memory");
+    tile_store(E.out + base, stg, head_len + tile_total + tail_len);
+}
+
+// ------------------------------------------------------------------ K11: DRA ResourceSlices (kxpu_dra_slices)
+// One CTA per slice of TILE devices.  A device fragment is literal D0, the variable fields and literals D1..D8 (D3 / D5 /
+// D6 with their field only when present), then ',' unless it is the slice's last device.  Every literal but D0 opens with
+// the closing bytes of the value before it, so an absent optional attribute simply drops its literal and field.
+#define KX_D0 "{\"name\":\"vfio"
+#define KX_D1 "\",\"attributes\":{\"deviceID\":{\"string\":\""
+#define KX_D2 "\"},\"iommuGroup\":{\"int\":"
+#define KX_D3 "},\"numaNode\":{\"int\":"
+#define KX_D4 "},\"pciAddress\":{\"string\":\""
+#define KX_D5 "\"},\"productName\":{\"string\":\""
+#define KX_D6 "\"},\"resource.kubernetes.io/pcieRoot\":{\"string\":\""
+#define KX_D7 "\"},\"vendorID\":{\"string\":\""
+#define KX_D8 "\"}}}"
+#define KX_DRA_TAIL "]}}\n"
+static const char *const h_dra_lits[9] = {KX_D0, KX_D1, KX_D2, KX_D3, KX_D4, KX_D5, KX_D6, KX_D7, KX_D8};
+constexpr uint32_t DRA_LIT_TOTAL = sizeof(KX_D0 KX_D1 KX_D2 KX_D3 KX_D4 KX_D5 KX_D6 KX_D7 KX_D8) - 1;
+// the longest fragment: every literal, a 10-digit group twice, node 63, a 16-byte bdf and root, 64 product bytes, two
+// 6-byte ids, the separator
+constexpr int MAX_FRAG_DRA = (int)DRA_LIT_TOTAL + 2 * 10 + 2 + 16 + 16 + 64 + 6 + 6 + 1;
+// literals | slice head | slice tail: the head holds the node name twice, the driver twice and the pool once
+// (2 * 253 + 2 * 63 + 253 bytes of names, about 1.1 KB in all)
+constexpr int DRA_POOL_MAX = 1536;
+constexpr int DRA_HEAD = 9, DRA_TAIL = 10, DRA_PARTS = 11;
+
+struct DraParams {
+    const kxpu_dradev *devs;
+    uint32_t n;
+    uint16_t off[DRA_PARTS], len[DRA_PARTS];  // literal k / head / tail inside the pool
+    uint32_t pool_len;
+    uint8_t *out;
+    unsigned long long *slice_off;  // [gridDim.x + 1]
+    unsigned long long *state;      // slice status words (scan.cuh look-back)
+    uint32_t epoch;
+    uint32_t *flags;                // one word per KXPU_E_UNSUPPORTED reason, DRA_F_*
+    uint8_t pool[DRA_POOL_MAX];
+};
+constexpr int DRA_F_PRODUCT = 0, DRA_F_BDF = 1, DRA_F_ROOT = 2, DRA_F_VENDOR = 3, DRA_F_DEVICE = 4, DRA_F_GROUP = 5,
+              DRA_F_PLEN = 6, DRA_F_COUNT = 7;
+
+struct DraSmem {
+    alignas(16) uint8_t stage[TILE * MAX_FRAG_DRA + DRA_POOL_MAX + 16];
+    uint8_t pool[DRA_POOL_MAX];
+    uint8_t dec[TILE][12];  // group digits at 0, NUMA node digits at 10
+    uint32_t meta[TILE];    // gl | nl << 4 | bl << 8 | rl << 13 | vl << 18 | dl << 21 | pl << 24
+    uint32_t start[TILE];   // fragment offset inside the slice
+    unsigned long long base;
+    uint32_t wsum[EMIT_THREADS / 32];
+    uint32_t tile_total;
+};
+
+template <int W>
+__device__ __forceinline__ uint32_t byte_at(const uint32_t (&w)[W], int k) { return (w[k >> 2] >> (8 * (k & 3))) & 0xffu; }
+// bytes before the first NUL (all 4 W when there is none)
+template <int W>
+__device__ __forceinline__ uint32_t nul_len(const uint32_t (&w)[W]) {
+    uint32_t l = 4u * W;
+#pragma unroll
+    for (int k = 4 * W - 1; k >= 0; k--) if (byte_at(w, k) == 0u) l = (uint32_t)k;
+    return l;
+}
+__device__ __forceinline__ bool is_lhex(uint32_t c) { return (c >= '0' && c <= '9') || (c >= 'a' && c <= 'f'); }
+// every byte k in [from, len) satisfies ok(c)
+template <int W, typename F>
+__device__ __forceinline__ bool bytes_ok(const uint32_t (&w)[W], uint32_t from, uint32_t len, F ok) {
+    bool good = true;
+#pragma unroll
+    for (int k = 0; k < 4 * W; k++) if ((uint32_t)k >= from && (uint32_t)k < len && !ok(byte_at(w, k))) good = false;
+    return good;
+}
+
+__global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_constant__ DraParams E) {
+    extern __shared__ __align__(16) uint8_t smem_raw[];
+    DraSmem &S = *reinterpret_cast<DraSmem *>(smem_raw);
+    const uint32_t tid = threadIdx.x, lane = tid & 31u, w = tid >> 5;
+    const uint32_t slice = blockIdx.x, i0 = slice * TILE;
+    const uint32_t in_slice = E.n > i0 ? min(E.n - i0, (uint32_t)TILE) : 0u;
+    for (uint32_t k = tid; k < E.pool_len; k += EMIT_THREADS) S.pool[k] = E.pool[k];
+
+    // ---- fragment lengths, digits and the domain checks: one thread per device
+    uint32_t flen = 0;
+    if (tid < in_slice) {
+        const uint4 *p = reinterpret_cast<const uint4 *>(E.devs + i0 + tid);
+        const uint4 q0 = p[0], q1 = p[1], q2 = p[2], q3 = p[3], q4 = p[4], q5 = p[5], q6 = p[6], q7 = p[7];
+        const uint32_t prod[16] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
+        const uint32_t bdf[4] = {q4.x, q4.y, q4.z, q4.w}, root[4] = {q5.x, q5.y, q5.z, q5.w};
+        const uint32_t ven[2] = {q6.x, q6.y}, dev[2] = {q6.z, q6.w};
+        const unsigned long long mask = ((unsigned long long)q7.y << 32) | q7.x;
+        const uint32_t group = q7.z, plen_raw = q7.w & 0xffu;
+        const uint32_t pl = plen_raw <= 64u ? plen_raw : 64u;  // out of the domain: reported below, bounded here
+        const uint32_t bl = nul_len(bdf), rl = nul_len(root), vl_raw = nul_len(ven), dl_raw = nul_len(dev);
+        const uint32_t vl = min(vl_raw, 6u), dl = min(dl_raw, 6u);  // bounded like pl
+        const auto hex = [](uint32_t c) { return is_lhex(c); };
+        if (plen_raw > 64u) E.flags[DRA_F_PLEN] = 1u;
+        if (!bytes_ok(prod, 0u, pl, [](uint32_t c) {
+                return (c >= '0' && c <= '9') || (c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z') || c == '_' || c == '.' || c == '-';
+            }))
+            E.flags[DRA_F_PRODUCT] = 1u;
+        if (bl == 0u || !bytes_ok(bdf, 0u, bl, [](uint32_t c) { return is_lhex(c) || c == ':' || c == '.'; })) E.flags[DRA_F_BDF] = 1u;
+        if (rl != 0u && (rl < 4u || byte_at(root, 0) != 'p' || byte_at(root, 1) != 'c' || byte_at(root, 2) != 'i' ||
+                         !bytes_ok(root, 3u, rl, [](uint32_t c) { return is_lhex(c) || c == ':'; })))
+            E.flags[DRA_F_ROOT] = 1u;
+        if (vl_raw == 0u || vl_raw > 6u || !bytes_ok(ven, 0u, vl, hex)) E.flags[DRA_F_VENDOR] = 1u;
+        if (dl_raw == 0u || dl_raw > 6u || !bytes_ok(dev, 0u, dl, hex)) E.flags[DRA_F_DEVICE] = 1u;
+        if (group == 0xFFFFFFFFu) E.flags[DRA_F_GROUP] = 1u;
+        const bool one_node = mask != 0ull && (mask & (mask - 1ull)) == 0ull;
+        const uint32_t node = one_node ? (uint32_t)__ffsll((long long)mask) - 1u : 0u;
+        const uint32_t gl = dec_len(group), nl = one_node ? dec_len(node) : 0u;
+        dec_write(group, gl, S.dec[tid]);
+        if (one_node) dec_write(node, nl, S.dec[tid] + 10);
+        S.meta[tid] = gl | (nl << 4) | (bl << 8) | (rl << 13) | (vl << 18) | (dl << 21) | (pl << 24);
+        flen = DRA_LIT_TOTAL - E.len[3] - E.len[5] - E.len[6] + 2u * gl + bl + vl + dl + (nl ? E.len[3] + nl : 0u) +
+               (pl ? E.len[5] + pl : 0u) + (rl ? E.len[6] + rl : 0u) + (tid + 1u < in_slice ? 1u : 0u);
     }
-    if (tid >= 32 && tid < 32 + lead) g[tid - 32] = stg[tid - 32];
-    const uint32_t rest = total - lead - body;
-    if (tid >= 64 && tid < 64 + rest) g[lead + body + tid - 64] = stg[lead + body + tid - 64];
-    if (tid == 0 && body) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");  // smem must outlive the read
+    // ---- scan of the 128 lengths (threads >= TILE contribute 0)
+    const uint32_t incl = kxscan::warp_incl(flen);
+    if (lane == 31) S.wsum[w] = incl;
+    __syncthreads();
+    if (w == 0) {
+        const uint32_t x = lane < EMIT_THREADS / 32 ? S.wsum[lane] : 0u;
+        const uint32_t xi = kxscan::warp_incl(x);
+        if (lane < EMIT_THREADS / 32) S.wsum[lane] = xi - x;
+        if (lane == EMIT_THREADS / 32 - 1) S.tile_total = xi;
+    }
+    __syncthreads();
+    const uint32_t head_len = E.len[DRA_HEAD], tail_len = E.len[DRA_TAIL], tile_total = S.tile_total;
+    if (tid < TILE) S.start[tid] = head_len + S.wsum[w] + incl - flen;
+    // ---- the slice's offset in the output: decoupled look-back over the slice totals; its exclusive prefix is slice_off[s]
+    if (w == 0) {
+        const unsigned long long agg = (unsigned long long)head_len + tile_total + tail_len;
+        const unsigned long long excl = kxscan::lookback(E.state, slice, agg, E.epoch);
+        if (lane == 0) {
+            S.base = excl;
+            E.slice_off[slice] = excl;
+            if (slice == gridDim.x - 1) E.slice_off[slice + 1] = excl + agg;
+        }
+    }
+    __syncthreads();
+    const unsigned long long base = S.base;
+    uint8_t *stg = S.stage + ((reinterpret_cast<uintptr_t>(E.out) + base) & 15u);  // same 16-byte phase in smem and global
+    for (uint32_t k = tid; k < head_len; k += EMIT_THREADS) stg[k] = S.pool[E.off[DRA_HEAD] + k];
+    for (uint32_t k = tid; k < tail_len; k += EMIT_THREADS) stg[head_len + tile_total + k] = S.pool[E.off[DRA_TAIL] + k];
+    // ---- fragments: one warp per device; the string fields straight from the record (L1 / L2)
+    for (uint32_t d = w; d < in_slice; d += EMIT_THREADS / 32) {
+        const uint32_t m = S.meta[d];
+        const uint32_t gl = m & 15u, nl = (m >> 4) & 3u, bl = (m >> 8) & 31u, rl = (m >> 13) & 31u, vl = (m >> 18) & 7u,
+                       dl = (m >> 21) & 7u, pl = m >> 24;
+        const kxpu_dradev *r = E.devs + i0 + d;
+        uint8_t *dst = stg + S.start[d];
+        uint32_t o = 0;
+        auto put = [&](const uint8_t *src, uint32_t L) {
+            for (uint32_t l = lane; l < L; l += 32u) dst[o + l] = src[l];
+            o += L;
+        };
+        auto lit = [&](int k) { put(S.pool + E.off[k], E.len[k]); };
+        lit(0); put(S.dec[d], gl); lit(1); put(reinterpret_cast<const uint8_t *>(r->device), dl);
+        lit(2); put(S.dec[d], gl);
+        if (nl) { lit(3); put(S.dec[d] + 10, nl); }
+        lit(4); put(reinterpret_cast<const uint8_t *>(r->bdf), bl);
+        if (pl) { lit(5); put(r->product, pl); }
+        if (rl) { lit(6); put(reinterpret_cast<const uint8_t *>(r->pcie_root), rl); }
+        lit(7); put(reinterpret_cast<const uint8_t *>(r->vendor), vl); lit(8);
+        if (d + 1u < in_slice && lane == 0) dst[o] = (uint8_t)',';
+    }
+    tile_store(E.out + base, stg, head_len + tile_total + tail_len);
 }
 
 // ------------------------------------------------------------------ Allocate names
@@ -685,4 +857,112 @@ extern "C" int32_t kxpu_lw_encode_topo(kxpu_ctx *ctx, const uint32_t *group_ids,
                                                              offs, o);
         },
         numa_mask, n * 8, &d_masks);
+}
+
+// ------------------------------------------------------------------ K11: DRA ResourceSlices
+// a lowercase RFC 1123 DNS subdomain of at most `max` bytes: labels of [a-z0-9-], 1..63 bytes, starting and ending with
+// [a-z0-9], joined by '.'
+static bool dns_subdomain_ok(const char *s, size_t max) {
+    if (!s) return false;
+    const size_t len = strnlen(s, max + 1);
+    if (len == 0 || len > max) return false;
+    size_t label = 0;
+    for (size_t i = 0; i <= len; i++) {
+        const char c = i < len ? s[i] : '.';
+        const bool alnum = (c >= 'a' && c <= 'z') || (c >= '0' && c <= '9');
+        if (c == '.') {
+            if (label == 0 || label > 63 || s[i - 1] == '-') return false;
+            label = 0;
+        } else if (alnum || (c == '-' && label > 0)) {
+            label++;
+        } else {
+            return false;
+        }
+    }
+    return true;
+}
+
+extern "C" int32_t kxpu_dra_slices(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                                   const kxpu_dradev *devs, size_t n, uint8_t *out, size_t cap, size_t *len,
+                                   uint64_t *slice_off, size_t *n_slices) {
+    static_assert(sizeof(kxpu_dradev) == 128 && offsetof(kxpu_dradev, numa_mask) == 112 &&
+                      offsetof(kxpu_dradev, product_len) == 124, "kxpu_dradev layout");
+    if (!ctx || !len || !n_slices || (n && !devs)) return KXPU_E_INVALID;
+    if (!dns_subdomain_ok(driver, 63) || !dns_subdomain_ok(pool, 253) || !dns_subdomain_ok(node, 253) ||
+        generation >= (1ull << 63)) {
+        KX_SET_ERR(ctx, "dra_slices: driver (<= 63 bytes), pool and node (<= 253 bytes) must be lowercase DNS subdomains "
+                        "and generation below 2^63");
+        return KXPU_E_INVALID;
+    }
+    if (n >= KXPU_DRA_MAX_DEVICES) {
+        KX_SET_ERR(ctx, "dra_slices: n = %zu is not below %u", n, KXPU_DRA_MAX_DEVICES);
+        return KXPU_E_UNSUPPORTED;
+    }
+    std::lock_guard<std::mutex> guard(ctx->mu);
+    cudaSetDevice(ctx->device);
+    kx_clear_timings(ctx);
+    const uint32_t N = (uint32_t)n, slices = N ? (N + TILE - 1) / TILE : 1u;
+    const std::string d = driver, p = pool, nd = node;
+    const std::string head = "{\"kind\":\"ResourceSlice\",\"apiVersion\":\"resource.k8s.io/v1\",\"metadata\":{\"generateName\":\"" +
+                             nd + "-" + d + "-\"},\"spec\":{\"driver\":\"" + d + "\",\"pool\":{\"name\":\"" + p +
+                             "\",\"generation\":" + std::to_string(generation) +
+                             ",\"resourceSliceCount\":" + std::to_string(slices) + "},\"nodeName\":\"" + nd +
+                             "\",\"devices\":[";
+    DraParams E;
+    memset(&E, 0, sizeof E);
+    uint32_t acc = 0;
+    for (int k = 0; k < DRA_PARTS; k++) {
+        const std::string s = k < 9 ? std::string(h_dra_lits[k]) : k == DRA_HEAD ? head : std::string(KX_DRA_TAIL);
+        if (acc + s.size() > (size_t)DRA_POOL_MAX) return KXPU_E_INVALID;  // the literals grew: DRA_POOL_MAX must follow
+        memcpy(E.pool + acc, s.data(), s.size());
+        E.off[k] = (uint16_t)acc;
+        E.len[k] = (uint16_t)s.size();
+        acc += E.len[k];
+    }
+    E.pool_len = acc;
+    const size_t bound = (size_t)slices * (E.len[DRA_HEAD] + E.len[DRA_TAIL]) + (size_t)n * MAX_FRAG_DRA + 64;
+    static bool attr_done = false;
+    if (!attr_done) {
+        cudaFuncSetAttribute(k_dra_slices, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DraSmem));
+        attr_done = true;
+    }
+    KxScratch sc(ctx);
+    kxpu_dradev *d_devs = nullptr;
+    uint8_t *d_out = nullptr;
+    unsigned long long *d_ctl = nullptr;  // slice_off [slices + 1] | DRA_F_COUNT flag words
+    const size_t ctl_words = slices + 1 + (DRA_F_COUNT + 1) / 2;
+    KX_CUDA(ctx, sc.alloc((void **)&d_devs, n * sizeof(kxpu_dradev)));
+    KX_CUDA(ctx, sc.alloc((void **)&d_out, bound));
+    KX_CUDA(ctx, sc.alloc((void **)&d_ctl, ctl_words * 8));
+    if (n) cudaMemcpyAsync(d_devs, devs, n * sizeof(kxpu_dradev), cudaMemcpyHostToDevice, ctx->stream);
+    cudaMemsetAsync(d_ctl + slices + 1, 0, (ctl_words - slices - 1) * 8, ctx->stream);
+    E.devs = d_devs; E.n = N; E.out = d_out; E.slice_off = d_ctl; E.flags = (uint32_t *)(d_ctl + slices + 1);
+    E.state = kx_scan_state(ctx, slices);
+    if (!E.state) return KXPU_E_NOMEM;
+    E.epoch = kx_next_epoch(ctx);
+    {
+        KxTimer tm(ctx, KXPU_T_EMIT);
+        k_dra_slices<<<slices, EMIT_THREADS, sizeof(DraSmem), ctx->stream>>>(E);
+        KX_LAUNCHED(ctx);
+    }
+    std::vector<unsigned long long> h(ctl_words);
+    cudaMemcpyAsync(h.data(), d_ctl, ctl_words * 8, cudaMemcpyDeviceToHost, ctx->stream);
+    cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "dra_slices failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    static const char *const why[DRA_F_COUNT] = {
+        "a product byte outside [A-Za-z0-9_.-]", "a bdf that is empty or holds a byte outside [0-9a-f:.]",
+        "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
+        "a device id that is not 1..6 bytes of [0-9a-f]", "iommu_group 4294967295", "product_len above 64"};
+    const uint32_t *flags = reinterpret_cast<const uint32_t *>(h.data() + slices + 1);
+    for (int f = 0; f < DRA_F_COUNT; f++)
+        if (flags[f]) { KX_SET_ERR(ctx, "dra_slices: %s", why[f]); return KXPU_E_UNSUPPORTED; }
+    const size_t total = (size_t)h[slices];
+    *len = total;
+    *n_slices = slices;
+    if (cap < total || !out) return KXPU_E_NOSPACE;
+    cudaMemcpyAsync(out, d_out, total, cudaMemcpyDeviceToHost, ctx->stream);
+    e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "dra_slices D2H failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    if (slice_off) memcpy(slice_off, h.data(), (slices + 1) * sizeof(uint64_t));
+    return KXPU_OK;
 }

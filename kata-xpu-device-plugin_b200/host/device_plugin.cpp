@@ -376,10 +376,10 @@ static Error walkDir(Plugin &p, const std::string &path, const std::string &name
     Error e = leafRecord(name, p.xpuClasses,
                          [&](const char *prop, std::string &out) { return p.readIDFromFile(p.basePath, name, prop, out); },
                          [&](const char *link, std::string &out) { return p.readLink(p.basePath, name, link, out); },
-                         p.topologyAware ? &readNuma : nullptr, allowedDrivers(p, allowed), r);
+                         p.readsNuma() ? &readNuma : nullptr, allowedDrivers(p, allowed), r);
     if (e) return e;
     recs.push_back(r);
-    if (paths) {  // pcieTopologyAware: the entry's link, one readlink
+    if (paths) {  // readsPaths(): the entry's link, one readlink
         kxpu_pcipath pp;
         std::string target;
         if (p.readPciPath(p.basePath, name, target)) pciPathRecord(target, pp);
@@ -394,7 +394,7 @@ Error Plugin::gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pci
     if (paths) paths->clear();
     size_t slash = basePath.find_last_of('/');
     return walkDir(*this, basePath, slash == std::string::npos ? basePath : basePath.substr(slash + 1), recs,
-                   pcieTopologyAware ? paths : nullptr);
+                   readsPaths() ? paths : nullptr);
 }
 
 // ---------------------------------------------------------------------------- SURVEY 8(f) row 2
@@ -407,7 +407,7 @@ Error Plugin::gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pci
 Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads, std::vector<kxpu_pcipath> *paths) {
     recs.clear();
     if (paths) paths->clear();
-    if (!pcieTopologyAware) paths = nullptr;
+    if (!readsPaths()) paths = nullptr;
     struct stat sb;
     if (lstat(basePath.c_str(), &sb) != 0) return fail("Error accessing file path \"" + basePath + "\": " + strerror(errno));
     // the fast reads bypass the seams: only when nobody replaced them (tests do, device_plugin.go:38-39)
@@ -417,7 +417,7 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
     NumaFn const *rn = readNumaNode.target<NumaFn>();
     NumaFn const *rp = readPciPath.target<NumaFn>();
     const bool defaultSeams = rl && *rl == readLinkFunc && ri && *ri == readIDFromFileFunc &&
-                              (!topologyAware || (rn && *rn == readNumaNodeFunc)) &&
+                              (!readsNuma() || (rn && *rn == readNumaNodeFunc)) &&
                               (!paths || (rp && *rp == readPciPathFunc));
     if (!S_ISDIR(sb.st_mode) || !defaultSeams) return gatherRecords(recs, paths);
     int basefd = open(basePath.c_str(), O_RDONLY | O_DIRECTORY | O_CLOEXEC);
@@ -494,7 +494,7 @@ Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads
             };
             errs[i] = leafRecord(name, xpuClasses, [&](const char *prop, std::string &out) { return readID(name, prop, out); },
                                  [&](const char *link, std::string &out) { return readLnk(name, link, out); },
-                                 topologyAware ? &readNuma : nullptr, allowed, flat[i]);
+                                 readsNuma() ? &readNuma : nullptr, allowed, flat[i]);
             if (paths && !errs[i]) {  // the entry's own link on the same directory descriptor
                 char buf[4096];
                 const ssize_t k = readlinkat(basefd, name.c_str(), buf, sizeof buf);
@@ -604,6 +604,30 @@ static std::string blockerOf(const kxpu_devrec &r) {
     return std::string(r.bdf, strnlen(r.bdf, sizeof r.bdf)) + " is bound to " + std::string(r.driver, strnlen(r.driver, sizeof r.driver));
 }
 
+// the ResourceSlice record of a group (product left empty): bdf, vendor and device of its first member r, the first
+// component of r's path when it is "pci" followed by 1..13 bytes of [0-9a-f:] (anything else leaves the root unknown), and
+// the group's NUMA mask
+static kxpu_dradev draRecord(const kxpu_devrec &r, const kxpu_pcipath *path, uint64_t numa) {
+    kxpu_dradev d;
+    memset(&d, 0, sizeof d);
+    memcpy(d.bdf, r.bdf, strnlen(r.bdf, sizeof r.bdf));
+    const std::string vendor = trimID(std::string((const char *)r.vendor_txt, std::min<size_t>(r.vendor_len, sizeof r.vendor_txt)));
+    const std::string device = trimID(std::string((const char *)r.device_txt, std::min<size_t>(r.device_len, sizeof r.device_txt)));
+    memcpy(d.vendor, vendor.data(), std::min(vendor.size(), sizeof d.vendor));
+    memcpy(d.device, device.data(), std::min(device.size(), sizeof d.device));
+    if (path && path->len > 0 && path->len <= sizeof path->path) {
+        const std::string p(path->path, path->len);
+        const std::string root = p.substr(0, p.find('/'));
+        bool ok = root.size() >= 4 && root.size() <= sizeof d.pcie_root && root.compare(0, 3, "pci") == 0;
+        for (size_t k = 3; ok && k < root.size(); k++)
+            ok = (root[k] >= '0' && root[k] <= '9') || (root[k] >= 'a' && root[k] <= 'f') || root[k] == ':';
+        if (ok) memcpy(d.pcie_root, root.data(), root.size());
+    }
+    d.numa_mask = numa;
+    d.iommu_group = r.iommu_group;
+    return d;
+}
+
 // the walk and classify of createIommuDeviceMap
 Error Plugin::classifyPci(PciWalk &w) {
     Error e = gatherRecordsFast(w.recs, 0, &w.paths);  // same records as gatherRecords (falls back to it when a seam was replaced)
@@ -619,12 +643,12 @@ Error Plugin::classifyPci(PciWalk &w) {
     if (groupViability) {
         c.gblk.assign(n ? n : 1, KXPU_VIABLE);
         rc = kxpu_classify_viable(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(),
-                                  topologyAware ? c.gnuma.data() : nullptr, c.gblk.data());
+                                  readsNuma() ? c.gnuma.data() : nullptr, c.gblk.data());
         what = "kxpu_classify_viable";
     } else {
-        rc = topologyAware ? kxpu_classify_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(), c.gnuma.data())
-                           : kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data());
-        what = topologyAware ? "kxpu_classify_topo" : "kxpu_classify_rules";
+        rc = readsNuma() ? kxpu_classify_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(), c.gnuma.data())
+                         : kxpu_classify_rules(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data());
+        what = readsNuma() ? "kxpu_classify_topo" : "kxpu_classify_rules";
     }
     if (rc != KXPU_OK) return kxfail(ctx_, what, rc);
     c.nGroups = out.n_groups;
@@ -652,6 +676,7 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
     iommuNuma.clear();
     iommuPcieNode.clear();
     iommuBlocker.clear();
+    iommuDra.clear();
     const ClassifyResult &c = w.out;
     std::map<uint32_t, size_t> groupClass = groupClasses(c);
     for (uint32_t g = 0; g < c.nGroups; g++) {
@@ -667,6 +692,10 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
         if (topologyAware) iommuNuma.push_back(c.gnuma[g]);
         if (pcieTopologyAware) iommuPcieNode.push_back(w.gnode[g]);
         if (groupViability) iommuBlocker.push_back(c.gblk[g] == KXPU_VIABLE ? std::string() : blockerOf(w.recs[c.gblk[g]]));
+        if (draEnabled()) {
+            const uint32_t first = c.gmem[c.goff[g]];
+            iommuDra.push_back(draRecord(w.recs[first], w.paths.size() > first ? &w.paths[first] : nullptr, c.gnuma[g]));
+        }
     }
     if (pcieTopologyAware) {
         pcieParent.assign(w.nodeParent.begin(), w.nodeParent.begin() + w.nNodes);
@@ -1212,8 +1241,27 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
     return Error();
 }
 
+bool Plugin::draEnabled() const {
+    for (const XpuClass &c : xpuClasses)
+        if (!c.draDriver.empty()) return true;
+    return false;
+}
+
+Error Plugin::checkDraClasses() const {
+    for (size_t c = 0; c < xpuClasses.size(); c++) {
+        const std::string &d = xpuClasses[c].draDriver;
+        if (d.empty()) continue;
+        if (nodeName.empty()) return fail("DRA driver " + d + " is set but the node name is empty (NODE_NAME)");
+        for (size_t k = 0; k < c; k++)
+            if (xpuClasses[k].draDriver == d) return fail("DRA driver " + d + " is set on two classes (" + std::to_string(k) + " and " + std::to_string(c) + ")");
+    }
+    return Error();
+}
+
 Error Plugin::InitiateDevicePlugin() {
-    Error e = createIommuDeviceMap();  // :46
+    Error e = checkDraClasses();
+    if (e) return e;
+    e = createIommuDeviceMap();  // :46
     if (e) return e;
     e = createMdevMap();
     if (e) return e;
@@ -1263,7 +1311,14 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     std::vector<uint64_t> pidx;
     e = reconcileWalk(ctx_, pw, snapshotOf(pw, nullptr), pciSnap_, pciNext_, report.pci, pidx);
     if (e) return e;
+    std::map<std::string, std::string> blockerWas;  // group id -> its blocker in the last walk
+    for (size_t g = 0; g < iommuBlocker.size() && g < iommuMap.size(); g++) blockerWas[iommuMap[g].first] = iommuBlocker[g];
     buildIommuMaps(pw, &pidx);
+    bool viabilityChanged = false;
+    for (size_t g = 0; g < iommuBlocker.size() && g < iommuMap.size(); g++) {
+        auto it = blockerWas.find(iommuMap[g].first);
+        viabilityChanged |= it != blockerWas.end() && it->second != iommuBlocker[g];
+    }
     if (!vgpuClasses.empty()) {
         MdevWalk mw;
         e = classifyMdev(mw);
@@ -1323,6 +1378,9 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         report.changedPlugins.push_back(k);
     }
     std::sort(report.changedPlugins.begin(), report.changedPlugins.end());
+    bool passthroughChanged = false;
+    for (size_t k : report.changedPlugins) passthroughChanged |= !devicePlugins[k].vgpu;
+    if (passthroughChanged || viabilityChanged) draGeneration_++;  // the ResourceSlices of the next publication replace these
     // 6. a fresh snapshot generation: Allocate answers from the snapshot again
     haveWalkGen_ = haveGen;
     walkGen_ = gen;
@@ -1409,6 +1467,68 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
     }
     resp.Envs.clear();
     resp.Envs[kK8SCDIVendorClass] = kind;  // :348-350 overwrites Envs
+    return Error();
+}
+
+Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) {
+    std::shared_lock<std::shared_mutex> lock(mu_);
+    if (xpuClass >= xpuClasses.size() || xpuClasses[xpuClass].draDriver.empty())
+        return fail("ResourceSlices: class " + std::to_string(xpuClass) + " has no DRA driver");
+    const std::string &driver = xpuClasses[xpuClass].draDriver;
+    std::map<std::string, const std::string *> productOf;  // group id -> the resource-name suffix of its plugin
+    for (const GenericDevicePlugin &dp : devicePlugins)
+        if (!dp.vgpu && dp.xpuClass == xpuClass)
+            for (const Device &d : dp.devs) productOf[d.ID] = &dp.devpluginName;
+    std::vector<kxpu_dradev> devs;
+    for (size_t g = 0; g < iommuMap.size() && g < iommuDra.size(); g++) {
+        if (iommuClass[g] != xpuClass || (g < iommuBlocker.size() && !iommuBlocker[g].empty())) continue;
+        kxpu_dradev d = iommuDra[g];
+        auto it = productOf.find(iommuMap[g].first);
+        if (it != productOf.end()) {
+            d.product_len = (uint8_t)std::min<size_t>(it->second->size(), sizeof d.product);
+            memcpy(d.product, it->second->data(), d.product_len);
+        }
+        devs.push_back(d);
+    }
+    size_t len = 0, nSlices = 0;
+    int32_t rc = kxpu_dra_slices(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), draGeneration_, devs.data(),
+                                 devs.size(), nullptr, 0, &len, nullptr, &nSlices);
+    if (rc == KXPU_E_NOSPACE) {
+        out.assign(len, 0);
+        sliceOff.assign(nSlices + 1, 0);
+        rc = kxpu_dra_slices(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), draGeneration_, devs.data(), devs.size(),
+                             out.data(), out.size(), &len, sliceOff.data(), &nSlices);
+    }
+    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_dra_slices", rc);
+    return Error();
+}
+
+Error Plugin::PrepareDraDevices(const std::string &driver, const std::string &pool, const std::vector<std::string> &deviceNames,
+                                std::vector<std::vector<std::string>> &cdiIds) {
+    std::vector<std::string> groups;
+    {
+        std::shared_lock<std::shared_mutex> lock(mu_);  // Allocate takes it again below
+        size_t cls = xpuClasses.size();
+        for (size_t c = 0; c < xpuClasses.size(); c++)
+            if (!driver.empty() && xpuClasses[c].draDriver == driver) cls = c;
+        if (cls == xpuClasses.size()) return fail("PrepareDraDevices: unknown DRA driver " + driver);
+        if (pool != nodeName) return fail("PrepareDraDevices: unknown pool " + pool + " of driver " + driver);
+        for (const std::string &name : deviceNames) {
+            const std::string g = name.compare(0, 4, "vfio") == 0 ? name.substr(4) : std::string();
+            size_t at = iommuMap.size();
+            for (size_t k = 0; k < iommuMap.size(); k++)
+                if (!g.empty() && iommuMap[k].first == g && iommuClass[k] == cls) at = k;
+            if (at == iommuMap.size()) return fail("PrepareDraDevices: unknown device " + name + " in pool " + pool);
+            groups.push_back(g);
+        }
+    }
+    cdiIds.clear();
+    for (const std::string &g : groups) {
+        ContainerAllocateResponse resp;
+        Error e = Allocate({g}, resp);
+        if (e) return e;
+        cdiIds.push_back(resp.CDIDevices);
+    }
     return Error();
 }
 
@@ -2176,6 +2296,79 @@ int kxh_gather_viab(const char *base_path, const char *classes, int on, const ch
     if (recs.size() > cap) return -2;
     memcpy(out, recs.data(), recs.size() * sizeof(kxpu_devrec));
     return 0;
+}
+
+// ---- DRA ResourceSlices (ABI v9)
+// draDriver of every class from a comma separated list (position = class; "" = not published), and the node name
+int kxh_set_dra(void *h, const char *drivers_csv, const char *node_name) {
+    Plugin *p = (Plugin *)h;
+    std::string all(drivers_csv);
+    size_t c = 0, a = 0;
+    for (;;) {
+        const size_t comma = all.find(',', a);
+        if (c >= p->xpuClasses.size()) return -1;
+        p->xpuClasses[c++].draDriver = all.substr(a, comma == std::string::npos ? std::string::npos : comma - a);
+        if (comma == std::string::npos) break;
+        a = comma + 1;
+    }
+    p->nodeName = node_name;
+    return 0;
+}
+// InitiateDevicePlugin (the configuration checks first); the error message into err
+int kxh_initiate(void *h, char *err, size_t cap) {
+    device_plugin::Error e = ((Plugin *)h)->InitiateDevicePlugin();
+    if (e) { copy_out(e.message, err, cap); return -1; }
+    return 0;
+}
+// ResourceSlices of one class: -1 with the message in out, -2 when out or offs is too small (*len / *n_slices hold the
+// sizes), else 0
+int kxh_resource_slices(void *h, int cls, uint8_t *out, size_t cap, size_t *len, uint64_t *offs, size_t offcap, size_t *n_slices) {
+    std::vector<uint8_t> o;
+    std::vector<uint64_t> so;
+    device_plugin::Error e = ((Plugin *)h)->ResourceSlices((size_t)cls, o, so);
+    if (e) { copy_out(e.message, (char *)out, cap); return -1; }
+    *len = o.size();
+    *n_slices = so.size() - 1;
+    if (o.size() > cap || so.size() > offcap) return -2;
+    memcpy(out, o.data(), o.size());
+    memcpy(offs, so.data(), so.size() * sizeof(uint64_t));
+    return 0;
+}
+uint64_t kxh_dra_generation(void *h) { return ((Plugin *)h)->draGeneration(); }
+// counting seams on a plugin: every numa_node read and every entry-link read of its gathers (through the walk) is counted
+void kxh_count_reads(void *h, uint64_t *numa_reads, uint64_t *path_reads) {
+    Plugin *p = (Plugin *)h;
+    auto dn = p->readNumaNode;
+    p->readNumaNode = [dn, numa_reads](const std::string &base, const std::string &entry, std::string &out) {
+        (*numa_reads)++;
+        return dn(base, entry, out);
+    };
+    auto dp = p->readPciPath;
+    p->readPciPath = [dp, path_reads](const std::string &base, const std::string &entry, std::string &target) {
+        (*path_reads)++;
+        return dp(base, entry, target);
+    };
+}
+// PrepareDraDevices; names_csv = comma separated device names.  json: [[cdi names of device 0], ...] or the message
+int kxh_prepare_dra(void *h, const char *driver, const char *pool, const char *names_csv, char *json, size_t cap) {
+    std::vector<std::string> names;
+    std::string all(names_csv);
+    for (size_t a = 0; !all.empty();) {
+        const size_t comma = all.find(',', a);
+        names.push_back(all.substr(a, comma == std::string::npos ? std::string::npos : comma - a));
+        if (comma == std::string::npos) break;
+        a = comma + 1;
+    }
+    std::vector<std::vector<std::string>> ids;
+    device_plugin::Error e = ((Plugin *)h)->PrepareDraDevices(driver, pool, names, ids);
+    if (e) { copy_out(e.message, json, cap); return -1; }
+    std::string o = "[";
+    for (size_t i = 0; i < ids.size(); i++) {
+        o += i ? ",[" : "[";
+        for (size_t k = 0; k < ids[i].size(); k++) { if (k) o += ','; jstr(o, ids[i][k]); }
+        o += ']';
+    }
+    return copy_out(o + "]", json, cap);
 }
 
 }  // extern "C"

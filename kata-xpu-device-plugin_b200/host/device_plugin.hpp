@@ -163,6 +163,9 @@ struct XpuClass {
     std::string resourceNamespace;  // resource = <resourceNamespace>/<device name>
     std::string cdiKind;            // CDI kind of this class's spec file and Allocate names
     std::string cdiFileStem;        // <cdiConfigPath><cdiFileStem>.yaml|.json
+    // DRA driver name that publishes this class's IOMMU groups as ResourceSlices (Plugin::ResourceSlices); empty: the
+    // class is not published
+    std::string draDriver{};
 };
 XpuClass defaultXpuClass();  // {"10de", "vfio-pci", "nvidia.com", "nvidia.com/gpu", "cdi-vfio-xxxx"}
 
@@ -260,6 +263,15 @@ class Plugin {
     // and vGPU plugins do not change.
     bool groupViability = false;
     std::vector<std::string> viabilityDrivers{"vfio-pci", "pci-stub", "pcieport"};
+    // DRA ResourceSlices (include/kxpu.h, ABI v9).  With no XpuClass::draDriver set (default) nothing more is read and
+    // every output is as above.  With one: the PCI gathers read numa_node and the entry link as topologyAware /
+    // pcieTopologyAware do (none of those settings' other effects turn on), and ResourceSlices publishes the class's
+    // groups in one pool named nodeName.  nodeName is a seam: the Go host takes it from NODE_NAME.
+    std::string nodeName;
+    bool draEnabled() const;  // some class has a draDriver
+    // the PCI gathers read numa_node (topologyAware or draEnabled) and the entry link (pcieTopologyAware or draEnabled)
+    bool readsNuma() const { return topologyAware || draEnabled(); }
+    bool readsPaths() const { return pcieTopologyAware || draEnabled(); }
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
 
     // ---- state (device_plugin.go:31,34)
@@ -277,6 +289,8 @@ class Plugin {
     std::vector<uint8_t> pcieDepth;
     // groupViability only: "<bdf> is bound to <driver>" of the first blocker of every iommuMap entry; empty = viable
     std::vector<std::string> iommuBlocker;
+    // draEnabled only: the ResourceSlice record of every iommuMap entry (from its first member; product left empty)
+    std::vector<kxpu_dradev> iommuDra;
     std::vector<std::string> cdiFiles;  // files the last generateCDISpec wrote, one per class
     // the mdev walk: IOMMU group -> mdevs, type key -> groups, and the vGPU class of every entry (same positions)
     OrderedMap<std::vector<MdevDevice>> mdevMap;
@@ -325,6 +339,21 @@ class Plugin {
     // plugins appended, a plugin whose devices all left keeps an empty list) and take a fresh snapshot generation.
     // A restart numbers by walk order again: the index high-water mark is not persisted.
     Error rediscover(RediscoverReport &report, const std::string &format = "YAML");
+    // The ResourceSlices of class xpuClass (kxpu_dra_slices): one pool named nodeName, one device per iommuMap group of
+    // the class in walk order (bdf, vendor, device and PCIe root of the group's first member, the group's NUMA mask, the
+    // plugin's resource-name suffix cut to 64 bytes as productName).  With groupViability a group that has a blocker is
+    // not published: DRA v1 has no per-device health and a published device is schedulable.  Health from the
+    // HealthWatcher is not consulted.  out: JSON Lines, one slice per line; sliceOff: the n_slices + 1 line bounds.
+    Error ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff);
+    // the pool generation of every class's ResourceSlices: 1 after start-up, +1 for each rediscover that changed a
+    // passthrough plugin or a group's viability
+    uint64_t draGeneration() const { return draGeneration_; }
+    // The data half of NodePrepareResources: cdiIds[i] = the CDI names Allocate({g}) returns for deviceNames[i] =
+    // "vfio<g>", a device of the pool `pool` of the class whose draDriver is `driver` (same live or snapshot
+    // re-validation, same viability refusal).  An unknown driver, pool or device is an error that names it.
+    Error PrepareDraDevices(const std::string &driver, const std::string &pool, const std::vector<std::string> &deviceNames,
+                            std::vector<std::vector<std::string>> &cdiIds);
+
     // has a pci (or, with vGPU classes, an mdev) uevent generation moved since the last walk?  true when it cannot tell
     bool discoveryStale();
     // the snapshot of the last walks (kxpu_snaprec per accepted function / mdev in walk order) and their next index
@@ -375,6 +404,8 @@ class Plugin {
     BindWatcher bindWatcher_;
     bool haveSnapshotGen_ = false;
     uint64_t snapshotGen_ = 0;
+    uint64_t draGeneration_ = 1;
+    Error checkDraClasses() const;
 };
 
 }  // namespace device_plugin

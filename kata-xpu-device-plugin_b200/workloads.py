@@ -566,3 +566,22 @@ def viab_records(n=1 << 20, seed=31):
     recs["flags"] = np.where(drv == b"", REC_DRIVER_ERR, 0).astype(np.uint8) | np.where(blocks, REC_BLOCKS, 0).astype(np.uint8)
     recs["iommu_group"] = group[slot].astype(np.uint32)
     return recs
+
+
+# ---------------------------------------------------------------- DRA ResourceSlices (ABI v9)
+def dra_devices(n=1 << 16, seed=41):
+    """n published devices with every optional attribute present and the longest fields the host produces: a 64-byte
+    product name, a 12-byte PCI address, a 10-byte PCIe root, 4-digit ids, one NUMA node, 9-digit groups"""
+    from .binding import DRADEV_DTYPE
+    rng = np.random.default_rng(seed)
+    d = np.zeros(n, DRADEV_DTYPE)
+    alnum = np.frombuffer(b"ABCDEFGHIJKLMNOPQRSTUVWXYZ0123456789_", np.uint8)
+    d["product"] = alnum[rng.integers(0, len(alnum), (n, 64))]
+    d["product_len"] = 64
+    i = np.arange(n)
+    d["bdf"] = [b"%04x:%02x:%02x.%d" % (k >> 13, (k >> 5) & 0xff, (k >> 3) & 0x1f, k & 7) for k in range(n)]
+    d["pcie_root"] = [b"pci%04x:%02x" % (k >> 13, (k >> 5) & 0xff) for k in range(n)]
+    d["vendor"], d["device"] = b"10de", b"2330"
+    d["numa_mask"] = np.left_shift(np.uint64(1), (i % 8).astype(np.uint64))
+    d["iommu_group"] = 100000000 + i
+    return d

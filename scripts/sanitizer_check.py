@@ -42,6 +42,10 @@ vrecs = W.viab_records(20000)
 for topo in (False, True):
     vres = kx.classify_viable(W.VIAB_RULES, vrecs, topo=topo)
     print("viable groups", vres["n_groups"], "blocked", int((vres["group_blocker"] != B.VIABLE).sum()))
+# DRA ResourceSlices: one pool of 24 slices (the last one partial), and the empty pool
+for dn_ in (3000, 0):
+    blob, soff = kx.dra_slices("vfio.nvidia.com", "node-a", "node-a", 1, W.dra_devices(dn_))
+    print("dra slices", len(soff) - 1, "bytes", len(blob))
 
 
 # look-back state across epoch wraps (tests/test_gpu_lookback_state.py at reduced sizes): every user of the status
