@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 9
+#define KXPU_ABI_VERSION 10
 
 /* status codes */
 #define KXPU_OK             0
@@ -764,6 +764,54 @@ typedef struct kxpu_dradev {
 int32_t kxpu_dra_slices(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
                         const kxpu_dradev *devs, size_t n, uint8_t *out, size_t cap, size_t *len,
                         uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
+/* ------------------------------------------- DRA ResourceSlices of vGPUs (ABI v10) */
+
+/* One published vGPU (one IOMMU group of one vGPU class, described by its first mdev).  208 bytes, a multiple of 16;
+ * alignof 8.  No new fact about the Kubernetes API is used: the [assumed] list above covers this call too. */
+typedef struct kxpu_dramdev {
+    uint8_t  product[64];   /* the PARENT's productName bytes, NUL padded                                    */
+    char     mdev_type[40]; /* the type key of kxpu_classify_mdev, NUL padded                                */
+    char     uuid[36];      /* the mdev's UUID                                                               */
+    uint32_t iommu_group;
+    char     parent[16];    /* parent PCI address                                                            */
+    char     pcie_root[16]; /* "pci<domain>:<bus>", the first component of the mdev entry's link; "" = unknown */
+    char     vendor[8];     /* the parent's vendor id, NUL padded                                            */
+    char     device[8];     /* the parent's device id; "" = not read                                         */
+    uint64_t numa_mask;     /* the group's NUMA mask (kxpu_classify_mdev_topo)                               */
+    uint8_t  product_len;   /* 0..64                                                                         */
+    uint8_t  reserved[7];
+} kxpu_dramdev;
+
+/* The ResourceSlices of one pool of vGPUs.  Everything but the device is kxpu_dra_slices' contract, unchanged: the
+ * slices, their header and tail, 128 devices per slice and one empty slice for n = 0, slice_off, the two-call sizing
+ * and KXPU_E_NOSPACE, the KXPU_E_INVALID argument checks, KXPU_DRA_MAX_DEVICES, and nothing written on KXPU_E_INVALID
+ * or KXPU_E_UNSUPPORTED.  A device is
+ *   {"name":"vfio<g>","attributes":{<attributes>}}
+ * with g = iommu_group in decimal (it mirrors the cdi.k8s.io/vfio<g> annotation of the mdev CDI spec), and the
+ * attributes, keys sorted bytewise:
+ *   "iommuGroup":{"int":<g>}                                          always
+ *   "mdevType":{"string":"<mdev_type>"}                               always
+ *   "numaNode":{"int":<k>}                                            only when numa_mask has exactly one bit k set
+ *   "parentAddress":{"string":"<parent>"}                             always
+ *   "parentDeviceID":{"string":"<device>"}                            only when device is not empty
+ *   "parentVendorID":{"string":"<vendor>"}                            always
+ *   "productName":{"string":"<product[0..product_len)>"}              only when product_len > 0
+ *   "resource.kubernetes.io/pcieRoot":{"string":"<pcie_root>"}        only when pcie_root is not empty
+ *   "uuid":{"string":"<uuid>"}                                        always
+ * KXPU_E_UNSUPPORTED, with *len, the output and slice_off untouched: n >= KXPU_DRA_MAX_DEVICES, or a record outside
+ * the domain:
+ *   - product[0..product_len) over [A-Za-z0-9_.-]; bytes past product_len are ignored; product_len <= 64;
+ *   - mdev_type: 1..40 bytes over [A-Za-z0-9_.-] before its first NUL (all 40 when there is none);
+ *   - uuid: the canonical lowercase 8-4-4-4-12 form;
+ *   - parent: 1..16 bytes over [0-9a-f:.] before its first NUL;
+ *   - pcie_root: empty, or "pci" followed by 1..13 bytes over [0-9a-f:] before its first NUL;
+ *   - vendor: 1..6 bytes over [0-9a-f] before the first NUL; device: 0..6 such bytes;
+ *   - iommu_group below 4294967295.
+ * GPU: the kernel of kxpu_dra_slices, instantiated for this record layout.  Timed under KXPU_T_EMIT. */
+int32_t kxpu_dra_slices_mdev(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                             const kxpu_dramdev *devs, size_t n, uint8_t *out, size_t cap, size_t *len,
+                             uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
 
 #ifdef __cplusplus
 }

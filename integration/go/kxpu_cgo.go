@@ -623,3 +623,31 @@ func (k *kxpu) draSlices(driver, node string, generation uint64, devs []C.kxpu_d
 	}
 	return lines, nil
 }
+
+// DRA ResourceSlices of vGPUs (ABI v10).  One pool per vGPU class with a DRA driver, named after the node: devs holds one
+// kxpu_dramdev per mdevMap group of the class in walk order.  Published and replaced exactly as draSlices' output.
+func (k *kxpu) draSlicesMdev(driver, node string, generation uint64, devs []C.kxpu_dramdev) ([]string, error) {
+	cd, cn := C.CString(driver), C.CString(node)
+	defer C.free(unsafe.Pointer(cd))
+	defer C.free(unsafe.Pointer(cn))
+	var p *C.kxpu_dramdev
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	var n, ns C.size_t
+	rc := C.kxpu_dra_slices_mdev(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), nil, 0, &n, nil, &ns) // sizing call
+	if rc != C.KXPU_E_NOSPACE {
+		return nil, kxCheck(k.ctx, "kxpu_dra_slices_mdev", rc)
+	}
+	buf := make([]byte, n)
+	off := make([]uint64, ns+1)
+	if err := kxCheck(k.ctx, "kxpu_dra_slices_mdev", C.kxpu_dra_slices_mdev(k.ctx, cd, cn, cn, C.uint64_t(generation), p,
+		C.size_t(len(devs)), (*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n, (*C.uint64_t)(unsafe.Pointer(&off[0])), &ns)); err != nil {
+		return nil, err
+	}
+	lines := make([]string, ns)
+	for s := range lines {
+		lines[s] = string(buf[off[s] : off[s+1]-1]) // without the '\n'
+	}
+	return lines, nil
+}

@@ -56,6 +56,11 @@ PCIE_NO_NODE = 0xFFFFFFFF
 DRADEV_DTYPE = np.dtype([("product", "u1", (64,)), ("bdf", "S16"), ("pcie_root", "S16"), ("vendor", "S8"), ("device", "S8"),
                          ("numa_mask", "<u8"), ("iommu_group", "<u4"), ("product_len", "u1"), ("reserved", "u1", (3,))])
 assert DRADEV_DTYPE.itemsize == 128
+# kxpu_dramdev (DRA ResourceSlices of vGPUs, ABI v10): one published vGPU
+DRAMDEV_DTYPE = np.dtype([("product", "u1", (64,)), ("mdev_type", "S40"), ("uuid", "S36"), ("iommu_group", "<u4"),
+                          ("parent", "S16"), ("pcie_root", "S16"), ("vendor", "S8"), ("device", "S8"), ("numa_mask", "<u8"),
+                          ("product_len", "u1"), ("reserved", "u1", (7,))])
+assert DRAMDEV_DTYPE.itemsize == 208
 DRA_SLICE_DEVICES = 128
 DRA_MAX_DEVICES = 1 << 24
 
@@ -73,7 +78,7 @@ ABI_SYMBOLS = [
     "kxpu_pciids_full_load_device", "kxpu_full_free", "kxpu_full_export", "kxpu_full_lookup",
     "kxpu_classify_topo", "kxpu_classify_mdev_topo", "kxpu_lw_encode_topo", "kxpu_preferred_allocation",
     "kxpu_reconcile", "kxpu_pcie_tree", "kxpu_preferred_allocation_pcie", "kxpu_classify_viable",
-    "kxpu_dra_slices",
+    "kxpu_dra_slices", "kxpu_dra_slices_mdev",
 ]
 
 
@@ -175,6 +180,8 @@ def load_library():
         "kxpu_classify_viable": (i32, [vp, vp, sz, vp, sz, C.POINTER(ClassifyOut), vp, vp, vp]),
         "kxpu_dra_slices": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, C.POINTER(sz), vp,
                                   C.POINTER(sz)]),
+        "kxpu_dra_slices_mdev": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, C.POINTER(sz), vp,
+                                       C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -660,16 +667,23 @@ class Kxpu:
     def dra_slices(self, driver, pool, node, generation, devs):
         """kxpu_dra_slices: (bytes, slice_off) of the ResourceSlices of one pool (DRADEV_DTYPE devices), with the two-call
         sizing.  Slice s is the JSON object bytes[slice_off[s]:slice_off[s + 1] - 1], each followed by '\\n'."""
+        return self._slices(self.L.kxpu_dra_slices, DRADEV_DTYPE, driver, pool, node, generation, devs)
+
+    def dra_slices_mdev(self, driver, pool, node, generation, devs):
+        """kxpu_dra_slices_mdev: the same for a pool of vGPUs (DRAMDEV_DTYPE devices)."""
+        return self._slices(self.L.kxpu_dra_slices_mdev, DRAMDEV_DTYPE, driver, pool, node, generation, devs)
+
+    def _slices(self, fn, dtype, driver, pool, node, generation, devs):
         devs = np.ascontiguousarray(devs)
-        assert devs.dtype == DRADEV_DTYPE
+        assert devs.dtype == dtype
         args = (self.ctx, _kind(driver), _kind(pool), _kind(node), generation, _ptr(devs) if len(devs) else None, len(devs))
         need, ns = C.c_size_t(0), C.c_size_t(0)
-        rc = self.L.kxpu_dra_slices(*args, None, 0, C.byref(need), None, C.byref(ns))
+        rc = fn(*args, None, 0, C.byref(need), None, C.byref(ns))
         if rc not in (KXPU_OK, E_NOSPACE):
             self._chk(rc)
         out = np.empty(max(need.value, 1), np.uint8)
         offs = np.empty(ns.value + 1, np.uint64)
-        self._chk(self.L.kxpu_dra_slices(*args, _ptr(out), need.value, C.byref(need), _ptr(offs), C.byref(ns)))
+        self._chk(fn(*args, _ptr(out), need.value, C.byref(need), _ptr(offs), C.byref(ns)))
         return out[:need.value].tobytes(), offs
 
     def cdi_emit(self, fmt, devs, kind=None):

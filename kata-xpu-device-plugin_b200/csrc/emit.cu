@@ -308,10 +308,11 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
     tile_store(E.out + base, stg, head_len + tile_total + tail_len);
 }
 
-// ------------------------------------------------------------------ K11: DRA ResourceSlices (kxpu_dra_slices)
-// One CTA per slice of TILE devices.  A device fragment is literal D0, the variable fields and literals D1..D8 (D3 / D5 /
-// D6 with their field only when present), then ',' unless it is the slice's last device.  Every literal but D0 opens with
-// the closing bytes of the value before it, so an absent optional attribute simply drops its literal and field.
+// ------------------------------------------------------------------ K11: DRA ResourceSlices (kxpu_dra_slices[_mdev])
+// One CTA per slice of TILE devices; k_dra_slices<LAYOUT> reads kxpu_dradev (LAYOUT_PCI) or kxpu_dramdev (LAYOUT_MDEV)
+// records.  A PCI device fragment is literal D0, the variable fields and literals D1..D8 (D3 / D5 / D6 with their field
+// only when present), then ',' unless it is the slice's last device.  Every literal but D0 opens with the closing bytes
+// of the value before it, so an absent optional attribute simply drops its literal and field.
 #define KX_D0 "{\"name\":\"vfio"
 #define KX_D1 "\",\"attributes\":{\"deviceID\":{\"string\":\""
 #define KX_D2 "\"},\"iommuGroup\":{\"int\":"
@@ -330,22 +331,54 @@ constexpr int MAX_FRAG_DRA = (int)DRA_LIT_TOTAL + 2 * 10 + 2 + 16 + 16 + 64 + 6 
 // literals | slice head | slice tail: the head holds the node name twice, the driver twice and the pool once
 // (2 * 253 + 2 * 63 + 253 bytes of names, about 1.1 KB in all)
 constexpr int DRA_POOL_MAX = 1536;
-constexpr int DRA_HEAD = 9, DRA_TAIL = 10, DRA_PARTS = 11;
+constexpr int DRA_PARTS = 11;  // nine literals, the slice head, the slice tail
 
+// An mdev device fragment: literal M0, the group, M1, the group and its closer; then for each attribute in key order its
+// opening literal (M2..M9), its value and the value's own closer (MS after a string, MI after an int); then ME and the
+// separator.  A value is never closed by the next attribute's literal: numaNode is an int between two strings, so an
+// absent attribute drops its opening literal, value and closer, and nothing else changes.
+#define KX_M0 "{\"name\":\"vfio"
+#define KX_M1 "\",\"attributes\":{\"iommuGroup\":{\"int\":"
+#define KX_M2 ",\"mdevType\":{\"string\":\""
+#define KX_M3 ",\"numaNode\":{\"int\":"
+#define KX_M4 ",\"parentAddress\":{\"string\":\""
+#define KX_M5 ",\"parentDeviceID\":{\"string\":\""
+#define KX_M6 ",\"parentVendorID\":{\"string\":\""
+#define KX_M7 ",\"productName\":{\"string\":\""
+#define KX_M8 ",\"resource.kubernetes.io/pcieRoot\":{\"string\":\""
+#define KX_M9 ",\"uuid\":{\"string\":\""
+#define KX_MS "\"}"
+#define KX_MI "}"
+#define KX_ME "}}"
+constexpr int DRAM_S = 10, DRAM_I = 11, DRAM_E = 12, DRAM_LITS = 13;
+static const char *const h_dram_lits[DRAM_LITS] = {KX_M0, KX_M1, KX_M2, KX_M3, KX_M4, KX_M5, KX_M6,
+                                                   KX_M7, KX_M8, KX_M9, KX_MS, KX_MI, KX_ME};
+// the longest fragment: every literal, seven string closers, two int closers, a 10-digit group twice, a 40-byte type,
+// node 63, a 16-byte parent and root, two 6-byte ids, 64 product bytes, the uuid, the separator
+constexpr int MAX_FRAG_DRA_MDEV = (int)sizeof(KX_M0 KX_M1 KX_M2 KX_M3 KX_M4 KX_M5 KX_M6 KX_M7 KX_M8 KX_M9 KX_ME) - 1 +
+                                  7 * ((int)sizeof(KX_MS) - 1) + 2 * ((int)sizeof(KX_MI) - 1) + 2 * 10 + 40 + 2 + 16 +
+                                  16 + 6 + 6 + 64 + 36 + 1;
+constexpr int DRAM_PARTS = DRAM_LITS + 2;
+
+// PARTS = literals + head + tail; the head is part PARTS - 2, the tail PARTS - 1
+template <int PARTS>
 struct DraParams {
-    const kxpu_dradev *devs;
+    const void *devs;               // kxpu_dradev[n] or kxpu_dramdev[n]
     uint32_t n;
-    uint16_t off[DRA_PARTS], len[DRA_PARTS];  // literal k / head / tail inside the pool
+    uint16_t off[PARTS], len[PARTS];  // literal k / head / tail inside the pool
     uint32_t pool_len;
     uint8_t *out;
     unsigned long long *slice_off;  // [gridDim.x + 1]
     unsigned long long *state;      // slice status words (scan.cuh look-back)
     uint32_t epoch;
-    uint32_t *flags;                // one word per KXPU_E_UNSUPPORTED reason, DRA_F_*
+    uint32_t *flags;                // one word per KXPU_E_UNSUPPORTED reason, DRA_F_* / DRAM_F_*
     uint8_t pool[DRA_POOL_MAX];
 };
 constexpr int DRA_F_PRODUCT = 0, DRA_F_BDF = 1, DRA_F_ROOT = 2, DRA_F_VENDOR = 3, DRA_F_DEVICE = 4, DRA_F_GROUP = 5,
               DRA_F_PLEN = 6, DRA_F_COUNT = 7;
+// the order of the header's domain list, which the oracle's `why` follows
+constexpr int DRAM_F_PRODUCT = 0, DRAM_F_TYPE = 1, DRAM_F_UUID = 2, DRAM_F_PARENT = 3, DRAM_F_ROOT = 4, DRAM_F_VENDOR = 5,
+              DRAM_F_DEVICE = 6, DRAM_F_GROUP = 7, DRAM_F_PLEN = 8, DRAM_F_COUNT = 9;
 
 struct DraSmem {
     alignas(16) uint8_t stage[TILE * MAX_FRAG_DRA + DRA_POOL_MAX + 16];
@@ -356,6 +389,27 @@ struct DraSmem {
     unsigned long long base;
     uint32_t wsum[EMIT_THREADS / 32];
     uint32_t tile_total;
+};
+struct DraMdevSmem {
+    alignas(16) uint8_t stage[TILE * MAX_FRAG_DRA_MDEV + DRA_POOL_MAX + 16];
+    uint8_t pool[DRA_POOL_MAX];
+    uint8_t dec[TILE][12];  // group digits at 0, NUMA node digits at 10
+    uint32_t meta[TILE];    // as DraSmem's, bl being the parent's length
+    uint8_t tlen[TILE];     // mdev_type length
+    uint32_t start[TILE];   // fragment offset inside the slice
+    unsigned long long base;
+    uint32_t wsum[EMIT_THREADS / 32];
+    uint32_t tile_total;
+};
+template <int LAYOUT> struct DraLayout {  // LAYOUT_PCI
+    using Rec = kxpu_dradev;
+    using Smem = DraSmem;
+    static constexpr int PARTS = DRA_PARTS;
+};
+template <> struct DraLayout<LAYOUT_MDEV> {
+    using Rec = kxpu_dramdev;
+    using Smem = DraMdevSmem;
+    static constexpr int PARTS = DRAM_PARTS;
 };
 
 template <int W>
@@ -378,18 +432,24 @@ __device__ __forceinline__ bool bytes_ok(const uint32_t (&w)[W], uint32_t from, 
     return good;
 }
 
-__global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_constant__ DraParams E) {
+template <int LAYOUT>
+__global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_constant__ DraParams<DraLayout<LAYOUT>::PARTS> E) {
+    using Rec = typename DraLayout<LAYOUT>::Rec;
+    constexpr int HEAD = DraLayout<LAYOUT>::PARTS - 2, TAIL = DraLayout<LAYOUT>::PARTS - 1;
     extern __shared__ __align__(16) uint8_t smem_raw[];
-    DraSmem &S = *reinterpret_cast<DraSmem *>(smem_raw);
+    typename DraLayout<LAYOUT>::Smem &S = *reinterpret_cast<typename DraLayout<LAYOUT>::Smem *>(smem_raw);
     const uint32_t tid = threadIdx.x, lane = tid & 31u, w = tid >> 5;
     const uint32_t slice = blockIdx.x, i0 = slice * TILE;
     const uint32_t in_slice = E.n > i0 ? min(E.n - i0, (uint32_t)TILE) : 0u;
     for (uint32_t k = tid; k < E.pool_len; k += EMIT_THREADS) S.pool[k] = E.pool[k];
+    const auto name_ok = [](uint32_t c) {
+        return (c >= '0' && c <= '9') || (c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z') || c == '_' || c == '.' || c == '-';
+    };
 
     // ---- fragment lengths, digits and the domain checks: one thread per device
     uint32_t flen = 0;
-    if (tid < in_slice) {
-        const uint4 *p = reinterpret_cast<const uint4 *>(E.devs + i0 + tid);
+    if (LAYOUT == LAYOUT_PCI && tid < in_slice) {
+        const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const Rec *>(E.devs) + i0 + tid);
         const uint4 q0 = p[0], q1 = p[1], q2 = p[2], q3 = p[3], q4 = p[4], q5 = p[5], q6 = p[6], q7 = p[7];
         const uint32_t prod[16] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
         const uint32_t bdf[4] = {q4.x, q4.y, q4.z, q4.w}, root[4] = {q5.x, q5.y, q5.z, q5.w};
@@ -401,10 +461,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
         const uint32_t vl = min(vl_raw, 6u), dl = min(dl_raw, 6u);  // bounded like pl
         const auto hex = [](uint32_t c) { return is_lhex(c); };
         if (plen_raw > 64u) E.flags[DRA_F_PLEN] = 1u;
-        if (!bytes_ok(prod, 0u, pl, [](uint32_t c) {
-                return (c >= '0' && c <= '9') || (c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z') || c == '_' || c == '.' || c == '-';
-            }))
-            E.flags[DRA_F_PRODUCT] = 1u;
+        if (!bytes_ok(prod, 0u, pl, name_ok)) E.flags[DRA_F_PRODUCT] = 1u;
         if (bl == 0u || !bytes_ok(bdf, 0u, bl, [](uint32_t c) { return is_lhex(c) || c == ':' || c == '.'; })) E.flags[DRA_F_BDF] = 1u;
         if (rl != 0u && (rl < 4u || byte_at(root, 0) != 'p' || byte_at(root, 1) != 'c' || byte_at(root, 2) != 'i' ||
                          !bytes_ok(root, 3u, rl, [](uint32_t c) { return is_lhex(c) || c == ':'; })))
@@ -421,6 +478,71 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
         flen = DRA_LIT_TOTAL - E.len[3] - E.len[5] - E.len[6] + 2u * gl + bl + vl + dl + (nl ? E.len[3] + nl : 0u) +
                (pl ? E.len[5] + pl : 0u) + (rl ? E.len[6] + rl : 0u) + (tid + 1u < in_slice ? 1u : 0u);
     }
+    if constexpr (LAYOUT == LAYOUT_MDEV) {
+        if (tid < in_slice) {
+            // 208 bytes = 13 uint4; read field by field so that no more than a few of them are live at once
+            const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const Rec *>(E.devs) + i0 + tid);
+            uint32_t pl, tl, bl, rl, vl, dl;
+            {  // product_len and product (q12, q0..q3)
+                const uint32_t plen_raw = p[12].z & 0xffu;
+                pl = plen_raw <= 64u ? plen_raw : 64u;  // out of the domain: reported, and bounded here
+                if (plen_raw > 64u) E.flags[DRAM_F_PLEN] = 1u;
+                const uint4 q0 = p[0], q1 = p[1], q2 = p[2], q3 = p[3];
+                const uint32_t prod[16] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w,
+                                           q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
+                if (plen_raw <= 64u && !bytes_ok(prod, 0u, pl, name_ok)) E.flags[DRAM_F_PRODUCT] = 1u;
+            }
+            {  // mdev_type: bytes 64..104 (q4, q5, q6.xy)
+                const uint4 q4 = p[4], q5 = p[5];
+                const uint2 q6 = reinterpret_cast<const uint2 *>(p + 6)[0];
+                const uint32_t ty[10] = {q4.x, q4.y, q4.z, q4.w, q5.x, q5.y, q5.z, q5.w, q6.x, q6.y};
+                tl = nul_len(ty);
+                if (tl == 0u || !bytes_ok(ty, 0u, tl, name_ok)) E.flags[DRAM_F_TYPE] = 1u;
+            }
+            {  // uuid: bytes 104..140 (q6.zw, q7, q8.xyz)
+                const uint2 q6 = reinterpret_cast<const uint2 *>(p + 6)[1];
+                const uint4 q7 = p[7], q8 = p[8];
+                const uint32_t uw[9] = {q6.x, q6.y, q7.x, q7.y, q7.z, q7.w, q8.x, q8.y, q8.z};
+                if (!kxmdev::uuid_ok(uw)) E.flags[DRAM_F_UUID] = 1u;
+            }
+            {  // parent and pcie_root (q9, q10)
+                const uint4 q9 = p[9], q10 = p[10];
+                const uint32_t par[4] = {q9.x, q9.y, q9.z, q9.w}, root[4] = {q10.x, q10.y, q10.z, q10.w};
+                bl = nul_len(par);
+                rl = nul_len(root);
+                if (bl == 0u || !bytes_ok(par, 0u, bl, [](uint32_t c) { return is_lhex(c) || c == ':' || c == '.'; }))
+                    E.flags[DRAM_F_PARENT] = 1u;
+                if (rl != 0u && (rl < 4u || byte_at(root, 0) != 'p' || byte_at(root, 1) != 'c' || byte_at(root, 2) != 'i' ||
+                                 !bytes_ok(root, 3u, rl, [](uint32_t c) { return is_lhex(c) || c == ':'; })))
+                    E.flags[DRAM_F_ROOT] = 1u;
+            }
+            {  // vendor and device (q11)
+                const uint4 q11 = p[11];
+                const uint32_t ven[2] = {q11.x, q11.y}, dev[2] = {q11.z, q11.w};
+                const uint32_t vl_raw = nul_len(ven), dl_raw = nul_len(dev);
+                vl = min(vl_raw, 6u);
+                dl = min(dl_raw, 6u);
+                const auto hex = [](uint32_t c) { return is_lhex(c); };
+                if (vl_raw == 0u || vl_raw > 6u || !bytes_ok(ven, 0u, vl, hex)) E.flags[DRAM_F_VENDOR] = 1u;
+                if (dl_raw > 6u || !bytes_ok(dev, 0u, dl, hex)) E.flags[DRAM_F_DEVICE] = 1u;
+            }
+            const uint32_t group = p[8].w;
+            const uint2 qm = reinterpret_cast<const uint2 *>(p + 12)[0];
+            const unsigned long long mask = ((unsigned long long)qm.y << 32) | qm.x;
+            if (group == 0xFFFFFFFFu) E.flags[DRAM_F_GROUP] = 1u;
+            const bool one_node = mask != 0ull && (mask & (mask - 1ull)) == 0ull;
+            const uint32_t node = one_node ? (uint32_t)__ffsll((long long)mask) - 1u : 0u;
+            const uint32_t gl = dec_len(group), nl = one_node ? dec_len(node) : 0u;
+            dec_write(group, gl, S.dec[tid]);
+            if (one_node) dec_write(node, nl, S.dec[tid] + 10);
+            S.meta[tid] = gl | (nl << 4) | (bl << 8) | (rl << 13) | (vl << 18) | (dl << 21) | (pl << 24);
+            S.tlen[tid] = (uint8_t)tl;
+            const uint32_t ls = E.len[DRAM_S], li = E.len[DRAM_I];
+            flen = E.len[0] + E.len[1] + 2u * gl + li + E.len[2] + tl + ls + E.len[4] + bl + ls + E.len[6] + vl + ls +
+                   E.len[9] + 36u + ls + E.len[DRAM_E] + (nl ? E.len[3] + nl + li : 0u) + (dl ? E.len[5] + dl + ls : 0u) +
+                   (pl ? E.len[7] + pl + ls : 0u) + (rl ? E.len[8] + rl + ls : 0u) + (tid + 1u < in_slice ? 1u : 0u);
+        }
+    }
     // ---- scan of the 128 lengths (threads >= TILE contribute 0)
     const uint32_t incl = kxscan::warp_incl(flen);
     if (lane == 31) S.wsum[w] = incl;
@@ -432,7 +554,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
         if (lane == EMIT_THREADS / 32 - 1) S.tile_total = xi;
     }
     __syncthreads();
-    const uint32_t head_len = E.len[DRA_HEAD], tail_len = E.len[DRA_TAIL], tile_total = S.tile_total;
+    const uint32_t head_len = E.len[HEAD], tail_len = E.len[TAIL], tile_total = S.tile_total;
     if (tid < TILE) S.start[tid] = head_len + S.wsum[w] + incl - flen;
     // ---- the slice's offset in the output: decoupled look-back over the slice totals; its exclusive prefix is slice_off[s]
     if (w == 0) {
@@ -447,14 +569,14 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
     __syncthreads();
     const unsigned long long base = S.base;
     uint8_t *stg = S.stage + ((reinterpret_cast<uintptr_t>(E.out) + base) & 15u);  // same 16-byte phase in smem and global
-    for (uint32_t k = tid; k < head_len; k += EMIT_THREADS) stg[k] = S.pool[E.off[DRA_HEAD] + k];
-    for (uint32_t k = tid; k < tail_len; k += EMIT_THREADS) stg[head_len + tile_total + k] = S.pool[E.off[DRA_TAIL] + k];
+    for (uint32_t k = tid; k < head_len; k += EMIT_THREADS) stg[k] = S.pool[E.off[HEAD] + k];
+    for (uint32_t k = tid; k < tail_len; k += EMIT_THREADS) stg[head_len + tile_total + k] = S.pool[E.off[TAIL] + k];
     // ---- fragments: one warp per device; the string fields straight from the record (L1 / L2)
     for (uint32_t d = w; d < in_slice; d += EMIT_THREADS / 32) {
         const uint32_t m = S.meta[d];
         const uint32_t gl = m & 15u, nl = (m >> 4) & 3u, bl = (m >> 8) & 31u, rl = (m >> 13) & 31u, vl = (m >> 18) & 7u,
                        dl = (m >> 21) & 7u, pl = m >> 24;
-        const kxpu_dradev *r = E.devs + i0 + d;
+        const Rec *r = static_cast<const Rec *>(E.devs) + i0 + d;
         uint8_t *dst = stg + S.start[d];
         uint32_t o = 0;
         auto put = [&](const uint8_t *src, uint32_t L) {
@@ -462,13 +584,27 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
             o += L;
         };
         auto lit = [&](int k) { put(S.pool + E.off[k], E.len[k]); };
-        lit(0); put(S.dec[d], gl); lit(1); put(reinterpret_cast<const uint8_t *>(r->device), dl);
-        lit(2); put(S.dec[d], gl);
-        if (nl) { lit(3); put(S.dec[d] + 10, nl); }
-        lit(4); put(reinterpret_cast<const uint8_t *>(r->bdf), bl);
-        if (pl) { lit(5); put(r->product, pl); }
-        if (rl) { lit(6); put(reinterpret_cast<const uint8_t *>(r->pcie_root), rl); }
-        lit(7); put(reinterpret_cast<const uint8_t *>(r->vendor), vl); lit(8);
+        const auto bytes = [](const char *s) { return reinterpret_cast<const uint8_t *>(s); };
+        if constexpr (LAYOUT == LAYOUT_PCI) {
+            lit(0); put(S.dec[d], gl); lit(1); put(bytes(r->device), dl);
+            lit(2); put(S.dec[d], gl);
+            if (nl) { lit(3); put(S.dec[d] + 10, nl); }
+            lit(4); put(bytes(r->bdf), bl);
+            if (pl) { lit(5); put(r->product, pl); }
+            if (rl) { lit(6); put(bytes(r->pcie_root), rl); }
+            lit(7); put(bytes(r->vendor), vl); lit(8);
+        } else {
+            const uint32_t tl = S.tlen[d];
+            lit(0); put(S.dec[d], gl); lit(1); put(S.dec[d], gl); lit(DRAM_I);
+            lit(2); put(bytes(r->mdev_type), tl); lit(DRAM_S);
+            if (nl) { lit(3); put(S.dec[d] + 10, nl); lit(DRAM_I); }
+            lit(4); put(bytes(r->parent), bl); lit(DRAM_S);
+            if (dl) { lit(5); put(bytes(r->device), dl); lit(DRAM_S); }
+            lit(6); put(bytes(r->vendor), vl); lit(DRAM_S);
+            if (pl) { lit(7); put(r->product, pl); lit(DRAM_S); }
+            if (rl) { lit(8); put(bytes(r->pcie_root), rl); lit(DRAM_S); }
+            lit(9); put(bytes(r->uuid), 36u); lit(DRAM_S); lit(DRAM_E);
+        }
         if (d + 1u < in_slice && lane == 0) dst[o] = (uint8_t)',';
     }
     tile_store(E.out + base, stg, head_len + tile_total + tail_len);
@@ -882,20 +1018,27 @@ static bool dns_subdomain_ok(const char *s, size_t max) {
     return true;
 }
 
-extern "C" int32_t kxpu_dra_slices(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
-                                   const kxpu_dradev *devs, size_t n, uint8_t *out, size_t cap, size_t *len,
-                                   uint64_t *slice_off, size_t *n_slices) {
-    static_assert(sizeof(kxpu_dradev) == 128 && offsetof(kxpu_dradev, numa_mask) == 112 &&
-                      offsetof(kxpu_dradev, product_len) == 124, "kxpu_dradev layout");
+// kxpu_dra_slices / kxpu_dra_slices_mdev: the argument checks, the pool (literals | head | tail), one k_dra_slices<LAYOUT>
+// launch, the domain flags and the copies
+template <int LAYOUT>
+static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, const char *pool, const char *node,
+                          uint64_t generation, const typename DraLayout<LAYOUT>::Rec *devs, size_t n, uint8_t *out, size_t cap,
+                          size_t *len, uint64_t *slice_off, size_t *n_slices) {
+    using Rec = typename DraLayout<LAYOUT>::Rec;
+    constexpr int PARTS = DraLayout<LAYOUT>::PARTS, HEAD = PARTS - 2, TAIL = PARTS - 1;
+    constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : DRAM_LITS;
+    constexpr int MAXF = LAYOUT == LAYOUT_PCI ? MAX_FRAG_DRA : MAX_FRAG_DRA_MDEV;
+    constexpr int F_COUNT = LAYOUT == LAYOUT_PCI ? DRA_F_COUNT : DRAM_F_COUNT;
+    const char *const *lits = LAYOUT == LAYOUT_PCI ? h_dra_lits : h_dram_lits;
     if (!ctx || !len || !n_slices || (n && !devs)) return KXPU_E_INVALID;
     if (!dns_subdomain_ok(driver, 63) || !dns_subdomain_ok(pool, 253) || !dns_subdomain_ok(node, 253) ||
         generation >= (1ull << 63)) {
-        KX_SET_ERR(ctx, "dra_slices: driver (<= 63 bytes), pool and node (<= 253 bytes) must be lowercase DNS subdomains "
-                        "and generation below 2^63");
+        KX_SET_ERR(ctx, "%s: driver (<= 63 bytes), pool and node (<= 253 bytes) must be lowercase DNS subdomains "
+                        "and generation below 2^63", what);
         return KXPU_E_INVALID;
     }
     if (n >= KXPU_DRA_MAX_DEVICES) {
-        KX_SET_ERR(ctx, "dra_slices: n = %zu is not below %u", n, KXPU_DRA_MAX_DEVICES);
+        KX_SET_ERR(ctx, "%s: n = %zu is not below %u", what, n, KXPU_DRA_MAX_DEVICES);
         return KXPU_E_UNSUPPORTED;
     }
     std::lock_guard<std::mutex> guard(ctx->mu);
@@ -908,11 +1051,11 @@ extern "C" int32_t kxpu_dra_slices(kxpu_ctx *ctx, const char *driver, const char
                              "\",\"generation\":" + std::to_string(generation) +
                              ",\"resourceSliceCount\":" + std::to_string(slices) + "},\"nodeName\":\"" + nd +
                              "\",\"devices\":[";
-    DraParams E;
+    DraParams<PARTS> E;
     memset(&E, 0, sizeof E);
     uint32_t acc = 0;
-    for (int k = 0; k < DRA_PARTS; k++) {
-        const std::string s = k < 9 ? std::string(h_dra_lits[k]) : k == DRA_HEAD ? head : std::string(KX_DRA_TAIL);
+    for (int k = 0; k < PARTS; k++) {
+        const std::string s = k < LITS ? std::string(lits[k]) : k == HEAD ? head : std::string(KX_DRA_TAIL);
         if (acc + s.size() > (size_t)DRA_POOL_MAX) return KXPU_E_INVALID;  // the literals grew: DRA_POOL_MAX must follow
         memcpy(E.pool + acc, s.data(), s.size());
         E.off[k] = (uint16_t)acc;
@@ -920,21 +1063,22 @@ extern "C" int32_t kxpu_dra_slices(kxpu_ctx *ctx, const char *driver, const char
         acc += E.len[k];
     }
     E.pool_len = acc;
-    const size_t bound = (size_t)slices * (E.len[DRA_HEAD] + E.len[DRA_TAIL]) + (size_t)n * MAX_FRAG_DRA + 64;
+    const size_t bound = (size_t)slices * (E.len[HEAD] + E.len[TAIL]) + (size_t)n * MAXF + 64;
+    const size_t smem = sizeof(typename DraLayout<LAYOUT>::Smem);
     static bool attr_done = false;
     if (!attr_done) {
-        cudaFuncSetAttribute(k_dra_slices, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(DraSmem));
+        cudaFuncSetAttribute(k_dra_slices<LAYOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         attr_done = true;
     }
     KxScratch sc(ctx);
-    kxpu_dradev *d_devs = nullptr;
+    Rec *d_devs = nullptr;
     uint8_t *d_out = nullptr;
-    unsigned long long *d_ctl = nullptr;  // slice_off [slices + 1] | DRA_F_COUNT flag words
-    const size_t ctl_words = slices + 1 + (DRA_F_COUNT + 1) / 2;
-    KX_CUDA(ctx, sc.alloc((void **)&d_devs, n * sizeof(kxpu_dradev)));
+    unsigned long long *d_ctl = nullptr;  // slice_off [slices + 1] | F_COUNT flag words
+    const size_t ctl_words = slices + 1 + (F_COUNT + 1) / 2;
+    KX_CUDA(ctx, sc.alloc((void **)&d_devs, n * sizeof(Rec)));
     KX_CUDA(ctx, sc.alloc((void **)&d_out, bound));
     KX_CUDA(ctx, sc.alloc((void **)&d_ctl, ctl_words * 8));
-    if (n) cudaMemcpyAsync(d_devs, devs, n * sizeof(kxpu_dradev), cudaMemcpyHostToDevice, ctx->stream);
+    if (n) cudaMemcpyAsync(d_devs, devs, n * sizeof(Rec), cudaMemcpyHostToDevice, ctx->stream);
     cudaMemsetAsync(d_ctl + slices + 1, 0, (ctl_words - slices - 1) * 8, ctx->stream);
     E.devs = d_devs; E.n = N; E.out = d_out; E.slice_off = d_ctl; E.flags = (uint32_t *)(d_ctl + slices + 1);
     E.state = kx_scan_state(ctx, slices);
@@ -942,27 +1086,54 @@ extern "C" int32_t kxpu_dra_slices(kxpu_ctx *ctx, const char *driver, const char
     E.epoch = kx_next_epoch(ctx);
     {
         KxTimer tm(ctx, KXPU_T_EMIT);
-        k_dra_slices<<<slices, EMIT_THREADS, sizeof(DraSmem), ctx->stream>>>(E);
+        k_dra_slices<LAYOUT><<<slices, EMIT_THREADS, smem, ctx->stream>>>(E);
         KX_LAUNCHED(ctx);
     }
     std::vector<unsigned long long> h(ctl_words);
     cudaMemcpyAsync(h.data(), d_ctl, ctl_words * 8, cudaMemcpyDeviceToHost, ctx->stream);
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { KX_SET_ERR(ctx, "dra_slices failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
-    static const char *const why[DRA_F_COUNT] = {
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "%s failed: %s", what, cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    static const char *const why_pci[DRA_F_COUNT] = {
         "a product byte outside [A-Za-z0-9_.-]", "a bdf that is empty or holds a byte outside [0-9a-f:.]",
         "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
         "a device id that is not 1..6 bytes of [0-9a-f]", "iommu_group 4294967295", "product_len above 64"};
+    static const char *const why_mdev[DRAM_F_COUNT] = {
+        "a product byte outside [A-Za-z0-9_.-]", "an mdev_type that is empty or holds a byte outside [A-Za-z0-9_.-]",
+        "a uuid outside the canonical lowercase 8-4-4-4-12 form", "a parent that is empty or holds a byte outside [0-9a-f:.]",
+        "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
+        "a device id that is not 0..6 bytes of [0-9a-f]", "iommu_group 4294967295", "product_len above 64"};
+    const char *const *why = LAYOUT == LAYOUT_PCI ? why_pci : why_mdev;
     const uint32_t *flags = reinterpret_cast<const uint32_t *>(h.data() + slices + 1);
-    for (int f = 0; f < DRA_F_COUNT; f++)
-        if (flags[f]) { KX_SET_ERR(ctx, "dra_slices: %s", why[f]); return KXPU_E_UNSUPPORTED; }
+    for (int f = 0; f < F_COUNT; f++)
+        if (flags[f]) { KX_SET_ERR(ctx, "%s: %s", what, why[f]); return KXPU_E_UNSUPPORTED; }
     const size_t total = (size_t)h[slices];
     *len = total;
     *n_slices = slices;
     if (cap < total || !out) return KXPU_E_NOSPACE;
     cudaMemcpyAsync(out, d_out, total, cudaMemcpyDeviceToHost, ctx->stream);
     e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) { KX_SET_ERR(ctx, "dra_slices D2H failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "%s D2H failed: %s", what, cudaGetErrorString(e)); return KXPU_E_CUDA; }
     if (slice_off) memcpy(slice_off, h.data(), (slices + 1) * sizeof(uint64_t));
     return KXPU_OK;
+}
+
+extern "C" int32_t kxpu_dra_slices(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                                   const kxpu_dradev *devs, size_t n, uint8_t *out, size_t cap, size_t *len,
+                                   uint64_t *slice_off, size_t *n_slices) {
+    static_assert(sizeof(kxpu_dradev) == 128 && offsetof(kxpu_dradev, numa_mask) == 112 &&
+                      offsetof(kxpu_dradev, product_len) == 124, "kxpu_dradev layout");
+    return dra_slices<LAYOUT_PCI>(ctx, "dra_slices", driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
+}
+
+extern "C" int32_t kxpu_dra_slices_mdev(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                        uint64_t generation, const kxpu_dramdev *devs, size_t n, uint8_t *out, size_t cap,
+                                        size_t *len, uint64_t *slice_off, size_t *n_slices) {
+    static_assert(sizeof(kxpu_dramdev) == 208 && alignof(kxpu_dramdev) == 8 && offsetof(kxpu_dramdev, mdev_type) == 64 &&
+                      offsetof(kxpu_dramdev, uuid) == 104 && offsetof(kxpu_dramdev, iommu_group) == 140 &&
+                      offsetof(kxpu_dramdev, parent) == 144 && offsetof(kxpu_dramdev, pcie_root) == 160 &&
+                      offsetof(kxpu_dramdev, vendor) == 176 && offsetof(kxpu_dramdev, numa_mask) == 192 &&
+                      offsetof(kxpu_dramdev, product_len) == 200,
+                  "kxpu_dramdev layout");
+    return dra_slices<LAYOUT_MDEV>(ctx, "dra_slices_mdev", driver, pool, node, generation, devs, n, out, cap, len, slice_off,
+                                   n_slices);
 }

@@ -604,9 +604,20 @@ static std::string blockerOf(const kxpu_devrec &r) {
     return std::string(r.bdf, strnlen(r.bdf, sizeof r.bdf)) + " is bound to " + std::string(r.driver, strnlen(r.driver, sizeof r.driver));
 }
 
-// the ResourceSlice record of a group (product left empty): bdf, vendor and device of its first member r, the first
-// component of r's path when it is "pci" followed by 1..13 bytes of [0-9a-f:] (anything else leaves the root unknown), and
-// the group's NUMA mask
+// the PCIe root of a kxpu_pcipath: its first component when that is "pci" followed by 1..13 bytes of [0-9a-f:]; "" for
+// anything else (unknown)
+static std::string pcieRootOf(const kxpu_pcipath *path) {
+    if (!path || path->len == 0 || path->len > sizeof path->path) return std::string();
+    const std::string p(path->path, path->len);
+    const std::string root = p.substr(0, p.find('/'));
+    bool ok = root.size() >= 4 && root.size() <= sizeof(kxpu_dradev::pcie_root) && root.compare(0, 3, "pci") == 0;
+    for (size_t k = 3; ok && k < root.size(); k++)
+        ok = (root[k] >= '0' && root[k] <= '9') || (root[k] >= 'a' && root[k] <= 'f') || root[k] == ':';
+    return ok ? root : std::string();
+}
+
+// the ResourceSlice record of a group (product left empty): bdf, vendor and device of its first member r, the PCIe root
+// of r's path (pcieRootOf), and the group's NUMA mask
 static kxpu_dradev draRecord(const kxpu_devrec &r, const kxpu_pcipath *path, uint64_t numa) {
     kxpu_dradev d;
     memset(&d, 0, sizeof d);
@@ -615,14 +626,8 @@ static kxpu_dradev draRecord(const kxpu_devrec &r, const kxpu_pcipath *path, uin
     const std::string device = trimID(std::string((const char *)r.device_txt, std::min<size_t>(r.device_len, sizeof r.device_txt)));
     memcpy(d.vendor, vendor.data(), std::min(vendor.size(), sizeof d.vendor));
     memcpy(d.device, device.data(), std::min(device.size(), sizeof d.device));
-    if (path && path->len > 0 && path->len <= sizeof path->path) {
-        const std::string p(path->path, path->len);
-        const std::string root = p.substr(0, p.find('/'));
-        bool ok = root.size() >= 4 && root.size() <= sizeof d.pcie_root && root.compare(0, 3, "pci") == 0;
-        for (size_t k = 3; ok && k < root.size(); k++)
-            ok = (root[k] >= '0' && root[k] <= '9') || (root[k] >= 'a' && root[k] <= 'f') || root[k] == ':';
-        if (ok) memcpy(d.pcie_root, root.data(), root.size());
-    }
+    const std::string root = pcieRootOf(path);
+    memcpy(d.pcie_root, root.data(), root.size());
     d.numa_mask = numa;
     d.iommu_group = r.iommu_group;
     return d;
@@ -775,7 +780,7 @@ static void mdevRecord(Plugin &p, const std::string &name, bool isDir, kxpu_mdev
     if (!p.readLink(p.mdevBasePath, name, "iommu_group", s) || !parseGroup(s, g)) { r.flags |= KXPU_REC_IOMMU_ERR; return; }
     r.iommu_group = g;
     // the parent's node; read before the name, since a record without a name can still join an existing group
-    if (p.topologyAware) numaRecord([&](std::string &out) { return p.readNumaNode(p.mdevBasePath, name + "/..", out); }, r.flags, r.numa_node);
+    if (p.readsMdevNuma()) numaRecord([&](std::string &out) { return p.readNumaNode(p.mdevBasePath, name + "/..", out); }, r.flags, r.numa_node);
     if (!p.readIDFromFile(p.mdevBasePath, name, "mdev_type/name", s) || s.size() > sizeof r.type_name) {
         r.flags |= KXPU_REC_NAME_ERR;
         return;
@@ -786,8 +791,10 @@ static void mdevRecord(Plugin &p, const std::string &name, bool isDir, kxpu_mdev
 
 // The entries of mdevBasePath in lexical order (filepath.Walk's order for the PCI walk).  The mdev bus directory only
 // holds one level of links, so a directory inside it is recorded as such and not descended into.
-Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs) {
+Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w) {
     recs.clear();
+    if (w) { w->parentDevice.clear(); w->pcieRoot.clear(); }
+    if (!vgpuDraEnabled()) w = nullptr;
     DIR *d = opendir(mdevBasePath.c_str());
     if (!d) return fail("Error accessing file path \"" + mdevBasePath + "\": " + strerror(errno));
     std::vector<std::string> names;
@@ -803,6 +810,24 @@ Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs) {
         kxpu_mdevrec r;
         mdevRecord(*this, n, isDir, r);
         recs.push_back(r);
+        if (!w) continue;
+        // the ResourceSlice reads of an entry that got as far as its iommu_group link
+        std::string dev, target;
+        const bool grouped = !isDir && n.size() == sizeof r.uuid &&
+                             !(r.flags & (KXPU_REC_VENDOR_ERR | KXPU_REC_DRIVER_ERR | KXPU_REC_IOMMU_ERR));
+        if (grouped && readIDFromFile(mdevBasePath, n, "../device", dev)) {
+            dev = trimID(dev);
+            bool ok = dev.size() <= 6;
+            for (char c : dev) ok = ok && ((c >= '0' && c <= '9') || (c >= 'a' && c <= 'f'));
+            if (!ok) dev.clear();
+        } else {
+            dev.clear();
+        }
+        kxpu_pcipath pp;
+        memset(&pp, 0, sizeof pp);
+        if (grouped && readPciPath(mdevBasePath, n, target)) pciPathRecord(target, pp);
+        w->parentDevice.push_back(dev);
+        w->pcieRoot.push_back(pcieRootOf(&pp));
     }
     return Error();
 }
@@ -841,16 +866,17 @@ Error Plugin::createMdevMap() {
 }
 
 Error Plugin::classifyMdev(MdevWalk &w) {
-    Error e = gatherMdevRecords(w.recs);
+    Error e = gatherMdevRecords(w.recs, &w);
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // like the PCI walk: an unreadable bus is an empty one
     const std::vector<kxpu_mdevrec> &recs = w.recs;
     const size_t n = recs.size();
     ClassifyResult &c = w.out;
     kxpu_classify_out out = c.wire(n);
     const std::vector<kxpu_xpu_rule> rules = classRules(vgpuClasses);
-    int32_t rc = topologyAware ? kxpu_classify_mdev_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(), c.gnuma.data())
-                               : kxpu_classify_mdev(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data());
-    if (rc != KXPU_OK) return kxfail(ctx_, topologyAware ? "kxpu_classify_mdev_topo" : "kxpu_classify_mdev", rc);
+    const bool topo = readsMdevNuma();
+    int32_t rc = topo ? kxpu_classify_mdev_topo(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(), c.gnuma.data())
+                      : kxpu_classify_mdev(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data());
+    if (rc != KXPU_OK) return kxfail(ctx_, topo ? "kxpu_classify_mdev_topo" : "kxpu_classify_mdev", rc);
     c.nGroups = out.n_groups;
     c.nDevids = out.n_devids;
     std::vector<uint32_t> first(out.n_devids);
@@ -891,6 +917,55 @@ void Plugin::buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index
         for (uint32_t k = c.doff[d]; k < c.doff[d + 1]; k++) groups.push_back(std::to_string(c.dgrp[k]));
         typeMap.emplace_back(std::string((const char *)w.keys.data() + w.koff[d], w.koff[d + 1] - w.koff[d]), std::move(groups));
         typeClass.push_back(c.drule[d]);
+    }
+    buildMdevDra(w);
+}
+
+// mdevDra of a walk (vgpuDraEnabled only): one kxpu_dramdev per group from its first mdev; the parents' model names come
+// from one getDeviceNames call over the distinct (vendor, device) ids
+void Plugin::buildMdevDra(const MdevWalk &w) {
+    mdevDra.clear();
+    if (!vgpuDraEnabled()) return;
+    const ClassifyResult &c = w.out;
+    std::map<uint32_t, std::string> keyOf;  // group id -> type key of its device-map entry
+    for (uint32_t d = 0; d < c.nDevids; d++)
+        for (uint32_t k = c.doff[d]; k < c.doff[d + 1]; k++)
+            keyOf[c.dgrp[k]] = std::string((const char *)w.keys.data() + w.koff[d], w.koff[d + 1] - w.koff[d]);
+    std::map<std::pair<std::string, std::string>, size_t> idAt;  // (vendor, device) -> position in the lookup batch
+    std::vector<std::string> ids, vendors;
+    std::vector<std::pair<std::string, std::string>> idOf;  // per group
+    for (uint32_t g = 0; g < c.nGroups; g++) {
+        const uint32_t first = c.gmem[c.goff[g]];
+        const kxpu_mdevrec &r = w.recs[first];
+        kxpu_dramdev d;
+        memset(&d, 0, sizeof d);
+        const std::string key = keyOf[c.gids[g]];
+        memcpy(d.mdev_type, key.data(), std::min(key.size(), sizeof d.mdev_type));
+        memcpy(d.uuid, r.uuid, sizeof d.uuid);
+        d.iommu_group = r.iommu_group;
+        memcpy(d.parent, r.parent, strnlen(r.parent, sizeof r.parent));
+        const std::string vendor = trimID(std::string((const char *)r.parent_vendor_txt, std::min<size_t>(r.vendor_len, sizeof r.parent_vendor_txt)));
+        memcpy(d.vendor, vendor.data(), std::min(vendor.size(), sizeof d.vendor));
+        const std::string device = first < w.parentDevice.size() ? w.parentDevice[first] : std::string();
+        memcpy(d.device, device.data(), std::min(device.size(), sizeof d.device));
+        const std::string root = first < w.pcieRoot.size() ? w.pcieRoot[first] : std::string();
+        memcpy(d.pcie_root, root.data(), std::min(root.size(), sizeof d.pcie_root));
+        d.numa_mask = c.gnuma.size() > g ? c.gnuma[g] : 0;
+        mdevDra.push_back(d);
+        idOf.emplace_back(vendor, device);
+        if (!device.empty() && idAt.emplace(idOf.back(), ids.size()).second) {
+            ids.push_back(device);
+            vendors.push_back(vendor);
+        }
+    }
+    const std::vector<std::string> names = ids.empty() ? std::vector<std::string>() : getDeviceNames(ids, vendors);
+    for (size_t g = 0; g < mdevDra.size(); g++) {
+        if (idOf[g].second.empty()) continue;  // no device id: no productName
+        const std::string &name = names[idAt[idOf[g]]];
+        const std::string &product = name.empty() ? idOf[g].second : name;
+        kxpu_dramdev &d = mdevDra[g];
+        d.product_len = (uint8_t)std::min(product.size(), sizeof d.product);
+        memcpy(d.product, product.data(), d.product_len);
     }
 }
 
@@ -1247,13 +1322,24 @@ bool Plugin::draEnabled() const {
     return false;
 }
 
+bool Plugin::vgpuDraEnabled() const {
+    for (const XpuClass &c : vgpuClasses)
+        if (!c.draDriver.empty()) return true;
+    return false;
+}
+
+// DRA drivers are distinct across xpuClasses and vgpuClasses (a passthrough class is named by its position, a vGPU
+// class by "vGPU <position>"), and a node name is required when any class has one
 Error Plugin::checkDraClasses() const {
-    for (size_t c = 0; c < xpuClasses.size(); c++) {
-        const std::string &d = xpuClasses[c].draDriver;
+    std::vector<std::pair<const std::string *, std::string>> all;  // (driver, class name)
+    for (size_t c = 0; c < xpuClasses.size(); c++) all.emplace_back(&xpuClasses[c].draDriver, std::to_string(c));
+    for (size_t c = 0; c < vgpuClasses.size(); c++) all.emplace_back(&vgpuClasses[c].draDriver, "vGPU " + std::to_string(c));
+    for (size_t c = 0; c < all.size(); c++) {
+        const std::string &d = *all[c].first;
         if (d.empty()) continue;
         if (nodeName.empty()) return fail("DRA driver " + d + " is set but the node name is empty (NODE_NAME)");
         for (size_t k = 0; k < c; k++)
-            if (xpuClasses[k].draDriver == d) return fail("DRA driver " + d + " is set on two classes (" + std::to_string(k) + " and " + std::to_string(c) + ")");
+            if (*all[k].first == d) return fail("DRA driver " + d + " is set on two classes (" + all[k].second + " and " + all[c].second + ")");
     }
     return Error();
 }
@@ -1378,9 +1464,10 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         report.changedPlugins.push_back(k);
     }
     std::sort(report.changedPlugins.begin(), report.changedPlugins.end());
-    bool passthroughChanged = false;
-    for (size_t k : report.changedPlugins) passthroughChanged |= !devicePlugins[k].vgpu;
+    bool passthroughChanged = false, vgpuChanged = false;
+    for (size_t k : report.changedPlugins) (devicePlugins[k].vgpu ? vgpuChanged : passthroughChanged) = true;
     if (passthroughChanged || viabilityChanged) draGeneration_++;  // the ResourceSlices of the next publication replace these
+    if (vgpuChanged) draVgpuGeneration_++;
     // 6. a fresh snapshot generation: Allocate answers from the snapshot again
     haveWalkGen_ = haveGen;
     walkGen_ = gen;
@@ -1503,22 +1590,51 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
     return Error();
 }
 
+Error Plugin::VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) {
+    std::shared_lock<std::shared_mutex> lock(mu_);
+    if (vgpuClass >= vgpuClasses.size() || vgpuClasses[vgpuClass].draDriver.empty())
+        return fail("VgpuResourceSlices: vGPU class " + std::to_string(vgpuClass) + " has no DRA driver");
+    const std::string &driver = vgpuClasses[vgpuClass].draDriver;
+    std::vector<kxpu_dramdev> devs;
+    for (size_t g = 0; g < mdevMap.size() && g < mdevDra.size() && g < mdevClass.size(); g++)
+        if (mdevClass[g] == vgpuClass) devs.push_back(mdevDra[g]);
+    size_t len = 0, nSlices = 0;
+    int32_t rc = kxpu_dra_slices_mdev(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), draVgpuGeneration_, devs.data(),
+                                      devs.size(), nullptr, 0, &len, nullptr, &nSlices);
+    if (rc == KXPU_E_NOSPACE) {
+        out.assign(len, 0);
+        sliceOff.assign(nSlices + 1, 0);
+        rc = kxpu_dra_slices_mdev(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), draVgpuGeneration_, devs.data(),
+                                  devs.size(), out.data(), out.size(), &len, sliceOff.data(), &nSlices);
+    }
+    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_dra_slices_mdev", rc);
+    return Error();
+}
+
 Error Plugin::PrepareDraDevices(const std::string &driver, const std::string &pool, const std::vector<std::string> &deviceNames,
                                 std::vector<std::vector<std::string>> &cdiIds) {
     std::vector<std::string> groups;
     {
         std::shared_lock<std::shared_mutex> lock(mu_);  // Allocate takes it again below
-        size_t cls = xpuClasses.size();
+        size_t cls = xpuClasses.size(), vcls = vgpuClasses.size();
         for (size_t c = 0; c < xpuClasses.size(); c++)
             if (!driver.empty() && xpuClasses[c].draDriver == driver) cls = c;
-        if (cls == xpuClasses.size()) return fail("PrepareDraDevices: unknown DRA driver " + driver);
+        for (size_t c = 0; c < vgpuClasses.size(); c++)
+            if (!driver.empty() && vgpuClasses[c].draDriver == driver) vcls = c;
+        const bool vgpu = vcls < vgpuClasses.size();
+        if (cls == xpuClasses.size() && !vgpu) return fail("PrepareDraDevices: unknown DRA driver " + driver);
         if (pool != nodeName) return fail("PrepareDraDevices: unknown pool " + pool + " of driver " + driver);
         for (const std::string &name : deviceNames) {
             const std::string g = name.compare(0, 4, "vfio") == 0 ? name.substr(4) : std::string();
-            size_t at = iommuMap.size();
-            for (size_t k = 0; k < iommuMap.size(); k++)
-                if (!g.empty() && iommuMap[k].first == g && iommuClass[k] == cls) at = k;
-            if (at == iommuMap.size()) return fail("PrepareDraDevices: unknown device " + name + " in pool " + pool);
+            bool found = false;
+            if (vgpu) {
+                for (size_t k = 0; k < mdevMap.size() && k < mdevClass.size(); k++)
+                    found |= !g.empty() && mdevMap[k].first == g && mdevClass[k] == vcls;
+            } else {
+                for (size_t k = 0; k < iommuMap.size(); k++)
+                    found |= !g.empty() && iommuMap[k].first == g && iommuClass[k] == cls;
+            }
+            if (!found) return fail("PrepareDraDevices: unknown device " + name + " in pool " + pool);
             groups.push_back(g);
         }
     }
@@ -2369,6 +2485,48 @@ int kxh_prepare_dra(void *h, const char *driver, const char *pool, const char *n
         o += ']';
     }
     return copy_out(o + "]", json, cap);
+}
+
+// ---- DRA ResourceSlices of vGPUs (ABI v10)
+// draDriver of every vGPU class from a comma separated list (position = vGPU class; "" = not published), and the node name
+int kxh_set_vgpu_dra(void *h, const char *drivers_csv, const char *node_name) {
+    Plugin *p = (Plugin *)h;
+    std::string all(drivers_csv);
+    size_t c = 0, a = 0;
+    for (;;) {
+        const size_t comma = all.find(',', a);
+        if (c >= p->vgpuClasses.size()) return -1;
+        p->vgpuClasses[c++].draDriver = all.substr(a, comma == std::string::npos ? std::string::npos : comma - a);
+        if (comma == std::string::npos) break;
+        a = comma + 1;
+    }
+    p->nodeName = node_name;
+    return 0;
+}
+// VgpuResourceSlices of one vGPU class, answered like kxh_resource_slices
+int kxh_vgpu_resource_slices(void *h, int cls, uint8_t *out, size_t cap, size_t *len, uint64_t *offs, size_t offcap,
+                             size_t *n_slices) {
+    std::vector<uint8_t> o;
+    std::vector<uint64_t> so;
+    device_plugin::Error e = ((Plugin *)h)->VgpuResourceSlices((size_t)cls, o, so);
+    if (e) { copy_out(e.message, (char *)out, cap); return -1; }
+    *len = o.size();
+    *n_slices = so.size() - 1;
+    if (o.size() > cap || so.size() > offcap) return -2;
+    memcpy(out, o.data(), o.size());
+    memcpy(offs, so.data(), so.size() * sizeof(uint64_t));
+    return 0;
+}
+uint64_t kxh_dra_vgpu_generation(void *h) { return ((Plugin *)h)->draVgpuGeneration(); }
+// a counting seam on readIDFromFile: every read of the file `prop` (e.g. "../device") is counted
+void kxh_count_id_reads(void *h, const char *prop, uint64_t *reads) {
+    Plugin *p = (Plugin *)h;
+    auto di = p->readIDFromFile;
+    const std::string want(prop);
+    p->readIDFromFile = [di, want, reads](const std::string &base, const std::string &addr, const std::string &pr, std::string &out) {
+        if (pr == want) (*reads)++;
+        return di(base, addr, pr, out);
+    };
 }
 
 }  // extern "C"

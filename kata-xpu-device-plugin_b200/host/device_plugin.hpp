@@ -163,8 +163,8 @@ struct XpuClass {
     std::string resourceNamespace;  // resource = <resourceNamespace>/<device name>
     std::string cdiKind;            // CDI kind of this class's spec file and Allocate names
     std::string cdiFileStem;        // <cdiConfigPath><cdiFileStem>.yaml|.json
-    // DRA driver name that publishes this class's IOMMU groups as ResourceSlices (Plugin::ResourceSlices); empty: the
-    // class is not published
+    // DRA driver name that publishes this class's IOMMU groups as ResourceSlices (Plugin::ResourceSlices, or
+    // Plugin::VgpuResourceSlices for a vGPU class); empty: the class is not published
     std::string draDriver{};
 };
 XpuClass defaultXpuClass();  // {"10de", "vfio-pci", "nvidia.com", "nvidia.com/gpu", "cdi-vfio-xxxx"}
@@ -207,6 +207,9 @@ struct MdevWalk {
     ClassifyResult out;
     std::vector<uint32_t> koff;
     std::vector<uint8_t> keys;
+    // vgpuDraEnabled only, one per record: the parent's device id (<uuid>/../device) and the PCIe root of the entry's
+    // link; "" = not read, failed or outside kxpu_dramdev's domain
+    std::vector<std::string> parentDevice, pcieRoot;
 };
 
 class Plugin {
@@ -272,6 +275,12 @@ class Plugin {
     // the PCI gathers read numa_node (topologyAware or draEnabled) and the entry link (pcieTopologyAware or draEnabled)
     bool readsNuma() const { return topologyAware || draEnabled(); }
     bool readsPaths() const { return pcieTopologyAware || draEnabled(); }
+    // DRA ResourceSlices of vGPUs (ABI v10): a draDriver on a vGPU class publishes its groups (VgpuResourceSlices) in
+    // the pool nodeName.  With one set, the mdev walk also reads, for every entry that got as far as its iommu_group
+    // link, the parent's numa_node (as topologyAware does), the entry's link (readPciPath) and <uuid>/../device; a failed
+    // read only leaves out its attribute.  The PCI walk and every device-plugin output stay as they are.
+    bool vgpuDraEnabled() const;  // some vGPU class has a draDriver
+    bool readsMdevNuma() const { return topologyAware || vgpuDraEnabled(); }
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
 
     // ---- state (device_plugin.go:31,34)
@@ -297,6 +306,8 @@ class Plugin {
     OrderedMap<std::vector<std::string>> typeMap;
     std::vector<size_t> mdevClass, typeClass;
     std::vector<std::string> mdevCdiFiles;  // files the last generateMdevCDISpec wrote, one per vGPU class
+    // vgpuDraEnabled only: the ResourceSlice record of every mdevMap entry (from its first mdev)
+    std::vector<kxpu_dramdev> mdevDra;
 
     explicit Plugin(kxpu_ctx *ctx);
     ~Plugin();
@@ -348,9 +359,18 @@ class Plugin {
     // the pool generation of every class's ResourceSlices: 1 after start-up, +1 for each rediscover that changed a
     // passthrough plugin or a group's viability
     uint64_t draGeneration() const { return draGeneration_; }
+    // The ResourceSlices of vGPU class vgpuClass (kxpu_dra_slices_mdev): one pool named nodeName, one device per mdevMap
+    // group of the class in walk order, described by the group's first mdev: its type key, UUID, parent address, the
+    // parent's vendor and device ids, the PCIe root of its link, the group's NUMA mask, and the parent's model name
+    // (getDeviceNames: the sanitised pci.ids name, else the raw device id; cut to 64 bytes) as productName.
+    Error VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff);
+    // the pool generation of every vGPU class's ResourceSlices: 1 after start-up, +1 for each rediscover that changed a
+    // vGPU plugin
+    uint64_t draVgpuGeneration() const { return draVgpuGeneration_; }
     // The data half of NodePrepareResources: cdiIds[i] = the CDI names Allocate({g}) returns for deviceNames[i] =
-    // "vfio<g>", a device of the pool `pool` of the class whose draDriver is `driver` (same live or snapshot
-    // re-validation, same viability refusal).  An unknown driver, pool or device is an error that names it.
+    // "vfio<g>", a device of the pool `pool` of the class (passthrough or vGPU) whose draDriver is `driver` (same live or
+    // snapshot re-validation, same viability refusal; a vGPU group is always re-read live).  An unknown driver, pool or
+    // device is an error that names it.
     Error PrepareDraDevices(const std::string &driver, const std::string &pool, const std::vector<std::string> &deviceNames,
                             std::vector<std::vector<std::string>> &cdiIds);
 
@@ -368,8 +388,9 @@ class Plugin {
     // the same records, read with openat / readlinkat relative to basePath by several threads
     // (SURVEY 8(f) row 2); falls back to gatherRecords when a seam was replaced.  threads = 0: automatic
     Error gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads = 0, std::vector<kxpu_pcipath> *paths = nullptr);
-    // raw gather of mdevBasePath under vgpuClasses (no GPU): one record per entry, lexical order
-    Error gatherMdevRecords(std::vector<kxpu_mdevrec> &recs);
+    // raw gather of mdevBasePath under vgpuClasses (no GPU): one record per entry, lexical order.  w (vgpuDraEnabled
+    // only, else left empty): the walk's parentDevice and pcieRoot, one per record
+    Error gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w = nullptr);
 
   private:
     kxpu_ctx *ctx_;
@@ -404,8 +425,9 @@ class Plugin {
     BindWatcher bindWatcher_;
     bool haveSnapshotGen_ = false;
     uint64_t snapshotGen_ = 0;
-    uint64_t draGeneration_ = 1;
+    uint64_t draGeneration_ = 1, draVgpuGeneration_ = 1;
     Error checkDraClasses() const;
+    void buildMdevDra(const MdevWalk &w);
 };
 
 }  // namespace device_plugin

@@ -585,3 +585,26 @@ def dra_devices(n=1 << 16, seed=41):
     d["numa_mask"] = np.left_shift(np.uint64(1), (i % 8).astype(np.uint64))
     d["iommu_group"] = 100000000 + i
     return d
+
+
+def dra_mdev_devices(n=1 << 16, seed=43):
+    """n published vGPUs with every optional attribute present and the longest fields the host produces: a 64-byte
+    product name, a 40-byte type key, a 12-byte parent address, a 10-byte PCIe root, 4-digit ids, one NUMA node, 9-digit
+    groups"""
+    from .binding import DRAMDEV_DTYPE
+    rng = np.random.default_rng(seed)
+    d = np.zeros(n, DRAMDEV_DTYPE)
+    alnum = np.frombuffer(b"ABCDEFGHIJKLMNOPQRSTUVWXYZ0123456789_", np.uint8)
+    d["product"] = alnum[rng.integers(0, len(alnum), (n, 64))]
+    d["product_len"] = 64
+    d["mdev_type"] = b"NVIDIA_H100XM-1-10C_with_a_long_type.key"
+    i = np.arange(n)
+    d["uuid"] = [b"%08x-%04x-4%03x-8%03x-%012x" % (k, k & 0xffff, k & 0xfff, (k >> 12) & 0xfff, (k * 2654435761) & (1 << 48) - 1)
+                 for k in range(n)]
+    par = i >> 4  # sixteen vGPUs per parent
+    d["parent"] = [b"%04x:%02x:%02x.%d" % (k >> 13, (k >> 5) & 0xff, (k >> 3) & 0x1f, k & 7) for k in par.tolist()]
+    d["pcie_root"] = [b"pci%04x:%02x" % (k >> 13, (k >> 5) & 0xff) for k in par.tolist()]
+    d["vendor"], d["device"] = b"10de", b"2330"
+    d["numa_mask"] = np.left_shift(np.uint64(1), (par % 8).astype(np.uint64))
+    d["iommu_group"] = 100000000 + i
+    return d

@@ -46,6 +46,10 @@ for topo in (False, True):
 for dn_ in (3000, 0):
     blob, soff = kx.dra_slices("vfio.nvidia.com", "node-a", "node-a", 1, W.dra_devices(dn_))
     print("dra slices", len(soff) - 1, "bytes", len(blob))
+# the vGPU layout of the same kernel: 24 slices and the empty pool
+for dn_ in (3000, 0):
+    blob, soff = kx.dra_slices_mdev("vgpu.nvidia.com", "node-a", "node-a", 1, W.dra_mdev_devices(dn_))
+    print("dra mdev slices", len(soff) - 1, "bytes", len(blob))
 
 
 # look-back state across epoch wraps (tests/test_gpu_lookback_state.py at reduced sizes): every user of the status
