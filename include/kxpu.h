@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 10
+#define KXPU_ABI_VERSION 11
 
 /* status codes */
 #define KXPU_OK             0
@@ -702,7 +702,8 @@ int32_t kxpu_lw_encode_topo(kxpu_ctx *ctx, const uint32_t *group_ids, const uint
  *             subdomains of at most 253 bytes;
  *   [assumed] resource.kubernetes.io/pcieRoot is the standard attribute that aligns devices of different drivers
  *             under one PCIe root complex;
- *   [assumed] v1 has no per-device health: a published device is schedulable. */
+ *   [assumed] without taints (ABI v11, below) a published device is schedulable: the v9 / v10 calls publish no
+ *             per-device health. */
 
 /* One published device (one IOMMU group of one class).  128 bytes: the kernel reads it with eight 16-byte loads. */
 typedef struct kxpu_dradev {
@@ -812,6 +813,52 @@ typedef struct kxpu_dramdev {
 int32_t kxpu_dra_slices_mdev(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
                              const kxpu_dramdev *devs, size_t n, uint8_t *out, size_t cap, size_t *len,
                              uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
+/* ------------------------------------------- DRA device taints (ABI v11) */
+
+/* A device that must not be allocated is published with a taint (KEP-5055), the DRA counterpart of ListAndWatch's
+ * Unhealthy.  These facts refine the list above; the "no per-device health" line there holds for the v9 / v10 calls,
+ * which never write taints:
+ *   [assumed] v1 Device has taints []DeviceTaint, declared after attributes.  The fields declared between them
+ *             (capacity, consumesCounters, nodeName, nodeSelector, allNodes) are never emitted here;
+ *   [assumed] DeviceTaint is key, value, effect, timeAdded in that order; effect is NoSchedule or NoExecute; a device
+ *             has at most 4 taints; the key is a qualified name and the value a label value;
+ *   [assumed] taints take effect only with the DRADeviceTaints feature gate.  With the gate off the API server drops
+ *             the field and the device looks untainted, which is what the v9 / v10 calls publish;
+ *   [assumed] a slice in which any device has taints lists at most 64 devices. */
+#define KXPU_DRA_TAINT_SLICE_DEVICES 64           /* devices per slice of the _taint calls with taint_since    */
+#define KXPU_DRA_TAINT_SINCE_MAX     253402300799ll /* 9999-12-31T23:59:59Z                                     */
+
+/* kxpu_dra_slices with at most one taint per device.  The contract is kxpu_dra_slices', with these additions:
+ *   - taint_since == NULL: the output, *len, slice_off and *n_slices are byte for byte kxpu_dra_slices'; the taint
+ *     arguments are not read.
+ *   - taint_since[i] < 0: device i has no taint.
+ *   - 0 <= taint_since[i] <= KXPU_DRA_TAINT_SINCE_MAX: device i carries one taint, a member after "attributes":
+ *       {"name":"vfio<g>","attributes":{...},"taints":[{"key":"<key>","value":"<value>","effect":"<effect>",
+ *        "timeAdded":"<YYYY-MM-DDTHH:MM:SSZ>"}]}
+ *     "value" is left out when taint_value is empty; timeAdded is taint_since[i] as RFC 3339 in UTC with whole
+ *     seconds, as metav1.Time marshals.
+ *   - With taint_since != NULL a slice holds at most KXPU_DRA_TAINT_SLICE_DEVICES devices: S = max(1, ceil(n / 64)),
+ *     also when no device is tainted, so the slice layout does not move when a device's health flips.
+ * KXPU_E_INVALID, nothing written: the checks of kxpu_dra_slices, and with taint_since != NULL: taint_key not a
+ * qualified name of at most 127 bytes (an optional lowercase DNS subdomain and '/', then a name of 1..63 bytes that
+ * starts and ends with [A-Za-z0-9] and holds [-A-Za-z0-9_.] between; 127 is this project's bound); taint_value NULL, or
+ * not empty and not such a name of at most 63 bytes; taint_effect not exactly "NoSchedule" or "NoExecute".
+ * KXPU_E_UNSUPPORTED, nothing written: the cases of kxpu_dra_slices, or a taint_since[i] above
+ * KXPU_DRA_TAINT_SINCE_MAX.
+ * GPU: the kernel of kxpu_dra_slices with the taint compiled in: one CTA per 64-device slice; the thread of a device
+ * range-checks its taint_since and formats timeAdded into shared memory.  Timed under KXPU_T_EMIT. */
+int32_t kxpu_dra_slices_taint(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                              const kxpu_dradev *devs, size_t n, const char *taint_key, const char *taint_value,
+                              const char *taint_effect, const int64_t *taint_since /* [n] or NULL */, uint8_t *out,
+                              size_t cap, size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+/* The same for a pool of vGPUs: kxpu_dra_slices_mdev's devices with kxpu_dra_slices_taint's taints, slices and checks;
+ * taint_since == NULL gives kxpu_dra_slices_mdev's bytes. */
+int32_t kxpu_dra_slices_mdev_taint(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                   uint64_t generation, const kxpu_dramdev *devs, size_t n, const char *taint_key,
+                                   const char *taint_value, const char *taint_effect,
+                                   const int64_t *taint_since /* [n] or NULL */, uint8_t *out, size_t cap, size_t *len,
+                                   uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
 
 #ifdef __cplusplus
 }

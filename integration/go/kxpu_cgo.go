@@ -651,3 +651,61 @@ func (k *kxpu) draSlicesMdev(driver, node string, generation uint64, devs []C.kx
 	}
 	return lines, nil
 }
+
+// DRA device taints (ABI v11): draSlices / draSlicesMdev with since[i] = the unix time group i was found unhealthy, or
+// -1.  The key is <driver>/unhealthy, the value vfio-device-missing, the effect NoSchedule: a missing device node keeps
+// new claims away but must not evict a VM that holds the group open.  64 devices per slice.
+func (k *kxpu) draSlicesTaint(driver, node string, generation uint64, devs []C.kxpu_dradev, since []int64) ([]string, error) {
+	var p *C.kxpu_dradev
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	return k.taintSlices("kxpu_dra_slices_taint", driver, node, len(devs), since, func(cd, cn, ck, cv, ce *C.char,
+		cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t, ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_taint(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), ck, cv, ce, cs, out,
+			capacity, n, off, ns)
+	})
+}
+
+func (k *kxpu) draSlicesMdevTaint(driver, node string, generation uint64, devs []C.kxpu_dramdev, since []int64) ([]string, error) {
+	var p *C.kxpu_dramdev
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	return k.taintSlices("kxpu_dra_slices_mdev_taint", driver, node, len(devs), since, func(cd, cn, ck, cv, ce *C.char,
+		cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t, ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_mdev_taint(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), ck, cv, ce, cs,
+			out, capacity, n, off, ns)
+	})
+}
+
+// the two-call sizing of one _taint call, the taint arguments in C memory
+func (k *kxpu) taintSlices(what, driver, node string, nDevs int, since []int64, call func(cd, cn, ck, cv, ce *C.char,
+	cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t, ns *C.size_t) C.int32_t) ([]string, error) {
+	if len(since) != nDevs {
+		return nil, fmt.Errorf("%s: %d taint times for %d devices", what, len(since), nDevs)
+	}
+	cd, cn := C.CString(driver), C.CString(node)
+	ck, cv, ce := C.CString(driver+"/unhealthy"), C.CString("vfio-device-missing"), C.CString("NoSchedule")
+	for _, s := range []*C.char{cd, cn, ck, cv, ce} {
+		defer C.free(unsafe.Pointer(s))
+	}
+	cs := (*C.int64_t)(C.malloc(C.size_t(8 * (nDevs + 1))))
+	defer C.free(unsafe.Pointer(cs))
+	copy(unsafe.Slice((*int64)(unsafe.Pointer(cs)), nDevs), since)
+	var n, ns C.size_t
+	if rc := call(cd, cn, ck, cv, ce, cs, nil, 0, &n, nil, &ns); rc != C.KXPU_E_NOSPACE { // sizing call
+		return nil, kxCheck(k.ctx, what, rc)
+	}
+	buf := make([]byte, n)
+	off := make([]uint64, ns+1)
+	if err := kxCheck(k.ctx, what, call(cd, cn, ck, cv, ce, cs, (*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n,
+		(*C.uint64_t)(unsafe.Pointer(&off[0])), &ns)); err != nil {
+		return nil, err
+	}
+	lines := make([]string, ns)
+	for s := range lines {
+		lines[s] = string(buf[off[s] : off[s+1]-1]) // without the '\n'
+	}
+	return lines, nil
+}

@@ -63,6 +63,8 @@ DRAMDEV_DTYPE = np.dtype([("product", "u1", (64,)), ("mdev_type", "S40"), ("uuid
 assert DRAMDEV_DTYPE.itemsize == 208
 DRA_SLICE_DEVICES = 128
 DRA_MAX_DEVICES = 1 << 24
+DRA_TAINT_SLICE_DEVICES = 64  # devices per slice of the _taint calls (ABI v11) when taint_since is given
+DRA_TAINT_SINCE_MAX = 253402300799  # 9999-12-31T23:59:59Z
 
 # every symbol include/kxpu.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -78,7 +80,7 @@ ABI_SYMBOLS = [
     "kxpu_pciids_full_load_device", "kxpu_full_free", "kxpu_full_export", "kxpu_full_lookup",
     "kxpu_classify_topo", "kxpu_classify_mdev_topo", "kxpu_lw_encode_topo", "kxpu_preferred_allocation",
     "kxpu_reconcile", "kxpu_pcie_tree", "kxpu_preferred_allocation_pcie", "kxpu_classify_viable",
-    "kxpu_dra_slices", "kxpu_dra_slices_mdev",
+    "kxpu_dra_slices", "kxpu_dra_slices_mdev", "kxpu_dra_slices_taint", "kxpu_dra_slices_mdev_taint",
 ]
 
 
@@ -182,6 +184,10 @@ def load_library():
                                   C.POINTER(sz)]),
         "kxpu_dra_slices_mdev": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, C.POINTER(sz), vp,
                                        C.POINTER(sz)]),
+        "kxpu_dra_slices_taint": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, C.c_char_p, C.c_char_p,
+                                        C.c_char_p, vp, vp, sz, C.POINTER(sz), vp, C.POINTER(sz)]),
+        "kxpu_dra_slices_mdev_taint": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, C.c_char_p, C.c_char_p,
+                                             C.c_char_p, vp, vp, sz, C.POINTER(sz), vp, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -673,10 +679,27 @@ class Kxpu:
         """kxpu_dra_slices_mdev: the same for a pool of vGPUs (DRAMDEV_DTYPE devices)."""
         return self._slices(self.L.kxpu_dra_slices_mdev, DRAMDEV_DTYPE, driver, pool, node, generation, devs)
 
-    def _slices(self, fn, dtype, driver, pool, node, generation, devs):
+    def dra_slices_taint(self, driver, pool, node, generation, devs, key, value, effect, since):
+        """kxpu_dra_slices_taint: dra_slices with at most one taint per device.  since: None (the untainted call's bytes)
+        or one int64 per device, the taint's unix time (< 0: untainted); 64 devices per slice when given."""
+        return self._slices(self.L.kxpu_dra_slices_taint, DRADEV_DTYPE, driver, pool, node, generation, devs,
+                            (key, value, effect, since))
+
+    def dra_slices_mdev_taint(self, driver, pool, node, generation, devs, key, value, effect, since):
+        """kxpu_dra_slices_mdev_taint: the same for a pool of vGPUs (DRAMDEV_DTYPE devices)."""
+        return self._slices(self.L.kxpu_dra_slices_mdev_taint, DRAMDEV_DTYPE, driver, pool, node, generation, devs,
+                            (key, value, effect, since))
+
+    def _slices(self, fn, dtype, driver, pool, node, generation, devs, taint=None):
         devs = np.ascontiguousarray(devs)
         assert devs.dtype == dtype
         args = (self.ctx, _kind(driver), _kind(pool), _kind(node), generation, _ptr(devs) if len(devs) else None, len(devs))
+        if taint is not None:
+            key, value, effect, since = taint
+            if since is not None:
+                since = np.ascontiguousarray(since, dtype=np.int64)
+                assert since.shape == (len(devs),)
+            args += (_kind(key), _kind(value), _kind(effect), None if since is None else _ptr(since))
         need, ns = C.c_size_t(0), C.c_size_t(0)
         rc = fn(*args, None, 0, C.byref(need), None, C.byref(ns))
         if rc not in (KXPU_OK, E_NOSPACE):

@@ -16,6 +16,7 @@
 // pass scan -> thread-per-item write.
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -360,8 +361,25 @@ constexpr int MAX_FRAG_DRA_MDEV = (int)sizeof(KX_M0 KX_M1 KX_M2 KX_M3 KX_M4 KX_M
                                   16 + 6 + 6 + 64 + 36 + 1;
 constexpr int DRAM_PARTS = DRAM_LITS + 2;
 
+// Taints (kxpu_dra_slices_taint / kxpu_dra_slices_mdev_taint).  A tainted device's fragment ends with its last literal
+// less that literal's final '}' (the one that closes the device), then the taint head, the 20-byte timeAdded and the
+// taint tail, which closes the taint, the list and the device.  The taint head holds the call's key, value and effect,
+// so it is assembled on the host like the slice head.  Slices hold TAINT_TILE devices whether or not one is tainted.
+#define KX_TAINT_TAIL "\"}]}"
+constexpr int TAINT_TILE = 64;
+constexpr long long TAINT_SINCE_MAX = 253402300799ll;  // 9999-12-31T23:59:59Z
+// ,"taints":[{"key":"<key>","value":"<value>","effect":"<effect>","timeAdded":"  with a 127-byte key, a 63-byte value
+// and "NoSchedule"
+constexpr int TAINT_HEAD_MAX =
+    (int)sizeof(",\"taints\":[{\"key\":\"\",\"value\":\"\",\"effect\":\"\",\"timeAdded\":\"") - 1 + 127 + 63 + 10;
+constexpr int TAINT_PART_MAX = TAINT_HEAD_MAX + 20 + (int)sizeof(KX_TAINT_TAIL) - 1 - 1;  // less the '}' it replaces
+// the untainted pool bound (its longest content is about 1.4 KB: the 1.1 KB head and the vGPU literals) plus the
+// longest taint head and tail
+constexpr int DRA_TAINT_POOL_MAX = DRA_POOL_MAX + 272;
+static_assert(TAINT_HEAD_MAX + (int)sizeof(KX_TAINT_TAIL) - 1 <= DRA_TAINT_POOL_MAX - DRA_POOL_MAX, "taint pool bound");
+
 // PARTS = literals + head + tail; the head is part PARTS - 2, the tail PARTS - 1
-template <int PARTS>
+template <int PARTS, int POOL = DRA_POOL_MAX>
 struct DraParams {
     const void *devs;               // kxpu_dradev[n] or kxpu_dramdev[n]
     uint32_t n;
@@ -372,7 +390,12 @@ struct DraParams {
     unsigned long long *state;      // slice status words (scan.cuh look-back)
     uint32_t epoch;
     uint32_t *flags;                // one word per KXPU_E_UNSUPPORTED reason, DRA_F_* / DRAM_F_*
-    uint8_t pool[DRA_POOL_MAX];
+    uint8_t pool[POOL];
+};
+// the taint instantiations: the literals, the taint head (part PARTS - 4) and tail (PARTS - 3), the slice head and tail
+template <int PARTS>
+struct DraTaintParams : DraParams<PARTS, DRA_TAINT_POOL_MAX> {
+    const long long *since;  // [n]: the taint's unix time, < 0 = untainted
 };
 constexpr int DRA_F_PRODUCT = 0, DRA_F_BDF = 1, DRA_F_ROOT = 2, DRA_F_VENDOR = 3, DRA_F_DEVICE = 4, DRA_F_GROUP = 5,
               DRA_F_PLEN = 6, DRA_F_COUNT = 7;
@@ -380,36 +403,55 @@ constexpr int DRA_F_PRODUCT = 0, DRA_F_BDF = 1, DRA_F_ROOT = 2, DRA_F_VENDOR = 3
 constexpr int DRAM_F_PRODUCT = 0, DRAM_F_TYPE = 1, DRAM_F_UUID = 2, DRAM_F_PARENT = 3, DRAM_F_ROOT = 4, DRAM_F_VENDOR = 5,
               DRAM_F_DEVICE = 6, DRAM_F_GROUP = 7, DRAM_F_PLEN = 8, DRAM_F_COUNT = 9;
 
+// T devices per slice, FRAG bytes per fragment, a POOL-byte pool
+template <int T = TILE, int FRAG = MAX_FRAG_DRA, int POOL = DRA_POOL_MAX>
 struct DraSmem {
-    alignas(16) uint8_t stage[TILE * MAX_FRAG_DRA + DRA_POOL_MAX + 16];
-    uint8_t pool[DRA_POOL_MAX];
-    uint8_t dec[TILE][12];  // group digits at 0, NUMA node digits at 10
-    uint32_t meta[TILE];    // gl | nl << 4 | bl << 8 | rl << 13 | vl << 18 | dl << 21 | pl << 24
-    uint32_t start[TILE];   // fragment offset inside the slice
+    alignas(16) uint8_t stage[T * FRAG + POOL + 16];
+    uint8_t pool[POOL];
+    uint8_t dec[T][12];  // group digits at 0, NUMA node digits at 10
+    uint32_t meta[T];    // gl | nl << 4 | bl << 8 | rl << 13 | vl << 18 | dl << 21 | pl << 24
+    uint32_t start[T];   // fragment offset inside the slice
     unsigned long long base;
     uint32_t wsum[EMIT_THREADS / 32];
     uint32_t tile_total;
 };
+template <int T = TILE, int FRAG = MAX_FRAG_DRA_MDEV, int POOL = DRA_POOL_MAX>
 struct DraMdevSmem {
-    alignas(16) uint8_t stage[TILE * MAX_FRAG_DRA_MDEV + DRA_POOL_MAX + 16];
-    uint8_t pool[DRA_POOL_MAX];
-    uint8_t dec[TILE][12];  // group digits at 0, NUMA node digits at 10
-    uint32_t meta[TILE];    // as DraSmem's, bl being the parent's length
-    uint8_t tlen[TILE];     // mdev_type length
-    uint32_t start[TILE];   // fragment offset inside the slice
+    alignas(16) uint8_t stage[T * FRAG + POOL + 16];
+    uint8_t pool[POOL];
+    uint8_t dec[T][12];  // group digits at 0, NUMA node digits at 10
+    uint32_t meta[T];    // as DraSmem's, bl being the parent's length
+    uint8_t tlen[T];     // mdev_type length
+    uint32_t start[T];   // fragment offset inside the slice
     unsigned long long base;
     uint32_t wsum[EMIT_THREADS / 32];
     uint32_t tile_total;
+};
+template <typename Base>
+struct DraTaintSmem : Base {
+    uint8_t ts[TAINT_TILE][20];  // timeAdded of device d; ts[d][0] == 0: untainted
 };
 template <int LAYOUT> struct DraLayout {  // LAYOUT_PCI
     using Rec = kxpu_dradev;
-    using Smem = DraSmem;
-    static constexpr int PARTS = DRA_PARTS;
+    using Smem = DraSmem<>;
+    using TaintSmem = DraTaintSmem<DraSmem<TAINT_TILE, MAX_FRAG_DRA + TAINT_PART_MAX, DRA_TAINT_POOL_MAX>>;
+    static constexpr int PARTS = DRA_PARTS, LAST = 8, F_COUNT = DRA_F_COUNT;
 };
 template <> struct DraLayout<LAYOUT_MDEV> {
     using Rec = kxpu_dramdev;
-    using Smem = DraMdevSmem;
-    static constexpr int PARTS = DRAM_PARTS;
+    using Smem = DraMdevSmem<>;
+    using TaintSmem = DraTaintSmem<DraMdevSmem<TAINT_TILE, MAX_FRAG_DRA_MDEV + TAINT_PART_MAX, DRA_TAINT_POOL_MAX>>;
+    static constexpr int PARTS = DRAM_PARTS, LAST = DRAM_E, F_COUNT = DRAM_F_COUNT;
+};
+// one k_dra_slices instantiation: LAST is the literal that closes a device; a taint reports F_SINCE
+template <int LAYOUT, bool TAINT> struct DraKernel {
+    static constexpr int T = TAINT ? TAINT_TILE : TILE;
+    static constexpr int PARTS = DraLayout<LAYOUT>::PARTS + (TAINT ? 2 : 0);
+    static constexpr int TAINT_HEAD = PARTS - 4, TAINT_TAIL = PARTS - 3, F_SINCE = DraLayout<LAYOUT>::F_COUNT;
+    static constexpr int POOL = TAINT ? DRA_TAINT_POOL_MAX : DRA_POOL_MAX;
+    static constexpr int MAXF = (LAYOUT == LAYOUT_PCI ? MAX_FRAG_DRA : MAX_FRAG_DRA_MDEV) + (TAINT ? TAINT_PART_MAX : 0);
+    using Params = std::conditional_t<TAINT, DraTaintParams<PARTS>, DraParams<PARTS>>;
+    using Smem = std::conditional_t<TAINT, typename DraLayout<LAYOUT>::TaintSmem, typename DraLayout<LAYOUT>::Smem>;
 };
 
 template <int W>
@@ -432,15 +474,41 @@ __device__ __forceinline__ bool bytes_ok(const uint32_t (&w)[W], uint32_t from, 
     return good;
 }
 
-template <int LAYOUT>
-__global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_constant__ DraParams<DraLayout<LAYOUT>::PARTS> E) {
+// t in [0, TAINT_SINCE_MAX] as RFC 3339 in UTC, "YYYY-MM-DDTHH:MM:SSZ": the days since 1970-01-01 become a proleptic
+// Gregorian date by the 400-year-era arithmetic of civil_from_days (H. Hinnant, "chrono-Compatible Low-Level Date
+// Algorithms"), all in 32 bits
+__device__ __forceinline__ void rfc3339(unsigned long long t, uint8_t *o) {
+    const uint32_t days = (uint32_t)(t >> 7) / 675u;  // t / 86400, 86400 = 2^7 * 675, t >> 7 < 2^31
+    const uint32_t sod = (uint32_t)(t - (unsigned long long)days * 86400ull);
+    const uint32_t z = days + 719468u, era = z / 146097u, doe = z - era * 146097u;  // days since 0000-03-01
+    const uint32_t yoe = (doe - doe / 1460u + doe / 36524u - doe / 146096u) / 365u;
+    const uint32_t doy = doe - (365u * yoe + yoe / 4u - yoe / 100u), mp = (5u * doy + 2u) / 153u;  // March = 0
+    const uint32_t day = doy - (153u * mp + 2u) / 5u + 1u, month = mp < 10u ? mp + 3u : mp - 9u;
+    const uint32_t year = era * 400u + yoe + (month <= 2u ? 1u : 0u);
+    dec_write(year, 4u, o);
+    const uint32_t two[5] = {month, day, sod / 3600u, sod / 60u % 60u, sod % 60u};
+    const char sep[6] = "--T::";
+#pragma unroll
+    for (int k = 0; k < 5; k++) {
+        o[4 + 3 * k] = (uint8_t)sep[k];
+        o[5 + 3 * k] = (uint8_t)('0' + two[k] / 10u);
+        o[6 + 3 * k] = (uint8_t)('0' + two[k] % 10u);
+    }
+    o[19] = (uint8_t)'Z';
+}
+
+// TAINT = false: kxpu_dra_slices[_mdev], TILE devices per slice.  TAINT = true: the _taint calls, TAINT_TILE devices per
+// slice and the taint part after a tainted device's attributes; everything it adds sits behind `if constexpr`.
+template <int LAYOUT, bool TAINT = false>
+__global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_constant__ typename DraKernel<LAYOUT, TAINT>::Params E) {
+    using K = DraKernel<LAYOUT, TAINT>;
     using Rec = typename DraLayout<LAYOUT>::Rec;
-    constexpr int HEAD = DraLayout<LAYOUT>::PARTS - 2, TAIL = DraLayout<LAYOUT>::PARTS - 1;
+    constexpr int HEAD = K::PARTS - 2, TAIL = K::PARTS - 1, T = K::T;
     extern __shared__ __align__(16) uint8_t smem_raw[];
-    typename DraLayout<LAYOUT>::Smem &S = *reinterpret_cast<typename DraLayout<LAYOUT>::Smem *>(smem_raw);
+    typename K::Smem &S = *reinterpret_cast<typename K::Smem *>(smem_raw);
     const uint32_t tid = threadIdx.x, lane = tid & 31u, w = tid >> 5;
-    const uint32_t slice = blockIdx.x, i0 = slice * TILE;
-    const uint32_t in_slice = E.n > i0 ? min(E.n - i0, (uint32_t)TILE) : 0u;
+    const uint32_t slice = blockIdx.x, i0 = slice * T;
+    const uint32_t in_slice = E.n > i0 ? min(E.n - i0, (uint32_t)T) : 0u;
     for (uint32_t k = tid; k < E.pool_len; k += EMIT_THREADS) S.pool[k] = E.pool[k];
     const auto name_ok = [](uint32_t c) {
         return (c >= '0' && c <= '9') || (c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z') || c == '_' || c == '.' || c == '-';
@@ -543,6 +611,17 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
                    (pl ? E.len[7] + pl + ls : 0u) + (rl ? E.len[8] + rl + ls : 0u) + (tid + 1u < in_slice ? 1u : 0u);
         }
     }
+    if constexpr (TAINT) {  // the taint's time, range-checked and formatted beside the record
+        if (tid < in_slice) {
+            const long long since = E.since[i0 + tid];
+            if (since > TAINT_SINCE_MAX) E.flags[K::F_SINCE] = 1u;
+            S.ts[tid][0] = 0;
+            if (since >= 0 && since <= TAINT_SINCE_MAX) {
+                rfc3339((unsigned long long)since, S.ts[tid]);
+                flen += E.len[K::TAINT_HEAD] + 20u + E.len[K::TAINT_TAIL] - 1u;
+            }
+        }
+    }
     // ---- scan of the 128 lengths (threads >= TILE contribute 0)
     const uint32_t incl = kxscan::warp_incl(flen);
     if (lane == 31) S.wsum[w] = incl;
@@ -555,7 +634,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
     }
     __syncthreads();
     const uint32_t head_len = E.len[HEAD], tail_len = E.len[TAIL], tile_total = S.tile_total;
-    if (tid < TILE) S.start[tid] = head_len + S.wsum[w] + incl - flen;
+    if (tid < T) S.start[tid] = head_len + S.wsum[w] + incl - flen;
     // ---- the slice's offset in the output: decoupled look-back over the slice totals; its exclusive prefix is slice_off[s]
     if (w == 0) {
         const unsigned long long agg = (unsigned long long)head_len + tile_total + tail_len;
@@ -584,6 +663,17 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
             o += L;
         };
         auto lit = [&](int k) { put(S.pool + E.off[k], E.len[k]); };
+        // the literal that closes the device (K's LAST); a tainted device's taint part goes before its final '}'
+        auto close = [&](int k) {
+            if constexpr (TAINT) {
+                if (S.ts[d][0]) {
+                    put(S.pool + E.off[k], E.len[k] - 1u);
+                    lit(K::TAINT_HEAD); put(S.ts[d], 20u); lit(K::TAINT_TAIL);
+                    return;
+                }
+            }
+            lit(k);
+        };
         const auto bytes = [](const char *s) { return reinterpret_cast<const uint8_t *>(s); };
         if constexpr (LAYOUT == LAYOUT_PCI) {
             lit(0); put(S.dec[d], gl); lit(1); put(bytes(r->device), dl);
@@ -592,7 +682,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
             lit(4); put(bytes(r->bdf), bl);
             if (pl) { lit(5); put(r->product, pl); }
             if (rl) { lit(6); put(bytes(r->pcie_root), rl); }
-            lit(7); put(bytes(r->vendor), vl); lit(8);
+            lit(7); put(bytes(r->vendor), vl); close(DraLayout<LAYOUT>::LAST);
         } else {
             const uint32_t tl = S.tlen[d];
             lit(0); put(S.dec[d], gl); lit(1); put(S.dec[d], gl); lit(DRAM_I);
@@ -603,7 +693,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
             lit(6); put(bytes(r->vendor), vl); lit(DRAM_S);
             if (pl) { lit(7); put(r->product, pl); lit(DRAM_S); }
             if (rl) { lit(8); put(bytes(r->pcie_root), rl); lit(DRAM_S); }
-            lit(9); put(bytes(r->uuid), 36u); lit(DRAM_S); lit(DRAM_E);
+            lit(9); put(bytes(r->uuid), 36u); lit(DRAM_S); close(DraLayout<LAYOUT>::LAST);
         }
         if (d + 1u < in_slice && lane == 0) dst[o] = (uint8_t)',';
     }
@@ -1018,23 +1108,62 @@ static bool dns_subdomain_ok(const char *s, size_t max) {
     return true;
 }
 
-// kxpu_dra_slices / kxpu_dra_slices_mdev: the argument checks, the pool (literals | head | tail), one k_dra_slices<LAYOUT>
-// launch, the domain flags and the copies
-template <int LAYOUT>
+// a Kubernetes name part: 1..max bytes, [A-Za-z0-9] at both ends, [-A-Za-z0-9_.] between
+static bool k8s_name_ok(const char *s, size_t len, size_t max) {
+    if (len == 0 || len > max) return false;
+    auto alnum = [](char c) { return (c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z') || (c >= '0' && c <= '9'); };
+    if (!alnum(s[0]) || !alnum(s[len - 1])) return false;
+    for (size_t i = 0; i < len; i++)
+        if (!alnum(s[i]) && s[i] != '-' && s[i] != '_' && s[i] != '.') return false;
+    return true;
+}
+// a taint key: a qualified name of at most 127 bytes, [<lowercase DNS subdomain>/]<name of 1..63 bytes>
+static bool taint_key_ok(const char *k) {
+    if (!k) return false;
+    const size_t len = strnlen(k, 128);
+    if (len == 0 || len > 127) return false;
+    const char *slash = (const char *)memchr(k, '/', len);
+    if (!slash) return k8s_name_ok(k, len, 63);
+    const size_t pl = (size_t)(slash - k);
+    return pl > 0 && dns_subdomain_ok(std::string(k, pl).c_str(), 253) && k8s_name_ok(slash + 1, len - pl - 1, 63);
+}
+// a taint value: empty or a name of at most 63 bytes
+static bool taint_value_ok(const char *v) {
+    if (!v) return false;
+    const size_t len = strnlen(v, 64);
+    return len == 0 || k8s_name_ok(v, len, 63);
+}
+
+// the taint arguments of the _taint calls; since == NULL: the untainted call
+struct DraTaint {
+    const char *key, *value, *effect;
+    const int64_t *since;
+};
+
+// kxpu_dra_slices[_mdev][_taint]: the argument checks, the pool (literals | [taint head | taint tail |] head | tail),
+// one k_dra_slices<LAYOUT, TAINT> launch, the domain flags and the copies
+template <int LAYOUT, bool TAINT = false>
 static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, const char *pool, const char *node,
                           uint64_t generation, const typename DraLayout<LAYOUT>::Rec *devs, size_t n, uint8_t *out, size_t cap,
-                          size_t *len, uint64_t *slice_off, size_t *n_slices) {
+                          size_t *len, uint64_t *slice_off, size_t *n_slices, const DraTaint &taint = DraTaint{}) {
     using Rec = typename DraLayout<LAYOUT>::Rec;
-    constexpr int PARTS = DraLayout<LAYOUT>::PARTS, HEAD = PARTS - 2, TAIL = PARTS - 1;
+    using K = DraKernel<LAYOUT, TAINT>;
+    constexpr int PARTS = K::PARTS, HEAD = PARTS - 2, TAIL = PARTS - 1;
     constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : DRAM_LITS;
-    constexpr int MAXF = LAYOUT == LAYOUT_PCI ? MAX_FRAG_DRA : MAX_FRAG_DRA_MDEV;
-    constexpr int F_COUNT = LAYOUT == LAYOUT_PCI ? DRA_F_COUNT : DRAM_F_COUNT;
+    constexpr int MAXF = K::MAXF;
+    constexpr int F_COUNT = DraLayout<LAYOUT>::F_COUNT + (TAINT ? 1 : 0);
     const char *const *lits = LAYOUT == LAYOUT_PCI ? h_dra_lits : h_dram_lits;
     if (!ctx || !len || !n_slices || (n && !devs)) return KXPU_E_INVALID;
     if (!dns_subdomain_ok(driver, 63) || !dns_subdomain_ok(pool, 253) || !dns_subdomain_ok(node, 253) ||
         generation >= (1ull << 63)) {
         KX_SET_ERR(ctx, "%s: driver (<= 63 bytes), pool and node (<= 253 bytes) must be lowercase DNS subdomains "
                         "and generation below 2^63", what);
+        return KXPU_E_INVALID;
+    }
+    if (TAINT && (!taint_key_ok(taint.key) || !taint_value_ok(taint.value) || !taint.effect ||
+                  (strcmp(taint.effect, "NoSchedule") != 0 && strcmp(taint.effect, "NoExecute") != 0))) {
+        KX_SET_ERR(ctx, "%s: taint_key must be a qualified name of at most 127 bytes, taint_value empty or a label value "
+                        "and taint_effect NoSchedule or NoExecute", what);
         return KXPU_E_INVALID;
     }
     if (n >= KXPU_DRA_MAX_DEVICES) {
@@ -1044,19 +1173,29 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
-    const uint32_t N = (uint32_t)n, slices = N ? (N + TILE - 1) / TILE : 1u;
+    const uint32_t N = (uint32_t)n, slices = N ? (N + K::T - 1) / K::T : 1u;
     const std::string d = driver, p = pool, nd = node;
     const std::string head = "{\"kind\":\"ResourceSlice\",\"apiVersion\":\"resource.k8s.io/v1\",\"metadata\":{\"generateName\":\"" +
                              nd + "-" + d + "-\"},\"spec\":{\"driver\":\"" + d + "\",\"pool\":{\"name\":\"" + p +
                              "\",\"generation\":" + std::to_string(generation) +
                              ",\"resourceSliceCount\":" + std::to_string(slices) + "},\"nodeName\":\"" + nd +
                              "\",\"devices\":[";
-    DraParams<PARTS> E;
+    std::string taint_head;
+    if (TAINT) {
+        taint_head = std::string(",\"taints\":[{\"key\":\"") + taint.key + "\"";
+        if (taint.value[0]) taint_head += std::string(",\"value\":\"") + taint.value + "\"";
+        taint_head += std::string(",\"effect\":\"") + taint.effect + "\",\"timeAdded\":\"";
+    }
+    typename K::Params E;
     memset(&E, 0, sizeof E);
     uint32_t acc = 0;
     for (int k = 0; k < PARTS; k++) {
-        const std::string s = k < LITS ? std::string(lits[k]) : k == HEAD ? head : std::string(KX_DRA_TAIL);
-        if (acc + s.size() > (size_t)DRA_POOL_MAX) return KXPU_E_INVALID;  // the literals grew: DRA_POOL_MAX must follow
+        const std::string s = k < LITS                       ? std::string(lits[k])
+                              : k == HEAD                    ? head
+                              : k == TAIL                    ? std::string(KX_DRA_TAIL)
+                              : k == LITS                    ? taint_head
+                                                             : std::string(KX_TAINT_TAIL);
+        if (acc + s.size() > (size_t)K::POOL) return KXPU_E_INVALID;  // the literals grew: the pool bound must follow
         memcpy(E.pool + acc, s.data(), s.size());
         E.off[k] = (uint16_t)acc;
         E.len[k] = (uint16_t)s.size();
@@ -1064,10 +1203,10 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     }
     E.pool_len = acc;
     const size_t bound = (size_t)slices * (E.len[HEAD] + E.len[TAIL]) + (size_t)n * MAXF + 64;
-    const size_t smem = sizeof(typename DraLayout<LAYOUT>::Smem);
+    const size_t smem = sizeof(typename K::Smem);
     static bool attr_done = false;
     if (!attr_done) {
-        cudaFuncSetAttribute(k_dra_slices<LAYOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaFuncSetAttribute(k_dra_slices<LAYOUT, TAINT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         attr_done = true;
     }
     KxScratch sc(ctx);
@@ -1081,12 +1220,18 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     if (n) cudaMemcpyAsync(d_devs, devs, n * sizeof(Rec), cudaMemcpyHostToDevice, ctx->stream);
     cudaMemsetAsync(d_ctl + slices + 1, 0, (ctl_words - slices - 1) * 8, ctx->stream);
     E.devs = d_devs; E.n = N; E.out = d_out; E.slice_off = d_ctl; E.flags = (uint32_t *)(d_ctl + slices + 1);
+    if constexpr (TAINT) {
+        long long *d_since = nullptr;
+        KX_CUDA(ctx, sc.alloc((void **)&d_since, n * sizeof(long long)));
+        if (n) cudaMemcpyAsync(d_since, taint.since, n * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream);
+        E.since = d_since;
+    }
     E.state = kx_scan_state(ctx, slices);
     if (!E.state) return KXPU_E_NOMEM;
     E.epoch = kx_next_epoch(ctx);
     {
         KxTimer tm(ctx, KXPU_T_EMIT);
-        k_dra_slices<LAYOUT><<<slices, EMIT_THREADS, smem, ctx->stream>>>(E);
+        k_dra_slices<LAYOUT, TAINT><<<slices, EMIT_THREADS, smem, ctx->stream>>>(E);
         KX_LAUNCHED(ctx);
     }
     std::vector<unsigned long long> h(ctl_words);
@@ -1105,7 +1250,10 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     const char *const *why = LAYOUT == LAYOUT_PCI ? why_pci : why_mdev;
     const uint32_t *flags = reinterpret_cast<const uint32_t *>(h.data() + slices + 1);
     for (int f = 0; f < F_COUNT; f++)
-        if (flags[f]) { KX_SET_ERR(ctx, "%s: %s", what, why[f]); return KXPU_E_UNSUPPORTED; }
+        if (flags[f]) {
+            KX_SET_ERR(ctx, "%s: %s", what, f == K::F_SINCE ? "a taint_since above 253402300799 (9999-12-31T23:59:59Z)" : why[f]);
+            return KXPU_E_UNSUPPORTED;
+        }
     const size_t total = (size_t)h[slices];
     *len = total;
     *n_slices = slices;
@@ -1136,4 +1284,24 @@ extern "C" int32_t kxpu_dra_slices_mdev(kxpu_ctx *ctx, const char *driver, const
                   "kxpu_dramdev layout");
     return dra_slices<LAYOUT_MDEV>(ctx, "dra_slices_mdev", driver, pool, node, generation, devs, n, out, cap, len, slice_off,
                                    n_slices);
+}
+
+// taint_since == NULL: exactly the untainted call, the taint arguments unread
+extern "C" int32_t kxpu_dra_slices_taint(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                         uint64_t generation, const kxpu_dradev *devs, size_t n, const char *taint_key,
+                                         const char *taint_value, const char *taint_effect, const int64_t *taint_since,
+                                         uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
+    if (!taint_since) return kxpu_dra_slices(ctx, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
+    return dra_slices<LAYOUT_PCI, true>(ctx, "dra_slices_taint", driver, pool, node, generation, devs, n, out, cap, len,
+                                        slice_off, n_slices, DraTaint{taint_key, taint_value, taint_effect, taint_since});
+}
+
+extern "C" int32_t kxpu_dra_slices_mdev_taint(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                              uint64_t generation, const kxpu_dramdev *devs, size_t n, const char *taint_key,
+                                              const char *taint_value, const char *taint_effect, const int64_t *taint_since,
+                                              uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
+    if (!taint_since)
+        return kxpu_dra_slices_mdev(ctx, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
+    return dra_slices<LAYOUT_MDEV, true>(ctx, "dra_slices_mdev_taint", driver, pool, node, generation, devs, n, out, cap, len,
+                                         slice_off, n_slices, DraTaint{taint_key, taint_value, taint_effect, taint_since});
 }

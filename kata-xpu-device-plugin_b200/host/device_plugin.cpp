@@ -20,6 +20,8 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <ctime>
+#include <set>
 #include <thread>
 
 namespace device_plugin {
@@ -1464,6 +1466,13 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         report.changedPlugins.push_back(k);
     }
     std::sort(report.changedPlugins.begin(), report.changedPlugins.end());
+    // a surviving group keeps its taint time, as it keeps its health; a group that left drops it
+    for (auto it = draTaintSince_.begin(); it != draTaintSince_.end();) {
+        bool present = false;
+        for (const auto &kv : iommuMap) present |= kv.first == it->first;
+        for (const auto &kv : mdevMap) present |= kv.first == it->first;
+        it = present ? std::next(it) : draTaintSince_.erase(it);
+    }
     bool passthroughChanged = false, vgpuChanged = false;
     for (size_t k : report.changedPlugins) (devicePlugins[k].vgpu ? vgpuChanged : passthroughChanged) = true;
     if (passthroughChanged || viabilityChanged) draGeneration_++;  // the ResourceSlices of the next publication replace these
@@ -1557,6 +1566,36 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
     return Error();
 }
 
+// The taint of a group whose device node the HealthWatcher saw disappear.  The effect is NoSchedule on purpose: it keeps
+// new claims away, and a missing /dev/vfio node must not evict a VM that already holds the group open, which NoExecute
+// would do.
+static const char *kDraTaintKeyName = "/unhealthy";  // the key is <draDriver>/unhealthy
+static const char *kDraTaintValue = "vfio-device-missing";
+static const char *kDraTaintEffect = "NoSchedule";
+
+// ResourceSlices / VgpuResourceSlices with draTaints: the two-call sizing of the _taint call fn
+template <typename Rec>
+static Error draTaintSlices(kxpu_ctx *ctx,
+                            int32_t (*fn)(kxpu_ctx *, const char *, const char *, const char *, uint64_t, const Rec *, size_t,
+                                          const char *, const char *, const char *, const int64_t *, uint8_t *, size_t,
+                                          size_t *, uint64_t *, size_t *),
+                            const char *what, const std::string &driver, const std::string &node, uint64_t generation,
+                            const std::vector<Rec> &devs, const std::vector<int64_t> &since, std::vector<uint8_t> &out,
+                            std::vector<uint64_t> &sliceOff) {
+    const std::string key = driver + kDraTaintKeyName;
+    size_t len = 0, nSlices = 0;
+    int32_t rc = fn(ctx, driver.c_str(), node.c_str(), node.c_str(), generation, devs.data(), devs.size(), key.c_str(),
+                    kDraTaintValue, kDraTaintEffect, since.data(), nullptr, 0, &len, nullptr, &nSlices);
+    if (rc == KXPU_E_NOSPACE) {
+        out.assign(len, 0);
+        sliceOff.assign(nSlices + 1, 0);
+        rc = fn(ctx, driver.c_str(), node.c_str(), node.c_str(), generation, devs.data(), devs.size(), key.c_str(),
+                kDraTaintValue, kDraTaintEffect, since.data(), out.data(), out.size(), &len, sliceOff.data(), &nSlices);
+    }
+    if (rc != KXPU_OK) return kxfail(ctx, what, rc);
+    return Error();
+}
+
 Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) {
     std::shared_lock<std::shared_mutex> lock(mu_);
     if (xpuClass >= xpuClasses.size() || xpuClasses[xpuClass].draDriver.empty())
@@ -1567,6 +1606,7 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
         if (!dp.vgpu && dp.xpuClass == xpuClass)
             for (const Device &d : dp.devs) productOf[d.ID] = &dp.devpluginName;
     std::vector<kxpu_dradev> devs;
+    std::vector<std::string> groups;
     for (size_t g = 0; g < iommuMap.size() && g < iommuDra.size(); g++) {
         if (iommuClass[g] != xpuClass || (g < iommuBlocker.size() && !iommuBlocker[g].empty())) continue;
         kxpu_dradev d = iommuDra[g];
@@ -1576,7 +1616,10 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
             memcpy(d.product, it->second->data(), d.product_len);
         }
         devs.push_back(d);
+        groups.push_back(iommuMap[g].first);
     }
+    if (draTaints) return draTaintSlices(ctx_, kxpu_dra_slices_taint, "kxpu_dra_slices_taint", driver, nodeName,
+                                         draGeneration_, devs, draSince(groups), out, sliceOff);
     size_t len = 0, nSlices = 0;
     int32_t rc = kxpu_dra_slices(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), draGeneration_, devs.data(),
                                  devs.size(), nullptr, 0, &len, nullptr, &nSlices);
@@ -1590,14 +1633,57 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
     return Error();
 }
 
+std::vector<int64_t> Plugin::draSince(const std::vector<std::string> &groups) const {
+    std::vector<int64_t> since;
+    for (const std::string &g : groups) {
+        auto it = draTaintSince_.find(g);
+        since.push_back(it == draTaintSince_.end() ? -1 : it->second);
+    }
+    return since;
+}
+
+Error Plugin::refreshDraHealth(bool &passthroughMoved, bool &vgpuMoved) {
+    std::unique_lock<std::shared_mutex> lock(mu_);
+    passthroughMoved = vgpuMoved = false;
+    if (!draTaints) return Error();
+    std::set<std::pair<bool, std::string>> unhealthy;  // (vgpu, group) that some plugin serving it has Unhealthy
+    for (const GenericDevicePlugin &dp : devicePlugins)
+        for (const Device &d : dp.devs)
+            if (d.Health != kHealthy) unhealthy.insert({dp.vgpu, d.ID});
+    const int64_t t = now ? now() : (int64_t)time(nullptr);
+    std::map<std::string, int64_t> next;
+    auto visit = [&](const std::string &g, bool vgpu, bool &moved) {
+        auto it = draTaintSince_.find(g);
+        const bool was = it != draTaintSince_.end(), is = unhealthy.count({vgpu, g}) > 0;
+        if (is) next[g] = was ? it->second : t;  // the time it turned unhealthy, kept while it stays so
+        moved |= was != is;
+    };
+    // the groups ResourceSlices / VgpuResourceSlices publish; a blocked group is not published, so it has no taint
+    for (size_t g = 0; g < iommuMap.size() && g < iommuClass.size(); g++)
+        if (!xpuClasses[iommuClass[g]].draDriver.empty() && (g >= iommuBlocker.size() || iommuBlocker[g].empty()))
+            visit(iommuMap[g].first, false, passthroughMoved);
+    for (size_t g = 0; g < mdevMap.size() && g < mdevClass.size(); g++)
+        if (!vgpuClasses[mdevClass[g]].draDriver.empty()) visit(mdevMap[g].first, true, vgpuMoved);
+    draTaintSince_ = std::move(next);
+    if (passthroughMoved) draGeneration_++;
+    if (vgpuMoved) draVgpuGeneration_++;
+    return Error();
+}
+
 Error Plugin::VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) {
     std::shared_lock<std::shared_mutex> lock(mu_);
     if (vgpuClass >= vgpuClasses.size() || vgpuClasses[vgpuClass].draDriver.empty())
         return fail("VgpuResourceSlices: vGPU class " + std::to_string(vgpuClass) + " has no DRA driver");
     const std::string &driver = vgpuClasses[vgpuClass].draDriver;
     std::vector<kxpu_dramdev> devs;
+    std::vector<std::string> groups;
     for (size_t g = 0; g < mdevMap.size() && g < mdevDra.size() && g < mdevClass.size(); g++)
-        if (mdevClass[g] == vgpuClass) devs.push_back(mdevDra[g]);
+        if (mdevClass[g] == vgpuClass) {
+            devs.push_back(mdevDra[g]);
+            groups.push_back(mdevMap[g].first);
+        }
+    if (draTaints) return draTaintSlices(ctx_, kxpu_dra_slices_mdev_taint, "kxpu_dra_slices_mdev_taint", driver, nodeName,
+                                         draVgpuGeneration_, devs, draSince(groups), out, sliceOff);
     size_t len = 0, nSlices = 0;
     int32_t rc = kxpu_dra_slices_mdev(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), draVgpuGeneration_, devs.data(),
                                       devs.size(), nullptr, 0, &len, nullptr, &nSlices);
@@ -1635,6 +1721,11 @@ Error Plugin::PrepareDraDevices(const std::string &driver, const std::string &po
                     found |= !g.empty() && iommuMap[k].first == g && iommuClass[k] == cls;
             }
             if (!found) return fail("PrepareDraDevices: unknown device " + name + " in pool " + pool);
+            // refused even when the claim tolerates the taint: the device node is missing, so the VM cannot start
+            if (draTaints && draTaintSince_.count(g))
+                return fail("PrepareDraDevices: device " + name + " is tainted " + driver + kDraTaintKeyName + "=" +
+                            kDraTaintValue + ":" + kDraTaintEffect + ": the VFIO device node of IOMMU group " + g +
+                            " is missing");
             groups.push_back(g);
         }
     }
@@ -2527,6 +2618,23 @@ void kxh_count_id_reads(void *h, const char *prop, uint64_t *reads) {
         if (pr == want) (*reads)++;
         return di(base, addr, pr, out);
     };
+}
+
+// ---- DRA device taints (ABI v11)
+void kxh_set_dra_taints(void *h, int on) { ((Plugin *)h)->draTaints = on != 0; }
+// the clock of refreshDraHealth reads *t (tests); NULL restores time(nullptr)
+void kxh_set_clock(void *h, const int64_t *t) {
+    Plugin *p = (Plugin *)h;
+    if (t) p->now = [t]() { return *t; };
+    else p->now = nullptr;
+}
+// refreshDraHealth: *moved = bit 0 passthrough pools, bit 1 vGPU pools; -1 with the message in err
+int kxh_refresh_dra_health(void *h, int *moved, char *err, size_t cap) {
+    bool pt = false, vg = false;
+    device_plugin::Error e = ((Plugin *)h)->refreshDraHealth(pt, vg);
+    if (e) { copy_out(e.message, err, cap); return -1; }
+    *moved = (pt ? 1 : 0) | (vg ? 2 : 0);
+    return 0;
 }
 
 }  // extern "C"

@@ -281,6 +281,13 @@ class Plugin {
     // read only leaves out its attribute.  The PCI walk and every device-plugin output stay as they are.
     bool vgpuDraEnabled() const;  // some vGPU class has a draDriver
     bool readsMdevNuma() const { return topologyAware || vgpuDraEnabled(); }
+    // DRA device taints (ABI v11).  false (default): the slices never carry taints and every output and generation is as
+    // above, even while a device is Unhealthy.  true: ResourceSlices and VgpuResourceSlices go through the _taint calls
+    // (64 devices per slice); a group that refreshDraHealth found unhealthy carries the taint <draDriver>/unhealthy =
+    // vfio-device-missing:NoSchedule since the time it was found so, and PrepareDraDevices refuses it.
+    bool draTaints = false;
+    // the clock of refreshDraHealth, unix seconds; a seam (time(nullptr) when empty)
+    std::function<int64_t()> now;
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
 
     // ---- state (device_plugin.go:31,34)
@@ -353,19 +360,27 @@ class Plugin {
     // The ResourceSlices of class xpuClass (kxpu_dra_slices): one pool named nodeName, one device per iommuMap group of
     // the class in walk order (bdf, vendor, device and PCIe root of the group's first member, the group's NUMA mask, the
     // plugin's resource-name suffix cut to 64 bytes as productName).  With groupViability a group that has a blocker is
-    // not published: DRA v1 has no per-device health and a published device is schedulable.  Health from the
-    // HealthWatcher is not consulted.  out: JSON Lines, one slice per line; sliceOff: the n_slices + 1 line bounds.
+    // not published, also with draTaints: a taint can be tolerated, and on a cluster without the DRADeviceTaints feature
+    // gate a tainted device looks healthy, so a group VFIO cannot open would be handed out.  Without draTaints health
+    // from the HealthWatcher is not consulted; with it, a group refreshDraHealth found unhealthy is published tainted.
+    // out: JSON Lines, one slice per line; sliceOff: the n_slices + 1 line bounds.
     Error ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff);
     // the pool generation of every class's ResourceSlices: 1 after start-up, +1 for each rediscover that changed a
-    // passthrough plugin or a group's viability
+    // passthrough plugin or a group's viability, +1 for each refreshDraHealth that changed their taints
     uint64_t draGeneration() const { return draGeneration_; }
+    // draTaints: the device-plugin health of every group published in a DRA pool becomes its taint.  The host calls it
+    // after HealthWatcher::poll returned > 0.  Under the exclusive lock: a group that any plugin serving it has
+    // Unhealthy is tainted since now() when it turns unhealthy, keeps that time while it stays so and loses it when it
+    // turns healthy; draGeneration / draVgpuGeneration grow by one when the taints of their pools changed, and
+    // passthroughMoved / vgpuMoved say which did.  Without draTaints nothing changes.
+    Error refreshDraHealth(bool &passthroughMoved, bool &vgpuMoved);
     // The ResourceSlices of vGPU class vgpuClass (kxpu_dra_slices_mdev): one pool named nodeName, one device per mdevMap
     // group of the class in walk order, described by the group's first mdev: its type key, UUID, parent address, the
     // parent's vendor and device ids, the PCIe root of its link, the group's NUMA mask, and the parent's model name
     // (getDeviceNames: the sanitised pci.ids name, else the raw device id; cut to 64 bytes) as productName.
     Error VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff);
     // the pool generation of every vGPU class's ResourceSlices: 1 after start-up, +1 for each rediscover that changed a
-    // vGPU plugin
+    // vGPU plugin, +1 for each refreshDraHealth that changed their taints
     uint64_t draVgpuGeneration() const { return draVgpuGeneration_; }
     // The data half of NodePrepareResources: cdiIds[i] = the CDI names Allocate({g}) returns for deviceNames[i] =
     // "vfio<g>", a device of the pool `pool` of the class (passthrough or vGPU) whose draDriver is `driver` (same live or
@@ -426,6 +441,8 @@ class Plugin {
     bool haveSnapshotGen_ = false;
     uint64_t snapshotGen_ = 0;
     uint64_t draGeneration_ = 1, draVgpuGeneration_ = 1;
+    std::map<std::string, int64_t> draTaintSince_;  // draTaints: IOMMU group id -> when its taint was added
+    std::vector<int64_t> draSince(const std::vector<std::string> &groups) const;  // per group: its time, or -1
     Error checkDraClasses() const;
     void buildMdevDra(const MdevWalk &w);
 };
