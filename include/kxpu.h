@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 11
+#define KXPU_ABI_VERSION 12
 
 /* status codes */
 #define KXPU_OK             0
@@ -859,6 +859,77 @@ int32_t kxpu_dra_slices_mdev_taint(kxpu_ctx *ctx, const char *driver, const char
                                    const char *taint_value, const char *taint_effect,
                                    const int64_t *taint_since /* [n] or NULL */, uint8_t *out, size_t cap, size_t *len,
                                    uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
+/* ------------------------------------------- PCIe AER health and several taints per device (ABI v12) */
+
+/* The uncorrectable PCIe errors a function has reported (Documentation/ABI/testing/sysfs-bus-pci-devices-aer_stats):
+ *   [assumed] /sys/bus/pci/devices/<bdf>/aer_dev_fatal and aer_dev_nonfatal exist since Linux 4.19;
+ *   [assumed] they exist only on functions that have an AER capability;
+ *   [assumed] each line is "<name> <count>", and a name may contain spaces;
+ *   [assumed] the total is the line "TOTAL_ERR_FATAL <n>" (aer_dev_fatal) or "TOTAL_ERR_NONFATAL <n>" (aer_dev_nonfatal);
+ *   [assumed] on firmware-first platforms the OS does not handle AER, and the counters may never move. */
+#define KXPU_AER_FATAL    1u  /* some member's known fatal count is above fatal_limit        */
+#define KXPU_AER_NONFATAL 2u  /* some member's known non-fatal count is above nonfatal_limit */
+#define KXPU_AER_UNKNOWN  4u  /* some member has an unknown count                            */
+#define KXPU_AER_FILE_MAX 4096 /* a longer file gives an unknown count                       */
+
+/* The AER counts of n records, folded per group.  Record i has two files: its fatal file is
+ * text[file_off[2i], +file_len[2i]) and its non-fatal file is entry 2i+1.  Files may share bytes (a vGPU uses its
+ * parent's files).  The count of a file:
+ *   - the last line of the file that begins with "TOTAL_ERR_FATAL " (fatal file) or "TOTAL_ERR_NONFATAL " (non-fatal
+ *     file), the space included;
+ *   - what follows the prefix, up to '\n' or the end of the file, is a canonical decimal: 1 to 20 digits, no leading
+ *     zero except "0" itself, value below 2^64 - 1;
+ *   - anything else makes the count UNKNOWN, never an error (like numa_node): no such line, a '\r', a bad number,
+ *     file_len == 0 (the host's failed read) or file_len > KXPU_AER_FILE_MAX.
+ * totals (may be NULL): totals[2i] / totals[2i+1] = the fatal / non-fatal count of record i, UINT64_MAX when unknown.
+ * group_aer[o], over the members group_members[group_off[o] .. group_off[o+1]) of group o: KXPU_AER_FATAL when some
+ * member's known fatal count is greater than fatal_limit, KXPU_AER_NONFATAL the same for the non-fatal count and
+ * nonfatal_limit, KXPU_AER_UNKNOWN when some member has an unknown count.  A group without members gets 0.
+ * KXPU_E_INVALID, nothing written: ctx NULL, text NULL with text_len > 0, file_off / file_len NULL with n > 0,
+ * group_off NULL, group_members NULL with members, group_aer NULL with n_groups > 0; a file range outside text_len;
+ * group_off decreasing; a member >= n.
+ * Limit (else KXPU_E_UNSUPPORTED): n and n_groups below 2^28.
+ * GPU: one warp per file reads its tail backward in 32-byte windows: a ballot finds the line starts, each starting lane
+ * tests the prefix and parses its number, and the highest match decides; then one warp per group ORs its members'
+ * bits.  Timed under KXPU_T_CLASSIFY. */
+int32_t kxpu_aer_health(kxpu_ctx *ctx, const uint8_t *text, size_t text_len, const uint64_t *file_off /* [2n] */,
+                        const uint32_t *file_len /* [2n] */, size_t n, uint64_t fatal_limit, uint64_t nonfatal_limit,
+                        const uint32_t *group_off /* [n_groups+1] */, const uint32_t *group_members, size_t n_groups,
+                        uint64_t *totals /* [2n] or NULL */, uint8_t *group_aer /* [n_groups] */);
+
+/* Several taints per device: a table of up to KXPU_DRA_MAX_TAINTS entries, each with the _taint calls' key, value and
+ * effect rules.
+ *   [assumed] the API rejects a device that carries two taints with the same key and effect. */
+typedef struct kxpu_dra_taint {
+    const char *key, *value, *effect;
+} kxpu_dra_taint;
+#define KXPU_DRA_MAX_TAINTS 4
+
+/* kxpu_dra_slices_taint with a table of n_taints taints.  The contract is kxpu_dra_slices_taint's, with these changes:
+ *   - taint_since == NULL: the output, *len, slice_off and *n_slices are byte for byte kxpu_dra_slices'; the taint
+ *     arguments are not read.
+ *   - taint_since[i * n_taints + t] < 0: device i does not carry taint t; 0 .. KXPU_DRA_TAINT_SINCE_MAX: it carries
+ *     taint t with that timeAdded.
+ *   - a device that carries some taint gets "taints":[{...},{...}], its taints in table order, each written as the
+ *     _taint call writes its one taint ("value" left out when empty).  n_taints == 1 gives kxpu_dra_slices_taint's bytes
+ *     for that key, value and effect.
+ *   - with taint_since != NULL a slice holds at most KXPU_DRA_TAINT_SLICE_DEVICES devices.
+ * KXPU_E_INVALID, nothing written: the checks of kxpu_dra_slices, and with taint_since != NULL: taints NULL, n_taints 0
+ * or above KXPU_DRA_MAX_TAINTS, or an entry whose key, value or effect fails kxpu_dra_slices_taint's checks.
+ * KXPU_E_UNSUPPORTED, nothing written: the cases of kxpu_dra_slices, a taint_since above KXPU_DRA_TAINT_SINCE_MAX, or a
+ * device that carries two entries with the same key and effect.
+ * GPU: the kernel of kxpu_dra_slices with the taint list compiled in.  Timed under KXPU_T_EMIT. */
+int32_t kxpu_dra_slices_taints(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                               const kxpu_dradev *devs, size_t n, const kxpu_dra_taint *taints, size_t n_taints,
+                               const int64_t *taint_since /* [n * n_taints], device-major, or NULL */, uint8_t *out,
+                               size_t cap, size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+/* The same for a pool of vGPUs: taint_since == NULL gives kxpu_dra_slices_mdev's bytes, n_taints == 1
+ * kxpu_dra_slices_mdev_taint's. */
+int32_t kxpu_dra_slices_mdev_taints(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                    uint64_t generation, const kxpu_dramdev *devs, size_t n, const kxpu_dra_taint *taints,
+                                    size_t n_taints, const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out,
+                                    size_t cap, size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
 
 #ifdef __cplusplus
 }

@@ -709,3 +709,103 @@ func (k *kxpu) taintSlices(what, driver, node string, nDevs int, since []int64, 
 	}
 	return lines, nil
 }
+
+// PCIe AER health (ABI v12).  text holds every file the host read (ReadFile of <bdf>/aer_dev_fatal and aer_dev_nonfatal,
+// at most 4097 bytes each; an mdev reads its parent's, a failed read is an empty file); fileOff / fileLen are 2n entries,
+// the fatal file of record i at 2i.  groupOff / groupMembers: the groups.  Returns each group's KXPU_AER_* bits.
+func (k *kxpu) aerHealth(text []byte, fileOff []uint64, fileLen []uint32, fatalLimit, nonfatalLimit uint64,
+	groupOff, groupMembers []uint32) ([]uint8, error) {
+	if len(fileOff) != len(fileLen) || len(fileOff)%2 != 0 || len(groupOff) == 0 {
+		return nil, fmt.Errorf("kxpu_aer_health: %d offsets, %d lengths, %d group offsets", len(fileOff), len(fileLen), len(groupOff))
+	}
+	nG := len(groupOff) - 1
+	// the inputs go through C memory: cgo forbids passing several Go pointers that the callee keeps together
+	ct := (*C.uint8_t)(C.malloc(C.size_t(len(text) + 1)))
+	defer C.free(unsafe.Pointer(ct))
+	copy(unsafe.Slice((*byte)(unsafe.Pointer(ct)), len(text)), text)
+	co := (*C.uint64_t)(C.malloc(C.size_t(8 * (len(fileOff) + 1))))
+	defer C.free(unsafe.Pointer(co))
+	copy(unsafe.Slice((*uint64)(unsafe.Pointer(co)), len(fileOff)), fileOff)
+	cl := (*C.uint32_t)(C.malloc(C.size_t(4 * (len(fileLen) + 1))))
+	defer C.free(unsafe.Pointer(cl))
+	copy(unsafe.Slice((*uint32)(unsafe.Pointer(cl)), len(fileLen)), fileLen)
+	cg := (*C.uint32_t)(C.malloc(C.size_t(4 * (len(groupOff) + len(groupMembers)))))
+	defer C.free(unsafe.Pointer(cg))
+	g := unsafe.Slice((*uint32)(unsafe.Pointer(cg)), len(groupOff)+len(groupMembers))
+	copy(g, groupOff)
+	copy(g[len(groupOff):], groupMembers)
+	out := (*C.uint8_t)(C.malloc(C.size_t(nG + 1)))
+	defer C.free(unsafe.Pointer(out))
+	if err := kxCheck(k.ctx, "kxpu_aer_health", C.kxpu_aer_health(k.ctx, ct, C.size_t(len(text)), co, cl,
+		C.size_t(len(fileOff)/2), C.uint64_t(fatalLimit), C.uint64_t(nonfatalLimit), cg,
+		(*C.uint32_t)(unsafe.Add(unsafe.Pointer(cg), 4*len(groupOff))), C.size_t(nG), nil, out)); err != nil {
+		return nil, err
+	}
+	return append([]uint8(nil), unsafe.Slice((*uint8)(unsafe.Pointer(out)), nG)...), nil
+}
+
+// draSlicesTaint / draSlicesMdevTaint with the table [<driver>/unhealthy=vfio-device-missing, <driver>/pcie-aer=fatal,
+// <driver>/pcie-aer=nonfatal], all NoSchedule (ABI v12).  since holds three times per device, device-major, -1 where the
+// device does not carry that taint; a device carries at most one of the two pcie-aer values.
+func (k *kxpu) draSlicesTaints(driver, node string, generation uint64, devs []C.kxpu_dradev, since []int64) ([]string, error) {
+	var p *C.kxpu_dradev
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	return k.taintsSlices("kxpu_dra_slices_taints", driver, node, len(devs), since, func(cd, cn *C.char, tab *C.kxpu_dra_taint,
+		cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t, ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_taints(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), tab, 3, cs, out,
+			capacity, n, off, ns)
+	})
+}
+
+func (k *kxpu) draSlicesMdevTaints(driver, node string, generation uint64, devs []C.kxpu_dramdev, since []int64) ([]string, error) {
+	var p *C.kxpu_dramdev
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	return k.taintsSlices("kxpu_dra_slices_mdev_taints", driver, node, len(devs), since, func(cd, cn *C.char,
+		tab *C.kxpu_dra_taint, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
+		ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_mdev_taints(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), tab, 3, cs,
+			out, capacity, n, off, ns)
+	})
+}
+
+// the two-call sizing of one _taints call, the table and the times in C memory
+func (k *kxpu) taintsSlices(what, driver, node string, nDevs int, since []int64, call func(cd, cn *C.char,
+	tab *C.kxpu_dra_taint, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
+	ns *C.size_t) C.int32_t) ([]string, error) {
+	if len(since) != 3*nDevs {
+		return nil, fmt.Errorf("%s: %d taint times for %d devices", what, len(since), nDevs)
+	}
+	strs := []*C.char{C.CString(driver), C.CString(node), C.CString(driver + "/unhealthy"), C.CString("vfio-device-missing"),
+		C.CString(driver + "/pcie-aer"), C.CString("fatal"), C.CString("nonfatal"), C.CString("NoSchedule")}
+	for _, s := range strs {
+		defer C.free(unsafe.Pointer(s))
+	}
+	tab := (*C.kxpu_dra_taint)(C.malloc(C.size_t(3 * unsafe.Sizeof(C.kxpu_dra_taint{}))))
+	defer C.free(unsafe.Pointer(tab))
+	t := unsafe.Slice(tab, 3)
+	t[0] = C.kxpu_dra_taint{key: strs[2], value: strs[3], effect: strs[7]}
+	t[1] = C.kxpu_dra_taint{key: strs[4], value: strs[5], effect: strs[7]}
+	t[2] = C.kxpu_dra_taint{key: strs[4], value: strs[6], effect: strs[7]}
+	cs := (*C.int64_t)(C.malloc(C.size_t(8 * (len(since) + 1))))
+	defer C.free(unsafe.Pointer(cs))
+	copy(unsafe.Slice((*int64)(unsafe.Pointer(cs)), len(since)), since)
+	var n, ns C.size_t
+	if rc := call(strs[0], strs[1], tab, cs, nil, 0, &n, nil, &ns); rc != C.KXPU_E_NOSPACE { // sizing call
+		return nil, kxCheck(k.ctx, what, rc)
+	}
+	buf := make([]byte, n)
+	off := make([]uint64, ns+1)
+	if err := kxCheck(k.ctx, what, call(strs[0], strs[1], tab, cs, (*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n,
+		(*C.uint64_t)(unsafe.Pointer(&off[0])), &ns)); err != nil {
+		return nil, err
+	}
+	lines := make([]string, ns)
+	for s := range lines {
+		lines[s] = string(buf[off[s] : off[s+1]-1]) // without the '\n'
+	}
+	return lines, nil
+}

@@ -65,6 +65,15 @@ DRA_SLICE_DEVICES = 128
 DRA_MAX_DEVICES = 1 << 24
 DRA_TAINT_SLICE_DEVICES = 64  # devices per slice of the _taint calls (ABI v11) when taint_since is given
 DRA_TAINT_SINCE_MAX = 253402300799  # 9999-12-31T23:59:59Z
+DRA_MAX_TAINTS = 4  # entries of the _taints calls' table (ABI v12)
+AER_FATAL, AER_NONFATAL, AER_UNKNOWN = 1, 2, 4  # kxpu_aer_health's group bits
+AER_FILE_MAX = 4096
+AER_UNKNOWN_COUNT = (1 << 64) - 1  # totals of an unknown count
+
+
+class DraTaint(C.Structure):
+    """kxpu_dra_taint: one entry of the _taints calls' table"""
+    _fields_ = [("key", C.c_char_p), ("value", C.c_char_p), ("effect", C.c_char_p)]
 
 # every symbol include/kxpu.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -81,6 +90,7 @@ ABI_SYMBOLS = [
     "kxpu_classify_topo", "kxpu_classify_mdev_topo", "kxpu_lw_encode_topo", "kxpu_preferred_allocation",
     "kxpu_reconcile", "kxpu_pcie_tree", "kxpu_preferred_allocation_pcie", "kxpu_classify_viable",
     "kxpu_dra_slices", "kxpu_dra_slices_mdev", "kxpu_dra_slices_taint", "kxpu_dra_slices_mdev_taint",
+    "kxpu_aer_health", "kxpu_dra_slices_taints", "kxpu_dra_slices_mdev_taints",
 ]
 
 
@@ -188,6 +198,11 @@ def load_library():
                                         C.c_char_p, vp, vp, sz, C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_mdev_taint": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, C.c_char_p, C.c_char_p,
                                              C.c_char_p, vp, vp, sz, C.POINTER(sz), vp, C.POINTER(sz)]),
+        "kxpu_aer_health": (i32, [vp, vp, sz, vp, vp, sz, u64, u64, vp, vp, sz, vp, vp]),
+        "kxpu_dra_slices_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
+                                         C.POINTER(sz), vp, C.POINTER(sz)]),
+        "kxpu_dra_slices_mdev_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
+                                              C.POINTER(sz), vp, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -690,10 +705,48 @@ class Kxpu:
         return self._slices(self.L.kxpu_dra_slices_mdev_taint, DRAMDEV_DTYPE, driver, pool, node, generation, devs,
                             (key, value, effect, since))
 
-    def _slices(self, fn, dtype, driver, pool, node, generation, devs, taint=None):
+    def dra_slices_taints(self, driver, pool, node, generation, devs, taints, since):
+        """kxpu_dra_slices_taints: dra_slices with a table of taints.  taints: a list of (key, value, effect); since: None
+        (the untainted call's bytes) or an int64 [n, len(taints)] array, since[i, t] < 0 when device i does not carry
+        taint t; 64 devices per slice when given."""
+        return self._slices(self.L.kxpu_dra_slices_taints, DRADEV_DTYPE, driver, pool, node, generation, devs,
+                            taints=(taints, since))
+
+    def dra_slices_mdev_taints(self, driver, pool, node, generation, devs, taints, since):
+        """kxpu_dra_slices_mdev_taints: the same for a pool of vGPUs (DRAMDEV_DTYPE devices)."""
+        return self._slices(self.L.kxpu_dra_slices_mdev_taints, DRAMDEV_DTYPE, driver, pool, node, generation, devs,
+                            taints=(taints, since))
+
+    def aer_health(self, text, file_off, file_len, fatal_limit, nonfatal_limit, group_off, group_members):
+        """kxpu_aer_health: (totals, group_aer).  text: bytes; file_off / file_len: 2n entries, the fatal file of record i
+        at 2i and its non-fatal file at 2i+1; group_off [G+1] / group_members: the groups.  totals[2i + k] is a count or
+        AER_UNKNOWN_COUNT; group_aer[o] holds AER_* bits."""
+        t = np.frombuffer(bytes(text), np.uint8)
+        file_off = np.ascontiguousarray(file_off, dtype=np.uint64)
+        file_len = np.ascontiguousarray(file_len, dtype=np.uint32)
+        assert len(file_off) == len(file_len) and len(file_off) % 2 == 0
+        group_off = np.ascontiguousarray(group_off, dtype=np.uint32)
+        group_members = np.ascontiguousarray(group_members, dtype=np.uint32)
+        n, G = len(file_off) // 2, len(group_off) - 1
+        totals = np.empty(max(2 * n, 1), np.uint64)
+        group_aer = np.empty(max(G, 1), np.uint8)
+        self._chk(self.L.kxpu_aer_health(
+            self.ctx, _ptr(t) if len(t) else None, len(t), _ptr(file_off) if n else None, _ptr(file_len) if n else None, n,
+            fatal_limit, nonfatal_limit, _ptr(group_off), _ptr(group_members) if len(group_members) else None, G,
+            _ptr(totals), _ptr(group_aer)))
+        return totals[:2 * n], group_aer[:G]
+
+    def _slices(self, fn, dtype, driver, pool, node, generation, devs, taint=None, taints=None):
         devs = np.ascontiguousarray(devs)
         assert devs.dtype == dtype
         args = (self.ctx, _kind(driver), _kind(pool), _kind(node), generation, _ptr(devs) if len(devs) else None, len(devs))
+        if taints is not None:
+            table, since = taints
+            tab = (DraTaint * max(len(table), 1))(*[DraTaint(_kind(k), _kind(v), _kind(e)) for k, v, e in table])
+            if since is not None:
+                since = np.ascontiguousarray(since, dtype=np.int64)
+                assert since.size == len(devs) * len(table)
+            args += (C.cast(tab, C.c_void_p), len(table), _ptr(since))
         if taint is not None:
             key, value, effect, since = taint
             if since is not None:

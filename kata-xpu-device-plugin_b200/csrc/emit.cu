@@ -378,6 +378,25 @@ constexpr int TAINT_PART_MAX = TAINT_HEAD_MAX + 20 + (int)sizeof(KX_TAINT_TAIL) 
 constexpr int DRA_TAINT_POOL_MAX = DRA_POOL_MAX + 272;
 static_assert(TAINT_HEAD_MAX + (int)sizeof(KX_TAINT_TAIL) - 1 <= DRA_TAINT_POOL_MAX - DRA_POOL_MAX, "taint pool bound");
 
+// Taint lists (kxpu_dra_slices_taints / kxpu_dra_slices_mdev_taints).  A device that carries some taint ends with its
+// last literal less its final '}', then KX_TAINTS_OPEN, for each carried taint in table order its entry head (the
+// table's key, value and effect, assembled on the host), the 20-byte timeAdded and KX_TAINT_ECLOSE, with ',' between
+// entries, then KX_TAINTS_CLOSE.  One entry gives the _taint calls' bytes.
+#define KX_TAINTS_OPEN ",\"taints\":["
+#define KX_TAINT_ECLOSE "\"}"
+#define KX_TAINTS_CLOSE "]}"
+constexpr int TAINT_ENTRY_MAX =  // {"key":"<key>","value":"<value>","effect":"<effect>","timeAdded":"  at the longest
+    (int)sizeof("{\"key\":\"\",\"value\":\"\",\"effect\":\"\",\"timeAdded\":\"") - 1 + 127 + 63 + 10;
+constexpr int TAINTS_PART_MAX = (int)sizeof(KX_TAINTS_OPEN) - 1 +
+                                KXPU_DRA_MAX_TAINTS * (TAINT_ENTRY_MAX + 20 + (int)sizeof(KX_TAINT_ECLOSE) - 1 + 1) - 1 +
+                                (int)sizeof(KX_TAINTS_CLOSE) - 1 - 1;  // less one ',' and the '}' it replaces
+constexpr int DRA_TAINTS_POOL_MAX = DRA_POOL_MAX + 1024;
+static_assert((int)sizeof(KX_TAINTS_OPEN KX_TAINT_ECLOSE KX_TAINTS_CLOSE) - 1 + KXPU_DRA_MAX_TAINTS * TAINT_ENTRY_MAX <=
+                  DRA_TAINTS_POOL_MAX - DRA_POOL_MAX,
+              "taint list pool bound");
+// k_dra_slices' taint mode: no taint, one taint for the call (the _taint calls), a table of taints (the _taints calls)
+constexpr int DRA_UNTAINTED = 0, DRA_TAINT_ONE = 1, DRA_TAINT_LIST = 2;
+
 // PARTS = literals + head + tail; the head is part PARTS - 2, the tail PARTS - 1
 template <int PARTS, int POOL = DRA_POOL_MAX>
 struct DraParams {
@@ -396,6 +415,14 @@ struct DraParams {
 template <int PARTS>
 struct DraTaintParams : DraParams<PARTS, DRA_TAINT_POOL_MAX> {
     const long long *since;  // [n]: the taint's unix time, < 0 = untainted
+};
+// the taint list instantiations: the literals, KX_TAINTS_OPEN (part PARTS - 9), the entry heads (PARTS - 8 ..
+// PARTS - 5), KX_TAINT_ECLOSE, KX_TAINTS_CLOSE, the slice head and tail
+template <int PARTS>
+struct DraTaintsParams : DraParams<PARTS, DRA_TAINTS_POOL_MAX> {
+    const long long *since;            // [n * nt], device-major: taint t of device i, < 0 = not carried
+    uint32_t nt;                       // table entries, 1..KXPU_DRA_MAX_TAINTS
+    uint8_t dup[KXPU_DRA_MAX_TAINTS];  // dup[t]: the earlier entries with taint t's key and effect
 };
 constexpr int DRA_F_PRODUCT = 0, DRA_F_BDF = 1, DRA_F_ROOT = 2, DRA_F_VENDOR = 3, DRA_F_DEVICE = 4, DRA_F_GROUP = 5,
               DRA_F_PLEN = 6, DRA_F_COUNT = 7;
@@ -431,27 +458,42 @@ template <typename Base>
 struct DraTaintSmem : Base {
     uint8_t ts[TAINT_TILE][20];  // timeAdded of device d; ts[d][0] == 0: untainted
 };
+template <typename Base>
+struct DraTaintsSmem : Base {
+    uint8_t ts[TAINT_TILE][KXPU_DRA_MAX_TAINTS][20];  // timeAdded of taint t of device d
+    uint8_t carried[TAINT_TILE];                      // bit t: device d carries taint t
+};
 template <int LAYOUT> struct DraLayout {  // LAYOUT_PCI
     using Rec = kxpu_dradev;
     using Smem = DraSmem<>;
     using TaintSmem = DraTaintSmem<DraSmem<TAINT_TILE, MAX_FRAG_DRA + TAINT_PART_MAX, DRA_TAINT_POOL_MAX>>;
+    using TaintsSmem = DraTaintsSmem<DraSmem<TAINT_TILE, MAX_FRAG_DRA + TAINTS_PART_MAX, DRA_TAINTS_POOL_MAX>>;
     static constexpr int PARTS = DRA_PARTS, LAST = 8, F_COUNT = DRA_F_COUNT;
 };
 template <> struct DraLayout<LAYOUT_MDEV> {
     using Rec = kxpu_dramdev;
     using Smem = DraMdevSmem<>;
     using TaintSmem = DraTaintSmem<DraMdevSmem<TAINT_TILE, MAX_FRAG_DRA_MDEV + TAINT_PART_MAX, DRA_TAINT_POOL_MAX>>;
+    using TaintsSmem = DraTaintsSmem<DraMdevSmem<TAINT_TILE, MAX_FRAG_DRA_MDEV + TAINTS_PART_MAX, DRA_TAINTS_POOL_MAX>>;
     static constexpr int PARTS = DRAM_PARTS, LAST = DRAM_E, F_COUNT = DRAM_F_COUNT;
 };
-// one k_dra_slices instantiation: LAST is the literal that closes a device; a taint reports F_SINCE
-template <int LAYOUT, bool TAINT> struct DraKernel {
+// one k_dra_slices instantiation: LAST is the literal that closes a device; a taint time above the maximum reports
+// F_SINCE, a device with two taints of one key and effect F_DUP
+template <int LAYOUT, int MODE> struct DraKernel {
+    static constexpr bool TAINT = MODE != DRA_UNTAINTED, LIST = MODE == DRA_TAINT_LIST;
     static constexpr int T = TAINT ? TAINT_TILE : TILE;
-    static constexpr int PARTS = DraLayout<LAYOUT>::PARTS + (TAINT ? 2 : 0);
+    static constexpr int PARTS = DraLayout<LAYOUT>::PARTS + (LIST ? 7 : TAINT ? 2 : 0);
     static constexpr int TAINT_HEAD = PARTS - 4, TAINT_TAIL = PARTS - 3, F_SINCE = DraLayout<LAYOUT>::F_COUNT;
-    static constexpr int POOL = TAINT ? DRA_TAINT_POOL_MAX : DRA_POOL_MAX;
-    static constexpr int MAXF = (LAYOUT == LAYOUT_PCI ? MAX_FRAG_DRA : MAX_FRAG_DRA_MDEV) + (TAINT ? TAINT_PART_MAX : 0);
-    using Params = std::conditional_t<TAINT, DraTaintParams<PARTS>, DraParams<PARTS>>;
-    using Smem = std::conditional_t<TAINT, typename DraLayout<LAYOUT>::TaintSmem, typename DraLayout<LAYOUT>::Smem>;
+    static constexpr int T_OPEN = PARTS - 9, T_ENTRY = PARTS - 8, T_ECLOSE = PARTS - 4, T_CLOSE = PARTS - 3;
+    static constexpr int F_DUP = F_SINCE + 1, F_COUNT = DraLayout<LAYOUT>::F_COUNT + (LIST ? 2 : TAINT ? 1 : 0);
+    static constexpr int POOL = LIST ? DRA_TAINTS_POOL_MAX : TAINT ? DRA_TAINT_POOL_MAX : DRA_POOL_MAX;
+    static constexpr int MAXF = (LAYOUT == LAYOUT_PCI ? MAX_FRAG_DRA : MAX_FRAG_DRA_MDEV) +
+                                (LIST ? TAINTS_PART_MAX : TAINT ? TAINT_PART_MAX : 0);
+    using Params = std::conditional_t<LIST, DraTaintsParams<PARTS>,
+                                      std::conditional_t<TAINT, DraTaintParams<PARTS>, DraParams<PARTS>>>;
+    using Smem = std::conditional_t<LIST, typename DraLayout<LAYOUT>::TaintsSmem,
+                                    std::conditional_t<TAINT, typename DraLayout<LAYOUT>::TaintSmem,
+                                                       typename DraLayout<LAYOUT>::Smem>>;
 };
 
 template <int W>
@@ -497,11 +539,12 @@ __device__ __forceinline__ void rfc3339(unsigned long long t, uint8_t *o) {
     o[19] = (uint8_t)'Z';
 }
 
-// TAINT = false: kxpu_dra_slices[_mdev], TILE devices per slice.  TAINT = true: the _taint calls, TAINT_TILE devices per
-// slice and the taint part after a tainted device's attributes; everything it adds sits behind `if constexpr`.
-template <int LAYOUT, bool TAINT = false>
-__global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_constant__ typename DraKernel<LAYOUT, TAINT>::Params E) {
-    using K = DraKernel<LAYOUT, TAINT>;
+// MODE = DRA_UNTAINTED: kxpu_dra_slices[_mdev], TILE devices per slice.  DRA_TAINT_ONE: the _taint calls, TAINT_TILE
+// devices per slice and the taint part after a tainted device's attributes.  DRA_TAINT_LIST: the _taints calls, the same
+// slices with a list of taints.  Everything a mode adds sits behind `if constexpr`.
+template <int LAYOUT, int MODE = DRA_UNTAINTED>
+__global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_constant__ typename DraKernel<LAYOUT, MODE>::Params E) {
+    using K = DraKernel<LAYOUT, MODE>;
     using Rec = typename DraLayout<LAYOUT>::Rec;
     constexpr int HEAD = K::PARTS - 2, TAIL = K::PARTS - 1, T = K::T;
     extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -611,7 +654,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
                    (pl ? E.len[7] + pl + ls : 0u) + (rl ? E.len[8] + rl + ls : 0u) + (tid + 1u < in_slice ? 1u : 0u);
         }
     }
-    if constexpr (TAINT) {  // the taint's time, range-checked and formatted beside the record
+    if constexpr (MODE == DRA_TAINT_ONE) {  // the taint's time, range-checked and formatted beside the record
         if (tid < in_slice) {
             const long long since = E.since[i0 + tid];
             if (since > TAINT_SINCE_MAX) E.flags[K::F_SINCE] = 1u;
@@ -620,6 +663,23 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
                 rfc3339((unsigned long long)since, S.ts[tid]);
                 flen += E.len[K::TAINT_HEAD] + 20u + E.len[K::TAINT_TAIL] - 1u;
             }
+        }
+    }
+    if constexpr (MODE == DRA_TAINT_LIST) {  // the device's row of the table: which taints it carries, and their times
+        if (tid < in_slice) {
+            const long long *row = E.since + (size_t)(i0 + tid) * E.nt;
+            uint32_t carried = 0, part = 0;
+            for (uint32_t t = 0; t < E.nt; t++) {
+                const long long since = row[t];
+                if (since > TAINT_SINCE_MAX) E.flags[K::F_SINCE] = 1u;
+                if (since < 0 || since > TAINT_SINCE_MAX) continue;
+                if (carried & E.dup[t]) E.flags[K::F_DUP] = 1u;
+                rfc3339((unsigned long long)since, S.ts[tid][t]);
+                part += (carried ? 1u : 0u) + E.len[K::T_ENTRY + t] + 20u + E.len[K::T_ECLOSE];
+                carried |= 1u << t;
+            }
+            S.carried[tid] = (uint8_t)carried;
+            if (carried) flen += E.len[K::T_OPEN] + part + E.len[K::T_CLOSE] - 1u;
         }
     }
     // ---- scan of the 128 lengths (threads >= TILE contribute 0)
@@ -665,7 +725,24 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
         auto lit = [&](int k) { put(S.pool + E.off[k], E.len[k]); };
         // the literal that closes the device (K's LAST); a tainted device's taint part goes before its final '}'
         auto close = [&](int k) {
-            if constexpr (TAINT) {
+            if constexpr (MODE == DRA_TAINT_LIST) {
+                const uint32_t carried = S.carried[d];
+                if (carried) {
+                    put(S.pool + E.off[k], E.len[k] - 1u);
+                    lit(K::T_OPEN);
+                    for (uint32_t t = 0; t < (uint32_t)KXPU_DRA_MAX_TAINTS; t++) {
+                        if (!((carried >> t) & 1u)) continue;
+                        if (carried & ((1u << t) - 1u)) {
+                            if (lane == 0) dst[o] = (uint8_t)',';
+                            o += 1u;
+                        }
+                        lit(K::T_ENTRY + t); put(S.ts[d][t], 20u); lit(K::T_ECLOSE);
+                    }
+                    lit(K::T_CLOSE);
+                    return;
+                }
+            }
+            if constexpr (MODE == DRA_TAINT_ONE) {
                 if (S.ts[d][0]) {
                     put(S.pool + E.off[k], E.len[k] - 1u);
                     lit(K::TAINT_HEAD); put(S.ts[d], 20u); lit(K::TAINT_TAIL);
@@ -1134,24 +1211,37 @@ static bool taint_value_ok(const char *v) {
     return len == 0 || k8s_name_ok(v, len, 63);
 }
 
-// the taint arguments of the _taint calls; since == NULL: the untainted call
+static bool taint_ok(const kxpu_dra_taint &t) {
+    return taint_key_ok(t.key) && taint_value_ok(t.value) && t.effect &&
+           (strcmp(t.effect, "NoSchedule") == 0 || strcmp(t.effect, "NoExecute") == 0);
+}
+// {"key":"<key>"[,"value":"<value>"],"effect":"<effect>","timeAdded":"  -- one taint up to its time
+static std::string taint_entry(const kxpu_dra_taint &t) {
+    std::string s = std::string("{\"key\":\"") + t.key + "\"";
+    if (t.value[0]) s += std::string(",\"value\":\"") + t.value + "\"";
+    return s + ",\"effect\":\"" + t.effect + "\",\"timeAdded\":\"";
+}
+
+// the taint arguments of the _taint (one entry) and _taints calls; since == NULL: the untainted call
 struct DraTaint {
-    const char *key, *value, *effect;
-    const int64_t *since;
+    const kxpu_dra_taint *table;
+    size_t n;
+    const int64_t *since;  // [devices * n]
 };
 
-// kxpu_dra_slices[_mdev][_taint]: the argument checks, the pool (literals | [taint head | taint tail |] head | tail),
-// one k_dra_slices<LAYOUT, TAINT> launch, the domain flags and the copies
-template <int LAYOUT, bool TAINT = false>
+// kxpu_dra_slices[_mdev][_taint[s]]: the argument checks, the pool (literals | taint parts | head | tail), one
+// k_dra_slices<LAYOUT, MODE> launch, the domain flags and the copies
+template <int LAYOUT, int MODE = DRA_UNTAINTED>
 static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, const char *pool, const char *node,
                           uint64_t generation, const typename DraLayout<LAYOUT>::Rec *devs, size_t n, uint8_t *out, size_t cap,
                           size_t *len, uint64_t *slice_off, size_t *n_slices, const DraTaint &taint = DraTaint{}) {
     using Rec = typename DraLayout<LAYOUT>::Rec;
-    using K = DraKernel<LAYOUT, TAINT>;
+    using K = DraKernel<LAYOUT, MODE>;
+    constexpr bool TAINT = K::TAINT;
     constexpr int PARTS = K::PARTS, HEAD = PARTS - 2, TAIL = PARTS - 1;
     constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : DRAM_LITS;
     constexpr int MAXF = K::MAXF;
-    constexpr int F_COUNT = DraLayout<LAYOUT>::F_COUNT + (TAINT ? 1 : 0);
+    constexpr int F_COUNT = K::F_COUNT;
     const char *const *lits = LAYOUT == LAYOUT_PCI ? h_dra_lits : h_dram_lits;
     if (!ctx || !len || !n_slices || (n && !devs)) return KXPU_E_INVALID;
     if (!dns_subdomain_ok(driver, 63) || !dns_subdomain_ok(pool, 253) || !dns_subdomain_ok(node, 253) ||
@@ -1160,12 +1250,16 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
                         "and generation below 2^63", what);
         return KXPU_E_INVALID;
     }
-    if (TAINT && (!taint_key_ok(taint.key) || !taint_value_ok(taint.value) || !taint.effect ||
-                  (strcmp(taint.effect, "NoSchedule") != 0 && strcmp(taint.effect, "NoExecute") != 0))) {
-        KX_SET_ERR(ctx, "%s: taint_key must be a qualified name of at most 127 bytes, taint_value empty or a label value "
-                        "and taint_effect NoSchedule or NoExecute", what);
+    if (K::LIST && (!taint.table || taint.n == 0 || taint.n > KXPU_DRA_MAX_TAINTS)) {
+        KX_SET_ERR(ctx, "%s: taints must hold 1..%d entries", what, KXPU_DRA_MAX_TAINTS);
         return KXPU_E_INVALID;
     }
+    for (size_t t = 0; TAINT && t < taint.n; t++)
+        if (!taint_ok(taint.table[t])) {
+            KX_SET_ERR(ctx, "%s: taint %zu: the key must be a qualified name of at most 127 bytes, the value empty or a "
+                            "label value and the effect NoSchedule or NoExecute", what, t);
+            return KXPU_E_INVALID;
+        }
     if (n >= KXPU_DRA_MAX_DEVICES) {
         KX_SET_ERR(ctx, "%s: n = %zu is not below %u", what, n, KXPU_DRA_MAX_DEVICES);
         return KXPU_E_UNSUPPORTED;
@@ -1180,21 +1274,22 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
                              "\",\"generation\":" + std::to_string(generation) +
                              ",\"resourceSliceCount\":" + std::to_string(slices) + "},\"nodeName\":\"" + nd +
                              "\",\"devices\":[";
-    std::string taint_head;
-    if (TAINT) {
-        taint_head = std::string(",\"taints\":[{\"key\":\"") + taint.key + "\"";
-        if (taint.value[0]) taint_head += std::string(",\"value\":\"") + taint.value + "\"";
-        taint_head += std::string(",\"effect\":\"") + taint.effect + "\",\"timeAdded\":\"";
+    // the taint parts, from part LITS on: DRA_TAINT_ONE the taint head and tail, DRA_TAINT_LIST KX_TAINTS_OPEN, four
+    // entry heads (empty past the table), KX_TAINT_ECLOSE and KX_TAINTS_CLOSE
+    std::vector<std::string> taint_parts;
+    if (MODE == DRA_TAINT_ONE) taint_parts = {KX_TAINTS_OPEN + taint_entry(taint.table[0]), KX_TAINT_TAIL};
+    if (MODE == DRA_TAINT_LIST) {
+        taint_parts.push_back(KX_TAINTS_OPEN);
+        for (size_t t = 0; t < KXPU_DRA_MAX_TAINTS; t++) taint_parts.push_back(t < taint.n ? taint_entry(taint.table[t]) : "");
+        taint_parts.push_back(KX_TAINT_ECLOSE);
+        taint_parts.push_back(KX_TAINTS_CLOSE);
     }
     typename K::Params E;
     memset(&E, 0, sizeof E);
     uint32_t acc = 0;
     for (int k = 0; k < PARTS; k++) {
-        const std::string s = k < LITS                       ? std::string(lits[k])
-                              : k == HEAD                    ? head
-                              : k == TAIL                    ? std::string(KX_DRA_TAIL)
-                              : k == LITS                    ? taint_head
-                                                             : std::string(KX_TAINT_TAIL);
+        const std::string s = k < LITS ? std::string(lits[k]) : k == HEAD ? head : k == TAIL ? std::string(KX_DRA_TAIL)
+                                                                                  : taint_parts[k - LITS];
         if (acc + s.size() > (size_t)K::POOL) return KXPU_E_INVALID;  // the literals grew: the pool bound must follow
         memcpy(E.pool + acc, s.data(), s.size());
         E.off[k] = (uint16_t)acc;
@@ -1206,7 +1301,7 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     const size_t smem = sizeof(typename K::Smem);
     static bool attr_done = false;
     if (!attr_done) {
-        cudaFuncSetAttribute(k_dra_slices<LAYOUT, TAINT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaFuncSetAttribute(k_dra_slices<LAYOUT, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         attr_done = true;
     }
     KxScratch sc(ctx);
@@ -1222,16 +1317,23 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     E.devs = d_devs; E.n = N; E.out = d_out; E.slice_off = d_ctl; E.flags = (uint32_t *)(d_ctl + slices + 1);
     if constexpr (TAINT) {
         long long *d_since = nullptr;
-        KX_CUDA(ctx, sc.alloc((void **)&d_since, n * sizeof(long long)));
-        if (n) cudaMemcpyAsync(d_since, taint.since, n * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream);
+        KX_CUDA(ctx, sc.alloc((void **)&d_since, n * taint.n * sizeof(long long)));
+        if (n) cudaMemcpyAsync(d_since, taint.since, n * taint.n * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream);
         E.since = d_since;
+    }
+    if constexpr (K::LIST) {
+        E.nt = (uint32_t)taint.n;
+        for (size_t t = 0; t < taint.n; t++)
+            for (size_t j = 0; j < t; j++)
+                if (strcmp(taint.table[t].key, taint.table[j].key) == 0 && strcmp(taint.table[t].effect, taint.table[j].effect) == 0)
+                    E.dup[t] |= (uint8_t)(1u << j);
     }
     E.state = kx_scan_state(ctx, slices);
     if (!E.state) return KXPU_E_NOMEM;
     E.epoch = kx_next_epoch(ctx);
     {
         KxTimer tm(ctx, KXPU_T_EMIT);
-        k_dra_slices<LAYOUT, TAINT><<<slices, EMIT_THREADS, smem, ctx->stream>>>(E);
+        k_dra_slices<LAYOUT, MODE><<<slices, EMIT_THREADS, smem, ctx->stream>>>(E);
         KX_LAUNCHED(ctx);
     }
     std::vector<unsigned long long> h(ctl_words);
@@ -1251,7 +1353,10 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     const uint32_t *flags = reinterpret_cast<const uint32_t *>(h.data() + slices + 1);
     for (int f = 0; f < F_COUNT; f++)
         if (flags[f]) {
-            KX_SET_ERR(ctx, "%s: %s", what, f == K::F_SINCE ? "a taint_since above 253402300799 (9999-12-31T23:59:59Z)" : why[f]);
+            KX_SET_ERR(ctx, "%s: %s", what,
+                       f == K::F_SINCE ? "a taint_since above 253402300799 (9999-12-31T23:59:59Z)"
+                       : f == K::F_DUP ? "a device carries two taints with the same key and effect"
+                                       : why[f]);
             return KXPU_E_UNSUPPORTED;
         }
     const size_t total = (size_t)h[slices];
@@ -1292,8 +1397,9 @@ extern "C" int32_t kxpu_dra_slices_taint(kxpu_ctx *ctx, const char *driver, cons
                                          const char *taint_value, const char *taint_effect, const int64_t *taint_since,
                                          uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
     if (!taint_since) return kxpu_dra_slices(ctx, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
-    return dra_slices<LAYOUT_PCI, true>(ctx, "dra_slices_taint", driver, pool, node, generation, devs, n, out, cap, len,
-                                        slice_off, n_slices, DraTaint{taint_key, taint_value, taint_effect, taint_since});
+    const kxpu_dra_taint t{taint_key, taint_value, taint_effect};
+    return dra_slices<LAYOUT_PCI, DRA_TAINT_ONE>(ctx, "dra_slices_taint", driver, pool, node, generation, devs, n, out, cap,
+                                                 len, slice_off, n_slices, DraTaint{&t, 1, taint_since});
 }
 
 extern "C" int32_t kxpu_dra_slices_mdev_taint(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
@@ -1302,6 +1408,27 @@ extern "C" int32_t kxpu_dra_slices_mdev_taint(kxpu_ctx *ctx, const char *driver,
                                               uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
     if (!taint_since)
         return kxpu_dra_slices_mdev(ctx, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
-    return dra_slices<LAYOUT_MDEV, true>(ctx, "dra_slices_mdev_taint", driver, pool, node, generation, devs, n, out, cap, len,
-                                         slice_off, n_slices, DraTaint{taint_key, taint_value, taint_effect, taint_since});
+    const kxpu_dra_taint t{taint_key, taint_value, taint_effect};
+    return dra_slices<LAYOUT_MDEV, DRA_TAINT_ONE>(ctx, "dra_slices_mdev_taint", driver, pool, node, generation, devs, n, out,
+                                                  cap, len, slice_off, n_slices, DraTaint{&t, 1, taint_since});
+}
+
+// taint_since == NULL: exactly the untainted call, the taint arguments unread
+extern "C" int32_t kxpu_dra_slices_taints(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                          uint64_t generation, const kxpu_dradev *devs, size_t n, const kxpu_dra_taint *taints,
+                                          size_t n_taints, const int64_t *taint_since, uint8_t *out, size_t cap, size_t *len,
+                                          uint64_t *slice_off, size_t *n_slices) {
+    if (!taint_since) return kxpu_dra_slices(ctx, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
+    return dra_slices<LAYOUT_PCI, DRA_TAINT_LIST>(ctx, "dra_slices_taints", driver, pool, node, generation, devs, n, out, cap,
+                                                  len, slice_off, n_slices, DraTaint{taints, n_taints, taint_since});
+}
+
+extern "C" int32_t kxpu_dra_slices_mdev_taints(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                               uint64_t generation, const kxpu_dramdev *devs, size_t n,
+                                               const kxpu_dra_taint *taints, size_t n_taints, const int64_t *taint_since,
+                                               uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
+    if (!taint_since)
+        return kxpu_dra_slices_mdev(ctx, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
+    return dra_slices<LAYOUT_MDEV, DRA_TAINT_LIST>(ctx, "dra_slices_mdev_taints", driver, pool, node, generation, devs, n, out,
+                                                   cap, len, slice_off, n_slices, DraTaint{taints, n_taints, taint_since});
 }

@@ -86,6 +86,21 @@ static bool readNumaNodeFunc(const std::string &base, const std::string &entry, 
     return true;
 }
 
+// <base>/<entry>/<name>, at most KXPU_AER_FILE_MAX + 1 bytes (one more than a count is read from, so a longer file
+// stays longer).  Quiet: a missing file only means "count unknown" (no AER capability, or a kernel before 4.19).
+static bool readAerFileFunc(const std::string &base, const std::string &entry, const std::string &name, std::string &out) {
+    const std::string path = base + "/" + entry + "/" + name;
+    FILE *f = fopen(path.c_str(), "rb");
+    if (!f) return false;
+    char buf[KXPU_AER_FILE_MAX + 1];
+    size_t n = fread(buf, 1, sizeof buf, f);
+    bool err = ferror(f) != 0;
+    fclose(f);
+    if (err) return false;
+    out.assign(buf, n);
+    return true;
+}
+
 // the numa_node rule of include/kxpu.h: one trailing '\n' stripped, then a canonical decimal 0..63
 static bool parseNumaNode(const std::string &raw, uint8_t &node) {
     std::string s = raw;
@@ -140,6 +155,7 @@ static void numaRecord(ReadNuma readNuma, uint8_t &flags, uint8_t &node) {
 
 Plugin::Plugin(kxpu_ctx *ctx) : ctx_(ctx) {
     readNumaNode = readNumaNodeFunc;
+    readAerFile = readAerFileFunc;
     readPciPath = readPciPathFunc;
     readLink = readLinkFunc;
     readIDFromFile = readIDFromFileFunc;
@@ -1253,7 +1269,11 @@ Error Plugin::generateMdevCDISpec(const std::string &format) {
 // createDevicePlugins, device_plugin.go:83-112 (nothing is started: no gRPC here)
 Error Plugin::createDevicePlugins() {
     std::vector<GenericDevicePlugin> dps;
-    Error e = buildPlugins(dps);
+    Error e = computeAer();  // the start-up walks are done: their AER counts
+    if (e) return e;
+    bool pt = false, vg = false;  // the first publication: generations stay 1
+    updateAerTaints(pt, vg);
+    e = buildPlugins(dps);
     devicePlugins.assign(std::make_move_iterator(dps.begin()), std::make_move_iterator(dps.end()));
     return e;
 }
@@ -1283,6 +1303,15 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
     std::map<std::string, std::string> blockerOfGroup;  // group id -> its first blocker (groupViability)
     for (size_t g = 0; g < iommuBlocker.size() && g < iommuMap.size(); g++)
         if (!iommuBlocker[g].empty()) blockerOfGroup[iommuMap[g].first] = iommuBlocker[g];
+    std::map<std::string, std::string> aerOfGroup, aerOfMdevGroup;  // group id -> its AER reason (aerHealth)
+    for (size_t g = 0; g < iommuAer.size() && g < iommuMap.size(); g++)
+        if (!iommuAer[g].empty()) aerOfGroup[iommuMap[g].first] = iommuAer[g];
+    for (size_t g = 0; g < mdevAer.size() && g < mdevMap.size(); g++)
+        if (!mdevAer[g].empty()) aerOfMdevGroup[mdevMap[g].first] = mdevAer[g];
+    auto aerOf = [](const std::map<std::string, std::string> &m, const std::string &g) {
+        auto it = m.find(g);
+        return it == m.end() ? std::string() : it->second;
+    };
     size_t at = 0;
     for (const auto &kv : deviceMap) {  // :91
         GenericDevicePlugin dp;
@@ -1290,7 +1319,8 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         dp.resourceNamespace = xpuClasses[dp.xpuClass].resourceNamespace;
         for (const std::string &dev : kv.second) {  // :93-98
             auto it = blockerOfGroup.find(dev);
-            dp.devs.push_back(Device{dev, kHealthy, maskOf(numaOf, dev), pcieNodeOf(dev), it == blockerOfGroup.end() ? std::string() : it->second});
+            dp.devs.push_back(Device{dev, kHealthy, maskOf(numaOf, dev), pcieNodeOf(dev),
+                                     it == blockerOfGroup.end() ? std::string() : it->second, aerOf(aerOfGroup, dev)});
         }
         std::string devpluginName = names[at++];
         if (devpluginName.empty()) {
@@ -1308,7 +1338,10 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         dp.vgpu = true;
         dp.xpuClass = typeClass[t];
         dp.resourceNamespace = vgpuClasses[dp.xpuClass].resourceNamespace;
-        for (const std::string &g : typeMap[t].second) dp.devs.push_back(Device{g, kHealthy, maskOf(mdevNumaOf, g)});
+        for (const std::string &g : typeMap[t].second) {
+            dp.devs.push_back(Device{g, kHealthy, maskOf(mdevNumaOf, g)});
+            dp.devs.back().aer = aerOf(aerOfMdevGroup, g);
+        }
         dp.devpluginName = typeMap[t].first;
         dp.devicePath = "/dev/vfio/";  // an mdev has its own IOMMU group and /dev/vfio/<group>
         dp.socketPath = std::string(kDevicePluginPath) + "kata-xpu-" + dp.devpluginName + ".sock";
@@ -1416,6 +1449,8 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         if (e) return e;
         buildMdevMaps(mw, &midx);
     }
+    e = computeAer();  // a re-enumerated function starts with zeroed counters
+    if (e) return e;
     // 4. the CDI specs: a file is rewritten only when its bytes changed, atomically
     atomicSpecs_ = true;
     specsWritten_.clear();
@@ -1454,7 +1489,7 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         bool same = cur.size() == w.devs.size();
         for (size_t i = 0; same && i < cur.size(); i++)
             same = cur[i].ID == w.devs[i].ID && cur[i].Health == w.devs[i].Health && cur[i].numa == w.devs[i].numa &&
-                   cur[i].pcieNode == w.devs[i].pcieNode && cur[i].blocker == w.devs[i].blocker;
+                   cur[i].pcieNode == w.devs[i].pcieNode && cur[i].blocker == w.devs[i].blocker && cur[i].aer == w.devs[i].aer;
         if (!same) {
             cur = std::move(w.devs);
             report.changedPlugins.push_back(at);
@@ -1475,8 +1510,10 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     }
     bool passthroughChanged = false, vgpuChanged = false;
     for (size_t k : report.changedPlugins) (devicePlugins[k].vgpu ? vgpuChanged : passthroughChanged) = true;
-    if (passthroughChanged || viabilityChanged) draGeneration_++;  // the ResourceSlices of the next publication replace these
-    if (vgpuChanged) draVgpuGeneration_++;
+    bool aerPt = false, aerVg = false;
+    updateAerTaints(aerPt, aerVg);
+    if (passthroughChanged || viabilityChanged || aerPt) draGeneration_++;  // the next publication replaces these slices
+    if (vgpuChanged || aerVg) draVgpuGeneration_++;
     // 6. a fresh snapshot generation: Allocate answers from the snapshot again
     haveWalkGen_ = haveGen;
     walkGen_ = gen;
@@ -1596,6 +1633,34 @@ static Error draTaintSlices(kxpu_ctx *ctx,
     return Error();
 }
 
+// With aerHealth too, the table of the _taints calls: the device-node taint, then the AER taint's two values.  The two
+// AER entries share key and effect, so a group carries at most one of them.
+static const char *kAerTaintKeyName = "/pcie-aer";  // the key is <draDriver>/pcie-aer
+template <typename Rec>
+static Error draTaintsSlices(kxpu_ctx *ctx,
+                             int32_t (*fn)(kxpu_ctx *, const char *, const char *, const char *, uint64_t, const Rec *, size_t,
+                                           const kxpu_dra_taint *, size_t, const int64_t *, uint8_t *, size_t, size_t *,
+                                           uint64_t *, size_t *),
+                             const char *what, const std::string &driver, const std::string &node, uint64_t generation,
+                             const std::vector<Rec> &devs, const std::vector<int64_t> &since, std::vector<uint8_t> &out,
+                             std::vector<uint64_t> &sliceOff) {
+    const std::string missing = driver + kDraTaintKeyName, aer = driver + kAerTaintKeyName;
+    const kxpu_dra_taint table[3] = {{missing.c_str(), kDraTaintValue, kDraTaintEffect},
+                                     {aer.c_str(), "fatal", kDraTaintEffect},
+                                     {aer.c_str(), "nonfatal", kDraTaintEffect}};
+    size_t len = 0, nSlices = 0;
+    int32_t rc = fn(ctx, driver.c_str(), node.c_str(), node.c_str(), generation, devs.data(), devs.size(), table, 3,
+                    since.data(), nullptr, 0, &len, nullptr, &nSlices);
+    if (rc == KXPU_E_NOSPACE) {
+        out.assign(len, 0);
+        sliceOff.assign(nSlices + 1, 0);
+        rc = fn(ctx, driver.c_str(), node.c_str(), node.c_str(), generation, devs.data(), devs.size(), table, 3,
+                since.data(), out.data(), out.size(), &len, sliceOff.data(), &nSlices);
+    }
+    if (rc != KXPU_OK) return kxfail(ctx, what, rc);
+    return Error();
+}
+
 Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) {
     std::shared_lock<std::shared_mutex> lock(mu_);
     if (xpuClass >= xpuClasses.size() || xpuClasses[xpuClass].draDriver.empty())
@@ -1618,6 +1683,9 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
         devs.push_back(d);
         groups.push_back(iommuMap[g].first);
     }
+    if (draTaints && aerHealth)
+        return draTaintsSlices(ctx_, kxpu_dra_slices_taints, "kxpu_dra_slices_taints", driver, nodeName, draGeneration_, devs,
+                               draSinceTable(groups), out, sliceOff);
     if (draTaints) return draTaintSlices(ctx_, kxpu_dra_slices_taint, "kxpu_dra_slices_taint", driver, nodeName,
                                          draGeneration_, devs, draSince(groups), out, sliceOff);
     size_t len = 0, nSlices = 0;
@@ -1640,6 +1708,124 @@ std::vector<int64_t> Plugin::draSince(const std::vector<std::string> &groups) co
         since.push_back(it == draTaintSince_.end() ? -1 : it->second);
     }
     return since;
+}
+
+std::vector<int64_t> Plugin::draSinceTable(const std::vector<std::string> &groups) const {
+    std::vector<int64_t> since;
+    for (const std::string &g : groups) {
+        auto it = draTaintSince_.find(g);
+        auto at = aerTaint_.find(g);
+        const uint8_t v = at == aerTaint_.end() ? 0 : at->second.first;
+        since.push_back(it == draTaintSince_.end() ? -1 : it->second);
+        since.push_back(v == KXPU_AER_FATAL ? at->second.second : -1);
+        since.push_back(v == KXPU_AER_NONFATAL ? at->second.second : -1);
+    }
+    return since;
+}
+
+Error Plugin::computeAer() {
+    iommuAer.assign(iommuMap.size(), std::string());
+    iommuAerBits.assign(iommuMap.size(), 0);
+    mdevAer.assign(mdevMap.size(), std::string());
+    mdevAerBits.assign(mdevMap.size(), 0);
+    if (!aerHealth) return Error();  // no aer_dev_* file is opened
+    // one record per member of every group, passthrough groups then vGPU groups; a vGPU reads its parent's files
+    std::string text;
+    std::vector<uint64_t> off;
+    std::vector<uint32_t> len, goff{0}, members;
+    std::vector<std::string> who;  // the function whose files record i read
+    auto read = [&](const std::string &base, const std::string &entry, const std::string &fn) {
+        for (const char *name : {"aer_dev_fatal", "aer_dev_nonfatal"}) {
+            std::string s;
+            aerReads++;
+            if (!readAerFile || !readAerFile(base, entry, name, s)) s.clear();
+            if (s.size() > KXPU_AER_FILE_MAX + 1) s.resize(KXPU_AER_FILE_MAX + 1);
+            off.push_back(text.size());
+            len.push_back((uint32_t)s.size());
+            text += s;
+        }
+        members.push_back((uint32_t)who.size());
+        who.push_back(fn);
+    };
+    for (const auto &kv : iommuMap) {
+        for (const NvidiaGpuDevice &d : kv.second) read(basePath, d.addr, d.addr);
+        goff.push_back((uint32_t)members.size());
+    }
+    for (const auto &kv : mdevMap) {
+        for (const MdevDevice &m : kv.second) read(mdevBasePath, m.uuid + "/..", m.parent);
+        goff.push_back((uint32_t)members.size());
+    }
+    const size_t n = who.size(), G = goff.size() - 1;
+    std::vector<uint64_t> totals(2 * n + 1);
+    std::vector<uint8_t> bits(G + 1);
+    const int32_t rc = kxpu_aer_health(ctx_, (const uint8_t *)text.data(), text.size(), off.data(), len.data(), n,
+                                       aerFatalLimit, aerNonFatalLimit, goff.data(), members.data(), G, totals.data(),
+                                       bits.data());
+    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_aer_health", rc);
+    for (size_t g = 0; g < G; g++) {
+        std::string why;  // the first member over a limit, fatal before non-fatal
+        for (int k = 0; k < 2 && why.empty(); k++)
+            for (uint32_t m = goff[g]; m < goff[g + 1] && why.empty(); m++) {
+                const uint64_t c = totals[2 * members[m] + k], limit = k ? aerNonFatalLimit : aerFatalLimit;
+                if (c != UINT64_MAX && c > limit)
+                    why = who[members[m]] + " reported " + std::to_string(c) + (k ? " non-fatal" : " fatal") +
+                          " uncorrectable PCIe errors (limit " + std::to_string(limit) + ")";
+            }
+        if (g < iommuMap.size()) { iommuAer[g] = why; iommuAerBits[g] = bits[g]; }
+        else { mdevAer[g - iommuMap.size()] = why; mdevAerBits[g - iommuMap.size()] = bits[g]; }
+    }
+    return Error();
+}
+
+void Plugin::updateAerTaints(bool &passthroughMoved, bool &vgpuMoved) {
+    passthroughMoved = vgpuMoved = false;
+    if (!draTaints || !aerHealth) {
+        aerTaint_.clear();
+        return;
+    }
+    const int64_t t = now ? now() : (int64_t)time(nullptr);
+    std::map<std::string, std::pair<uint8_t, int64_t>> next;
+    auto visit = [&](const std::string &g, uint8_t bits, bool &moved) {
+        const uint8_t v = (bits & KXPU_AER_FATAL) ? KXPU_AER_FATAL : (bits & KXPU_AER_NONFATAL) ? KXPU_AER_NONFATAL : 0;
+        auto it = aerTaint_.find(g);
+        const uint8_t was = it == aerTaint_.end() ? 0 : it->second.first;
+        if (v) next[g] = {v, was == v ? it->second.second : t};  // a new value gets a new time
+        moved |= was != v;
+    };
+    // the groups ResourceSlices / VgpuResourceSlices publish
+    for (size_t g = 0; g < iommuMap.size() && g < iommuClass.size() && g < iommuAerBits.size(); g++)
+        if (!xpuClasses[iommuClass[g]].draDriver.empty() && (g >= iommuBlocker.size() || iommuBlocker[g].empty()))
+            visit(iommuMap[g].first, iommuAerBits[g], passthroughMoved);
+    for (size_t g = 0; g < mdevMap.size() && g < mdevClass.size() && g < mdevAerBits.size(); g++)
+        if (!vgpuClasses[mdevClass[g]].draDriver.empty()) visit(mdevMap[g].first, mdevAerBits[g], vgpuMoved);
+    aerTaint_ = std::move(next);
+}
+
+Error Plugin::refreshAerHealth(std::vector<size_t> &changedPlugins, bool &passthroughMoved, bool &vgpuMoved) {
+    std::unique_lock<std::shared_mutex> lock(mu_);
+    changedPlugins.clear();
+    passthroughMoved = vgpuMoved = false;
+    if (!aerHealth) return Error();
+    Error e = computeAer();
+    if (e) return e;
+    std::map<std::string, std::string> aerOf, mdevAerOf;
+    for (size_t g = 0; g < iommuAer.size(); g++) aerOf[iommuMap[g].first] = iommuAer[g];
+    for (size_t g = 0; g < mdevAer.size(); g++) mdevAerOf[mdevMap[g].first] = mdevAer[g];
+    for (size_t k = 0; k < devicePlugins.size(); k++) {
+        bool moved = false;
+        for (Device &d : devicePlugins[k].devs) {
+            const auto &m = devicePlugins[k].vgpu ? mdevAerOf : aerOf;
+            auto it = m.find(d.ID);
+            const std::string reason = it == m.end() ? std::string() : it->second;
+            moved |= d.aer.empty() != reason.empty();  // ListAndWatch sends health, not the reason
+            d.aer = reason;
+        }
+        if (moved) changedPlugins.push_back(k);
+    }
+    updateAerTaints(passthroughMoved, vgpuMoved);
+    if (passthroughMoved) draGeneration_++;
+    if (vgpuMoved) draVgpuGeneration_++;
+    return Error();
 }
 
 Error Plugin::refreshDraHealth(bool &passthroughMoved, bool &vgpuMoved) {
@@ -1682,6 +1868,9 @@ Error Plugin::VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, st
             devs.push_back(mdevDra[g]);
             groups.push_back(mdevMap[g].first);
         }
+    if (draTaints && aerHealth)
+        return draTaintsSlices(ctx_, kxpu_dra_slices_mdev_taints, "kxpu_dra_slices_mdev_taints", driver, nodeName,
+                               draVgpuGeneration_, devs, draSinceTable(groups), out, sliceOff);
     if (draTaints) return draTaintSlices(ctx_, kxpu_dra_slices_mdev_taint, "kxpu_dra_slices_mdev_taint", driver, nodeName,
                                          draVgpuGeneration_, devs, draSince(groups), out, sliceOff);
     size_t len = 0, nSlices = 0;
@@ -1746,7 +1935,7 @@ Error Plugin::ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8
     std::vector<uint64_t> masks;
     for (const Device &d : dp.devs) {
         groups.push_back((uint32_t)strtoul(d.ID.c_str(), nullptr, 10));
-        healthy.push_back(d.Health == kHealthy && d.blocker.empty());  // a group VFIO cannot open is never offered
+        healthy.push_back(d.Health == kHealthy && d.blocker.empty() && d.aer.empty());  // nor one whose link reports errors
         masks.push_back(d.numa);
     }
     // topologyAware: Device.topology from each device's mask (the HealthWatcher's re-sends come through here too)
@@ -2628,6 +2817,38 @@ void kxh_set_clock(void *h, const int64_t *t) {
     if (t) p->now = [t]() { return *t; };
     else p->now = nullptr;
 }
+// ---- PCIe AER health (ABI v12)
+void kxh_set_aer_health(void *h, int on, uint64_t fatal_limit, uint64_t nonfatal_limit) {
+    Plugin *p = (Plugin *)h;
+    p->aerHealth = on != 0;
+    p->aerFatalLimit = fatal_limit;
+    p->aerNonFatalLimit = nonfatal_limit;
+}
+uint64_t kxh_aer_reads(void *h) { return ((Plugin *)h)->aerReads; }
+// refreshAerHealth: changed[0 .. *n_changed) = the plugins whose ListAndWatch bytes changed (at most cap written),
+// *moved as kxh_refresh_dra_health's; -1 with the message in err
+int kxh_refresh_aer_health(void *h, size_t *changed, size_t cap, size_t *n_changed, int *moved, char *err, size_t errcap) {
+    std::vector<size_t> c;
+    bool pt = false, vg = false;
+    device_plugin::Error e = ((Plugin *)h)->refreshAerHealth(c, pt, vg);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    for (size_t k = 0; k < c.size() && k < cap; k++) changed[k] = c[k];
+    *n_changed = c.size();
+    *moved = (pt ? 1 : 0) | (vg ? 2 : 0);
+    return 0;
+}
+// "id=<aer reason>,..." of one plugin (an empty reason: within the limits)
+int kxh_devs_aer(void *h, int plugin_index, char *out, size_t cap) {
+    Plugin *p = (Plugin *)h;
+    if (plugin_index < 0 || (size_t)plugin_index >= p->devicePlugins.size()) return -1;
+    std::string o;
+    for (const auto &d : p->devicePlugins[(size_t)plugin_index].devs) {
+        if (!o.empty()) o += ',';
+        o += d.ID + "=" + d.aer;
+    }
+    return copy_out(o, out, cap);
+}
+
 // refreshDraHealth: *moved = bit 0 passthrough pools, bit 1 vGPU pools; -1 with the message in err
 int kxh_refresh_dra_health(void *h, int *moved, char *err, size_t cap) {
     bool pt = false, vg = false;

@@ -55,6 +55,9 @@ struct Device {  // pluginapi.Device
     // groupViability: why VFIO cannot open the group ("<bdf> is bound to <driver>"), from the last walk; empty = viable.
     // Separate from Health, which the HealthWatcher flips: the device is sent Unhealthy when either says so.
     std::string blocker{};
+    // aerHealth: why the group's PCIe AER counters are over a limit ("<bdf> reported <n> fatal uncorrectable PCIe errors
+    // (limit <l>)"), from the last walk or refreshAerHealth; empty = within the limits.  Also sent Unhealthy.
+    std::string aer{};
 };
 // pluginapi.DevicePluginOptions (GetDevicePluginOptions, generic_device_plugin.go:253-258)
 struct DevicePluginOptions {
@@ -288,7 +291,21 @@ class Plugin {
     bool draTaints = false;
     // the clock of refreshDraHealth, unix seconds; a seam (time(nullptr) when empty)
     std::function<int64_t()> now;
+    // PCIe AER health (include/kxpu.h, ABI v12).  false (default): no aer_dev_* file is opened and every output is as
+    // above.  true: after every walk and on refreshAerHealth, <bdf>/aer_dev_fatal and aer_dev_nonfatal of every accepted
+    // PCI function and of every accepted mdev's parent (entry "<uuid>/.." under mdevBasePath) are read through
+    // readAerFile, and a group where some member's count is above aerFatalLimit / aerNonFatalLimit gets Device::aer and
+    // is sent Unhealthy.  Allocate does not refuse it: the kubelet does not hand out Unhealthy devices.  With draTaints
+    // too, such a group is published with the taint <draDriver>/pcie-aer=fatal (else =nonfatal):NoSchedule, and
+    // PrepareDraDevices prepares it, since a claim that tolerates the taint asked for it.  A function that is
+    // re-enumerated starts with zeroed counters, so its taint clears at the next rediscover.
+    bool aerHealth = false;
+    // the non-fatal limit is separate because Unsupported Request errors count as non-fatal and some hosts see them often
+    uint64_t aerFatalLimit = 0, aerNonFatalLimit = 0;
+    // <base>/<entry>/<name>, at most KXPU_AER_FILE_MAX + 1 bytes; false or an empty out: a failed read (unknown count)
+    std::function<bool(const std::string &base, const std::string &entry, const std::string &name, std::string &out)> readAerFile;
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
+    uint64_t aerReads = 0;  // aer_dev_* files read (tests, metrics)
 
     // ---- state (device_plugin.go:31,34)
     OrderedMap<std::vector<NvidiaGpuDevice>> iommuMap;  // group id -> devices
@@ -374,6 +391,11 @@ class Plugin {
     // turns healthy; draGeneration / draVgpuGeneration grow by one when the taints of their pools changed, and
     // passthroughMoved / vgpuMoved say which did.  Without draTaints nothing changes.
     Error refreshDraHealth(bool &passthroughMoved, bool &vgpuMoved);
+    // aerHealth: re-read every AER file and fold the counts again (kxpu_aer_health), with no walk, under the exclusive
+    // lock.  Sysfs attributes send no inotify or uevent, so the host calls this on a timer.  changedPlugins: the plugins
+    // whose ListAndWatch bytes changed; with draTaints, passthroughMoved / vgpuMoved say which pools' AER taints changed
+    // (their generation grew by one).  Without aerHealth nothing is read and nothing changes.
+    Error refreshAerHealth(std::vector<size_t> &changedPlugins, bool &passthroughMoved, bool &vgpuMoved);
     // The ResourceSlices of vGPU class vgpuClass (kxpu_dra_slices_mdev): one pool named nodeName, one device per mdevMap
     // group of the class in walk order, described by the group's first mdev: its type key, UUID, parent address, the
     // parent's vendor and device ids, the PCIe root of its link, the group's NUMA mask, and the parent's model name
@@ -443,6 +465,15 @@ class Plugin {
     uint64_t draGeneration_ = 1, draVgpuGeneration_ = 1;
     std::map<std::string, int64_t> draTaintSince_;  // draTaints: IOMMU group id -> when its taint was added
     std::vector<int64_t> draSince(const std::vector<std::string> &groups) const;  // per group: its time, or -1
+    // aerHealth: the reason and the KXPU_AER_* bits of every iommuMap / mdevMap entry (same positions)
+    std::vector<std::string> iommuAer, mdevAer;
+    std::vector<uint8_t> iommuAerBits, mdevAerBits;
+    // draTaints && aerHealth: IOMMU group id -> (KXPU_AER_FATAL or KXPU_AER_NONFATAL, when that value was first seen)
+    std::map<std::string, std::pair<uint8_t, int64_t>> aerTaint_;
+    Error computeAer();  // the reads and the kxpu_aer_health call for the current maps
+    // aerTaint_ from the last computeAer for the groups the DRA pools publish; which pools' taints changed
+    void updateAerTaints(bool &passthroughMoved, bool &vgpuMoved);
+    std::vector<int64_t> draSinceTable(const std::vector<std::string> &groups) const;  // [groups * 3] for the _taints call
     Error checkDraClasses() const;
     void buildMdevDra(const MdevWalk &w);
 };

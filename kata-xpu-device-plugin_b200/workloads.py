@@ -608,3 +608,54 @@ def dra_mdev_devices(n=1 << 16, seed=43):
     d["numa_mask"] = np.left_shift(np.uint64(1), (par % 8).astype(np.uint64))
     d["iommu_group"] = 100000000 + i
     return d
+
+
+AER_FATAL_NAMES = ["Undefined", "DLP", "SDES", "TLP", "FCP", "CmpltTO", "CmpltAbrt", "UnxCmplt", "RxOF", "MalfTLP",
+                   "ECRC", "UnsupReq", "ACSViol", "UncorrIntErr", "BlockedTLP", "AtomicOpBlocked", "TLPBlockedErr",
+                   "PoisonTLPBlocked"]
+
+
+def aer_file(total_name, counts):
+    """an aer_dev_fatal / aer_dev_nonfatal text as the kernel writes it: one "<name> <count>" line per error kind, then
+    "<total_name> <sum>" (total_name TOTAL_ERR_FATAL or TOTAL_ERR_NONFATAL)"""
+    lines = ["%s %d\n" % (nm, c) for nm, c in zip(AER_FATAL_NAMES, counts)]
+    return ("".join(lines) + "%s %d\n" % (total_name, sum(counts))).encode()
+
+
+def aer_records(n=1 << 20, seed=51, vgpus_per_parent=0):
+    """kxpu_aer_health inputs for n records: dict(text, file_off, file_len, group_off, group_members).  Each physical
+    function has its own pair of sysfs-format files, most with zero counts, about one in 64 with fatal or non-fatal
+    errors; with vgpus_per_parent = k, runs of k records share their parent's two files, as vGPUs do.  The files are
+    packed at odd offsets (each one follows a 1..7-byte gap), and the records are grouped one to four per group."""
+    rng = np.random.default_rng(seed)
+    share = max(1, vgpus_per_parent)
+    n_fn = (n + share - 1) // share
+    zero_f, zero_n = aer_file("TOTAL_ERR_FATAL", [0] * 18), aer_file("TOTAL_ERR_NONFATAL", [0] * 18)
+    parts, off, pos = [], np.zeros(2 * n_fn, np.uint64), 0
+    flen = np.zeros(2 * n_fn, np.uint32)
+    bad = rng.integers(0, 64, n_fn) == 0
+    for f in range(n_fn):
+        for k, (name, zero) in enumerate((("TOTAL_ERR_FATAL", zero_f), ("TOTAL_ERR_NONFATAL", zero_n))):
+            txt = zero
+            if bad[f]:
+                counts = [0] * 18
+                counts[int(rng.integers(0, 18))] = int(rng.integers(1, 1000))
+                txt = aer_file(name, counts)
+            gap = int(rng.integers(1, 8))
+            parts.append(b"\n" * gap)
+            pos += gap
+            off[2 * f + k], flen[2 * f + k] = pos, len(txt)
+            parts.append(txt)
+            pos += len(txt)
+    fn_of = np.arange(n) // share
+    file_off = np.empty(2 * n, np.uint64)
+    file_len = np.empty(2 * n, np.uint32)
+    file_off[0::2], file_off[1::2] = off[2 * fn_of], off[2 * fn_of + 1]
+    file_len[0::2], file_len[1::2] = flen[2 * fn_of], flen[2 * fn_of + 1]
+    sizes = rng.integers(1, 5, n)
+    group_off = np.concatenate([[0], np.cumsum(sizes)])
+    group_off = group_off[group_off <= n]
+    if group_off[-1] != n:
+        group_off = np.append(group_off, n)
+    return dict(text=b"".join(parts), file_off=file_off, file_len=file_len, group_off=group_off.astype(np.uint32),
+                group_members=rng.permutation(n).astype(np.uint32))
