@@ -390,8 +390,8 @@ int32_t kx_launch_parse(kxpu_ctx *ctx, kxpu_table *t, const uint8_t *d_text, siz
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kxparse5::parse_kernel_v5, NT, smem);
         if (per_sm < 1) per_sm = 1;
     }
-    // ranges of 8 chunks; shorter ones when the text is too small to give every warp about eight
-    // ranges (with two or three 16 KiB ranges per warp the last wave is half empty, and a range of a
+    // ranges of RCH5_MAX chunks; shorter ones when the text is too small to give every warp about eight
+    // ranges (with two or three ranges per warp the last wave is half empty, and a range of a
     // first-seen vendor block costs its warp ~10 us per chunk)
     const uint32_t wave_warps = (uint32_t)per_sm * ctx->sm_count * WARPS;
     P.rch = std::min<uint32_t>(std::max<uint32_t>(num_chunks / (wave_warps * 8u), 1u), kxparse5::RCH5_MAX);

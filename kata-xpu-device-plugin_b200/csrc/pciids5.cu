@@ -4,11 +4,15 @@
 // pkg/device_plugin/device_plugin.go:208-275): the text is streamed through shared memory ONCE
 // and every (vendor,device) pair is folded into a hash table with "first occurrence wins"
 // semantics; lookups are then O(1) probes.
-//   * the text is cut into RANGES of 8 chunks (16 KiB; fewer for texts too small to give every
+//   * the text is cut into RANGES of 6 chunks (12 KiB; fewer for texts too small to give every
 //     warp of the grid a range) handed out to WARPS by ticket (a static
 //     split leaves the SM half empty at the end: the issue arbiter favours some warps, they
-//     finish early); a warp streams its ranges 2 KiB at a time through a private 3-stage ring
-//     of 1-D TMA bulk copies (cp.async.bulk + mbarrier) -- no CTA barrier, no shared status;
+//     finish early); a warp streams its range through a private 2-stage ring of 1-D TMA bulk
+//     copies of 3 chunks (6 KiB + 16 trailing bytes; cp.async.bulk + mbarrier), 2 CTAs per SM,
+//     and works each copy off one 2 KiB chunk at a time.  A range is one ring: both copies are
+//     issued when the warp takes the range, and nothing of the next range is fetched before
+//     this one is through (measured faster than 2 KiB copies in a ring that runs across ranges,
+//     DESIGN K1) -- no CTA barrier, no shared status;
 //   * per chunk: newline masks (SWAR + IDP.4A) and line classes, then the TOP-LEVEL lines only
 //     (hex prefix, vendor_first check/update -> alive bit).  A device line matters only under
 //     the FIRST line with its vendor id (device_plugin.go:265): lines under a dead line are
@@ -31,12 +35,15 @@ namespace kxparse5 {
 
 using namespace kxparse;
 
-constexpr int STAGES5 = 3;
-constexpr int RCH5_MAX = 8;  // chunks per range (16 KiB); fewer for small texts so that every warp gets a range
+constexpr int CPC5 = 3;                   // chunks per bulk copy (6 KiB)
+constexpr int STAGES5 = 2;                // copies in a warp's ring: one full range
+constexpr int CTAS5 = 2;                  // CTAs per SM (the rings take 99 KB of shared memory per CTA)
+constexpr int COPY5 = CPC5 * CW + TRAIL;  // bytes per stage: CPC5 chunks and the bytes after the last one
+constexpr int RCH5_MAX = CPC5 * STAGES5;  // chunks per range (12 KiB, one ring); fewer for small texts so that every warp gets a range
 constexpr int RES_WARPS = 8;
 
 struct WarpSmem5 {
-    alignas(16) uint8_t stage[STAGES5][STG_BYTES];
+    alignas(16) uint8_t stage[STAGES5][COPY5];
     alignas(8) unsigned long long bar[STAGES5];
 };
 
@@ -45,7 +52,7 @@ struct Params5 {
     unsigned long long n, base;
     uint32_t num_chunks;
     uint32_t tma_limit;               // chunks [0, tma_limit) can be staged with one bulk copy of STG_BYTES
-    uint32_t rch;                     // chunks per range, 1..RCH5_MAX
+    uint32_t rch;                     // chunks per range, 1..RCH5_MAX (KXPU_RCH may force up to 8)
     uint32_t num_ranges;
     unsigned long long *range_state;  // [num_ranges] inclusive carry at the end of the range (ST_*/CV_*)
     uint32_t *lead;                   // [num_ranges] leading chunks whose head lines wait for the resolve kernels
@@ -123,7 +130,7 @@ __device__ __forceinline__ uint32_t devs_of(uint32_t lp, uint32_t mm) {
     return km;
 }
 
-__global__ void __launch_bounds__(NT, 4) parse_kernel_v5(const Params5 P) {
+__global__ void __launch_bounds__(NT, CTAS5) parse_kernel_v5(const Params5 P) {
     extern __shared__ __align__(128) uint8_t smem_raw[];
     WarpSmem5 *W = reinterpret_cast<WarpSmem5 *>(smem_raw);
     uint32_t lane = threadIdx.x & 31u;
@@ -141,7 +148,7 @@ __global__ void __launch_bounds__(NT, 4) parse_kernel_v5(const Params5 P) {
     if (r >= P.num_ranges) return;
 
     // shared-window addresses (see kxparse::lds128)
-    uint32_t a_stage0 = smem_u32(smem_raw) + w * (uint32_t)sizeof(WarpSmem5);  // stage s: + s * STG_BYTES
+    uint32_t a_stage0 = smem_u32(smem_raw) + w * (uint32_t)sizeof(WarpSmem5);  // stage s: + s * COPY5
     asm volatile("" : "+r"(a_stage0));  // opaque: keep it in a register instead of re-deriving it (S2R + LEA + IMAD) at every use
     const uint32_t a_bar0 = a_stage0 + (uint32_t)offsetof(WarpSmem5, bar);     // bar s:   + 8 * s
 
@@ -149,21 +156,24 @@ __global__ void __launch_bounds__(NT, 4) parse_kernel_v5(const Params5 P) {
     asm volatile("" : "+r"(k7f), "+r"(k0a), "+r"(k80));
 
     const unsigned long long pol = l2_evict_first_policy();
-    auto issue = [&](uint32_t g, uint32_t s) {  // lane 0: start the TMA copy of chunk g into stage s
-        if (g < P.tma_limit) {
-            mbar_expect_tx_a(a_bar0 + 8u * s, STG_BYTES);
-            tma_load_a(a_stage0 + s * (uint32_t)STG_BYTES, P.text + (unsigned long long)g * CW, STG_BYTES, a_bar0 + 8u * s, pol);
+    const uint32_t rch = P.rch;
+    // copy k of a range of cnt chunks holds chunks k * CPC5 .. (the last copy of a range may hold fewer); it goes
+    // by TMA when all its chunks can, otherwise (the text's last chunks) its chunks are staged by hand one at a time
+    auto copy_chunks = [](uint32_t cnt, uint32_t k) -> uint32_t {
+        return cnt - k * (uint32_t)CPC5 < (uint32_t)CPC5 ? cnt - k * (uint32_t)CPC5 : (uint32_t)CPC5;
+    };
+    auto issue = [&](uint32_t g0, uint32_t m, uint32_t s) {  // lane 0: start the copy of chunks g0 .. g0+m-1 into stage s
+        if (g0 + m - 1u < P.tma_limit) {
+            mbar_expect_tx_a(a_bar0 + 8u * s, m * (uint32_t)CW + (uint32_t)TRAIL);
+            tma_load_a(a_stage0 + s * (uint32_t)COPY5, P.text + (unsigned long long)g0 * CW, m * (uint32_t)CW + (uint32_t)TRAIL, a_bar0 + 8u * s, pol);
         }
     };
-    const uint32_t rch = P.rch;
-    bool staged = false;  // the first chunks of the coming range are already on their way
 
     uint32_t phase_bits = 0, s = 0;
     uint32_t nfresh = 0;  // table slots this lane claimed in the current chunk (flushed once per warp and chunk)
     for (;;) {
-        // ticket of the next range, drawn one range early; looked at (shuffled) late in this range
-        uint32_t tk2 = 0, r_next = 0xffffffffu;
-        bool have_next = false;
+        // ticket of the next range, drawn one range early; looked at (shuffled) at the end of this range
+        uint32_t tk2 = 0;
         if (lane == 0) tk2 = atomicAdd(&P.tab.counters[KX_C_TICKET], 1u);
         // carry along the range: the governing line at the start of the next chunk as a status word
         // (LS_* of parse_common.cuh; 0 = not known) plus the chunk that holds the line (0xffffffff = the
@@ -179,181 +189,173 @@ __global__ void __launch_bounds__(NT, 4) parse_kernel_v5(const Params5 P) {
         const bool table_dead = *reinterpret_cast<volatile uint32_t *>(&P.tab.counters[KX_C_OVERFLOW]) != 0u;
         const uint32_t gb = r * rch;
         const uint32_t cnt = P.num_chunks - gb < rch ? P.num_chunks - gb : rch;
-        if (!staged && lane == 0) {
-            for (uint32_t j = 0; j < (uint32_t)STAGES5 && j < cnt; j++) issue(gb + j, (s + j) % (uint32_t)STAGES5);
+        const uint32_t ncp = (cnt + (uint32_t)CPC5 - 1u) / (uint32_t)CPC5;  // copies of the range
+        // the copies a warp has in flight all belong to its current range: nothing is fetched for the next range
+        // before this one is through (see DESIGN K1: contiguous copies read faster than a ring across two ranges)
+        if (lane == 0) {
+            for (uint32_t j = 0; j < (uint32_t)STAGES5 && j < ncp; j++) issue(gb + j * (uint32_t)CPC5, copy_chunks(cnt, j), (s + j) % (uint32_t)STAGES5);
         }
-        staged = false;
-        for (uint32_t i = 0; i < cnt; i++) {
-            if (!have_next && rch > (uint32_t)STAGES5 && i + (uint32_t)STAGES5 >= rch) {
-                r_next = __shfl_sync(0xffffffffu, tk2, 0);
-                have_next = true;
-            }
-            const uint32_t g = gb + i;
-            const uint32_t st = a_stage0 + s * (uint32_t)STG_BYTES;
-            const unsigned long long cbase = P.base + (unsigned long long)g * CW;
-            uint32_t n_rel = CW + 1;  // line starts at p < n_rel are real (p == CW: first byte of the next chunk)
-            if (g < P.tma_limit) {
+        for (uint32_t k = 0; k < ncp; k++) {
+            const uint32_t g0 = gb + k * (uint32_t)CPC5, m = copy_chunks(cnt, k);
+            const bool by_tma = g0 + m - 1u < P.tma_limit;
+            if (by_tma) {
                 const uint32_t bar = a_bar0 + 8u * s, par = (phase_bits >> s) & 1u;
                 while (!mbar_try_a(bar, par)) {
                 }
                 phase_bits ^= 1u << s;
-            } else {
-                n_rel = stage_chunk_manual(P.text, P.n, g, lane, W[w].stage[s]);
             }
+            // the copy's chunks one at a time, in text order
+            for (uint32_t j = 0; j < m; j++) {
+                const uint32_t i = k * (uint32_t)CPC5 + j;  // chunk of the range
+                const uint32_t g = g0 + j;
+                const uint32_t st = a_stage0 + s * (uint32_t)COPY5 + j * (uint32_t)CW;
+                const unsigned long long cbase = P.base + (unsigned long long)g * CW;
+                uint32_t n_rel = CW + 1;  // line starts at p < n_rel are real (p == CW: first byte of the next chunk)
+                if (!by_tma) n_rel = stage_chunk_manual(P.text, P.n, g, lane, W[w].stage[s] + j * CW);
 
-            uint32_t nl[2], th[2], rawnl;
-            nl_masks(st, lane, n_rel, k7f, k0a, k80, nl, rawnl);
-            tops_of2(st + lane * 32u + 1u, nl[0], nl[1], th[0], th[1]);
+                uint32_t nl[2], th[2], rawnl;
+                nl_masks(st, lane, n_rel, k7f, k0a, k80, nl, rawnl);
+                tops_of2(st + lane * 32u + 1u, nl[0], nl[1], th[0], th[1]);
 
-            // top-level lines, by the lane that owns them: a candidate vendor anchor; only the FIRST
-            // line with this prefix counts (:265).  If an earlier one is already known, this block
-            // can never produce a hit (a hit needs min_anchor == vendor_first): it is dead.
-            uint32_t linfo0 = P_NONE, linfo1 = P_NONE;  // last top-level line of my windows: alive<<31 | vendor<<15 | position
-            bool any_alive = (g == 0u) || (rc_x & LS_VOK) != 0u;  // the shard's first chunk and alive carries take the full path
-            {
-                uint32_t t0 = th[0], t1 = th[1];
-                while (t0 | t1) {
-                    const bool second = t0 == 0u;
-                    const uint32_t tmv = second ? t1 : t0;
-                    const uint32_t bit = tmv & (0u - tmv);
-                    if (second) t1 = tmv ^ bit; else t0 = tmv ^ bit;
-                    const uint32_t p = (second ? (uint32_t)HALF : 0u) + lane * 32u + 1u + (31u - (uint32_t)__clz((int)bit));
-                    uint32_t val;
-                    const bool ok = hex4_swar(lds32_unaligned(st + p), val);
-                    const unsigned long long line_g = cbase + p;
-                    bool alive = ok;
-                    if (ok) {
-                        const unsigned long long vf = P.tab.vendor_first[val];
-                        if (line_g < vf) atomicMin(&P.tab.vendor_first[val], line_g);
-                        alive = line_g <= vf;
-                    }
-                    any_alive |= alive;
-                    const uint32_t info = (alive ? 0x80000000u : 0u) | ((ok ? val : 0u) << 15) | p;
-                    if (second) linfo1 = info; else linfo0 = info;
-                }
-            }
-            const uint32_t bal0 = __ballot_sync(0xffffffffu, th[0] != 0u);
-            const uint32_t bal1 = __ballot_sync(0xffffffffu, th[1] != 0u);
-            uint32_t last1;  // the chunk's last top-level line
-            if (!__any_sync(0xffffffffu, any_alive)) {
-                // common case: nothing alive in or in front of this chunk -- no device line of it
-                // can matter, none is looked at
-                const uint32_t bl = bal1 ? bal1 : bal0;
-                last1 = __shfl_sync(0xffffffffu, bal1 ? linfo1 : linfo0, bl ? 31 - __clz((int)bl) : 0);
-                if (bl == 0u) last1 = P_NONE;
-            } else {
-                // full path: device line candidates, governing line of every window
-                uint32_t kh[2];
-                kh[0] = th[0] | devs_of(st + lane * 32u + 1u, nl[0] & ~th[0]);
-                kh[1] = th[1] | devs_of(st + (uint32_t)HALF + lane * 32u + 1u, nl[1] & ~th[1]);
-                if (table_dead) { kh[0] = th[0]; kh[1] = th[1]; }
-
-                // the shard starts with a line start at p = 0 (no newline before it)
-                uint32_t base_info = P_NONE;  // top-level line in front of the lane windows (only that one)
-                if (g == 0u && n_rel > 0u) {
-                    const uint32_t c0 = lds8(st), c1 = lds8(st + 1u);
-                    if (c0 != (uint32_t)'#' && c0 != (uint32_t)'\t') {
-                        uint32_t val;
-                        const bool ok = hex4_swar(lds32_unaligned(st), val);
-                        bool alive = ok;
-                        if (ok) {
-                            const unsigned long long vf = P.tab.vendor_first[val];
-                            if (lane == 0 && cbase < vf) atomicMin(&P.tab.vendor_first[val], cbase);
-                            alive = cbase <= vf;
-                        }
-                        base_info = (alive ? 0x80000000u : 0u) | ((ok ? val : 0u) << 15);
-                    } else if (c0 == (uint32_t)'\t' && c1 != (uint32_t)'\t') {
-                        // device line at the very start: governed by the shard's carry-in, which is known
-                        uint32_t dv;
-                        if (lane == 0 && !table_dead && (P.carry_in & CV_HAS_TOP) && (P.carry_in & CV_VOK) && hex4_swar(lds32_unaligned(st + 1u), dv))
-                            table_fold(P.tab, (((uint32_t)(P.carry_in >> 44) & 0xffffu) << 16) | dv, cbase, P.carry_in & CV_ANCHOR_MASK, nfresh);
-                    }
-                }
-                // device lines behind the top-level lines of my windows (alive ones only)
-                linfo0 = linfo1 = P_NONE;
+                // top-level lines, by the lane that owns them: a candidate vendor anchor; only the FIRST
+                // line with this prefix counts (:265).  If an earlier one is already known, this block
+                // can never produce a hit (a hit needs min_anchor == vendor_first): it is dead.
+                uint32_t linfo0 = P_NONE, linfo1 = P_NONE;  // last top-level line of my windows: alive<<31 | vendor<<15 | position
+                bool any_alive = (g == 0u) || (rc_x & LS_VOK) != 0u;  // the shard's first chunk and alive carries take the full path
                 {
                     uint32_t t0 = th[0], t1 = th[1];
                     while (t0 | t1) {
                         const bool second = t0 == 0u;
                         const uint32_t tmv = second ? t1 : t0;
                         const uint32_t bit = tmv & (0u - tmv);
-                        const uint32_t rest = tmv ^ bit;
-                        if (second) t1 = rest; else t0 = rest;
-                        const uint32_t pbase = (second ? (uint32_t)HALF : 0u) + lane * 32u + 1u;
-                        const uint32_t p = pbase + (31u - (uint32_t)__clz((int)bit));
+                        if (second) t1 = tmv ^ bit; else t0 = tmv ^ bit;
+                        const uint32_t p = (second ? (uint32_t)HALF : 0u) + lane * 32u + 1u + (31u - (uint32_t)__clz((int)bit));
                         uint32_t val;
                         const bool ok = hex4_swar(lds32_unaligned(st + p), val);
                         const unsigned long long line_g = cbase + p;
-                        const bool alive = ok && line_g <= P.tab.vendor_first[val];  // updated by the loop above
-                        if (alive) {
-                            const uint32_t nxt = rest & (0u - rest);
-                            const uint32_t seg = (second ? kh[1] & ~th[1] : kh[0] & ~th[0]) & ~(bit | (bit - 1u)) & (nxt ? nxt - 1u : 0xffffffffu);
-                            fold_lines(P.tab, st, cbase, seg, pbase, val << 16, line_g, nfresh);
+                        bool alive = ok;
+                        if (ok) {
+                            const unsigned long long vf = P.tab.vendor_first[val];
+                            if (line_g < vf) atomicMin(&P.tab.vendor_first[val], line_g);
+                            alive = line_g <= vf;
                         }
+                        any_alive |= alive;
                         const uint32_t info = (alive ? 0x80000000u : 0u) | ((ok ? val : 0u) << 15) | p;
                         if (second) linfo1 = info; else linfo0 = info;
                     }
                 }
-                // device lines in front of a window's first top-level line
-                const uint32_t pre0 = kh[0] & ~th[0] & (th[0] ? (th[0] & (0u - th[0])) - 1u : 0xffffffffu);
-                const uint32_t pre1 = kh[1] & ~th[1] & (th[1] ? (th[1] & (0u - th[1])) - 1u : 0xffffffffu);
-                const uint32_t s0 = bal0 & lt_mask, s1 = bal1 & lt_mask;
-                const uint32_t x0 = __shfl_sync(0xffffffffu, linfo0, s0 ? 31 - __clz((int)s0) : 0);
-                const uint32_t l0 = __shfl_sync(0xffffffffu, linfo0, bal0 ? 31 - __clz((int)bal0) : 0);
-                const uint32_t x1 = __shfl_sync(0xffffffffu, linfo1, s1 ? 31 - __clz((int)s1) : 0);
-                const uint32_t l1 = __shfl_sync(0xffffffffu, linfo1, bal1 ? 31 - __clz((int)bal1) : 0);
-                const uint32_t last0 = bal0 ? l0 : base_info;
-                const uint32_t cin0 = s0 ? x0 : base_info;
-                const uint32_t cin1 = s1 ? x1 : last0;
-                last1 = bal1 ? l1 : last0;
-                // governed by an alive line of an earlier window of this chunk
-                if (cin0 != P_NONE && (cin0 >> 31))
-                    fold_lines(P.tab, st, cbase, pre0, lane * 32u + 1u, ((cin0 >> 15) & 0xffffu) << 16, cbase + (cin0 & 0x7fffu), nfresh);
-                if (cin1 != P_NONE && (cin1 >> 31))
-                    fold_lines(P.tab, st, cbase, pre1, (uint32_t)HALF + lane * 32u + 1u, ((cin1 >> 15) & 0xffffu) << 16, cbase + (cin1 & 0x7fffu), nfresh);
-                // head lines (in front of the chunk's first top-level line): governed by the carry; if
-                // that is not known yet, the resolve kernels look at them
-                const uint32_t hw0 = cin0 == P_NONE ? pre0 : 0u;
-                const uint32_t hw1 = cin1 == P_NONE ? pre1 : 0u;
-                if (rc_x & LS_VOK) {
-                    uint32_t key_hi = ((rc_x >> 12) & 0xffffu) << 16;
-                    unsigned long long anchor = P.base + (unsigned long long)rc_g * CW + (rc_x & 0xfffu);
-                    if (rc_g == 0xffffffffu) {
-                        key_hi = ((uint32_t)(P.carry_in >> 44) & 0xffffu) << 16;
-                        anchor = P.carry_in & CV_ANCHOR_MASK;
-                    }
-                    // still the first line of its id?
-                    if ((hw0 | hw1) != 0u && P.tab.vendor_first[key_hi >> 16] >= anchor) {
-                        fold_lines(P.tab, st, cbase, hw0, lane * 32u + 1u, key_hi, anchor, nfresh);
-                        fold_lines(P.tab, st, cbase, hw1, (uint32_t)HALF + lane * 32u + 1u, key_hi, anchor, nfresh);
-                    }
-                }
-                flush_fresh(P.tab, nfresh);  // full path only: the branch is warp-uniform (__any_sync above)
-            }
-            if (last1 != P_NONE) {
-                if (rc_x == 0u) lead = i + 1u;  // chunks 0..i have head lines nobody judged
-                rc_x = LS_PUB | LS_TOP | ((last1 >> 31) ? LS_VOK : 0u) | (((last1 >> 15) & 0xffffu) << 12) | (last1 & 0xfffu);
-                rc_g = g;
-            }
-            // 2 KiB without a newline may belong to a >= 64 KiB line (bufio.ErrTooLong): raise the
-            // hint, the exact cut-off is then computed by trunc_kernel (never for real pci.ids)
-            if ((bal0 | bal1) == 0u && n_rel > (uint32_t)CW && __reduce_or_sync(0xffffffffu, rawnl) == 0u && lane == 0)
-                atomicOr(&P.tab.counters[KX_C_LONGLINE_HINT], 1u);
+                const uint32_t bal0 = __ballot_sync(0xffffffffu, th[0] != 0u);
+                const uint32_t bal1 = __ballot_sync(0xffffffffu, th[1] != 0u);
+                uint32_t last1;  // the chunk's last top-level line
+                if (!__any_sync(0xffffffffu, any_alive)) {
+                    // common case: nothing alive in or in front of this chunk -- no device line of it
+                    // can matter, none is looked at
+                    const uint32_t bl = bal1 ? bal1 : bal0;
+                    last1 = __shfl_sync(0xffffffffu, bal1 ? linfo1 : linfo0, bl ? 31 - __clz((int)bl) : 0);
+                    if (bl == 0u) last1 = P_NONE;
+                } else {
+                    // full path: device line candidates, governing line of every window
+                    uint32_t kh[2];
+                    kh[0] = th[0] | devs_of(st + lane * 32u + 1u, nl[0] & ~th[0]);
+                    kh[1] = th[1] | devs_of(st + (uint32_t)HALF + lane * 32u + 1u, nl[1] & ~th[1]);
+                    if (table_dead) { kh[0] = th[0]; kh[1] = th[1]; }
 
-            // the stage is free: prefetch the chunk three steps ahead into it -- of this range, or (ranges
-            // longer than the ring only) of the next one
-            __syncwarp();
-            {
-                const uint32_t fi = i + (uint32_t)STAGES5;
-                uint32_t fg = 0xffffffffu;
-                if (fi < rch) {
-                    fg = g + (uint32_t)STAGES5;
-                } else if (rch > (uint32_t)STAGES5 && cnt == rch && r_next < P.num_ranges) {
-                    fg = r_next * rch + (fi - rch);
-                    staged = true;
+                    // the shard starts with a line start at p = 0 (no newline before it)
+                    uint32_t base_info = P_NONE;  // top-level line in front of the lane windows (only that one)
+                    if (g == 0u && n_rel > 0u) {
+                        const uint32_t c0 = lds8(st), c1 = lds8(st + 1u);
+                        if (c0 != (uint32_t)'#' && c0 != (uint32_t)'\t') {
+                            uint32_t val;
+                            const bool ok = hex4_swar(lds32_unaligned(st), val);
+                            bool alive = ok;
+                            if (ok) {
+                                const unsigned long long vf = P.tab.vendor_first[val];
+                                if (lane == 0 && cbase < vf) atomicMin(&P.tab.vendor_first[val], cbase);
+                                alive = cbase <= vf;
+                            }
+                            base_info = (alive ? 0x80000000u : 0u) | ((ok ? val : 0u) << 15);
+                        } else if (c0 == (uint32_t)'\t' && c1 != (uint32_t)'\t') {
+                            // device line at the very start: governed by the shard's carry-in, which is known
+                            uint32_t dv;
+                            if (lane == 0 && !table_dead && (P.carry_in & CV_HAS_TOP) && (P.carry_in & CV_VOK) && hex4_swar(lds32_unaligned(st + 1u), dv))
+                                table_fold(P.tab, (((uint32_t)(P.carry_in >> 44) & 0xffffu) << 16) | dv, cbase, P.carry_in & CV_ANCHOR_MASK, nfresh);
+                        }
+                    }
+                    // device lines behind the top-level lines of my windows (alive ones only)
+                    linfo0 = linfo1 = P_NONE;
+                    {
+                        uint32_t t0 = th[0], t1 = th[1];
+                        while (t0 | t1) {
+                            const bool second = t0 == 0u;
+                            const uint32_t tmv = second ? t1 : t0;
+                            const uint32_t bit = tmv & (0u - tmv);
+                            const uint32_t rest = tmv ^ bit;
+                            if (second) t1 = rest; else t0 = rest;
+                            const uint32_t pbase = (second ? (uint32_t)HALF : 0u) + lane * 32u + 1u;
+                            const uint32_t p = pbase + (31u - (uint32_t)__clz((int)bit));
+                            uint32_t val;
+                            const bool ok = hex4_swar(lds32_unaligned(st + p), val);
+                            const unsigned long long line_g = cbase + p;
+                            const bool alive = ok && line_g <= P.tab.vendor_first[val];  // updated by the loop above
+                            if (alive) {
+                                const uint32_t nxt = rest & (0u - rest);
+                                const uint32_t seg = (second ? kh[1] & ~th[1] : kh[0] & ~th[0]) & ~(bit | (bit - 1u)) & (nxt ? nxt - 1u : 0xffffffffu);
+                                fold_lines(P.tab, st, cbase, seg, pbase, val << 16, line_g, nfresh);
+                            }
+                            const uint32_t info = (alive ? 0x80000000u : 0u) | ((ok ? val : 0u) << 15) | p;
+                            if (second) linfo1 = info; else linfo0 = info;
+                        }
+                    }
+                    // device lines in front of a window's first top-level line
+                    const uint32_t pre0 = kh[0] & ~th[0] & (th[0] ? (th[0] & (0u - th[0])) - 1u : 0xffffffffu);
+                    const uint32_t pre1 = kh[1] & ~th[1] & (th[1] ? (th[1] & (0u - th[1])) - 1u : 0xffffffffu);
+                    const uint32_t s0 = bal0 & lt_mask, s1 = bal1 & lt_mask;
+                    const uint32_t x0 = __shfl_sync(0xffffffffu, linfo0, s0 ? 31 - __clz((int)s0) : 0);
+                    const uint32_t l0 = __shfl_sync(0xffffffffu, linfo0, bal0 ? 31 - __clz((int)bal0) : 0);
+                    const uint32_t x1 = __shfl_sync(0xffffffffu, linfo1, s1 ? 31 - __clz((int)s1) : 0);
+                    const uint32_t l1 = __shfl_sync(0xffffffffu, linfo1, bal1 ? 31 - __clz((int)bal1) : 0);
+                    const uint32_t last0 = bal0 ? l0 : base_info;
+                    const uint32_t cin0 = s0 ? x0 : base_info;
+                    const uint32_t cin1 = s1 ? x1 : last0;
+                    last1 = bal1 ? l1 : last0;
+                    // governed by an alive line of an earlier window of this chunk
+                    if (cin0 != P_NONE && (cin0 >> 31))
+                        fold_lines(P.tab, st, cbase, pre0, lane * 32u + 1u, ((cin0 >> 15) & 0xffffu) << 16, cbase + (cin0 & 0x7fffu), nfresh);
+                    if (cin1 != P_NONE && (cin1 >> 31))
+                        fold_lines(P.tab, st, cbase, pre1, (uint32_t)HALF + lane * 32u + 1u, ((cin1 >> 15) & 0xffffu) << 16, cbase + (cin1 & 0x7fffu), nfresh);
+                    // head lines (in front of the chunk's first top-level line): governed by the carry; if
+                    // that is not known yet, the resolve kernels look at them
+                    const uint32_t hw0 = cin0 == P_NONE ? pre0 : 0u;
+                    const uint32_t hw1 = cin1 == P_NONE ? pre1 : 0u;
+                    if (rc_x & LS_VOK) {
+                        uint32_t key_hi = ((rc_x >> 12) & 0xffffu) << 16;
+                        unsigned long long anchor = P.base + (unsigned long long)rc_g * CW + (rc_x & 0xfffu);
+                        if (rc_g == 0xffffffffu) {
+                            key_hi = ((uint32_t)(P.carry_in >> 44) & 0xffffu) << 16;
+                            anchor = P.carry_in & CV_ANCHOR_MASK;
+                        }
+                        // still the first line of its id?
+                        if ((hw0 | hw1) != 0u && P.tab.vendor_first[key_hi >> 16] >= anchor) {
+                            fold_lines(P.tab, st, cbase, hw0, lane * 32u + 1u, key_hi, anchor, nfresh);
+                            fold_lines(P.tab, st, cbase, hw1, (uint32_t)HALF + lane * 32u + 1u, key_hi, anchor, nfresh);
+                        }
+                    }
+                    flush_fresh(P.tab, nfresh);  // full path only: the branch is warp-uniform (__any_sync above)
                 }
-                if (lane == 0) issue(fg, s);
+                if (last1 != P_NONE) {
+                    if (rc_x == 0u) lead = i + 1u;  // chunks 0..i have head lines nobody judged
+                    rc_x = LS_PUB | LS_TOP | ((last1 >> 31) ? LS_VOK : 0u) | (((last1 >> 15) & 0xffffu) << 12) | (last1 & 0xfffu);
+                    rc_g = g;
+                }
+                // 2 KiB without a newline may belong to a >= 64 KiB line (bufio.ErrTooLong): raise the
+                // hint, the exact cut-off is then computed by trunc_kernel (never for real pci.ids)
+                if ((bal0 | bal1) == 0u && n_rel > (uint32_t)CW && __reduce_or_sync(0xffffffffu, rawnl) == 0u && lane == 0)
+                    atomicOr(&P.tab.counters[KX_C_LONGLINE_HINT], 1u);
+                __syncwarp();  // a hand-staged next chunk overwrites this one's trailing bytes
             }
+
+            // the stage is free: refill it with the range's copy STAGES5 steps ahead
+            if (lane == 0 && k + (uint32_t)STAGES5 < ncp) issue(gb + (k + (uint32_t)STAGES5) * (uint32_t)CPC5, copy_chunks(cnt, k + (uint32_t)STAGES5), s);
             s = s == (uint32_t)STAGES5 - 1u ? 0u : s + 1u;
         }
         // the range's inclusive carry and its unjudged leading chunks for the resolve kernel
@@ -369,8 +371,7 @@ __global__ void __launch_bounds__(NT, 4) parse_kernel_v5(const Params5 P) {
             P.range_state[r] = v;
             P.lead[r] = lead < cnt ? lead : cnt;
         }
-        if (!have_next) r_next = __shfl_sync(0xffffffffu, tk2, 0);
-        r = r_next;
+        r = __shfl_sync(0xffffffffu, tk2, 0);
         if (r >= P.num_ranges) break;
     }
 }
