@@ -919,7 +919,8 @@ typedef struct kxpu_dra_taint {
  * or above KXPU_DRA_MAX_TAINTS, or an entry whose key, value or effect fails kxpu_dra_slices_taint's checks.
  * KXPU_E_UNSUPPORTED, nothing written: the cases of kxpu_dra_slices, a taint_since above KXPU_DRA_TAINT_SINCE_MAX, or a
  * device that carries two entries with the same key and effect.
- * GPU: the kernel of kxpu_dra_slices with the taint list compiled in.  Timed under KXPU_T_EMIT. */
+ * GPU: n_taints == 1 runs kxpu_dra_slices_taint's kernel; two or more entries run the kernel of kxpu_dra_slices with
+ * the taint list compiled in.  Timed under KXPU_T_EMIT. */
 int32_t kxpu_dra_slices_taints(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
                                const kxpu_dradev *devs, size_t n, const kxpu_dra_taint *taints, size_t n_taints,
                                const int64_t *taint_since /* [n * n_taints], device-major, or NULL */, uint8_t *out,

@@ -598,108 +598,75 @@ func (k *kxpu) reconcile(prev []C.kxpu_snaprec, nextIndex uint64, cur []C.kxpu_s
 // kxpu_dradev per published IOMMU group in walk order (groups with a viability blocker left out).  Returns the slices
 // as JSON Lines, one object per line; the caller POSTs each line to /apis/resource.k8s.io/v1/resourceslices and then
 // deletes the slices of its driver and node with an older spec.pool.generation.
-func (k *kxpu) draSlices(driver, node string, generation uint64, devs []C.kxpu_dradev) ([]string, error) {
-	cd, cn := C.CString(driver), C.CString(node)
-	defer C.free(unsafe.Pointer(cd))
-	defer C.free(unsafe.Pointer(cn))
+//
+// DRA device taints (ABI v11, v12): since == nil publishes no taints.  Otherwise since holds one or three times per
+// device, device-major, -1 where the device does not carry that taint, for the first one or all three entries of the
+// table [<driver>/unhealthy=vfio-device-missing, <driver>/pcie-aer=fatal, <driver>/pcie-aer=nonfatal], all
+// NoSchedule: a missing device node keeps new claims away but must not evict a VM that holds the group open.  A device
+// carries at most one of the two pcie-aer values.  With taints a slice holds 64 devices.
+func (k *kxpu) draSlices(driver, node string, generation uint64, devs []C.kxpu_dradev, since []int64) ([]string, error) {
 	var p *C.kxpu_dradev
 	if len(devs) > 0 {
 		p = &devs[0]
 	}
-	var n, ns C.size_t
-	rc := C.kxpu_dra_slices(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), nil, 0, &n, nil, &ns) // sizing call
-	if rc != C.KXPU_E_NOSPACE {
-		return nil, kxCheck(k.ctx, "kxpu_dra_slices", rc)
-	}
-	buf := make([]byte, n)
-	off := make([]uint64, ns+1)
-	if err := kxCheck(k.ctx, "kxpu_dra_slices", C.kxpu_dra_slices(k.ctx, cd, cn, cn, C.uint64_t(generation), p,
-		C.size_t(len(devs)), (*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n, (*C.uint64_t)(unsafe.Pointer(&off[0])), &ns)); err != nil {
-		return nil, err
-	}
-	lines := make([]string, ns)
-	for s := range lines {
-		lines[s] = string(buf[off[s] : off[s+1]-1]) // without the '\n'
-	}
-	return lines, nil
-}
-
-// DRA ResourceSlices of vGPUs (ABI v10).  One pool per vGPU class with a DRA driver, named after the node: devs holds one
-// kxpu_dramdev per mdevMap group of the class in walk order.  Published and replaced exactly as draSlices' output.
-func (k *kxpu) draSlicesMdev(driver, node string, generation uint64, devs []C.kxpu_dramdev) ([]string, error) {
-	cd, cn := C.CString(driver), C.CString(node)
-	defer C.free(unsafe.Pointer(cd))
-	defer C.free(unsafe.Pointer(cn))
-	var p *C.kxpu_dramdev
-	if len(devs) > 0 {
-		p = &devs[0]
-	}
-	var n, ns C.size_t
-	rc := C.kxpu_dra_slices_mdev(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), nil, 0, &n, nil, &ns) // sizing call
-	if rc != C.KXPU_E_NOSPACE {
-		return nil, kxCheck(k.ctx, "kxpu_dra_slices_mdev", rc)
-	}
-	buf := make([]byte, n)
-	off := make([]uint64, ns+1)
-	if err := kxCheck(k.ctx, "kxpu_dra_slices_mdev", C.kxpu_dra_slices_mdev(k.ctx, cd, cn, cn, C.uint64_t(generation), p,
-		C.size_t(len(devs)), (*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n, (*C.uint64_t)(unsafe.Pointer(&off[0])), &ns)); err != nil {
-		return nil, err
-	}
-	lines := make([]string, ns)
-	for s := range lines {
-		lines[s] = string(buf[off[s] : off[s+1]-1]) // without the '\n'
-	}
-	return lines, nil
-}
-
-// DRA device taints (ABI v11): draSlices / draSlicesMdev with since[i] = the unix time group i was found unhealthy, or
-// -1.  The key is <driver>/unhealthy, the value vfio-device-missing, the effect NoSchedule: a missing device node keeps
-// new claims away but must not evict a VM that holds the group open.  64 devices per slice.
-func (k *kxpu) draSlicesTaint(driver, node string, generation uint64, devs []C.kxpu_dradev, since []int64) ([]string, error) {
-	var p *C.kxpu_dradev
-	if len(devs) > 0 {
-		p = &devs[0]
-	}
-	return k.taintSlices("kxpu_dra_slices_taint", driver, node, len(devs), since, func(cd, cn, ck, cv, ce *C.char,
-		cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t, ns *C.size_t) C.int32_t {
-		return C.kxpu_dra_slices_taint(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), ck, cv, ce, cs, out,
+	return k.slices("kxpu_dra_slices_taints", driver, node, len(devs), since, func(cd, cn *C.char, tab *C.kxpu_dra_taint,
+		nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t, ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_taints(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), tab, nt, cs, out,
 			capacity, n, off, ns)
 	})
 }
 
-func (k *kxpu) draSlicesMdevTaint(driver, node string, generation uint64, devs []C.kxpu_dramdev, since []int64) ([]string, error) {
+// DRA ResourceSlices of vGPUs (ABI v10).  One pool per vGPU class with a DRA driver, named after the node: devs holds one
+// kxpu_dramdev per mdevMap group of the class in walk order.  Tainted, published and replaced exactly as draSlices'
+// output.
+func (k *kxpu) draSlicesMdev(driver, node string, generation uint64, devs []C.kxpu_dramdev, since []int64) ([]string, error) {
 	var p *C.kxpu_dramdev
 	if len(devs) > 0 {
 		p = &devs[0]
 	}
-	return k.taintSlices("kxpu_dra_slices_mdev_taint", driver, node, len(devs), since, func(cd, cn, ck, cv, ce *C.char,
-		cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t, ns *C.size_t) C.int32_t {
-		return C.kxpu_dra_slices_mdev_taint(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), ck, cv, ce, cs,
+	return k.slices("kxpu_dra_slices_mdev_taints", driver, node, len(devs), since, func(cd, cn *C.char,
+		tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
+		ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_mdev_taints(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), tab, nt, cs,
 			out, capacity, n, off, ns)
 	})
 }
 
-// the two-call sizing of one _taint call, the taint arguments in C memory
-func (k *kxpu) taintSlices(what, driver, node string, nDevs int, since []int64, call func(cd, cn, ck, cv, ce *C.char,
-	cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t, ns *C.size_t) C.int32_t) ([]string, error) {
-	if len(since) != nDevs {
+// the two-call sizing of one slice call, the table and the times in C memory; the table width is len(since) / nDevs
+func (k *kxpu) slices(what, driver, node string, nDevs int, since []int64, call func(cd, cn *C.char,
+	tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
+	ns *C.size_t) C.int32_t) ([]string, error) {
+	nt := 1
+	if since != nil && nDevs > 0 {
+		nt = len(since) / nDevs
+	}
+	if since != nil && (nt < 1 || nt > 3 || len(since) != nt*nDevs) {
 		return nil, fmt.Errorf("%s: %d taint times for %d devices", what, len(since), nDevs)
 	}
-	cd, cn := C.CString(driver), C.CString(node)
-	ck, cv, ce := C.CString(driver+"/unhealthy"), C.CString("vfio-device-missing"), C.CString("NoSchedule")
-	for _, s := range []*C.char{cd, cn, ck, cv, ce} {
+	strs := []*C.char{C.CString(driver), C.CString(node), C.CString(driver + "/unhealthy"), C.CString("vfio-device-missing"),
+		C.CString(driver + "/pcie-aer"), C.CString("fatal"), C.CString("nonfatal"), C.CString("NoSchedule")}
+	for _, s := range strs {
 		defer C.free(unsafe.Pointer(s))
 	}
-	cs := (*C.int64_t)(C.malloc(C.size_t(8 * (nDevs + 1))))
-	defer C.free(unsafe.Pointer(cs))
-	copy(unsafe.Slice((*int64)(unsafe.Pointer(cs)), nDevs), since)
+	tab := (*C.kxpu_dra_taint)(C.malloc(C.size_t(3 * unsafe.Sizeof(C.kxpu_dra_taint{}))))
+	defer C.free(unsafe.Pointer(tab))
+	t := unsafe.Slice(tab, 3)
+	t[0] = C.kxpu_dra_taint{key: strs[2], value: strs[3], effect: strs[7]}
+	t[1] = C.kxpu_dra_taint{key: strs[4], value: strs[5], effect: strs[7]}
+	t[2] = C.kxpu_dra_taint{key: strs[4], value: strs[6], effect: strs[7]}
+	var cs *C.int64_t // nil: taint_since NULL, the untainted slices
+	if since != nil {
+		cs = (*C.int64_t)(C.malloc(C.size_t(8 * (len(since) + 1))))
+		defer C.free(unsafe.Pointer(cs))
+		copy(unsafe.Slice((*int64)(unsafe.Pointer(cs)), len(since)), since)
+	}
 	var n, ns C.size_t
-	if rc := call(cd, cn, ck, cv, ce, cs, nil, 0, &n, nil, &ns); rc != C.KXPU_E_NOSPACE { // sizing call
+	if rc := call(strs[0], strs[1], tab, C.size_t(nt), cs, nil, 0, &n, nil, &ns); rc != C.KXPU_E_NOSPACE { // sizing call
 		return nil, kxCheck(k.ctx, what, rc)
 	}
 	buf := make([]byte, n)
 	off := make([]uint64, ns+1)
-	if err := kxCheck(k.ctx, what, call(cd, cn, ck, cv, ce, cs, (*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n,
+	if err := kxCheck(k.ctx, what, call(strs[0], strs[1], tab, C.size_t(nt), cs, (*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n,
 		(*C.uint64_t)(unsafe.Pointer(&off[0])), &ns)); err != nil {
 		return nil, err
 	}
@@ -742,70 +709,4 @@ func (k *kxpu) aerHealth(text []byte, fileOff []uint64, fileLen []uint32, fatalL
 		return nil, err
 	}
 	return append([]uint8(nil), unsafe.Slice((*uint8)(unsafe.Pointer(out)), nG)...), nil
-}
-
-// draSlicesTaint / draSlicesMdevTaint with the table [<driver>/unhealthy=vfio-device-missing, <driver>/pcie-aer=fatal,
-// <driver>/pcie-aer=nonfatal], all NoSchedule (ABI v12).  since holds three times per device, device-major, -1 where the
-// device does not carry that taint; a device carries at most one of the two pcie-aer values.
-func (k *kxpu) draSlicesTaints(driver, node string, generation uint64, devs []C.kxpu_dradev, since []int64) ([]string, error) {
-	var p *C.kxpu_dradev
-	if len(devs) > 0 {
-		p = &devs[0]
-	}
-	return k.taintsSlices("kxpu_dra_slices_taints", driver, node, len(devs), since, func(cd, cn *C.char, tab *C.kxpu_dra_taint,
-		cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t, ns *C.size_t) C.int32_t {
-		return C.kxpu_dra_slices_taints(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), tab, 3, cs, out,
-			capacity, n, off, ns)
-	})
-}
-
-func (k *kxpu) draSlicesMdevTaints(driver, node string, generation uint64, devs []C.kxpu_dramdev, since []int64) ([]string, error) {
-	var p *C.kxpu_dramdev
-	if len(devs) > 0 {
-		p = &devs[0]
-	}
-	return k.taintsSlices("kxpu_dra_slices_mdev_taints", driver, node, len(devs), since, func(cd, cn *C.char,
-		tab *C.kxpu_dra_taint, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
-		ns *C.size_t) C.int32_t {
-		return C.kxpu_dra_slices_mdev_taints(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), tab, 3, cs,
-			out, capacity, n, off, ns)
-	})
-}
-
-// the two-call sizing of one _taints call, the table and the times in C memory
-func (k *kxpu) taintsSlices(what, driver, node string, nDevs int, since []int64, call func(cd, cn *C.char,
-	tab *C.kxpu_dra_taint, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
-	ns *C.size_t) C.int32_t) ([]string, error) {
-	if len(since) != 3*nDevs {
-		return nil, fmt.Errorf("%s: %d taint times for %d devices", what, len(since), nDevs)
-	}
-	strs := []*C.char{C.CString(driver), C.CString(node), C.CString(driver + "/unhealthy"), C.CString("vfio-device-missing"),
-		C.CString(driver + "/pcie-aer"), C.CString("fatal"), C.CString("nonfatal"), C.CString("NoSchedule")}
-	for _, s := range strs {
-		defer C.free(unsafe.Pointer(s))
-	}
-	tab := (*C.kxpu_dra_taint)(C.malloc(C.size_t(3 * unsafe.Sizeof(C.kxpu_dra_taint{}))))
-	defer C.free(unsafe.Pointer(tab))
-	t := unsafe.Slice(tab, 3)
-	t[0] = C.kxpu_dra_taint{key: strs[2], value: strs[3], effect: strs[7]}
-	t[1] = C.kxpu_dra_taint{key: strs[4], value: strs[5], effect: strs[7]}
-	t[2] = C.kxpu_dra_taint{key: strs[4], value: strs[6], effect: strs[7]}
-	cs := (*C.int64_t)(C.malloc(C.size_t(8 * (len(since) + 1))))
-	defer C.free(unsafe.Pointer(cs))
-	copy(unsafe.Slice((*int64)(unsafe.Pointer(cs)), len(since)), since)
-	var n, ns C.size_t
-	if rc := call(strs[0], strs[1], tab, cs, nil, 0, &n, nil, &ns); rc != C.KXPU_E_NOSPACE { // sizing call
-		return nil, kxCheck(k.ctx, what, rc)
-	}
-	buf := make([]byte, n)
-	off := make([]uint64, ns+1)
-	if err := kxCheck(k.ctx, what, call(strs[0], strs[1], tab, cs, (*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n,
-		(*C.uint64_t)(unsafe.Pointer(&off[0])), &ns)); err != nil {
-		return nil, err
-	}
-	lines := make([]string, ns)
-	for s := range lines {
-		lines[s] = string(buf[off[s] : off[s+1]-1]) // without the '\n'
-	}
-	return lines, nil
 }

@@ -1250,7 +1250,7 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
                         "and generation below 2^63", what);
         return KXPU_E_INVALID;
     }
-    if (K::LIST && (!taint.table || taint.n == 0 || taint.n > KXPU_DRA_MAX_TAINTS)) {
+    if (TAINT && (!taint.table || taint.n == 0 || taint.n > KXPU_DRA_MAX_TAINTS)) {
         KX_SET_ERR(ctx, "%s: taints must hold 1..%d entries", what, KXPU_DRA_MAX_TAINTS);
         return KXPU_E_INVALID;
     }
@@ -1391,44 +1391,54 @@ extern "C" int32_t kxpu_dra_slices_mdev(kxpu_ctx *ctx, const char *driver, const
                                    n_slices);
 }
 
-// taint_since == NULL: exactly the untainted call, the taint arguments unread
+// kxpu_dra_slices[_mdev]_taint[s]: taint_since == NULL runs the untainted call with the taint arguments unread, one
+// entry the one-taint kernel, more the list kernel; dra_slices checks the table before either instantiation reads it
+template <int LAYOUT>
+static int32_t dra_slices_tainted(kxpu_ctx *ctx, const char *what, const char *driver, const char *pool, const char *node,
+                                  uint64_t generation, const typename DraLayout<LAYOUT>::Rec *devs, size_t n,
+                                  const kxpu_dra_taint *taints, size_t n_taints, const int64_t *taint_since, uint8_t *out,
+                                  size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
+    if (!taint_since)
+        return dra_slices<LAYOUT>(ctx, LAYOUT == LAYOUT_PCI ? "dra_slices" : "dra_slices_mdev", driver, pool, node, generation,
+                                  devs, n, out, cap, len, slice_off, n_slices);
+    const DraTaint taint{taints, n_taints, taint_since};
+    if (n_taints == 1)
+        return dra_slices<LAYOUT, DRA_TAINT_ONE>(ctx, what, driver, pool, node, generation, devs, n, out, cap, len, slice_off,
+                                                 n_slices, taint);
+    return dra_slices<LAYOUT, DRA_TAINT_LIST>(ctx, what, driver, pool, node, generation, devs, n, out, cap, len, slice_off,
+                                              n_slices, taint);
+}
+
 extern "C" int32_t kxpu_dra_slices_taint(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
                                          uint64_t generation, const kxpu_dradev *devs, size_t n, const char *taint_key,
                                          const char *taint_value, const char *taint_effect, const int64_t *taint_since,
                                          uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
-    if (!taint_since) return kxpu_dra_slices(ctx, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
     const kxpu_dra_taint t{taint_key, taint_value, taint_effect};
-    return dra_slices<LAYOUT_PCI, DRA_TAINT_ONE>(ctx, "dra_slices_taint", driver, pool, node, generation, devs, n, out, cap,
-                                                 len, slice_off, n_slices, DraTaint{&t, 1, taint_since});
+    return dra_slices_tainted<LAYOUT_PCI>(ctx, "dra_slices_taint", driver, pool, node, generation, devs, n, &t, 1, taint_since,
+                                          out, cap, len, slice_off, n_slices);
 }
 
 extern "C" int32_t kxpu_dra_slices_mdev_taint(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
                                               uint64_t generation, const kxpu_dramdev *devs, size_t n, const char *taint_key,
                                               const char *taint_value, const char *taint_effect, const int64_t *taint_since,
                                               uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
-    if (!taint_since)
-        return kxpu_dra_slices_mdev(ctx, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
     const kxpu_dra_taint t{taint_key, taint_value, taint_effect};
-    return dra_slices<LAYOUT_MDEV, DRA_TAINT_ONE>(ctx, "dra_slices_mdev_taint", driver, pool, node, generation, devs, n, out,
-                                                  cap, len, slice_off, n_slices, DraTaint{&t, 1, taint_since});
+    return dra_slices_tainted<LAYOUT_MDEV>(ctx, "dra_slices_mdev_taint", driver, pool, node, generation, devs, n, &t, 1,
+                                           taint_since, out, cap, len, slice_off, n_slices);
 }
 
-// taint_since == NULL: exactly the untainted call, the taint arguments unread
 extern "C" int32_t kxpu_dra_slices_taints(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
                                           uint64_t generation, const kxpu_dradev *devs, size_t n, const kxpu_dra_taint *taints,
                                           size_t n_taints, const int64_t *taint_since, uint8_t *out, size_t cap, size_t *len,
                                           uint64_t *slice_off, size_t *n_slices) {
-    if (!taint_since) return kxpu_dra_slices(ctx, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
-    return dra_slices<LAYOUT_PCI, DRA_TAINT_LIST>(ctx, "dra_slices_taints", driver, pool, node, generation, devs, n, out, cap,
-                                                  len, slice_off, n_slices, DraTaint{taints, n_taints, taint_since});
+    return dra_slices_tainted<LAYOUT_PCI>(ctx, "dra_slices_taints", driver, pool, node, generation, devs, n, taints, n_taints,
+                                          taint_since, out, cap, len, slice_off, n_slices);
 }
 
 extern "C" int32_t kxpu_dra_slices_mdev_taints(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
                                                uint64_t generation, const kxpu_dramdev *devs, size_t n,
                                                const kxpu_dra_taint *taints, size_t n_taints, const int64_t *taint_since,
                                                uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
-    if (!taint_since)
-        return kxpu_dra_slices_mdev(ctx, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
-    return dra_slices<LAYOUT_MDEV, DRA_TAINT_LIST>(ctx, "dra_slices_mdev_taints", driver, pool, node, generation, devs, n, out,
-                                                   cap, len, slice_off, n_slices, DraTaint{taints, n_taints, taint_since});
+    return dra_slices_tainted<LAYOUT_MDEV>(ctx, "dra_slices_mdev_taints", driver, pool, node, generation, devs, n, taints,
+                                           n_taints, taint_since, out, cap, len, slice_off, n_slices);
 }

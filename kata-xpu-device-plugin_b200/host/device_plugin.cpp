@@ -1610,54 +1610,40 @@ static const char *kDraTaintKeyName = "/unhealthy";  // the key is <draDriver>/u
 static const char *kDraTaintValue = "vfio-device-missing";
 static const char *kDraTaintEffect = "NoSchedule";
 
-// ResourceSlices / VgpuResourceSlices with draTaints: the two-call sizing of the _taint call fn
-template <typename Rec>
-static Error draTaintSlices(kxpu_ctx *ctx,
-                            int32_t (*fn)(kxpu_ctx *, const char *, const char *, const char *, uint64_t, const Rec *, size_t,
-                                          const char *, const char *, const char *, const int64_t *, uint8_t *, size_t,
-                                          size_t *, uint64_t *, size_t *),
-                            const char *what, const std::string &driver, const std::string &node, uint64_t generation,
-                            const std::vector<Rec> &devs, const std::vector<int64_t> &since, std::vector<uint8_t> &out,
-                            std::vector<uint64_t> &sliceOff) {
-    const std::string key = driver + kDraTaintKeyName;
-    size_t len = 0, nSlices = 0;
-    int32_t rc = fn(ctx, driver.c_str(), node.c_str(), node.c_str(), generation, devs.data(), devs.size(), key.c_str(),
-                    kDraTaintValue, kDraTaintEffect, since.data(), nullptr, 0, &len, nullptr, &nSlices);
-    if (rc == KXPU_E_NOSPACE) {
-        out.assign(len, 0);
-        sliceOff.assign(nSlices + 1, 0);
-        rc = fn(ctx, driver.c_str(), node.c_str(), node.c_str(), generation, devs.data(), devs.size(), key.c_str(),
-                kDraTaintValue, kDraTaintEffect, since.data(), out.data(), out.size(), &len, sliceOff.data(), &nSlices);
-    }
-    if (rc != KXPU_OK) return kxfail(ctx, what, rc);
-    return Error();
+// With aerHealth, the table goes on with the AER taint's two values.  The two AER entries share key and effect, so a
+// group carries at most one of them.
+static const char *kAerTaintKeyName = "/pcie-aer";  // the key is <draDriver>/pcie-aer
+
+bool Plugin::draPublished(bool vgpu, size_t g) const {
+    if (vgpu)
+        return g < mdevMap.size() && g < mdevDra.size() && g < mdevClass.size() && !vgpuClasses[mdevClass[g]].draDriver.empty();
+    return g < iommuMap.size() && g < iommuDra.size() && g < iommuClass.size() && !xpuClasses[iommuClass[g]].draDriver.empty() &&
+           (g >= iommuBlocker.size() || iommuBlocker[g].empty());
 }
 
-// With aerHealth too, the table of the _taints calls: the device-node taint, then the AER taint's two values.  The two
-// AER entries share key and effect, so a group carries at most one of them.
-static const char *kAerTaintKeyName = "/pcie-aer";  // the key is <draDriver>/pcie-aer
 template <typename Rec>
-static Error draTaintsSlices(kxpu_ctx *ctx,
-                             int32_t (*fn)(kxpu_ctx *, const char *, const char *, const char *, uint64_t, const Rec *, size_t,
-                                           const kxpu_dra_taint *, size_t, const int64_t *, uint8_t *, size_t, size_t *,
-                                           uint64_t *, size_t *),
-                             const char *what, const std::string &driver, const std::string &node, uint64_t generation,
-                             const std::vector<Rec> &devs, const std::vector<int64_t> &since, std::vector<uint8_t> &out,
-                             std::vector<uint64_t> &sliceOff) {
+Error Plugin::draSlices(int32_t (*fn)(kxpu_ctx *, const char *, const char *, const char *, uint64_t, const Rec *, size_t,
+                                      const kxpu_dra_taint *, size_t, const int64_t *, uint8_t *, size_t, size_t *, uint64_t *,
+                                      size_t *),
+                        const char *what, const std::string &driver, uint64_t generation, const std::vector<Rec> &devs,
+                        const std::vector<std::string> &groups, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) const {
     const std::string missing = driver + kDraTaintKeyName, aer = driver + kAerTaintKeyName;
     const kxpu_dra_taint table[3] = {{missing.c_str(), kDraTaintValue, kDraTaintEffect},
                                      {aer.c_str(), "fatal", kDraTaintEffect},
                                      {aer.c_str(), "nonfatal", kDraTaintEffect}};
+    const size_t nt = aerHealth ? 3 : 1;
+    const std::vector<int64_t> since = draTaints ? draSinceTable(groups) : std::vector<int64_t>();
+    const int64_t *ts = draTaints ? since.data() : nullptr;  // NULL: the untainted slices
     size_t len = 0, nSlices = 0;
-    int32_t rc = fn(ctx, driver.c_str(), node.c_str(), node.c_str(), generation, devs.data(), devs.size(), table, 3,
-                    since.data(), nullptr, 0, &len, nullptr, &nSlices);
+    int32_t rc = fn(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), generation, devs.data(), devs.size(), table, nt,
+                    ts, nullptr, 0, &len, nullptr, &nSlices);
     if (rc == KXPU_E_NOSPACE) {
         out.assign(len, 0);
         sliceOff.assign(nSlices + 1, 0);
-        rc = fn(ctx, driver.c_str(), node.c_str(), node.c_str(), generation, devs.data(), devs.size(), table, 3,
-                since.data(), out.data(), out.size(), &len, sliceOff.data(), &nSlices);
+        rc = fn(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), generation, devs.data(), devs.size(), table, nt, ts,
+                out.data(), out.size(), &len, sliceOff.data(), &nSlices);
     }
-    if (rc != KXPU_OK) return kxfail(ctx, what, rc);
+    if (rc != KXPU_OK) return kxfail(ctx_, what, rc);
     return Error();
 }
 
@@ -1665,15 +1651,14 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
     std::shared_lock<std::shared_mutex> lock(mu_);
     if (xpuClass >= xpuClasses.size() || xpuClasses[xpuClass].draDriver.empty())
         return fail("ResourceSlices: class " + std::to_string(xpuClass) + " has no DRA driver");
-    const std::string &driver = xpuClasses[xpuClass].draDriver;
     std::map<std::string, const std::string *> productOf;  // group id -> the resource-name suffix of its plugin
     for (const GenericDevicePlugin &dp : devicePlugins)
         if (!dp.vgpu && dp.xpuClass == xpuClass)
             for (const Device &d : dp.devs) productOf[d.ID] = &dp.devpluginName;
     std::vector<kxpu_dradev> devs;
     std::vector<std::string> groups;
-    for (size_t g = 0; g < iommuMap.size() && g < iommuDra.size(); g++) {
-        if (iommuClass[g] != xpuClass || (g < iommuBlocker.size() && !iommuBlocker[g].empty())) continue;
+    for (size_t g = 0; g < iommuMap.size(); g++) {
+        if (!draPublished(false, g) || iommuClass[g] != xpuClass) continue;
         kxpu_dradev d = iommuDra[g];
         auto it = productOf.find(iommuMap[g].first);
         if (it != productOf.end()) {
@@ -1683,40 +1668,18 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
         devs.push_back(d);
         groups.push_back(iommuMap[g].first);
     }
-    if (draTaints && aerHealth)
-        return draTaintsSlices(ctx_, kxpu_dra_slices_taints, "kxpu_dra_slices_taints", driver, nodeName, draGeneration_, devs,
-                               draSinceTable(groups), out, sliceOff);
-    if (draTaints) return draTaintSlices(ctx_, kxpu_dra_slices_taint, "kxpu_dra_slices_taint", driver, nodeName,
-                                         draGeneration_, devs, draSince(groups), out, sliceOff);
-    size_t len = 0, nSlices = 0;
-    int32_t rc = kxpu_dra_slices(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), draGeneration_, devs.data(),
-                                 devs.size(), nullptr, 0, &len, nullptr, &nSlices);
-    if (rc == KXPU_E_NOSPACE) {
-        out.assign(len, 0);
-        sliceOff.assign(nSlices + 1, 0);
-        rc = kxpu_dra_slices(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), draGeneration_, devs.data(), devs.size(),
-                             out.data(), out.size(), &len, sliceOff.data(), &nSlices);
-    }
-    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_dra_slices", rc);
-    return Error();
-}
-
-std::vector<int64_t> Plugin::draSince(const std::vector<std::string> &groups) const {
-    std::vector<int64_t> since;
-    for (const std::string &g : groups) {
-        auto it = draTaintSince_.find(g);
-        since.push_back(it == draTaintSince_.end() ? -1 : it->second);
-    }
-    return since;
+    return draSlices(kxpu_dra_slices_taints, "kxpu_dra_slices_taints", xpuClasses[xpuClass].draDriver, draGeneration_, devs,
+                     groups, out, sliceOff);
 }
 
 std::vector<int64_t> Plugin::draSinceTable(const std::vector<std::string> &groups) const {
     std::vector<int64_t> since;
     for (const std::string &g : groups) {
         auto it = draTaintSince_.find(g);
+        since.push_back(it == draTaintSince_.end() ? -1 : it->second);
+        if (!aerHealth) continue;
         auto at = aerTaint_.find(g);
         const uint8_t v = at == aerTaint_.end() ? 0 : at->second.first;
-        since.push_back(it == draTaintSince_.end() ? -1 : it->second);
         since.push_back(v == KXPU_AER_FATAL ? at->second.second : -1);
         since.push_back(v == KXPU_AER_NONFATAL ? at->second.second : -1);
     }
@@ -1792,12 +1755,10 @@ void Plugin::updateAerTaints(bool &passthroughMoved, bool &vgpuMoved) {
         if (v) next[g] = {v, was == v ? it->second.second : t};  // a new value gets a new time
         moved |= was != v;
     };
-    // the groups ResourceSlices / VgpuResourceSlices publish
-    for (size_t g = 0; g < iommuMap.size() && g < iommuClass.size() && g < iommuAerBits.size(); g++)
-        if (!xpuClasses[iommuClass[g]].draDriver.empty() && (g >= iommuBlocker.size() || iommuBlocker[g].empty()))
-            visit(iommuMap[g].first, iommuAerBits[g], passthroughMoved);
-    for (size_t g = 0; g < mdevMap.size() && g < mdevClass.size() && g < mdevAerBits.size(); g++)
-        if (!vgpuClasses[mdevClass[g]].draDriver.empty()) visit(mdevMap[g].first, mdevAerBits[g], vgpuMoved);
+    for (size_t g = 0; g < iommuAerBits.size(); g++)
+        if (draPublished(false, g)) visit(iommuMap[g].first, iommuAerBits[g], passthroughMoved);
+    for (size_t g = 0; g < mdevAerBits.size(); g++)
+        if (draPublished(true, g)) visit(mdevMap[g].first, mdevAerBits[g], vgpuMoved);
     aerTaint_ = std::move(next);
 }
 
@@ -1844,12 +1805,10 @@ Error Plugin::refreshDraHealth(bool &passthroughMoved, bool &vgpuMoved) {
         if (is) next[g] = was ? it->second : t;  // the time it turned unhealthy, kept while it stays so
         moved |= was != is;
     };
-    // the groups ResourceSlices / VgpuResourceSlices publish; a blocked group is not published, so it has no taint
-    for (size_t g = 0; g < iommuMap.size() && g < iommuClass.size(); g++)
-        if (!xpuClasses[iommuClass[g]].draDriver.empty() && (g >= iommuBlocker.size() || iommuBlocker[g].empty()))
-            visit(iommuMap[g].first, false, passthroughMoved);
-    for (size_t g = 0; g < mdevMap.size() && g < mdevClass.size(); g++)
-        if (!vgpuClasses[mdevClass[g]].draDriver.empty()) visit(mdevMap[g].first, true, vgpuMoved);
+    for (size_t g = 0; g < iommuMap.size(); g++)
+        if (draPublished(false, g)) visit(iommuMap[g].first, false, passthroughMoved);
+    for (size_t g = 0; g < mdevMap.size(); g++)
+        if (draPublished(true, g)) visit(mdevMap[g].first, true, vgpuMoved);
     draTaintSince_ = std::move(next);
     if (passthroughMoved) draGeneration_++;
     if (vgpuMoved) draVgpuGeneration_++;
@@ -1860,30 +1819,15 @@ Error Plugin::VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, st
     std::shared_lock<std::shared_mutex> lock(mu_);
     if (vgpuClass >= vgpuClasses.size() || vgpuClasses[vgpuClass].draDriver.empty())
         return fail("VgpuResourceSlices: vGPU class " + std::to_string(vgpuClass) + " has no DRA driver");
-    const std::string &driver = vgpuClasses[vgpuClass].draDriver;
     std::vector<kxpu_dramdev> devs;
     std::vector<std::string> groups;
-    for (size_t g = 0; g < mdevMap.size() && g < mdevDra.size() && g < mdevClass.size(); g++)
-        if (mdevClass[g] == vgpuClass) {
+    for (size_t g = 0; g < mdevMap.size(); g++)
+        if (draPublished(true, g) && mdevClass[g] == vgpuClass) {
             devs.push_back(mdevDra[g]);
             groups.push_back(mdevMap[g].first);
         }
-    if (draTaints && aerHealth)
-        return draTaintsSlices(ctx_, kxpu_dra_slices_mdev_taints, "kxpu_dra_slices_mdev_taints", driver, nodeName,
-                               draVgpuGeneration_, devs, draSinceTable(groups), out, sliceOff);
-    if (draTaints) return draTaintSlices(ctx_, kxpu_dra_slices_mdev_taint, "kxpu_dra_slices_mdev_taint", driver, nodeName,
-                                         draVgpuGeneration_, devs, draSince(groups), out, sliceOff);
-    size_t len = 0, nSlices = 0;
-    int32_t rc = kxpu_dra_slices_mdev(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), draVgpuGeneration_, devs.data(),
-                                      devs.size(), nullptr, 0, &len, nullptr, &nSlices);
-    if (rc == KXPU_E_NOSPACE) {
-        out.assign(len, 0);
-        sliceOff.assign(nSlices + 1, 0);
-        rc = kxpu_dra_slices_mdev(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), draVgpuGeneration_, devs.data(),
-                                  devs.size(), out.data(), out.size(), &len, sliceOff.data(), &nSlices);
-    }
-    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_dra_slices_mdev", rc);
-    return Error();
+    return draSlices(kxpu_dra_slices_mdev_taints, "kxpu_dra_slices_mdev_taints", vgpuClasses[vgpuClass].draDriver,
+                     draVgpuGeneration_, devs, groups, out, sliceOff);
 }
 
 Error Plugin::PrepareDraDevices(const std::string &driver, const std::string &pool, const std::vector<std::string> &deviceNames,

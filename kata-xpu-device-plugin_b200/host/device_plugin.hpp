@@ -285,9 +285,10 @@ class Plugin {
     bool vgpuDraEnabled() const;  // some vGPU class has a draDriver
     bool readsMdevNuma() const { return topologyAware || vgpuDraEnabled(); }
     // DRA device taints (ABI v11).  false (default): the slices never carry taints and every output and generation is as
-    // above, even while a device is Unhealthy.  true: ResourceSlices and VgpuResourceSlices go through the _taint calls
-    // (64 devices per slice); a group that refreshDraHealth found unhealthy carries the taint <draDriver>/unhealthy =
-    // vfio-device-missing:NoSchedule since the time it was found so, and PrepareDraDevices refuses it.
+    // above, even while a device is Unhealthy.  true: ResourceSlices and VgpuResourceSlices pass taint times to the
+    // slice call (64 devices per slice); a group that refreshDraHealth found unhealthy carries the taint
+    // <draDriver>/unhealthy=vfio-device-missing:NoSchedule since the time it was found so, and PrepareDraDevices refuses
+    // it.
     bool draTaints = false;
     // the clock of refreshDraHealth, unix seconds; a seam (time(nullptr) when empty)
     std::function<int64_t()> now;
@@ -464,7 +465,6 @@ class Plugin {
     uint64_t snapshotGen_ = 0;
     uint64_t draGeneration_ = 1, draVgpuGeneration_ = 1;
     std::map<std::string, int64_t> draTaintSince_;  // draTaints: IOMMU group id -> when its taint was added
-    std::vector<int64_t> draSince(const std::vector<std::string> &groups) const;  // per group: its time, or -1
     // aerHealth: the reason and the KXPU_AER_* bits of every iommuMap / mdevMap entry (same positions)
     std::vector<std::string> iommuAer, mdevAer;
     std::vector<uint8_t> iommuAerBits, mdevAerBits;
@@ -473,7 +473,19 @@ class Plugin {
     Error computeAer();  // the reads and the kxpu_aer_health call for the current maps
     // aerTaint_ from the last computeAer for the groups the DRA pools publish; which pools' taints changed
     void updateAerTaints(bool &passthroughMoved, bool &vgpuMoved);
-    std::vector<int64_t> draSinceTable(const std::vector<std::string> &groups) const;  // [groups * 3] for the _taints call
+    // per group its time in draTaintSince_, then with aerHealth its pcie-aer=fatal and =nonfatal times; -1: no such taint
+    std::vector<int64_t> draSinceTable(const std::vector<std::string> &groups) const;
+    // group g of iommuMap (vgpu: mdevMap) is published in its class's pool: the class has a draDriver and, for
+    // passthrough, the group has no viability blocker.  Only a published group gets taints.
+    bool draPublished(bool vgpu, size_t g) const;
+    // one pool's slices of devs, the records of groups, through fn (kxpu_dra_slices_taints or _mdev_taints) with the
+    // table <driver>/unhealthy=vfio-device-missing, then with aerHealth <driver>/pcie-aer=fatal and =nonfatal, all
+    // NoSchedule; without draTaints taint_since is NULL (the untainted bytes)
+    template <typename Rec>
+    Error draSlices(int32_t (*fn)(kxpu_ctx *, const char *, const char *, const char *, uint64_t, const Rec *, size_t,
+                                  const kxpu_dra_taint *, size_t, const int64_t *, uint8_t *, size_t, size_t *, uint64_t *, size_t *),
+                    const char *what, const std::string &driver, uint64_t generation, const std::vector<Rec> &devs,
+                    const std::vector<std::string> &groups, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) const;
     Error checkDraClasses() const;
     void buildMdevDra(const MdevWalk &w);
 };

@@ -160,7 +160,8 @@ def test_refusals_leave_outputs(kx, layout):
                                                       for e in entries])
     t3 = tab(AC.TABLE3)
     ok = np.full((5, 3), -1, np.int64); ok[:, 0] = 7; ok[2, 1] = 8; ok[3, 2] = 9
-    cases = [(t3, 0, ok, -1), (None, 3, ok, -1), (tab(AC.long_table(4) + [AC.TABLE3[0]]), 5, np.zeros((5, 5), np.int64), -1)]
+    cases = [(t3, 0, ok, -1), (None, 3, ok, -1), (None, 1, ok[:, :1], -1),
+             (tab(AC.long_table(4) + [AC.TABLE3[0]]), 5, np.zeros((5, 5), np.int64), -1)]
     for key, value, effect in TC.INVALID:
         cases.append((tab([AC.TABLE3[0], (key, value, effect)]), 2, np.zeros((5, 2), np.int64), -1))
     dup = ok.copy(); dup[4, 1:] = [0, 0]
