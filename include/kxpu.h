@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 12
+#define KXPU_ABI_VERSION 13
 
 /* status codes */
 #define KXPU_OK             0
@@ -72,7 +72,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
 #define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's and kxpu_pcie_tree's kernels: the slot holds the most recent call's */
-#define KXPU_T_EMIT     5
+#define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
 #define KXPU_T_COUNT    8
@@ -657,6 +657,37 @@ typedef struct kxpu_mdevcdi {
  *   - JSON: it holds no '"', '\\', control byte, '<', '>' or '&', so encoding/json escapes nothing. */
 int32_t kxpu_cdi_emit_mdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_mdevcdi *devs, size_t n,
                            uint8_t *out, size_t cap, size_t *len);
+
+/* ------------------------------------------------- CDI spec parse (ABI v13) */
+
+/* The shortest device fragment of any document kxpu_cdi_emit_kind / kxpu_cdi_emit_mdev write (YAML, a 3-byte kind,
+ * one-digit index and group, a one-byte bdf): a document of len bytes names at most len / KXPU_CDI_FRAG_MIN devices,
+ * so cap = len / KXPU_CDI_FRAG_MIN needs no second call. */
+#define KXPU_CDI_FRAG_MIN 166
+
+/* The inverse of kxpu_cdi_emit_kind: the records of a CDI spec this library wrote, so that a restarted plugin can read
+ * back the indices it handed out (the container runtime resolves <kind>=<index> against these very bytes).
+ *   - KXPU_OK with *n records exactly when kxpu_cdi_emit_kind(format, kind, out, *n) returns doc byte for byte.  The
+ *     records come back in document order; any device order is accepted, not only ascending index.  bdf is NUL padded
+ *     and reserved is 0, as the emitter's input would hold them.  The zero-device documents (YAML "devices: []", JSON
+ *     "devices": null) give *n = 0.
+ *   - KXPU_E_INVALID for every other document (nothing written to out, *n untouched), and for ctx, n or kind NULL, doc
+ *     NULL with len > 0, out NULL with cap > 0, or a format other than KXPU_FMT_YAML / KXPU_FMT_JSON.  A document whose
+ *     bdf the emitter refuses (KXPU_E_UNSUPPORTED) is not one it writes: KXPU_E_INVALID.
+ *   - cap < *n: *n is stored and the call returns KXPU_E_NOSPACE, nothing written to out (KXPU_CDI_FRAG_MIN bounds *n).
+ *   - KXPU_E_UNSUPPORTED: kind outside kxpu_cdi_emit_kind's domain, or len >= 2^32.
+ * GPU: one decode kernel over the document in 8 KiB tiles (device starts by ballot, record slots by the decoupled
+ * look-back), then the emitter's own kernel re-emits the decoded records into device scratch and a compare kernel
+ * holds them against the document, so "accepted" and "round-trips" are the same statement.  The span from the decode
+ * to the compare (one host read of the device count in between) is timed under KXPU_T_EMIT. */
+int32_t kxpu_cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
+                       kxpu_cdidev *out, size_t cap, size_t *n);
+
+/* The same for kxpu_cdi_emit_mdev's documents: KXPU_OK with *n records exactly when kxpu_cdi_emit_mdev(format, kind, out,
+ * *n) returns doc byte for byte; a uuid outside the canonical lowercase form or a parent the emitter refuses makes the
+ * document KXPU_E_INVALID.  Everything else as kxpu_cdi_parse. */
+int32_t kxpu_cdi_parse_mdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
+                            kxpu_mdevcdi *out, size_t cap, size_t *n);
 
 /* ------------------------------------------------------ S5: Allocate names */
 

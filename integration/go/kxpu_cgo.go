@@ -594,6 +594,100 @@ func (k *kxpu) reconcile(prev []C.kxpu_snaprec, nextIndex uint64, cur []C.kxpu_s
 	return snap, curState[:len(cur)], prevState[:len(prev)], counts, nil
 }
 
+// Restart resume (ABI v13).  cdiParse / cdiParseMdev read back a CDI spec this library wrote: the records, in document
+// order, of which kxpu_cdi_emit_kind / kxpu_cdi_emit_mdev write exactly these bytes; any other document is an error
+// (KXPU_E_INVALID).  One call: len(doc) / KXPU_CDI_FRAG_MIN records hold every document.
+func (k *kxpu) cdiParse(format int, doc []byte, kind string) ([]C.kxpu_cdidev, error) {
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	out := make([]C.kxpu_cdidev, len(doc)/C.KXPU_CDI_FRAG_MIN+1)
+	var n C.size_t
+	var dp *C.uint8_t
+	if len(doc) > 0 {
+		dp = (*C.uint8_t)(unsafe.Pointer(&doc[0]))
+	}
+	err := kxCheck(k.ctx, "kxpu_cdi_parse", C.kxpu_cdi_parse(k.ctx, C.int32_t(format), ck, dp, C.size_t(len(doc)), &out[0],
+		C.size_t(len(out)), &n))
+	if err != nil {
+		return nil, err
+	}
+	return out[:n], nil
+}
+
+func (k *kxpu) cdiParseMdev(format int, doc []byte, kind string) ([]C.kxpu_mdevcdi, error) {
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	out := make([]C.kxpu_mdevcdi, len(doc)/C.KXPU_CDI_FRAG_MIN+1)
+	var n C.size_t
+	var dp *C.uint8_t
+	if len(doc) > 0 {
+		dp = (*C.uint8_t)(unsafe.Pointer(&doc[0]))
+	}
+	err := kxCheck(k.ctx, "kxpu_cdi_parse_mdev", C.kxpu_cdi_parse_mdev(k.ctx, C.int32_t(format), ck, dp, C.size_t(len(doc)),
+		&out[0], C.size_t(len(out)), &n))
+	if err != nil {
+		return nil, err
+	}
+	return out[:n], nil
+}
+
+// The index state file of the restart resume: <cdiConfigPath>.kata-xpu-cdi-index, "pci <next>\nmdev <next>\n".  The CDI
+// cache loads only *.json / *.yaml.  Write it (tmp + fsync + rename, only when its bytes change) whenever a next index
+// grows, before any spec that names the new indices.
+const indexStateName = ".kata-xpu-cdi-index"
+
+func readIndexState(cdiConfigPath string) (pciNext, mdevNext uint64, ok bool) {
+	b, err := os.ReadFile(cdiConfigPath + indexStateName)
+	if err != nil {
+		return 0, 0, false
+	}
+	var p, m uint64
+	if n, err := fmt.Sscanf(string(b), "pci %d\nmdev %d\n", &p, &m); err != nil || n != 2 ||
+		fmt.Sprintf("pci %d\nmdev %d\n", p, m) != string(b) {
+		fmt.Fprintf(os.Stderr, "CDI index state %s: malformed, resuming without it\n", cdiConfigPath+indexStateName)
+		return 0, 0, false
+	}
+	return p, m, true
+}
+
+// resumeWalk: the start-up reconcile of one walk against the previous specs.  prev holds one entry per parsed record
+// (key = bdf or UUID, the parsed group, klass = the position of the class whose file it came from, tag 0, the parsed
+// index), cur the first walk's entries in walk order (klass = the class of the entry's group, tag 0), stateNext the
+// state file's value (0 without one).  fallback != "" (a file that did not parse, an index or key named twice, an index
+// of 2^64-1) or a refused reconcile numbers the walk afresh from stateNext.  The caller rebuilds its maps with the
+// returned indices and keeps the usual snapshot (real tags) and counts.next_index_out, exactly as Plugin::resumeIndices
+// does in host/device_plugin.cpp.
+func (k *kxpu) resumeWalk(prev []C.kxpu_snaprec, stateNext uint64, cur []C.kxpu_snaprec, fallback string) (
+	index []uint64, counts C.kxpu_reconcile_counts, why string, err error) {
+	next := stateNext
+	for _, p := range prev {
+		if uint64(p.index)+1 > next {
+			next = uint64(p.index) + 1
+		}
+	}
+	why = fallback
+	for attempt := 0; attempt < 2; attempt++ {
+		if why != "" {
+			fmt.Fprintf(os.Stderr, "CDI index resume: %s; numbering this walk afresh from %d\n", why, stateNext)
+			prev, next = nil, stateNext
+		}
+		var snap []C.kxpu_snaprec
+		snap, _, _, counts, err = k.reconcile(prev, next, cur)
+		if err == nil {
+			index = make([]uint64, len(snap))
+			for i := range snap {
+				index[i] = uint64(snap[i].index)
+			}
+			return index, counts, why, nil
+		}
+		if why != "" || !strings.Contains(err.Error(), "invalid") {
+			return nil, counts, why, err
+		}
+		why = "kxpu_reconcile refused the previous entries: " + err.Error()
+	}
+	return nil, counts, why, err
+}
+
 // DRA ResourceSlices (ABI v9).  One pool per class with a DRA driver, named after the node (NODE_NAME): devs holds one
 // kxpu_dradev per published IOMMU group in walk order (groups with a viability blocker left out).  Returns the slices
 // as JSON Lines, one object per line; the caller POSTs each line to /apis/resource.k8s.io/v1/resourceslices and then

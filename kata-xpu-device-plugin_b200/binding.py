@@ -69,6 +69,7 @@ DRA_MAX_TAINTS = 4  # entries of the _taints calls' table (ABI v12)
 AER_FATAL, AER_NONFATAL, AER_UNKNOWN = 1, 2, 4  # kxpu_aer_health's group bits
 AER_FILE_MAX = 4096
 AER_UNKNOWN_COUNT = (1 << 64) - 1  # totals of an unknown count
+CDI_FRAG_MIN = 166  # the shortest device fragment of a CDI spec: len // CDI_FRAG_MIN records hold any document (ABI v13)
 
 
 class DraTaint(C.Structure):
@@ -90,7 +91,7 @@ ABI_SYMBOLS = [
     "kxpu_classify_topo", "kxpu_classify_mdev_topo", "kxpu_lw_encode_topo", "kxpu_preferred_allocation",
     "kxpu_reconcile", "kxpu_pcie_tree", "kxpu_preferred_allocation_pcie", "kxpu_classify_viable",
     "kxpu_dra_slices", "kxpu_dra_slices_mdev", "kxpu_dra_slices_taint", "kxpu_dra_slices_mdev_taint",
-    "kxpu_aer_health", "kxpu_dra_slices_taints", "kxpu_dra_slices_mdev_taints",
+    "kxpu_aer_health", "kxpu_dra_slices_taints", "kxpu_dra_slices_mdev_taints", "kxpu_cdi_parse", "kxpu_cdi_parse_mdev",
 ]
 
 
@@ -199,6 +200,8 @@ def load_library():
         "kxpu_dra_slices_mdev_taint": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, C.c_char_p, C.c_char_p,
                                              C.c_char_p, vp, vp, sz, C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_aer_health": (i32, [vp, vp, sz, vp, vp, sz, u64, u64, vp, vp, sz, vp, vp]),
+        "kxpu_cdi_parse": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_cdi_parse_mdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_dra_slices_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                          C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_mdev_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
@@ -778,6 +781,38 @@ class Kxpu:
         else:
             self._chk(self.L.kxpu_cdi_emit_kind(self.ctx, fmt, kb, dp, len(devs), _ptr(out), cap, C.byref(got)))
         return out[:got.value].tobytes()
+
+    def cdi_parse(self, fmt, doc, kind):
+        """kxpu_cdi_parse: the CDIDEV_DTYPE records of a CDI spec kxpu_cdi_emit_kind wrote (doc bytes, kind bytes or
+        str), in document order; KxpuError(E_INVALID) for any other document."""
+        return self._parse(self.L.kxpu_cdi_parse, CDIDEV_DTYPE, fmt, doc, kind)
+
+    def cdi_parse_mdev(self, fmt, doc, kind):
+        """kxpu_cdi_parse_mdev: the MDEVCDI_DTYPE records of a vGPU class's CDI spec."""
+        return self._parse(self.L.kxpu_cdi_parse_mdev, MDEVCDI_DTYPE, fmt, doc, kind)
+
+    def cdi_parse_raw(self, fmt, doc, kind, cap, mdev=False, offset=0):
+        """The bare call: doc placed at `offset` bytes past a 16-byte aligned host buffer, out of `cap` records.
+        Returns (status, n, records) with n and the records as the call left them (n = -1: not stored)."""
+        dtype = MDEVCDI_DTYPE if mdev else CDIDEV_DTYPE
+        fn = self.L.kxpu_cdi_parse_mdev if mdev else self.L.kxpu_cdi_parse
+        buf = np.zeros(len(doc) + offset + 16, np.uint8)
+        base = (-buf.ctypes.data) % 16
+        buf = buf[base:]
+        buf[offset:offset + len(doc)] = np.frombuffer(bytes(doc), np.uint8)
+        out = np.zeros(max(cap, 1), dtype)
+        n = C.c_size_t((1 << 64) - 1)
+        rc = fn(self.ctx, fmt, _kind(kind), buf.ctypes.data + offset if len(doc) else None, len(doc),
+                _ptr(out) if cap else None, cap, C.byref(n))
+        return rc, (-1 if n.value == (1 << 64) - 1 else n.value), out[:cap]
+
+    def _parse(self, fn, dtype, fmt, doc, kind):
+        doc = bytes(doc)
+        cap = len(doc) // CDI_FRAG_MIN
+        out = np.zeros(max(cap, 1), dtype)
+        n = C.c_size_t(0)
+        self._chk(fn(self.ctx, fmt, _kind(kind), doc, len(doc), _ptr(out), cap, C.byref(n)))
+        return out[:n.value].copy()
 
     def cdi_emit_len(self, fmt, devs, kind=None):
         """Sizing call of the two-call protocol: out = NULL, returns the required length."""

@@ -19,6 +19,7 @@
 #include <type_traits>
 #include <vector>
 
+#include "cdi.cuh"
 #include "common.cuh"
 #include "mdev.cuh"
 #include "scan.cuh"
@@ -893,21 +894,18 @@ static void emit_launch(kxpu_ctx *ctx, uint32_t tiles, const EmitParams &E) {
     k_cdi_fused<FMT, MAXF, LAYOUT><<<tiles, EMIT_THREADS, sizeof(TileSmem<MAXF>), ctx->stream>>>(E);
 }
 
-// mdev: devs is kxpu_mdevcdi[n], else kxpu_cdidev[n]
-static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const void *devs, size_t n, uint8_t *out,
-                        size_t cap, size_t *len, bool mdev = false) {
-    std::lock_guard<std::mutex> guard(ctx->mu);
-    cudaSetDevice(ctx->device);
-    kx_clear_timings(ctx);
-    const Parts &parts = mdev ? (format == KXPU_FMT_YAML ? h_yaml_mdev_parts : h_json_mdev_parts)
-                              : (format == KXPU_FMT_YAML ? h_yaml_parts : h_json_parts);
-    if (n == 0) {  // Devices stays nil: yaml "devices: []", json "devices": null (cdi/spec.go:42-49)
-        const std::string doc = part_text(parts, 8, kind);
-        *len = doc.size();
-        if (cap < *len || !out) return KXPU_E_NOSPACE;
-        memcpy(out, doc.data(), *len);
-        return KXPU_OK;
-    }
+static const Parts &parts_of(int32_t format, bool mdev) {
+    return mdev ? (format == KXPU_FMT_YAML ? h_yaml_mdev_parts : h_json_mdev_parts)
+                : (format == KXPU_FMT_YAML ? h_yaml_parts : h_json_parts);
+}
+
+bool kx_cdi_kind_ok(const char *kind) { return kind_ok(kind); }
+
+std::string kx_cdi_part(int32_t format, bool mdev, int k, const char *kind) { return part_text(parts_of(format, mdev), k, kind); }
+
+int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, const void *d_devs, size_t n, bool mdev,
+                            KxScratch &sc, uint8_t **d_out_p, unsigned long long **d_total_p, bool timed) {
+    const Parts &parts = parts_of(format, mdev);
     static bool attr_done = false;
     if (!attr_done) {
         cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAX_FRAG, LAYOUT_PCI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -945,22 +943,16 @@ static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const v
     // mdev kind the MAX_FRAG_MDEV one
     const bool long_frag = frag > (uint32_t)MAX_FRAG;
     if (frag > (uint32_t)(mdev ? MAX_FRAG_MDEV : MAX_FRAG_LONG)) return KXPU_E_INVALID;  // the literals grew: the bound must follow
-    const size_t dev_bytes = mdev ? sizeof(kxpu_mdevcdi) : sizeof(kxpu_cdidev);
-    KxScratch sc(ctx);
-    void *d_devs = nullptr;
     uint8_t *d_out = nullptr;
     unsigned long long *d_total = nullptr;
-    KX_CUDA(ctx, sc.alloc((void **)&d_devs, n * dev_bytes));
     KX_CUDA(ctx, sc.alloc((void **)&d_out, bound));
     KX_CUDA(ctx, sc.alloc((void **)&d_total, 16));
-    cudaMemcpyAsync(d_devs, devs, n * dev_bytes, cudaMemcpyHostToDevice, ctx->stream);
     cudaMemsetAsync(d_total, 0, 16, ctx->stream);
     E.devs = d_devs; E.n = N; E.out = d_out; E.total_out = d_total; E.flags = (uint32_t *)(d_total + 1);
     E.state = kx_scan_state(ctx, tiles);
     if (!E.state) return KXPU_E_NOMEM;
     E.epoch = kx_next_epoch(ctx);
-    {
-        KxTimer tm(ctx, KXPU_T_EMIT);
+    auto launch = [&]() {
         if (mdev) {
             if (format == KXPU_FMT_YAML) emit_launch<KXPU_FMT_YAML, MAX_FRAG_MDEV, LAYOUT_MDEV>(ctx, tiles, E);
             else emit_launch<KXPU_FMT_JSON, MAX_FRAG_MDEV, LAYOUT_MDEV>(ctx, tiles, E);
@@ -972,7 +964,40 @@ static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const v
             else emit_launch<KXPU_FMT_JSON, MAX_FRAG, LAYOUT_PCI>(ctx, tiles, E);
         }
         KX_LAUNCHED(ctx);
+    };
+    if (timed) {
+        KxTimer tm(ctx, KXPU_T_EMIT);
+        launch();
+    } else {
+        launch();
     }
+    *d_out_p = d_out;
+    *d_total_p = d_total;
+    return KXPU_OK;
+}
+
+// mdev: devs is kxpu_mdevcdi[n], else kxpu_cdidev[n]
+static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const void *devs, size_t n, uint8_t *out,
+                        size_t cap, size_t *len, bool mdev = false) {
+    std::lock_guard<std::mutex> guard(ctx->mu);
+    cudaSetDevice(ctx->device);
+    kx_clear_timings(ctx);
+    if (n == 0) {  // Devices stays nil: yaml "devices: []", json "devices": null (cdi/spec.go:42-49)
+        const std::string doc = kx_cdi_part(format, mdev, 8, kind);
+        *len = doc.size();
+        if (cap < *len || !out) return KXPU_E_NOSPACE;
+        memcpy(out, doc.data(), *len);
+        return KXPU_OK;
+    }
+    const size_t dev_bytes = mdev ? sizeof(kxpu_mdevcdi) : sizeof(kxpu_cdidev);
+    KxScratch sc(ctx);
+    void *d_devs = nullptr;
+    uint8_t *d_out = nullptr;
+    unsigned long long *d_total = nullptr;
+    KX_CUDA(ctx, sc.alloc((void **)&d_devs, n * dev_bytes));
+    cudaMemcpyAsync(d_devs, devs, n * dev_bytes, cudaMemcpyHostToDevice, ctx->stream);
+    const int32_t rc = kx_cdi_emit_enqueue(ctx, format, kind, d_devs, n, mdev, sc, &d_out, &d_total, true);
+    if (rc != KXPU_OK) return rc;
     unsigned long long h[2] = {0, 0};
     cudaMemcpyAsync(h, d_total, 16, cudaMemcpyDeviceToHost, ctx->stream);
     cudaError_t e = cudaStreamSynchronize(ctx->stream);

@@ -23,6 +23,7 @@
 #include <ctime>
 #include <set>
 #include <thread>
+#include <type_traits>
 
 namespace device_plugin {
 
@@ -569,6 +570,11 @@ Error Plugin::createIommuDeviceMap() {
     buildIommuMaps(w, nullptr);
     pciSnap_ = snapshotOf(w, nullptr);  // host bookkeeping for a later rediscovery: no GPU call
     pciNext_ = pciSnap_.size();
+    if (resumeIndices) {
+        resume_ = ResumeReport();
+        readIndexState();
+        return resumePci(w);
+    }
     return Error();
 }
 
@@ -880,6 +886,7 @@ Error Plugin::createMdevMap() {
     buildMdevMaps(w, nullptr);
     mdevSnap_ = snapshotOf(w, nullptr);
     mdevNext_ = mdevSnap_.size();
+    if (resumeIndices) return resumeMdev(w);
     return Error();
 }
 
@@ -1386,11 +1393,186 @@ Error Plugin::InitiateDevicePlugin() {
     if (e) return e;
     e = createMdevMap();
     if (e) return e;
+    if (resumeIndices) {  // the state file first, then the specs, atomically and only when their bytes changed
+        e = writeIndexState(&resume_.filesWritten);
+        if (e) return e;
+        atomicSpecs_ = true;
+        specsWritten_.clear();
+    }
     e = generateCDISpec(iommuMap);  // :49
-    if (e) return e;
-    e = generateMdevCDISpec();
+    if (!e) e = generateMdevCDISpec();
+    if (resumeIndices) {
+        atomicSpecs_ = false;
+        resume_.filesWritten.insert(resume_.filesWritten.end(), specsWritten_.begin(), specsWritten_.end());
+    }
     if (e) return e;
     return createDevicePlugins();  // :52
+}
+
+// ---------------------------------------------------------------------------- restart resume (resumeIndices)
+std::string formatIndexState(uint64_t pciNext, uint64_t mdevNext) {
+    return "pci " + std::to_string(pciNext) + "\nmdev " + std::to_string(mdevNext) + "\n";
+}
+
+// a canonical decimal below 2^64
+static bool parseU64(const std::string &s, uint64_t &v) {
+    if (s.empty() || s.size() > 20 || (s.size() > 1 && s[0] == '0')) return false;
+    uint64_t x = 0;
+    for (char c : s) {
+        if (c < '0' || c > '9') return false;
+        const uint64_t d = (uint64_t)(c - '0');
+        if (x > (UINT64_MAX - d) / 10) return false;
+        x = x * 10 + d;
+    }
+    v = x;
+    return true;
+}
+
+bool parseIndexState(const std::string &text, uint64_t &pciNext, uint64_t &mdevNext) {
+    const size_t nl = text.find('\n');
+    if (text.compare(0, 4, "pci ") != 0 || nl == std::string::npos || text.compare(nl + 1, 5, "mdev ") != 0) return false;
+    const size_t nl2 = text.find('\n', nl + 1);
+    if (nl2 == std::string::npos || nl2 + 1 != text.size()) return false;
+    uint64_t p = 0, m = 0;
+    if (!parseU64(text.substr(4, nl - 4), p) || !parseU64(text.substr(nl + 6, nl2 - nl - 6), m)) return false;
+    pciNext = p;
+    mdevNext = m;
+    return true;
+}
+
+static const char *kIndexStateName = ".kata-xpu-cdi-index";  // not *.json / *.yaml: the CDI cache ignores it
+
+static bool readWholeFile(const std::string &path, std::string &out, bool &missing) {
+    missing = false;
+    FILE *f = fopen(path.c_str(), "rb");
+    if (!f) { missing = errno == ENOENT; return false; }
+    out.clear();
+    char buf[1 << 16];
+    size_t k;
+    while ((k = fread(buf, 1, sizeof buf, f)) > 0) out.append(buf, k);
+    const bool ok = !ferror(f);
+    fclose(f);
+    return ok;
+}
+
+void Plugin::readIndexState() {
+    const std::string path = cdiConfigPath + kIndexStateName;
+    std::string text;
+    bool missing = false;
+    if (!readWholeFile(path, text, missing)) {
+        if (!missing) fprintf(stderr, "CDI index state %s: unreadable (%s), resuming without it\n", path.c_str(), strerror(errno));
+        return;
+    }
+    resume_.stateRead = parseIndexState(text, resume_.statePci, resume_.stateMdev);
+    if (!resume_.stateRead) fprintf(stderr, "CDI index state %s: malformed, resuming without it\n", path.c_str());
+}
+
+Error Plugin::writeIndexState(std::vector<std::string> *written) {
+    const std::string path = cdiConfigPath + kIndexStateName;
+    const std::string text = formatIndexState(pciNext_, mdevNext_);
+    bool w = false;
+    Error e = writeSpecFileAtomic(path, reinterpret_cast<const uint8_t *>(text.data()), text.size(), w);
+    if (w && written) written->push_back(path);
+    return e;
+}
+
+template <typename Rec>
+void Plugin::previousEntries(const std::vector<XpuClass> &classes,
+                             int32_t (*parse)(kxpu_ctx *, int32_t, const char *, const uint8_t *, size_t, Rec *, size_t, size_t *),
+                             uint64_t stateNext, ResumeWalk &rw, std::vector<kxpu_snaprec> &prev, uint64_t &next) {
+    prev.clear();
+    next = stateNext;
+    std::set<std::string> keys;
+    std::set<uint64_t> indices;
+    for (size_t c = 0; c < classes.size() && rw.fallback.empty(); c++) {
+        const std::string path = cdiConfigPath + classes[c].cdiFileStem + ".yaml";
+        std::string doc;
+        bool missing = false;
+        if (!readWholeFile(path, doc, missing)) {
+            if (!missing) rw.fallback = path + ": unreadable: " + strerror(errno);
+            continue;  // a missing file holds no entries
+        }
+        std::vector<Rec> recs(doc.size() / KXPU_CDI_FRAG_MIN + 1);
+        size_t n = 0;
+        const int32_t rc = parse(ctx_, KXPU_FMT_YAML, classes[c].cdiKind.c_str(), reinterpret_cast<const uint8_t *>(doc.data()),
+                                 doc.size(), recs.data(), recs.size(), &n);
+        if (rc != KXPU_OK) {
+            rw.fallback = path + ": not a CDI spec this plugin writes (" + kxpu_strerror(rc) + ": " + kxpu_last_error(ctx_) + ")";
+            break;
+        }
+        rw.filesRead.push_back(path);
+        for (size_t i = 0; i < n && rw.fallback.empty(); i++) {
+            const Rec &r = recs[i];
+            kxpu_snaprec s;
+            memset(&s, 0, sizeof s);
+            if constexpr (std::is_same<Rec, kxpu_mdevcdi>::value) memcpy(s.key, r.uuid, sizeof r.uuid);
+            else memcpy(s.key, r.bdf, strnlen(r.bdf, sizeof r.bdf));
+            s.iommu_group = r.iommu_group;
+            s.klass = (uint32_t)c;
+            s.index = r.index;
+            const std::string key(s.key, strnlen(s.key, sizeof s.key));
+            if (r.index == UINT64_MAX) rw.fallback = path + ": index 18446744073709551615";
+            else if (!indices.insert(r.index).second) rw.fallback = path + ": index " + std::to_string(r.index) + " named twice";
+            else if (!keys.insert(key).second) rw.fallback = path + ": " + key + " named twice";
+            else {
+                prev.push_back(s);
+                next = std::max(next, r.index + 1);
+            }
+        }
+    }
+}
+
+Error Plugin::resumeWalk(std::vector<kxpu_snaprec> prev, uint64_t next, uint64_t stateNext, const std::vector<kxpu_snaprec> &cur,
+                         ResumeWalk &rw, std::vector<uint64_t> &index, uint64_t &nextOut) {
+    index.assign(cur.size() + 1, 0);
+    for (int attempt = 0; attempt < 2; attempt++) {
+        if (!rw.fallback.empty()) {  // nothing known: fresh indices above everything the state file says was handed out
+            fprintf(stderr, "CDI index resume: %s; numbering this walk afresh from %llu\n", rw.fallback.c_str(),
+                    (unsigned long long)stateNext);
+            prev.clear();
+            next = stateNext;
+        }
+        const int32_t rc = kxpu_reconcile(ctx_, prev.data(), prev.size(), next, cur.data(), cur.size(), index.data(), nullptr,
+                                          nullptr, &rw.counts);
+        if (rc == KXPU_OK) break;
+        if (rc != KXPU_E_INVALID || !rw.fallback.empty()) return kxfail(ctx_, "kxpu_reconcile", rc);
+        rw.fallback = std::string("kxpu_reconcile refused the previous entries: ") + kxpu_last_error(ctx_);
+    }
+    index.resize(cur.size());
+    nextOut = rw.counts.next_index_out;
+    return Error();
+}
+
+Error Plugin::resumePci(const PciWalk &w) {
+    std::vector<kxpu_snaprec> prev;
+    uint64_t next = 0;
+    const uint64_t stateNext = resume_.stateRead ? resume_.statePci : 0;
+    previousEntries<kxpu_cdidev>(xpuClasses, kxpu_cdi_parse, stateNext, resume_.pci, prev, next);
+    std::vector<kxpu_snaprec> cur = snapshotOf(w, nullptr);
+    std::map<uint32_t, size_t> groupClass = groupClasses(w.out);  // the file generateClassSpecs puts the entry in
+    for (kxpu_snaprec &s : cur) { s.klass = (uint32_t)groupClass[s.iommu_group]; s.tag = 0; }
+    std::vector<uint64_t> index;
+    Error e = resumeWalk(std::move(prev), next, stateNext, cur, resume_.pci, index, pciNext_);
+    if (e) return e;
+    buildIommuMaps(w, &index);
+    pciSnap_ = snapshotOf(w, &index);
+    return Error();
+}
+
+Error Plugin::resumeMdev(const MdevWalk &w) {
+    std::vector<kxpu_snaprec> prev;
+    uint64_t next = 0;
+    const uint64_t stateNext = resume_.stateRead ? resume_.stateMdev : 0;
+    previousEntries<kxpu_mdevcdi>(vgpuClasses, kxpu_cdi_parse_mdev, stateNext, resume_.mdev, prev, next);
+    std::vector<kxpu_snaprec> cur = snapshotOf(w, nullptr);
+    std::map<uint32_t, size_t> groupClass = groupClasses(w.out);
+    for (kxpu_snaprec &s : cur) { s.klass = (uint32_t)groupClass[s.iommu_group]; s.tag = 0; }
+    std::vector<uint64_t> index;
+    Error e = resumeWalk(std::move(prev), next, stateNext, cur, resume_.mdev, index, mdevNext_);
+    if (e) return e;
+    buildMdevMaps(w, &index);
+    mdevSnap_ = snapshotOf(w, &index);
+    return Error();
 }
 
 bool Plugin::discoveryStale() {
@@ -1451,6 +1633,10 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     }
     e = computeAer();  // a re-enumerated function starts with zeroed counters
     if (e) return e;
+    if (resumeIndices) {  // the next indices reach the state file before any spec names one of them
+        e = writeIndexState(nullptr);
+        if (e) return e;
+    }
     // 4. the CDI specs: a file is rewritten only when its bytes changed, atomically
     atomicSpecs_ = true;
     specsWritten_.clear();
@@ -2769,6 +2955,37 @@ void kxh_set_aer_health(void *h, int on, uint64_t fatal_limit, uint64_t nonfatal
     p->aerNonFatalLimit = nonfatal_limit;
 }
 uint64_t kxh_aer_reads(void *h) { return ((Plugin *)h)->aerReads; }
+
+// ---- restart resume of CDI indices (ABI v13)
+void kxh_set_resume(void *h, int on) { ((Plugin *)h)->resumeIndices = on != 0; }
+// kxh_init's state of the plugin as it stands (after kxh_initiate), with the resume report
+int kxh_state(void *h, char *json, size_t cap) {
+    Plugin *p = (Plugin *)h;
+    const device_plugin::ResumeReport &r = p->resumeReport();
+    std::string o = dumpState(p) + ",\"resume\":{";
+    for (const auto &c : {std::make_pair("pci", &r.pci), std::make_pair("mdev", &r.mdev)}) {
+        const kxpu_reconcile_counts &k = c.second->counts;
+        o += "\"" + std::string(c.first) + "\":{\"n_kept\":" + std::to_string(k.n_kept) + ",\"n_new\":" + std::to_string(k.n_new) +
+             ",\"n_changed\":" + std::to_string(k.n_changed) + ",\"n_retired\":" + std::to_string(k.n_retired) +
+             ",\"next_index_out\":" + std::to_string(k.next_index_out) + ",\"files\":[";
+        for (size_t i = 0; i < c.second->filesRead.size(); i++) { if (i) o += ','; jstr(o, c.second->filesRead[i]); }
+        o += "],\"fallback\":";
+        jstr(o, c.second->fallback);
+        o += "},";
+    }
+    o += "\"stateRead\":" + std::string(r.stateRead ? "true" : "false") + ",\"statePci\":" + std::to_string(r.statePci) +
+         ",\"stateMdev\":" + std::to_string(r.stateMdev) + ",\"written\":[";
+    for (size_t i = 0; i < r.filesWritten.size(); i++) { if (i) o += ','; jstr(o, r.filesWritten[i]); }
+    o += "]}}";
+    return copy_out(o, json, cap);
+}
+// CPU only: the index state file's text for (pci, mdev), and its parse (1 = well formed)
+int kxh_index_state_format(uint64_t pci, uint64_t mdev, char *out, size_t cap) {
+    return copy_out(device_plugin::formatIndexState(pci, mdev), out, cap);
+}
+int kxh_index_state_parse(const char *text, size_t len, uint64_t *pci, uint64_t *mdev) {
+    return device_plugin::parseIndexState(std::string(text, len), *pci, *mdev) ? 1 : 0;
+}
 // refreshAerHealth: changed[0 .. *n_changed) = the plugins whose ListAndWatch bytes changed (at most cap written),
 // *moved as kxh_refresh_dra_health's; -1 with the message in err
 int kxh_refresh_aer_health(void *h, size_t *changed, size_t cap, size_t *n_changed, int *moved, char *err, size_t errcap) {

@@ -180,8 +180,25 @@ struct RediscoverReport {
     std::vector<std::string> cdiFilesWritten;  // spec files whose bytes changed (rewritten atomically)
 };
 
+// What Plugin::resumeIndices did at start-up for one walk (PCI or mdev).
+struct ResumeWalk {
+    kxpu_reconcile_counts counts{};      // the previous specs' entries against the first walk, and the next index
+    std::vector<std::string> filesRead;  // spec files read and parsed (a missing file is not listed)
+    std::string fallback;                // why the walk resumed from nothing known; empty: it resumed from its specs
+};
+struct ResumeReport {
+    ResumeWalk pci, mdev;
+    bool stateRead = false;                    // the index state file was there and well formed
+    uint64_t statePci = 0, stateMdev = 0;      // its values (0 when it was not read)
+    std::vector<std::string> filesWritten;     // spec and state files whose bytes changed at start-up
+};
+
 // the atomic spec writer of Plugin::rediscover (exposed for CPU tests)
 Error writeSpecFileAtomicForTests(const std::string &file_path, const uint8_t *doc, size_t len, bool &written);
+// The index state file of Plugin::resumeIndices: "pci <next>\nmdev <next>\n", canonical decimals.  format / parse are
+// exact inverses; parse refuses anything else.
+std::string formatIndexState(uint64_t pciNext, uint64_t mdevNext);
+bool parseIndexState(const std::string &text, uint64_t &pciNext, uint64_t &mdevNext);
 
 // The output arrays of one classify call (kxpu_classify_out + dev_rule + group_numa) and their counts.
 struct ClassifyResult {
@@ -305,6 +322,21 @@ class Plugin {
     uint64_t aerFatalLimit = 0, aerNonFatalLimit = 0;
     // <base>/<entry>/<name>, at most KXPU_AER_FILE_MAX + 1 bytes; false or an empty out: a failed read (unknown count)
     std::function<bool(const std::string &base, const std::string &entry, const std::string &name, std::string &out)> readAerFile;
+    // Restart resume of CDI indices (include/kxpu.h, ABI v13).  false (default): nothing more is read or written and every
+    // index is the walk order of the first walk.  true: InitiateDevicePlugin reads back the CDI specs a previous process
+    // wrote (<cdiConfigPath><cdiFileStem>.yaml of every class, kxpu_cdi_parse / kxpu_cdi_parse_mdev) and the index state
+    // file <cdiConfigPath>.kata-xpu-cdi-index, and reconciles the first walks against them (kxpu_reconcile), so that a
+    // function at the same bdf (a vGPU: the same UUID) in the same IOMMU group, whose group belongs to the same class file,
+    // keeps the index its spec names.  The spec does not hold the device id, so a function whose model changed at the
+    // same bdf and group keeps its index too; the runtime resolves the name to the same /dev/vfio/<g> either way.  Every
+    // other function gets an index above every index handed out before.  A walk whose specs cannot be trusted (a file
+    // that does not parse, an index or key in two entries, an index of 2^64-1) resumes from nothing known: fresh indices
+    // from the state file's value (walk order without one), with a log line.  Start-up then writes the specs like
+    // rediscover does (atomically, only when their bytes changed), and both start-up and rediscover keep the state file
+    // current before any spec is written.  It rests on the kubelet reusing a restarted container's checkpointed
+    // Allocate response [assumed].
+    bool resumeIndices = false;
+    const ResumeReport &resumeReport() const { return resume_; }
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
     uint64_t aerReads = 0;  // aer_dev_* files read (tests, metrics)
 
@@ -373,7 +405,7 @@ class Plugin {
     // never handed out before), rebuild the maps, rewrite each CDI spec whose bytes changed (atomically), update
     // devicePlugins in place (matched by vgpu, class and device key; health carried per group, new groups Healthy, new
     // plugins appended, a plugin whose devices all left keeps an empty list) and take a fresh snapshot generation.
-    // A restart numbers by walk order again: the index high-water mark is not persisted.
+    // A restart numbers by walk order again unless resumeIndices is on.
     Error rediscover(RediscoverReport &report, const std::string &format = "YAML");
     // The ResourceSlices of class xpuClass (kxpu_dra_slices): one pool named nodeName, one device per iommuMap group of
     // the class in walk order (bdf, vendor, device and PCIe root of the group's first member, the group's NUMA mask, the
@@ -452,6 +484,20 @@ class Plugin {
     std::vector<kxpu_snaprec> snapshotOf(const PciWalk &w, const std::vector<uint64_t> *index) const;
     std::vector<kxpu_snaprec> snapshotOf(const MdevWalk &w, const std::vector<uint64_t> *index) const;
     Error buildPlugins(std::vector<GenericDevicePlugin> &out);
+    // resumeIndices: the previous specs' entries of one walk and its next index, from the state file and the specs
+    template <typename Rec>
+    void previousEntries(const std::vector<XpuClass> &classes,
+                         int32_t (*parse)(kxpu_ctx *, int32_t, const char *, const uint8_t *, size_t, Rec *, size_t, size_t *),
+                         uint64_t stateNext, ResumeWalk &rw, std::vector<kxpu_snaprec> &prev, uint64_t &next);
+    // resumeIndices: reconcile the first walk's entries `cur` (klass = the class of the entry's group, tag 0) against the
+    // previous specs; index gets one index per cur entry, nextOut the walk's next index
+    Error resumeWalk(std::vector<kxpu_snaprec> prev, uint64_t next, uint64_t stateNext, const std::vector<kxpu_snaprec> &cur,
+                     ResumeWalk &rw, std::vector<uint64_t> &index, uint64_t &nextOut);
+    Error resumePci(const PciWalk &w);
+    Error resumeMdev(const MdevWalk &w);
+    void readIndexState();  // into resume_
+    Error writeIndexState(std::vector<std::string> *written);
+    ResumeReport resume_;
     bool atomicSpecs_ = false;  // rediscover: specs are written only when changed, through .tmp + fsync + rename
     std::vector<std::string> specsWritten_;
     Error writeSpec(const std::string &path, const std::vector<uint8_t> &doc, size_t len, bool &written);
