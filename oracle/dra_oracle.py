@@ -3,15 +3,11 @@
 TEST INFRASTRUCTURE ONLY, like oracle.py: imported by tests/, never by the product package.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "kxpu_dra_oracle.c")
-_SO = os.path.join(_HERE, "libkxpu_dra_oracle.so")
-_LIB = None
+from . import oracle as O
+from .oracle import _HERE  # noqa: F401  (the layout tests find include/kxpu.h from it)
 
 # kxpu_dradev, as include/kxpu.h declares it (tests compare it with the product binding's dtype)
 DRADEV_DTYPE = np.dtype([("product", "u1", (64,)), ("bdf", "S16"), ("pcie_root", "S16"), ("vendor", "S8"), ("device", "S8"),
@@ -20,46 +16,32 @@ assert DRADEV_DTYPE.itemsize == 128
 WHY = ["product", "bdf", "pcie_root", "vendor", "device", "iommu_group", "product_len"]
 
 
-def build():
-    deps = [_SRC, os.path.join(_HERE, "..", "include", "kxpu.h")]
-    if os.path.exists(_SO) and os.path.getmtime(_SO) >= max(os.path.getmtime(d) for d in deps):
-        return
-    subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-Wall", "-Wextra", "-fPIC", "-shared", "-o", _SO, _SRC])
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        build()
-        L = C.CDLL(_SO)
-        vp, sz = C.c_void_p, C.c_size_t
-        L.kxo_dra_slices.restype = C.c_int32
-        L.kxo_dra_slices.argtypes = [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, vp, sz, vp, sz, C.POINTER(sz), vp,
-                                     C.POINTER(sz), C.POINTER(C.c_int32)]
-        _LIB = L
-    return _LIB
-
-
 def _b(s):
     return s.encode() if isinstance(s, str) else s
+
+
+def slices_call(fn, dtype, why_names, driver, pool, node, generation, devs, *rest):
+    """The two-call sizing of every kxo_dra_slices* call: fn(driver, pool, node, generation, devs, n, *rest, out, cap,
+    &need, slice_off, &n_slices, &why), once to size the outputs and once to fill them.  Returns (bytes, slice_off), or
+    the failing status: -1 for a bad argument; for a record outside the domain (-7, why_names[*why])."""
+    devs = np.ascontiguousarray(devs)
+    assert devs.dtype == dtype
+    dp = devs.ctypes.data if len(devs) else None
+    need, ns, why = C.c_size_t(0), C.c_size_t(0), C.c_int32(-1)
+    args = (_b(driver), _b(pool), _b(node), generation, dp, len(devs)) + rest
+    rc = fn(*args, None, 0, C.byref(need), None, C.byref(ns), C.byref(why))
+    if rc == -7:
+        return rc, why_names[why.value] if why.value >= 0 else None
+    if rc != -4:
+        return rc
+    out = np.empty(max(need.value, 1), np.uint8)
+    offs = np.empty(ns.value + 1, np.uint64)
+    rc = fn(*args, out.ctypes.data, need.value, C.byref(need), offs.ctypes.data, C.byref(ns), C.byref(why))
+    assert rc == 0, rc
+    return out[:need.value].tobytes(), offs
 
 
 def dra_slices(driver, pool, node, generation, devs):
     """(bytes, slice_off) of kxo_dra_slices, or the failing status: -1 for a bad argument; for a record outside the
     domain (-7, name of the first failing rule)."""
-    L = lib()
-    devs = np.ascontiguousarray(devs)
-    assert devs.dtype == DRADEV_DTYPE
-    dp = devs.ctypes.data if len(devs) else None
-    need, ns, why = C.c_size_t(0), C.c_size_t(0), C.c_int32(-1)
-    args = (_b(driver), _b(pool), _b(node), generation, dp, len(devs))
-    rc = L.kxo_dra_slices(*args, None, 0, C.byref(need), None, C.byref(ns), C.byref(why))
-    if rc == -7:
-        return rc, WHY[why.value] if why.value >= 0 else None
-    if rc != -4:
-        return rc
-    out = np.empty(max(need.value, 1), np.uint8)
-    offs = np.empty(ns.value + 1, np.uint64)
-    rc = L.kxo_dra_slices(*args, out.ctypes.data, need.value, C.byref(need), offs.ctypes.data, C.byref(ns), C.byref(why))
-    assert rc == 0, rc
-    return out[:need.value].tobytes(), offs
+    return slices_call(O.lib().kxo_dra_slices, DRADEV_DTYPE, WHY, driver, pool, node, generation, devs)

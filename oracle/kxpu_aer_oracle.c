@@ -10,6 +10,10 @@
  * TEST INFRASTRUCTURE ONLY, like kxpu_oracle.c.  Arguments and status codes are the product calls' without the context;
  * on KXPU_E_UNSUPPORTED *why names the first rule the first record outside the domain breaks (the record rules of the
  * layout, then "taint_since", then "taint_duplicate").
+ *
+ * This file is the root of the DRA oracles' one translation unit: it includes kxpu_dra_taint_oracle.c, which includes
+ * kxpu_dra_mdev_oracle.c, which includes kxpu_dra_oracle.c, so the four share the static Buf writer and domain helpers.
+ * oracle/Makefile compiles this file into libkxpu_oracle.so and not those three.
  */
 #include "kxpu_dra_taint_oracle.c"
 

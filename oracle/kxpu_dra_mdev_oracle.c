@@ -3,10 +3,10 @@
  * DRA pool of vGPUs as JSON Lines, written sequentially with snprintf from the rules stated in the header.
  *
  * TEST INFRASTRUCTURE ONLY, like kxpu_oracle.c.  The slices around the devices are kxpu_dra_slices' (the name, pool and
- * argument rules, the Buf writer), so this file builds on kxpu_dra_oracle.c's helpers; the library it becomes also
- * exports kxo_dra_slices.  kxo_dra_slices_mdev takes kxpu_dra_slices_mdev's arguments without the context and returns
- * the same status codes; on KXPU_E_UNSUPPORTED *why names the first rule (the order of the header's domain list) that
- * the first record outside the domain breaks.
+ * argument rules, the Buf writer), so this file includes kxpu_dra_oracle.c and builds on its helpers; it is compiled
+ * as part of kxpu_aer_oracle.c's translation unit.  kxo_dra_slices_mdev takes kxpu_dra_slices_mdev's arguments without
+ * the context and returns the same status codes; on KXPU_E_UNSUPPORTED *why names the first rule (the order of the
+ * header's domain list) that the first record outside the domain breaks.
  */
 #include "kxpu_dra_oracle.c"
 

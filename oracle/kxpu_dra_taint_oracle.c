@@ -4,8 +4,8 @@
  * from the rules stated in the header.  timeAdded comes from gmtime_r, so this checker shares no date arithmetic with
  * the GPU kernel.
  *
- * TEST INFRASTRUCTURE ONLY, like kxpu_oracle.c.  It builds on the passthrough and vGPU DRA oracles' helpers (names,
- * record domains, the Buf writer); the library it becomes also exports kxo_dra_slices and kxo_dra_slices_mdev.  The
+ * TEST INFRASTRUCTURE ONLY, like kxpu_oracle.c.  It includes the passthrough and vGPU DRA oracles and builds on their
+ * helpers (names, record domains, the Buf writer); it is compiled as part of kxpu_aer_oracle.c's translation unit.  The
  * devices are written here again rather than taken from those oracles, so that taint_since == NULL giving their bytes
  * is a check and not an identity.  Arguments and status codes are the product calls' without the context; on
  * KXPU_E_UNSUPPORTED *why names the first rule the first record outside the domain breaks (the record rules of the

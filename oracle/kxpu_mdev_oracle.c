@@ -15,9 +15,7 @@
 #include <string.h>
 
 #include "../include/kxpu.h"
-
-int kxo_is_base60(const uint8_t *s, size_t len); /* kxpu_oracle.c */
-int kxo_kind_ok(const char *kind);                /* kxpu_xpu_oracle.c */
+#include "kxpu_oracle.h"
 
 /* readIDFromFileFunc :183-191; -1 for a file under 2 or over 8 bytes */
 static int read_id(const uint8_t *txt, unsigned flen, uint8_t id[8]) {

@@ -28,6 +28,7 @@
 #include <time.h>
 
 #include "../include/kxpu.h"
+#include "kxpu_oracle.h"
 
 #define KXO_MAX_TOKEN 65536 /* bufio.MaxScanTokenSize = 64*1024 */
 

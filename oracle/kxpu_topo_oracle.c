@@ -13,11 +13,7 @@
 #include <string.h>
 
 #include "../include/kxpu.h"
-
-int32_t kxo_classify_rules(const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs, size_t n,
-                           kxpu_classify_out *out, uint8_t *dev_rule);                 /* kxpu_xpu_oracle.c  */
-int32_t kxo_mdev_classify(const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_mdevrec *recs, size_t n,
-                          kxpu_classify_out *out, uint8_t *dev_rule);                  /* kxpu_mdev_oracle.c */
+#include "kxpu_oracle.h"
 
 /* mask of group g = OR of 1 << numa_node over its members (the accepted records) that carry a valid node */
 static void group_masks(const kxpu_classify_out *out, const uint8_t *flags, const uint8_t *node, size_t stride,

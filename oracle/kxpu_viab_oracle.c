@@ -10,11 +10,7 @@
 #include <string.h>
 
 #include "../include/kxpu.h"
-
-int32_t kxo_classify_rules(const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs, size_t n,
-                           kxpu_classify_out *out, uint8_t *dev_rule);                         /* kxpu_xpu_oracle.c  */
-int32_t kxo_classify_topo(const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs, size_t n,
-                          kxpu_classify_out *out, uint8_t *dev_rule, uint64_t *group_numa);    /* kxpu_topo_oracle.c */
+#include "kxpu_oracle.h"
 
 /* readIDFromFile: data[2:] with '\n' trimmed at both ends; -1 when the file is shorter than 2 or longer than 8 bytes */
 static int read_id(const uint8_t *txt, unsigned flen, uint8_t id[8]) {

@@ -8,8 +8,7 @@
  * TEST INFRASTRUCTURE ONLY, like kxpu_oracle.c: loaded by tests/ through oracle/xpu_oracle.py, never by the
  * product.  It is a separate restatement of the walk; kxpu_oracle.c stays the pinned NVIDIA-only one, and the
  * CPU tests check that this file with the NVIDIA rule / kind gives its bytes.  The yaml.v3 base-60 predicate
- * is taken from there (kxo_is_base60, linked against libkxpu_oracle.so), so both documents quote the same
- * bdf strings.
+ * is taken from there (kxo_is_base60, declared in kxpu_oracle.h), so both documents quote the same bdf strings.
  */
 #define _GNU_SOURCE
 #include <stdint.h>
@@ -18,8 +17,7 @@
 #include <string.h>
 
 #include "../include/kxpu.h"
-
-int kxo_is_base60(const uint8_t *s, size_t len); /* kxpu_oracle.c */
+#include "kxpu_oracle.h"
 
 /* readIDFromFileFunc :183-191: data[2:] with all leading/trailing '\n' trimmed.
  * Returns length (<= 8) or -1 for "would panic" (file < 2 bytes) / unsupported. */

@@ -44,47 +44,81 @@ def build():
 
 
 def lib():
+    """libkxpu_oracle.so, every oracle file in one library; make rebuilds it first if a source is newer."""
     global _LIB
     if _LIB is None:
-        path = os.path.join(_HERE, "libkxpu_oracle.so")
-        if not os.path.exists(path):
-            build()
-        L = C.CDLL(path)
-        L.kxo_scan_lookup.restype = C.c_int64
-        L.kxo_scan_lookup.argtypes = [C.c_void_p, C.c_size_t, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t,
-                                      C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]
-        L.kxo_sanitise.restype = C.c_size_t
-        L.kxo_sanitise.argtypes = [C.c_char_p, C.c_size_t, C.c_void_p]
-        L.kxo_device_name.restype = C.c_int64
-        L.kxo_device_name.argtypes = [C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_size_t,
-                                      C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]
-        L.kxo_table_build.restype = C.c_size_t
-        L.kxo_table_build.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
-        L.kxo_line_rest.restype = C.c_size_t
-        L.kxo_line_rest.argtypes = [C.c_void_p, C.c_size_t, C.c_uint64, C.POINTER(C.c_size_t)]
-        L.kxo_names_bulk.restype = C.c_size_t
-        L.kxo_names_bulk.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
-        L.kxo_classify.restype = C.c_int32
-        L.kxo_classify.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(ClassifyOut)]
-        L.kxo_is_base60.restype = C.c_int
-        L.kxo_is_base60.argtypes = [C.c_char_p, C.c_size_t]
-        L.kxo_cdi_emit.restype = C.c_size_t
-        L.kxo_cdi_emit.argtypes = [C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
-        L.kxo_alloc_names.restype = C.c_size_t
-        L.kxo_alloc_names.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]
-        L.kxo_lw_encode.restype = C.c_size_t
-        L.kxo_lw_encode.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
-        L.kxo_bench_scan.restype = C.c_double
-        L.kxo_bench_scan.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p,
-                                     C.POINTER(C.c_uint64)]
-        L.kxo_bench_parse_once.restype = C.c_double
-        L.kxo_bench_parse_once.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
-                                           C.POINTER(C.c_double)]
-        L.kxo_table_build_mt.restype = C.c_size_t
-        L.kxo_table_build_mt.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t]
-        L.kxo_bench_parse_mt.restype = C.c_double
-        L.kxo_bench_parse_mt.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p,
-                                         C.POINTER(C.c_double)]
+        build()
+        L = C.CDLL(os.path.join(_HERE, "libkxpu_oracle.so"))
+        vp, sz, s = C.c_void_p, C.c_size_t, C.c_char_p
+        sig = {
+            # kxpu_oracle.c
+            "kxo_scan_lookup": (C.c_int64, [C.c_void_p, C.c_size_t, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t,
+                                            C.POINTER(C.c_size_t), C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
+            "kxo_sanitise": (C.c_size_t, [C.c_char_p, C.c_size_t, C.c_void_p]),
+            "kxo_device_name": (C.c_int64, [C.c_void_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_size_t,
+                                            C.POINTER(C.c_int64), C.POINTER(C.c_uint64)]),
+            "kxo_table_build": (C.c_size_t, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
+            "kxo_line_rest": (C.c_size_t, [C.c_void_p, C.c_size_t, C.c_uint64, C.POINTER(C.c_size_t)]),
+            "kxo_names_bulk": (C.c_size_t, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
+                                            C.c_void_p]),
+            "kxo_classify": (C.c_int32, [C.c_void_p, C.c_size_t, C.POINTER(ClassifyOut)]),
+            "kxo_is_base60": (C.c_int, [C.c_char_p, C.c_size_t]),
+            "kxo_cdi_emit": (C.c_size_t, [C.c_int32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
+            "kxo_alloc_names": (C.c_size_t, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
+            "kxo_lw_encode": (C.c_size_t, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
+            "kxo_bench_scan": (C.c_double, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p,
+                                            C.POINTER(C.c_uint64)]),
+            "kxo_bench_parse_once": (C.c_double, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                  C.POINTER(C.c_double)]),
+            "kxo_table_build_mt": (C.c_size_t, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t]),
+            "kxo_bench_parse_mt": (C.c_double, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p,
+                                                C.POINTER(C.c_double)]),
+            "kxo_full_build": (C.c_size_t, [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t]),
+            # kxpu_xpu_oracle.c
+            "kxo_classify_rules": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(ClassifyOut),
+                                               C.c_void_p]),
+            "kxo_kind_ok": (C.c_int, [C.c_char_p]),
+            "kxo_cdi_emit_kind": (C.c_size_t, [C.c_int32, C.c_char_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
+            "kxo_alloc_names_kind": (C.c_size_t, [C.c_char_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
+                                                  C.c_void_p]),
+            # kxpu_mdev_oracle.c
+            "kxo_mdev_classify": (C.c_int32, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(ClassifyOut),
+                                              C.c_void_p]),
+            "kxo_type_key": (C.c_size_t, [C.c_char_p, C.c_size_t, C.c_void_p]),
+            "kxo_uuid_ok": (C.c_int, [C.c_char_p]),
+            "kxo_mdev_names": (C.c_size_t, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+            "kxo_cdi_emit_mdev": (C.c_size_t, [C.c_int32, C.c_char_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]),
+            # kxpu_topo_oracle.c
+            "kxo_classify_topo": (C.c_int32, [vp, sz, vp, sz, C.POINTER(ClassifyOut), vp, vp]),
+            "kxo_classify_mdev_topo": (C.c_int32, [vp, sz, vp, sz, C.POINTER(ClassifyOut), vp, vp]),
+            "kxo_lw_encode_topo": (sz, [vp, vp, vp, sz, vp, sz]),
+            "kxo_preferred_allocation": (C.c_int32, [vp, sz, vp, vp, vp, vp, vp, sz, vp, vp]),
+            # kxpu_viab_oracle.c
+            "kxo_classify_viable": (C.c_int32, [vp, sz, vp, sz, C.POINTER(ClassifyOut), vp, vp, vp]),
+            # kxpu_reconcile_oracle.c
+            "kxo_reconcile": (C.c_int32, [vp, sz, C.c_uint64, vp, sz, vp, vp, vp, vp]),
+            # kxpu_pcie_oracle.c
+            "kxo_pcie_parse": (C.c_int32, [vp, vp, vp]),
+            "kxo_pcie_tree": (C.c_int32, [vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp]),
+            "kxo_preferred_allocation_pcie": (C.c_int32, [vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp, sz, vp, vp]),
+            # kxpu_aer_oracle.c and the DRA oracles it includes
+            "kxo_dra_slices": (C.c_int32, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, vp, sz, vp, sz,
+                                           C.POINTER(sz), vp, C.POINTER(sz), C.POINTER(C.c_int32)]),
+            "kxo_dra_slices_mdev": (C.c_int32, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint64, vp, sz, vp, sz,
+                                                C.POINTER(sz), vp, C.POINTER(sz), C.POINTER(C.c_int32)]),
+            "kxo_dra_slices_taint": (C.c_int32, [s, s, s, C.c_uint64, vp, sz, s, s, s, vp, vp, sz, C.POINTER(sz), vp,
+                                                 C.POINTER(sz), C.POINTER(C.c_int32)]),
+            "kxo_dra_slices_mdev_taint": (C.c_int32, [s, s, s, C.c_uint64, vp, sz, s, s, s, vp, vp, sz, C.POINTER(sz),
+                                                      vp, C.POINTER(sz), C.POINTER(C.c_int32)]),
+            "kxo_aer_health": (C.c_int32, [vp, sz, vp, vp, sz, C.c_uint64, C.c_uint64, vp, vp, sz, vp, vp]),
+            "kxo_dra_slices_taints": (C.c_int32, [s, s, s, C.c_uint64, vp, sz, vp, sz, vp, vp, sz, C.POINTER(sz), vp,
+                                                  C.POINTER(sz), C.POINTER(C.c_int32)]),
+            "kxo_dra_slices_mdev_taints": (C.c_int32, [s, s, s, C.c_uint64, vp, sz, vp, sz, vp, vp, sz, C.POINTER(sz),
+                                                       vp, C.POINTER(sz), C.POINTER(C.c_int32)]),
+        }
+        for name, (res, args) in sig.items():
+            f = getattr(L, name)
+            f.restype, f.argtypes = res, args
         _LIB = L
     return _LIB
 
@@ -167,7 +201,12 @@ def names_bulk(text, line_offs):
     return blob[:need].tobytes(), offs
 
 
-def classify(recs: np.ndarray):
+def classify_call(fn, head, recs, dev=(), group=()):
+    """fn(*head, recs, n, &out, *dev outputs, *group outputs), the shape of every kxo_*classify* call: allocates the
+    seven CSR arrays of kxpu_classify_out and the extra outputs, runs the call and returns (status, result).
+    dev / group: (name, dtype) of the extra outputs with one entry per device id / per group, dtype None for a NULL
+    argument.  result is classify's dict plus the extra outputs trimmed to the counts the call wrote, or None when the
+    status is not 0."""
     n = len(recs)
     recs = np.ascontiguousarray(recs)
     arrs = dict(accept_index=np.empty(n, np.uint32), group_ids=np.empty(n, np.uint32),
@@ -175,13 +214,24 @@ def classify(recs: np.ndarray):
                 dev_ids=np.empty(n, np.uint64), dev_off=np.empty(n + 1, np.uint32),
                 dev_groups=np.empty(n, np.uint32))
     out = ClassifyOut(**{k: v.ctypes.data for k, v in arrs.items()})
-    rc = lib().kxo_classify(recs.ctypes.data, n, C.byref(out))
-    assert rc == 0
+    extra = [(name, None if dt is None else np.empty(max(n, 1), dt), per)
+             for per, outs in (("dev", dev), ("group", group)) for name, dt in outs]
+    rc = fn(*head, recs.ctypes.data, n, C.byref(out), *[None if e is None else e.ctypes.data for _, e, _ in extra])
+    if rc != 0:
+        return rc, None
     g, d, a = out.n_groups, out.n_devids, out.n_accepted
-    return dict(accept_index=arrs["accept_index"], n_accepted=a, n_groups=g, n_devids=d,
-                group_ids=arrs["group_ids"][:g], group_off=arrs["group_off"][:g + 1],
-                group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
-                dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g])
+    res = dict(accept_index=arrs["accept_index"], n_accepted=a, n_groups=g, n_devids=d,
+               group_ids=arrs["group_ids"][:g], group_off=arrs["group_off"][:g + 1],
+               group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
+               dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g])
+    res.update((name, arr[:d if per == "dev" else g]) for name, arr, per in extra if arr is not None)
+    return rc, res
+
+
+def classify(recs: np.ndarray):
+    rc, res = classify_call(lib().kxo_classify, (), recs)
+    assert rc == 0
+    return res
 
 
 def cdi_emit(fmt: int, devs: np.ndarray) -> bytes:
@@ -265,8 +315,6 @@ ROW64_DTYPE = np.dtype([("key", "<u8"), ("line_off", "<u8")])
 def full_build(text, kind):
     """SURVEY 8(f) row 4: vendor (0) / subsystem (1) / class-section (2) rows (key, line_off) in file order."""
     L = lib()
-    L.kxo_full_build.restype = C.c_size_t
-    L.kxo_full_build.argtypes = [C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.c_size_t]
     p, n, keep = _buf(text)
     cap = 1 << 15
     rows = np.zeros(cap, dtype=ROW64_DTYPE)

@@ -4,40 +4,13 @@ kxpu_preferred_allocation_pcie, and of the path grammar of one record.
 TEST INFRASTRUCTURE ONLY, like oracle.py: imported by tests/, never by the product package.
 """
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_SRC = os.path.join(_HERE, "kxpu_pcie_oracle.c")
-_SO = os.path.join(_HERE, "libkxpu_pcie_oracle.so")
-_LIB = None
+from . import oracle as O
+
 NO_NODE = 0xFFFFFFFF
 MAX_DEPTH = 8
-
-
-def build():
-    deps = [_SRC, os.path.join(_HERE, "..", "include", "kxpu.h")]
-    if os.path.exists(_SO) and os.path.getmtime(_SO) >= max(os.path.getmtime(d) for d in deps):
-        return
-    subprocess.check_call([os.environ.get("CC", "gcc"), "-O2", "-Wall", "-Wextra", "-fPIC", "-shared", "-o", _SO, _SRC])
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        build()
-        L = C.CDLL(_SO)
-        vp, sz = C.c_void_p, C.c_size_t
-        L.kxo_pcie_parse.restype = C.c_int32
-        L.kxo_pcie_parse.argtypes = [vp, vp, vp]
-        L.kxo_pcie_tree.restype = C.c_int32
-        L.kxo_pcie_tree.argtypes = [vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp]
-        L.kxo_preferred_allocation_pcie.restype = C.c_int32
-        L.kxo_preferred_allocation_pcie.argtypes = [vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, vp, sz, vp, vp]
-        _LIB = L
-    return _LIB
 
 
 def _p(a):
@@ -49,7 +22,7 @@ def parse(rec, path):
     rec = np.ascontiguousarray(np.asarray(rec).reshape(1))
     path = np.ascontiguousarray(np.asarray(path).reshape(1))
     chain = np.zeros(MAX_DEPTH, np.uint64)
-    n = lib().kxo_pcie_parse(rec.ctypes.data, path.ctypes.data, chain.ctypes.data)
+    n = O.lib().kxo_pcie_parse(rec.ctypes.data, path.ctypes.data, chain.ctypes.data)
     return [int(k) for k in chain[:n]]
 
 
@@ -63,8 +36,8 @@ def tree(recs, paths, group_off, group_members):
     gnode = np.zeros(max(G, 1), np.uint32)
     key, parent, depth = np.zeros(cap, np.uint64), np.zeros(cap, np.uint32), np.zeros(cap, np.uint8)
     nn = C.c_uint32(0)
-    rc = lib().kxo_pcie_tree(_p(recs), _p(paths), len(recs), group_off.ctypes.data, _p(group_members), G,
-                             gnode.ctypes.data, key.ctypes.data, parent.ctypes.data, depth.ctypes.data, C.byref(nn))
+    rc = O.lib().kxo_pcie_tree(_p(recs), _p(paths), len(recs), group_off.ctypes.data, _p(group_members), G,
+                               gnode.ctypes.data, key.ctypes.data, parent.ctypes.data, depth.ctypes.data, C.byref(nn))
     if rc != 0:
         return None
     n = nn.value
@@ -82,10 +55,10 @@ def preferred_allocation_pcie(dev_numa, dev_node, parent, depth, requests):
     depth = np.ascontiguousarray(depth, dtype=np.uint8)
     out = np.zeros(max(int(a["size"].sum()), 1), np.uint32)
     out_off = np.zeros(len(requests) + 1, np.uint32)
-    rc = lib().kxo_preferred_allocation_pcie(_p(dev_numa), _p(dn), len(dev_numa), _p(parent), _p(depth), len(parent),
-                                             a["avail_off"].ctypes.data, a["avail"].ctypes.data,
-                                             a["must_off"].ctypes.data, a["must"].ctypes.data, a["size"].ctypes.data,
-                                             len(requests), out.ctypes.data, out_off.ctypes.data)
+    rc = O.lib().kxo_preferred_allocation_pcie(_p(dev_numa), _p(dn), len(dev_numa), _p(parent), _p(depth), len(parent),
+                                               a["avail_off"].ctypes.data, a["avail"].ctypes.data,
+                                               a["must_off"].ctypes.data, a["must"].ctypes.data, a["size"].ctypes.data,
+                                               len(requests), out.ctypes.data, out_off.ctypes.data)
     if rc != 0:
         return None
     return [out[out_off[q]:out_off[q + 1]].tolist() for q in range(len(requests))]
