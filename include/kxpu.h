@@ -877,8 +877,9 @@ int32_t kxpu_dra_slices_mdev(kxpu_ctx *ctx, const char *driver, const char *pool
  * not empty and not such a name of at most 63 bytes; taint_effect not exactly "NoSchedule" or "NoExecute".
  * KXPU_E_UNSUPPORTED, nothing written: the cases of kxpu_dra_slices, or a taint_since[i] above
  * KXPU_DRA_TAINT_SINCE_MAX.
- * GPU: the kernel of kxpu_dra_slices with the taint compiled in: one CTA per 64-device slice; the thread of a device
- * range-checks its taint_since and formats timeAdded into shared memory.  Timed under KXPU_T_EMIT. */
+ * GPU: kxpu_dra_slices_taints with this taint as a one-entry table: the kernel of kxpu_dra_slices with a taint list
+ * of one entry compiled in, one CTA per 64-device slice; the thread of a device range-checks its taint_since and
+ * formats timeAdded into shared memory.  Timed under KXPU_T_EMIT. */
 int32_t kxpu_dra_slices_taint(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
                               const kxpu_dradev *devs, size_t n, const char *taint_key, const char *taint_value,
                               const char *taint_effect, const int64_t *taint_since /* [n] or NULL */, uint8_t *out,
@@ -950,8 +951,8 @@ typedef struct kxpu_dra_taint {
  * or above KXPU_DRA_MAX_TAINTS, or an entry whose key, value or effect fails kxpu_dra_slices_taint's checks.
  * KXPU_E_UNSUPPORTED, nothing written: the cases of kxpu_dra_slices, a taint_since above KXPU_DRA_TAINT_SINCE_MAX, or a
  * device that carries two entries with the same key and effect.
- * GPU: n_taints == 1 runs kxpu_dra_slices_taint's kernel; two or more entries run the kernel of kxpu_dra_slices with
- * the taint list compiled in.  Timed under KXPU_T_EMIT. */
+ * GPU: the kernel of kxpu_dra_slices with the taint list compiled in, its shared memory sized for the table's capacity:
+ * one entry for n_taints == 1, KXPU_DRA_MAX_TAINTS for more.  Timed under KXPU_T_EMIT. */
 int32_t kxpu_dra_slices_taints(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
                                const kxpu_dradev *devs, size_t n, const kxpu_dra_taint *taints, size_t n_taints,
                                const int64_t *taint_since /* [n * n_taints], device-major, or NULL */, uint8_t *out,

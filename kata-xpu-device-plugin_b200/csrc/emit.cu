@@ -362,44 +362,33 @@ constexpr int MAX_FRAG_DRA_MDEV = (int)sizeof(KX_M0 KX_M1 KX_M2 KX_M3 KX_M4 KX_M
                                   16 + 6 + 6 + 64 + 36 + 1;
 constexpr int DRAM_PARTS = DRAM_LITS + 2;
 
-// Taints (kxpu_dra_slices_taint / kxpu_dra_slices_mdev_taint).  A tainted device's fragment ends with its last literal
-// less that literal's final '}' (the one that closes the device), then the taint head, the 20-byte timeAdded and the
-// taint tail, which closes the taint, the list and the device.  The taint head holds the call's key, value and effect,
-// so it is assembled on the host like the slice head.  Slices hold TAINT_TILE devices whether or not one is tainted.
-#define KX_TAINT_TAIL "\"}]}"
-constexpr int TAINT_TILE = 64;
-constexpr long long TAINT_SINCE_MAX = 253402300799ll;  // 9999-12-31T23:59:59Z
-// ,"taints":[{"key":"<key>","value":"<value>","effect":"<effect>","timeAdded":"  with a 127-byte key, a 63-byte value
-// and "NoSchedule"
-constexpr int TAINT_HEAD_MAX =
-    (int)sizeof(",\"taints\":[{\"key\":\"\",\"value\":\"\",\"effect\":\"\",\"timeAdded\":\"") - 1 + 127 + 63 + 10;
-constexpr int TAINT_PART_MAX = TAINT_HEAD_MAX + 20 + (int)sizeof(KX_TAINT_TAIL) - 1 - 1;  // less the '}' it replaces
-// the untainted pool bound (its longest content is about 1.4 KB: the 1.1 KB head and the vGPU literals) plus the
-// longest taint head and tail
-constexpr int DRA_TAINT_POOL_MAX = DRA_POOL_MAX + 272;
-static_assert(TAINT_HEAD_MAX + (int)sizeof(KX_TAINT_TAIL) - 1 <= DRA_TAINT_POOL_MAX - DRA_POOL_MAX, "taint pool bound");
-
-// Taint lists (kxpu_dra_slices_taints / kxpu_dra_slices_mdev_taints).  A device that carries some taint ends with its
-// last literal less its final '}', then KX_TAINTS_OPEN, for each carried taint in table order its entry head (the
-// table's key, value and effect, assembled on the host), the 20-byte timeAdded and KX_TAINT_ECLOSE, with ',' between
-// entries, then KX_TAINTS_CLOSE.  One entry gives the _taint calls' bytes.
+// Taints (kxpu_dra_slices[_mdev]_taint[s]).  A device that carries some taint ends with its last literal less that
+// literal's final '}' (the one that closes the device), then KX_TAINTS_OPEN, for each carried taint in table order its
+// entry head (the table's key, value and effect, assembled on the host like the slice head), the 20-byte timeAdded and
+// KX_TAINT_ECLOSE, with ',' between entries, then KX_TAINTS_CLOSE.  Slices hold TAINT_TILE devices whether or not one
+// is tainted.
 #define KX_TAINTS_OPEN ",\"taints\":["
 #define KX_TAINT_ECLOSE "\"}"
 #define KX_TAINTS_CLOSE "]}"
+constexpr int TAINT_TILE = 64;
+constexpr long long TAINT_SINCE_MAX = 253402300799ll;  // 9999-12-31T23:59:59Z
 constexpr int TAINT_ENTRY_MAX =  // {"key":"<key>","value":"<value>","effect":"<effect>","timeAdded":"  at the longest
     (int)sizeof("{\"key\":\"\",\"value\":\"\",\"effect\":\"\",\"timeAdded\":\"") - 1 + 127 + 63 + 10;
-constexpr int TAINTS_PART_MAX = (int)sizeof(KX_TAINTS_OPEN) - 1 +
-                                KXPU_DRA_MAX_TAINTS * (TAINT_ENTRY_MAX + 20 + (int)sizeof(KX_TAINT_ECLOSE) - 1 + 1) - 1 +
-                                (int)sizeof(KX_TAINTS_CLOSE) - 1 - 1;  // less one ',' and the '}' it replaces
-constexpr int DRA_TAINTS_POOL_MAX = DRA_POOL_MAX + 1024;
-static_assert((int)sizeof(KX_TAINTS_OPEN KX_TAINT_ECLOSE KX_TAINTS_CLOSE) - 1 + KXPU_DRA_MAX_TAINTS * TAINT_ENTRY_MAX <=
-                  DRA_TAINTS_POOL_MAX - DRA_POOL_MAX,
-              "taint list pool bound");
-// k_dra_slices' taint mode: no taint, one taint for the call (the _taint calls), a table of taints (the _taints calls)
-constexpr int DRA_UNTAINTED = 0, DRA_TAINT_ONE = 1, DRA_TAINT_LIST = 2;
+// what nt carried taints add to a fragment at most
+constexpr int taints_part_max(int nt) {
+    return (int)sizeof(KX_TAINTS_OPEN) - 1 + nt * (TAINT_ENTRY_MAX + 20 + (int)sizeof(KX_TAINT_ECLOSE) - 1 + 1) - 1 +
+           (int)sizeof(KX_TAINTS_CLOSE) - 1 - 1;  // less one ',' and the '}' it replaces
+}
+// the pool of a table of up to nt entries: the untainted bound (its longest content is about 1.4 KB: the 1.1 KB head
+// and the vGPU literals) plus room for KX_TAINTS_OPEN, nt entry heads, KX_TAINT_ECLOSE and KX_TAINTS_CLOSE: 272 bytes
+// for the 261 of one entry, 1 KB for the 999 of four
+constexpr int dra_pool_max(int nt) { return DRA_POOL_MAX + (nt == 0 ? 0 : nt == 1 ? 272 : 1024); }
+constexpr int taints_pool_need(int nt) {
+    return (int)sizeof(KX_TAINTS_OPEN KX_TAINT_ECLOSE KX_TAINTS_CLOSE) - 1 + nt * TAINT_ENTRY_MAX;
+}
 
 // PARTS = literals + head + tail; the head is part PARTS - 2, the tail PARTS - 1
-template <int PARTS, int POOL = DRA_POOL_MAX>
+template <int PARTS, int POOL>
 struct DraParams {
     const void *devs;               // kxpu_dradev[n] or kxpu_dramdev[n]
     uint32_t n;
@@ -412,18 +401,13 @@ struct DraParams {
     uint32_t *flags;                // one word per KXPU_E_UNSUPPORTED reason, DRA_F_* / DRAM_F_*
     uint8_t pool[POOL];
 };
-// the taint instantiations: the literals, the taint head (part PARTS - 4) and tail (PARTS - 3), the slice head and tail
-template <int PARTS>
-struct DraTaintParams : DraParams<PARTS, DRA_TAINT_POOL_MAX> {
-    const long long *since;  // [n]: the taint's unix time, < 0 = untainted
-};
-// the taint list instantiations: the literals, KX_TAINTS_OPEN (part PARTS - 9), the entry heads (PARTS - 8 ..
-// PARTS - 5), KX_TAINT_ECLOSE, KX_TAINTS_CLOSE, the slice head and tail
-template <int PARTS>
-struct DraTaintsParams : DraParams<PARTS, DRA_TAINTS_POOL_MAX> {
-    const long long *since;            // [n * nt], device-major: taint t of device i, < 0 = not carried
-    uint32_t nt;                       // table entries, 1..KXPU_DRA_MAX_TAINTS
-    uint8_t dup[KXPU_DRA_MAX_TAINTS];  // dup[t]: the earlier entries with taint t's key and effect
+// the tainted instantiations, for tables of up to NT entries: the literals, KX_TAINTS_OPEN (part PARTS - NT - 5), the
+// entry heads (PARTS - NT - 4 .. PARTS - 5), KX_TAINT_ECLOSE, KX_TAINTS_CLOSE, the slice head and tail
+template <int PARTS, int NT>
+struct DraTaintsParams : DraParams<PARTS, dra_pool_max(NT)> {
+    const long long *since;  // [n * nt], device-major: taint t of device i, < 0 = not carried
+    uint32_t nt;             // table entries, 1..NT
+    uint8_t dup[NT];         // dup[t]: the earlier entries with taint t's key and effect
 };
 constexpr int DRA_F_PRODUCT = 0, DRA_F_BDF = 1, DRA_F_ROOT = 2, DRA_F_VENDOR = 3, DRA_F_DEVICE = 4, DRA_F_GROUP = 5,
               DRA_F_PLEN = 6, DRA_F_COUNT = 7;
@@ -432,7 +416,7 @@ constexpr int DRAM_F_PRODUCT = 0, DRAM_F_TYPE = 1, DRAM_F_UUID = 2, DRAM_F_PAREN
               DRAM_F_DEVICE = 6, DRAM_F_GROUP = 7, DRAM_F_PLEN = 8, DRAM_F_COUNT = 9;
 
 // T devices per slice, FRAG bytes per fragment, a POOL-byte pool
-template <int T = TILE, int FRAG = MAX_FRAG_DRA, int POOL = DRA_POOL_MAX>
+template <int T, int FRAG, int POOL>
 struct DraSmem {
     alignas(16) uint8_t stage[T * FRAG + POOL + 16];
     uint8_t pool[POOL];
@@ -443,7 +427,7 @@ struct DraSmem {
     uint32_t wsum[EMIT_THREADS / 32];
     uint32_t tile_total;
 };
-template <int T = TILE, int FRAG = MAX_FRAG_DRA_MDEV, int POOL = DRA_POOL_MAX>
+template <int T, int FRAG, int POOL>
 struct DraMdevSmem {
     alignas(16) uint8_t stage[T * FRAG + POOL + 16];
     uint8_t pool[POOL];
@@ -455,46 +439,39 @@ struct DraMdevSmem {
     uint32_t wsum[EMIT_THREADS / 32];
     uint32_t tile_total;
 };
-template <typename Base>
-struct DraTaintSmem : Base {
-    uint8_t ts[TAINT_TILE][20];  // timeAdded of device d; ts[d][0] == 0: untainted
-};
-template <typename Base>
+template <typename Base, int NT>
 struct DraTaintsSmem : Base {
-    uint8_t ts[TAINT_TILE][KXPU_DRA_MAX_TAINTS][20];  // timeAdded of taint t of device d
-    uint8_t carried[TAINT_TILE];                      // bit t: device d carries taint t
+    uint8_t ts[TAINT_TILE][NT][20];  // timeAdded of taint t of device d
+    uint8_t carried[TAINT_TILE];     // bit t: device d carries taint t
 };
 template <int LAYOUT> struct DraLayout {  // LAYOUT_PCI
     using Rec = kxpu_dradev;
-    using Smem = DraSmem<>;
-    using TaintSmem = DraTaintSmem<DraSmem<TAINT_TILE, MAX_FRAG_DRA + TAINT_PART_MAX, DRA_TAINT_POOL_MAX>>;
-    using TaintsSmem = DraTaintsSmem<DraSmem<TAINT_TILE, MAX_FRAG_DRA + TAINTS_PART_MAX, DRA_TAINTS_POOL_MAX>>;
-    static constexpr int PARTS = DRA_PARTS, LAST = 8, F_COUNT = DRA_F_COUNT;
+    template <int T, int FRAG, int POOL> using Smem = DraSmem<T, FRAG, POOL>;
+    static constexpr int PARTS = DRA_PARTS, LAST = 8, F_COUNT = DRA_F_COUNT, MAX_FRAG = MAX_FRAG_DRA;
 };
 template <> struct DraLayout<LAYOUT_MDEV> {
     using Rec = kxpu_dramdev;
-    using Smem = DraMdevSmem<>;
-    using TaintSmem = DraTaintSmem<DraMdevSmem<TAINT_TILE, MAX_FRAG_DRA_MDEV + TAINT_PART_MAX, DRA_TAINT_POOL_MAX>>;
-    using TaintsSmem = DraTaintsSmem<DraMdevSmem<TAINT_TILE, MAX_FRAG_DRA_MDEV + TAINTS_PART_MAX, DRA_TAINTS_POOL_MAX>>;
-    static constexpr int PARTS = DRAM_PARTS, LAST = DRAM_E, F_COUNT = DRAM_F_COUNT;
+    template <int T, int FRAG, int POOL> using Smem = DraMdevSmem<T, FRAG, POOL>;
+    static constexpr int PARTS = DRAM_PARTS, LAST = DRAM_E, F_COUNT = DRAM_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_MDEV;
 };
-// one k_dra_slices instantiation: LAST is the literal that closes a device; a taint time above the maximum reports
-// F_SINCE, a device with two taints of one key and effect F_DUP
-template <int LAYOUT, int MODE> struct DraKernel {
-    static constexpr bool TAINT = MODE != DRA_UNTAINTED, LIST = MODE == DRA_TAINT_LIST;
+// one k_dra_slices instantiation for tables of up to NT taints (NT = 0: untainted): LAST is the literal that closes a
+// device; a taint time above the maximum reports F_SINCE, a device with two taints of one key and effect F_DUP
+template <int LAYOUT, int NT> struct DraKernel {
+    using L = DraLayout<LAYOUT>;
+    static constexpr bool TAINT = NT > 0;
     static constexpr int T = TAINT ? TAINT_TILE : TILE;
-    static constexpr int PARTS = DraLayout<LAYOUT>::PARTS + (LIST ? 7 : TAINT ? 2 : 0);
-    static constexpr int TAINT_HEAD = PARTS - 4, TAINT_TAIL = PARTS - 3, F_SINCE = DraLayout<LAYOUT>::F_COUNT;
-    static constexpr int T_OPEN = PARTS - 9, T_ENTRY = PARTS - 8, T_ECLOSE = PARTS - 4, T_CLOSE = PARTS - 3;
-    static constexpr int F_DUP = F_SINCE + 1, F_COUNT = DraLayout<LAYOUT>::F_COUNT + (LIST ? 2 : TAINT ? 1 : 0);
-    static constexpr int POOL = LIST ? DRA_TAINTS_POOL_MAX : TAINT ? DRA_TAINT_POOL_MAX : DRA_POOL_MAX;
-    static constexpr int MAXF = (LAYOUT == LAYOUT_PCI ? MAX_FRAG_DRA : MAX_FRAG_DRA_MDEV) +
-                                (LIST ? TAINTS_PART_MAX : TAINT ? TAINT_PART_MAX : 0);
-    using Params = std::conditional_t<LIST, DraTaintsParams<PARTS>,
-                                      std::conditional_t<TAINT, DraTaintParams<PARTS>, DraParams<PARTS>>>;
-    using Smem = std::conditional_t<LIST, typename DraLayout<LAYOUT>::TaintsSmem,
-                                    std::conditional_t<TAINT, typename DraLayout<LAYOUT>::TaintSmem,
-                                                       typename DraLayout<LAYOUT>::Smem>>;
+    static constexpr int PARTS = L::PARTS + (TAINT ? NT + 3 : 0);
+    static constexpr int T_OPEN = L::PARTS - 2, T_ENTRY = T_OPEN + 1, T_ECLOSE = T_ENTRY + NT, T_CLOSE = T_ECLOSE + 1;
+    static constexpr int F_SINCE = L::F_COUNT, F_DUP = F_SINCE + 1, F_COUNT = L::F_COUNT + (TAINT ? 2 : 0);
+    static constexpr int POOL = dra_pool_max(NT);
+    static_assert(!TAINT || taints_pool_need(NT) <= POOL - DRA_POOL_MAX, "taint pool bound");
+    static constexpr int MAXF = L::MAX_FRAG + (TAINT ? taints_part_max(NT) : 0);
+    // CTAs per SM asked of ptxas, 0 for none.  Left to itself ptxas gives NT = 1 96 registers (PCI) or 101 (vGPU), so
+    // two CTAs per SM, where its 47 / 56 KB of shared memory allow four; asked for three it takes 48, without spills
+    static constexpr int MIN_CTAS = NT == 1 ? 3 : 0;
+    using Base = typename L::template Smem<T, MAXF, POOL>;
+    using Params = std::conditional_t<TAINT, DraTaintsParams<PARTS, NT>, DraParams<PARTS, POOL>>;
+    using Smem = std::conditional_t<TAINT, DraTaintsSmem<Base, NT>, Base>;
 };
 
 template <int W>
@@ -540,12 +517,13 @@ __device__ __forceinline__ void rfc3339(unsigned long long t, uint8_t *o) {
     o[19] = (uint8_t)'Z';
 }
 
-// MODE = DRA_UNTAINTED: kxpu_dra_slices[_mdev], TILE devices per slice.  DRA_TAINT_ONE: the _taint calls, TAINT_TILE
-// devices per slice and the taint part after a tainted device's attributes.  DRA_TAINT_LIST: the _taints calls, the same
-// slices with a list of taints.  Everything a mode adds sits behind `if constexpr`.
-template <int LAYOUT, int MODE = DRA_UNTAINTED>
-__global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_constant__ typename DraKernel<LAYOUT, MODE>::Params E) {
-    using K = DraKernel<LAYOUT, MODE>;
+// NT = 0: kxpu_dra_slices[_mdev], TILE devices per slice.  NT > 0: the taint calls with a table of up to NT entries,
+// TAINT_TILE devices per slice and a list of taints after a tainted device's attributes.  Everything the taints add sits
+// behind `if constexpr`.
+template <int LAYOUT, int NT = 0>
+__global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
+    k_dra_slices(const __grid_constant__ typename DraKernel<LAYOUT, NT>::Params E) {
+    using K = DraKernel<LAYOUT, NT>;
     using Rec = typename DraLayout<LAYOUT>::Rec;
     constexpr int HEAD = K::PARTS - 2, TAIL = K::PARTS - 1, T = K::T;
     extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -655,18 +633,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
                    (pl ? E.len[7] + pl + ls : 0u) + (rl ? E.len[8] + rl + ls : 0u) + (tid + 1u < in_slice ? 1u : 0u);
         }
     }
-    if constexpr (MODE == DRA_TAINT_ONE) {  // the taint's time, range-checked and formatted beside the record
-        if (tid < in_slice) {
-            const long long since = E.since[i0 + tid];
-            if (since > TAINT_SINCE_MAX) E.flags[K::F_SINCE] = 1u;
-            S.ts[tid][0] = 0;
-            if (since >= 0 && since <= TAINT_SINCE_MAX) {
-                rfc3339((unsigned long long)since, S.ts[tid]);
-                flen += E.len[K::TAINT_HEAD] + 20u + E.len[K::TAINT_TAIL] - 1u;
-            }
-        }
-    }
-    if constexpr (MODE == DRA_TAINT_LIST) {  // the device's row of the table: which taints it carries, and their times
+    if constexpr (K::TAINT) {  // the device's row of the table: which taints it carries, and their times
         if (tid < in_slice) {
             const long long *row = E.since + (size_t)(i0 + tid) * E.nt;
             uint32_t carried = 0, part = 0;
@@ -726,12 +693,12 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
         auto lit = [&](int k) { put(S.pool + E.off[k], E.len[k]); };
         // the literal that closes the device (K's LAST); a tainted device's taint part goes before its final '}'
         auto close = [&](int k) {
-            if constexpr (MODE == DRA_TAINT_LIST) {
+            if constexpr (K::TAINT) {
                 const uint32_t carried = S.carried[d];
                 if (carried) {
                     put(S.pool + E.off[k], E.len[k] - 1u);
                     lit(K::T_OPEN);
-                    for (uint32_t t = 0; t < (uint32_t)KXPU_DRA_MAX_TAINTS; t++) {
+                    for (uint32_t t = 0; t < (uint32_t)NT; t++) {
                         if (!((carried >> t) & 1u)) continue;
                         if (carried & ((1u << t) - 1u)) {
                             if (lane == 0) dst[o] = (uint8_t)',';
@@ -740,13 +707,6 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_dra_slices(const __grid_consta
                         lit(K::T_ENTRY + t); put(S.ts[d][t], 20u); lit(K::T_ECLOSE);
                     }
                     lit(K::T_CLOSE);
-                    return;
-                }
-            }
-            if constexpr (MODE == DRA_TAINT_ONE) {
-                if (S.ts[d][0]) {
-                    put(S.pool + E.off[k], E.len[k] - 1u);
-                    lit(K::TAINT_HEAD); put(S.ts[d], 20u); lit(K::TAINT_TAIL);
                     return;
                 }
             }
@@ -1255,13 +1215,13 @@ struct DraTaint {
 };
 
 // kxpu_dra_slices[_mdev][_taint[s]]: the argument checks, the pool (literals | taint parts | head | tail), one
-// k_dra_slices<LAYOUT, MODE> launch, the domain flags and the copies
-template <int LAYOUT, int MODE = DRA_UNTAINTED>
+// k_dra_slices<LAYOUT, NT> launch, the domain flags and the copies
+template <int LAYOUT, int NT = 0>
 static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, const char *pool, const char *node,
                           uint64_t generation, const typename DraLayout<LAYOUT>::Rec *devs, size_t n, uint8_t *out, size_t cap,
-                          size_t *len, uint64_t *slice_off, size_t *n_slices, const DraTaint &taint = DraTaint{}) {
+                          size_t *len, uint64_t *slice_off, size_t *n_slices, const DraTaint taint = DraTaint{}) {
     using Rec = typename DraLayout<LAYOUT>::Rec;
-    using K = DraKernel<LAYOUT, MODE>;
+    using K = DraKernel<LAYOUT, NT>;
     constexpr bool TAINT = K::TAINT;
     constexpr int PARTS = K::PARTS, HEAD = PARTS - 2, TAIL = PARTS - 1;
     constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : DRAM_LITS;
@@ -1275,7 +1235,8 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
                         "and generation below 2^63", what);
         return KXPU_E_INVALID;
     }
-    if (TAINT && (!taint.table || taint.n == 0 || taint.n > KXPU_DRA_MAX_TAINTS)) {
+    // callers see the bound of the NT = KXPU_DRA_MAX_TAINTS instantiation, which gets every table but the one-entry one
+    if (TAINT && (!taint.table || taint.n == 0 || taint.n > (size_t)NT)) {
         KX_SET_ERR(ctx, "%s: taints must hold 1..%d entries", what, KXPU_DRA_MAX_TAINTS);
         return KXPU_E_INVALID;
     }
@@ -1299,13 +1260,12 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
                              "\",\"generation\":" + std::to_string(generation) +
                              ",\"resourceSliceCount\":" + std::to_string(slices) + "},\"nodeName\":\"" + nd +
                              "\",\"devices\":[";
-    // the taint parts, from part LITS on: DRA_TAINT_ONE the taint head and tail, DRA_TAINT_LIST KX_TAINTS_OPEN, four
-    // entry heads (empty past the table), KX_TAINT_ECLOSE and KX_TAINTS_CLOSE
+    // the taint parts, from part LITS on: KX_TAINTS_OPEN, NT entry heads (empty past the table), KX_TAINT_ECLOSE and
+    // KX_TAINTS_CLOSE
     std::vector<std::string> taint_parts;
-    if (MODE == DRA_TAINT_ONE) taint_parts = {KX_TAINTS_OPEN + taint_entry(taint.table[0]), KX_TAINT_TAIL};
-    if (MODE == DRA_TAINT_LIST) {
+    if constexpr (TAINT) {
         taint_parts.push_back(KX_TAINTS_OPEN);
-        for (size_t t = 0; t < KXPU_DRA_MAX_TAINTS; t++) taint_parts.push_back(t < taint.n ? taint_entry(taint.table[t]) : "");
+        for (size_t t = 0; t < (size_t)NT; t++) taint_parts.push_back(t < taint.n ? taint_entry(taint.table[t]) : "");
         taint_parts.push_back(KX_TAINT_ECLOSE);
         taint_parts.push_back(KX_TAINTS_CLOSE);
     }
@@ -1326,7 +1286,7 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     const size_t smem = sizeof(typename K::Smem);
     static bool attr_done = false;
     if (!attr_done) {
-        cudaFuncSetAttribute(k_dra_slices<LAYOUT, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaFuncSetAttribute(k_dra_slices<LAYOUT, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         attr_done = true;
     }
     KxScratch sc(ctx);
@@ -1345,8 +1305,6 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
         KX_CUDA(ctx, sc.alloc((void **)&d_since, n * taint.n * sizeof(long long)));
         if (n) cudaMemcpyAsync(d_since, taint.since, n * taint.n * sizeof(long long), cudaMemcpyHostToDevice, ctx->stream);
         E.since = d_since;
-    }
-    if constexpr (K::LIST) {
         E.nt = (uint32_t)taint.n;
         for (size_t t = 0; t < taint.n; t++)
             for (size_t j = 0; j < t; j++)
@@ -1358,7 +1316,7 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     E.epoch = kx_next_epoch(ctx);
     {
         KxTimer tm(ctx, KXPU_T_EMIT);
-        k_dra_slices<LAYOUT, MODE><<<slices, EMIT_THREADS, smem, ctx->stream>>>(E);
+        k_dra_slices<LAYOUT, NT><<<slices, EMIT_THREADS, smem, ctx->stream>>>(E);
         KX_LAUNCHED(ctx);
     }
     std::vector<unsigned long long> h(ctl_words);
@@ -1417,7 +1375,8 @@ extern "C" int32_t kxpu_dra_slices_mdev(kxpu_ctx *ctx, const char *driver, const
 }
 
 // kxpu_dra_slices[_mdev]_taint[s]: taint_since == NULL runs the untainted call with the taint arguments unread, one
-// entry the one-taint kernel, more the list kernel; dra_slices checks the table before either instantiation reads it
+// entry the kernel sized for one taint, any other count the one sized for KXPU_DRA_MAX_TAINTS; dra_slices checks the
+// table before either instantiation reads it
 template <int LAYOUT>
 static int32_t dra_slices_tainted(kxpu_ctx *ctx, const char *what, const char *driver, const char *pool, const char *node,
                                   uint64_t generation, const typename DraLayout<LAYOUT>::Rec *devs, size_t n,
@@ -1428,10 +1387,10 @@ static int32_t dra_slices_tainted(kxpu_ctx *ctx, const char *what, const char *d
                                   devs, n, out, cap, len, slice_off, n_slices);
     const DraTaint taint{taints, n_taints, taint_since};
     if (n_taints == 1)
-        return dra_slices<LAYOUT, DRA_TAINT_ONE>(ctx, what, driver, pool, node, generation, devs, n, out, cap, len, slice_off,
-                                                 n_slices, taint);
-    return dra_slices<LAYOUT, DRA_TAINT_LIST>(ctx, what, driver, pool, node, generation, devs, n, out, cap, len, slice_off,
-                                              n_slices, taint);
+        return dra_slices<LAYOUT, 1>(ctx, what, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices,
+                                     taint);
+    return dra_slices<LAYOUT, KXPU_DRA_MAX_TAINTS>(ctx, what, driver, pool, node, generation, devs, n, out, cap, len,
+                                                   slice_off, n_slices, taint);
 }
 
 extern "C" int32_t kxpu_dra_slices_taint(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,

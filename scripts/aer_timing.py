@@ -5,8 +5,10 @@
     attribute present): 65 536 and 2^20 devices, 0 %, 1 % and 100 % of them tainted, tables of 1 and 3 entries (the
     3-entry table is the host's: vfio-device-missing, pcie-aer=fatal, pcie-aer=nonfatal, a device carrying the first
     and one of the other two), 40 calls of each, alternating; KXPU_T_EMIT.
-Median [p10, p90].  Prints the card and its power limit, and one JSON object (also written to argv[1] when given)."""
+Median [p10, p90].  Prints the card and its power limit, and one JSON object (also written to argv[1] when given), with
+the SHA-256 of each taint call's output and slice offsets, so that two builds can be checked for identical bytes."""
 import ctypes as C
+import hashlib
 import json
 import os
 import subprocess
@@ -28,6 +30,13 @@ def stats(v):
     v = np.asarray(v)
     return {"median_ms": round(float(np.median(v)), 4), "p10_ms": round(float(np.percentile(v, 10)), 4),
             "p90_ms": round(float(np.percentile(v, 90)), 4), "n": len(v)}
+
+
+def digest(out, length, offs, n_slices):
+    """SHA-256 of a call's output bytes and its slice offsets"""
+    h = hashlib.sha256(memoryview(out[:length]))
+    h.update(memoryview(offs[:n_slices + 1]))
+    return h.hexdigest()
 
 
 def since_of(n, share, k, seed=5):
@@ -86,6 +95,8 @@ def main():
 
                     for _ in range(3):
                         call_one(); call_list()
+                    list_sha = digest(out, call_list(), offs, ns.value)
+                    one_sha = digest(out, call_one(), offs, ns.value)
                     k_l, k_o = [], []
                     for _ in range(REPS):
                         list_len = call_list()
@@ -95,6 +106,7 @@ def main():
                     name = "%s_%d_taint%g_entries%d" % (layout, n, 100 * share, k)
                     res["taints"][name] = {"taints_kernel": stats(k_l), "taint_kernel": stats(k_o),
                                            "taints_out_bytes": list_len, "taint_out_bytes": one_len,
+                                           "taints_sha256": list_sha, "taint_sha256": one_sha,
                                            "ratio_median": round(float(np.median(k_l) / np.median(k_o)), 3)}
                     print("%-4s n=%-8d %5.1f %% tainted, %d entries: _taints %.4f ms [%.4f, %.4f] %d B | _taint %.4f ms "
                           "[%.4f, %.4f] %d B | x%.2f" % (layout, n, 100 * share, k, np.median(k_l), np.percentile(k_l, 10),

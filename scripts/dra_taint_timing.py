@@ -3,8 +3,10 @@ kxpu_dra_slices / kxpu_dra_slices_mdev on the same records: 65 536 and 2^20 devi
 attribute present (workloads.dra_devices / dra_mdev_devices), 0 %, 1 % and 100 % of them tainted with the longest key
 (127 bytes) and value (63 bytes), 40 calls of each taint share alternating with the untainted call.  Kernel times come
 from the library's per-stage CUDA events (KXPU_T_EMIT): median [p10, p90].  Prints the card and its power limit and one
-JSON object (also written to argv[1] when given)."""
+JSON object (also written to argv[1] when given), with the SHA-256 of each call's output and slice offsets, so that two
+builds can be checked for identical bytes."""
 import ctypes as C
+import hashlib
 import json
 import os
 import subprocess
@@ -26,6 +28,13 @@ def stats(v):
     v = np.asarray(v)
     return {"median_ms": round(float(np.median(v)), 4), "p10_ms": round(float(np.percentile(v, 10)), 4),
             "p90_ms": round(float(np.percentile(v, 90)), 4), "n": len(v)}
+
+
+def digest(out, length, offs, n_slices):
+    """SHA-256 of a call's output bytes and its slice offsets"""
+    h = hashlib.sha256(memoryview(out[:length]))
+    h.update(memoryview(offs[:n_slices + 1]))
+    return h.hexdigest()
 
 
 def since_of(n, share, seed=5):
@@ -69,6 +78,9 @@ def main():
                 for _ in range(3):  # warm-up
                     call_taint(); call_plain()
                 taint_len = call_taint()
+                taint_sha = digest(out, taint_len, offs, ns.value)
+                call_plain()
+                plain_sha = digest(out, plain_len, offs, ns.value)
                 k_t, k_p = [], []
                 for _ in range(REPS):
                     call_taint()
@@ -77,7 +89,7 @@ def main():
                     k_p.append(kx.timings()[B.T_EMIT])
                 name = "%s_%d_taint%g" % (layout, n, 100 * share)
                 t[name] = {"taint_kernel": stats(k_t), "untainted_kernel": stats(k_p), "taint_out_bytes": taint_len,
-                           "untainted_out_bytes": plain_len,
+                           "untainted_out_bytes": plain_len, "taint_sha256": taint_sha, "untainted_sha256": plain_sha,
                            "ratio_median": round(float(np.median(k_t) / np.median(k_p)), 3)}
                 print("%-4s n=%-8d %5.1f %% tainted: taint kernel %.4f ms [%.4f, %.4f] %d B | untainted %.4f ms [%.4f, %.4f] "
                       "%d B | x%.2f" % (layout, n, 100 * share, np.median(k_t), np.percentile(k_t, 10), np.percentile(k_t, 90),

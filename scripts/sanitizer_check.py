@@ -50,7 +50,8 @@ for dn_ in (3000, 0):
 for dn_ in (3000, 0):
     blob, soff = kx.dra_slices_mdev("vgpu.nvidia.com", "node-a", "node-a", 1, W.dra_mdev_devices(dn_))
     print("dra mdev slices", len(soff) - 1, "bytes", len(blob))
-# PCIe AER health: files shared by four vGPUs each at odd offsets; the taint list emitter with three entries, both layouts
+# PCIe AER health: files shared by four vGPUs each at odd offsets; the taint list emitter with one and three entries,
+# both layouts
 ar = W.aer_records(20000, vgpus_per_parent=4)
 _, gaer = kx.aer_health(ar["text"], ar["file_off"], ar["file_len"], 0, 0, ar["group_off"], ar["group_members"])
 print("aer groups", len(gaer), "flagged", int(((gaer & 3) != 0).sum()))
@@ -58,8 +59,13 @@ tab3 = [("vfio.nvidia.com/unhealthy", "vfio-device-missing", "NoSchedule"),
         ("vfio.nvidia.com/pcie-aer", "fatal", "NoSchedule"), ("vfio.nvidia.com/pcie-aer", "nonfatal", "NoSchedule")]
 since3 = np.full((3000, 3), -1, np.int64)
 since3[::7, 0], since3[::5, 1], since3[1::5, 2] = 1767225600, 1767225660, 1767225720
+blob, soff = kx.dra_slices_taints("vfio.nvidia.com", "node-a", "node-a", 1, W.dra_devices(3000), tab3[:1], since3[:, :1])
+print("dra taints slices, one entry", len(soff) - 1, "bytes", len(blob))
 blob, soff = kx.dra_slices_taints("vfio.nvidia.com", "node-a", "node-a", 1, W.dra_devices(3000), tab3, since3)
 print("dra taints slices", len(soff) - 1, "bytes", len(blob))
+blob, soff = kx.dra_slices_mdev_taints("vgpu.nvidia.com", "node-a", "node-a", 1, W.dra_mdev_devices(3000), tab3[:1],
+                                       since3[:, :1])
+print("dra mdev taints slices, one entry", len(soff) - 1, "bytes", len(blob))
 blob, soff = kx.dra_slices_mdev_taints("vgpu.nvidia.com", "node-a", "node-a", 1, W.dra_mdev_devices(3000), tab3, since3)
 print("dra mdev taints slices", len(soff) - 1, "bytes", len(blob))
 
