@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KXPU_ABI_VERSION 13
+#define KXPU_ABI_VERSION 14
 
 /* status codes */
 #define KXPU_OK             0
@@ -72,7 +72,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
 #define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's and kxpu_pcie_tree's kernels: the slot holds the most recent call's */
-#define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev]: decode, re-emit and compare of the most recent call */
+#define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
 #define KXPU_T_COUNT    8
@@ -596,7 +596,9 @@ int32_t kxpu_reconcile(kxpu_ctx *ctx, const kxpu_snaprec *prev, size_t n_prev, u
 typedef struct kxpu_cdidev {
     char     bdf[16];       /* dev.addr, NUL padded                                       */
     uint32_t iommu_group;   /* devName (decimal)                                          */
-    uint32_t reserved;
+    uint32_t vfio_cdev;     /* N of the function's VFIO cdev /dev/vfio/devices/vfio<N>: read by
+                               kxpu_cdi_emit_cdev only (returned by kxpu_cdi_parse_cdev); the
+                               other calls ignore it, and kxpu_cdi_parse returns 0 (ABI v14)  */
     uint64_t index;         /* dev.index                                                  */
 } kxpu_cdidev;
 
@@ -669,7 +671,7 @@ int32_t kxpu_cdi_emit_mdev(kxpu_ctx *ctx, int32_t format, const char *kind, cons
  * back the indices it handed out (the container runtime resolves <kind>=<index> against these very bytes).
  *   - KXPU_OK with *n records exactly when kxpu_cdi_emit_kind(format, kind, out, *n) returns doc byte for byte.  The
  *     records come back in document order; any device order is accepted, not only ascending index.  bdf is NUL padded
- *     and reserved is 0, as the emitter's input would hold them.  The zero-device documents (YAML "devices: []", JSON
+ *     and vfio_cdev is 0, as the emitter's input would hold them.  The zero-device documents (YAML "devices: []", JSON
  *     "devices": null) give *n = 0.
  *   - KXPU_E_INVALID for every other document (nothing written to out, *n untouched), and for ctx, n or kind NULL, doc
  *     NULL with len > 0, out NULL with cap > 0, or a format other than KXPU_FMT_YAML / KXPU_FMT_JSON.  A document whose
@@ -688,6 +690,37 @@ int32_t kxpu_cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const ui
  * document KXPU_E_INVALID.  Everything else as kxpu_cdi_parse. */
 int32_t kxpu_cdi_parse_mdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
                             kxpu_mdevcdi *out, size_t cap, size_t *n);
+
+/* ------------------------------------------ CDI specs naming VFIO device cdevs (ABI v14) */
+
+/* A function bound to vfio-pci can also be opened through its own VFIO character device instead of its group's
+ * /dev/vfio/<g>:
+ *   [assumed] since Linux 6.6 such a function has /dev/vfio/devices/vfio<N>, and its sysfs directory holds vfio-dev/
+ *             with the one entry vfio<N>;
+ *   [assumed] a kernel built with CONFIG_VFIO_GROUP=n has no /dev/vfio/<g> at all;
+ *   [assumed] a VMM opens the cdev through iommufd (/dev/iommu), which the runtime opens itself, as it opens
+ *             /dev/vfio/vfio for a group; Kata attaches a /dev/vfio/devices/vfio<N> node through QEMU's iommufd
+ *             backend.  So the spec names no /dev/iommu node;
+ *   [assumed] cdev numbers are handed out at bind time and reused: two functions unbound and re-bound in the other order
+ *             swap numbers.
+ * The IOMMU group stays the unit of allocation (iommufd claims DMA ownership for the whole group). */
+
+/* kxpu_cdi_emit_kind's document, byte for byte, except that the device node of device i is
+ * /dev/vfio/devices/vfio<N> with N = devs[i].vfio_cdev (every uint32 is valid) in place of /dev/vfio/<g>.  The
+ * annotations (cdi.k8s.io/vfio<g> included), head, tail, zero-device form, device order, kind domain, sizing protocol and
+ * KXPU_E_UNSUPPORTED cases are kxpu_cdi_emit_kind's.
+ * GPU: the kernel of kxpu_cdi_emit_kind with the node literal and number compiled in; the longest fragment is 12 bytes
+ * longer, and kinds up to 22 bytes still run at four CTAs per SM (DESIGN.md K6).  Timed under KXPU_T_EMIT. */
+int32_t kxpu_cdi_emit_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_cdidev *devs, size_t n,
+                           uint8_t *out, size_t cap, size_t *len);
+
+/* The inverse of kxpu_cdi_emit_cdev: KXPU_OK with *n records exactly when kxpu_cdi_emit_cdev(format, kind, out, *n)
+ * returns doc byte for byte; vfio_cdev holds each device's N.  A document of kxpu_cdi_emit_kind (a group node) is
+ * KXPU_E_INVALID here, as a document of kxpu_cdi_emit_cdev is for kxpu_cdi_parse; the zero-device documents are the same
+ * bytes in both layouts, and both calls return *n = 0 for them.  KXPU_CDI_FRAG_MIN still bounds *n.  Everything else as
+ * kxpu_cdi_parse. */
+int32_t kxpu_cdi_parse_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
+                            kxpu_cdidev *out, size_t cap, size_t *n);
 
 /* ------------------------------------------------------ S5: Allocate names */
 

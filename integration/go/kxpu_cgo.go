@@ -631,6 +631,41 @@ func (k *kxpu) cdiParseMdev(format int, doc []byte, kind string) ([]C.kxpu_mdevc
 	return out[:n], nil
 }
 
+// VFIO cdevs (ABI v14).  cdiEmitCdev writes cdiEmitKind's document with each device's node /dev/vfio/devices/vfio<N>,
+// N = devs[i].vfio_cdev (read from <bdf>/vfio-dev/vfio<N>); cdiParseCdev is its inverse and returns N in vfio_cdev.  A
+// group-layout document is an error for cdiParseCdev, and a cdev document for cdiParse.
+func (k *kxpu) cdiEmitCdev(format int, kind string, devs []C.kxpu_cdidev) ([]byte, error) {
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	var p *C.kxpu_cdidev
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	var n C.size_t
+	C.kxpu_cdi_emit_cdev(k.ctx, C.int32_t(format), ck, p, C.size_t(len(devs)), nil, 0, &n) // sizing call
+	buf := make([]byte, n+1)
+	err := kxCheck(k.ctx, "kxpu_cdi_emit_cdev", C.kxpu_cdi_emit_cdev(k.ctx, C.int32_t(format), ck, p, C.size_t(len(devs)),
+		(*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n))
+	return buf[:n], err
+}
+
+func (k *kxpu) cdiParseCdev(format int, doc []byte, kind string) ([]C.kxpu_cdidev, error) {
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	out := make([]C.kxpu_cdidev, len(doc)/C.KXPU_CDI_FRAG_MIN+1)
+	var n C.size_t
+	var dp *C.uint8_t
+	if len(doc) > 0 {
+		dp = (*C.uint8_t)(unsafe.Pointer(&doc[0]))
+	}
+	err := kxCheck(k.ctx, "kxpu_cdi_parse_cdev", C.kxpu_cdi_parse_cdev(k.ctx, C.int32_t(format), ck, dp, C.size_t(len(doc)),
+		&out[0], C.size_t(len(out)), &n))
+	if err != nil {
+		return nil, err
+	}
+	return out[:n], nil
+}
+
 // The index state file of the restart resume: <cdiConfigPath>.kata-xpu-cdi-index, "pci <next>\nmdev <next>\n".  The CDI
 // cache loads only *.json / *.yaml.  Write it (tmp + fsync + rename, only when its bytes change) whenever a next index
 // grows, before any spec that names the new indices.

@@ -32,6 +32,8 @@ DEVREC_DTYPE = np.dtype([("bdf", "S16"), ("vendor_txt", "u1", (8,)), ("device_tx
                          ("device_len", "u1"), ("flags", "u1"), ("reserved0", "u1"),
                          ("reserved1", "<u4", (2,))])
 CDIDEV_DTYPE = np.dtype([("bdf", "S16"), ("iommu_group", "<u4"), ("reserved", "<u4"), ("index", "<u8")])
+# kxpu_cdidev.vfio_cdev (ABI v14: N of /dev/vfio/devices/vfio<N>) keeps its pre-v14 numpy field name, as NUMA_FIELD does
+CDEV_FIELD = "reserved"
 RULE_DTYPE = np.dtype([("vendor", "S8"), ("driver", "S16"), ("reserved", "<u4", (2,))])  # kxpu_xpu_rule
 assert DEVREC_DTYPE.itemsize == 64 and CDIDEV_DTYPE.itemsize == 32 and RULE_DTYPE.itemsize == 32
 MAX_RULES = 16
@@ -92,6 +94,7 @@ ABI_SYMBOLS = [
     "kxpu_reconcile", "kxpu_pcie_tree", "kxpu_preferred_allocation_pcie", "kxpu_classify_viable",
     "kxpu_dra_slices", "kxpu_dra_slices_mdev", "kxpu_dra_slices_taint", "kxpu_dra_slices_mdev_taint",
     "kxpu_aer_health", "kxpu_dra_slices_taints", "kxpu_dra_slices_mdev_taints", "kxpu_cdi_parse", "kxpu_cdi_parse_mdev",
+    "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev",
 ]
 
 
@@ -202,6 +205,8 @@ def load_library():
         "kxpu_aer_health": (i32, [vp, vp, sz, vp, vp, sz, u64, u64, vp, vp, sz, vp, vp]),
         "kxpu_cdi_parse": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_cdi_parse_mdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_cdi_emit_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_cdi_parse_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_dra_slices_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                          C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_mdev_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
@@ -675,17 +680,26 @@ class Kxpu:
 
     def cdi_emit_mdev(self, fmt, devs, kind):
         """kxpu_cdi_emit_mdev: the CDI spec of a vGPU class (MDEVCDI_DTYPE devices, kind bytes or str)."""
+        return self._emit_sized(self.L.kxpu_cdi_emit_mdev, MDEVCDI_DTYPE, fmt, devs, kind)
+
+    def cdi_emit_cdev(self, fmt, devs, kind):
+        """kxpu_cdi_emit_cdev: the CDI spec of a passthrough class whose functions are reached through their VFIO cdevs
+        (CDIDEV_DTYPE devices, N of /dev/vfio/devices/vfio<N> in the CDEV_FIELD field; kind bytes or str)."""
+        return self._emit_sized(self.L.kxpu_cdi_emit_cdev, CDIDEV_DTYPE, fmt, devs, kind)
+
+    def _emit_sized(self, fn, dtype, fmt, devs, kind):
+        """the two-call sizing protocol: out = NULL gives the length, the second call writes the document"""
         devs = np.ascontiguousarray(devs)
-        assert devs.dtype == MDEVCDI_DTYPE
+        assert devs.dtype == dtype
         kb = _kind(kind)
         need = C.c_size_t(0)
         dp = _ptr(devs) if len(devs) else None
-        rc = self.L.kxpu_cdi_emit_mdev(self.ctx, fmt, kb, dp, len(devs), None, 0, C.byref(need))
+        rc = fn(self.ctx, fmt, kb, dp, len(devs), None, 0, C.byref(need))
         if rc not in (KXPU_OK, E_NOSPACE):
             self._chk(rc)
         out = np.empty(max(need.value, 1), np.uint8)
         got = C.c_size_t(0)
-        self._chk(self.L.kxpu_cdi_emit_mdev(self.ctx, fmt, kb, dp, len(devs), _ptr(out), need.value, C.byref(got)))
+        self._chk(fn(self.ctx, fmt, kb, dp, len(devs), _ptr(out), need.value, C.byref(got)))
         return out[:got.value].tobytes()
 
     def dra_slices(self, driver, pool, node, generation, devs):
@@ -791,11 +805,17 @@ class Kxpu:
         """kxpu_cdi_parse_mdev: the MDEVCDI_DTYPE records of a vGPU class's CDI spec."""
         return self._parse(self.L.kxpu_cdi_parse_mdev, MDEVCDI_DTYPE, fmt, doc, kind)
 
-    def cdi_parse_raw(self, fmt, doc, kind, cap, mdev=False, offset=0):
+    def cdi_parse_cdev(self, fmt, doc, kind):
+        """kxpu_cdi_parse_cdev: the CDIDEV_DTYPE records (N in CDEV_FIELD) of a spec kxpu_cdi_emit_cdev wrote."""
+        return self._parse(self.L.kxpu_cdi_parse_cdev, CDIDEV_DTYPE, fmt, doc, kind)
+
+    def cdi_parse_raw(self, fmt, doc, kind, cap, mdev=False, offset=0, cdev=False):
         """The bare call: doc placed at `offset` bytes past a 16-byte aligned host buffer, out of `cap` records.
-        Returns (status, n, records) with n and the records as the call left them (n = -1: not stored)."""
+        Returns (status, n, records) with n and the records as the call left them (n = -1: not stored).
+        mdev: kxpu_cdi_parse_mdev, cdev: kxpu_cdi_parse_cdev, neither: kxpu_cdi_parse."""
+        assert not (mdev and cdev)
         dtype = MDEVCDI_DTYPE if mdev else CDIDEV_DTYPE
-        fn = self.L.kxpu_cdi_parse_mdev if mdev else self.L.kxpu_cdi_parse
+        fn = self.L.kxpu_cdi_parse_mdev if mdev else self.L.kxpu_cdi_parse_cdev if cdev else self.L.kxpu_cdi_parse
         buf = np.zeros(len(doc) + offset + 16, np.uint8)
         base = (-buf.ctypes.data) % 16
         buf = buf[base:]

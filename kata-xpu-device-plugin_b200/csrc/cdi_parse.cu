@@ -22,11 +22,12 @@ namespace kxparse {
 constexpr int PT = 8192;         // document bytes per CTA
 constexpr int PARSE_THREADS = 256;
 constexpr int ROWS = PT / PARSE_THREADS;  // positions per thread, one row of 256 consecutive positions each
-constexpr int HALO = 512;        // >= the longest fragment (emit.cu MAX_FRAG_MDEV = 480) plus the start pattern
+constexpr int HALO = 512;        // >= the longest fragment of any layout plus the start pattern
 constexpr int LEAD = 16;         // bytes staged in front of the tile: the '\n' before a start at the tile's first byte
 constexpr int WIN = LEAD + PT + HALO;
 constexpr int PAT_MAX = 32;
-constexpr int LAYOUT_PCI = 0, LAYOUT_MDEV = 1;
+constexpr int LAYOUT_PCI = KX_CDI_PCI, LAYOUT_MDEV = KX_CDI_MDEV, LAYOUT_CDEV = KX_CDI_CDEV;
+static_assert(HALO >= KX_CDI_FRAG_MAX + PAT_MAX, "a fragment that starts in the tile must end inside the window");
 
 struct ParseParams {
     const uint8_t *doc;           // padded with zeros to a whole tile plus HALO + LEAD bytes
@@ -37,7 +38,8 @@ struct ParseParams {
     uint32_t epoch;
     unsigned long long *count;    // written by the last tile: the number of starts
     uint32_t pat_len;             // '\n' + literal 0
-    uint32_t l1, l2, l3, lm;      // literal 1, literal 2, literal 3 (with the kind), the mdev annotation's opening
+    uint32_t l1, l2, l3, lm;      // literal 1, literal 2, literal 3 (with the kind), literal 4 (mdev: the annotation's
+                                  // opening, cdev: the node literal)
     uint8_t pat[PAT_MAX];
 };
 
@@ -97,7 +99,9 @@ __global__ void __launch_bounds__(PARSE_THREADS) k_cdi_decode(const __grid_const
         const uint32_t l = (uint32_t)__ffs((int)m) - 1u;
         uint32_t q = LEAD + r * PARSE_THREADS + ww * 32u + l + P.pat_len - 1u;  // after literal 0
         unsigned long long index = 0;
+        const uint32_t name_at = q;
         for (uint32_t k = 0; k < 20u && is_digit(at(q)); k++, q++) index = index * 10ull + (at(q) - '0');
+        const uint32_t name_end = q;
         q += P.l1;
         const bool quoted = FMT == KXPU_FMT_YAML && at(q) == '"';
         if (quoted) q++;
@@ -116,7 +120,17 @@ __global__ void __launch_bounds__(PARSE_THREADS) k_cdi_decode(const __grid_const
             kxpu_cdidev d;
             memcpy(d.bdf, bdf, 16);
             d.iommu_group = group;
-            d.reserved = 0;
+            d.vfio_cdev = 0;
+            d.index = index;
+            static_cast<kxpu_cdidev *>(P.recs)[slot] = d;
+        } else if constexpr (LAYOUT == LAYOUT_CDEV) {  // N follows the name's second copy and the node literal
+            q += P.l3 + (name_end - name_at) + P.lm;  // the second copy is as long as the first in a valid fragment
+            uint32_t node = 0;
+            for (uint32_t k = 0; k < 10u && is_digit(at(q)); k++, q++) node = node * 10u + (at(q) - '0');
+            kxpu_cdidev d;
+            memcpy(d.bdf, bdf, 16);
+            d.iommu_group = group;
+            d.vfio_cdev = node;
             d.index = index;
             static_cast<kxpu_cdidev *>(P.recs)[slot] = d;
         } else {  // the uuid follows the name's second copy: "<kind>=<index>" and the mdev annotation's opening
@@ -160,9 +174,10 @@ static void decode_launch(kxpu_ctx *ctx, uint32_t tiles, const ParseParams &P) {
     k_cdi_decode<FMT, LAYOUT><<<tiles, PARSE_THREADS, 0, ctx->stream>>>(P);
 }
 
-// mdev: out is kxpu_mdevcdi[cap], else kxpu_cdidev[cap]
+// LAYOUT_MDEV: out is kxpu_mdevcdi[cap], else kxpu_cdidev[cap]
 static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len, void *out,
-                         size_t cap, size_t *n, bool mdev, const char *what) {
+                         size_t cap, size_t *n, int layout, const char *what) {
+    const bool mdev = layout == LAYOUT_MDEV;
     if (!ctx || !n || !kind || (len && !doc) || (cap && !out) || (format != KXPU_FMT_YAML && format != KXPU_FMT_JSON))
         return KXPU_E_INVALID;
     if (len >= (1ull << 32)) { KX_SET_ERR(ctx, "%s: a document of 2^32 bytes or more", what); return KXPU_E_UNSUPPORTED; }
@@ -171,13 +186,13 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
     std::string part[10];
-    for (int k = 0; k < 10; k++) part[k] = kx_cdi_part(format, mdev, k, kind);
+    for (int k = 0; k < 10; k++) part[k] = kx_cdi_part(format, layout, k, kind);
     if (len == part[8].size() && memcmp(doc, part[8].data(), len) == 0) {  // the zero-device document
         *n = 0;
         return KXPU_OK;
     }
-    // the shortest fragment: the literals, one-digit index (twice) and group (twice), a one-byte bdf, the uuid, and in
-    // JSON the separator after the device
+    // the shortest fragment: the literals, one-digit index (twice) and group (twice; cdev: the group and N), a one-byte
+    // bdf, the uuid, and in JSON the separator after the device
     size_t lits = 0;
     for (int k : {0, 1, 2, 3, 4, 5, 9}) lits += part[k].size();
     const size_t frag_min = lits + 5 + (mdev ? 36 : 0) + (format == KXPU_FMT_JSON ? 1 : 0);
@@ -222,6 +237,9 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
     if (mdev) {
         if (format == KXPU_FMT_YAML) decode_launch<KXPU_FMT_YAML, LAYOUT_MDEV>(ctx, tiles, P);
         else decode_launch<KXPU_FMT_JSON, LAYOUT_MDEV>(ctx, tiles, P);
+    } else if (layout == LAYOUT_CDEV) {
+        if (format == KXPU_FMT_YAML) decode_launch<KXPU_FMT_YAML, LAYOUT_CDEV>(ctx, tiles, P);
+        else decode_launch<KXPU_FMT_JSON, LAYOUT_CDEV>(ctx, tiles, P);
     } else {
         if (format == KXPU_FMT_YAML) decode_launch<KXPU_FMT_YAML, LAYOUT_PCI>(ctx, tiles, P);
         else decode_launch<KXPU_FMT_JSON, LAYOUT_PCI>(ctx, tiles, P);
@@ -234,7 +252,7 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
     if (count == 0 || count > max_n) { KX_SET_ERR(ctx, "%s: not a document the emitter writes", what); return KXPU_E_INVALID; }
     uint8_t *d_emit = nullptr;
     unsigned long long *d_total = nullptr;
-    int32_t rc = kx_cdi_emit_enqueue(ctx, format, kind, d_recs, (size_t)count, mdev, sc, &d_emit, &d_total, false);
+    int32_t rc = kx_cdi_emit_enqueue(ctx, format, kind, d_recs, (size_t)count, layout, sc, &d_emit, &d_total, false);
     if (rc != KXPU_OK) return rc;
     k_cdi_compare<<<(unsigned)ctx->sm_count * 4, 256, 0, ctx->stream>>>(d_doc, d_emit, len, d_total,
                                                                          reinterpret_cast<uint32_t *>(d_ctl + 1));
@@ -259,10 +277,15 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
 
 extern "C" int32_t kxpu_cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
                                   kxpu_cdidev *out, size_t cap, size_t *n) {
-    return cdi_parse(ctx, format, kind, doc, len, out, cap, n, false, "cdi_parse");
+    return cdi_parse(ctx, format, kind, doc, len, out, cap, n, LAYOUT_PCI, "cdi_parse");
 }
 
 extern "C" int32_t kxpu_cdi_parse_mdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
                                        kxpu_mdevcdi *out, size_t cap, size_t *n) {
-    return cdi_parse(ctx, format, kind, doc, len, out, cap, n, true, "cdi_parse_mdev");
+    return cdi_parse(ctx, format, kind, doc, len, out, cap, n, LAYOUT_MDEV, "cdi_parse_mdev");
+}
+
+extern "C" int32_t kxpu_cdi_parse_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
+                                       kxpu_cdidev *out, size_t cap, size_t *n) {
+    return cdi_parse(ctx, format, kind, doc, len, out, cap, n, LAYOUT_CDEV, "cdi_parse_cdev");
 }

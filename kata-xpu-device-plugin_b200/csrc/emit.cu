@@ -34,7 +34,14 @@ constexpr int MAX_FRAG = 368;  // upper bound of one fragment: literals (<= 267 
 constexpr int MAX_FRAG_LONG = 416;  // kinds of 23..63 bytes: 62.7 KB per CTA, three CTAs per SM
 constexpr int MAX_FRAG_MDEV = 480;  // kxpu_cdi_emit_mdev, every kind: the PCI bound + the mdev annotation (<= 20 + 36 bytes);
                                     // 69.8 KB per CTA, three CTAs per SM
-constexpr int LAYOUT_PCI = 0, LAYOUT_MDEV = 1;  // kxpu_cdidev / kxpu_mdevcdi
+// kxpu_cdi_emit_cdev: the node literal is "devices/vfio" longer, and N takes the place of the group's second copy (both
+// at most 10 digits), so every fragment bound grows by exactly that literal and the kind split stays at 22 bytes
+#define KX_CDEV_NODE "devices/vfio"
+constexpr int CDEV_EXTRA = sizeof(KX_CDEV_NODE) - 1;
+constexpr int MAX_FRAG_CDEV = MAX_FRAG + CDEV_EXTRA;
+constexpr int MAX_FRAG_CDEV_LONG = MAX_FRAG_LONG + CDEV_EXTRA;
+constexpr int LAYOUT_PCI = KX_CDI_PCI, LAYOUT_MDEV = KX_CDI_MDEV, LAYOUT_CDEV = KX_CDI_CDEV;
+static_assert(MAX_FRAG_MDEV <= KX_CDI_FRAG_MAX && MAX_FRAG_CDEV_LONG <= KX_CDI_FRAG_MAX, "the parse halo must follow");
 constexpr int POOL_MAX = 640;
 constexpr int KIND_MAX = 63;
 
@@ -81,6 +88,10 @@ static const Parts h_json_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_J4, KX_J5, K
 static const Parts h_yaml_mdev_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_YM, KX_Y5, KX_YHA, KX_YT, KX_YHA, KX_Y4},
                                         {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB, nullptr}};
 static const Parts h_json_mdev_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_JM, KX_J5, KX_JHA, KX_JT, KX_JHA, KX_J4},
+                                        {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB, nullptr}};
+static const Parts h_yaml_cdev_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_Y4 KX_CDEV_NODE, KX_Y5, KX_YHA, KX_YT, KX_YHA, nullptr},
+                                        {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB, nullptr}};
+static const Parts h_json_cdev_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_J4 KX_CDEV_NODE, KX_J5, KX_JHA, KX_JT, KX_JHA, nullptr},
                                         {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB, nullptr}};
 static const char *kDefaultKind = "nvidia.com/gpu";  // CdiVendorClass, generic_device_plugin.go:31
 
@@ -202,6 +213,8 @@ struct TileSmem {
     uint32_t wsum[EMIT_THREADS / 32];
     uint32_t tile_total;
 };
+// four CTAs per SM (228 KB of shared memory, 1 KB of it reserved per CTA) for the short-kind tiles of both node layouts
+static_assert(4 * (sizeof(TileSmem<MAX_FRAG_CDEV>) + 1024) <= 228 * 1024, "the cdev short-kind tile lost an SM slot");
 
 template <int FMT, int MAXF, int LAYOUT>
 __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constant__ EmitParams E) {
@@ -216,13 +229,14 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
     uint32_t flen = 0;
     if (tid < TILE && i0 + tid < E.n) {
         uint4 bq;  // the bdf / parent address
-        uint32_t group;
+        uint32_t group, node = 0;
         unsigned long long index;
-        if (LAYOUT == LAYOUT_PCI) {
+        if (LAYOUT != LAYOUT_MDEV) {  // bdf[16] | iommu_group | vfio_cdev | index
             const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const kxpu_cdidev *>(E.devs) + i0 + tid);
             const uint4 q0 = p[0], q1 = p[1];
             bq = q0;
             group = q1.x;
+            if constexpr (LAYOUT == LAYOUT_CDEV) node = q1.y;
             index = ((unsigned long long)q1.w << 32) | q1.z;
         } else {  // uuid[36] | iommu_group | parent[16] | index
             const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const kxpu_mdevcdi *>(E.devs) + i0 + tid);
@@ -242,6 +256,12 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
         *reinterpret_cast<uint4 *>(S.bdf[tid]) = bq;
         S.meta[tid] = il | (gl << 8) | (bl << 16) | ((quoted ? 1u : 0u) << 24);
         flen = E.lit_total + 2u * il + 2u * gl + bl + (quoted ? 2u : 0u) + (LAYOUT == LAYOUT_MDEV ? 36u : 0u);
+        if constexpr (LAYOUT == LAYOUT_CDEV) {  // N in place of the group's second copy; its length in grp's spare byte 11
+            uint32_t nl = 1;
+            for (uint32_t p = 10u; nl < 10u && node >= p; p *= 10u) nl++;
+            S.grp[tid][11] = (uint8_t)nl;
+            flen = flen - gl + nl;
+        }
         if (FMT == KXPU_FMT_JSON) flen += (i0 + tid + 1u < E.n) ? 2u : 1u;  // ",\n" between devices, "\n" after the last
     }
     // ---- scan of the 128 lengths (threads >= TILE contribute 0)
@@ -274,6 +294,11 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
     if (first_tile) for (uint32_t k = tid; k < head_len; k += EMIT_THREADS) stg[k] = S.pool[E.off[6] + k];
     if (last_tile) for (uint32_t k = tid; k < tail_len; k += EMIT_THREADS) stg[head_len + tile_total + k] = S.pool[E.off[7] + k];
     // ---- fragments: one warp per device, segment by segment
+    uint32_t cdev_n = 0;  // cdev: lane j holds N of the warp's j-th device, read from the device array (L2) ahead of the loop
+    if constexpr (LAYOUT == LAYOUT_CDEV) {
+        const uint32_t dj = w + lane * (EMIT_THREADS / 32);
+        if (dj < (uint32_t)TILE && i0 + dj < E.n) cdev_n = static_cast<const kxpu_cdidev *>(E.devs)[i0 + dj].vfio_cdev;
+    }
     for (uint32_t d = w; d < (uint32_t)TILE && i0 + d < E.n; d += EMIT_THREADS / 32) {
         const uint32_t m = S.meta[d];
         const uint32_t il = m & 0xffu, gl = (m >> 8) & 0xffu, bl = (m >> 16) & 0xffu;
@@ -301,7 +326,19 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
             o += 36u;
             lit(8);
         }
-        var(S.grp[d], gl); lit(5);
+        if constexpr (LAYOUT == LAYOUT_CDEV) {  // lane k writes digit k of N
+            const uint32_t N = __shfl_sync(0xffffffffu, cdev_n, d / (EMIT_THREADS / 32));
+            const uint32_t nl = S.grp[d][11];
+            if (lane < nl) {
+                uint32_t v = N;
+                for (uint32_t k = lane + 1u; k < nl; k++) v /= 10u;
+                dst[o + lane] = (uint8_t)('0' + v % 10u);
+            }
+            o += nl;
+        } else {
+            var(S.grp[d], gl);
+        }
+        lit(5);
         if (FMT == KXPU_FMT_JSON) {
             const bool more = i0 + d + 1u < E.n;
             if (lane == 0) { if (more) { dst[o] = (uint8_t)','; dst[o + 1] = (uint8_t)'\n'; } else dst[o] = (uint8_t)'\n'; }
@@ -854,18 +891,35 @@ static void emit_launch(kxpu_ctx *ctx, uint32_t tiles, const EmitParams &E) {
     k_cdi_fused<FMT, MAXF, LAYOUT><<<tiles, EMIT_THREADS, sizeof(TileSmem<MAXF>), ctx->stream>>>(E);
 }
 
-static const Parts &parts_of(int32_t format, bool mdev) {
-    return mdev ? (format == KXPU_FMT_YAML ? h_yaml_mdev_parts : h_json_mdev_parts)
-                : (format == KXPU_FMT_YAML ? h_yaml_parts : h_json_parts);
+static const Parts &parts_of(int32_t format, int layout) {
+    const bool yaml = format == KXPU_FMT_YAML;
+    if (layout == LAYOUT_MDEV) return yaml ? h_yaml_mdev_parts : h_json_mdev_parts;
+    if (layout == LAYOUT_CDEV) return yaml ? h_yaml_cdev_parts : h_json_cdev_parts;
+    return yaml ? h_yaml_parts : h_json_parts;
 }
 
 bool kx_cdi_kind_ok(const char *kind) { return kind_ok(kind); }
 
-std::string kx_cdi_part(int32_t format, bool mdev, int k, const char *kind) { return part_text(parts_of(format, mdev), k, kind); }
+std::string kx_cdi_part(int32_t format, int layout, int k, const char *kind) { return part_text(parts_of(format, layout), k, kind); }
 
-int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, const void *d_devs, size_t n, bool mdev,
+template <int MAXF, int LAYOUT>
+static void emit_smem_attr() {
+    cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAXF, LAYOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)sizeof(TileSmem<MAXF>));
+    cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_JSON, MAXF, LAYOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)sizeof(TileSmem<MAXF>));
+}
+
+int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, const void *d_devs, size_t n, int layout,
                             KxScratch &sc, uint8_t **d_out_p, unsigned long long **d_total_p, bool timed) {
-    const Parts &parts = parts_of(format, mdev);
+    const bool mdev = layout == LAYOUT_MDEV;
+    const Parts &parts = parts_of(format, layout);
+    static bool cdev_attr_done = false;
+    if (layout == LAYOUT_CDEV && !cdev_attr_done) {
+        emit_smem_attr<MAX_FRAG_CDEV, LAYOUT_CDEV>();
+        emit_smem_attr<MAX_FRAG_CDEV_LONG, LAYOUT_CDEV>();
+        cdev_attr_done = true;
+    }
     static bool attr_done = false;
     if (!attr_done) {
         cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAX_FRAG, LAYOUT_PCI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -899,10 +953,12 @@ int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, con
     const uint32_t tiles = (N + TILE - 1) / TILE;
     const uint32_t frag = E.lit_total + 2 * 20 + 2 * 10 + 15 + 2 + 2 + (mdev ? 36 : 0);  // no fragment is longer
     const size_t bound = (size_t)n * frag + E.len[6] + E.len[7] + 64;
-    // kinds up to 22 bytes fit the four-CTAs-per-SM tile, longer ones take the MAX_FRAG_LONG instantiation; every
-    // mdev kind the MAX_FRAG_MDEV one
-    const bool long_frag = frag > (uint32_t)MAX_FRAG;
-    if (frag > (uint32_t)(mdev ? MAX_FRAG_MDEV : MAX_FRAG_LONG)) return KXPU_E_INVALID;  // the literals grew: the bound must follow
+    // kinds up to 22 bytes fit the four-CTAs-per-SM tile, longer ones take the MAX_FRAG_LONG instantiation (cdev: both
+    // bounds CDEV_EXTRA larger, so the same kinds); every mdev kind the MAX_FRAG_MDEV one
+    const bool cdev = layout == LAYOUT_CDEV;
+    const bool long_frag = frag > (uint32_t)(cdev ? MAX_FRAG_CDEV : MAX_FRAG);
+    if (frag > (uint32_t)(mdev ? MAX_FRAG_MDEV : cdev ? MAX_FRAG_CDEV_LONG : MAX_FRAG_LONG))
+        return KXPU_E_INVALID;  // the literals grew: the bound must follow
     uint8_t *d_out = nullptr;
     unsigned long long *d_total = nullptr;
     KX_CUDA(ctx, sc.alloc((void **)&d_out, bound));
@@ -916,6 +972,14 @@ int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, con
         if (mdev) {
             if (format == KXPU_FMT_YAML) emit_launch<KXPU_FMT_YAML, MAX_FRAG_MDEV, LAYOUT_MDEV>(ctx, tiles, E);
             else emit_launch<KXPU_FMT_JSON, MAX_FRAG_MDEV, LAYOUT_MDEV>(ctx, tiles, E);
+        } else if (cdev) {
+            if (format == KXPU_FMT_YAML) {
+                if (long_frag) emit_launch<KXPU_FMT_YAML, MAX_FRAG_CDEV_LONG, LAYOUT_CDEV>(ctx, tiles, E);
+                else emit_launch<KXPU_FMT_YAML, MAX_FRAG_CDEV, LAYOUT_CDEV>(ctx, tiles, E);
+            } else {
+                if (long_frag) emit_launch<KXPU_FMT_JSON, MAX_FRAG_CDEV_LONG, LAYOUT_CDEV>(ctx, tiles, E);
+                else emit_launch<KXPU_FMT_JSON, MAX_FRAG_CDEV, LAYOUT_CDEV>(ctx, tiles, E);
+            }
         } else if (format == KXPU_FMT_YAML) {
             if (long_frag) emit_launch<KXPU_FMT_YAML, MAX_FRAG_LONG, LAYOUT_PCI>(ctx, tiles, E);
             else emit_launch<KXPU_FMT_YAML, MAX_FRAG, LAYOUT_PCI>(ctx, tiles, E);
@@ -936,14 +1000,15 @@ int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, con
     return KXPU_OK;
 }
 
-// mdev: devs is kxpu_mdevcdi[n], else kxpu_cdidev[n]
+// LAYOUT_MDEV: devs is kxpu_mdevcdi[n], else kxpu_cdidev[n]
 static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const void *devs, size_t n, uint8_t *out,
-                        size_t cap, size_t *len, bool mdev = false) {
+                        size_t cap, size_t *len, int layout = LAYOUT_PCI) {
+    const bool mdev = layout == LAYOUT_MDEV;
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
     if (n == 0) {  // Devices stays nil: yaml "devices: []", json "devices": null (cdi/spec.go:42-49)
-        const std::string doc = kx_cdi_part(format, mdev, 8, kind);
+        const std::string doc = kx_cdi_part(format, layout, 8, kind);
         *len = doc.size();
         if (cap < *len || !out) return KXPU_E_NOSPACE;
         memcpy(out, doc.data(), *len);
@@ -956,7 +1021,7 @@ static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const v
     unsigned long long *d_total = nullptr;
     KX_CUDA(ctx, sc.alloc((void **)&d_devs, n * dev_bytes));
     cudaMemcpyAsync(d_devs, devs, n * dev_bytes, cudaMemcpyHostToDevice, ctx->stream);
-    const int32_t rc = kx_cdi_emit_enqueue(ctx, format, kind, d_devs, n, mdev, sc, &d_out, &d_total, true);
+    const int32_t rc = kx_cdi_emit_enqueue(ctx, format, kind, d_devs, n, layout, sc, &d_out, &d_total, true);
     if (rc != KXPU_OK) return rc;
     unsigned long long h[2] = {0, 0};
     cudaMemcpyAsync(h, d_total, 16, cudaMemcpyDeviceToHost, ctx->stream);
@@ -994,7 +1059,16 @@ extern "C" int32_t kxpu_cdi_emit_mdev(kxpu_ctx *ctx, int32_t format, const char 
     if (!ctx || !len || !kind || (n && !devs) || (format != KXPU_FMT_YAML && format != KXPU_FMT_JSON)) return KXPU_E_INVALID;
     if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
     if (!kind_ok(kind)) { KX_SET_ERR(ctx, "cdi_emit_mdev: kind is not a CDI vendor/class of at most 63 bytes"); return KXPU_E_UNSUPPORTED; }
-    return cdi_emit(ctx, format, kind, devs, n, out, cap, len, true);
+    return cdi_emit(ctx, format, kind, devs, n, out, cap, len, LAYOUT_MDEV);
+}
+
+extern "C" int32_t kxpu_cdi_emit_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_cdidev *devs, size_t n,
+                                      uint8_t *out, size_t cap, size_t *len) {
+    static_assert(offsetof(kxpu_cdidev, vfio_cdev) == 20, "kxpu_cdidev layout");
+    if (!ctx || !len || !kind || (n && !devs) || (format != KXPU_FMT_YAML && format != KXPU_FMT_JSON)) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    if (!kind_ok(kind)) { KX_SET_ERR(ctx, "cdi_emit_cdev: kind is not a CDI vendor/class of at most 63 bytes"); return KXPU_E_UNSUPPORTED; }
+    return cdi_emit(ctx, format, kind, devs, n, out, cap, len, LAYOUT_CDEV);
 }
 
 // shared driver of the "thread per item" emitters.  h_in3 (optional, in3_bytes): one more input, uploaded like the

@@ -408,12 +408,59 @@ static Error walkDir(Plugin &p, const std::string &path, const std::string &name
     return Error();
 }
 
-Error Plugin::gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pcipath> *paths) {
+Error Plugin::gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pcipath> *paths, std::vector<int64_t> *cdevs) {
     recs.clear();
     if (paths) paths->clear();
     size_t slash = basePath.find_last_of('/');
-    return walkDir(*this, basePath, slash == std::string::npos ? basePath : basePath.substr(slash + 1), recs,
-                   readsPaths() ? paths : nullptr);
+    Error e = walkDir(*this, basePath, slash == std::string::npos ? basePath : basePath.substr(slash + 1), recs,
+                      readsPaths() ? paths : nullptr);
+    readCdevs(recs, cdevs);
+    return e;
+}
+
+bool Plugin::cdevEnabled() const {
+    for (const XpuClass &c : xpuClasses)
+        if (c.vfioCdev) return true;
+    return false;
+}
+
+int64_t Plugin::readVfioCdev(const std::string &bdf) {
+    cdevReads++;
+    DIR *d = opendir((basePath + "/" + bdf + "/vfio-dev").c_str());
+    if (!d) return -1;
+    std::string entry;
+    int entries = 0;
+    while (struct dirent *de = readdir(d)) {
+        if (strcmp(de->d_name, ".") == 0 || strcmp(de->d_name, "..") == 0) continue;
+        if (++entries == 1) entry = de->d_name;
+    }
+    closedir(d);
+    if (entries != 1 || entry.size() < 5 || entry.size() > 14 || entry.compare(0, 4, "vfio") != 0) return -1;
+    const std::string num = entry.substr(4);
+    if (num.size() > 1 && num[0] == '0') return -1;  // canonical decimals only
+    uint64_t v = 0;
+    for (char ch : num) {
+        if (ch < '0' || ch > '9') return -1;
+        v = v * 10 + (uint64_t)(ch - '0');
+    }
+    return v < (1ull << 32) ? (int64_t)v : -1;
+}
+
+// the vfio-dev/ read of every record that matches a vfioCdev class (vendor and driver), after either gather
+void Plugin::readCdevs(const std::vector<kxpu_devrec> &recs, std::vector<int64_t> *cdevs) {
+    if (!cdevs) return;
+    cdevs->clear();
+    if (!cdevEnabled()) return;
+    cdevs->assign(recs.size(), -1);
+    for (size_t i = 0; i < recs.size(); i++) {
+        const kxpu_devrec &r = recs[i];
+        if (r.flags & (KXPU_REC_IS_DIR | KXPU_REC_VENDOR_ERR | KXPU_REC_DRIVER_ERR)) continue;
+        const std::string vendor = trimID(std::string((const char *)r.vendor_txt, std::min<size_t>(r.vendor_len, sizeof r.vendor_txt)));
+        const std::string drv(r.driver, strnlen(r.driver, sizeof r.driver));
+        bool match = false;
+        for (const XpuClass &c : xpuClasses) match |= c.vfioCdev && c.vendor == vendor && c.driver == drv;
+        if (match) (*cdevs)[i] = readVfioCdev(std::string(r.bdf, strnlen(r.bdf, sizeof r.bdf)));
+    }
 }
 
 // ---------------------------------------------------------------------------- SURVEY 8(f) row 2
@@ -423,7 +470,14 @@ Error Plugin::gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pci
 // buffering) and by several threads, each filling its own slice of the record table, so that S1 ends
 // in one contiguous table ready for a single H2D copy.  Only with the default seams; real directories
 // under basePath (never on sysfs) go through the generic walk at their position.
-Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads, std::vector<kxpu_pcipath> *paths) {
+Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads, std::vector<kxpu_pcipath> *paths,
+                                std::vector<int64_t> *cdevs) {
+    Error e = gatherRecordsFastWalk(recs, threads, paths);
+    readCdevs(recs, cdevs);
+    return e;
+}
+
+Error Plugin::gatherRecordsFastWalk(std::vector<kxpu_devrec> &recs, unsigned threads, std::vector<kxpu_pcipath> *paths) {
     recs.clear();
     if (paths) paths->clear();
     if (!readsPaths()) paths = nullptr;
@@ -659,7 +713,7 @@ static kxpu_dradev draRecord(const kxpu_devrec &r, const kxpu_pcipath *path, uin
 
 // the walk and classify of createIommuDeviceMap
 Error Plugin::classifyPci(PciWalk &w) {
-    Error e = gatherRecordsFast(w.recs, 0, &w.paths);  // same records as gatherRecords (falls back to it when a seam was replaced)
+    Error e = gatherRecordsFast(w.recs, 0, &w.paths, &w.cdevs);  // same records as gatherRecords (falls back to it when a seam was replaced)
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // Walk's error is ignored by the reference (:132)
     const std::vector<kxpu_devrec> &recs = w.recs;
     const size_t n = recs.size();
@@ -715,12 +769,18 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
             const uint64_t idx = index ? (*index)[c.accept[c.gmem[k]]] : c.accept[c.gmem[k]];
             devs.push_back(NvidiaGpuDevice{std::string(r.bdf), idx});  // :171-174
             devs.back().xpuClass = recordClass(xpuClasses, r.vendor_txt, r.vendor_len, r.driver, sizeof r.driver);
+            if (!w.cdevs.empty()) devs.back().cdev = w.cdevs[c.gmem[k]];
         }
+        std::string blocker;
+        if (groupViability && c.gblk[g] != KXPU_VIABLE) blocker = blockerOf(w.recs[c.gblk[g]]);
+        if (blocker.empty() && xpuClasses[groupClass[c.gids[g]]].vfioCdev)  // a member without a cdev: VFIO cannot open it
+            for (const NvidiaGpuDevice &d : devs)
+                if (d.cdev < 0) { blocker = d.addr + " has no VFIO cdev"; break; }
         iommuMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
         iommuClass.push_back(groupClass[c.gids[g]]);
         if (topologyAware) iommuNuma.push_back(c.gnuma[g]);
         if (pcieTopologyAware) iommuPcieNode.push_back(w.gnode[g]);
-        if (groupViability) iommuBlocker.push_back(c.gblk[g] == KXPU_VIABLE ? std::string() : blockerOf(w.recs[c.gblk[g]]));
+        if (groupViability || cdevEnabled()) iommuBlocker.push_back(blocker);
         if (draEnabled()) {
             const uint32_t first = c.gmem[c.goff[g]];
             iommuDra.push_back(draRecord(w.recs[first], w.paths.size() > first ? &w.paths[first] : nullptr, c.gnuma[g]));
@@ -865,6 +925,8 @@ Error Plugin::checkVgpuClasses() const {
             if (o != v && (all[o]->cdiKind == all[v]->cdiKind || all[o]->cdiFileStem == all[v]->cdiFileStem))
                 return fail("vGPU class " + all[v]->vendor + "/" + all[v]->driver + ": CDI kind and file stem must differ from every other class's");
     if (vgpuClasses.size() > KXPU_MAX_RULES) return fail("more vGPU classes than KXPU_MAX_RULES");
+    for (const XpuClass &c : vgpuClasses)
+        if (c.vfioCdev) return fail("vGPU class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + "): vfioCdev applies to passthrough classes only");
     return Error();
 }
 
@@ -1205,9 +1267,12 @@ static kxpu_cdidev cdiRecord(const std::string &group, const NvidiaGpuDevice &de
     memset(&d, 0, sizeof d);
     strncpy(d.bdf, dev.addr.c_str(), sizeof d.bdf - 1);
     d.iommu_group = (uint32_t)strtoul(group.c_str(), nullptr, 10);
+    d.vfio_cdev = dev.cdev < 0 ? 0u : (uint32_t)dev.cdev;
     d.index = dev.index;
     return d;
 }
+static bool hasCdev(const NvidiaGpuDevice &dev) { return dev.cdev >= 0; }
+static bool hasCdev(const MdevDevice &) { return true; }
 static kxpu_mdevcdi cdiRecord(const std::string &group, const MdevDevice &m) {
     kxpu_mdevcdi d;
     memset(&d, 0, sizeof d);
@@ -1227,17 +1292,24 @@ Error Plugin::generateClassSpecs(const std::vector<XpuClass> &classes, const Ord
                                  int32_t (*emit)(kxpu_ctx *, int32_t, const char *, const Rec *, size_t, uint8_t *, size_t, size_t *),
                                  std::vector<std::string> &files) {
     std::vector<std::vector<Rec>> per(classes.size());
-    for (size_t g = 0; g < m.size(); g++)
+    for (size_t g = 0; g < m.size(); g++) {
+        bool cdevs = true;  // a vfioCdev class's spec leaves out a group with a member without a cdev
+        for (const Dev &dev : m[g].second) cdevs &= hasCdev(dev);
+        if (classes[entryClass[g]].vfioCdev && !cdevs) continue;
         for (const Dev &dev : m[g].second) per[entryClass[g]].push_back(cdiRecord(m[g].first, dev));
+    }
     for (size_t c = 0; c < classes.size(); c++) {
         std::vector<Rec> &devs = per[c];
         std::sort(devs.begin(), devs.end(), [](const Rec &a, const Rec &b) { return a.index < b.index; });
         const char *kind = classes[c].cdiKind.c_str();
         size_t len = 0;
-        int32_t rc = emit(ctx_, fmt, kind, devs.data(), devs.size(), nullptr, 0, &len);
+        auto *fn = emit;
+        if constexpr (std::is_same<Rec, kxpu_cdidev>::value)
+            if (classes[c].vfioCdev) fn = kxpu_cdi_emit_cdev;
+        int32_t rc = fn(ctx_, fmt, kind, devs.data(), devs.size(), nullptr, 0, &len);
         if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, what, rc);
         std::vector<uint8_t> doc(len ? len : 1);
-        rc = emit(ctx_, fmt, kind, devs.data(), devs.size(), doc.data(), len, &len);
+        rc = fn(ctx_, fmt, kind, devs.data(), devs.size(), doc.data(), len, &len);
         if (rc != KXPU_OK) return kxfail(ctx_, what, rc);
         const std::string file_path = cdiConfigPath + classes[c].cdiFileStem + (fmt == KXPU_FMT_YAML ? ".yaml" : ".json");  // spec.go:92
         bool written = false;
@@ -1336,6 +1408,15 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         }
         dp.devpluginName = devpluginName;
         dp.devicePath = "/dev/vfio/";                                                          // :105
+        if (xpuClasses[dp.xpuClass].vfioCdev) {  // every member's cdev node
+            dp.devicePath = "/dev/vfio/devices/";
+            for (const auto &g : iommuMap) {
+                if (std::find(kv.second.begin(), kv.second.end(), g.first) == kv.second.end()) continue;
+                std::vector<std::string> &nodes = dp.nodes[g.first];
+                for (const NvidiaGpuDevice &d : g.second)
+                    if (d.cdev >= 0) nodes.push_back("vfio" + std::to_string(d.cdev));
+            }
+        }
         dp.socketPath = std::string(kDevicePluginPath) + "kata-xpu-" + devpluginName + ".sock";  // generic:76
         dp.deviceKey = kv.first;
         devicePlugins.push_back(std::move(dp));
@@ -1494,8 +1575,17 @@ void Plugin::previousEntries(const std::vector<XpuClass> &classes,
         }
         std::vector<Rec> recs(doc.size() / KXPU_CDI_FRAG_MIN + 1);
         size_t n = 0;
-        const int32_t rc = parse(ctx_, KXPU_FMT_YAML, classes[c].cdiKind.c_str(), reinterpret_cast<const uint8_t *>(doc.data()),
-                                 doc.size(), recs.data(), recs.size(), &n);
+        auto parseWith = [&](decltype(parse) fn) {
+            return fn(ctx_, KXPU_FMT_YAML, classes[c].cdiKind.c_str(), reinterpret_cast<const uint8_t *>(doc.data()), doc.size(),
+                      recs.data(), recs.size(), &n);
+        };
+        int32_t rc;
+        if constexpr (std::is_same<Rec, kxpu_cdidev>::value) {  // the layout the class uses now, then the other one
+            rc = parseWith(classes[c].vfioCdev ? kxpu_cdi_parse_cdev : kxpu_cdi_parse);
+            if (rc == KXPU_E_INVALID) rc = parseWith(classes[c].vfioCdev ? kxpu_cdi_parse : kxpu_cdi_parse_cdev);
+        } else {
+            rc = parseWith(parse);
+        }
         if (rc != KXPU_OK) {
             rw.fallback = path + ": not a CDI spec this plugin writes (" + kxpu_strerror(rc) + ": " + kxpu_last_error(ctx_) + ")";
             break;
@@ -1676,8 +1766,9 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         for (size_t i = 0; same && i < cur.size(); i++)
             same = cur[i].ID == w.devs[i].ID && cur[i].Health == w.devs[i].Health && cur[i].numa == w.devs[i].numa &&
                    cur[i].pcieNode == w.devs[i].pcieNode && cur[i].blocker == w.devs[i].blocker && cur[i].aer == w.devs[i].aer;
-        if (!same) {
+        if (!same || devicePlugins[at].nodes != w.nodes) {  // changed cdev nodes: the watcher must follow them
             cur = std::move(w.devs);
+            devicePlugins[at].nodes = std::move(w.nodes);
             report.changedPlugins.push_back(at);
         }
     }
@@ -1769,6 +1860,8 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
             const std::string &want = xpuClasses[dev.xpuClass].vendor;  // the device's class
             if (!readIDFromFile(basePath, dev.addr, "vendor", vendor) || trimID(vendor) != want)  // :334-338
                 return fail("invalid allocation request: unknown device: " + dev.addr);
+            if (xpuClasses[c].vfioCdev && readVfioCdev(dev.addr) != dev.cdev)  // cdev numbers are reused across re-binds
+                return fail("invalid allocation request: the VFIO cdev of " + dev.addr + " changed since discovery");
             devIndexes.push_back(dev.index);  // :340
         }
     }
@@ -2153,16 +2246,24 @@ static std::string joinPath(const std::string &dir, const std::string &name) {
     return dir.back() == '/' ? dir + name : dir + "/" + name;
 }
 
+std::vector<std::string> HealthWatcher::nodesOf(const std::string &id) const {
+    auto it = dp_.nodes.find(id);
+    return it == dp_.nodes.end() ? std::vector<std::string>{id} : it->second;
+}
+
 Error HealthWatcher::start() {
     fd_ = inotify_init1(IN_NONBLOCK | IN_CLOEXEC);  // fsnotify.NewWatcher (:396)
     if (fd_ < 0) return fail(std::string("Unable to create fsnotify watcher: ") + strerror(errno));
     // fsnotify's inotify backend adds every path with this mask; only the ops healthCheck looks at matter
     const uint32_t mask = IN_DELETE_SELF | IN_MOVE_SELF | IN_ATTRIB | IN_MODIFY;
     for (const Device &dev : dp_.devs) {  // :421-430
-        const std::string devicePath = joinPath(dp_.devicePath, dev.ID);
-        int wd = inotify_add_watch(fd_, devicePath.c_str(), mask);
-        if (wd < 0) return fail("Unable to add device path to fsnotify watcher: " + devicePath + ": " + strerror(errno));
-        wdToId_[wd] = dev.ID;
+        for (const std::string &node : nodesOf(dev.ID)) {
+            const std::string devicePath = joinPath(dp_.devicePath, node);
+            int wd = inotify_add_watch(fd_, devicePath.c_str(), mask);
+            if (wd < 0) return fail("Unable to add device path to fsnotify watcher: " + devicePath + ": " + strerror(errno));
+            wdToId_[wd] = dev.ID;
+            wdToNode_[wd] = node;
+        }
     }
     if (watchCreates_) {
         dirWd_ = inotify_add_watch(fd_, dp_.devicePath.c_str(), IN_CREATE | IN_MOVED_TO);
@@ -2171,28 +2272,37 @@ Error HealthWatcher::start() {
     return Error();
 }
 
+// follows the device list and, for cdev plugins, the node names: a watch whose (ID, node) left is dropped
 Error HealthWatcher::resync() {
     if (fd_ < 0) return fail("health watcher not started");
-    std::map<std::string, bool> want;
-    for (const Device &dev : dp_.devs) want[dev.ID] = true;
-    std::map<std::string, bool> have;
+    std::set<std::pair<std::string, std::string>> want;
+    for (const Device &dev : dp_.devs)
+        for (const std::string &node : nodesOf(dev.ID)) want.insert({dev.ID, node});
+    std::set<std::pair<std::string, std::string>> have;
     for (auto it = wdToId_.begin(); it != wdToId_.end();) {
-        if (!want.count(it->second)) {
+        const std::pair<std::string, std::string> key{it->second, wdToNode_[it->first]};
+        if (!want.count(key)) {
             inotify_rm_watch(fd_, it->first);  // the IN_IGNORED that follows finds no entry
+            wdToNode_.erase(it->first);
             it = wdToId_.erase(it);
         } else {
-            have[it->second] = true;
+            have.insert(key);
             ++it;
         }
     }
     Error err;
     const uint32_t mask = IN_DELETE_SELF | IN_MOVE_SELF | IN_ATTRIB | IN_MODIFY;
     for (const auto &kv : want) {
-        if (have.count(kv.first)) continue;
-        const std::string devicePath = joinPath(dp_.devicePath, kv.first);
+        if (have.count(kv)) continue;
+        const std::string devicePath = joinPath(dp_.devicePath, kv.second);
         int wd = inotify_add_watch(fd_, devicePath.c_str(), mask);
-        if (wd < 0) { err = fail("Unable to add device path to fsnotify watcher: " + devicePath + ": " + strerror(errno)); continue; }
+        if (wd < 0) {
+            err = fail("Unable to add device path to fsnotify watcher: " + devicePath + ": " + strerror(errno));
+            if (dp_.nodes.count(kv.first)) setHealth(kv.first, kUnhealthy);  // a cdev node that is not there
+            continue;
+        }
         wdToId_[wd] = kv.first;
+        wdToNode_[wd] = kv.second;
     }
     return err;
 }
@@ -2223,22 +2333,25 @@ int HealthWatcher::poll(int timeout_ms) {
             if (ev->wd == dirWd_ && ev->len > 0) {
                 // fsnotify.Create of devicePath/<name> (:441-443)
                 const std::string name(ev->name);
-                for (const Device &d : dp_.devs)
-                    if (d.ID == name) {
-                        changed += setHealth(name, kHealthy);
-                        // the old watch died with the old inode: watch the new file like a restarted healthCheck would
-                        int wd = inotify_add_watch(fd_, joinPath(dp_.devicePath, name).c_str(),
-                                                   IN_DELETE_SELF | IN_MOVE_SELF | IN_ATTRIB | IN_MODIFY);
-                        if (wd >= 0) wdToId_[wd] = name;
-                        break;
-                    }
+                for (const Device &d : dp_.devs) {
+                    const std::vector<std::string> nodes = nodesOf(d.ID);
+                    if (std::find(nodes.begin(), nodes.end(), name) == nodes.end()) continue;
+                    // the old watch died with the old inode: watch the new file like a restarted healthCheck would
+                    int wd = inotify_add_watch(fd_, joinPath(dp_.devicePath, name).c_str(),
+                                               IN_DELETE_SELF | IN_MOVE_SELF | IN_ATTRIB | IN_MODIFY);
+                    if (wd >= 0) { wdToId_[wd] = d.ID; wdToNode_[wd] = name; }
+                    bool all = true;  // a group is Healthy again only when every member's node is back
+                    for (const std::string &n : nodes) all &= access(joinPath(dp_.devicePath, n).c_str(), F_OK) == 0;
+                    if (all) changed += setHealth(d.ID, kHealthy);
+                    break;
+                }
                 continue;
             }
             auto it = wdToId_.find(ev->wd);
             if (it == wdToId_.end()) continue;
             if (ev->mask & (IN_DELETE_SELF | IN_MOVE_SELF))  // fsnotify.Remove / fsnotify.Rename (:444-448)
                 changed += setHealth(it->second, kUnhealthy);
-            if (ev->mask & IN_IGNORED) wdToId_.erase(it);   // the kernel dropped the watch (file gone)
+            if (ev->mask & IN_IGNORED) { wdToNode_.erase(ev->wd); wdToId_.erase(it); }  // the kernel dropped the watch (file gone)
         }
     }
     return changed;
@@ -2311,8 +2424,9 @@ static bool parseClasses(const char *spec, std::vector<device_plugin::XpuClass> 
             if (c == std::string::npos) break;
             a = c + 1;
         }
-        if (f.size() != 5) return false;
+        if (f.size() != 5 && !(f.size() == 6 && f[5] == "cdev")) return false;
         out.push_back(device_plugin::XpuClass{f[0], f[1], f[2], f[3], f[4]});
+        out.back().vfioCdev = f.size() == 6;
     }
     return !out.empty();
 }
@@ -2331,6 +2445,66 @@ int kxh_gather_classes(const char *base_path, const char *classes, int fast, uns
     memcpy(out, recs.data(), recs.size() * sizeof(kxpu_devrec));
     return 0;
 }
+
+// CPU only: the raw gather under a class list ("...,cdev" marks a vfioCdev class) with the walk's cdev side array
+// (-1 = none or not read) and the number of vfio-dev/ directories listed
+int kxh_gather_cdev(const char *base_path, const char *classes, int fast, unsigned threads, kxpu_devrec *out, int64_t *cdevs,
+                    size_t cap, size_t *n, uint64_t *reads, char *err, size_t errcap) {
+    Plugin p(nullptr);
+    p.basePath = base_path;
+    if (!parseClasses(classes, p.xpuClasses)) { copy_out("malformed class list", err, errcap); return -1; }
+    std::vector<kxpu_devrec> recs;
+    std::vector<int64_t> cd;
+    device_plugin::Error e = fast ? p.gatherRecordsFast(recs, threads, nullptr, &cd) : p.gatherRecords(recs, nullptr, &cd);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    *n = recs.size();
+    *reads = p.cdevReads;
+    if (recs.size() > cap) return -2;
+    memcpy(out, recs.data(), recs.size() * sizeof(kxpu_devrec));
+    for (size_t i = 0; i < recs.size(); i++) cdevs[i] = cd.empty() ? -1 : cd[i];
+    return 0;
+}
+
+// CPU only: Plugin::checkVgpuClasses for these class lists
+int kxh_check_vgpu_classes(const char *classes, const char *vgpu_classes, char *err, size_t errcap) {
+    Plugin p(nullptr);
+    if (!parseClasses(classes, p.xpuClasses) || !parseClasses(vgpu_classes, p.vgpuClasses)) {
+        copy_out("malformed class list", err, errcap);
+        return -1;
+    }
+    device_plugin::Error e = p.checkVgpuClasses();
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    return 0;
+}
+
+// a plugin's devicePath and its cdev nodes: {"path": "...", "nodes": {"<id>": ["vfio<N>", ...]}, "blockers": {"<id>": "..."}}
+int kxh_plugin_nodes(void *h, int plugin_index, char *out, size_t cap) {
+    Plugin *p = (Plugin *)h;
+    if (plugin_index < 0 || (size_t)plugin_index >= p->devicePlugins.size()) return -1;
+    const device_plugin::GenericDevicePlugin &dp = p->devicePlugins[(size_t)plugin_index];
+    std::string o = "{\"path\":";
+    jstr(o, dp.devicePath);
+    o += ",\"nodes\":{";
+    bool first = true;
+    for (const auto &kv : dp.nodes) {
+        if (!first) o += ',';
+        first = false;
+        jstr(o, kv.first);
+        o += ":[";
+        for (size_t i = 0; i < kv.second.size(); i++) { if (i) o += ','; jstr(o, kv.second[i]); }
+        o += ']';
+    }
+    o += "},\"blockers\":{";
+    first = true;
+    for (const auto &d : dp.devs) {
+        if (d.blocker.empty()) continue;
+        if (!first) o += ',';
+        first = false;
+        jstr(o, d.ID); o += ':'; jstr(o, d.blocker);
+    }
+    return copy_out(o + "}}", out, cap);
+}
+uint64_t kxh_cdev_reads(void *h) { return ((Plugin *)h)->cdevReads; }
 
 // the class list of a plugin (xpuClasses seam)
 int kxh_set_classes(void *h, const char *classes) {

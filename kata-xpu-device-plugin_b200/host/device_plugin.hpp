@@ -31,6 +31,7 @@ struct NvidiaGpuDevice {
     std::string addr;    // PCI address of device
     uint64_t index;      // PCI device index on PCI bus
     size_t xpuClass = 0; // index into Plugin::xpuClasses of the class this function matched
+    int64_t cdev = -1;   // N of its VFIO cdev /dev/vfio/devices/vfio<N> (XpuClass::vfioCdev only); -1 = none
 };
 
 // One mediated device (vGPU) of the mdev walk: the mdevMap counterpart of NvidiaGpuDevice
@@ -82,6 +83,9 @@ struct GenericDevicePlugin {
     std::string devicePath;      // "/dev/vfio/" (device_plugin.go:105)
     std::vector<Device> devs;
     std::string deviceKey;       // the device id (passthrough) or type key (vgpu) the plugin serves; matches it on rediscovery
+    // XpuClass::vfioCdev only: device ID -> the node names under devicePath the health watcher watches (one per member,
+    // "vfio<N>"); an ID not listed is watched as devicePath/<ID>
+    std::map<std::string, std::vector<std::string>> nodes;
 };
 
 // pluginapi.ContainerAllocateResponse as Allocate fills it (generic_device_plugin.go:304-350)
@@ -122,6 +126,8 @@ class HealthWatcher {
     bool watchCreates_;
     int fd_ = -1, dirWd_ = -1;
     std::map<int, std::string> wdToId_;
+    std::map<int, std::string> wdToNode_;  // the node name each watch is on
+    std::vector<std::string> nodesOf(const std::string &id) const;
     uint64_t events_ = 0;
     int setHealth(const std::string &id, const char *health);
 };
@@ -169,6 +175,11 @@ struct XpuClass {
     // DRA driver name that publishes this class's IOMMU groups as ResourceSlices (Plugin::ResourceSlices, or
     // Plugin::VgpuResourceSlices for a vGPU class); empty: the class is not published
     std::string draDriver{};
+    // passthrough only (a vGPU class with it is refused): the class's functions are reached through their VFIO cdevs.  The
+    // gathers read <bdf>/vfio-dev/ of every function that matches the class, the CDI spec names /dev/vfio/devices/vfio<N>
+    // (kxpu_cdi_emit_cdev), the health watcher watches those nodes, and a group with a member without a cdev is treated
+    // like a group that is not viable.  false: nothing under vfio-dev/ is opened and every output is as without it.
+    bool vfioCdev = false;
 };
 XpuClass defaultXpuClass();  // {"10de", "vfio-pci", "nvidia.com", "nvidia.com/gpu", "cdi-vfio-xxxx"}
 
@@ -221,6 +232,8 @@ struct PciWalk {
     std::vector<uint64_t> nodeKey;
     std::vector<uint8_t> nodeDepth;
     uint32_t nNodes = 0;
+    // some class has vfioCdev: per record, N of its VFIO cdev, -1 = none or not read
+    std::vector<int64_t> cdevs;
 };
 struct MdevWalk {
     std::vector<kxpu_mdevrec> recs;
@@ -339,6 +352,8 @@ class Plugin {
     const ResumeReport &resumeReport() const { return resume_; }
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
     uint64_t aerReads = 0;  // aer_dev_* files read (tests, metrics)
+    uint64_t cdevReads = 0;  // vfio-dev/ directories listed (tests, metrics)
+    bool cdevEnabled() const;  // some passthrough class has vfioCdev
 
     // ---- state (device_plugin.go:31,34)
     OrderedMap<std::vector<NvidiaGpuDevice>> iommuMap;  // group id -> devices
@@ -454,20 +469,29 @@ class Plugin {
 
     // raw gather only (no GPU): exposed for CPU tests of the walk.  paths (pcieTopologyAware only, else left empty):
     // one kxpu_pcipath per record, same index
-    Error gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pcipath> *paths = nullptr);
+    // cdevs (cdevEnabled only, else left empty): per record N of its VFIO cdev, -1 = none or not read
+    Error gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pcipath> *paths = nullptr,
+                        std::vector<int64_t> *cdevs = nullptr);
     // the same records, read with openat / readlinkat relative to basePath by several threads
     // (SURVEY 8(f) row 2); falls back to gatherRecords when a seam was replaced.  threads = 0: automatic
-    Error gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads = 0, std::vector<kxpu_pcipath> *paths = nullptr);
+    Error gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads = 0, std::vector<kxpu_pcipath> *paths = nullptr,
+                            std::vector<int64_t> *cdevs = nullptr);
+    // the cdev of <basePath>/<bdf>: N when vfio-dev/ holds exactly one entry besides . and .., and it is "vfio" followed by
+    // a canonical decimal below 2^32; -1 for anything else (never an error)
+    int64_t readVfioCdev(const std::string &bdf);
     // raw gather of mdevBasePath under vgpuClasses (no GPU): one record per entry, lexical order.  w (vgpuDraEnabled
     // only, else left empty): the walk's parentDevice and pcieRoot, one per record
     Error gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w = nullptr);
+    // the vGPU class list against the passthrough one (distinct CDI kinds and file stems, no vfioCdev); createMdevMap runs it
+    Error checkVgpuClasses() const;
 
   private:
     kxpu_ctx *ctx_;
     kxpu_table *table_ = nullptr;
     Error ensureTable();
     size_t classOfGroup(const std::string &group) const;
-    Error checkVgpuClasses() const;
+    Error gatherRecordsFastWalk(std::vector<kxpu_devrec> &recs, unsigned threads, std::vector<kxpu_pcipath> *paths);
+    void readCdevs(const std::vector<kxpu_devrec> &recs, std::vector<int64_t> *cdevs);
     // one CDI spec per class: the devices of m whose entry has that class (entryClass, same positions as m)
     template <typename Dev, typename Rec>
     Error generateClassSpecs(const std::vector<XpuClass> &classes, const OrderedMap<std::vector<Dev>> &m,
