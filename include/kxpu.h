@@ -72,7 +72,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
 #define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's and kxpu_pcie_tree's kernels: the slot holds the most recent call's */
-#define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev]: decode, re-emit and compare of the most recent call */
+#define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
 #define KXPU_T_COUNT    8
@@ -721,6 +721,44 @@ int32_t kxpu_cdi_emit_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, cons
  * kxpu_cdi_parse. */
 int32_t kxpu_cdi_parse_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
                             kxpu_cdidev *out, size_t cap, size_t *n);
+
+/* ------------------------------- CDI specs naming the VFIO cdevs of vGPUs (additions to ABI v14) */
+
+/* These two calls were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym), as the ctypes
+ * binding and the Go shim do.  An mdev can be opened through its own VFIO character device like a PCI function:
+ *   [assumed] on a kernel with CONFIG_VFIO_DEVICE_CDEV=y, an mdev whose vendor driver registers a VFIO device gets
+ *             /dev/vfio/devices/vfio<N>, and <mdevBasePath>/<uuid>/vfio-dev/ holds the one entry vfio<N>, the layout of
+ *             a PCI function.  With CONFIG_IOMMUFD the kernel requires iommufd ops of every VFIO driver, so a working
+ *             vGPU driver has a cdev; only the operator knows whether the node's vGPU driver does, so a vGPU class
+ *             opts in on its own;
+ *   [assumed] mdev and PCI cdev numbers come from one number space and are reused: re-creating an mdev with the same
+ *             UUID can give it another N;
+ *   [assumed] Kata attaches an mdev cdev through QEMU's iommufd backend, as it does a function's, so the spec names no
+ *             /dev/iommu node (the runtime opens it itself). */
+
+/* One accepted vGPU of a class served through VFIO cdevs.  80 bytes (16-byte strides for the kernels' vector loads). */
+typedef struct kxpu_mdevcdev {
+    kxpu_mdevcdi dev;        /* exactly what kxpu_cdi_emit_mdev reads                    */
+    uint32_t     vfio_cdev;  /* N of /dev/vfio/devices/vfio<N>; every uint32 is valid    */
+    uint32_t     reserved[3];/* ignored by the emitter, written 0 by the parser           */
+} kxpu_mdevcdev;
+
+/* kxpu_cdi_emit_mdev's document for devs[i].dev, byte for byte, except that the device node of device i is
+ * /dev/vfio/devices/vfio<N> with N = devs[i].vfio_cdev in place of /dev/vfio/<g>.  The four annotations (cdi.k8s.io/vfio<g>
+ * and mdev: <uuid> included), head, tail, zero-device form, device order, kind domain, uuid and parent refusals
+ * (KXPU_E_UNSUPPORTED) and sizing protocol are kxpu_cdi_emit_mdev's.
+ * GPU: the kernel of kxpu_cdi_emit_mdev with the node literal and number compiled in; the longest fragment is 12 bytes
+ * longer (492), and the tile still runs three CTAs per SM (DESIGN.md K6).  Timed under KXPU_T_EMIT. */
+int32_t kxpu_cdi_emit_mdev_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_mdevcdev *devs, size_t n,
+                                uint8_t *out, size_t cap, size_t *len);
+
+/* The inverse of kxpu_cdi_emit_mdev_cdev: KXPU_OK with *n records exactly when kxpu_cdi_emit_mdev_cdev(format, kind, out,
+ * *n) returns doc byte for byte; vfio_cdev holds each device's N and reserved is 0.  A document of kxpu_cdi_emit_mdev,
+ * kxpu_cdi_emit_kind or kxpu_cdi_emit_cdev is KXPU_E_INVALID here (and each of their parsers refuses this call's
+ * documents); the zero-device documents are the same bytes in every layout, and every parser returns *n = 0 for them.
+ * KXPU_CDI_FRAG_MIN still bounds *n.  Everything else as kxpu_cdi_parse_mdev. */
+int32_t kxpu_cdi_parse_mdev_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
+                                 kxpu_mdevcdev *out, size_t cap, size_t *n);
 
 /* ------------------------------------------------------ S5: Allocate names */
 

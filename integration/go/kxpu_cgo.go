@@ -666,6 +666,69 @@ func (k *kxpu) cdiParseCdev(format int, doc []byte, kind string) ([]C.kxpu_cdide
 	return out[:n], nil
 }
 
+// VFIO cdevs of vGPUs (additions to ABI v14, detected by symbol).  cdiEmitMdevCdev writes cdiEmitMdev's document for
+// devs[i].dev with each device's node /dev/vfio/devices/vfio<N>, N = devs[i].vfio_cdev (read from
+// <mdevBasePath>/<uuid>/vfio-dev/vfio<N>); cdiParseMdevCdev is its inverse and returns N in vfio_cdev.  Each of the four
+// parsers refuses the other layouts' documents, except the zero-device document, which all of them accept.
+func (k *kxpu) cdiEmitMdevCdev(format int, kind string, devs []C.kxpu_mdevcdev) ([]byte, error) {
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	var p *C.kxpu_mdevcdev
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	var n C.size_t
+	C.kxpu_cdi_emit_mdev_cdev(k.ctx, C.int32_t(format), ck, p, C.size_t(len(devs)), nil, 0, &n) // sizing call
+	buf := make([]byte, n+1)
+	err := kxCheck(k.ctx, "kxpu_cdi_emit_mdev_cdev", C.kxpu_cdi_emit_mdev_cdev(k.ctx, C.int32_t(format), ck, p,
+		C.size_t(len(devs)), (*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n))
+	return buf[:n], err
+}
+
+func (k *kxpu) cdiParseMdevCdev(format int, doc []byte, kind string) ([]C.kxpu_mdevcdev, error) {
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	out := make([]C.kxpu_mdevcdev, len(doc)/C.KXPU_CDI_FRAG_MIN+1)
+	var n C.size_t
+	var dp *C.uint8_t
+	if len(doc) > 0 {
+		dp = (*C.uint8_t)(unsafe.Pointer(&doc[0]))
+	}
+	err := kxCheck(k.ctx, "kxpu_cdi_parse_mdev_cdev", C.kxpu_cdi_parse_mdev_cdev(k.ctx, C.int32_t(format), ck, dp,
+		C.size_t(len(doc)), &out[0], C.size_t(len(out)), &n))
+	if err != nil {
+		return nil, err
+	}
+	return out[:n], nil
+}
+
+// cdiParseVgpuSpec: the records of a vGPU class's previous spec for the restart resume (resumeWalk's prev entries).  It
+// is parsed with the layout the class uses now (mdevCdev: the cdev layout), then with the other one, so a class that
+// switched mdevCdev across the restart keeps its indices; only the kxpu_mdevcdi part (uuid, group, index) is returned.
+func (k *kxpu) cdiParseVgpuSpec(doc []byte, kind string, mdevCdev bool) ([]C.kxpu_mdevcdi, error) {
+	viaCdev := func() ([]C.kxpu_mdevcdi, error) {
+		recs, err := k.cdiParseMdevCdev(C.KXPU_FMT_YAML, doc, kind)
+		if err != nil {
+			return nil, err
+		}
+		out := make([]C.kxpu_mdevcdi, len(recs))
+		for i := range recs {
+			out[i] = recs[i].dev
+		}
+		return out, nil
+	}
+	viaGroup := func() ([]C.kxpu_mdevcdi, error) { return k.cdiParseMdev(C.KXPU_FMT_YAML, doc, kind) }
+	first, second := viaGroup, viaCdev
+	if mdevCdev {
+		first, second = viaCdev, viaGroup
+	}
+	recs, err := first()
+	if err != nil && strings.Contains(err.Error(), "invalid") {
+		recs, err = second()
+	}
+	return recs, err
+}
+
 // The index state file of the restart resume: <cdiConfigPath>.kata-xpu-cdi-index, "pci <next>\nmdev <next>\n".  The CDI
 // cache loads only *.json / *.yaml.  Write it (tmp + fsync + rename, only when its bytes change) whenever a next index
 // grows, before any spec that names the new indices.

@@ -43,6 +43,9 @@ MDEVREC_DTYPE = np.dtype([("uuid", "S36"), ("parent", "S16"), ("parent_vendor_tx
                           ("flags", "u1"), ("reserved0", "u1"), ("reserved1", "<u4")])
 MDEVCDI_DTYPE = np.dtype([("uuid", "S36"), ("iommu_group", "<u4"), ("parent", "S16"), ("index", "<u8")])
 assert MDEVREC_DTYPE.itemsize == 128 and MDEVCDI_DTYPE.itemsize == 64
+# kxpu_mdevcdev: a vGPU of a class served through VFIO cdevs (an addition to ABI v14)
+MDEVCDEV_DTYPE = np.dtype([("dev", MDEVCDI_DTYPE), ("vfio_cdev", "<u4"), ("reserved", "<u4", (3,))])
+assert MDEVCDEV_DTYPE.itemsize == 80 and MDEVCDEV_DTYPE.fields["vfio_cdev"][1] == 64
 # kxpu_snaprec / kxpu_reconcile_counts (runtime rediscovery, ABI v6)
 SNAPREC_DTYPE = np.dtype([("key", "S40"), ("iommu_group", "<u4"), ("klass", "<u4"), ("tag", "<u8"), ("index", "<u8")])
 RC_COUNTS_DTYPE = np.dtype([("n_kept", "<u8"), ("n_new", "<u8"), ("n_changed", "<u8"), ("n_retired", "<u8"),
@@ -94,7 +97,7 @@ ABI_SYMBOLS = [
     "kxpu_reconcile", "kxpu_pcie_tree", "kxpu_preferred_allocation_pcie", "kxpu_classify_viable",
     "kxpu_dra_slices", "kxpu_dra_slices_mdev", "kxpu_dra_slices_taint", "kxpu_dra_slices_mdev_taint",
     "kxpu_aer_health", "kxpu_dra_slices_taints", "kxpu_dra_slices_mdev_taints", "kxpu_cdi_parse", "kxpu_cdi_parse_mdev",
-    "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev",
+    "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev", "kxpu_cdi_emit_mdev_cdev", "kxpu_cdi_parse_mdev_cdev",
 ]
 
 
@@ -207,6 +210,8 @@ def load_library():
         "kxpu_cdi_parse_mdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_cdi_emit_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_cdi_parse_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_cdi_emit_mdev_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_cdi_parse_mdev_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_dra_slices_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                          C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_mdev_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
@@ -687,6 +692,11 @@ class Kxpu:
         (CDIDEV_DTYPE devices, N of /dev/vfio/devices/vfio<N> in the CDEV_FIELD field; kind bytes or str)."""
         return self._emit_sized(self.L.kxpu_cdi_emit_cdev, CDIDEV_DTYPE, fmt, devs, kind)
 
+    def cdi_emit_mdev_cdev(self, fmt, devs, kind):
+        """kxpu_cdi_emit_mdev_cdev: the CDI spec of a vGPU class whose mdevs are reached through their VFIO cdevs
+        (MDEVCDEV_DTYPE devices; kind bytes or str)."""
+        return self._emit_sized(self.L.kxpu_cdi_emit_mdev_cdev, MDEVCDEV_DTYPE, fmt, devs, kind)
+
     def _emit_sized(self, fn, dtype, fmt, devs, kind):
         """the two-call sizing protocol: out = NULL gives the length, the second call writes the document"""
         devs = np.ascontiguousarray(devs)
@@ -809,13 +819,20 @@ class Kxpu:
         """kxpu_cdi_parse_cdev: the CDIDEV_DTYPE records (N in CDEV_FIELD) of a spec kxpu_cdi_emit_cdev wrote."""
         return self._parse(self.L.kxpu_cdi_parse_cdev, CDIDEV_DTYPE, fmt, doc, kind)
 
+    def cdi_parse_mdev_cdev(self, fmt, doc, kind):
+        """kxpu_cdi_parse_mdev_cdev: the MDEVCDEV_DTYPE records of a spec kxpu_cdi_emit_mdev_cdev wrote."""
+        return self._parse(self.L.kxpu_cdi_parse_mdev_cdev, MDEVCDEV_DTYPE, fmt, doc, kind)
+
     def cdi_parse_raw(self, fmt, doc, kind, cap, mdev=False, offset=0, cdev=False):
         """The bare call: doc placed at `offset` bytes past a 16-byte aligned host buffer, out of `cap` records.
         Returns (status, n, records) with n and the records as the call left them (n = -1: not stored).
-        mdev: kxpu_cdi_parse_mdev, cdev: kxpu_cdi_parse_cdev, neither: kxpu_cdi_parse."""
-        assert not (mdev and cdev)
-        dtype = MDEVCDI_DTYPE if mdev else CDIDEV_DTYPE
-        fn = self.L.kxpu_cdi_parse_mdev if mdev else self.L.kxpu_cdi_parse_cdev if cdev else self.L.kxpu_cdi_parse
+        mdev and cdev: kxpu_cdi_parse_mdev_cdev, mdev: kxpu_cdi_parse_mdev, cdev: kxpu_cdi_parse_cdev, neither:
+        kxpu_cdi_parse."""
+        if mdev and cdev:
+            dtype, fn = MDEVCDEV_DTYPE, self.L.kxpu_cdi_parse_mdev_cdev
+        else:
+            dtype = MDEVCDI_DTYPE if mdev else CDIDEV_DTYPE
+            fn = self.L.kxpu_cdi_parse_mdev if mdev else self.L.kxpu_cdi_parse_cdev if cdev else self.L.kxpu_cdi_parse
         buf = np.zeros(len(doc) + offset + 16, np.uint8)
         base = (-buf.ctypes.data) % 16
         buf = buf[base:]

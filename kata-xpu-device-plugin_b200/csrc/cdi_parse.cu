@@ -1,4 +1,4 @@
-// cdi_parse.cu -- K13: kxpu_cdi_parse / kxpu_cdi_parse_mdev, the inverse of the CDI spec emitter (emit.cu, K6).
+// cdi_parse.cu -- K13: kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev], the inverse of the CDI spec emitter (emit.cu, K6).
 //
 // A call accepts a document exactly when the emitter, given the records it decodes, writes the same bytes.  It runs in
 // two steps:
@@ -22,17 +22,23 @@ namespace kxparse {
 constexpr int PT = 8192;         // document bytes per CTA
 constexpr int PARSE_THREADS = 256;
 constexpr int ROWS = PT / PARSE_THREADS;  // positions per thread, one row of 256 consecutive positions each
-constexpr int HALO = 512;        // >= the longest fragment of any layout plus the start pattern
 constexpr int LEAD = 16;         // bytes staged in front of the tile: the '\n' before a start at the tile's first byte
-constexpr int WIN = LEAD + PT + HALO;
 constexpr int PAT_MAX = 32;
-constexpr int LAYOUT_PCI = KX_CDI_PCI, LAYOUT_MDEV = KX_CDI_MDEV, LAYOUT_CDEV = KX_CDI_CDEV;
-static_assert(HALO >= KX_CDI_FRAG_MAX + PAT_MAX, "a fragment that starts in the tile must end inside the window");
+constexpr int LAYOUT_PCI = KX_CDI_PCI, LAYOUT_MDEV = KX_CDI_MDEV, LAYOUT_CDEV = KX_CDI_CDEV,
+              LAYOUT_MDEV_CDEV = KX_CDI_MDEV_CDEV;
+// bytes staged past the tile: >= the layout's longest fragment plus the start pattern, in whole 16-byte words
+template <int LAYOUT> constexpr int HALO = LAYOUT == LAYOUT_MDEV_CDEV ? 528 : 512;
+constexpr int HALO_MAX = HALO<LAYOUT_MDEV_CDEV>;  // the host pads every document for the largest halo
+static_assert(HALO<LAYOUT_PCI> >= KX_CDI_FRAG_MAX + PAT_MAX, "a fragment that starts in the tile must end inside the window");
+static_assert(HALO<LAYOUT_MDEV_CDEV> >= KX_CDI_FRAG_MAX_MDEV_CDEV + PAT_MAX && HALO<LAYOUT_MDEV_CDEV> % 16 == 0,
+              "a fragment that starts in the tile must end inside the window");
+static_assert(HALO_MAX >= HALO<LAYOUT_PCI>, "the host padding must cover every layout's window");
+template <int LAYOUT> constexpr int WIN = LEAD + PT + HALO<LAYOUT>;
 
 struct ParseParams {
-    const uint8_t *doc;           // padded with zeros to a whole tile plus HALO + LEAD bytes
+    const uint8_t *doc;           // padded with zeros to a whole tile plus HALO_MAX + LEAD bytes
     unsigned long long len;
-    void *recs;                   // kxpu_cdidev[cap] or kxpu_mdevcdi[cap]
+    void *recs;                   // kxpu_cdidev[cap], kxpu_mdevcdi[cap] or kxpu_mdevcdev[cap]
     unsigned long long cap;       // records beyond it are counted, not written
     unsigned long long *state;    // tile status words (scan.cuh look-back)
     uint32_t epoch;
@@ -41,10 +47,12 @@ struct ParseParams {
     uint32_t l1, l2, l3, lm;      // literal 1, literal 2, literal 3 (with the kind), literal 4 (mdev: the annotation's
                                   // opening, cdev: the node literal)
     uint8_t pat[PAT_MAX];
+    uint32_t l9;                  // mdev cdev: the literal after the uuid, which ends in the node literal
 };
 
+template <int LAYOUT>
 struct ParseSmem {
-    alignas(16) uint8_t win[WIN];
+    alignas(16) uint8_t win[WIN<LAYOUT>];
     uint32_t mask[ROWS * (PARSE_THREADS / 32)];  // row-major: mask[row * 8 + warp] = the warp's ballot in that row
     uint32_t base[ROWS * (PARSE_THREADS / 32)];  // exclusive count of starts in front of that row-warp inside the tile
     unsigned long long tile_base;
@@ -54,20 +62,21 @@ __device__ __forceinline__ bool is_digit(uint8_t c) { return c >= '0' && c <= '9
 
 template <int FMT, int LAYOUT>
 __global__ void __launch_bounds__(PARSE_THREADS) k_cdi_decode(const __grid_constant__ ParseParams P) {
-    __shared__ ParseSmem S;
+    constexpr int HALO_L = HALO<LAYOUT>, WIN_L = WIN<LAYOUT>;
+    __shared__ ParseSmem<LAYOUT> S;
     const uint32_t tid = threadIdx.x, lane = tid & 31u, w = tid >> 5;
     const unsigned long long t0 = (unsigned long long)blockIdx.x * PT;
     // ---- stage [t0 - LEAD, t0 + PT + HALO): the buffer is padded, so only the front of tile 0 needs a guard
     {
         const uint4 *src = reinterpret_cast<const uint4 *>(P.doc + t0) - 1;
         uint4 *dst = reinterpret_cast<uint4 *>(S.win);
-        for (uint32_t k = tid; k < (uint32_t)(WIN / 16); k += PARSE_THREADS)
+        for (uint32_t k = tid; k < (uint32_t)(WIN_L / 16); k += PARSE_THREADS)
             dst[k] = (blockIdx.x == 0 && k == 0) ? make_uint4(0, 0, 0, 0) : src[k];
     }
     __syncthreads();
     // bytes at or past the document's end read as 0 (the padding is zero and the window ends with the halo)
     const unsigned long long rest = P.len - t0;  // > 0: every tile holds a byte of the document
-    const uint32_t wend = (uint32_t)(LEAD + (rest < (unsigned long long)(PT + HALO) ? rest : (unsigned long long)(PT + HALO)));
+    const uint32_t wend = (uint32_t)(LEAD + (rest < (unsigned long long)(PT + HALO_L) ? rest : (unsigned long long)(PT + HALO_L)));
     auto at = [&](uint32_t q) -> uint8_t { return q < wend ? S.win[q] : (uint8_t)0; };
     // ---- starts: row r holds positions t0 + r * 256 + tid
     for (uint32_t r = 0; r < (uint32_t)ROWS; r++) {
@@ -142,7 +151,16 @@ __global__ void __launch_bounds__(PARSE_THREADS) k_cdi_decode(const __grid_const
             d.iommu_group = group;
             memcpy(d.parent, bdf, 16);
             d.index = index;
-            static_cast<kxpu_mdevcdi *>(P.recs)[slot] = d;
+            if constexpr (LAYOUT == LAYOUT_MDEV_CDEV) {  // N follows the uuid and the literal after it
+                q += 36u + P.l9;
+                uint32_t node = 0;
+                for (uint32_t k = 0; k < 10u && is_digit(at(q)); k++, q++) node = node * 10u + (at(q) - '0');
+                kxpu_mdevcdev *c = static_cast<kxpu_mdevcdev *>(P.recs) + slot;
+                c->dev = d;
+                *reinterpret_cast<uint4 *>(&c->vfio_cdev) = make_uint4(node, 0u, 0u, 0u);  // vfio_cdev, reserved[3]
+            } else {
+                static_cast<kxpu_mdevcdi *>(P.recs)[slot] = d;
+            }
         }
     }
 }
@@ -174,10 +192,10 @@ static void decode_launch(kxpu_ctx *ctx, uint32_t tiles, const ParseParams &P) {
     k_cdi_decode<FMT, LAYOUT><<<tiles, PARSE_THREADS, 0, ctx->stream>>>(P);
 }
 
-// LAYOUT_MDEV: out is kxpu_mdevcdi[cap], else kxpu_cdidev[cap]
+// LAYOUT_MDEV: out is kxpu_mdevcdi[cap], LAYOUT_MDEV_CDEV: kxpu_mdevcdev[cap], else kxpu_cdidev[cap]
 static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len, void *out,
                          size_t cap, size_t *n, int layout, const char *what) {
-    const bool mdev = layout == LAYOUT_MDEV;
+    const bool mdev = layout == LAYOUT_MDEV || layout == LAYOUT_MDEV_CDEV;
     if (!ctx || !n || !kind || (len && !doc) || (cap && !out) || (format != KXPU_FMT_YAML && format != KXPU_FMT_JSON))
         return KXPU_E_INVALID;
     if (len >= (1ull << 32)) { KX_SET_ERR(ctx, "%s: a document of 2^32 bytes or more", what); return KXPU_E_UNSUPPORTED; }
@@ -199,9 +217,10 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
     const size_t fixed = part[6].size() + part[7].size();
     if (len < fixed + frag_min) { KX_SET_ERR(ctx, "%s: not a document the emitter writes", what); return KXPU_E_INVALID; }
     const size_t max_n = (len - fixed) / frag_min;  // no valid document of len bytes holds more devices
-    const size_t rec_bytes = mdev ? sizeof(kxpu_mdevcdi) : sizeof(kxpu_cdidev);
+    const size_t rec_bytes = layout == LAYOUT_MDEV ? sizeof(kxpu_mdevcdi)
+                             : layout == LAYOUT_MDEV_CDEV ? sizeof(kxpu_mdevcdev) : sizeof(kxpu_cdidev);
     const uint32_t tiles = (uint32_t)((len + PT - 1) / PT);
-    const size_t padded = (size_t)tiles * PT + HALO + LEAD;
+    const size_t padded = (size_t)tiles * PT + HALO_MAX + LEAD;
 
     ParseParams P;
     memset(&P, 0, sizeof P);
@@ -213,6 +232,7 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
     P.l2 = (uint32_t)part[2].size();
     P.l3 = (uint32_t)part[3].size();
     P.lm = (uint32_t)part[4].size();
+    P.l9 = (uint32_t)part[9].size();
 
     KxScratch sc(ctx);
     uint8_t *d_doc = nullptr;
@@ -234,7 +254,10 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
     P.epoch = kx_next_epoch(ctx);
 
     KxTimer tm(ctx, KXPU_T_EMIT);  // decode, the re-emit and the compare, with the one host read of the count between
-    if (mdev) {
+    if (layout == LAYOUT_MDEV_CDEV) {
+        if (format == KXPU_FMT_YAML) decode_launch<KXPU_FMT_YAML, LAYOUT_MDEV_CDEV>(ctx, tiles, P);
+        else decode_launch<KXPU_FMT_JSON, LAYOUT_MDEV_CDEV>(ctx, tiles, P);
+    } else if (mdev) {
         if (format == KXPU_FMT_YAML) decode_launch<KXPU_FMT_YAML, LAYOUT_MDEV>(ctx, tiles, P);
         else decode_launch<KXPU_FMT_JSON, LAYOUT_MDEV>(ctx, tiles, P);
     } else if (layout == LAYOUT_CDEV) {
@@ -288,4 +311,9 @@ extern "C" int32_t kxpu_cdi_parse_mdev(kxpu_ctx *ctx, int32_t format, const char
 extern "C" int32_t kxpu_cdi_parse_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
                                        kxpu_cdidev *out, size_t cap, size_t *n) {
     return cdi_parse(ctx, format, kind, doc, len, out, cap, n, LAYOUT_CDEV, "cdi_parse_cdev");
+}
+
+extern "C" int32_t kxpu_cdi_parse_mdev_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc,
+                                            size_t len, kxpu_mdevcdev *out, size_t cap, size_t *n) {
+    return cdi_parse(ctx, format, kind, doc, len, out, cap, n, LAYOUT_MDEV_CDEV, "cdi_parse_mdev_cdev");
 }

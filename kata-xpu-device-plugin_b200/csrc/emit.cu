@@ -40,8 +40,16 @@ constexpr int MAX_FRAG_MDEV = 480;  // kxpu_cdi_emit_mdev, every kind: the PCI b
 constexpr int CDEV_EXTRA = sizeof(KX_CDEV_NODE) - 1;
 constexpr int MAX_FRAG_CDEV = MAX_FRAG + CDEV_EXTRA;
 constexpr int MAX_FRAG_CDEV_LONG = MAX_FRAG_LONG + CDEV_EXTRA;
-constexpr int LAYOUT_PCI = KX_CDI_PCI, LAYOUT_MDEV = KX_CDI_MDEV, LAYOUT_CDEV = KX_CDI_CDEV;
+// kxpu_cdi_emit_mdev_cdev: the same for the mdev bound; 71.3 KB per CTA, still three CTAs per SM
+constexpr int MAX_FRAG_MDEV_CDEV = MAX_FRAG_MDEV + CDEV_EXTRA;
+constexpr int LAYOUT_PCI = KX_CDI_PCI, LAYOUT_MDEV = KX_CDI_MDEV, LAYOUT_CDEV = KX_CDI_CDEV,
+              LAYOUT_MDEV_CDEV = KX_CDI_MDEV_CDEV;
 static_assert(MAX_FRAG_MDEV <= KX_CDI_FRAG_MAX && MAX_FRAG_CDEV_LONG <= KX_CDI_FRAG_MAX, "the parse halo must follow");
+static_assert(MAX_FRAG_MDEV_CDEV <= KX_CDI_FRAG_MAX_MDEV_CDEV, "the mdev cdev parse halo must follow");
+// the records of the two mdev layouts: kxpu_mdevcdev starts with the kxpu_mdevcdi the group layout reads
+template <int LAYOUT> constexpr bool is_mdev_layout = LAYOUT == LAYOUT_MDEV || LAYOUT == LAYOUT_MDEV_CDEV;
+template <int LAYOUT> constexpr bool is_cdev_layout = LAYOUT == LAYOUT_CDEV || LAYOUT == LAYOUT_MDEV_CDEV;
+template <int LAYOUT> using MdevRec = std::conditional_t<LAYOUT == LAYOUT_MDEV_CDEV, kxpu_mdevcdev, kxpu_mdevcdi>;
 constexpr int POOL_MAX = 640;
 constexpr int KIND_MAX = 63;
 
@@ -93,6 +101,10 @@ static const Parts h_yaml_cdev_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_Y4 KX_C
                                         {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB, nullptr}};
 static const Parts h_json_cdev_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_J4 KX_CDEV_NODE, KX_J5, KX_JHA, KX_JT, KX_JHA, nullptr},
                                         {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB, nullptr}};
+static const Parts h_yaml_mdev_cdev_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_YM, KX_Y5, KX_YHA, KX_YT, KX_YHA, KX_Y4 KX_CDEV_NODE},
+                                             {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB, nullptr}};
+static const Parts h_json_mdev_cdev_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_JM, KX_J5, KX_JHA, KX_JT, KX_JHA, KX_J4 KX_CDEV_NODE},
+                                             {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB, nullptr}};
 static const char *kDefaultKind = "nvidia.com/gpu";  // CdiVendorClass, generic_device_plugin.go:31
 
 // The supported kind domain (include/kxpu.h): "vendor/class", <= 63 bytes; vendor = letter [A-Za-z0-9_.-]*
@@ -215,6 +227,8 @@ struct TileSmem {
 };
 // four CTAs per SM (228 KB of shared memory, 1 KB of it reserved per CTA) for the short-kind tiles of both node layouts
 static_assert(4 * (sizeof(TileSmem<MAX_FRAG_CDEV>) + 1024) <= 228 * 1024, "the cdev short-kind tile lost an SM slot");
+// three CTAs per SM for the tiles of both mdev layouts
+static_assert(3 * (sizeof(TileSmem<MAX_FRAG_MDEV_CDEV>) + 1024) <= 228 * 1024, "the mdev cdev tile lost an SM slot");
 
 template <int FMT, int MAXF, int LAYOUT>
 __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constant__ EmitParams E) {
@@ -231,15 +245,15 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
         uint4 bq;  // the bdf / parent address
         uint32_t group, node = 0;
         unsigned long long index;
-        if (LAYOUT != LAYOUT_MDEV) {  // bdf[16] | iommu_group | vfio_cdev | index
+        if (!is_mdev_layout<LAYOUT>) {  // bdf[16] | iommu_group | vfio_cdev | index
             const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const kxpu_cdidev *>(E.devs) + i0 + tid);
             const uint4 q0 = p[0], q1 = p[1];
             bq = q0;
             group = q1.x;
             if constexpr (LAYOUT == LAYOUT_CDEV) node = q1.y;
             index = ((unsigned long long)q1.w << 32) | q1.z;
-        } else {  // uuid[36] | iommu_group | parent[16] | index
-            const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const kxpu_mdevcdi *>(E.devs) + i0 + tid);
+        } else {  // uuid[36] | iommu_group | parent[16] | index (mdev cdev: the first 64 of 80 bytes; N is read below)
+            const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const MdevRec<LAYOUT> *>(E.devs) + i0 + tid);
             const uint4 q0 = p[0], q1 = p[1], q2 = p[2], q3 = p[3];
             const uint32_t uw[9] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x};
             if (!kxmdev::uuid_ok(uw)) E.flags[1] = 1u;
@@ -255,8 +269,9 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
         dec_write(group, gl, S.grp[tid]);
         *reinterpret_cast<uint4 *>(S.bdf[tid]) = bq;
         S.meta[tid] = il | (gl << 8) | (bl << 16) | ((quoted ? 1u : 0u) << 24);
-        flen = E.lit_total + 2u * il + 2u * gl + bl + (quoted ? 2u : 0u) + (LAYOUT == LAYOUT_MDEV ? 36u : 0u);
-        if constexpr (LAYOUT == LAYOUT_CDEV) {  // N in place of the group's second copy; its length in grp's spare byte 11
+        flen = E.lit_total + 2u * il + 2u * gl + bl + (quoted ? 2u : 0u) + (is_mdev_layout<LAYOUT> ? 36u : 0u);
+        if constexpr (LAYOUT == LAYOUT_MDEV_CDEV) node = static_cast<const kxpu_mdevcdev *>(E.devs)[i0 + tid].vfio_cdev;
+        if constexpr (is_cdev_layout<LAYOUT>) {  // N in place of the group's second copy; its length in grp's spare byte 11
             uint32_t nl = 1;
             for (uint32_t p = 10u; nl < 10u && node >= p; p *= 10u) nl++;
             S.grp[tid][11] = (uint8_t)nl;
@@ -295,9 +310,12 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
     if (last_tile) for (uint32_t k = tid; k < tail_len; k += EMIT_THREADS) stg[head_len + tile_total + k] = S.pool[E.off[7] + k];
     // ---- fragments: one warp per device, segment by segment
     uint32_t cdev_n = 0;  // cdev: lane j holds N of the warp's j-th device, read from the device array (L2) ahead of the loop
-    if constexpr (LAYOUT == LAYOUT_CDEV) {
+    if constexpr (is_cdev_layout<LAYOUT>) {
         const uint32_t dj = w + lane * (EMIT_THREADS / 32);
-        if (dj < (uint32_t)TILE && i0 + dj < E.n) cdev_n = static_cast<const kxpu_cdidev *>(E.devs)[i0 + dj].vfio_cdev;
+        if (dj < (uint32_t)TILE && i0 + dj < E.n) {
+            if constexpr (LAYOUT == LAYOUT_CDEV) cdev_n = static_cast<const kxpu_cdidev *>(E.devs)[i0 + dj].vfio_cdev;
+            else cdev_n = static_cast<const kxpu_mdevcdev *>(E.devs)[i0 + dj].vfio_cdev;
+        }
     }
     for (uint32_t d = w; d < (uint32_t)TILE && i0 + d < E.n; d += EMIT_THREADS / 32) {
         const uint32_t m = S.meta[d];
@@ -320,13 +338,14 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
         };
         lit(0); var(S.idx[d], il); lit(1); quote(); var(S.bdf[d], bl); quote(); lit(2); var(S.grp[d], gl);
         lit(3); var(S.idx[d], il); lit(4);
-        if (LAYOUT == LAYOUT_MDEV) {  // the uuid straight from the device array (L2), then the PCI literal 4
-            const uint8_t *u = static_cast<const uint8_t *>(E.devs) + (size_t)(i0 + d) * sizeof(kxpu_mdevcdi);
+        if (is_mdev_layout<LAYOUT>) {  // the uuid straight from the device array (L2), then the PCI literal 4 (mdev cdev:
+                                       // with the node literal)
+            const uint8_t *u = static_cast<const uint8_t *>(E.devs) + (size_t)(i0 + d) * sizeof(MdevRec<LAYOUT>);
             for (uint32_t l = lane; l < 36u; l += 32u) dst[o + l] = u[l];
             o += 36u;
             lit(8);
         }
-        if constexpr (LAYOUT == LAYOUT_CDEV) {  // lane k writes digit k of N
+        if constexpr (is_cdev_layout<LAYOUT>) {  // lane k writes digit k of N
             const uint32_t N = __shfl_sync(0xffffffffu, cdev_n, d / (EMIT_THREADS / 32));
             const uint32_t nl = S.grp[d][11];
             if (lane < nl) {
@@ -895,6 +914,7 @@ static const Parts &parts_of(int32_t format, int layout) {
     const bool yaml = format == KXPU_FMT_YAML;
     if (layout == LAYOUT_MDEV) return yaml ? h_yaml_mdev_parts : h_json_mdev_parts;
     if (layout == LAYOUT_CDEV) return yaml ? h_yaml_cdev_parts : h_json_cdev_parts;
+    if (layout == LAYOUT_MDEV_CDEV) return yaml ? h_yaml_mdev_cdev_parts : h_json_mdev_cdev_parts;
     return yaml ? h_yaml_parts : h_json_parts;
 }
 
@@ -912,13 +932,18 @@ static void emit_smem_attr() {
 
 int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, const void *d_devs, size_t n, int layout,
                             KxScratch &sc, uint8_t **d_out_p, unsigned long long **d_total_p, bool timed) {
-    const bool mdev = layout == LAYOUT_MDEV;
+    const bool mdev = layout == LAYOUT_MDEV || layout == LAYOUT_MDEV_CDEV;
     const Parts &parts = parts_of(format, layout);
     static bool cdev_attr_done = false;
     if (layout == LAYOUT_CDEV && !cdev_attr_done) {
         emit_smem_attr<MAX_FRAG_CDEV, LAYOUT_CDEV>();
         emit_smem_attr<MAX_FRAG_CDEV_LONG, LAYOUT_CDEV>();
         cdev_attr_done = true;
+    }
+    static bool mdev_cdev_attr_done = false;
+    if (layout == LAYOUT_MDEV_CDEV && !mdev_cdev_attr_done) {
+        emit_smem_attr<MAX_FRAG_MDEV_CDEV, LAYOUT_MDEV_CDEV>();
+        mdev_cdev_attr_done = true;
     }
     static bool attr_done = false;
     if (!attr_done) {
@@ -954,11 +979,12 @@ int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, con
     const uint32_t frag = E.lit_total + 2 * 20 + 2 * 10 + 15 + 2 + 2 + (mdev ? 36 : 0);  // no fragment is longer
     const size_t bound = (size_t)n * frag + E.len[6] + E.len[7] + 64;
     // kinds up to 22 bytes fit the four-CTAs-per-SM tile, longer ones take the MAX_FRAG_LONG instantiation (cdev: both
-    // bounds CDEV_EXTRA larger, so the same kinds); every mdev kind the MAX_FRAG_MDEV one
+    // bounds CDEV_EXTRA larger, so the same kinds); every mdev kind the MAX_FRAG_MDEV one (mdev cdev: MAX_FRAG_MDEV_CDEV)
     const bool cdev = layout == LAYOUT_CDEV;
     const bool long_frag = frag > (uint32_t)(cdev ? MAX_FRAG_CDEV : MAX_FRAG);
-    if (frag > (uint32_t)(mdev ? MAX_FRAG_MDEV : cdev ? MAX_FRAG_CDEV_LONG : MAX_FRAG_LONG))
-        return KXPU_E_INVALID;  // the literals grew: the bound must follow
+    const int max_frag = layout == LAYOUT_MDEV_CDEV ? MAX_FRAG_MDEV_CDEV : mdev ? MAX_FRAG_MDEV
+                         : cdev ? MAX_FRAG_CDEV_LONG : MAX_FRAG_LONG;
+    if (frag > (uint32_t)max_frag) return KXPU_E_INVALID;  // the literals grew: the bound must follow
     uint8_t *d_out = nullptr;
     unsigned long long *d_total = nullptr;
     KX_CUDA(ctx, sc.alloc((void **)&d_out, bound));
@@ -969,7 +995,10 @@ int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, con
     if (!E.state) return KXPU_E_NOMEM;
     E.epoch = kx_next_epoch(ctx);
     auto launch = [&]() {
-        if (mdev) {
+        if (layout == LAYOUT_MDEV_CDEV) {
+            if (format == KXPU_FMT_YAML) emit_launch<KXPU_FMT_YAML, MAX_FRAG_MDEV_CDEV, LAYOUT_MDEV_CDEV>(ctx, tiles, E);
+            else emit_launch<KXPU_FMT_JSON, MAX_FRAG_MDEV_CDEV, LAYOUT_MDEV_CDEV>(ctx, tiles, E);
+        } else if (mdev) {
             if (format == KXPU_FMT_YAML) emit_launch<KXPU_FMT_YAML, MAX_FRAG_MDEV, LAYOUT_MDEV>(ctx, tiles, E);
             else emit_launch<KXPU_FMT_JSON, MAX_FRAG_MDEV, LAYOUT_MDEV>(ctx, tiles, E);
         } else if (cdev) {
@@ -1000,10 +1029,9 @@ int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, con
     return KXPU_OK;
 }
 
-// LAYOUT_MDEV: devs is kxpu_mdevcdi[n], else kxpu_cdidev[n]
+// LAYOUT_MDEV: devs is kxpu_mdevcdi[n], LAYOUT_MDEV_CDEV: kxpu_mdevcdev[n], else kxpu_cdidev[n]
 static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const void *devs, size_t n, uint8_t *out,
                         size_t cap, size_t *len, int layout = LAYOUT_PCI) {
-    const bool mdev = layout == LAYOUT_MDEV;
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
@@ -1014,7 +1042,8 @@ static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const v
         memcpy(out, doc.data(), *len);
         return KXPU_OK;
     }
-    const size_t dev_bytes = mdev ? sizeof(kxpu_mdevcdi) : sizeof(kxpu_cdidev);
+    const size_t dev_bytes = layout == LAYOUT_MDEV ? sizeof(kxpu_mdevcdi)
+                             : layout == LAYOUT_MDEV_CDEV ? sizeof(kxpu_mdevcdev) : sizeof(kxpu_cdidev);
     KxScratch sc(ctx);
     void *d_devs = nullptr;
     uint8_t *d_out = nullptr;
@@ -1069,6 +1098,15 @@ extern "C" int32_t kxpu_cdi_emit_cdev(kxpu_ctx *ctx, int32_t format, const char 
     if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
     if (!kind_ok(kind)) { KX_SET_ERR(ctx, "cdi_emit_cdev: kind is not a CDI vendor/class of at most 63 bytes"); return KXPU_E_UNSUPPORTED; }
     return cdi_emit(ctx, format, kind, devs, n, out, cap, len, LAYOUT_CDEV);
+}
+
+extern "C" int32_t kxpu_cdi_emit_mdev_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_mdevcdev *devs,
+                                           size_t n, uint8_t *out, size_t cap, size_t *len) {
+    static_assert(sizeof(kxpu_mdevcdev) == 80 && offsetof(kxpu_mdevcdev, vfio_cdev) == 64, "kxpu_mdevcdev layout");
+    if (!ctx || !len || !kind || (n && !devs) || (format != KXPU_FMT_YAML && format != KXPU_FMT_JSON)) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    if (!kind_ok(kind)) { KX_SET_ERR(ctx, "cdi_emit_mdev_cdev: kind is not a CDI vendor/class of at most 63 bytes"); return KXPU_E_UNSUPPORTED; }
+    return cdi_emit(ctx, format, kind, devs, n, out, cap, len, LAYOUT_MDEV_CDEV);
 }
 
 // shared driver of the "thread per item" emitters.  h_in3 (optional, in3_bytes): one more input, uploaded like the

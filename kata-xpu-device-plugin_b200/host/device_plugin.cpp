@@ -424,19 +424,25 @@ bool Plugin::cdevEnabled() const {
     return false;
 }
 
-int64_t Plugin::readVfioCdev(const std::string &bdf) {
+bool Plugin::mdevCdevEnabled() const {
+    for (const XpuClass &c : vgpuClasses)
+        if (c.mdevCdev) return true;
+    return false;
+}
+
+int64_t Plugin::readVfioCdev(const std::string &base, const std::string &entry) {
     cdevReads++;
-    DIR *d = opendir((basePath + "/" + bdf + "/vfio-dev").c_str());
+    DIR *d = opendir((base + "/" + entry + "/vfio-dev").c_str());
     if (!d) return -1;
-    std::string entry;
+    std::string node;
     int entries = 0;
     while (struct dirent *de = readdir(d)) {
         if (strcmp(de->d_name, ".") == 0 || strcmp(de->d_name, "..") == 0) continue;
-        if (++entries == 1) entry = de->d_name;
+        if (++entries == 1) node = de->d_name;
     }
     closedir(d);
-    if (entries != 1 || entry.size() < 5 || entry.size() > 14 || entry.compare(0, 4, "vfio") != 0) return -1;
-    const std::string num = entry.substr(4);
+    if (entries != 1 || node.size() < 5 || node.size() > 14 || node.compare(0, 4, "vfio") != 0) return -1;
+    const std::string num = node.substr(4);
     if (num.size() > 1 && num[0] == '0') return -1;  // canonical decimals only
     uint64_t v = 0;
     for (char ch : num) {
@@ -444,6 +450,18 @@ int64_t Plugin::readVfioCdev(const std::string &bdf) {
         v = v * 10 + (uint64_t)(ch - '0');
     }
     return v < (1ull << 32) ? (int64_t)v : -1;
+}
+
+// does a record with this vendor and driver match a class that sets `flag` (vfioCdev or mdevCdev)?
+template <typename Rec>
+static bool cdevClassOf(const std::vector<XpuClass> &classes, bool XpuClass::*flag, const Rec &r, const uint8_t *vendorTxt,
+                        size_t vendorCap) {
+    if (r.flags & (KXPU_REC_IS_DIR | KXPU_REC_VENDOR_ERR | KXPU_REC_DRIVER_ERR)) return false;
+    const std::string vendor = trimID(std::string((const char *)vendorTxt, std::min<size_t>(r.vendor_len, vendorCap)));
+    const std::string drv(r.driver, strnlen(r.driver, sizeof r.driver));
+    bool match = false;
+    for (const XpuClass &c : classes) match |= c.*flag && c.vendor == vendor && c.driver == drv;
+    return match;
 }
 
 // the vfio-dev/ read of every record that matches a vfioCdev class (vendor and driver), after either gather
@@ -454,12 +472,8 @@ void Plugin::readCdevs(const std::vector<kxpu_devrec> &recs, std::vector<int64_t
     cdevs->assign(recs.size(), -1);
     for (size_t i = 0; i < recs.size(); i++) {
         const kxpu_devrec &r = recs[i];
-        if (r.flags & (KXPU_REC_IS_DIR | KXPU_REC_VENDOR_ERR | KXPU_REC_DRIVER_ERR)) continue;
-        const std::string vendor = trimID(std::string((const char *)r.vendor_txt, std::min<size_t>(r.vendor_len, sizeof r.vendor_txt)));
-        const std::string drv(r.driver, strnlen(r.driver, sizeof r.driver));
-        bool match = false;
-        for (const XpuClass &c : xpuClasses) match |= c.vfioCdev && c.vendor == vendor && c.driver == drv;
-        if (match) (*cdevs)[i] = readVfioCdev(std::string(r.bdf, strnlen(r.bdf, sizeof r.bdf)));
+        if (cdevClassOf(xpuClasses, &XpuClass::vfioCdev, r, r.vendor_txt, sizeof r.vendor_txt))
+            (*cdevs)[i] = readVfioCdev(basePath, std::string(r.bdf, strnlen(r.bdf, sizeof r.bdf)));
     }
 }
 
@@ -607,8 +621,20 @@ static std::string devIdString(uint64_t packed) {
     return std::string(b);
 }
 
+// mdevCdev names an mdev's cdev: a passthrough class with it is refused
+static Error checkPassthroughClasses(const std::vector<XpuClass> &classes) {
+    for (const XpuClass &c : classes)
+        if (c.mdevCdev)
+            return fail("passthrough class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + "): mdevCdev applies to vGPU classes only; a passthrough class sets vfioCdev");
+    return Error();
+}
+
 // createIommuDeviceMap, device_plugin.go:126-180
 Error Plugin::createIommuDeviceMap() {
+    {
+        Error e = checkPassthroughClasses(xpuClasses);
+        if (e) return e;
+    }
     iommuMap.clear();   // :127
     deviceMap.clear();  // :128
     iommuClass.clear();
@@ -877,7 +903,8 @@ static void mdevRecord(Plugin &p, const std::string &name, bool isDir, kxpu_mdev
 // holds one level of links, so a directory inside it is recorded as such and not descended into.
 Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w) {
     recs.clear();
-    if (w) { w->parentDevice.clear(); w->pcieRoot.clear(); }
+    if (w) { w->parentDevice.clear(); w->pcieRoot.clear(); w->cdevs.clear(); }
+    std::vector<int64_t> *cdevs = w && mdevCdevEnabled() ? &w->cdevs : nullptr;
     if (!vgpuDraEnabled()) w = nullptr;
     DIR *d = opendir(mdevBasePath.c_str());
     if (!d) return fail("Error accessing file path \"" + mdevBasePath + "\": " + strerror(errno));
@@ -894,6 +921,10 @@ Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w) {
         kxpu_mdevrec r;
         mdevRecord(*this, n, isDir, r);
         recs.push_back(r);
+        // the vfio-dev/ read of an entry that matches an mdevCdev class (parent vendor and driver)
+        if (cdevs)
+            cdevs->push_back(cdevClassOf(vgpuClasses, &XpuClass::mdevCdev, r, r.parent_vendor_txt, sizeof r.parent_vendor_txt)
+                                 ? readVfioCdev(mdevBasePath, n) : -1);
         if (!w) continue;
         // the ResourceSlice reads of an entry that got as far as its iommu_group link
         std::string dev, target;
@@ -926,8 +957,8 @@ Error Plugin::checkVgpuClasses() const {
                 return fail("vGPU class " + all[v]->vendor + "/" + all[v]->driver + ": CDI kind and file stem must differ from every other class's");
     if (vgpuClasses.size() > KXPU_MAX_RULES) return fail("more vGPU classes than KXPU_MAX_RULES");
     for (const XpuClass &c : vgpuClasses)
-        if (c.vfioCdev) return fail("vGPU class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + "): vfioCdev applies to passthrough classes only");
-    return Error();
+        if (c.vfioCdev) return fail("vGPU class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + "): vfioCdev applies to passthrough classes only; a vGPU class sets mdevCdev");
+    return checkPassthroughClasses(xpuClasses);
 }
 
 Error Plugin::createMdevMap() {
@@ -936,6 +967,7 @@ Error Plugin::createMdevMap() {
     mdevClass.clear();
     typeClass.clear();
     mdevNuma.clear();
+    mdevBlocker.clear();
     mdevSnap_.clear();
     mdevNext_ = 0;
     if (vgpuClasses.empty()) return Error();  // nothing under mdevBasePath is read
@@ -984,6 +1016,7 @@ void Plugin::buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index
     mdevClass.clear();
     typeClass.clear();
     mdevNuma.clear();
+    mdevBlocker.clear();
     const ClassifyResult &c = w.out;
     std::map<uint32_t, size_t> groupClass = groupClasses(c);
     for (uint32_t g = 0; g < c.nGroups; g++) {
@@ -993,7 +1026,15 @@ void Plugin::buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index
             const uint64_t idx = index ? (*index)[c.accept[c.gmem[k]]] : c.accept[c.gmem[k]];
             MdevDevice m{std::string(r.uuid, sizeof r.uuid), std::string(r.parent, strnlen(r.parent, sizeof r.parent)), idx, 0};
             m.vgpuClass = recordClass(vgpuClasses, r.parent_vendor_txt, r.vendor_len, r.driver, sizeof r.driver);
+            if (!w.cdevs.empty()) m.cdev = w.cdevs[c.gmem[k]];
             devs.push_back(std::move(m));
+        }
+        if (mdevCdevEnabled()) {  // an mdev without a cdev: VFIO cannot open it
+            std::string blocker;
+            if (vgpuClasses[groupClass[c.gids[g]]].mdevCdev)
+                for (const MdevDevice &m : devs)
+                    if (m.cdev < 0) { blocker = m.uuid + " has no VFIO cdev"; break; }
+            mdevBlocker.push_back(blocker);
         }
         mdevMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
         mdevClass.push_back(groupClass[c.gids[g]]);
@@ -1272,15 +1313,36 @@ static kxpu_cdidev cdiRecord(const std::string &group, const NvidiaGpuDevice &de
     return d;
 }
 static bool hasCdev(const NvidiaGpuDevice &dev) { return dev.cdev >= 0; }
-static bool hasCdev(const MdevDevice &) { return true; }
-static kxpu_mdevcdi cdiRecord(const std::string &group, const MdevDevice &m) {
-    kxpu_mdevcdi d;
+static bool hasCdev(const MdevDevice &m) { return m.cdev >= 0; }
+// the vGPU spec paths hold one record type for both node layouts: the group layout reads and writes each record's dev
+static kxpu_mdevcdev cdiRecord(const std::string &group, const MdevDevice &m) {
+    kxpu_mdevcdev d;
     memset(&d, 0, sizeof d);
-    memcpy(d.uuid, m.uuid.data(), std::min(m.uuid.size(), sizeof d.uuid));
-    strncpy(d.parent, m.parent.c_str(), sizeof d.parent - 1);
-    d.iommu_group = (uint32_t)strtoul(group.c_str(), nullptr, 10);
-    d.index = m.index;
+    memcpy(d.dev.uuid, m.uuid.data(), std::min(m.uuid.size(), sizeof d.dev.uuid));
+    strncpy(d.dev.parent, m.parent.c_str(), sizeof d.dev.parent - 1);
+    d.dev.iommu_group = (uint32_t)strtoul(group.c_str(), nullptr, 10);
+    d.dev.index = m.index;
+    d.vfio_cdev = m.cdev < 0 ? 0u : (uint32_t)m.cdev;
     return d;
+}
+static const kxpu_cdidev &cdiBase(const kxpu_cdidev &r) { return r; }
+static const kxpu_mdevcdi &cdiBase(const kxpu_mdevcdev &r) { return r.dev; }
+static int32_t emitMdevGroup(kxpu_ctx *ctx, int32_t fmt, const char *kind, const kxpu_mdevcdev *devs, size_t n, uint8_t *out,
+                             size_t cap, size_t *len) {
+    std::vector<kxpu_mdevcdi> d(n);
+    for (size_t i = 0; i < n; i++) d[i] = devs[i].dev;
+    return kxpu_cdi_emit_mdev(ctx, fmt, kind, d.data(), n, out, cap, len);
+}
+static int32_t parseMdevGroup(kxpu_ctx *ctx, int32_t fmt, const char *kind, const uint8_t *doc, size_t len, kxpu_mdevcdev *out,
+                              size_t cap, size_t *n) {
+    std::vector<kxpu_mdevcdi> d(cap);
+    const int32_t rc = kxpu_cdi_parse_mdev(ctx, fmt, kind, doc, len, d.data(), cap, n);
+    if (rc == KXPU_OK)
+        for (size_t i = 0; i < *n; i++) {
+            memset(&out[i], 0, sizeof out[i]);
+            out[i].dev = d[i];
+        }
+    return rc;
 }
 
 // One file per class, <stem>.yaml|.json, with that class's kind and only the devices of its entries in ascending index
@@ -1293,19 +1355,21 @@ Error Plugin::generateClassSpecs(const std::vector<XpuClass> &classes, const Ord
                                  std::vector<std::string> &files) {
     std::vector<std::vector<Rec>> per(classes.size());
     for (size_t g = 0; g < m.size(); g++) {
-        bool cdevs = true;  // a vfioCdev class's spec leaves out a group with a member without a cdev
+        bool cdevs = true;  // a vfioCdev / mdevCdev class's spec leaves out a group with a member without a cdev
         for (const Dev &dev : m[g].second) cdevs &= hasCdev(dev);
-        if (classes[entryClass[g]].vfioCdev && !cdevs) continue;
+        if ((classes[entryClass[g]].vfioCdev || classes[entryClass[g]].mdevCdev) && !cdevs) continue;
         for (const Dev &dev : m[g].second) per[entryClass[g]].push_back(cdiRecord(m[g].first, dev));
     }
     for (size_t c = 0; c < classes.size(); c++) {
         std::vector<Rec> &devs = per[c];
-        std::sort(devs.begin(), devs.end(), [](const Rec &a, const Rec &b) { return a.index < b.index; });
+        std::sort(devs.begin(), devs.end(), [](const Rec &a, const Rec &b) { return cdiBase(a).index < cdiBase(b).index; });
         const char *kind = classes[c].cdiKind.c_str();
         size_t len = 0;
         auto *fn = emit;
         if constexpr (std::is_same<Rec, kxpu_cdidev>::value)
             if (classes[c].vfioCdev) fn = kxpu_cdi_emit_cdev;
+        if constexpr (std::is_same<Rec, kxpu_mdevcdev>::value)
+            if (classes[c].mdevCdev) fn = kxpu_cdi_emit_mdev_cdev;
         int32_t rc = fn(ctx_, fmt, kind, devs.data(), devs.size(), nullptr, 0, &len);
         if (rc != KXPU_OK && rc != KXPU_E_NOSPACE) return kxfail(ctx_, what, rc);
         std::vector<uint8_t> doc(len ? len : 1);
@@ -1342,7 +1406,7 @@ Error Plugin::generateMdevCDISpec(const std::string &format) {
     mdevCdiFiles.clear();
     if (vgpuClasses.empty()) return Error();
     const int32_t fmt = format == "YAML" ? KXPU_FMT_YAML : KXPU_FMT_JSON;
-    return generateClassSpecs(vgpuClasses, mdevMap, mdevClass, fmt, "kxpu_cdi_emit_mdev", kxpu_cdi_emit_mdev, mdevCdiFiles);
+    return generateClassSpecs(vgpuClasses, mdevMap, mdevClass, fmt, "kxpu_cdi_emit_mdev", emitMdevGroup, mdevCdiFiles);
 }
 
 // createDevicePlugins, device_plugin.go:83-112 (nothing is started: no gRPC here)
@@ -1379,7 +1443,7 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         auto it = nodeOf.find(g);
         return it == nodeOf.end() ? KXPU_PCIE_NO_NODE : it->second;
     };
-    std::map<std::string, std::string> blockerOfGroup;  // group id -> its first blocker (groupViability)
+    std::map<std::string, std::string> blockerOfGroup;  // group id -> its first blocker (groupViability, cdevs)
     for (size_t g = 0; g < iommuBlocker.size() && g < iommuMap.size(); g++)
         if (!iommuBlocker[g].empty()) blockerOfGroup[iommuMap[g].first] = iommuBlocker[g];
     std::map<std::string, std::string> aerOfGroup, aerOfMdevGroup;  // group id -> its AER reason (aerHealth)
@@ -1387,6 +1451,8 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         if (!iommuAer[g].empty()) aerOfGroup[iommuMap[g].first] = iommuAer[g];
     for (size_t g = 0; g < mdevAer.size() && g < mdevMap.size(); g++)
         if (!mdevAer[g].empty()) aerOfMdevGroup[mdevMap[g].first] = mdevAer[g];
+    for (size_t g = 0; g < mdevBlocker.size() && g < mdevMap.size(); g++)  // mdev groups: "<uuid> has no VFIO cdev"
+        if (!mdevBlocker[g].empty()) blockerOfGroup[mdevMap[g].first] = mdevBlocker[g];
     auto aerOf = [](const std::map<std::string, std::string> &m, const std::string &g) {
         auto it = m.find(g);
         return it == m.end() ? std::string() : it->second;
@@ -1429,9 +1495,21 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         for (const std::string &g : typeMap[t].second) {
             dp.devs.push_back(Device{g, kHealthy, maskOf(mdevNumaOf, g)});
             dp.devs.back().aer = aerOf(aerOfMdevGroup, g);
+            auto it = blockerOfGroup.find(g);
+            if (it != blockerOfGroup.end()) dp.devs.back().blocker = it->second;
         }
         dp.devpluginName = typeMap[t].first;
         dp.devicePath = "/dev/vfio/";  // an mdev has its own IOMMU group and /dev/vfio/<group>
+        if (vgpuClasses[dp.xpuClass].mdevCdev) {  // every mdev's cdev node
+            dp.devicePath = "/dev/vfio/devices/";
+            for (const auto &g : mdevMap) {
+                const std::vector<std::string> &groups = typeMap[t].second;
+                if (std::find(groups.begin(), groups.end(), g.first) == groups.end()) continue;
+                std::vector<std::string> &nodes = dp.nodes[g.first];
+                for (const MdevDevice &m : g.second)
+                    if (m.cdev >= 0) nodes.push_back("vfio" + std::to_string(m.cdev));
+            }
+        }
         dp.socketPath = std::string(kDevicePluginPath) + "kata-xpu-" + dp.devpluginName + ".sock";
         dp.deviceKey = typeMap[t].first;
         devicePlugins.push_back(std::move(dp));
@@ -1584,7 +1662,8 @@ void Plugin::previousEntries(const std::vector<XpuClass> &classes,
             rc = parseWith(classes[c].vfioCdev ? kxpu_cdi_parse_cdev : kxpu_cdi_parse);
             if (rc == KXPU_E_INVALID) rc = parseWith(classes[c].vfioCdev ? kxpu_cdi_parse : kxpu_cdi_parse_cdev);
         } else {
-            rc = parseWith(parse);
+            rc = parseWith(classes[c].mdevCdev ? kxpu_cdi_parse_mdev_cdev : parse);
+            if (rc == KXPU_E_INVALID) rc = parseWith(classes[c].mdevCdev ? parse : kxpu_cdi_parse_mdev_cdev);
         }
         if (rc != KXPU_OK) {
             rw.fallback = path + ": not a CDI spec this plugin writes (" + kxpu_strerror(rc) + ": " + kxpu_last_error(ctx_) + ")";
@@ -1592,10 +1671,10 @@ void Plugin::previousEntries(const std::vector<XpuClass> &classes,
         }
         rw.filesRead.push_back(path);
         for (size_t i = 0; i < n && rw.fallback.empty(); i++) {
-            const Rec &r = recs[i];
+            const auto &r = cdiBase(recs[i]);
             kxpu_snaprec s;
             memset(&s, 0, sizeof s);
-            if constexpr (std::is_same<Rec, kxpu_mdevcdi>::value) memcpy(s.key, r.uuid, sizeof r.uuid);
+            if constexpr (std::is_same<Rec, kxpu_mdevcdev>::value) memcpy(s.key, r.uuid, sizeof r.uuid);
             else memcpy(s.key, r.bdf, strnlen(r.bdf, sizeof r.bdf));
             s.iommu_group = r.iommu_group;
             s.klass = (uint32_t)c;
@@ -1653,7 +1732,7 @@ Error Plugin::resumeMdev(const MdevWalk &w) {
     std::vector<kxpu_snaprec> prev;
     uint64_t next = 0;
     const uint64_t stateNext = resume_.stateRead ? resume_.stateMdev : 0;
-    previousEntries<kxpu_mdevcdi>(vgpuClasses, kxpu_cdi_parse_mdev, stateNext, resume_.mdev, prev, next);
+    previousEntries<kxpu_mdevcdev>(vgpuClasses, parseMdevGroup, stateNext, resume_.mdev, prev, next);
     std::vector<kxpu_snaprec> cur = snapshotOf(w, nullptr);
     std::map<uint32_t, size_t> groupClass = groupClasses(w.out);
     for (kxpu_snaprec &s : cur) { s.klass = (uint32_t)groupClass[s.iommu_group]; s.tag = 0; }
@@ -1823,6 +1902,8 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
         size_t mg = 0;
         for (; mg < mdevs.size(); mg++) if (mdevs[mg].first == iommuId) { mDevs = &mdevs[mg].second; break; }
         if (mDevs) {  // a vGPU group: always live reads (the uevent snapshot only follows PCI binds)
+            if (mg < mdevBlocker.size() && !mdevBlocker[mg].empty())  // the verdict of the last walk, before any read
+                return fail("invalid allocation request: IOMMU group " + iommuId + " is not viable: " + mdevBlocker[mg]);
             const size_t c = mg < mdevClass.size() ? mdevClass[mg] : 0;
             if (havePci || (haveVgpu && c != vgpuClass)) return fail("invalid allocation request: devices of more than one class");
             haveVgpu = true;
@@ -1833,6 +1914,8 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
                 if (!readLink(mdevBasePath, m.uuid, "iommu_group", iommuGroup) || iommuGroup != iommuId ||
                     !readIDFromFile(mdevBasePath, m.uuid, "../vendor", vendor) || trimID(vendor) != vgpuClasses[m.vgpuClass].vendor)
                     return fail("invalid allocation request: unknown device: " + m.uuid);
+                if (vgpuClasses[c].mdevCdev && readVfioCdev(mdevBasePath, m.uuid) != m.cdev)  // numbers are reused
+                    return fail("invalid allocation request: the VFIO cdev of " + m.uuid + " changed since discovery");
                 devIndexes.push_back(m.index);
             }
             continue;
@@ -1860,7 +1943,7 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
             const std::string &want = xpuClasses[dev.xpuClass].vendor;  // the device's class
             if (!readIDFromFile(basePath, dev.addr, "vendor", vendor) || trimID(vendor) != want)  // :334-338
                 return fail("invalid allocation request: unknown device: " + dev.addr);
-            if (xpuClasses[c].vfioCdev && readVfioCdev(dev.addr) != dev.cdev)  // cdev numbers are reused across re-binds
+            if (xpuClasses[c].vfioCdev && readVfioCdev(basePath, dev.addr) != dev.cdev)  // cdev numbers are reused across re-binds
                 return fail("invalid allocation request: the VFIO cdev of " + dev.addr + " changed since discovery");
             devIndexes.push_back(dev.index);  // :340
         }
@@ -1895,7 +1978,8 @@ static const char *kAerTaintKeyName = "/pcie-aer";  // the key is <draDriver>/pc
 
 bool Plugin::draPublished(bool vgpu, size_t g) const {
     if (vgpu)
-        return g < mdevMap.size() && g < mdevDra.size() && g < mdevClass.size() && !vgpuClasses[mdevClass[g]].draDriver.empty();
+        return g < mdevMap.size() && g < mdevDra.size() && g < mdevClass.size() && !vgpuClasses[mdevClass[g]].draDriver.empty() &&
+               (g >= mdevBlocker.size() || mdevBlocker[g].empty());
     return g < iommuMap.size() && g < iommuDra.size() && g < iommuClass.size() && !xpuClasses[iommuClass[g]].draDriver.empty() &&
            (g >= iommuBlocker.size() || iommuBlocker[g].empty());
 }
@@ -2424,9 +2508,10 @@ static bool parseClasses(const char *spec, std::vector<device_plugin::XpuClass> 
             if (c == std::string::npos) break;
             a = c + 1;
         }
-        if (f.size() != 5 && !(f.size() == 6 && f[5] == "cdev")) return false;
+        if (f.size() != 5 && !(f.size() == 6 && (f[5] == "cdev" || f[5] == "mdev-cdev"))) return false;
         out.push_back(device_plugin::XpuClass{f[0], f[1], f[2], f[3], f[4]});
-        out.back().vfioCdev = f.size() == 6;
+        out.back().vfioCdev = f.size() == 6 && f[5] == "cdev";
+        out.back().mdevCdev = f.size() == 6 && f[5] == "mdev-cdev";
     }
     return !out.empty();
 }
@@ -2532,6 +2617,25 @@ int kxh_set_device_path(void *h, int plugin_index, const char *path) {
     Plugin *p = (Plugin *)h;
     if (plugin_index < 0 || (size_t)plugin_index >= p->devicePlugins.size()) return -1;
     p->devicePlugins[(size_t)plugin_index].devicePath = path;
+    return 0;
+}
+
+// CPU only: the raw mdev gather under a vGPU class list ("...,mdev-cdev" marks an mdevCdev class) with the walk's cdev
+// side array (-1 = none or not read) and the number of vfio-dev/ directories listed
+int kxh_gather_mdev_cdev(const char *mdev_base, const char *classes, kxpu_mdevrec *out, int64_t *cdevs, size_t cap, size_t *n,
+                         uint64_t *reads, char *err, size_t errcap) {
+    Plugin p(nullptr);
+    p.mdevBasePath = mdev_base;
+    if (!parseClasses(classes, p.vgpuClasses)) { copy_out("malformed class list", err, errcap); return -1; }
+    std::vector<kxpu_mdevrec> recs;
+    device_plugin::MdevWalk w;
+    device_plugin::Error e = p.gatherMdevRecords(recs, &w);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    *n = recs.size();
+    *reads = p.cdevReads;
+    if (recs.size() > cap) return -2;
+    memcpy(out, recs.data(), recs.size() * sizeof(kxpu_mdevrec));
+    for (size_t i = 0; i < recs.size(); i++) cdevs[i] = w.cdevs.empty() ? -1 : w.cdevs[i];
     return 0;
 }
 

@@ -40,6 +40,7 @@ struct MdevDevice {
     std::string parent;    // PCI address of the parent device
     uint64_t index;        // busIndex of the mdev walk
     size_t vgpuClass = 0;  // index into Plugin::vgpuClasses of the class this mdev matched
+    int64_t cdev = -1;     // N of its VFIO cdev /dev/vfio/devices/vfio<N> (XpuClass::mdevCdev only); -1 = none
 };
 
 // Go maps iterate in random order; the canonical order used here (and by the oracle) is
@@ -180,6 +181,12 @@ struct XpuClass {
     // (kxpu_cdi_emit_cdev), the health watcher watches those nodes, and a group with a member without a cdev is treated
     // like a group that is not viable.  false: nothing under vfio-dev/ is opened and every output is as without it.
     bool vfioCdev = false;
+    // vGPU only (a passthrough class with it is refused): the class's mdevs are reached through their VFIO cdevs.  The mdev
+    // walk reads <uuid>/vfio-dev/ of every mdev that matches the class, the CDI spec names /dev/vfio/devices/vfio<N>
+    // (kxpu_cdi_emit_mdev_cdev), the health watcher watches those nodes, and a group whose mdev has no cdev is withheld
+    // like a passthrough group that is not viable.  Kept apart from vfioCdev because it also rests on the vGPU driver
+    // registering a cdev.  false: nothing under vfio-dev/ is opened and every output is as without it.
+    bool mdevCdev = false;
 };
 XpuClass defaultXpuClass();  // {"10de", "vfio-pci", "nvidia.com", "nvidia.com/gpu", "cdi-vfio-xxxx"}
 
@@ -243,6 +250,8 @@ struct MdevWalk {
     // vgpuDraEnabled only, one per record: the parent's device id (<uuid>/../device) and the PCIe root of the entry's
     // link; "" = not read, failed or outside kxpu_dramdev's domain
     std::vector<std::string> parentDevice, pcieRoot;
+    // mdevCdevEnabled only, one per record: N of its VFIO cdev, -1 = none or not read
+    std::vector<int64_t> cdevs;
 };
 
 class Plugin {
@@ -354,6 +363,7 @@ class Plugin {
     uint64_t aerReads = 0;  // aer_dev_* files read (tests, metrics)
     uint64_t cdevReads = 0;  // vfio-dev/ directories listed (tests, metrics)
     bool cdevEnabled() const;  // some passthrough class has vfioCdev
+    bool mdevCdevEnabled() const;  // some vGPU class has mdevCdev
 
     // ---- state (device_plugin.go:31,34)
     OrderedMap<std::vector<NvidiaGpuDevice>> iommuMap;  // group id -> devices
@@ -378,6 +388,9 @@ class Plugin {
     OrderedMap<std::vector<std::string>> typeMap;
     std::vector<size_t> mdevClass, typeClass;
     std::vector<std::string> mdevCdiFiles;  // files the last generateMdevCDISpec wrote, one per vGPU class
+    // mdevCdevEnabled only: "<uuid> has no VFIO cdev" of the first such mdev of every mdevMap entry of an mdevCdev class;
+    // empty = served
+    std::vector<std::string> mdevBlocker;
     // vgpuDraEnabled only: the ResourceSlice record of every mdevMap entry (from its first mdev)
     std::vector<kxpu_dramdev> mdevDra;
 
@@ -476,13 +489,16 @@ class Plugin {
     // (SURVEY 8(f) row 2); falls back to gatherRecords when a seam was replaced.  threads = 0: automatic
     Error gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads = 0, std::vector<kxpu_pcipath> *paths = nullptr,
                             std::vector<int64_t> *cdevs = nullptr);
-    // the cdev of <basePath>/<bdf>: N when vfio-dev/ holds exactly one entry besides . and .., and it is "vfio" followed by
-    // a canonical decimal below 2^32; -1 for anything else (never an error)
-    int64_t readVfioCdev(const std::string &bdf);
+    // the cdev of <base>/<entry> (a function's bdf under basePath, an mdev's uuid under mdevBasePath): N when vfio-dev/
+    // holds exactly one entry besides . and .., and it is "vfio" followed by a canonical decimal below 2^32; -1 for
+    // anything else (never an error)
+    int64_t readVfioCdev(const std::string &base, const std::string &entry);
     // raw gather of mdevBasePath under vgpuClasses (no GPU): one record per entry, lexical order.  w (vgpuDraEnabled
-    // only, else left empty): the walk's parentDevice and pcieRoot, one per record
+    // only, else left empty): the walk's parentDevice and pcieRoot, one per record; (mdevCdevEnabled only, else left
+    // empty) its cdevs
     Error gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w = nullptr);
-    // the vGPU class list against the passthrough one (distinct CDI kinds and file stems, no vfioCdev); createMdevMap runs it
+    // the vGPU class list against the passthrough one (distinct CDI kinds and file stems, no vfioCdev on a vGPU class, no
+    // mdevCdev on a passthrough class); createMdevMap runs it
     Error checkVgpuClasses() const;
 
   private:

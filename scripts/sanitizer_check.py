@@ -17,6 +17,13 @@ res = kx.classify(recs)
 devs = W.cfg5_devices(3000)
 print("classify", res["n_accepted"], "json", len(kx.cdi_emit(1, devs)), "yaml", len(kx.cdi_emit(0, devs)))
 print("alloc", len(kx.alloc_names(devs["index"])[0]), "lw", len(kx.lw_encode(res["group_ids"][:100])))
+# the vGPU cdev layout: 3000 mdevs with cdev numbers of every width, emitted and parsed back
+mcd = np.zeros(3000, B.MDEVCDEV_DTYPE)
+mcd["dev"], mcd["vfio_cdev"] = W.mdev_devices(3000), (np.arange(3000, dtype=np.uint64) * 1431655765) % (1 << 32)
+for fmt_ in (0, 1):
+    mdoc = kx.cdi_emit_mdev_cdev(fmt_, mcd, "nvidia.com/vgpu")
+    assert kx.cdi_parse_mdev_cdev(fmt_, mdoc, "nvidia.com/vgpu").tobytes() == mcd.tobytes()
+    print("mdev cdev spec", fmt_, len(mdoc))
 # NUMA topology: classify masks (PCI and mdev), topology wire bytes, both preferred-allocation shapes
 tres = kx.classify_topo([(b"10de", b"vfio-pci")], W.topo_records(keys, n=20000, nodes=4))
 mres = kx.classify_topo(W.MDEV_RULES, W.topo_mdev_records(n=20000), mdev=True)
