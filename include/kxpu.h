@@ -71,7 +71,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_FINALIZE 1
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
-#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's and kxpu_pcie_tree's kernels: the slot holds the most recent call's */
+#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov]'s and kxpu_sriov's kernels: the slot holds the most recent call's */
 #define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
@@ -542,6 +542,76 @@ int32_t kxpu_preferred_allocation_pcie(kxpu_ctx *ctx, const uint64_t *dev_numa, 
                                        const uint32_t *must_off /* [n_req+1] */, const uint32_t *must,
                                        const uint32_t *size /* [n_req] */, size_t n_req,
                                        uint32_t *out /* [sum of size] */, uint32_t *out_off /* [n_req+1] */);
+
+/* ------------------------------------------- SR-IOV virtual functions (additions to ABI v14) */
+
+/* These calls and kxpu_sriovrec were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym), as
+ * the ctypes binding and the Go shim do.  A virtual function (VF) bound to vfio-pci is a PCI function like any other, so
+ * a passthrough class serves it.  What makes VFs different rests on sysfs ABI (Documentation/ABI/testing/sysfs-bus-pci:
+ * physfn, virtfnN, sriov_numvfs) and on these facts:
+ *   [assumed] since Linux 5.7, vfio-pci refuses to open a VF whose physical function (PF) is bound to vfio-pci unless
+ *             the opener presents the PF's VF token ("VF token required to access device"), and refuses a PF on
+ *             vfio-pci whose VFs are in use in the same way;
+ *   [assumed] Kata's QEMU command line presents no VF token;
+ *   [assumed] a VF reports its PF's vendor ID, so the PF's record, with its driver, is in the same walk;
+ *   [assumed] <bdf>/physfn is a symlink whose basename is the PF's PCI address.
+ * Host side: for every record that is a candidate of a passthrough class (vendor and driver of some class), the host
+ * reads readlink(<bdf>/physfn) (basename) and the first 8 bytes of <bdf>/sriov_numvfs into a side record at the same
+ * index; every other record gets a zero-filled one.  A missing link or file is not an error: the function is no VF, or
+ * has no SR-IOV capability. */
+typedef struct kxpu_sriovrec {
+    char    physfn[16];     /* basename of the `physfn` link, NUL padded; empty: no link              */
+    uint8_t numvfs_txt[8];  /* first 8 bytes of `sriov_numvfs`                                       */
+    uint8_t numvfs_len;     /* length of the file (0..8; longer => 9)                                */
+    uint8_t flags;          /* KXPU_SR_*                                                             */
+    uint8_t reserved[6];
+} kxpu_sriovrec;            /* 32 bytes: the kernel reads one with two 16-byte vector loads          */
+#define KXPU_SR_PHYSFN_ERR 0x01u  /* readlink(physfn) failed for a reason other than "no such link"      */
+#define KXPU_SR_NUMVFS_ERR 0x02u  /* reading sriov_numvfs failed for a reason other than "no such file"   */
+#define KXPU_NO_PF 0xFFFFFFFFu
+
+/* The SR-IOV verdict of a walk.  recs / srs: the n records and side records a classify call saw; group_ids / group_off /
+ * group_members / n_groups: that call's iommuMap CSR (kxpu_classify_out of kxpu_classify_rules, _topo or _viable with the
+ * same rules).  Outputs:
+ *   - numvfs[i] = sriov_numvfs of record i: numvfs_txt[0..numvfs_len) with at most one trailing '\n' removed must be a
+ *     canonical decimal 0..65535 (no sign, no leading zero except "0" itself); anything else -- empty, "07", "65536",
+ *     "-1", junk, numvfs_len > 8, KXPU_SR_NUMVFS_ERR -- counts as 0 and is never an error (the numa_node rule);
+ *   - pf_of[i] = p, the lowest index whose bdf (up to its first NUL) equals physfn (up to its first NUL), or KXPU_NO_PF
+ *     when physfn is not a canonical lowercase "dddd:bb:dd.f" (4 hex digits, 2, 2 at most 1f, one digit 0..7), carries
+ *     KXPU_SR_PHYSFN_ERR, no record matches, or p == i (a record never resolves to itself).  A VF whose PF is outside
+ *     the walk gets KXPU_NO_PF, no verdict, and is served as any function is;
+ *   - group_sriov[o], o < n_groups: the lowest member index i of group o (members are the accepted records) for which
+ *       (a) pf_of[i] != KXPU_NO_PF and the PF record's driver equals the driver of some rule and the PF does not carry
+ *           KXPU_REC_DRIVER_ERR (a class driver is a VFIO driver, so the VF needs the PF's VF token), or
+ *       (b) numvfs[i] > 0 (a PF with VFs enabled: its tenant would own the device other tenants' VFs live on);
+ *     KXPU_VIABLE when no member qualifies.
+ * group_ids is not read (a group's ordinal is its position in the CSR) and may be NULL.
+ * Argument checks are kxpu_classify_viable's (the rule list included); KXPU_E_INVALID, and nothing written, when
+ * group_off decreases or a member index is >= n.  Limit (else KXPU_E_UNSUPPORTED, checked before any array is read): n
+ * and n_groups below 2^30 (the address table has a power-of-two size of at least 2n slots).
+ * GPU: three launches timed under KXPU_T_CLASSIFY -- (1) one thread per record parses sriov_numvfs and inserts its
+ * canonical bdf, packed as domain << 16 | bus << 8 | dev << 3 | fn, into an open-addressing table holding the lowest
+ * index per key (atomic min); (2) one thread per record probes its physfn; (3) one thread per group member folds the
+ * verdict with an atomic min.  The records are read with 16-byte vector loads. */
+int32_t kxpu_sriov(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs,
+                   const kxpu_sriovrec *srs, size_t n, const uint32_t *group_ids, const uint32_t *group_off /* [n_groups+1] */,
+                   const uint32_t *group_members, size_t n_groups, uint32_t *pf_of /* [n] */, uint32_t *numvfs /* [n] */,
+                   uint32_t *group_sriov /* [n_groups] */);
+
+/* kxpu_pcie_tree with the VFs of a PF placed below it.  pf_of: kxpu_sriov's (n entries, each < n or KXPU_NO_PF).  The
+ * chain of a member i with pf_of[i] = p != KXPU_NO_PF, where p's path is known and p's chain is shorter than
+ * KXPU_PCIE_MAX_DEPTH, is p's chain followed by p's own node key (the function key of p's bdf): the PF becomes a node and
+ * its VFs sit below it, whatever the VF's own path says.  When p's chain already has KXPU_PCIE_MAX_DEPTH keys the longer
+ * chain would not fit, and i keeps its own chain, as in kxpu_pcie_tree; so does i when p's path is unknown.  Only one
+ * level is followed: p's own pf_of is not read.  With pf_of all KXPU_NO_PF every output is bitwise kxpu_pcie_tree's.
+ * KXPU_E_INVALID (nothing written): kxpu_pcie_tree's cases, pf_of == NULL with n > 0, or pf_of[i] >= n other than
+ * KXPU_NO_PF.  kxpu_preferred_allocation_pcie needs no change: its best fit then packs a request's VFs by PF.
+ * GPU: kxpu_pcie_tree's kernels; the parse keeps each record's own key and the longest-common-prefix pass reads a VF's
+ * chain through its PF (compile-time variants: kxpu_pcie_tree's kernels are unchanged). */
+int32_t kxpu_pcie_tree_sriov(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
+                             const uint32_t *group_off /* [n_groups+1] */, const uint32_t *group_members, size_t n_groups,
+                             uint32_t *group_node /* [n_groups] */, uint64_t *key, uint32_t *parent, uint8_t *depth,
+                             uint32_t *n_nodes, const uint32_t *pf_of /* [n] */);
 
 /* ------------------------------------------------- runtime rediscovery (ABI v6) */
 

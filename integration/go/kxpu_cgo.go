@@ -902,3 +902,79 @@ func (k *kxpu) aerHealth(text []byte, fileOff []uint64, fileLen []uint32, fatalL
 	}
 	return append([]uint8(nil), unsafe.Slice((*uint8)(unsafe.Pointer(out)), nG)...), nil
 }
+
+// SR-IOV virtual functions (additions to ABI v14, detected by symbol).  With sriovAware on, the PCI walk also reads
+// os.Readlink(<bdf>/physfn) (its basename) and the first 8 bytes of <bdf>/sriov_numvfs of every candidate of a
+// passthrough class into a kxpu_sriovrec at the record's index (sriovRecord); a missing link or file is not an error.
+// After classify, sriov gives each group's first blocking member: a group with one is sent Unhealthy, refused by
+// Allocate and NodePrepareResources, and left out of the CDI spec and the DRA pool.  The reason names the function:
+// "<vf> needs the VF token of <pf> (bound to <driver>)" when pfOf[i] is set and that PF's driver is a class driver, else
+// "<pf> has <k> VFs enabled".  With pcieTopology on too, the forest comes from pcieTreeSriov(..., pfOf).
+
+// the kxpu_sriovrec of one function from its two reads (physfnErr / numvfsErr: a failure other than "does not exist")
+func sriovRecord(physfn string, physfnErr bool, numvfs []byte, numvfsErr bool) C.kxpu_sriovrec {
+	var s C.kxpu_sriovrec
+	if len(physfn) < len(s.physfn) {
+		for i := 0; i < len(physfn); i++ {
+			s.physfn[i] = C.char(physfn[i])
+		}
+	} else {
+		physfnErr = true // no PCI address is this long
+	}
+	for i := 0; i < len(numvfs) && i < len(s.numvfs_txt); i++ {
+		s.numvfs_txt[i] = C.uint8_t(numvfs[i])
+	}
+	n := len(numvfs)
+	if n > len(s.numvfs_txt) {
+		n = len(s.numvfs_txt) + 1
+	}
+	s.numvfs_len = C.uint8_t(n)
+	if physfnErr {
+		s.flags |= C.KXPU_SR_PHYSFN_ERR
+	}
+	if numvfsErr {
+		s.flags |= C.KXPU_SR_NUMVFS_ERR
+	}
+	return s
+}
+
+// the SR-IOV verdict of a walk: recs / srs at the same indices, rules and the CSR (gids, goff, gmem) of its classify call.
+// pfOf and numvfs have one entry per record, gsriov one per group (C.KXPU_VIABLE: served).
+func (k *kxpu) sriov(rules []C.kxpu_xpu_rule, recs []C.kxpu_devrec, srs []C.kxpu_sriovrec, gids, goff, gmem []uint32) (pfOf,
+	numvfs, gsriov []uint32, err error) {
+	n, nGroups := len(recs), len(goff)-1
+	pfOf, numvfs, gsriov = make([]uint32, n+1), make([]uint32, n+1), make([]uint32, nGroups+1)
+	var r *C.kxpu_devrec
+	var s *C.kxpu_sriovrec
+	if n > 0 {
+		r, s = &recs[0], &srs[0]
+	}
+	gi, gm := append(gids, 0), append(gmem, 0) // valid pointers for an empty walk
+	err = kxCheck(k.ctx, "kxpu_sriov", C.kxpu_sriov(k.ctx, &rules[0], C.size_t(len(rules)), r, s, C.size_t(n),
+		(*C.uint32_t)(unsafe.Pointer(&gi[0])), (*C.uint32_t)(unsafe.Pointer(&goff[0])), (*C.uint32_t)(unsafe.Pointer(&gm[0])),
+		C.size_t(nGroups), (*C.uint32_t)(unsafe.Pointer(&pfOf[0])), (*C.uint32_t)(unsafe.Pointer(&numvfs[0])),
+		(*C.uint32_t)(unsafe.Pointer(&gsriov[0]))))
+	return pfOf[:n], numvfs[:n], gsriov[:nGroups], err
+}
+
+// pcieTree with every VF below its PF (pfOf: sriov's)
+func (k *kxpu) pcieTreeSriov(recs []C.kxpu_devrec, paths []C.kxpu_pcipath, goff, gmem []uint32, nGroups int,
+	pfOf []uint32) (gnode, parent []uint32, depth []uint8, err error) {
+	capN := 8*nGroups + 1
+	gnode, parent, depth = make([]uint32, nGroups+1), make([]uint32, capN), make([]uint8, capN)
+	key := make([]uint64, capN)
+	var nn C.uint32_t
+	var r unsafe.Pointer
+	var pp *C.kxpu_pcipath
+	pf := append(pfOf, 0) // a valid pointer for an empty walk
+	if len(recs) > 0 {
+		r, pp = unsafe.Pointer(&recs[0]), &paths[0]
+	}
+	gm := append(gmem, 0)
+	err = kxCheck(k.ctx, "kxpu_pcie_tree_sriov", C.kxpu_pcie_tree_sriov(k.ctx, (*C.kxpu_devrec)(r), pp, C.size_t(len(recs)),
+		(*C.uint32_t)(unsafe.Pointer(&goff[0])), (*C.uint32_t)(unsafe.Pointer(&gm[0])), C.size_t(nGroups),
+		(*C.uint32_t)(unsafe.Pointer(&gnode[0])), (*C.uint64_t)(unsafe.Pointer(&key[0])),
+		(*C.uint32_t)(unsafe.Pointer(&parent[0])), (*C.uint8_t)(unsafe.Pointer(&depth[0])), &nn,
+		(*C.uint32_t)(unsafe.Pointer(&pf[0]))))
+	return gnode[:nGroups], parent[:nn], depth[:nn], err
+}

@@ -74,6 +74,12 @@ DRA_MAX_TAINTS = 4  # entries of the _taints calls' table (ABI v12)
 AER_FATAL, AER_NONFATAL, AER_UNKNOWN = 1, 2, 4  # kxpu_aer_health's group bits
 AER_FILE_MAX = 4096
 AER_UNKNOWN_COUNT = (1 << 64) - 1  # totals of an unknown count
+# kxpu_sriovrec (SR-IOV virtual functions, an addition to ABI v14): one per kxpu_devrec, at the same index
+SRIOVREC_DTYPE = np.dtype([("physfn", "S16"), ("numvfs_txt", "u1", (8,)), ("numvfs_len", "u1"), ("flags", "u1"),
+                           ("reserved", "u1", (6,))])
+assert SRIOVREC_DTYPE.itemsize == 32
+SR_PHYSFN_ERR, SR_NUMVFS_ERR = 1, 2
+NO_PF = 0xFFFFFFFF
 CDI_FRAG_MIN = 166  # the shortest device fragment of a CDI spec: len // CDI_FRAG_MIN records hold any document (ABI v13)
 
 
@@ -98,6 +104,7 @@ ABI_SYMBOLS = [
     "kxpu_dra_slices", "kxpu_dra_slices_mdev", "kxpu_dra_slices_taint", "kxpu_dra_slices_mdev_taint",
     "kxpu_aer_health", "kxpu_dra_slices_taints", "kxpu_dra_slices_mdev_taints", "kxpu_cdi_parse", "kxpu_cdi_parse_mdev",
     "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev", "kxpu_cdi_emit_mdev_cdev", "kxpu_cdi_parse_mdev_cdev",
+    "kxpu_sriov", "kxpu_pcie_tree_sriov",
 ]
 
 
@@ -212,6 +219,8 @@ def load_library():
         "kxpu_cdi_parse_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_cdi_emit_mdev_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_cdi_parse_mdev_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_sriov": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp, sz, vp, vp, vp]),
+        "kxpu_pcie_tree_sriov": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32), vp]),
         "kxpu_dra_slices_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                          C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_mdev_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
@@ -609,9 +618,28 @@ class Kxpu:
                                                    _ptr(a["must"]), _ptr(a["size"]), len(a["size"]), _ptr(out),
                                                    _ptr(out_off)))
 
-    def pcie_tree(self, recs, paths, group_off, group_members):
+    def sriov(self, rules, recs, srs, group_ids, group_off, group_members):
+        """kxpu_sriov: recs (DEVREC_DTYPE) and srs (SRIOVREC_DTYPE) at the same indices, the rules and group CSR of a
+        classify call.  Returns dict(pf_of, numvfs, group_sriov)."""
+        ra = rules_array(rules)
+        recs, srs = np.ascontiguousarray(recs), np.ascontiguousarray(srs)
+        assert recs.dtype == DEVREC_DTYPE and srs.dtype == SRIOVREC_DTYPE and len(recs) == len(srs)
+        group_ids = np.ascontiguousarray(group_ids, dtype=np.uint32)
+        group_off = np.ascontiguousarray(group_off, dtype=np.uint32)
+        group_members = np.ascontiguousarray(group_members, dtype=np.uint32)
+        n, G = len(recs), len(group_off) - 1
+        pf_of, numvfs = np.empty(max(n, 1), np.uint32), np.empty(max(n, 1), np.uint32)
+        gs = np.empty(max(G, 1), np.uint32)
+        self._chk(self.L.kxpu_sriov(self.ctx, _ptr(ra) if len(ra) else None, len(ra), _ptr(recs) if n else None,
+                                    _ptr(srs) if n else None, n, _ptr(group_ids) if len(group_ids) else None, _ptr(group_off),
+                                    _ptr(group_members) if len(group_members) else None, G, _ptr(pf_of), _ptr(numvfs),
+                                    _ptr(gs)))
+        return dict(pf_of=pf_of[:n], numvfs=numvfs[:n], group_sriov=gs[:G])
+
+    def pcie_tree(self, recs, paths, group_off, group_members, pf_of=None):
         """kxpu_pcie_tree: recs (DEVREC_DTYPE) and paths (PCIPATH_DTYPE) at the same indices, the group CSR of a classify
-        call.  Returns dict(group_node, key, parent, depth), the forest trimmed to its node count."""
+        call.  Returns dict(group_node, key, parent, depth), the forest trimmed to its node count.  With pf_of (kxpu_sriov's,
+        one per record): kxpu_pcie_tree_sriov."""
         recs, paths = np.ascontiguousarray(recs), np.ascontiguousarray(paths)
         assert recs.dtype == DEVREC_DTYPE and paths.dtype == PCIPATH_DTYPE and len(recs) == len(paths)
         group_off = np.ascontiguousarray(group_off, dtype=np.uint32)
@@ -622,9 +650,15 @@ class Kxpu:
         key, parent, depth = np.empty(cap, np.uint64), np.empty(cap, np.uint32), np.empty(cap, np.uint8)
         nn = C.c_uint32(0)
         n = len(recs)
-        self._chk(self.L.kxpu_pcie_tree(self.ctx, _ptr(recs) if n else None, _ptr(paths) if n else None, n,
-                                        _ptr(group_off), _ptr(group_members) if len(group_members) else None, G,
-                                        _ptr(gnode), _ptr(key), _ptr(parent), _ptr(depth), C.byref(nn)))
+        args = (self.ctx, _ptr(recs) if n else None, _ptr(paths) if n else None, n, _ptr(group_off),
+                _ptr(group_members) if len(group_members) else None, G, _ptr(gnode), _ptr(key), _ptr(parent), _ptr(depth),
+                C.byref(nn))
+        if pf_of is None:
+            self._chk(self.L.kxpu_pcie_tree(*args))
+        else:
+            pf_of = np.ascontiguousarray(pf_of, dtype=np.uint32)
+            assert len(pf_of) == n
+            self._chk(self.L.kxpu_pcie_tree_sriov(*args, _ptr(pf_of) if n else None))
         m = nn.value
         return dict(group_node=gnode[:G], key=key[:m], parent=parent[:m], depth=depth[:m])
 

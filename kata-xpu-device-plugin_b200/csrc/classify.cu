@@ -744,6 +744,16 @@ extern "C" int32_t kxpu_classify_viable(kxpu_ctx *ctx, const kxpu_xpu_rule *rule
     return classify_run(ctx, recs, n, out, &R, false, dev_rule, group_numa, group_blocker);
 }
 
+int32_t kx_rule_drivers(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, unsigned long long drv[][4]) {
+    RuleTable R;
+    const int32_t rc = rule_table(ctx, rules, n_rules, R);
+    if (rc != KXPU_OK) return rc;
+    for (size_t r = 0; r < n_rules; r++) {
+        drv[r][0] = R.d0[r]; drv[r][1] = R.d1[r]; drv[r][2] = R.m0[r]; drv[r][3] = R.m1[r];
+    }
+    return KXPU_OK;
+}
+
 static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
                              bool mdev, uint8_t *dev_rule, uint64_t *group_numa, uint32_t *group_blocker, bool small_dtab,
                              bool *retry) {

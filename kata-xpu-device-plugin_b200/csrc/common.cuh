@@ -97,6 +97,11 @@ static inline void kx_clear_timings(kxpu_ctx *c) { memset(c->ev_used, 0, sizeof(
 unsigned long long *kx_scan_state(kxpu_ctx *ctx, size_t words);
 uint32_t kx_next_epoch(kxpu_ctx *ctx);
 
+// kxpu_classify_rules' rule-list check (classify.cu), for the calls that take the same list: KXPU_E_INVALID with a
+// message for an invalid list, else per rule the driver field as two words and the masks that cover its bytes and its
+// NUL: drv[r] = {d0, d1, m0, m1}, and a 16-byte driver field f matches rule r when (f0 & m0) == d0 && (f1 & m1) == d1
+int32_t kx_rule_drivers(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, unsigned long long drv[][4]);
+
 // stream-ordered scratch that is released on every path out of a call
 struct KxScratch {
     kxpu_ctx *c;

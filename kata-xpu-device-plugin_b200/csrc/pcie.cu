@@ -13,6 +13,8 @@
 //   - the single-pass scan (scan.cuh) of the new-node counts gives each group's first ordinal; the total is n_nodes.
 //   - k_emit: ordinal of prefix (g, t) = base[f] + t - (len(f) - new(f)), f its first group; a group writes key,
 //     parent and depth of its own new nodes and its group_node.
+// kxpu_pcie_tree_sriov runs the same launches with k_parse<true> (which also stores each record's own key) and
+// k_lcp<true> (which reads a VF's chain through its PF); the <false> instantiations are kxpu_pcie_tree's kernels.
 #include <algorithm>
 
 #include "common.cuh"
@@ -63,9 +65,12 @@ __device__ int parse_comp(const char *t, int s, int e, unsigned long long *key) 
     return 1;
 }
 
-// chain[i * MAXD + t] = key of component t of record i, clen[i] = chain length (0: unknown path)
+// chain[i * MAXD + t] = key of component t of record i, clen[i] = chain length (0: unknown path).  SR
+// (kxpu_pcie_tree_sriov): self[i] = the key of the record's own component when its path is known.
+template <bool SR>
 __global__ void __launch_bounds__(PARSE_THREADS) k_parse(const kxpu_devrec *__restrict__ recs, const kxpu_pcipath *__restrict__ paths,
-                                                         uint32_t n, unsigned long long *__restrict__ chain, uint8_t *__restrict__ clen) {
+                                                         uint32_t n, unsigned long long *__restrict__ chain, uint8_t *__restrict__ clen,
+                                                         unsigned long long *__restrict__ self) {
     __shared__ __align__(16) char txt[PARSE_RECS][128];
     const uint32_t lane = threadIdx.x & (PATH_LANES - 1), slot = threadIdx.x / PATH_LANES;
     const uint32_t i = blockIdx.x * PARSE_RECS + slot;
@@ -106,6 +111,9 @@ __global__ void __launch_bounds__(PARSE_THREADS) k_parse(const kxpu_devrec *__re
     ok = ok && bad == 0;
     if (!have) return;
     if (ok && (int)lane < ncomp - 1) chain[(size_t)i * MAXD + lane] = key;
+    if constexpr (SR) {
+        if (ok && (int)lane == ncomp - 1) self[i] = key;
+    }
     if (lane == 0) clen[i] = ok ? (uint8_t)(ncomp - 1) : 0;
 }
 
@@ -124,8 +132,13 @@ struct Tree {
     unsigned long long *key;
     uint8_t *depth;
     uint32_t *err;               // [0] = 1: a member index >= n
+    // kxpu_pcie_tree_sriov only: the PF of every record (each < n or NO_PF) and every record's own key
+    const uint32_t *pf_of;
+    const unsigned long long *self;
 };
 
+// SR: a member whose PF has a known chain shorter than MAXD reads the PF's chain followed by the PF's own key
+template <bool SR>
 __global__ void __launch_bounds__(256) k_lcp(const Tree T) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= T.G) return;
@@ -135,14 +148,26 @@ __global__ void __launch_bounds__(256) k_lcp(const Tree T) {
     for (uint32_t m = T.goff[g]; m < T.goff[g + 1]; m++) {
         const uint32_t i = T.gmem[m];
         if (i >= T.n) { bad = true; continue; }
-        const int l = T.clen[i];
-        if (!l) continue;
+        int l = T.clen[i];
         const unsigned long long *c = T.chain + (size_t)i * MAXD;
+        unsigned long long tail = 0;  // SR, through the PF (via): the key at position l - 1
+        bool via = false;
+        if constexpr (SR) {
+            const uint32_t p = T.pf_of[i];
+            const int pl = p == KXPU_NO_PF ? 0 : T.clen[p];
+            if (pl > 0 && pl < MAXD) {
+                c = T.chain + (size_t)p * MAXD;
+                l = pl + 1;
+                tail = T.self[p];
+                via = true;
+            }
+        }
+        if (!l) continue;
         int nl = L < 0 ? l : min(L, l);
 #pragma unroll
         for (int t = 0; t < MAXD; t++) {
             if (t >= nl) continue;
-            const unsigned long long x = c[t];
+            const unsigned long long x = SR && via && t == l - 1 ? tail : c[t];
             if (L < 0) k[t] = x;
             else if (x != k[t]) nl = min(nl, t);
         }
@@ -233,9 +258,10 @@ __global__ void __launch_bounds__(256) k_emit(const Tree T) {
 
 using namespace kxpcie;
 
-extern "C" int32_t kxpu_pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
-                                  const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
-                                  uint32_t *group_node, uint64_t *key, uint32_t *parent, uint8_t *depth, uint32_t *n_nodes) {
+// pf_of == nullptr: kxpu_pcie_tree; else kxpu_pcie_tree_sriov (pf_of checked by the caller)
+static int32_t pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n, const uint32_t *group_off,
+                         const uint32_t *group_members, size_t n_groups, uint32_t *group_node, uint64_t *key, uint32_t *parent,
+                         uint8_t *depth, uint32_t *n_nodes, const uint32_t *pf_of) {
     static_assert(sizeof(kxpu_pcipath) == 128 && offsetof(kxpu_pcipath, len) == 120, "kxpu_pcipath layout");
     if (!ctx || !n_nodes || (n && (!recs || !paths)) || !group_off) return KXPU_E_INVALID;
     if (n >= (1ull << 28) || n_groups >= (1ull << 28)) return KXPU_E_UNSUPPORTED;
@@ -260,6 +286,7 @@ extern "C" int32_t kxpu_pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const 
     const size_t o_gchain = take(GD * 8), o_glen = take(G), o_slots = take((size_t)slots * 8), o_first = take(GD * 4);
     const size_t o_cnt = take(G * 4), o_base = take(G * 4), o_gnode = take(G * 4), o_parent = take(GD * 4);
     const size_t o_key = take(GD * 8), o_depth = take(GD), o_err = take(8 + 8);
+    const size_t o_pf = pf_of ? take(n * 4) : 0, o_self = pf_of ? take(n * 8) : 0;
     KxScratch sc(ctx);
     uint8_t *b = nullptr;
     KX_CUDA(ctx, sc.alloc((void **)&b, off));
@@ -267,6 +294,7 @@ extern "C" int32_t kxpu_pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const 
     auto up = [&](size_t o, const void *h, size_t bytes) { if (bytes) cudaMemcpyAsync(b + o, h, bytes, cudaMemcpyHostToDevice, st); };
     up(o_recs, recs, n * sizeof(kxpu_devrec)); up(o_paths, paths, n * sizeof(kxpu_pcipath));
     up(o_goff, group_off, (G + 1) * 4); up(o_gmem, group_members, nm * 4);
+    if (pf_of) up(o_pf, pf_of, n * 4);
     cudaMemsetAsync(b + o_slots, 0xFF, (size_t)slots * 8, st);
     cudaMemsetAsync(b + o_err, 0, 16, st);
     Tree T;
@@ -278,17 +306,20 @@ extern "C" int32_t kxpu_pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const 
     T.first = (uint32_t *)(b + o_first); T.cnt = (uint32_t *)(b + o_cnt); T.base = (uint32_t *)(b + o_base);
     T.group_node = (uint32_t *)(b + o_gnode); T.parent = (uint32_t *)(b + o_parent);
     T.key = (unsigned long long *)(b + o_key); T.depth = b + o_depth; T.err = (uint32_t *)(b + o_err);
+    T.pf_of = pf_of ? (const uint32_t *)(b + o_pf) : nullptr;
+    T.self = pf_of ? (const unsigned long long *)(b + o_self) : nullptr;
     unsigned long long *d_total = (unsigned long long *)(b + o_err + 8);
     {
         KxTimer tm(ctx, KXPU_T_CLASSIFY);
         if (n) {
-            k_parse<<<(unsigned)((n + PARSE_RECS - 1) / PARSE_RECS), PARSE_THREADS, 0, st>>>(
+            auto *parse = pf_of ? k_parse<true> : k_parse<false>;
+            parse<<<(unsigned)((n + PARSE_RECS - 1) / PARSE_RECS), PARSE_THREADS, 0, st>>>(
                 (const kxpu_devrec *)(b + o_recs), (const kxpu_pcipath *)(b + o_paths), (uint32_t)n,
-                (unsigned long long *)(b + o_chain), b + o_clen);
+                (unsigned long long *)(b + o_chain), b + o_clen, (unsigned long long *)(b + o_self));
             ctx->launches++;
         }
         const unsigned gb = (unsigned)((G + 255) / 256);
-        k_lcp<<<gb, 256, 0, st>>>(T);
+        (pf_of ? k_lcp<true> : k_lcp<false>)<<<gb, 256, 0, st>>>(T);
         k_insert<<<gb, 256, 0, st>>>(T);
         k_count<<<gb, 256, 0, st>>>(T);
         ctx->launches += 3;
@@ -314,4 +345,26 @@ extern "C" int32_t kxpu_pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const 
     if (e != cudaSuccess) { KX_SET_ERR(ctx, "pcie_tree D2H failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
     *n_nodes = nn;
     return KXPU_OK;
+}
+
+extern "C" int32_t kxpu_pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
+                                  const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
+                                  uint32_t *group_node, uint64_t *key, uint32_t *parent, uint8_t *depth, uint32_t *n_nodes) {
+    return pcie_tree(ctx, recs, paths, n, group_off, group_members, n_groups, group_node, key, parent, depth, n_nodes, nullptr);
+}
+
+extern "C" int32_t kxpu_pcie_tree_sriov(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
+                                        const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
+                                        uint32_t *group_node, uint64_t *key, uint32_t *parent, uint8_t *depth,
+                                        uint32_t *n_nodes, const uint32_t *pf_of) {
+    if (!ctx || (n && !pf_of)) return KXPU_E_INVALID;
+    if (n >= (1ull << 28)) return KXPU_E_UNSUPPORTED;
+    for (size_t i = 0; i < n; i++)
+        if (pf_of[i] != KXPU_NO_PF && pf_of[i] >= n) {
+            KX_SET_ERR(ctx, "pcie_tree_sriov: pf_of[%zu] = %u is >= n", i, pf_of[i]);
+            return KXPU_E_INVALID;
+        }
+    static const uint32_t none = KXPU_NO_PF;  // n == 0: nothing to upload, but still the variant
+    return pcie_tree(ctx, recs, paths, n, group_off, group_members, n_groups, group_node, key, parent, depth, n_nodes,
+                     n ? pf_of : &none);
 }

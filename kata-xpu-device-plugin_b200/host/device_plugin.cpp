@@ -408,13 +408,15 @@ static Error walkDir(Plugin &p, const std::string &path, const std::string &name
     return Error();
 }
 
-Error Plugin::gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pcipath> *paths, std::vector<int64_t> *cdevs) {
+Error Plugin::gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pcipath> *paths, std::vector<int64_t> *cdevs,
+                            std::vector<kxpu_sriovrec> *srs) {
     recs.clear();
     if (paths) paths->clear();
     size_t slash = basePath.find_last_of('/');
     Error e = walkDir(*this, basePath, slash == std::string::npos ? basePath : basePath.substr(slash + 1), recs,
                       readsPaths() ? paths : nullptr);
     readCdevs(recs, cdevs);
+    readSriovs(recs, srs);
     return e;
 }
 
@@ -452,7 +454,7 @@ int64_t Plugin::readVfioCdev(const std::string &base, const std::string &entry) 
     return v < (1ull << 32) ? (int64_t)v : -1;
 }
 
-// does a record with this vendor and driver match a class that sets `flag` (vfioCdev or mdevCdev)?
+// does a record with this vendor and driver match a class that sets `flag` (vfioCdev or mdevCdev; nullptr: any class)?
 template <typename Rec>
 static bool cdevClassOf(const std::vector<XpuClass> &classes, bool XpuClass::*flag, const Rec &r, const uint8_t *vendorTxt,
                         size_t vendorCap) {
@@ -460,7 +462,7 @@ static bool cdevClassOf(const std::vector<XpuClass> &classes, bool XpuClass::*fl
     const std::string vendor = trimID(std::string((const char *)vendorTxt, std::min<size_t>(r.vendor_len, vendorCap)));
     const std::string drv(r.driver, strnlen(r.driver, sizeof r.driver));
     bool match = false;
-    for (const XpuClass &c : classes) match |= c.*flag && c.vendor == vendor && c.driver == drv;
+    for (const XpuClass &c : classes) match |= (!flag || c.*flag) && c.vendor == vendor && c.driver == drv;
     return match;
 }
 
@@ -477,6 +479,51 @@ void Plugin::readCdevs(const std::vector<kxpu_devrec> &recs, std::vector<int64_t
     }
 }
 
+kxpu_sriovrec Plugin::readSriov(const std::string &bdf) {
+    sriovReads++;
+    kxpu_sriovrec s;
+    memset(&s, 0, sizeof s);
+    const std::string dir = basePath + "/" + bdf + "/";
+    char buf[4096];
+    const ssize_t n = readlink((dir + "physfn").c_str(), buf, sizeof buf - 1);
+    if (n >= 0) {
+        const std::string target(buf, (size_t)n);
+        const size_t slash = target.find_last_of('/');
+        const std::string pf = slash == std::string::npos ? target : target.substr(slash + 1);
+        if (pf.size() < sizeof s.physfn) memcpy(s.physfn, pf.data(), pf.size());
+        else s.flags |= KXPU_SR_PHYSFN_ERR;  // no PCI address is this long
+    } else if (errno != ENOENT) {
+        s.flags |= KXPU_SR_PHYSFN_ERR;
+    }
+    FILE *f = fopen((dir + "sriov_numvfs").c_str(), "rb");
+    if (f) {
+        uint8_t txt[sizeof s.numvfs_txt + 1];
+        const size_t got = fread(txt, 1, sizeof txt, f);
+        if (ferror(f)) s.flags |= KXPU_SR_NUMVFS_ERR;
+        fclose(f);
+        memcpy(s.numvfs_txt, txt, std::min(got, sizeof s.numvfs_txt));
+        s.numvfs_len = (uint8_t)got;  // 9: longer than the record holds
+    } else if (errno != ENOENT) {
+        s.flags |= KXPU_SR_NUMVFS_ERR;
+    }
+    return s;
+}
+
+// the SR-IOV reads of every candidate of a passthrough class, after either gather
+void Plugin::readSriovs(const std::vector<kxpu_devrec> &recs, std::vector<kxpu_sriovrec> *srs) {
+    if (!srs) return;
+    srs->clear();
+    if (!sriovAware) return;
+    kxpu_sriovrec zero;
+    memset(&zero, 0, sizeof zero);
+    srs->assign(recs.size(), zero);
+    for (size_t i = 0; i < recs.size(); i++) {
+        const kxpu_devrec &r = recs[i];
+        if (!(r.flags & KXPU_REC_IOMMU_ERR) && cdevClassOf(xpuClasses, nullptr, r, r.vendor_txt, sizeof r.vendor_txt))
+            (*srs)[i] = readSriov(std::string(r.bdf, strnlen(r.bdf, sizeof r.bdf)));
+    }
+}
+
 // ---------------------------------------------------------------------------- SURVEY 8(f) row 2
 // Batched sysfs ingestion: the same records as gatherRecords, but the entries of basePath are read
 // with paths RELATIVE to one directory descriptor (openat / readlinkat on "<bdf>/vendor": no lstat per
@@ -485,9 +532,10 @@ void Plugin::readCdevs(const std::vector<kxpu_devrec> &recs, std::vector<int64_t
 // in one contiguous table ready for a single H2D copy.  Only with the default seams; real directories
 // under basePath (never on sysfs) go through the generic walk at their position.
 Error Plugin::gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads, std::vector<kxpu_pcipath> *paths,
-                                std::vector<int64_t> *cdevs) {
+                                std::vector<int64_t> *cdevs, std::vector<kxpu_sriovrec> *srs) {
     Error e = gatherRecordsFastWalk(recs, threads, paths);
     readCdevs(recs, cdevs);
+    readSriovs(recs, srs);
     return e;
 }
 
@@ -737,9 +785,35 @@ static kxpu_dradev draRecord(const kxpu_devrec &r, const kxpu_pcipath *path, uin
     return d;
 }
 
+static bool isClassDriver(const std::vector<XpuClass> &classes, const std::string &driver) {
+    for (const XpuClass &c : classes)
+        if (c.driver == driver) return true;
+    return false;
+}
+
+static std::string sriovVfReason(const std::string &vf, const std::string &pf, const std::string &driver) {
+    return vf + " needs the VF token of " + pf + " (bound to " + driver + ")";
+}
+static std::string sriovPfReason(const std::string &pf, uint32_t numvfs) {
+    return pf + " has " + std::to_string(numvfs) + " VFs enabled";
+}
+
+// the reason kxpu_sriov blocked on record i of a walk: a VF whose PF is bound to a class driver, else a PF with VFs
+static std::string sriovReasonOf(const std::vector<XpuClass> &classes, const PciWalk &w, uint32_t i) {
+    const kxpu_devrec &r = w.recs[i];
+    const std::string me(r.bdf, strnlen(r.bdf, sizeof r.bdf));
+    if (w.pfOf[i] != KXPU_NO_PF) {
+        const kxpu_devrec &pf = w.recs[w.pfOf[i]];
+        const std::string drv(pf.driver, strnlen(pf.driver, sizeof pf.driver));
+        if (!(pf.flags & KXPU_REC_DRIVER_ERR) && isClassDriver(classes, drv))
+            return sriovVfReason(me, std::string(pf.bdf, strnlen(pf.bdf, sizeof pf.bdf)), drv);
+    }
+    return sriovPfReason(me, w.numvfs[i]);
+}
+
 // the walk and classify of createIommuDeviceMap
 Error Plugin::classifyPci(PciWalk &w) {
-    Error e = gatherRecordsFast(w.recs, 0, &w.paths, &w.cdevs);  // same records as gatherRecords (falls back to it when a seam was replaced)
+    Error e = gatherRecordsFast(w.recs, 0, &w.paths, &w.cdevs, &w.srs);  // same records as gatherRecords (falls back to it when a seam was replaced)
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // Walk's error is ignored by the reference (:132)
     const std::vector<kxpu_devrec> &recs = w.recs;
     const size_t n = recs.size();
@@ -766,13 +840,30 @@ Error Plugin::classifyPci(PciWalk &w) {
         for (uint32_t g = 0; g < c.nGroups; g++)
             if (c.gblk[g] != KXPU_VIABLE)
                 fprintf(stderr, "IOMMU group %u is not viable: %s\n", c.gids[g], blockerOf(recs[c.gblk[g]]).c_str());
-    if (pcieTopologyAware) {  // the forest of the walk, one node per group
+    if (sriovAware) {  // the SR-IOV verdict of every group, on the classify CSR
+        w.pfOf.assign(n ? n : 1, KXPU_NO_PF);
+        w.numvfs.assign(n ? n : 1, 0);
+        w.gsriov.assign(c.nGroups + 1, KXPU_VIABLE);
+        rc = kxpu_sriov(ctx_, rules.data(), rules.size(), recs.data(), w.srs.data(), n, c.gids.data(), c.goff.data(),
+                        c.gmem.data(), c.nGroups, w.pfOf.data(), w.numvfs.data(), w.gsriov.data());
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_sriov", rc);
+        for (uint32_t g = 0; g < c.nGroups; g++)
+            if (w.gsriov[g] != KXPU_VIABLE)
+                fprintf(stderr, "IOMMU group %u is not served: %s\n", c.gids[g], sriovReasonOf(xpuClasses, w, w.gsriov[g]).c_str());
+    }
+    if (pcieTopologyAware) {  // the forest of the walk, one node per group; sriovAware: VFs below their PF
         const size_t cap = (size_t)KXPU_PCIE_MAX_DEPTH * c.nGroups + 1;
         w.gnode.assign(c.nGroups + 1, KXPU_PCIE_NO_NODE);
         w.nodeKey.assign(cap, 0); w.nodeParent.assign(cap, 0); w.nodeDepth.assign(cap, 0);
-        rc = kxpu_pcie_tree(ctx_, recs.data(), w.paths.data(), n, c.goff.data(), c.gmem.data(), c.nGroups, w.gnode.data(),
-                            w.nodeKey.data(), w.nodeParent.data(), w.nodeDepth.data(), &w.nNodes);
-        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_pcie_tree", rc);
+        if (sriovAware) {
+            rc = kxpu_pcie_tree_sriov(ctx_, recs.data(), w.paths.data(), n, c.goff.data(), c.gmem.data(), c.nGroups,
+                                      w.gnode.data(), w.nodeKey.data(), w.nodeParent.data(), w.nodeDepth.data(), &w.nNodes,
+                                      w.pfOf.data());
+        } else {
+            rc = kxpu_pcie_tree(ctx_, recs.data(), w.paths.data(), n, c.goff.data(), c.gmem.data(), c.nGroups, w.gnode.data(),
+                                w.nodeKey.data(), w.nodeParent.data(), w.nodeDepth.data(), &w.nNodes);
+        }
+        if (rc != KXPU_OK) return kxfail(ctx_, sriovAware ? "kxpu_pcie_tree_sriov" : "kxpu_pcie_tree", rc);
     }
     return Error();
 }
@@ -785,6 +876,7 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
     iommuNuma.clear();
     iommuPcieNode.clear();
     iommuBlocker.clear();
+    iommuSriov.clear();
     iommuDra.clear();
     const ClassifyResult &c = w.out;
     std::map<uint32_t, size_t> groupClass = groupClasses(c);
@@ -802,11 +894,15 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
         if (blocker.empty() && xpuClasses[groupClass[c.gids[g]]].vfioCdev)  // a member without a cdev: VFIO cannot open it
             for (const NvidiaGpuDevice &d : devs)
                 if (d.cdev < 0) { blocker = d.addr + " has no VFIO cdev"; break; }
+        if (sriovAware) {
+            iommuSriov.push_back(w.gsriov[g] == KXPU_VIABLE ? std::string() : sriovReasonOf(xpuClasses, w, w.gsriov[g]));
+            if (blocker.empty()) blocker = iommuSriov.back();
+        }
         iommuMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
         iommuClass.push_back(groupClass[c.gids[g]]);
         if (topologyAware) iommuNuma.push_back(c.gnuma[g]);
         if (pcieTopologyAware) iommuPcieNode.push_back(w.gnode[g]);
-        if (groupViability || cdevEnabled()) iommuBlocker.push_back(blocker);
+        if (groupViability || cdevEnabled() || sriovAware) iommuBlocker.push_back(blocker);
         if (draEnabled()) {
             const uint32_t first = c.gmem[c.goff[g]];
             iommuDra.push_back(draRecord(w.recs[first], w.paths.size() > first ? &w.paths[first] : nullptr, c.gnuma[g]));
@@ -1389,13 +1485,20 @@ Error Plugin::generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m,
     cdiFiles.clear();
     std::map<std::string, size_t> classOf;  // group -> class, from the maps of the last walk
     for (size_t g = 0; g < iommuMap.size() && g < iommuClass.size(); g++) classOf.emplace(iommuMap[g].first, iommuClass[g]);
+    std::set<std::string> withheld;  // sriovAware: a group with an SR-IOV reason, which VFIO would refuse to open
+    for (size_t g = 0; g < iommuSriov.size() && g < iommuMap.size(); g++)
+        if (!iommuSriov[g].empty()) withheld.insert(iommuMap[g].first);
+    OrderedMap<std::vector<NvidiaGpuDevice>> served;  // m without them (only built when some group is withheld)
     std::vector<size_t> entryClass;
     for (const auto &kv : m) {
+        if (withheld.count(kv.first)) continue;
+        if (!withheld.empty()) served.push_back(kv);
         auto it = classOf.find(kv.first);
         entryClass.push_back(it == classOf.end() ? 0 : it->second);
     }
     const int32_t fmt = format == "YAML" ? KXPU_FMT_YAML : KXPU_FMT_JSON;  // spec.go:86-89,102-114
-    Error e = generateClassSpecs(xpuClasses, m, entryClass, fmt, "kxpu_cdi_emit_kind", kxpu_cdi_emit_kind, cdiFiles);
+    Error e = generateClassSpecs(xpuClasses, withheld.empty() ? m : served, entryClass, fmt, "kxpu_cdi_emit_kind",
+                                 kxpu_cdi_emit_kind, cdiFiles);
     if (!cdiFiles.empty()) lastCdiFile = cdiFiles.back();
     return e;
 }
@@ -1880,6 +1983,44 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     return Error();
 }
 
+// kxpu_sriov's canonical PCI address: "dddd:bb:dd.f", lowercase hex, device at most 1f, function 0..7
+static bool canonicalBdf(const std::string &a) {
+    if (a.size() != 12 || a[4] != ':' || a[7] != ':' || a[10] != '.' || a[11] < '0' || a[11] > '7' || a[8] > '1') return false;
+    for (int k : {0, 1, 2, 3, 5, 6, 8, 9})
+        if (!((a[k] >= '0' && a[k] <= '9') || (a[k] >= 'a' && a[k] <= 'f'))) return false;
+    return true;
+}
+
+// kxpu_sriov's sriov_numvfs rule: at most one trailing '\n', then a canonical decimal 0..65535; anything else 0
+static uint32_t parseNumvfs(const kxpu_sriovrec &s) {
+    if ((s.flags & KXPU_SR_NUMVFS_ERR) || s.numvfs_len > sizeof s.numvfs_txt) return 0;
+    std::string t((const char *)s.numvfs_txt, s.numvfs_len);
+    if (!t.empty() && t.back() == '\n') t.pop_back();
+    if (t.empty() || t.size() > 5 || (t.size() > 1 && t[0] == '0')) return 0;
+    uint32_t v = 0;
+    for (char ch : t) {
+        if (ch < '0' || ch > '9') return 0;
+        v = v * 10 + (uint32_t)(ch - '0');
+    }
+    return v <= 65535 ? v : 0;
+}
+
+std::string Plugin::sriovLive(const std::string &bdf) {
+    const kxpu_sriovrec s = readSriov(bdf);
+    const std::string pf(s.physfn, strnlen(s.physfn, sizeof s.physfn));
+    if (!(s.flags & KXPU_SR_PHYSFN_ERR) && canonicalBdf(pf) && pf != bdf) {
+        char buf[4096];
+        const ssize_t n = readlink((basePath + "/" + pf + "/driver").c_str(), buf, sizeof buf - 1);
+        if (n >= 0) {
+            const std::string target(buf, (size_t)n);
+            const std::string drv = target.substr(target.find_last_of('/') + 1);  // npos + 1 == 0
+            if (isClassDriver(xpuClasses, drv)) return sriovVfReason(bdf, pf, drv);
+        }
+    }
+    const uint32_t k = parseNumvfs(s);
+    return k ? sriovPfReason(bdf, k) : std::string();
+}
+
 // Allocate, generic_device_plugin.go:320-355, for one ContainerAllocateRequest
 Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllocateResponse &resp) {
     std::shared_lock<std::shared_mutex> lock(mu_);  // a rediscovery rebuilds the maps under the exclusive lock
@@ -1945,6 +2086,10 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
                 return fail("invalid allocation request: unknown device: " + dev.addr);
             if (xpuClasses[c].vfioCdev && readVfioCdev(basePath, dev.addr) != dev.cdev)  // cdev numbers are reused across re-binds
                 return fail("invalid allocation request: the VFIO cdev of " + dev.addr + " changed since discovery");
+            if (sriovAware) {  // a PF rebound, or VFs enabled, since the walk
+                const std::string why = sriovLive(dev.addr);
+                if (!why.empty()) return fail("invalid allocation request: " + why);
+            }
             devIndexes.push_back(dev.index);  // :340
         }
     }
@@ -2676,6 +2821,32 @@ static void jsnap(std::string &o, const std::vector<kxpu_snaprec> &snap) {
              ',' + std::to_string(snap[i].index) + ']';
     }
     o += ']';
+}
+
+void kxh_set_sriov(void *h, int on) { ((Plugin *)h)->sriovAware = on != 0; }
+uint64_t kxh_sriov_reads(void *h) { return ((Plugin *)h)->sriovReads; }
+
+// CPU only: the raw PCI gather under a class list with sriovAware = on, its SR-IOV side records and sriovReads
+int kxh_gather_sriov(const char *base_path, const char *classes, int on, int fast, unsigned threads, kxpu_devrec *out,
+                     kxpu_sriovrec *srs, size_t cap, size_t *n, uint64_t *reads, char *err, size_t errcap) {
+    Plugin p(nullptr);
+    p.basePath = base_path;
+    p.sriovAware = on != 0;
+    if (!parseClasses(classes, p.xpuClasses)) { copy_out("malformed class list", err, errcap); return -1; }
+    std::vector<kxpu_devrec> recs;
+    std::vector<kxpu_sriovrec> sr;
+    device_plugin::Error e = fast ? p.gatherRecordsFast(recs, threads, nullptr, nullptr, &sr)
+                                  : p.gatherRecords(recs, nullptr, nullptr, &sr);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    *n = recs.size();
+    *reads = p.sriovReads;
+    if (recs.size() > cap) return -2;
+    memcpy(out, recs.data(), recs.size() * sizeof(kxpu_devrec));
+    for (size_t i = 0; i < recs.size(); i++) {
+        if (sr.empty()) memset(&srs[i], 0, sizeof srs[i]);
+        else srs[i] = sr[i];
+    }
+    return 0;
 }
 
 // the state kxh_init reports, without the closing brace

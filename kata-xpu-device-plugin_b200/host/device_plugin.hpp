@@ -241,6 +241,10 @@ struct PciWalk {
     uint32_t nNodes = 0;
     // some class has vfioCdev: per record, N of its VFIO cdev, -1 = none or not read
     std::vector<int64_t> cdevs;
+    // sriovAware: per record its physfn / sriov_numvfs reads, and kxpu_sriov's pf_of and numvfs; per group ordinal the
+    // first blocking member or KXPU_VIABLE
+    std::vector<kxpu_sriovrec> srs;
+    std::vector<uint32_t> pfOf, numvfs, gsriov;
 };
 struct MdevWalk {
     std::vector<kxpu_mdevrec> recs;
@@ -362,6 +366,16 @@ class Plugin {
     uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
     uint64_t aerReads = 0;  // aer_dev_* files read (tests, metrics)
     uint64_t cdevReads = 0;  // vfio-dev/ directories listed (tests, metrics)
+    // SR-IOV virtual functions (include/kxpu.h, additions to ABI v14).  false (default): nothing named physfn or
+    // sriov_numvfs is opened and every output is as above.  true: after either gather, physfn (readlink, basename) and
+    // sriov_numvfs of every candidate of a passthrough class are read, and kxpu_sriov decides per group.  A group with a VF
+    // whose PF is bound to a class driver ("<vf> needs the VF token of <pf> (bound to <driver>)": vfio-pci would ask for
+    // the PF's VF token) or with a PF that has VFs enabled ("<pf> has <k> VFs enabled") goes through the blocker path:
+    // sent Unhealthy, refused by Allocate and PrepareDraDevices, left out of the CDI spec and the DRA pool.  Allocate's live
+    // path re-reads physfn, the PF's driver and sriov_numvfs.  With pcieTopologyAware the forest is kxpu_pcie_tree_sriov's,
+    // so GetPreferredAllocation packs a request's VFs by PF.
+    bool sriovAware = false;
+    uint64_t sriovReads = 0;  // functions whose physfn and sriov_numvfs were read (tests, metrics)
     bool cdevEnabled() const;  // some passthrough class has vfioCdev
     bool mdevCdevEnabled() const;  // some vGPU class has mdevCdev
 
@@ -380,6 +394,9 @@ class Plugin {
     std::vector<uint8_t> pcieDepth;
     // groupViability only: "<bdf> is bound to <driver>" of the first blocker of every iommuMap entry; empty = viable
     std::vector<std::string> iommuBlocker;
+    // sriovAware only: the SR-IOV reason of every iommuMap entry (also in iommuBlocker unless an earlier reason is);
+    // empty = served
+    std::vector<std::string> iommuSriov;
     // draEnabled only: the ResourceSlice record of every iommuMap entry (from its first member; product left empty)
     std::vector<kxpu_dradev> iommuDra;
     std::vector<std::string> cdiFiles;  // files the last generateCDISpec wrote, one per class
@@ -483,12 +500,17 @@ class Plugin {
     // raw gather only (no GPU): exposed for CPU tests of the walk.  paths (pcieTopologyAware only, else left empty):
     // one kxpu_pcipath per record, same index
     // cdevs (cdevEnabled only, else left empty): per record N of its VFIO cdev, -1 = none or not read
+    // srs (sriovAware only, else left empty): per record its physfn and sriov_numvfs reads, zero-filled for a record that
+    // is no candidate of a passthrough class
     Error gatherRecords(std::vector<kxpu_devrec> &recs, std::vector<kxpu_pcipath> *paths = nullptr,
-                        std::vector<int64_t> *cdevs = nullptr);
+                        std::vector<int64_t> *cdevs = nullptr, std::vector<kxpu_sriovrec> *srs = nullptr);
     // the same records, read with openat / readlinkat relative to basePath by several threads
     // (SURVEY 8(f) row 2); falls back to gatherRecords when a seam was replaced.  threads = 0: automatic
     Error gatherRecordsFast(std::vector<kxpu_devrec> &recs, unsigned threads = 0, std::vector<kxpu_pcipath> *paths = nullptr,
-                            std::vector<int64_t> *cdevs = nullptr);
+                            std::vector<int64_t> *cdevs = nullptr, std::vector<kxpu_sriovrec> *srs = nullptr);
+    // physfn (readlink, basename) and the first 8 bytes of sriov_numvfs of <basePath>/<bdf>; a missing link or file is
+    // no error, any other failure sets KXPU_SR_PHYSFN_ERR / KXPU_SR_NUMVFS_ERR.  Counts in sriovReads.
+    kxpu_sriovrec readSriov(const std::string &bdf);
     // the cdev of <base>/<entry> (a function's bdf under basePath, an mdev's uuid under mdevBasePath): N when vfio-dev/
     // holds exactly one entry besides . and .., and it is "vfio" followed by a canonical decimal below 2^32; -1 for
     // anything else (never an error)
@@ -508,6 +530,9 @@ class Plugin {
     size_t classOfGroup(const std::string &group) const;
     Error gatherRecordsFastWalk(std::vector<kxpu_devrec> &recs, unsigned threads, std::vector<kxpu_pcipath> *paths);
     void readCdevs(const std::vector<kxpu_devrec> &recs, std::vector<int64_t> *cdevs);
+    void readSriovs(const std::vector<kxpu_devrec> &recs, std::vector<kxpu_sriovrec> *srs);
+    // Allocate's live SR-IOV check of one function: the reason kxpu_sriov's rule now gives, or ""
+    std::string sriovLive(const std::string &bdf);
     // one CDI spec per class: the devices of m whose entry has that class (entryClass, same positions as m)
     template <typename Dev, typename Rec>
     Error generateClassSpecs(const std::vector<XpuClass> &classes, const OrderedMap<std::vector<Dev>> &m,

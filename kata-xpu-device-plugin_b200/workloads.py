@@ -659,3 +659,28 @@ def aer_records(n=1 << 20, seed=51, vgpus_per_parent=0):
         group_off = np.append(group_off, n)
     return dict(text=b"".join(parts), file_off=file_off, file_len=file_len, group_off=group_off.astype(np.uint32),
                 group_members=rng.permutation(n).astype(np.uint32))
+
+
+def sriov_walk(n=1 << 20, seed=41):
+    """n records (DEVREC_DTYPE, bdfs in walk order, one group each) with their kxpu_sriovrec side records: function 0 of
+    every device is a PF and functions 1..7 are its VFs (1 record in 8 a PF carrying 7 VFs).  PFs alternate between
+    vfio-pci with sriov_numvfs "7\\n" and a host driver; VFs are on vfio-pci and name their PF; 1 in 64 physfn reads
+    failed.  Returns (recs, srs)."""
+    from .binding import SR_PHYSFN_ERR, SRIOVREC_DTYPE
+    rng = np.random.default_rng(seed)
+    i = np.arange(n, dtype=np.int64)
+    is_pf = (i & 7) == 0
+    vfio_pf = ((i >> 3) & 1) == 0
+    recs = np.zeros(n, dtype=DEVREC_DTYPE)
+    recs["bdf"] = enumerate_bdfs(n).view("S16").reshape(n)
+    recs["driver"] = np.where(is_pf & ~vfio_pf, b"nvidia", b"vfio-pci")
+    recs["vendor_txt"] = _id_text(np.full(n, 0x10DE))
+    recs["device_txt"] = _id_text(np.full(n, 0x2330))
+    recs["vendor_len"] = recs["device_len"] = 7
+    recs["iommu_group"] = i + 1
+    srs = np.zeros(n, dtype=SRIOVREC_DTYPE)
+    srs["physfn"] = np.where(is_pf, b"", recs["bdf"][i & ~7])
+    srs["numvfs_txt"][is_pf & vfio_pf, :2] = np.frombuffer(b"7\n", np.uint8)
+    srs["numvfs_len"] = np.where(is_pf & vfio_pf, 2, 0)
+    srs["flags"] = np.where(rng.integers(0, 64, n) == 0, SR_PHYSFN_ERR, 0)
+    return recs, srs

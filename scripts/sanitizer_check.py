@@ -49,6 +49,13 @@ vrecs = W.viab_records(20000)
 for topo in (False, True):
     vres = kx.classify_viable(W.VIAB_RULES, vrecs, topo=topo)
     print("viable groups", vres["n_groups"], "blocked", int((vres["group_blocker"] != B.VIABLE).sum()))
+# SR-IOV: the verdict of a walk with PFs and VFs, and the forest with VFs below their PFs
+srecs, ssrs = W.sriov_walk(20000)
+sres = kx.classify_rules([(b"10de", b"vfio-pci")], srecs)
+sv = kx.sriov([(b"10de", b"vfio-pci")], srecs, ssrs, sres["group_ids"], sres["group_off"], sres["group_members"])
+ppf = np.where(np.arange(len(precs)) & 7, np.arange(len(precs)) & ~7, B.NO_PF).astype(np.uint32)
+print("sriov withheld", int((sv["group_sriov"] != B.VIABLE).sum()), "pcie sriov nodes",
+      len(kx.pcie_tree(precs, ppaths, poff, pmem, ppf)["key"]))
 # DRA ResourceSlices: one pool of 24 slices (the last one partial), and the empty pool
 for dn_ in (3000, 0):
     blob, soff = kx.dra_slices("vfio.nvidia.com", "node-a", "node-a", 1, W.dra_devices(dn_))
