@@ -685,9 +685,8 @@ Error Plugin::createIommuDeviceMap() {
     }
     iommuMap.clear();   // :127
     deviceMap.clear();  // :128
-    iommuClass.clear();
+    iommuState.clear();
     deviceClass.clear();
-    iommuNuma.clear();
     // the generation is read BEFORE the walk: an event during the walk makes the snapshot stale, never fresh
     haveWalkGen_ = bindGeneration && bindGeneration(walkGen_);
     haveSnapshotGen_ = snapshotValidation && haveWalkGen_;
@@ -871,13 +870,8 @@ Error Plugin::classifyPci(PciWalk &w) {
 void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
     iommuMap.clear();
     deviceMap.clear();
-    iommuClass.clear();
+    iommuState.clear();
     deviceClass.clear();
-    iommuNuma.clear();
-    iommuPcieNode.clear();
-    iommuBlocker.clear();
-    iommuSriov.clear();
-    iommuDra.clear();
     const ClassifyResult &c = w.out;
     std::map<uint32_t, size_t> groupClass = groupClasses(c);
     for (uint32_t g = 0; g < c.nGroups; g++) {
@@ -889,24 +883,24 @@ void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index
             devs.back().xpuClass = recordClass(xpuClasses, r.vendor_txt, r.vendor_len, r.driver, sizeof r.driver);
             if (!w.cdevs.empty()) devs.back().cdev = w.cdevs[c.gmem[k]];
         }
-        std::string blocker;
-        if (groupViability && c.gblk[g] != KXPU_VIABLE) blocker = blockerOf(w.recs[c.gblk[g]]);
-        if (blocker.empty() && xpuClasses[groupClass[c.gids[g]]].vfioCdev)  // a member without a cdev: VFIO cannot open it
+        GroupState<kxpu_dradev> s;
+        s.klass = groupClass[c.gids[g]];
+        if (topologyAware) s.numa = c.gnuma[g];
+        if (pcieTopologyAware) s.pcieNode = w.gnode[g];
+        if (groupViability && c.gblk[g] != KXPU_VIABLE) s.blocker = blockerOf(w.recs[c.gblk[g]]);
+        if (s.blocker.empty() && xpuClasses[s.klass].vfioCdev)  // a member without a cdev: VFIO cannot open it
             for (const NvidiaGpuDevice &d : devs)
-                if (d.cdev < 0) { blocker = d.addr + " has no VFIO cdev"; break; }
-        if (sriovAware) {
-            iommuSriov.push_back(w.gsriov[g] == KXPU_VIABLE ? std::string() : sriovReasonOf(xpuClasses, w, w.gsriov[g]));
-            if (blocker.empty()) blocker = iommuSriov.back();
+                if (d.cdev < 0) { s.blocker = d.addr + " has no VFIO cdev"; break; }
+        if (sriovAware && w.gsriov[g] != KXPU_VIABLE) {
+            s.sriov = sriovReasonOf(xpuClasses, w, w.gsriov[g]);
+            if (s.blocker.empty()) s.blocker = s.sriov;
         }
-        iommuMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
-        iommuClass.push_back(groupClass[c.gids[g]]);
-        if (topologyAware) iommuNuma.push_back(c.gnuma[g]);
-        if (pcieTopologyAware) iommuPcieNode.push_back(w.gnode[g]);
-        if (groupViability || cdevEnabled() || sriovAware) iommuBlocker.push_back(blocker);
         if (draEnabled()) {
             const uint32_t first = c.gmem[c.goff[g]];
-            iommuDra.push_back(draRecord(w.recs[first], w.paths.size() > first ? &w.paths[first] : nullptr, c.gnuma[g]));
+            s.dra = draRecord(w.recs[first], w.paths.size() > first ? &w.paths[first] : nullptr, c.gnuma[g]);
         }
+        iommuMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
+        iommuState.push_back(std::move(s));
     }
     if (pcieTopologyAware) {
         pcieParent.assign(w.nodeParent.begin(), w.nodeParent.begin() + w.nNodes);
@@ -1060,10 +1054,8 @@ Error Plugin::checkVgpuClasses() const {
 Error Plugin::createMdevMap() {
     mdevMap.clear();
     typeMap.clear();
-    mdevClass.clear();
+    mdevState.clear();
     typeClass.clear();
-    mdevNuma.clear();
-    mdevBlocker.clear();
     mdevSnap_.clear();
     mdevNext_ = 0;
     if (vgpuClasses.empty()) return Error();  // nothing under mdevBasePath is read
@@ -1109,10 +1101,8 @@ Error Plugin::classifyMdev(MdevWalk &w) {
 void Plugin::buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
     mdevMap.clear();
     typeMap.clear();
-    mdevClass.clear();
+    mdevState.clear();
     typeClass.clear();
-    mdevNuma.clear();
-    mdevBlocker.clear();
     const ClassifyResult &c = w.out;
     std::map<uint32_t, size_t> groupClass = groupClasses(c);
     for (uint32_t g = 0; g < c.nGroups; g++) {
@@ -1125,16 +1115,14 @@ void Plugin::buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index
             if (!w.cdevs.empty()) m.cdev = w.cdevs[c.gmem[k]];
             devs.push_back(std::move(m));
         }
-        if (mdevCdevEnabled()) {  // an mdev without a cdev: VFIO cannot open it
-            std::string blocker;
-            if (vgpuClasses[groupClass[c.gids[g]]].mdevCdev)
-                for (const MdevDevice &m : devs)
-                    if (m.cdev < 0) { blocker = m.uuid + " has no VFIO cdev"; break; }
-            mdevBlocker.push_back(blocker);
-        }
+        GroupState<kxpu_dramdev> s;
+        s.klass = groupClass[c.gids[g]];
+        if (topologyAware) s.numa = c.gnuma[g];
+        if (vgpuClasses[s.klass].mdevCdev)  // an mdev without a cdev: VFIO cannot open it
+            for (const MdevDevice &m : devs)
+                if (m.cdev < 0) { s.blocker = m.uuid + " has no VFIO cdev"; break; }
         mdevMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
-        mdevClass.push_back(groupClass[c.gids[g]]);
-        if (topologyAware) mdevNuma.push_back(c.gnuma[g]);
+        mdevState.push_back(std::move(s));
     }
     for (uint32_t d = 0; d < c.nDevids; d++) {
         std::vector<std::string> groups;
@@ -1145,10 +1133,9 @@ void Plugin::buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index
     buildMdevDra(w);
 }
 
-// mdevDra of a walk (vgpuDraEnabled only): one kxpu_dramdev per group from its first mdev; the parents' model names come
-// from one getDeviceNames call over the distinct (vendor, device) ids
+// the dra record of every mdevState entry (vgpuDraEnabled only): one kxpu_dramdev per group from its first mdev; the
+// parents' model names come from one getDeviceNames call over the distinct (vendor, device) ids
 void Plugin::buildMdevDra(const MdevWalk &w) {
-    mdevDra.clear();
     if (!vgpuDraEnabled()) return;
     const ClassifyResult &c = w.out;
     std::map<uint32_t, std::string> keyOf;  // group id -> type key of its device-map entry
@@ -1175,7 +1162,7 @@ void Plugin::buildMdevDra(const MdevWalk &w) {
         const std::string root = first < w.pcieRoot.size() ? w.pcieRoot[first] : std::string();
         memcpy(d.pcie_root, root.data(), std::min(root.size(), sizeof d.pcie_root));
         d.numa_mask = c.gnuma.size() > g ? c.gnuma[g] : 0;
-        mdevDra.push_back(d);
+        mdevState[g].dra = d;
         idOf.emplace_back(vendor, device);
         if (!device.empty() && idAt.emplace(idOf.back(), ids.size()).second) {
             ids.push_back(device);
@@ -1183,11 +1170,11 @@ void Plugin::buildMdevDra(const MdevWalk &w) {
         }
     }
     const std::vector<std::string> names = ids.empty() ? std::vector<std::string>() : getDeviceNames(ids, vendors);
-    for (size_t g = 0; g < mdevDra.size(); g++) {
+    for (size_t g = 0; g < mdevState.size(); g++) {
         if (idOf[g].second.empty()) continue;  // no device id: no productName
         const std::string &name = names[idAt[idOf[g]]];
         const std::string &product = name.empty() ? idOf[g].second : name;
-        kxpu_dramdev &d = mdevDra[g];
+        kxpu_dramdev &d = *mdevState[g].dra;
         d.product_len = (uint8_t)std::min(product.size(), sizeof d.product);
         memcpy(d.product, product.data(), d.product_len);
     }
@@ -1224,10 +1211,20 @@ std::vector<kxpu_snaprec> Plugin::snapshotOf(const MdevWalk &w, const std::vecto
     return snap;
 }
 
-size_t Plugin::classOfGroup(const std::string &group) const {
-    for (size_t g = 0; g < iommuMap.size() && g < iommuClass.size(); g++)
-        if (iommuMap[g].first == group) return iommuClass[g];
-    return 0;
+// group id -> position in a walk's map, which is also its position in the walk's states
+template <typename V>
+static std::map<std::string, size_t> positions(const OrderedMap<V> &m) {
+    std::map<std::string, size_t> at;
+    for (size_t g = 0; g < m.size(); g++) at.emplace(m[g].first, g);
+    return at;
+}
+
+// the state of group `id` of a walk (its map and states, same positions); nullptr when the walk has no such group
+template <typename V, typename Dra>
+static const GroupState<Dra> *stateOf(const OrderedMap<V> &m, const std::vector<GroupState<Dra>> &state, const std::string &id) {
+    for (size_t g = 0; g < m.size(); g++)
+        if (m[g].first == id) return &state[g];
+    return nullptr;
 }
 
 // The pci.ids file into page-locked memory the GPU can address (kxpu_pinned_alloc): with text, keys and rows in
@@ -1484,10 +1481,11 @@ Error Plugin::generateClassSpecs(const std::vector<XpuClass> &classes, const Ord
 Error Plugin::generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, const std::string &format) {
     cdiFiles.clear();
     std::map<std::string, size_t> classOf;  // group -> class, from the maps of the last walk
-    for (size_t g = 0; g < iommuMap.size() && g < iommuClass.size(); g++) classOf.emplace(iommuMap[g].first, iommuClass[g]);
     std::set<std::string> withheld;  // sriovAware: a group with an SR-IOV reason, which VFIO would refuse to open
-    for (size_t g = 0; g < iommuSriov.size() && g < iommuMap.size(); g++)
-        if (!iommuSriov[g].empty()) withheld.insert(iommuMap[g].first);
+    for (size_t g = 0; g < iommuMap.size(); g++) {
+        classOf.emplace(iommuMap[g].first, iommuState[g].klass);
+        if (!iommuState[g].sriov.empty()) withheld.insert(iommuMap[g].first);
+    }
     OrderedMap<std::vector<NvidiaGpuDevice>> served;  // m without them (only built when some group is withheld)
     std::vector<size_t> entryClass;
     for (const auto &kv : m) {
@@ -1509,7 +1507,9 @@ Error Plugin::generateMdevCDISpec(const std::string &format) {
     mdevCdiFiles.clear();
     if (vgpuClasses.empty()) return Error();
     const int32_t fmt = format == "YAML" ? KXPU_FMT_YAML : KXPU_FMT_JSON;
-    return generateClassSpecs(vgpuClasses, mdevMap, mdevClass, fmt, "kxpu_cdi_emit_mdev", emitMdevGroup, mdevCdiFiles);
+    std::vector<size_t> entryClass;
+    for (const auto &s : mdevState) entryClass.push_back(s.klass);
+    return generateClassSpecs(vgpuClasses, mdevMap, entryClass, fmt, "kxpu_cdi_emit_mdev", emitMdevGroup, mdevCdiFiles);
 }
 
 // createDevicePlugins, device_plugin.go:83-112 (nothing is started: no gRPC here)
@@ -1533,43 +1533,25 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         vendors.push_back(xpuClasses[d < deviceClass.size() ? deviceClass[d] : 0].vendor);
     }
     const std::vector<std::string> names = getDeviceNames(ids, vendors);  // :99 for every device id at once
-    std::map<std::string, uint64_t> numaOf, mdevNumaOf;  // group id -> NUMA mask (topologyAware)
-    for (size_t g = 0; g < iommuNuma.size() && g < iommuMap.size(); g++) numaOf[iommuMap[g].first] = iommuNuma[g];
-    for (size_t g = 0; g < mdevNuma.size() && g < mdevMap.size(); g++) mdevNumaOf[mdevMap[g].first] = mdevNuma[g];
-    auto maskOf = [](const std::map<std::string, uint64_t> &m, const std::string &g) {
-        auto it = m.find(g);
-        return it == m.end() ? uint64_t(0) : it->second;
+    // the Device of group id of a walk, Healthy, with the group's state
+    auto device = [](const std::string &id, const std::map<std::string, size_t> &at, const auto &state) {
+        Device d{id, kHealthy};
+        auto it = at.find(id);
+        if (it == at.end()) return d;
+        const auto &s = state[it->second];
+        d.numa = s.numa;
+        d.pcieNode = s.pcieNode;
+        d.blocker = s.blocker;
+        d.aer = s.aer;
+        return d;
     };
-    std::map<std::string, uint32_t> nodeOf;  // group id -> PCIe node (pcieTopologyAware)
-    for (size_t g = 0; g < iommuPcieNode.size() && g < iommuMap.size(); g++) nodeOf[iommuMap[g].first] = iommuPcieNode[g];
-    auto pcieNodeOf = [&](const std::string &g) {
-        auto it = nodeOf.find(g);
-        return it == nodeOf.end() ? KXPU_PCIE_NO_NODE : it->second;
-    };
-    std::map<std::string, std::string> blockerOfGroup;  // group id -> its first blocker (groupViability, cdevs)
-    for (size_t g = 0; g < iommuBlocker.size() && g < iommuMap.size(); g++)
-        if (!iommuBlocker[g].empty()) blockerOfGroup[iommuMap[g].first] = iommuBlocker[g];
-    std::map<std::string, std::string> aerOfGroup, aerOfMdevGroup;  // group id -> its AER reason (aerHealth)
-    for (size_t g = 0; g < iommuAer.size() && g < iommuMap.size(); g++)
-        if (!iommuAer[g].empty()) aerOfGroup[iommuMap[g].first] = iommuAer[g];
-    for (size_t g = 0; g < mdevAer.size() && g < mdevMap.size(); g++)
-        if (!mdevAer[g].empty()) aerOfMdevGroup[mdevMap[g].first] = mdevAer[g];
-    for (size_t g = 0; g < mdevBlocker.size() && g < mdevMap.size(); g++)  // mdev groups: "<uuid> has no VFIO cdev"
-        if (!mdevBlocker[g].empty()) blockerOfGroup[mdevMap[g].first] = mdevBlocker[g];
-    auto aerOf = [](const std::map<std::string, std::string> &m, const std::string &g) {
-        auto it = m.find(g);
-        return it == m.end() ? std::string() : it->second;
-    };
+    const std::map<std::string, size_t> iommuAt = positions(iommuMap), mdevAt = positions(mdevMap);
     size_t at = 0;
     for (const auto &kv : deviceMap) {  // :91
         GenericDevicePlugin dp;
         dp.xpuClass = at < deviceClass.size() ? deviceClass[at] : 0;
         dp.resourceNamespace = xpuClasses[dp.xpuClass].resourceNamespace;
-        for (const std::string &dev : kv.second) {  // :93-98
-            auto it = blockerOfGroup.find(dev);
-            dp.devs.push_back(Device{dev, kHealthy, maskOf(numaOf, dev), pcieNodeOf(dev),
-                                     it == blockerOfGroup.end() ? std::string() : it->second, aerOf(aerOfGroup, dev)});
-        }
+        for (const std::string &dev : kv.second) dp.devs.push_back(device(dev, iommuAt, iommuState));  // :93-98
         std::string devpluginName = names[at++];
         if (devpluginName.empty()) {
             fprintf(stderr, "Error: Could not find device name for device id: %s\n", kv.first.c_str());
@@ -1595,12 +1577,7 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         dp.vgpu = true;
         dp.xpuClass = typeClass[t];
         dp.resourceNamespace = vgpuClasses[dp.xpuClass].resourceNamespace;
-        for (const std::string &g : typeMap[t].second) {
-            dp.devs.push_back(Device{g, kHealthy, maskOf(mdevNumaOf, g)});
-            dp.devs.back().aer = aerOf(aerOfMdevGroup, g);
-            auto it = blockerOfGroup.find(g);
-            if (it != blockerOfGroup.end()) dp.devs.back().blocker = it->second;
-        }
+        for (const std::string &g : typeMap[t].second) dp.devs.push_back(device(g, mdevAt, mdevState));
         dp.devpluginName = typeMap[t].first;
         dp.devicePath = "/dev/vfio/";  // an mdev has its own IOMMU group and /dev/vfio/<group>
         if (vgpuClasses[dp.xpuClass].mdevCdev) {  // every mdev's cdev node
@@ -1887,12 +1864,12 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     e = reconcileWalk(ctx_, pw, snapshotOf(pw, nullptr), pciSnap_, pciNext_, report.pci, pidx);
     if (e) return e;
     std::map<std::string, std::string> blockerWas;  // group id -> its blocker in the last walk
-    for (size_t g = 0; g < iommuBlocker.size() && g < iommuMap.size(); g++) blockerWas[iommuMap[g].first] = iommuBlocker[g];
+    for (size_t g = 0; g < iommuMap.size(); g++) blockerWas[iommuMap[g].first] = iommuState[g].blocker;
     buildIommuMaps(pw, &pidx);
     bool viabilityChanged = false;
-    for (size_t g = 0; g < iommuBlocker.size() && g < iommuMap.size(); g++) {
+    for (size_t g = 0; g < iommuMap.size(); g++) {
         auto it = blockerWas.find(iommuMap[g].first);
-        viabilityChanged |= it != blockerWas.end() && it->second != iommuBlocker[g];
+        viabilityChanged |= it != blockerWas.end() && it->second != iommuState[g].blocker;
     }
     if (!vgpuClasses.empty()) {
         MdevWalk mw;
@@ -2040,12 +2017,12 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
     size_t vgpuClass = 0;
     for (const std::string &iommuId : devicesIDs) {  // :324
         const std::vector<MdevDevice> *mDevs = nullptr;
-        size_t mg = 0;
-        for (; mg < mdevs.size(); mg++) if (mdevs[mg].first == iommuId) { mDevs = &mdevs[mg].second; break; }
+        for (const auto &kv : mdevs) if (kv.first == iommuId) { mDevs = &kv.second; break; }
         if (mDevs) {  // a vGPU group: always live reads (the uevent snapshot only follows PCI binds)
-            if (mg < mdevBlocker.size() && !mdevBlocker[mg].empty())  // the verdict of the last walk, before any read
-                return fail("invalid allocation request: IOMMU group " + iommuId + " is not viable: " + mdevBlocker[mg]);
-            const size_t c = mg < mdevClass.size() ? mdevClass[mg] : 0;
+            const GroupState<kxpu_dramdev> *s = stateOf(mdevMap, mdevState, iommuId);
+            if (s && !s->blocker.empty())  // the verdict of the last walk, before any read
+                return fail("invalid allocation request: IOMMU group " + iommuId + " is not viable: " + s->blocker);
+            const size_t c = s ? s->klass : 0;
             if (havePci || (haveVgpu && c != vgpuClass)) return fail("invalid allocation request: devices of more than one class");
             haveVgpu = true;
             vgpuClass = c;
@@ -2064,10 +2041,10 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
         const std::vector<NvidiaGpuDevice> *nvDevs = nullptr;
         for (const auto &kv : returnedMap) if (kv.first == iommuId) { nvDevs = &kv.second; break; }
         if (!nvDevs) continue;  // unknown group id: empty nvDevs, no error (:327)
-        for (size_t g = 0; g < iommuBlocker.size() && g < iommuMap.size(); g++)  // the verdict of the last walk, before any read
-            if (iommuMap[g].first == iommuId && !iommuBlocker[g].empty())
-                return fail("invalid allocation request: IOMMU group " + iommuId + " is not viable: " + iommuBlocker[g]);
-        const size_t c = classOfGroup(iommuId);
+        const GroupState<kxpu_dradev> *s = stateOf(iommuMap, iommuState, iommuId);
+        if (s && !s->blocker.empty())  // the verdict of the last walk, before any read
+            return fail("invalid allocation request: IOMMU group " + iommuId + " is not viable: " + s->blocker);
+        const size_t c = s ? s->klass : 0;
         if (haveVgpu || (havePci && c != reqClass)) return fail("invalid allocation request: devices of more than one class");
         havePci = true;
         reqClass = c;
@@ -2121,12 +2098,14 @@ static const char *kDraTaintEffect = "NoSchedule";
 // group carries at most one of them.
 static const char *kAerTaintKeyName = "/pcie-aer";  // the key is <draDriver>/pcie-aer
 
-bool Plugin::draPublished(bool vgpu, size_t g) const {
-    if (vgpu)
-        return g < mdevMap.size() && g < mdevDra.size() && g < mdevClass.size() && !vgpuClasses[mdevClass[g]].draDriver.empty() &&
-               (g >= mdevBlocker.size() || mdevBlocker[g].empty());
-    return g < iommuMap.size() && g < iommuDra.size() && g < iommuClass.size() && !xpuClasses[iommuClass[g]].draDriver.empty() &&
-           (g >= iommuBlocker.size() || iommuBlocker[g].empty());
+// f(group id, state) for every group of a walk (map, states, the walk's class list) that is published in its class's
+// pool, in walk order: the group has a ResourceSlice record, its class a draDriver, and it has no blocker.  Only a
+// published group gets taints.
+template <typename V, typename Dra, typename F>
+static void forPublished(const OrderedMap<V> &m, const std::vector<GroupState<Dra>> &state, const std::vector<XpuClass> &classes,
+                         F f) {
+    for (size_t g = 0; g < m.size(); g++)
+        if (state[g].dra && !classes[state[g].klass].draDriver.empty() && state[g].blocker.empty()) f(m[g].first, state[g]);
 }
 
 template <typename Rec>
@@ -2165,17 +2144,17 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
             for (const Device &d : dp.devs) productOf[d.ID] = &dp.devpluginName;
     std::vector<kxpu_dradev> devs;
     std::vector<std::string> groups;
-    for (size_t g = 0; g < iommuMap.size(); g++) {
-        if (!draPublished(false, g) || iommuClass[g] != xpuClass) continue;
-        kxpu_dradev d = iommuDra[g];
-        auto it = productOf.find(iommuMap[g].first);
+    forPublished(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const GroupState<kxpu_dradev> &s) {
+        if (s.klass != xpuClass) return;
+        kxpu_dradev d = *s.dra;
+        auto it = productOf.find(g);
         if (it != productOf.end()) {
             d.product_len = (uint8_t)std::min<size_t>(it->second->size(), sizeof d.product);
             memcpy(d.product, it->second->data(), d.product_len);
         }
         devs.push_back(d);
-        groups.push_back(iommuMap[g].first);
-    }
+        groups.push_back(g);
+    });
     return draSlices(kxpu_dra_slices_taints, "kxpu_dra_slices_taints", xpuClasses[xpuClass].draDriver, draGeneration_, devs,
                      groups, out, sliceOff);
 }
@@ -2195,10 +2174,9 @@ std::vector<int64_t> Plugin::draSinceTable(const std::vector<std::string> &group
 }
 
 Error Plugin::computeAer() {
-    iommuAer.assign(iommuMap.size(), std::string());
-    iommuAerBits.assign(iommuMap.size(), 0);
-    mdevAer.assign(mdevMap.size(), std::string());
-    mdevAerBits.assign(mdevMap.size(), 0);
+    auto set = [](auto &s, const std::string &why, uint8_t bits) { s.aer = why; s.aerBits = bits; };
+    for (auto &s : iommuState) set(s, std::string(), 0);
+    for (auto &s : mdevState) set(s, std::string(), 0);
     if (!aerHealth) return Error();  // no aer_dev_* file is opened
     // one record per member of every group, passthrough groups then vGPU groups; a vGPU reads its parent's files
     std::string text;
@@ -2242,8 +2220,8 @@ Error Plugin::computeAer() {
                     why = who[members[m]] + " reported " + std::to_string(c) + (k ? " non-fatal" : " fatal") +
                           " uncorrectable PCIe errors (limit " + std::to_string(limit) + ")";
             }
-        if (g < iommuMap.size()) { iommuAer[g] = why; iommuAerBits[g] = bits[g]; }
-        else { mdevAer[g - iommuMap.size()] = why; mdevAerBits[g - iommuMap.size()] = bits[g]; }
+        if (g < iommuState.size()) set(iommuState[g], why, bits[g]);
+        else set(mdevState[g - iommuState.size()], why, bits[g]);
     }
     return Error();
 }
@@ -2256,17 +2234,15 @@ void Plugin::updateAerTaints(bool &passthroughMoved, bool &vgpuMoved) {
     }
     const int64_t t = now ? now() : (int64_t)time(nullptr);
     std::map<std::string, std::pair<uint8_t, int64_t>> next;
-    auto visit = [&](const std::string &g, uint8_t bits, bool &moved) {
+    auto visit = [&](const std::string &g, uint8_t bits) {  // whether group g's taint changed
         const uint8_t v = (bits & KXPU_AER_FATAL) ? KXPU_AER_FATAL : (bits & KXPU_AER_NONFATAL) ? KXPU_AER_NONFATAL : 0;
         auto it = aerTaint_.find(g);
         const uint8_t was = it == aerTaint_.end() ? 0 : it->second.first;
         if (v) next[g] = {v, was == v ? it->second.second : t};  // a new value gets a new time
-        moved |= was != v;
+        return was != v;
     };
-    for (size_t g = 0; g < iommuAerBits.size(); g++)
-        if (draPublished(false, g)) visit(iommuMap[g].first, iommuAerBits[g], passthroughMoved);
-    for (size_t g = 0; g < mdevAerBits.size(); g++)
-        if (draPublished(true, g)) visit(mdevMap[g].first, mdevAerBits[g], vgpuMoved);
+    forPublished(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const auto &s) { passthroughMoved |= visit(g, s.aerBits); });
+    forPublished(mdevMap, mdevState, vgpuClasses, [&](const std::string &g, const auto &s) { vgpuMoved |= visit(g, s.aerBits); });
     aerTaint_ = std::move(next);
 }
 
@@ -2277,15 +2253,15 @@ Error Plugin::refreshAerHealth(std::vector<size_t> &changedPlugins, bool &passth
     if (!aerHealth) return Error();
     Error e = computeAer();
     if (e) return e;
-    std::map<std::string, std::string> aerOf, mdevAerOf;
-    for (size_t g = 0; g < iommuAer.size(); g++) aerOf[iommuMap[g].first] = iommuAer[g];
-    for (size_t g = 0; g < mdevAer.size(); g++) mdevAerOf[mdevMap[g].first] = mdevAer[g];
+    const std::map<std::string, size_t> iommuAt = positions(iommuMap), mdevAt = positions(mdevMap);
+    auto aerOf = [](const std::string &id, const std::map<std::string, size_t> &at, const auto &state) {
+        auto it = at.find(id);
+        return it == at.end() ? std::string() : state[it->second].aer;
+    };
     for (size_t k = 0; k < devicePlugins.size(); k++) {
         bool moved = false;
         for (Device &d : devicePlugins[k].devs) {
-            const auto &m = devicePlugins[k].vgpu ? mdevAerOf : aerOf;
-            auto it = m.find(d.ID);
-            const std::string reason = it == m.end() ? std::string() : it->second;
+            const std::string reason = devicePlugins[k].vgpu ? aerOf(d.ID, mdevAt, mdevState) : aerOf(d.ID, iommuAt, iommuState);
             moved |= d.aer.empty() != reason.empty();  // ListAndWatch sends health, not the reason
             d.aer = reason;
         }
@@ -2307,16 +2283,14 @@ Error Plugin::refreshDraHealth(bool &passthroughMoved, bool &vgpuMoved) {
             if (d.Health != kHealthy) unhealthy.insert({dp.vgpu, d.ID});
     const int64_t t = now ? now() : (int64_t)time(nullptr);
     std::map<std::string, int64_t> next;
-    auto visit = [&](const std::string &g, bool vgpu, bool &moved) {
+    auto visit = [&](const std::string &g, bool vgpu) {  // whether group g's taint changed
         auto it = draTaintSince_.find(g);
         const bool was = it != draTaintSince_.end(), is = unhealthy.count({vgpu, g}) > 0;
         if (is) next[g] = was ? it->second : t;  // the time it turned unhealthy, kept while it stays so
-        moved |= was != is;
+        return was != is;
     };
-    for (size_t g = 0; g < iommuMap.size(); g++)
-        if (draPublished(false, g)) visit(iommuMap[g].first, false, passthroughMoved);
-    for (size_t g = 0; g < mdevMap.size(); g++)
-        if (draPublished(true, g)) visit(mdevMap[g].first, true, vgpuMoved);
+    forPublished(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const auto &) { passthroughMoved |= visit(g, false); });
+    forPublished(mdevMap, mdevState, vgpuClasses, [&](const std::string &g, const auto &) { vgpuMoved |= visit(g, true); });
     draTaintSince_ = std::move(next);
     if (passthroughMoved) draGeneration_++;
     if (vgpuMoved) draVgpuGeneration_++;
@@ -2329,11 +2303,11 @@ Error Plugin::VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, st
         return fail("VgpuResourceSlices: vGPU class " + std::to_string(vgpuClass) + " has no DRA driver");
     std::vector<kxpu_dramdev> devs;
     std::vector<std::string> groups;
-    for (size_t g = 0; g < mdevMap.size(); g++)
-        if (draPublished(true, g) && mdevClass[g] == vgpuClass) {
-            devs.push_back(mdevDra[g]);
-            groups.push_back(mdevMap[g].first);
-        }
+    forPublished(mdevMap, mdevState, vgpuClasses, [&](const std::string &g, const GroupState<kxpu_dramdev> &s) {
+        if (s.klass != vgpuClass) return;
+        devs.push_back(*s.dra);
+        groups.push_back(g);
+    });
     return draSlices(kxpu_dra_slices_mdev_taints, "kxpu_dra_slices_mdev_taints", vgpuClasses[vgpuClass].draDriver,
                      draVgpuGeneration_, devs, groups, out, sliceOff);
 }
@@ -2353,13 +2327,13 @@ Error Plugin::PrepareDraDevices(const std::string &driver, const std::string &po
         if (pool != nodeName) return fail("PrepareDraDevices: unknown pool " + pool + " of driver " + driver);
         for (const std::string &name : deviceNames) {
             const std::string g = name.compare(0, 4, "vfio") == 0 ? name.substr(4) : std::string();
-            bool found = false;
+            bool found;  // a group of the driver's class
             if (vgpu) {
-                for (size_t k = 0; k < mdevMap.size() && k < mdevClass.size(); k++)
-                    found |= !g.empty() && mdevMap[k].first == g && mdevClass[k] == vcls;
+                const GroupState<kxpu_dramdev> *s = stateOf(mdevMap, mdevState, g);
+                found = s && s->klass == vcls;
             } else {
-                for (size_t k = 0; k < iommuMap.size(); k++)
-                    found |= !g.empty() && iommuMap[k].first == g && iommuClass[k] == cls;
+                const GroupState<kxpu_dradev> *s = stateOf(iommuMap, iommuState, g);
+                found = s && s->klass == cls;
             }
             if (!found) return fail("PrepareDraDevices: unknown device " + name + " in pool " + pool);
             // refused even when the claim tolerates the taint: the device node is missing, so the VM cannot start
@@ -2889,7 +2863,7 @@ static std::string dumpState(Plugin *p) {
     }
     o += "],\"cdiFile\":"; jstr(o, p->lastCdiFile);
     o += ",\"iommuClass\":[";
-    for (size_t i = 0; i < p->iommuClass.size(); i++) o += (i ? "," : "") + std::to_string(p->iommuClass[i]);
+    for (size_t i = 0; i < p->iommuState.size(); i++) o += (i ? "," : "") + std::to_string(p->iommuState[i].klass);
     o += "],\"deviceClass\":[";
     for (size_t i = 0; i < p->deviceClass.size(); i++) o += (i ? "," : "") + std::to_string(p->deviceClass[i]);
     o += "],\"cdiFiles\":[";
@@ -2907,7 +2881,7 @@ static std::string dumpState(Plugin *p) {
         o += "]]";
     }
     o += "],\"mdevClass\":[";
-    for (size_t i = 0; i < p->mdevClass.size(); i++) o += (i ? "," : "") + std::to_string(p->mdevClass[i]);
+    for (size_t i = 0; i < p->mdevState.size(); i++) o += (i ? "," : "") + std::to_string(p->mdevState[i].klass);
     o += "],\"typeMap\":[";
     for (size_t t = 0; t < p->typeMap.size(); t++) {
         if (t) o += ',';

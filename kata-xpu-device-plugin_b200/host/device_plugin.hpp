@@ -17,6 +17,7 @@
 #include <deque>
 #include <functional>
 #include <map>
+#include <optional>
 #include <shared_mutex>
 #include <string>
 #include <utility>
@@ -258,6 +259,22 @@ struct MdevWalk {
     std::vector<int64_t> cdevs;
 };
 
+// The host state of one IOMMU group of a walk (Plugin::iommuState / mdevState, same positions as iommuMap / mdevMap).
+// A field whose setting is off keeps its default.
+template <typename Dra>  // kxpu_dradev (passthrough) or kxpu_dramdev (vGPU)
+struct GroupState {
+    size_t klass = 0;  // index into xpuClasses (vgpuClasses): the class of the group's first member
+    uint64_t numa = 0;  // topologyAware: the group's NUMA mask; 0 = no topology
+    uint32_t pcieNode = KXPU_PCIE_NO_NODE;  // pcieTopologyAware, passthrough only: the group's node in pcieParent / pcieDepth
+    // why VFIO cannot open the group, empty = it can: "<bdf> is bound to <driver>" (groupViability), else "<bdf> has no
+    // VFIO cdev" (vfioCdev), else sriov; a vGPU group: "<uuid> has no VFIO cdev" (mdevCdev)
+    std::string blocker{};
+    std::string sriov{};  // sriovAware, passthrough only: the SR-IOV reason; empty = served
+    std::string aer{};    // aerHealth: the first member over an AER limit (computeAer); empty = within the limits
+    uint8_t aerBits = 0;  // aerHealth: the group's KXPU_AER_* bits (computeAer)
+    std::optional<Dra> dra{};  // draEnabled (vgpuDraEnabled): the ResourceSlice record of its first member; none = unpublished
+};
+
 class Plugin {
   public:
     // ---- seams (device_plugin.go:36-39, generic_device_plugin.go:34)
@@ -385,31 +402,19 @@ class Plugin {
     // a deque: a rediscovery appends plugins without moving the others (HealthWatcher holds a reference)
     std::deque<GenericDevicePlugin> devicePlugins;
     std::string lastCdiFile;
-    // class of every iommuMap / deviceMap entry (same positions); all 0 with the default class list
-    std::vector<size_t> iommuClass, deviceClass;
-    std::vector<uint64_t> iommuNuma, mdevNuma;  // NUMA mask of every iommuMap / mdevMap entry (topologyAware only)
-    // pcieTopologyAware only: the PCIe node of every iommuMap entry and the forest of the last PCI walk, shared by all
-    // passthrough plugins
-    std::vector<uint32_t> iommuPcieNode, pcieParent;
+    std::vector<GroupState<kxpu_dradev>> iommuState;  // the state of every iommuMap entry (same positions)
+    std::vector<size_t> deviceClass;  // class of every deviceMap entry (same positions); all 0 with the default class list
+    // pcieTopologyAware only: the forest of the last PCI walk, shared by all passthrough plugins
+    std::vector<uint32_t> pcieParent;
     std::vector<uint8_t> pcieDepth;
-    // groupViability only: "<bdf> is bound to <driver>" of the first blocker of every iommuMap entry; empty = viable
-    std::vector<std::string> iommuBlocker;
-    // sriovAware only: the SR-IOV reason of every iommuMap entry (also in iommuBlocker unless an earlier reason is);
-    // empty = served
-    std::vector<std::string> iommuSriov;
-    // draEnabled only: the ResourceSlice record of every iommuMap entry (from its first member; product left empty)
-    std::vector<kxpu_dradev> iommuDra;
     std::vector<std::string> cdiFiles;  // files the last generateCDISpec wrote, one per class
-    // the mdev walk: IOMMU group -> mdevs, type key -> groups, and the vGPU class of every entry (same positions)
+    // the mdev walk: IOMMU group -> mdevs and type key -> groups, the state of every mdevMap entry and the vGPU class of
+    // every typeMap entry (same positions)
     OrderedMap<std::vector<MdevDevice>> mdevMap;
     OrderedMap<std::vector<std::string>> typeMap;
-    std::vector<size_t> mdevClass, typeClass;
+    std::vector<GroupState<kxpu_dramdev>> mdevState;
+    std::vector<size_t> typeClass;
     std::vector<std::string> mdevCdiFiles;  // files the last generateMdevCDISpec wrote, one per vGPU class
-    // mdevCdevEnabled only: "<uuid> has no VFIO cdev" of the first such mdev of every mdevMap entry of an mdevCdev class;
-    // empty = served
-    std::vector<std::string> mdevBlocker;
-    // vgpuDraEnabled only: the ResourceSlice record of every mdevMap entry (from its first mdev)
-    std::vector<kxpu_dramdev> mdevDra;
 
     explicit Plugin(kxpu_ctx *ctx);
     ~Plugin();
@@ -527,7 +532,6 @@ class Plugin {
     kxpu_ctx *ctx_;
     kxpu_table *table_ = nullptr;
     Error ensureTable();
-    size_t classOfGroup(const std::string &group) const;
     Error gatherRecordsFastWalk(std::vector<kxpu_devrec> &recs, unsigned threads, std::vector<kxpu_pcipath> *paths);
     void readCdevs(const std::vector<kxpu_devrec> &recs, std::vector<int64_t> *cdevs);
     void readSriovs(const std::vector<kxpu_devrec> &recs, std::vector<kxpu_sriovrec> *srs);
@@ -576,19 +580,13 @@ class Plugin {
     uint64_t snapshotGen_ = 0;
     uint64_t draGeneration_ = 1, draVgpuGeneration_ = 1;
     std::map<std::string, int64_t> draTaintSince_;  // draTaints: IOMMU group id -> when its taint was added
-    // aerHealth: the reason and the KXPU_AER_* bits of every iommuMap / mdevMap entry (same positions)
-    std::vector<std::string> iommuAer, mdevAer;
-    std::vector<uint8_t> iommuAerBits, mdevAerBits;
     // draTaints && aerHealth: IOMMU group id -> (KXPU_AER_FATAL or KXPU_AER_NONFATAL, when that value was first seen)
     std::map<std::string, std::pair<uint8_t, int64_t>> aerTaint_;
-    Error computeAer();  // the reads and the kxpu_aer_health call for the current maps
+    Error computeAer();  // the reads and the kxpu_aer_health call for the current maps, into their states' aer / aerBits
     // aerTaint_ from the last computeAer for the groups the DRA pools publish; which pools' taints changed
     void updateAerTaints(bool &passthroughMoved, bool &vgpuMoved);
     // per group its time in draTaintSince_, then with aerHealth its pcie-aer=fatal and =nonfatal times; -1: no such taint
     std::vector<int64_t> draSinceTable(const std::vector<std::string> &groups) const;
-    // group g of iommuMap (vgpu: mdevMap) is published in its class's pool: the class has a draDriver and, for
-    // passthrough, the group has no viability blocker.  Only a published group gets taints.
-    bool draPublished(bool vgpu, size_t g) const;
     // one pool's slices of devs, the records of groups, through fn (kxpu_dra_slices_taints or _mdev_taints) with the
     // table <driver>/unhealthy=vfio-device-missing, then with aerHealth <driver>/pcie-aer=fatal and =nonfatal, all
     // NoSchedule; without draTaints taint_since is NULL (the untainted bytes)
