@@ -688,20 +688,24 @@ Error Plugin::createIommuDeviceMap() {
     iommuState.clear();
     deviceClass.clear();
     // the generation is read BEFORE the walk: an event during the walk makes the snapshot stale, never fresh
-    haveWalkGen_ = bindGeneration && bindGeneration(walkGen_);
-    haveSnapshotGen_ = snapshotValidation && haveWalkGen_;
-    snapshotGen_ = walkGen_;
+    pci_.haveGen = bindGeneration && bindGeneration(pci_.gen);
+    haveSnapshotGen_ = snapshotValidation && pci_.haveGen;
+    snapshotGen_ = pci_.gen;
     PciWalk w;
-    Error e = classifyPci(w);
+    Error e = firstWalk(w, pci_);
+    if (e || !resumeIndices) return e;
+    resume_ = ResumeReport();  // the mdev walk resumes from the same report and state file
+    readIndexState();
+    return resume(w, pci_, resume_.pci, resume_.stateRead ? resume_.statePci : 0, xpuClasses, kxpu_cdi_parse);
+}
+
+template <typename Walk>
+Error Plugin::firstWalk(Walk &w, WalkBook &book) {
+    Error e = classify(w);
     if (e) return e;
-    buildIommuMaps(w, nullptr);
-    pciSnap_ = snapshotOf(w, nullptr);  // host bookkeeping for a later rediscovery: no GPU call
-    pciNext_ = pciSnap_.size();
-    if (resumeIndices) {
-        resume_ = ResumeReport();
-        readIndexState();
-        return resumePci(w);
-    }
+    buildMaps(w, nullptr);
+    book.snap = snapshotOf(w, nullptr);  // host bookkeeping for a later rediscovery: no GPU call
+    book.next = book.snap.size();
     return Error();
 }
 
@@ -811,7 +815,7 @@ static std::string sriovReasonOf(const std::vector<XpuClass> &classes, const Pci
 }
 
 // the walk and classify of createIommuDeviceMap
-Error Plugin::classifyPci(PciWalk &w) {
+Error Plugin::classify(PciWalk &w) {
     Error e = gatherRecordsFast(w.recs, 0, &w.paths, &w.cdevs, &w.srs);  // same records as gatherRecords (falls back to it when a seam was replaced)
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // Walk's error is ignored by the reference (:132)
     const std::vector<kxpu_devrec> &recs = w.recs;
@@ -867,7 +871,7 @@ Error Plugin::classifyPci(PciWalk &w) {
     return Error();
 }
 
-void Plugin::buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
+void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
     iommuMap.clear();
     deviceMap.clear();
     iommuState.clear();
@@ -1051,28 +1055,37 @@ Error Plugin::checkVgpuClasses() const {
     return checkPassthroughClasses(xpuClasses);
 }
 
+// the parse call of the mdev resume: kxpu_cdi_parse_mdev into the record type of the vGPU spec paths (cdiRecord)
+static int32_t parseMdevGroup(kxpu_ctx *ctx, int32_t fmt, const char *kind, const uint8_t *doc, size_t len, kxpu_mdevcdev *out,
+                              size_t cap, size_t *n) {
+    std::vector<kxpu_mdevcdi> d(cap);
+    const int32_t rc = kxpu_cdi_parse_mdev(ctx, fmt, kind, doc, len, d.data(), cap, n);
+    if (rc == KXPU_OK)
+        for (size_t i = 0; i < *n; i++) {
+            memset(&out[i], 0, sizeof out[i]);
+            out[i].dev = d[i];
+        }
+    return rc;
+}
+
 Error Plugin::createMdevMap() {
     mdevMap.clear();
     typeMap.clear();
     mdevState.clear();
     typeClass.clear();
-    mdevSnap_.clear();
-    mdevNext_ = 0;
+    mdev_.snap.clear();
+    mdev_.next = 0;
     if (vgpuClasses.empty()) return Error();  // nothing under mdevBasePath is read
     Error e = checkVgpuClasses();
     if (e) return e;
-    haveWalkMdevGen_ = mdevGeneration && mdevGeneration(walkMdevGen_);
+    mdev_.haveGen = mdevGeneration && mdevGeneration(mdev_.gen);
     MdevWalk w;
-    e = classifyMdev(w);
-    if (e) return e;
-    buildMdevMaps(w, nullptr);
-    mdevSnap_ = snapshotOf(w, nullptr);
-    mdevNext_ = mdevSnap_.size();
-    if (resumeIndices) return resumeMdev(w);
-    return Error();
+    e = firstWalk(w, mdev_);
+    if (e || !resumeIndices) return e;
+    return resume(w, mdev_, resume_.mdev, resume_.stateRead ? resume_.stateMdev : 0, vgpuClasses, parseMdevGroup);
 }
 
-Error Plugin::classifyMdev(MdevWalk &w) {
+Error Plugin::classify(MdevWalk &w) {
     Error e = gatherMdevRecords(w.recs, &w);
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // like the PCI walk: an unreadable bus is an empty one
     const std::vector<kxpu_mdevrec> &recs = w.recs;
@@ -1098,7 +1111,7 @@ Error Plugin::classifyMdev(MdevWalk &w) {
     return Error();
 }
 
-void Plugin::buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
+void Plugin::buildMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
     mdevMap.clear();
     typeMap.clear();
     mdevState.clear();
@@ -1426,17 +1439,6 @@ static int32_t emitMdevGroup(kxpu_ctx *ctx, int32_t fmt, const char *kind, const
     for (size_t i = 0; i < n; i++) d[i] = devs[i].dev;
     return kxpu_cdi_emit_mdev(ctx, fmt, kind, d.data(), n, out, cap, len);
 }
-static int32_t parseMdevGroup(kxpu_ctx *ctx, int32_t fmt, const char *kind, const uint8_t *doc, size_t len, kxpu_mdevcdev *out,
-                              size_t cap, size_t *n) {
-    std::vector<kxpu_mdevcdi> d(cap);
-    const int32_t rc = kxpu_cdi_parse_mdev(ctx, fmt, kind, doc, len, d.data(), cap, n);
-    if (rc == KXPU_OK)
-        for (size_t i = 0; i < *n; i++) {
-            memset(&out[i], 0, sizeof out[i]);
-            out[i].dev = d[i];
-        }
-    return rc;
-}
 
 // One file per class, <stem>.yaml|.json, with that class's kind and only the devices of its entries in ascending index
 // (Go ranges over the map in random order, device_plugin.go:59); a class without devices gets the empty document (the
@@ -1708,7 +1710,7 @@ void Plugin::readIndexState() {
 
 Error Plugin::writeIndexState(std::vector<std::string> *written) {
     const std::string path = cdiConfigPath + kIndexStateName;
-    const std::string text = formatIndexState(pciNext_, mdevNext_);
+    const std::string text = formatIndexState(pci_.next, mdev_.next);
     bool w = false;
     Error e = writeSpecFileAtomic(path, reinterpret_cast<const uint8_t *>(text.data()), text.size(), w);
     if (w && written) written->push_back(path);
@@ -1792,80 +1794,59 @@ Error Plugin::resumeWalk(std::vector<kxpu_snaprec> prev, uint64_t next, uint64_t
     return Error();
 }
 
-Error Plugin::resumePci(const PciWalk &w) {
+template <typename Walk, typename Rec>
+Error Plugin::resume(const Walk &w, WalkBook &book, ResumeWalk &rw, uint64_t stateNext, const std::vector<XpuClass> &classes,
+                     int32_t (*parse)(kxpu_ctx *, int32_t, const char *, const uint8_t *, size_t, Rec *, size_t, size_t *)) {
     std::vector<kxpu_snaprec> prev;
     uint64_t next = 0;
-    const uint64_t stateNext = resume_.stateRead ? resume_.statePci : 0;
-    previousEntries<kxpu_cdidev>(xpuClasses, kxpu_cdi_parse, stateNext, resume_.pci, prev, next);
+    previousEntries<Rec>(classes, parse, stateNext, rw, prev, next);
     std::vector<kxpu_snaprec> cur = snapshotOf(w, nullptr);
     std::map<uint32_t, size_t> groupClass = groupClasses(w.out);  // the file generateClassSpecs puts the entry in
     for (kxpu_snaprec &s : cur) { s.klass = (uint32_t)groupClass[s.iommu_group]; s.tag = 0; }
     std::vector<uint64_t> index;
-    Error e = resumeWalk(std::move(prev), next, stateNext, cur, resume_.pci, index, pciNext_);
+    Error e = resumeWalk(std::move(prev), next, stateNext, cur, rw, index, book.next);
     if (e) return e;
-    buildIommuMaps(w, &index);
-    pciSnap_ = snapshotOf(w, &index);
-    return Error();
-}
-
-Error Plugin::resumeMdev(const MdevWalk &w) {
-    std::vector<kxpu_snaprec> prev;
-    uint64_t next = 0;
-    const uint64_t stateNext = resume_.stateRead ? resume_.stateMdev : 0;
-    previousEntries<kxpu_mdevcdev>(vgpuClasses, parseMdevGroup, stateNext, resume_.mdev, prev, next);
-    std::vector<kxpu_snaprec> cur = snapshotOf(w, nullptr);
-    std::map<uint32_t, size_t> groupClass = groupClasses(w.out);
-    for (kxpu_snaprec &s : cur) { s.klass = (uint32_t)groupClass[s.iommu_group]; s.tag = 0; }
-    std::vector<uint64_t> index;
-    Error e = resumeWalk(std::move(prev), next, stateNext, cur, resume_.mdev, index, mdevNext_);
-    if (e) return e;
-    buildMdevMaps(w, &index);
-    mdevSnap_ = snapshotOf(w, &index);
+    buildMaps(w, &index);
+    book.snap = snapshotOf(w, &index);
     return Error();
 }
 
 bool Plugin::discoveryStale() {
-    uint64_t g = 0;
-    bool fresh = haveWalkGen_ && bindGeneration && bindGeneration(g) && g == walkGen_;
-    if (fresh && !vgpuClasses.empty()) fresh = haveWalkMdevGen_ && mdevGeneration && mdevGeneration(g) && g == walkMdevGen_;
-    return !fresh;
+    return !(pci_.current(bindGeneration) && (vgpuClasses.empty() || mdev_.current(mdevGeneration)));
 }
 
-// walk, classify and reconcile one kind of walk against its snapshot; the maps get the reconciled indices
 template <typename Walk>
-static Error reconcileWalk(kxpu_ctx *ctx, const Walk &w, const std::vector<kxpu_snaprec> &cur, std::vector<kxpu_snaprec> &snap,
-                           uint64_t &next, kxpu_reconcile_counts &counts, std::vector<uint64_t> &index) {
-    index.assign(cur.size() + 1, 0);
-    const int32_t rc = kxpu_reconcile(ctx, snap.data(), snap.size(), next, cur.data(), cur.size(), index.data(), nullptr,
-                                      nullptr, &counts);
-    if (rc != KXPU_OK) return kxfail(ctx, "kxpu_reconcile", rc);
+Error Plugin::rewalk(Walk &w, WalkBook &book, kxpu_reconcile_counts &counts) {
+    Error e = classify(w);
+    if (e) return e;
+    const std::vector<kxpu_snaprec> cur = snapshotOf(w, nullptr);
+    std::vector<uint64_t> index(cur.size() + 1, 0);
+    const int32_t rc = kxpu_reconcile(ctx_, book.snap.data(), book.snap.size(), book.next, cur.data(), cur.size(), index.data(),
+                                      nullptr, nullptr, &counts);
+    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_reconcile", rc);
     index.resize(cur.size());
-    snap = cur;
-    for (size_t i = 0; i < snap.size(); i++) snap[i].index = index[i];
-    next = counts.next_index_out;
-    (void)w;
+    book.snap = cur;
+    for (size_t i = 0; i < book.snap.size(); i++) book.snap[i].index = index[i];
+    book.next = counts.next_index_out;
+    buildMaps(w, &index);
     return Error();
 }
 
 Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     std::unique_lock<std::shared_mutex> lock(mu_);
     report = RediscoverReport();
-    report.pci.next_index_out = pciNext_;
-    report.mdev.next_index_out = mdevNext_;
+    report.pci.next_index_out = pci_.next;
+    report.mdev.next_index_out = mdev_.next;
     // 1. the generations BEFORE the walks (an event during a walk makes the result stale, never fresh)
     uint64_t gen = 0, mgen = 0;
     const bool haveGen = bindGeneration && bindGeneration(gen);
     const bool haveMgen = !vgpuClasses.empty() && mdevGeneration && mdevGeneration(mgen);
     // 2.-3. the same walks and classify variants as start-up, reconciled against the snapshots
-    PciWalk pw;
-    Error e = classifyPci(pw);
-    if (e) return e;
-    std::vector<uint64_t> pidx;
-    e = reconcileWalk(ctx_, pw, snapshotOf(pw, nullptr), pciSnap_, pciNext_, report.pci, pidx);
-    if (e) return e;
     std::map<std::string, std::string> blockerWas;  // group id -> its blocker in the last walk
     for (size_t g = 0; g < iommuMap.size(); g++) blockerWas[iommuMap[g].first] = iommuState[g].blocker;
-    buildIommuMaps(pw, &pidx);
+    PciWalk pw;
+    Error e = rewalk(pw, pci_, report.pci);
+    if (e) return e;
     bool viabilityChanged = false;
     for (size_t g = 0; g < iommuMap.size(); g++) {
         auto it = blockerWas.find(iommuMap[g].first);
@@ -1873,12 +1854,8 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     }
     if (!vgpuClasses.empty()) {
         MdevWalk mw;
-        e = classifyMdev(mw);
+        e = rewalk(mw, mdev_, report.mdev);
         if (e) return e;
-        std::vector<uint64_t> midx;
-        e = reconcileWalk(ctx_, mw, snapshotOf(mw, nullptr), mdevSnap_, mdevNext_, report.mdev, midx);
-        if (e) return e;
-        buildMdevMaps(mw, &midx);
     }
     e = computeAer();  // a re-enumerated function starts with zeroed counters
     if (e) return e;
@@ -1948,13 +1925,13 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     for (size_t k : report.changedPlugins) (devicePlugins[k].vgpu ? vgpuChanged : passthroughChanged) = true;
     bool aerPt = false, aerVg = false;
     updateAerTaints(aerPt, aerVg);
-    if (passthroughChanged || viabilityChanged || aerPt) draGeneration_++;  // the next publication replaces these slices
-    if (vgpuChanged || aerVg) draVgpuGeneration_++;
+    if (passthroughChanged || viabilityChanged || aerPt) pci_.draGeneration++;  // the next publication replaces these slices
+    if (vgpuChanged || aerVg) mdev_.draGeneration++;
     // 6. a fresh snapshot generation: Allocate answers from the snapshot again
-    haveWalkGen_ = haveGen;
-    walkGen_ = gen;
-    haveWalkMdevGen_ = haveMgen;
-    walkMdevGen_ = mgen;
+    pci_.haveGen = haveGen;
+    pci_.gen = gen;
+    mdev_.haveGen = haveMgen;
+    mdev_.gen = mgen;
     haveSnapshotGen_ = snapshotValidation && haveGen;
     snapshotGen_ = gen;
     return Error();
@@ -2155,7 +2132,7 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
         devs.push_back(d);
         groups.push_back(g);
     });
-    return draSlices(kxpu_dra_slices_taints, "kxpu_dra_slices_taints", xpuClasses[xpuClass].draDriver, draGeneration_, devs,
+    return draSlices(kxpu_dra_slices_taints, "kxpu_dra_slices_taints", xpuClasses[xpuClass].draDriver, pci_.draGeneration, devs,
                      groups, out, sliceOff);
 }
 
@@ -2268,8 +2245,8 @@ Error Plugin::refreshAerHealth(std::vector<size_t> &changedPlugins, bool &passth
         if (moved) changedPlugins.push_back(k);
     }
     updateAerTaints(passthroughMoved, vgpuMoved);
-    if (passthroughMoved) draGeneration_++;
-    if (vgpuMoved) draVgpuGeneration_++;
+    if (passthroughMoved) pci_.draGeneration++;
+    if (vgpuMoved) mdev_.draGeneration++;
     return Error();
 }
 
@@ -2292,8 +2269,8 @@ Error Plugin::refreshDraHealth(bool &passthroughMoved, bool &vgpuMoved) {
     forPublished(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const auto &) { passthroughMoved |= visit(g, false); });
     forPublished(mdevMap, mdevState, vgpuClasses, [&](const std::string &g, const auto &) { vgpuMoved |= visit(g, true); });
     draTaintSince_ = std::move(next);
-    if (passthroughMoved) draGeneration_++;
-    if (vgpuMoved) draVgpuGeneration_++;
+    if (passthroughMoved) pci_.draGeneration++;
+    if (vgpuMoved) mdev_.draGeneration++;
     return Error();
 }
 
@@ -2309,7 +2286,7 @@ Error Plugin::VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, st
         groups.push_back(g);
     });
     return draSlices(kxpu_dra_slices_mdev_taints, "kxpu_dra_slices_mdev_taints", vgpuClasses[vgpuClass].draDriver,
-                     draVgpuGeneration_, devs, groups, out, sliceOff);
+                     mdev_.draGeneration, devs, groups, out, sliceOff);
 }
 
 Error Plugin::PrepareDraDevices(const std::string &driver, const std::string &pool, const std::vector<std::string> &deviceNames,

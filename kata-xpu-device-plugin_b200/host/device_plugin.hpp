@@ -467,7 +467,7 @@ class Plugin {
     Error ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff);
     // the pool generation of every class's ResourceSlices: 1 after start-up, +1 for each rediscover that changed a
     // passthrough plugin or a group's viability, +1 for each refreshDraHealth that changed their taints
-    uint64_t draGeneration() const { return draGeneration_; }
+    uint64_t draGeneration() const { return pci_.draGeneration; }
     // draTaints: the device-plugin health of every group published in a DRA pool becomes its taint.  The host calls it
     // after HealthWatcher::poll returned > 0.  Under the exclusive lock: a group that any plugin serving it has
     // Unhealthy is tainted since now() when it turns unhealthy, keeps that time while it stays so and loses it when it
@@ -486,7 +486,7 @@ class Plugin {
     Error VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff);
     // the pool generation of every vGPU class's ResourceSlices: 1 after start-up, +1 for each rediscover that changed a
     // vGPU plugin, +1 for each refreshDraHealth that changed their taints
-    uint64_t draVgpuGeneration() const { return draVgpuGeneration_; }
+    uint64_t draVgpuGeneration() const { return mdev_.draGeneration; }
     // The data half of NodePrepareResources: cdiIds[i] = the CDI names Allocate({g}) returns for deviceNames[i] =
     // "vfio<g>", a device of the pool `pool` of the class (passthrough or vGPU) whose draDriver is `driver` (same live or
     // snapshot re-validation, same viability refusal; a vGPU group is always re-read live).  An unknown driver, pool or
@@ -497,10 +497,10 @@ class Plugin {
     // has a pci (or, with vGPU classes, an mdev) uevent generation moved since the last walk?  true when it cannot tell
     bool discoveryStale();
     // the snapshot of the last walks (kxpu_snaprec per accepted function / mdev in walk order) and their next index
-    const std::vector<kxpu_snaprec> &pciSnapshot() const { return pciSnap_; }
-    const std::vector<kxpu_snaprec> &mdevSnapshot() const { return mdevSnap_; }
-    uint64_t pciNextIndex() const { return pciNext_; }
-    uint64_t mdevNextIndex() const { return mdevNext_; }
+    const std::vector<kxpu_snaprec> &pciSnapshot() const { return pci_.snap; }
+    const std::vector<kxpu_snaprec> &mdevSnapshot() const { return mdev_.snap; }
+    uint64_t pciNextIndex() const { return pci_.next; }
+    uint64_t mdevNextIndex() const { return mdev_.next; }
 
     // raw gather only (no GPU): exposed for CPU tests of the walk.  paths (pcieTopologyAware only, else left empty):
     // one kxpu_pcipath per record, same index
@@ -545,13 +545,35 @@ class Plugin {
                              std::vector<std::string> &files);
     // first use: kxpu_pciids_join on pinned buffers = file -> table -> row handles of `keys` in one call
     Error loadAndJoin(const std::vector<uint32_t> &keys, std::vector<int32_t> &rows);
-    Error classifyPci(PciWalk &w);
-    Error classifyMdev(MdevWalk &w);
+    // One walk's bookkeeping between its walks: pci_ for the PCI functions, mdev_ for the mdevs
+    struct WalkBook {
+        std::vector<kxpu_snaprec> snap;  // the last walk's snapshot: one kxpu_snaprec per accepted entry, walk order
+        uint64_t next = 0;               // the next CDI index
+        bool haveGen = false;            // the uevent generation read before the last walk, when it could be read
+        uint64_t gen = 0;
+        uint64_t draGeneration = 1;      // the generation of the walk's DRA pools
+        // whether source still returns the generation read before the last walk; false when it cannot tell
+        bool current(const std::function<bool(uint64_t &generation)> &source) const {
+            uint64_t g = 0;
+            return haveGen && source && source(g) && g == gen;
+        }
+    };
+    WalkBook pci_, mdev_;
+    // the walk and classify of one kind of walk
+    Error classify(PciWalk &w);
+    Error classify(MdevWalk &w);
     // iommuMap / deviceMap (mdevMap / typeMap) of a walk; index == nullptr: busIndex, else index[busIndex]
-    void buildIommuMaps(const PciWalk &w, const std::vector<uint64_t> *index);
-    void buildMdevMaps(const MdevWalk &w, const std::vector<uint64_t> *index);
+    void buildMaps(const PciWalk &w, const std::vector<uint64_t> *index);
+    void buildMaps(const MdevWalk &w, const std::vector<uint64_t> *index);
     std::vector<kxpu_snaprec> snapshotOf(const PciWalk &w, const std::vector<uint64_t> *index) const;
     std::vector<kxpu_snaprec> snapshotOf(const MdevWalk &w, const std::vector<uint64_t> *index) const;
+    // the first walk of createIommuDeviceMap / createMdevMap: classify, the maps with walk-order indices, and the record
+    template <typename Walk>
+    Error firstWalk(Walk &w, WalkBook &book);
+    // rediscover: classify, reconcile against the record's snapshot (a surviving entry keeps its index, every other one
+    // gets an index never handed out before), then the maps with the reconciled indices
+    template <typename Walk>
+    Error rewalk(Walk &w, WalkBook &book, kxpu_reconcile_counts &counts);
     Error buildPlugins(std::vector<GenericDevicePlugin> &out);
     // resumeIndices: the previous specs' entries of one walk and its next index, from the state file and the specs
     template <typename Rec>
@@ -562,8 +584,11 @@ class Plugin {
     // previous specs; index gets one index per cur entry, nextOut the walk's next index
     Error resumeWalk(std::vector<kxpu_snaprec> prev, uint64_t next, uint64_t stateNext, const std::vector<kxpu_snaprec> &cur,
                      ResumeWalk &rw, std::vector<uint64_t> &index, uint64_t &nextOut);
-    Error resumePci(const PciWalk &w);
-    Error resumeMdev(const MdevWalk &w);
+    // resumeIndices: the first walk against the previous specs of classes (parse: their parse call), with stateNext the
+    // state file's value; rebuilds the walk's maps and record with the resumed indices
+    template <typename Walk, typename Rec>
+    Error resume(const Walk &w, WalkBook &book, ResumeWalk &rw, uint64_t stateNext, const std::vector<XpuClass> &classes,
+                 int32_t (*parse)(kxpu_ctx *, int32_t, const char *, const uint8_t *, size_t, Rec *, size_t, size_t *));
     void readIndexState();  // into resume_
     Error writeIndexState(std::vector<std::string> *written);
     ResumeReport resume_;
@@ -571,14 +596,9 @@ class Plugin {
     std::vector<std::string> specsWritten_;
     Error writeSpec(const std::string &path, const std::vector<uint8_t> &doc, size_t len, bool &written);
     mutable std::shared_mutex mu_;
-    std::vector<kxpu_snaprec> pciSnap_, mdevSnap_;
-    uint64_t pciNext_ = 0, mdevNext_ = 0;
-    bool haveWalkGen_ = false, haveWalkMdevGen_ = false;
-    uint64_t walkGen_ = 0, walkMdevGen_ = 0;
     BindWatcher bindWatcher_;
     bool haveSnapshotGen_ = false;
     uint64_t snapshotGen_ = 0;
-    uint64_t draGeneration_ = 1, draVgpuGeneration_ = 1;
     std::map<std::string, int64_t> draTaintSince_;  // draTaints: IOMMU group id -> when its taint was added
     // draTaints && aerHealth: IOMMU group id -> (KXPU_AER_FATAL or KXPU_AER_NONFATAL, when that value was first seen)
     std::map<std::string, std::pair<uint8_t, int64_t>> aerTaint_;
