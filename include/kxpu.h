@@ -613,6 +613,94 @@ int32_t kxpu_pcie_tree_sriov(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_
                              uint32_t *group_node /* [n_groups] */, uint64_t *key, uint32_t *parent, uint8_t *depth,
                              uint32_t *n_nodes, const uint32_t *pf_of /* [n] */);
 
+/* ------------------------------------ vGPUs on SR-IOV virtual functions (additions to ABI v14) */
+
+/* These calls and their records were added to ABI v14 without a version bump: a caller detects them by symbol, as for
+ * kxpu_sriov.  On a host with NVIDIA's vendor-specific VFIO framework (vGPU 17 and later on Linux 6.8 and later) no mdev
+ * exists: each vGPU is an SR-IOV virtual function of the GPU whose profile the admin picks by writing a type ID to
+ * <vf>/nvidia/current_vgpu_type, and the VF is then handed to the VM as a VFIO PCI function.  These facts are taken as
+ * given, since no such host and no vendor document were at hand; a different layout only needs a different reader:
+ *   [assumed] each such vGPU is a VF (<vf>/physfn exists) of an NVIDIA PF;
+ *   [assumed] <vf>/nvidia/current_vgpu_type holds the VF's vGPU type ID as a decimal, and 0 when no vGPU is created on it;
+ *   [assumed] <vf>/nvidia/creatable_vgpu_types holds a header line ("ID    : vGPU Name") and then one "<id> : <name>"
+ *             line for each type the VF can take now.  A VF that already carries a type, and every VF of a full GPU,
+ *             may list nothing, so the name of a type cannot be taken from the VF that carries it;
+ *   [assumed] a type ID means the same name on every GPU of one host under one driver;
+ *   [assumed] writing current_vgpu_type sends no bind uevent, so a type change does not move the uevent generation.
+ * The driver a vGPU-carrying VF is bound to is configuration (the class's driver), not an assumption.
+ * Host side: for every non-directory record whose vendor and driver match a class that serves vGPUs on VFs and that has
+ * a physfn link, the host reads the first 16 bytes of nvidia/current_vgpu_type into a side record at the same index; every
+ * other record gets a zero-filled one. */
+typedef struct kxpu_vfvgpurec {
+    uint8_t cur_txt[16];   /* first 16 bytes of nvidia/current_vgpu_type                                   */
+    uint8_t cur_len;       /* length of the file (0..16; longer => 17)                                      */
+    uint8_t flags;         /* KXPU_VT_READ / KXPU_VT_CUR_ERR                                                */
+    uint8_t reserved[14];
+} kxpu_vfvgpurec;          /* 32 bytes: the kernel reads one with two 16-byte vector loads                  */
+#define KXPU_VT_READ    0x01u  /* the host read this record's files                                          */
+#define KXPU_VT_CUR_ERR 0x02u  /* reading current_vgpu_type failed ("no such file" included)                 */
+#define KXPU_VGPU_FILE_MAX 16384  /* the host uses no creatable_vgpu_types text longer than this (it logs it)   */
+
+/* One record's type key: the layout of kxpu_classify_mdev's per-record key rows.  48 bytes. */
+typedef struct kxpu_vgpukey {
+    uint8_t key[40];       /* the type key, zero padded                                                     */
+    uint8_t zero[7];       /* always 0: nothing else may live in the row, which is hashed and compared whole */
+    uint8_t len;           /* key length, 0 = no key                                                        */
+} kxpu_vgpukey;
+/* kxpu_vf_vgpu_types' per-record status */
+#define KXPU_VT_NONE    0u  /* the record was not read (no KXPU_VT_READ), or its type is 0                  */
+#define KXPU_VT_NAMED   1u  /* a type ID that some table names: keys_out holds the key of that name          */
+#define KXPU_VT_UNNAMED 2u  /* a type ID that no line of any table names                                     */
+#define KXPU_VT_BAD     3u  /* KXPU_VT_CUR_ERR, cur_len > 16, or a text that is not a canonical decimal       */
+
+/* The type join of a walk's vGPU VFs.  recs_vt: n side records.  blob: n_tables name tables, table t being
+ * blob[table_off[t] .. table_off[t+1]), in priority order (the host sends the class's configured names, then the
+ * creatable_vgpu_types text of every VF it read in walk order, then the names it learned in earlier walks; the call
+ * treats them all alike).
+ *   - a LINE ends at '\n' (the last line of a table may not); one trailing '\r' is dropped.  A line NAMES a type when it
+ *     is [blanks] ID [blanks] ':' [blanks] NAME [blanks], blanks being ' ' and '\t', ID a canonical decimal
+ *     1..4294967295 (no sign, no leading zero), NAME non-empty, at most 40 bytes, with a non-empty type key.  Every other
+ *     line (the header included) is skipped;
+ *   - the TYPE KEY of a NAME is kxpu_classify_mdev's: trim "\t\n\v\f\r " at both ends, ' ' -> '_', drop every byte
+ *     outside [A-Za-z0-9_.-].  The rule is idempotent, so a key written back as a NAME gives the same key;
+ *   - the name of an ID is the first line, in table order and then line order, that names it;
+ *   - the current type of record i: cur_txt[0..cur_len) with at most one trailing '\n' removed must be a canonical
+ *     decimal below 2^32 ("0" included).
+ * Outputs, per record i:
+ *   - status[i]: KXPU_VT_NONE when the record lacks KXPU_VT_READ or its type is 0; else KXPU_VT_BAD for
+ *     KXPU_VT_CUR_ERR, cur_len > 16 or a text that is not canonical; else KXPU_VT_NAMED or KXPU_VT_UNNAMED;
+ *   - type_id[i]: the parsed ID of a NAMED or UNNAMED record, else 0;
+ *   - keys_out[i]: the key of the ID's name for a NAMED record, else all zero.
+ * Limits (else KXPU_E_UNSUPPORTED): n below 2^30, checked before any array is read; table_off[n_tables] below 2^40,
+ * checked before anything else is read; the number of lines below 2^30, counted on the GPU, with nothing written.
+ * KXPU_E_INVALID, and nothing written: a table_off that decreases, a NULL array that is needed.
+ * GPU: launches timed under KXPU_T_CLASSIFY -- (1) one warp per 2 KiB chunk of the blob finds the lines that start in
+ * it, parses each and inserts its ID into an open-addressing table that keeps the lowest line offset per ID with an
+ * atomic min (a line's blob offset orders lines by table, then by line); (2) one thread per record parses its current
+ * type, probes the table, re-parses the winning line and writes the key row with three 16-byte stores.  The table starts
+ * with 4096 slots; when more than half of them hold distinct IDs, both launches run again with room for every naming
+ * line (four launches instead of two).  KXPU_T_CLASSIFY spans every run, table resets included. */
+int32_t kxpu_vf_vgpu_types(kxpu_ctx *ctx, const kxpu_vfvgpurec *recs_vt, size_t n, const uint8_t *blob,
+                           const uint64_t *table_off /* [n_tables+1] */, size_t n_tables, kxpu_vgpukey *keys_out /* [n] */,
+                           uint32_t *type_id /* [n] */, uint8_t *status /* [n] */);
+
+/* kxpu_classify_rules with one resource per vGPU type for the rules whose bit is set in vgpu_rules.  keys: n rows in
+ * kxpu_vf_vgpu_types' layout (keys_out of that call).
+ *   - a record that matches rule r with bit r set is a candidate only when its key row is non-empty (len > 0).  That
+ *     test also stands in for the "device read works" rule: such a group comes into existence at its first candidate;
+ *   - the deviceMap key of such a record is (r, type key), interned from the key rows as kxpu_classify_mdev interns its
+ *     keys, so two IDs with one key share one entry; dev_ids[d] of such an entry is the lowest index of a candidate
+ *     that carries the key (kxpu_classify_mdev's convention), dev_rule[d] its rule;
+ *   - rules whose bit is clear behave exactly as in kxpu_classify_rules.
+ * With vgpu_rules == 0 (keys may then be NULL) every output is bitwise that of kxpu_classify_rules (group_numa and
+ * group_blocker NULL), kxpu_classify_topo (group_numa only) or kxpu_classify_viable (group_blocker given).
+ * KXPU_E_INVALID: those calls' cases, a bit at or above n_rules, or vgpu_rules != 0 with keys == NULL.
+ * GPU: compile-time variants of the candidate, intern and per-group kernels; every existing kernel is unchanged. */
+int32_t kxpu_classify_vf_vgpu(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, uint32_t vgpu_rules,
+                              const kxpu_devrec *recs, size_t n, const kxpu_vgpukey *keys /* [n] or NULL */,
+                              kxpu_classify_out *out, uint8_t *dev_rule /* [n] */, uint64_t *group_numa /* [n] or NULL */,
+                              uint32_t *group_blocker /* [n] or NULL */);
+
 /* ------------------------------------------------- runtime rediscovery (ABI v6) */
 
 /* One accepted entry of a walk, as a rediscovery compares two walks.  64 bytes. */

@@ -978,3 +978,87 @@ func (k *kxpu) pcieTreeSriov(recs []C.kxpu_devrec, paths []C.kxpu_pcipath, goff,
 		(*C.uint32_t)(unsafe.Pointer(&pf[0]))))
 	return gnode[:nGroups], parent[:nn], depth[:nn], err
 }
+
+// vGPUs on SR-IOV virtual functions (additions to ABI v14, detected by symbol).  On a host with NVIDIA's
+// vendor-specific VFIO framework each vGPU is a VF whose profile is <vf>/nvidia/current_vgpu_type; include/kxpu.h lists
+// the facts this rests on as [assumed].  After the PCI walk, read current_vgpu_type (the first 16 bytes) and
+// creatable_vgpu_types of every VF (a record with a physfn link) whose vendor and driver match a class that serves
+// vGPUs on VFs; vfVgpuTypes joins each VF's type ID to a name and returns its key row, and classifyVfVgpu then gives
+// one device-map entry per (class, type key).  This code was not compiled: the image has no Go toolchain.
+
+// the kxpu_vfvgpurec of one VF from its current_vgpu_type read (curErr: the read failed, "does not exist" included)
+func vfVgpuRecord(cur []byte, curErr bool) C.kxpu_vfvgpurec {
+	var r C.kxpu_vfvgpurec
+	r.flags = C.KXPU_VT_READ
+	if curErr {
+		r.flags |= C.KXPU_VT_CUR_ERR
+		return r
+	}
+	for i := 0; i < len(cur) && i < len(r.cur_txt); i++ {
+		r.cur_txt[i] = C.uint8_t(cur[i])
+	}
+	l := len(cur)
+	if l > 16 {
+		l = 17
+	}
+	r.cur_len = C.uint8_t(l)
+	return r
+}
+
+// the type join: recs one side record per walk record, tables the name tables in priority order (the class's
+// configured names, then every read creatable_vgpu_types in walk order, then the names learned in earlier walks).
+// Returns one key row, type ID and status (C.KXPU_VT_*) per record.
+func (k *kxpu) vfVgpuTypes(recs []C.kxpu_vfvgpurec, tables [][]byte) (keys []C.kxpu_vgpukey, typeID []uint32,
+	status []uint8, err error) {
+	n := len(recs)
+	keys, typeID, status = make([]C.kxpu_vgpukey, n+1), make([]uint32, n+1), make([]uint8, n+1)
+	off := make([]uint64, len(tables)+1)
+	var blob []byte
+	for i, t := range tables {
+		blob = append(blob, t...)
+		off[i+1] = uint64(len(blob))
+	}
+	blob = append(blob, 0) // a valid pointer for an empty blob
+	var r *C.kxpu_vfvgpurec
+	if n > 0 {
+		r = &recs[0]
+	}
+	err = kxCheck(k.ctx, "kxpu_vf_vgpu_types", C.kxpu_vf_vgpu_types(k.ctx, r, C.size_t(n),
+		(*C.uint8_t)(unsafe.Pointer(&blob[0])), (*C.uint64_t)(unsafe.Pointer(&off[0])), C.size_t(len(tables)), &keys[0],
+		(*C.uint32_t)(unsafe.Pointer(&typeID[0])), (*C.uint8_t)(unsafe.Pointer(&status[0]))))
+	return keys[:n], typeID[:n], status[:n], err
+}
+
+// classifyViable's contract with one resource per vGPU type for the rules of vgpuRules (bit r: rule r); keys is
+// vfVgpuTypes' output.  gnuma is filled when topo, blockers when viable (else both nil).  out must be wired and pinned as
+// for classifyRules.
+func (k *kxpu) classifyVfVgpu(out *C.kxpu_classify_out, rules []C.kxpu_xpu_rule, vgpuRules uint32, recs []C.kxpu_devrec,
+	keys []C.kxpu_vgpukey, devRule []uint8, topo, viable bool) (blockers []uint32, gnuma []uint64, err error) {
+	n := len(recs)
+	if n == 0 {
+		return nil, nil, nil
+	}
+	var np *C.uint64_t
+	var bp *C.uint32_t
+	if topo {
+		gnuma = make([]uint64, n)
+		np = (*C.uint64_t)(unsafe.Pointer(&gnuma[0]))
+	}
+	if viable {
+		blockers = make([]uint32, n)
+		bp = (*C.uint32_t)(unsafe.Pointer(&blockers[0]))
+	}
+	var kp *C.kxpu_vgpukey
+	if len(keys) > 0 {
+		kp = &keys[0]
+	}
+	rc := C.kxpu_classify_vf_vgpu(k.ctx, &rules[0], C.size_t(len(rules)), C.uint32_t(vgpuRules), &recs[0], C.size_t(n), kp,
+		out, (*C.uint8_t)(unsafe.Pointer(&devRule[0])), np, bp)
+	if topo {
+		gnuma = gnuma[:out.n_groups]
+	}
+	if viable {
+		blockers = blockers[:out.n_groups]
+	}
+	return blockers, gnuma, kxCheck(k.ctx, "kxpu_classify_vf_vgpu", rc)
+}

@@ -80,6 +80,14 @@ SRIOVREC_DTYPE = np.dtype([("physfn", "S16"), ("numvfs_txt", "u1", (8,)), ("numv
 assert SRIOVREC_DTYPE.itemsize == 32
 SR_PHYSFN_ERR, SR_NUMVFS_ERR = 1, 2
 NO_PF = 0xFFFFFFFF
+# vGPUs on SR-IOV VFs (additions to ABI v14): kxpu_vfvgpurec, one per kxpu_devrec at the same index, and the 48-byte key
+# rows of kxpu_vf_vgpu_types / kxpu_classify_vf_vgpu
+VFVGPUREC_DTYPE = np.dtype([("cur_txt", "u1", (16,)), ("cur_len", "u1"), ("flags", "u1"), ("reserved", "u1", (14,))])
+assert VFVGPUREC_DTYPE.itemsize == 32
+VGPUKEY_DTYPE = np.dtype([("key", "u1", (40,)), ("zero", "u1", (7,)), ("len", "u1")])
+assert VGPUKEY_DTYPE.itemsize == 48
+VT_READ, VT_CUR_ERR = 1, 2
+VT_NONE, VT_NAMED, VT_UNNAMED, VT_BAD = 0, 1, 2, 3
 CDI_FRAG_MIN = 166  # the shortest device fragment of a CDI spec: len // CDI_FRAG_MIN records hold any document (ABI v13)
 
 
@@ -104,7 +112,7 @@ ABI_SYMBOLS = [
     "kxpu_dra_slices", "kxpu_dra_slices_mdev", "kxpu_dra_slices_taint", "kxpu_dra_slices_mdev_taint",
     "kxpu_aer_health", "kxpu_dra_slices_taints", "kxpu_dra_slices_mdev_taints", "kxpu_cdi_parse", "kxpu_cdi_parse_mdev",
     "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev", "kxpu_cdi_emit_mdev_cdev", "kxpu_cdi_parse_mdev_cdev",
-    "kxpu_sriov", "kxpu_pcie_tree_sriov",
+    "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu",
 ]
 
 
@@ -220,6 +228,8 @@ def load_library():
         "kxpu_cdi_emit_mdev_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_cdi_parse_mdev_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_sriov": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp, sz, vp, vp, vp]),
+        "kxpu_vf_vgpu_types": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp]),
+        "kxpu_classify_vf_vgpu": (i32, [vp, vp, sz, C.c_uint32, vp, sz, vp, C.POINTER(ClassifyOut), vp, vp, vp]),
         "kxpu_pcie_tree_sriov": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32), vp]),
         "kxpu_dra_slices_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                          C.POINTER(sz), vp, C.POINTER(sz)]),
@@ -239,6 +249,17 @@ def _ptr(a):
 
 def _kind(kind):
     return kind.encode() if isinstance(kind, str) else kind
+
+
+def vgpu_tables(tables):
+    """(blob uint8, table_off uint64) of kxpu_vf_vgpu_types from a list of table texts, or a (blob, table_off) pair
+    passed through."""
+    if isinstance(tables, tuple):
+        blob, toff = tables
+        return np.frombuffer(bytes(blob), np.uint8), np.ascontiguousarray(toff, dtype=np.uint64)
+    toff = np.zeros(len(tables) + 1, np.uint64)
+    toff[1:] = np.cumsum([len(t) for t in tables]) if tables else []
+    return np.frombuffer(b"".join(tables), np.uint8), toff
 
 
 def rules_array(rules):
@@ -617,6 +638,52 @@ class Kxpu:
                                                    _ptr(a["avail_off"]), _ptr(a["avail"]), _ptr(a["must_off"]),
                                                    _ptr(a["must"]), _ptr(a["size"]), len(a["size"]), _ptr(out),
                                                    _ptr(out_off)))
+
+    def vf_vgpu_types(self, recs_vt, tables):
+        """kxpu_vf_vgpu_types: recs_vt (VFVGPUREC_DTYPE) and the name tables in priority order (a list of bytes, or a
+        (blob, table_off) pair).  Returns dict(keys (VGPUKEY_DTYPE), type_id, status)."""
+        recs_vt = np.ascontiguousarray(recs_vt)
+        assert recs_vt.dtype == VFVGPUREC_DTYPE
+        blob, toff = vgpu_tables(tables)
+        n = len(recs_vt)
+        keys, tid, st = np.zeros(max(n, 1), VGPUKEY_DTYPE), np.zeros(max(n, 1), np.uint32), np.zeros(max(n, 1), np.uint8)
+        self._chk(self.L.kxpu_vf_vgpu_types(self.ctx, _ptr(recs_vt) if n else None, n, _ptr(blob) if len(blob) else None,
+                                            _ptr(toff), len(toff) - 1, _ptr(keys), _ptr(tid), _ptr(st)))
+        return dict(keys=keys[:n], type_id=tid[:n], status=st[:n])
+
+    def classify_vf_vgpu(self, rules, vgpu_rules, recs, keys, topo=False, viable=False):
+        """kxpu_classify_vf_vgpu: the dict of classify_rules, plus group_numa (topo) and group_blocker (viable).  keys:
+        VGPUKEY_DTYPE rows, one per record (None: NULL)."""
+        ra = rules_array(rules)
+        recs = np.ascontiguousarray(recs)
+        assert recs.dtype == DEVREC_DTYPE
+        if keys is not None:
+            keys = np.ascontiguousarray(keys)
+            assert keys.dtype == VGPUKEY_DTYPE and len(keys) == len(recs)
+        n = len(recs)
+        arrs = dict(accept_index=np.empty(n, np.uint32), group_ids=np.empty(n, np.uint32),
+                    group_off=np.empty(n + 1, np.uint32), group_members=np.empty(n, np.uint32),
+                    dev_ids=np.empty(n, np.uint64), dev_off=np.empty(n + 1, np.uint32),
+                    dev_groups=np.empty(n, np.uint32))
+        dev_rule = np.empty(max(n, 1), np.uint8)
+        gnuma = np.empty(max(n, 1), np.uint64) if topo else None
+        gblk = np.empty(max(n, 1), np.uint32) if viable else None
+        out = ClassifyOut(**{k: v.ctypes.data for k, v in arrs.items()})
+        self._chk(self.L.kxpu_classify_vf_vgpu(self.ctx, _ptr(ra) if len(ra) else None, len(ra), vgpu_rules,
+                                               _ptr(recs) if n else None, n,
+                                               None if keys is None else _ptr(keys if n else np.zeros(1, VGPUKEY_DTYPE)),
+                                               C.byref(out),
+                                               _ptr(dev_rule), _ptr(gnuma), _ptr(gblk)))
+        g, d, a = out.n_groups, out.n_devids, out.n_accepted
+        res = dict(accept_index=arrs["accept_index"], n_accepted=a, n_groups=g, n_devids=d,
+                   group_ids=arrs["group_ids"][:g], group_off=arrs["group_off"][:g + 1],
+                   group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
+                   dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g], dev_rule=dev_rule[:d])
+        if topo:
+            res["group_numa"] = gnuma[:g]
+        if viable:
+            res["group_blocker"] = gblk[:g]
+        return res
 
     def sriov(self, rules, recs, srs, group_ids, group_off, group_members):
         """kxpu_sriov: recs (DEVREC_DTYPE) and srs (SRIOVREC_DTYPE) at the same indices, the rules and group CSR of a

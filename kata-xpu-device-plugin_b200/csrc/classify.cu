@@ -17,6 +17,8 @@
 // kxpu_classify_mdev: the candidate kernel reads 128-byte mdev records and writes each candidate's type key; a
 // name-intern pass maps every key to the first candidate carrying it (hash table, keys compared byte for byte);
 // the device-id key becomes (rule << 48 | that record's index).  Everything from k_accept_scan on is shared.
+// kxpu_classify_vf_vgpu: k_candidates_vf(_viable) reads the caller's key row of a record that matched a vGPU rule, k_intern_vf
+// interns those rows as k_intern does the mdev keys, k_groups<MODE_VF(_VIAB)> keys such a group like an mdev group.
 // kxpu_classify_viable: k_candidates_viable also folds the first blocker of every group into the group table's spare
 // word, k_groups<MODE_VIAB> copies it out per ordinal (both on kxpu_classify_rules' launches).
 // kxpu_classify_topo / _mdev_topo: k_pairs<true> also ORs each accepted record's NUMA node into its group ordinal's mask
@@ -79,7 +81,7 @@ struct Work {
     // kxpu_classify_topo / _mdev_topo only: [n] NUMA mask per group ordinal (zeroed by k_reset)
     unsigned long long *group_numa;
 };
-enum { MODE_NV = 0, MODE_RULES = 1, MODE_MDEV = 2, MODE_VIAB = 3 };
+enum { MODE_NV = 0, MODE_RULES = 1, MODE_MDEV = 2, MODE_VIAB = 3, MODE_VF = 4, MODE_VF_VIAB = 5 };
 
 // The rule list of kxpu_classify_rules as k_candidates compares it: per rule the vendor id bytes with the id
 // length in bits 56-63 (the same packing as read_id's result), and the driver as two 64-bit words with
@@ -87,7 +89,12 @@ enum { MODE_NV = 0, MODE_RULES = 1, MODE_MDEV = 2, MODE_VIAB = 3 };
 struct RuleTable {
     unsigned long long vend[KXPU_MAX_RULES], d0[KXPU_MAX_RULES], d1[KXPU_MAX_RULES], m0[KXPU_MAX_RULES], m1[KXPU_MAX_RULES];
     uint32_t n;
+    uint32_t vgpu_mask;  // kxpu_classify_vf_vgpu: bit r = rule r serves vGPU types (0 elsewhere; the struct's padding word)
 };
+// kxpu_classify_vf_vgpu keeps its key rows in keybuf and each record's intern slot (EMPTY32: no key to intern) in the
+// member sort's key buffer `ak`, which nothing reads before k_pairs writes it: Work keeps its size and layout, so the
+// existing kernels read their parameters where they always did.
+__device__ __forceinline__ uint32_t *vf_islot(const Work &W) { return W.ak; }
 // the device-id key carries the rule in bits 48-63: an id is at most 6 bytes after data[2:]
 constexpr unsigned long long DEVID_MASK = 0x0000FFFFFFFFFFFFull;
 
@@ -146,7 +153,9 @@ __device__ __forceinline__ uint32_t dinsert(const Work &W, unsigned long long ke
 // VIAB (kxpu_classify_viable): a blocker -- KXPU_REC_BLOCKS, not a directory, not a candidate -- inserts its group too
 // and lowers the slot's pad word (all ones from k_reset) to its index.  Its slot never gets an ordinal: the scans
 // read gslot[i], which stays EMPTY32 for a non-candidate.  Each record inserts at most one group, so gcap >= 2n holds.
-template <bool RULES, bool VIAB = false>
+// VF (kxpu_classify_vf_vgpu): a record of a rule in R.vgpu_mask is a candidate only with a non-empty key row, which also
+// replaces its device read; its device file is not looked at.  Such a candidate's key goes to k_intern_vf (vf_islot).
+template <bool RULES, bool VIAB = false, bool VF = false>
 __device__ __forceinline__ void candidates(const Work &W, const RuleTable &R) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= W.n) return;
@@ -182,7 +191,17 @@ __device__ __forceinline__ void candidates(const Work &W, const RuleTable &R) {
                 !(fl & KXPU_REC_IOMMU_ERR);
     bool dok = !(fl & KXPU_REC_DEVICE_ERR) && read_id(dtxt, dlen, did, dl);
     if (!(fl & (KXPU_REC_IS_DIR | KXPU_REC_VENDOR_ERR)) && vlen > 8u) atomicOr(&W.totals[3], 1u);
-    if (cand && (group == EMPTY32 || (dok && did == EMPTY64) || (!(fl & KXPU_REC_DEVICE_ERR) && dlen > 8u)))
+    bool vr = false;  // VF: the record matched a vGPU rule
+    if (VF) {
+        vr = match && ((R.vgpu_mask >> rule) & 1u);
+        if (vr) {
+            dok = reinterpret_cast<const uint8_t *>(W.keybuf + 3 * (size_t)i)[47] != 0u;  // the key length
+            cand = cand && dok;
+            if (cand && group == EMPTY32) atomicOr(&W.totals[3], 1u);
+        }
+        vf_islot(W)[i] = vr && cand ? 0u : EMPTY32;
+    }
+    if (!vr && cand && (group == EMPTY32 || (dok && did == EMPTY64) || (!(fl & KXPU_REC_DEVICE_ERR) && dlen > 8u)))
         atomicOr(&W.totals[3], 1u);  // outside the supported domain
     uint32_t slot = EMPTY32;
     if (cand) {
@@ -206,6 +225,12 @@ __global__ void __launch_bounds__(256) k_candidates_rules(const Work W, const __
 }
 __global__ void __launch_bounds__(256) k_candidates_viable(const Work W, const __grid_constant__ RuleTable R) {
     candidates<true, true>(W, R);
+}
+__global__ void __launch_bounds__(256) k_candidates_vf(const Work W, const __grid_constant__ RuleTable R) {
+    candidates<true, false, true>(W, R);
+}
+__global__ void __launch_bounds__(256) k_candidates_vf_viable(const Work W, const __grid_constant__ RuleTable R) {
+    candidates<true, true, true>(W, R);
 }
 
 // pass 1 of kxpu_classify_mdev: candidates, group table, gfirst (a group starts at a candidate with a non-empty type
@@ -267,10 +292,11 @@ __device__ __forceinline__ bool key_eq(const uint4 &a, const uint4 &b) { return 
 // pass 1b of kxpu_classify_mdev: intern the type keys.  A slot holds (hash << 32 | some record with the key), claimed by
 // CAS; a hash hit compares the 48 key bytes with that record's.  The slot's `first` is the lowest record with the key
 // (atomicMin).  Like the device-id table the intern table starts small: a probe run of 512 flags it (totals[3] bit 2)
-// and the host runs again with both tables at full size.
-__global__ void __launch_bounds__(256) k_intern(const Work W) {
+// and the host runs again with both tables at full size.  VF: the slots of kxpu_classify_vf_vgpu (vf_islot).
+template <bool VF>
+__device__ __forceinline__ void intern(const Work &W) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= W.n || W.islot[i] == EMPTY32) return;
+    if (i >= W.n || (VF ? vf_islot(W)[i] : W.islot[i]) == EMPTY32) return;
     const uint4 *kp = W.keybuf + 3 * (size_t)i;
     const uint4 k0 = kp[0], k1 = kp[1], k2 = kp[2];
     unsigned long long hv = 0x9E3779B97F4A7C15ull;
@@ -290,7 +316,7 @@ __global__ void __launch_bounds__(256) k_intern(const Work W) {
             const uint4 *op = W.keybuf + 3 * (size_t)(uint32_t)t;
             if (key_eq(op[0], k0) && key_eq(op[1], k1) && key_eq(op[2], k2)) {
                 if (i < __ldcg(&W.itab[slot].first)) atomicMin(&W.itab[slot].first, i);
-                W.islot[i] = slot;
+                (VF ? vf_islot(W)[i] : W.islot[i]) = slot;
                 return;
             }
         }
@@ -298,6 +324,8 @@ __global__ void __launch_bounds__(256) k_intern(const Work W) {
     }
     atomicOr(&W.totals[3], 4u);
 }
+__global__ void __launch_bounds__(256) k_intern(const Work W) { intern<false>(W); }
+__global__ void __launch_bounds__(256) k_intern_vf(const Work W) { intern<true>(W); }
 
 // pass 2: accept / group-first flags of a 2048-record tile, both exclusive scans in the same kernel
 // (two look-backs, warp 0 and warp 1), busIndex out, group ordinals out, device-id table insert.
@@ -380,6 +408,8 @@ __global__ void __launch_bounds__(C_THREADS) k_accept_scan(const Work W) {
 // divergent loop (6 % issue utilisation); here every group is an independent thread.
 // MODE_RULES: the device-id key is (rule of the first member) << 48 | device id; MODE_MDEV: (rule of the first member)
 // << 48 | first record with its type key.  MODE_VIAB: MODE_RULES plus the group's first blocker from its slot.
+// MODE_VF / MODE_VF_VIAB: MODE_RULES / MODE_VIAB, except that a group whose first member matched a vGPU rule is keyed
+// like MODE_MDEV's, by (rule, first record with its type key).
 template <int MODE>
 __global__ void __launch_bounds__(256) k_groups(const Work W) {
     const uint32_t o = blockIdx.x * blockDim.x + threadIdx.x;
@@ -400,8 +430,10 @@ __global__ void __launch_bounds__(256) k_groups(const Work W) {
     unsigned long long did;
     uint32_t dl;
     read_id(reinterpret_cast<const uint8_t *>(&dq), dlen, did, dl);
-    if (MODE == MODE_RULES || MODE == MODE_VIAB) did |= (unsigned long long)W.rrule[i] << 48;
-    if (MODE == MODE_VIAB) W.group_blocker[o] = W.gtab[W.gslot[i]].pad;
+    if (MODE == MODE_RULES || MODE == MODE_VIAB || MODE == MODE_VF || MODE == MODE_VF_VIAB) did |= (unsigned long long)W.rrule[i] << 48;
+    if ((MODE == MODE_VF || MODE == MODE_VF_VIAB) && vf_islot(W)[i] != EMPTY32)  // the first member matched a vGPU rule
+        did = ((unsigned long long)W.rrule[i] << 48) | W.itab[vf_islot(W)[i]].first;
+    if (MODE == MODE_VIAB || MODE == MODE_VF_VIAB) W.group_blocker[o] = W.gtab[W.gslot[i]].pad;
     const uint32_t ds = dinsert(W, did);
     // a few hot device ids own most groups: same-address atomics run at ~1 per ns, so only a group that can
     // still lower the minimum issues one
@@ -629,19 +661,22 @@ static uint32_t bits_for(uint32_t n) {
 // R == nullptr: kxpu_classify (the NVIDIA constants); else the rule list of kxpu_classify_rules, or with mdev of
 // kxpu_classify_mdev (recs then points at kxpu_mdevrec records)
 // group_numa != nullptr: the _topo calls (NUMA mask per group); group_blocker != nullptr: kxpu_classify_viable
+// vgpu_mask != 0: kxpu_classify_vf_vgpu (keys: its key rows)
 static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
-                             bool mdev, uint8_t *dev_rule, uint64_t *group_numa, uint32_t *group_blocker, bool small_dtab,
-                             bool *retry);
+                             bool mdev, uint8_t *dev_rule, uint64_t *group_numa, uint32_t *group_blocker, uint32_t vgpu_mask,
+                             const kxpu_vgpukey *keys, bool small_dtab, bool *retry);
 
 static int32_t classify_run(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R, bool mdev,
-                            uint8_t *dev_rule, uint64_t *group_numa = nullptr, uint32_t *group_blocker = nullptr) {
+                            uint8_t *dev_rule, uint64_t *group_numa = nullptr, uint32_t *group_blocker = nullptr,
+                            uint32_t vgpu_mask = 0, const kxpu_vgpukey *keys = nullptr) {
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
     bool retry = false;
-    int32_t rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, group_blocker, true, &retry);
+    int32_t rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, group_blocker, vgpu_mask, keys, true, &retry);
     // more distinct device ids (or type keys) than the small tables hold; the rerun resets every table, blockers included
-    if (retry) rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, group_blocker, false, &retry);
+    if (retry)
+        rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, group_blocker, vgpu_mask, keys, false, &retry);
     return rc;
 }
 
@@ -744,6 +779,18 @@ extern "C" int32_t kxpu_classify_viable(kxpu_ctx *ctx, const kxpu_xpu_rule *rule
     return classify_run(ctx, recs, n, out, &R, false, dev_rule, group_numa, group_blocker);
 }
 
+extern "C" int32_t kxpu_classify_vf_vgpu(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, uint32_t vgpu_rules,
+                                         const kxpu_devrec *recs, size_t n, const kxpu_vgpukey *keys, kxpu_classify_out *out,
+                                         uint8_t *dev_rule, uint64_t *group_numa, uint32_t *group_blocker) {
+    if (!ctx || !out || (n && !recs) || !rules || n_rules == 0 || n_rules > KXPU_MAX_RULES) return KXPU_E_INVALID;
+    if ((vgpu_rules >> n_rules) || (vgpu_rules && !keys)) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    RuleTable R;
+    const int32_t rc = rule_table(ctx, rules, n_rules, R);
+    if (rc != KXPU_OK) return rc;
+    return classify_run(ctx, recs, n, out, &R, false, dev_rule, group_numa, group_blocker, vgpu_rules, keys);
+}
+
 int32_t kx_rule_drivers(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, unsigned long long drv[][4]) {
     RuleTable R;
     const int32_t rc = rule_table(ctx, rules, n_rules, R);
@@ -755,8 +802,8 @@ int32_t kx_rule_drivers(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rule
 }
 
 static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
-                             bool mdev, uint8_t *dev_rule, uint64_t *group_numa, uint32_t *group_blocker, bool small_dtab,
-                             bool *retry) {
+                             bool mdev, uint8_t *dev_rule, uint64_t *group_numa, uint32_t *group_blocker, uint32_t vgpu_mask,
+                             const kxpu_vgpukey *keys, bool small_dtab, bool *retry) {
     *retry = false;
     out->n_accepted = out->n_groups = out->n_devids = 0;
     if (n == 0) {
@@ -783,9 +830,10 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
     // one arena; [ff-region | zero-region | rest]
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
-    const uint32_t icap = mdev ? dcap : 0u;  // the intern table grows with the device-id table
+    const bool interns = mdev || vgpu_mask;
+    const uint32_t icap = interns ? dcap : 0u;  // the intern table grows with the device-id table
     const size_t o_gtab = take((size_t)gcap * sizeof(GSlot)), o_dtab = take((size_t)dcap * sizeof(DSlot));
-    const size_t o_itab = mdev ? take((size_t)icap * sizeof(ISlot)) : 0;
+    const size_t o_itab = interns ? take((size_t)icap * sizeof(ISlot)) : 0;
     const size_t ff_bytes = off;
     const size_t o_totals = take(16), o_ghist = take(2 * 4 * 256 * 4);
     const size_t o_gnuma = group_numa ? take(n * 8) : 0;  // zeroed with the totals: one reset launch either way
@@ -800,6 +848,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
     const size_t o_rrule = R ? take(n) : 0, o_drule = R ? take(n) : 0;
     const size_t o_keys = mdev ? take(n * 48) : 0, o_islot = mdev ? take(n * 4) : 0;
     const size_t o_gblk = group_blocker ? take(n * 4) : 0;  // every ordinal is written by k_groups: no reset
+    const size_t o_vkeys = vgpu_mask ? take(n * 48) : 0;
     KxScratch sc(ctx);
     uint8_t *b = nullptr;
     KX_CUDA(ctx, sc.alloc((void **)&b, off));
@@ -827,6 +876,11 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
         W.keybuf = (uint4 *)(b + o_keys); W.islot = (uint32_t *)(b + o_islot);
         W.itab = (ISlot *)(b + o_itab); W.icap = icap; W.ishift = 32 - dlg;
     }
+    if (vgpu_mask) {
+        W.keybuf = (uint4 *)(b + o_vkeys);
+        W.itab = (ISlot *)(b + o_itab); W.icap = icap; W.ishift = 32 - dlg;
+        cudaMemcpyAsync(W.keybuf, keys, n * 48, cudaMemcpyHostToDevice, ctx->stream);
+    }
 
     cudaMemcpyAsync(b + o_recs, recs, n * rec_bytes, cudaMemcpyHostToDevice, ctx->stream);
     const unsigned g = (N + 255) / 256;
@@ -840,11 +894,20 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
             k_candidates_mdev<<<g, 256, 0, ctx->stream>>>(W, *R);
             k_intern<<<g, 256, 0, ctx->stream>>>(W);
             ctx->launches++;
+        } else if (vgpu_mask) {
+            RuleTable RV = *R;
+            RV.vgpu_mask = vgpu_mask;
+            if (group_blocker) k_candidates_vf_viable<<<g, 256, 0, ctx->stream>>>(W, RV);
+            else k_candidates_vf<<<g, 256, 0, ctx->stream>>>(W, RV);
+            k_intern_vf<<<g, 256, 0, ctx->stream>>>(W);
+            ctx->launches++;
         } else if (group_blocker) k_candidates_viable<<<g, 256, 0, ctx->stream>>>(W, *R);
         else if (R) k_candidates_rules<<<g, 256, 0, ctx->stream>>>(W, *R);
         else k_candidates<<<g, 256, 0, ctx->stream>>>(W);
         k_accept_scan<<<c_tiles, C_THREADS, 0, ctx->stream>>>(W);
         if (mdev) k_groups<MODE_MDEV><<<g, 256, 0, ctx->stream>>>(W);
+        else if (vgpu_mask && group_blocker) k_groups<MODE_VF_VIAB><<<g, 256, 0, ctx->stream>>>(W);
+        else if (vgpu_mask) k_groups<MODE_VF><<<g, 256, 0, ctx->stream>>>(W);
         else if (group_blocker) k_groups<MODE_VIAB><<<g, 256, 0, ctx->stream>>>(W);
         else if (R) k_groups<MODE_RULES><<<g, 256, 0, ctx->stream>>>(W);
         else k_groups<MODE_NV><<<g, 256, 0, ctx->stream>>>(W);

@@ -102,6 +102,18 @@ static bool readAerFileFunc(const std::string &base, const std::string &entry, c
     return true;
 }
 
+static bool readVgpuFileFunc(const std::string &base, const std::string &bdf, const std::string &name, std::string &out) {
+    FILE *f = fopen((base + "/" + bdf + "/nvidia/" + name).c_str(), "rb");
+    if (!f) return false;
+    std::vector<char> buf(KXPU_VGPU_FILE_MAX + 1);
+    const size_t n = fread(buf.data(), 1, buf.size(), f);
+    const bool err = ferror(f) != 0;
+    fclose(f);
+    if (err) return false;
+    out.assign(buf.data(), n);
+    return true;
+}
+
 // the numa_node rule of include/kxpu.h: one trailing '\n' stripped, then a canonical decimal 0..63
 static bool parseNumaNode(const std::string &raw, uint8_t &node) {
     std::string s = raw;
@@ -157,6 +169,7 @@ static void numaRecord(ReadNuma readNuma, uint8_t &flags, uint8_t &node) {
 Plugin::Plugin(kxpu_ctx *ctx) : ctx_(ctx) {
     readNumaNode = readNumaNodeFunc;
     readAerFile = readAerFileFunc;
+    readVgpuFile = readVgpuFileFunc;
     readPciPath = readPciPathFunc;
     readLink = readLinkFunc;
     readIDFromFile = readIDFromFileFunc;
@@ -524,6 +537,110 @@ void Plugin::readSriovs(const std::vector<kxpu_devrec> &recs, std::vector<kxpu_s
     }
 }
 
+bool Plugin::vfVgpuEnabled() const {
+    for (const XpuClass &c : xpuClasses)
+        if (c.vfVgpu) return true;
+    return false;
+}
+
+bool Plugin::passthroughDriver(const std::string &driver) const {
+    for (const XpuClass &c : xpuClasses)
+        if (!c.vfVgpu && c.driver == driver) return true;
+    return false;
+}
+
+// vfVgpu: current_vgpu_type and creatable_vgpu_types of every VF (a record with a physfn link) of such a class
+void Plugin::readVfVgpus(PciWalk &w) {
+    w.vts.clear();
+    w.creatable.clear();
+    if (!vfVgpuEnabled()) return;
+    kxpu_vfvgpurec zero;
+    memset(&zero, 0, sizeof zero);
+    w.vts.assign(w.recs.size(), zero);
+    w.creatable.assign(w.recs.size(), std::string());
+    for (size_t i = 0; i < w.recs.size(); i++) {
+        const kxpu_devrec &r = w.recs[i];
+        if (!cdevClassOf(xpuClasses, &XpuClass::vfVgpu, r, r.vendor_txt, sizeof r.vendor_txt)) continue;
+        const std::string bdf(r.bdf, strnlen(r.bdf, sizeof r.bdf));
+        char buf[256];
+        if (readlink((basePath + "/" + bdf + "/physfn").c_str(), buf, sizeof buf) < 0) continue;  // no VF: the PF
+        kxpu_vfvgpurec &v = w.vts[i];
+        v.flags = KXPU_VT_READ;
+        std::string cur, tab;
+        vfVgpuReads++;
+        if (readVgpuFile(basePath, bdf, "current_vgpu_type", cur)) {
+            memcpy(v.cur_txt, cur.data(), std::min(cur.size(), sizeof v.cur_txt));
+            v.cur_len = (uint8_t)std::min<size_t>(cur.size(), sizeof v.cur_txt + 1);
+        } else {
+            v.flags |= KXPU_VT_CUR_ERR;
+        }
+        vfVgpuReads++;
+        if (readVgpuFile(basePath, bdf, "creatable_vgpu_types", tab)) {
+            if (tab.size() > KXPU_VGPU_FILE_MAX)
+                fprintf(stderr, "%s: nvidia/creatable_vgpu_types is longer than %d bytes and is not used\n", bdf.c_str(),
+                        KXPU_VGPU_FILE_MAX);
+            else
+                w.creatable[i] = std::move(tab);
+        }
+    }
+}
+
+// kxpu_vf_vgpu_types over the name tables: every vfVgpu class's vgpuTypeNames, the VFs' creatable_vgpu_types in walk
+// order, then the types learned by earlier walks.  A NAMED VF's type joins the learned ones.
+Error Plugin::joinVgpuTypes(PciWalk &w) {
+    const size_t n = w.recs.size();
+    std::string blob;
+    std::vector<uint64_t> off{0};
+    auto table = [&](const std::string &t) { blob += t; off.push_back(blob.size()); };
+    for (const XpuClass &c : xpuClasses) {
+        if (!c.vfVgpu) continue;
+        std::string t;
+        for (const auto &kv : c.vgpuTypeNames) t += std::to_string(kv.first) + " : " + kv.second + "\n";
+        table(t);
+    }
+    for (const std::string &t : w.creatable)
+        if (!t.empty()) table(t);
+    std::string learned;
+    for (const auto &kv : learnedVgpuTypes_) learned += std::to_string(kv.first) + " : " + kv.second + "\n";
+    table(learned);
+    kxpu_vgpukey zero;
+    memset(&zero, 0, sizeof zero);
+    w.vkeys.assign(n ? n : 1, zero);
+    w.vtype.assign(n ? n : 1, 0);
+    w.vstatus.assign(n ? n : 1, KXPU_VT_NONE);
+    const int32_t rc = kxpu_vf_vgpu_types(ctx_, w.vts.data(), n, (const uint8_t *)blob.data(), off.data(), off.size() - 1,
+                                          w.vkeys.data(), w.vtype.data(), w.vstatus.data());
+    if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_vf_vgpu_types", rc);
+    for (size_t i = 0; i < n; i++) {
+        const std::string bdf(w.recs[i].bdf, strnlen(w.recs[i].bdf, sizeof w.recs[i].bdf));
+        if (w.vstatus[i] == KXPU_VT_NAMED)
+            learnedVgpuTypes_.emplace(w.vtype[i], std::string((const char *)w.vkeys[i].key, w.vkeys[i].len));
+        else if (w.vstatus[i] == KXPU_VT_UNNAMED)
+            fprintf(stderr, "%s carries vGPU type %u, which no creatable_vgpu_types list or vgpuTypeNames entry names; not served\n",
+                    bdf.c_str(), w.vtype[i]);
+        else if (w.vstatus[i] == KXPU_VT_BAD)
+            fprintf(stderr, "%s: nvidia/current_vgpu_type could not be read or holds no vGPU type ID; not served\n", bdf.c_str());
+    }
+    return Error();
+}
+
+Error Plugin::gatherVfVgpu(PciWalk &w) {
+    Error e = gatherRecords(w.recs);
+    readVfVgpus(w);
+    return e;
+}
+
+// vfVgpu with draDriver, or on a vGPU class: refused, naming the class
+Error Plugin::checkVfVgpuClasses() const {
+    for (const XpuClass &c : xpuClasses)
+        if (c.vfVgpu && !c.draDriver.empty())
+            return fail("class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + "): vfVgpu cannot be published as DRA ResourceSlices (draDriver " + c.draDriver + ")");
+    for (const XpuClass &c : vgpuClasses)
+        if (c.vfVgpu)
+            return fail("vGPU class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + "): vfVgpu applies to passthrough classes only");
+    return Error();
+}
+
 // ---------------------------------------------------------------------------- SURVEY 8(f) row 2
 // Batched sysfs ingestion: the same records as gatherRecords, but the entries of basePath are read
 // with paths RELATIVE to one directory descriptor (openat / readlinkat on "<bdf>/vendor": no lstat per
@@ -802,6 +919,7 @@ static std::string sriovPfReason(const std::string &pf, uint32_t numvfs) {
 }
 
 // the reason kxpu_sriov blocked on record i of a walk: a VF whose PF is bound to a class driver, else a PF with VFs
+// classes: the passthrough classes (a vfVgpu class's driver is the vGPU manager's, which needs no VF token)
 static std::string sriovReasonOf(const std::vector<XpuClass> &classes, const PciWalk &w, uint32_t i) {
     const kxpu_devrec &r = w.recs[i];
     const std::string me(r.bdf, strnlen(r.bdf, sizeof r.bdf));
@@ -826,7 +944,19 @@ Error Plugin::classify(PciWalk &w) {
     // fatal on failure: there is no CPU path
     int32_t rc;
     const char *what;
-    if (groupViability) {
+    readVfVgpus(w);
+    uint32_t vgpuRules = 0;  // vfVgpu: bit r = class r serves vGPU types
+    for (size_t k = 0; k < xpuClasses.size(); k++)
+        if (xpuClasses[k].vfVgpu) vgpuRules |= 1u << k;
+    if (vgpuRules) {
+        Error je = joinVgpuTypes(w);
+        if (je) return je;
+        if (groupViability) c.gblk.assign(n ? n : 1, KXPU_VIABLE);
+        rc = kxpu_classify_vf_vgpu(ctx_, rules.data(), rules.size(), vgpuRules, recs.data(), n, w.vkeys.data(), &out,
+                                   c.drule.data(), readsNuma() ? c.gnuma.data() : nullptr,
+                                   groupViability ? c.gblk.data() : nullptr);
+        what = "kxpu_classify_vf_vgpu";
+    } else if (groupViability) {
         c.gblk.assign(n ? n : 1, KXPU_VIABLE);
         rc = kxpu_classify_viable(ctx_, rules.data(), rules.size(), recs.data(), n, &out, c.drule.data(),
                                   readsNuma() ? c.gnuma.data() : nullptr, c.gblk.data());
@@ -843,16 +973,24 @@ Error Plugin::classify(PciWalk &w) {
         for (uint32_t g = 0; g < c.nGroups; g++)
             if (c.gblk[g] != KXPU_VIABLE)
                 fprintf(stderr, "IOMMU group %u is not viable: %s\n", c.gids[g], blockerOf(recs[c.gblk[g]]).c_str());
+    // the rules of the classes passed through whole: a vfVgpu class's VFs sit on the vGPU manager's driver and need no VF
+    // token, so its rule takes no part in the verdict; with none left there is no call
+    std::vector<XpuClass> whole;
+    for (const XpuClass &k : xpuClasses)
+        if (!k.vfVgpu) whole.push_back(k);
     if (sriovAware) {  // the SR-IOV verdict of every group, on the classify CSR
         w.pfOf.assign(n ? n : 1, KXPU_NO_PF);
         w.numvfs.assign(n ? n : 1, 0);
         w.gsriov.assign(c.nGroups + 1, KXPU_VIABLE);
-        rc = kxpu_sriov(ctx_, rules.data(), rules.size(), recs.data(), w.srs.data(), n, c.gids.data(), c.goff.data(),
-                        c.gmem.data(), c.nGroups, w.pfOf.data(), w.numvfs.data(), w.gsriov.data());
-        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_sriov", rc);
+        const std::vector<kxpu_xpu_rule> srules = vgpuRules ? classRules(whole) : rules;
+        if (!srules.empty()) {
+            rc = kxpu_sriov(ctx_, srules.data(), srules.size(), recs.data(), w.srs.data(), n, c.gids.data(), c.goff.data(),
+                            c.gmem.data(), c.nGroups, w.pfOf.data(), w.numvfs.data(), w.gsriov.data());
+            if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_sriov", rc);
+        }
         for (uint32_t g = 0; g < c.nGroups; g++)
             if (w.gsriov[g] != KXPU_VIABLE)
-                fprintf(stderr, "IOMMU group %u is not served: %s\n", c.gids[g], sriovReasonOf(xpuClasses, w, w.gsriov[g]).c_str());
+                fprintf(stderr, "IOMMU group %u is not served: %s\n", c.gids[g], sriovReasonOf(whole, w, w.gsriov[g]).c_str());
     }
     if (pcieTopologyAware) {  // the forest of the walk, one node per group; sriovAware: VFs below their PF
         const size_t cap = (size_t)KXPU_PCIE_MAX_DEPTH * c.nGroups + 1;
@@ -886,6 +1024,7 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
             devs.push_back(NvidiaGpuDevice{std::string(r.bdf), idx});  // :171-174
             devs.back().xpuClass = recordClass(xpuClasses, r.vendor_txt, r.vendor_len, r.driver, sizeof r.driver);
             if (!w.cdevs.empty()) devs.back().cdev = w.cdevs[c.gmem[k]];
+            if (!w.vtype.empty() && xpuClasses[devs.back().xpuClass].vfVgpu) devs.back().vgpuType = w.vtype[c.gmem[k]];
         }
         GroupState<kxpu_dradev> s;
         s.klass = groupClass[c.gids[g]];
@@ -896,7 +1035,10 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
             for (const NvidiaGpuDevice &d : devs)
                 if (d.cdev < 0) { s.blocker = d.addr + " has no VFIO cdev"; break; }
         if (sriovAware && w.gsriov[g] != KXPU_VIABLE) {
-            s.sriov = sriovReasonOf(xpuClasses, w, w.gsriov[g]);
+            std::vector<XpuClass> whole;
+            for (const XpuClass &k : xpuClasses)
+                if (!k.vfVgpu) whole.push_back(k);
+            s.sriov = sriovReasonOf(whole, w, w.gsriov[g]);
             if (s.blocker.empty()) s.blocker = s.sriov;
         }
         if (draEnabled()) {
@@ -913,7 +1055,12 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
     for (uint32_t d = 0; d < c.nDevids; d++) {
         std::vector<std::string> groups;
         for (uint32_t k = c.doff[d]; k < c.doff[d + 1]; k++) groups.push_back(std::to_string(c.dgrp[k]));  // :169
-        deviceMap.emplace_back(devIdString(c.dids[d]), std::move(groups));
+        if (xpuClasses[c.drule[d]].vfVgpu) {  // dids[d]: the first VF carrying the entry's type key
+            const kxpu_vgpukey &k = w.vkeys[c.dids[d]];
+            deviceMap.emplace_back(std::string((const char *)k.key, k.len), std::move(groups));
+        } else {
+            deviceMap.emplace_back(devIdString(c.dids[d]), std::move(groups));
+        }
         deviceClass.push_back(c.drule[d]);
     }
 }
@@ -931,6 +1078,9 @@ std::vector<kxpu_snaprec> Plugin::snapshotOf(const PciWalk &w, const std::vector
         s.klass = (uint32_t)recordClass(xpuClasses, r.vendor_txt, r.vendor_len, r.driver, sizeof r.driver);
         const std::string id = trimID(std::string((const char *)r.device_txt, std::min<size_t>(r.device_len, sizeof r.device_txt)));
         memcpy(&s.tag, id.data(), std::min<size_t>(id.size(), 8));
+        // a vGPU VF: its type ID, so a VF whose type changed is CHANGED and gets a fresh index (a CDI name handed out for
+        // the old profile never resolves to the new one); bit 63 keeps it apart from a device id text
+        if (!w.vtype.empty() && xpuClasses[s.klass].vfVgpu) s.tag = 1ull << 63 | w.vtype[i];
         s.index = index ? (*index)[w.out.accept[i]] : w.out.accept[i];
         snap.push_back(s);
     }
@@ -1530,9 +1680,13 @@ Error Plugin::createDevicePlugins() {
 Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
     devicePlugins.clear();
     std::vector<std::string> ids, vendors;
+    std::vector<size_t> nameAt(deviceMap.size(), 0);  // position in names; a vfVgpu entry is named by its type key
     for (size_t d = 0; d < deviceMap.size(); d++) {
+        const XpuClass &k = xpuClasses[d < deviceClass.size() ? deviceClass[d] : 0];
+        if (k.vfVgpu) continue;
+        nameAt[d] = ids.size();
         ids.push_back(deviceMap[d].first);
-        vendors.push_back(xpuClasses[d < deviceClass.size() ? deviceClass[d] : 0].vendor);
+        vendors.push_back(k.vendor);
     }
     const std::vector<std::string> names = getDeviceNames(ids, vendors);  // :99 for every device id at once
     // the Device of group id of a walk, Healthy, with the group's state
@@ -1554,7 +1708,8 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         dp.xpuClass = at < deviceClass.size() ? deviceClass[at] : 0;
         dp.resourceNamespace = xpuClasses[dp.xpuClass].resourceNamespace;
         for (const std::string &dev : kv.second) dp.devs.push_back(device(dev, iommuAt, iommuState));  // :93-98
-        std::string devpluginName = names[at++];
+        std::string devpluginName = xpuClasses[dp.xpuClass].vfVgpu ? kv.first : names[nameAt[at]];
+        at++;
         if (devpluginName.empty()) {
             fprintf(stderr, "Error: Could not find device name for device id: %s\n", kv.first.c_str());
             devpluginName = kv.first;  // :100-103
@@ -1629,6 +1784,7 @@ Error Plugin::checkDraClasses() const {
 
 Error Plugin::InitiateDevicePlugin() {
     Error e = checkDraClasses();
+    if (!e) e = checkVfVgpuClasses();
     if (e) return e;
     e = createIommuDeviceMap();  // :46
     if (e) return e;
@@ -1968,11 +2124,24 @@ std::string Plugin::sriovLive(const std::string &bdf) {
         if (n >= 0) {
             const std::string target(buf, (size_t)n);
             const std::string drv = target.substr(target.find_last_of('/') + 1);  // npos + 1 == 0
-            if (isClassDriver(xpuClasses, drv)) return sriovVfReason(bdf, pf, drv);
+            if (passthroughDriver(drv)) return sriovVfReason(bdf, pf, drv);
         }
     }
     const uint32_t k = parseNumvfs(s);
     return k ? sriovPfReason(bdf, k) : std::string();
+}
+
+// kxpu_vf_vgpu_types' current-type rule: at most one trailing '\n', then a canonical decimal below 2^32; 0 for anything
+// else (no vGPU, or not a type ID)
+static uint32_t parseVgpuType(std::string t) {
+    if (!t.empty() && t.back() == '\n') t.pop_back();
+    if (t.empty() || t.size() > 10 || (t.size() > 1 && t[0] == '0')) return 0;
+    uint64_t v = 0;
+    for (char ch : t) {
+        if (ch < '0' || ch > '9') return 0;
+        v = v * 10 + (uint64_t)(ch - '0');
+    }
+    return v < (1ull << 32) ? (uint32_t)v : 0;
 }
 
 // Allocate, generic_device_plugin.go:320-355, for one ContainerAllocateRequest
@@ -2026,7 +2195,7 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
         havePci = true;
         reqClass = c;
         for (const NvidiaGpuDevice &dev : *nvDevs) {
-            if (fromSnapshot) {
+            if (fromSnapshot && !xpuClasses[c].vfVgpu) {  // a type change sends no uevent: a vGPU VF is always re-read
                 snapshotValidations++;
                 devIndexes.push_back(dev.index);  // :340
                 continue;
@@ -2040,6 +2209,14 @@ Error Plugin::Allocate(const std::vector<std::string> &devicesIDs, ContainerAllo
                 return fail("invalid allocation request: unknown device: " + dev.addr);
             if (xpuClasses[c].vfioCdev && readVfioCdev(basePath, dev.addr) != dev.cdev)  // cdev numbers are reused across re-binds
                 return fail("invalid allocation request: the VFIO cdev of " + dev.addr + " changed since discovery");
+            if (xpuClasses[c].vfVgpu) {  // the profile the walk saw, or the CDI index names another vGPU now
+                std::string cur;
+                const uint32_t now = readVgpuFile(basePath, dev.addr, "current_vgpu_type", cur) ? parseVgpuType(cur) : 0;
+                vfVgpuReads++;
+                if (now != dev.vgpuType)
+                    return fail("invalid allocation request: " + dev.addr + " carries vGPU type " + std::to_string(now) +
+                                ", not type " + std::to_string(dev.vgpuType) + " as discovered");
+            }
             if (sriovAware) {  // a PF rebound, or VFs enabled, since the walk
                 const std::string why = sriovLive(dev.addr);
                 if (!why.empty()) return fail("invalid allocation request: " + why);
@@ -2776,6 +2953,67 @@ static void jsnap(std::string &o, const std::vector<kxpu_snaprec> &snap) {
 
 void kxh_set_sriov(void *h, int on) { ((Plugin *)h)->sriovAware = on != 0; }
 uint64_t kxh_sriov_reads(void *h) { return ((Plugin *)h)->sriovReads; }
+
+// "id=name;id=name" -> vgpuTypeNames; false for a malformed list
+static bool parseTypeNames(const char *spec, std::map<uint32_t, std::string> &out) {
+    out.clear();
+    std::string all(spec ? spec : ""), item;
+    size_t pos = 0;
+    while (pos < all.size()) {
+        size_t semi = all.find(';', pos);
+        if (semi == std::string::npos) semi = all.size();
+        item = all.substr(pos, semi - pos);
+        pos = semi + 1;
+        const size_t eq = item.find('=');
+        if (eq == std::string::npos || eq == 0) return false;
+        out[(uint32_t)strtoul(item.substr(0, eq).c_str(), nullptr, 10)] = item.substr(eq + 1);
+    }
+    return true;
+}
+
+// vfVgpu of class cls (vgpu != 0: of vGPU class cls, which InitiateDevicePlugin refuses) and its vgpuTypeNames
+int kxh_set_vf_vgpu(void *h, int vgpu, int cls, int on, const char *names) {
+    Plugin *p = (Plugin *)h;
+    std::vector<device_plugin::XpuClass> &list = vgpu ? p->vgpuClasses : p->xpuClasses;
+    if (cls < 0 || (size_t)cls >= list.size()) return -1;
+    list[cls].vfVgpu = on != 0;
+    return parseTypeNames(names, list[cls].vgpuTypeNames) ? 0 : -1;
+}
+uint64_t kxh_vf_vgpu_reads(void *h) { return ((Plugin *)h)->vfVgpuReads; }
+
+// the learned (type ID, type key) pairs as {"id":"key",...}
+int kxh_vgpu_learned(void *h, char *json, size_t cap) {
+    std::string o = "{";
+    for (const auto &kv : ((Plugin *)h)->learnedVgpuTypes()) {
+        if (o.size() > 1) o += ',';
+        jstr(o, std::to_string(kv.first));
+        o += ':';
+        jstr(o, kv.second);
+    }
+    return copy_out(o + "}", json, cap);
+}
+
+// CPU only: the raw PCI gather under a class list, classes whose bit is set in vf_mask serving vGPUs on VFs; the side
+// records and the number of nvidia/ files read
+int kxh_gather_vf_vgpu(const char *base_path, const char *classes, uint32_t vf_mask, kxpu_devrec *out, kxpu_vfvgpurec *vts,
+                       size_t cap, size_t *n, uint64_t *reads, char *err, size_t errcap) {
+    Plugin p(nullptr);
+    p.basePath = base_path;
+    if (!parseClasses(classes, p.xpuClasses)) { copy_out("malformed class list", err, errcap); return -1; }
+    for (size_t k = 0; k < p.xpuClasses.size() && k < 32; k++) p.xpuClasses[k].vfVgpu = (vf_mask >> k) & 1u;
+    device_plugin::PciWalk w;
+    device_plugin::Error e = p.gatherVfVgpu(w);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    *n = w.recs.size();
+    *reads = p.vfVgpuReads;
+    if (w.recs.size() > cap) return -2;
+    memcpy(out, w.recs.data(), w.recs.size() * sizeof(kxpu_devrec));
+    for (size_t i = 0; i < w.recs.size(); i++) {
+        if (w.vts.empty()) memset(&vts[i], 0, sizeof vts[i]);
+        else vts[i] = w.vts[i];
+    }
+    return 0;
+}
 
 // CPU only: the raw PCI gather under a class list with sriovAware = on, its SR-IOV side records and sriovReads
 int kxh_gather_sriov(const char *base_path, const char *classes, int on, int fast, unsigned threads, kxpu_devrec *out,

@@ -33,6 +33,7 @@ struct NvidiaGpuDevice {
     uint64_t index;      // PCI device index on PCI bus
     size_t xpuClass = 0; // index into Plugin::xpuClasses of the class this function matched
     int64_t cdev = -1;   // N of its VFIO cdev /dev/vfio/devices/vfio<N> (XpuClass::vfioCdev only); -1 = none
+    uint32_t vgpuType = 0;  // XpuClass::vfVgpu only: the vGPU type ID the walk read from nvidia/current_vgpu_type
 };
 
 // One mediated device (vGPU) of the mdev walk: the mdevMap counterpart of NvidiaGpuDevice
@@ -188,6 +189,15 @@ struct XpuClass {
     // like a passthrough group that is not viable.  Kept apart from vfioCdev because it also rests on the vGPU driver
     // registering a cdev.  false: nothing under vfio-dev/ is opened and every output is as without it.
     bool mdevCdev = false;
+    // passthrough only (refused on a vGPU class and together with draDriver): the class serves vGPUs that live on SR-IOV
+    // virtual functions (include/kxpu.h, kxpu_vf_vgpu_types).  For every VF of the class (a record with a physfn link) the
+    // PCI walk reads nvidia/current_vgpu_type and nvidia/creatable_vgpu_types; the class gets one plugin per vGPU type
+    // key, <resourceNamespace>/<type key>, with no pci.ids lookup, and a VF that carries no type (the PF, a free VF) is
+    // never offered.  false: nothing under nvidia/ is opened and every output is as without it.
+    bool vfVgpu = false;
+    // vfVgpu only: type ID -> name, the first name table of kxpu_vf_vgpu_types.  A restart on a GPU whose VFs are all taken
+    // finds no creatable_vgpu_types list to learn names from, so only these names serve it then.
+    std::map<uint32_t, std::string> vgpuTypeNames{};
 };
 XpuClass defaultXpuClass();  // {"10de", "vfio-pci", "nvidia.com", "nvidia.com/gpu", "cdi-vfio-xxxx"}
 
@@ -246,6 +256,13 @@ struct PciWalk {
     // first blocking member or KXPU_VIABLE
     std::vector<kxpu_sriovrec> srs;
     std::vector<uint32_t> pfOf, numvfs, gsriov;
+    // some class has vfVgpu: per record its current_vgpu_type read and creatable_vgpu_types text, and kxpu_vf_vgpu_types'
+    // key row, type ID and status
+    std::vector<kxpu_vfvgpurec> vts;
+    std::vector<std::string> creatable;
+    std::vector<kxpu_vgpukey> vkeys;
+    std::vector<uint32_t> vtype;
+    std::vector<uint8_t> vstatus;
 };
 struct MdevWalk {
     std::vector<kxpu_mdevrec> recs;
@@ -393,6 +410,14 @@ class Plugin {
     // so GetPreferredAllocation packs a request's VFs by PF.
     bool sriovAware = false;
     uint64_t sriovReads = 0;  // functions whose physfn and sriov_numvfs were read (tests, metrics)
+    // <base>/<bdf>/nvidia/<name>, at most KXPU_VGPU_FILE_MAX + 1 bytes; false: the read failed ("no such file" included).
+    // A seam: tests replace it.  Every call counts in vfVgpuReads.
+    std::function<bool(const std::string &base, const std::string &bdf, const std::string &name, std::string &out)> readVgpuFile;
+    uint64_t vfVgpuReads = 0;  // nvidia/ files read (tests, metrics)
+    // (type ID, type key) of every vGPU type a walk of this process named: the last name table of kxpu_vf_vgpu_types, so a
+    // GPU that became full keeps its names across rediscover
+    const std::map<uint32_t, std::string> &learnedVgpuTypes() const { return learnedVgpuTypes_; }
+    bool vfVgpuEnabled() const;  // some passthrough class has vfVgpu
     bool cdevEnabled() const;  // some passthrough class has vfioCdev
     bool mdevCdevEnabled() const;  // some vGPU class has mdevCdev
 
@@ -527,6 +552,8 @@ class Plugin {
     // the vGPU class list against the passthrough one (distinct CDI kinds and file stems, no vfioCdev on a vGPU class, no
     // mdevCdev on a passthrough class); createMdevMap runs it
     Error checkVgpuClasses() const;
+    // the gather with the vfVgpu reads (no GPU): w.vts and w.creatable, one per record
+    Error gatherVfVgpu(PciWalk &w);
 
   private:
     kxpu_ctx *ctx_;
@@ -535,6 +562,13 @@ class Plugin {
     Error gatherRecordsFastWalk(std::vector<kxpu_devrec> &recs, unsigned threads, std::vector<kxpu_pcipath> *paths);
     void readCdevs(const std::vector<kxpu_devrec> &recs, std::vector<int64_t> *cdevs);
     void readSriovs(const std::vector<kxpu_devrec> &recs, std::vector<kxpu_sriovrec> *srs);
+    std::map<uint32_t, std::string> learnedVgpuTypes_;
+    // vfVgpu: the nvidia/ reads of every VF of such a class into w, then the type join (kxpu_vf_vgpu_types)
+    void readVfVgpus(PciWalk &w);
+    Error joinVgpuTypes(PciWalk &w);
+    // the classes whose functions are passed through whole: xpuClasses, a vfVgpu class's driver counting as none
+    bool passthroughDriver(const std::string &driver) const;
+    Error checkVfVgpuClasses() const;
     // Allocate's live SR-IOV check of one function: the reason kxpu_sriov's rule now gives, or ""
     std::string sriovLive(const std::string &bdf);
     // one CDI spec per class: the devices of m whose entry has that class (entryClass, same positions as m)

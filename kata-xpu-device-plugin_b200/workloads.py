@@ -684,3 +684,48 @@ def sriov_walk(n=1 << 20, seed=41):
     srs["numvfs_len"] = np.where(is_pf & vfio_pf, 2, 0)
     srs["flags"] = np.where(rng.integers(0, 64, n) == 0, SR_PHYSFN_ERR, 0)
     return recs, srs
+
+
+# An H100 80GB vGPU type table: (type ID, name).  The IDs are synthetic; the names follow NVIDIA's time-sliced and
+# MIG-backed C-series profiles.
+H100_VGPU_TYPES = [(1000 + k, n) for k, n in enumerate(
+    ["NVIDIA H100-1-10C", "NVIDIA H100-1-20C", "NVIDIA H100-2-20C", "NVIDIA H100-3-40C", "NVIDIA H100-4-40C",
+     "NVIDIA H100-7-80C", "NVIDIA H100-4C", "NVIDIA H100-5C", "NVIDIA H100-8C", "NVIDIA H100-10C", "NVIDIA H100-16C",
+     "NVIDIA H100-20C", "NVIDIA H100-40C", "NVIDIA H100-80C"])]
+
+
+def vf_vgpu_walk(n=1 << 20, seed=61):
+    """n records (DEVREC_DTYPE, bdfs in walk order, one group each) of GPUs on the vGPU manager's driver "nvidia": record
+    32k is a PF, records 32k+1 .. 32k+31 its VFs.  Of the VFs, 1 in 4 is free (type 0) and lists the H100 type table in
+    creatable_vgpu_types; the others carry a type: mostly one of the table's, 1 in 64 an ID no table names, 1 in 128 a
+    text that does not parse.  Returns (recs, vts, tables): the side records (the PFs are not read) and one table per free
+    VF in walk order."""
+    from .binding import VFVGPUREC_DTYPE, VT_READ
+    rng = np.random.default_rng(seed)
+    i = np.arange(n, dtype=np.int64)
+    is_pf = (i & 31) == 0
+    recs = np.zeros(n, dtype=DEVREC_DTYPE)
+    recs["bdf"] = enumerate_bdfs(n).view("S16").reshape(n)
+    recs["driver"] = b"nvidia"
+    recs["vendor_txt"] = _id_text(np.full(n, 0x10DE))
+    recs["device_txt"] = _id_text(np.where(is_pf, 0x2330, 0x2331))
+    recs["vendor_len"] = recs["device_len"] = 7
+    recs["iommu_group"] = i + 1
+    ids = np.array([t for t, _ in H100_VGPU_TYPES])
+    kind = rng.integers(0, 512, n)
+    cur = np.where(kind < 128, 0, ids[rng.integers(0, len(ids), n)])
+    cur = np.where((kind >= 128) & (kind < 136), 4242, cur)  # unnamed
+    texts = [b"%d\n" % c for c in cur]
+    bad = (kind >= 136) & (kind < 140)
+    vts = np.zeros(n, dtype=VFVGPUREC_DTYPE)
+    flat = np.zeros((n, 16), np.uint8)
+    lens = np.zeros(n, np.uint8)
+    for k in np.nonzero(~is_pf)[0]:
+        t = b"x\n" if bad[k] else texts[k]
+        flat[k, :len(t)] = np.frombuffer(t, np.uint8)
+        lens[k] = len(t)
+    vts["cur_txt"], vts["cur_len"] = flat, lens
+    vts["flags"] = np.where(is_pf, 0, VT_READ)
+    table = b"ID    : vGPU Name\n" + b"".join(b"%d : %s\n" % (t, nm.encode()) for t, nm in H100_VGPU_TYPES)
+    tables = [table] * int(((cur == 0) & ~is_pf & ~bad).sum())
+    return recs, vts, tables

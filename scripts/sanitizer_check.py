@@ -56,6 +56,12 @@ sv = kx.sriov([(b"10de", b"vfio-pci")], srecs, ssrs, sres["group_ids"], sres["gr
 ppf = np.where(np.arange(len(precs)) & 7, np.arange(len(precs)) & ~7, B.NO_PF).astype(np.uint32)
 print("sriov withheld", int((sv["group_sriov"] != B.VIABLE).sum()), "pcie sriov nodes",
       len(kx.pcie_tree(precs, ppaths, poff, pmem, ppf)["key"]))
+# vGPUs on VFs: the type join and the per-type classify, with and without blockers
+vrecs_, vvts, vtables = W.vf_vgpu_walk(20000)
+vt = kx.vf_vgpu_types(vvts, vtables)
+for viable in (False, True):
+    vc = kx.classify_vf_vgpu([(b"10de", b"nvidia")], 1, vrecs_, vt["keys"], topo=viable, viable=viable)
+    print("vf vgpu named", int((vt["status"] == B.VT_NAMED).sum()), "groups", vc["n_groups"], "types", vc["n_devids"])
 # DRA ResourceSlices: one pool of 24 slices (the last one partial), and the empty pool
 for dn_ in (3000, 0):
     blob, soff = kx.dra_slices("vfio.nvidia.com", "node-a", "node-a", 1, W.dra_devices(dn_))
