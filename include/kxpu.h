@@ -71,7 +71,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_FINALIZE 1
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
-#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov]'s and kxpu_sriov's kernels: the slot holds the most recent call's */
+#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s and kxpu_sriov's kernels: the slot holds the most recent call's */
 #define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
@@ -535,7 +535,8 @@ int32_t kxpu_pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipat
  * KXPU_PCIE_NO_NODE; parent[v] >= v other than KXPU_PCIE_NO_NODE; depth[v] != depth[parent[v]] + 1, or != 0 for a
  * root; depth[v] >= KXPU_PCIE_MAX_DEPTH.
  * dev_node == NULL, or every entry KXPU_PCIE_NO_NODE, gives kxpu_preferred_allocation's answer byte for byte.
- * Shapes, limits and out_off as kxpu_preferred_allocation; n_nodes below 2^31. */
+ * Shapes, limits and out_off as kxpu_preferred_allocation; n_nodes below 2^31.
+ * The forest may be any walk's: kxpu_pcie_tree's, kxpu_pcie_tree_sriov's, or kxpu_pcie_tree_mdev's for vGPUs. */
 int32_t kxpu_preferred_allocation_pcie(kxpu_ctx *ctx, const uint64_t *dev_numa, const uint32_t *dev_node, size_t n_devs,
                                        const uint32_t *parent, const uint8_t *depth, size_t n_nodes,
                                        const uint32_t *avail_off /* [n_req+1] */, const uint32_t *avail,
@@ -612,6 +613,35 @@ int32_t kxpu_pcie_tree_sriov(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_
                              const uint32_t *group_off /* [n_groups+1] */, const uint32_t *group_members, size_t n_groups,
                              uint32_t *group_node /* [n_groups] */, uint64_t *key, uint32_t *parent, uint8_t *depth,
                              uint32_t *n_nodes, const uint32_t *pf_of /* [n] */);
+
+/* ------------------------------------------ PCIe forest of the mdev walk (addition to ABI v14) */
+
+/* kxpu_pcie_tree for the mdev walk's records: same outputs, same CSR inputs (a kxpu_classify_mdev[_topo] call's), same
+ * limits and errors.  Added to ABI v14 without a version bump: a caller detects it by symbol, as for kxpu_pcie_tree_sriov.
+ * paths[i] is readlink(<mdevBasePath>/<uuid>) of record i, cut as kxpu_pcipath states: from its first component that
+ * begins with "pci", unknown when over 120 bytes from there.  An mdev is a child device of its parent in the driver model, so the
+ * target runs through the parent function, e.g.
+ *   "../../../devices/pci0000:00/0000:00:01.0/0000:01:00.0/0000:02:00.0/0000:03:00.0/<uuid>".
+ * Grammar: kxpu_pcipath's, except for the leaf (anything else makes the path unknown, never an error):
+ *   - the last component equals recs[i].uuid, all 36 bytes, and is a canonical lowercase UUID (8-4-4-4-12 over
+ *     [0-9a-f] with '-' between);
+ *   - the component before it is a function (not a host bridge) equal to recs[i].parent (up to its first NUL);
+ *   - the CHAIN is every component before the UUID, the parent included, 1..KXPU_PCIE_MAX_DEPTH keys.  So the parent
+ *     function is the deepest node of a group whose members share it, and every vGPU of one GPU sits below one node.
+ *     With the first component a host bridge, a known chain has at least 2 keys; the 120-byte cap, 37 bytes of which
+ *     the UUID takes, bounds it at 7 (a host bridge and 5 functions at most, on paths of host bridge and functions).
+ * Node keys, VMD domains, the per-group longest common prefix and first-seen numbering are kxpu_pcie_tree's.  An mdev
+ * whose parent is a VF needs nothing more: the VF is its chain's last key, below the PF's upstream port; the PF itself
+ * (physfn) is not consulted.
+ * Host-side policy, Plugin::vgpuPcieTopologyAware (off by default), rests on one fact:
+ *   [assumed] the vGPU manager accepts several vGPUs of one physical GPU in one VM for the profiles a class serves, so
+ *             packing a request under its parent GPU (kxpu_preferred_allocation_pcie's best fit) is what the user wants.
+ * GPU: kxpu_pcie_tree's launches, the parse a compile-time variant for this record type and leaf (kxpu_pcie_tree's and
+ * kxpu_pcie_tree_sriov's kernels are unchanged). */
+int32_t kxpu_pcie_tree_mdev(kxpu_ctx *ctx, const kxpu_mdevrec *recs, const kxpu_pcipath *paths, size_t n,
+                            const uint32_t *group_off /* [n_groups+1] */, const uint32_t *group_members, size_t n_groups,
+                            uint32_t *group_node /* [n_groups] */, uint64_t *key, uint32_t *parent, uint8_t *depth,
+                            uint32_t *n_nodes);
 
 /* ------------------------------------ vGPUs on SR-IOV virtual functions (additions to ABI v14) */
 

@@ -979,6 +979,31 @@ func (k *kxpu) pcieTreeSriov(recs []C.kxpu_devrec, paths []C.kxpu_pcipath, goff,
 	return gnode[:nGroups], parent[:nn], depth[:nn], err
 }
 
+// PCIe forest of the mdev walk (addition to ABI v14, detected by symbol).  With vgpuPcieTopology on, the mdev walk runs
+// os.Readlink(<mdevBasePath>/<uuid>) per entry that got as far as its iommu_group link (the read the vGPU DRA pool
+// already does) and keeps pciPath of the target; after classifyMdev, pcieTreeMdev builds the forest on the classify
+// CSR, every vGPU pluginapi.Device keeps its group's node, and GetPreferredAllocation of a vGPU plugin calls
+// preferredAllocationPcie with this forest (passthrough plugins keep the PCI walk's).  An mdev's parent function is the
+// deepest node of its chain, so a request is packed under one GPU, then one switch.
+func (k *kxpu) pcieTreeMdev(recs []C.kxpu_mdevrec, paths []C.kxpu_pcipath, goff, gmem []uint32, nGroups int) (gnode,
+	parent []uint32, depth []uint8, err error) {
+	capN := 8*nGroups + 1
+	gnode, parent, depth = make([]uint32, nGroups+1), make([]uint32, capN), make([]uint8, capN)
+	key := make([]uint64, capN)
+	var nn C.uint32_t
+	var r unsafe.Pointer
+	var pp *C.kxpu_pcipath
+	if len(recs) > 0 {
+		r, pp = unsafe.Pointer(&recs[0]), &paths[0]
+	}
+	gm := append(gmem, 0) // a valid pointer for an empty walk
+	err = kxCheck(k.ctx, "kxpu_pcie_tree_mdev", C.kxpu_pcie_tree_mdev(k.ctx, (*C.kxpu_mdevrec)(r), pp, C.size_t(len(recs)),
+		(*C.uint32_t)(unsafe.Pointer(&goff[0])), (*C.uint32_t)(unsafe.Pointer(&gm[0])), C.size_t(nGroups),
+		(*C.uint32_t)(unsafe.Pointer(&gnode[0])), (*C.uint64_t)(unsafe.Pointer(&key[0])),
+		(*C.uint32_t)(unsafe.Pointer(&parent[0])), (*C.uint8_t)(unsafe.Pointer(&depth[0])), &nn))
+	return gnode[:nGroups], parent[:nn], depth[:nn], err
+}
+
 // vGPUs on SR-IOV virtual functions (additions to ABI v14, detected by symbol).  On a host with NVIDIA's
 // vendor-specific VFIO framework each vGPU is a VF whose profile is <vf>/nvidia/current_vgpu_type; include/kxpu.h lists
 // the facts this rests on as [assumed].  After the PCI walk, read current_vgpu_type (the first 16 bytes) and

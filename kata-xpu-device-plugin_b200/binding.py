@@ -112,7 +112,7 @@ ABI_SYMBOLS = [
     "kxpu_dra_slices", "kxpu_dra_slices_mdev", "kxpu_dra_slices_taint", "kxpu_dra_slices_mdev_taint",
     "kxpu_aer_health", "kxpu_dra_slices_taints", "kxpu_dra_slices_mdev_taints", "kxpu_cdi_parse", "kxpu_cdi_parse_mdev",
     "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev", "kxpu_cdi_emit_mdev_cdev", "kxpu_cdi_parse_mdev_cdev",
-    "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu",
+    "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu", "kxpu_pcie_tree_mdev",
 ]
 
 
@@ -231,6 +231,7 @@ def load_library():
         "kxpu_vf_vgpu_types": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp]),
         "kxpu_classify_vf_vgpu": (i32, [vp, vp, sz, C.c_uint32, vp, sz, vp, C.POINTER(ClassifyOut), vp, vp, vp]),
         "kxpu_pcie_tree_sriov": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32), vp]),
+        "kxpu_pcie_tree_mdev": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32)]),
         "kxpu_dra_slices_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                          C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_mdev_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
@@ -726,6 +727,25 @@ class Kxpu:
             pf_of = np.ascontiguousarray(pf_of, dtype=np.uint32)
             assert len(pf_of) == n
             self._chk(self.L.kxpu_pcie_tree_sriov(*args, _ptr(pf_of) if n else None))
+        m = nn.value
+        return dict(group_node=gnode[:G], key=key[:m], parent=parent[:m], depth=depth[:m])
+
+    def pcie_tree_mdev(self, recs, paths, group_off, group_members):
+        """kxpu_pcie_tree_mdev: recs (MDEVREC_DTYPE) and paths (PCIPATH_DTYPE, the entries' links) at the same indices,
+        the group CSR of an mdev classify call.  Returns pcie_tree's dict."""
+        recs, paths = np.ascontiguousarray(recs), np.ascontiguousarray(paths)
+        assert recs.dtype == MDEVREC_DTYPE and paths.dtype == PCIPATH_DTYPE and len(recs) == len(paths)
+        group_off = np.ascontiguousarray(group_off, dtype=np.uint32)
+        group_members = np.ascontiguousarray(group_members, dtype=np.uint32)
+        G = len(group_off) - 1
+        cap = max(PCIE_MAX_DEPTH * G, 1)
+        gnode = np.empty(max(G, 1), np.uint32)
+        key, parent, depth = np.empty(cap, np.uint64), np.empty(cap, np.uint32), np.empty(cap, np.uint8)
+        nn = C.c_uint32(0)
+        n = len(recs)
+        self._chk(self.L.kxpu_pcie_tree_mdev(self.ctx, _ptr(recs) if n else None, _ptr(paths) if n else None, n,
+                                             _ptr(group_off), _ptr(group_members) if len(group_members) else None, G,
+                                             _ptr(gnode), _ptr(key), _ptr(parent), _ptr(depth), C.byref(nn)))
         m = nn.value
         return dict(group_node=gnode[:G], key=key[:m], parent=parent[:m], depth=depth[:m])
 

@@ -13,9 +13,13 @@
 //   - the single-pass scan (scan.cuh) of the new-node counts gives each group's first ordinal; the total is n_nodes.
 //   - k_emit: ordinal of prefix (g, t) = base[f] + t - (len(f) - new(f)), f its first group; a group writes key,
 //     parent and depth of its own new nodes and its group_node.
-// kxpu_pcie_tree_sriov runs the same launches with k_parse<true> (which also stores each record's own key) and
-// k_lcp<true> (which reads a VF's chain through its PF); the <false> instantiations are kxpu_pcie_tree's kernels.
+// kxpu_pcie_tree_sriov runs the same launches with k_parse<kxpu_devrec, true> (which also stores each record's own key)
+// and k_lcp<true> (which reads a VF's chain through its PF); the <kxpu_devrec, false> / <false> instantiations are
+// kxpu_pcie_tree's kernels.  kxpu_pcie_tree_mdev runs k_parse<kxpu_mdevrec, false>, whose leaf is the record's UUID
+// below its parent function (lanes 8..11 stage the record's UUID and parent next to the path), and kxpu_pcie_tree's
+// other kernels.
 #include <algorithm>
+#include <type_traits>
 
 #include "common.cuh"
 #include "scan.cuh"
@@ -65,17 +69,47 @@ __device__ int parse_comp(const char *t, int s, int e, unsigned long long *key) 
     return 1;
 }
 
+// component t[s, e) equals the name b[0 .. 16) up to its first NUL
+__device__ __forceinline__ bool same_name(const char *t, int s, int e, const char *b) {
+    int bl = 0;
+    while (bl < 16 && b[bl]) bl++;
+    bool same = e - s == bl;
+    for (int k = 0; same && k < bl; k++) same = t[s + k] == b[k];
+    return same;
+}
+
+// component t[s, e) is a canonical lowercase UUID (8-4-4-4-12) equal to uuid[0 .. 36)
+__device__ __forceinline__ bool uuid_leaf(const char *t, int s, int e, const char *uuid) {
+    bool same = e - s == 36;
+    for (int k = 0; same && k < 36; k++) {
+        const char c = t[s + k];
+        same = c == uuid[k] && ((k == 8 || k == 13 || k == 18 || k == 23) ? c == '-' : hexv(c) >= 0);
+    }
+    return same;
+}
+
 // chain[i * MAXD + t] = key of component t of record i, clen[i] = chain length (0: unknown path).  SR
-// (kxpu_pcie_tree_sriov): self[i] = the key of the record's own component when its path is known.
-template <bool SR>
-__global__ void __launch_bounds__(PARSE_THREADS) k_parse(const kxpu_devrec *__restrict__ recs, const kxpu_pcipath *__restrict__ paths,
+// (kxpu_pcie_tree_sriov): self[i] = the key of the record's own component when its path is known.  Rec = kxpu_mdevrec
+// (kxpu_pcie_tree_mdev): the last component is the record's UUID and the one before it its parent function, which
+// ends the chain.
+template <typename Rec, bool SR>
+__global__ void __launch_bounds__(PARSE_THREADS) k_parse(const Rec *__restrict__ recs, const kxpu_pcipath *__restrict__ paths,
                                                          uint32_t n, unsigned long long *__restrict__ chain, uint8_t *__restrict__ clen,
                                                          unsigned long long *__restrict__ self) {
+    constexpr bool MD = std::is_same<Rec, kxpu_mdevrec>::value;
+    static_assert(!(MD && SR), "the SR-IOV forest reads kxpu_devrec records");
     __shared__ __align__(16) char txt[PARSE_RECS][128];
     const uint32_t lane = threadIdx.x & (PATH_LANES - 1), slot = threadIdx.x / PATH_LANES;
     const uint32_t i = blockIdx.x * PARSE_RECS + slot;
     const bool have = i < n;
     if (have && lane < 8) reinterpret_cast<uint4 *>(txt[slot])[lane] = reinterpret_cast<const uint4 *>(paths + i)[lane];
+    const char *own = nullptr;  // MD: the record's first 64 bytes (uuid at 0, parent at 36), staged by lanes 8..11
+    if constexpr (MD) {
+        __shared__ __align__(16) char head[PARSE_RECS][64];
+        if (have && lane >= 8 && lane < 12)
+            reinterpret_cast<uint4 *>(head[slot])[lane - 8] = reinterpret_cast<const uint4 *>(recs + i)[lane - 8];
+        own = head[slot];
+    }
     __syncwarp();
     const char *t = txt[slot];
     const int len = have ? (uint8_t)t[120] : 0;
@@ -95,15 +129,21 @@ __global__ void __launch_bounds__(PARSE_THREADS) k_parse(const kxpu_devrec *__re
     bool mine = true;
     unsigned long long key = 0;
     if (ok && (int)lane < ncomp) {
-        const int kind = parse_comp(t, s, e, &key);
-        if (lane == 0) mine = kind == 2;
-        else mine = kind != 0;
-        if ((int)lane == ncomp - 1 && mine) {  // the function itself: equals the record's bdf
-            const char *b = recs[i].bdf;
-            int bl = 0;
-            while (bl < 16 && b[bl]) bl++;
-            mine = e - s == bl;
-            for (int k = 0; mine && k < bl; k++) mine = t[s + k] == b[k];
+        if constexpr (MD) {
+            if ((int)lane == ncomp - 1) {  // the mdev itself: its UUID
+                mine = uuid_leaf(t, s, e, own + offsetof(kxpu_mdevrec, uuid));
+            } else {
+                const int kind = parse_comp(t, s, e, &key);
+                if (lane == 0) mine = kind == 2;
+                else mine = kind != 0;
+                // its parent: a function equal to the record's parent (a host bridge there is unknown, also at lane 0)
+                if ((int)lane == ncomp - 2) mine = mine && kind == 1 && same_name(t, s, e, own + offsetof(kxpu_mdevrec, parent));
+            }
+        } else {
+            const int kind = parse_comp(t, s, e, &key);
+            if (lane == 0) mine = kind == 2;
+            else mine = kind != 0;
+            if ((int)lane == ncomp - 1 && mine) mine = same_name(t, s, e, recs[i].bdf);  // the function itself
         }
     }
     const uint32_t half = (threadIdx.x & 31u) & ~(uint32_t)(PATH_LANES - 1);
@@ -258,8 +298,10 @@ __global__ void __launch_bounds__(256) k_emit(const Tree T) {
 
 using namespace kxpcie;
 
-// pf_of == nullptr: kxpu_pcie_tree; else kxpu_pcie_tree_sriov (pf_of checked by the caller)
-static int32_t pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n, const uint32_t *group_off,
+// Rec = kxpu_devrec: pf_of == nullptr: kxpu_pcie_tree; else kxpu_pcie_tree_sriov (pf_of checked by the caller).
+// Rec = kxpu_mdevrec: kxpu_pcie_tree_mdev (pf_of == nullptr).
+template <typename Rec>
+static int32_t pcie_tree(kxpu_ctx *ctx, const Rec *recs, const kxpu_pcipath *paths, size_t n, const uint32_t *group_off,
                          const uint32_t *group_members, size_t n_groups, uint32_t *group_node, uint64_t *key, uint32_t *parent,
                          uint8_t *depth, uint32_t *n_nodes, const uint32_t *pf_of) {
     static_assert(sizeof(kxpu_pcipath) == 128 && offsetof(kxpu_pcipath, len) == 120, "kxpu_pcipath layout");
@@ -281,7 +323,7 @@ static int32_t pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcip
     while (slots < 2 * GD) slots <<= 1;
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
-    const size_t o_recs = take(n * sizeof(kxpu_devrec)), o_paths = take(n * sizeof(kxpu_pcipath));
+    const size_t o_recs = take(n * sizeof(Rec)), o_paths = take(n * sizeof(kxpu_pcipath));
     const size_t o_goff = take((G + 1) * 4), o_gmem = take(nm * 4), o_chain = take(n * MAXD * 8), o_clen = take(n);
     const size_t o_gchain = take(GD * 8), o_glen = take(G), o_slots = take((size_t)slots * 8), o_first = take(GD * 4);
     const size_t o_cnt = take(G * 4), o_base = take(G * 4), o_gnode = take(G * 4), o_parent = take(GD * 4);
@@ -292,7 +334,7 @@ static int32_t pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcip
     KX_CUDA(ctx, sc.alloc((void **)&b, off));
     cudaStream_t st = ctx->stream;
     auto up = [&](size_t o, const void *h, size_t bytes) { if (bytes) cudaMemcpyAsync(b + o, h, bytes, cudaMemcpyHostToDevice, st); };
-    up(o_recs, recs, n * sizeof(kxpu_devrec)); up(o_paths, paths, n * sizeof(kxpu_pcipath));
+    up(o_recs, recs, n * sizeof(Rec)); up(o_paths, paths, n * sizeof(kxpu_pcipath));
     up(o_goff, group_off, (G + 1) * 4); up(o_gmem, group_members, nm * 4);
     if (pf_of) up(o_pf, pf_of, n * 4);
     cudaMemsetAsync(b + o_slots, 0xFF, (size_t)slots * 8, st);
@@ -312,9 +354,10 @@ static int32_t pcie_tree(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcip
     {
         KxTimer tm(ctx, KXPU_T_CLASSIFY);
         if (n) {
-            auto *parse = pf_of ? k_parse<true> : k_parse<false>;
+            auto *parse = k_parse<Rec, false>;
+            if constexpr (std::is_same<Rec, kxpu_devrec>::value) if (pf_of) parse = k_parse<Rec, true>;
             parse<<<(unsigned)((n + PARSE_RECS - 1) / PARSE_RECS), PARSE_THREADS, 0, st>>>(
-                (const kxpu_devrec *)(b + o_recs), (const kxpu_pcipath *)(b + o_paths), (uint32_t)n,
+                (const Rec *)(b + o_recs), (const kxpu_pcipath *)(b + o_paths), (uint32_t)n,
                 (unsigned long long *)(b + o_chain), b + o_clen, (unsigned long long *)(b + o_self));
             ctx->launches++;
         }
@@ -367,4 +410,11 @@ extern "C" int32_t kxpu_pcie_tree_sriov(kxpu_ctx *ctx, const kxpu_devrec *recs, 
     static const uint32_t none = KXPU_NO_PF;  // n == 0: nothing to upload, but still the variant
     return pcie_tree(ctx, recs, paths, n, group_off, group_members, n_groups, group_node, key, parent, depth, n_nodes,
                      n ? pf_of : &none);
+}
+
+extern "C" int32_t kxpu_pcie_tree_mdev(kxpu_ctx *ctx, const kxpu_mdevrec *recs, const kxpu_pcipath *paths, size_t n,
+                                       const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
+                                       uint32_t *group_node, uint64_t *key, uint32_t *parent, uint8_t *depth, uint32_t *n_nodes) {
+    static_assert(sizeof(kxpu_mdevrec) == 128 && offsetof(kxpu_mdevrec, parent) + 16 <= 64, "kxpu_mdevrec layout");
+    return pcie_tree(ctx, recs, paths, n, group_off, group_members, n_groups, group_node, key, parent, depth, n_nodes, nullptr);
 }

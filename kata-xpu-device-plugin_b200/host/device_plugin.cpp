@@ -1147,9 +1147,10 @@ static void mdevRecord(Plugin &p, const std::string &name, bool isDir, kxpu_mdev
 // holds one level of links, so a directory inside it is recorded as such and not descended into.
 Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w) {
     recs.clear();
-    if (w) { w->parentDevice.clear(); w->pcieRoot.clear(); w->cdevs.clear(); }
+    if (w) { w->parentDevice.clear(); w->pcieRoot.clear(); w->paths.clear(); w->cdevs.clear(); }
     std::vector<int64_t> *cdevs = w && mdevCdevEnabled() ? &w->cdevs : nullptr;
-    if (!vgpuDraEnabled()) w = nullptr;
+    const bool dra = vgpuDraEnabled();
+    if (!readsMdevPaths()) w = nullptr;
     DIR *d = opendir(mdevBasePath.c_str());
     if (!d) return fail("Error accessing file path \"" + mdevBasePath + "\": " + strerror(errno));
     std::vector<std::string> names;
@@ -1170,11 +1171,11 @@ Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w) {
             cdevs->push_back(cdevClassOf(vgpuClasses, &XpuClass::mdevCdev, r, r.parent_vendor_txt, sizeof r.parent_vendor_txt)
                                  ? readVfioCdev(mdevBasePath, n) : -1);
         if (!w) continue;
-        // the ResourceSlice reads of an entry that got as far as its iommu_group link
+        // the ResourceSlice and PCIe forest reads of an entry that got as far as its iommu_group link
         std::string dev, target;
         const bool grouped = !isDir && n.size() == sizeof r.uuid &&
                              !(r.flags & (KXPU_REC_VENDOR_ERR | KXPU_REC_DRIVER_ERR | KXPU_REC_IOMMU_ERR));
-        if (grouped && readIDFromFile(mdevBasePath, n, "../device", dev)) {
+        if (dra && grouped && readIDFromFile(mdevBasePath, n, "../device", dev)) {
             dev = trimID(dev);
             bool ok = dev.size() <= 6;
             for (char c : dev) ok = ok && ((c >= '0' && c <= '9') || (c >= 'a' && c <= 'f'));
@@ -1185,6 +1186,8 @@ Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w) {
         kxpu_pcipath pp;
         memset(&pp, 0, sizeof pp);
         if (grouped && readPciPath(mdevBasePath, n, target)) pciPathRecord(target, pp);
+        w->paths.push_back(pp);
+        if (!dra) continue;
         w->parentDevice.push_back(dev);
         w->pcieRoot.push_back(pcieRootOf(&pp));
     }
@@ -1258,6 +1261,14 @@ Error Plugin::classify(MdevWalk &w) {
     w.keys.assign(need ? need : 1, 0);
     rc = kxpu_mdev_names(ctx_, recs.data(), n, first.data(), first.size(), w.keys.data(), need, w.koff.data(), &need);
     if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_mdev_names", rc);
+    if (vgpuPcieTopologyAware) {  // the forest of the walk, one node per group, every mdev below its parent function
+        const size_t cap = (size_t)KXPU_PCIE_MAX_DEPTH * c.nGroups + 1;
+        w.gnode.assign(c.nGroups + 1, KXPU_PCIE_NO_NODE);
+        w.nodeKey.assign(cap, 0); w.nodeParent.assign(cap, 0); w.nodeDepth.assign(cap, 0);
+        rc = kxpu_pcie_tree_mdev(ctx_, recs.data(), w.paths.data(), n, c.goff.data(), c.gmem.data(), c.nGroups, w.gnode.data(),
+                                 w.nodeKey.data(), w.nodeParent.data(), w.nodeDepth.data(), &w.nNodes);
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_pcie_tree_mdev", rc);
+    }
     return Error();
 }
 
@@ -1281,6 +1292,7 @@ void Plugin::buildMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
         GroupState<kxpu_dramdev> s;
         s.klass = groupClass[c.gids[g]];
         if (topologyAware) s.numa = c.gnuma[g];
+        if (vgpuPcieTopologyAware) s.pcieNode = w.gnode[g];
         if (vgpuClasses[s.klass].mdevCdev)  // an mdev without a cdev: VFIO cannot open it
             for (const MdevDevice &m : devs)
                 if (m.cdev < 0) { s.blocker = m.uuid + " has no VFIO cdev"; break; }
@@ -1292,6 +1304,10 @@ void Plugin::buildMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
         for (uint32_t k = c.doff[d]; k < c.doff[d + 1]; k++) groups.push_back(std::to_string(c.dgrp[k]));
         typeMap.emplace_back(std::string((const char *)w.keys.data() + w.koff[d], w.koff[d + 1] - w.koff[d]), std::move(groups));
         typeClass.push_back(c.drule[d]);
+    }
+    if (vgpuPcieTopologyAware) {
+        mdevPcieParent.assign(w.nodeParent.begin(), w.nodeParent.begin() + w.nNodes);
+        mdevPcieDepth.assign(w.nodeDepth.begin(), w.nodeDepth.begin() + w.nNodes);
     }
     buildMdevDra(w);
 }
@@ -2536,7 +2552,7 @@ Error Plugin::ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8
 
 DevicePluginOptions Plugin::GetDevicePluginOptions() const {
     DevicePluginOptions o;  // PreStartRequired: false (generic_device_plugin.go:255)
-    o.GetPreferredAllocationAvailable = topologyAware || pcieTopologyAware;
+    o.GetPreferredAllocationAvailable = topologyAware || pcieTopologyAware || vgpuPcieTopologyAware;
     return o;
 }
 
@@ -2544,7 +2560,8 @@ Error Plugin::GetPreferredAllocation(const GenericDevicePlugin &dp, const std::v
                                      std::vector<ContainerPreferredAllocationResponse> &responses) {
     std::shared_lock<std::shared_mutex> lock(mu_);
     responses.clear();
-    if (!topologyAware && !pcieTopologyAware) return Error();  // the reference's empty response (generic_device_plugin.go:378-386)
+    // the reference's empty response (generic_device_plugin.go:378-386)
+    if (!GetDevicePluginOptions().GetPreferredAllocationAvailable) return Error();
     std::map<std::string, uint32_t> posOf;
     std::vector<uint64_t> numa(dp.devs.size());
     std::vector<uint32_t> node(dp.devs.size());
@@ -2574,9 +2591,12 @@ Error Plugin::GetPreferredAllocation(const GenericDevicePlugin &dp, const std::v
     size_t total = 0;
     for (uint32_t s : size) total += s;
     std::vector<uint32_t> out(total ? total : 1), outOff(requests.size() + 1);
-    const bool pcie = pcieTopologyAware && !dp.vgpu;  // one forest for all passthrough plugins of the walk
-    int32_t rc = pcie ? kxpu_preferred_allocation_pcie(ctx_, numa.data(), node.data(), numa.size(), pcieParent.data(),
-                                                       pcieDepth.data(), pcieParent.size(), availOff.data(), avail.data(),
+    // one forest for all passthrough plugins of the PCI walk, one for all vGPU plugins of the mdev walk
+    const bool pcie = dp.vgpu ? vgpuPcieTopologyAware : pcieTopologyAware;
+    const std::vector<uint32_t> &fParent = dp.vgpu ? mdevPcieParent : pcieParent;
+    const std::vector<uint8_t> &fDepth = dp.vgpu ? mdevPcieDepth : pcieDepth;
+    int32_t rc = pcie ? kxpu_preferred_allocation_pcie(ctx_, numa.data(), node.data(), numa.size(), fParent.data(),
+                                                       fDepth.data(), fParent.size(), availOff.data(), avail.data(),
                                                        mustOff.data(), must.data(), size.data(), requests.size(), out.data(),
                                                        outOff.data())
                       : kxpu_preferred_allocation(ctx_, numa.data(), numa.size(), availOff.data(), avail.data(), mustOff.data(),
@@ -3312,6 +3332,7 @@ int kxh_gather_mdev_topo(const char *mdev_base, const char *classes, int topo, i
 
 // ---- PCIe topology (tests)
 void kxh_set_pcie_topology(void *h, int on) { ((Plugin *)h)->pcieTopologyAware = on != 0; }
+void kxh_set_vgpu_pcie_topology(void *h, int on) { ((Plugin *)h)->vgpuPcieTopologyAware = on != 0; }
 
 // CPU only: the raw PCI gather with pcieTopologyAware = pcie; counting_seam != 0 wraps readPciPath in a counter of its
 // calls (*path_reads), which also sends the fast gather down the walk

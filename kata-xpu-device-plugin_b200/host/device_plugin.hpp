@@ -55,7 +55,9 @@ struct Device {  // pluginapi.Device
     std::string ID;
     std::string Health;
     uint64_t numa = 0;  // Device.Topology: bit k = NUMA node k (the group's mask); 0 = no topology
-    uint32_t pcieNode = KXPU_PCIE_NO_NODE;  // the group's node in Plugin::pcieParent / pcieDepth (pcieTopologyAware)
+    // the group's node in Plugin::pcieParent / pcieDepth (pcieTopologyAware); a vGPU plugin's device: in
+    // Plugin::mdevPcieParent / mdevPcieDepth (vgpuPcieTopologyAware)
+    uint32_t pcieNode = KXPU_PCIE_NO_NODE;
     // groupViability: why VFIO cannot open the group ("<bdf> is bound to <driver>"), from the last walk; empty = viable.
     // Separate from Health, which the HealthWatcher flips: the device is sent Unhealthy when either says so.
     std::string blocker{};
@@ -272,6 +274,13 @@ struct MdevWalk {
     // vgpuDraEnabled only, one per record: the parent's device id (<uuid>/../device) and the PCIe root of the entry's
     // link; "" = not read, failed or outside kxpu_dramdev's domain
     std::vector<std::string> parentDevice, pcieRoot;
+    // readsMdevPaths, one per record: the entry's link as a kxpu_pcipath (len 0: not read or unknown); with
+    // vgpuPcieTopologyAware, the walk's PCIe forest (kxpu_pcie_tree_mdev)
+    std::vector<kxpu_pcipath> paths;
+    std::vector<uint32_t> gnode, nodeParent;
+    std::vector<uint64_t> nodeKey;
+    std::vector<uint8_t> nodeDepth;
+    uint32_t nNodes = 0;
     // mdevCdevEnabled only, one per record: N of its VFIO cdev, -1 = none or not read
     std::vector<int64_t> cdevs;
 };
@@ -282,7 +291,9 @@ template <typename Dra>  // kxpu_dradev (passthrough) or kxpu_dramdev (vGPU)
 struct GroupState {
     size_t klass = 0;  // index into xpuClasses (vgpuClasses): the class of the group's first member
     uint64_t numa = 0;  // topologyAware: the group's NUMA mask; 0 = no topology
-    uint32_t pcieNode = KXPU_PCIE_NO_NODE;  // pcieTopologyAware, passthrough only: the group's node in pcieParent / pcieDepth
+    // pcieTopologyAware: the group's node in pcieParent / pcieDepth; a vGPU group (vgpuPcieTopologyAware): in
+    // mdevPcieParent / mdevPcieDepth
+    uint32_t pcieNode = KXPU_PCIE_NO_NODE;
     // why VFIO cannot open the group, empty = it can: "<bdf> is bound to <driver>" (groupViability), else "<bdf> has no
     // VFIO cdev" (vfioCdev), else sriov; a vGPU group: "<uuid> has no VFIO cdev" (mdevCdev)
     std::string blocker{};
@@ -335,9 +346,18 @@ class Plugin {
     // the PCI gathers read the link <basePath>/<entry> through readPciPath (the whole target), each record keeps its path
     // from the first component that begins with "pci", kxpu_pcie_tree builds the walk's forest, every passthrough Device
     // carries its group's node, and GetPreferredAllocation keeps an allocation under as few PCIe switches as it can
-    // (kxpu_preferred_allocation_pcie; vGPU plugins keep the NUMA answer).  Both settings may be on together.
+    // (kxpu_preferred_allocation_pcie; vGPU plugins keep the NUMA answer unless vgpuPcieTopologyAware is on).  Both
+    // settings may be on together.
     bool pcieTopologyAware = false;
     std::function<bool(const std::string &base, const std::string &entry, std::string &target)> readPciPath;
+    // PCIe topology of vGPUs (include/kxpu.h, kxpu_pcie_tree_mdev).  false (default): nothing more is read and every
+    // output is as above, the NUMA answer of vGPU plugins under pcieTopologyAware included.  true: the mdev walk reads the
+    // link <mdevBasePath>/<uuid> of every entry that got as far as its iommu_group link (readPciPath, the read
+    // vgpuDraEnabled does), kxpu_pcie_tree_mdev builds the walk's forest with each mdev below its parent function, every
+    // vGPU Device carries its group's node, and GetPreferredAllocation of a vGPU plugin keeps an allocation under as few
+    // GPUs, then switches, as it can (kxpu_preferred_allocation_pcie).  It rests on the vGPU manager accepting several
+    // vGPUs of one GPU in one VM [assumed], which is why it is a setting of its own.
+    bool vgpuPcieTopologyAware = false;
     // IOMMU group viability (include/kxpu.h, ABI v8).  false (default): nothing more is read and every output is as
     // above.  true: for every non-directory entry that is not a class candidate the gathers read its `driver` link (when
     // not read yet); a bound driver that is neither in viabilityDrivers nor the driver of a class makes the entry a
@@ -361,6 +381,8 @@ class Plugin {
     // read only leaves out its attribute.  The PCI walk and every device-plugin output stay as they are.
     bool vgpuDraEnabled() const;  // some vGPU class has a draDriver
     bool readsMdevNuma() const { return topologyAware || vgpuDraEnabled(); }
+    // the mdev walk reads each grouped entry's link (vgpuPcieTopologyAware or vgpuDraEnabled); one read serves both
+    bool readsMdevPaths() const { return vgpuPcieTopologyAware || vgpuDraEnabled(); }
     // DRA device taints (ABI v11).  false (default): the slices never carry taints and every output and generation is as
     // above, even while a device is Unhealthy.  true: ResourceSlices and VgpuResourceSlices pass taint times to the
     // slice call (64 devices per slice); a group that refreshDraHealth found unhealthy carries the taint
@@ -439,6 +461,9 @@ class Plugin {
     OrderedMap<std::vector<std::string>> typeMap;
     std::vector<GroupState<kxpu_dramdev>> mdevState;
     std::vector<size_t> typeClass;
+    // vgpuPcieTopologyAware only: the forest of the last mdev walk, shared by all vGPU plugins
+    std::vector<uint32_t> mdevPcieParent;
+    std::vector<uint8_t> mdevPcieDepth;
     std::vector<std::string> mdevCdiFiles;  // files the last generateMdevCDISpec wrote, one per vGPU class
 
     explicit Plugin(kxpu_ctx *ctx);
@@ -467,7 +492,8 @@ class Plugin {
     Error Allocate(const std::vector<std::string> &devicesIDs, ContainerAllocateResponse &resp);
     // generic_device_plugin.go:224: the bytes of ListAndWatchResponse{Devices: dpi.devs}
     Error ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8_t> &out);
-    // generic_device_plugin.go:253-258: GetPreferredAllocationAvailable = topologyAware || pcieTopologyAware
+    // generic_device_plugin.go:253-258: GetPreferredAllocationAvailable = topologyAware || pcieTopologyAware ||
+    // vgpuPcieTopologyAware
     DevicePluginOptions GetDevicePluginOptions() const;
     // generic_device_plugin.go:378-386 (the reference: nil, nil).  topologyAware: one kxpu_preferred_allocation call for
     // all container requests, device IDs mapped to positions in dp.devs; an ID not in dp.devs is an error naming it.
@@ -546,8 +572,8 @@ class Plugin {
     // anything else (never an error)
     int64_t readVfioCdev(const std::string &base, const std::string &entry);
     // raw gather of mdevBasePath under vgpuClasses (no GPU): one record per entry, lexical order.  w (vgpuDraEnabled
-    // only, else left empty): the walk's parentDevice and pcieRoot, one per record; (mdevCdevEnabled only, else left
-    // empty) its cdevs
+    // only, else left empty): the walk's parentDevice and pcieRoot, one per record; (readsMdevPaths only, else left
+    // empty) its paths; (mdevCdevEnabled only, else left empty) its cdevs
     Error gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w = nullptr);
     // the vGPU class list against the passthrough one (distinct CDI kinds and file stems, no vfioCdev on a vGPU class, no
     // mdevCdev on a passthrough class); createMdevMap runs it

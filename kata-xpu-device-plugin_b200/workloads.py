@@ -426,6 +426,51 @@ def pcie_walk(n=1 << 20, seed=21, group_max=4):
     return recs, paths, np.array(off, np.uint32), np.array(members, np.uint32)
 
 
+def pcie_mdev_walk(n=1 << 20, seed=23, per_gpu=32):
+    """n mdev records (MDEVREC_DTYPE, UUIDs in lexical order, one group each) with the kxpu_pcipath of each entry's link,
+    and a PCI twin with the same forest shape.  per_gpu vGPUs per parent GPU, the parents scattered over the walk order
+    (lexical UUID order says nothing about the hardware).  Per domain: a host bridge, 8 root ports, a switch under each
+    with one down port per GPU; 3 % of the paths unknown (len 0), 1 % with an upper-case UUID (unknown).  The twin's
+    record k is a PCI function whose path is the same chain followed by its own bdf, so kxpu_pcie_tree gives it the
+    chain of mdev k.  Returns (recs, paths, group_off, group_members, twin_recs, twin_paths)."""
+    from .binding import PCIPATH_DTYPE
+    rng = np.random.default_rng(seed)
+    n_gpu = max((n + per_gpu - 1) // per_gpu, 1)
+    g = np.arange(n_gpu, dtype=np.int64)
+    dom, bus = g >> 8, g & 255
+    pre, gpu = [], []
+    for d, b in zip(dom.tolist(), bus.tolist()):
+        gb = "%04x:%02x:00.0" % (d, b)
+        pre.append("pci%04x:00/%04x:00:%02x.0/%04x:%02x:00.0/%04x:%02x:%02x.0/%s"
+                   % (d, d, 1 + (b >> 5), d, 0xE0 | (b >> 5), d, 0xE8 | (b >> 5), b & 31, gb))
+        gpu.append(gb)
+    pre, gpu = np.array(pre, dtype="S96"), np.array(gpu, dtype="S16")
+    gpu_of = rng.permutation(n) // per_gpu
+    recs = np.zeros(n, dtype=MDEVREC_DTYPE)
+    u = uuids(n, seed).view("S36").reshape(n)
+    recs["uuid"] = u
+    recs["parent"] = gpu[gpu_of]
+    recs["parent_vendor_txt"] = _id_text(np.full(n, 0x10DE))
+    recs["vendor_len"] = 7
+    recs["driver"] = b"nvidia-vgpu"
+    recs["iommu_group"] = np.arange(n, dtype=np.uint32) + 100
+    r = rng.random(n)
+    leaf = np.where((r >= 0.03) & (r < 0.04), np.char.upper(u), u)
+    text = np.char.add(np.char.add(pre[gpu_of], b"/"), leaf)
+    paths = np.zeros(n, dtype=PCIPATH_DTYPE)
+    paths["path"] = text.astype("S120")
+    paths["len"] = np.where(r < 0.03, 0, np.char.str_len(text)).astype(np.uint8)
+    twin = np.zeros(n, dtype=DEVREC_DTYPE)
+    bdfs = enumerate_bdfs(n).view("S16").reshape(n)
+    twin["bdf"] = bdfs
+    twin_text = np.char.add(np.char.add(pre[gpu_of], b"/"), bdfs)
+    twin_paths = np.zeros(n, dtype=PCIPATH_DTYPE)
+    twin_paths["path"] = twin_text.astype("S120")
+    twin_paths["len"] = np.where(r < 0.04, 0, np.char.str_len(twin_text)).astype(np.uint8)
+    off = np.arange(n + 1, dtype=np.uint32)
+    return recs, paths, off, np.arange(n, dtype=np.uint32), twin, twin_paths
+
+
 # ---------------------------------------------------------------- runtime rediscovery (ABI v6)
 def fnv1a64(data: bytes) -> int:
     """64-bit FNV-1a: the snapshot tag of an mdev (over its type key)."""
