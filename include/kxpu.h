@@ -72,7 +72,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
 #define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s and kxpu_sriov's kernels: the slot holds the most recent call's */
-#define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev]: decode, re-emit and compare of the most recent call */
+#define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev|_vf_vgpu[_cdev]]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
 #define KXPU_T_COUNT    8
@@ -947,6 +947,60 @@ int32_t kxpu_cdi_emit_mdev_cdev(kxpu_ctx *ctx, int32_t format, const char *kind,
  * KXPU_CDI_FRAG_MIN still bounds *n.  Everything else as kxpu_cdi_parse_mdev. */
 int32_t kxpu_cdi_parse_mdev_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
                                  kxpu_mdevcdev *out, size_t cap, size_t *n);
+
+/* ------------------------- CDI specs that carry the vGPU type of each SR-IOV VF (additions to ABI v14) */
+
+/* These four calls were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym), as the ctypes
+ * binding and the Go shim do.  A VF that carries a vGPU type lists nothing in creatable_vgpu_types, so a restarted
+ * plugin on a full GPU cannot learn the names of the types it serves from sysfs; and a spec that does not hold each VF's
+ * type cannot tell a restarted plugin that a VF changed type while it was down.  These layouts put the type ID and the
+ * type key of each VF in two more device annotations, so the spec itself carries both facts across a restart.
+ *   [assumed] the container runtime's CDI registry accepts any string value of a device annotation and ignores keys it
+ *             does not know (the bdf and mdev annotations already rest on this). */
+
+/* One served VF of a class that serves vGPUs on SR-IOV VFs.  80 bytes (16-byte strides for the kernels' vector loads). */
+typedef struct kxpu_vfvgpucdi {
+    kxpu_cdidev dev;         /* exactly what kxpu_cdi_emit_kind / kxpu_cdi_emit_cdev read                    */
+    uint32_t    type_id;     /* the VF's vGPU type ID, 1 .. 2^32-1                                            */
+    uint8_t     key_len;     /* 1 .. 40                                                                       */
+    uint8_t     reserved[3]; /* ignored by the emitters, written 0 by the parsers                             */
+    char        key[40];     /* its type key (kxpu_vgpukey.key): bytes past key_len are ignored, written 0    */
+} kxpu_vfvgpucdi;
+
+/* kxpu_cdi_emit_kind's document for devs[i].dev, byte for byte, except for two more annotations per device.  The
+ * annotations, in sorted key order (the same for yaml.v3 and encoding/json):
+ *   attach-pci: "true"
+ *   bdf: <address>                    (yaml.v3's isBase60Float quoting, as for kxpu_cdi_emit)
+ *   cdi.k8s.io/vfio<g>: <kind>=<index>
+ *   vgpu-type: "<type_id>"            (canonical decimal)
+ *   vgpu-type-key: "<key>"
+ * Both new values are always double-quoted, in YAML too: this is this project's canonical form.  A plain 557, or a key
+ * such as 1e5, true, No, 0x1F, .inf or 2024-01-01, would resolve as a non-string, and a CDI registry that reads
+ * annotations as map[string]string would then refuse the whole spec.  Over the key alphabet [A-Za-z0-9_.-] and the
+ * digits a quoted value needs no escape in either format.
+ * KXPU_E_UNSUPPORTED, with nothing written: every case kxpu_cdi_emit_kind refuses, type_id 0, key_len 0 or above 40, or
+ * a key byte (of the first key_len) outside [A-Za-z0-9_.-].
+ * GPU: the kernel of kxpu_cdi_emit_kind with the annotations compiled in; each record is read with five 16-byte loads
+ * and a warp copies the key straight from the device array.  The longest fragment grows by 104 bytes, and kinds up to 22
+ * bytes run at three CTAs per SM, longer ones at two (DESIGN.md K6).  Timed under KXPU_T_EMIT. */
+int32_t kxpu_cdi_emit_vf_vgpu(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_vfvgpucdi *devs, size_t n,
+                              uint8_t *out, size_t cap, size_t *len);
+/* kxpu_cdi_emit_vf_vgpu's document, except that the device node of device i is /dev/vfio/devices/vfio<N> with
+ * N = devs[i].dev.vfio_cdev in place of /dev/vfio/<g> (kxpu_cdi_emit_cdev's node).  Everything else as
+ * kxpu_cdi_emit_vf_vgpu. */
+int32_t kxpu_cdi_emit_vf_vgpu_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_vfvgpucdi *devs, size_t n,
+                                   uint8_t *out, size_t cap, size_t *len);
+
+/* The inverses: KXPU_OK with *n records exactly when kxpu_cdi_emit_vf_vgpu (_cdev: kxpu_cdi_emit_vf_vgpu_cdev) given
+ * them returns doc byte for byte.  dev is what kxpu_cdi_parse (_cdev: kxpu_cdi_parse_cdev) returns; type_id, key_len and
+ * key come from the annotations, reserved and the key bytes past key_len are 0.  The six CDI layouts (kind, cdev, mdev,
+ * mdev cdev and these two) refuse each other's documents with KXPU_E_INVALID; the zero-device documents are the same
+ * bytes in every layout, and every parser returns *n = 0 for them.  KXPU_CDI_FRAG_MIN still bounds *n.  Everything else
+ * as kxpu_cdi_parse. */
+int32_t kxpu_cdi_parse_vf_vgpu(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
+                               kxpu_vfvgpucdi *out, size_t cap, size_t *n);
+int32_t kxpu_cdi_parse_vf_vgpu_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
+                                    kxpu_vfvgpucdi *out, size_t cap, size_t *n);
 
 /* ------------------------------------------------------ S5: Allocate names */
 

@@ -702,6 +702,77 @@ func (k *kxpu) cdiParseMdevCdev(format int, doc []byte, kind string) ([]C.kxpu_m
 	return out[:n], nil
 }
 
+// The spec of a class that serves vGPUs on SR-IOV VFs, with each VF's vGPU type (additions to ABI v14, detected by
+// symbol).  cdiEmitVfVgpu writes cdiEmitKind's document (cdev: cdiEmitCdev's) for devs[i].dev with two more annotations
+// per device, vgpu-type: "<type_id>" and vgpu-type-key: "<key>"; cdiParseVfVgpu is its inverse.  Written when indices
+// are resumed across restarts, so that a restarted plugin reads back the names of the types it serves (a full GPU
+// lists none in creatable_vgpu_types) and gives a VF whose type changed while it was down a fresh index.  The six CDI
+// parsers refuse each other's documents, except the zero-device document, which all of them accept.
+func (k *kxpu) cdiEmitVfVgpu(format int, kind string, devs []C.kxpu_vfvgpucdi) ([]byte, error) {
+	return k.cdiEmitVfVgpuCall(format, kind, devs, false)
+}
+
+func (k *kxpu) cdiEmitVfVgpuCdev(format int, kind string, devs []C.kxpu_vfvgpucdi) ([]byte, error) {
+	return k.cdiEmitVfVgpuCall(format, kind, devs, true)
+}
+
+func (k *kxpu) cdiEmitVfVgpuCall(format int, kind string, devs []C.kxpu_vfvgpucdi, cdev bool) ([]byte, error) {
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	var p *C.kxpu_vfvgpucdi
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	// cgo calls a C function only by name, so each layout has its own call
+	call := func(out *C.uint8_t, cap C.size_t, n *C.size_t) C.int32_t {
+		if cdev {
+			return C.kxpu_cdi_emit_vf_vgpu_cdev(k.ctx, C.int32_t(format), ck, p, C.size_t(len(devs)), out, cap, n)
+		}
+		return C.kxpu_cdi_emit_vf_vgpu(k.ctx, C.int32_t(format), ck, p, C.size_t(len(devs)), out, cap, n)
+	}
+	what := "kxpu_cdi_emit_vf_vgpu"
+	if cdev {
+		what = "kxpu_cdi_emit_vf_vgpu_cdev"
+	}
+	var n C.size_t
+	call(nil, 0, &n) // sizing call
+	buf := make([]byte, n+1)
+	err := kxCheck(k.ctx, what, call((*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n))
+	return buf[:n], err
+}
+
+func (k *kxpu) cdiParseVfVgpu(format int, doc []byte, kind string) ([]C.kxpu_vfvgpucdi, error) {
+	return k.cdiParseVfVgpuCall(format, doc, kind, false)
+}
+
+func (k *kxpu) cdiParseVfVgpuCdev(format int, doc []byte, kind string) ([]C.kxpu_vfvgpucdi, error) {
+	return k.cdiParseVfVgpuCall(format, doc, kind, true)
+}
+
+func (k *kxpu) cdiParseVfVgpuCall(format int, doc []byte, kind string, cdev bool) ([]C.kxpu_vfvgpucdi, error) {
+	ck := C.CString(kind)
+	defer C.free(unsafe.Pointer(ck))
+	out := make([]C.kxpu_vfvgpucdi, len(doc)/C.KXPU_CDI_FRAG_MIN+1)
+	var n C.size_t
+	var dp *C.uint8_t
+	if len(doc) > 0 {
+		dp = (*C.uint8_t)(unsafe.Pointer(&doc[0]))
+	}
+	var rc C.int32_t
+	what := "kxpu_cdi_parse_vf_vgpu"
+	if cdev {
+		what = "kxpu_cdi_parse_vf_vgpu_cdev"
+		rc = C.kxpu_cdi_parse_vf_vgpu_cdev(k.ctx, C.int32_t(format), ck, dp, C.size_t(len(doc)), &out[0], C.size_t(len(out)), &n)
+	} else {
+		rc = C.kxpu_cdi_parse_vf_vgpu(k.ctx, C.int32_t(format), ck, dp, C.size_t(len(doc)), &out[0], C.size_t(len(out)), &n)
+	}
+	err := kxCheck(k.ctx, what, rc)
+	if err != nil {
+		return nil, err
+	}
+	return out[:n], nil
+}
+
 // cdiParseVgpuSpec: the records of a vGPU class's previous spec for the restart resume (resumeWalk's prev entries).  It
 // is parsed with the layout the class uses now (mdevCdev: the cdev layout), then with the other one, so a class that
 // switched mdevCdev across the restart keeps its indices; only the kxpu_mdevcdi part (uuid, group, index) is returned.

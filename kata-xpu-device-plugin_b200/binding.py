@@ -46,6 +46,10 @@ assert MDEVREC_DTYPE.itemsize == 128 and MDEVCDI_DTYPE.itemsize == 64
 # kxpu_mdevcdev: a vGPU of a class served through VFIO cdevs (an addition to ABI v14)
 MDEVCDEV_DTYPE = np.dtype([("dev", MDEVCDI_DTYPE), ("vfio_cdev", "<u4"), ("reserved", "<u4", (3,))])
 assert MDEVCDEV_DTYPE.itemsize == 80 and MDEVCDEV_DTYPE.fields["vfio_cdev"][1] == 64
+# kxpu_vfvgpucdi: a served VF of a class that serves vGPUs on SR-IOV VFs, with its type (an addition to ABI v14)
+VFVGPUCDI_DTYPE = np.dtype([("dev", CDIDEV_DTYPE), ("type_id", "<u4"), ("key_len", "u1"), ("reserved", "u1", (3,)),
+                            ("key", "S40")])
+assert VFVGPUCDI_DTYPE.itemsize == 80 and VFVGPUCDI_DTYPE.fields["key"][1] == 40
 # kxpu_snaprec / kxpu_reconcile_counts (runtime rediscovery, ABI v6)
 SNAPREC_DTYPE = np.dtype([("key", "S40"), ("iommu_group", "<u4"), ("klass", "<u4"), ("tag", "<u8"), ("index", "<u8")])
 RC_COUNTS_DTYPE = np.dtype([("n_kept", "<u8"), ("n_new", "<u8"), ("n_changed", "<u8"), ("n_retired", "<u8"),
@@ -113,6 +117,7 @@ ABI_SYMBOLS = [
     "kxpu_aer_health", "kxpu_dra_slices_taints", "kxpu_dra_slices_mdev_taints", "kxpu_cdi_parse", "kxpu_cdi_parse_mdev",
     "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev", "kxpu_cdi_emit_mdev_cdev", "kxpu_cdi_parse_mdev_cdev",
     "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu", "kxpu_pcie_tree_mdev",
+    "kxpu_cdi_emit_vf_vgpu", "kxpu_cdi_emit_vf_vgpu_cdev", "kxpu_cdi_parse_vf_vgpu", "kxpu_cdi_parse_vf_vgpu_cdev",
 ]
 
 
@@ -227,6 +232,10 @@ def load_library():
         "kxpu_cdi_parse_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_cdi_emit_mdev_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_cdi_parse_mdev_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_cdi_emit_vf_vgpu": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_cdi_emit_vf_vgpu_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_cdi_parse_vf_vgpu": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
+        "kxpu_cdi_parse_vf_vgpu_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_sriov": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp, sz, vp, vp, vp]),
         "kxpu_vf_vgpu_types": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp]),
         "kxpu_classify_vf_vgpu": (i32, [vp, vp, sz, C.c_uint32, vp, sz, vp, C.POINTER(ClassifyOut), vp, vp, vp]),
@@ -818,6 +827,12 @@ class Kxpu:
         (MDEVCDEV_DTYPE devices; kind bytes or str)."""
         return self._emit_sized(self.L.kxpu_cdi_emit_mdev_cdev, MDEVCDEV_DTYPE, fmt, devs, kind)
 
+    def cdi_emit_vf_vgpu(self, fmt, devs, kind, cdev=False):
+        """kxpu_cdi_emit_vf_vgpu (cdev: kxpu_cdi_emit_vf_vgpu_cdev): the CDI spec of a class that serves vGPUs on SR-IOV
+        VFs, with each VF's type ID and key (VFVGPUCDI_DTYPE devices; kind bytes or str)."""
+        fn = self.L.kxpu_cdi_emit_vf_vgpu_cdev if cdev else self.L.kxpu_cdi_emit_vf_vgpu
+        return self._emit_sized(fn, VFVGPUCDI_DTYPE, fmt, devs, kind)
+
     def _emit_sized(self, fn, dtype, fmt, devs, kind):
         """the two-call sizing protocol: out = NULL gives the length, the second call writes the document"""
         devs = np.ascontiguousarray(devs)
@@ -944,12 +959,21 @@ class Kxpu:
         """kxpu_cdi_parse_mdev_cdev: the MDEVCDEV_DTYPE records of a spec kxpu_cdi_emit_mdev_cdev wrote."""
         return self._parse(self.L.kxpu_cdi_parse_mdev_cdev, MDEVCDEV_DTYPE, fmt, doc, kind)
 
-    def cdi_parse_raw(self, fmt, doc, kind, cap, mdev=False, offset=0, cdev=False):
+    def cdi_parse_vf_vgpu(self, fmt, doc, kind, cdev=False):
+        """kxpu_cdi_parse_vf_vgpu (cdev: kxpu_cdi_parse_vf_vgpu_cdev): the VFVGPUCDI_DTYPE records of a spec the matching
+        emit call wrote."""
+        fn = self.L.kxpu_cdi_parse_vf_vgpu_cdev if cdev else self.L.kxpu_cdi_parse_vf_vgpu
+        return self._parse(fn, VFVGPUCDI_DTYPE, fmt, doc, kind)
+
+    def cdi_parse_raw(self, fmt, doc, kind, cap, mdev=False, offset=0, cdev=False, typed=False):
         """The bare call: doc placed at `offset` bytes past a 16-byte aligned host buffer, out of `cap` records.
         Returns (status, n, records) with n and the records as the call left them (n = -1: not stored).
         mdev and cdev: kxpu_cdi_parse_mdev_cdev, mdev: kxpu_cdi_parse_mdev, cdev: kxpu_cdi_parse_cdev, neither:
-        kxpu_cdi_parse."""
-        if mdev and cdev:
+        kxpu_cdi_parse; typed: kxpu_cdi_parse_vf_vgpu, or with cdev kxpu_cdi_parse_vf_vgpu_cdev."""
+        if typed:
+            dtype = VFVGPUCDI_DTYPE
+            fn = self.L.kxpu_cdi_parse_vf_vgpu_cdev if cdev else self.L.kxpu_cdi_parse_vf_vgpu
+        elif mdev and cdev:
             dtype, fn = MDEVCDEV_DTYPE, self.L.kxpu_cdi_parse_mdev_cdev
         else:
             dtype = MDEVCDI_DTYPE if mdev else CDIDEV_DTYPE

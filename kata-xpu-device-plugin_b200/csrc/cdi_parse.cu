@@ -1,4 +1,4 @@
-// cdi_parse.cu -- K13: kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev], the inverse of the CDI spec emitter (emit.cu, K6).
+// cdi_parse.cu -- K13: kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev|_vf_vgpu[_cdev]], the inverse of the CDI spec emitter (emit.cu, K6).
 //
 // A call accepts a document exactly when the emitter, given the records it decodes, writes the same bytes.  It runs in
 // two steps:
@@ -25,14 +25,17 @@ constexpr int ROWS = PT / PARSE_THREADS;  // positions per thread, one row of 25
 constexpr int LEAD = 16;         // bytes staged in front of the tile: the '\n' before a start at the tile's first byte
 constexpr int PAT_MAX = 32;
 constexpr int LAYOUT_PCI = KX_CDI_PCI, LAYOUT_MDEV = KX_CDI_MDEV, LAYOUT_CDEV = KX_CDI_CDEV,
-              LAYOUT_MDEV_CDEV = KX_CDI_MDEV_CDEV;
+              LAYOUT_MDEV_CDEV = KX_CDI_MDEV_CDEV, LAYOUT_TYPED = KX_CDI_TYPED, LAYOUT_TYPED_CDEV = KX_CDI_TYPED_CDEV;
+template <int LAYOUT> constexpr bool is_typed_layout = LAYOUT == LAYOUT_TYPED || LAYOUT == LAYOUT_TYPED_CDEV;
 // bytes staged past the tile: >= the layout's longest fragment plus the start pattern, in whole 16-byte words
-template <int LAYOUT> constexpr int HALO = LAYOUT == LAYOUT_MDEV_CDEV ? 528 : 512;
-constexpr int HALO_MAX = HALO<LAYOUT_MDEV_CDEV>;  // the host pads every document for the largest halo
+template <int LAYOUT> constexpr int HALO = is_typed_layout<LAYOUT> ? 576 : LAYOUT == LAYOUT_MDEV_CDEV ? 528 : 512;
+constexpr int HALO_MAX = HALO<LAYOUT_TYPED>;  // the host pads every document for the largest halo
 static_assert(HALO<LAYOUT_PCI> >= KX_CDI_FRAG_MAX + PAT_MAX, "a fragment that starts in the tile must end inside the window");
 static_assert(HALO<LAYOUT_MDEV_CDEV> >= KX_CDI_FRAG_MAX_MDEV_CDEV + PAT_MAX && HALO<LAYOUT_MDEV_CDEV> % 16 == 0,
               "a fragment that starts in the tile must end inside the window");
-static_assert(HALO_MAX >= HALO<LAYOUT_PCI>, "the host padding must cover every layout's window");
+static_assert(HALO<LAYOUT_TYPED> >= KX_CDI_FRAG_MAX_TYPED + PAT_MAX && HALO<LAYOUT_TYPED> % 16 == 0,
+              "a fragment that starts in the tile must end inside the window");
+static_assert(HALO_MAX >= HALO<LAYOUT_PCI> && HALO_MAX >= HALO<LAYOUT_MDEV_CDEV>, "the host padding must cover every layout's window");
 template <int LAYOUT> constexpr int WIN = LEAD + PT + HALO<LAYOUT>;
 
 struct ParseParams {
@@ -47,7 +50,9 @@ struct ParseParams {
     uint32_t l1, l2, l3, lm;      // literal 1, literal 2, literal 3 (with the kind), literal 4 (mdev: the annotation's
                                   // opening, cdev: the node literal)
     uint8_t pat[PAT_MAX];
-    uint32_t l9;                  // mdev cdev: the literal after the uuid, which ends in the node literal
+    uint32_t l9;                  // mdev cdev: the literal after the uuid, which ends in the node literal; the typed
+                                  // layouts: the literal between the type ID and the key
+    uint32_t l10;                 // the typed layouts: the literal after the key (the node literal)
 };
 
 template <int LAYOUT>
@@ -125,7 +130,35 @@ __global__ void __launch_bounds__(PARSE_THREADS) k_cdi_decode(const __grid_const
         uint32_t group = 0;
         for (uint32_t k = 0; k < 10u && is_digit(at(q)); k++, q++) group = group * 10u + (at(q) - '0');
         if (slot >= P.cap) continue;
-        if (LAYOUT == LAYOUT_PCI) {
+        if constexpr (is_typed_layout<LAYOUT>) {  // the type ID follows the name's second copy and literal 4, then literal 9,
+                                                  // the key up to its closing quote, literal 10 and (typed cdev) N
+            q += P.l3 + (name_end - name_at) + P.lm;
+            uint32_t type_id = 0;
+            for (uint32_t k = 0; k < 10u && is_digit(at(q)); k++, q++) type_id = type_id * 10u + (at(q) - '0');
+            q += P.l9;
+            uint32_t kw[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0}, kl = 0;  // the key, packed as it sits in the record
+            bool open = true;
+#pragma unroll
+            for (uint32_t k = 0; k < 40u; k++) {
+                const uint8_t c = open ? at(q + k) : (uint8_t)0;
+                open = open && c != '"' && c != '\n' && c != 0;
+                if (open) { kw[k >> 2] |= (uint32_t)c << (8u * (k & 3u)); kl++; }
+            }
+            q += kl;
+            uint32_t node = 0;
+            if constexpr (LAYOUT == LAYOUT_TYPED_CDEV) {
+                q += P.l10;
+                for (uint32_t k = 0; k < 10u && is_digit(at(q)); k++, q++) node = node * 10u + (at(q) - '0');
+            }
+            uint32_t bw[4];
+            memcpy(bw, bdf, 16);
+            uint4 *o = reinterpret_cast<uint4 *>(static_cast<kxpu_vfvgpucdi *>(P.recs) + slot);
+            o[0] = make_uint4(bw[0], bw[1], bw[2], bw[3]);
+            o[1] = make_uint4(group, node, (uint32_t)index, (uint32_t)(index >> 32));
+            o[2] = make_uint4(type_id, kl, kw[0], kw[1]);  // key_len, reserved[3] = 0
+            o[3] = make_uint4(kw[2], kw[3], kw[4], kw[5]);
+            o[4] = make_uint4(kw[6], kw[7], kw[8], kw[9]);
+        } else if (LAYOUT == LAYOUT_PCI) {
             kxpu_cdidev d;
             memcpy(d.bdf, bdf, 16);
             d.iommu_group = group;
@@ -192,7 +225,8 @@ static void decode_launch(kxpu_ctx *ctx, uint32_t tiles, const ParseParams &P) {
     k_cdi_decode<FMT, LAYOUT><<<tiles, PARSE_THREADS, 0, ctx->stream>>>(P);
 }
 
-// LAYOUT_MDEV: out is kxpu_mdevcdi[cap], LAYOUT_MDEV_CDEV: kxpu_mdevcdev[cap], else kxpu_cdidev[cap]
+// LAYOUT_MDEV: out is kxpu_mdevcdi[cap], LAYOUT_MDEV_CDEV: kxpu_mdevcdev[cap], the typed layouts kxpu_vfvgpucdi[cap],
+// else kxpu_cdidev[cap]
 static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len, void *out,
                          size_t cap, size_t *n, int layout, const char *what) {
     const bool mdev = layout == LAYOUT_MDEV || layout == LAYOUT_MDEV_CDEV;
@@ -203,22 +237,24 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
-    std::string part[10];
-    for (int k = 0; k < 10; k++) part[k] = kx_cdi_part(format, layout, k, kind);
+    const bool typed = layout == LAYOUT_TYPED || layout == LAYOUT_TYPED_CDEV;
+    std::string part[11];
+    for (int k = 0; k < 11; k++) part[k] = kx_cdi_part(format, layout, k, kind);
     if (len == part[8].size() && memcmp(doc, part[8].data(), len) == 0) {  // the zero-device document
         *n = 0;
         return KXPU_OK;
     }
     // the shortest fragment: the literals, one-digit index (twice) and group (twice; cdev: the group and N), a one-byte
-    // bdf, the uuid, and in JSON the separator after the device
+    // bdf, the uuid, a one-digit type ID and a one-byte key, and in JSON the separator after the device
     size_t lits = 0;
-    for (int k : {0, 1, 2, 3, 4, 5, 9}) lits += part[k].size();
-    const size_t frag_min = lits + 5 + (mdev ? 36 : 0) + (format == KXPU_FMT_JSON ? 1 : 0);
+    for (int k : {0, 1, 2, 3, 4, 5, 9, 10}) lits += part[k].size();
+    const size_t frag_min = lits + 5 + (mdev ? 36 : 0) + (typed ? 2 : 0) + (format == KXPU_FMT_JSON ? 1 : 0);
     const size_t fixed = part[6].size() + part[7].size();
     if (len < fixed + frag_min) { KX_SET_ERR(ctx, "%s: not a document the emitter writes", what); return KXPU_E_INVALID; }
     const size_t max_n = (len - fixed) / frag_min;  // no valid document of len bytes holds more devices
     const size_t rec_bytes = layout == LAYOUT_MDEV ? sizeof(kxpu_mdevcdi)
-                             : layout == LAYOUT_MDEV_CDEV ? sizeof(kxpu_mdevcdev) : sizeof(kxpu_cdidev);
+                             : layout == LAYOUT_MDEV_CDEV ? sizeof(kxpu_mdevcdev)
+                             : typed ? sizeof(kxpu_vfvgpucdi) : sizeof(kxpu_cdidev);
     const uint32_t tiles = (uint32_t)((len + PT - 1) / PT);
     const size_t padded = (size_t)tiles * PT + HALO_MAX + LEAD;
 
@@ -233,6 +269,7 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
     P.l3 = (uint32_t)part[3].size();
     P.lm = (uint32_t)part[4].size();
     P.l9 = (uint32_t)part[9].size();
+    P.l10 = (uint32_t)part[10].size();
 
     KxScratch sc(ctx);
     uint8_t *d_doc = nullptr;
@@ -254,7 +291,13 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
     P.epoch = kx_next_epoch(ctx);
 
     KxTimer tm(ctx, KXPU_T_EMIT);  // decode, the re-emit and the compare, with the one host read of the count between
-    if (layout == LAYOUT_MDEV_CDEV) {
+    if (layout == LAYOUT_TYPED) {
+        if (format == KXPU_FMT_YAML) decode_launch<KXPU_FMT_YAML, LAYOUT_TYPED>(ctx, tiles, P);
+        else decode_launch<KXPU_FMT_JSON, LAYOUT_TYPED>(ctx, tiles, P);
+    } else if (layout == LAYOUT_TYPED_CDEV) {
+        if (format == KXPU_FMT_YAML) decode_launch<KXPU_FMT_YAML, LAYOUT_TYPED_CDEV>(ctx, tiles, P);
+        else decode_launch<KXPU_FMT_JSON, LAYOUT_TYPED_CDEV>(ctx, tiles, P);
+    } else if (layout == LAYOUT_MDEV_CDEV) {
         if (format == KXPU_FMT_YAML) decode_launch<KXPU_FMT_YAML, LAYOUT_MDEV_CDEV>(ctx, tiles, P);
         else decode_launch<KXPU_FMT_JSON, LAYOUT_MDEV_CDEV>(ctx, tiles, P);
     } else if (mdev) {
@@ -286,7 +329,7 @@ static int32_t cdi_parse(kxpu_ctx *ctx, int32_t format, const char *kind, const 
     cudaMemcpyAsync(h + 2, d_ctl + 1, 8, cudaMemcpyDeviceToHost, ctx->stream);
     e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) { KX_SET_ERR(ctx, "%s verify failed: %s", what, cudaGetErrorString(e)); return KXPU_E_CUDA; }
-    if (h[1] || h[2]) {  // a bdf / uuid the emitter refuses, or bytes it would not write
+    if (h[1] || h[2]) {  // a bdf / uuid / type the emitter refuses, or bytes it would not write
         KX_SET_ERR(ctx, "%s: not a document the emitter writes", what);
         return KXPU_E_INVALID;
     }
@@ -316,4 +359,14 @@ extern "C" int32_t kxpu_cdi_parse_cdev(kxpu_ctx *ctx, int32_t format, const char
 extern "C" int32_t kxpu_cdi_parse_mdev_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc,
                                             size_t len, kxpu_mdevcdev *out, size_t cap, size_t *n) {
     return cdi_parse(ctx, format, kind, doc, len, out, cap, n, LAYOUT_MDEV_CDEV, "cdi_parse_mdev_cdev");
+}
+
+extern "C" int32_t kxpu_cdi_parse_vf_vgpu(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc, size_t len,
+                                          kxpu_vfvgpucdi *out, size_t cap, size_t *n) {
+    return cdi_parse(ctx, format, kind, doc, len, out, cap, n, LAYOUT_TYPED, "cdi_parse_vf_vgpu");
+}
+
+extern "C" int32_t kxpu_cdi_parse_vf_vgpu_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const uint8_t *doc,
+                                               size_t len, kxpu_vfvgpucdi *out, size_t cap, size_t *n) {
+    return cdi_parse(ctx, format, kind, doc, len, out, cap, n, LAYOUT_TYPED_CDEV, "cdi_parse_vf_vgpu_cdev");
 }

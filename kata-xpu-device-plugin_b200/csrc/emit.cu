@@ -43,13 +43,30 @@ constexpr int MAX_FRAG_CDEV_LONG = MAX_FRAG_LONG + CDEV_EXTRA;
 // kxpu_cdi_emit_mdev_cdev: the same for the mdev bound; 71.3 KB per CTA, still three CTAs per SM
 constexpr int MAX_FRAG_MDEV_CDEV = MAX_FRAG_MDEV + CDEV_EXTRA;
 constexpr int LAYOUT_PCI = KX_CDI_PCI, LAYOUT_MDEV = KX_CDI_MDEV, LAYOUT_CDEV = KX_CDI_CDEV,
-              LAYOUT_MDEV_CDEV = KX_CDI_MDEV_CDEV;
+              LAYOUT_MDEV_CDEV = KX_CDI_MDEV_CDEV, LAYOUT_TYPED = KX_CDI_TYPED, LAYOUT_TYPED_CDEV = KX_CDI_TYPED_CDEV;
+// kxpu_cdi_emit_vf_vgpu[_cdev]: two more annotations, vgpu-type: "<id>" and vgpu-type-key: "<key>".  The fragment grows
+// by the JSON literals (the YAML ones are shorter), a 10-digit ID and a 40-byte key, for every kind, so the kind split
+// stays at 22 bytes
+#define KX_YV4 "\n      vgpu-type: \""
+#define KX_YV9 "\"\n      vgpu-type-key: \""
+#define KX_JV4 "\",\n        \"vgpu-type\": \""
+#define KX_JV9 "\",\n        \"vgpu-type-key\": \""
+constexpr int TYPED_EXTRA = (int)sizeof(KX_JV4 KX_JV9) - 1 + 10 + 40;  // 104
+static_assert(sizeof(KX_YV4 KX_YV9 "\"") <= sizeof(KX_JV4 KX_JV9), "the YAML annotations must not outgrow the JSON ones");
+constexpr int MAX_FRAG_TYPED = MAX_FRAG + TYPED_EXTRA, MAX_FRAG_TYPED_LONG = MAX_FRAG_LONG + TYPED_EXTRA;
+constexpr int MAX_FRAG_TYPED_CDEV = MAX_FRAG_CDEV + TYPED_EXTRA, MAX_FRAG_TYPED_CDEV_LONG = MAX_FRAG_CDEV_LONG + TYPED_EXTRA;
 static_assert(MAX_FRAG_MDEV <= KX_CDI_FRAG_MAX && MAX_FRAG_CDEV_LONG <= KX_CDI_FRAG_MAX, "the parse halo must follow");
 static_assert(MAX_FRAG_MDEV_CDEV <= KX_CDI_FRAG_MAX_MDEV_CDEV, "the mdev cdev parse halo must follow");
+static_assert(MAX_FRAG_TYPED_LONG <= KX_CDI_FRAG_MAX_TYPED && MAX_FRAG_TYPED_CDEV_LONG <= KX_CDI_FRAG_MAX_TYPED,
+              "the typed parse halo must follow");
 // the records of the two mdev layouts: kxpu_mdevcdev starts with the kxpu_mdevcdi the group layout reads
 template <int LAYOUT> constexpr bool is_mdev_layout = LAYOUT == LAYOUT_MDEV || LAYOUT == LAYOUT_MDEV_CDEV;
-template <int LAYOUT> constexpr bool is_cdev_layout = LAYOUT == LAYOUT_CDEV || LAYOUT == LAYOUT_MDEV_CDEV;
+template <int LAYOUT> constexpr bool is_typed_layout = LAYOUT == LAYOUT_TYPED || LAYOUT == LAYOUT_TYPED_CDEV;
+template <int LAYOUT>
+constexpr bool is_cdev_layout = LAYOUT == LAYOUT_CDEV || LAYOUT == LAYOUT_MDEV_CDEV || LAYOUT == LAYOUT_TYPED_CDEV;
 template <int LAYOUT> using MdevRec = std::conditional_t<LAYOUT == LAYOUT_MDEV_CDEV, kxpu_mdevcdev, kxpu_mdevcdi>;
+// the records of the PCI layouts: kxpu_vfvgpucdi starts with the kxpu_cdidev the untyped layouts read
+template <int LAYOUT> using PciRec = std::conditional_t<is_typed_layout<LAYOUT>, kxpu_vfvgpucdi, kxpu_cdidev>;
 constexpr int POOL_MAX = 640;
 constexpr int KIND_MAX = 63;
 
@@ -87,8 +104,8 @@ constexpr int KIND_MAX = 63;
 #define KX_JM "\",\n        \"mdev\": \""
 // part k = before[k] (+ kind + after[k] when after[k] != NULL); parts 0-5 are the literals, 6 the document head,
 // 7 the tail, 8 the whole document for zero devices (Devices stays nil, cdi/spec.go:42-49), 9 the literal after the
-// mdev uuid (NULL: none)
-struct Parts { const char *before[10], *after[10]; };
+// mdev uuid or the type ID, 10 the literal after the type key (NULL: none)
+struct Parts { const char *before[11], *after[11]; };
 static const Parts h_yaml_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_Y4, KX_Y5, KX_YHA, KX_YT, KX_YHA, nullptr},
                                    {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB, nullptr}};
 static const Parts h_json_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_J4, KX_J5, KX_JHA, KX_JT, KX_JHA, nullptr},
@@ -105,6 +122,18 @@ static const Parts h_yaml_mdev_cdev_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_YM
                                              {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB, nullptr}};
 static const Parts h_json_mdev_cdev_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_JM, KX_J5, KX_JHA, KX_JT, KX_JHA, KX_J4 KX_CDEV_NODE},
                                              {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB, nullptr}};
+// the typed layouts: literal 4 opens vgpu-type, 9 sits between the ID and the key, 10 closes the key and is the PCI
+// literal 4 (typed cdev: with the node literal)
+static const Parts h_yaml_typed_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_YV4, KX_Y5, KX_YHA, KX_YT, KX_YHA, KX_YV9, "\"" KX_Y4},
+                                         {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB, nullptr, nullptr}};
+static const Parts h_json_typed_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_JV4, KX_J5, KX_JHA, KX_JT, KX_JHA, KX_JV9, KX_J4},
+                                         {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB, nullptr, nullptr}};
+static const Parts h_yaml_typed_cdev_parts = {{KX_Y0, KX_Y1, KX_Y2, KX_Y3A, KX_YV4, KX_Y5, KX_YHA, KX_YT, KX_YHA, KX_YV9,
+                                               "\"" KX_Y4 KX_CDEV_NODE},
+                                              {nullptr, nullptr, nullptr, KX_Y3B, nullptr, nullptr, KX_YHB, nullptr, KX_YEB, nullptr, nullptr}};
+static const Parts h_json_typed_cdev_parts = {{KX_J0, KX_J1, KX_J2, KX_J3A, KX_JV4, KX_J5, KX_JHA, KX_JT, KX_JHA, KX_JV9,
+                                               KX_J4 KX_CDEV_NODE},
+                                              {nullptr, nullptr, nullptr, KX_J3B, nullptr, nullptr, KX_JHB, nullptr, KX_JEB, nullptr, nullptr}};
 static const char *kDefaultKind = "nvidia.com/gpu";  // CdiVendorClass, generic_device_plugin.go:31
 
 // The supported kind domain (include/kxpu.h): "vendor/class", <= 63 bytes; vendor = letter [A-Za-z0-9_.-]*
@@ -212,6 +241,7 @@ struct EmitParams {
     unsigned long long *total_out;
     uint32_t *flags;          // [0]: a bdf outside [0-9a-f:.], [1]: a uuid outside the canonical form
     uint8_t pool[POOL_MAX];   // literals | head | tail, built on the host for the call's kind
+    uint16_t off10, len10;    // the typed layouts: the literal after the type key inside the pool
 };
 
 template <int MAXF>
@@ -225,15 +255,37 @@ struct TileSmem {
     uint32_t wsum[EMIT_THREADS / 32];
     uint32_t tile_total;
 };
+// the typed layouts: the type ID's digits and the key's length, appended so that the untyped tiles keep their layout
+template <int MAXF>
+struct TileSmemTyped : TileSmem<MAXF> {
+    uint8_t tdec[TILE][12];  // type ID digits at 0, their count at 10, the key length at 11
+};
+template <int MAXF, int LAYOUT> using EmitSmem = std::conditional_t<is_typed_layout<LAYOUT>, TileSmemTyped<MAXF>, TileSmem<MAXF>>;
 // four CTAs per SM (228 KB of shared memory, 1 KB of it reserved per CTA) for the short-kind tiles of both node layouts
 static_assert(4 * (sizeof(TileSmem<MAX_FRAG_CDEV>) + 1024) <= 228 * 1024, "the cdev short-kind tile lost an SM slot");
 // three CTAs per SM for the tiles of both mdev layouts
 static_assert(3 * (sizeof(TileSmem<MAX_FRAG_MDEV_CDEV>) + 1024) <= 228 * 1024, "the mdev cdev tile lost an SM slot");
+// the typed layouts: three CTAs per SM for kinds up to 22 bytes, two for longer ones
+static_assert(3 * (sizeof(TileSmemTyped<MAX_FRAG_TYPED_CDEV>) + 1024) <= 228 * 1024, "the typed short-kind tile lost an SM slot");
+static_assert(2 * (sizeof(TileSmemTyped<MAX_FRAG_TYPED_CDEV_LONG>) + 1024) <= 228 * 1024, "the typed long-kind tile lost an SM slot");
+
+// a type key byte: [A-Za-z0-9_.-]; the first kl of the 40 key bytes in k must all be one
+__device__ __forceinline__ bool type_key_ok(const uint32_t (&k)[10], uint32_t kl) {
+    bool good = true;
+#pragma unroll
+    for (int b = 0; b < 40; b++) {
+        const uint32_t c = (k[b >> 2] >> (8 * (b & 3))) & 0xffu;
+        const bool ok = (c >= '0' && c <= '9') || (c >= 'a' && c <= 'z') || (c >= 'A' && c <= 'Z') || c == '_' || c == '.' ||
+                        c == '-';
+        if ((uint32_t)b < kl && !ok) good = false;
+    }
+    return good;
+}
 
 template <int FMT, int MAXF, int LAYOUT>
 __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constant__ EmitParams E) {
     extern __shared__ __align__(16) uint8_t smem_raw[];
-    TileSmem<MAXF> &S = *reinterpret_cast<TileSmem<MAXF> *>(smem_raw);
+    EmitSmem<MAXF, LAYOUT> &S = *reinterpret_cast<EmitSmem<MAXF, LAYOUT> *>(smem_raw);
     const uint32_t tid = threadIdx.x, lane = tid & 31u, w = tid >> 5;
     const uint32_t tile = blockIdx.x, i0 = tile * TILE;
     const bool first_tile = tile == 0, last_tile = tile == gridDim.x - 1;
@@ -245,13 +297,26 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
         uint4 bq;  // the bdf / parent address
         uint32_t group, node = 0;
         unsigned long long index;
+        uint32_t typed_len = 0;  // the typed layouts: the type ID's digits and the key
         if (!is_mdev_layout<LAYOUT>) {  // bdf[16] | iommu_group | vfio_cdev | index
-            const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const kxpu_cdidev *>(E.devs) + i0 + tid);
+            const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const PciRec<LAYOUT> *>(E.devs) + i0 + tid);
             const uint4 q0 = p[0], q1 = p[1];
             bq = q0;
             group = q1.x;
-            if constexpr (LAYOUT == LAYOUT_CDEV) node = q1.y;
+            if constexpr (LAYOUT == LAYOUT_CDEV || LAYOUT == LAYOUT_TYPED_CDEV) node = q1.y;
             index = ((unsigned long long)q1.w << 32) | q1.z;
+            if constexpr (is_typed_layout<LAYOUT>) {  // then type_id | key_len | reserved[3] | key[40]
+                const uint4 q2 = p[2], q3 = p[3], q4 = p[4];
+                const uint32_t key[10] = {q2.z, q2.w, q3.x, q3.y, q3.z, q3.w, q4.x, q4.y, q4.z, q4.w};
+                const uint32_t type_id = q2.x, kl_raw = q2.y & 0xffu;
+                const uint32_t kl = kl_raw <= 40u ? kl_raw : 40u;  // out of the domain: reported, and bounded here
+                if (type_id == 0u || kl_raw == 0u || kl_raw > 40u || !type_key_ok(key, kl)) E.flags[1] = 1u;
+                const uint32_t tl = dec_len(type_id);
+                dec_write(type_id, tl, S.tdec[tid]);
+                S.tdec[tid][10] = (uint8_t)tl;
+                S.tdec[tid][11] = (uint8_t)kl;
+                typed_len = tl + kl;
+            }
         } else {  // uuid[36] | iommu_group | parent[16] | index (mdev cdev: the first 64 of 80 bytes; N is read below)
             const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const MdevRec<LAYOUT> *>(E.devs) + i0 + tid);
             const uint4 q0 = p[0], q1 = p[1], q2 = p[2], q3 = p[3];
@@ -277,6 +342,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
             S.grp[tid][11] = (uint8_t)nl;
             flen = flen - gl + nl;
         }
+        if constexpr (is_typed_layout<LAYOUT>) flen += typed_len;
         if (FMT == KXPU_FMT_JSON) flen += (i0 + tid + 1u < E.n) ? 2u : 1u;  // ",\n" between devices, "\n" after the last
     }
     // ---- scan of the 128 lengths (threads >= TILE contribute 0)
@@ -314,6 +380,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
         const uint32_t dj = w + lane * (EMIT_THREADS / 32);
         if (dj < (uint32_t)TILE && i0 + dj < E.n) {
             if constexpr (LAYOUT == LAYOUT_CDEV) cdev_n = static_cast<const kxpu_cdidev *>(E.devs)[i0 + dj].vfio_cdev;
+            else if constexpr (LAYOUT == LAYOUT_TYPED_CDEV) cdev_n = static_cast<const kxpu_vfvgpucdi *>(E.devs)[i0 + dj].dev.vfio_cdev;
             else cdev_n = static_cast<const kxpu_mdevcdev *>(E.devs)[i0 + dj].vfio_cdev;
         }
     }
@@ -338,6 +405,17 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
         };
         lit(0); var(S.idx[d], il); lit(1); quote(); var(S.bdf[d], bl); quote(); lit(2); var(S.grp[d], gl);
         lit(3); var(S.idx[d], il); lit(4);
+        if constexpr (is_typed_layout<LAYOUT>) {  // the type ID, literal 9, the key straight from the device array (L2),
+                                                  // literal 10 (the node literal)
+            var(S.tdec[d], S.tdec[d][10]);
+            lit(8);
+            const uint32_t kl = S.tdec[d][11];
+            const uint8_t *k = reinterpret_cast<const uint8_t *>(static_cast<const kxpu_vfvgpucdi *>(E.devs)[i0 + d].key);
+            for (uint32_t l = lane; l < kl; l += 32u) dst[o + l] = k[l];
+            o += kl;
+            for (uint32_t l = lane; l < E.len10; l += 32u) dst[o + l] = S.pool[E.off10 + l];
+            o += E.len10;
+        }
         if (is_mdev_layout<LAYOUT>) {  // the uuid straight from the device array (L2), then the PCI literal 4 (mdev cdev:
                                        // with the node literal)
             const uint8_t *u = static_cast<const uint8_t *>(E.devs) + (size_t)(i0 + d) * sizeof(MdevRec<LAYOUT>);
@@ -907,7 +985,7 @@ using namespace kxemit;
 
 template <int FMT, int MAXF, int LAYOUT>
 static void emit_launch(kxpu_ctx *ctx, uint32_t tiles, const EmitParams &E) {
-    k_cdi_fused<FMT, MAXF, LAYOUT><<<tiles, EMIT_THREADS, sizeof(TileSmem<MAXF>), ctx->stream>>>(E);
+    k_cdi_fused<FMT, MAXF, LAYOUT><<<tiles, EMIT_THREADS, sizeof(EmitSmem<MAXF, LAYOUT>), ctx->stream>>>(E);
 }
 
 static const Parts &parts_of(int32_t format, int layout) {
@@ -915,6 +993,8 @@ static const Parts &parts_of(int32_t format, int layout) {
     if (layout == LAYOUT_MDEV) return yaml ? h_yaml_mdev_parts : h_json_mdev_parts;
     if (layout == LAYOUT_CDEV) return yaml ? h_yaml_cdev_parts : h_json_cdev_parts;
     if (layout == LAYOUT_MDEV_CDEV) return yaml ? h_yaml_mdev_cdev_parts : h_json_mdev_cdev_parts;
+    if (layout == LAYOUT_TYPED) return yaml ? h_yaml_typed_parts : h_json_typed_parts;
+    if (layout == LAYOUT_TYPED_CDEV) return yaml ? h_yaml_typed_cdev_parts : h_json_typed_cdev_parts;
     return yaml ? h_yaml_parts : h_json_parts;
 }
 
@@ -925,9 +1005,9 @@ std::string kx_cdi_part(int32_t format, int layout, int k, const char *kind) { r
 template <int MAXF, int LAYOUT>
 static void emit_smem_attr() {
     cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_YAML, MAXF, LAYOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)sizeof(TileSmem<MAXF>));
+                         (int)sizeof(EmitSmem<MAXF, LAYOUT>));
     cudaFuncSetAttribute(k_cdi_fused<KXPU_FMT_JSON, MAXF, LAYOUT>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                         (int)sizeof(TileSmem<MAXF>));
+                         (int)sizeof(EmitSmem<MAXF, LAYOUT>));
 }
 
 int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, const void *d_devs, size_t n, int layout,
@@ -944,6 +1024,15 @@ int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, con
     if (layout == LAYOUT_MDEV_CDEV && !mdev_cdev_attr_done) {
         emit_smem_attr<MAX_FRAG_MDEV_CDEV, LAYOUT_MDEV_CDEV>();
         mdev_cdev_attr_done = true;
+    }
+    const bool typed = layout == LAYOUT_TYPED || layout == LAYOUT_TYPED_CDEV;
+    static bool typed_attr_done = false;
+    if (typed && !typed_attr_done) {
+        emit_smem_attr<MAX_FRAG_TYPED, LAYOUT_TYPED>();
+        emit_smem_attr<MAX_FRAG_TYPED_LONG, LAYOUT_TYPED>();
+        emit_smem_attr<MAX_FRAG_TYPED_CDEV, LAYOUT_TYPED_CDEV>();
+        emit_smem_attr<MAX_FRAG_TYPED_CDEV_LONG, LAYOUT_TYPED_CDEV>();
+        typed_attr_done = true;
     }
     static bool attr_done = false;
     if (!attr_done) {
@@ -973,17 +1062,32 @@ int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, con
         acc += E.len[k];
         if (k < 6 || k == 8) E.lit_total += E.len[k];
     }
+    if (typed) {  // part 10, the literal after the type key
+        const std::string s = part_text(parts, 10, kind);
+        if (acc + s.size() > (size_t)POOL_MAX) return KXPU_E_INVALID;
+        memcpy(E.pool + acc, s.data(), s.size());
+        E.off10 = (uint16_t)acc;
+        E.len10 = (uint16_t)s.size();
+        acc += E.len10;
+        E.lit_total += E.len10;
+    }
     E.pool_len = acc;
     const uint32_t N = (uint32_t)n;
     const uint32_t tiles = (N + TILE - 1) / TILE;
-    const uint32_t frag = E.lit_total + 2 * 20 + 2 * 10 + 15 + 2 + 2 + (mdev ? 36 : 0);  // no fragment is longer
+    const uint32_t frag = E.lit_total + 2 * 20 + 2 * 10 + 15 + 2 + 2 + (mdev ? 36 : 0) + (typed ? 10 + 40 : 0);  // no fragment is longer
     const size_t bound = (size_t)n * frag + E.len[6] + E.len[7] + 64;
     // kinds up to 22 bytes fit the four-CTAs-per-SM tile, longer ones take the MAX_FRAG_LONG instantiation (cdev: both
-    // bounds CDEV_EXTRA larger, so the same kinds); every mdev kind the MAX_FRAG_MDEV one (mdev cdev: MAX_FRAG_MDEV_CDEV)
+    // bounds CDEV_EXTRA larger, so the same kinds); every mdev kind the MAX_FRAG_MDEV one (mdev cdev: MAX_FRAG_MDEV_CDEV).
+    // The typed layouts split the kinds the same way, with bounds TYPED_EXTRA larger.
     const bool cdev = layout == LAYOUT_CDEV;
-    const bool long_frag = frag > (uint32_t)(cdev ? MAX_FRAG_CDEV : MAX_FRAG);
-    const int max_frag = layout == LAYOUT_MDEV_CDEV ? MAX_FRAG_MDEV_CDEV : mdev ? MAX_FRAG_MDEV
-                         : cdev ? MAX_FRAG_CDEV_LONG : MAX_FRAG_LONG;
+    const bool long_frag = layout == LAYOUT_TYPED        ? frag > (uint32_t)MAX_FRAG_TYPED
+                           : layout == LAYOUT_TYPED_CDEV ? frag > (uint32_t)MAX_FRAG_TYPED_CDEV
+                                                         : frag > (uint32_t)(cdev ? MAX_FRAG_CDEV : MAX_FRAG);
+    const int max_frag = layout == LAYOUT_TYPED        ? MAX_FRAG_TYPED_LONG
+                         : layout == LAYOUT_TYPED_CDEV ? MAX_FRAG_TYPED_CDEV_LONG
+                         : layout == LAYOUT_MDEV_CDEV  ? MAX_FRAG_MDEV_CDEV
+                         : mdev                        ? MAX_FRAG_MDEV
+                         : cdev                        ? MAX_FRAG_CDEV_LONG : MAX_FRAG_LONG;
     if (frag > (uint32_t)max_frag) return KXPU_E_INVALID;  // the literals grew: the bound must follow
     uint8_t *d_out = nullptr;
     unsigned long long *d_total = nullptr;
@@ -995,7 +1099,23 @@ int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, con
     if (!E.state) return KXPU_E_NOMEM;
     E.epoch = kx_next_epoch(ctx);
     auto launch = [&]() {
-        if (layout == LAYOUT_MDEV_CDEV) {
+        if (layout == LAYOUT_TYPED) {
+            if (format == KXPU_FMT_YAML) {
+                if (long_frag) emit_launch<KXPU_FMT_YAML, MAX_FRAG_TYPED_LONG, LAYOUT_TYPED>(ctx, tiles, E);
+                else emit_launch<KXPU_FMT_YAML, MAX_FRAG_TYPED, LAYOUT_TYPED>(ctx, tiles, E);
+            } else {
+                if (long_frag) emit_launch<KXPU_FMT_JSON, MAX_FRAG_TYPED_LONG, LAYOUT_TYPED>(ctx, tiles, E);
+                else emit_launch<KXPU_FMT_JSON, MAX_FRAG_TYPED, LAYOUT_TYPED>(ctx, tiles, E);
+            }
+        } else if (layout == LAYOUT_TYPED_CDEV) {
+            if (format == KXPU_FMT_YAML) {
+                if (long_frag) emit_launch<KXPU_FMT_YAML, MAX_FRAG_TYPED_CDEV_LONG, LAYOUT_TYPED_CDEV>(ctx, tiles, E);
+                else emit_launch<KXPU_FMT_YAML, MAX_FRAG_TYPED_CDEV, LAYOUT_TYPED_CDEV>(ctx, tiles, E);
+            } else {
+                if (long_frag) emit_launch<KXPU_FMT_JSON, MAX_FRAG_TYPED_CDEV_LONG, LAYOUT_TYPED_CDEV>(ctx, tiles, E);
+                else emit_launch<KXPU_FMT_JSON, MAX_FRAG_TYPED_CDEV, LAYOUT_TYPED_CDEV>(ctx, tiles, E);
+            }
+        } else if (layout == LAYOUT_MDEV_CDEV) {
             if (format == KXPU_FMT_YAML) emit_launch<KXPU_FMT_YAML, MAX_FRAG_MDEV_CDEV, LAYOUT_MDEV_CDEV>(ctx, tiles, E);
             else emit_launch<KXPU_FMT_JSON, MAX_FRAG_MDEV_CDEV, LAYOUT_MDEV_CDEV>(ctx, tiles, E);
         } else if (mdev) {
@@ -1029,7 +1149,8 @@ int32_t kx_cdi_emit_enqueue(kxpu_ctx *ctx, int32_t format, const char *kind, con
     return KXPU_OK;
 }
 
-// LAYOUT_MDEV: devs is kxpu_mdevcdi[n], LAYOUT_MDEV_CDEV: kxpu_mdevcdev[n], else kxpu_cdidev[n]
+// LAYOUT_MDEV: devs is kxpu_mdevcdi[n], LAYOUT_MDEV_CDEV: kxpu_mdevcdev[n], the typed layouts kxpu_vfvgpucdi[n], else
+// kxpu_cdidev[n]
 static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const void *devs, size_t n, uint8_t *out,
                         size_t cap, size_t *len, int layout = LAYOUT_PCI) {
     std::lock_guard<std::mutex> guard(ctx->mu);
@@ -1042,8 +1163,10 @@ static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const v
         memcpy(out, doc.data(), *len);
         return KXPU_OK;
     }
+    const bool typed = layout == LAYOUT_TYPED || layout == LAYOUT_TYPED_CDEV;
     const size_t dev_bytes = layout == LAYOUT_MDEV ? sizeof(kxpu_mdevcdi)
-                             : layout == LAYOUT_MDEV_CDEV ? sizeof(kxpu_mdevcdev) : sizeof(kxpu_cdidev);
+                             : layout == LAYOUT_MDEV_CDEV ? sizeof(kxpu_mdevcdev)
+                             : typed ? sizeof(kxpu_vfvgpucdi) : sizeof(kxpu_cdidev);
     KxScratch sc(ctx);
     void *d_devs = nullptr;
     uint8_t *d_out = nullptr;
@@ -1057,6 +1180,10 @@ static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const v
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) { KX_SET_ERR(ctx, "cdi_emit failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
     if ((uint32_t)h[1]) { KX_SET_ERR(ctx, "cdi_emit: bdf outside [0-9a-f:.]"); return KXPU_E_UNSUPPORTED; }
+    if ((uint32_t)(h[1] >> 32) && typed) {
+        KX_SET_ERR(ctx, "cdi_emit_vf_vgpu: a type ID of 0, or a type key that is empty, longer than 40 bytes or outside [A-Za-z0-9_.-]");
+        return KXPU_E_UNSUPPORTED;
+    }
     if ((uint32_t)(h[1] >> 32)) { KX_SET_ERR(ctx, "cdi_emit_mdev: uuid outside the canonical lowercase form"); return KXPU_E_UNSUPPORTED; }
     const size_t total = (size_t)h[0];
     *len = total;
@@ -1107,6 +1234,26 @@ extern "C" int32_t kxpu_cdi_emit_mdev_cdev(kxpu_ctx *ctx, int32_t format, const 
     if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
     if (!kind_ok(kind)) { KX_SET_ERR(ctx, "cdi_emit_mdev_cdev: kind is not a CDI vendor/class of at most 63 bytes"); return KXPU_E_UNSUPPORTED; }
     return cdi_emit(ctx, format, kind, devs, n, out, cap, len, LAYOUT_MDEV_CDEV);
+}
+
+static int32_t cdi_emit_typed(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_vfvgpucdi *devs, size_t n,
+                              uint8_t *out, size_t cap, size_t *len, int layout, const char *what) {
+    static_assert(sizeof(kxpu_vfvgpucdi) == 80 && offsetof(kxpu_vfvgpucdi, type_id) == 32 && offsetof(kxpu_vfvgpucdi, key) == 40,
+                  "kxpu_vfvgpucdi layout");
+    if (!ctx || !len || !kind || (n && !devs) || (format != KXPU_FMT_YAML && format != KXPU_FMT_JSON)) return KXPU_E_INVALID;
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    if (!kind_ok(kind)) { KX_SET_ERR(ctx, "%s: kind is not a CDI vendor/class of at most 63 bytes", what); return KXPU_E_UNSUPPORTED; }
+    return cdi_emit(ctx, format, kind, devs, n, out, cap, len, layout);
+}
+
+extern "C" int32_t kxpu_cdi_emit_vf_vgpu(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_vfvgpucdi *devs,
+                                         size_t n, uint8_t *out, size_t cap, size_t *len) {
+    return cdi_emit_typed(ctx, format, kind, devs, n, out, cap, len, LAYOUT_TYPED, "cdi_emit_vf_vgpu");
+}
+
+extern "C" int32_t kxpu_cdi_emit_vf_vgpu_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_vfvgpucdi *devs,
+                                              size_t n, uint8_t *out, size_t cap, size_t *len) {
+    return cdi_emit_typed(ctx, format, kind, devs, n, out, cap, len, LAYOUT_TYPED_CDEV, "cdi_emit_vf_vgpu_cdev");
 }
 
 // shared driver of the "thread per item" emitters.  h_in3 (optional, in3_bytes): one more input, uploaded like the

@@ -794,6 +794,29 @@ static Error checkPassthroughClasses(const std::vector<XpuClass> &classes) {
     return Error();
 }
 
+// the parse calls of the PCI resume into the record type of the passthrough spec paths (cdiRecord): the untyped layouts
+// give type_id 0
+template <int32_t (*parse)(kxpu_ctx *, int32_t, const char *, const uint8_t *, size_t, kxpu_cdidev *, size_t, size_t *)>
+static int32_t parseUntyped(kxpu_ctx *ctx, int32_t fmt, const char *kind, const uint8_t *doc, size_t len, kxpu_vfvgpucdi *out,
+                            size_t cap, size_t *n) {
+    std::vector<kxpu_cdidev> d(cap);
+    const int32_t rc = parse(ctx, fmt, kind, doc, len, d.data(), cap, n);
+    if (rc == KXPU_OK)
+        for (size_t i = 0; i < *n; i++) {
+            memset(&out[i], 0, sizeof out[i]);
+            out[i].dev = d[i];
+        }
+    return rc;
+}
+static int32_t parsePciGroup(kxpu_ctx *ctx, int32_t fmt, const char *kind, const uint8_t *doc, size_t len, kxpu_vfvgpucdi *out,
+                             size_t cap, size_t *n) {
+    return parseUntyped<kxpu_cdi_parse>(ctx, fmt, kind, doc, len, out, cap, n);
+}
+static int32_t parsePciCdev(kxpu_ctx *ctx, int32_t fmt, const char *kind, const uint8_t *doc, size_t len, kxpu_vfvgpucdi *out,
+                            size_t cap, size_t *n) {
+    return parseUntyped<kxpu_cdi_parse_cdev>(ctx, fmt, kind, doc, len, out, cap, n);
+}
+
 // createIommuDeviceMap, device_plugin.go:126-180
 Error Plugin::createIommuDeviceMap() {
     {
@@ -809,11 +832,17 @@ Error Plugin::createIommuDeviceMap() {
     haveSnapshotGen_ = snapshotValidation && pci_.haveGen;
     snapshotGen_ = pci_.gen;
     PciWalk w;
+    std::vector<kxpu_snaprec> prev;
+    uint64_t next = 0;
+    if (resumeIndices) {  // the previous specs before the walk: a typed spec names the vGPU types of the VFs it lists
+        resume_ = ResumeReport();  // the mdev walk resumes from the same report and state file
+        readIndexState();
+        previousEntries<kxpu_vfvgpucdi>(xpuClasses, parsePciGroup, resume_.stateRead ? resume_.statePci : 0, resume_.pci,
+                                        prev, next);
+    }
     Error e = firstWalk(w, pci_);
     if (e || !resumeIndices) return e;
-    resume_ = ResumeReport();  // the mdev walk resumes from the same report and state file
-    readIndexState();
-    return resume(w, pci_, resume_.pci, resume_.stateRead ? resume_.statePci : 0, xpuClasses, kxpu_cdi_parse);
+    return resume(w, pci_, resume_.pci, resume_.stateRead ? resume_.statePci : 0, std::move(prev), next);
 }
 
 template <typename Walk>
@@ -1024,7 +1053,11 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
             devs.push_back(NvidiaGpuDevice{std::string(r.bdf), idx});  // :171-174
             devs.back().xpuClass = recordClass(xpuClasses, r.vendor_txt, r.vendor_len, r.driver, sizeof r.driver);
             if (!w.cdevs.empty()) devs.back().cdev = w.cdevs[c.gmem[k]];
-            if (!w.vtype.empty() && xpuClasses[devs.back().xpuClass].vfVgpu) devs.back().vgpuType = w.vtype[c.gmem[k]];
+            if (!w.vtype.empty() && xpuClasses[devs.back().xpuClass].vfVgpu) {
+                devs.back().vgpuType = w.vtype[c.gmem[k]];
+                const kxpu_vgpukey &key = w.vkeys[c.gmem[k]];
+                devs.back().vgpuKey.assign((const char *)key.key, key.len);
+            }
         }
         GroupState<kxpu_dradev> s;
         s.klass = groupClass[c.gids[g]];
@@ -1235,7 +1268,11 @@ Error Plugin::createMdevMap() {
     MdevWalk w;
     e = firstWalk(w, mdev_);
     if (e || !resumeIndices) return e;
-    return resume(w, mdev_, resume_.mdev, resume_.stateRead ? resume_.stateMdev : 0, vgpuClasses, parseMdevGroup);
+    const uint64_t stateNext = resume_.stateRead ? resume_.stateMdev : 0;
+    std::vector<kxpu_snaprec> prev;
+    uint64_t next = 0;
+    previousEntries<kxpu_mdevcdev>(vgpuClasses, parseMdevGroup, stateNext, resume_.mdev, prev, next);
+    return resume(w, mdev_, resume_.mdev, stateNext, std::move(prev), next);
 }
 
 Error Plugin::classify(MdevWalk &w) {
@@ -1574,14 +1611,18 @@ Error Plugin::writeSpec(const std::string &path, const std::vector<uint8_t> &doc
     return e;
 }
 
-// the CDI record of one device of group `group`
-static kxpu_cdidev cdiRecord(const std::string &group, const NvidiaGpuDevice &dev) {
-    kxpu_cdidev d;
+// the CDI record of one device of group `group`: the passthrough spec paths hold one record type for every layout, the
+// untyped layouts read each record's dev
+static kxpu_vfvgpucdi cdiRecord(const std::string &group, const NvidiaGpuDevice &dev) {
+    kxpu_vfvgpucdi d;
     memset(&d, 0, sizeof d);
-    strncpy(d.bdf, dev.addr.c_str(), sizeof d.bdf - 1);
-    d.iommu_group = (uint32_t)strtoul(group.c_str(), nullptr, 10);
-    d.vfio_cdev = dev.cdev < 0 ? 0u : (uint32_t)dev.cdev;
-    d.index = dev.index;
+    strncpy(d.dev.bdf, dev.addr.c_str(), sizeof d.dev.bdf - 1);
+    d.dev.iommu_group = (uint32_t)strtoul(group.c_str(), nullptr, 10);
+    d.dev.vfio_cdev = dev.cdev < 0 ? 0u : (uint32_t)dev.cdev;
+    d.dev.index = dev.index;
+    d.type_id = dev.vgpuType;
+    d.key_len = (uint8_t)std::min(dev.vgpuKey.size(), sizeof d.key);
+    memcpy(d.key, dev.vgpuKey.data(), d.key_len);
     return d;
 }
 static bool hasCdev(const NvidiaGpuDevice &dev) { return dev.cdev >= 0; }
@@ -1597,8 +1638,15 @@ static kxpu_mdevcdev cdiRecord(const std::string &group, const MdevDevice &m) {
     d.vfio_cdev = m.cdev < 0 ? 0u : (uint32_t)m.cdev;
     return d;
 }
-static const kxpu_cdidev &cdiBase(const kxpu_cdidev &r) { return r; }
+static const kxpu_cdidev &cdiBase(const kxpu_vfvgpucdi &r) { return r.dev; }
 static const kxpu_mdevcdi &cdiBase(const kxpu_mdevcdev &r) { return r.dev; }
+template <int32_t (*emit)(kxpu_ctx *, int32_t, const char *, const kxpu_cdidev *, size_t, uint8_t *, size_t, size_t *)>
+static int32_t emitUntyped(kxpu_ctx *ctx, int32_t fmt, const char *kind, const kxpu_vfvgpucdi *devs, size_t n, uint8_t *out,
+                           size_t cap, size_t *len) {
+    std::vector<kxpu_cdidev> d(n);
+    for (size_t i = 0; i < n; i++) d[i] = devs[i].dev;
+    return emit(ctx, fmt, kind, d.data(), n, out, cap, len);
+}
 static int32_t emitMdevGroup(kxpu_ctx *ctx, int32_t fmt, const char *kind, const kxpu_mdevcdev *devs, size_t n, uint8_t *out,
                              size_t cap, size_t *len) {
     std::vector<kxpu_mdevcdi> d(n);
@@ -1627,8 +1675,11 @@ Error Plugin::generateClassSpecs(const std::vector<XpuClass> &classes, const Ord
         const char *kind = classes[c].cdiKind.c_str();
         size_t len = 0;
         auto *fn = emit;
-        if constexpr (std::is_same<Rec, kxpu_cdidev>::value)
-            if (classes[c].vfioCdev) fn = kxpu_cdi_emit_cdev;
+        if constexpr (std::is_same<Rec, kxpu_vfvgpucdi>::value) {
+            if (classes[c].vfioCdev) fn = emitUntyped<kxpu_cdi_emit_cdev>;
+            // resumeIndices: a vfVgpu class's spec carries each VF's type, which a restart reads back
+            if (classes[c].vfVgpu && resumeIndices) fn = classes[c].vfioCdev ? kxpu_cdi_emit_vf_vgpu_cdev : kxpu_cdi_emit_vf_vgpu;
+        }
         if constexpr (std::is_same<Rec, kxpu_mdevcdev>::value)
             if (classes[c].mdevCdev) fn = kxpu_cdi_emit_mdev_cdev;
         int32_t rc = fn(ctx_, fmt, kind, devs.data(), devs.size(), nullptr, 0, &len);
@@ -1664,7 +1715,7 @@ Error Plugin::generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m,
     }
     const int32_t fmt = format == "YAML" ? KXPU_FMT_YAML : KXPU_FMT_JSON;  // spec.go:86-89,102-114
     Error e = generateClassSpecs(xpuClasses, withheld.empty() ? m : served, entryClass, fmt, "kxpu_cdi_emit_kind",
-                                 kxpu_cdi_emit_kind, cdiFiles);
+                                 emitUntyped<kxpu_cdi_emit_kind>, cdiFiles);
     if (!cdiFiles.empty()) lastCdiFile = cdiFiles.back();
     return e;
 }
@@ -1912,9 +1963,17 @@ void Plugin::previousEntries(const std::vector<XpuClass> &classes,
                       recs.data(), recs.size(), &n);
         };
         int32_t rc;
-        if constexpr (std::is_same<Rec, kxpu_cdidev>::value) {  // the layout the class uses now, then the other one
-            rc = parseWith(classes[c].vfioCdev ? kxpu_cdi_parse_cdev : kxpu_cdi_parse);
-            if (rc == KXPU_E_INVALID) rc = parseWith(classes[c].vfioCdev ? kxpu_cdi_parse : kxpu_cdi_parse_cdev);
+        bool typed = false;  // each entry's vGPU type was read back
+        if constexpr (std::is_same<Rec, kxpu_vfvgpucdi>::value) {
+            // the layout the class uses now, then the other one; a vfVgpu class tries its typed layouts first
+            rc = KXPU_E_INVALID;
+            if (classes[c].vfVgpu) {
+                rc = parseWith(classes[c].vfioCdev ? kxpu_cdi_parse_vf_vgpu_cdev : kxpu_cdi_parse_vf_vgpu);
+                if (rc == KXPU_E_INVALID) rc = parseWith(classes[c].vfioCdev ? kxpu_cdi_parse_vf_vgpu : kxpu_cdi_parse_vf_vgpu_cdev);
+                typed = rc != KXPU_E_INVALID;
+            }
+            if (rc == KXPU_E_INVALID) rc = parseWith(classes[c].vfioCdev ? parsePciCdev : parsePciGroup);
+            if (rc == KXPU_E_INVALID) rc = parseWith(classes[c].vfioCdev ? parsePciGroup : parsePciCdev);
         } else {
             rc = parseWith(classes[c].mdevCdev ? kxpu_cdi_parse_mdev_cdev : parse);
             if (rc == KXPU_E_INVALID) rc = parseWith(classes[c].mdevCdev ? parse : kxpu_cdi_parse_mdev_cdev);
@@ -1924,6 +1983,18 @@ void Plugin::previousEntries(const std::vector<XpuClass> &classes,
             break;
         }
         rw.filesRead.push_back(path);
+        if constexpr (std::is_same<Rec, kxpu_vfvgpucdi>::value) {
+            if (typed) {  // the names of the types the spec lists, for the walk's type join: the first key of an ID wins
+                rw.typedClasses.insert(c);
+                for (size_t i = 0; i < n; i++) {
+                    const std::string key(recs[i].key, recs[i].key_len);
+                    auto it = learnedVgpuTypes_.emplace(recs[i].type_id, key).first;
+                    if (it->second != key)
+                        fprintf(stderr, "%s: vGPU type %u is named %s here and %s before; keeping %s\n", path.c_str(),
+                                recs[i].type_id, key.c_str(), it->second.c_str(), it->second.c_str());
+                }
+            }
+        }
         for (size_t i = 0; i < n && rw.fallback.empty(); i++) {
             const auto &r = cdiBase(recs[i]);
             kxpu_snaprec s;
@@ -1933,6 +2004,9 @@ void Plugin::previousEntries(const std::vector<XpuClass> &classes,
             s.iommu_group = r.iommu_group;
             s.klass = (uint32_t)c;
             s.index = r.index;
+            // a typed entry carries the tag snapshotOf gives a vGPU VF: a VF whose type changed gets a fresh index
+            if constexpr (std::is_same<Rec, kxpu_vfvgpucdi>::value)
+                if (typed) s.tag = 1ull << 63 | recs[i].type_id;
             const std::string key(s.key, strnlen(s.key, sizeof s.key));
             if (r.index == UINT64_MAX) rw.fallback = path + ": index 18446744073709551615";
             else if (!indices.insert(r.index).second) rw.fallback = path + ": index " + std::to_string(r.index) + " named twice";
@@ -1966,15 +2040,16 @@ Error Plugin::resumeWalk(std::vector<kxpu_snaprec> prev, uint64_t next, uint64_t
     return Error();
 }
 
-template <typename Walk, typename Rec>
-Error Plugin::resume(const Walk &w, WalkBook &book, ResumeWalk &rw, uint64_t stateNext, const std::vector<XpuClass> &classes,
-                     int32_t (*parse)(kxpu_ctx *, int32_t, const char *, const uint8_t *, size_t, Rec *, size_t, size_t *)) {
-    std::vector<kxpu_snaprec> prev;
-    uint64_t next = 0;
-    previousEntries<Rec>(classes, parse, stateNext, rw, prev, next);
+template <typename Walk>
+Error Plugin::resume(const Walk &w, WalkBook &book, ResumeWalk &rw, uint64_t stateNext, std::vector<kxpu_snaprec> prev,
+                     uint64_t next) {
     std::vector<kxpu_snaprec> cur = snapshotOf(w, nullptr);
     std::map<uint32_t, size_t> groupClass = groupClasses(w.out);  // the file generateClassSpecs puts the entry in
-    for (kxpu_snaprec &s : cur) { s.klass = (uint32_t)groupClass[s.iommu_group]; s.tag = 0; }
+    // tag 0, but a vGPU VF of a class whose spec was read typed keeps its type tag, as the entries read from that spec do
+    for (kxpu_snaprec &s : cur) {
+        s.klass = (uint32_t)groupClass[s.iommu_group];
+        if (!(rw.typedClasses.count(s.klass) && (s.tag >> 63))) s.tag = 0;
+    }
     std::vector<uint64_t> index;
     Error e = resumeWalk(std::move(prev), next, stateNext, cur, rw, index, book.next);
     if (e) return e;
@@ -3630,7 +3705,10 @@ int kxh_state(void *h, char *json, size_t cap) {
         for (size_t i = 0; i < c.second->filesRead.size(); i++) { if (i) o += ','; jstr(o, c.second->filesRead[i]); }
         o += "],\"fallback\":";
         jstr(o, c.second->fallback);
-        o += "},";
+        o += ",\"typed\":[";
+        size_t k2 = 0;
+        for (size_t cls : c.second->typedClasses) o += (k2++ ? "," : "") + std::to_string(cls);
+        o += "]},";
     }
     o += "\"stateRead\":" + std::string(r.stateRead ? "true" : "false") + ",\"statePci\":" + std::to_string(r.statePci) +
          ",\"stateMdev\":" + std::to_string(r.stateMdev) + ",\"written\":[";

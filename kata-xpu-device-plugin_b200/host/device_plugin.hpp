@@ -18,6 +18,7 @@
 #include <functional>
 #include <map>
 #include <optional>
+#include <set>
 #include <shared_mutex>
 #include <string>
 #include <utility>
@@ -34,6 +35,7 @@ struct NvidiaGpuDevice {
     size_t xpuClass = 0; // index into Plugin::xpuClasses of the class this function matched
     int64_t cdev = -1;   // N of its VFIO cdev /dev/vfio/devices/vfio<N> (XpuClass::vfioCdev only); -1 = none
     uint32_t vgpuType = 0;  // XpuClass::vfVgpu only: the vGPU type ID the walk read from nvidia/current_vgpu_type
+    std::string vgpuKey{};  // XpuClass::vfVgpu only: that type's key, the name of the plugin that serves the VF
 };
 
 // One mediated device (vGPU) of the mdev walk: the mdevMap counterpart of NvidiaGpuDevice
@@ -198,7 +200,8 @@ struct XpuClass {
     // never offered.  false: nothing under nvidia/ is opened and every output is as without it.
     bool vfVgpu = false;
     // vfVgpu only: type ID -> name, the first name table of kxpu_vf_vgpu_types.  A restart on a GPU whose VFs are all taken
-    // finds no creatable_vgpu_types list to learn names from, so only these names serve it then.
+    // finds no creatable_vgpu_types list to learn names from; with Plugin::resumeIndices the class's spec carries the type
+    // of every VF it names, and the restart learns the names from it, so these are needed only without resumeIndices.
     std::map<uint32_t, std::string> vgpuTypeNames{};
 };
 XpuClass defaultXpuClass();  // {"10de", "vfio-pci", "nvidia.com", "nvidia.com/gpu", "cdi-vfio-xxxx"}
@@ -216,6 +219,7 @@ struct ResumeWalk {
     kxpu_reconcile_counts counts{};      // the previous specs' entries against the first walk, and the next index
     std::vector<std::string> filesRead;  // spec files read and parsed (a missing file is not listed)
     std::string fallback;                // why the walk resumed from nothing known; empty: it resumed from its specs
+    std::set<size_t> typedClasses;       // vfVgpu classes whose spec was read in a typed layout (each VF's vGPU type)
 };
 struct ResumeReport {
     ResumeWalk pci, mdev;
@@ -640,15 +644,16 @@ class Plugin {
     void previousEntries(const std::vector<XpuClass> &classes,
                          int32_t (*parse)(kxpu_ctx *, int32_t, const char *, const uint8_t *, size_t, Rec *, size_t, size_t *),
                          uint64_t stateNext, ResumeWalk &rw, std::vector<kxpu_snaprec> &prev, uint64_t &next);
-    // resumeIndices: reconcile the first walk's entries `cur` (klass = the class of the entry's group, tag 0) against the
-    // previous specs; index gets one index per cur entry, nextOut the walk's next index
+    // resumeIndices: reconcile the first walk's entries `cur` (klass = the class of the entry's group, tag 0 but for the
+    // vGPU VFs of a class whose spec was read typed) against the previous specs; index gets one index per cur entry,
+    // nextOut the walk's next index
     Error resumeWalk(std::vector<kxpu_snaprec> prev, uint64_t next, uint64_t stateNext, const std::vector<kxpu_snaprec> &cur,
                      ResumeWalk &rw, std::vector<uint64_t> &index, uint64_t &nextOut);
-    // resumeIndices: the first walk against the previous specs of classes (parse: their parse call), with stateNext the
-    // state file's value; rebuilds the walk's maps and record with the resumed indices
-    template <typename Walk, typename Rec>
-    Error resume(const Walk &w, WalkBook &book, ResumeWalk &rw, uint64_t stateNext, const std::vector<XpuClass> &classes,
-                 int32_t (*parse)(kxpu_ctx *, int32_t, const char *, const uint8_t *, size_t, Rec *, size_t, size_t *));
+    // resumeIndices: the first walk against the previous specs' entries prev (next: their next index, stateNext the state
+    // file's value); rebuilds the walk's maps and record with the resumed indices
+    template <typename Walk>
+    Error resume(const Walk &w, WalkBook &book, ResumeWalk &rw, uint64_t stateNext, std::vector<kxpu_snaprec> prev,
+                 uint64_t next);
     void readIndexState();  // into resume_
     Error writeIndexState(std::vector<std::string> *written);
     ResumeReport resume_;

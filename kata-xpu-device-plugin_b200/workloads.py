@@ -774,3 +774,19 @@ def vf_vgpu_walk(n=1 << 20, seed=61):
     table = b"ID    : vGPU Name\n" + b"".join(b"%d : %s\n" % (t, nm.encode()) for t, nm in H100_VGPU_TYPES)
     tables = [table] * int(((cur == 0) & ~is_pf & ~bad).sum())
     return recs, vts, tables
+
+
+def vf_vgpu_cdi_devices(n=1 << 20, seed=63):
+    """n served VFs (VFVGPUCDI_DTYPE) for the typed CDI layouts: cfg5_devices' bdfs, groups and indices, cdev numbers of
+    every width, and a type of the H100 table with its type key (keys of 12 to 19 bytes, IDs of four digits)."""
+    from .binding import VFVGPUCDI_DTYPE
+    rng = np.random.default_rng(seed)
+    devs = np.zeros(n, dtype=VFVGPUCDI_DTYPE)
+    devs["dev"] = cfg5_devices(n)
+    devs["dev"]["reserved"] = (np.arange(n, dtype=np.uint64) * 2654435761) % (1 << 32)  # the cdev number
+    pick = rng.integers(0, len(H100_VGPU_TYPES), n)
+    keys = np.array([nm.replace(" ", "_").encode() for _, nm in H100_VGPU_TYPES])
+    devs["type_id"] = np.array([t for t, _ in H100_VGPU_TYPES], np.uint32)[pick]
+    devs["key"] = keys[pick]
+    devs["key_len"] = np.array([len(k) for k in keys], np.uint8)[pick]
+    return devs

@@ -24,6 +24,17 @@ for fmt_ in (0, 1):
     mdoc = kx.cdi_emit_mdev_cdev(fmt_, mcd, "nvidia.com/vgpu")
     assert kx.cdi_parse_mdev_cdev(fmt_, mdoc, "nvidia.com/vgpu").tobytes() == mcd.tobytes()
     print("mdev cdev spec", fmt_, len(mdoc))
+# the typed VF-vGPU layouts: 3000 VFs with their vGPU types, emitted and parsed back in both node layouts
+vcd = W.vf_vgpu_cdi_devices(3000)
+for fmt_ in (0, 1):
+    for cdev in (False, True):
+        vdoc = kx.cdi_emit_vf_vgpu(fmt_, vcd, "nvidia.com/vgpu", cdev=cdev)
+        got = kx.cdi_parse_vf_vgpu(fmt_, vdoc, "nvidia.com/vgpu", cdev=cdev)
+        want = vcd.copy()
+        if not cdev:
+            want["dev"]["reserved"] = 0  # the group layout carries no cdev number
+        assert got.tobytes() == want.tobytes()
+        print("vf vgpu spec", fmt_, cdev, len(vdoc))
 # NUMA topology: classify masks (PCI and mdev), topology wire bytes, both preferred-allocation shapes
 tres = kx.classify_topo([(b"10de", b"vfio-pci")], W.topo_records(keys, n=20000, nodes=4))
 mres = kx.classify_topo(W.MDEV_RULES, W.topo_mdev_records(n=20000), mdev=True)
