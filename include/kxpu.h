@@ -811,6 +811,19 @@ int32_t kxpu_cdi_emit(kxpu_ctx *ctx, int32_t format, const kxpu_cdidev *devs, si
  *     leading digit / sign or a whole-word boolean); no character of it is an indicator that forces
  *     quoting in a plain scalar.  "kind=<index>" stays plain for the same reasons.
  *   - JSON: it holds no '"', '\\', control byte, '<', '>' or '&', so encoding/json escapes nothing.
+ * The bdf domain of every kxpu_cdi_emit* call (kxpu_cdi_emit included; the parent of the vGPU calls alike), in both
+ * formats (else KXPU_E_UNSUPPORTED, nothing written, the sizing call included): the bytes before the first NUL (all 16
+ * when there is none), 1..16 of them over [0-9a-f:.], that yaml.v3 writes either plain or, when isBase60Float matches
+ * them, double-quoted.  Restated from yaml.v3 v3.0.1 (resolve.go, encode.go, emitterc.go) for this alphabet, which
+ * holds no sign, '_', 'x', 'o', letter of a bool / null word or '-' of a timestamp; refused are the bdfs that
+ *   - are all decimal digits (resolve reads an int, or a float for 08 / 09 ...; the encoder would double-quote them);
+ *   - are "0b" and one or more binary digits (an int: double-quoted);
+ *   - match [0-9]+(\.[0-9]*)?(e[0-9]+)? or \.[0-9]+(e[0-9]+)? (a float, e.g. 1.5, .5, 0., 1e3: double-quoted);
+ *   - end in ':' (the emitter's analysis forbids a plain scalar there and yaml.v3 single-quotes it);
+ *   - start with "..." (a document end marker: single-quoted).
+ * The last two would need a quoting style this library neither writes nor parses; refusing all five keeps the YAML
+ * document's bdf a plain string to every YAML loader (a YAML 1.1 one such as PyYAML reads fewer of these as numbers, and
+ * none of the accepted ones), and keeps both formats to one domain.  Every PCI address sysfs names is inside it.
  * Kinds up to 22 bytes run on the same kernel configuration as kxpu_cdi_emit; longer ones on a variant
  * with a larger per-device fragment bound (fewer CTAs per SM, DESIGN.md K6). */
 int32_t kxpu_cdi_emit_kind(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_cdidev *devs, size_t n,
@@ -833,8 +846,8 @@ typedef struct kxpu_mdevcdi {
  *   cdi.k8s.io/vfio<g>: <kind>=<index>
  *   mdev: <uuid>
  * and the device node is /dev/vfio/<g> with g = iommu_group.  A uuid outside the canonical lowercase form
- * (8-4-4-4-12 over [0-9a-f], '-' between) or a parent that is empty or holds a byte outside [0-9a-f:.] is
- * KXPU_E_UNSUPPORTED.
+ * (8-4-4-4-12 over [0-9a-f], '-' between) or a parent outside kxpu_cdi_emit_kind's bdf domain (empty, a byte outside
+ * [0-9a-f:.], or one of the five YAML classes listed there) is KXPU_E_UNSUPPORTED.
  * A canonical UUID is always written as it is:
  *   - YAML: it has exactly four '-' and 32 hex digits.  yaml.v3's resolve reads a plain scalar as int / float
  *     only when it is [-+]?digits (with an optional 0x / 0o / 0b prefix, '_' separators) or a float of the form
@@ -851,7 +864,7 @@ int32_t kxpu_cdi_emit_mdev(kxpu_ctx *ctx, int32_t format, const char *kind, cons
 /* ------------------------------------------------- CDI spec parse (ABI v13) */
 
 /* The shortest device fragment of any document kxpu_cdi_emit_kind / kxpu_cdi_emit_mdev write (YAML, a 3-byte kind,
- * one-digit index and group, a one-byte bdf): a document of len bytes names at most len / KXPU_CDI_FRAG_MIN devices,
+ * one-digit index and group, a one-byte bdf such as "a", which stays plain): a document of len bytes names at most len / KXPU_CDI_FRAG_MIN devices,
  * so cap = len / KXPU_CDI_FRAG_MIN needs no second call. */
 #define KXPU_CDI_FRAG_MIN 166
 
@@ -895,8 +908,8 @@ int32_t kxpu_cdi_parse_mdev(kxpu_ctx *ctx, int32_t format, const char *kind, con
 
 /* kxpu_cdi_emit_kind's document, byte for byte, except that the device node of device i is
  * /dev/vfio/devices/vfio<N> with N = devs[i].vfio_cdev (every uint32 is valid) in place of /dev/vfio/<g>.  The
- * annotations (cdi.k8s.io/vfio<g> included), head, tail, zero-device form, device order, kind domain, sizing protocol and
- * KXPU_E_UNSUPPORTED cases are kxpu_cdi_emit_kind's.
+ * annotations (cdi.k8s.io/vfio<g> included), head, tail, zero-device form, device order, kind and bdf domains, sizing
+ * protocol and KXPU_E_UNSUPPORTED cases are kxpu_cdi_emit_kind's.
  * GPU: the kernel of kxpu_cdi_emit_kind with the node literal and number compiled in; the longest fragment is 12 bytes
  * longer, and kinds up to 22 bytes still run at four CTAs per SM (DESIGN.md K6).  Timed under KXPU_T_EMIT. */
 int32_t kxpu_cdi_emit_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_cdidev *devs, size_t n,
@@ -934,7 +947,7 @@ typedef struct kxpu_mdevcdev {
 /* kxpu_cdi_emit_mdev's document for devs[i].dev, byte for byte, except that the device node of device i is
  * /dev/vfio/devices/vfio<N> with N = devs[i].vfio_cdev in place of /dev/vfio/<g>.  The four annotations (cdi.k8s.io/vfio<g>
  * and mdev: <uuid> included), head, tail, zero-device form, device order, kind domain, uuid and parent refusals
- * (KXPU_E_UNSUPPORTED) and sizing protocol are kxpu_cdi_emit_mdev's.
+ * (KXPU_E_UNSUPPORTED; the parent has kxpu_cdi_emit_kind's bdf domain) and sizing protocol are kxpu_cdi_emit_mdev's.
  * GPU: the kernel of kxpu_cdi_emit_mdev with the node literal and number compiled in; the longest fragment is 12 bytes
  * longer (492), and the tile still runs three CTAs per SM (DESIGN.md K6).  Timed under KXPU_T_EMIT. */
 int32_t kxpu_cdi_emit_mdev_cdev(kxpu_ctx *ctx, int32_t format, const char *kind, const kxpu_mdevcdev *devs, size_t n,
@@ -978,8 +991,8 @@ typedef struct kxpu_vfvgpucdi {
  * such as 1e5, true, No, 0x1F, .inf or 2024-01-01, would resolve as a non-string, and a CDI registry that reads
  * annotations as map[string]string would then refuse the whole spec.  Over the key alphabet [A-Za-z0-9_.-] and the
  * digits a quoted value needs no escape in either format.
- * KXPU_E_UNSUPPORTED, with nothing written: every case kxpu_cdi_emit_kind refuses, type_id 0, key_len 0 or above 40, or
- * a key byte (of the first key_len) outside [A-Za-z0-9_.-].
+ * KXPU_E_UNSUPPORTED, with nothing written: every case kxpu_cdi_emit_kind refuses (its bdf domain included), type_id 0,
+ * key_len 0 or above 40, or a key byte (of the first key_len) outside [A-Za-z0-9_.-].
  * GPU: the kernel of kxpu_cdi_emit_kind with the annotations compiled in; each record is read with five 16-byte loads
  * and a warp copies the key straight from the device array.  The longest fragment grows by 104 bytes, and kinds up to 22
  * bytes run at three CTAs per SM, longer ones at two (DESIGN.md K6).  Timed under KXPU_T_EMIT. */

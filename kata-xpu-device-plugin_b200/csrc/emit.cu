@@ -206,6 +206,34 @@ __device__ __forceinline__ bool bdf_charset_ok(const uint8_t *s, uint32_t len) {
     }
     return true;
 }
+// a bdf over [0-9a-f:.] that yaml.v3 writes as a plain string, or as the double-quoted base-60 form above (include/kxpu.h
+// states the classes and why): not all digits, not 0b + binary digits, not a float of resolve.go's yamlStyleFloat
+// ([0-9]+(\.[0-9]*)?(e[0-9]+)? or \.[0-9]+(e[0-9]+)?), no trailing ':' and no leading "..."
+__device__ __forceinline__ bool bdf_yaml_plain(const uint8_t *s, uint32_t len) {
+    auto dig = [](uint8_t c) { return c >= '0' && c <= '9'; };
+    if (len == 0 || s[len - 1] == ':') return false;
+    if (len >= 3 && s[0] == '.' && s[1] == '.' && s[2] == '.') return false;
+    if (len >= 3 && s[0] == '0' && s[1] == 'b') {
+        uint32_t i = 2;
+        while (i < len && (s[i] == '0' || s[i] == '1')) i++;
+        if (i == len) return false;
+    }
+    uint32_t i = 0, m = 0;  // m: mantissa digits
+    while (i < len && dig(s[i])) { i++; m++; }
+    if (i < len && s[i] == '.') {
+        const bool lead = m == 0;
+        i++;
+        while (i < len && dig(s[i])) { i++; m++; }
+        if (lead && m == 0) return true;  // "." alone or "." followed by no digit
+    }
+    if (m == 0) return true;
+    if (i < len && s[i] == 'e') {
+        const uint32_t e0 = ++i;
+        while (i < len && dig(s[i])) i++;
+        if (i == e0) return true;
+    }
+    return i != len;
+}
 
 // The store epilogue of a staged tile: stg[0, total) sits in shared memory at g's 16-byte phase and goes to g with one
 // bulk store for the 16-byte aligned body and byte stores for the ragged ends.  Called by every thread of a CTA of at
@@ -328,7 +356,7 @@ __global__ void __launch_bounds__(EMIT_THREADS) k_cdi_fused(const __grid_constan
         }
         const uint8_t *bdf = reinterpret_cast<const uint8_t *>(&bq);
         const uint32_t bl = bdf_len16(bdf), il = dec_len(index), gl = dec_len(group);
-        if (!bdf_charset_ok(bdf, bl)) E.flags[0] = 1u;
+        if (!bdf_charset_ok(bdf, bl) || !bdf_yaml_plain(bdf, bl)) E.flags[0] = 1u;
         const bool quoted = FMT == KXPU_FMT_YAML && is_base60(bdf, bl);
         dec_write(index, il, S.idx[tid]);
         dec_write(group, gl, S.grp[tid]);
@@ -1179,7 +1207,10 @@ static int32_t cdi_emit(kxpu_ctx *ctx, int32_t format, const char *kind, const v
     cudaMemcpyAsync(h, d_total, 16, cudaMemcpyDeviceToHost, ctx->stream);
     cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (e != cudaSuccess) { KX_SET_ERR(ctx, "cdi_emit failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
-    if ((uint32_t)h[1]) { KX_SET_ERR(ctx, "cdi_emit: bdf outside [0-9a-f:.]"); return KXPU_E_UNSUPPORTED; }
+    if ((uint32_t)h[1]) {
+        KX_SET_ERR(ctx, "cdi_emit: bdf outside [0-9a-f:.]{1,16}, or one YAML would read as a number or not as a plain string");
+        return KXPU_E_UNSUPPORTED;
+    }
     if ((uint32_t)(h[1] >> 32) && typed) {
         KX_SET_ERR(ctx, "cdi_emit_vf_vgpu: a type ID of 0, or a type key that is empty, longer than 40 bytes or outside [A-Za-z0-9_.-]");
         return KXPU_E_UNSUPPORTED;

@@ -60,6 +60,16 @@ def get_device_name(data: bytes, vendor: bytes, device: bytes):
 
 
 BASE60 = re.compile(r"^[-+]?[0-9][0-9_]*(?::[0-5]?[0-9])+(?:\.[0-9_]*)?$")
+# the bdfs over [0-9a-f:.] that yaml.v3 would not write plain or base-60 double-quoted (include/kxpu.h, the bdf domain of
+# kxpu_cdi_emit_kind): an int (all digits, 0b + binary digits), a float of resolve.go's yamlStyleFloat, a trailing ':',
+# a leading "..."
+_BDF_NOT_PLAIN = re.compile(r"[0-9]+|0b[01]+|[0-9]+(\.[0-9]*)?(e[0-9]+)?|\.[0-9]+(e[0-9]+)?|.*:|\.\.\..*", re.S)
+
+
+def bdf_ok(bdf) -> bool:
+    """The bdf (or mdev parent) domain of every CDI spec emitter: 1..16 bytes over [0-9a-f:.] that YAML keeps a string."""
+    s = bdf.decode("latin-1") if isinstance(bdf, (bytes, bytearray)) else bdf
+    return re.fullmatch(r"[0-9a-f:.]{1,16}", s) is not None and _BDF_NOT_PLAIN.fullmatch(s) is None
 
 
 def yaml_scalar(s: str) -> str:
@@ -71,7 +81,9 @@ def yaml_scalar(s: str) -> str:
 
 
 def cdi_yaml(devs):
-    """devs: list of (bdf, group, index)."""
+    """devs: list of (bdf, group, index); None when a bdf is outside bdf_ok."""
+    if not all(bdf_ok(bdf) for bdf, _, _ in devs):
+        return None
     out = ["cdiVersion: 0.6.0", "kind: nvidia.com/gpu"]
     if not devs:
         out.append("devices: []")
@@ -90,6 +102,8 @@ def cdi_yaml(devs):
 
 
 def cdi_json(devs):
+    if not all(bdf_ok(bdf) for bdf, _, _ in devs):
+        return None
     spec = {"cdiVersion": "0.6.0", "kind": "nvidia.com/gpu"}
     if not devs:
         spec["devices"] = None

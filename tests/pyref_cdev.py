@@ -25,11 +25,14 @@ def _bdf_yaml(bdf):
 
 
 def emit(fmt, kind, recs):
-    """The document of CDIDEV_DTYPE records (N in CDEV_FIELD), or None when the kind is outside the supported domain."""
+    """The document of CDIDEV_DTYPE records (N in CDEV_FIELD), or None when the kind or a bdf is outside the supported
+    domain."""
     kind = kind.decode() if isinstance(kind, bytes) else kind
     if not XO.kind_ok(kind.encode()):
         return None
-    devs = [(r["bdf"].decode(), int(r["iommu_group"]), int(r["index"]), int(r[CDEV_FIELD])) for r in recs]
+    devs = [(r["bdf"].decode("latin-1"), int(r["iommu_group"]), int(r["index"]), int(r[CDEV_FIELD])) for r in recs]
+    if not all(pyref.bdf_ok(d[0]) for d in devs):
+        return None
     if fmt == FMT_YAML:
         out = ["cdiVersion: 0.6.0", "kind: %s" % kind]
         if not devs:
@@ -63,7 +66,6 @@ HEAD = {FMT_YAML: re.compile(rb'(\d{1,20})"\n    annotations:\n      attach-pci:
                              rb'([^"]{0,16})",\n        "cdi\.k8s\.io/vfio(\d{1,10})": "[^=\n]*=\d{1,20}"\n      \},\n'
                              rb'      "containerEdits": \{\n        "deviceNodes": \[\n          \{\n'
                              rb'            "path": "/dev/vfio/devices/vfio(\d{1,10})"')}
-BDF = re.compile(rb"[0-9a-f:.]{1,16}")
 
 
 def parse(fmt, doc, kind):
@@ -78,7 +80,7 @@ def parse(fmt, doc, kind):
     recs = np.zeros(len(starts), XO.CDIDEV_DTYPE)
     for i, p in enumerate(starts):
         m = HEAD[fmt].match(doc, p)
-        if not m or not BDF.fullmatch(m.group(3)):  # kxpu_cdi_emit_cdev refuses such a bdf
+        if not m or not pyref.bdf_ok(m.group(3)):  # kxpu_cdi_emit_cdev refuses such a bdf
             return E_INVALID, None
         index, group, node = int(m.group(1)), int(m.group(4)), int(m.group(5))
         if index >= 1 << 64 or group >= 1 << 32 or node >= 1 << 32:

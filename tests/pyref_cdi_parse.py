@@ -5,6 +5,8 @@ import re
 
 import numpy as np
 
+import pyref
+
 from oracle import mdev_oracle as MO
 from oracle import xpu_oracle as XO
 
@@ -16,7 +18,6 @@ HEAD = {FMT_YAML: re.compile(rb'(\d{1,20})"\n    annotations:\n      attach-pci:
                              rb'      cdi\.k8s\.io/vfio(\d{1,10}): '),
         FMT_JSON: re.compile(rb'(\d{1,20})",\n      "annotations": \{\n        "attach-pci": "true",\n        "bdf": "()'
                              rb'([^"]{0,16})",\n        "cdi\.k8s\.io/vfio(\d{1,10})": "')}
-BDF = re.compile(rb"[0-9a-f:.]{1,16}")
 UUID = {FMT_YAML: re.compile(rb'[^=\n]*=\d{1,20}\n      mdev: (.{36})', re.S),
         FMT_JSON: re.compile(rb'[^=\n]*=\d{1,20}",\n        "mdev": "(.{36})', re.S)}
 
@@ -43,7 +44,7 @@ def parse(fmt, doc, kind, mdev=False):
         index, group = int(m.group(1)), int(m.group(4))
         if index >= 1 << 64 or group >= 1 << 32:
             return E_INVALID, None
-        if not BDF.fullmatch(m.group(3)):  # kxpu_cdi_emit_kind refuses such a bdf; the PCI oracle does not check it
+        if not pyref.bdf_ok(m.group(3)):  # kxpu_cdi_emit_kind refuses such a bdf; the PCI oracle does not check it
             return E_INVALID, None
         if mdev:
             u = UUID[fmt].match(doc, m.end())

@@ -76,6 +76,8 @@ def _frag_yaml(kind, d):
 
 
 def cdi_yaml(kind: bytes, devs):
+    if not all(pyref.bdf_ok(d["parent"]) for d in devs):
+        return None
     head = b"cdiVersion: 0.6.0\nkind: " + kind + b"\n"
     if not devs:
         return head + b"devices: []\n"
@@ -83,6 +85,8 @@ def cdi_yaml(kind: bytes, devs):
 
 
 def cdi_json(kind: bytes, devs):
+    if not all(pyref.bdf_ok(d["parent"]) for d in devs):
+        return None
     head = b'{\n  "cdiVersion": "0.6.0",\n  "kind": "' + kind + b'",\n'
     if not devs:
         return head + b'  "devices": null,\n  "containerEdits": {}\n}'

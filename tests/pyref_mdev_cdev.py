@@ -7,6 +7,7 @@ import re
 
 import numpy as np
 
+import pyref
 import pyref_mdev as PM
 from oracle import mdev_oracle as MO
 from oracle import xpu_oracle as XO
@@ -15,7 +16,6 @@ OK, E_INVALID, E_UNSUPPORTED = 0, -1, -7
 FMT_YAML, FMT_JSON = 0, 1
 # kxpu_mdevcdev: kxpu_mdevcdi, then N and three reserved words (80 bytes)
 MDEVCDEV_DTYPE = np.dtype([("dev", MO.MDEVCDI_DTYPE), ("vfio_cdev", "<u4"), ("reserved", "<u4", (3,))])
-BDF = re.compile(rb"[0-9a-f:.]{1,16}")
 
 
 def node_path(n):
@@ -37,7 +37,7 @@ def emit(fmt, kind, recs):
     for r in recs:
         d = r["dev"]
         uuid, parent = bytes(d["uuid"]), bytes(d["parent"])
-        if len(uuid) != 36 or not PM.uuid_ok(uuid) or not BDF.fullmatch(parent):
+        if len(uuid) != 36 or not PM.uuid_ok(uuid) or not pyref.bdf_ok(parent):
             return None
         devs.append({"index": int(d["index"]), "parent": parent, "group": int(d["iommu_group"]), "uuid": uuid})
     doc = (PM.cdi_yaml if fmt == FMT_YAML else PM.cdi_json)(kind, devs)
@@ -70,7 +70,7 @@ def parse(fmt, doc, kind):
     recs = np.zeros(len(starts), MDEVCDEV_DTYPE)
     for i, p in enumerate(starts):
         m = HEAD[fmt].match(doc, p)
-        if not m or not BDF.fullmatch(m.group(3)) or not PM.uuid_ok(m.group(5)):  # the emitter refuses these
+        if not m or not pyref.bdf_ok(m.group(3)) or not PM.uuid_ok(m.group(5)):  # the emitter refuses these
             return E_INVALID, None
         index, group, node = int(m.group(1)), int(m.group(4)), int(m.group(6))
         if index >= 1 << 64 or group >= 1 << 32 or node >= 1 << 32:

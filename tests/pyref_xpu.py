@@ -5,11 +5,13 @@ oracle/kxpu_xpu_oracle.c."""
 import json
 import re
 
-from pyref import yaml_scalar
+from pyref import bdf_ok, yaml_scalar
 
 
 def cdi_yaml(devs, kind):
     """pyref.cdi_yaml with the CDI kind (CdiVendorClass in the reference) as a parameter; devs: (bdf, group, index)."""
+    if not all(bdf_ok(bdf) for bdf, _, _ in devs):
+        return None
     out = ["cdiVersion: 0.6.0", "kind: %s" % yaml_scalar(kind)]
     if not devs:
         out.append("devices: []")
@@ -28,6 +30,8 @@ def cdi_yaml(devs, kind):
 
 
 def cdi_json(devs, kind):
+    if not all(bdf_ok(bdf) for bdf, _, _ in devs):
+        return None
     spec = {"cdiVersion": "0.6.0", "kind": kind}
     if not devs:
         spec["devices"] = None

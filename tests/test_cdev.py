@@ -101,6 +101,6 @@ def test_frag_min_bounds_cdev_documents():
     """The shortest cdev fragment is longer than the group layout's, so KXPU_CDI_FRAG_MIN still bounds the count."""
     from kxpu_b200 import binding as B
     recs = np.zeros(64, K.records(0).dtype)
-    recs["bdf"], recs["index"] = b"1", np.arange(64) % 10
+    recs["bdf"], recs["index"] = b"a", np.arange(64) % 10  # a one-byte bdf that YAML keeps plain
     doc = PC.emit(K.FMT_YAML, b"a/b", recs)
     assert len(doc) // B.CDI_FRAG_MIN >= 64

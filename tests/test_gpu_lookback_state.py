@@ -12,6 +12,8 @@ least two; the Call objects below restate the host code's sizes and every test a
 
   scan_kernel    names, alloc_names(_kind), mdev_names, lw_encode(_topo)   4096 items (n + 1 are scanned)  1 epoch
   k_cdi_fused    cdi_emit(_kind, _mdev)                                    128 devices                     1 epoch
+  k_cdi_decode   cdi_parse(_mdev, _cdev, _mdev_cdev, _vf_vgpu[_cdev])      8192 bytes                      1 epoch
+                 (tests/test_gpu_cdi_edges.py interleaves it with the emits of all six layouts under the epoch wrap)
   classify       classify(_rules, _mdev, _topo, _mdev_topo)                2048 / 4096 records   3 + 1 per sort pass,
                                                                                                  twice on the retry
   k_rc_probe     reconcile                                                 1024 entries                    1 epoch

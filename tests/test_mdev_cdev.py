@@ -136,7 +136,7 @@ def test_frag_min_bounds_mdev_cdev_documents():
     """The shortest mdev cdev fragment is longer than the shortest group fragment, so KXPU_CDI_FRAG_MIN bounds the count."""
     from kxpu_b200 import binding as B
     recs = K.records(64)
-    recs["dev"]["parent"], recs["dev"]["index"], recs["dev"]["iommu_group"] = b"1", np.arange(64) % 10, 0
+    recs["dev"]["parent"], recs["dev"]["index"], recs["dev"]["iommu_group"] = b"a", np.arange(64) % 10, 0  # plain in YAML
     recs["vfio_cdev"] = 0
     doc = PMC.emit(K.FMT_YAML, b"a/b", recs)
     assert len(doc) // B.CDI_FRAG_MIN >= 64

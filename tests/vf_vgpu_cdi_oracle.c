@@ -74,6 +74,25 @@ static int base60(const char *s) {
     return s[i] == 0;
 }
 
+/* yaml.v3 would write s as something other than a plain string (or the base-60 double-quoted form above): all digits,
+ * 0b and binary digits, a float [0-9]+(\.[0-9]*)?(e[0-9]+)? or \.[0-9]+(e[0-9]+)?, a trailing ':' or a leading "..." */
+static int yaml_not_plain(const char *s) {
+    const size_t len = strlen(s);
+    if (len && s[len - 1] == ':') return 1;
+    if (strncmp(s, "...", 3) == 0) return 1;
+    if (strncmp(s, "0b", 2) == 0 && len > 2 && strspn(s + 2, "01") == len - 2) return 1;
+    size_t i = strspn(s, "0123456789");
+    const size_t whole = i;
+    if (s[i] == '.') i += 1 + strspn(s + i + 1, "0123456789");
+    if (whole == 0 && i < 2) return 0;  /* neither digits before the point nor after it */
+    if (s[i] == 'e') {
+        const size_t e = strspn(s + i + 1, "0123456789");
+        if (e == 0) return 0;
+        i += 1 + e;
+    }
+    return i == len;
+}
+
 /* 0: the document in *out (malloc'd, *len bytes); -7: a record or the kind outside the domain; -1: out of memory */
 int kxv_cdi_vf_vgpu(int fmt, const char *kind, const kxpu_vfvgpucdi *devs, size_t n, int cdev, uint8_t **out, size_t *len) {
     if (!kind_ok(kind)) return -7;
@@ -85,6 +104,9 @@ int kxv_cdi_vf_vgpu(int fmt, const char *kind, const kxpu_vfvgpucdi *devs, size_
             if (!(digit(d->dev.bdf[k]) || (d->dev.bdf[k] >= 'a' && d->dev.bdf[k] <= 'f') || d->dev.bdf[k] == ':' ||
                   d->dev.bdf[k] == '.'))
                 return -7;
+        char bdf[17] = {0};
+        memcpy(bdf, d->dev.bdf, bl);
+        if (yaml_not_plain(bdf)) return -7;
         for (size_t k = 0; k < d->key_len; k++) {
             const char c = d->key[k];
             if (!(alpha(c) || digit(c) || c == '_' || c == '.' || c == '-')) return -7;
