@@ -51,6 +51,15 @@ print("pcie nodes", len(ptree["key"]), "pref",
       len(kx.preferred_allocation_pcie(pdn, pnode, ptree["parent"], ptree["depth"], W.topo_requests(pdn, n_req=300))),
       len(kx.preferred_allocation_pcie(pdn, pnode, ptree["parent"], ptree["depth"],
                                        W.topo_requests(pdn, n_req=1, avail=len(pnode), size=5000, must_max=3))[0]))
+# one large PCIe request over 3 tiles + 1 position with r on the first tile seam: roots of 2048 positions, leaves of 16
+# (776 nodes, so k_pick runs 4 CTAs), one home; size 4096 fits no node, so the answer is positions 0 .. 4095
+sn = 3 * 4096 + 1
+snode = (sn // 2048 + 1 + np.arange(sn) // 16).astype(np.uint32)
+spar = np.concatenate([np.full(sn // 2048 + 1, B.PCIE_NO_NODE), np.arange(sn // 16 + 1) * 16 // 2048]).astype(np.uint32)
+sdep = np.concatenate([np.zeros(sn // 2048 + 1), np.ones(sn // 16 + 1)]).astype(np.uint8)
+seam = kx.preferred_allocation_pcie(np.ones(sn, np.uint64), snode, spar, sdep, [(np.arange(sn)[::-1].copy(), [], 4096)])[0]
+assert seam == list(range(4096)) and len(spar) > 3 * 256
+print("pcie seam request", len(seam), "nodes", len(spar))
 # rediscovery: index reconciliation over PCI and UUID keys
 for mdev in (False, True):
     prev, cur, ni = W.reconcile_pair(3, 20000, mdev=mdev)

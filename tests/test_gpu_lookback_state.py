@@ -19,13 +19,18 @@ least two; the Call objects below restate the host code's sizes and every test a
   k_rc_probe     reconcile                                                 1024 entries                    1 epoch
   k_big_scatter  preferred_allocation                                      4096 device positions  1 per request of
                                                                                                   > 256 positions
+                 preferred_allocation_pcie (585 status words per tile:     4096 device positions  1 per request of
+                 9 lca levels x 65 NUMA bins; more than 28 tiles grow                             > 256 positions
+                 the state past the first buffer)
 """
 import threading
 
 import numpy as np
 import pytest
 
+import pref_edge_cases as PE
 from oracle import mdev_oracle as MO
+from oracle import pcie_oracle as PO
 from oracle import reconcile_oracle as RO
 from oracle import topo_oracle as TO
 from oracle import xpu_oracle as XO
@@ -37,6 +42,7 @@ EMIT_TILE = 128                # emit.cu TILE
 C_TILE, OS_TILE = 2048, 4096   # classify.cu: the accept / device-first scans, the one-sweep sort
 RC_TILE = 1024                 # reconcile.cu RC_TILE
 BS_TILE, BINS = 4096, 65       # topology.cu k_big_scatter: positions per tile, status words per tile
+PCIE_BINS = 9 * 65             # the same in the PCIe call: lca levels of depth 7 .. 0 and "none", 65 bins each
 WARP_MAX = 256                 # topology.cu: larger requests take k_big_scatter
 FIRST_WORDS = 1 << 14          # kx_scan_state: the first buffer of a context
 KIND = b"amd.com/gpu"
@@ -186,6 +192,16 @@ class Cases:
         t = cdiv(n_devs, BS_TILE)
         return Call("preferred_allocation", (dev_numa, reqs), TO.preferred_allocation(dev_numa, reqs), nb, t * BINS, t)
 
+    def preferred_allocation_pcie(self, k, n_big, n_warp, seed):
+        """preferred_allocation's requests over a forest of the devices (tests/pref_edge_cases.py range_forest), with
+        the 585 status words per tile of the PCIe call."""
+        c = self.preferred_allocation(k, n_big, n_warp, seed)
+        dev_numa, reqs = c.args
+        node, parent, depth = PE.range_forest(len(dev_numa))
+        want = PO.preferred_allocation_pcie(dev_numa, node, parent, depth, reqs)
+        return Call("preferred_allocation_pcie", (dev_numa, node, parent, depth, reqs), want, c.epochs,
+                    c.tiles * PCIE_BINS, c.tiles)
+
 
 def same(got, want, what):
     if isinstance(want, dict):
@@ -238,6 +254,8 @@ def run(kx, c, what, tab=None, rows=None):
         got = kx.reconcile(a[0], a[1], a[2])
     elif c.op == "preferred_allocation":
         got = kx.preferred_allocation(a[0], a[1])
+    elif c.op == "preferred_allocation_pcie":
+        got = kx.preferred_allocation_pcie(*a)
     else:
         raise AssertionError(c.op)
     same(got, c.want, "%s %r" % (what, c))
@@ -275,7 +293,7 @@ def small_round(cs, seed):
             cs.classify_mdev(4500 + 17 * seed, seed), cs.cdi_emit_mdev(257 + 9 * seed, seed),
             cs.lw_encode(4200 + 23 * seed, seed), cs.lw_encode(4096 + 29 * seed, seed, topo=True),
             cs.classify_topo(5000 + 31 * seed, seed), cs.classify_mdev_topo(4200 + 19 * seed, seed),
-            cs.preferred_allocation(1 + seed % 2, 3, 5, seed)]
+            cs.preferred_allocation(1 + seed % 2, 3, 5, seed), cs.preferred_allocation_pcie(2 - seed % 2, 3, 5, seed)]
 
 
 @pytest.fixture(scope="module")
@@ -291,7 +309,8 @@ def daemon_script(cases):
     grow = [cases.classify(1 << 18, 100)]
     rest = small_round(cases, 1) + small_round(cases, 2) + [
         cases.classify_retry(), cases.preferred_allocation(2, 12, 20, 101), cases.preferred_allocation(3, 10, 4, 102),
-        cases.preferred_allocation(1, 16, 0, 103), cases.classify_topo(70000, 104), cases.reconcile(5000, 105),
+        cases.preferred_allocation(1, 16, 0, 103), cases.preferred_allocation_pcie(3, 8, 6, 108),
+        cases.preferred_allocation_pcie(2, 12, 0, 109), cases.classify_topo(70000, 104), cases.reconcile(5000, 105),
         cases.names(20000, 106), cases.cdi_emit(3000, 107)]
     order = np.random.default_rng(2024).permutation(len(rest))
     script = first + grow + [rest[i] for i in order] + small_round(cases, 3)
@@ -309,7 +328,7 @@ def check_multi_tile(calls):
 @pytest.mark.parametrize("limit", ["2", "3", "5", "64", None, "0", "1", "16777217", "abc"],
                          ids=["limit2", "limit3", "limit5", "limit64", "default", "bad0", "bad1", "bad16777217", "badabc"])
 def test_daemon_life_across_wraps(limit, fresh, monkeypatch, life_script, pci_text, oracle_rows):
-    """One long-lived context runs the daemon's scripted life of 73 calls (every entry point that uses the state; 238
+    """One long-lived context runs the daemon's scripted life of 79 calls (every entry point that uses the state; 270
     epochs, counting the binding's sizing calls and the classify retry) under KXPU_SCAN_EPOCH_LIMIT = limit.  With
     limit 64 every epoch value 1..63 is taken at least three times, over words that earlier calls left with the same
     value; with 2 .. 5 the wrap also falls inside single calls (the classify epochs, the large requests of one
@@ -320,7 +339,7 @@ def test_daemon_life_across_wraps(limit, fresh, monkeypatch, life_script, pci_te
     script = life_script
     check_multi_tile(script)
     epochs = sum(c.epochs for c in script)
-    assert len(script) == 73 and epochs == 238 >= 3 * 63  # limit 64: each of the 63 values taken at least three times
+    assert len(script) == 79 and epochs == 270 >= 3 * 63  # limit 64: each of the 63 values taken at least three times
     if limit is None:
         monkeypatch.delenv("KXPU_SCAN_EPOCH_LIMIT", raising=False)
         kx = fresh()
@@ -336,7 +355,7 @@ def test_daemon_life_across_wraps(limit, fresh, monkeypatch, life_script, pci_te
 
 ENTRY_POINTS = ["names", "alloc_names", "alloc_names_kind", "mdev_names", "lw_encode", "lw_encode_topo", "cdi_emit",
                 "cdi_emit_kind", "cdi_emit_mdev", "classify", "classify_rules", "classify_mdev", "classify_topo",
-                "classify_mdev_topo", "reconcile", "preferred_allocation"]
+                "classify_mdev_topo", "reconcile", "preferred_allocation", "preferred_allocation_pcie"]
 
 
 @pytest.fixture(scope="module")
@@ -350,7 +369,8 @@ def first_calls(cases):
                 classify=cases.classify(9000, s), classify_rules=cases.classify_rules(9000, s),
                 classify_mdev=cases.classify_mdev(9000, s), classify_topo=cases.classify_topo(9000, s),
                 classify_mdev_topo=cases.classify_mdev_topo(9000, s), reconcile=cases.reconcile(4000, s),
-                preferred_allocation=cases.preferred_allocation(2, 4, 4, s))
+                preferred_allocation=cases.preferred_allocation(2, 4, 4, s),
+                preferred_allocation_pcie=cases.preferred_allocation_pcie(2, 4, 4, s))
 
 
 @pytest.mark.parametrize("entry", ENTRY_POINTS)
@@ -383,13 +403,15 @@ def test_mixed_callers_on_one_context(fresh, cases, pci_text, oracle_rows):
     """8 threads share one context with KXPU_SCAN_EPOCH_LIMIT=5, so the epoch wraps every few calls while other
     threads wait on the context's lock.  Four rediscovery-shaped threads run classify_rules -> reconcile ->
     cdi_emit_kind, four Allocate-shaped threads alloc_names_kind -> preferred_allocation (warp and large requests in
-    one call) -> lw_encode_topo -> names; 10 rounds each, inputs picked by a per-thread seed from answers computed
-    before the threads start.  Fails when calls interleave inside the context's lock, or when one caller's epochs
+    one call) -> lw_encode_topo -> preferred_allocation_pcie -> names; 10 rounds each, inputs picked by a per-thread
+    seed from answers computed before the threads start.  Fails when calls interleave inside the context's lock, or when one caller's epochs
     or words leak into another's look-back."""
     redisc = [[cases.classify_rules(4097 + 1000 * v, 60 + v), cases.reconcile(1500 + 700 * v, 60 + v),
                cases.cdi_emit(200 + 300 * v, 60 + v, KIND)] for v in range(3)]
     alloc = [[cases.alloc_names(4096 + 2000 * v, 70 + v, KIND), cases.preferred_allocation(1 + v % 2, 2, 6, 70 + v),
-              cases.lw_encode(5000 + 1000 * v, 70 + v, topo=True), cases.names(4500 + 1500 * v, 70 + v)] for v in range(3)]
+              cases.lw_encode(5000 + 1000 * v, 70 + v, topo=True),
+              cases.preferred_allocation_pcie(2 - v % 2, 2, 6, 80 + v), cases.names(4500 + 1500 * v, 70 + v)]
+             for v in range(3)]
     check_multi_tile([c for v in redisc + alloc for c in v])
     kx = fresh(KXPU_SCAN_EPOCH_LIMIT="5")
     tab, rows = load_names_table(kx, pci_text, oracle_rows)
@@ -414,3 +436,23 @@ def test_mixed_callers_on_one_context(fresh, cases, pci_text, oracle_rows):
     finally:
         tab.free()
     assert not errors, errors[:3]
+
+
+@pytest.mark.parametrize("limit", ["3", None], ids=["limit3", "default"])
+def test_pcie_allocation_grows_the_state(limit, fresh, monkeypatch, cases):
+    """The PCIe allocation's 585 words per tile take the state past the first 2^14-word buffer at 29 tiles: a context
+    runs small PCIe and NUMA allocations, one PCIe allocation over 32 tiles + 1 position (33 tiles, 19305 words) that
+    grows the buffer, then the small ones again over the grown buffer's stale words.  Fails when the grown buffer is
+    not zeroed in front of the look-back that asked for it, or when a later call reads words the large one left."""
+    small = [cases.preferred_allocation_pcie(2, 3, 3, 120), cases.preferred_allocation(2, 3, 3, 121),
+             cases.preferred_allocation_pcie(1, 2, 4, 122)]
+    grow = cases.preferred_allocation_pcie(32, 3, 2, 123)
+    check_multi_tile(small + [grow])
+    assert all(c.words <= FIRST_WORDS for c in small) and grow.words == 33 * PCIE_BINS > FIRST_WORDS
+    if limit is None:
+        monkeypatch.delenv("KXPU_SCAN_EPOCH_LIMIT", raising=False)
+        kx = fresh()
+    else:
+        kx = fresh(KXPU_SCAN_EPOCH_LIMIT=limit)
+    for i, c in enumerate(small + [grow] + small + [grow] + small[::-1]):
+        run(kx, c, "call %d" % i)
