@@ -1290,6 +1290,66 @@ int32_t kxpu_dra_slices_mdev_taints(kxpu_ctx *ctx, const char *driver, const cha
                                     size_t n_taints, const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out,
                                     size_t cap, size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
 
+/* ------------------------------- DRA ResourceSlices of vGPUs on SR-IOV virtual functions (addition to ABI v14) */
+
+/* This call and its record were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym), as for
+ * kxpu_sriov.  It publishes the vGPUs of kxpu_vf_vgpu_types (a VF that carries a vGPU type) as the mdev layout publishes
+ * mediated vGPUs.  No new fact about the Kubernetes API is used: the [assumed] lists of the v9 and v11 calls above cover
+ * this call too; the VF facts are those of kxpu_vf_vgpu_types.
+ *
+ * One published vGPU (one IOMMU group whose first member is a VF that carries a vGPU type).  192 bytes, a multiple of
+ * 16; alignof 8. */
+typedef struct kxpu_dravfvgpu {
+    uint8_t  product[64];   /* the PF's productName bytes, NUL padded (as kxpu_dramdev.product)              */
+    char     type_key[40];  /* the VF's type key (kxpu_vf_vgpu_types' key row), NUL padded                  */
+    char     bdf[16];       /* the VF's PCI address                                                         */
+    char     parent[16];    /* the PF's PCI address (basename of <vf>/physfn)                               */
+    char     pcie_root[16]; /* "pci<domain>:<bus>" of the VF's entry link; "" = unknown                     */
+    char     vendor[8];     /* the PF's vendor id                                                           */
+    char     device[8];     /* the PF's device id; "" = not known                                           */
+    uint64_t numa_mask;     /* the group's NUMA mask                                                        */
+    uint32_t iommu_group;
+    uint32_t type_id;       /* the VF's vGPU type ID (current_vgpu_type)                                    */
+    uint8_t  product_len;   /* 0..64                                                                        */
+    uint8_t  reserved[7];
+} kxpu_dravfvgpu;
+
+/* The ResourceSlices of one pool of vGPUs on VFs.  The contract is kxpu_dra_slices_mdev_taints', word for word, except
+ * for the device: the slices, their header and tail, 128 devices per slice (64 with taint_since), one empty slice for
+ * n = 0, slice_off, the two-call sizing and KXPU_E_NOSPACE, the KXPU_E_INVALID argument checks, the taint table rules,
+ * taint_since == NULL giving the untainted bytes, and nothing written on KXPU_E_INVALID or KXPU_E_UNSUPPORTED.  There
+ * is no one-taint or untainted entry point for this layout.  A device is
+ *   {"name":"vfio<g>","attributes":{<attributes>}[,"taints":[...]]}
+ * with g = iommu_group in decimal (it mirrors the cdi.k8s.io/vfio<g> annotation of the typed CDI spec), and the
+ * attributes, keys sorted bytewise:
+ *   "iommuGroup":{"int":<g>}                                          always
+ *   "numaNode":{"int":<k>}                                            only when numa_mask has exactly one bit k set
+ *   "parentAddress":{"string":"<parent>"}                             always
+ *   "parentDeviceID":{"string":"<device>"}                            only when device is not empty
+ *   "parentVendorID":{"string":"<vendor>"}                            always
+ *   "pciAddress":{"string":"<bdf>"}                                   always
+ *   "productName":{"string":"<product[0..product_len)>"}              only when product_len > 0
+ *   "resource.kubernetes.io/pcieRoot":{"string":"<pcie_root>"}        only when pcie_root is not empty
+ *   "vgpuType":{"string":"<type_key>"}                                always
+ *   "vgpuTypeID":{"int":<type_id>}                                    always
+ * KXPU_E_UNSUPPORTED, with *len, the output and slice_off untouched: the taint cases of kxpu_dra_slices_mdev_taints,
+ * n >= KXPU_DRA_MAX_DEVICES, or a record outside the domain (in the order the kernel's flags report them):
+ *   - product[0..product_len) over [A-Za-z0-9_.-]; bytes past product_len are ignored;
+ *   - type_key: 1..40 bytes over [A-Za-z0-9_.-] before its first NUL (all 40 when there is none);
+ *   - bdf: 1..16 bytes over [0-9a-f:.] before its first NUL;
+ *   - parent: 1..16 bytes over [0-9a-f:.] before its first NUL;
+ *   - pcie_root: empty, or "pci" followed by 1..13 bytes over [0-9a-f:] before its first NUL;
+ *   - vendor: 1..6 bytes over [0-9a-f] before the first NUL; device: 0..6 such bytes;
+ *   - iommu_group below 4294967295;
+ *   - type_id not 0;
+ *   - product_len <= 64.
+ * GPU: the kernel of kxpu_dra_slices, instantiated for this record layout, untainted and with the taint list (one entry
+ * for n_taints == 1, KXPU_DRA_MAX_TAINTS for more).  Timed under KXPU_T_EMIT. */
+int32_t kxpu_dra_slices_vf_vgpu(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                                const kxpu_dravfvgpu *devs, size_t n, const kxpu_dra_taint *taints, size_t n_taints,
+                                const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out, size_t cap,
+                                size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
 #ifdef __cplusplus
 }
 #endif

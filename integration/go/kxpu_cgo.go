@@ -895,6 +895,22 @@ func (k *kxpu) draSlicesMdev(driver, node string, generation uint64, devs []C.kx
 	})
 }
 
+// DRA ResourceSlices of vGPUs on SR-IOV VFs (an addition to ABI v14).  One pool per vfVgpu class with a vgpuDraDriver,
+// named after the node: devs holds one kxpu_dravfvgpu per published VF group of the class in walk order, and generation
+// is the PCI walk's pool generation.  Tainted, published and replaced exactly as draSlices' output.
+func (k *kxpu) draSlicesVfVgpu(driver, node string, generation uint64, devs []C.kxpu_dravfvgpu, since []int64) ([]string, error) {
+	var p *C.kxpu_dravfvgpu
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	return k.slices("kxpu_dra_slices_vf_vgpu", driver, node, len(devs), since, func(cd, cn *C.char,
+		tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
+		ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_vf_vgpu(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), tab, nt, cs,
+			out, capacity, n, off, ns)
+	})
+}
+
 // the two-call sizing of one slice call, the table and the times in C memory; the table width is len(since) / nDevs
 func (k *kxpu) slices(what, driver, node string, nDevs int, since []int64, call func(cd, cn *C.char,
 	tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,

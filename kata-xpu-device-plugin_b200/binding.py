@@ -70,6 +70,11 @@ DRAMDEV_DTYPE = np.dtype([("product", "u1", (64,)), ("mdev_type", "S40"), ("uuid
                           ("parent", "S16"), ("pcie_root", "S16"), ("vendor", "S8"), ("device", "S8"), ("numa_mask", "<u8"),
                           ("product_len", "u1"), ("reserved", "u1", (7,))])
 assert DRAMDEV_DTYPE.itemsize == 208
+# kxpu_dravfvgpu (DRA ResourceSlices of vGPUs on SR-IOV VFs, an addition to ABI v14): one published vGPU
+DRAVFVGPU_DTYPE = np.dtype([("product", "u1", (64,)), ("type_key", "S40"), ("bdf", "S16"), ("parent", "S16"),
+                            ("pcie_root", "S16"), ("vendor", "S8"), ("device", "S8"), ("numa_mask", "<u8"),
+                            ("iommu_group", "<u4"), ("type_id", "<u4"), ("product_len", "u1"), ("reserved", "u1", (7,))])
+assert DRAVFVGPU_DTYPE.itemsize == 192
 DRA_SLICE_DEVICES = 128
 DRA_MAX_DEVICES = 1 << 24
 DRA_TAINT_SLICE_DEVICES = 64  # devices per slice of the _taint calls (ABI v11) when taint_since is given
@@ -118,6 +123,7 @@ ABI_SYMBOLS = [
     "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev", "kxpu_cdi_emit_mdev_cdev", "kxpu_cdi_parse_mdev_cdev",
     "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu", "kxpu_pcie_tree_mdev",
     "kxpu_cdi_emit_vf_vgpu", "kxpu_cdi_emit_vf_vgpu_cdev", "kxpu_cdi_parse_vf_vgpu", "kxpu_cdi_parse_vf_vgpu_cdev",
+    "kxpu_dra_slices_vf_vgpu",
 ]
 
 
@@ -245,6 +251,8 @@ def load_library():
                                          C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_mdev_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                               C.POINTER(sz), vp, C.POINTER(sz)]),
+        "kxpu_dra_slices_vf_vgpu": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
+                                          C.POINTER(sz), vp, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():
         f = getattr(L, name)
@@ -878,6 +886,12 @@ class Kxpu:
     def dra_slices_mdev_taints(self, driver, pool, node, generation, devs, taints, since):
         """kxpu_dra_slices_mdev_taints: the same for a pool of vGPUs (DRAMDEV_DTYPE devices)."""
         return self._slices(self.L.kxpu_dra_slices_mdev_taints, DRAMDEV_DTYPE, driver, pool, node, generation, devs,
+                            taints=(taints, since))
+
+    def dra_slices_vf_vgpu(self, driver, pool, node, generation, devs, taints, since):
+        """kxpu_dra_slices_vf_vgpu: the same for a pool of vGPUs on SR-IOV VFs (DRAVFVGPU_DTYPE devices); since None gives
+        the untainted bytes."""
+        return self._slices(self.L.kxpu_dra_slices_vf_vgpu, DRAVFVGPU_DTYPE, driver, pool, node, generation, devs,
                             taints=(taints, since))
 
     def aer_health(self, text, file_off, file_len, fatal_limit, nonfatal_limit, group_off, group_members):

@@ -524,6 +524,34 @@ constexpr int MAX_FRAG_DRA_MDEV = (int)sizeof(KX_M0 KX_M1 KX_M2 KX_M3 KX_M4 KX_M
                                   16 + 6 + 6 + 64 + 36 + 1;
 constexpr int DRAM_PARTS = DRAM_LITS + 2;
 
+// A vGPU on an SR-IOV VF (kxpu_dra_slices_vf_vgpu): built like the mdev fragment, each value closed by its own bytes
+// (two ints, numaNode and vgpuTypeID, sit between strings).  V0, the group, V1, the group and its closer; then for
+// each attribute in key order its opening literal (V2..V10), its value and closer (VS / VI); then VE and the separator.
+// LAYOUT_VF_VGPU is a layout of k_dra_slices only; the CDI emitters never see it.
+constexpr int LAYOUT_VF_VGPU = 6;
+static_assert(LAYOUT_VF_VGPU != LAYOUT_PCI && LAYOUT_VF_VGPU != LAYOUT_MDEV, "a DRA layout of its own");
+#define KX_V0 "{\"name\":\"vfio"
+#define KX_V1 "\",\"attributes\":{\"iommuGroup\":{\"int\":"
+#define KX_V2 ",\"numaNode\":{\"int\":"
+#define KX_V3 ",\"parentAddress\":{\"string\":\""
+#define KX_V4 ",\"parentDeviceID\":{\"string\":\""
+#define KX_V5 ",\"parentVendorID\":{\"string\":\""
+#define KX_V6 ",\"pciAddress\":{\"string\":\""
+#define KX_V7 ",\"productName\":{\"string\":\""
+#define KX_V8 ",\"resource.kubernetes.io/pcieRoot\":{\"string\":\""
+#define KX_V9 ",\"vgpuType\":{\"string\":\""
+#define KX_V10 ",\"vgpuTypeID\":{\"int\":"
+constexpr int DRAV_S = 11, DRAV_I = 12, DRAV_E = 13, DRAV_LITS = 14;
+static const char *const h_drav_lits[DRAV_LITS] = {KX_V0, KX_V1, KX_V2, KX_V3, KX_V4, KX_V5, KX_V6,
+                                                   KX_V7, KX_V8, KX_V9, KX_V10, KX_MS, KX_MI, KX_ME};
+// the longest fragment: every literal, seven string closers, three int closers, a 10-digit group twice, node 63, a
+// 16-byte parent, two 6-byte ids, a 16-byte bdf, 64 product bytes, a 16-byte root, a 40-byte type key, a 10-digit type
+// ID, the separator
+constexpr int MAX_FRAG_DRA_VF_VGPU =
+    (int)sizeof(KX_V0 KX_V1 KX_V2 KX_V3 KX_V4 KX_V5 KX_V6 KX_V7 KX_V8 KX_V9 KX_V10 KX_ME) - 1 +
+    7 * ((int)sizeof(KX_MS) - 1) + 3 * ((int)sizeof(KX_MI) - 1) + 2 * 10 + 2 + 16 + 6 + 6 + 16 + 64 + 16 + 40 + 10 + 1;
+constexpr int DRAV_PARTS = DRAV_LITS + 2;
+
 // Taints (kxpu_dra_slices[_mdev]_taint[s]).  A device that carries some taint ends with its last literal less that
 // literal's final '}' (the one that closes the device), then KX_TAINTS_OPEN, for each carried taint in table order its
 // entry head (the table's key, value and effect, assembled on the host like the slice head), the 20-byte timeAdded and
@@ -576,6 +604,8 @@ constexpr int DRA_F_PRODUCT = 0, DRA_F_BDF = 1, DRA_F_ROOT = 2, DRA_F_VENDOR = 3
 // the order of the header's domain list, which the oracle's `why` follows
 constexpr int DRAM_F_PRODUCT = 0, DRAM_F_TYPE = 1, DRAM_F_UUID = 2, DRAM_F_PARENT = 3, DRAM_F_ROOT = 4, DRAM_F_VENDOR = 5,
               DRAM_F_DEVICE = 6, DRAM_F_GROUP = 7, DRAM_F_PLEN = 8, DRAM_F_COUNT = 9;
+constexpr int DRAV_F_PRODUCT = 0, DRAV_F_KEY = 1, DRAV_F_BDF = 2, DRAV_F_PARENT = 3, DRAV_F_ROOT = 4, DRAV_F_VENDOR = 5,
+              DRAV_F_DEVICE = 6, DRAV_F_GROUP = 7, DRAV_F_TYPE_ID = 8, DRAV_F_PLEN = 9, DRAV_F_COUNT = 10;
 
 // T devices per slice, FRAG bytes per fragment, a POOL-byte pool
 template <int T, int FRAG, int POOL>
@@ -601,6 +631,18 @@ struct DraMdevSmem {
     uint32_t wsum[EMIT_THREADS / 32];
     uint32_t tile_total;
 };
+template <int T, int FRAG, int POOL>
+struct DraVfVgpuSmem {
+    alignas(16) uint8_t stage[T * FRAG + POOL + 16];
+    uint8_t pool[POOL];
+    uint8_t dec[T][22];  // group digits at 0, NUMA node digits at 10, type ID digits at 12
+    uint32_t meta[T];    // as DraSmem's, bl being the parent's length
+    uint32_t meta2[T];   // type key length | bdf length << 6 | type ID digits << 11
+    uint32_t start[T];   // fragment offset inside the slice
+    unsigned long long base;
+    uint32_t wsum[EMIT_THREADS / 32];
+    uint32_t tile_total;
+};
 template <typename Base, int NT>
 struct DraTaintsSmem : Base {
     uint8_t ts[TAINT_TILE][NT][20];  // timeAdded of taint t of device d
@@ -615,6 +657,11 @@ template <> struct DraLayout<LAYOUT_MDEV> {
     using Rec = kxpu_dramdev;
     template <int T, int FRAG, int POOL> using Smem = DraMdevSmem<T, FRAG, POOL>;
     static constexpr int PARTS = DRAM_PARTS, LAST = DRAM_E, F_COUNT = DRAM_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_MDEV;
+};
+template <> struct DraLayout<LAYOUT_VF_VGPU> {
+    using Rec = kxpu_dravfvgpu;
+    template <int T, int FRAG, int POOL> using Smem = DraVfVgpuSmem<T, FRAG, POOL>;
+    static constexpr int PARTS = DRAV_PARTS, LAST = DRAV_E, F_COUNT = DRAV_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_VF_VGPU;
 };
 // one k_dra_slices instantiation for tables of up to NT taints (NT = 0: untainted): LAST is the literal that closes a
 // device; a taint time above the maximum reports F_SINCE, a device with two taints of one key and effect F_DUP
@@ -635,6 +682,11 @@ template <int LAYOUT, int NT> struct DraKernel {
     using Params = std::conditional_t<TAINT, DraTaintsParams<PARTS, NT>, DraParams<PARTS, POOL>>;
     using Smem = std::conditional_t<TAINT, DraTaintsSmem<Base, NT>, Base>;
 };
+// the VF-vGPU fragment bound: its widest instantiation still stages a whole slice in one CTA's shared memory, and its
+// untainted one leaves room for two CTAs per SM, as the mdev layout's does
+static_assert(sizeof(DraKernel<LAYOUT_VF_VGPU, KXPU_DRA_MAX_TAINTS>::Smem) <= 227 * 1024 &&
+                  2 * (sizeof(DraKernel<LAYOUT_VF_VGPU, 0>::Smem) + 1024) <= 228 * 1024,
+              "MAX_FRAG_DRA_VF_VGPU: the VF-vGPU staging outgrew the shared memory");
 
 template <int W>
 __device__ __forceinline__ uint32_t byte_at(const uint32_t (&w)[W], int k) { return (w[k >> 2] >> (8 * (k & 3))) & 0xffu; }
@@ -795,6 +847,75 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
                    (pl ? E.len[7] + pl + ls : 0u) + (rl ? E.len[8] + rl + ls : 0u) + (tid + 1u < in_slice ? 1u : 0u);
         }
     }
+    if constexpr (LAYOUT == LAYOUT_VF_VGPU) {
+        if (tid < in_slice) {
+            // 192 bytes = 12 uint4; read field by field, as the mdev layout does, so that few of them are live at once
+            const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const Rec *>(E.devs) + i0 + tid);
+            uint32_t pl, tl, xl, bl, rl, vl, dl;
+            {  // product_len and product (q11, q0..q3)
+                const uint32_t plen_raw = p[11].z & 0xffu;
+                pl = plen_raw <= 64u ? plen_raw : 64u;  // out of the domain: reported, and bounded here
+                if (plen_raw > 64u) E.flags[DRAV_F_PLEN] = 1u;
+                const uint4 q0 = p[0], q1 = p[1], q2 = p[2], q3 = p[3];
+                const uint32_t prod[16] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w,
+                                           q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
+                if (plen_raw <= 64u && !bytes_ok(prod, 0u, pl, name_ok)) E.flags[DRAV_F_PRODUCT] = 1u;
+            }
+            {  // type_key: bytes 64..104 (q4, q5, q6.xy)
+                const uint4 q4 = p[4], q5 = p[5];
+                const uint2 q6 = reinterpret_cast<const uint2 *>(p + 6)[0];
+                const uint32_t ky[10] = {q4.x, q4.y, q4.z, q4.w, q5.x, q5.y, q5.z, q5.w, q6.x, q6.y};
+                tl = nul_len(ky);
+                if (tl == 0u || !bytes_ok(ky, 0u, tl, name_ok)) E.flags[DRAV_F_KEY] = 1u;
+            }
+            const auto addr = [](uint32_t c) { return is_lhex(c) || c == ':' || c == '.'; };
+            {  // bdf: bytes 104..120 (q6.zw, q7.xy)
+                const uint2 a = reinterpret_cast<const uint2 *>(p + 6)[1], b = reinterpret_cast<const uint2 *>(p + 7)[0];
+                const uint32_t bdf[4] = {a.x, a.y, b.x, b.y};
+                xl = nul_len(bdf);
+                if (xl == 0u || !bytes_ok(bdf, 0u, xl, addr)) E.flags[DRAV_F_BDF] = 1u;
+            }
+            {  // parent and pcie_root: bytes 120..152 (q7.zw, q8, q9.xy)
+                const uint2 a = reinterpret_cast<const uint2 *>(p + 7)[1], c = reinterpret_cast<const uint2 *>(p + 9)[0];
+                const uint4 b = p[8];
+                const uint32_t par[4] = {a.x, a.y, b.x, b.y}, root[4] = {b.z, b.w, c.x, c.y};
+                bl = nul_len(par);
+                rl = nul_len(root);
+                if (bl == 0u || !bytes_ok(par, 0u, bl, addr)) E.flags[DRAV_F_PARENT] = 1u;
+                if (rl != 0u && (rl < 4u || byte_at(root, 0) != 'p' || byte_at(root, 1) != 'c' || byte_at(root, 2) != 'i' ||
+                                 !bytes_ok(root, 3u, rl, [](uint32_t c) { return is_lhex(c) || c == ':'; })))
+                    E.flags[DRAV_F_ROOT] = 1u;
+            }
+            {  // vendor and device: bytes 152..168 (q9.zw, q10.xy)
+                const uint2 a = reinterpret_cast<const uint2 *>(p + 9)[1], b = reinterpret_cast<const uint2 *>(p + 10)[0];
+                const uint32_t ven[2] = {a.x, a.y}, dev[2] = {b.x, b.y};
+                const uint32_t vl_raw = nul_len(ven), dl_raw = nul_len(dev);
+                vl = min(vl_raw, 6u);
+                dl = min(dl_raw, 6u);
+                const auto hex = [](uint32_t c) { return is_lhex(c); };
+                if (vl_raw == 0u || vl_raw > 6u || !bytes_ok(ven, 0u, vl, hex)) E.flags[DRAV_F_VENDOR] = 1u;
+                if (dl_raw > 6u || !bytes_ok(dev, 0u, dl, hex)) E.flags[DRAV_F_DEVICE] = 1u;
+            }
+            const uint2 qm = reinterpret_cast<const uint2 *>(p + 10)[1], qg = reinterpret_cast<const uint2 *>(p + 11)[0];
+            const unsigned long long mask = ((unsigned long long)qm.y << 32) | qm.x;
+            const uint32_t group = qg.x, type_id = qg.y;
+            if (group == 0xFFFFFFFFu) E.flags[DRAV_F_GROUP] = 1u;
+            if (type_id == 0u) E.flags[DRAV_F_TYPE_ID] = 1u;
+            const bool one_node = mask != 0ull && (mask & (mask - 1ull)) == 0ull;
+            const uint32_t node = one_node ? (uint32_t)__ffsll((long long)mask) - 1u : 0u;
+            const uint32_t gl = dec_len(group), nl = one_node ? dec_len(node) : 0u, il = dec_len(type_id);
+            dec_write(group, gl, S.dec[tid]);
+            if (one_node) dec_write(node, nl, S.dec[tid] + 10);
+            dec_write(type_id, il, S.dec[tid] + 12);
+            S.meta[tid] = gl | (nl << 4) | (bl << 8) | (rl << 13) | (vl << 18) | (dl << 21) | (pl << 24);
+            S.meta2[tid] = tl | (xl << 6) | (il << 11);
+            const uint32_t ls = E.len[DRAV_S], li = E.len[DRAV_I];
+            flen = E.len[0] + E.len[1] + 2u * gl + li + E.len[3] + bl + ls + E.len[5] + vl + ls + E.len[6] + xl + ls +
+                   E.len[9] + tl + ls + E.len[10] + il + li + E.len[DRAV_E] + (nl ? E.len[2] + nl + li : 0u) +
+                   (dl ? E.len[4] + dl + ls : 0u) + (pl ? E.len[7] + pl + ls : 0u) + (rl ? E.len[8] + rl + ls : 0u) +
+                   (tid + 1u < in_slice ? 1u : 0u);
+        }
+    }
     if constexpr (K::TAINT) {  // the device's row of the table: which taints it carries, and their times
         if (tid < in_slice) {
             const long long *row = E.since + (size_t)(i0 + tid) * E.nt;
@@ -883,6 +1004,18 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             if (pl) { lit(5); put(r->product, pl); }
             if (rl) { lit(6); put(bytes(r->pcie_root), rl); }
             lit(7); put(bytes(r->vendor), vl); close(DraLayout<LAYOUT>::LAST);
+        } else if constexpr (LAYOUT == LAYOUT_VF_VGPU) {
+            const uint32_t m2 = S.meta2[d], tl = m2 & 63u, xl = (m2 >> 6) & 31u, il = m2 >> 11;
+            lit(0); put(S.dec[d], gl); lit(1); put(S.dec[d], gl); lit(DRAV_I);
+            if (nl) { lit(2); put(S.dec[d] + 10, nl); lit(DRAV_I); }
+            lit(3); put(bytes(r->parent), bl); lit(DRAV_S);
+            if (dl) { lit(4); put(bytes(r->device), dl); lit(DRAV_S); }
+            lit(5); put(bytes(r->vendor), vl); lit(DRAV_S);
+            lit(6); put(bytes(r->bdf), xl); lit(DRAV_S);
+            if (pl) { lit(7); put(r->product, pl); lit(DRAV_S); }
+            if (rl) { lit(8); put(bytes(r->pcie_root), rl); lit(DRAV_S); }
+            lit(9); put(bytes(r->type_key), tl); lit(DRAV_S);
+            lit(10); put(S.dec[d] + 12, il); lit(DRAV_I); close(DraLayout<LAYOUT>::LAST);
         } else {
             const uint32_t tl = S.tlen[d];
             lit(0); put(S.dec[d], gl); lit(1); put(S.dec[d], gl); lit(DRAM_I);
@@ -1514,10 +1647,10 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     using K = DraKernel<LAYOUT, NT>;
     constexpr bool TAINT = K::TAINT;
     constexpr int PARTS = K::PARTS, HEAD = PARTS - 2, TAIL = PARTS - 1;
-    constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : DRAM_LITS;
+    constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : LAYOUT == LAYOUT_MDEV ? DRAM_LITS : DRAV_LITS;
     constexpr int MAXF = K::MAXF;
     constexpr int F_COUNT = K::F_COUNT;
-    const char *const *lits = LAYOUT == LAYOUT_PCI ? h_dra_lits : h_dram_lits;
+    const char *const *lits = LAYOUT == LAYOUT_PCI ? h_dra_lits : LAYOUT == LAYOUT_MDEV ? h_dram_lits : h_drav_lits;
     if (!ctx || !len || !n_slices || (n && !devs)) return KXPU_E_INVALID;
     if (!dns_subdomain_ok(driver, 63) || !dns_subdomain_ok(pool, 253) || !dns_subdomain_ok(node, 253) ||
         generation >= (1ull << 63)) {
@@ -1622,7 +1755,12 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
         "a uuid outside the canonical lowercase 8-4-4-4-12 form", "a parent that is empty or holds a byte outside [0-9a-f:.]",
         "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
         "a device id that is not 0..6 bytes of [0-9a-f]", "iommu_group 4294967295", "product_len above 64"};
-    const char *const *why = LAYOUT == LAYOUT_PCI ? why_pci : why_mdev;
+    static const char *const why_vf_vgpu[DRAV_F_COUNT] = {
+        "a product byte outside [A-Za-z0-9_.-]", "a type_key that is empty or holds a byte outside [A-Za-z0-9_.-]",
+        "a bdf that is empty or holds a byte outside [0-9a-f:.]", "a parent that is empty or holds a byte outside [0-9a-f:.]",
+        "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
+        "a device id that is not 0..6 bytes of [0-9a-f]", "iommu_group 4294967295", "type_id 0", "product_len above 64"};
+    const char *const *why = LAYOUT == LAYOUT_PCI ? why_pci : LAYOUT == LAYOUT_MDEV ? why_mdev : why_vf_vgpu;
     const uint32_t *flags = reinterpret_cast<const uint32_t *>(h.data() + slices + 1);
     for (int f = 0; f < F_COUNT; f++)
         if (flags[f]) {
@@ -1673,8 +1811,8 @@ static int32_t dra_slices_tainted(kxpu_ctx *ctx, const char *what, const char *d
                                   const kxpu_dra_taint *taints, size_t n_taints, const int64_t *taint_since, uint8_t *out,
                                   size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
     if (!taint_since)
-        return dra_slices<LAYOUT>(ctx, LAYOUT == LAYOUT_PCI ? "dra_slices" : "dra_slices_mdev", driver, pool, node, generation,
-                                  devs, n, out, cap, len, slice_off, n_slices);
+        return dra_slices<LAYOUT>(ctx, LAYOUT == LAYOUT_PCI ? "dra_slices" : LAYOUT == LAYOUT_MDEV ? "dra_slices_mdev" : what,
+                                  driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
     const DraTaint taint{taints, n_taints, taint_since};
     if (n_taints == 1)
         return dra_slices<LAYOUT, 1>(ctx, what, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices,
@@ -1715,4 +1853,20 @@ extern "C" int32_t kxpu_dra_slices_mdev_taints(kxpu_ctx *ctx, const char *driver
                                                uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
     return dra_slices_tainted<LAYOUT_MDEV>(ctx, "dra_slices_mdev_taints", driver, pool, node, generation, devs, n, taints,
                                            n_taints, taint_since, out, cap, len, slice_off, n_slices);
+}
+
+// the one entry point of the VF-vGPU layout: the taint-list form, taint_since == NULL giving the untainted bytes
+extern "C" int32_t kxpu_dra_slices_vf_vgpu(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                           uint64_t generation, const kxpu_dravfvgpu *devs, size_t n,
+                                           const kxpu_dra_taint *taints, size_t n_taints, const int64_t *taint_since,
+                                           uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
+    static_assert(sizeof(kxpu_dravfvgpu) == 192 && alignof(kxpu_dravfvgpu) == 8 && offsetof(kxpu_dravfvgpu, type_key) == 64 &&
+                      offsetof(kxpu_dravfvgpu, bdf) == 104 && offsetof(kxpu_dravfvgpu, parent) == 120 &&
+                      offsetof(kxpu_dravfvgpu, pcie_root) == 136 && offsetof(kxpu_dravfvgpu, vendor) == 152 &&
+                      offsetof(kxpu_dravfvgpu, device) == 160 && offsetof(kxpu_dravfvgpu, numa_mask) == 168 &&
+                      offsetof(kxpu_dravfvgpu, iommu_group) == 176 && offsetof(kxpu_dravfvgpu, type_id) == 180 &&
+                      offsetof(kxpu_dravfvgpu, product_len) == 184,
+                  "kxpu_dravfvgpu layout");
+    return dra_slices_tainted<LAYOUT_VF_VGPU>(ctx, "dra_slices_vf_vgpu", driver, pool, node, generation, devs, n, taints,
+                                              n_taints, taint_since, out, cap, len, slice_off, n_slices);
 }

@@ -549,21 +549,29 @@ bool Plugin::passthroughDriver(const std::string &driver) const {
     return false;
 }
 
-// vfVgpu: current_vgpu_type and creatable_vgpu_types of every VF (a record with a physfn link) of such a class
+// vfVgpu: current_vgpu_type and creatable_vgpu_types of every VF (a record with a physfn link) of such a class; with
+// vfVgpuDraEnabled also the basename of that link
 void Plugin::readVfVgpus(PciWalk &w) {
     w.vts.clear();
     w.creatable.clear();
+    w.physfn.clear();
     if (!vfVgpuEnabled()) return;
     kxpu_vfvgpurec zero;
     memset(&zero, 0, sizeof zero);
     w.vts.assign(w.recs.size(), zero);
     w.creatable.assign(w.recs.size(), std::string());
+    if (vfVgpuDraEnabled()) w.physfn.assign(w.recs.size(), std::string());
     for (size_t i = 0; i < w.recs.size(); i++) {
         const kxpu_devrec &r = w.recs[i];
         if (!cdevClassOf(xpuClasses, &XpuClass::vfVgpu, r, r.vendor_txt, sizeof r.vendor_txt)) continue;
         const std::string bdf(r.bdf, strnlen(r.bdf, sizeof r.bdf));
         char buf[256];
-        if (readlink((basePath + "/" + bdf + "/physfn").c_str(), buf, sizeof buf) < 0) continue;  // no VF: the PF
+        const ssize_t ln = readlink((basePath + "/" + bdf + "/physfn").c_str(), buf, sizeof buf);
+        if (ln < 0) continue;  // no VF: the PF
+        if (!w.physfn.empty()) {
+            const std::string target(buf, (size_t)ln);
+            w.physfn[i] = target.substr(target.rfind('/') + 1);
+        }
         kxpu_vfvgpurec &v = w.vts[i];
         v.flags = KXPU_VT_READ;
         std::string cur, tab;
@@ -630,7 +638,7 @@ Error Plugin::gatherVfVgpu(PciWalk &w) {
     return e;
 }
 
-// vfVgpu with draDriver, or on a vGPU class: refused, naming the class
+// vfVgpu with draDriver, or on a vGPU class, and vgpuDraDriver without vfVgpu: refused, naming the class
 Error Plugin::checkVfVgpuClasses() const {
     for (const XpuClass &c : xpuClasses)
         if (c.vfVgpu && !c.draDriver.empty())
@@ -638,6 +646,14 @@ Error Plugin::checkVfVgpuClasses() const {
     for (const XpuClass &c : vgpuClasses)
         if (c.vfVgpu)
             return fail("vGPU class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + "): vfVgpu applies to passthrough classes only");
+    for (const XpuClass &c : xpuClasses)
+        if (!c.vfVgpu && !c.vgpuDraDriver.empty())
+            return fail("class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + "): vgpuDraDriver " + c.vgpuDraDriver +
+                        " needs vfVgpu on the class");
+    for (const XpuClass &c : vgpuClasses)
+        if (!c.vgpuDraDriver.empty())
+            return fail("vGPU class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + "): vgpuDraDriver " + c.vgpuDraDriver +
+                        " applies to vfVgpu classes only");
     return Error();
 }
 
@@ -1085,6 +1101,7 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
         pcieParent.assign(w.nodeParent.begin(), w.nodeParent.begin() + w.nNodes);
         pcieDepth.assign(w.nodeDepth.begin(), w.nodeDepth.begin() + w.nNodes);
     }
+    buildVfVgpuDra(w);
     for (uint32_t d = 0; d < c.nDevids; d++) {
         std::vector<std::string> groups;
         for (uint32_t k = c.doff[d]; k < c.doff[d + 1]; k++) groups.push_back(std::to_string(c.dgrp[k]));  // :169
@@ -1391,6 +1408,65 @@ void Plugin::buildMdevDra(const MdevWalk &w) {
         const std::string &name = names[idAt[idOf[g]]];
         const std::string &product = name.empty() ? idOf[g].second : name;
         kxpu_dramdev &d = *mdevState[g].dra;
+        d.product_len = (uint8_t)std::min(product.size(), sizeof d.product);
+        memcpy(d.product, product.data(), d.product_len);
+    }
+}
+
+// the VF-vGPU record of every iommuState entry of a class with a vgpuDraDriver (vfVgpuDraEnabled only) whose first
+// member is a VF with a named type: one kxpu_dravfvgpu from that VF and its PF.  The PF's vendor and device ids come from
+// its own record in this walk; the PFs' model names from one getDeviceNames call over the distinct (vendor, device) ids
+void Plugin::buildVfVgpuDra(const PciWalk &w) {
+    if (!vfVgpuDraEnabled()) return;
+    const ClassifyResult &c = w.out;
+    std::map<std::string, size_t> recAt;  // PCI address -> record
+    for (size_t i = 0; i < w.recs.size(); i++) recAt.emplace(std::string(w.recs[i].bdf, strnlen(w.recs[i].bdf, sizeof w.recs[i].bdf)), i);
+    std::map<std::pair<std::string, std::string>, size_t> idAt;  // (vendor, device) -> position in the lookup batch
+    std::vector<std::string> ids, vendors;
+    std::vector<std::pair<size_t, std::pair<std::string, std::string>>> idOf;  // (group, its PF's ids)
+    auto idText = [](const uint8_t *txt, uint8_t len, size_t cap) {
+        return trimID(std::string((const char *)txt, std::min<size_t>(len, cap)));
+    };
+    for (uint32_t g = 0; g < c.nGroups; g++) {
+        const uint32_t first = c.gmem[c.goff[g]];
+        const kxpu_devrec &r = w.recs[first];
+        const XpuClass &k = xpuClasses[iommuState[g].klass];
+        if (k.vgpuDraDriver.empty() || !xpuClasses[recordClass(xpuClasses, r.vendor_txt, r.vendor_len, r.driver, sizeof r.driver)].vfVgpu ||
+            w.vstatus[first] != KXPU_VT_NAMED || w.physfn[first].empty())
+            continue;
+        kxpu_dravfvgpu d;
+        memset(&d, 0, sizeof d);
+        memcpy(d.type_key, w.vkeys[first].key, std::min<size_t>(w.vkeys[first].len, sizeof d.type_key));
+        d.type_id = w.vtype[first];
+        memcpy(d.bdf, r.bdf, strnlen(r.bdf, sizeof r.bdf));
+        const std::string &pf = w.physfn[first];
+        memcpy(d.parent, pf.data(), std::min(pf.size(), sizeof d.parent));
+        const std::string root = pcieRootOf(w.paths.size() > first ? &w.paths[first] : nullptr);
+        memcpy(d.pcie_root, root.data(), root.size());
+        std::string vendor = idText(r.vendor_txt, r.vendor_len, sizeof r.vendor_txt), device;
+        auto at = recAt.find(pf);
+        if (at != recAt.end()) {
+            const kxpu_devrec &p = w.recs[at->second];
+            if (!(p.flags & KXPU_REC_VENDOR_ERR)) vendor = idText(p.vendor_txt, p.vendor_len, sizeof p.vendor_txt);
+            if (p.device_len && !(p.flags & KXPU_REC_DEVICE_ERR)) device = idText(p.device_txt, p.device_len, sizeof p.device_txt);
+        }
+        memcpy(d.vendor, vendor.data(), std::min(vendor.size(), sizeof d.vendor));
+        memcpy(d.device, device.data(), std::min(device.size(), sizeof d.device));
+        d.numa_mask = c.gnuma.size() > g ? c.gnuma[g] : 0;
+        d.iommu_group = r.iommu_group;
+        iommuState[g].vfVgpuDra = d;
+        idOf.emplace_back(g, std::make_pair(vendor, device));
+        if (!device.empty() && idAt.emplace(idOf.back().second, ids.size()).second) {
+            ids.push_back(device);
+            vendors.push_back(vendor);
+        }
+    }
+    const std::vector<std::string> names = ids.empty() ? std::vector<std::string>() : getDeviceNames(ids, vendors);
+    for (const auto &gi : idOf) {
+        if (gi.second.second.empty()) continue;  // no device id: no productName
+        const std::string &name = names[idAt[gi.second]];
+        const std::string &product = name.empty() ? gi.second.second : name;
+        kxpu_dravfvgpu &d = *iommuState[gi.first].vfVgpuDra;
         d.product_len = (uint8_t)std::min(product.size(), sizeof d.product);
         memcpy(d.product, product.data(), d.product_len);
     }
@@ -1827,18 +1903,28 @@ bool Plugin::draEnabled() const {
     return false;
 }
 
+bool Plugin::vfVgpuDraEnabled() const {
+    for (const XpuClass &c : xpuClasses)
+        if (!c.vgpuDraDriver.empty()) return true;
+    return false;
+}
+
 bool Plugin::vgpuDraEnabled() const {
     for (const XpuClass &c : vgpuClasses)
         if (!c.draDriver.empty()) return true;
     return false;
 }
 
-// DRA drivers are distinct across xpuClasses and vgpuClasses (a passthrough class is named by its position, a vGPU
-// class by "vGPU <position>"), and a node name is required when any class has one
+// DRA drivers (draDriver and vgpuDraDriver) are distinct across xpuClasses and vgpuClasses (a passthrough class is named
+// by its position, a vGPU class by "vGPU <position>", a vgpuDraDriver by its class's name and " vGPUs"), and a node name
+// is required when any class has one
 Error Plugin::checkDraClasses() const {
     std::vector<std::pair<const std::string *, std::string>> all;  // (driver, class name)
     for (size_t c = 0; c < xpuClasses.size(); c++) all.emplace_back(&xpuClasses[c].draDriver, std::to_string(c));
     for (size_t c = 0; c < vgpuClasses.size(); c++) all.emplace_back(&vgpuClasses[c].draDriver, "vGPU " + std::to_string(c));
+    for (size_t c = 0; c < xpuClasses.size(); c++) all.emplace_back(&xpuClasses[c].vgpuDraDriver, std::to_string(c) + " vGPUs");
+    for (size_t c = 0; c < vgpuClasses.size(); c++)
+        all.emplace_back(&vgpuClasses[c].vgpuDraDriver, "vGPU " + std::to_string(c) + " vGPUs");
     for (size_t c = 0; c < all.size(); c++) {
         const std::string &d = *all[c].first;
         if (d.empty()) continue;
@@ -2352,6 +2438,15 @@ static void forPublished(const OrderedMap<V> &m, const std::vector<GroupState<Dr
     for (size_t g = 0; g < m.size(); g++)
         if (state[g].dra && !classes[state[g].klass].draDriver.empty() && state[g].blocker.empty()) f(m[g].first, state[g]);
 }
+// the same for the VF-vGPU pools of the PCI walk: the group has a VF-vGPU record, its class a vgpuDraDriver, and it has
+// no blocker
+template <typename F>
+static void forPublishedVfVgpu(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, const std::vector<GroupState<kxpu_dradev>> &state,
+                               const std::vector<XpuClass> &classes, F f) {
+    for (size_t g = 0; g < m.size(); g++)
+        if (state[g].vfVgpuDra && !classes[state[g].klass].vgpuDraDriver.empty() && state[g].blocker.empty())
+            f(m[g].first, state[g]);
+}
 
 template <typename Rec>
 Error Plugin::draSlices(int32_t (*fn)(kxpu_ctx *, const char *, const char *, const char *, uint64_t, const Rec *, size_t,
@@ -2487,6 +2582,7 @@ void Plugin::updateAerTaints(bool &passthroughMoved, bool &vgpuMoved) {
         return was != v;
     };
     forPublished(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const auto &s) { passthroughMoved |= visit(g, s.aerBits); });
+    forPublishedVfVgpu(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const auto &s) { passthroughMoved |= visit(g, s.aerBits); });
     forPublished(mdevMap, mdevState, vgpuClasses, [&](const std::string &g, const auto &s) { vgpuMoved |= visit(g, s.aerBits); });
     aerTaint_ = std::move(next);
 }
@@ -2535,6 +2631,7 @@ Error Plugin::refreshDraHealth(bool &passthroughMoved, bool &vgpuMoved) {
         return was != is;
     };
     forPublished(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const auto &) { passthroughMoved |= visit(g, false); });
+    forPublishedVfVgpu(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const auto &) { passthroughMoved |= visit(g, false); });
     forPublished(mdevMap, mdevState, vgpuClasses, [&](const std::string &g, const auto &) { vgpuMoved |= visit(g, true); });
     draTaintSince_ = std::move(next);
     if (passthroughMoved) pci_.draGeneration++;
@@ -2557,6 +2654,21 @@ Error Plugin::VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, st
                      mdev_.draGeneration, devs, groups, out, sliceOff);
 }
 
+Error Plugin::VfVgpuResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) {
+    std::shared_lock<std::shared_mutex> lock(mu_);
+    if (xpuClass >= xpuClasses.size() || xpuClasses[xpuClass].vgpuDraDriver.empty())
+        return fail("VfVgpuResourceSlices: class " + std::to_string(xpuClass) + " has no vGPU DRA driver");
+    std::vector<kxpu_dravfvgpu> devs;
+    std::vector<std::string> groups;
+    forPublishedVfVgpu(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const GroupState<kxpu_dradev> &s) {
+        if (s.klass != xpuClass) return;
+        devs.push_back(*s.vfVgpuDra);
+        groups.push_back(g);
+    });
+    return draSlices(kxpu_dra_slices_vf_vgpu, "kxpu_dra_slices_vf_vgpu", xpuClasses[xpuClass].vgpuDraDriver,
+                     pci_.draGeneration, devs, groups, out, sliceOff);
+}
+
 Error Plugin::PrepareDraDevices(const std::string &driver, const std::string &pool, const std::vector<std::string> &deviceNames,
                                 std::vector<std::vector<std::string>> &cdiIds) {
     std::vector<std::string> groups;
@@ -2564,7 +2676,7 @@ Error Plugin::PrepareDraDevices(const std::string &driver, const std::string &po
         std::shared_lock<std::shared_mutex> lock(mu_);  // Allocate takes it again below
         size_t cls = xpuClasses.size(), vcls = vgpuClasses.size();
         for (size_t c = 0; c < xpuClasses.size(); c++)
-            if (!driver.empty() && xpuClasses[c].draDriver == driver) cls = c;
+            if (!driver.empty() && (xpuClasses[c].draDriver == driver || xpuClasses[c].vgpuDraDriver == driver)) cls = c;
         for (size_t c = 0; c < vgpuClasses.size(); c++)
             if (!driver.empty() && vgpuClasses[c].draDriver == driver) vcls = c;
         const bool vgpu = vcls < vgpuClasses.size();
@@ -3662,6 +3774,31 @@ int kxh_vgpu_resource_slices(void *h, int cls, uint8_t *out, size_t cap, size_t 
     return 0;
 }
 uint64_t kxh_dra_vgpu_generation(void *h) { return ((Plugin *)h)->draVgpuGeneration(); }
+
+// ---- DRA ResourceSlices of vGPUs on SR-IOV VFs (kxpu_dra_slices_vf_vgpu)
+// vgpuDraDriver of passthrough class cls (vgpu: of vGPU class cls; "" = not published), and the node name
+int kxh_set_vf_vgpu_dra(void *h, int vgpu, int cls, const char *driver, const char *node_name) {
+    Plugin *p = (Plugin *)h;
+    std::vector<device_plugin::XpuClass> &classes = vgpu ? p->vgpuClasses : p->xpuClasses;
+    if (cls < 0 || (size_t)cls >= classes.size()) return -1;
+    classes[cls].vgpuDraDriver = driver;
+    p->nodeName = node_name;
+    return 0;
+}
+// VfVgpuResourceSlices of one class, answered like kxh_resource_slices
+int kxh_vf_vgpu_slices(void *h, int cls, uint8_t *out, size_t cap, size_t *len, uint64_t *offs, size_t offcap,
+                       size_t *n_slices) {
+    std::vector<uint8_t> o;
+    std::vector<uint64_t> so;
+    device_plugin::Error e = ((Plugin *)h)->VfVgpuResourceSlices((size_t)cls, o, so);
+    if (e) { copy_out(e.message, (char *)out, cap); return -1; }
+    *len = o.size();
+    *n_slices = so.size() - 1;
+    if (o.size() > cap || so.size() > offcap) return -2;
+    memcpy(out, o.data(), o.size());
+    memcpy(offs, so.data(), so.size() * sizeof(uint64_t));
+    return 0;
+}
 // a counting seam on readIDFromFile: every read of the file `prop` (e.g. "../device") is counted
 void kxh_count_id_reads(void *h, const char *prop, uint64_t *reads) {
     Plugin *p = (Plugin *)h;

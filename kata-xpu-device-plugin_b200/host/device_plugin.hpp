@@ -203,6 +203,10 @@ struct XpuClass {
     // finds no creatable_vgpu_types list to learn names from; with Plugin::resumeIndices the class's spec carries the type
     // of every VF it names, and the restart learns the names from it, so these are needed only without resumeIndices.
     std::map<uint32_t, std::string> vgpuTypeNames{};
+    // vfVgpu only (refused on any other class): the DRA driver that publishes the class's vGPUs as ResourceSlices
+    // (Plugin::VfVgpuResourceSlices, kxpu_dra_slices_vf_vgpu), one pool named nodeName.  Kept apart from draDriver, which
+    // promises the passthrough record layout (kxpu_dradev).  Empty: the class's vGPUs are not published.
+    std::string vgpuDraDriver{};
 };
 XpuClass defaultXpuClass();  // {"10de", "vfio-pci", "nvidia.com", "nvidia.com/gpu", "cdi-vfio-xxxx"}
 
@@ -269,6 +273,8 @@ struct PciWalk {
     std::vector<kxpu_vgpukey> vkeys;
     std::vector<uint32_t> vtype;
     std::vector<uint8_t> vstatus;
+    // vfVgpuDraEnabled only, one per record of vts: the basename of its physfn link (the PF's address); "" = not read
+    std::vector<std::string> physfn;
 };
 struct MdevWalk {
     std::vector<kxpu_mdevrec> recs;
@@ -305,6 +311,9 @@ struct GroupState {
     std::string aer{};    // aerHealth: the first member over an AER limit (computeAer); empty = within the limits
     uint8_t aerBits = 0;  // aerHealth: the group's KXPU_AER_* bits (computeAer)
     std::optional<Dra> dra{};  // draEnabled (vgpuDraEnabled): the ResourceSlice record of its first member; none = unpublished
+    // vfVgpuDraEnabled, a group of a class with a vgpuDraDriver whose first member is a VF that carries a named vGPU type:
+    // its VF-vGPU ResourceSlice record; none = unpublished
+    std::optional<kxpu_dravfvgpu> vfVgpuDra{};
 };
 
 class Plugin {
@@ -376,9 +385,15 @@ class Plugin {
     // groups in one pool named nodeName.  nodeName is a seam: the Go host takes it from NODE_NAME.
     std::string nodeName;
     bool draEnabled() const;  // some class has a draDriver
-    // the PCI gathers read numa_node (topologyAware or draEnabled) and the entry link (pcieTopologyAware or draEnabled)
-    bool readsNuma() const { return topologyAware || draEnabled(); }
-    bool readsPaths() const { return pcieTopologyAware || draEnabled(); }
+    // the PCI gathers read numa_node (topologyAware, draEnabled or vfVgpuDraEnabled) and the entry link
+    // (pcieTopologyAware, draEnabled or vfVgpuDraEnabled)
+    bool readsNuma() const { return topologyAware || draEnabled() || vfVgpuDraEnabled(); }
+    bool readsPaths() const { return pcieTopologyAware || draEnabled() || vfVgpuDraEnabled(); }
+    // DRA ResourceSlices of vGPUs on SR-IOV VFs (include/kxpu.h, kxpu_dra_slices_vf_vgpu): a vgpuDraDriver on a vfVgpu
+    // class publishes its vGPUs (VfVgpuResourceSlices) in the pool nodeName.  With one set, the PCI gathers read
+    // numa_node and the entry link as draEnabled does, and readVfVgpus keeps each VF's physfn basename; nothing else is
+    // read.  With none set, every read, output and generation is as without the setting.
+    bool vfVgpuDraEnabled() const;  // some passthrough class has a vgpuDraDriver
     // DRA ResourceSlices of vGPUs (ABI v10): a draDriver on a vGPU class publishes its groups (VgpuResourceSlices) in
     // the pool nodeName.  With one set, the mdev walk also reads, for every entry that got as far as its iommu_group
     // link, the parent's numa_node (as topologyAware does), the entry's link (readPciPath) and <uuid>/../device; a failed
@@ -388,7 +403,7 @@ class Plugin {
     // the mdev walk reads each grouped entry's link (vgpuPcieTopologyAware or vgpuDraEnabled); one read serves both
     bool readsMdevPaths() const { return vgpuPcieTopologyAware || vgpuDraEnabled(); }
     // DRA device taints (ABI v11).  false (default): the slices never carry taints and every output and generation is as
-    // above, even while a device is Unhealthy.  true: ResourceSlices and VgpuResourceSlices pass taint times to the
+    // above, even while a device is Unhealthy.  true: ResourceSlices, VfVgpuResourceSlices and VgpuResourceSlices pass taint times to the
     // slice call (64 devices per slice); a group that refreshDraHealth found unhealthy carries the taint
     // <draDriver>/unhealthy=vfio-device-missing:NoSchedule since the time it was found so, and PrepareDraDevices refuses
     // it.
@@ -521,7 +536,8 @@ class Plugin {
     // out: JSON Lines, one slice per line; sliceOff: the n_slices + 1 line bounds.
     Error ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff);
     // the pool generation of every class's ResourceSlices: 1 after start-up, +1 for each rediscover that changed a
-    // passthrough plugin or a group's viability, +1 for each refreshDraHealth that changed their taints
+    // passthrough plugin or a group's viability, +1 for each refreshDraHealth that changed their taints; the VF-vGPU
+    // pools (VfVgpuResourceSlices) share it, their VFs being functions of the PCI walk
     uint64_t draGeneration() const { return pci_.draGeneration; }
     // draTaints: the device-plugin health of every group published in a DRA pool becomes its taint.  The host calls it
     // after HealthWatcher::poll returned > 0.  Under the exclusive lock: a group that any plugin serving it has
@@ -534,6 +550,15 @@ class Plugin {
     // whose ListAndWatch bytes changed; with draTaints, passthroughMoved / vgpuMoved say which pools' AER taints changed
     // (their generation grew by one).  Without aerHealth nothing is read and nothing changes.
     Error refreshAerHealth(std::vector<size_t> &changedPlugins, bool &passthroughMoved, bool &vgpuMoved);
+    // The ResourceSlices of the vGPUs of vfVgpu class xpuClass (kxpu_dra_slices_vf_vgpu): one pool named nodeName, one
+    // device per iommuMap group of the class in walk order whose first member is a VF that carries a named vGPU type,
+    // unless the group has a blocker (as ResourceSlices).  The device is described by that VF: its address, type key and
+    // type ID, the PCIe root of its link, the group's NUMA mask, and its PF (the physfn basename): the PF's address, the
+    // vendor and device ids of the PF's record in the same walk (a PF the walk did not read: the VF's vendor id and no
+    // device id), and the PF's model name (getDeviceNames: the sanitised pci.ids name, else the raw device id; cut to 64
+    // bytes) as productName.  Generation: draGeneration, since these VFs are functions of the PCI walk; taints as for
+    // ResourceSlices.
+    Error VfVgpuResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff);
     // The ResourceSlices of vGPU class vgpuClass (kxpu_dra_slices_mdev): one pool named nodeName, one device per mdevMap
     // group of the class in walk order, described by the group's first mdev: its type key, UUID, parent address, the
     // parent's vendor and device ids, the PCIe root of its link, the group's NUMA mask, and the parent's model name
@@ -543,8 +568,9 @@ class Plugin {
     // vGPU plugin, +1 for each refreshDraHealth that changed their taints
     uint64_t draVgpuGeneration() const { return mdev_.draGeneration; }
     // The data half of NodePrepareResources: cdiIds[i] = the CDI names Allocate({g}) returns for deviceNames[i] =
-    // "vfio<g>", a device of the pool `pool` of the class (passthrough or vGPU) whose draDriver is `driver` (same live or
-    // snapshot re-validation, same viability refusal; a vGPU group is always re-read live).  An unknown driver, pool or
+    // "vfio<g>", a device of the pool `pool` of the class (passthrough or vGPU) whose draDriver is `driver`, or of the vfVgpu
+    // class whose vgpuDraDriver it is (same live or snapshot re-validation, same viability refusal; a vGPU group is always
+    // re-read live, and Allocate refuses a VF whose vGPU type changed since the walk).  An unknown driver, pool or
     // device is an error that names it.
     Error PrepareDraDevices(const std::string &driver, const std::string &pool, const std::vector<std::string> &deviceNames,
                             std::vector<std::vector<std::string>> &cdiIds);
@@ -682,6 +708,7 @@ class Plugin {
                     const std::vector<std::string> &groups, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) const;
     Error checkDraClasses() const;
     void buildMdevDra(const MdevWalk &w);
+    void buildVfVgpuDra(const PciWalk &w);
 };
 
 }  // namespace device_plugin

@@ -655,6 +655,29 @@ def dra_mdev_devices(n=1 << 16, seed=43):
     return d
 
 
+def dra_vf_vgpu_devices(n=1 << 16, seed=47):
+    """n published vGPUs on SR-IOV VFs with every optional attribute present and the longest fields the host produces:
+    a 64-byte product name, a 40-byte type key, 12-byte VF and PF addresses, a 10-byte PCIe root, 4-digit ids, a 4-digit
+    type ID, one NUMA node, 9-digit groups"""
+    from .binding import DRAVFVGPU_DTYPE
+    rng = np.random.default_rng(seed)
+    d = np.zeros(n, DRAVFVGPU_DTYPE)
+    alnum = np.frombuffer(b"ABCDEFGHIJKLMNOPQRSTUVWXYZ0123456789_", np.uint8)
+    d["product"] = alnum[rng.integers(0, len(alnum), (n, 64))]
+    d["product_len"] = 64
+    d["type_key"] = b"NVIDIA_H100XM-1-10C_with_a_long_type.key"
+    d["type_id"] = 1058 + np.arange(n) % 4
+    i = np.arange(n)
+    par = i >> 4  # sixteen VFs per PF
+    d["parent"] = [b"%04x:%02x:%02x.0" % (k >> 13, (k >> 5) & 0xff, k & 0x1f) for k in par.tolist()]
+    d["bdf"] = [b"%04x:%02x:%02x.%d" % (k >> 17, (k >> 9) & 0xff, (k >> 4) & 0x1f, 1 + (k & 7) % 7) for k in i.tolist()]
+    d["pcie_root"] = [b"pci%04x:%02x" % (k >> 13, (k >> 5) & 0xff) for k in par.tolist()]
+    d["vendor"], d["device"] = b"10de", b"2330"
+    d["numa_mask"] = np.left_shift(np.uint64(1), (par % 8).astype(np.uint64))
+    d["iommu_group"] = 100000000 + i
+    return d
+
+
 AER_FATAL_NAMES = ["Undefined", "DLP", "SDES", "TLP", "FCP", "CmpltTO", "CmpltAbrt", "UnxCmplt", "RxOF", "MalfTLP",
                    "ECRC", "UnsupReq", "ACSViol", "UncorrIntErr", "BlockedTLP", "AtomicOpBlocked", "TLPBlockedErr",
                    "PoisonTLPBlocked"]

@@ -108,6 +108,15 @@ blob, soff = kx.dra_slices_mdev_taints("vgpu.nvidia.com", "node-a", "node-a", 1,
 print("dra mdev taints slices, one entry", len(soff) - 1, "bytes", len(blob))
 blob, soff = kx.dra_slices_mdev_taints("vgpu.nvidia.com", "node-a", "node-a", 1, W.dra_mdev_devices(3000), tab3, since3)
 print("dra mdev taints slices", len(soff) - 1, "bytes", len(blob))
+# the VF-vGPU layout: untainted (24 slices and the empty pool) and with one and three taint entries
+for dn_ in (3000, 0):
+    blob, soff = kx.dra_slices_vf_vgpu("vgpu-vf.nvidia.com", "node-a", "node-a", 1, W.dra_vf_vgpu_devices(dn_), tab3, None)
+    print("dra vf vgpu slices", len(soff) - 1, "bytes", len(blob))
+blob, soff = kx.dra_slices_vf_vgpu("vgpu-vf.nvidia.com", "node-a", "node-a", 1, W.dra_vf_vgpu_devices(3000), tab3[:1],
+                                   since3[:, :1])
+print("dra vf vgpu taints slices, one entry", len(soff) - 1, "bytes", len(blob))
+blob, soff = kx.dra_slices_vf_vgpu("vgpu-vf.nvidia.com", "node-a", "node-a", 1, W.dra_vf_vgpu_devices(3000), tab3, since3)
+print("dra vf vgpu taints slices", len(soff) - 1, "bytes", len(blob))
 
 
 # look-back state across epoch wraps (tests/test_gpu_lookback_state.py at reduced sizes): every user of the status
