@@ -731,6 +731,34 @@ int32_t kxpu_classify_vf_vgpu(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t 
                               kxpu_classify_out *out, uint8_t *dev_rule /* [n] */, uint64_t *group_numa /* [n] or NULL */,
                               uint32_t *group_blocker /* [n] or NULL */);
 
+/* kxpu_vf_vgpu_drift's per-record status */
+#define KXPU_VD_SAME    0u  /* the type read back is the walk's (also a record without KXPU_VT_READ: not compared)  */
+#define KXPU_VD_CLEARED 1u  /* the type is 0 now: the vGPU was destroyed                                          */
+#define KXPU_VD_CHANGED 2u  /* another type ID than the walk's                                                    */
+#define KXPU_VD_BAD     3u  /* KXPU_VT_CUR_ERR, cur_len > 16, or a text that is not a canonical decimal            */
+#define KXPU_VD_STEADY  0xFFFFFFFFu  /* group_first of a group none of whose members drifted                      */
+
+/* Has the vGPU type of a served VF changed since the walk?  Writing current_vgpu_type sends no uevent (see above), so a
+ * host re-reads the file of each VF it serves on a timer and compares.  recs_vt: n re-read side records (only cur_txt,
+ * cur_len and flags are used; creatable_vgpu_types is not read again); type_was[i]: the walk's type ID of record i
+ * (kxpu_vf_vgpu_types' type_id, 0 for none).  Groups: group_members[group_off[o] .. group_off[o+1]) are the records of
+ * group o, in kxpu_aer_health's conventions (a record may be a member of several groups).
+ *   - the current type of record i is parsed by kxpu_vf_vgpu_types' current-type rule, the same device code;
+ *   - status_now[i]: KXPU_VD_SAME when record i lacks KXPU_VT_READ or its type equals type_was[i]; else KXPU_VD_BAD for
+ *     a text that rule refuses; else KXPU_VD_CLEARED for type 0 and KXPU_VD_CHANGED for any other ID;
+ *   - type_now[i]: the parsed type (0 for KXPU_VD_BAD), type_was[i] for a record without KXPU_VT_READ;
+ *   - group_first[o]: the smallest position p (0-based, counted from group_off[o]) of a member whose status is not
+ *     KXPU_VD_SAME, or KXPU_VD_STEADY when there is none (an empty group included).
+ * KXPU_E_INVALID, and nothing written: ctx NULL; recs_vt, type_was, type_now or status_now NULL with n > 0; group_off
+ * NULL; group_members NULL with members; group_first NULL with n_groups > 0; group_off decreasing; a member >= n.
+ * Limit (else KXPU_E_UNSUPPORTED): n and n_groups below 2^28.
+ * GPU: one launch timed under KXPU_T_CLASSIFY: the first CTAs give one thread per record (two 16-byte loads, the parse,
+ * the compare), the rest one warp per group, whose lanes parse their members themselves and take a warp min of the
+ * drifted positions, so no second launch waits for the records. */
+int32_t kxpu_vf_vgpu_drift(kxpu_ctx *ctx, const kxpu_vfvgpurec *recs_vt, const uint32_t *type_was /* [n] */, size_t n,
+                           const uint32_t *group_off /* [n_groups+1] */, const uint32_t *group_members, size_t n_groups,
+                           uint32_t *type_now /* [n] */, uint8_t *status_now /* [n] */, uint32_t *group_first /* [n_groups] */);
+
 /* ------------------------------------------------- runtime rediscovery (ABI v6) */
 
 /* One accepted entry of a walk, as a rediscovery compares two walks.  64 bytes. */

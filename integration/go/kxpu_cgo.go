@@ -1141,6 +1141,26 @@ func (k *kxpu) vfVgpuTypes(recs []C.kxpu_vfvgpurec, tables [][]byte) (keys []C.k
 	return keys[:n], typeID[:n], status[:n], err
 }
 
+// the drift check: recs the re-read side records of the served VFs, was their walk's type IDs, one one-member group per
+// VF.  Returns per record the type read back and its status (C.KXPU_VD_*), and per group the position of its first
+// drifted member or C.KXPU_VD_STEADY.
+func (k *kxpu) vfVgpuDrift(recs []C.kxpu_vfvgpurec, was []uint32, groupOff, groupMembers []uint32) (typeNow []uint32,
+	status []uint8, first []uint32, err error) {
+	n, g := len(recs), len(groupOff)-1
+	typeNow, status, first = make([]uint32, n+1), make([]uint8, n+1), make([]uint32, g+1)
+	was = append(was, 0)                   // valid pointers for n == 0
+	groupMembers = append(groupMembers, 0) // and for no members
+	var r *C.kxpu_vfvgpurec
+	if n > 0 {
+		r = &recs[0]
+	}
+	err = kxCheck(k.ctx, "kxpu_vf_vgpu_drift", C.kxpu_vf_vgpu_drift(k.ctx, r, (*C.uint32_t)(unsafe.Pointer(&was[0])),
+		C.size_t(n), (*C.uint32_t)(unsafe.Pointer(&groupOff[0])), (*C.uint32_t)(unsafe.Pointer(&groupMembers[0])),
+		C.size_t(g), (*C.uint32_t)(unsafe.Pointer(&typeNow[0])), (*C.uint8_t)(unsafe.Pointer(&status[0])),
+		(*C.uint32_t)(unsafe.Pointer(&first[0]))))
+	return typeNow[:n], status[:n], first[:g], err
+}
+
 // classifyViable's contract with one resource per vGPU type for the rules of vgpuRules (bit r: rule r); keys is
 // vfVgpuTypes' output.  gnuma is filled when topo, blockers when viable (else both nil).  out must be wired and pinned as
 // for classifyRules.

@@ -97,6 +97,8 @@ VGPUKEY_DTYPE = np.dtype([("key", "u1", (40,)), ("zero", "u1", (7,)), ("len", "u
 assert VGPUKEY_DTYPE.itemsize == 48
 VT_READ, VT_CUR_ERR = 1, 2
 VT_NONE, VT_NAMED, VT_UNNAMED, VT_BAD = 0, 1, 2, 3
+VD_SAME, VD_CLEARED, VD_CHANGED, VD_BAD = 0, 1, 2, 3  # kxpu_vf_vgpu_drift's per-record status
+VD_STEADY = 0xFFFFFFFF  # kxpu_vf_vgpu_drift's group_first of a group with no drifted member
 CDI_FRAG_MIN = 166  # the shortest device fragment of a CDI spec: len // CDI_FRAG_MIN records hold any document (ABI v13)
 
 
@@ -123,7 +125,7 @@ ABI_SYMBOLS = [
     "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev", "kxpu_cdi_emit_mdev_cdev", "kxpu_cdi_parse_mdev_cdev",
     "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu", "kxpu_pcie_tree_mdev",
     "kxpu_cdi_emit_vf_vgpu", "kxpu_cdi_emit_vf_vgpu_cdev", "kxpu_cdi_parse_vf_vgpu", "kxpu_cdi_parse_vf_vgpu_cdev",
-    "kxpu_dra_slices_vf_vgpu",
+    "kxpu_dra_slices_vf_vgpu", "kxpu_vf_vgpu_drift",
 ]
 
 
@@ -244,6 +246,7 @@ def load_library():
         "kxpu_cdi_parse_vf_vgpu_cdev": (i32, [vp, i32, C.c_char_p, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_sriov": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp, sz, vp, vp, vp]),
         "kxpu_vf_vgpu_types": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp]),
+        "kxpu_vf_vgpu_drift": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp]),
         "kxpu_classify_vf_vgpu": (i32, [vp, vp, sz, C.c_uint32, vp, sz, vp, C.POINTER(ClassifyOut), vp, vp, vp]),
         "kxpu_pcie_tree_sriov": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32), vp]),
         "kxpu_pcie_tree_mdev": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32)]),
@@ -668,6 +671,21 @@ class Kxpu:
         self._chk(self.L.kxpu_vf_vgpu_types(self.ctx, _ptr(recs_vt) if n else None, n, _ptr(blob) if len(blob) else None,
                                             _ptr(toff), len(toff) - 1, _ptr(keys), _ptr(tid), _ptr(st)))
         return dict(keys=keys[:n], type_id=tid[:n], status=st[:n])
+
+    def vf_vgpu_drift(self, recs_vt, type_was, group_off, group_members):
+        """kxpu_vf_vgpu_drift: recs_vt (VFVGPUREC_DTYPE) re-read, type_was the walk's type IDs, group_off [G+1] /
+        group_members the groups.  Returns dict(type_now, status_now (VD_*), group_first (VD_STEADY: none drifted))."""
+        recs_vt = np.ascontiguousarray(recs_vt)
+        assert recs_vt.dtype == VFVGPUREC_DTYPE
+        was = np.ascontiguousarray(type_was, dtype=np.uint32)
+        goff = np.ascontiguousarray(group_off, dtype=np.uint32)
+        gmem = np.ascontiguousarray(group_members, dtype=np.uint32)
+        n, G = len(recs_vt), len(goff) - 1
+        assert len(was) == n
+        now, st, first = np.zeros(max(n, 1), np.uint32), np.zeros(max(n, 1), np.uint8), np.zeros(max(G, 1), np.uint32)
+        self._chk(self.L.kxpu_vf_vgpu_drift(self.ctx, _ptr(recs_vt) if n else None, _ptr(was) if n else None, n, _ptr(goff),
+                                            _ptr(gmem) if len(gmem) else None, G, _ptr(now), _ptr(st), _ptr(first)))
+        return dict(type_now=now[:n], status_now=st[:n], group_first=first[:G])
 
     def classify_vf_vgpu(self, rules, vgpu_rules, recs, keys, topo=False, viable=False):
         """kxpu_classify_vf_vgpu: the dict of classify_rules, plus group_numa (topo) and group_blocker (viable).  keys:

@@ -14,6 +14,8 @@
 //     (kxmdev::type_key, the rule kxpu_classify_mdev uses) and writes it with three 16-byte stores.
 // The table starts with SMALL_CAP slots; when more than half of them hold distinct IDs (or a probe run passes
 // PROBE_LIMIT) the host runs both launches again with room for every naming line the first run counted.
+//
+// kxpu_vf_vgpu_drift: one launch, k_vd_drift (records, then groups), parsing through current_type as k_vt_records does.
 #include "common.cuh"
 #include "mdev.cuh"
 
@@ -132,6 +134,28 @@ __global__ void __launch_bounds__(256) k_vt_lines(const Work W) {
     }
 }
 
+// The current-type rule (include/kxpu.h) on one kxpu_vfvgpurec: cw = cur_txt as four words, len = cur_len, fl = flags.
+// Returns the type, with ok set when the read did not fail and cur_txt[0..len), with at most one trailing '\n' removed,
+// is a canonical decimal below 2^32.  The caller tests KXPU_VT_READ.  k_vt_records and k_vd_drift both parse through
+// it, so the type join and the drift check cannot read one text two ways.
+__device__ __forceinline__ unsigned long long current_type(const uint32_t cw[4], uint32_t len, uint32_t fl, bool &ok) {
+    uint32_t l = len;
+    ok = !(fl & KXPU_VT_CUR_ERR) && len <= 16u;
+    if (ok && l && kxmdev::byte_at(cw, l - 1) == '\n') l--;
+    ok &= l > 0 && l <= 10u && !(l > 1 && kxmdev::byte_at(cw, 0) == '0');
+    unsigned long long v = 0;
+#pragma unroll
+    for (uint32_t k = 0; k < 16; k++) {
+        const uint32_t d = kxmdev::byte_at(cw, k) - '0';
+        if (k < l) {
+            ok &= d <= 9u;
+            v = v * 10 + d;
+        }
+    }
+    ok &= v <= 0xFFFFFFFFull;
+    return v;
+}
+
 __global__ void __launch_bounds__(256) k_vt_records(const Work W) {
     __shared__ __align__(16) uint8_t skey[256][48];
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -145,20 +169,8 @@ __global__ void __launch_bounds__(256) k_vt_records(const Work W) {
     uint32_t st = KXPU_VT_NONE, tid = 0;
     if (fl & KXPU_VT_READ) {
         const uint32_t cw[4] = {q0.x, q0.y, q0.z, q0.w};
-        uint32_t l = len;
-        bool ok = !(fl & KXPU_VT_CUR_ERR) && len <= 16u;
-        if (ok && l && kxmdev::byte_at(cw, l - 1) == '\n') l--;
-        ok &= l > 0 && l <= 10u && !(l > 1 && kxmdev::byte_at(cw, 0) == '0');
-        unsigned long long v = 0;
-#pragma unroll
-        for (uint32_t k = 0; k < 16; k++) {
-            const uint32_t d = kxmdev::byte_at(cw, k) - '0';
-            if (k < l) {
-                ok &= d <= 9u;
-                v = v * 10 + d;
-            }
-        }
-        ok &= v <= 0xFFFFFFFFull;
+        bool ok;
+        const unsigned long long v = current_type(cw, len, fl, ok);
         if (!ok) st = KXPU_VT_BAD;
         else if (v != 0) {
             tid = (uint32_t)v;
@@ -182,6 +194,60 @@ __global__ void __launch_bounds__(256) k_vt_records(const Work W) {
     kp[0] = row4[0]; kp[1] = row4[1]; kp[2] = row4[2];
     W.type_id[i] = tid;
     W.status[i] = (uint8_t)st;
+}
+
+// kxpu_vf_vgpu_drift: the status of record i against the walk's type was, and the type read back in now
+__device__ __forceinline__ uint32_t drift_of(const kxpu_vfvgpurec *recs, uint32_t i, uint32_t was, uint32_t &now) {
+    const uint4 *rp = reinterpret_cast<const uint4 *>(recs + i);
+    const uint4 q0 = rp[0], q1 = rp[1];
+    if (!((q1.x >> 8) & KXPU_VT_READ)) {
+        now = was;
+        return KXPU_VD_SAME;
+    }
+    const uint32_t cw[4] = {q0.x, q0.y, q0.z, q0.w};
+    bool ok;
+    const unsigned long long v = current_type(cw, q1.x & 0xffu, (q1.x >> 8) & 0xffu, ok);
+    if (!ok) {
+        now = 0;
+        return KXPU_VD_BAD;
+    }
+    now = (uint32_t)v;
+    return now == was ? KXPU_VD_SAME : now == 0 ? KXPU_VD_CLEARED : KXPU_VD_CHANGED;
+}
+
+// One launch: CTAs [0, rec_ctas) give one thread per record; the rest give one warp per group, whose lanes re-parse
+// their members (a member is one 32-byte record) and fold the drifted positions with a warp min.  Parsing a member
+// again costs less than a second launch that waits for the records.
+__global__ void __launch_bounds__(256) k_vd_drift(const kxpu_vfvgpurec *__restrict__ recs, const uint32_t *__restrict__ was,
+                                                  uint32_t n, uint32_t rec_ctas, const uint32_t *__restrict__ goff,
+                                                  const uint32_t *__restrict__ gmem, uint32_t n_groups,
+                                                  uint32_t *__restrict__ type_now, uint8_t *__restrict__ status,
+                                                  uint32_t *__restrict__ first, uint32_t *__restrict__ err) {
+    if (blockIdx.x < rec_ctas) {
+        const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+        if (i >= n) return;
+        uint32_t now;
+        status[i] = (uint8_t)drift_of(recs, i, was[i], now);
+        type_now[i] = now;
+        return;
+    }
+    const uint32_t o = (blockIdx.x - rec_ctas) * (blockDim.x / 32) + (threadIdx.x >> 5), lane = threadIdx.x & 31u;
+    if (o >= n_groups) return;  // warp-uniform
+    const uint32_t a = goff[o], b = goff[o + 1];
+    uint32_t best = KXPU_VD_STEADY;
+    bool bad = false;
+    for (uint32_t m = a + lane; m < b; m += 32u) {  // every member is range-checked; parsing stops at a lane's first drift
+        const uint32_t i = gmem[m];
+        if (i >= n) { bad = true; continue; }
+        uint32_t now;
+        if (best == KXPU_VD_STEADY && drift_of(recs, i, was[i], now) != KXPU_VD_SAME) best = m - a;
+    }
+    best = __reduce_min_sync(0xffffffffu, best);
+    bad = __any_sync(0xffffffffu, bad);
+    if (lane == 0) {
+        first[o] = best;
+        if (bad) atomicOr(err, 1u);
+    }
 }
 
 }  // namespace kxvt
@@ -266,4 +332,57 @@ extern "C" int32_t kxpu_vf_vgpu_types(kxpu_ctx *ctx, const kxpu_vfvgpurec *recs_
         if (e != cudaSuccess) { KX_SET_ERR(ctx, "vf_vgpu_types D2H failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
         return KXPU_OK;
     }
+}
+
+extern "C" int32_t kxpu_vf_vgpu_drift(kxpu_ctx *ctx, const kxpu_vfvgpurec *recs_vt, const uint32_t *type_was, size_t n,
+                                      const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
+                                      uint32_t *type_now, uint8_t *status_now, uint32_t *group_first) {
+    if (!ctx || (n && (!recs_vt || !type_was || !type_now || !status_now)) || !group_off || (n_groups && !group_first))
+        return KXPU_E_INVALID;
+    if (n >= (1ull << 28) || n_groups >= (1ull << 28)) return KXPU_E_UNSUPPORTED;
+    for (size_t g = 0; g < n_groups; g++)
+        if (group_off[g + 1] < group_off[g]) { KX_SET_ERR(ctx, "vf_vgpu_drift: group %zu: offsets decrease", g); return KXPU_E_INVALID; }
+    const size_t nm = group_off[n_groups];
+    if (nm && !group_members) return KXPU_E_INVALID;
+    if (n == 0 && n_groups == 0) return KXPU_OK;
+
+    std::lock_guard<std::mutex> guard(ctx->mu);
+    cudaSetDevice(ctx->device);
+    kx_clear_timings(ctx);
+    const size_t G = n_groups;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
+    const size_t o_recs = take(n * sizeof(kxpu_vfvgpurec)), o_was = take(n * 4), o_goff = take((G + 1) * 4);
+    const size_t o_gmem = take(nm * 4), o_now = take(n * 4), o_st = take(n), o_first = take(G * 4), o_err = take(16);
+    KxScratch sc(ctx);
+    uint8_t *b = nullptr;
+    KX_CUDA(ctx, sc.alloc((void **)&b, off));
+    cudaStream_t st = ctx->stream;
+    auto up = [&](size_t o, const void *h, size_t bytes) { if (bytes) cudaMemcpyAsync(b + o, h, bytes, cudaMemcpyHostToDevice, st); };
+    up(o_recs, recs_vt, n * sizeof(kxpu_vfvgpurec)); up(o_was, type_was, n * 4);
+    up(o_goff, group_off, (G + 1) * 4); up(o_gmem, group_members, nm * 4);
+    cudaMemsetAsync(b + o_err, 0, 16, st);
+    uint32_t *d_err = (uint32_t *)(b + o_err);
+    {
+        KxTimer tm(ctx, KXPU_T_CLASSIFY);
+        const size_t rec_ctas = (n + 255) / 256, grp_ctas = (G + 7) / 8;
+        k_vd_drift<<<(unsigned)(rec_ctas + grp_ctas), 256, 0, st>>>(
+            (const kxpu_vfvgpurec *)(b + o_recs), (const uint32_t *)(b + o_was), (uint32_t)n, (uint32_t)rec_ctas,
+            (const uint32_t *)(b + o_goff), (const uint32_t *)(b + o_gmem), (uint32_t)G, (uint32_t *)(b + o_now),
+            b + o_st, (uint32_t *)(b + o_first), d_err);
+        KX_LAUNCHED(ctx);
+    }
+    uint32_t *h = ctx->h_ctl;
+    cudaMemcpyAsync(h, d_err, 4, cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "vf_vgpu_drift failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    if (h[0]) { KX_SET_ERR(ctx, "vf_vgpu_drift: a group member index is >= n"); return KXPU_E_INVALID; }
+    if (n) {
+        cudaMemcpyAsync(type_now, b + o_now, n * 4, cudaMemcpyDeviceToHost, st);
+        cudaMemcpyAsync(status_now, b + o_st, n, cudaMemcpyDeviceToHost, st);
+    }
+    if (G) cudaMemcpyAsync(group_first, b + o_first, G * 4, cudaMemcpyDeviceToHost, st);
+    e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "vf_vgpu_drift D2H failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    return KXPU_OK;
 }

@@ -549,8 +549,21 @@ bool Plugin::passthroughDriver(const std::string &driver) const {
     return false;
 }
 
+// current_vgpu_type of <basePath>/<bdf> into a side record marked read; counts in vfVgpuReads
+static void readCurrentType(Plugin &p, const std::string &bdf, kxpu_vfvgpurec &v) {
+    v.flags = KXPU_VT_READ;
+    std::string cur;
+    p.vfVgpuReads++;
+    if (p.readVgpuFile(p.basePath, bdf, "current_vgpu_type", cur)) {
+        memcpy(v.cur_txt, cur.data(), std::min(cur.size(), sizeof v.cur_txt));
+        v.cur_len = (uint8_t)std::min<size_t>(cur.size(), sizeof v.cur_txt + 1);
+    } else {
+        v.flags |= KXPU_VT_CUR_ERR;
+    }
+}
+
 // vfVgpu: current_vgpu_type and creatable_vgpu_types of every VF (a record with a physfn link) of such a class; with
-// vfVgpuDraEnabled also the basename of that link
+// vfVgpuDraEnabled or vfVgpuHealth also the basename of that link
 void Plugin::readVfVgpus(PciWalk &w) {
     w.vts.clear();
     w.creatable.clear();
@@ -560,7 +573,7 @@ void Plugin::readVfVgpus(PciWalk &w) {
     memset(&zero, 0, sizeof zero);
     w.vts.assign(w.recs.size(), zero);
     w.creatable.assign(w.recs.size(), std::string());
-    if (vfVgpuDraEnabled()) w.physfn.assign(w.recs.size(), std::string());
+    if (vfVgpuDraEnabled() || vfVgpuHealth) w.physfn.assign(w.recs.size(), std::string());
     for (size_t i = 0; i < w.recs.size(); i++) {
         const kxpu_devrec &r = w.recs[i];
         if (!cdevClassOf(xpuClasses, &XpuClass::vfVgpu, r, r.vendor_txt, sizeof r.vendor_txt)) continue;
@@ -572,16 +585,8 @@ void Plugin::readVfVgpus(PciWalk &w) {
             const std::string target(buf, (size_t)ln);
             w.physfn[i] = target.substr(target.rfind('/') + 1);
         }
-        kxpu_vfvgpurec &v = w.vts[i];
-        v.flags = KXPU_VT_READ;
-        std::string cur, tab;
-        vfVgpuReads++;
-        if (readVgpuFile(basePath, bdf, "current_vgpu_type", cur)) {
-            memcpy(v.cur_txt, cur.data(), std::min(cur.size(), sizeof v.cur_txt));
-            v.cur_len = (uint8_t)std::min<size_t>(cur.size(), sizeof v.cur_txt + 1);
-        } else {
-            v.flags |= KXPU_VT_CUR_ERR;
-        }
+        readCurrentType(*this, bdf, w.vts[i]);
+        std::string tab;
         vfVgpuReads++;
         if (readVgpuFile(basePath, bdf, "creatable_vgpu_types", tab)) {
             if (tab.size() > KXPU_VGPU_FILE_MAX)
@@ -638,8 +643,10 @@ Error Plugin::gatherVfVgpu(PciWalk &w) {
     return e;
 }
 
-// vfVgpu with draDriver, or on a vGPU class, and vgpuDraDriver without vfVgpu: refused, naming the class
+// vfVgpuHealth without a vfVgpu class; vfVgpu with draDriver, or on a vGPU class, and vgpuDraDriver without vfVgpu:
+// refused, naming the class
 Error Plugin::checkVfVgpuClasses() const {
+    if (vfVgpuHealth && !vfVgpuEnabled()) return fail("vfVgpuHealth is set but no class has vfVgpu");
     for (const XpuClass &c : xpuClasses)
         if (c.vfVgpu && !c.draDriver.empty())
             return fail("class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + "): vfVgpu cannot be published as DRA ResourceSlices (draDriver " + c.draDriver + ")");
@@ -1094,6 +1101,7 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
             const uint32_t first = c.gmem[c.goff[g]];
             s.dra = draRecord(w.recs[first], w.paths.size() > first ? &w.paths[first] : nullptr, c.gnuma[g]);
         }
+        if (vfVgpuHealth && xpuClasses[s.klass].vfVgpu && !w.physfn.empty()) s.pf = w.physfn[c.gmem[c.goff[g]]];
         iommuMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
         iommuState.push_back(std::move(s));
     }
@@ -2234,7 +2242,8 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         bool same = cur.size() == w.devs.size();
         for (size_t i = 0; same && i < cur.size(); i++)
             same = cur[i].ID == w.devs[i].ID && cur[i].Health == w.devs[i].Health && cur[i].numa == w.devs[i].numa &&
-                   cur[i].pcieNode == w.devs[i].pcieNode && cur[i].blocker == w.devs[i].blocker && cur[i].aer == w.devs[i].aer;
+                   cur[i].pcieNode == w.devs[i].pcieNode && cur[i].blocker == w.devs[i].blocker && cur[i].aer == w.devs[i].aer &&
+                   cur[i].drift == w.devs[i].drift;
         if (!same || devicePlugins[at].nodes != w.nodes) {  // changed cdev nodes: the watcher must follow them
             cur = std::move(w.devs);
             devicePlugins[at].nodes = std::move(w.nodes);
@@ -2258,7 +2267,9 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     for (size_t k : report.changedPlugins) (devicePlugins[k].vgpu ? vgpuChanged : passthroughChanged) = true;
     bool aerPt = false, aerVg = false;
     updateAerTaints(aerPt, aerVg);
-    if (passthroughChanged || viabilityChanged || aerPt) pci_.draGeneration++;  // the next publication replaces these slices
+    const bool driftCleared = !driftTaint_.empty();  // the walk is the new truth: every drift reason is gone
+    driftTaint_.clear();
+    if (passthroughChanged || viabilityChanged || aerPt || driftCleared) pci_.draGeneration++;  // the next publication replaces these slices
     if (vgpuChanged || aerVg) mdev_.draGeneration++;
     // 6. a fresh snapshot generation: Allocate answers from the snapshot again
     pci_.haveGen = haveGen;
@@ -2429,6 +2440,10 @@ static const char *kDraTaintEffect = "NoSchedule";
 // group carries at most one of them.
 static const char *kAerTaintKeyName = "/pcie-aer";  // the key is <draDriver>/pcie-aer
 
+// With vfVgpuHealth, a VF-vGPU pool's table has a fourth entry: the VF no longer carries the type it is published with.
+static const char *kTypeTaintKeyName = "/vgpu-type";  // the key is <vgpuDraDriver>/vgpu-type
+static const char *kTypeTaintValue = "changed";
+
 // f(group id, state) for every group of a walk (map, states, the walk's class list) that is published in its class's
 // pool, in walk order: the group has a ResourceSlice record, its class a draDriver, and it has no blocker.  Only a
 // published group gets taints.
@@ -2453,13 +2468,15 @@ Error Plugin::draSlices(int32_t (*fn)(kxpu_ctx *, const char *, const char *, co
                                       const kxpu_dra_taint *, size_t, const int64_t *, uint8_t *, size_t, size_t *, uint64_t *,
                                       size_t *),
                         const char *what, const std::string &driver, uint64_t generation, const std::vector<Rec> &devs,
-                        const std::vector<std::string> &groups, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) const {
-    const std::string missing = driver + kDraTaintKeyName, aer = driver + kAerTaintKeyName;
-    const kxpu_dra_taint table[3] = {{missing.c_str(), kDraTaintValue, kDraTaintEffect},
+                        const std::vector<std::string> &groups, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff,
+                        bool typeTaint) const {
+    const std::string missing = driver + kDraTaintKeyName, aer = driver + kAerTaintKeyName, type = driver + kTypeTaintKeyName;
+    const kxpu_dra_taint table[4] = {{missing.c_str(), kDraTaintValue, kDraTaintEffect},
                                      {aer.c_str(), "fatal", kDraTaintEffect},
-                                     {aer.c_str(), "nonfatal", kDraTaintEffect}};
-    const size_t nt = aerHealth ? 3 : 1;
-    const std::vector<int64_t> since = draTaints ? draSinceTable(groups) : std::vector<int64_t>();
+                                     {aer.c_str(), "nonfatal", kDraTaintEffect},
+                                     {type.c_str(), kTypeTaintValue, kDraTaintEffect}};
+    const size_t nt = typeTaint ? 4 : aerHealth ? 3 : 1;
+    const std::vector<int64_t> since = draTaints ? draSinceTable(groups, typeTaint) : std::vector<int64_t>();
     const int64_t *ts = draTaints ? since.data() : nullptr;  // NULL: the untainted slices
     size_t len = 0, nSlices = 0;
     int32_t rc = fn(ctx_, driver.c_str(), nodeName.c_str(), nodeName.c_str(), generation, devs.data(), devs.size(), table, nt,
@@ -2499,16 +2516,19 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
                      groups, out, sliceOff);
 }
 
-std::vector<int64_t> Plugin::draSinceTable(const std::vector<std::string> &groups) const {
+std::vector<int64_t> Plugin::draSinceTable(const std::vector<std::string> &groups, bool typeTaint) const {
     std::vector<int64_t> since;
     for (const std::string &g : groups) {
         auto it = draTaintSince_.find(g);
         since.push_back(it == draTaintSince_.end() ? -1 : it->second);
-        if (!aerHealth) continue;
-        auto at = aerTaint_.find(g);
+        if (!aerHealth && !typeTaint) continue;
+        auto at = aerTaint_.find(g);  // empty without aerHealth
         const uint8_t v = at == aerTaint_.end() ? 0 : at->second.first;
         since.push_back(v == KXPU_AER_FATAL ? at->second.second : -1);
         since.push_back(v == KXPU_AER_NONFATAL ? at->second.second : -1);
+        if (!typeTaint) continue;
+        auto dt = driftTaint_.find(g);
+        since.push_back(dt == driftTaint_.end() ? -1 : dt->second);
     }
     return since;
 }
@@ -2518,12 +2538,14 @@ Error Plugin::computeAer() {
     for (auto &s : iommuState) set(s, std::string(), 0);
     for (auto &s : mdevState) set(s, std::string(), 0);
     if (!aerHealth) return Error();  // no aer_dev_* file is opened
-    // one record per member of every group, passthrough groups then vGPU groups; a vGPU reads its parent's files
+    // one record per member of every group, passthrough groups then vGPU groups; a vGPU reads its parent's files.  With
+    // vfVgpuHealth a group whose first member is a VF of a vfVgpu class has its PF as one more member, one record per PF.
     std::string text;
     std::vector<uint64_t> off;
     std::vector<uint32_t> len, goff{0}, members;
     std::vector<std::string> who;  // the function whose files record i read
-    auto read = [&](const std::string &base, const std::string &entry, const std::string &fn) {
+    std::map<std::string, uint32_t> pfRecord;  // PF address -> its record
+    auto read = [&](const std::string &base, const std::string &entry, const std::string &fn) {  // the new record's index
         for (const char *name : {"aer_dev_fatal", "aer_dev_nonfatal"}) {
             std::string s;
             aerReads++;
@@ -2533,15 +2555,21 @@ Error Plugin::computeAer() {
             len.push_back((uint32_t)s.size());
             text += s;
         }
-        members.push_back((uint32_t)who.size());
         who.push_back(fn);
+        return (uint32_t)(who.size() - 1);
     };
-    for (const auto &kv : iommuMap) {
-        for (const NvidiaGpuDevice &d : kv.second) read(basePath, d.addr, d.addr);
+    for (size_t g = 0; g < iommuMap.size(); g++) {
+        for (const NvidiaGpuDevice &d : iommuMap[g].second) members.push_back(read(basePath, d.addr, d.addr));
+        const std::string &pf = iommuState[g].pf;  // set only under vfVgpuHealth
+        if (!pf.empty()) {
+            auto it = pfRecord.find(pf);
+            if (it == pfRecord.end()) it = pfRecord.emplace(pf, read(basePath, pf, pf)).first;
+            members.push_back(it->second);
+        }
         goff.push_back((uint32_t)members.size());
     }
     for (const auto &kv : mdevMap) {
-        for (const MdevDevice &m : kv.second) read(mdevBasePath, m.uuid + "/..", m.parent);
+        for (const MdevDevice &m : kv.second) members.push_back(read(mdevBasePath, m.uuid + "/..", m.parent));
         goff.push_back((uint32_t)members.size());
     }
     const size_t n = who.size(), G = goff.size() - 1;
@@ -2614,6 +2642,74 @@ Error Plugin::refreshAerHealth(std::vector<size_t> &changedPlugins, bool &passth
     return Error();
 }
 
+Error Plugin::refreshVfVgpuTypes(std::vector<size_t> &changedPlugins, bool &passthroughMoved, bool &typesMoved) {
+    std::unique_lock<std::shared_mutex> lock(mu_);
+    changedPlugins.clear();
+    passthroughMoved = typesMoved = false;
+    if (!vfVgpuHealth) return Error();
+    // the groups that vfVgpu plugins serve, in plugin order, each once; one record and one one-member group per VF
+    const std::map<std::string, size_t> at = positions(iommuMap);
+    std::vector<size_t> groups;
+    std::set<size_t> seen;
+    for (const GenericDevicePlugin &dp : devicePlugins) {
+        if (dp.vgpu || !xpuClasses[dp.xpuClass].vfVgpu) continue;
+        for (const Device &d : dp.devs) {
+            auto it = at.find(d.ID);
+            if (it != at.end() && !iommuMap[it->second].second.empty() && seen.insert(it->second).second) groups.push_back(it->second);
+        }
+    }
+    const size_t n = groups.size();
+    kxpu_vfvgpurec zero;
+    memset(&zero, 0, sizeof zero);
+    std::vector<kxpu_vfvgpurec> recs(n, zero);
+    std::vector<uint32_t> was(n), goff(n + 1, 0), members(n), typeNow(n + 1), first(n + 1);
+    std::vector<uint8_t> status(n + 1);
+    for (size_t k = 0; k < n; k++) {
+        const NvidiaGpuDevice &vf = iommuMap[groups[k]].second.front();
+        readCurrentType(*this, vf.addr, recs[k]);
+        was[k] = vf.vgpuType;
+        members[k] = (uint32_t)k;
+        goff[k + 1] = (uint32_t)(k + 1);
+    }
+    if (n) {
+        const int32_t rc = kxpu_vf_vgpu_drift(ctx_, recs.data(), was.data(), n, goff.data(), members.data(), n, typeNow.data(),
+                                              status.data(), first.data());
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_vf_vgpu_drift", rc);
+    }
+    for (GroupState<kxpu_dradev> &s : iommuState) s.drift.clear();
+    for (size_t k = 0; k < n; k++) {
+        if (first[k] == KXPU_VD_STEADY) continue;
+        const uint32_t i = members[goff[k] + first[k]];
+        const std::string &bdf = iommuMap[groups[k]].second.front().addr, wasText = " (was " + std::to_string(was[i]) + ")";
+        iommuState[groups[k]].drift = status[i] == KXPU_VD_BAD ? bdf + " has an unreadable vGPU type" + wasText
+                                                               : bdf + " now carries vGPU type " + std::to_string(typeNow[i]) + wasText;
+        typesMoved |= status[i] == KXPU_VD_CHANGED;
+    }
+    for (size_t k = 0; k < devicePlugins.size(); k++) {
+        if (devicePlugins[k].vgpu) continue;
+        bool moved = false;
+        for (Device &d : devicePlugins[k].devs) {
+            auto it = at.find(d.ID);
+            const std::string &reason = it == at.end() ? std::string() : iommuState[it->second].drift;
+            moved |= d.drift.empty() != reason.empty();  // ListAndWatch sends health, not the reason
+            d.drift = reason;
+        }
+        if (moved) changedPlugins.push_back(k);
+    }
+    if (!draTaints) return Error();
+    const int64_t t = now ? now() : (int64_t)time(nullptr);
+    std::map<std::string, int64_t> next;
+    forPublishedVfVgpu(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const GroupState<kxpu_dradev> &s) {
+        auto it = driftTaint_.find(g);
+        const bool had = it != driftTaint_.end(), has = !s.drift.empty();
+        if (has) next[g] = had ? it->second : t;  // the time the drift was first seen, kept while it lasts
+        passthroughMoved |= had != has;
+    });
+    driftTaint_ = std::move(next);
+    if (passthroughMoved) pci_.draGeneration++;
+    return Error();
+}
+
 Error Plugin::refreshDraHealth(bool &passthroughMoved, bool &vgpuMoved) {
     std::unique_lock<std::shared_mutex> lock(mu_);
     passthroughMoved = vgpuMoved = false;
@@ -2666,7 +2762,7 @@ Error Plugin::VfVgpuResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, s
         groups.push_back(g);
     });
     return draSlices(kxpu_dra_slices_vf_vgpu, "kxpu_dra_slices_vf_vgpu", xpuClasses[xpuClass].vgpuDraDriver,
-                     pci_.draGeneration, devs, groups, out, sliceOff);
+                     pci_.draGeneration, devs, groups, out, sliceOff, vfVgpuHealth);
 }
 
 Error Plugin::PrepareDraDevices(const std::string &driver, const std::string &pool, const std::vector<std::string> &deviceNames,
@@ -2691,6 +2787,8 @@ Error Plugin::PrepareDraDevices(const std::string &driver, const std::string &po
             } else {
                 const GroupState<kxpu_dradev> *s = stateOf(iommuMap, iommuState, g);
                 found = s && s->klass == cls;
+                if (found && !s->drift.empty())  // vfVgpuHealth: the profile the claim asked for is gone
+                    return fail("PrepareDraDevices: device " + name + " no longer carries its published vGPU type: " + s->drift);
             }
             if (!found) return fail("PrepareDraDevices: unknown device " + name + " in pool " + pool);
             // refused even when the claim tolerates the taint: the device node is missing, so the VM cannot start
@@ -2718,7 +2816,8 @@ Error Plugin::ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8
     std::vector<uint64_t> masks;
     for (const Device &d : dp.devs) {
         groups.push_back((uint32_t)strtoul(d.ID.c_str(), nullptr, 10));
-        healthy.push_back(d.Health == kHealthy && d.blocker.empty() && d.aer.empty());  // nor one whose link reports errors
+        // nor one whose link reports errors, nor a VF whose vGPU type changed
+        healthy.push_back(d.Health == kHealthy && d.blocker.empty() && d.aer.empty() && d.drift.empty());
         masks.push_back(d.numa);
     }
     // topologyAware: Device.topology from each device's mask (the HealthWatcher's re-sends come through here too)
@@ -3880,6 +3979,31 @@ int kxh_devs_aer(void *h, int plugin_index, char *out, size_t cap) {
     for (const auto &d : p->devicePlugins[(size_t)plugin_index].devs) {
         if (!o.empty()) o += ',';
         o += d.ID + "=" + d.aer;
+    }
+    return copy_out(o, out, cap);
+}
+
+// ---- health of vGPUs on SR-IOV VFs (kxpu_vf_vgpu_drift)
+void kxh_set_vf_vgpu_health(void *h, int on) { ((Plugin *)h)->vfVgpuHealth = on != 0; }
+// refreshVfVgpuTypes: changed as kxh_refresh_aer_health's; *moved = bit 0 passthroughMoved, bit 1 typesMoved
+int kxh_refresh_vf_vgpu_types(void *h, size_t *changed, size_t cap, size_t *n_changed, int *moved, char *err, size_t errcap) {
+    std::vector<size_t> c;
+    bool pt = false, types = false;
+    device_plugin::Error e = ((Plugin *)h)->refreshVfVgpuTypes(c, pt, types);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    for (size_t k = 0; k < c.size() && k < cap; k++) changed[k] = c[k];
+    *n_changed = c.size();
+    *moved = (pt ? 1 : 0) | (types ? 2 : 0);
+    return 0;
+}
+// "id=<drift reason>,..." of one plugin (an empty reason: the walk's type)
+int kxh_devs_drift(void *h, int plugin_index, char *out, size_t cap) {
+    Plugin *p = (Plugin *)h;
+    if (plugin_index < 0 || (size_t)plugin_index >= p->devicePlugins.size()) return -1;
+    std::string o;
+    for (const auto &d : p->devicePlugins[(size_t)plugin_index].devs) {
+        if (!o.empty()) o += ',';
+        o += d.ID + "=" + d.drift;
     }
     return copy_out(o, out, cap);
 }

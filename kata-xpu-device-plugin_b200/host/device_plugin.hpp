@@ -66,6 +66,9 @@ struct Device {  // pluginapi.Device
     // aerHealth: why the group's PCIe AER counters are over a limit ("<bdf> reported <n> fatal uncorrectable PCIe errors
     // (limit <l>)"), from the last walk or refreshAerHealth; empty = within the limits.  Also sent Unhealthy.
     std::string aer{};
+    // vfVgpuHealth: why the VF's vGPU type is no longer the one the walk saw ("<vf> now carries vGPU type 0 (was 557)"),
+    // from the last refreshVfVgpuTypes; empty = unchanged, and after every rediscover.  Also sent Unhealthy.
+    std::string drift{};
 };
 // pluginapi.DevicePluginOptions (GetDevicePluginOptions, generic_device_plugin.go:253-258)
 struct DevicePluginOptions {
@@ -273,7 +276,8 @@ struct PciWalk {
     std::vector<kxpu_vgpukey> vkeys;
     std::vector<uint32_t> vtype;
     std::vector<uint8_t> vstatus;
-    // vfVgpuDraEnabled only, one per record of vts: the basename of its physfn link (the PF's address); "" = not read
+    // vfVgpuDraEnabled or vfVgpuHealth only, one per record of vts: the basename of its physfn link (the PF's address);
+    // "" = not read
     std::vector<std::string> physfn;
 };
 struct MdevWalk {
@@ -314,6 +318,10 @@ struct GroupState {
     // vfVgpuDraEnabled, a group of a class with a vgpuDraDriver whose first member is a VF that carries a named vGPU type:
     // its VF-vGPU ResourceSlice record; none = unpublished
     std::optional<kxpu_dravfvgpu> vfVgpuDra{};
+    // vfVgpuHealth, a group of a vfVgpu class whose first member is a VF: the PF's address (its physfn basename)
+    std::string pf{};
+    // vfVgpuHealth: the drift reason of the group's first member (Device::drift); empty = its type is the walk's
+    std::string drift{};
 };
 
 class Plugin {
@@ -455,6 +463,15 @@ class Plugin {
     // A seam: tests replace it.  Every call counts in vfVgpuReads.
     std::function<bool(const std::string &base, const std::string &bdf, const std::string &name, std::string &out)> readVgpuFile;
     uint64_t vfVgpuReads = 0;  // nvidia/ files read (tests, metrics)
+    // Health of vGPUs on SR-IOV VFs (include/kxpu.h, kxpu_vf_vgpu_drift).  Refused by InitiateDevicePlugin unless some class
+    // has vfVgpu.  false (default): no file more is opened and every output, generation and counter is as above.  true:
+    //   - refreshVfVgpuTypes re-reads the type of every served VF and withholds one whose type changed;
+    //   - the PCI walk keeps each VF's physfn basename (as vfVgpuDraEnabled does), and with aerHealth the PF's aer_dev_*
+    //     files count as one more member of each group whose first member is a VF of a vfVgpu class: errors that no one
+    //     function owns (a surprise down, a fatal link error, a completion timeout of the GPU) are logged on the PF;
+    //   - with draTaints, a drifted group in a vgpuDraDriver pool carries <vgpuDraDriver>/vgpu-type=changed:NoSchedule,
+    //     a fourth entry of that pool's taint table, and PrepareDraDevices refuses it.
+    bool vfVgpuHealth = false;
     // (type ID, type key) of every vGPU type a walk of this process named: the last name table of kxpu_vf_vgpu_types, so a
     // GPU that became full keeps its names across rediscover
     const std::map<uint32_t, std::string> &learnedVgpuTypes() const { return learnedVgpuTypes_; }
@@ -550,6 +567,15 @@ class Plugin {
     // whose ListAndWatch bytes changed; with draTaints, passthroughMoved / vgpuMoved say which pools' AER taints changed
     // (their generation grew by one).  Without aerHealth nothing is read and nothing changes.
     Error refreshAerHealth(std::vector<size_t> &changedPlugins, bool &passthroughMoved, bool &vgpuMoved);
+    // vfVgpuHealth: re-read nvidia/current_vgpu_type (readVgpuFile) of the VF each vfVgpu plugin device stands for (the
+    // first member of its group; free VFs are not read) and compare it with the walk's type (kxpu_vf_vgpu_drift), under
+    // the exclusive lock.  Writing the file sends no event, so the host calls this on a timer, like refreshAerHealth.  A
+    // VF whose type is cleared, changed or unreadable gets Device::drift and is sent Unhealthy; one that reads back its
+    // walk's type loses it.  changedPlugins: the plugins whose ListAndWatch bytes changed; passthroughMoved: the taints
+    // of a VF-vGPU pool changed (draGeneration grew by one); typesMoved: some served VF carries another non-zero type, so
+    // a rediscover would now move it to that type's resource.  The maps, indices and specs are never rebuilt here.
+    // Without vfVgpuHealth nothing is read and nothing changes.
+    Error refreshVfVgpuTypes(std::vector<size_t> &changedPlugins, bool &passthroughMoved, bool &typesMoved);
     // The ResourceSlices of the vGPUs of vfVgpu class xpuClass (kxpu_dra_slices_vf_vgpu): one pool named nodeName, one
     // device per iommuMap group of the class in walk order whose first member is a VF that carries a named vGPU type,
     // unless the group has a blocker (as ResourceSlices).  The device is described by that VF: its address, type key and
@@ -693,19 +719,24 @@ class Plugin {
     std::map<std::string, int64_t> draTaintSince_;  // draTaints: IOMMU group id -> when its taint was added
     // draTaints && aerHealth: IOMMU group id -> (KXPU_AER_FATAL or KXPU_AER_NONFATAL, when that value was first seen)
     std::map<std::string, std::pair<uint8_t, int64_t>> aerTaint_;
+    // draTaints && vfVgpuHealth: IOMMU group id -> when refreshVfVgpuTypes first saw its VF drift (the vgpu-type taint)
+    std::map<std::string, int64_t> driftTaint_;
     Error computeAer();  // the reads and the kxpu_aer_health call for the current maps, into their states' aer / aerBits
     // aerTaint_ from the last computeAer for the groups the DRA pools publish; which pools' taints changed
     void updateAerTaints(bool &passthroughMoved, bool &vgpuMoved);
-    // per group its time in draTaintSince_, then with aerHealth its pcie-aer=fatal and =nonfatal times; -1: no such taint
-    std::vector<int64_t> draSinceTable(const std::vector<std::string> &groups) const;
+    // per group its time in draTaintSince_, then with aerHealth (or typeTaint) its pcie-aer=fatal and =nonfatal times,
+    // then with typeTaint its time in driftTaint_; -1: no such taint
+    std::vector<int64_t> draSinceTable(const std::vector<std::string> &groups, bool typeTaint) const;
     // one pool's slices of devs, the records of groups, through fn (kxpu_dra_slices_taints or _mdev_taints) with the
-    // table <driver>/unhealthy=vfio-device-missing, then with aerHealth <driver>/pcie-aer=fatal and =nonfatal, all
-    // NoSchedule; without draTaints taint_since is NULL (the untainted bytes)
+    // table <driver>/unhealthy=vfio-device-missing, then with aerHealth <driver>/pcie-aer=fatal and =nonfatal, then with
+    // typeTaint (a VF-vGPU pool under vfVgpuHealth) all three and <driver>/vgpu-type=changed, all NoSchedule; without
+    // draTaints taint_since is NULL (the untainted bytes)
     template <typename Rec>
     Error draSlices(int32_t (*fn)(kxpu_ctx *, const char *, const char *, const char *, uint64_t, const Rec *, size_t,
                                   const kxpu_dra_taint *, size_t, const int64_t *, uint8_t *, size_t, size_t *, uint64_t *, size_t *),
                     const char *what, const std::string &driver, uint64_t generation, const std::vector<Rec> &devs,
-                    const std::vector<std::string> &groups, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff) const;
+                    const std::vector<std::string> &groups, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff,
+                    bool typeTaint = false) const;
     Error checkDraClasses() const;
     void buildMdevDra(const MdevWalk &w);
     void buildVfVgpuDra(const PciWalk &w);
