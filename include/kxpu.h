@@ -71,7 +71,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_FINALIZE 1
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
-#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s and kxpu_sriov's kernels: the slot holds the most recent call's */
+#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s, kxpu_sriov's and kxpu_reset_check's kernels: the slot holds the most recent call's */
 #define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev|_vf_vgpu[_cdev]]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
@@ -1377,6 +1377,85 @@ int32_t kxpu_dra_slices_vf_vgpu(kxpu_ctx *ctx, const char *driver, const char *p
                                 const kxpu_dravfvgpu *devs, size_t n, const kxpu_dra_taint *taints, size_t n_taints,
                                 const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out, size_t cap,
                                 size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
+/* ------------------------------------- resets between tenants (addition to ABI v14) */
+
+/* This call and kxpu_resetrec were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym), as
+ * for kxpu_sriov.  Kata hands an IOMMU group to one VM after another; only a reset between them keeps the next tenant
+ * from inheriting device state, memory contents or a device that cannot initialise again.  It rests on these facts:
+ *   [assumed] vfio-pci resets a function when it is opened and when it is released, with a method the kernel knows for
+ *             it: <bdf>/reset_method (Linux 5.15 and later) lists them, space separated, ending in '\n'; the names are
+ *             flr, af_flr, pm, bus, cxl_bus, device_specific and acpi, and the file is hidden when there is none;
+ *   [assumed] before 5.15 there is no reset_method, and <bdf>/reset exists exactly when the function has some method;
+ *   [assumed] failing a method, vfio-pci resets the function's secondary bus (its "device set") only when every function
+ *             the reset would hit is bound to a VFIO driver and none of them is in use (vfio_pci_dev_set_resettable);
+ *             Kata passes a whole group to one VM, so a set that lies in one group is closed together and reset;
+ *   [assumed] a function whose parent in its PCIe path is a host bridge (a root bus; a VMD domain's bus counts as one)
+ *             has no bridge whose secondary bus could be reset;
+ *   [assumed] a class driver is a VFIO driver (as kxpu_sriov assumes).
+ * Host side: for every record that is a candidate of a passthrough class, the host reads the first KXPU_RESET_FILE_MAX
+ * bytes of <bdf>/reset_method, and only when that file does not exist, whether <bdf>/reset exists; every other record
+ * gets a zero-filled side record.  The host also reads the `driver` link of every entry (and the `iommu_group` link of
+ * an entry bound to a class driver) and the entry link of every entry (kxpu_pcipath). */
+#define KXPU_RESET_FILE_MAX 64  /* the longest list of all seven names is 48 bytes */
+typedef struct kxpu_resetrec {
+    uint8_t txt[KXPU_RESET_FILE_MAX]; /* first KXPU_RESET_FILE_MAX bytes of reset_method                           */
+    uint8_t len;                      /* length of the file (0..KXPU_RESET_FILE_MAX; longer => KXPU_RESET_FILE_MAX+1) */
+    uint8_t flags;                    /* KXPU_RS_*                                                              */
+    uint8_t reserved[14];
+} kxpu_resetrec;                      /* 80 bytes: the kernel reads one with five 16-byte vector loads          */
+#define KXPU_RS_ABSENT   0x01u  /* reset_method does not exist                                                      */
+#define KXPU_RS_READ_ERR 0x02u  /* reading reset_method failed for a reason other than "no such file"                */
+#define KXPU_RS_LEGACY   0x04u  /* with KXPU_RS_ABSENT: <bdf>/reset exists                                           */
+/* Method bits: the allow-list and kxpu_reset_check's per-record methods */
+#define KXPU_RM_FLR             0x01u
+#define KXPU_RM_AF_FLR          0x02u
+#define KXPU_RM_PM              0x04u
+#define KXPU_RM_BUS             0x08u
+#define KXPU_RM_CXL_BUS         0x10u
+#define KXPU_RM_DEVICE_SPECIFIC 0x20u
+#define KXPU_RM_ACPI            0x40u
+#define KXPU_RM_ALL             0x7Fu
+#define KXPU_RM_UNNAMED         0x80u  /* methods only: the legacy reset file, some method whose name is unknown */
+/* kxpu_reset_check's set verdict of a record that is not the index of a blocking record */
+#define KXPU_RESET_SET_OK   0xFFFFFFFFu  /* the bus-reset set is closed by one group                   */
+#define KXPU_RESET_NO_PATH  0xFFFFFFFEu  /* the record's path is unknown                               */
+#define KXPU_RESET_ROOT_BUS 0xFFFFFFFDu  /* the record's parent is a host bridge: it sits on a root bus */
+
+/* Can VFIO reset every member of each group between tenants?  recs / paths / rrs: the n records of a walk, their paths
+ * and side records (same index); rules: the classify call's rule list (only the drivers are read); allow: a mask of
+ * KXPU_RM_* method bits the caller accepts (0 accepts none: only set resets count); group_off / group_members /
+ * n_groups: that call's iommuMap CSR.
+ *   - methods[i]: with KXPU_RS_READ_ERR, or len > KXPU_RESET_FILE_MAX (an over-long file is unknown), 0.  Else with
+ *     KXPU_RS_ABSENT, KXPU_RM_UNNAMED when KXPU_RS_LEGACY is set and 0 otherwise.  Else txt[0..len) with at most one
+ *     trailing '\n' removed, split at every ' ': each piece that is one of the seven names sets its bit; every other
+ *     piece (an unknown name, an empty piece, a piece holding '\n') is ignored, and a name given twice sets its bit once;
+ *   - FUNCTION RESET of i: methods[i] & allow != 0, or methods[i] has KXPU_RM_UNNAMED and allow is KXPU_RM_ALL (the
+ *     name is unknown, so only an allow-list of every method accepts it);
+ *   - CHAIN of i as kxpu_pcie_tree parses it (the same device code); a record with an unknown path has none.
+ *     CLASS-BOUND j: recs[j].driver equals the driver of some rule and j carries none of KXPU_REC_DRIVER_ERR,
+ *     KXPU_REC_IOMMU_ERR and KXPU_REC_IS_DIR.  For a function key B, S(B) = every record (of the walk, not only the
+ *     candidates) whose chain holds B at any depth;
+ *   - set_verdict[i]: KXPU_RESET_NO_PATH without a chain; else, B the last key of its chain, KXPU_RESET_ROOT_BUS when B
+ *     is a host bridge; else the lowest j in S(B) that is not class-bound, if any; else KXPU_RESET_SET_OK when every
+ *     record of S(B) has i's iommu_group; else, with lo / hi the lowest and highest iommu_group in S(B), the lowest j in
+ *     S(B) whose group is lo when i's group is not lo, and hi otherwise.  So the index names a function that keeps the
+ *     set from being closed: a sibling bridge, an unbound function, one on another driver, or one in another group;
+ *   - group_reset[o]: the lowest member i of group o with neither a function reset nor set_verdict[i] ==
+ *     KXPU_RESET_SET_OK (the group's RESET BLOCKER), or KXPU_VIABLE.
+ * KXPU_E_INVALID, and nothing written: ctx, rules, group_off NULL; recs, paths, rrs, methods or set_verdict NULL with
+ * n > 0; group_members NULL with members; group_reset NULL with n_groups > 0; an invalid rule list (kxpu_classify_rules'
+ * checks); allow outside KXPU_RM_ALL; group_off decreasing; a member >= n.  Limit (else KXPU_E_UNSUPPORTED, checked
+ * before any array is read): n and n_groups below 2^28.
+ * GPU: five launches timed under KXPU_T_CLASSIFY -- kxpu_pcie_tree's path parse; one thread per record parses
+ * reset_method and inserts its parent bridge's key into an open-addressing table; one thread per record folds, for every
+ * function key of its chain that is in the table, the lowest record that is not class-bound (atomic min) and the lowest /
+ * highest (iommu_group, index) pair (64-bit atomic min / max); one thread per record reads its verdict from its parent's
+ * slot; one thread per group member lowers the group's blocker with an atomic min. */
+int32_t kxpu_reset_check(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, const kxpu_devrec *recs,
+                         const kxpu_pcipath *paths, const kxpu_resetrec *rrs, size_t n, uint32_t allow,
+                         const uint32_t *group_off /* [n_groups+1] */, const uint32_t *group_members, size_t n_groups,
+                         uint8_t *methods /* [n] */, uint32_t *set_verdict /* [n] */, uint32_t *group_reset /* [n_groups] */);
 
 #ifdef __cplusplus
 }

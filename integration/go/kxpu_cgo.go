@@ -1044,6 +1044,59 @@ func (k *kxpu) sriov(rules []C.kxpu_xpu_rule, recs []C.kxpu_devrec, srs []C.kxpu
 	return pfOf[:n], numvfs[:n], gsriov[:nGroups], err
 }
 
+// Resets between tenants (an addition to ABI v14, detected by symbol).  With resetCheck on, the PCI walk also reads the
+// entry link of every entry (pciPath), the driver link of every entry whose driver the class test did not read (and the
+// iommu_group link of one bound to a class driver), and, for every candidate of a passthrough class, the first
+// KXPU_RESET_FILE_MAX+1 bytes of <bdf>/reset_method, or when that does not exist whether <bdf>/reset exists
+// (resetRecord).  After classify, resetCheck gives each group's reset blocker: a group with one is sent Unhealthy,
+// refused by Allocate and NodePrepareResources, and left out of the CDI spec and every DRA pool, with the reason naming
+// the function (methods[i] != 0: the methods resetMethods does not accept; else setVerdict[i]: a root bus, an unknown
+// path, or the record on its bus that is bound to another driver, unbound, or in another group).
+
+// the kxpu_resetrec of one candidate: text of reset_method (absent: no such file; readErr: any other failure), and
+// legacy: <bdf>/reset exists (read only when reset_method is absent)
+func resetRecord(text []byte, absent, readErr, legacy bool) C.kxpu_resetrec {
+	var r C.kxpu_resetrec
+	for i := 0; i < len(text) && i < len(r.txt); i++ {
+		r.txt[i] = C.uint8_t(text[i])
+	}
+	n := len(text)
+	if n > len(r.txt) {
+		n = len(r.txt) + 1
+	}
+	r.len = C.uint8_t(n)
+	if readErr {
+		r.flags |= C.KXPU_RS_READ_ERR
+	} else if absent {
+		r.flags |= C.KXPU_RS_ABSENT
+		if legacy {
+			r.flags |= C.KXPU_RS_LEGACY
+		}
+	}
+	return r
+}
+
+// the reset verdict of a walk: recs / paths / rrs at the same indices, the rules and CSR (goff, gmem) of its classify call,
+// allow the KXPU_RM_* bits of resetMethods.  methods and setVerdict have one entry per record, greset one per group
+// (C.KXPU_VIABLE: served).
+func (k *kxpu) resetCheck(rules []C.kxpu_xpu_rule, recs []C.kxpu_devrec, paths []C.kxpu_pcipath, rrs []C.kxpu_resetrec,
+	allow uint32, goff, gmem []uint32) (methods []uint8, setVerdict, greset []uint32, err error) {
+	n, nGroups := len(recs), len(goff)-1
+	methods, setVerdict, greset = make([]uint8, n+1), make([]uint32, n+1), make([]uint32, nGroups+1)
+	var r *C.kxpu_devrec
+	var pp *C.kxpu_pcipath
+	var rr *C.kxpu_resetrec
+	if n > 0 {
+		r, pp, rr = &recs[0], &paths[0], &rrs[0]
+	}
+	gm := append(gmem, 0) // a valid pointer for an empty walk
+	err = kxCheck(k.ctx, "kxpu_reset_check", C.kxpu_reset_check(k.ctx, &rules[0], C.size_t(len(rules)), r, pp, rr,
+		C.size_t(n), C.uint32_t(allow), (*C.uint32_t)(unsafe.Pointer(&goff[0])), (*C.uint32_t)(unsafe.Pointer(&gm[0])),
+		C.size_t(nGroups), (*C.uint8_t)(unsafe.Pointer(&methods[0])), (*C.uint32_t)(unsafe.Pointer(&setVerdict[0])),
+		(*C.uint32_t)(unsafe.Pointer(&greset[0]))))
+	return methods[:n], setVerdict[:n], greset[:nGroups], err
+}
+
 // pcieTree with every VF below its PF (pfOf: sriov's)
 func (k *kxpu) pcieTreeSriov(recs []C.kxpu_devrec, paths []C.kxpu_pcipath, goff, gmem []uint32, nGroups int,
 	pfOf []uint32) (gnode, parent []uint32, depth []uint8, err error) {

@@ -99,6 +99,15 @@ VT_READ, VT_CUR_ERR = 1, 2
 VT_NONE, VT_NAMED, VT_UNNAMED, VT_BAD = 0, 1, 2, 3
 VD_SAME, VD_CLEARED, VD_CHANGED, VD_BAD = 0, 1, 2, 3  # kxpu_vf_vgpu_drift's per-record status
 VD_STEADY = 0xFFFFFFFF  # kxpu_vf_vgpu_drift's group_first of a group with no drifted member
+# kxpu_resetrec (resets between tenants, an addition to ABI v14): one per kxpu_devrec, at the same index
+RESET_FILE_MAX = 64
+RESETREC_DTYPE = np.dtype([("txt", "u1", (RESET_FILE_MAX,)), ("len", "u1"), ("flags", "u1"), ("reserved", "u1", (14,))])
+assert RESETREC_DTYPE.itemsize == 80
+RS_ABSENT, RS_READ_ERR, RS_LEGACY = 1, 2, 4
+# method bits, in the order of RESET_METHODS
+RESET_METHODS = ("flr", "af_flr", "pm", "bus", "cxl_bus", "device_specific", "acpi")
+RM_ALL, RM_UNNAMED = 0x7F, 0x80
+RESET_SET_OK, RESET_NO_PATH, RESET_ROOT_BUS = 0xFFFFFFFF, 0xFFFFFFFE, 0xFFFFFFFD
 CDI_FRAG_MIN = 166  # the shortest device fragment of a CDI spec: len // CDI_FRAG_MIN records hold any document (ABI v13)
 
 
@@ -125,7 +134,7 @@ ABI_SYMBOLS = [
     "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev", "kxpu_cdi_emit_mdev_cdev", "kxpu_cdi_parse_mdev_cdev",
     "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu", "kxpu_pcie_tree_mdev",
     "kxpu_cdi_emit_vf_vgpu", "kxpu_cdi_emit_vf_vgpu_cdev", "kxpu_cdi_parse_vf_vgpu", "kxpu_cdi_parse_vf_vgpu_cdev",
-    "kxpu_dra_slices_vf_vgpu", "kxpu_vf_vgpu_drift",
+    "kxpu_dra_slices_vf_vgpu", "kxpu_vf_vgpu_drift", "kxpu_reset_check",
 ]
 
 
@@ -247,6 +256,7 @@ def load_library():
         "kxpu_sriov": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp, sz, vp, vp, vp]),
         "kxpu_vf_vgpu_types": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp]),
         "kxpu_vf_vgpu_drift": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp]),
+        "kxpu_reset_check": (i32, [vp, vp, sz, vp, vp, vp, sz, C.c_uint32, vp, vp, sz, vp, vp, vp]),
         "kxpu_classify_vf_vgpu": (i32, [vp, vp, sz, C.c_uint32, vp, sz, vp, C.POINTER(ClassifyOut), vp, vp, vp]),
         "kxpu_pcie_tree_sriov": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32), vp]),
         "kxpu_pcie_tree_mdev": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32)]),
@@ -686,6 +696,23 @@ class Kxpu:
         self._chk(self.L.kxpu_vf_vgpu_drift(self.ctx, _ptr(recs_vt) if n else None, _ptr(was) if n else None, n, _ptr(goff),
                                             _ptr(gmem) if len(gmem) else None, G, _ptr(now), _ptr(st), _ptr(first)))
         return dict(type_now=now[:n], status_now=st[:n], group_first=first[:G])
+
+    def reset_check(self, rules, recs, paths, rrs, allow, group_off, group_members):
+        """kxpu_reset_check: recs (DEVREC_DTYPE), paths (PCIPATH_DTYPE) and rrs (RESETREC_DTYPE) at the same indices, the
+        rules and group CSR of a classify call, allow a mask of method bits.  Returns dict(methods, set_verdict,
+        group_reset (VIABLE: every member can be reset))."""
+        ra = rules_array(rules)
+        recs, paths, rrs = np.ascontiguousarray(recs), np.ascontiguousarray(paths), np.ascontiguousarray(rrs)
+        assert recs.dtype == DEVREC_DTYPE and paths.dtype == PCIPATH_DTYPE and rrs.dtype == RESETREC_DTYPE
+        assert len(recs) == len(paths) == len(rrs)
+        goff = np.ascontiguousarray(group_off, dtype=np.uint32)
+        gmem = np.ascontiguousarray(group_members, dtype=np.uint32)
+        n, G = len(recs), len(goff) - 1
+        meth, sv, gr = np.zeros(max(n, 1), np.uint8), np.zeros(max(n, 1), np.uint32), np.zeros(max(G, 1), np.uint32)
+        self._chk(self.L.kxpu_reset_check(self.ctx, _ptr(ra) if len(ra) else None, len(ra), _ptr(recs) if n else None,
+                                          _ptr(paths) if n else None, _ptr(rrs) if n else None, n, allow, _ptr(goff),
+                                          _ptr(gmem) if len(gmem) else None, G, _ptr(meth), _ptr(sv), _ptr(gr)))
+        return dict(methods=meth[:n], set_verdict=sv[:n], group_reset=gr[:G])
 
     def classify_vf_vgpu(self, rules, vgpu_rules, recs, keys, topo=False, viable=False):
         """kxpu_classify_vf_vgpu: the dict of classify_rules, plus group_numa (topo) and group_blocker (viable).  keys:

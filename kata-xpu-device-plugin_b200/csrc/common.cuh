@@ -102,6 +102,11 @@ uint32_t kx_next_epoch(kxpu_ctx *ctx);
 // NUL: drv[r] = {d0, d1, m0, m1}, and a 16-byte driver field f matches rule r when (f0 & m0) == d0 && (f1 & m1) == d1
 int32_t kx_rule_drivers(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, unsigned long long drv[][4]);
 
+// kxpu_pcie_tree's path parse (pcie.cu), for the calls that need the chains of a walk: one launch on st over n device
+// records and paths; chain[i * KXPU_PCIE_MAX_DEPTH + t] = key t of record i's chain, clen[i] its length (0: unknown)
+void kx_pcie_parse(cudaStream_t st, const kxpu_devrec *recs, const kxpu_pcipath *paths, uint32_t n, unsigned long long *chain,
+                   uint8_t *clen);
+
 // stream-ordered scratch that is released on every path out of a call
 struct KxScratch {
     kxpu_ctx *c;

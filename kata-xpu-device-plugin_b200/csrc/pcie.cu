@@ -298,6 +298,11 @@ __global__ void __launch_bounds__(256) k_emit(const Tree T) {
 
 using namespace kxpcie;
 
+void kx_pcie_parse(cudaStream_t st, const kxpu_devrec *recs, const kxpu_pcipath *paths, uint32_t n, unsigned long long *chain,
+                   uint8_t *clen) {
+    k_parse<kxpu_devrec, false><<<(n + PARSE_RECS - 1) / PARSE_RECS, PARSE_THREADS, 0, st>>>(recs, paths, n, chain, clen, nullptr);
+}
+
 // Rec = kxpu_devrec: pf_of == nullptr: kxpu_pcie_tree; else kxpu_pcie_tree_sriov (pf_of checked by the caller).
 // Rec = kxpu_mdevrec: kxpu_pcie_tree_mdev (pf_of == nullptr).
 template <typename Rec>

@@ -114,6 +114,28 @@ static bool readVgpuFileFunc(const std::string &base, const std::string &bdf, co
     return true;
 }
 
+// reset_method: its first KXPU_RESET_FILE_MAX + 1 bytes; reset: whether it exists (the file is write-only)
+static bool readResetFileFunc(const std::string &base, const std::string &bdf, const std::string &name, std::string &out) {
+    const std::string path = base + "/" + bdf + "/" + name;
+    out.clear();
+    if (name == "reset") {
+        struct stat sb;
+        return stat(path.c_str(), &sb) == 0;
+    }
+    FILE *f = fopen(path.c_str(), "rb");
+    if (!f) return false;
+    char buf[KXPU_RESET_FILE_MAX + 1];
+    const size_t n = fread(buf, 1, sizeof buf, f);
+    const bool err = ferror(f) != 0;
+    fclose(f);
+    if (err) {
+        errno = EIO;
+        return false;
+    }
+    out.assign(buf, n);
+    return true;
+}
+
 // the numa_node rule of include/kxpu.h: one trailing '\n' stripped, then a canonical decimal 0..63
 static bool parseNumaNode(const std::string &raw, uint8_t &node) {
     std::string s = raw;
@@ -170,6 +192,7 @@ Plugin::Plugin(kxpu_ctx *ctx) : ctx_(ctx) {
     readNumaNode = readNumaNodeFunc;
     readAerFile = readAerFileFunc;
     readVgpuFile = readVgpuFileFunc;
+    readResetFile = readResetFileFunc;
     readPciPath = readPciPathFunc;
     readLink = readLinkFunc;
     readIDFromFile = readIDFromFileFunc;
@@ -534,6 +557,44 @@ void Plugin::readSriovs(const std::vector<kxpu_devrec> &recs, std::vector<kxpu_s
         const kxpu_devrec &r = recs[i];
         if (!(r.flags & KXPU_REC_IOMMU_ERR) && cdevClassOf(xpuClasses, nullptr, r, r.vendor_txt, sizeof r.vendor_txt))
             (*srs)[i] = readSriov(std::string(r.bdf, strnlen(r.bdf, sizeof r.bdf)));
+    }
+}
+
+static bool isClassDriver(const std::vector<XpuClass> &classes, const std::string &driver);
+
+void Plugin::readResets(std::vector<kxpu_devrec> &recs, std::vector<kxpu_resetrec> &rrs) {
+    rrs.clear();
+    if (!resetCheck) return;
+    kxpu_resetrec zero;
+    memset(&zero, 0, sizeof zero);
+    rrs.assign(recs.size(), zero);
+    for (size_t i = 0; i < recs.size(); i++) {
+        kxpu_devrec &r = recs[i];
+        if (r.flags & KXPU_REC_IS_DIR) continue;
+        const std::string bdf(r.bdf, strnlen(r.bdf, sizeof r.bdf));
+        std::string s;
+        if (!r.driver[0] && !(r.flags & KXPU_REC_DRIVER_ERR) && readLink(basePath, bdf, "driver", s))  // the class test
+            memcpy(r.driver, s.data(), std::min(s.size(), sizeof r.driver - 1));  // did not need it: bus-reset sets do
+        const std::string drv(r.driver, strnlen(r.driver, sizeof r.driver));
+        const bool candidate = cdevClassOf(xpuClasses, nullptr, r, r.vendor_txt, sizeof r.vendor_txt);
+        if (!candidate && !(r.flags & KXPU_REC_BLOCKS) && isClassDriver(xpuClasses, drv)) {  // its group is not known yet
+            uint32_t g = 0;
+            if (readLink(basePath, bdf, "iommu_group", s) && parseGroup(s, g)) r.iommu_group = g;
+            else r.flags |= KXPU_REC_IOMMU_ERR;
+        }
+        if (!candidate || (r.flags & KXPU_REC_IOMMU_ERR)) continue;
+        kxpu_resetrec &rr = rrs[i];
+        resetReads++;
+        if (readResetFile(basePath, bdf, "reset_method", s)) {
+            memcpy(rr.txt, s.data(), std::min(s.size(), sizeof rr.txt));
+            rr.len = (uint8_t)std::min<size_t>(s.size(), sizeof rr.txt + 1);
+        } else if (errno != ENOENT) {
+            rr.flags |= KXPU_RS_READ_ERR;
+        } else {
+            rr.flags |= KXPU_RS_ABSENT;
+            resetReads++;
+            if (readResetFile(basePath, bdf, "reset", s)) rr.flags |= KXPU_RS_LEGACY;
+        }
     }
 }
 
@@ -984,10 +1045,57 @@ static std::string sriovReasonOf(const std::vector<XpuClass> &classes, const Pci
     return sriovPfReason(me, w.numvfs[i]);
 }
 
+static const char *const kResetMethods[7] = {"flr", "af_flr", "pm", "bus", "cxl_bus", "device_specific", "acpi"};
+
+// resetMethods as KXPU_RM_* bits (checkResetMethods refused every other name)
+uint32_t Plugin::resetAllow() const {
+    uint32_t allow = 0;
+    for (const std::string &m : resetMethods)
+        for (uint32_t k = 0; k < 7; k++)
+            if (m == kResetMethods[k]) allow |= 1u << k;
+    return allow;
+}
+
+Error Plugin::checkResetMethods() const {
+    std::set<std::string> seen;
+    for (const std::string &m : resetMethods) {
+        if (std::find(std::begin(kResetMethods), std::end(kResetMethods), m) == std::end(kResetMethods))
+            return fail("resetMethods: " + m + " is not a reset method (flr, af_flr, pm, bus, cxl_bus, device_specific, acpi)");
+        if (!seen.insert(m).second) return fail("resetMethods: " + m + " is listed twice");
+    }
+    return Error();
+}
+
+// why kxpu_reset_check found record i of a walk without a reset: the methods it has that resetMethods does not accept,
+// else the function that keeps its bus-reset set from being closed
+std::string Plugin::resetReasonOf(const PciWalk &w, uint32_t i) const {
+    const std::string me(w.recs[i].bdf, strnlen(w.recs[i].bdf, sizeof w.recs[i].bdf));
+    const uint8_t m = w.rmeth[i];
+    if (m & KXPU_RM_UNNAMED) return me + " has no reset method in resetMethods (reset: some method, name unknown)";
+    if (m) {
+        std::string names;
+        for (uint32_t k = 0; k < 7; k++)
+            if (m & (1u << k)) names += (names.empty() ? "" : " ") + std::string(kResetMethods[k]);
+        return me + " has no reset method in resetMethods (reset_method: " + names + ")";
+    }
+    const uint32_t v = w.rset[i];
+    if (v == KXPU_RESET_ROOT_BUS) return me + " has no function reset and sits on a root bus";
+    if (v == KXPU_RESET_NO_PATH) return me + " has no function reset and its PCIe path is unknown";
+    const kxpu_devrec &r = w.recs[v];
+    const std::string other(r.bdf, strnlen(r.bdf, sizeof r.bdf)), drv(r.driver, strnlen(r.driver, sizeof r.driver));
+    std::string why;
+    if (drv.empty() || (r.flags & KXPU_REC_DRIVER_ERR)) why = "is not bound to a driver";
+    else if (!isClassDriver(xpuClasses, drv)) why = "is bound to " + drv;
+    else if (r.flags & KXPU_REC_IOMMU_ERR) why = "has no IOMMU group";
+    else why = "is in IOMMU group " + std::to_string(r.iommu_group);
+    return me + " has no function reset and " + other + " on its bus " + why;  // v != i: a member is class-bound
+}
+
 // the walk and classify of createIommuDeviceMap
 Error Plugin::classify(PciWalk &w) {
     Error e = gatherRecordsFast(w.recs, 0, &w.paths, &w.cdevs, &w.srs);  // same records as gatherRecords (falls back to it when a seam was replaced)
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // Walk's error is ignored by the reference (:132)
+    readResets(w.recs, w.rrs);
     const std::vector<kxpu_devrec> &recs = w.recs;
     const size_t n = recs.size();
     ClassifyResult &c = w.out;
@@ -1044,6 +1152,17 @@ Error Plugin::classify(PciWalk &w) {
             if (w.gsriov[g] != KXPU_VIABLE)
                 fprintf(stderr, "IOMMU group %u is not served: %s\n", c.gids[g], sriovReasonOf(whole, w, w.gsriov[g]).c_str());
     }
+    if (resetCheck) {  // every member's function reset or bus-reset set, on the classify CSR
+        w.rmeth.assign(n ? n : 1, 0);
+        w.rset.assign(n ? n : 1, KXPU_RESET_SET_OK);
+        w.greset.assign(c.nGroups + 1, KXPU_VIABLE);
+        rc = kxpu_reset_check(ctx_, rules.data(), rules.size(), recs.data(), w.paths.data(), w.rrs.data(), n, resetAllow(),
+                              c.goff.data(), c.gmem.data(), c.nGroups, w.rmeth.data(), w.rset.data(), w.greset.data());
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_reset_check", rc);
+        for (uint32_t g = 0; g < c.nGroups; g++)
+            if (w.greset[g] != KXPU_VIABLE)
+                fprintf(stderr, "IOMMU group %u is not served: %s\n", c.gids[g], resetReasonOf(w, w.greset[g]).c_str());
+    }
     if (pcieTopologyAware) {  // the forest of the walk, one node per group; sriovAware: VFs below their PF
         const size_t cap = (size_t)KXPU_PCIE_MAX_DEPTH * c.nGroups + 1;
         w.gnode.assign(c.nGroups + 1, KXPU_PCIE_NO_NODE);
@@ -1096,6 +1215,10 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
                 if (!k.vfVgpu) whole.push_back(k);
             s.sriov = sriovReasonOf(whole, w, w.gsriov[g]);
             if (s.blocker.empty()) s.blocker = s.sriov;
+        }
+        if (resetCheck && w.greset[g] != KXPU_VIABLE) {
+            s.reset = resetReasonOf(w, w.greset[g]);
+            if (s.blocker.empty()) s.blocker = s.reset;
         }
         if (draEnabled()) {
             const uint32_t first = c.gmem[c.goff[g]];
@@ -1784,10 +1907,11 @@ Error Plugin::generateClassSpecs(const std::vector<XpuClass> &classes, const Ord
 Error Plugin::generateCDISpec(const OrderedMap<std::vector<NvidiaGpuDevice>> &m, const std::string &format) {
     cdiFiles.clear();
     std::map<std::string, size_t> classOf;  // group -> class, from the maps of the last walk
-    std::set<std::string> withheld;  // sriovAware: a group with an SR-IOV reason, which VFIO would refuse to open
+    // sriovAware: a group with an SR-IOV reason, which VFIO would refuse to open; resetCheck: one VFIO cannot reset
+    std::set<std::string> withheld;
     for (size_t g = 0; g < iommuMap.size(); g++) {
         classOf.emplace(iommuMap[g].first, iommuState[g].klass);
-        if (!iommuState[g].sriov.empty()) withheld.insert(iommuMap[g].first);
+        if (!iommuState[g].sriov.empty() || !iommuState[g].reset.empty()) withheld.insert(iommuMap[g].first);
     }
     OrderedMap<std::vector<NvidiaGpuDevice>> served;  // m without them (only built when some group is withheld)
     std::vector<size_t> entryClass;
@@ -1946,6 +2070,7 @@ Error Plugin::checkDraClasses() const {
 Error Plugin::InitiateDevicePlugin() {
     Error e = checkDraClasses();
     if (!e) e = checkVfVgpuClasses();
+    if (!e) e = checkResetMethods();
     if (e) return e;
     e = createIommuDeviceMap();  // :46
     if (e) return e;
@@ -3258,6 +3383,54 @@ static void jsnap(std::string &o, const std::vector<kxpu_snaprec> &snap) {
 }
 
 void kxh_set_sriov(void *h, int on) { ((Plugin *)h)->sriovAware = on != 0; }
+
+// ---- resets between tenants (tests)
+// on != 0: resetCheck; methods_csv != NULL replaces resetMethods ("" = none)
+void kxh_set_reset(void *h, int on, const char *methods_csv) {
+    Plugin *p = (Plugin *)h;
+    p->resetCheck = on != 0;
+    if (!methods_csv) return;
+    p->resetMethods.clear();
+    std::string cur;
+    for (const char *c = methods_csv;; c++) {
+        if (*c == ',' || *c == 0) {
+            if (!cur.empty()) p->resetMethods.push_back(cur);
+            cur.clear();
+            if (*c == 0) break;
+        } else {
+            cur += *c;
+        }
+    }
+}
+uint64_t kxh_reset_reads(void *h) { return ((Plugin *)h)->resetReads; }
+
+// CPU only: the raw PCI gather under a class list with resetCheck = on, then the reset reads (Plugin::readResets): the
+// records, their paths and side records, and resetReads.  With on = 0 paths and rrs are zero-filled.
+int kxh_gather_reset(const char *base_path, const char *classes, int on, int fast, unsigned threads, kxpu_devrec *out,
+                     kxpu_pcipath *paths_out, kxpu_resetrec *rrs_out, size_t cap, size_t *n, uint64_t *reads, char *err,
+                     size_t errcap) {
+    Plugin p(nullptr);
+    p.basePath = base_path;
+    p.resetCheck = on != 0;
+    if (!parseClasses(classes, p.xpuClasses)) { copy_out("malformed class list", err, errcap); return -1; }
+    std::vector<kxpu_devrec> recs;
+    std::vector<kxpu_pcipath> paths;
+    std::vector<kxpu_resetrec> rrs;
+    device_plugin::Error e = fast ? p.gatherRecordsFast(recs, threads, &paths) : p.gatherRecords(recs, &paths);
+    if (e) { copy_out(e.message, err, errcap); return -1; }
+    p.readResets(recs, rrs);
+    *n = recs.size();
+    *reads = p.resetReads;
+    if (recs.size() > cap) return -2;
+    memcpy(out, recs.data(), recs.size() * sizeof(kxpu_devrec));
+    for (size_t i = 0; i < recs.size(); i++) {
+        if (paths.size() > i) paths_out[i] = paths[i];
+        else memset(&paths_out[i], 0, sizeof paths_out[i]);
+        if (rrs.size() > i) rrs_out[i] = rrs[i];
+        else memset(&rrs_out[i], 0, sizeof rrs_out[i]);
+    }
+    return 0;
+}
 uint64_t kxh_sriov_reads(void *h) { return ((Plugin *)h)->sriovReads; }
 
 // "id=name;id=name" -> vgpuTypeNames; false for a malformed list

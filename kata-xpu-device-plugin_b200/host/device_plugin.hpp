@@ -269,6 +269,11 @@ struct PciWalk {
     // first blocking member or KXPU_VIABLE
     std::vector<kxpu_sriovrec> srs;
     std::vector<uint32_t> pfOf, numvfs, gsriov;
+    // resetCheck: per record its reset_method (or reset) read, and kxpu_reset_check's methods and set verdict; per group
+    // ordinal the reset blocker or KXPU_VIABLE
+    std::vector<kxpu_resetrec> rrs;
+    std::vector<uint8_t> rmeth;
+    std::vector<uint32_t> rset, greset;
     // some class has vfVgpu: per record its current_vgpu_type read and creatable_vgpu_types text, and kxpu_vf_vgpu_types'
     // key row, type ID and status
     std::vector<kxpu_vfvgpurec> vts;
@@ -312,6 +317,7 @@ struct GroupState {
     // VFIO cdev" (vfioCdev), else sriov; a vGPU group: "<uuid> has no VFIO cdev" (mdevCdev)
     std::string blocker{};
     std::string sriov{};  // sriovAware, passthrough only: the SR-IOV reason; empty = served
+    std::string reset{};  // resetCheck, passthrough only: why a member cannot be reset between tenants; empty = served
     std::string aer{};    // aerHealth: the first member over an AER limit (computeAer); empty = within the limits
     uint8_t aerBits = 0;  // aerHealth: the group's KXPU_AER_* bits (computeAer)
     std::optional<Dra> dra{};  // draEnabled (vgpuDraEnabled): the ResourceSlice record of its first member; none = unpublished
@@ -394,9 +400,9 @@ class Plugin {
     std::string nodeName;
     bool draEnabled() const;  // some class has a draDriver
     // the PCI gathers read numa_node (topologyAware, draEnabled or vfVgpuDraEnabled) and the entry link
-    // (pcieTopologyAware, draEnabled or vfVgpuDraEnabled)
+    // (pcieTopologyAware, draEnabled, vfVgpuDraEnabled or resetCheck)
     bool readsNuma() const { return topologyAware || draEnabled() || vfVgpuDraEnabled(); }
-    bool readsPaths() const { return pcieTopologyAware || draEnabled() || vfVgpuDraEnabled(); }
+    bool readsPaths() const { return pcieTopologyAware || draEnabled() || vfVgpuDraEnabled() || resetCheck; }
     // DRA ResourceSlices of vGPUs on SR-IOV VFs (include/kxpu.h, kxpu_dra_slices_vf_vgpu): a vgpuDraDriver on a vfVgpu
     // class publishes its vGPUs (VfVgpuResourceSlices) in the pool nodeName.  With one set, the PCI gathers read
     // numa_node and the entry link as draEnabled does, and readVfVgpus keeps each VF's physfn basename; nothing else is
@@ -459,6 +465,27 @@ class Plugin {
     // so GetPreferredAllocation packs a request's VFs by PF.
     bool sriovAware = false;
     uint64_t sriovReads = 0;  // functions whose physfn and sriov_numvfs were read (tests, metrics)
+    // Resets between tenants (include/kxpu.h, kxpu_reset_check).  false (default): no reset_method or reset file is opened
+    // and every output, generation and counter is as above.  true: after either gather, the PCI walk reads the entry link
+    // of every entry (as readsPaths), the `driver` link of every entry whose driver is not known yet (and `iommu_group` of
+    // one bound to a class driver), and reset_method of every candidate of a passthrough class, falling back to whether
+    // `reset` exists (kernels before 5.15).  A group with a member that has neither a method in resetMethods nor a
+    // secondary-bus reset VFIO can do (every function below its parent bridge bound to a class driver and in its own
+    // group) goes through the blocker path, with a reason naming the function ("0000:41:00.0 has no reset method in
+    // resetMethods (reset_method: pm)", "... has no function reset and 0000:41:00.1 on its bus is bound to
+    // snd_hda_intel", "... has no function reset and sits on a root bus"): sent Unhealthy, refused by Allocate and
+    // PrepareDraDevices, left out of the CDI spec and every DRA pool.  rediscover reads everything again; Allocate reads
+    // nothing more, since reset_method changes only when an administrator writes to it.  vGPU (mdev) groups are out of
+    // scope: their reset is the vendor driver's.
+    bool resetCheck = false;
+    // the reset methods the plugin accepts: names of reset_method (flr, af_flr, pm, bus, cxl_bus, device_specific, acpi),
+    // each at most once; InitiateDevicePlugin refuses any other.  A kernel without reset_method only counts with all seven.
+    std::vector<std::string> resetMethods{"flr", "af_flr", "pm", "bus", "cxl_bus", "device_specific", "acpi"};
+    // <base>/<bdf>/<name> for name "reset_method" (out: at most KXPU_RESET_FILE_MAX + 1 bytes) or "reset" (only whether
+    // it exists: the file is write-only).  false with errno ENOENT: no such file; false with any other errno: a failed
+    // read.  A seam: tests replace it.  Every call counts in resetReads.
+    std::function<bool(const std::string &base, const std::string &bdf, const std::string &name, std::string &out)> readResetFile;
+    uint64_t resetReads = 0;  // reset_method and reset files opened (tests, metrics)
     // <base>/<bdf>/nvidia/<name>, at most KXPU_VGPU_FILE_MAX + 1 bytes; false: the read failed ("no such file" included).
     // A seam: tests replace it.  Every call counts in vfVgpuReads.
     std::function<bool(const std::string &base, const std::string &bdf, const std::string &name, std::string &out)> readVgpuFile;
@@ -631,6 +658,10 @@ class Plugin {
     // only, else left empty): the walk's parentDevice and pcieRoot, one per record; (readsMdevPaths only, else left
     // empty) its paths; (mdevCdevEnabled only, else left empty) its cdevs
     Error gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w = nullptr);
+    // resetCheck: the reads kxpu_reset_check needs after a gather (no GPU): the driver (and iommu_group) of every entry
+    // that lacks it into recs, and one kxpu_resetrec per record into rrs, zero-filled for a record that is no candidate of
+    // a passthrough class.  Off: rrs is left empty and nothing is read.
+    void readResets(std::vector<kxpu_devrec> &recs, std::vector<kxpu_resetrec> &rrs);
     // the vGPU class list against the passthrough one (distinct CDI kinds and file stems, no vfioCdev on a vGPU class, no
     // mdevCdev on a passthrough class); createMdevMap runs it
     Error checkVgpuClasses() const;
@@ -651,6 +682,10 @@ class Plugin {
     // the classes whose functions are passed through whole: xpuClasses, a vfVgpu class's driver counting as none
     bool passthroughDriver(const std::string &driver) const;
     Error checkVfVgpuClasses() const;
+    // resetMethods against the seven names; InitiateDevicePlugin runs it
+    Error checkResetMethods() const;
+    uint32_t resetAllow() const;  // resetMethods as KXPU_RM_* bits
+    std::string resetReasonOf(const PciWalk &w, uint32_t i) const;  // the reason of kxpu_reset_check's blocker i
     // Allocate's live SR-IOV check of one function: the reason kxpu_sriov's rule now gives, or ""
     std::string sriovLive(const std::string &bdf);
     // one CDI spec per class: the devices of m whose entry has that class (entryClass, same positions as m)

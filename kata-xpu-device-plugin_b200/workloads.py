@@ -813,3 +813,43 @@ def vf_vgpu_cdi_devices(n=1 << 20, seed=63):
     devs["key"] = keys[pick]
     devs["key_len"] = np.array([len(k) for k in keys], np.uint8)[pick]
     return devs
+
+
+def reset_walk(n=1 << 20, seed=71):
+    """n records (DEVREC_DTYPE, bdfs in walk order, one group each) with their kxpu_pcipath and kxpu_resetrec side
+    records, on pcie_walk's board (8 functions per down port; 2 % of the buses behind a VMD domain, 1 % with chains of
+    exactly 8, 1 % of 9 (unknown)).  reset_method: 70 % "flr bus\\n", 15 % "bus\\n", 2 % "pm\\n", 1 % a kernel without
+    reset_method but with reset, 12 % neither file (no method: withheld, since a down port's eight functions lie in eight
+    groups).  Returns (recs, paths, rrs)."""
+    from .binding import PCIPATH_DTYPE, RESETREC_DTYPE, RS_ABSENT, RS_LEGACY
+    rng = np.random.default_rng(seed)
+    recs = np.zeros(n, dtype=DEVREC_DTYPE)
+    bdfs = enumerate_bdfs(n)
+    recs["bdf"] = bdfs.view("S16").reshape(n)
+    recs["driver"] = b"vfio-pci"
+    recs["vendor_txt"] = _id_text(np.full(n, 0x10DE))
+    recs["device_txt"] = _id_text(np.full(n, 0x2330))
+    recs["vendor_len"] = recs["device_len"] = 7
+    recs["iommu_group"] = np.arange(1, n + 1, dtype=np.uint32)
+    i = np.arange(n, dtype=np.int64)
+    dom, bus, dev = i >> 16, (i >> 8) & 255, (i >> 3) & 31
+    bus_kind = rng.choice(4, size=int((n + 255) >> 8), p=[0.96, 0.02, 0.01, 0.01])
+    prefix = {}
+    texts = []
+    for k in range(n):
+        pre = prefix.get(k >> 3)
+        if pre is None:
+            pre = prefix[k >> 3] = _pcie_prefix(int(dom[k]), int(bus[k]), int(dev[k]), int(bus_kind[k >> 8])).encode()
+        texts.append(pre + bytes(bdfs[k][:12]))
+    paths = np.zeros(n, dtype=PCIPATH_DTYPE)
+    paths["path"] = np.array(texts, dtype="S120")
+    paths["len"] = np.array([len(t) for t in texts], np.uint8)
+    rrs = np.zeros(n, dtype=RESETREC_DTYPE)
+    kind = rng.choice(5, size=n, p=[0.70, 0.15, 0.02, 0.01, 0.12])
+    for k, text in enumerate((b"flr bus\n", b"bus\n", b"pm\n")):
+        rows = kind == k
+        rrs["txt"][rows, :len(text)] = np.frombuffer(text, np.uint8)
+        rrs["len"][rows] = len(text)
+    rrs["flags"][kind == 3] = RS_ABSENT | RS_LEGACY
+    rrs["flags"][kind == 4] = RS_ABSENT
+    return recs, paths, rrs

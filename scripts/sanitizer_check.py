@@ -76,6 +76,11 @@ sv = kx.sriov([(b"10de", b"vfio-pci")], srecs, ssrs, sres["group_ids"], sres["gr
 ppf = np.where(np.arange(len(precs)) & 7, np.arange(len(precs)) & ~7, B.NO_PF).astype(np.uint32)
 print("sriov withheld", int((sv["group_sriov"] != B.VIABLE).sum()), "pcie sriov nodes",
       len(kx.pcie_tree(precs, ppaths, poff, pmem, ppf)["key"]))
+# resets between tenants: every member's function reset or bus-reset set, on the classify CSR
+rrecs, rpaths, rrrs = W.reset_walk(20000)
+rres = kx.classify_rules([(b"10de", b"vfio-pci")], rrecs)
+rv = kx.reset_check([(b"10de", b"vfio-pci")], rrecs, rpaths, rrrs, B.RM_ALL, rres["group_off"], rres["group_members"])
+print("reset withheld", int((rv["group_reset"] != B.VIABLE).sum()))
 # vGPUs on VFs: the type join and the per-type classify, with and without blockers
 vrecs_, vvts, vtables = W.vf_vgpu_walk(20000)
 vt = kx.vf_vgpu_types(vvts, vtables)
