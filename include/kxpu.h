@@ -1457,6 +1457,98 @@ int32_t kxpu_reset_check(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rul
                          const uint32_t *group_off /* [n_groups+1] */, const uint32_t *group_members, size_t n_groups,
                          uint8_t *methods /* [n] */, uint32_t *set_verdict /* [n] */, uint32_t *group_reset /* [n_groups] */);
 
+/* ------------------------------------------------- Prometheus metrics (an addition to ABI v14, detected by symbol) */
+
+/* Why a host reports a device Unhealthy, as metrics can be scraped.  The document is the Prometheus text exposition
+ * format, version 0.0.4: UTF-8, '\n' line ends, the last line ending in '\n', no "# EOF" line (that is OpenMetrics').
+ * One sample per line, `name{labels} value`, the value an unsigned decimal.  Each family's "# HELP" and "# TYPE" lines
+ * (KXPU_METRICS_*_HEAD below) come right before its samples, the samples of one family are contiguous, and a family
+ * with no sample is left out, its HELP and TYPE lines included.  kxpu_metrics_devices writes families 1 to 3 in this
+ * order; the host appends its process counters (family 4, KXPU_METRICS_READS_HEAD and KXPU_METRICS_VALIDATIONS_HEAD).
+ *   1. kata_xpu_device_healthy (gauge): one sample per device, in array order,
+ *        kata_xpu_device_healthy{resource="<R>",device="<G>",address="<A>"} <healthy>
+ *      R and A are the device's resource and address strings, G its group as a decimal, healthy 1 or 0;
+ *   2. kata_xpu_device_unhealthy_reason (gauge): one sample per reason entry, devices in array order and each device's
+ *      run of entries in order,
+ *        kata_xpu_device_unhealthy_reason{resource="<R>",device="<G>",address="<A>",reason="<K>",detail="<D>"} 1
+ *      K the kind's name (KXPU_METRICS_REASONS), D the entry's detail string;
+ *   3. kata_xpu_pcie_aer_errors (gauge): per device in array order, one sample for each of aer_fatal and aer_nonfatal
+ *      that is not KXPU_METRICS_NO_VALUE, fatal first,
+ *        kata_xpu_pcie_aer_errors{resource="<R>",device="<G>",address="<A>",severity="fatal|nonfatal"} <count>
+ * LABEL VALUES: every string above (R, A, D) is taken as bytes and repaired to UTF-8 first: a byte sequence that is not
+ * well-formed UTF-8 becomes U+FFFD (EF BF BD), one per maximal subpart (Unicode's recommended practice, which is what
+ * Python's bytes.decode("utf-8", "replace") does); then '\' becomes "\\", '"' becomes "\"" and LF becomes "\n".
+ * No other byte changes.  Two-call sizing as everywhere: *len gets the document's size; out == NULL or cap < *len
+ * returns KXPU_E_NOSPACE with nothing written (n == 0, or a document with no family: KXPU_OK, *len = 0).
+ * KXPU_E_INVALID, with nothing written: ctx or len NULL; devs NULL with n > 0; strings NULL with strings_len > 0;
+ * reasons NULL with n_reasons > 0; a resource, address or detail range [off, off + len) not inside [0, strings_len);
+ * a device's run [reason_off, reason_off + reason_count) not inside [0, n_reasons); healthy other than 0 or 1; a kind at
+ * or above KXPU_MR_COUNT; kinds within one device's run not strictly increasing (out of order or repeated).
+ * KXPU_E_UNSUPPORTED, with nothing written: n at or above 2^28 (checked before any array is read); a resource, address
+ * or detail longer than KXPU_METRICS_STRING_MAX bytes; a document of 2^40 bytes or more.  A document over 2^38 bytes
+ * has its size stored but cannot be staged in device memory: KXPU_E_NOMEM.  The escaping of a device's samples is
+ * bounded by these limits, so every sample length and every sum over one scan tile fits 32 bits.
+ * GPU: three launches timed under KXPU_T_EMIT -- a size pass (one warp per device: each sample's length in each family,
+ * the escaped and repaired widths included, and each family's total), the single-pass exclusive scan over the 3n
+ * lengths in family-major order, which gives every sample its offset (family base plus prefix), and a write pass (one
+ * warp per device, plus the family headers). */
+#define KXPU_MR_VFIO_DEVICE_MISSING 0u /* the health watcher saw the device node go (Health), detail ""         */
+#define KXPU_MR_NOT_VIABLE          1u /* groupViability: a member bound to a driver VFIO cannot share the group */
+#define KXPU_MR_VFIO_CDEV_MISSING   2u /* vfioCdev / mdevCdev: a member without a VFIO cdev                      */
+#define KXPU_MR_SRIOV               3u /* sriovAware: a VF token or a PF with VFs enabled                         */
+#define KXPU_MR_RESET               4u /* resetCheck: a member VFIO cannot reset between tenants                  */
+#define KXPU_MR_PCIE_AER            5u /* aerHealth: an AER count over its limit                                  */
+#define KXPU_MR_VGPU_TYPE_CHANGED   6u /* vfVgpuHealth: the VF's vGPU type is no longer the walk's                */
+#define KXPU_MR_COUNT               7u
+/* the kinds' names, comma separated: kind k is the k-th name */
+#define KXPU_METRICS_REASONS "vfio-device-missing,not-viable,vfio-cdev-missing,sriov,reset,pcie-aer,vgpu-type-changed"
+#define KXPU_METRICS_STRING_MAX 4096u
+#define KXPU_METRICS_NO_VALUE   UINT64_MAX /* aer_fatal / aer_nonfatal: no sample */
+#define KXPU_METRICS_HEALTHY_HEAD                                                                                      \
+    "# HELP kata_xpu_device_healthy Whether ListAndWatch reports the device Healthy (1) or Unhealthy (0).\n"           \
+    "# TYPE kata_xpu_device_healthy gauge\n"
+#define KXPU_METRICS_REASON_HEAD                                                                                       \
+    "# HELP kata_xpu_device_unhealthy_reason Why the plugin reports the device Unhealthy, one sample per reason.\n"    \
+    "# TYPE kata_xpu_device_unhealthy_reason gauge\n"
+#define KXPU_METRICS_AER_HEAD                                                                                          \
+    "# HELP kata_xpu_pcie_aer_errors The highest TOTAL_ERR count the device's aer_dev files reported at the last "     \
+    "read.\n"                                                                                                          \
+    "# TYPE kata_xpu_pcie_aer_errors gauge\n"
+/* family 4, written by the host: kata_xpu_sysfs_reads_total{file="aer_dev"|"vfio-dev"|"sriov"|"reset"|"nvidia"} and
+ * kata_xpu_allocate_validations_total{path="live"|"snapshot"}, in that order */
+#define KXPU_METRICS_READS_HEAD                                                                                        \
+    "# HELP kata_xpu_sysfs_reads_total Files and directories the plugin read for its health checks, by kind.\n"        \
+    "# TYPE kata_xpu_sysfs_reads_total counter\n"
+#define KXPU_METRICS_VALIDATIONS_HEAD                                                                                  \
+    "# HELP kata_xpu_allocate_validations_total Devices Allocate re-validated, from live sysfs reads or the snapshot.\n" \
+    "# TYPE kata_xpu_allocate_validations_total counter\n"
+
+/* One device of kxpu_metrics_devices.  64 bytes: the kernel reads one with four 16-byte vector loads. */
+typedef struct kxpu_metricdev {
+    uint64_t resource_off;  /* "<resourceNamespace>/<devpluginName>" at strings[resource_off, +resource_len)   */
+    uint64_t address_off;   /* the group's first member's bdf (a vGPU: its first mdev's UUID), likewise        */
+    uint32_t resource_len;
+    uint32_t address_len;
+    uint32_t group;         /* the device label: Device.ID, the IOMMU group, written as a decimal              */
+    uint32_t healthy;       /* 1: ListAndWatch sends the device Healthy; 0: Unhealthy                          */
+    uint64_t aer_fatal;     /* the group's highest known TOTAL_ERR_FATAL; KXPU_METRICS_NO_VALUE: no sample     */
+    uint64_t aer_nonfatal;  /* the same for TOTAL_ERR_NONFATAL                                                 */
+    uint64_t reason_off;    /* the device's reasons: reasons[reason_off, reason_off + reason_count)            */
+    uint32_t reason_count;
+    uint32_t reserved;      /* not read                                                                        */
+} kxpu_metricdev;
+
+/* One reason entry: its kind (KXPU_MR_*) and its detail at strings[detail_off, + detail_len).  16 bytes. */
+typedef struct kxpu_metricreason {
+    uint32_t kind;
+    uint32_t detail_len;
+    uint64_t detail_off;
+} kxpu_metricreason;
+
+int32_t kxpu_metrics_devices(kxpu_ctx *ctx, const kxpu_metricdev *devs, size_t n, const uint8_t *strings,
+                             size_t strings_len, const kxpu_metricreason *reasons, size_t n_reasons, uint8_t *out,
+                             size_t cap, size_t *len);
+
 #ifdef __cplusplus
 }
 #endif

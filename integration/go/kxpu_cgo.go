@@ -1097,6 +1097,57 @@ func (k *kxpu) resetCheck(rules []C.kxpu_xpu_rule, recs []C.kxpu_devrec, paths [
 	return methods[:n], setVerdict[:n], greset[:nGroups], err
 }
 
+// Prometheus metrics (an addition to ABI v14, detected by symbol).  metricsDevices writes the device families of the
+// text kxpu.h specifies (kata_xpu_device_healthy, _unhealthy_reason, kata_xpu_pcie_aer_errors) from one
+// C.kxpu_metricdev per device and one C.kxpu_metricreason per reason, their strings in one byte table; metricsText
+// appends the host's counters.  A host serves it on GET /metrics (INTEGRATION.md).
+func (k *kxpu) metricsDevices(devs []C.kxpu_metricdev, strs []byte, reasons []C.kxpu_metricreason) ([]byte, error) {
+	if len(devs) == 0 {
+		return nil, nil
+	}
+	var s *C.uint8_t // NULL for an empty table: the caller's slices are only read
+	var r *C.kxpu_metricreason
+	if len(strs) > 0 {
+		s = (*C.uint8_t)(unsafe.Pointer(&strs[0]))
+	}
+	if len(reasons) > 0 {
+		r = &reasons[0]
+	}
+	call := func(out *C.uint8_t, cap C.size_t, n *C.size_t) C.int32_t {
+		return C.kxpu_metrics_devices(k.ctx, &devs[0], C.size_t(len(devs)), s, C.size_t(len(strs)), r,
+			C.size_t(len(reasons)), out, cap, n)
+	}
+	var n C.size_t
+	if rc := call(nil, 0, &n); rc != C.KXPU_OK && rc != C.KXPU_E_NOSPACE { // sizing call
+		return nil, kxCheck(k.ctx, "kxpu_metrics_devices", rc)
+	}
+	buf := make([]byte, n+1)
+	err := kxCheck(k.ctx, "kxpu_metrics_devices", call((*C.uint8_t)(unsafe.Pointer(&buf[0])), n, &n))
+	return buf[:n], err
+}
+
+// metricsCounters: the host's process counters, in the order and with the headers of kxpu.h
+type metricsCounters struct {
+	AerReads, CdevReads, SriovReads, ResetReads, VfVgpuReads uint64
+	LiveValidations, SnapshotValidations                    uint64
+}
+
+func metricsText(device []byte, c metricsCounters) []byte {
+	out := append([]byte(nil), device...)
+	out = append(out, C.KXPU_METRICS_READS_HEAD...)
+	for _, f := range []struct {
+		name string
+		v    uint64
+	}{{"aer_dev", c.AerReads}, {"vfio-dev", c.CdevReads}, {"sriov", c.SriovReads}, {"reset", c.ResetReads},
+		{"nvidia", c.VfVgpuReads}} {
+		out = append(out, fmt.Sprintf("kata_xpu_sysfs_reads_total{file=%q} %d\n", f.name, f.v)...)
+	}
+	out = append(out, C.KXPU_METRICS_VALIDATIONS_HEAD...)
+	out = append(out, fmt.Sprintf("kata_xpu_allocate_validations_total{path=\"live\"} %d\n", c.LiveValidations)...)
+	out = append(out, fmt.Sprintf("kata_xpu_allocate_validations_total{path=\"snapshot\"} %d\n", c.SnapshotValidations)...)
+	return out
+}
+
 // pcieTree with every VF below its PF (pfOf: sriov's)
 func (k *kxpu) pcieTreeSriov(recs []C.kxpu_devrec, paths []C.kxpu_pcipath, goff, gmem []uint32, nGroups int,
 	pfOf []uint32) (gnode, parent []uint32, depth []uint8, err error) {

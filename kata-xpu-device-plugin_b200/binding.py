@@ -5,6 +5,7 @@ compute: numpy arrays are only used as typed host buffers.
 """
 import ctypes as C
 import os
+import re
 
 import numpy as np
 
@@ -108,6 +109,30 @@ RS_ABSENT, RS_READ_ERR, RS_LEGACY = 1, 2, 4
 RESET_METHODS = ("flr", "af_flr", "pm", "bus", "cxl_bus", "device_specific", "acpi")
 RM_ALL, RM_UNNAMED = 0x7F, 0x80
 RESET_SET_OK, RESET_NO_PATH, RESET_ROOT_BUS = 0xFFFFFFFF, 0xFFFFFFFE, 0xFFFFFFFD
+# kxpu_metricdev / kxpu_metricreason (Prometheus metrics, an addition to ABI v14)
+METRICDEV_DTYPE = np.dtype([("resource_off", "<u8"), ("address_off", "<u8"), ("resource_len", "<u4"), ("address_len", "<u4"),
+                            ("group", "<u4"), ("healthy", "<u4"), ("aer_fatal", "<u8"), ("aer_nonfatal", "<u8"),
+                            ("reason_off", "<u8"), ("reason_count", "<u4"), ("reserved", "<u4")])
+assert METRICDEV_DTYPE.itemsize == 64
+METRICREASON_DTYPE = np.dtype([("kind", "<u4"), ("detail_len", "<u4"), ("detail_off", "<u8")])
+assert METRICREASON_DTYPE.itemsize == 16
+METRICS_NO_VALUE = 0xFFFFFFFFFFFFFFFF
+METRICS_STRING_MAX = 4096
+
+
+def _header_macros():
+    """The string macros of include/kxpu.h the metrics document is made of: {name: bytes}, adjacent literals joined."""
+    text = open(os.path.join(os.path.dirname(_HERE), "include", "kxpu.h")).read().replace("\\\n", " ")
+    out = {}
+    for m in re.finditer(r'^#define (KXPU_METRICS_\w+)\s+((?:"(?:[^"\\]|\\.)*"\s*)+)$', text, re.M):
+        lits = re.findall(r'"((?:[^"\\]|\\.)*)"', m.group(2))
+        out[m.group(1)] = "".join(lits).encode().decode("unicode_escape").encode()
+    return out
+
+
+_MACROS = _header_macros()
+METRICS_REASONS = tuple(_MACROS["KXPU_METRICS_REASONS"].decode().split(","))  # kind k = METRICS_REASONS[k]
+METRICS_HEADS = tuple(_MACROS["KXPU_METRICS_%s_HEAD" % f] for f in ("HEALTHY", "REASON", "AER", "READS", "VALIDATIONS"))
 CDI_FRAG_MIN = 166  # the shortest device fragment of a CDI spec: len // CDI_FRAG_MIN records hold any document (ABI v13)
 
 
@@ -134,7 +159,7 @@ ABI_SYMBOLS = [
     "kxpu_cdi_emit_cdev", "kxpu_cdi_parse_cdev", "kxpu_cdi_emit_mdev_cdev", "kxpu_cdi_parse_mdev_cdev",
     "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu", "kxpu_pcie_tree_mdev",
     "kxpu_cdi_emit_vf_vgpu", "kxpu_cdi_emit_vf_vgpu_cdev", "kxpu_cdi_parse_vf_vgpu", "kxpu_cdi_parse_vf_vgpu_cdev",
-    "kxpu_dra_slices_vf_vgpu", "kxpu_vf_vgpu_drift", "kxpu_reset_check",
+    "kxpu_dra_slices_vf_vgpu", "kxpu_vf_vgpu_drift", "kxpu_reset_check", "kxpu_metrics_devices",
 ]
 
 
@@ -257,6 +282,7 @@ def load_library():
         "kxpu_vf_vgpu_types": (i32, [vp, vp, sz, vp, vp, sz, vp, vp, vp]),
         "kxpu_vf_vgpu_drift": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp]),
         "kxpu_reset_check": (i32, [vp, vp, sz, vp, vp, vp, sz, C.c_uint32, vp, vp, sz, vp, vp, vp]),
+        "kxpu_metrics_devices": (i32, [vp, vp, sz, vp, sz, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_classify_vf_vgpu": (i32, [vp, vp, sz, C.c_uint32, vp, sz, vp, C.POINTER(ClassifyOut), vp, vp, vp]),
         "kxpu_pcie_tree_sriov": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32), vp]),
         "kxpu_pcie_tree_mdev": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32)]),
@@ -713,6 +739,28 @@ class Kxpu:
                                           _ptr(paths) if n else None, _ptr(rrs) if n else None, n, allow, _ptr(goff),
                                           _ptr(gmem) if len(gmem) else None, G, _ptr(meth), _ptr(sv), _ptr(gr)))
         return dict(methods=meth[:n], set_verdict=sv[:n], group_reset=gr[:G])
+
+    def metrics_devices_raw(self, devs, strings, reasons, out, cap):
+        """The bare kxpu_metrics_devices call: (status, *len).  out: a uint8 array or None."""
+        devs, reasons = np.ascontiguousarray(devs), np.ascontiguousarray(reasons)
+        assert devs.dtype == METRICDEV_DTYPE and reasons.dtype == METRICREASON_DTYPE
+        sb = np.frombuffer(bytes(strings), np.uint8)
+        n = C.c_size_t(0)
+        rc = self.L.kxpu_metrics_devices(self.ctx, _ptr(devs) if len(devs) else None, len(devs), _ptr(sb) if len(sb) else None,
+                                         len(sb), _ptr(reasons) if len(reasons) else None, len(reasons), _ptr(out), cap,
+                                         C.byref(n))
+        return rc, n.value
+
+    def metrics_devices(self, devs, strings, reasons):
+        """kxpu_metrics_devices: families 1 to 3 of the Prometheus text of devs (METRICDEV_DTYPE) and reasons
+        (METRICREASON_DTYPE), their strings in `strings` (bytes).  Sizes with a first call, writes with a second."""
+        rc, need = self.metrics_devices_raw(devs, strings, reasons, None, 0)
+        if rc not in (KXPU_OK, E_NOSPACE):
+            self._chk(rc)
+        out = np.empty(max(need, 1), np.uint8)
+        rc, got = self.metrics_devices_raw(devs, strings, reasons, out, need)
+        self._chk(rc)
+        return out[:got].tobytes()
 
     def classify_vf_vgpu(self, rules, vgpu_rules, recs, keys, topo=False, viable=False):
         """kxpu_classify_vf_vgpu: the dict of classify_rules, plus group_numa (topo) and group_blocker (viable).  keys:

@@ -21,6 +21,7 @@
 
 #include "cdi.cuh"
 #include "common.cuh"
+#include "emit.cuh"
 #include "mdev.cuh"
 #include "scan.cuh"
 
@@ -162,14 +163,6 @@ static std::string part_text(const Parts &P, int k, const char *kind) {
     return s;
 }
 
-__device__ __forceinline__ uint32_t dec_len(unsigned long long v) {
-    uint32_t l = 1;
-    while (v >= 10ull) { v /= 10ull; l++; }
-    return l;
-}
-__device__ __forceinline__ void dec_write(unsigned long long v, uint32_t len, uint8_t *dst) {
-    for (uint32_t k = len; k > 0; k--) { dst[k - 1] = (uint8_t)('0' + (uint32_t)(v % 10ull)); v /= 10ull; }
-}
 __device__ __forceinline__ uint32_t bdf_len16(const uint8_t *b) {
     uint32_t l = 0;
     while (l < 16u && b[l]) l++;

@@ -35,6 +35,10 @@ static const char *kCdiVendorClass = "nvidia.com/gpu";                       // 
 
 XpuClass defaultXpuClass() { return XpuClass{"10de", "vfio-pci", "nvidia.com", kCdiVendorClass, "cdi-vfio-xxxx"}; }
 
+// What ListAndWatch sends a device: Healthy only while the watcher has its node, the last walk found its group viable,
+// its link reports no errors over the limits and (a VF) its vGPU type is the walk's.  MetricsText reports the same bit.
+static bool sentHealthy(const Device &d) { return d.Health == kHealthy && d.blocker.empty() && d.aer.empty() && d.drift.empty(); }
+
 static Error fail(const std::string &m) { Error e; e.failed = true; e.message = m; return e; }
 static Error kxfail(kxpu_ctx *ctx, const char *what, int32_t rc) {
     return fail(std::string(what) + ": " + kxpu_strerror(rc) + " (" + kxpu_last_error(ctx) + ")");
@@ -1208,17 +1212,17 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
         if (groupViability && c.gblk[g] != KXPU_VIABLE) s.blocker = blockerOf(w.recs[c.gblk[g]]);
         if (s.blocker.empty() && xpuClasses[s.klass].vfioCdev)  // a member without a cdev: VFIO cannot open it
             for (const NvidiaGpuDevice &d : devs)
-                if (d.cdev < 0) { s.blocker = d.addr + " has no VFIO cdev"; break; }
+                if (d.cdev < 0) { s.blocker = d.addr + " has no VFIO cdev"; s.blockerKind = KXPU_MR_VFIO_CDEV_MISSING; break; }
         if (sriovAware && w.gsriov[g] != KXPU_VIABLE) {
             std::vector<XpuClass> whole;
             for (const XpuClass &k : xpuClasses)
                 if (!k.vfVgpu) whole.push_back(k);
             s.sriov = sriovReasonOf(whole, w, w.gsriov[g]);
-            if (s.blocker.empty()) s.blocker = s.sriov;
+            if (s.blocker.empty()) { s.blocker = s.sriov; s.blockerKind = KXPU_MR_SRIOV; }
         }
         if (resetCheck && w.greset[g] != KXPU_VIABLE) {
             s.reset = resetReasonOf(w, w.greset[g]);
-            if (s.blocker.empty()) s.blocker = s.reset;
+            if (s.blocker.empty()) { s.blocker = s.reset; s.blockerKind = KXPU_MR_RESET; }
         }
         if (draEnabled()) {
             const uint32_t first = c.gmem[c.goff[g]];
@@ -1480,7 +1484,7 @@ void Plugin::buildMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
         if (vgpuPcieTopologyAware) s.pcieNode = w.gnode[g];
         if (vgpuClasses[s.klass].mdevCdev)  // an mdev without a cdev: VFIO cannot open it
             for (const MdevDevice &m : devs)
-                if (m.cdev < 0) { s.blocker = m.uuid + " has no VFIO cdev"; break; }
+                if (m.cdev < 0) { s.blocker = m.uuid + " has no VFIO cdev"; s.blockerKind = KXPU_MR_VFIO_CDEV_MISSING; break; }
         mdevMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
         mdevState.push_back(std::move(s));
     }
@@ -2659,7 +2663,11 @@ std::vector<int64_t> Plugin::draSinceTable(const std::vector<std::string> &group
 }
 
 Error Plugin::computeAer() {
-    auto set = [](auto &s, const std::string &why, uint8_t bits) { s.aer = why; s.aerBits = bits; };
+    auto set = [](auto &s, const std::string &why, uint8_t bits) {
+        s.aer = why;
+        s.aerBits = bits;
+        s.aerMax[0] = s.aerMax[1] = KXPU_METRICS_NO_VALUE;
+    };
     for (auto &s : iommuState) set(s, std::string(), 0);
     for (auto &s : mdevState) set(s, std::string(), 0);
     if (!aerHealth) return Error();  // no aer_dev_* file is opened
@@ -2713,8 +2721,17 @@ Error Plugin::computeAer() {
                     why = who[members[m]] + " reported " + std::to_string(c) + (k ? " non-fatal" : " fatal") +
                           " uncorrectable PCIe errors (limit " + std::to_string(limit) + ")";
             }
+        uint64_t most[2] = {KXPU_METRICS_NO_VALUE, KXPU_METRICS_NO_VALUE};  // the highest known count of each severity
+        for (int k = 0; k < 2; k++)
+            for (uint32_t m = goff[g]; m < goff[g + 1]; m++) {
+                const uint64_t c = totals[2 * members[m] + k];
+                if (c != UINT64_MAX && (most[k] == KXPU_METRICS_NO_VALUE || c > most[k])) most[k] = c;
+            }
+        auto &st = g < iommuState.size() ? iommuState[g].aerMax : mdevState[g - iommuState.size()].aerMax;
         if (g < iommuState.size()) set(iommuState[g], why, bits[g]);
         else set(mdevState[g - iommuState.size()], why, bits[g]);
+        st[0] = most[0];
+        st[1] = most[1];
     }
     return Error();
 }
@@ -2941,8 +2958,7 @@ Error Plugin::ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8
     std::vector<uint64_t> masks;
     for (const Device &d : dp.devs) {
         groups.push_back((uint32_t)strtoul(d.ID.c_str(), nullptr, 10));
-        // nor one whose link reports errors, nor a VF whose vGPU type changed
-        healthy.push_back(d.Health == kHealthy && d.blocker.empty() && d.aer.empty() && d.drift.empty());
+        healthy.push_back(sentHealthy(d));
         masks.push_back(d.numa);
     }
     // topologyAware: Device.topology from each device's mask (the HealthWatcher's re-sends come through here too)
@@ -2958,6 +2974,110 @@ Error Plugin::ListAndWatchBytes(const GenericDevicePlugin &dp, std::vector<uint8
     if (len == 0) return Error();
     rc = encode(out.data(), len, &len);
     if (rc != KXPU_OK) return kxfail(ctx_, what, rc);
+    return Error();
+}
+
+// The length MetricsText keeps of a label string: all of it up to KXPU_METRICS_STRING_MAX bytes (the kernel's limit),
+// else the limit moved back to the start of a UTF-8 sequence that would be split there, so that the cut adds no U+FFFD.
+size_t metricsCut(const uint8_t *s, size_t len) {
+    const size_t max = KXPU_METRICS_STRING_MAX;
+    if (len <= max) return len;
+    size_t k = max;  // s[max] is the first byte left out; the nearest non-continuation byte at most three in front of it
+    while (k > max - 3 && (s[k] & 0xC0u) == 0x80u) k--;
+    const uint32_t c = s[k], need = c < 0xC2u ? 0u : c < 0xE0u ? 1u : c < 0xF0u ? 2u : c < 0xF5u ? 3u : 0u;
+    return k < max && need && k + need >= max ? k : max;  // a lead whose sequence the limit would split
+}
+
+Error Plugin::MetricsText(std::vector<uint8_t> &out) {
+    std::shared_lock<std::shared_mutex> lock(mu_);
+    out.clear();
+    std::string strings;
+    std::vector<kxpu_metricdev> devs;
+    std::vector<kxpu_metricreason> reasons;
+    auto put = [&strings](const std::string &s, uint64_t &off, uint32_t &len) {
+        off = strings.size();
+        len = (uint32_t)metricsCut((const uint8_t *)s.data(), s.size());
+        strings.append(s, 0, len);
+    };
+    // an upper bound of the document: every label byte at most three bytes once repaired or escaped, and at most 128
+    // bytes of names, literals and decimals per sample; the headers within 512
+    size_t bound = 512;
+    const std::map<std::string, size_t> iommuAt = positions(iommuMap), mdevAt = positions(mdevMap);
+    for (const GenericDevicePlugin &dp : devicePlugins) {
+        kxpu_metricdev proto;
+        memset(&proto, 0, sizeof proto);
+        put(dp.resourceNamespace + "/" + dp.devpluginName, proto.resource_off, proto.resource_len);
+        const std::map<std::string, size_t> &at = dp.vgpu ? mdevAt : iommuAt;
+        for (const Device &d : dp.devs) {
+            kxpu_metricdev m = proto;
+            m.group = (uint32_t)strtoul(d.ID.c_str(), nullptr, 10);  // as ListAndWatchBytes writes Device.ID
+            m.healthy = sentHealthy(d) ? 1u : 0u;
+            m.aer_fatal = m.aer_nonfatal = KXPU_METRICS_NO_VALUE;
+            m.reason_off = reasons.size();
+            std::string address;
+            uint32_t blockerKind = KXPU_MR_NOT_VIABLE;
+            const std::string *sriov = nullptr, *reset = nullptr;
+            auto it = at.find(d.ID);
+            if (it != at.end() && dp.vgpu) {
+                const GroupState<kxpu_dramdev> &s = mdevState[it->second];
+                address = mdevMap[it->second].second.front().uuid;
+                blockerKind = s.blockerKind;
+                m.aer_fatal = s.aerMax[0];
+                m.aer_nonfatal = s.aerMax[1];
+            } else if (it != at.end()) {
+                const GroupState<kxpu_dradev> &s = iommuState[it->second];
+                address = iommuMap[it->second].second.front().addr;
+                blockerKind = s.blockerKind;
+                sriov = &s.sriov;
+                reset = &s.reset;
+                m.aer_fatal = s.aerMax[0];
+                m.aer_nonfatal = s.aerMax[1];
+            }
+            put(address, m.address_off, m.address_len);
+            size_t details = 0;
+            auto reason = [&](uint32_t kind, const std::string &detail) {
+                kxpu_metricreason r;
+                memset(&r, 0, sizeof r);
+                r.kind = kind;
+                put(detail, r.detail_off, r.detail_len);
+                reasons.push_back(r);
+                details += detail.size();
+            };
+            // in kind order; sriov and reset are computed even when an earlier check holds the blocker, the cdev check only
+            // without a viability blocker, so a reason never computed has no entry
+            if (d.Health != kHealthy) reason(KXPU_MR_VFIO_DEVICE_MISSING, std::string());
+            if (!d.blocker.empty()) reason(blockerKind, d.blocker);
+            if (sriov && !sriov->empty() && (d.blocker.empty() || blockerKind < KXPU_MR_SRIOV)) reason(KXPU_MR_SRIOV, *sriov);
+            if (reset && !reset->empty() && (d.blocker.empty() || blockerKind < KXPU_MR_RESET)) reason(KXPU_MR_RESET, *reset);
+            if (!d.aer.empty()) reason(KXPU_MR_PCIE_AER, d.aer);
+            if (!d.drift.empty()) reason(KXPU_MR_VGPU_TYPE_CHANGED, d.drift);
+            m.reason_count = (uint32_t)(reasons.size() - m.reason_off);
+            bound += (3 + m.reason_count) * (128 + 3 * (size_t)(m.resource_len + m.address_len)) + 3 * details;
+            devs.push_back(m);
+        }
+    }
+    if (!devs.empty()) {  // with no device there is nothing for the GPU to write
+        out.resize(bound);
+        size_t len = 0;
+        const int32_t rc = kxpu_metrics_devices(ctx_, devs.data(), devs.size(), (const uint8_t *)strings.data(), strings.size(),
+                                                reasons.data(), reasons.size(), out.data(), out.size(), &len);
+        if (rc != KXPU_OK) {
+            out.clear();
+            return kxfail(ctx_, "kxpu_metrics_devices", rc);
+        }
+        out.resize(len);
+    }
+    auto line = [&out](const std::string &l) { out.insert(out.end(), l.begin(), l.end()); };
+    line(KXPU_METRICS_READS_HEAD);
+    const std::pair<const char *, uint64_t> reads[] = {{"aer_dev", aerReads.load(std::memory_order_relaxed)},
+                                                       {"vfio-dev", cdevReads.load(std::memory_order_relaxed)},
+                                                       {"sriov", sriovReads.load(std::memory_order_relaxed)},
+                                                       {"reset", resetReads.load(std::memory_order_relaxed)},
+                                                       {"nvidia", vfVgpuReads.load(std::memory_order_relaxed)}};
+    for (const auto &r : reads) line(std::string("kata_xpu_sysfs_reads_total{file=\"") + r.first + "\"} " + std::to_string(r.second) + "\n");
+    line(KXPU_METRICS_VALIDATIONS_HEAD);
+    line("kata_xpu_allocate_validations_total{path=\"live\"} " + std::to_string(liveValidations.load(std::memory_order_relaxed)) + "\n");
+    line("kata_xpu_allocate_validations_total{path=\"snapshot\"} " + std::to_string(snapshotValidations.load(std::memory_order_relaxed)) + "\n");
     return Error();
 }
 
@@ -3734,6 +3854,23 @@ int kxh_list_and_watch(void *h, int plugin_index, uint8_t *out, size_t cap) {
     if (b.size() > cap) return -2;
     memcpy(out, b.data(), b.size());
     return (int)b.size();
+}
+
+// MetricsText into out (cap bytes); *len = its size.  0, -1 with the message in err, -2 when cap is too small
+// metricsCut (CPU tests)
+size_t kxh_metrics_cut(const char *s, size_t len) { return device_plugin::metricsCut((const uint8_t *)s, len); }
+
+int kxh_metrics(void *h, uint8_t *out, size_t cap, size_t *len, char *err, size_t errcap) {
+    std::vector<uint8_t> b;
+    device_plugin::Error e = ((Plugin *)h)->MetricsText(b);
+    if (e) {
+        snprintf(err, errcap, "%s", e.message.c_str());
+        return -1;
+    }
+    *len = b.size();
+    if (b.size() > cap) return -2;
+    memcpy(out, b.data(), b.size());
+    return 0;
 }
 
 // ---- NUMA topology (tests)

@@ -13,6 +13,7 @@
 // generic_device_plugin.go:128-220) is out of scope and stays in the Go binary; the Go
 // cgo shim that replaces this file in production is shown in INTEGRATION.md.
 #pragma once
+#include <atomic>
 #include <cstdint>
 #include <deque>
 #include <functional>
@@ -235,6 +236,9 @@ struct ResumeReport {
     std::vector<std::string> filesWritten;     // spec and state files whose bytes changed at start-up
 };
 
+// The length of a label string Plugin::MetricsText keeps: len up to KXPU_METRICS_STRING_MAX, else that limit, moved back
+// to the lead of a UTF-8 sequence the limit would split (exposed for CPU tests)
+size_t metricsCut(const uint8_t *s, size_t len);
 // the atomic spec writer of Plugin::rediscover (exposed for CPU tests)
 Error writeSpecFileAtomicForTests(const std::string &file_path, const uint8_t *doc, size_t len, bool &written);
 // The index state file of Plugin::resumeIndices: "pci <next>\nmdev <next>\n", canonical decimals.  format / parse are
@@ -316,10 +320,16 @@ struct GroupState {
     // why VFIO cannot open the group, empty = it can: "<bdf> is bound to <driver>" (groupViability), else "<bdf> has no
     // VFIO cdev" (vfioCdev), else sriov; a vGPU group: "<uuid> has no VFIO cdev" (mdevCdev)
     std::string blocker{};
+    // the check that produced blocker (KXPU_MR_NOT_VIABLE, _VFIO_CDEV_MISSING, _SRIOV or _RESET); read only while blocker
+    // is not empty.  The metrics name the reason by it (Plugin::MetricsText)
+    uint32_t blockerKind = KXPU_MR_NOT_VIABLE;
     std::string sriov{};  // sriovAware, passthrough only: the SR-IOV reason; empty = served
     std::string reset{};  // resetCheck, passthrough only: why a member cannot be reset between tenants; empty = served
     std::string aer{};    // aerHealth: the first member over an AER limit (computeAer); empty = within the limits
     uint8_t aerBits = 0;  // aerHealth: the group's KXPU_AER_* bits (computeAer)
+    // aerHealth: the highest known TOTAL_ERR_FATAL / _NONFATAL over the files computeAer folded for the group (members, an
+    // mdev's parent, a VF's PF); KXPU_METRICS_NO_VALUE = none known.  Reported by MetricsText only
+    uint64_t aerMax[2] = {KXPU_METRICS_NO_VALUE, KXPU_METRICS_NO_VALUE};
     std::optional<Dra> dra{};  // draEnabled (vgpuDraEnabled): the ResourceSlice record of its first member; none = unpublished
     // vfVgpuDraEnabled, a group of a class with a vgpuDraDriver whose first member is a VF that carries a named vGPU type:
     // its VF-vGPU ResourceSlice record; none = unpublished
@@ -452,9 +462,11 @@ class Plugin {
     // Allocate response [assumed].
     bool resumeIndices = false;
     const ResumeReport &resumeReport() const { return resume_; }
-    uint64_t liveValidations = 0, snapshotValidations = 0;  // devices validated either way (tests, metrics)
-    uint64_t aerReads = 0;  // aer_dev_* files read (tests, metrics)
-    uint64_t cdevReads = 0;  // vfio-dev/ directories listed (tests, metrics)
+    // devices validated either way (tests, metrics).  The counters are atomic: Allocate counts under the shared lock, and
+    // MetricsText reads them under it too
+    std::atomic<uint64_t> liveValidations{0}, snapshotValidations{0};
+    std::atomic<uint64_t> aerReads{0};  // aer_dev_* files read (tests, metrics)
+    std::atomic<uint64_t> cdevReads{0};  // vfio-dev/ directories listed (tests, metrics)
     // SR-IOV virtual functions (include/kxpu.h, additions to ABI v14).  false (default): nothing named physfn or
     // sriov_numvfs is opened and every output is as above.  true: after either gather, physfn (readlink, basename) and
     // sriov_numvfs of every candidate of a passthrough class are read, and kxpu_sriov decides per group.  A group with a VF
@@ -464,7 +476,7 @@ class Plugin {
     // path re-reads physfn, the PF's driver and sriov_numvfs.  With pcieTopologyAware the forest is kxpu_pcie_tree_sriov's,
     // so GetPreferredAllocation packs a request's VFs by PF.
     bool sriovAware = false;
-    uint64_t sriovReads = 0;  // functions whose physfn and sriov_numvfs were read (tests, metrics)
+    std::atomic<uint64_t> sriovReads{0};  // functions whose physfn and sriov_numvfs were read (tests, metrics)
     // Resets between tenants (include/kxpu.h, kxpu_reset_check).  false (default): no reset_method or reset file is opened
     // and every output, generation and counter is as above.  true: after either gather, the PCI walk reads the entry link
     // of every entry (as readsPaths), the `driver` link of every entry whose driver is not known yet (and `iommu_group` of
@@ -485,11 +497,11 @@ class Plugin {
     // it exists: the file is write-only).  false with errno ENOENT: no such file; false with any other errno: a failed
     // read.  A seam: tests replace it.  Every call counts in resetReads.
     std::function<bool(const std::string &base, const std::string &bdf, const std::string &name, std::string &out)> readResetFile;
-    uint64_t resetReads = 0;  // reset_method and reset files opened (tests, metrics)
+    std::atomic<uint64_t> resetReads{0};  // reset_method and reset files opened (tests, metrics)
     // <base>/<bdf>/nvidia/<name>, at most KXPU_VGPU_FILE_MAX + 1 bytes; false: the read failed ("no such file" included).
     // A seam: tests replace it.  Every call counts in vfVgpuReads.
     std::function<bool(const std::string &base, const std::string &bdf, const std::string &name, std::string &out)> readVgpuFile;
-    uint64_t vfVgpuReads = 0;  // nvidia/ files read (tests, metrics)
+    std::atomic<uint64_t> vfVgpuReads{0};  // nvidia/ files read (tests, metrics)
     // Health of vGPUs on SR-IOV VFs (include/kxpu.h, kxpu_vf_vgpu_drift).  Refused by InitiateDevicePlugin unless some class
     // has vfVgpu.  false (default): no file more is opened and every output, generation and counter is as above.  true:
     //   - refreshVfVgpuTypes re-reads the type of every served VF and withholds one whose type changed;
@@ -603,6 +615,13 @@ class Plugin {
     // a rediscover would now move it to that type's resource.  The maps, indices and specs are never rebuilt here.
     // Without vfVgpuHealth nothing is read and nothing changes.
     Error refreshVfVgpuTypes(std::vector<size_t> &changedPlugins, bool &passthroughMoved, bool &typesMoved);
+    // The Prometheus text (format 0.0.4, include/kxpu.h) of the current plugins and group state, under the shared lock:
+    // one kxpu_metrics_devices call for every device of every plugin in devicePlugins order (whether ListAndWatch sends
+    // it Healthy, each reason the host holds for it, its group's AER maxima), then the host's read and validation
+    // counters.  It reads nothing from sysfs and changes no state: it reports what the last walk and refreshes found.  A
+    // host that serves GET /metrics calls it per scrape.  A label string longer than KXPU_METRICS_STRING_MAX bytes is cut
+    // there (metricsCut), so one long reason cannot make the whole scrape fail.
+    Error MetricsText(std::vector<uint8_t> &out);
     // The ResourceSlices of the vGPUs of vfVgpu class xpuClass (kxpu_dra_slices_vf_vgpu): one pool named nodeName, one
     // device per iommuMap group of the class in walk order whose first member is a VF that carries a named vGPU type,
     // unless the group has a blocker (as ResourceSlices).  The device is described by that VF: its address, type key and

@@ -853,3 +853,50 @@ def reset_walk(n=1 << 20, seed=71):
     rrs["flags"][kind == 3] = RS_ABSENT | RS_LEGACY
     rrs["flags"][kind == 4] = RS_ABSENT
     return recs, paths, rrs
+
+
+def metrics_devices(n=1 << 20, seed=81):
+    """n devices of kxpu_metrics_devices (METRICDEV_DTYPE), their strings and reasons (METRICREASON_DTYPE): eight
+    resources, one bdf per device, 1 in 8 devices with one reason, 1 in 64 with three, details of about 80 bytes of
+    which 1 in 256 carries a non-ASCII or escaped byte, every device with both AER values.  Returns (devs, strings,
+    reasons)."""
+    from .binding import METRICDEV_DTYPE, METRICREASON_DTYPE
+    rng = np.random.default_rng(seed)
+    resources = [b"nvidia.com/GH100_H100_SXM5_80GB", b"nvidia.com/GH100_H100_NVL", b"amd.com/MI300X",
+                 b"nvidia.com/NVIDIA_H100-4C", b"nvidia.com/NVIDIA_H100-10C", b"nvidia.com/NVIDIA_H100-20C",
+                 b"nvidia.com/GA100_A100_PCIE_80GB", b"intel.com/Gaudi3"]
+    parts = [b"".join(resources)]
+    roff = np.cumsum([0] + [len(r) for r in resources])[:-1]
+    base = len(parts[0])
+    bdfs = enumerate_bdfs(n)
+    parts.append(bdfs[:, :12].tobytes())
+    devs = np.zeros(n, METRICDEV_DTYPE)
+    which = rng.integers(0, len(resources), n)
+    devs["resource_off"] = roff[which]
+    devs["resource_len"] = np.array([len(r) for r in resources], np.uint32)[which]
+    devs["address_off"] = base + 12 * np.arange(n, dtype=np.uint64)
+    devs["address_len"] = 12
+    devs["group"] = rng.permutation(n).astype(np.uint32) + 1
+    devs["aer_fatal"] = rng.integers(0, 3, n)
+    devs["aer_nonfatal"] = rng.integers(0, 1000, n)
+    count = np.zeros(n, np.uint32)
+    count[rng.random(n) < 1 / 8] = 1
+    count[rng.random(n) < 1 / 64] = 3
+    devs["reason_count"] = count
+    devs["reason_off"] = np.concatenate([[0], np.cumsum(count)[:-1]])
+    devs["healthy"] = count == 0
+    m = int(count.sum())
+    reasons = np.zeros(m, METRICREASON_DTYPE)
+    first = np.repeat(rng.integers(1, 5, n).astype(np.uint32), count)  # a kind, then kind + 1, kind + 2 for three
+    step = np.arange(m) - np.repeat(devs["reason_off"].astype(np.int64), count)
+    reasons["kind"] = np.minimum(first, 4) + step
+    texts = (b"0000:%02x:00.1 on its bus is bound to snd_hda_intel and cannot be reset between tenants%s" % (k, t)
+             for k, t in enumerate([b"", b" \xe2\x80\x94 \"x\"", b"\\n", b"\xff"] * 64))
+    pool = list(texts)
+    pick = np.where(rng.random(m) < 1 / 256, rng.integers(0, len(pool), m), (rng.integers(0, len(pool) // 4, m) * 4))
+    off = base + 12 * n
+    pool_off = np.cumsum([0] + [len(t) for t in pool])[:-1] + off
+    parts.append(b"".join(pool))
+    reasons["detail_off"] = pool_off[pick]
+    reasons["detail_len"] = np.array([len(t) for t in pool], np.uint32)[pick]
+    return devs, b"".join(parts), reasons

@@ -81,6 +81,9 @@ rrecs, rpaths, rrrs = W.reset_walk(20000)
 rres = kx.classify_rules([(b"10de", b"vfio-pci")], rrecs)
 rv = kx.reset_check([(b"10de", b"vfio-pci")], rrecs, rpaths, rrrs, B.RM_ALL, rres["group_off"], rres["group_members"])
 print("reset withheld", int((rv["group_reset"] != B.VIABLE).sum()))
+# Prometheus metrics: the size pass, the scan and the write pass over devices with reasons and AER values
+mdevs, mstr, mrs = W.metrics_devices(20000)
+print("metrics bytes", len(kx.metrics_devices(mdevs, mstr, mrs)))
 # vGPUs on VFs: the type join and the per-type classify, with and without blockers
 vrecs_, vvts, vtables = W.vf_vgpu_walk(20000)
 vt = kx.vf_vgpu_types(vvts, vtables)
