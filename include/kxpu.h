@@ -71,7 +71,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_FINALIZE 1
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
-#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s, kxpu_sriov's and kxpu_reset_check's kernels: the slot holds the most recent call's */
+#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s, kxpu_sriov's, kxpu_mdev_pf's and kxpu_reset_check's kernels: the slot holds the most recent call's */
 #define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev|_vf_vgpu[_cdev]]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
@@ -1375,6 +1375,77 @@ typedef struct kxpu_dravfvgpu {
  * for n_taints == 1, KXPU_DRA_MAX_TAINTS for more).  Timed under KXPU_T_EMIT. */
 int32_t kxpu_dra_slices_vf_vgpu(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
                                 const kxpu_dravfvgpu *devs, size_t n, const kxpu_dra_taint *taints, size_t n_taints,
+                                const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out, size_t cap,
+                                size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
+/* ------------------------------------- mdev vGPUs on SR-IOV virtual functions (additions to ABI v14) */
+
+/* These calls and kxpu_dramdevpf were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym), as
+ * for kxpu_sriov.  On the vGPU releases most hosts run (before NVIDIA's vendor-specific VFIO framework) a vGPU is an
+ * mdev; on an SR-IOV GPU the admin enables the VFs (sriov-manage -e) and each VF gets its own mdev_supported_types.  The
+ * mdev walk records the VF as the parent.  These facts are taken as given:
+ *   [assumed] on an SR-IOV GPU, a vGPU release before the vendor-specific VFIO framework creates mdevs on VFs, never on
+ *             the PF;
+ *   [assumed] <uuid>/../physfn is the VF's link to its PF, and its basename is the PF's PCI address;
+ *   [assumed] errors of the whole GPU (a surprise down, a completion timeout, a fatal link error) are logged on the PF,
+ *             and a VF may have no aer_dev_* files of its own.
+ * Host side: for every mdev that got as far as its iommu_group link, the host reads readlink(<uuid>/../physfn) (basename)
+ * into a kxpu_sriovrec at the mdev's index, physfn only: numvfs_txt and numvfs_len stay zero and are not read; every other
+ * mdev gets a zero-filled one.  A missing link is not an error: the parent is no VF. */
+
+/* The PF of each mdev's parent VF, joined against the PCI walk's records.  recs / n_recs: the records of a PCI walk
+ * (kxpu_classify*'s input); mrecs / msrs / n_mdevs: the mdev walk's records and one side record per mdev.  Output:
+ *   - pf_of[i] = p, the lowest index of recs whose bdf (up to its first NUL) equals msrs[i].physfn (up to its first NUL),
+ *     or KXPU_NO_PF when physfn is not canonical (kxpu_sriov's grammar: lowercase "dddd:bb:dd.f", device at most 1f,
+ *     function 0..7), carries KXPU_SR_PHYSFN_ERR, no record matches, or physfn equals mrecs[i].parent (up to its first
+ *     NUL): a parent never resolves to itself.  An mdev whose PF is outside the walk gets KXPU_NO_PF and is served as an
+ *     mdev on a PF is.
+ * mrecs is read for parent only; numvfs_txt, numvfs_len and the records' other fields are not read.
+ * KXPU_E_INVALID, nothing written: ctx NULL, recs NULL with n_recs > 0, mrecs, msrs or pf_of NULL with n_mdevs > 0.
+ * Limit (else KXPU_E_UNSUPPORTED, checked before any array is read): n_recs and n_mdevs below 2^30.
+ * GPU: kxpu_sriov's table and probe as compile-time variants, two launches timed under KXPU_T_CLASSIFY -- (1) one thread
+ * per PCI record inserts its canonical bdf into the open-addressing table holding the lowest index per key; (2) one
+ * thread per mdev probes its physfn. */
+int32_t kxpu_mdev_pf(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n_recs, const kxpu_mdevrec *mrecs,
+                     const kxpu_sriovrec *msrs, size_t n_mdevs, uint32_t *pf_of /* [n_mdevs] */);
+
+/* One published vGPU of the mdev layout with its parent's PF.  240 bytes, a multiple of 16; alignof 8. */
+typedef struct kxpu_dramdevpf {
+    kxpu_dramdev dev;       /* the mdev layout's record, unchanged                                           */
+    char     physfn[16];    /* the PF's PCI address (kxpu_mdev_pf's match), NUL padded; "" = the parent is no VF */
+    char     physfn_device[8]; /* the PF's device id; "" = not known                                         */
+    uint8_t  reserved[8];
+} kxpu_dramdevpf;
+
+/* The ResourceSlices of one pool of vGPUs whose parents may be VFs.  The contract is kxpu_dra_slices_mdev_taints', word
+ * for word, except for the device: the slices, their header and tail, 128 devices per slice (64 with taint_since), one
+ * empty slice for n = 0, slice_off, the two-call sizing and KXPU_E_NOSPACE, the KXPU_E_INVALID argument checks, the
+ * taint table rules, taint_since == NULL giving the untainted bytes, and nothing written on KXPU_E_INVALID or
+ * KXPU_E_UNSUPPORTED.  There is no one-taint or untainted entry point for this layout.  A device is the mdev layout's
+ * with two more attributes, keys sorted bytewise:
+ *   "iommuGroup":{"int":<g>}                                          always
+ *   "mdevType":{"string":"<mdev_type>"}                               always
+ *   "numaNode":{"int":<k>}                                            only when numa_mask has exactly one bit k set
+ *   "parentAddress":{"string":"<parent>"}                             always
+ *   "parentDeviceID":{"string":"<device>"}                            only when device is not empty
+ *   "parentVendorID":{"string":"<vendor>"}                            always
+ *   "physfnAddress":{"string":"<physfn>"}                             only when physfn is not empty
+ *   "physfnDeviceID":{"string":"<physfn_device>"}                     only when physfn_device is not empty
+ *   "productName":{"string":"<product[0..product_len)>"}              only when product_len > 0
+ *   "resource.kubernetes.io/pcieRoot":{"string":"<pcie_root>"}        only when pcie_root is not empty
+ *   "uuid":{"string":"<uuid>"}                                        always
+ * So a record whose physfn is empty (its physfn_device is then empty too: the domain says so) gives the device bytes of
+ * kxpu_dra_slices_mdev_taints for its dev, and a pool where every physfn is empty gives that call's bytes.
+ * KXPU_E_UNSUPPORTED, with *len, the output and slice_off untouched: the taint cases of kxpu_dra_slices_mdev_taints,
+ * n >= KXPU_DRA_MAX_DEVICES, or a record outside the domain (in the order the kernel's flags report them):
+ *   - dev: kxpu_dra_slices_mdev's domain, in its order (product, mdev_type, uuid, parent, pcie_root, vendor, device,
+ *     iommu_group, product_len);
+ *   - physfn: empty, or 1..16 bytes over [0-9a-f:.] before its first NUL;
+ *   - physfn_device: 0..6 bytes over [0-9a-f] before its first NUL, and empty when physfn is empty.
+ * GPU: the kernel of kxpu_dra_slices, instantiated for this record layout, untainted and with the taint list (one entry
+ * for n_taints == 1, KXPU_DRA_MAX_TAINTS for more).  Timed under KXPU_T_EMIT. */
+int32_t kxpu_dra_slices_mdev_pf(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                                const kxpu_dramdevpf *devs, size_t n, const kxpu_dra_taint *taints, size_t n_taints,
                                 const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out, size_t cap,
                                 size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
 

@@ -911,6 +911,24 @@ func (k *kxpu) draSlicesVfVgpu(driver, node string, generation uint64, devs []C.
 	})
 }
 
+// DRA ResourceSlices of mdev vGPUs whose parents may be SR-IOV VFs (an addition to ABI v14, detected by symbol).  With
+// vgpuSriovAware a vGPU class's pool is published through this call instead of draSlicesMdev: devs holds one
+// kxpu_dramdevpf per mdevMap group of the class in walk order, its PF's address and device id next to the mdev record
+// (both empty for an mdev on a PF, which then gives draSlicesMdev's bytes).  Tainted, published and replaced exactly as
+// draSlicesMdev's output.
+func (k *kxpu) draSlicesMdevPf(driver, node string, generation uint64, devs []C.kxpu_dramdevpf, since []int64) ([]string, error) {
+	var p *C.kxpu_dramdevpf
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	return k.slices("kxpu_dra_slices_mdev_pf", driver, node, len(devs), since, func(cd, cn *C.char,
+		tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
+		ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_mdev_pf(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), tab, nt, cs,
+			out, capacity, n, off, ns)
+	})
+}
+
 // the two-call sizing of one slice call, the table and the times in C memory; the table width is len(since) / nDevs
 func (k *kxpu) slices(what, driver, node string, nDevs int, since []int64, call func(cd, cn *C.char,
 	tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
@@ -1027,6 +1045,26 @@ func sriovRecord(physfn string, physfnErr bool, numvfs []byte, numvfsErr bool) C
 
 // the SR-IOV verdict of a walk: recs / srs at the same indices, rules and the CSR (gids, goff, gmem) of its classify call.
 // pfOf and numvfs have one entry per record, gsriov one per group (C.KXPU_VIABLE: served).
+// mdevPf: each mdev's PF in the PCI walk (kxpu_mdev_pf, an addition to ABI v14).  recs: the PCI walk's records, which
+// runs first; mrecs / msrs: the mdev walk's records and their physfn reads (readLink(<uuid>/../physfn), basename, in a
+// kxpu_sriovrec whose numvfs fields stay zero).  pfOf[i] is a record index or KXPU_NO_PF.
+func (k *kxpu) mdevPf(recs []C.kxpu_devrec, mrecs []C.kxpu_mdevrec, msrs []C.kxpu_sriovrec) ([]uint32, error) {
+	n, m := len(recs), len(mrecs)
+	pfOf := make([]uint32, m+1)
+	var r *C.kxpu_devrec
+	var mr *C.kxpu_mdevrec
+	var ms *C.kxpu_sriovrec
+	if n > 0 {
+		r = &recs[0]
+	}
+	if m > 0 {
+		mr, ms = &mrecs[0], &msrs[0]
+	}
+	err := kxCheck(k.ctx, "kxpu_mdev_pf", C.kxpu_mdev_pf(k.ctx, r, C.size_t(n), mr, ms, C.size_t(m),
+		(*C.uint32_t)(unsafe.Pointer(&pfOf[0]))))
+	return pfOf[:m], err
+}
+
 func (k *kxpu) sriov(rules []C.kxpu_xpu_rule, recs []C.kxpu_devrec, srs []C.kxpu_sriovrec, gids, goff, gmem []uint32) (pfOf,
 	numvfs, gsriov []uint32, err error) {
 	n, nGroups := len(recs), len(goff)-1

@@ -76,6 +76,9 @@ DRAVFVGPU_DTYPE = np.dtype([("product", "u1", (64,)), ("type_key", "S40"), ("bdf
                             ("pcie_root", "S16"), ("vendor", "S8"), ("device", "S8"), ("numa_mask", "<u8"),
                             ("iommu_group", "<u4"), ("type_id", "<u4"), ("product_len", "u1"), ("reserved", "u1", (7,))])
 assert DRAVFVGPU_DTYPE.itemsize == 192
+# kxpu_dramdevpf (DRA ResourceSlices of mdev vGPUs with their parent's PF, an addition to ABI v14): one published vGPU
+DRAMDEVPF_DTYPE = np.dtype([("dev", DRAMDEV_DTYPE), ("physfn", "S16"), ("physfn_device", "S8"), ("reserved", "u1", (8,))])
+assert DRAMDEVPF_DTYPE.itemsize == 240
 DRA_SLICE_DEVICES = 128
 DRA_MAX_DEVICES = 1 << 24
 DRA_TAINT_SLICE_DEVICES = 64  # devices per slice of the _taint calls (ABI v11) when taint_since is given
@@ -160,6 +163,7 @@ ABI_SYMBOLS = [
     "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu", "kxpu_pcie_tree_mdev",
     "kxpu_cdi_emit_vf_vgpu", "kxpu_cdi_emit_vf_vgpu_cdev", "kxpu_cdi_parse_vf_vgpu", "kxpu_cdi_parse_vf_vgpu_cdev",
     "kxpu_dra_slices_vf_vgpu", "kxpu_vf_vgpu_drift", "kxpu_reset_check", "kxpu_metrics_devices",
+    "kxpu_mdev_pf", "kxpu_dra_slices_mdev_pf",
 ]
 
 
@@ -291,6 +295,9 @@ def load_library():
         "kxpu_dra_slices_mdev_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                               C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_vf_vgpu": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
+                                          C.POINTER(sz), vp, C.POINTER(sz)]),
+        "kxpu_mdev_pf": (i32, [vp, vp, sz, vp, vp, sz, vp]),
+        "kxpu_dra_slices_mdev_pf": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                           C.POINTER(sz), vp, C.POINTER(sz)]),
     }
     for name, (res, args) in sig.items():
@@ -814,6 +821,23 @@ class Kxpu:
                                     _ptr(gs)))
         return dict(pf_of=pf_of[:n], numvfs=numvfs[:n], group_sriov=gs[:G])
 
+    def mdev_pf(self, recs, mrecs, msrs):
+        """kxpu_mdev_pf: recs (DEVREC_DTYPE) of a PCI walk, mrecs (MDEVREC_DTYPE) and msrs (SRIOVREC_DTYPE, physfn only)
+        of an mdev walk at the same indices.  Returns pf_of, one PCI-record index or NO_PF per mdev."""
+        recs, mrecs, msrs = np.ascontiguousarray(recs), np.ascontiguousarray(mrecs), np.ascontiguousarray(msrs)
+        assert recs.dtype == DEVREC_DTYPE and mrecs.dtype == MDEVREC_DTYPE and msrs.dtype == SRIOVREC_DTYPE
+        assert len(mrecs) == len(msrs)
+        m = len(mrecs)
+        pf_of = np.empty(max(m, 1), np.uint32)
+        self.mdev_pf_raw(recs, mrecs, msrs, pf_of)
+        return pf_of[:m]
+
+    def mdev_pf_raw(self, recs, mrecs, msrs, pf_of):
+        """The bare call into a caller buffer (timing loops, untouched-output checks)."""
+        n, m = len(recs), len(mrecs)
+        self._chk(self.L.kxpu_mdev_pf(self.ctx, _ptr(recs) if n else None, n, _ptr(mrecs) if m else None,
+                                      _ptr(msrs) if m else None, m, _ptr(pf_of) if m else None))
+
     def pcie_tree(self, recs, paths, group_off, group_members, pf_of=None):
         """kxpu_pcie_tree: recs (DEVREC_DTYPE) and paths (PCIPATH_DTYPE) at the same indices, the group CSR of a classify
         call.  Returns dict(group_node, key, parent, depth), the forest trimmed to its node count.  With pf_of (kxpu_sriov's,
@@ -985,6 +1009,12 @@ class Kxpu:
         """kxpu_dra_slices_vf_vgpu: the same for a pool of vGPUs on SR-IOV VFs (DRAVFVGPU_DTYPE devices); since None gives
         the untainted bytes."""
         return self._slices(self.L.kxpu_dra_slices_vf_vgpu, DRAVFVGPU_DTYPE, driver, pool, node, generation, devs,
+                            taints=(taints, since))
+
+    def dra_slices_mdev_pf(self, driver, pool, node, generation, devs, taints, since):
+        """kxpu_dra_slices_mdev_pf: the same for a pool of vGPUs with their parent's PF (DRAMDEVPF_DTYPE devices); since
+        None gives the untainted bytes."""
+        return self._slices(self.L.kxpu_dra_slices_mdev_pf, DRAMDEVPF_DTYPE, driver, pool, node, generation, devs,
                             taints=(taints, since))
 
     def aer_health(self, text, file_off, file_len, fatal_limit, nonfatal_limit, group_off, group_members):

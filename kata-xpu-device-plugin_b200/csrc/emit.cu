@@ -545,6 +545,23 @@ constexpr int MAX_FRAG_DRA_VF_VGPU =
     7 * ((int)sizeof(KX_MS) - 1) + 3 * ((int)sizeof(KX_MI) - 1) + 2 * 10 + 2 + 16 + 6 + 6 + 16 + 64 + 16 + 40 + 10 + 1;
 constexpr int DRAV_PARTS = DRAV_LITS + 2;
 
+// An mdev whose parent may be an SR-IOV VF (kxpu_dra_slices_mdev_pf): the mdev fragment, with physfnAddress and
+// physfnDeviceID (P0, P1, each value closed by MS) between parentVendorID and productName.  The mdev literals keep their
+// indices and P0 / P1 follow them, so the shared code reads the same parts; a record with neither attribute gives the
+// mdev fragment's bytes.  LAYOUT_MDEV_PF is a layout of k_dra_slices only.
+constexpr int LAYOUT_MDEV_PF = 7;
+static_assert(LAYOUT_MDEV_PF != LAYOUT_PCI && LAYOUT_MDEV_PF != LAYOUT_MDEV && LAYOUT_MDEV_PF != LAYOUT_VF_VGPU,
+              "a DRA layout of its own");
+#define KX_P0 ",\"physfnAddress\":{\"string\":\""
+#define KX_P1 ",\"physfnDeviceID\":{\"string\":\""
+constexpr int DRAMP_P0 = DRAM_LITS, DRAMP_P1 = DRAM_LITS + 1, DRAMP_LITS = DRAM_LITS + 2;
+static const char *const h_dramp_lits[DRAMP_LITS] = {KX_M0, KX_M1, KX_M2, KX_M3, KX_M4, KX_M5, KX_M6, KX_M7,
+                                                     KX_M8, KX_M9, KX_MS, KX_MI, KX_ME, KX_P0, KX_P1};
+// the mdev bound, two more literals with their string closers, a 16-byte physfn and a 6-byte id
+constexpr int MAX_FRAG_DRA_MDEV_PF =
+    MAX_FRAG_DRA_MDEV + (int)sizeof(KX_P0 KX_P1) - 1 + 2 * ((int)sizeof(KX_MS) - 1) + 16 + 6;
+constexpr int DRAMP_PARTS = DRAMP_LITS + 2;
+
 // Taints (kxpu_dra_slices[_mdev]_taint[s]).  A device that carries some taint ends with its last literal less that
 // literal's final '}' (the one that closes the device), then KX_TAINTS_OPEN, for each carried taint in table order its
 // entry head (the table's key, value and effect, assembled on the host like the slice head), the 20-byte timeAdded and
@@ -597,6 +614,8 @@ constexpr int DRA_F_PRODUCT = 0, DRA_F_BDF = 1, DRA_F_ROOT = 2, DRA_F_VENDOR = 3
 // the order of the header's domain list, which the oracle's `why` follows
 constexpr int DRAM_F_PRODUCT = 0, DRAM_F_TYPE = 1, DRAM_F_UUID = 2, DRAM_F_PARENT = 3, DRAM_F_ROOT = 4, DRAM_F_VENDOR = 5,
               DRAM_F_DEVICE = 6, DRAM_F_GROUP = 7, DRAM_F_PLEN = 8, DRAM_F_COUNT = 9;
+// kxpu_dramdevpf: the mdev flags for its dev, then its own two
+constexpr int DRAMP_F_PHYSFN = DRAM_F_COUNT, DRAMP_F_PHYSFN_DEVICE = DRAM_F_COUNT + 1, DRAMP_F_COUNT = DRAM_F_COUNT + 2;
 constexpr int DRAV_F_PRODUCT = 0, DRAV_F_KEY = 1, DRAV_F_BDF = 2, DRAV_F_PARENT = 3, DRAV_F_ROOT = 4, DRAV_F_VENDOR = 5,
               DRAV_F_DEVICE = 6, DRAV_F_GROUP = 7, DRAV_F_TYPE_ID = 8, DRAV_F_PLEN = 9, DRAV_F_COUNT = 10;
 
@@ -636,6 +655,10 @@ struct DraVfVgpuSmem {
     uint32_t wsum[EMIT_THREADS / 32];
     uint32_t tile_total;
 };
+template <int T, int FRAG, int POOL>
+struct DraMdevPfSmem : DraMdevSmem<T, FRAG, POOL> {
+    uint8_t xlen[T];     // physfn length | physfn_device length << 5
+};
 template <typename Base, int NT>
 struct DraTaintsSmem : Base {
     uint8_t ts[TAINT_TILE][NT][20];  // timeAdded of taint t of device d
@@ -656,6 +679,14 @@ template <> struct DraLayout<LAYOUT_VF_VGPU> {
     template <int T, int FRAG, int POOL> using Smem = DraVfVgpuSmem<T, FRAG, POOL>;
     static constexpr int PARTS = DRAV_PARTS, LAST = DRAV_E, F_COUNT = DRAV_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_VF_VGPU;
 };
+template <> struct DraLayout<LAYOUT_MDEV_PF> {
+    using Rec = kxpu_dramdevpf;
+    template <int T, int FRAG, int POOL> using Smem = DraMdevPfSmem<T, FRAG, POOL>;
+    static constexpr int PARTS = DRAMP_PARTS, LAST = DRAM_E, F_COUNT = DRAMP_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_MDEV_PF;
+};
+// the mdev record of either mdev layout
+__device__ __forceinline__ const kxpu_dramdev *dram_of(const kxpu_dramdev *r) { return r; }
+__device__ __forceinline__ const kxpu_dramdev *dram_of(const kxpu_dramdevpf *r) { return &r->dev; }
 // one k_dra_slices instantiation for tables of up to NT taints (NT = 0: untainted): LAST is the literal that closes a
 // device; a taint time above the maximum reports F_SINCE, a device with two taints of one key and effect F_DUP
 template <int LAYOUT, int NT> struct DraKernel {
@@ -680,6 +711,9 @@ template <int LAYOUT, int NT> struct DraKernel {
 static_assert(sizeof(DraKernel<LAYOUT_VF_VGPU, KXPU_DRA_MAX_TAINTS>::Smem) <= 227 * 1024 &&
                   2 * (sizeof(DraKernel<LAYOUT_VF_VGPU, 0>::Smem) + 1024) <= 228 * 1024,
               "MAX_FRAG_DRA_VF_VGPU: the VF-vGPU staging outgrew the shared memory");
+static_assert(sizeof(DraKernel<LAYOUT_MDEV_PF, KXPU_DRA_MAX_TAINTS>::Smem) <= 227 * 1024 &&
+                  2 * (sizeof(DraKernel<LAYOUT_MDEV_PF, 0>::Smem) + 1024) <= 228 * 1024,
+              "MAX_FRAG_DRA_MDEV_PF: the mdev-PF staging outgrew the shared memory");
 
 template <int W>
 __device__ __forceinline__ uint32_t byte_at(const uint32_t (&w)[W], int k) { return (w[k >> 2] >> (8 * (k & 3))) & 0xffu; }
@@ -775,9 +809,10 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
         flen = DRA_LIT_TOTAL - E.len[3] - E.len[5] - E.len[6] + 2u * gl + bl + vl + dl + (nl ? E.len[3] + nl : 0u) +
                (pl ? E.len[5] + pl : 0u) + (rl ? E.len[6] + rl : 0u) + (tid + 1u < in_slice ? 1u : 0u);
     }
-    if constexpr (LAYOUT == LAYOUT_MDEV) {
+    if constexpr (LAYOUT == LAYOUT_MDEV || LAYOUT == LAYOUT_MDEV_PF) {
         if (tid < in_slice) {
-            // 208 bytes = 13 uint4; read field by field so that no more than a few of them are live at once
+            // 208 bytes = 13 uint4 (kxpu_dramdevpf: its dev); read field by field so that no more than a few of them are
+            // live at once
             const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const Rec *>(E.devs) + i0 + tid);
             uint32_t pl, tl, bl, rl, vl, dl;
             {  // product_len and product (q12, q0..q3)
@@ -838,6 +873,18 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             flen = E.len[0] + E.len[1] + 2u * gl + li + E.len[2] + tl + ls + E.len[4] + bl + ls + E.len[6] + vl + ls +
                    E.len[9] + 36u + ls + E.len[DRAM_E] + (nl ? E.len[3] + nl + li : 0u) + (dl ? E.len[5] + dl + ls : 0u) +
                    (pl ? E.len[7] + pl + ls : 0u) + (rl ? E.len[8] + rl + ls : 0u) + (tid + 1u < in_slice ? 1u : 0u);
+            if constexpr (LAYOUT == LAYOUT_MDEV_PF) {  // physfn and physfn_device: bytes 208..232 (q13, q14.xy)
+                const uint4 q13 = p[13];
+                const uint2 q14 = reinterpret_cast<const uint2 *>(p + 14)[0];
+                const uint32_t pf[4] = {q13.x, q13.y, q13.z, q13.w}, pd[2] = {q14.x, q14.y};
+                const uint32_t xl = nul_len(pf), yl_raw = nul_len(pd), yl = min(yl_raw, 6u);
+                if (!bytes_ok(pf, 0u, xl, [](uint32_t c) { return is_lhex(c) || c == ':' || c == '.'; }))
+                    E.flags[DRAMP_F_PHYSFN] = 1u;
+                if (yl_raw > 6u || (yl_raw && !xl) || !bytes_ok(pd, 0u, yl, [](uint32_t c) { return is_lhex(c); }))
+                    E.flags[DRAMP_F_PHYSFN_DEVICE] = 1u;
+                S.xlen[tid] = (uint8_t)(xl | yl << 5);
+                flen += (xl ? E.len[DRAMP_P0] + xl + ls : 0u) + (yl ? E.len[DRAMP_P1] + yl + ls : 0u);
+            }
         }
     }
     if constexpr (LAYOUT == LAYOUT_VF_VGPU) {
@@ -1010,16 +1057,22 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             lit(9); put(bytes(r->type_key), tl); lit(DRAV_S);
             lit(10); put(S.dec[d] + 12, il); lit(DRAV_I); close(DraLayout<LAYOUT>::LAST);
         } else {
+            const kxpu_dramdev *m = dram_of(r);
             const uint32_t tl = S.tlen[d];
             lit(0); put(S.dec[d], gl); lit(1); put(S.dec[d], gl); lit(DRAM_I);
-            lit(2); put(bytes(r->mdev_type), tl); lit(DRAM_S);
+            lit(2); put(bytes(m->mdev_type), tl); lit(DRAM_S);
             if (nl) { lit(3); put(S.dec[d] + 10, nl); lit(DRAM_I); }
-            lit(4); put(bytes(r->parent), bl); lit(DRAM_S);
-            if (dl) { lit(5); put(bytes(r->device), dl); lit(DRAM_S); }
-            lit(6); put(bytes(r->vendor), vl); lit(DRAM_S);
-            if (pl) { lit(7); put(r->product, pl); lit(DRAM_S); }
-            if (rl) { lit(8); put(bytes(r->pcie_root), rl); lit(DRAM_S); }
-            lit(9); put(bytes(r->uuid), 36u); lit(DRAM_S); close(DraLayout<LAYOUT>::LAST);
+            lit(4); put(bytes(m->parent), bl); lit(DRAM_S);
+            if (dl) { lit(5); put(bytes(m->device), dl); lit(DRAM_S); }
+            lit(6); put(bytes(m->vendor), vl); lit(DRAM_S);
+            if constexpr (LAYOUT == LAYOUT_MDEV_PF) {
+                const uint32_t x = S.xlen[d], xl = x & 31u, yl = x >> 5;
+                if (xl) { lit(DRAMP_P0); put(bytes(r->physfn), xl); lit(DRAM_S); }
+                if (yl) { lit(DRAMP_P1); put(bytes(r->physfn_device), yl); lit(DRAM_S); }
+            }
+            if (pl) { lit(7); put(m->product, pl); lit(DRAM_S); }
+            if (rl) { lit(8); put(bytes(m->pcie_root), rl); lit(DRAM_S); }
+            lit(9); put(bytes(m->uuid), 36u); lit(DRAM_S); close(DraLayout<LAYOUT>::LAST);
         }
         if (d + 1u < in_slice && lane == 0) dst[o] = (uint8_t)',';
     }
@@ -1640,10 +1693,11 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     using K = DraKernel<LAYOUT, NT>;
     constexpr bool TAINT = K::TAINT;
     constexpr int PARTS = K::PARTS, HEAD = PARTS - 2, TAIL = PARTS - 1;
-    constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : LAYOUT == LAYOUT_MDEV ? DRAM_LITS : DRAV_LITS;
+    constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : LAYOUT == LAYOUT_MDEV ? DRAM_LITS : LAYOUT == LAYOUT_MDEV_PF ? DRAMP_LITS : DRAV_LITS;
     constexpr int MAXF = K::MAXF;
     constexpr int F_COUNT = K::F_COUNT;
-    const char *const *lits = LAYOUT == LAYOUT_PCI ? h_dra_lits : LAYOUT == LAYOUT_MDEV ? h_dram_lits : h_drav_lits;
+    const char *const *lits = LAYOUT == LAYOUT_PCI ? h_dra_lits : LAYOUT == LAYOUT_MDEV ? h_dram_lits
+                              : LAYOUT == LAYOUT_MDEV_PF ? h_dramp_lits : h_drav_lits;
     if (!ctx || !len || !n_slices || (n && !devs)) return KXPU_E_INVALID;
     if (!dns_subdomain_ok(driver, 63) || !dns_subdomain_ok(pool, 253) || !dns_subdomain_ok(node, 253) ||
         generation >= (1ull << 63)) {
@@ -1753,7 +1807,15 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
         "a bdf that is empty or holds a byte outside [0-9a-f:.]", "a parent that is empty or holds a byte outside [0-9a-f:.]",
         "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
         "a device id that is not 0..6 bytes of [0-9a-f]", "iommu_group 4294967295", "type_id 0", "product_len above 64"};
-    const char *const *why = LAYOUT == LAYOUT_PCI ? why_pci : LAYOUT == LAYOUT_MDEV ? why_mdev : why_vf_vgpu;
+    static const char *const why_mdev_pf[DRAMP_F_COUNT] = {
+        "a product byte outside [A-Za-z0-9_.-]", "an mdev_type that is empty or holds a byte outside [A-Za-z0-9_.-]",
+        "a uuid outside the canonical lowercase 8-4-4-4-12 form", "a parent that is empty or holds a byte outside [0-9a-f:.]",
+        "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
+        "a device id that is not 0..6 bytes of [0-9a-f]", "iommu_group 4294967295", "product_len above 64",
+        "a physfn that holds a byte outside [0-9a-f:.]",
+        "a physfn_device that is not 0..6 bytes of [0-9a-f], or is set without a physfn"};
+    const char *const *why = LAYOUT == LAYOUT_PCI ? why_pci : LAYOUT == LAYOUT_MDEV ? why_mdev
+                             : LAYOUT == LAYOUT_MDEV_PF ? why_mdev_pf : why_vf_vgpu;
     const uint32_t *flags = reinterpret_cast<const uint32_t *>(h.data() + slices + 1);
     for (int f = 0; f < F_COUNT; f++)
         if (flags[f]) {
@@ -1861,5 +1923,17 @@ extern "C" int32_t kxpu_dra_slices_vf_vgpu(kxpu_ctx *ctx, const char *driver, co
                       offsetof(kxpu_dravfvgpu, product_len) == 184,
                   "kxpu_dravfvgpu layout");
     return dra_slices_tainted<LAYOUT_VF_VGPU>(ctx, "dra_slices_vf_vgpu", driver, pool, node, generation, devs, n, taints,
+                                              n_taints, taint_since, out, cap, len, slice_off, n_slices);
+}
+
+// the one entry point of the mdev-PF layout: the taint-list form, taint_since == NULL giving the untainted bytes
+extern "C" int32_t kxpu_dra_slices_mdev_pf(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                           uint64_t generation, const kxpu_dramdevpf *devs, size_t n,
+                                           const kxpu_dra_taint *taints, size_t n_taints, const int64_t *taint_since,
+                                           uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
+    static_assert(sizeof(kxpu_dramdevpf) == 240 && alignof(kxpu_dramdevpf) == 8 && offsetof(kxpu_dramdevpf, physfn) == 208 &&
+                      offsetof(kxpu_dramdevpf, physfn_device) == 224,
+                  "kxpu_dramdevpf layout");
+    return dra_slices_tainted<LAYOUT_MDEV_PF>(ctx, "dra_slices_mdev_pf", driver, pool, node, generation, devs, n, taints,
                                               n_taints, taint_since, out, cap, len, slice_off, n_slices);
 }

@@ -11,6 +11,8 @@
 //   - k_sr_fold: one thread per group member finds its group ordinal by binary search over group_off and lowers
 //     group_sriov[o] (all ones from a memset) to its index with an atomic min when it blocks; a member index >= n sets
 //     the error word instead.
+// kxpu_mdev_pf runs the same table with k_sr_insert<true> (one thread per PCI record, its bdf only) and k_sr_probe<true>
+// (one thread per mdev, the physfn of its side record; no verdict); the <false> instantiations are kxpu_sriov's kernels.
 #include "common.cuh"
 
 namespace kxsriov {
@@ -37,6 +39,13 @@ struct Work {
     uint32_t G, m0, m1;          // members [m0, m1) = [goff[0], goff[G])
     uint32_t *group_sriov;
     uint32_t *err;               // [0] = 1: a member index >= n
+};
+
+// kxpu_mdev_pf's probe side: the mdevs whose side records Work::srs are (pf_of has nm entries).  A parameter of its own,
+// after Work and Drivers, so kxpu_sriov's kernels keep their parameter layout
+struct MdevSide {
+    const kxpu_mdevrec *mrecs;
+    uint32_t nm;
 };
 
 __device__ __forceinline__ int hexv(uint32_t c) {
@@ -79,15 +88,28 @@ __device__ __forceinline__ uint32_t parse_numvfs(unsigned long long txt, uint32_
 
 __device__ __forceinline__ uint32_t slot_of(uint32_t key, uint32_t mask) { return kx_hash(key) & mask; }
 
+// the key of physfn (s0: its 16 bytes; flags: the side record's) for a probe, NONE when it cannot match
+__device__ __forceinline__ uint32_t physfn_key(const uint4 &s0, uint32_t flags) {
+    return (flags & KXPU_SR_PHYSFN_ERR) ? NONE : bdf_key(s0);
+}
+
+// MP (kxpu_mdev_pf): the PCI records' bdfs only; their side records are the mdevs', read by the probe
+template <bool MP>
 __global__ void __launch_bounds__(256) k_sr_insert(const Work W) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= W.n) return;
-    const uint4 *sp = reinterpret_cast<const uint4 *>(W.srs + i);
-    const uint4 s0 = sp[0], s1 = sp[1];  // physfn[16]; numvfs_txt[8], numvfs_len, flags, reserved
+    uint4 s0, s1;  // physfn[16]; numvfs_txt[8], numvfs_len, flags, reserved
+    if constexpr (!MP) {
+        const uint4 *sp = reinterpret_cast<const uint4 *>(W.srs + i);
+        s0 = sp[0];
+        s1 = sp[1];
+    }
     const uint4 b0 = reinterpret_cast<const uint4 *>(W.recs + i)[0];  // bdf[16]
-    const uint32_t len = s1.z & 0xffu, flags = (s1.z >> 8) & 0xffu;
-    W.numvfs[i] = parse_numvfs((unsigned long long)s1.y << 32 | s1.x, len, flags);
-    W.pf_of[i] = (flags & KXPU_SR_PHYSFN_ERR) ? NONE : bdf_key(s0);
+    if constexpr (!MP) {
+        const uint32_t len = s1.z & 0xffu, flags = (s1.z >> 8) & 0xffu;
+        W.numvfs[i] = parse_numvfs((unsigned long long)s1.y << 32 | s1.x, len, flags);
+        W.pf_of[i] = physfn_key(s0, flags);
+    }
     const uint32_t key = bdf_key(b0);
     if (key == NONE) return;
     const unsigned long long mine = (unsigned long long)key << 32 | i;
@@ -104,10 +126,24 @@ __global__ void __launch_bounds__(256) k_sr_insert(const Work W) {
     }
 }
 
-__global__ void __launch_bounds__(256) k_sr_probe(const Work W, const __grid_constant__ Drivers D) {
+// MP (kxpu_mdev_pf): thread i is mdev i; its key comes from its side record, a physfn equal to its parent never matches,
+// and there is no verdict
+template <bool MP>
+__global__ void __launch_bounds__(256) k_sr_probe(const Work W, const __grid_constant__ Drivers D, const MdevSide M) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= W.n) return;
-    const uint32_t key = W.pf_of[i];
+    uint32_t key;
+    if constexpr (MP) {
+        if (i >= M.nm) return;
+        const uint4 *sp = reinterpret_cast<const uint4 *>(W.srs + i);
+        key = physfn_key(sp[0], (sp[1].z >> 8) & 0xffu);
+        // parent: bytes 36..51 of the mdev record, 4-byte aligned
+        const uint32_t *pw = reinterpret_cast<const uint32_t *>(reinterpret_cast<const uint8_t *>(M.mrecs + i) + 36);
+        const uint4 par = make_uint4(pw[0], pw[1], pw[2], pw[3]);
+        if (key != NONE && bdf_key(par) == key) key = NONE;
+    } else {
+        if (i >= W.n) return;
+        key = W.pf_of[i];
+    }
     uint32_t p = NO_PF;
     if (key != NONE) {
         for (uint32_t s = slot_of(key, W.mask);; s = (s + 1) & W.mask) {
@@ -118,9 +154,10 @@ __global__ void __launch_bounds__(256) k_sr_probe(const Work W, const __grid_con
                 break;
             }
         }
-        if (p == i) p = NO_PF;
+        if (!MP && p == i) p = NO_PF;
     }
     W.pf_of[i] = p;
+    if constexpr (MP) return;
     bool blocks = W.numvfs[i] > 0;
     if (p != NO_PF) {  // the PF's driver (bytes 32..47) and flags (byte 54)
         const uint4 *rp = reinterpret_cast<const uint4 *>(W.recs + p);
@@ -216,8 +253,8 @@ extern "C" int32_t kxpu_sriov(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t 
         KxTimer tm(ctx, KXPU_T_CLASSIFY);
         if (n) {
             const unsigned g = (unsigned)((n + 255) / 256);
-            k_sr_insert<<<g, 256, 0, st>>>(W);
-            k_sr_probe<<<g, 256, 0, st>>>(W, D);
+            k_sr_insert<false><<<g, 256, 0, st>>>(W);
+            k_sr_probe<false><<<g, 256, 0, st>>>(W, D, MdevSide{nullptr, 0});
             ctx->launches += 2;
         }
         if (m1 > m0) {
@@ -237,5 +274,53 @@ extern "C" int32_t kxpu_sriov(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t 
     if (n_groups) cudaMemcpyAsync(group_sriov, W.group_sriov, n_groups * 4, cudaMemcpyDeviceToHost, st);
     e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) { KX_SET_ERR(ctx, "sriov D2H failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    return KXPU_OK;
+}
+
+extern "C" int32_t kxpu_mdev_pf(kxpu_ctx *ctx, const kxpu_devrec *recs, size_t n_recs, const kxpu_mdevrec *mrecs,
+                                const kxpu_sriovrec *msrs, size_t n_mdevs, uint32_t *pf_of) {
+    static_assert(offsetof(kxpu_mdevrec, parent) == 36 && sizeof(kxpu_mdevrec) % 16 == 0, "kxpu_mdevrec layout");
+    if (!ctx || (n_recs && !recs) || (n_mdevs && (!mrecs || !msrs || !pf_of))) return KXPU_E_INVALID;
+    if (n_recs >= (1ull << 30) || n_mdevs >= (1ull << 30)) return KXPU_E_UNSUPPORTED;  // as kxpu_sriov's table
+    if (n_mdevs == 0) return KXPU_OK;
+
+    std::lock_guard<std::mutex> guard(ctx->mu);
+    cudaSetDevice(ctx->device);
+    kx_clear_timings(ctx);
+    size_t cap = 1024;
+    while (cap < 2 * n_recs) cap <<= 1;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
+    const size_t o_recs = take(n_recs * sizeof(kxpu_devrec)), o_mrecs = take(n_mdevs * sizeof(kxpu_mdevrec));
+    const size_t o_srs = take(n_mdevs * sizeof(kxpu_sriovrec)), o_slots = take((size_t)cap * 8), o_pf = take(n_mdevs * 4);
+    KxScratch sc(ctx);
+    uint8_t *b = nullptr;
+    KX_CUDA(ctx, sc.alloc((void **)&b, off));
+    cudaStream_t st = ctx->stream;
+    auto up = [&](size_t o, const void *h, size_t bytes) { if (bytes) cudaMemcpyAsync(b + o, h, bytes, cudaMemcpyHostToDevice, st); };
+    up(o_recs, recs, n_recs * sizeof(kxpu_devrec));
+    up(o_mrecs, mrecs, n_mdevs * sizeof(kxpu_mdevrec));
+    up(o_srs, msrs, n_mdevs * sizeof(kxpu_sriovrec));
+    cudaMemsetAsync(b + o_slots, 0xFF, (size_t)cap * 8, st);
+    Work W;
+    memset(&W, 0, sizeof W);
+    W.recs = (const kxpu_devrec *)(b + o_recs); W.srs = (const kxpu_sriovrec *)(b + o_srs); W.n = (uint32_t)n_recs;
+    W.slots = (unsigned long long *)(b + o_slots); W.mask = (uint32_t)(cap - 1);
+    W.pf_of = (uint32_t *)(b + o_pf);
+    const MdevSide M{(const kxpu_mdevrec *)(b + o_mrecs), (uint32_t)n_mdevs};
+    Drivers D;
+    memset(&D, 0, sizeof D);  // not read: the mdev probe gives no verdict
+    {
+        KxTimer tm(ctx, KXPU_T_CLASSIFY);
+        if (n_recs) {
+            k_sr_insert<true><<<(unsigned)((n_recs + 255) / 256), 256, 0, st>>>(W);
+            ctx->launches++;
+        }
+        k_sr_probe<true><<<(unsigned)((n_mdevs + 255) / 256), 256, 0, st>>>(W, D, M);
+        ctx->launches++;
+    }
+    cudaMemcpyAsync(pf_of, W.pf_of, n_mdevs * 4, cudaMemcpyDeviceToHost, st);
+    const cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "mdev_pf failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
     return KXPU_OK;
 }

@@ -1100,6 +1100,7 @@ Error Plugin::classify(PciWalk &w) {
     Error e = gatherRecordsFast(w.recs, 0, &w.paths, &w.cdevs, &w.srs);  // same records as gatherRecords (falls back to it when a seam was replaced)
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // Walk's error is ignored by the reference (:132)
     readResets(w.recs, w.rrs);
+    if (vgpuSriovAware) pciRecs_ = w.recs;  // the mdev walk that follows joins its parents' PFs against them
     const std::vector<kxpu_devrec> &recs = w.recs;
     const size_t n = recs.size();
     ClassifyResult &c = w.out;
@@ -1332,8 +1333,9 @@ static void mdevRecord(Plugin &p, const std::string &name, bool isDir, kxpu_mdev
 // holds one level of links, so a directory inside it is recorded as such and not descended into.
 Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w) {
     recs.clear();
-    if (w) { w->parentDevice.clear(); w->pcieRoot.clear(); w->paths.clear(); w->cdevs.clear(); }
+    if (w) { w->parentDevice.clear(); w->pcieRoot.clear(); w->paths.clear(); w->cdevs.clear(); w->srs.clear(); }
     std::vector<int64_t> *cdevs = w && mdevCdevEnabled() ? &w->cdevs : nullptr;
+    std::vector<kxpu_sriovrec> *srs = w && vgpuSriovAware ? &w->srs : nullptr;
     const bool dra = vgpuDraEnabled();
     if (!readsMdevPaths()) w = nullptr;
     DIR *d = opendir(mdevBasePath.c_str());
@@ -1355,6 +1357,19 @@ Error Plugin::gatherMdevRecords(std::vector<kxpu_mdevrec> &recs, MdevWalk *w) {
         if (cdevs)
             cdevs->push_back(cdevClassOf(vgpuClasses, &XpuClass::mdevCdev, r, r.parent_vendor_txt, sizeof r.parent_vendor_txt)
                                  ? readVfioCdev(mdevBasePath, n) : -1);
+        if (srs) {  // the physfn link of an entry that got as far as its iommu_group link; none: the parent is no VF
+            kxpu_sriovrec s;
+            memset(&s, 0, sizeof s);
+            std::string pf;
+            if (!isDir && n.size() == sizeof r.uuid && !(r.flags & (KXPU_REC_VENDOR_ERR | KXPU_REC_DRIVER_ERR | KXPU_REC_IOMMU_ERR))) {
+                mdevPhysfnReads++;
+                if (readLink(mdevBasePath, n, "../physfn", pf)) {
+                    if (pf.size() < sizeof s.physfn) memcpy(s.physfn, pf.data(), pf.size());
+                    else s.flags |= KXPU_SR_PHYSFN_ERR;  // no PCI address is this long
+                }
+            }
+            srs->push_back(s);
+        }
         if (!w) continue;
         // the ResourceSlice and PCIe forest reads of an entry that got as far as its iommu_group link
         std::string dev, target;
@@ -1432,6 +1447,11 @@ Error Plugin::classify(MdevWalk &w) {
     if (e) { fprintf(stderr, "%s\n", e.message.c_str()); }  // like the PCI walk: an unreadable bus is an empty one
     const std::vector<kxpu_mdevrec> &recs = w.recs;
     const size_t n = recs.size();
+    if (vgpuSriovAware) {  // each mdev's PF in the PCI walk, which ran first
+        w.pfOf.assign(n + 1, KXPU_NO_PF);
+        const int32_t rc = kxpu_mdev_pf(ctx_, pciRecs_.data(), pciRecs_.size(), recs.data(), w.srs.data(), n, w.pfOf.data());
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_mdev_pf", rc);
+    }
     ClassifyResult &c = w.out;
     kxpu_classify_out out = c.wire(n);
     const std::vector<kxpu_xpu_rule> rules = classRules(vgpuClasses);
@@ -1482,6 +1502,10 @@ void Plugin::buildMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
         s.klass = groupClass[c.gids[g]];
         if (topologyAware) s.numa = c.gnuma[g];
         if (vgpuPcieTopologyAware) s.pcieNode = w.gnode[g];
+        if (vgpuSriovAware && w.pfOf[c.gmem[c.goff[g]]] != KXPU_NO_PF) {
+            const kxpu_devrec &pf = pciRecs_[w.pfOf[c.gmem[c.goff[g]]]];
+            s.pf.assign(pf.bdf, strnlen(pf.bdf, sizeof pf.bdf));
+        }
         if (vgpuClasses[s.klass].mdevCdev)  // an mdev without a cdev: VFIO cannot open it
             for (const MdevDevice &m : devs)
                 if (m.cdev < 0) { s.blocker = m.uuid + " has no VFIO cdev"; s.blockerKind = KXPU_MR_VFIO_CDEV_MISSING; break; }
@@ -1513,6 +1537,8 @@ void Plugin::buildMdevDra(const MdevWalk &w) {
     std::map<std::pair<std::string, std::string>, size_t> idAt;  // (vendor, device) -> position in the lookup batch
     std::vector<std::string> ids, vendors;
     std::vector<std::pair<std::string, std::string>> idOf;  // per group
+    std::vector<std::pair<uint32_t, std::pair<std::string, std::string>>> pfIds;  // (group, its PF's ids)
+    std::map<std::string, std::string> pfDeviceRead;  // PF address -> its device file, for PFs the walk did not read
     for (uint32_t g = 0; g < c.nGroups; g++) {
         const uint32_t first = c.gmem[c.goff[g]];
         const kxpu_mdevrec &r = w.recs[first];
@@ -1536,8 +1562,33 @@ void Plugin::buildMdevDra(const MdevWalk &w) {
             ids.push_back(device);
             vendors.push_back(vendor);
         }
+        if (!mdevState[g].pf.empty()) {  // vgpuSriovAware: the PF's ids from its own record in the PCI walk
+            const kxpu_devrec &pf = pciRecs_[w.pfOf[first]];
+            const std::string pv = trimID(std::string((const char *)pf.vendor_txt, std::min<size_t>(pf.vendor_len, sizeof pf.vendor_txt)));
+            std::string pd = (pf.flags & KXPU_REC_DEVICE_ERR) ? std::string()
+                             : trimID(std::string((const char *)pf.device_txt, std::min<size_t>(pf.device_len, sizeof pf.device_txt)));
+            if (pd.empty() && !pfDeviceRead.count(mdevState[g].pf)) {  // a PF that is no class candidate: the walk left
+                std::string raw;                                       // its device id unread; read it once here
+                pfDeviceRead[mdevState[g].pf] = readIDFromFile(basePath, mdevState[g].pf, "device", raw) ? trimID(raw) : "";
+            }
+            if (pd.empty()) pd = pfDeviceRead[mdevState[g].pf];
+            bool ok = pd.size() <= 6;
+            for (char ch : pd) ok = ok && ((ch >= '0' && ch <= '9') || (ch >= 'a' && ch <= 'f'));
+            if (!ok) pd.clear();
+            mdevState[g].pfDevice = pd;
+            if (!pd.empty() && idAt.emplace(std::make_pair(pv, pd), ids.size()).second) {
+                ids.push_back(pd);
+                vendors.push_back(pv);
+            }
+            pfIds.emplace_back(g, std::make_pair(pv, pd));
+        }
     }
     const std::vector<std::string> names = ids.empty() ? std::vector<std::string>() : getDeviceNames(ids, vendors);
+    for (const auto &gi : pfIds) {
+        if (gi.second.second.empty()) continue;
+        const std::string &name = names[idAt[gi.second]];
+        mdevState[gi.first].pfProduct = (name.empty() ? gi.second.second : name).substr(0, sizeof(kxpu_dramdev::product));
+    }
     for (size_t g = 0; g < mdevState.size(); g++) {
         if (idOf[g].second.empty()) continue;  // no device id: no productName
         const std::string &name = names[idAt[idOf[g]]];
@@ -2075,6 +2126,7 @@ Error Plugin::InitiateDevicePlugin() {
     Error e = checkDraClasses();
     if (!e) e = checkVfVgpuClasses();
     if (!e) e = checkResetMethods();
+    if (!e && vgpuSriovAware && vgpuClasses.empty()) e = fail("vgpuSriovAware is set but no vGPU class is configured");
     if (e) return e;
     e = createIommuDeviceMap();  // :46
     if (e) return e;
@@ -2672,7 +2724,8 @@ Error Plugin::computeAer() {
     for (auto &s : mdevState) set(s, std::string(), 0);
     if (!aerHealth) return Error();  // no aer_dev_* file is opened
     // one record per member of every group, passthrough groups then vGPU groups; a vGPU reads its parent's files.  With
-    // vfVgpuHealth a group whose first member is a VF of a vfVgpu class has its PF as one more member, one record per PF.
+    // vfVgpuHealth a group whose first member is a VF of a vfVgpu class, and with vgpuSriovAware a vGPU group whose first
+    // mdev's parent is a VF, has its PF as one more member, one record per PF.
     std::string text;
     std::vector<uint64_t> off;
     std::vector<uint32_t> len, goff{0}, members;
@@ -2701,8 +2754,14 @@ Error Plugin::computeAer() {
         }
         goff.push_back((uint32_t)members.size());
     }
-    for (const auto &kv : mdevMap) {
-        for (const MdevDevice &m : kv.second) members.push_back(read(mdevBasePath, m.uuid + "/..", m.parent));
+    for (size_t g = 0; g < mdevMap.size(); g++) {
+        for (const MdevDevice &m : mdevMap[g].second) members.push_back(read(mdevBasePath, m.uuid + "/..", m.parent));
+        const std::string &pf = mdevState[g].pf;  // set only under vgpuSriovAware
+        if (!pf.empty()) {
+            auto it = pfRecord.find(pf);
+            if (it == pfRecord.end()) it = pfRecord.emplace(pf, read(basePath, pf, pf)).first;
+            members.push_back(it->second);
+        }
         goff.push_back((uint32_t)members.size());
     }
     const size_t n = who.size(), G = goff.size() - 1;
@@ -2882,12 +2941,30 @@ Error Plugin::VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, st
     if (vgpuClass >= vgpuClasses.size() || vgpuClasses[vgpuClass].draDriver.empty())
         return fail("VgpuResourceSlices: vGPU class " + std::to_string(vgpuClass) + " has no DRA driver");
     std::vector<kxpu_dramdev> devs;
+    std::vector<kxpu_dramdevpf> pfDevs;  // vgpuSriovAware: the same devices with their PFs
     std::vector<std::string> groups;
     forPublished(mdevMap, mdevState, vgpuClasses, [&](const std::string &g, const GroupState<kxpu_dramdev> &s) {
         if (s.klass != vgpuClass) return;
-        devs.push_back(*s.dra);
         groups.push_back(g);
+        if (!vgpuSriovAware) {
+            devs.push_back(*s.dra);
+            return;
+        }
+        kxpu_dramdevpf d;
+        memset(&d, 0, sizeof d);
+        d.dev = *s.dra;
+        memcpy(d.physfn, s.pf.data(), std::min(s.pf.size(), sizeof d.physfn));
+        memcpy(d.physfn_device, s.pfDevice.data(), std::min(s.pfDevice.size(), sizeof d.physfn_device));
+        if (!s.pfProduct.empty()) {  // the GPU's model, not the VF's
+            memset(d.dev.product, 0, sizeof d.dev.product);
+            d.dev.product_len = (uint8_t)std::min(s.pfProduct.size(), sizeof d.dev.product);
+            memcpy(d.dev.product, s.pfProduct.data(), d.dev.product_len);
+        }
+        pfDevs.push_back(d);
     });
+    if (vgpuSriovAware)
+        return draSlices(kxpu_dra_slices_mdev_pf, "kxpu_dra_slices_mdev_pf", vgpuClasses[vgpuClass].draDriver,
+                         mdev_.draGeneration, pfDevs, groups, out, sliceOff);
     return draSlices(kxpu_dra_slices_mdev_taints, "kxpu_dra_slices_mdev_taints", vgpuClasses[vgpuClass].draDriver,
                      mdev_.draGeneration, devs, groups, out, sliceOff);
 }
@@ -4295,6 +4372,8 @@ int kxh_devs_aer(void *h, int plugin_index, char *out, size_t cap) {
 
 // ---- health of vGPUs on SR-IOV VFs (kxpu_vf_vgpu_drift)
 void kxh_set_vf_vgpu_health(void *h, int on) { ((Plugin *)h)->vfVgpuHealth = on != 0; }
+void kxh_set_vgpu_sriov(void *h, int on) { ((Plugin *)h)->vgpuSriovAware = on != 0; }
+uint64_t kxh_mdev_physfn_reads(void *h) { return ((Plugin *)h)->mdevPhysfnReads; }
 // refreshVfVgpuTypes: changed as kxh_refresh_aer_health's; *moved = bit 0 passthroughMoved, bit 1 typesMoved
 int kxh_refresh_vf_vgpu_types(void *h, size_t *changed, size_t cap, size_t *n_changed, int *moved, char *err, size_t errcap) {
     std::vector<size_t> c;

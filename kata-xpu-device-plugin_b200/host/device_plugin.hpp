@@ -306,6 +306,10 @@ struct MdevWalk {
     uint32_t nNodes = 0;
     // mdevCdevEnabled only, one per record: N of its VFIO cdev, -1 = none or not read
     std::vector<int64_t> cdevs;
+    // vgpuSriovAware only, one per record: its physfn read (kxpu_sriovrec, physfn only) and kxpu_mdev_pf's answer, the
+    // PF's index in the PCI walk's records or KXPU_NO_PF
+    std::vector<kxpu_sriovrec> srs;
+    std::vector<uint32_t> pfOf;
 };
 
 // The host state of one IOMMU group of a walk (Plugin::iommuState / mdevState, same positions as iommuMap / mdevMap).
@@ -334,8 +338,12 @@ struct GroupState {
     // vfVgpuDraEnabled, a group of a class with a vgpuDraDriver whose first member is a VF that carries a named vGPU type:
     // its VF-vGPU ResourceSlice record; none = unpublished
     std::optional<kxpu_dravfvgpu> vfVgpuDra{};
-    // vfVgpuHealth, a group of a vfVgpu class whose first member is a VF: the PF's address (its physfn basename)
+    // vfVgpuHealth, a group of a vfVgpu class whose first member is a VF: the PF's address (its physfn basename);
+    // vgpuSriovAware, a vGPU group whose first mdev's parent is a VF of a PF in the PCI walk: that PF's address
     std::string pf{};
+    // vgpuSriovAware and vgpuDraEnabled, a vGPU group with a pf: the PF's device id and model name (getDeviceNames);
+    // "" = not known
+    std::string pfDevice{}, pfProduct{};
     // vfVgpuHealth: the drift reason of the group's first member (Device::drift); empty = its type is the walk's
     std::string drift{};
 };
@@ -511,6 +519,20 @@ class Plugin {
     //   - with draTaints, a drifted group in a vgpuDraDriver pool carries <vgpuDraDriver>/vgpu-type=changed:NoSchedule,
     //     a fourth entry of that pool's taint table, and PrepareDraDevices refuses it.
     bool vfVgpuHealth = false;
+    // mdev vGPUs on SR-IOV virtual functions (include/kxpu.h, kxpu_mdev_pf).  Refused by InitiateDevicePlugin unless some
+    // vGPU class is configured.  On vGPU releases before the vendor-specific VFIO framework, an SR-IOV GPU's mdevs are
+    // created on its VFs, so the mdev walk's parent is a VF.  false (default): nothing more is opened and every output,
+    // generation and counter is as above.  true:
+    //   - the mdev walk reads <uuid>/../physfn (readLink) of every entry that got as far as its iommu_group link, and
+    //     kxpu_mdev_pf joins it to the PCI walk's records; a group whose first mdev's parent is a VF keeps its PF's
+    //     address (GroupState::pf);
+    //   - with aerHealth the PF's aer_dev_* files count as one more member of that group, each PF read once per call:
+    //     errors of the whole GPU are logged on the PF, and a VF may have no files of its own;
+    //   - VgpuResourceSlices publishes through kxpu_dra_slices_mdev_pf: such a vGPU carries physfnAddress, the PF's
+    //     device id as physfnDeviceID and the PF's model name as productName, so claims can group or spread vGPUs by
+    //     physical GPU.  A vGPU whose parent is not a VF is published exactly as without the setting.
+    bool vgpuSriovAware = false;
+    std::atomic<uint64_t> mdevPhysfnReads{0};  // <uuid>/../physfn links read (tests, metrics)
     // (type ID, type key) of every vGPU type a walk of this process named: the last name table of kxpu_vf_vgpu_types, so a
     // GPU that became full keeps its names across rediscover
     const std::map<uint32_t, std::string> &learnedVgpuTypes() const { return learnedVgpuTypes_; }
@@ -695,6 +717,7 @@ class Plugin {
     void readCdevs(const std::vector<kxpu_devrec> &recs, std::vector<int64_t> *cdevs);
     void readSriovs(const std::vector<kxpu_devrec> &recs, std::vector<kxpu_sriovrec> *srs);
     std::map<uint32_t, std::string> learnedVgpuTypes_;
+    std::vector<kxpu_devrec> pciRecs_;  // vgpuSriovAware only: the last PCI walk's records, which kxpu_mdev_pf joins against
     // vfVgpu: the nvidia/ reads of every VF of such a class into w, then the type join (kxpu_vf_vgpu_types)
     void readVfVgpus(PciWalk &w);
     Error joinVgpuTypes(PciWalk &w);

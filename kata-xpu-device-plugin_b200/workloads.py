@@ -754,6 +754,42 @@ def sriov_walk(n=1 << 20, seed=41):
     return recs, srs
 
 
+
+def mdev_pf_walk(n_recs=1 << 20, n_pfs=1 << 15, n_mdevs=1 << 20, seed=91):
+    """kxpu_mdev_pf's input at scale: a PCI walk of n_recs records (DEVREC_DTYPE, canonical bdfs in walk order) in which
+    record k * (n_recs // n_pfs) is the PF of card k < n_pfs and the records after it are its VFs, and n_mdevs mdevs
+    (MDEVREC_DTYPE, parent only) with their side records (SRIOVREC_DTYPE, physfn only).  An mdev sits on a random VF and
+    names that VF's PF, except: 1 in 16 sits on a PF (no physfn), and 1 in 16 has a link that cannot resolve -- a
+    non-canonical address, a failed read, a PF outside the walk, or a link to its own parent, in turn.  Returns (recs, mrecs,
+    msrs, want), want being the pf_of the header's rules give."""
+    from .binding import MDEVREC_DTYPE, NO_PF, SR_PHYSFN_ERR, SRIOVREC_DTYPE
+    rng = np.random.default_rng(seed)
+    per = n_recs // n_pfs
+    recs = np.zeros(n_recs, dtype=DEVREC_DTYPE)
+    bdf = enumerate_bdfs(n_recs).view("S16").reshape(n_recs)
+    recs["bdf"] = bdf
+    recs["driver"] = b"nvidia"
+    recs["vendor_txt"] = _id_text(np.full(n_recs, 0x10DE))
+    recs["device_txt"] = _id_text(np.full(n_recs, 0x2330))
+    recs["vendor_len"] = recs["device_len"] = 7
+    recs["iommu_group"] = np.arange(n_recs) + 1
+    card = rng.integers(0, n_pfs, n_mdevs)
+    pf = card * per
+    vf = pf + rng.integers(1, per, n_mdevs)
+    kind = rng.integers(0, 64, n_mdevs)  # 0..3: an unresolvable link; 4..7: an mdev on a PF; else on a VF
+    on_pf = (kind >= 4) & (kind < 8)
+    mrecs = np.zeros(n_mdevs, dtype=MDEVREC_DTYPE)
+    mrecs["uuid"] = uuids(n_mdevs, seed).view("S36").reshape(n_mdevs)
+    mrecs["parent"] = np.where(on_pf, bdf[pf], bdf[vf])
+    msrs = np.zeros(n_mdevs, dtype=SRIOVREC_DTYPE)
+    msrs["physfn"] = np.where(on_pf, b"", bdf[pf])
+    msrs["physfn"] = np.where(kind == 0, np.char.replace(bdf[pf], b":", b"-"), msrs["physfn"])
+    msrs["flags"] = np.where(kind == 1, SR_PHYSFN_ERR, 0)
+    msrs["physfn"] = np.where(kind == 2, b"ffff:ff:1f.7", msrs["physfn"])
+    msrs["physfn"] = np.where(kind == 3, mrecs["parent"], msrs["physfn"])
+    want = np.where(kind >= 8, pf, NO_PF).astype(np.uint32)
+    return recs, mrecs, msrs, want
+
 # An H100 80GB vGPU type table: (type ID, name).  The IDs are synthetic; the names follow NVIDIA's time-sliced and
 # MIG-backed C-series profiles.
 H100_VGPU_TYPES = [(1000 + k, n) for k, n in enumerate(

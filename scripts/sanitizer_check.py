@@ -76,6 +76,14 @@ sv = kx.sriov([(b"10de", b"vfio-pci")], srecs, ssrs, sres["group_ids"], sres["gr
 ppf = np.where(np.arange(len(precs)) & 7, np.arange(len(precs)) & ~7, B.NO_PF).astype(np.uint32)
 print("sriov withheld", int((sv["group_sriov"] != B.VIABLE).sum()), "pcie sriov nodes",
       len(kx.pcie_tree(precs, ppaths, poff, pmem, ppf)["key"]))
+# mdev vGPUs on SR-IOV VFs: each mdev's PF joined against a PCI walk, and the slices with each vGPU's PF
+mprecs, mpm, mps, mpwant = W.mdev_pf_walk(20480, 640, 20000)
+assert np.array_equal(kx.mdev_pf(mprecs, mpm, mps), mpwant)
+mpdevs = np.zeros(300, B.DRAMDEVPF_DTYPE)
+mpdevs["dev"] = W.dra_mdev_devices(300)
+mpdevs["physfn"][::2], mpdevs["physfn_device"][::2] = b"0000:41:00.0", b"2330"
+print("mdev_pf resolved", int((mpwant != B.NO_PF).sum()), "slice bytes",
+      len(kx.dra_slices_mdev_pf("d", "p", "n", 1, mpdevs, [("d/k", "", "NoSchedule")], np.full((300, 1), 5, np.int64))[0]))
 # resets between tenants: every member's function reset or bus-reset set, on the classify CSR
 rrecs, rpaths, rrrs = W.reset_walk(20000)
 rres = kx.classify_rules([(b"10de", b"vfio-pci")], rrecs)
