@@ -731,6 +731,46 @@ int32_t kxpu_classify_vf_vgpu(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t 
                               kxpu_classify_out *out, uint8_t *dev_rule /* [n] */, uint64_t *group_numa /* [n] or NULL */,
                               uint32_t *group_blocker /* [n] or NULL */);
 
+/* ------------------------------------------- configured resource names (addition to ABI v14) */
+
+/* One entry of kxpu_classify_named's name table.  16 bytes.  Added to ABI v14 without a version bump: a caller detects
+ * the call by symbol, as for kxpu_sriov. */
+typedef struct kxpu_name_entry {
+    uint32_t rule;       /* index into the rule list                                                         */
+    uint32_t slot;       /* the name's slot, < n_names; entries that share a slot share one deviceMap entry   */
+    char     device[8];  /* a device id exactly as readIDFromFile returns it, 4 lowercase hex digits ("2330"),
+                            or "*" (every other id of the rule); NUL padded                                   */
+} kxpu_name_entry;
+#define KXPU_MAX_NAMES 64
+#define KXPU_NO_SLOT   0xFFFFFFFFu
+
+/* kxpu_classify_vf_vgpu with deviceMap entries keyed by configured resource names.  A candidate of rule r whose device
+ * read works and whose bit in vgpu_rules is clear takes the slot of the entry (r, its device id) when there is one, else
+ * the slot of (r, "*"), else none.  The id is compared with its length: only a 4-byte id matches a listed one.
+ *   - the deviceMap key of a group whose first member has slot s is (r, s) instead of (r, device id); a group whose
+ *     first member has no slot keeps kxpu_classify_rules' key, and a vGPU rule's group kxpu_classify_vf_vgpu's.  Two ids
+ *     with one slot share one entry, whose groups stay in first-seen walk order like every entry's;
+ *   - dev_slot[d] (caller array of n entries) is the slot of entry d, or KXPU_NO_SLOT;
+ *   - dev_ids[d] of a slotted entry is the lowest index of a candidate that has its (rule, slot), whether or not that
+ *     candidate is the first member of a group (kxpu_classify_vf_vgpu's convention); of every other entry it keeps
+ *     kxpu_classify_vf_vgpu's meaning;
+ *   - every other output (dev_rule, group_numa, group_blocker included) means what it means in kxpu_classify_vf_vgpu.
+ * With n_names == 0 (names and dev_slot may then be NULL) every output is bitwise kxpu_classify_vf_vgpu's and dev_slot is
+ * not written.
+ * KXPU_E_INVALID, and nothing written: kxpu_classify_vf_vgpu's cases; n_names > KXPU_MAX_NAMES; names == NULL, or
+ * dev_slot == NULL with n > 0, when n_names > 0; an entry whose rule is >= n_rules or has its bit set in vgpu_rules
+ * (vGPU types are named by their type keys); a device that is neither 4 lowercase hex digits nor "*", NUL padded; two
+ * entries with one (rule, device); a slot >= n_names.
+ * GPU: kxpu_classify_vf_vgpu's launches and one more.  The candidate pass looks the id up in the table (a
+ * __grid_constant__ parameter, compared at constant indices) and writes a name row that the type-key intern pass interns
+ * with the type keys; the per-group pass is a compile-time variant; one thread per group then writes dev_slot.  Every
+ * existing kernel is unchanged. */
+int32_t kxpu_classify_named(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, uint32_t vgpu_rules,
+                            const kxpu_devrec *recs, size_t n, const kxpu_vgpukey *keys /* [n] or NULL */,
+                            const kxpu_name_entry *names /* [n_names] */, size_t n_names, kxpu_classify_out *out,
+                            uint8_t *dev_rule /* [n] */, uint32_t *dev_slot /* [n] */, uint64_t *group_numa /* [n] or NULL */,
+                            uint32_t *group_blocker /* [n] or NULL */);
+
 /* kxpu_vf_vgpu_drift's per-record status */
 #define KXPU_VD_SAME    0u  /* the type read back is the walk's (also a record without KXPU_VT_READ: not compared)  */
 #define KXPU_VD_CLEARED 1u  /* the type is 0 now: the vGPU was destroyed                                          */

@@ -191,6 +191,8 @@ func (k *kxpu) allocNames(idx []uint64) ([]string, error) {
 // "nvidia.com/gpu", "cdi-vfio-xxxx"}.
 type xpuClass struct {
 	Vendor, Driver, Namespace, Kind, FileStem string
+	// device id ("2330") or "*" -> resource name (kxpu_classify_named); nil: named by pci.ids, one resource per id
+	ResourceNames map[string]string
 }
 
 // S1 with a class list: one rule per class (rule index == class index).  devRule[d] is the class of deviceMap

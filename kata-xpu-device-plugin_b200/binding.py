@@ -99,6 +99,11 @@ VFVGPUREC_DTYPE = np.dtype([("cur_txt", "u1", (16,)), ("cur_len", "u1"), ("flags
 assert VFVGPUREC_DTYPE.itemsize == 32
 VGPUKEY_DTYPE = np.dtype([("key", "u1", (40,)), ("zero", "u1", (7,)), ("len", "u1")])
 assert VGPUKEY_DTYPE.itemsize == 48
+# kxpu_name_entry: one entry of kxpu_classify_named's name table
+NAME_DTYPE = np.dtype([("rule", "<u4"), ("slot", "<u4"), ("device", "S8")])
+assert NAME_DTYPE.itemsize == 16
+MAX_NAMES = 64
+NO_SLOT = 0xFFFFFFFF
 VT_READ, VT_CUR_ERR = 1, 2
 VT_NONE, VT_NAMED, VT_UNNAMED, VT_BAD = 0, 1, 2, 3
 VD_SAME, VD_CLEARED, VD_CHANGED, VD_BAD = 0, 1, 2, 3  # kxpu_vf_vgpu_drift's per-record status
@@ -163,7 +168,7 @@ ABI_SYMBOLS = [
     "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu", "kxpu_pcie_tree_mdev",
     "kxpu_cdi_emit_vf_vgpu", "kxpu_cdi_emit_vf_vgpu_cdev", "kxpu_cdi_parse_vf_vgpu", "kxpu_cdi_parse_vf_vgpu_cdev",
     "kxpu_dra_slices_vf_vgpu", "kxpu_vf_vgpu_drift", "kxpu_reset_check", "kxpu_metrics_devices",
-    "kxpu_mdev_pf", "kxpu_dra_slices_mdev_pf",
+    "kxpu_mdev_pf", "kxpu_dra_slices_mdev_pf", "kxpu_classify_named",
 ]
 
 
@@ -288,6 +293,7 @@ def load_library():
         "kxpu_reset_check": (i32, [vp, vp, sz, vp, vp, vp, sz, C.c_uint32, vp, vp, sz, vp, vp, vp]),
         "kxpu_metrics_devices": (i32, [vp, vp, sz, vp, sz, vp, sz, vp, sz, C.POINTER(sz)]),
         "kxpu_classify_vf_vgpu": (i32, [vp, vp, sz, C.c_uint32, vp, sz, vp, C.POINTER(ClassifyOut), vp, vp, vp]),
+        "kxpu_classify_named": (i32, [vp, vp, sz, C.c_uint32, vp, sz, vp, vp, sz, C.POINTER(ClassifyOut), vp, vp, vp, vp]),
         "kxpu_pcie_tree_sriov": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32), vp]),
         "kxpu_pcie_tree_mdev": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp, vp, vp, C.POINTER(C.c_uint32)]),
         "kxpu_dra_slices_taints": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
@@ -797,6 +803,47 @@ class Kxpu:
                    group_ids=arrs["group_ids"][:g], group_off=arrs["group_off"][:g + 1],
                    group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
                    dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g], dev_rule=dev_rule[:d])
+        if topo:
+            res["group_numa"] = gnuma[:g]
+        if viable:
+            res["group_blocker"] = gblk[:g]
+        return res
+
+    def classify_named(self, rules, vgpu_rules, recs, keys, names, topo=False, viable=False):
+        """kxpu_classify_named: classify_vf_vgpu's dict plus dev_slot.  names: a NAME_DTYPE array or
+        [(rule, device bytes, slot)]; an empty table passes NULL and leaves dev_slot absent from the dict."""
+        if not isinstance(names, np.ndarray):
+            names = np.array([(r, s, d) for r, d, s in names], NAME_DTYPE)
+        names = np.ascontiguousarray(names)
+        assert names.dtype == NAME_DTYPE
+        ra = rules_array(rules)
+        recs = np.ascontiguousarray(recs)
+        assert recs.dtype == DEVREC_DTYPE
+        if keys is not None:
+            keys = np.ascontiguousarray(keys)
+            assert keys.dtype == VGPUKEY_DTYPE and len(keys) == len(recs)
+        n = len(recs)
+        arrs = dict(accept_index=np.empty(n, np.uint32), group_ids=np.empty(n, np.uint32),
+                    group_off=np.empty(n + 1, np.uint32), group_members=np.empty(n, np.uint32),
+                    dev_ids=np.empty(n, np.uint64), dev_off=np.empty(n + 1, np.uint32),
+                    dev_groups=np.empty(n, np.uint32))
+        dev_rule = np.empty(max(n, 1), np.uint8)
+        dev_slot = np.empty(max(n, 1), np.uint32)
+        gnuma = np.empty(max(n, 1), np.uint64) if topo else None
+        gblk = np.empty(max(n, 1), np.uint32) if viable else None
+        out = ClassifyOut(**{k: v.ctypes.data for k, v in arrs.items()})
+        self._chk(self.L.kxpu_classify_named(self.ctx, _ptr(ra) if len(ra) else None, len(ra), vgpu_rules,
+                                             _ptr(recs) if n else None, n,
+                                             None if keys is None else _ptr(keys if n else np.zeros(1, VGPUKEY_DTYPE)),
+                                             _ptr(names) if len(names) else None, len(names), C.byref(out),
+                                             _ptr(dev_rule), _ptr(dev_slot) if len(names) else None, _ptr(gnuma), _ptr(gblk)))
+        g, d, a = out.n_groups, out.n_devids, out.n_accepted
+        res = dict(accept_index=arrs["accept_index"], n_accepted=a, n_groups=g, n_devids=d,
+                   group_ids=arrs["group_ids"][:g], group_off=arrs["group_off"][:g + 1],
+                   group_members=arrs["group_members"][:a], dev_ids=arrs["dev_ids"][:d],
+                   dev_off=arrs["dev_off"][:d + 1], dev_groups=arrs["dev_groups"][:g], dev_rule=dev_rule[:d])
+        if len(names):
+            res["dev_slot"] = dev_slot[:d]
         if topo:
             res["group_numa"] = gnuma[:g]
         if viable:

@@ -81,7 +81,7 @@ struct Work {
     // kxpu_classify_topo / _mdev_topo only: [n] NUMA mask per group ordinal (zeroed by k_reset)
     unsigned long long *group_numa;
 };
-enum { MODE_NV = 0, MODE_RULES = 1, MODE_MDEV = 2, MODE_VIAB = 3, MODE_VF = 4, MODE_VF_VIAB = 5 };
+enum { MODE_NV = 0, MODE_RULES = 1, MODE_MDEV = 2, MODE_VIAB = 3, MODE_VF = 4, MODE_VF_VIAB = 5, MODE_NAMED = 6, MODE_NAMED_VIAB = 7 };
 
 // The rule list of kxpu_classify_rules as k_candidates compares it: per rule the vendor id bytes with the id
 // length in bits 56-63 (the same packing as read_id's result), and the driver as two 64-bit words with
@@ -97,6 +97,21 @@ struct RuleTable {
 __device__ __forceinline__ uint32_t *vf_islot(const Work &W) { return W.ak; }
 // the device-id key carries the rule in bits 48-63: an id is at most 6 bytes after data[2:]
 constexpr unsigned long long DEVID_MASK = 0x0000FFFFFFFFFFFFull;
+
+// The name table of kxpu_classify_named as the candidate pass compares it: per exact entry the id packed like read_id's
+// result with its length in bits 56-63, its rule and its slot; per rule the slot of its "*" entry (NO_STAR: none).
+// A named candidate's key row is (slot, rule, 0..., NAME_ROW in byte 47): byte 47 of a type-key row is its length
+// (at most 40), so the two kinds never intern together.  Its deviceMap key sets NAMED_KEY, which no id key and no
+// type key carries, so a slotted entry never merges with an entry keyed by a device id of the same rule.
+struct NameTable {
+    unsigned long long id[KXPU_MAX_NAMES];
+    uint8_t rule[KXPU_MAX_NAMES], slot[KXPU_MAX_NAMES];
+    uint8_t star[KXPU_MAX_RULES];
+    uint32_t n;
+};
+constexpr uint8_t NO_STAR = 0xFFu;
+constexpr uint8_t NAME_ROW = 0xFFu;
+constexpr unsigned long long NAMED_KEY = 1ull << 63;
 
 // readIDFromFileFunc (device_plugin.go:183-191): data[2:] with '\n' trimmed at both ends.
 // Returns false when the file is shorter than 2 bytes (the reference would panic) or longer
@@ -155,8 +170,10 @@ __device__ __forceinline__ uint32_t dinsert(const Work &W, unsigned long long ke
 // read gslot[i], which stays EMPTY32 for a non-candidate.  Each record inserts at most one group, so gcap >= 2n holds.
 // VF (kxpu_classify_vf_vgpu): a record of a rule in R.vgpu_mask is a candidate only with a non-empty key row, which also
 // replaces its device read; its device file is not looked at.  Such a candidate's key goes to k_intern_vf (vf_islot).
-template <bool RULES, bool VIAB = false, bool VF = false>
-__device__ __forceinline__ void candidates(const Work &W, const RuleTable &R) {
+// NAMED (kxpu_classify_named, always with VF): a candidate of any other rule whose device read works looks its id up in
+// the name table, exact entry first, then its rule's "*"; with a slot it writes a name row and goes to k_intern_vf too.
+template <bool RULES, bool VIAB = false, bool VF = false, bool NAMED = false>
+__device__ __forceinline__ void candidates(const Work &W, const RuleTable &R, const NameTable *NT = nullptr) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= W.n) return;
     // one 64-byte record per thread: three 16-byte vector loads (the bdf is not needed to classify)
@@ -201,6 +218,23 @@ __device__ __forceinline__ void candidates(const Work &W, const RuleTable &R) {
         }
         vf_islot(W)[i] = vr && cand ? 0u : EMPTY32;
     }
+    if (NAMED && !vr && cand && dok) {
+        const unsigned long long dkey = did | ((unsigned long long)dl << 56);
+        uint32_t s = NO_STAR;
+#pragma unroll
+        for (uint32_t r = 0; r < KXPU_MAX_RULES; r++)
+            if (r == rule) s = NT->star[r];
+#pragma unroll
+        for (uint32_t e = 0; e < KXPU_MAX_NAMES; e++)  // constant indices: the table stays in the parameter bank
+            if (e < NT->n && NT->rule[e] == rule && NT->id[e] == dkey) s = NT->slot[e];
+        if (s != NO_STAR) {
+            uint4 *kb = W.keybuf + 3 * (size_t)i;
+            kb[0] = make_uint4(s | (rule << 8), 0u, 0u, 0u);
+            kb[1] = make_uint4(0u, 0u, 0u, 0u);
+            kb[2] = make_uint4(0u, 0u, 0u, (uint32_t)NAME_ROW << 24);
+            vf_islot(W)[i] = 0u;
+        }
+    }
     if (!vr && cand && (group == EMPTY32 || (dok && did == EMPTY64) || (!(fl & KXPU_REC_DEVICE_ERR) && dlen > 8u)))
         atomicOr(&W.totals[3], 1u);  // outside the supported domain
     uint32_t slot = EMPTY32;
@@ -231,6 +265,14 @@ __global__ void __launch_bounds__(256) k_candidates_vf(const Work W, const __gri
 }
 __global__ void __launch_bounds__(256) k_candidates_vf_viable(const Work W, const __grid_constant__ RuleTable R) {
     candidates<true, true, true>(W, R);
+}
+__global__ void __launch_bounds__(256) k_candidates_named(const Work W, const __grid_constant__ RuleTable R,
+                                                          const __grid_constant__ NameTable N) {
+    candidates<true, false, true, true>(W, R, &N);
+}
+__global__ void __launch_bounds__(256) k_candidates_named_viable(const Work W, const __grid_constant__ RuleTable R,
+                                                                 const __grid_constant__ NameTable N) {
+    candidates<true, true, true, true>(W, R, &N);
 }
 
 // pass 1 of kxpu_classify_mdev: candidates, group table, gfirst (a group starts at a candidate with a non-empty type
@@ -409,7 +451,8 @@ __global__ void __launch_bounds__(C_THREADS) k_accept_scan(const Work W) {
 // MODE_RULES: the device-id key is (rule of the first member) << 48 | device id; MODE_MDEV: (rule of the first member)
 // << 48 | first record with its type key.  MODE_VIAB: MODE_RULES plus the group's first blocker from its slot.
 // MODE_VF / MODE_VF_VIAB: MODE_RULES / MODE_VIAB, except that a group whose first member matched a vGPU rule is keyed
-// like MODE_MDEV's, by (rule, first record with its type key).
+// like MODE_MDEV's, by (rule, first record with its type key).  MODE_NAMED / MODE_NAMED_VIAB: MODE_VF / MODE_VF_VIAB,
+// and a group whose first member has a slot is keyed NAMED_KEY | (rule, first record with that (rule, slot)).
 template <int MODE>
 __global__ void __launch_bounds__(256) k_groups(const Work W) {
     const uint32_t o = blockIdx.x * blockDim.x + threadIdx.x;
@@ -430,10 +473,16 @@ __global__ void __launch_bounds__(256) k_groups(const Work W) {
     unsigned long long did;
     uint32_t dl;
     read_id(reinterpret_cast<const uint8_t *>(&dq), dlen, did, dl);
-    if (MODE == MODE_RULES || MODE == MODE_VIAB || MODE == MODE_VF || MODE == MODE_VF_VIAB) did |= (unsigned long long)W.rrule[i] << 48;
+    if (MODE == MODE_RULES || MODE == MODE_VIAB || MODE == MODE_VF || MODE == MODE_VF_VIAB || MODE == MODE_NAMED ||
+        MODE == MODE_NAMED_VIAB)
+        did |= (unsigned long long)W.rrule[i] << 48;
     if ((MODE == MODE_VF || MODE == MODE_VF_VIAB) && vf_islot(W)[i] != EMPTY32)  // the first member matched a vGPU rule
         did = ((unsigned long long)W.rrule[i] << 48) | W.itab[vf_islot(W)[i]].first;
-    if (MODE == MODE_VIAB || MODE == MODE_VF_VIAB) W.group_blocker[o] = W.gtab[W.gslot[i]].pad;
+    if ((MODE == MODE_NAMED || MODE == MODE_NAMED_VIAB) && vf_islot(W)[i] != EMPTY32) {  // a vGPU rule or a slot
+        const bool slotted = reinterpret_cast<const uint8_t *>(W.keybuf + 3 * (size_t)i)[47] == NAME_ROW;
+        did = (slotted ? NAMED_KEY : 0ull) | ((unsigned long long)W.rrule[i] << 48) | W.itab[vf_islot(W)[i]].first;
+    }
+    if (MODE == MODE_VIAB || MODE == MODE_VF_VIAB || MODE == MODE_NAMED_VIAB) W.group_blocker[o] = W.gtab[W.gslot[i]].pad;
     const uint32_t ds = dinsert(W, did);
     // a few hot device ids own most groups: same-address atomics run at ~1 per ns, so only a group that can
     // still lower the minimum issues one
@@ -473,6 +522,17 @@ __global__ void __launch_bounds__(C_THREADS) k_devfirst_scan(const Work W) {
             run++;
         }
     }
+}
+
+// pass 3b of kxpu_classify_named: one thread per group; the first group of each entry writes the entry's slot, from the
+// name row of the record its key names, or KXPU_NO_SLOT.  A launch of its own keeps k_devfirst_scan as it is.
+__global__ void __launch_bounds__(256) k_dev_slots(const Work W, uint32_t *dev_slot) {
+    const uint32_t o = blockIdx.x * blockDim.x + threadIdx.x;
+    if (o >= W.totals[1]) return;
+    const DSlot &d = W.dtab[W.grp_dslot[o]];
+    if (d.first != W.grp_rec[o]) return;
+    dev_slot[d.ord] = (d.key & NAMED_KEY) ? reinterpret_cast<const uint8_t *>(W.keybuf + 3 * (size_t)(uint32_t)d.key)[0]
+                                           : KXPU_NO_SLOT;
 }
 
 // pass 4: sort inputs -- members (group ordinal, record) at busIndex, groups (device ordinal, group id)
@@ -664,19 +724,22 @@ static uint32_t bits_for(uint32_t n) {
 // vgpu_mask != 0: kxpu_classify_vf_vgpu (keys: its key rows)
 static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
                              bool mdev, uint8_t *dev_rule, uint64_t *group_numa, uint32_t *group_blocker, uint32_t vgpu_mask,
-                             const kxpu_vgpukey *keys, bool small_dtab, bool *retry);
+                             const kxpu_vgpukey *keys, const NameTable *NT, uint32_t *dev_slot, bool small_dtab, bool *retry);
 
 static int32_t classify_run(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R, bool mdev,
                             uint8_t *dev_rule, uint64_t *group_numa = nullptr, uint32_t *group_blocker = nullptr,
-                            uint32_t vgpu_mask = 0, const kxpu_vgpukey *keys = nullptr) {
+                            uint32_t vgpu_mask = 0, const kxpu_vgpukey *keys = nullptr, const NameTable *NT = nullptr,
+                            uint32_t *dev_slot = nullptr) {
     std::lock_guard<std::mutex> guard(ctx->mu);
     cudaSetDevice(ctx->device);
     kx_clear_timings(ctx);
     bool retry = false;
-    int32_t rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, group_blocker, vgpu_mask, keys, true, &retry);
+    int32_t rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, group_blocker, vgpu_mask, keys, NT, dev_slot, true,
+                               &retry);
     // more distinct device ids (or type keys) than the small tables hold; the rerun resets every table, blockers included
     if (retry)
-        rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, group_blocker, vgpu_mask, keys, false, &retry);
+        rc = classify_once(ctx, recs, n, out, R, mdev, dev_rule, group_numa, group_blocker, vgpu_mask, keys, NT, dev_slot, false,
+                           &retry);
     return rc;
 }
 
@@ -791,6 +854,61 @@ extern "C" int32_t kxpu_classify_vf_vgpu(kxpu_ctx *ctx, const kxpu_xpu_rule *rul
     return classify_run(ctx, recs, n, out, &R, false, dev_rule, group_numa, group_blocker, vgpu_rules, keys);
 }
 
+extern "C" int32_t kxpu_classify_named(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, uint32_t vgpu_rules,
+                                       const kxpu_devrec *recs, size_t n, const kxpu_vgpukey *keys, const kxpu_name_entry *names,
+                                       size_t n_names, kxpu_classify_out *out, uint8_t *dev_rule, uint32_t *dev_slot,
+                                       uint64_t *group_numa, uint32_t *group_blocker) {
+    static_assert(sizeof(kxpu_name_entry) == 16, "kxpu_name_entry layout");
+    if (!ctx || !out || (n && !recs) || !rules || n_rules == 0 || n_rules > KXPU_MAX_RULES) return KXPU_E_INVALID;
+    if ((vgpu_rules >> n_rules) || (vgpu_rules && !keys)) return KXPU_E_INVALID;
+    if (n_names > KXPU_MAX_NAMES || (n_names && (!names || (n && !dev_slot)))) return KXPU_E_INVALID;
+    if (n_names == 0)  // kxpu_classify_vf_vgpu's call, byte for byte
+        return kxpu_classify_vf_vgpu(ctx, rules, n_rules, vgpu_rules, recs, n, keys, out, dev_rule, group_numa, group_blocker);
+    NameTable NT;
+    memset(&NT, 0, sizeof NT);
+    memset(NT.star, NO_STAR, sizeof NT.star);
+    for (size_t e = 0; e < n_names; e++) {
+        const kxpu_name_entry &u = names[e];
+        const int il = field_len(u.device, (int)sizeof u.device);
+        const bool star = il == 1 && u.device[0] == '*';
+        bool hex = il == 4;
+        for (int k = 0; hex && k < 4; k++) hex = (u.device[k] >= '0' && u.device[k] <= '9') || (u.device[k] >= 'a' && u.device[k] <= 'f');
+        if (u.rule >= n_rules || ((vgpu_rules >> u.rule) & 1u)) {
+            KX_SET_ERR(ctx, "classify_named: name %zu: rule %u is not a passthrough rule of the list", e, u.rule);
+            return KXPU_E_INVALID;
+        }
+        if (!star && !hex) {
+            KX_SET_ERR(ctx, "classify_named: name %zu: device must be 4 lowercase hex digits or \"*\", NUL padded", e);
+            return KXPU_E_INVALID;
+        }
+        if (u.slot >= n_names) {
+            KX_SET_ERR(ctx, "classify_named: name %zu: slot %u is not below n_names (%zu)", e, u.slot, n_names);
+            return KXPU_E_INVALID;
+        }
+        for (size_t q = 0; q < e; q++) {
+            if (names[q].rule == u.rule && memcmp(names[q].device, u.device, sizeof u.device) == 0) {
+                KX_SET_ERR(ctx, "classify_named: names %zu and %zu are the same (rule, device) pair", q, e);
+                return KXPU_E_INVALID;
+            }
+        }
+        if (star) {
+            NT.star[u.rule] = (uint8_t)u.slot;
+        } else {
+            unsigned long long v = 0;
+            memcpy(&v, u.device, 4);
+            NT.id[NT.n] = v | (4ull << 56);
+            NT.rule[NT.n] = (uint8_t)u.rule;
+            NT.slot[NT.n] = (uint8_t)u.slot;
+            NT.n++;
+        }
+    }
+    if (n >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+    RuleTable R;
+    const int32_t rc = rule_table(ctx, rules, n_rules, R);
+    if (rc != KXPU_OK) return rc;
+    return classify_run(ctx, recs, n, out, &R, false, dev_rule, group_numa, group_blocker, vgpu_rules, keys, &NT, dev_slot);
+}
+
 int32_t kx_rule_drivers(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rules, unsigned long long drv[][4]) {
     RuleTable R;
     const int32_t rc = rule_table(ctx, rules, n_rules, R);
@@ -803,7 +921,7 @@ int32_t kx_rule_drivers(kxpu_ctx *ctx, const kxpu_xpu_rule *rules, size_t n_rule
 
 static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_classify_out *out, const RuleTable *R,
                              bool mdev, uint8_t *dev_rule, uint64_t *group_numa, uint32_t *group_blocker, uint32_t vgpu_mask,
-                             const kxpu_vgpukey *keys, bool small_dtab, bool *retry) {
+                             const kxpu_vgpukey *keys, const NameTable *NT, uint32_t *dev_slot, bool small_dtab, bool *retry) {
     *retry = false;
     out->n_accepted = out->n_groups = out->n_devids = 0;
     if (n == 0) {
@@ -830,7 +948,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
     // one arena; [ff-region | zero-region | rest]
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
-    const bool interns = mdev || vgpu_mask;
+    const bool interns = mdev || vgpu_mask || NT;
     const uint32_t icap = interns ? dcap : 0u;  // the intern table grows with the device-id table
     const size_t o_gtab = take((size_t)gcap * sizeof(GSlot)), o_dtab = take((size_t)dcap * sizeof(DSlot));
     const size_t o_itab = interns ? take((size_t)icap * sizeof(ISlot)) : 0;
@@ -848,7 +966,8 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
     const size_t o_rrule = R ? take(n) : 0, o_drule = R ? take(n) : 0;
     const size_t o_keys = mdev ? take(n * 48) : 0, o_islot = mdev ? take(n * 4) : 0;
     const size_t o_gblk = group_blocker ? take(n * 4) : 0;  // every ordinal is written by k_groups: no reset
-    const size_t o_vkeys = vgpu_mask ? take(n * 48) : 0;
+    const size_t o_vkeys = vgpu_mask || NT ? take(n * 48) : 0;  // NT: the name rows of the slotted candidates
+    const size_t o_dslot = NT ? take(n * 4) : 0;
     KxScratch sc(ctx);
     uint8_t *b = nullptr;
     KX_CUDA(ctx, sc.alloc((void **)&b, off));
@@ -876,10 +995,10 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
         W.keybuf = (uint4 *)(b + o_keys); W.islot = (uint32_t *)(b + o_islot);
         W.itab = (ISlot *)(b + o_itab); W.icap = icap; W.ishift = 32 - dlg;
     }
-    if (vgpu_mask) {
+    if (vgpu_mask || NT) {
         W.keybuf = (uint4 *)(b + o_vkeys);
         W.itab = (ISlot *)(b + o_itab); W.icap = icap; W.ishift = 32 - dlg;
-        cudaMemcpyAsync(W.keybuf, keys, n * 48, cudaMemcpyHostToDevice, ctx->stream);
+        if (vgpu_mask) cudaMemcpyAsync(W.keybuf, keys, n * 48, cudaMemcpyHostToDevice, ctx->stream);
     }
 
     cudaMemcpyAsync(b + o_recs, recs, n * rec_bytes, cudaMemcpyHostToDevice, ctx->stream);
@@ -894,6 +1013,13 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
             k_candidates_mdev<<<g, 256, 0, ctx->stream>>>(W, *R);
             k_intern<<<g, 256, 0, ctx->stream>>>(W);
             ctx->launches++;
+        } else if (NT) {
+            RuleTable RV = *R;
+            RV.vgpu_mask = vgpu_mask;
+            if (group_blocker) k_candidates_named_viable<<<g, 256, 0, ctx->stream>>>(W, RV, *NT);
+            else k_candidates_named<<<g, 256, 0, ctx->stream>>>(W, RV, *NT);
+            k_intern_vf<<<g, 256, 0, ctx->stream>>>(W);
+            ctx->launches++;
         } else if (vgpu_mask) {
             RuleTable RV = *R;
             RV.vgpu_mask = vgpu_mask;
@@ -906,12 +1032,18 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
         else k_candidates<<<g, 256, 0, ctx->stream>>>(W);
         k_accept_scan<<<c_tiles, C_THREADS, 0, ctx->stream>>>(W);
         if (mdev) k_groups<MODE_MDEV><<<g, 256, 0, ctx->stream>>>(W);
+        else if (NT && group_blocker) k_groups<MODE_NAMED_VIAB><<<g, 256, 0, ctx->stream>>>(W);
+        else if (NT) k_groups<MODE_NAMED><<<g, 256, 0, ctx->stream>>>(W);
         else if (vgpu_mask && group_blocker) k_groups<MODE_VF_VIAB><<<g, 256, 0, ctx->stream>>>(W);
         else if (vgpu_mask) k_groups<MODE_VF><<<g, 256, 0, ctx->stream>>>(W);
         else if (group_blocker) k_groups<MODE_VIAB><<<g, 256, 0, ctx->stream>>>(W);
         else if (R) k_groups<MODE_RULES><<<g, 256, 0, ctx->stream>>>(W);
         else k_groups<MODE_NV><<<g, 256, 0, ctx->stream>>>(W);
         k_devfirst_scan<<<c_tiles, C_THREADS, 0, ctx->stream>>>(W);
+        if (NT) {
+            k_dev_slots<<<g, 256, 0, ctx->stream>>>(W, (uint32_t *)(b + o_dslot));
+            ctx->launches++;
+        }
         if (group_numa) k_pairs<true><<<std::min<unsigned>(g, 4u * ctx->sm_count), 256, 0, ctx->stream>>>(W, passes);
         else k_pairs<false><<<std::min<unsigned>(g, 4u * ctx->sm_count), 256, 0, ctx->stream>>>(W, passes);
         ctx->launches += 6;
@@ -953,6 +1085,7 @@ static int32_t classify_once(kxpu_ctx *ctx, const void *recs, size_t n, kxpu_cla
         if (dev_rule && nd) cudaMemcpyAsync(dev_rule, W.dev_rule, nd, cudaMemcpyDeviceToHost, ctx->stream);
         if (group_numa && ng) cudaMemcpyAsync(group_numa, W.group_numa, (size_t)ng * 8, cudaMemcpyDeviceToHost, ctx->stream);
         if (group_blocker && ng) cudaMemcpyAsync(group_blocker, W.group_blocker, (size_t)ng * 4, cudaMemcpyDeviceToHost, ctx->stream);
+        if (NT && nd) cudaMemcpyAsync(dev_slot, b + o_dslot, (size_t)nd * 4, cudaMemcpyDeviceToHost, ctx->stream);
         e = cudaStreamSynchronize(ctx->stream);
         if (e != cudaSuccess) { KX_SET_ERR(ctx, "classify D2H failed: %s", cudaGetErrorString(e)); rc = KXPU_E_CUDA; }
         if (ng == 0) out->group_off[0] = 0;

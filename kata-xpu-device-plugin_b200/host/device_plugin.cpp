@@ -729,6 +729,71 @@ Error Plugin::checkVfVgpuClasses() const {
     return Error();
 }
 
+// a Kubernetes qualified name (the part after the prefix): 1-63 bytes, alphanumeric at both ends, [-A-Za-z0-9_.] inside
+static bool qualifiedName(const std::string &v) {
+    auto alnum = [](char ch) { return (ch >= '0' && ch <= '9') || (ch >= 'a' && ch <= 'z') || (ch >= 'A' && ch <= 'Z'); };
+    if (v.empty() || v.size() > 63 || !alnum(v.front()) || !alnum(v.back())) return false;
+    for (char ch : v)
+        if (!alnum(ch) && ch != '-' && ch != '_' && ch != '.') return false;
+    return true;
+}
+
+Error Plugin::checkResourceNames() const {
+    size_t total = 0;
+    std::map<std::string, size_t> classOf;  // name -> the class that configures it
+    for (size_t k = 0; k < xpuClasses.size(); k++) {
+        const XpuClass &c = xpuClasses[k];
+        const std::string cls = "class " + c.vendor + "/" + c.driver + " (" + c.cdiKind + ")";
+        if (c.resourceNames.empty()) continue;
+        if (c.vfVgpu) return fail(cls + ": resourceNames cannot rename a vfVgpu class, whose vGPUs are named by their type keys");
+        for (const auto &kv : c.resourceNames) {
+            bool hex = kv.first.size() == 4;
+            for (char ch : kv.first) hex = hex && ((ch >= '0' && ch <= '9') || (ch >= 'a' && ch <= 'f'));
+            if (!hex && kv.first != "*")
+                return fail(cls + ": resourceNames key \"" + kv.first + "\" is neither 4 lowercase hex digits nor \"*\"");
+            if (!qualifiedName(kv.second))
+                return fail(cls + ": resourceNames[\"" + kv.first + "\"] = \"" + kv.second +
+                            "\" is not a qualified name (1-63 bytes, alphanumeric at both ends, [-A-Za-z0-9_.] inside)");
+            auto it = classOf.find(kv.second);
+            if (it != classOf.end() && it->second != k)
+                return fail(cls + ": resourceNames[\"" + kv.first + "\"] = \"" + kv.second + "\" is also configured on class " +
+                            xpuClasses[it->second].vendor + "/" + xpuClasses[it->second].driver + " (" +
+                            xpuClasses[it->second].cdiKind + "); socket names ignore the namespace");
+            classOf.emplace(kv.second, k);
+        }
+        total += c.resourceNames.size();
+        if (total > KXPU_MAX_NAMES)
+            return fail(cls + ": resourceNames brings the entries of all classes to " + std::to_string(total) + ", over " +
+                        std::to_string(KXPU_MAX_NAMES));
+    }
+    for (const XpuClass &c : vgpuClasses)
+        if (!c.resourceNames.empty())
+            return fail("vGPU class " + c.vendor + "/" + c.driver + " (" + c.cdiKind +
+                        "): resourceNames cannot rename a vGPU class, whose vGPUs are named by their type keys");
+    return Error();
+}
+
+void Plugin::nameTable(std::vector<kxpu_name_entry> &entries, std::vector<std::string> &slotNames) const {
+    entries.clear();
+    slotNames.clear();
+    for (size_t k = 0; k < xpuClasses.size(); k++) {
+        std::map<std::string, uint32_t> slotOf;  // this class's names
+        for (const auto &kv : xpuClasses[k].resourceNames) {
+            auto it = slotOf.find(kv.second);
+            if (it == slotOf.end()) {
+                it = slotOf.emplace(kv.second, (uint32_t)slotNames.size()).first;
+                slotNames.push_back(kv.second);
+            }
+            kxpu_name_entry e;
+            memset(&e, 0, sizeof e);
+            e.rule = (uint32_t)k;
+            e.slot = it->second;
+            memcpy(e.device, kv.first.data(), std::min(kv.first.size(), sizeof e.device));
+            entries.push_back(e);
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------- SURVEY 8(f) row 2
 // Batched sysfs ingestion: the same records as gatherRecords, but the entries of basePath are read
 // with paths RELATIVE to one directory descriptor (openat / readlinkat on "<bdf>/vendor": no lstat per
@@ -915,6 +980,7 @@ Error Plugin::createIommuDeviceMap() {
     deviceMap.clear();  // :128
     iommuState.clear();
     deviceClass.clear();
+    deviceNamed.clear();
     // the generation is read BEFORE the walk: an event during the walk makes the snapshot stale, never fresh
     pci_.haveGen = bindGeneration && bindGeneration(pci_.gen);
     haveSnapshotGen_ = snapshotValidation && pci_.haveGen;
@@ -1113,7 +1179,23 @@ Error Plugin::classify(PciWalk &w) {
     uint32_t vgpuRules = 0;  // vfVgpu: bit r = class r serves vGPU types
     for (size_t k = 0; k < xpuClasses.size(); k++)
         if (xpuClasses[k].vfVgpu) vgpuRules |= 1u << k;
-    if (vgpuRules) {
+    std::vector<kxpu_name_entry> names;
+    std::vector<std::string> slotNames;
+    nameTable(names, slotNames);
+    c.dslot.clear();
+    if (!names.empty()) {  // some class has resourceNames: the same call with the name table
+        if (vgpuRules) {
+            Error je = joinVgpuTypes(w);
+            if (je) return je;
+        }
+        if (groupViability) c.gblk.assign(n ? n : 1, KXPU_VIABLE);
+        c.dslot.assign(n ? n : 1, KXPU_NO_SLOT);
+        rc = kxpu_classify_named(ctx_, rules.data(), rules.size(), vgpuRules, recs.data(), n,
+                                 vgpuRules ? w.vkeys.data() : nullptr, names.data(), names.size(), &out, c.drule.data(),
+                                 c.dslot.data(), readsNuma() ? c.gnuma.data() : nullptr,
+                                 groupViability ? c.gblk.data() : nullptr);
+        what = "kxpu_classify_named";
+    } else if (vgpuRules) {
         Error je = joinVgpuTypes(w);
         if (je) return je;
         if (groupViability) c.gblk.assign(n ? n : 1, KXPU_VIABLE);
@@ -1190,6 +1272,7 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
     deviceMap.clear();
     iommuState.clear();
     deviceClass.clear();
+    deviceNamed.clear();
     const ClassifyResult &c = w.out;
     std::map<uint32_t, size_t> groupClass = groupClasses(c);
     for (uint32_t g = 0; g < c.nGroups; g++) {
@@ -1230,6 +1313,10 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
             s.dra = draRecord(w.recs[first], w.paths.size() > first ? &w.paths[first] : nullptr, c.gnuma[g]);
         }
         if (vfVgpuHealth && xpuClasses[s.klass].vfVgpu && !w.physfn.empty()) s.pf = w.physfn[c.gmem[c.goff[g]]];
+        if (!xpuClasses[s.klass].resourceNames.empty()) {
+            const kxpu_devrec &r = w.recs[c.gmem[c.goff[g]]];
+            s.firstDevice = trimID(std::string((const char *)r.device_txt, std::min<size_t>(r.device_len, sizeof r.device_txt)));
+        }
         iommuMap.emplace_back(std::to_string(c.gids[g]), std::move(devs));
         iommuState.push_back(std::move(s));
     }
@@ -1238,16 +1325,22 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
         pcieDepth.assign(w.nodeDepth.begin(), w.nodeDepth.begin() + w.nNodes);
     }
     buildVfVgpuDra(w);
+    std::vector<kxpu_name_entry> names;
+    std::vector<std::string> slotNames;  // the names classify's dev_slot indexes
+    if (!c.dslot.empty()) nameTable(names, slotNames);
     for (uint32_t d = 0; d < c.nDevids; d++) {
         std::vector<std::string> groups;
         for (uint32_t k = c.doff[d]; k < c.doff[d + 1]; k++) groups.push_back(std::to_string(c.dgrp[k]));  // :169
         if (xpuClasses[c.drule[d]].vfVgpu) {  // dids[d]: the first VF carrying the entry's type key
             const kxpu_vgpukey &k = w.vkeys[c.dids[d]];
             deviceMap.emplace_back(std::string((const char *)k.key, k.len), std::move(groups));
+        } else if (!c.dslot.empty() && c.dslot[d] != KXPU_NO_SLOT) {  // a configured name
+            deviceMap.emplace_back(slotNames[c.dslot[d]], std::move(groups));
         } else {
             deviceMap.emplace_back(devIdString(c.dids[d]), std::move(groups));
         }
         deviceClass.push_back(c.drule[d]);
+        deviceNamed.push_back(!c.dslot.empty() && c.dslot[d] != KXPU_NO_SLOT);
     }
 }
 
@@ -2010,13 +2103,22 @@ Error Plugin::createDevicePlugins() {
 Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
     devicePlugins.clear();
     std::vector<std::string> ids, vendors;
-    std::vector<size_t> nameAt(deviceMap.size(), 0);  // position in names; a vfVgpu entry is named by its type key
+    // position in names; a vfVgpu entry is named by its type key, an entry of a configured name by that name
+    std::vector<size_t> nameAt(deviceMap.size(), 0);
     for (size_t d = 0; d < deviceMap.size(); d++) {
         const XpuClass &k = xpuClasses[d < deviceClass.size() ? deviceClass[d] : 0];
-        if (k.vfVgpu) continue;
+        if (k.vfVgpu || (d < deviceNamed.size() && deviceNamed[d])) continue;
         nameAt[d] = ids.size();
         ids.push_back(deviceMap[d].first);
         vendors.push_back(k.vendor);
+    }
+    std::map<std::string, size_t> modelAt;  // group of a class with resourceNames -> position of its model name in names
+    for (size_t g = 0; g < iommuMap.size(); g++) {
+        const GroupState<kxpu_dradev> &s = iommuState[g];
+        if (xpuClasses[s.klass].resourceNames.empty()) continue;
+        modelAt[iommuMap[g].first] = ids.size();
+        ids.push_back(s.firstDevice);
+        vendors.push_back(xpuClasses[s.klass].vendor);
     }
     const std::vector<std::string> names = getDeviceNames(ids, vendors);  // :99 for every device id at once
     // the Device of group id of a walk, Healthy, with the group's state
@@ -2032,17 +2134,43 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
         return d;
     };
     const std::map<std::string, size_t> iommuAt = positions(iommuMap), mdevAt = positions(mdevMap);
+    // a class with resourceNames: (class, final name) -> its plugin, which takes every entry of that name
+    std::map<std::pair<size_t, std::string>, size_t> namedAt;
+    std::set<size_t> merged;  // plugins that took a second entry: their groups go back to walk order
     size_t at = 0;
     for (const auto &kv : deviceMap) {  // :91
         GenericDevicePlugin dp;
         dp.xpuClass = at < deviceClass.size() ? deviceClass[at] : 0;
         dp.resourceNamespace = xpuClasses[dp.xpuClass].resourceNamespace;
-        for (const std::string &dev : kv.second) dp.devs.push_back(device(dev, iommuAt, iommuState));  // :93-98
-        std::string devpluginName = xpuClasses[dp.xpuClass].vfVgpu ? kv.first : names[nameAt[at]];
+        const bool renamed = !xpuClasses[dp.xpuClass].resourceNames.empty();
+        for (const std::string &dev : kv.second) {  // :93-98
+            dp.devs.push_back(device(dev, iommuAt, iommuState));
+            auto m = modelAt.find(dev);
+            if (m != modelAt.end()) dp.devs.back().model = names[m->second].empty() ? ids[m->second] : names[m->second];
+        }
+        const bool configured = at < deviceNamed.size() && deviceNamed[at];
+        std::string devpluginName = xpuClasses[dp.xpuClass].vfVgpu || configured ? kv.first : names[nameAt[at]];
         at++;
         if (devpluginName.empty()) {
             fprintf(stderr, "Error: Could not find device name for device id: %s\n", kv.first.c_str());
             devpluginName = kv.first;  // :100-103
+        }
+        if (renamed) {
+            auto it = namedAt.find({dp.xpuClass, devpluginName});
+            if (it != namedAt.end()) {
+                GenericDevicePlugin &into = devicePlugins[it->second];
+                for (Device &d : dp.devs) into.devs.push_back(std::move(d));
+                if (xpuClasses[dp.xpuClass].vfioCdev)
+                    for (const auto &g : iommuMap) {
+                        if (std::find(kv.second.begin(), kv.second.end(), g.first) == kv.second.end()) continue;
+                        std::vector<std::string> &nodes = into.nodes[g.first];
+                        for (const NvidiaGpuDevice &d : g.second)
+                            if (d.cdev >= 0) nodes.push_back("vfio" + std::to_string(d.cdev));
+                    }
+                merged.insert(it->second);
+                continue;
+            }
+            namedAt[{dp.xpuClass, devpluginName}] = devicePlugins.size();
         }
         dp.devpluginName = devpluginName;
         dp.devicePath = "/dev/vfio/";                                                          // :105
@@ -2056,9 +2184,13 @@ Error Plugin::buildPlugins(std::vector<GenericDevicePlugin> &devicePlugins) {
             }
         }
         dp.socketPath = std::string(kDevicePluginPath) + "kata-xpu-" + devpluginName + ".sock";  // generic:76
-        dp.deviceKey = kv.first;
+        dp.deviceKey = renamed ? devpluginName : kv.first;
         devicePlugins.push_back(std::move(dp));
     }
+    for (size_t k : merged)
+        std::stable_sort(devicePlugins[k].devs.begin(), devicePlugins[k].devs.end(), [&](const Device &a, const Device &b) {
+            return iommuAt.at(a.ID) < iommuAt.at(b.ID);
+        });
     for (size_t t = 0; t < typeMap.size(); t++) {  // one plugin per (vGPU class, type key)
         GenericDevicePlugin dp;
         dp.vgpu = true;
@@ -2125,6 +2257,7 @@ Error Plugin::checkDraClasses() const {
 Error Plugin::InitiateDevicePlugin() {
     Error e = checkDraClasses();
     if (!e) e = checkVfVgpuClasses();
+    if (!e) e = checkResourceNames();
     if (!e) e = checkResetMethods();
     if (!e && vgpuSriovAware && vgpuClasses.empty()) e = fail("vgpuSriovAware is set but no vGPU class is configured");
     if (e) return e;
@@ -2424,7 +2557,7 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         for (size_t i = 0; same && i < cur.size(); i++)
             same = cur[i].ID == w.devs[i].ID && cur[i].Health == w.devs[i].Health && cur[i].numa == w.devs[i].numa &&
                    cur[i].pcieNode == w.devs[i].pcieNode && cur[i].blocker == w.devs[i].blocker && cur[i].aer == w.devs[i].aer &&
-                   cur[i].drift == w.devs[i].drift;
+                   cur[i].drift == w.devs[i].drift && cur[i].model == w.devs[i].model;
         if (!same || devicePlugins[at].nodes != w.nodes) {  // changed cdev nodes: the watcher must follow them
             cur = std::move(w.devs);
             devicePlugins[at].nodes = std::move(w.nodes);
@@ -2676,10 +2809,11 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
     std::shared_lock<std::shared_mutex> lock(mu_);
     if (xpuClass >= xpuClasses.size() || xpuClasses[xpuClass].draDriver.empty())
         return fail("ResourceSlices: class " + std::to_string(xpuClass) + " has no DRA driver");
-    std::map<std::string, const std::string *> productOf;  // group id -> the resource-name suffix of its plugin
+    // group id -> its model name: the resource-name suffix of its plugin, or with resourceNames the group's own
+    std::map<std::string, const std::string *> productOf;
     for (const GenericDevicePlugin &dp : devicePlugins)
         if (!dp.vgpu && dp.xpuClass == xpuClass)
-            for (const Device &d : dp.devs) productOf[d.ID] = &dp.devpluginName;
+            for (const Device &d : dp.devs) productOf[d.ID] = d.model.empty() ? &dp.devpluginName : &d.model;
     std::vector<kxpu_dradev> devs;
     std::vector<std::string> groups;
     forPublished(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const GroupState<kxpu_dradev> &s) {
@@ -3656,6 +3790,25 @@ int kxh_set_vf_vgpu(void *h, int vgpu, int cls, int on, const char *names) {
     return parseTypeNames(names, list[cls].vgpuTypeNames) ? 0 : -1;
 }
 uint64_t kxh_vf_vgpu_reads(void *h) { return ((Plugin *)h)->vfVgpuReads; }
+
+// resourceNames of class cls (vgpu != 0: of vGPU class cls, which InitiateDevicePlugin refuses) from "id=name;id=name"
+int kxh_set_resource_names(void *h, int vgpu, int cls, const char *spec) {
+    Plugin *p = (Plugin *)h;
+    std::vector<device_plugin::XpuClass> &list = vgpu ? p->vgpuClasses : p->xpuClasses;
+    if (cls < 0 || (size_t)cls >= list.size()) return -1;
+    list[cls].resourceNames.clear();
+    std::string all(spec ? spec : "");
+    for (size_t pos = 0; pos < all.size();) {
+        size_t semi = all.find(';', pos);
+        if (semi == std::string::npos) semi = all.size();
+        const std::string item = all.substr(pos, semi - pos);
+        pos = semi + 1;
+        const size_t eq = item.find('=');
+        if (eq == std::string::npos) return -1;
+        list[cls].resourceNames[item.substr(0, eq)] = item.substr(eq + 1);
+    }
+    return 0;
+}
 
 // the learned (type ID, type key) pairs as {"id":"key",...}
 int kxh_vgpu_learned(void *h, char *json, size_t cap) {

@@ -70,6 +70,10 @@ struct Device {  // pluginapi.Device
     // vfVgpuHealth: why the VF's vGPU type is no longer the one the walk saw ("<vf> now carries vGPU type 0 (was 557)"),
     // from the last refreshVfVgpuTypes; empty = unchanged, and after every rediscover.  Also sent Unhealthy.
     std::string drift{};
+    // a plugin of a class with XpuClass::resourceNames: the model name of the group (the pci.ids name of its first
+    // member's device id, else that raw id), which ResourceSlices publishes as productName; empty elsewhere, where the
+    // plugin's devpluginName is that name
+    std::string model{};
 };
 // pluginapi.DevicePluginOptions (GetDevicePluginOptions, generic_device_plugin.go:253-258)
 struct DevicePluginOptions {
@@ -211,6 +215,13 @@ struct XpuClass {
     // (Plugin::VfVgpuResourceSlices, kxpu_dra_slices_vf_vgpu), one pool named nodeName.  Kept apart from draDriver, which
     // promises the passthrough record layout (kxpu_dradev).  Empty: the class's vGPUs are not published.
     std::string vgpuDraDriver{};
+    // passthrough only (refused on a vfVgpu class and on a vGPU class): device id -> resource name, replacing the pci.ids
+    // name (include/kxpu.h, kxpu_classify_named).  A key is a device id exactly as readIDFromFile returns it ("2330"),
+    // or "*" for every other device id of the class; a value is a Kubernetes qualified name.  {"*": "pgpu"} serves
+    // every device of the class as <resourceNamespace>/pgpu.  The class's entries whose final names are equal -- two ids
+    // with one configured name, or two unlisted ids with one pci.ids name -- are served by one plugin, groups in walk
+    // order, whose deviceKey is that name.  Empty (default): the class is named and split per device id as above.
+    std::map<std::string, std::string> resourceNames{};
 };
 XpuClass defaultXpuClass();  // {"10de", "vfio-pci", "nvidia.com", "nvidia.com/gpu", "cdi-vfio-xxxx"}
 
@@ -252,6 +263,7 @@ struct ClassifyResult {
     std::vector<uint64_t> dids, gnuma;
     std::vector<uint32_t> gblk;  // groupViability: first blocking record per group ordinal, or KXPU_VIABLE
     std::vector<uint8_t> drule;
+    std::vector<uint32_t> dslot;  // some class has resourceNames: the slot of every deviceMap entry, or KXPU_NO_SLOT
     uint32_t nGroups = 0, nDevids = 0;
     // sizes the arrays for n records and points a kxpu_classify_out at them
     kxpu_classify_out wire(size_t n);
@@ -346,6 +358,8 @@ struct GroupState {
     std::string pfDevice{}, pfProduct{};
     // vfVgpuHealth: the drift reason of the group's first member (Device::drift); empty = its type is the walk's
     std::string drift{};
+    // passthrough: the device id of the group's first member (readIDFromFile's text); names Device::model
+    std::string firstDevice{};
 };
 
 class Plugin {
@@ -367,8 +381,8 @@ class Plugin {
     // kxpu_classify_rules / kxpu_cdi_emit_kind / kxpu_alloc_names_kind; with the default list these return the bytes
     // of the reference's NVIDIA-only calls (include/kxpu.h).  Classes must be distinct (vendor, driver) pairs, at most
     // KXPU_MAX_RULES.  Socket names stay kata-xpu-<name>.sock, so two classes whose devices get the same name collide
-    // like two NVIDIA device ids with the same name do in the reference (generic_device_plugin.go:76); nothing
-    // resolves that.
+    // like two NVIDIA device ids with the same name do in the reference (generic_device_plugin.go:76); only a class
+    // with XpuClass::resourceNames resolves that, for its own devices.
     std::vector<XpuClass> xpuClasses{defaultXpuClass()};
     // vGPU classes: mediated devices under mdevBasePath, one resource <resourceNamespace>/<type key> per (class, type
     // key).  vendor = the parent PCI device's vendor id, driver = the mdev's driver.  Empty (default): nothing under
@@ -548,6 +562,7 @@ class Plugin {
     std::string lastCdiFile;
     std::vector<GroupState<kxpu_dradev>> iommuState;  // the state of every iommuMap entry (same positions)
     std::vector<size_t> deviceClass;  // class of every deviceMap entry (same positions); all 0 with the default class list
+    std::vector<bool> deviceNamed;    // deviceMap entry keyed by a configured resource name (same positions)
     // pcieTopologyAware only: the forest of the last PCI walk, shared by all passthrough plugins
     std::vector<uint32_t> pcieParent;
     std::vector<uint8_t> pcieDepth;
@@ -607,7 +622,8 @@ class Plugin {
     Error rediscover(RediscoverReport &report, const std::string &format = "YAML");
     // The ResourceSlices of class xpuClass (kxpu_dra_slices): one pool named nodeName, one device per iommuMap group of
     // the class in walk order (bdf, vendor, device and PCIe root of the group's first member, the group's NUMA mask, the
-    // plugin's resource-name suffix cut to 64 bytes as productName).  With groupViability a group that has a blocker is
+    // plugin's resource-name suffix -- with resourceNames the group's model name, Device::model -- cut to 64 bytes as
+    // productName).  With groupViability a group that has a blocker is
     // not published, also with draTaints: a taint can be tolerated, and on a cluster without the DRADeviceTaints feature
     // gate a tainted device looks healthy, so a group VFIO cannot open would be handed out.  Without draTaints health
     // from the HealthWatcher is not consulted; with it, a group refreshDraHealth found unhealthy is published tainted.
@@ -724,6 +740,12 @@ class Plugin {
     // the classes whose functions are passed through whole: xpuClasses, a vfVgpu class's driver counting as none
     bool passthroughDriver(const std::string &driver) const;
     Error checkVfVgpuClasses() const;
+    // resourceNames: each key and value well formed, no name on two classes, at most KXPU_MAX_NAMES entries, none on a
+    // vfVgpu or vGPU class; InitiateDevicePlugin runs it
+    Error checkResourceNames() const;
+    // the name table of kxpu_classify_named over xpuClasses (one slot per distinct (class, name), in class and key
+    // order) and the name of each slot
+    void nameTable(std::vector<kxpu_name_entry> &entries, std::vector<std::string> &slotNames) const;
     // resetMethods against the seven names; InitiateDevicePlugin runs it
     Error checkResetMethods() const;
     uint32_t resetAllow() const;  // resetMethods as KXPU_RM_* bits

@@ -98,6 +98,11 @@ vt = kx.vf_vgpu_types(vvts, vtables)
 for viable in (False, True):
     vc = kx.classify_vf_vgpu([(b"10de", b"nvidia")], 1, vrecs_, vt["keys"], topo=viable, viable=viable)
     print("vf vgpu named", int((vt["status"] == B.VT_NAMED).sum()), "groups", vc["n_groups"], "types", vc["n_devids"])
+# configured resource names: "*" on the passthrough rule beside the vGPU rule, with and without blockers
+for viable in (False, True):
+    nc = kx.classify_named([(b"10de", b"vfio-pci"), (b"10de", b"nvidia")], 2, vrecs_, vt["keys"], [(0, b"*", 0)],
+                           topo=viable, viable=viable)
+    print("named entries", nc["n_devids"], "slotted", int((nc["dev_slot"] != B.NO_SLOT).sum()))
 # DRA ResourceSlices: one pool of 24 slices (the last one partial), and the empty pool
 for dn_ in (3000, 0):
     blob, soff = kx.dra_slices("vfio.nvidia.com", "node-a", "node-a", 1, W.dra_devices(dn_))
