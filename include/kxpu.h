@@ -1489,6 +1489,52 @@ int32_t kxpu_dra_slices_mdev_pf(kxpu_ctx *ctx, const char *driver, const char *p
                                 const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out, size_t cap,
                                 size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
 
+/* ------------------------------------- passthrough SR-IOV virtual functions in DRA (addition to ABI v14) */
+
+/* This call and kxpu_dradevpf were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym), as
+ * for kxpu_dra_slices_mdev_pf.  A VF served whole by a passthrough class (an AMD Instinct MxGPU VF, an Intel Data Center
+ * GPU Flex / Max VF, a NIC VF on vfio-pci) is published as any function is, under its own address and device id; this
+ * layout adds its PF's, so that a claim can ask for VFs of one physical device (matchAttribute on physfnAddress) or
+ * of different ones.  The host takes the PF from kxpu_sriov's pf_of; no new fact about sysfs or the Kubernetes API is
+ * used: the [assumed] lists above kxpu_dra_slices and kxpu_mdev_pf cover it. */
+
+/* One published passthrough device with its PF.  160 bytes, a multiple of 16; alignof 8. */
+typedef struct kxpu_dradevpf {
+    kxpu_dradev dev;          /* kxpu_dra_slices' record, unchanged                                            */
+    char     physfn[16];      /* the PF's PCI address, NUL padded; "" = the group's first member is not a VF     */
+    char     physfn_device[8]; /* the PF's device id (from the PF's own walk record); "" = not known             */
+    uint8_t  reserved[8];
+} kxpu_dradevpf;
+
+/* The ResourceSlices of one pool of passthrough devices, some of which may be VFs.  The contract is
+ * kxpu_dra_slices_taints', word for word, except for the device: the slices, their header and tail, 128 devices per
+ * slice (64 with taint_since), one empty slice for n = 0, slice_off, the two-call sizing and KXPU_E_NOSPACE, the
+ * KXPU_E_INVALID argument checks, the taint table rules, taint_since == NULL giving the untainted bytes, and nothing
+ * written on KXPU_E_INVALID or KXPU_E_UNSUPPORTED.  There is no one-taint or untainted entry point for this layout.  A
+ * device is kxpu_dra_slices' with two more attributes, keys sorted bytewise:
+ *   "deviceID":{"string":"<device>"}                                  always
+ *   "iommuGroup":{"int":<g>}                                          always
+ *   "numaNode":{"int":<k>}                                            only when numa_mask has exactly one bit k set
+ *   "pciAddress":{"string":"<bdf>"}                                   always
+ *   "physfnAddress":{"string":"<physfn>"}                             only when physfn is not empty
+ *   "physfnDeviceID":{"string":"<physfn_device>"}                     only when physfn_device is not empty
+ *   "productName":{"string":"<product[0..product_len)>"}              only when product_len > 0
+ *   "resource.kubernetes.io/pcieRoot":{"string":"<pcie_root>"}        only when pcie_root is not empty
+ *   "vendorID":{"string":"<vendor>"}                                  always
+ * So a record whose physfn is empty (its physfn_device is then empty too: the domain says so) gives the device bytes of
+ * kxpu_dra_slices_taints for its dev, and a pool where every physfn is empty gives that call's bytes.
+ * KXPU_E_UNSUPPORTED, with *len, the output and slice_off untouched: the taint cases of kxpu_dra_slices_taints,
+ * n >= KXPU_DRA_MAX_DEVICES, or a record outside the domain (in the order the kernel's flags report them):
+ *   - dev: kxpu_dra_slices' domain, in its order (product, bdf, pcie_root, vendor, device, iommu_group, product_len);
+ *   - physfn: empty, or 1..16 bytes over [0-9a-f:.] before its first NUL;
+ *   - physfn_device: 0..6 bytes over [0-9a-f] before its first NUL, and empty when physfn is empty.
+ * GPU: the kernel of kxpu_dra_slices, instantiated for this record layout, untainted and with the taint list (one entry
+ * for n_taints == 1, KXPU_DRA_MAX_TAINTS for more).  Timed under KXPU_T_EMIT. */
+int32_t kxpu_dra_slices_pf(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                           const kxpu_dradevpf *devs, size_t n, const kxpu_dra_taint *taints, size_t n_taints,
+                           const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out, size_t cap, size_t *len,
+                           uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
 /* ------------------------------------- resets between tenants (addition to ABI v14) */
 
 /* This call and kxpu_resetrec were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym), as

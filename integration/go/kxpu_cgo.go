@@ -931,6 +931,24 @@ func (k *kxpu) draSlicesMdevPf(driver, node string, generation uint64, devs []C.
 	})
 }
 
+// DRA ResourceSlices of passthrough devices that may be SR-IOV VFs (an addition to ABI v14, detected by symbol).  With
+// sriovPfAware a passthrough class's pool is published through this call instead of draSlices: devs holds one
+// kxpu_dradevpf per published group of the class in walk order, the PF's address (pfOf of the group's first member,
+// from sriov) and the PF's device id next to the record (both empty for a function that is no VF, which then gives
+// draSlices' bytes).  Tainted, published and replaced exactly as draSlices' output.
+func (k *kxpu) draSlicesPf(driver, node string, generation uint64, devs []C.kxpu_dradevpf, since []int64) ([]string, error) {
+	var p *C.kxpu_dradevpf
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	return k.slices("kxpu_dra_slices_pf", driver, node, len(devs), since, func(cd, cn *C.char,
+		tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
+		ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_pf(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), tab, nt, cs,
+			out, capacity, n, off, ns)
+	})
+}
+
 // the two-call sizing of one slice call, the table and the times in C memory; the table width is len(since) / nDevs
 func (k *kxpu) slices(what, driver, node string, nDevs int, since []int64, call func(cd, cn *C.char,
 	tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,

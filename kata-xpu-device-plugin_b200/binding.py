@@ -79,6 +79,9 @@ assert DRAVFVGPU_DTYPE.itemsize == 192
 # kxpu_dramdevpf (DRA ResourceSlices of mdev vGPUs with their parent's PF, an addition to ABI v14): one published vGPU
 DRAMDEVPF_DTYPE = np.dtype([("dev", DRAMDEV_DTYPE), ("physfn", "S16"), ("physfn_device", "S8"), ("reserved", "u1", (8,))])
 assert DRAMDEVPF_DTYPE.itemsize == 240
+# kxpu_dradevpf (DRA ResourceSlices of passthrough devices with their PF, an addition to ABI v14): one published device
+DRADEVPF_DTYPE = np.dtype([("dev", DRADEV_DTYPE), ("physfn", "S16"), ("physfn_device", "S8"), ("reserved", "u1", (8,))])
+assert DRADEVPF_DTYPE.itemsize == 160
 DRA_SLICE_DEVICES = 128
 DRA_MAX_DEVICES = 1 << 24
 DRA_TAINT_SLICE_DEVICES = 64  # devices per slice of the _taint calls (ABI v11) when taint_since is given
@@ -168,7 +171,7 @@ ABI_SYMBOLS = [
     "kxpu_sriov", "kxpu_pcie_tree_sriov", "kxpu_vf_vgpu_types", "kxpu_classify_vf_vgpu", "kxpu_pcie_tree_mdev",
     "kxpu_cdi_emit_vf_vgpu", "kxpu_cdi_emit_vf_vgpu_cdev", "kxpu_cdi_parse_vf_vgpu", "kxpu_cdi_parse_vf_vgpu_cdev",
     "kxpu_dra_slices_vf_vgpu", "kxpu_vf_vgpu_drift", "kxpu_reset_check", "kxpu_metrics_devices",
-    "kxpu_mdev_pf", "kxpu_dra_slices_mdev_pf", "kxpu_classify_named",
+    "kxpu_mdev_pf", "kxpu_dra_slices_mdev_pf", "kxpu_classify_named", "kxpu_dra_slices_pf",
 ]
 
 
@@ -303,6 +306,8 @@ def load_library():
         "kxpu_dra_slices_vf_vgpu": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                           C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_mdev_pf": (i32, [vp, vp, sz, vp, vp, sz, vp]),
+        "kxpu_dra_slices_pf": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
+                                     C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_mdev_pf": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                           C.POINTER(sz), vp, C.POINTER(sz)]),
     }
@@ -1062,6 +1067,12 @@ class Kxpu:
         """kxpu_dra_slices_mdev_pf: the same for a pool of vGPUs with their parent's PF (DRAMDEVPF_DTYPE devices); since
         None gives the untainted bytes."""
         return self._slices(self.L.kxpu_dra_slices_mdev_pf, DRAMDEVPF_DTYPE, driver, pool, node, generation, devs,
+                            taints=(taints, since))
+
+    def dra_slices_pf(self, driver, pool, node, generation, devs, taints, since):
+        """kxpu_dra_slices_pf: the same for a pool of passthrough devices with their PF (DRADEVPF_DTYPE devices); since
+        None gives the untainted bytes."""
+        return self._slices(self.L.kxpu_dra_slices_pf, DRADEVPF_DTYPE, driver, pool, node, generation, devs,
                             taints=(taints, since))
 
     def aer_health(self, text, file_off, file_len, fatal_limit, nonfatal_limit, group_off, group_members):

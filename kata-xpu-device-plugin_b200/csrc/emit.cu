@@ -562,6 +562,24 @@ constexpr int MAX_FRAG_DRA_MDEV_PF =
     MAX_FRAG_DRA_MDEV + (int)sizeof(KX_P0 KX_P1) - 1 + 2 * ((int)sizeof(KX_MS) - 1) + 16 + 6;
 constexpr int DRAMP_PARTS = DRAMP_LITS + 2;
 
+// A passthrough device that may be an SR-IOV VF (kxpu_dra_slices_pf): the PCI fragment, with physfnAddress and
+// physfnDeviceID (Q0, Q1) between pciAddress and productName.  Their neighbours are strings, so the PCI scheme holds:
+// each opens with the closer of the string before it and is dropped with its value when absent.  The PCI literals keep
+// their indices and Q0 / Q1 follow them; a record with neither attribute gives the PCI fragment's bytes.  LAYOUT_PCI_PF
+// is a layout of k_dra_slices only.
+constexpr int LAYOUT_PCI_PF = 8;
+static_assert(LAYOUT_PCI_PF != LAYOUT_PCI && LAYOUT_PCI_PF != LAYOUT_MDEV && LAYOUT_PCI_PF != LAYOUT_VF_VGPU &&
+                  LAYOUT_PCI_PF != LAYOUT_MDEV_PF,
+              "a DRA layout of its own");
+#define KX_Q0 "\"},\"physfnAddress\":{\"string\":\""
+#define KX_Q1 "\"},\"physfnDeviceID\":{\"string\":\""
+constexpr int DRAP_Q0 = 9, DRAP_Q1 = 10, DRAP_LITS = 11;
+static const char *const h_drap_lits[DRAP_LITS] = {KX_D0, KX_D1, KX_D2, KX_D3, KX_D4, KX_D5,
+                                                   KX_D6, KX_D7, KX_D8, KX_Q0, KX_Q1};
+// the PCI bound, two more literals, a 16-byte physfn and a 6-byte id
+constexpr int MAX_FRAG_DRA_PF = MAX_FRAG_DRA + (int)sizeof(KX_Q0 KX_Q1) - 1 + 16 + 6;
+constexpr int DRAP_PARTS = DRAP_LITS + 2;
+
 // Taints (kxpu_dra_slices[_mdev]_taint[s]).  A device that carries some taint ends with its last literal less that
 // literal's final '}' (the one that closes the device), then KX_TAINTS_OPEN, for each carried taint in table order its
 // entry head (the table's key, value and effect, assembled on the host like the slice head), the 20-byte timeAdded and
@@ -616,6 +634,8 @@ constexpr int DRAM_F_PRODUCT = 0, DRAM_F_TYPE = 1, DRAM_F_UUID = 2, DRAM_F_PAREN
               DRAM_F_DEVICE = 6, DRAM_F_GROUP = 7, DRAM_F_PLEN = 8, DRAM_F_COUNT = 9;
 // kxpu_dramdevpf: the mdev flags for its dev, then its own two
 constexpr int DRAMP_F_PHYSFN = DRAM_F_COUNT, DRAMP_F_PHYSFN_DEVICE = DRAM_F_COUNT + 1, DRAMP_F_COUNT = DRAM_F_COUNT + 2;
+// kxpu_dradevpf: the PCI flags for its dev, then its own two
+constexpr int DRAP_F_PHYSFN = DRA_F_COUNT, DRAP_F_PHYSFN_DEVICE = DRA_F_COUNT + 1, DRAP_F_COUNT = DRA_F_COUNT + 2;
 constexpr int DRAV_F_PRODUCT = 0, DRAV_F_KEY = 1, DRAV_F_BDF = 2, DRAV_F_PARENT = 3, DRAV_F_ROOT = 4, DRAV_F_VENDOR = 5,
               DRAV_F_DEVICE = 6, DRAV_F_GROUP = 7, DRAV_F_TYPE_ID = 8, DRAV_F_PLEN = 9, DRAV_F_COUNT = 10;
 
@@ -659,6 +679,10 @@ template <int T, int FRAG, int POOL>
 struct DraMdevPfSmem : DraMdevSmem<T, FRAG, POOL> {
     uint8_t xlen[T];     // physfn length | physfn_device length << 5
 };
+template <int T, int FRAG, int POOL>
+struct DraPfSmem : DraSmem<T, FRAG, POOL> {
+    uint8_t xlen[T];     // physfn length | physfn_device length << 5
+};
 template <typename Base, int NT>
 struct DraTaintsSmem : Base {
     uint8_t ts[TAINT_TILE][NT][20];  // timeAdded of taint t of device d
@@ -684,9 +708,16 @@ template <> struct DraLayout<LAYOUT_MDEV_PF> {
     template <int T, int FRAG, int POOL> using Smem = DraMdevPfSmem<T, FRAG, POOL>;
     static constexpr int PARTS = DRAMP_PARTS, LAST = DRAM_E, F_COUNT = DRAMP_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_MDEV_PF;
 };
-// the mdev record of either mdev layout
+template <> struct DraLayout<LAYOUT_PCI_PF> {
+    using Rec = kxpu_dradevpf;
+    template <int T, int FRAG, int POOL> using Smem = DraPfSmem<T, FRAG, POOL>;
+    static constexpr int PARTS = DRAP_PARTS, LAST = 8, F_COUNT = DRAP_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_PF;
+};
+// the mdev record of either mdev layout, the PCI record of either PCI layout
 __device__ __forceinline__ const kxpu_dramdev *dram_of(const kxpu_dramdev *r) { return r; }
 __device__ __forceinline__ const kxpu_dramdev *dram_of(const kxpu_dramdevpf *r) { return &r->dev; }
+__device__ __forceinline__ const kxpu_dradev *dra_of(const kxpu_dradev *r) { return r; }
+__device__ __forceinline__ const kxpu_dradev *dra_of(const kxpu_dradevpf *r) { return &r->dev; }
 // one k_dra_slices instantiation for tables of up to NT taints (NT = 0: untainted): LAST is the literal that closes a
 // device; a taint time above the maximum reports F_SINCE, a device with two taints of one key and effect F_DUP
 template <int LAYOUT, int NT> struct DraKernel {
@@ -714,6 +745,9 @@ static_assert(sizeof(DraKernel<LAYOUT_VF_VGPU, KXPU_DRA_MAX_TAINTS>::Smem) <= 22
 static_assert(sizeof(DraKernel<LAYOUT_MDEV_PF, KXPU_DRA_MAX_TAINTS>::Smem) <= 227 * 1024 &&
                   2 * (sizeof(DraKernel<LAYOUT_MDEV_PF, 0>::Smem) + 1024) <= 228 * 1024,
               "MAX_FRAG_DRA_MDEV_PF: the mdev-PF staging outgrew the shared memory");
+static_assert(sizeof(DraKernel<LAYOUT_PCI_PF, KXPU_DRA_MAX_TAINTS>::Smem) <= 227 * 1024 &&
+                  2 * (sizeof(DraKernel<LAYOUT_PCI_PF, 0>::Smem) + 1024) <= 228 * 1024,
+              "MAX_FRAG_DRA_PF: the PCI-PF staging outgrew the shared memory");
 
 template <int W>
 __device__ __forceinline__ uint32_t byte_at(const uint32_t (&w)[W], int k) { return (w[k >> 2] >> (8 * (k & 3))) & 0xffu; }
@@ -779,7 +813,8 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
 
     // ---- fragment lengths, digits and the domain checks: one thread per device
     uint32_t flen = 0;
-    if (LAYOUT == LAYOUT_PCI && tid < in_slice) {
+    if ((LAYOUT == LAYOUT_PCI || LAYOUT == LAYOUT_PCI_PF) && tid < in_slice) {
+        // kxpu_dradevpf: its dev is the first 128 bytes
         const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const Rec *>(E.devs) + i0 + tid);
         const uint4 q0 = p[0], q1 = p[1], q2 = p[2], q3 = p[3], q4 = p[4], q5 = p[5], q6 = p[6], q7 = p[7];
         const uint32_t prod[16] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
@@ -808,6 +843,17 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
         S.meta[tid] = gl | (nl << 4) | (bl << 8) | (rl << 13) | (vl << 18) | (dl << 21) | (pl << 24);
         flen = DRA_LIT_TOTAL - E.len[3] - E.len[5] - E.len[6] + 2u * gl + bl + vl + dl + (nl ? E.len[3] + nl : 0u) +
                (pl ? E.len[5] + pl : 0u) + (rl ? E.len[6] + rl : 0u) + (tid + 1u < in_slice ? 1u : 0u);
+        if constexpr (LAYOUT == LAYOUT_PCI_PF) {  // physfn and physfn_device: bytes 128..152 (q8, q9.xy)
+            const uint4 q8 = p[8];
+            const uint2 q9 = reinterpret_cast<const uint2 *>(p + 9)[0];
+            const uint32_t pf[4] = {q8.x, q8.y, q8.z, q8.w}, pd[2] = {q9.x, q9.y};
+            const uint32_t xl = nul_len(pf), yl_raw = nul_len(pd), yl = min(yl_raw, 6u);
+            if (!bytes_ok(pf, 0u, xl, [](uint32_t c) { return is_lhex(c) || c == ':' || c == '.'; }))
+                E.flags[DRAP_F_PHYSFN] = 1u;
+            if (yl_raw > 6u || (yl_raw && !xl) || !bytes_ok(pd, 0u, yl, hex)) E.flags[DRAP_F_PHYSFN_DEVICE] = 1u;
+            S.xlen[tid] = (uint8_t)(xl | yl << 5);
+            flen += (xl ? E.len[DRAP_Q0] + xl : 0u) + (yl ? E.len[DRAP_Q1] + yl : 0u);
+        }
     }
     if constexpr (LAYOUT == LAYOUT_MDEV || LAYOUT == LAYOUT_MDEV_PF) {
         if (tid < in_slice) {
@@ -1036,14 +1082,20 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             lit(k);
         };
         const auto bytes = [](const char *s) { return reinterpret_cast<const uint8_t *>(s); };
-        if constexpr (LAYOUT == LAYOUT_PCI) {
-            lit(0); put(S.dec[d], gl); lit(1); put(bytes(r->device), dl);
+        if constexpr (LAYOUT == LAYOUT_PCI || LAYOUT == LAYOUT_PCI_PF) {
+            const kxpu_dradev *q = dra_of(r);
+            lit(0); put(S.dec[d], gl); lit(1); put(bytes(q->device), dl);
             lit(2); put(S.dec[d], gl);
             if (nl) { lit(3); put(S.dec[d] + 10, nl); }
-            lit(4); put(bytes(r->bdf), bl);
-            if (pl) { lit(5); put(r->product, pl); }
-            if (rl) { lit(6); put(bytes(r->pcie_root), rl); }
-            lit(7); put(bytes(r->vendor), vl); close(DraLayout<LAYOUT>::LAST);
+            lit(4); put(bytes(q->bdf), bl);
+            if constexpr (LAYOUT == LAYOUT_PCI_PF) {
+                const uint32_t x = S.xlen[d], xl = x & 31u, yl = x >> 5;
+                if (xl) { lit(DRAP_Q0); put(bytes(r->physfn), xl); }
+                if (yl) { lit(DRAP_Q1); put(bytes(r->physfn_device), yl); }
+            }
+            if (pl) { lit(5); put(q->product, pl); }
+            if (rl) { lit(6); put(bytes(q->pcie_root), rl); }
+            lit(7); put(bytes(q->vendor), vl); close(DraLayout<LAYOUT>::LAST);
         } else if constexpr (LAYOUT == LAYOUT_VF_VGPU) {
             const uint32_t m2 = S.meta2[d], tl = m2 & 63u, xl = (m2 >> 6) & 31u, il = m2 >> 11;
             lit(0); put(S.dec[d], gl); lit(1); put(S.dec[d], gl); lit(DRAV_I);
@@ -1693,11 +1745,12 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     using K = DraKernel<LAYOUT, NT>;
     constexpr bool TAINT = K::TAINT;
     constexpr int PARTS = K::PARTS, HEAD = PARTS - 2, TAIL = PARTS - 1;
-    constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : LAYOUT == LAYOUT_MDEV ? DRAM_LITS : LAYOUT == LAYOUT_MDEV_PF ? DRAMP_LITS : DRAV_LITS;
+    constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : LAYOUT == LAYOUT_MDEV ? DRAM_LITS : LAYOUT == LAYOUT_MDEV_PF ? DRAMP_LITS
+                         : LAYOUT == LAYOUT_PCI_PF ? DRAP_LITS : DRAV_LITS;
     constexpr int MAXF = K::MAXF;
     constexpr int F_COUNT = K::F_COUNT;
     const char *const *lits = LAYOUT == LAYOUT_PCI ? h_dra_lits : LAYOUT == LAYOUT_MDEV ? h_dram_lits
-                              : LAYOUT == LAYOUT_MDEV_PF ? h_dramp_lits : h_drav_lits;
+                              : LAYOUT == LAYOUT_MDEV_PF ? h_dramp_lits : LAYOUT == LAYOUT_PCI_PF ? h_drap_lits : h_drav_lits;
     if (!ctx || !len || !n_slices || (n && !devs)) return KXPU_E_INVALID;
     if (!dns_subdomain_ok(driver, 63) || !dns_subdomain_ok(pool, 253) || !dns_subdomain_ok(node, 253) ||
         generation >= (1ull << 63)) {
@@ -1814,8 +1867,14 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
         "a device id that is not 0..6 bytes of [0-9a-f]", "iommu_group 4294967295", "product_len above 64",
         "a physfn that holds a byte outside [0-9a-f:.]",
         "a physfn_device that is not 0..6 bytes of [0-9a-f], or is set without a physfn"};
+    static const char *const why_pci_pf[DRAP_F_COUNT] = {
+        "a product byte outside [A-Za-z0-9_.-]", "a bdf that is empty or holds a byte outside [0-9a-f:.]",
+        "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
+        "a device id that is not 1..6 bytes of [0-9a-f]", "iommu_group 4294967295", "product_len above 64",
+        "a physfn that holds a byte outside [0-9a-f:.]",
+        "a physfn_device that is not 0..6 bytes of [0-9a-f], or is set without a physfn"};
     const char *const *why = LAYOUT == LAYOUT_PCI ? why_pci : LAYOUT == LAYOUT_MDEV ? why_mdev
-                             : LAYOUT == LAYOUT_MDEV_PF ? why_mdev_pf : why_vf_vgpu;
+                             : LAYOUT == LAYOUT_MDEV_PF ? why_mdev_pf : LAYOUT == LAYOUT_PCI_PF ? why_pci_pf : why_vf_vgpu;
     const uint32_t *flags = reinterpret_cast<const uint32_t *>(h.data() + slices + 1);
     for (int f = 0; f < F_COUNT; f++)
         if (flags[f]) {
@@ -1936,4 +1995,16 @@ extern "C" int32_t kxpu_dra_slices_mdev_pf(kxpu_ctx *ctx, const char *driver, co
                   "kxpu_dramdevpf layout");
     return dra_slices_tainted<LAYOUT_MDEV_PF>(ctx, "dra_slices_mdev_pf", driver, pool, node, generation, devs, n, taints,
                                               n_taints, taint_since, out, cap, len, slice_off, n_slices);
+}
+
+// the one entry point of the PCI-PF layout: the taint-list form, taint_since == NULL giving the untainted bytes
+extern "C" int32_t kxpu_dra_slices_pf(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                      uint64_t generation, const kxpu_dradevpf *devs, size_t n, const kxpu_dra_taint *taints,
+                                      size_t n_taints, const int64_t *taint_since, uint8_t *out, size_t cap, size_t *len,
+                                      uint64_t *slice_off, size_t *n_slices) {
+    static_assert(sizeof(kxpu_dradevpf) == 160 && alignof(kxpu_dradevpf) == 8 && offsetof(kxpu_dradevpf, physfn) == 128 &&
+                      offsetof(kxpu_dradevpf, physfn_device) == 144,
+                  "kxpu_dradevpf layout");
+    return dra_slices_tainted<LAYOUT_PCI_PF>(ctx, "dra_slices_pf", driver, pool, node, generation, devs, n, taints, n_taints,
+                                             taint_since, out, cap, len, slice_off, n_slices);
 }

@@ -1267,7 +1267,27 @@ Error Plugin::classify(PciWalk &w) {
     return Error();
 }
 
+// the device id of a PF record for kxpu_dradevpf: the record's, else (a PF that is no class candidate, whose id the walk
+// left unread) <basePath>/<pf>/device read once per PF into `read`; "" when unknown or outside 0..6 bytes of [0-9a-f]
+std::string Plugin::pfDeviceOf(const kxpu_devrec &pf, std::map<std::string, std::string> &read) const {
+    const std::string bdf(pf.bdf, strnlen(pf.bdf, sizeof pf.bdf));
+    std::string id = (pf.flags & KXPU_REC_DEVICE_ERR) ? std::string()
+                     : trimID(std::string((const char *)pf.device_txt, std::min<size_t>(pf.device_len, sizeof pf.device_txt)));
+    if (id.empty()) {
+        auto it = read.find(bdf);
+        if (it == read.end()) {
+            std::string raw;
+            it = read.emplace(bdf, readIDFromFile(basePath, bdf, "device", raw) ? trimID(raw) : "").first;
+        }
+        id = it->second;
+    }
+    bool ok = id.size() <= 6;
+    for (char ch : id) ok = ok && ((ch >= '0' && ch <= '9') || (ch >= 'a' && ch <= 'f'));
+    return ok ? id : std::string();
+}
+
 void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
+    std::map<std::string, std::string> pfDeviceRead;  // sriovPfAware: PF address -> its device file, read once
     iommuMap.clear();
     deviceMap.clear();
     iommuState.clear();
@@ -1313,6 +1333,11 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
             s.dra = draRecord(w.recs[first], w.paths.size() > first ? &w.paths[first] : nullptr, c.gnuma[g]);
         }
         if (vfVgpuHealth && xpuClasses[s.klass].vfVgpu && !w.physfn.empty()) s.pf = w.physfn[c.gmem[c.goff[g]]];
+        if (sriovPfAware && !xpuClasses[s.klass].vfVgpu && w.pfOf[c.gmem[c.goff[g]]] != KXPU_NO_PF) {
+            const kxpu_devrec &pf = w.recs[w.pfOf[c.gmem[c.goff[g]]]];
+            s.pf.assign(pf.bdf, strnlen(pf.bdf, sizeof pf.bdf));
+            if (draEnabled()) s.pfDevice = pfDeviceOf(pf, pfDeviceRead);
+        }
         if (!xpuClasses[s.klass].resourceNames.empty()) {
             const kxpu_devrec &r = w.recs[c.gmem[c.goff[g]]];
             s.firstDevice = trimID(std::string((const char *)r.device_txt, std::min<size_t>(r.device_len, sizeof r.device_txt)));
@@ -2260,6 +2285,7 @@ Error Plugin::InitiateDevicePlugin() {
     if (!e) e = checkResourceNames();
     if (!e) e = checkResetMethods();
     if (!e && vgpuSriovAware && vgpuClasses.empty()) e = fail("vgpuSriovAware is set but no vGPU class is configured");
+    if (!e && sriovPfAware && !sriovAware) e = fail("sriovPfAware is set but sriovAware is off");
     if (e) return e;
     e = createIommuDeviceMap();  // :46
     if (e) return e;
@@ -2499,13 +2525,18 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     // 2.-3. the same walks and classify variants as start-up, reconciled against the snapshots
     std::map<std::string, std::string> blockerWas;  // group id -> its blocker in the last walk
     for (size_t g = 0; g < iommuMap.size(); g++) blockerWas[iommuMap[g].first] = iommuState[g].blocker;
+    std::map<std::string, std::pair<std::string, std::string>> pfWas;  // sriovPfAware: group id -> its PF and PF device id
+    for (size_t g = 0; sriovPfAware && g < iommuMap.size(); g++)
+        pfWas[iommuMap[g].first] = {iommuState[g].pf, iommuState[g].pfDevice};
     PciWalk pw;
     Error e = rewalk(pw, pci_, report.pci);
     if (e) return e;
-    bool viabilityChanged = false;
+    bool viabilityChanged = false, pfChanged = false;
     for (size_t g = 0; g < iommuMap.size(); g++) {
         auto it = blockerWas.find(iommuMap[g].first);
         viabilityChanged |= it != blockerWas.end() && it->second != iommuState[g].blocker;
+        auto pt = pfWas.find(iommuMap[g].first);  // a VF whose PF changed is published with other attributes
+        pfChanged |= pt != pfWas.end() && pt->second != std::make_pair(iommuState[g].pf, iommuState[g].pfDevice);
     }
     if (!vgpuClasses.empty()) {
         MdevWalk mw;
@@ -2583,7 +2614,7 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     updateAerTaints(aerPt, aerVg);
     const bool driftCleared = !driftTaint_.empty();  // the walk is the new truth: every drift reason is gone
     driftTaint_.clear();
-    if (passthroughChanged || viabilityChanged || aerPt || driftCleared) pci_.draGeneration++;  // the next publication replaces these slices
+    if (passthroughChanged || viabilityChanged || pfChanged || aerPt || driftCleared) pci_.draGeneration++;  // the next publication replaces these slices
     if (vgpuChanged || aerVg) mdev_.draGeneration++;
     // 6. a fresh snapshot generation: Allocate answers from the snapshot again
     pci_.haveGen = haveGen;
@@ -2815,6 +2846,7 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
         if (!dp.vgpu && dp.xpuClass == xpuClass)
             for (const Device &d : dp.devs) productOf[d.ID] = d.model.empty() ? &dp.devpluginName : &d.model;
     std::vector<kxpu_dradev> devs;
+    std::vector<kxpu_dradevpf> pfDevs;  // sriovPfAware: the same devices with their PFs
     std::vector<std::string> groups;
     forPublished(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const GroupState<kxpu_dradev> &s) {
         if (s.klass != xpuClass) return;
@@ -2824,9 +2856,21 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
             d.product_len = (uint8_t)std::min<size_t>(it->second->size(), sizeof d.product);
             memcpy(d.product, it->second->data(), d.product_len);
         }
-        devs.push_back(d);
         groups.push_back(g);
+        if (!sriovPfAware) {
+            devs.push_back(d);
+            return;
+        }
+        kxpu_dradevpf p;
+        memset(&p, 0, sizeof p);
+        p.dev = d;
+        memcpy(p.physfn, s.pf.data(), std::min(s.pf.size(), sizeof p.physfn));
+        memcpy(p.physfn_device, s.pfDevice.data(), std::min(s.pfDevice.size(), sizeof p.physfn_device));
+        pfDevs.push_back(p);
     });
+    if (sriovPfAware)
+        return draSlices(kxpu_dra_slices_pf, "kxpu_dra_slices_pf", xpuClasses[xpuClass].draDriver, pci_.draGeneration,
+                         pfDevs, groups, out, sliceOff);
     return draSlices(kxpu_dra_slices_taints, "kxpu_dra_slices_taints", xpuClasses[xpuClass].draDriver, pci_.draGeneration, devs,
                      groups, out, sliceOff);
 }
@@ -2858,8 +2902,9 @@ Error Plugin::computeAer() {
     for (auto &s : mdevState) set(s, std::string(), 0);
     if (!aerHealth) return Error();  // no aer_dev_* file is opened
     // one record per member of every group, passthrough groups then vGPU groups; a vGPU reads its parent's files.  With
-    // vfVgpuHealth a group whose first member is a VF of a vfVgpu class, and with vgpuSriovAware a vGPU group whose first
-    // mdev's parent is a VF, has its PF as one more member, one record per PF.
+    // vfVgpuHealth a group whose first member is a VF of a vfVgpu class, with sriovPfAware a group of another class whose
+    // first member is a VF, and with vgpuSriovAware a vGPU group whose first mdev's parent is a VF, has its PF as one
+    // more member, one record per PF.
     std::string text;
     std::vector<uint64_t> off;
     std::vector<uint32_t> len, goff{0}, members;
@@ -2880,7 +2925,7 @@ Error Plugin::computeAer() {
     };
     for (size_t g = 0; g < iommuMap.size(); g++) {
         for (const NvidiaGpuDevice &d : iommuMap[g].second) members.push_back(read(basePath, d.addr, d.addr));
-        const std::string &pf = iommuState[g].pf;  // set only under vfVgpuHealth
+        const std::string &pf = iommuState[g].pf;  // set only under vfVgpuHealth or sriovPfAware
         if (!pf.empty()) {
             auto it = pfRecord.find(pf);
             if (it == pfRecord.end()) it = pfRecord.emplace(pf, read(basePath, pf, pf)).first;
@@ -4526,6 +4571,7 @@ int kxh_devs_aer(void *h, int plugin_index, char *out, size_t cap) {
 // ---- health of vGPUs on SR-IOV VFs (kxpu_vf_vgpu_drift)
 void kxh_set_vf_vgpu_health(void *h, int on) { ((Plugin *)h)->vfVgpuHealth = on != 0; }
 void kxh_set_vgpu_sriov(void *h, int on) { ((Plugin *)h)->vgpuSriovAware = on != 0; }
+void kxh_set_sriov_pf(void *h, int on) { ((Plugin *)h)->sriovPfAware = on != 0; }
 uint64_t kxh_mdev_physfn_reads(void *h) { return ((Plugin *)h)->mdevPhysfnReads; }
 // refreshVfVgpuTypes: changed as kxh_refresh_aer_health's; *moved = bit 0 passthroughMoved, bit 1 typesMoved
 int kxh_refresh_vf_vgpu_types(void *h, size_t *changed, size_t cap, size_t *n_changed, int *moved, char *err, size_t errcap) {

@@ -351,10 +351,13 @@ struct GroupState {
     // its VF-vGPU ResourceSlice record; none = unpublished
     std::optional<kxpu_dravfvgpu> vfVgpuDra{};
     // vfVgpuHealth, a group of a vfVgpu class whose first member is a VF: the PF's address (its physfn basename);
-    // vgpuSriovAware, a vGPU group whose first mdev's parent is a VF of a PF in the PCI walk: that PF's address
+    // sriovPfAware, a group of another passthrough class whose first member is a VF of a PF in the walk (kxpu_sriov's
+    // pf_of): that PF's address; vgpuSriovAware, a vGPU group whose first mdev's parent is a VF of a PF in the PCI walk:
+    // that PF's address
     std::string pf{};
     // vgpuSriovAware and vgpuDraEnabled, a vGPU group with a pf: the PF's device id and model name (getDeviceNames);
-    // "" = not known
+    // sriovPfAware and draEnabled, a passthrough group with a pf: the PF's device id (pfProduct stays empty); "" = not
+    // known
     std::string pfDevice{}, pfProduct{};
     // vfVgpuHealth: the drift reason of the group's first member (Device::drift); empty = its type is the walk's
     std::string drift{};
@@ -547,6 +550,22 @@ class Plugin {
     //     physical GPU.  A vGPU whose parent is not a VF is published exactly as without the setting.
     bool vgpuSriovAware = false;
     std::atomic<uint64_t> mdevPhysfnReads{0};  // <uuid>/../physfn links read (tests, metrics)
+    // Passthrough SR-IOV VFs held to their PF (include/kxpu.h, kxpu_dra_slices_pf).  Refused by InitiateDevicePlugin
+    // unless sriovAware is on, whose pf_of it reads.  It applies to the groups of passthrough classes without vfVgpu (an
+    // AMD MxGPU VF, an Intel Flex / Max VF, a NIC VF on vfio-pci); a vfVgpu class keeps vfVgpuHealth's path.  false
+    // (default): nothing more is opened and every output, generation and counter is as above.  true:
+    //   - a group whose first member is a VF of a PF in the walk keeps that PF's address (GroupState::pf) and, with a
+    //     draDriver, its device id: the PF's own record's, else its `device` file read once per walk (a PF on its
+    //     vendor driver is no class candidate, so the gather left the id unread);
+    //   - with aerHealth the PF's aer_dev_* files count as one more member of that group, each PF read once per call:
+    //     errors of the whole device (a surprise down, a fatal link error, a completion timeout) are logged on the PF,
+    //     and a VF may have no files of its own.  The reason names the PF, draTaints taints the group pcie-aer, and the
+    //     metrics count the PF's errors;
+    //   - ResourceSlices publishes through kxpu_dra_slices_pf: such a device carries physfnAddress and physfnDeviceID, so
+    //     a claim can ask for VFs of one physical device or of different ones.  A function that is not a VF is published
+    //     exactly as without the setting, and a rediscovery that changes a published VF's PF moves draGeneration().
+    // Allocate, CDI specs, GetPreferredAllocation and ListAndWatch topology do not change.
+    bool sriovPfAware = false;
     // (type ID, type key) of every vGPU type a walk of this process named: the last name table of kxpu_vf_vgpu_types, so a
     // GPU that became full keeps its names across rediscover
     const std::map<uint32_t, std::string> &learnedVgpuTypes() const { return learnedVgpuTypes_; }
@@ -733,6 +752,7 @@ class Plugin {
     void readCdevs(const std::vector<kxpu_devrec> &recs, std::vector<int64_t> *cdevs);
     void readSriovs(const std::vector<kxpu_devrec> &recs, std::vector<kxpu_sriovrec> *srs);
     std::map<uint32_t, std::string> learnedVgpuTypes_;
+    std::string pfDeviceOf(const kxpu_devrec &pf, std::map<std::string, std::string> &read) const;
     std::vector<kxpu_devrec> pciRecs_;  // vgpuSriovAware only: the last PCI walk's records, which kxpu_mdev_pf joins against
     // vfVgpu: the nvidia/ reads of every VF of such a class into w, then the type join (kxpu_vf_vgpu_types)
     void readVfVgpus(PciWalk &w);

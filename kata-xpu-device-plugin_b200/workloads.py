@@ -632,6 +632,19 @@ def dra_devices(n=1 << 16, seed=41):
     return d
 
 
+def dra_pf_devices(n=1 << 16, vf_every=8, seed=41):
+    """kxpu_dra_slices_pf's input: dra_devices(n), one in vf_every of them a VF that names its PF -- the function 0 of
+    its bus, a 12-byte address -- and the PF's 4-digit device id; the others are no VF (both fields empty)"""
+    from .binding import DRADEVPF_DTYPE
+    d = np.zeros(n, DRADEVPF_DTYPE)
+    d["dev"] = dra_devices(n, seed)
+    vf = np.arange(n) % vf_every == 0
+    pf = np.array([b"%04x:%02x:00.0" % (k >> 13, (k >> 5) & 0xff) for k in range(n)], "S16")
+    d["physfn"] = np.where(vf, pf, b"")
+    d["physfn_device"] = np.where(vf, b"2330", b"")
+    return d
+
+
 def dra_mdev_devices(n=1 << 16, seed=43):
     """n published vGPUs with every optional attribute present and the longest fields the host produces: a 64-byte
     product name, a 40-byte type key, a 12-byte parent address, a 10-byte PCIe root, 4-digit ids, one NUMA node, 9-digit

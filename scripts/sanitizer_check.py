@@ -84,6 +84,10 @@ mpdevs["dev"] = W.dra_mdev_devices(300)
 mpdevs["physfn"][::2], mpdevs["physfn_device"][::2] = b"0000:41:00.0", b"2330"
 print("mdev_pf resolved", int((mpwant != B.NO_PF).sum()), "slice bytes",
       len(kx.dra_slices_mdev_pf("d", "p", "n", 1, mpdevs, [("d/k", "", "NoSchedule")], np.full((300, 1), 5, np.int64))[0]))
+# passthrough SR-IOV VFs: the slices with each VF's PF, untainted and with a one-entry table
+pfdevs = W.dra_pf_devices(300)
+print("dra_pf slice bytes", len(kx.dra_slices_pf("d", "p", "n", 1, pfdevs, [], None)[0]),
+      len(kx.dra_slices_pf("d", "p", "n", 1, pfdevs, [("d/k", "", "NoSchedule")], np.full((300, 1), 5, np.int64))[0]))
 # resets between tenants: every member's function reset or bus-reset set, on the classify CSR
 rrecs, rpaths, rrrs = W.reset_walk(20000)
 rres = kx.classify_rules([(b"10de", b"vfio-pci")], rrecs)
