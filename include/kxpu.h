@@ -71,7 +71,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_FINALIZE 1
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
-#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s, kxpu_sriov's, kxpu_mdev_pf's and kxpu_reset_check's kernels: the slot holds the most recent call's */
+#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s, kxpu_pcie_ports', kxpu_sriov's, kxpu_mdev_pf's and kxpu_reset_check's kernels: the slot holds the most recent call's */
 #define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev|_vf_vgpu[_cdev]]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
@@ -1534,6 +1534,75 @@ int32_t kxpu_dra_slices_pf(kxpu_ctx *ctx, const char *driver, const char *pool, 
                            const kxpu_dradevpf *devs, size_t n, const kxpu_dra_taint *taints, size_t n_taints,
                            const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out, size_t cap, size_t *len,
                            uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
+/* ------------------------------------- PCIe root ports and switches in DRA (addition to ABI v14) */
+
+/* These calls and kxpu_dradevpcie were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym),
+ * as for kxpu_dra_slices_pf.  resource.kubernetes.io/pcieRoot names a device's host bridge, which often has several root
+ * ports, each maybe with a switch tree below it.  These calls name the root port and the nearest switch above each
+ * group, so that claims of different DRA drivers (a GPU class and a NIC-VF class) can ask for devices under one root
+ * port or one switch: the levels nvidia-smi topo calls PHB (pcieRoot), PXB (pcieRootPort) and PIX (pcieSwitch).
+ *
+ * THE RULE.  The CHAIN of a group is kxpu_pcie_tree's: the longest common prefix of its members' chains whose path is
+ * known (the plain chains; kxpu_pcie_tree_sriov's placement of a VF below its PF is never used: a VF's sysfs path already
+ * sits beside its PF's, so the plain chain gives a VF its PF's ports).  Let f0, f1, f2, ... be the function components
+ * of the chain after its LAST host-bridge component (with VMD that is the VMD domain's, e.g. pci10000:e0, not the first
+ * one).
+ *   - root port = key(f0);
+ *   - switch = key(f_j) for the greatest odd j in the chain;
+ *   - either is KXPU_PCIE_NO_KEY when it does not exist: an unknown path, no function after the last host bridge (a
+ *     group that spans two root ports), or only f0 (a device directly below its root port: no odd j).
+ *   [assumed] Below a root port sysfs paths alternate switch upstream and downstream ports, so f1, f3, ... are upstream
+ *             ports.  Config space is not read to tell port types apart, so a PCIe-to-PCI bridge at an odd position is
+ *             reported as a switch.
+ * A group that spans two downstream ports of one switch has a chain that ends at that switch's upstream port, so it
+ * still gets that switch.  Keys are kxpu_pcie_tree's function keys (domain << 16 | bus << 8 | dev << 3 | fn). */
+#define KXPU_PCIE_NO_KEY 0xFFFFFFFFFFFFFFFFull
+
+/* The root port and switch of each group, by the rule above.  recs / paths / n / group_off / group_members / n_groups
+ * are kxpu_pcie_tree's; root_port[g] and pcie_switch[g] (n_groups entries each) receive the two keys of group g.
+ * KXPU_E_INVALID, nothing written: kxpu_pcie_tree's cases (ctx or group_off NULL, recs or paths NULL with n > 0,
+ * group_members NULL with members, root_port or pcie_switch NULL with n_groups > 0, group_off decreasing, a member index
+ * >= n).  Limits (else KXPU_E_UNSUPPORTED, nothing written): kxpu_pcie_tree's.
+ * GPU: kxpu_pcie_tree's path parse, then its longest-common-prefix pass as a compile-time variant that writes the two
+ * keys of each group (no node numbering, no prefix table).  Timed under KXPU_T_CLASSIFY. */
+int32_t kxpu_pcie_ports(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
+                        const uint32_t *group_off /* [n_groups+1] */, const uint32_t *group_members, size_t n_groups,
+                        uint64_t *root_port /* [n_groups] */, uint64_t *pcie_switch /* [n_groups] */);
+
+/* One published passthrough device with its PF and its ports.  176 bytes, a multiple of 16; alignof 8. */
+typedef struct kxpu_dradevpcie {
+    kxpu_dradevpf pf;         /* kxpu_dra_slices_pf's record, unchanged                                          */
+    uint64_t root_port;       /* the group's root port (kxpu_pcie_ports), or KXPU_PCIE_NO_KEY                      */
+    uint64_t pcie_switch;     /* the group's nearest switch upstream port, or KXPU_PCIE_NO_KEY                     */
+} kxpu_dradevpcie;
+
+/* The ResourceSlices of one pool of passthrough devices with their PCIe ports.  The contract is kxpu_dra_slices_pf's,
+ * word for word, with these additions.  A device carries two more attributes, each only when its key is not
+ * KXPU_PCIE_NO_KEY, their keys sorted bytewise among kxpu_dra_slices_pf's nine:
+ *   "<attr_domain>/pcieRootPort":{"string":"<address of root_port>"}
+ *   "<attr_domain>/pcieSwitch":{"string":"<address of pcie_switch>"}
+ * The two names are adjacent in that order (no other key starts with "<attr_domain>/"), so they sit at one of the
+ * positions among the nine.  No lowercase domain sorts between physfnAddress and physfnDeviceID, so that position never
+ * occurs.  The ADDRESS of a key is its sysfs form: the domain as 4 hex digits, or, above ffff (VMD), as 5..8 with no
+ * leading zero; then ":<bus>:<dev>.<fn>" in lowercase hex (2, 2 and 1 digits): at most 16 bytes.
+ * With every key KXPU_PCIE_NO_KEY the bytes are kxpu_dra_slices_pf's for any valid attr_domain, and with every physfn
+ * empty too, kxpu_dra_slices_taints'.
+ * KXPU_E_INVALID, nothing written: kxpu_dra_slices_pf's cases, or an attr_domain that is NULL, not a lowercase DNS
+ * subdomain of at most 63 bytes, or equal to kubernetes.io or k8s.io or a subdomain of either.
+ *   [assumed] names under kubernetes.io and k8s.io are reserved for standard attributes; there is no standard attribute
+ *             for a device's root port or switch, only pcieRoot.
+ * KXPU_E_UNSUPPORTED, with *len, the output and slice_off untouched: kxpu_dra_slices_pf's cases (its domain of each
+ * record's pf in its order), then
+ *   - root_port or pcie_switch other than KXPU_PCIE_NO_KEY with bit 63 set (a host-bridge key) or any of bits 48..62 set;
+ *   - pcie_switch set while root_port is KXPU_PCIE_NO_KEY.
+ * GPU: the kernel of kxpu_dra_slices for this record layout, untainted and with the taint list (one entry for
+ * n_taints == 1, KXPU_DRA_MAX_TAINTS for more).  The host computes the names' position once per call; each device's
+ * thread checks its keys and the device's warp formats the addresses.  Timed under KXPU_T_EMIT. */
+int32_t kxpu_dra_slices_pcie(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                             const char *attr_domain, const kxpu_dradevpcie *devs, size_t n, const kxpu_dra_taint *taints,
+                             size_t n_taints, const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out,
+                             size_t cap, size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
 
 /* ------------------------------------- resets between tenants (addition to ABI v14) */
 

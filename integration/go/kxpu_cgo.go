@@ -525,6 +525,24 @@ func (k *kxpu) pcieTree(recs []C.kxpu_devrec, paths []C.kxpu_pcipath, goff, gmem
 	return gnode[:nGroups], parent[:nn], depth[:nn], err
 }
 
+// the root port and nearest switch of each group (an addition to ABI v14, detected by symbol): pcieTree's inputs, one
+// function key per group or C.KXPU_PCIE_NO_KEY in each output.  Called once per PCI walk when draPcieConfig.DraPcieDomain
+// is set.
+func (k *kxpu) pciePorts(recs []C.kxpu_devrec, paths []C.kxpu_pcipath, goff, gmem []uint32, nGroups int) (rootPort,
+	pcieSwitch []uint64, err error) {
+	rootPort, pcieSwitch = make([]uint64, nGroups+1), make([]uint64, nGroups+1)
+	var r unsafe.Pointer
+	var pp *C.kxpu_pcipath
+	if len(recs) > 0 {
+		r, pp = unsafe.Pointer(&recs[0]), &paths[0]
+	}
+	gm := append(gmem, 0) // a valid pointer for an empty walk
+	err = kxCheck(k.ctx, "kxpu_pcie_ports", C.kxpu_pcie_ports(k.ctx, (*C.kxpu_devrec)(r), pp, C.size_t(len(recs)),
+		(*C.uint32_t)(unsafe.Pointer(&goff[0])), (*C.uint32_t)(unsafe.Pointer(&gm[0])), C.size_t(nGroups),
+		(*C.uint64_t)(unsafe.Pointer(&rootPort[0])), (*C.uint64_t)(unsafe.Pointer(&pcieSwitch[0]))))
+	return rootPort[:nGroups], pcieSwitch[:nGroups], err
+}
+
 // pcieTree over records that carry only their address, one per link target (walk order): what pcieTree sees of a walk
 func (k *kxpu) pcieTreeOfLinks(bdfs, targets []string, goff, gmem []uint32) (gnode, parent []uint32, depth []uint8, err error) {
 	recs, paths := make([]C.kxpu_devrec, len(bdfs)), make([]C.kxpu_pcipath, len(bdfs))
@@ -945,6 +963,33 @@ func (k *kxpu) draSlicesPf(driver, node string, generation uint64, devs []C.kxpu
 		tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
 		ns *C.size_t) C.int32_t {
 		return C.kxpu_dra_slices_pf(k.ctx, cd, cn, cn, C.uint64_t(generation), p, C.size_t(len(devs)), tab, nt, cs,
+			out, capacity, n, off, ns)
+	})
+}
+
+// draPcieConfig is Plugin::draPcieDomain: empty (default) publishes every passthrough pool as before; a lowercase DNS
+// subdomain of at most 63 bytes, not kubernetes.io or k8s.io nor under either, and only with a draDriver on some
+// passthrough class, publishes every passthrough pool through draSlicesPcie.
+type draPcieConfig struct {
+	DraPcieDomain string
+}
+
+// DRA ResourceSlices with each device's PCIe root port and switch (an addition to ABI v14, detected by symbol).  devs
+// holds one kxpu_dradevpcie per published group in walk order: the kxpu_dradevpf of draSlicesPf (its physfn fields
+// filled only with sriovPfAware) and the group's two keys from pciePorts.  Tainted, published and replaced exactly as
+// draSlices' output; with every key C.KXPU_PCIE_NO_KEY the bytes are draSlicesPf's.
+func (k *kxpu) draSlicesPcie(driver, node string, generation uint64, domain string, devs []C.kxpu_dradevpcie,
+	since []int64) ([]string, error) {
+	var p *C.kxpu_dradevpcie
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	cdom := C.CString(domain)
+	defer C.free(unsafe.Pointer(cdom))
+	return k.slices("kxpu_dra_slices_pcie", driver, node, len(devs), since, func(cd, cn *C.char,
+		tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
+		ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_pcie(k.ctx, cd, cn, cn, C.uint64_t(generation), cdom, p, C.size_t(len(devs)), tab, nt, cs,
 			out, capacity, n, off, ns)
 	})
 }

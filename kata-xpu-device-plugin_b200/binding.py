@@ -82,6 +82,10 @@ assert DRAMDEVPF_DTYPE.itemsize == 240
 # kxpu_dradevpf (DRA ResourceSlices of passthrough devices with their PF, an addition to ABI v14): one published device
 DRADEVPF_DTYPE = np.dtype([("dev", DRADEV_DTYPE), ("physfn", "S16"), ("physfn_device", "S8"), ("reserved", "u1", (8,))])
 assert DRADEVPF_DTYPE.itemsize == 160
+# kxpu_dradevpcie (DRA ResourceSlices with PCIe root ports and switches, an addition to ABI v14): one published device
+DRADEVPCIE_DTYPE = np.dtype([("pf", DRADEVPF_DTYPE), ("root_port", "u8"), ("pcie_switch", "u8")])
+assert DRADEVPCIE_DTYPE.itemsize == 176
+PCIE_NO_KEY = 0xFFFFFFFFFFFFFFFF
 DRA_SLICE_DEVICES = 128
 DRA_MAX_DEVICES = 1 << 24
 DRA_TAINT_SLICE_DEVICES = 64  # devices per slice of the _taint calls (ABI v11) when taint_since is given
@@ -172,6 +176,7 @@ ABI_SYMBOLS = [
     "kxpu_cdi_emit_vf_vgpu", "kxpu_cdi_emit_vf_vgpu_cdev", "kxpu_cdi_parse_vf_vgpu", "kxpu_cdi_parse_vf_vgpu_cdev",
     "kxpu_dra_slices_vf_vgpu", "kxpu_vf_vgpu_drift", "kxpu_reset_check", "kxpu_metrics_devices",
     "kxpu_mdev_pf", "kxpu_dra_slices_mdev_pf", "kxpu_classify_named", "kxpu_dra_slices_pf",
+    "kxpu_pcie_ports", "kxpu_dra_slices_pcie",
 ]
 
 
@@ -308,6 +313,9 @@ def load_library():
         "kxpu_mdev_pf": (i32, [vp, vp, sz, vp, vp, sz, vp]),
         "kxpu_dra_slices_pf": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                      C.POINTER(sz), vp, C.POINTER(sz)]),
+        "kxpu_pcie_ports": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp]),
+        "kxpu_dra_slices_pcie": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, C.c_char_p, vp, sz, vp, sz, vp, vp,
+                                       sz, C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_mdev_pf": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                           C.POINTER(sz), vp, C.POINTER(sz)]),
     }
@@ -916,6 +924,25 @@ class Kxpu:
         m = nn.value
         return dict(group_node=gnode[:G], key=key[:m], parent=parent[:m], depth=depth[:m])
 
+    def pcie_ports(self, recs, paths, group_off, group_members):
+        """kxpu_pcie_ports: pcie_tree's inputs; returns (root_port, pcie_switch), one function key per group or
+        PCIE_NO_KEY."""
+        recs, paths = np.ascontiguousarray(recs), np.ascontiguousarray(paths)
+        assert recs.dtype == DEVREC_DTYPE and paths.dtype == PCIPATH_DTYPE and len(recs) == len(paths)
+        group_off = np.ascontiguousarray(group_off, dtype=np.uint32)
+        group_members = np.ascontiguousarray(group_members, dtype=np.uint32)
+        G = len(group_off) - 1
+        rp, sw = np.empty(max(G, 1), np.uint64), np.empty(max(G, 1), np.uint64)
+        self.pcie_ports_raw(recs, paths, group_off, group_members, rp, sw)
+        return rp[:G], sw[:G]
+
+    def pcie_ports_raw(self, recs, paths, group_off, group_members, root_port, pcie_switch):
+        """The bare call into caller buffers (timing loops, untouched-output checks); group_off is taken as given."""
+        n = len(recs)
+        self._chk(self.L.kxpu_pcie_ports(self.ctx, _ptr(recs) if n else None, _ptr(paths) if n else None, n,
+                                         _ptr(group_off), _ptr(group_members) if len(group_members) else None,
+                                         len(group_off) - 1, _ptr(root_port), _ptr(pcie_switch)))
+
     def pcie_tree_mdev(self, recs, paths, group_off, group_members):
         """kxpu_pcie_tree_mdev: recs (MDEVREC_DTYPE) and paths (PCIPATH_DTYPE, the entries' links) at the same indices,
         the group CSR of an mdev classify call.  Returns pcie_tree's dict."""
@@ -1074,6 +1101,16 @@ class Kxpu:
         None gives the untainted bytes."""
         return self._slices(self.L.kxpu_dra_slices_pf, DRADEVPF_DTYPE, driver, pool, node, generation, devs,
                             taints=(taints, since))
+
+    def dra_slices_pcie(self, driver, pool, node, generation, attr_domain, devs, taints, since):
+        """kxpu_dra_slices_pcie: the same for a pool of passthrough devices with their PF and PCIe ports
+        (DRADEVPCIE_DTYPE devices), the two port attributes qualified by attr_domain; since None gives the untainted
+        bytes."""
+        dom = _kind(attr_domain)
+
+        def fn(ctx, d, p, nd, g, *rest):
+            return self.L.kxpu_dra_slices_pcie(ctx, d, p, nd, g, dom, *rest)
+        return self._slices(fn, DRADEVPCIE_DTYPE, driver, pool, node, generation, devs, taints=(taints, since))
 
     def aer_health(self, text, file_off, file_len, fatal_limit, nonfatal_limit, group_off, group_members):
         """kxpu_aer_health: (totals, group_aer).  text: bytes; file_off / file_len: 2n entries, the fatal file of record i

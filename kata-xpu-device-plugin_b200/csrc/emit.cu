@@ -580,6 +580,35 @@ static const char *const h_drap_lits[DRAP_LITS] = {KX_D0, KX_D1, KX_D2, KX_D3, K
 constexpr int MAX_FRAG_DRA_PF = MAX_FRAG_DRA + (int)sizeof(KX_Q0 KX_Q1) - 1 + 16 + 6;
 constexpr int DRAP_PARTS = DRAP_LITS + 2;
 
+// A passthrough device with its PCIe ports (kxpu_dra_slices_pcie): the PCI-PF fragment with "<domain>/pcieRootPort" and
+// "<domain>/pcieSwitch", adjacent in key order, at one position POS among the nine keys (0: before deviceID .. 9: after
+// vendorID), which the host computes once per call.  D1 is split in two (C1A, C1B: "attributes":{ and the deviceID key)
+// so that position 0 lies between literals too; the other literals keep their PCI-PF indices.  The block is R0, the
+// root port's address, [R1, the switch's address,] R2; the host builds R0 and R2 for POS so that the literal after the
+// block closes it:
+//   POS 0         R0 = "<d>/pcieRootPort":{"string":"        R2 = "},    (the deviceID literal C1B follows)
+//   POS 2, 3      R0 = },"<d>/pcieRootPort":{"string":"      R2 = "      (after an int: the next literal opens with })
+//   otherwise     R0 = "},"<d>/pcieRootPort":{"string":"     R2 = empty  (after a string: the next literal closes it)
+// and R1 = "},"<d>/pcieSwitch":{"string":" .  A record with neither key gives the PCI-PF fragment's bytes.
+// LAYOUT_PCI_PCIE is a layout of k_dra_slices only.
+constexpr int LAYOUT_PCI_PCIE = 9;
+static_assert(LAYOUT_PCI_PCIE != LAYOUT_PCI && LAYOUT_PCI_PCIE != LAYOUT_MDEV && LAYOUT_PCI_PCIE != LAYOUT_VF_VGPU &&
+                  LAYOUT_PCI_PCIE != LAYOUT_MDEV_PF && LAYOUT_PCI_PCIE != LAYOUT_PCI_PF,
+              "a DRA layout of its own");
+#define KX_C1A "\",\"attributes\":{"
+#define KX_C1B "\"deviceID\":{\"string\":\""
+static_assert(sizeof(KX_C1A KX_C1B) == sizeof(KX_D1), "C1A and C1B are D1");
+constexpr int DRAC_C1B = DRAP_LITS, DRAC_R0 = DRAP_LITS + 1, DRAC_R1 = DRAP_LITS + 2, DRAC_R2 = DRAP_LITS + 3,
+              DRAC_LITS = DRAP_LITS + 4;
+constexpr int DRAC_DOMAIN_MAX = 63;
+// the PCI-PF bound, the three block literals at the longest domain and two 16-byte addresses
+constexpr int MAX_FRAG_DRA_PCIE = MAX_FRAG_DRA_PF + (int)sizeof("\"},\"/pcieRootPort\":{\"string\":\"") - 1 +
+                                  (int)sizeof("\"},\"/pcieSwitch\":{\"string\":\"") - 1 + 2 * DRAC_DOMAIN_MAX +
+                                  (int)sizeof("\"},") - 1 + 2 * 16;
+constexpr int DRAC_PARTS = DRAC_LITS + 2;
+// the pool grows by the three block literals and C1B: 256 bytes more than the other layouts'
+constexpr int DRAC_POOL_EXTRA = 256;
+
 // Taints (kxpu_dra_slices[_mdev]_taint[s]).  A device that carries some taint ends with its last literal less that
 // literal's final '}' (the one that closes the device), then KX_TAINTS_OPEN, for each carried taint in table order its
 // entry head (the table's key, value and effect, assembled on the host like the slice head), the 20-byte timeAdded and
@@ -621,8 +650,8 @@ struct DraParams {
 };
 // the tainted instantiations, for tables of up to NT entries: the literals, KX_TAINTS_OPEN (part PARTS - NT - 5), the
 // entry heads (PARTS - NT - 4 .. PARTS - 5), KX_TAINT_ECLOSE, KX_TAINTS_CLOSE, the slice head and tail
-template <int PARTS, int NT>
-struct DraTaintsParams : DraParams<PARTS, dra_pool_max(NT)> {
+template <int PARTS, int NT, int POOL = dra_pool_max(NT)>
+struct DraTaintsParams : DraParams<PARTS, POOL> {
     const long long *since;  // [n * nt], device-major: taint t of device i, < 0 = not carried
     uint32_t nt;             // table entries, 1..NT
     uint8_t dup[NT];         // dup[t]: the earlier entries with taint t's key and effect
@@ -636,6 +665,8 @@ constexpr int DRAM_F_PRODUCT = 0, DRAM_F_TYPE = 1, DRAM_F_UUID = 2, DRAM_F_PAREN
 constexpr int DRAMP_F_PHYSFN = DRAM_F_COUNT, DRAMP_F_PHYSFN_DEVICE = DRAM_F_COUNT + 1, DRAMP_F_COUNT = DRAM_F_COUNT + 2;
 // kxpu_dradevpf: the PCI flags for its dev, then its own two
 constexpr int DRAP_F_PHYSFN = DRA_F_COUNT, DRAP_F_PHYSFN_DEVICE = DRA_F_COUNT + 1, DRAP_F_COUNT = DRA_F_COUNT + 2;
+// kxpu_dradevpcie: the PCI-PF flags for its pf, then a key outside the function-key range, a switch without a root port
+constexpr int DRAC_F_KEY = DRAP_F_COUNT, DRAC_F_ORPHAN = DRAP_F_COUNT + 1, DRAC_F_COUNT = DRAP_F_COUNT + 2;
 constexpr int DRAV_F_PRODUCT = 0, DRAV_F_KEY = 1, DRAV_F_BDF = 2, DRAV_F_PARENT = 3, DRAV_F_ROOT = 4, DRAV_F_VENDOR = 5,
               DRAV_F_DEVICE = 6, DRAV_F_GROUP = 7, DRAV_F_TYPE_ID = 8, DRAV_F_PLEN = 9, DRAV_F_COUNT = 10;
 
@@ -683,6 +714,10 @@ template <int T, int FRAG, int POOL>
 struct DraPfSmem : DraSmem<T, FRAG, POOL> {
     uint8_t xlen[T];     // physfn length | physfn_device length << 5
 };
+template <int T, int FRAG, int POOL>
+struct DraPcieSmem : DraPfSmem<T, FRAG, POOL> {
+    uint8_t klen[T];     // root port | switch << 3, each address length less 11 (12..16 -> 1..5), 0 = absent
+};
 template <typename Base, int NT>
 struct DraTaintsSmem : Base {
     uint8_t ts[TAINT_TILE][NT][20];  // timeAdded of taint t of device d
@@ -713,11 +748,24 @@ template <> struct DraLayout<LAYOUT_PCI_PF> {
     template <int T, int FRAG, int POOL> using Smem = DraPfSmem<T, FRAG, POOL>;
     static constexpr int PARTS = DRAP_PARTS, LAST = 8, F_COUNT = DRAP_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_PF;
 };
-// the mdev record of either mdev layout, the PCI record of either PCI layout
+template <> struct DraLayout<LAYOUT_PCI_PCIE> {
+    using Rec = kxpu_dradevpcie;
+    template <int T, int FRAG, int POOL> using Smem = DraPcieSmem<T, FRAG, POOL>;
+    static constexpr int PARTS = DRAC_PARTS, LAST = 8, F_COUNT = DRAC_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_PCIE;
+};
+// the mdev record of either mdev layout, the PCI record of each PCI layout, the PF fields of the PCI-PF and PCIe ones
 __device__ __forceinline__ const kxpu_dramdev *dram_of(const kxpu_dramdev *r) { return r; }
 __device__ __forceinline__ const kxpu_dramdev *dram_of(const kxpu_dramdevpf *r) { return &r->dev; }
 __device__ __forceinline__ const kxpu_dradev *dra_of(const kxpu_dradev *r) { return r; }
 __device__ __forceinline__ const kxpu_dradev *dra_of(const kxpu_dradevpf *r) { return &r->dev; }
+__device__ __forceinline__ const kxpu_dradev *dra_of(const kxpu_dradevpcie *r) { return &r->pf.dev; }
+__device__ __forceinline__ const kxpu_dradevpf *drapf_of(const kxpu_dradevpf *r) { return r; }
+__device__ __forceinline__ const kxpu_dradevpf *drapf_of(const kxpu_dradevpcie *r) { return &r->pf; }
+// the PCIe layout's kernel parameters: the other layouts' and the names' position among the nine keys
+template <typename Base>
+struct DraPcieParams : Base {
+    uint32_t pos;
+};
 // one k_dra_slices instantiation for tables of up to NT taints (NT = 0: untainted): LAST is the literal that closes a
 // device; a taint time above the maximum reports F_SINCE, a device with two taints of one key and effect F_DUP
 template <int LAYOUT, int NT> struct DraKernel {
@@ -727,14 +775,15 @@ template <int LAYOUT, int NT> struct DraKernel {
     static constexpr int PARTS = L::PARTS + (TAINT ? NT + 3 : 0);
     static constexpr int T_OPEN = L::PARTS - 2, T_ENTRY = T_OPEN + 1, T_ECLOSE = T_ENTRY + NT, T_CLOSE = T_ECLOSE + 1;
     static constexpr int F_SINCE = L::F_COUNT, F_DUP = F_SINCE + 1, F_COUNT = L::F_COUNT + (TAINT ? 2 : 0);
-    static constexpr int POOL = dra_pool_max(NT);
-    static_assert(!TAINT || taints_pool_need(NT) <= POOL - DRA_POOL_MAX, "taint pool bound");
+    static constexpr int POOL = dra_pool_max(NT) + (LAYOUT == LAYOUT_PCI_PCIE ? DRAC_POOL_EXTRA : 0);
+    static_assert(!TAINT || taints_pool_need(NT) <= dra_pool_max(NT) - DRA_POOL_MAX, "taint pool bound");
     static constexpr int MAXF = L::MAX_FRAG + (TAINT ? taints_part_max(NT) : 0);
     // CTAs per SM asked of ptxas, 0 for none.  Left to itself ptxas gives NT = 1 96 registers (PCI) or 101 (vGPU), so
     // two CTAs per SM, where its 47 / 56 KB of shared memory allow four; asked for three it takes 48, without spills
     static constexpr int MIN_CTAS = NT == 1 ? 3 : 0;
     using Base = typename L::template Smem<T, MAXF, POOL>;
-    using Params = std::conditional_t<TAINT, DraTaintsParams<PARTS, NT>, DraParams<PARTS, POOL>>;
+    using BaseParams = std::conditional_t<TAINT, DraTaintsParams<PARTS, NT, POOL>, DraParams<PARTS, POOL>>;
+    using Params = std::conditional_t<LAYOUT == LAYOUT_PCI_PCIE, DraPcieParams<BaseParams>, BaseParams>;
     using Smem = std::conditional_t<TAINT, DraTaintsSmem<Base, NT>, Base>;
 };
 // the VF-vGPU fragment bound: its widest instantiation still stages a whole slice in one CTA's shared memory, and its
@@ -748,6 +797,30 @@ static_assert(sizeof(DraKernel<LAYOUT_MDEV_PF, KXPU_DRA_MAX_TAINTS>::Smem) <= 22
 static_assert(sizeof(DraKernel<LAYOUT_PCI_PF, KXPU_DRA_MAX_TAINTS>::Smem) <= 227 * 1024 &&
                   2 * (sizeof(DraKernel<LAYOUT_PCI_PF, 0>::Smem) + 1024) <= 228 * 1024,
               "MAX_FRAG_DRA_PF: the PCI-PF staging outgrew the shared memory");
+static_assert(sizeof(DraKernel<LAYOUT_PCI_PCIE, KXPU_DRA_MAX_TAINTS>::Smem) <= 227 * 1024 &&
+                  2 * (sizeof(DraKernel<LAYOUT_PCI_PCIE, 0>::Smem) + 1024) <= 228 * 1024,
+              "MAX_FRAG_DRA_PCIE: the PCIe staging outgrew the shared memory");
+
+// a function key's sysfs address (include/kxpu.h, kxpu_dra_slices_pcie): the domain's digit count (4, or 5..8 without a
+// leading zero above ffff) and byte l of "<domain>:<bus>:<dev>.<fn>"; the domain is bounded to 32 bits, so a key outside
+// the range (reported by its flag) still gives at most 16 bytes
+__device__ __forceinline__ uint32_t key_dom_digits(unsigned long long k) {
+    const uint32_t dom = (uint32_t)(k >> 16);
+    return dom > 0xffffu ? (35u - (uint32_t)__clz(dom)) / 4u : 4u;
+}
+__device__ __forceinline__ uint8_t key_addr_byte(unsigned long long k, uint32_t dl, uint32_t l) {
+    const auto hx = [](uint32_t v) { v &= 15u; return (uint8_t)(v < 10u ? '0' + v : 'a' + v - 10u); };
+    if (l < dl) return hx((uint32_t)(k >> 16) >> (4u * (dl - 1u - l)));
+    switch (l - dl) {
+    case 0: case 3: return (uint8_t)':';
+    case 1: return hx((uint32_t)k >> 12);
+    case 2: return hx((uint32_t)k >> 8);
+    case 4: return hx((uint32_t)k >> 7 & 1u);
+    case 5: return hx((uint32_t)k >> 3);
+    case 6: return (uint8_t)'.';
+    default: return hx((uint32_t)k & 7u);
+    }
+}
 
 template <int W>
 __device__ __forceinline__ uint32_t byte_at(const uint32_t (&w)[W], int k) { return (w[k >> 2] >> (8 * (k & 3))) & 0xffu; }
@@ -813,8 +886,8 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
 
     // ---- fragment lengths, digits and the domain checks: one thread per device
     uint32_t flen = 0;
-    if ((LAYOUT == LAYOUT_PCI || LAYOUT == LAYOUT_PCI_PF) && tid < in_slice) {
-        // kxpu_dradevpf: its dev is the first 128 bytes
+    if ((LAYOUT == LAYOUT_PCI || LAYOUT == LAYOUT_PCI_PF || LAYOUT == LAYOUT_PCI_PCIE) && tid < in_slice) {
+        // kxpu_dradevpf (kxpu_dradevpcie): its dev is the first 128 bytes
         const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const Rec *>(E.devs) + i0 + tid);
         const uint4 q0 = p[0], q1 = p[1], q2 = p[2], q3 = p[3], q4 = p[4], q5 = p[5], q6 = p[6], q7 = p[7];
         const uint32_t prod[16] = {q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, q3.x, q3.y, q3.z, q3.w};
@@ -843,7 +916,7 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
         S.meta[tid] = gl | (nl << 4) | (bl << 8) | (rl << 13) | (vl << 18) | (dl << 21) | (pl << 24);
         flen = DRA_LIT_TOTAL - E.len[3] - E.len[5] - E.len[6] + 2u * gl + bl + vl + dl + (nl ? E.len[3] + nl : 0u) +
                (pl ? E.len[5] + pl : 0u) + (rl ? E.len[6] + rl : 0u) + (tid + 1u < in_slice ? 1u : 0u);
-        if constexpr (LAYOUT == LAYOUT_PCI_PF) {  // physfn and physfn_device: bytes 128..152 (q8, q9.xy)
+        if constexpr (LAYOUT == LAYOUT_PCI_PF || LAYOUT == LAYOUT_PCI_PCIE) {  // physfn and physfn_device: bytes 128..152 (q8, q9.xy)
             const uint4 q8 = p[8];
             const uint2 q9 = reinterpret_cast<const uint2 *>(p + 9)[0];
             const uint32_t pf[4] = {q8.x, q8.y, q8.z, q8.w}, pd[2] = {q9.x, q9.y};
@@ -853,6 +926,16 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             if (yl_raw > 6u || (yl_raw && !xl) || !bytes_ok(pd, 0u, yl, hex)) E.flags[DRAP_F_PHYSFN_DEVICE] = 1u;
             S.xlen[tid] = (uint8_t)(xl | yl << 5);
             flen += (xl ? E.len[DRAP_Q0] + xl : 0u) + (yl ? E.len[DRAP_Q1] + yl : 0u);
+        }
+        if constexpr (LAYOUT == LAYOUT_PCI_PCIE) {  // root_port and pcie_switch: bytes 160..176 (q10)
+            const uint4 q10 = p[10];
+            const unsigned long long rp = ((unsigned long long)q10.y << 32) | q10.x, sw = ((unsigned long long)q10.w << 32) | q10.z;
+            const bool hr = rp != KXPU_PCIE_NO_KEY, hs = sw != KXPU_PCIE_NO_KEY;
+            if ((hr && (rp >> 48)) || (hs && (sw >> 48))) E.flags[DRAC_F_KEY] = 1u;
+            if (hs && !hr) E.flags[DRAC_F_ORPHAN] = 1u;
+            const uint32_t kl = hr ? key_dom_digits(rp) + 8u : 0u, sl = hs ? key_dom_digits(sw) + 8u : 0u;
+            S.klen[tid] = (uint8_t)((kl ? kl - 11u : 0u) | (sl ? sl - 11u : 0u) << 3);
+            flen += (kl ? E.len[DRAC_R0] + kl + E.len[DRAC_R2] : 0u) + (sl ? E.len[DRAC_R1] + sl : 0u);
         }
     }
     if constexpr (LAYOUT == LAYOUT_MDEV || LAYOUT == LAYOUT_MDEV_PF) {
@@ -1096,6 +1179,37 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             if (pl) { lit(5); put(q->product, pl); }
             if (rl) { lit(6); put(bytes(q->pcie_root), rl); }
             lit(7); put(bytes(q->vendor), vl); close(DraLayout<LAYOUT>::LAST);
+        } else if constexpr (LAYOUT == LAYOUT_PCI_PCIE) {
+            const kxpu_dradev *q = dra_of(r);
+            const kxpu_dradevpf *f = drapf_of(r);
+            const uint32_t x = S.xlen[d], xl = x & 31u, yl = x >> 5, kk = S.klen[d];
+            const uint32_t kl = kk & 7u ? (kk & 7u) + 11u : 0u, sl = kk >> 3 ? (kk >> 3) + 11u : 0u;
+            const auto addr = [&](unsigned long long key, uint32_t L) {
+                const uint32_t dd = L - 8u;
+                for (uint32_t l = lane; l < L; l += 32u) dst[o + l] = key_addr_byte(key, dd, l);
+                o += L;
+            };
+            // the two attributes when the names sit at position at
+            const auto ports = [&](uint32_t at) {
+                if (E.pos != at || !kl) return;
+                lit(DRAC_R0); addr(r->root_port, kl);
+                if (sl) { lit(DRAC_R1); addr(r->pcie_switch, sl); }
+                lit(DRAC_R2);
+            };
+            lit(0); put(S.dec[d], gl); lit(1); ports(0u); lit(DRAC_C1B); put(bytes(q->device), dl); ports(1u);
+            lit(2); put(S.dec[d], gl); ports(2u);
+            if (nl) { lit(3); put(S.dec[d] + 10, nl); }
+            ports(3u);
+            lit(4); put(bytes(q->bdf), bl); ports(4u);
+            if (xl) { lit(DRAP_Q0); put(bytes(f->physfn), xl); }
+            ports(5u);
+            if (yl) { lit(DRAP_Q1); put(bytes(f->physfn_device), yl); }
+            ports(6u);
+            if (pl) { lit(5); put(q->product, pl); }
+            ports(7u);
+            if (rl) { lit(6); put(bytes(q->pcie_root), rl); }
+            ports(8u);
+            lit(7); put(bytes(q->vendor), vl); ports(9u); close(DraLayout<LAYOUT>::LAST);
         } else if constexpr (LAYOUT == LAYOUT_VF_VGPU) {
             const uint32_t m2 = S.meta2[d], tl = m2 & 63u, xl = (m2 >> 6) & 31u, il = m2 >> 11;
             lit(0); put(S.dec[d], gl); lit(1); put(S.dec[d], gl); lit(DRAV_I);
@@ -1737,20 +1851,23 @@ struct DraTaint {
 
 // kxpu_dra_slices[_mdev][_taint[s]]: the argument checks, the pool (literals | taint parts | head | tail), one
 // k_dra_slices<LAYOUT, NT> launch, the domain flags and the copies
+// attr_domain: the PCIe layout's attribute domain (checked by its entry point), else unread
 template <int LAYOUT, int NT = 0>
 static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, const char *pool, const char *node,
                           uint64_t generation, const typename DraLayout<LAYOUT>::Rec *devs, size_t n, uint8_t *out, size_t cap,
-                          size_t *len, uint64_t *slice_off, size_t *n_slices, const DraTaint taint = DraTaint{}) {
+                          size_t *len, uint64_t *slice_off, size_t *n_slices, const DraTaint taint = DraTaint{},
+                          const char *attr_domain = nullptr) {
     using Rec = typename DraLayout<LAYOUT>::Rec;
     using K = DraKernel<LAYOUT, NT>;
     constexpr bool TAINT = K::TAINT;
     constexpr int PARTS = K::PARTS, HEAD = PARTS - 2, TAIL = PARTS - 1;
     constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : LAYOUT == LAYOUT_MDEV ? DRAM_LITS : LAYOUT == LAYOUT_MDEV_PF ? DRAMP_LITS
-                         : LAYOUT == LAYOUT_PCI_PF ? DRAP_LITS : DRAV_LITS;
+                         : LAYOUT == LAYOUT_PCI_PF ? DRAP_LITS : LAYOUT == LAYOUT_PCI_PCIE ? DRAC_LITS : DRAV_LITS;
     constexpr int MAXF = K::MAXF;
     constexpr int F_COUNT = K::F_COUNT;
     const char *const *lits = LAYOUT == LAYOUT_PCI ? h_dra_lits : LAYOUT == LAYOUT_MDEV ? h_dram_lits
-                              : LAYOUT == LAYOUT_MDEV_PF ? h_dramp_lits : LAYOUT == LAYOUT_PCI_PF ? h_drap_lits : h_drav_lits;
+                              : LAYOUT == LAYOUT_MDEV_PF ? h_dramp_lits
+                              : LAYOUT == LAYOUT_PCI_PF || LAYOUT == LAYOUT_PCI_PCIE ? h_drap_lits : h_drav_lits;
     if (!ctx || !len || !n_slices || (n && !devs)) return KXPU_E_INVALID;
     if (!dns_subdomain_ok(driver, 63) || !dns_subdomain_ok(pool, 253) || !dns_subdomain_ok(node, 253) ||
         generation >= (1ull << 63)) {
@@ -1794,10 +1911,29 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     }
     typename K::Params E;
     memset(&E, 0, sizeof E);
+    // the PCIe layout: D1 split in C1A / C1B, and the block literals R0 / R1 / R2 for the names' position (the count of
+    // the nine keys that sort before "<attr_domain>/pcieRootPort")
+    std::vector<std::string> pcie_lits;
+    if constexpr (LAYOUT == LAYOUT_PCI_PCIE) {
+        static const char *const nine[9] = {"deviceID", "iommuGroup", "numaNode", "pciAddress", "physfnAddress",
+                                            "physfnDeviceID", "productName", "resource.kubernetes.io/pcieRoot", "vendorID"};
+        const std::string rk = std::string(attr_domain) + "/pcieRootPort", sk = std::string(attr_domain) + "/pcieSwitch";
+        uint32_t pos = 0;
+        while (pos < 9 && strcmp(nine[pos], rk.c_str()) < 0) pos++;
+        E.pos = pos;
+        const std::string after_int = "}", after_str = "\"}";
+        const std::string open = pos == 0 ? std::string() : (pos == 2 || pos == 3 ? after_int : after_str) + ",";
+        pcie_lits.assign(h_drap_lits, h_drap_lits + DRAP_LITS);
+        pcie_lits[1] = KX_C1A;
+        pcie_lits.push_back(KX_C1B);
+        pcie_lits.push_back(open + "\"" + rk + "\":{\"string\":\"");
+        pcie_lits.push_back("\"},\"" + sk + "\":{\"string\":\"");
+        pcie_lits.push_back(pos == 0 ? "\"}," : pos == 2 || pos == 3 ? "\"" : "");
+    }
     uint32_t acc = 0;
     for (int k = 0; k < PARTS; k++) {
-        const std::string s = k < LITS ? std::string(lits[k]) : k == HEAD ? head : k == TAIL ? std::string(KX_DRA_TAIL)
-                                                                                  : taint_parts[k - LITS];
+        const std::string s = k < LITS ? (LAYOUT == LAYOUT_PCI_PCIE ? pcie_lits[k] : std::string(lits[k]))
+                              : k == HEAD ? head : k == TAIL ? std::string(KX_DRA_TAIL) : taint_parts[k - LITS];
         if (acc + s.size() > (size_t)K::POOL) return KXPU_E_INVALID;  // the literals grew: the pool bound must follow
         memcpy(E.pool + acc, s.data(), s.size());
         E.off[k] = (uint16_t)acc;
@@ -1873,8 +2009,17 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
         "a device id that is not 1..6 bytes of [0-9a-f]", "iommu_group 4294967295", "product_len above 64",
         "a physfn that holds a byte outside [0-9a-f:.]",
         "a physfn_device that is not 0..6 bytes of [0-9a-f], or is set without a physfn"};
+    static const char *const why_pci_pcie[DRAC_F_COUNT] = {
+        "a product byte outside [A-Za-z0-9_.-]", "a bdf that is empty or holds a byte outside [0-9a-f:.]",
+        "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
+        "a device id that is not 1..6 bytes of [0-9a-f]", "iommu_group 4294967295", "product_len above 64",
+        "a physfn that holds a byte outside [0-9a-f:.]",
+        "a physfn_device that is not 0..6 bytes of [0-9a-f], or is set without a physfn",
+        "a root_port or pcie_switch that is a host-bridge key or has a bit of 48..62 set",
+        "a pcie_switch without a root_port"};
     const char *const *why = LAYOUT == LAYOUT_PCI ? why_pci : LAYOUT == LAYOUT_MDEV ? why_mdev
-                             : LAYOUT == LAYOUT_MDEV_PF ? why_mdev_pf : LAYOUT == LAYOUT_PCI_PF ? why_pci_pf : why_vf_vgpu;
+                             : LAYOUT == LAYOUT_MDEV_PF ? why_mdev_pf : LAYOUT == LAYOUT_PCI_PF ? why_pci_pf
+                             : LAYOUT == LAYOUT_PCI_PCIE ? why_pci_pcie : why_vf_vgpu;
     const uint32_t *flags = reinterpret_cast<const uint32_t *>(h.data() + slices + 1);
     for (int f = 0; f < F_COUNT; f++)
         if (flags[f]) {
@@ -1923,16 +2068,18 @@ template <int LAYOUT>
 static int32_t dra_slices_tainted(kxpu_ctx *ctx, const char *what, const char *driver, const char *pool, const char *node,
                                   uint64_t generation, const typename DraLayout<LAYOUT>::Rec *devs, size_t n,
                                   const kxpu_dra_taint *taints, size_t n_taints, const int64_t *taint_since, uint8_t *out,
-                                  size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
+                                  size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices,
+                                  const char *attr_domain = nullptr) {
     if (!taint_since)
         return dra_slices<LAYOUT>(ctx, LAYOUT == LAYOUT_PCI ? "dra_slices" : LAYOUT == LAYOUT_MDEV ? "dra_slices_mdev" : what,
-                                  driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices);
+                                  driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices, DraTaint{},
+                                  attr_domain);
     const DraTaint taint{taints, n_taints, taint_since};
     if (n_taints == 1)
         return dra_slices<LAYOUT, 1>(ctx, what, driver, pool, node, generation, devs, n, out, cap, len, slice_off, n_slices,
-                                     taint);
+                                     taint, attr_domain);
     return dra_slices<LAYOUT, KXPU_DRA_MAX_TAINTS>(ctx, what, driver, pool, node, generation, devs, n, out, cap, len,
-                                                   slice_off, n_slices, taint);
+                                                   slice_off, n_slices, taint, attr_domain);
 }
 
 extern "C" int32_t kxpu_dra_slices_taint(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
@@ -2007,4 +2154,35 @@ extern "C" int32_t kxpu_dra_slices_pf(kxpu_ctx *ctx, const char *driver, const c
                   "kxpu_dradevpf layout");
     return dra_slices_tainted<LAYOUT_PCI_PF>(ctx, "dra_slices_pf", driver, pool, node, generation, devs, n, taints, n_taints,
                                              taint_since, out, cap, len, slice_off, n_slices);
+}
+
+// an attribute domain of the PCIe layout: a lowercase DNS subdomain of at most 63 bytes, not kubernetes.io or k8s.io
+// nor under either
+static bool attr_domain_ok(const char *d) {
+    if (!d || !dns_subdomain_ok(d, DRAC_DOMAIN_MAX)) return false;
+    const std::string s(d);
+    for (const char *r : {"kubernetes.io", "k8s.io"}) {
+        const std::string rs(r);
+        if (s == rs || (s.size() > rs.size() && s.compare(s.size() - rs.size() - 1, rs.size() + 1, "." + rs) == 0))
+            return false;
+    }
+    return true;
+}
+
+// the one entry point of the PCIe layout: the taint-list form, taint_since == NULL giving the untainted bytes
+extern "C" int32_t kxpu_dra_slices_pcie(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                        uint64_t generation, const char *attr_domain, const kxpu_dradevpcie *devs, size_t n,
+                                        const kxpu_dra_taint *taints, size_t n_taints, const int64_t *taint_since,
+                                        uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
+    static_assert(sizeof(kxpu_dradevpcie) == 176 && alignof(kxpu_dradevpcie) == 8 &&
+                      offsetof(kxpu_dradevpcie, root_port) == 160 && offsetof(kxpu_dradevpcie, pcie_switch) == 168,
+                  "kxpu_dradevpcie layout");
+    if (!ctx) return KXPU_E_INVALID;
+    if (!attr_domain_ok(attr_domain)) {
+        KX_SET_ERR(ctx, "dra_slices_pcie: attr_domain must be a lowercase DNS subdomain of at most 63 bytes outside "
+                        "kubernetes.io and k8s.io");
+        return KXPU_E_INVALID;
+    }
+    return dra_slices_tainted<LAYOUT_PCI_PCIE>(ctx, "dra_slices_pcie", driver, pool, node, generation, devs, n, taints,
+                                               n_taints, taint_since, out, cap, len, slice_off, n_slices, attr_domain);
 }

@@ -17,7 +17,8 @@
 // and k_lcp<true> (which reads a VF's chain through its PF); the <kxpu_devrec, false> / <false> instantiations are
 // kxpu_pcie_tree's kernels.  kxpu_pcie_tree_mdev runs k_parse<kxpu_mdevrec, false>, whose leaf is the record's UUID
 // below its parent function (lanes 8..11 stage the record's UUID and parent next to the path), and kxpu_pcie_tree's
-// other kernels.
+// other kernels.  kxpu_pcie_ports runs kxpu_pcie_tree's parse, then k_ports: the LCP pass (group_lcp<false>, shared
+// with k_lcp) writing each group's root port and switch instead of its prefix.
 #include <algorithm>
 #include <type_traits>
 
@@ -177,14 +178,11 @@ struct Tree {
     const unsigned long long *self;
 };
 
-// SR: a member whose PF has a known chain shorter than MAXD reads the PF's chain followed by the PF's own key
+// the longest common prefix of group g's member chains into k[0 .. return value); *bad: a member index >= n.  SR: a
+// member whose PF has a known chain shorter than MAXD reads the PF's chain followed by the PF's own key
 template <bool SR>
-__global__ void __launch_bounds__(256) k_lcp(const Tree T) {
-    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= T.G) return;
-    unsigned long long k[MAXD];
+__device__ __forceinline__ int group_lcp(const Tree &T, uint32_t g, unsigned long long (&k)[MAXD], bool &bad) {
     int L = -1;
-    bool bad = false;
     for (uint32_t m = T.goff[g]; m < T.goff[g + 1]; m++) {
         const uint32_t i = T.gmem[m];
         if (i >= T.n) { bad = true; continue; }
@@ -213,12 +211,50 @@ __global__ void __launch_bounds__(256) k_lcp(const Tree T) {
         }
         L = nl;
     }
+    return max(L, 0);
+}
+
+template <bool SR>
+__global__ void __launch_bounds__(256) k_lcp(const Tree T) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= T.G) return;
+    unsigned long long k[MAXD];
+    bool bad = false;
+    const int L = group_lcp<SR>(T, g, k, bad);
     if (bad) atomicOr(T.err, 1u);
-    L = max(L, 0);
 #pragma unroll
     for (int t = 0; t < MAXD; t++)
         if (t < L) T.gchain[(size_t)g * MAXD + t] = k[t];
     T.glen[g] = (uint8_t)L;
+}
+
+// kxpu_pcie_ports: the LCP pass of kxpu_pcie_tree (plain chains), then the rule of include/kxpu.h on the prefix: the
+// functions after its last host bridge are f0, f1, ...; the root port is f0, the switch f_j for the greatest odd j
+__global__ void __launch_bounds__(256) k_ports(const Tree T, unsigned long long *__restrict__ root_port,
+                                               unsigned long long *__restrict__ pcie_switch) {
+    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= T.G) return;
+    unsigned long long k[MAXD];
+    bool bad = false;
+    const int L = group_lcp<false>(T, g, k, bad);
+    if (bad) atomicOr(T.err, 1u);
+    // one pass root to leaf: a host bridge starts the function list again, f0 is the root port, each odd f_j the switch
+    unsigned long long rp = KXPU_PCIE_NO_KEY, sw = KXPU_PCIE_NO_KEY;
+    uint32_t j = 0;
+#pragma unroll
+    for (int t = 0; t < MAXD; t++) {
+        if (t >= L) continue;
+        if (k[t] & HOST_BRIDGE) {
+            rp = sw = KXPU_PCIE_NO_KEY;
+            j = 0;
+            continue;
+        }
+        if (j == 0) rp = k[t];
+        else if (j & 1u) sw = k[t];
+        j++;
+    }
+    root_port[g] = rp;
+    pcie_switch[g] = sw;
 }
 
 __device__ __forceinline__ unsigned long long mix(unsigned long long h, unsigned long long x) {
@@ -422,4 +458,64 @@ extern "C" int32_t kxpu_pcie_tree_mdev(kxpu_ctx *ctx, const kxpu_mdevrec *recs, 
                                        uint32_t *group_node, uint64_t *key, uint32_t *parent, uint8_t *depth, uint32_t *n_nodes) {
     static_assert(sizeof(kxpu_mdevrec) == 128 && offsetof(kxpu_mdevrec, parent) + 16 <= 64, "kxpu_mdevrec layout");
     return pcie_tree(ctx, recs, paths, n, group_off, group_members, n_groups, group_node, key, parent, depth, n_nodes, nullptr);
+}
+
+extern "C" int32_t kxpu_pcie_ports(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
+                                   const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
+                                   uint64_t *root_port, uint64_t *pcie_switch) {
+    static_assert(sizeof(unsigned long long) == sizeof(uint64_t), "keys");
+    if (!ctx || (n && (!recs || !paths)) || !group_off) return KXPU_E_INVALID;
+    if (n >= (1ull << 28) || n_groups >= (1ull << 28)) return KXPU_E_UNSUPPORTED;
+    for (size_t g = 0; g < n_groups; g++)
+        if (group_off[g + 1] < group_off[g]) { KX_SET_ERR(ctx, "pcie_ports: group %zu: offsets decrease", g); return KXPU_E_INVALID; }
+    const size_t nm = group_off[n_groups];
+    if ((nm && !group_members) || (n_groups && (!root_port || !pcie_switch))) return KXPU_E_INVALID;
+    if (n_groups == 0) return KXPU_OK;
+    if (nm >= 0x7FFFFFFFull) return KXPU_E_UNSUPPORTED;
+
+    std::lock_guard<std::mutex> guard(ctx->mu);
+    cudaSetDevice(ctx->device);
+    kx_clear_timings(ctx);
+    const size_t G = n_groups;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
+    const size_t o_recs = take(n * sizeof(kxpu_devrec)), o_paths = take(n * sizeof(kxpu_pcipath));
+    const size_t o_goff = take((G + 1) * 4), o_gmem = take(nm * 4), o_chain = take(n * MAXD * 8), o_clen = take(n);
+    const size_t o_rp = take(G * 8), o_sw = take(G * 8), o_err = take(16);
+    KxScratch sc(ctx);
+    uint8_t *b = nullptr;
+    KX_CUDA(ctx, sc.alloc((void **)&b, off));
+    cudaStream_t st = ctx->stream;
+    auto up = [&](size_t o, const void *h, size_t bytes) { if (bytes) cudaMemcpyAsync(b + o, h, bytes, cudaMemcpyHostToDevice, st); };
+    up(o_recs, recs, n * sizeof(kxpu_devrec)); up(o_paths, paths, n * sizeof(kxpu_pcipath));
+    up(o_goff, group_off, (G + 1) * 4); up(o_gmem, group_members, nm * 4);
+    cudaMemsetAsync(b + o_err, 0, 16, st);
+    Tree T;
+    memset(&T, 0, sizeof T);  // k_ports reads goff, gmem, n, G, chain, clen and err only
+    T.goff = (const uint32_t *)(b + o_goff); T.gmem = (const uint32_t *)(b + o_gmem);
+    T.n = (uint32_t)n; T.G = (uint32_t)G;
+    T.chain = (const unsigned long long *)(b + o_chain); T.clen = (const uint8_t *)(b + o_clen);
+    T.err = (uint32_t *)(b + o_err);
+    unsigned long long *d_rp = (unsigned long long *)(b + o_rp), *d_sw = (unsigned long long *)(b + o_sw);
+    {
+        KxTimer tm(ctx, KXPU_T_CLASSIFY);
+        if (n) {
+            k_parse<kxpu_devrec, false><<<(unsigned)((n + PARSE_RECS - 1) / PARSE_RECS), PARSE_THREADS, 0, st>>>(
+                (const kxpu_devrec *)(b + o_recs), (const kxpu_pcipath *)(b + o_paths), (uint32_t)n,
+                (unsigned long long *)(b + o_chain), b + o_clen, nullptr);
+            ctx->launches++;
+        }
+        k_ports<<<(unsigned)((G + 255) / 256), 256, 0, st>>>(T, d_rp, d_sw);
+        ctx->launches++;
+    }
+    uint32_t *h = ctx->h_ctl;
+    cudaMemcpyAsync(h, T.err, 4, cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "pcie_ports failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    if (h[0]) { KX_SET_ERR(ctx, "pcie_ports: a group member index is >= n"); return KXPU_E_INVALID; }
+    cudaMemcpyAsync(root_port, d_rp, G * 8, cudaMemcpyDeviceToHost, st);
+    cudaMemcpyAsync(pcie_switch, d_sw, G * 8, cudaMemcpyDeviceToHost, st);
+    e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "pcie_ports D2H failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    return KXPU_OK;
 }

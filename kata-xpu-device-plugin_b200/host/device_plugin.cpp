@@ -738,6 +738,31 @@ static bool qualifiedName(const std::string &v) {
     return true;
 }
 
+// draPcieDomain (kxpu_dra_slices_pcie's attr_domain): empty, or a lowercase DNS subdomain of at most 63 bytes that is
+// neither kubernetes.io nor k8s.io nor under either, and only with a passthrough class that has a draDriver
+Error Plugin::checkDraPcieDomain() const {
+    const std::string &d = draPcieDomain;
+    if (d.empty()) return Error();
+    const std::string what = "draPcieDomain \"" + d + "\"";
+    bool ok = d.size() <= 63;
+    for (size_t start = 0; ok && start <= d.size();) {
+        size_t end = d.find('.', start);
+        if (end == std::string::npos) end = d.size();
+        auto lower = [](char ch) { return (ch >= '0' && ch <= '9') || (ch >= 'a' && ch <= 'z'); };
+        ok = end > start && end - start <= 63 && lower(d[start]) && lower(d[end - 1]);
+        for (size_t i = start; ok && i < end; i++) ok = lower(d[i]) || d[i] == '-';
+        start = end + 1;
+    }
+    if (!ok) return fail(what + " is not a lowercase DNS subdomain of at most 63 bytes");
+    for (const char *reserved : {"kubernetes.io", "k8s.io"}) {
+        const std::string r(reserved);
+        if (d == r || (d.size() > r.size() && d.compare(d.size() - r.size() - 1, std::string::npos, "." + r) == 0))
+            return fail(what + " is reserved: names under " + r + " are the standard attributes'");
+    }
+    if (!draEnabled()) return fail(what + " is set but no passthrough class has a draDriver");
+    return Error();
+}
+
 Error Plugin::checkResourceNames() const {
     size_t total = 0;
     std::map<std::string, size_t> classOf;  // name -> the class that configures it
@@ -1264,6 +1289,13 @@ Error Plugin::classify(PciWalk &w) {
         }
         if (rc != KXPU_OK) return kxfail(ctx_, sriovAware ? "kxpu_pcie_tree_sriov" : "kxpu_pcie_tree", rc);
     }
+    if (!draPcieDomain.empty()) {  // each group's root port and switch, from the paths every DRA walk reads
+        w.rootPort.assign(c.nGroups + 1, KXPU_PCIE_NO_KEY);
+        w.pcieSwitch.assign(c.nGroups + 1, KXPU_PCIE_NO_KEY);
+        rc = kxpu_pcie_ports(ctx_, recs.data(), w.paths.data(), n, c.goff.data(), c.gmem.data(), c.nGroups,
+                             w.rootPort.data(), w.pcieSwitch.data());
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_pcie_ports", rc);
+    }
     return Error();
 }
 
@@ -1313,6 +1345,7 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
         s.klass = groupClass[c.gids[g]];
         if (topologyAware) s.numa = c.gnuma[g];
         if (pcieTopologyAware) s.pcieNode = w.gnode[g];
+        if (!draPcieDomain.empty()) { s.rootPort = w.rootPort[g]; s.pcieSwitch = w.pcieSwitch[g]; }
         if (groupViability && c.gblk[g] != KXPU_VIABLE) s.blocker = blockerOf(w.recs[c.gblk[g]]);
         if (s.blocker.empty() && xpuClasses[s.klass].vfioCdev)  // a member without a cdev: VFIO cannot open it
             for (const NvidiaGpuDevice &d : devs)
@@ -2286,6 +2319,7 @@ Error Plugin::InitiateDevicePlugin() {
     if (!e) e = checkResetMethods();
     if (!e && vgpuSriovAware && vgpuClasses.empty()) e = fail("vgpuSriovAware is set but no vGPU class is configured");
     if (!e && sriovPfAware && !sriovAware) e = fail("sriovPfAware is set but sriovAware is off");
+    if (!e) e = checkDraPcieDomain();
     if (e) return e;
     e = createIommuDeviceMap();  // :46
     if (e) return e;
@@ -2528,15 +2562,20 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     std::map<std::string, std::pair<std::string, std::string>> pfWas;  // sriovPfAware: group id -> its PF and PF device id
     for (size_t g = 0; sriovPfAware && g < iommuMap.size(); g++)
         pfWas[iommuMap[g].first] = {iommuState[g].pf, iommuState[g].pfDevice};
+    std::map<std::string, std::pair<uint64_t, uint64_t>> portsWas;  // draPcieDomain: group id -> its root port and switch
+    for (size_t g = 0; !draPcieDomain.empty() && g < iommuMap.size(); g++)
+        portsWas[iommuMap[g].first] = {iommuState[g].rootPort, iommuState[g].pcieSwitch};
     PciWalk pw;
     Error e = rewalk(pw, pci_, report.pci);
     if (e) return e;
-    bool viabilityChanged = false, pfChanged = false;
+    bool viabilityChanged = false, pfChanged = false, portsChanged = false;
     for (size_t g = 0; g < iommuMap.size(); g++) {
         auto it = blockerWas.find(iommuMap[g].first);
         viabilityChanged |= it != blockerWas.end() && it->second != iommuState[g].blocker;
         auto pt = pfWas.find(iommuMap[g].first);  // a VF whose PF changed is published with other attributes
         pfChanged |= pt != pfWas.end() && pt->second != std::make_pair(iommuState[g].pf, iommuState[g].pfDevice);
+        auto qt = portsWas.find(iommuMap[g].first);  // a device moved under another root port or switch
+        portsChanged |= qt != portsWas.end() && qt->second != std::make_pair(iommuState[g].rootPort, iommuState[g].pcieSwitch);
     }
     if (!vgpuClasses.empty()) {
         MdevWalk mw;
@@ -2614,7 +2653,7 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     updateAerTaints(aerPt, aerVg);
     const bool driftCleared = !driftTaint_.empty();  // the walk is the new truth: every drift reason is gone
     driftTaint_.clear();
-    if (passthroughChanged || viabilityChanged || pfChanged || aerPt || driftCleared) pci_.draGeneration++;  // the next publication replaces these slices
+    if (passthroughChanged || viabilityChanged || pfChanged || portsChanged || aerPt || driftCleared) pci_.draGeneration++;  // the next publication replaces these slices
     if (vgpuChanged || aerVg) mdev_.draGeneration++;
     // 6. a fresh snapshot generation: Allocate answers from the snapshot again
     pci_.haveGen = haveGen;
@@ -2808,11 +2847,8 @@ static void forPublishedVfVgpu(const OrderedMap<std::vector<NvidiaGpuDevice>> &m
             f(m[g].first, state[g]);
 }
 
-template <typename Rec>
-Error Plugin::draSlices(int32_t (*fn)(kxpu_ctx *, const char *, const char *, const char *, uint64_t, const Rec *, size_t,
-                                      const kxpu_dra_taint *, size_t, const int64_t *, uint8_t *, size_t, size_t *, uint64_t *,
-                                      size_t *),
-                        const char *what, const std::string &driver, uint64_t generation, const std::vector<Rec> &devs,
+template <typename Rec, typename Fn>
+Error Plugin::draSlices(Fn fn, const char *what, const std::string &driver, uint64_t generation, const std::vector<Rec> &devs,
                         const std::vector<std::string> &groups, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff,
                         bool typeTaint) const {
     const std::string missing = driver + kDraTaintKeyName, aer = driver + kAerTaintKeyName, type = driver + kTypeTaintKeyName;
@@ -2847,6 +2883,7 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
             for (const Device &d : dp.devs) productOf[d.ID] = d.model.empty() ? &dp.devpluginName : &d.model;
     std::vector<kxpu_dradev> devs;
     std::vector<kxpu_dradevpf> pfDevs;  // sriovPfAware: the same devices with their PFs
+    std::vector<kxpu_dradevpcie> pcieDevs;  // draPcieDomain: the same devices with their PFs (sriovPfAware) and ports
     std::vector<std::string> groups;
     forPublished(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const GroupState<kxpu_dradev> &s) {
         if (s.klass != xpuClass) return;
@@ -2857,17 +2894,39 @@ Error Plugin::ResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, std::ve
             memcpy(d.product, it->second->data(), d.product_len);
         }
         groups.push_back(g);
-        if (!sriovPfAware) {
+        if (!sriovPfAware && draPcieDomain.empty()) {
             devs.push_back(d);
             return;
         }
         kxpu_dradevpf p;
         memset(&p, 0, sizeof p);
         p.dev = d;
-        memcpy(p.physfn, s.pf.data(), std::min(s.pf.size(), sizeof p.physfn));
-        memcpy(p.physfn_device, s.pfDevice.data(), std::min(s.pfDevice.size(), sizeof p.physfn_device));
-        pfDevs.push_back(p);
+        if (sriovPfAware) {
+            memcpy(p.physfn, s.pf.data(), std::min(s.pf.size(), sizeof p.physfn));
+            memcpy(p.physfn_device, s.pfDevice.data(), std::min(s.pfDevice.size(), sizeof p.physfn_device));
+        }
+        if (draPcieDomain.empty()) {
+            pfDevs.push_back(p);
+            return;
+        }
+        kxpu_dradevpcie q;
+        memset(&q, 0, sizeof q);
+        q.pf = p;
+        q.root_port = s.rootPort;
+        q.pcie_switch = s.pcieSwitch;
+        pcieDevs.push_back(q);
     });
+    if (!draPcieDomain.empty()) {
+        const char *domain = draPcieDomain.c_str();
+        auto fn = [domain](kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                           const kxpu_dradevpcie *v, size_t n, const kxpu_dra_taint *taints, size_t nt, const int64_t *since,
+                           uint8_t *o, size_t cap, size_t *len, uint64_t *off, size_t *ns) {
+            return kxpu_dra_slices_pcie(ctx, driver, pool, node, generation, domain, v, n, taints, nt, since, o, cap, len,
+                                        off, ns);
+        };
+        return draSlices(fn, "kxpu_dra_slices_pcie", xpuClasses[xpuClass].draDriver, pci_.draGeneration, pcieDevs, groups,
+                         out, sliceOff);
+    }
     if (sriovPfAware)
         return draSlices(kxpu_dra_slices_pf, "kxpu_dra_slices_pf", xpuClasses[xpuClass].draDriver, pci_.draGeneration,
                          pfDevs, groups, out, sliceOff);
@@ -4572,6 +4631,7 @@ int kxh_devs_aer(void *h, int plugin_index, char *out, size_t cap) {
 void kxh_set_vf_vgpu_health(void *h, int on) { ((Plugin *)h)->vfVgpuHealth = on != 0; }
 void kxh_set_vgpu_sriov(void *h, int on) { ((Plugin *)h)->vgpuSriovAware = on != 0; }
 void kxh_set_sriov_pf(void *h, int on) { ((Plugin *)h)->sriovPfAware = on != 0; }
+void kxh_set_dra_pcie_domain(void *h, const char *domain) { ((Plugin *)h)->draPcieDomain = domain ? domain : ""; }
 uint64_t kxh_mdev_physfn_reads(void *h) { return ((Plugin *)h)->mdevPhysfnReads; }
 // refreshVfVgpuTypes: changed as kxh_refresh_aer_health's; *moved = bit 0 passthroughMoved, bit 1 typesMoved
 int kxh_refresh_vf_vgpu_types(void *h, size_t *changed, size_t cap, size_t *n_changed, int *moved, char *err, size_t errcap) {

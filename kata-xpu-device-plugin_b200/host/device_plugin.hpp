@@ -285,6 +285,8 @@ struct PciWalk {
     // first blocking member or KXPU_VIABLE
     std::vector<kxpu_sriovrec> srs;
     std::vector<uint32_t> pfOf, numvfs, gsriov;
+    // draPcieDomain: per group ordinal its root port and switch (kxpu_pcie_ports), or KXPU_PCIE_NO_KEY
+    std::vector<uint64_t> rootPort, pcieSwitch;
     // resetCheck: per record its reset_method (or reset) read, and kxpu_reset_check's methods and set verdict; per group
     // ordinal the reset blocker or KXPU_VIABLE
     std::vector<kxpu_resetrec> rrs;
@@ -363,6 +365,9 @@ struct GroupState {
     std::string drift{};
     // passthrough: the device id of the group's first member (readIDFromFile's text); names Device::model
     std::string firstDevice{};
+    // draPcieDomain, passthrough only: the group's root port and nearest switch upstream port (kxpu_pcie_ports' function
+    // keys), or KXPU_PCIE_NO_KEY
+    uint64_t rootPort = KXPU_PCIE_NO_KEY, pcieSwitch = KXPU_PCIE_NO_KEY;
 };
 
 class Plugin {
@@ -566,6 +571,21 @@ class Plugin {
     //     exactly as without the setting, and a rediscovery that changes a published VF's PF moves draGeneration().
     // Allocate, CDI specs, GetPreferredAllocation and ListAndWatch topology do not change.
     bool sriovPfAware = false;
+    // PCIe root ports and switches in DRA (include/kxpu.h, kxpu_pcie_ports and kxpu_dra_slices_pcie): a DNS subdomain
+    // that qualifies two more attributes of every passthrough DRA pool.  InitiateDevicePlugin refuses a value that is not
+    // a lowercase DNS subdomain of at most 63 bytes, one equal to or under kubernetes.io or k8s.io, and any value while
+    // no passthrough class has a draDriver.  Empty (default): no new call runs and every output, generation and counter
+    // is as above.  Set:
+    //   - each PCI walk makes one kxpu_pcie_ports call over the classify CSR, on the paths every DRA walk reads (no new
+    //     file or link is read), and each group keeps its root port and switch (GroupState::rootPort / pcieSwitch);
+    //   - ResourceSlices publishes every passthrough class through kxpu_dra_slices_pcie: a device carries
+    //     <draPcieDomain>/pcieRootPort and <draPcieDomain>/pcieSwitch where they exist, one name for every class, so a
+    //     claim can keep a GPU and a NIC VF of two DRA drivers under one root port or one switch (matchAttribute).  The
+    //     PF attributes follow sriovPfAware as above;
+    //   - a rediscovery that moves a published group under another root port or switch moves draGeneration().
+    // Allocate, PrepareDraDevices, CDI specs, ListAndWatch, GetPreferredAllocation, metrics and the vGPU pools do not
+    // change.
+    std::string draPcieDomain;
     // (type ID, type key) of every vGPU type a walk of this process named: the last name table of kxpu_vf_vgpu_types, so a
     // GPU that became full keeps its names across rediscover
     const std::map<uint32_t, std::string> &learnedVgpuTypes() const { return learnedVgpuTypes_; }
@@ -850,13 +870,13 @@ class Plugin {
     // table <driver>/unhealthy=vfio-device-missing, then with aerHealth <driver>/pcie-aer=fatal and =nonfatal, then with
     // typeTaint (a VF-vGPU pool under vfVgpuHealth) all three and <driver>/vgpu-type=changed, all NoSchedule; without
     // draTaints taint_since is NULL (the untainted bytes)
-    template <typename Rec>
-    Error draSlices(int32_t (*fn)(kxpu_ctx *, const char *, const char *, const char *, uint64_t, const Rec *, size_t,
-                                  const kxpu_dra_taint *, size_t, const int64_t *, uint8_t *, size_t, size_t *, uint64_t *, size_t *),
-                    const char *what, const std::string &driver, uint64_t generation, const std::vector<Rec> &devs,
+    // fn: a slice call of the taint-list form (kxpu_dra_slices_taints' signature for Rec), or one wrapping such a call
+    template <typename Rec, typename Fn>
+    Error draSlices(Fn fn, const char *what, const std::string &driver, uint64_t generation, const std::vector<Rec> &devs,
                     const std::vector<std::string> &groups, std::vector<uint8_t> &out, std::vector<uint64_t> &sliceOff,
                     bool typeTaint = false) const;
     Error checkDraClasses() const;
+    Error checkDraPcieDomain() const;
     void buildMdevDra(const MdevWalk &w);
     void buildVfVgpuDra(const PciWalk &w);
 };

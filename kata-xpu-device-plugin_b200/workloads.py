@@ -645,6 +645,40 @@ def dra_pf_devices(n=1 << 16, vf_every=8, seed=41):
     return d
 
 
+def dra_pcie_devices(n=1 << 16, vf_every=8, seed=41):
+    """kxpu_dra_slices_pcie's input: dra_pf_devices(n, vf_every) with a root port on every device and a switch on three
+    in four: 4-digit domains, 12-byte addresses"""
+    from .binding import DRADEVPCIE_DTYPE, PCIE_NO_KEY
+    d = np.zeros(n, DRADEVPCIE_DTYPE)
+    d["pf"] = dra_pf_devices(n, vf_every, seed)
+    k = np.arange(n, dtype=np.uint64)
+    d["root_port"] = (k >> np.uint64(6) & np.uint64(0xff)) << np.uint64(8) | np.uint64(8)
+    d["pcie_switch"] = np.where(k % 4 != 3, d["root_port"] + np.uint64(0x100), np.uint64(PCIE_NO_KEY))
+    return d
+
+
+def pcie_ports_walk(n=1 << 20, vf_every=8):
+    """kxpu_pcie_ports' and kxpu_pcie_tree's input: n functions, one group each, two sockets of four root ports, a switch
+    below each root port and 256 down ports below each switch; one in vf_every functions is a VF beside function 0 of
+    its bus"""
+    from .binding import DEVREC_DTYPE, PCIPATH_DTYPE
+    recs = np.zeros(n, DEVREC_DTYPE)
+    paths = np.zeros(n, PCIPATH_DTYPE)
+    bdfs, ps = [], []
+    for i in range(n):
+        sock, rp, dp, fn = i >> 19 & 1, i >> 17 & 3, i >> 9 & 0xff, i & 0x1ff
+        hb = 0x80 * sock
+        bus = 0x10 + (dp & 0x3f)
+        bdf = "%04x:%02x:%02x.%d" % (1 + (i >> 15), bus, fn >> 4 & 0x1f, (fn & 7) if i % vf_every == 0 else 0)
+        bdfs.append(bdf.encode())
+        ps.append(("pci0000:%02x/0000:%02x:%02x.0/0000:%02x:00.0/0000:%02x:%02x.0/%s" %
+                   (hb, hb, 1 + rp, hb + 1 + rp, hb + 8, dp & 0x1f, bdf)).encode())
+    recs["bdf"] = bdfs
+    paths["path"] = ps
+    paths["len"] = [len(p) for p in ps]
+    return recs, paths, np.arange(n + 1, dtype=np.uint32), np.arange(n, dtype=np.uint32)
+
+
 def dra_mdev_devices(n=1 << 16, seed=43):
     """n published vGPUs with every optional attribute present and the longest fields the host produces: a 64-byte
     product name, a 40-byte type key, a 12-byte parent address, a 10-byte PCIe root, 4-digit ids, one NUMA node, 9-digit

@@ -88,6 +88,14 @@ print("mdev_pf resolved", int((mpwant != B.NO_PF).sum()), "slice bytes",
 pfdevs = W.dra_pf_devices(300)
 print("dra_pf slice bytes", len(kx.dra_slices_pf("d", "p", "n", 1, pfdevs, [], None)[0]),
       len(kx.dra_slices_pf("d", "p", "n", 1, pfdevs, [("d/k", "", "NoSchedule")], np.full((300, 1), 5, np.int64))[0]))
+# PCIe root ports and switches: the ports of a walk, then the slices untainted and with a one-entry table
+prr, prp, pro, prm = W.pcie_ports_walk(3000)
+prt, pst = kx.pcie_ports(prr, prp, pro, prm)
+pcdevs = W.dra_pcie_devices(300)
+print("pcie_ports switches", int((pst != B.PCIE_NO_KEY).sum()), "dra_pcie slice bytes",
+      len(kx.dra_slices_pcie("d", "p", "n", 1, "pcie.example.com", pcdevs, [], None)[0]),
+      len(kx.dra_slices_pcie("d", "p", "n", 1, "pcie.example.com", pcdevs, [("d/k", "", "NoSchedule")],
+                             np.full((300, 1), 5, np.int64))[0]))
 # resets between tenants: every member's function reset or bus-reset set, on the classify CSR
 rrecs, rpaths, rrrs = W.reset_walk(20000)
 rres = kx.classify_rules([(b"10de", b"vfio-pci")], rrecs)
