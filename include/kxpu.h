@@ -71,7 +71,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_FINALIZE 1
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
-#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s, kxpu_pcie_ports', kxpu_sriov's, kxpu_mdev_pf's and kxpu_reset_check's kernels: the slot holds the most recent call's */
+#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s, kxpu_pcie_ports[_mdev]', kxpu_sriov's, kxpu_mdev_pf's and kxpu_reset_check's kernels: the slot holds the most recent call's */
 #define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev|_vf_vgpu[_cdev]]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
@@ -1603,6 +1603,81 @@ int32_t kxpu_dra_slices_pcie(kxpu_ctx *ctx, const char *driver, const char *pool
                              const char *attr_domain, const kxpu_dradevpcie *devs, size_t n, const kxpu_dra_taint *taints,
                              size_t n_taints, const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out,
                              size_t cap, size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
+/* ------------------------------ PCIe root ports and switches of vGPUs in DRA (addition to ABI v14) */
+
+/* These calls and their records were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym), as
+ * for kxpu_pcie_ports.  They publish the same two attributes for the vGPU pools, so that a claim can keep a vGPU and a
+ * device of another DRA driver (a NIC VF) under one root port or one switch.
+ *
+ * THE RULE FOR vGPUs.  The PARENT CHAIN of an mdev is its kxpu_pcie_tree_mdev chain without its last key (the parent
+ * function): the parent GPU's own chain, the one kxpu_pcie_tree gives the parent as a PCI record.  A group's chain is the
+ * longest common prefix of its members' parent chains whose path is known (members with an unknown path are skipped, as
+ * in kxpu_pcie_tree).  Root port and switch follow kxpu_pcie_ports' rule on that chain, unchanged.  So:
+ *   - a parent that is a VF needs nothing more: its path sits beside its PF's, so its parent chain gives the PF's ports
+ *     (physfn is not consulted);
+ *   - a parent directly below a host bridge gets KXPU_PCIE_NO_KEY for both;
+ *   - when the parent functions are also in a PCI walk, every mdev gets exactly the keys kxpu_pcie_ports gives its
+ *     parent's record (alone in its group).
+ * A vGPU on a VF (kxpu_dravfvgpu) is a PCI record: kxpu_pcie_ports' output for its group is used as is. */
+
+/* The root port and switch of each mdev group, by the rule above.  recs / paths / n / group_off / group_members /
+ * n_groups are kxpu_pcie_tree_mdev's (paths in its grammar: the leaf is the record's UUID below its parent function);
+ * root_port[g] and pcie_switch[g] (n_groups entries each) receive the two keys of group g.  The contract is
+ * kxpu_pcie_ports', word for word: its KXPU_E_INVALID cases and limits, nothing written on either.
+ * GPU: kxpu_pcie_tree_mdev's path parse, then kxpu_pcie_ports' kernel as a compile-time variant that reads each member's
+ * chain one key short.  Timed under KXPU_T_CLASSIFY. */
+int32_t kxpu_pcie_ports_mdev(kxpu_ctx *ctx, const kxpu_mdevrec *recs, const kxpu_pcipath *paths, size_t n,
+                             const uint32_t *group_off /* [n_groups+1] */, const uint32_t *group_members, size_t n_groups,
+                             uint64_t *root_port /* [n_groups] */, uint64_t *pcie_switch /* [n_groups] */);
+
+/* One published mdev vGPU with its parent's PF and its ports.  256 bytes, a multiple of 16; alignof 8. */
+typedef struct kxpu_dramdevpcie {
+    kxpu_dramdevpf pf;        /* kxpu_dra_slices_mdev_pf's record, unchanged                                      */
+    uint64_t root_port;       /* the group's root port (kxpu_pcie_ports_mdev), or KXPU_PCIE_NO_KEY                 */
+    uint64_t pcie_switch;     /* the group's nearest switch upstream port, or KXPU_PCIE_NO_KEY                     */
+} kxpu_dramdevpcie;
+
+/* The ResourceSlices of one pool of mdev vGPUs with their PCIe ports.  The contract is kxpu_dra_slices_mdev_pf's, word
+ * for word, with kxpu_dra_slices_pcie's additions: the attr_domain checks (KXPU_E_INVALID), the key checks
+ * (KXPU_E_UNSUPPORTED, after kxpu_dra_slices_mdev_pf's domain of each record's pf, in its order) and the two attributes
+ *   "<attr_domain>/pcieRootPort":{"string":"<address of root_port>"}
+ *   "<attr_domain>/pcieSwitch":{"string":"<address of pcie_switch>"}
+ * each only when its key is not KXPU_PCIE_NO_KEY, with kxpu_dra_slices_pcie's address form.  The two names are adjacent
+ * and sort as one block at one of the 12 positions among the layout's 11 keys (0: before iommuGroup .. 11: after
+ * uuid): "example.com" sorts before iommuGroup, "x.io" after uuid.  No lowercase domain sorts between parentAddress and
+ * parentDeviceID, between parentDeviceID and parentVendorID, or between physfnAddress and physfnDeviceID (the two keys
+ * differ from the name in an uppercase byte), so positions 4, 5 and 7 never occur.  With every key KXPU_PCIE_NO_KEY the
+ * bytes are kxpu_dra_slices_mdev_pf's for any valid attr_domain, and with every physfn empty too,
+ * kxpu_dra_slices_mdev_taints'.
+ * GPU: the kernel of kxpu_dra_slices for this record layout, untainted and with the taint list (one entry for
+ * n_taints == 1, KXPU_DRA_MAX_TAINTS for more).  The host computes the names' position once per call; the device's warp
+ * formats the addresses.  Timed under KXPU_T_EMIT. */
+int32_t kxpu_dra_slices_mdev_pcie(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                  uint64_t generation, const char *attr_domain, const kxpu_dramdevpcie *devs, size_t n,
+                                  const kxpu_dra_taint *taints, size_t n_taints,
+                                  const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out, size_t cap,
+                                  size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
+/* One published vGPU on a VF with its ports.  208 bytes, a multiple of 16; alignof 8. */
+typedef struct kxpu_dravfvgpupcie {
+    kxpu_dravfvgpu dev;       /* kxpu_dra_slices_vf_vgpu's record, unchanged                                      */
+    uint64_t root_port;       /* the VF's group's root port (kxpu_pcie_ports), or KXPU_PCIE_NO_KEY                 */
+    uint64_t pcie_switch;     /* the VF's group's nearest switch upstream port, or KXPU_PCIE_NO_KEY                */
+} kxpu_dravfvgpupcie;
+
+/* The ResourceSlices of one pool of vGPUs on VFs with their PCIe ports.  The contract is kxpu_dra_slices_vf_vgpu's, word
+ * for word, with the same additions as kxpu_dra_slices_mdev_pcie (the key checks after kxpu_dra_slices_vf_vgpu's
+ * domain).  The block of the two names sits at one of the 11 positions among the layout's 10 keys (0: before
+ * iommuGroup .. 10: after vgpuTypeID).  No lowercase domain sorts between parentAddress and parentDeviceID, between
+ * parentDeviceID and parentVendorID, or between vgpuType and vgpuTypeID, so positions 3, 4 and 9 never occur.  With every
+ * key KXPU_PCIE_NO_KEY the bytes are kxpu_dra_slices_vf_vgpu's for any valid attr_domain.
+ * GPU: as kxpu_dra_slices_mdev_pcie, for this record layout.  Timed under KXPU_T_EMIT. */
+int32_t kxpu_dra_slices_vf_vgpu_pcie(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                     uint64_t generation, const char *attr_domain, const kxpu_dravfvgpupcie *devs,
+                                     size_t n, const kxpu_dra_taint *taints, size_t n_taints,
+                                     const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out, size_t cap,
+                                     size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
 
 /* ------------------------------------- resets between tenants (addition to ABI v14) */
 

@@ -543,6 +543,24 @@ func (k *kxpu) pciePorts(recs []C.kxpu_devrec, paths []C.kxpu_pcipath, goff, gme
 	return rootPort[:nGroups], pcieSwitch[:nGroups], err
 }
 
+// the root port and nearest switch of each mdev group (an addition to ABI v14, detected by symbol): pcieTreeMdev's
+// inputs, the keys of each group's parent GPU, or C.KXPU_PCIE_NO_KEY.  Called once per mdev walk when
+// draVgpuPcieConfig.DraVgpuPcie is set and a vGPU class has a draDriver.
+func (k *kxpu) pciePortsMdev(recs []C.kxpu_mdevrec, paths []C.kxpu_pcipath, goff, gmem []uint32, nGroups int) (rootPort,
+	pcieSwitch []uint64, err error) {
+	rootPort, pcieSwitch = make([]uint64, nGroups+1), make([]uint64, nGroups+1)
+	var r unsafe.Pointer
+	var pp *C.kxpu_pcipath
+	if len(recs) > 0 {
+		r, pp = unsafe.Pointer(&recs[0]), &paths[0]
+	}
+	gm := append(gmem, 0) // a valid pointer for an empty walk
+	err = kxCheck(k.ctx, "kxpu_pcie_ports_mdev", C.kxpu_pcie_ports_mdev(k.ctx, (*C.kxpu_mdevrec)(r), pp,
+		C.size_t(len(recs)), (*C.uint32_t)(unsafe.Pointer(&goff[0])), (*C.uint32_t)(unsafe.Pointer(&gm[0])),
+		C.size_t(nGroups), (*C.uint64_t)(unsafe.Pointer(&rootPort[0])), (*C.uint64_t)(unsafe.Pointer(&pcieSwitch[0]))))
+	return rootPort[:nGroups], pcieSwitch[:nGroups], err
+}
+
 // pcieTree over records that carry only their address, one per link target (walk order): what pcieTree sees of a walk
 func (k *kxpu) pcieTreeOfLinks(bdfs, targets []string, goff, gmem []uint32) (gnode, parent []uint32, depth []uint8, err error) {
 	recs, paths := make([]C.kxpu_devrec, len(bdfs)), make([]C.kxpu_pcipath, len(bdfs))
@@ -991,6 +1009,51 @@ func (k *kxpu) draSlicesPcie(driver, node string, generation uint64, domain stri
 		ns *C.size_t) C.int32_t {
 		return C.kxpu_dra_slices_pcie(k.ctx, cd, cn, cn, C.uint64_t(generation), cdom, p, C.size_t(len(devs)), tab, nt, cs,
 			out, capacity, n, off, ns)
+	})
+}
+
+// draVgpuPcieConfig is Plugin::draVgpuPcie: false (default) publishes the vGPU pools as before; true, only with
+// DraPcieDomain set and a vGPU class that publishes DRA, publishes them through draSlicesMdevPcie and
+// draSlicesVfVgpuPcie under DraPcieDomain's names.
+type draVgpuPcieConfig struct {
+	DraVgpuPcie bool
+}
+
+// DRA ResourceSlices of mdev vGPUs with their parent GPU's PCIe root port and switch (an addition to ABI v14, detected
+// by symbol).  devs: one kxpu_dramdevpcie per published group, draSlicesMdevPf's record and pciePortsMdev's keys; with
+// every key C.KXPU_PCIE_NO_KEY the bytes are draSlicesMdevPf's.
+func (k *kxpu) draSlicesMdevPcie(driver, node string, generation uint64, domain string, devs []C.kxpu_dramdevpcie,
+	since []int64) ([]string, error) {
+	var p *C.kxpu_dramdevpcie
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	cdom := C.CString(domain)
+	defer C.free(unsafe.Pointer(cdom))
+	return k.slices("kxpu_dra_slices_mdev_pcie", driver, node, len(devs), since, func(cd, cn *C.char,
+		tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
+		ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_mdev_pcie(k.ctx, cd, cn, cn, C.uint64_t(generation), cdom, p, C.size_t(len(devs)), tab, nt,
+			cs, out, capacity, n, off, ns)
+	})
+}
+
+// DRA ResourceSlices of vGPUs on VFs with their PCIe ports (an addition to ABI v14, detected by symbol).  devs: one
+// kxpu_dravfvgpupcie per published group, draSlicesVfVgpu's record and the keys pciePorts gave the VF's group; with every
+// key C.KXPU_PCIE_NO_KEY the bytes are draSlicesVfVgpu's.
+func (k *kxpu) draSlicesVfVgpuPcie(driver, node string, generation uint64, domain string, devs []C.kxpu_dravfvgpupcie,
+	since []int64) ([]string, error) {
+	var p *C.kxpu_dravfvgpupcie
+	if len(devs) > 0 {
+		p = &devs[0]
+	}
+	cdom := C.CString(domain)
+	defer C.free(unsafe.Pointer(cdom))
+	return k.slices("kxpu_dra_slices_vf_vgpu_pcie", driver, node, len(devs), since, func(cd, cn *C.char,
+		tab *C.kxpu_dra_taint, nt C.size_t, cs *C.int64_t, out *C.uint8_t, capacity C.size_t, n *C.size_t, off *C.uint64_t,
+		ns *C.size_t) C.int32_t {
+		return C.kxpu_dra_slices_vf_vgpu_pcie(k.ctx, cd, cn, cn, C.uint64_t(generation), cdom, p, C.size_t(len(devs)), tab,
+			nt, cs, out, capacity, n, off, ns)
 	})
 }
 

@@ -86,6 +86,11 @@ assert DRADEVPF_DTYPE.itemsize == 160
 DRADEVPCIE_DTYPE = np.dtype([("pf", DRADEVPF_DTYPE), ("root_port", "u8"), ("pcie_switch", "u8")])
 assert DRADEVPCIE_DTYPE.itemsize == 176
 PCIE_NO_KEY = 0xFFFFFFFFFFFFFFFF
+# kxpu_dramdevpcie / kxpu_dravfvgpupcie (vGPU DRA ResourceSlices with PCIe root ports and switches, additions to ABI v14)
+DRAMDEVPCIE_DTYPE = np.dtype([("pf", DRAMDEVPF_DTYPE), ("root_port", "u8"), ("pcie_switch", "u8")])
+assert DRAMDEVPCIE_DTYPE.itemsize == 256
+DRAVFVGPUPCIE_DTYPE = np.dtype([("dev", DRAVFVGPU_DTYPE), ("root_port", "u8"), ("pcie_switch", "u8")])
+assert DRAVFVGPUPCIE_DTYPE.itemsize == 208
 DRA_SLICE_DEVICES = 128
 DRA_MAX_DEVICES = 1 << 24
 DRA_TAINT_SLICE_DEVICES = 64  # devices per slice of the _taint calls (ABI v11) when taint_since is given
@@ -177,6 +182,7 @@ ABI_SYMBOLS = [
     "kxpu_dra_slices_vf_vgpu", "kxpu_vf_vgpu_drift", "kxpu_reset_check", "kxpu_metrics_devices",
     "kxpu_mdev_pf", "kxpu_dra_slices_mdev_pf", "kxpu_classify_named", "kxpu_dra_slices_pf",
     "kxpu_pcie_ports", "kxpu_dra_slices_pcie",
+    "kxpu_pcie_ports_mdev", "kxpu_dra_slices_mdev_pcie", "kxpu_dra_slices_vf_vgpu_pcie",
 ]
 
 
@@ -316,6 +322,11 @@ def load_library():
         "kxpu_pcie_ports": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp]),
         "kxpu_dra_slices_pcie": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, C.c_char_p, vp, sz, vp, sz, vp, vp,
                                        sz, C.POINTER(sz), vp, C.POINTER(sz)]),
+        "kxpu_pcie_ports_mdev": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp]),
+        "kxpu_dra_slices_mdev_pcie": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, C.c_char_p, vp, sz, vp, sz, vp,
+                                            vp, sz, C.POINTER(sz), vp, C.POINTER(sz)]),
+        "kxpu_dra_slices_vf_vgpu_pcie": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, C.c_char_p, vp, sz, vp, sz,
+                                               vp, vp, sz, C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_mdev_pf": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, vp, sz, vp, sz, vp, vp, sz,
                                           C.POINTER(sz), vp, C.POINTER(sz)]),
     }
@@ -943,6 +954,25 @@ class Kxpu:
                                          _ptr(group_off), _ptr(group_members) if len(group_members) else None,
                                          len(group_off) - 1, _ptr(root_port), _ptr(pcie_switch)))
 
+    def pcie_ports_mdev(self, recs, paths, group_off, group_members):
+        """kxpu_pcie_ports_mdev: pcie_tree_mdev's inputs; returns (root_port, pcie_switch), one function key per group
+        or PCIE_NO_KEY."""
+        recs, paths = np.ascontiguousarray(recs), np.ascontiguousarray(paths)
+        assert recs.dtype == MDEVREC_DTYPE and paths.dtype == PCIPATH_DTYPE and len(recs) == len(paths)
+        group_off = np.ascontiguousarray(group_off, dtype=np.uint32)
+        group_members = np.ascontiguousarray(group_members, dtype=np.uint32)
+        G = len(group_off) - 1
+        rp, sw = np.empty(max(G, 1), np.uint64), np.empty(max(G, 1), np.uint64)
+        self.pcie_ports_mdev_raw(recs, paths, group_off, group_members, rp, sw)
+        return rp[:G], sw[:G]
+
+    def pcie_ports_mdev_raw(self, recs, paths, group_off, group_members, root_port, pcie_switch):
+        """The bare call into caller buffers (timing loops, untouched-output checks); group_off is taken as given."""
+        n = len(recs)
+        self._chk(self.L.kxpu_pcie_ports_mdev(self.ctx, _ptr(recs) if n else None, _ptr(paths) if n else None, n,
+                                              _ptr(group_off), _ptr(group_members) if len(group_members) else None,
+                                              len(group_off) - 1, _ptr(root_port), _ptr(pcie_switch)))
+
     def pcie_tree_mdev(self, recs, paths, group_off, group_members):
         """kxpu_pcie_tree_mdev: recs (MDEVREC_DTYPE) and paths (PCIPATH_DTYPE, the entries' links) at the same indices,
         the group CSR of an mdev classify call.  Returns pcie_tree's dict."""
@@ -1111,6 +1141,55 @@ class Kxpu:
         def fn(ctx, d, p, nd, g, *rest):
             return self.L.kxpu_dra_slices_pcie(ctx, d, p, nd, g, dom, *rest)
         return self._slices(fn, DRADEVPCIE_DTYPE, driver, pool, node, generation, devs, taints=(taints, since))
+
+    def dra_slices_mdev_pcie(self, driver, pool, node, generation, attr_domain, devs, taints, since):
+        """kxpu_dra_slices_mdev_pcie: the same for a pool of mdev vGPUs with their parent's PF and PCIe ports
+        (DRAMDEVPCIE_DTYPE devices), the two port attributes qualified by attr_domain; since None gives the untainted
+        bytes."""
+        return self._slices(self._ports_fn(self.L.kxpu_dra_slices_mdev_pcie, attr_domain), DRAMDEVPCIE_DTYPE, driver,
+                            pool, node, generation, devs, taints=(taints, since))
+
+    def dra_slices_vf_vgpu_pcie(self, driver, pool, node, generation, attr_domain, devs, taints, since):
+        """kxpu_dra_slices_vf_vgpu_pcie: the same for a pool of vGPUs on VFs with their PCIe ports
+        (DRAVFVGPUPCIE_DTYPE devices)."""
+        return self._slices(self._ports_fn(self.L.kxpu_dra_slices_vf_vgpu_pcie, attr_domain), DRAVFVGPUPCIE_DTYPE, driver,
+                            pool, node, generation, devs, taints=(taints, since))
+
+    def dra_slices_mdev_pcie_raw(self, driver, pool, node, generation, attr_domain, devs, taints, since, out, length,
+                                 slice_off):
+        """The bare kxpu_dra_slices_mdev_pcie call into caller buffers (refusal checks): returns the status code, no
+        exception; length is a ctypes size_t, out / slice_off numpy arrays or None."""
+        return self._slices_raw(self.L.kxpu_dra_slices_mdev_pcie, DRAMDEVPCIE_DTYPE, driver, pool, node, generation,
+                                attr_domain, devs, taints, since, out, length, slice_off)
+
+    def dra_slices_vf_vgpu_pcie_raw(self, driver, pool, node, generation, attr_domain, devs, taints, since, out, length,
+                                    slice_off):
+        """The bare kxpu_dra_slices_vf_vgpu_pcie call, as dra_slices_mdev_pcie_raw."""
+        return self._slices_raw(self.L.kxpu_dra_slices_vf_vgpu_pcie, DRAVFVGPUPCIE_DTYPE, driver, pool, node, generation,
+                                attr_domain, devs, taints, since, out, length, slice_off)
+
+    @staticmethod
+    def _ports_fn(call, attr_domain):
+        """a slice call of the PCIe layouts with its attr_domain bound, in _slices' argument order"""
+        dom = _kind(attr_domain)
+
+        def fn(ctx, d, p, nd, g, *rest):
+            return call(ctx, d, p, nd, g, dom, *rest)
+        return fn
+
+    def _slices_raw(self, call, dtype, driver, pool, node, generation, attr_domain, devs, taints, since, out, length,
+                    slice_off):
+        devs = np.ascontiguousarray(devs)
+        assert devs.dtype == dtype
+        tab = (DraTaint * max(len(taints), 1))(*[DraTaint(_kind(k), _kind(v), _kind(e)) for k, v, e in taints])
+        if since is not None:
+            since = np.ascontiguousarray(since, dtype=np.int64)
+        ns = C.c_size_t(0)
+        return call(self.ctx, _kind(driver), _kind(pool), _kind(node), generation, _kind(attr_domain),
+                    _ptr(devs) if len(devs) else None, len(devs), C.cast(tab, C.c_void_p), len(taints),
+                    None if since is None else _ptr(since), None if out is None else _ptr(out),
+                    0 if out is None else len(out), C.byref(length), None if slice_off is None else _ptr(slice_off),
+                    C.byref(ns))
 
     def aer_health(self, text, file_off, file_len, fatal_limit, nonfatal_limit, group_off, group_members):
         """kxpu_aer_health: (totals, group_aer).  text: bytes; file_off / file_len: 2n entries, the fatal file of record i

@@ -608,6 +608,44 @@ constexpr int MAX_FRAG_DRA_PCIE = MAX_FRAG_DRA_PF + (int)sizeof("\"},\"/pcieRoot
 constexpr int DRAC_PARTS = DRAC_LITS + 2;
 // the pool grows by the three block literals and C1B: 256 bytes more than the other layouts'
 constexpr int DRAC_POOL_EXTRA = 256;
+// what the block adds to a fragment at most: R0 with the three closing bytes of the PCI layout's, R1, R2 and two
+// addresses
+constexpr int PCIE_BLOCK_MAX = MAX_FRAG_DRA_PCIE - MAX_FRAG_DRA_PF;
+
+// An mdev vGPU with its PCIe ports (kxpu_dra_slices_mdev_pcie): the mdev-PF fragment with the same block at one position
+// POS among its eleven keys (0: before iommuGroup .. 11: after uuid).  M1 is split as D1 is (C1A, then M1B: the
+// iommuGroup key) so that position 0 lies between literals; the other literals keep their mdev-PF indices, M1B, R0, R1
+// and R2 follow them.  Every value of this layout is closed by its own bytes, so the block needs no closer of the value
+// before it:
+//   POS 0         R0 = "<d>/pcieRootPort":{"string":"        R2 = "},    (the iommuGroup literal M1B follows)
+//   otherwise     R0 = ,"<d>/pcieRootPort":{"string":"       R2 = "}
+// and R1 as the PCI layout's.  A record with neither key gives the mdev-PF fragment's bytes.  LAYOUT_MDEV_PCIE is a
+// layout of k_dra_slices only.
+constexpr int LAYOUT_MDEV_PCIE = 10;
+// A vGPU on a VF with its PCIe ports (kxpu_dra_slices_vf_vgpu_pcie): the VF-vGPU fragment with the block built as the
+// mdev one's, at one position among its ten keys (0: before iommuGroup .. 10: after vgpuTypeID).  LAYOUT_VF_VGPU_PCIE is
+// a layout of k_dra_slices only.
+constexpr int LAYOUT_VF_VGPU_PCIE = 11;
+static_assert(LAYOUT_MDEV_PCIE != LAYOUT_PCI && LAYOUT_MDEV_PCIE != LAYOUT_MDEV && LAYOUT_MDEV_PCIE != LAYOUT_VF_VGPU &&
+                  LAYOUT_MDEV_PCIE != LAYOUT_MDEV_PF && LAYOUT_MDEV_PCIE != LAYOUT_PCI_PF &&
+                  LAYOUT_MDEV_PCIE != LAYOUT_PCI_PCIE && LAYOUT_VF_VGPU_PCIE != LAYOUT_PCI &&
+                  LAYOUT_VF_VGPU_PCIE != LAYOUT_MDEV && LAYOUT_VF_VGPU_PCIE != LAYOUT_VF_VGPU &&
+                  LAYOUT_VF_VGPU_PCIE != LAYOUT_MDEV_PF && LAYOUT_VF_VGPU_PCIE != LAYOUT_PCI_PF &&
+                  LAYOUT_VF_VGPU_PCIE != LAYOUT_PCI_PCIE,
+              "DRA layouts of their own");
+static_assert(sizeof(KX_C1A) - 1 + sizeof("\"iommuGroup\":{\"int\":") == sizeof(KX_M1) && sizeof(KX_M1) == sizeof(KX_V1),
+              "C1A opens M1 and V1 as it opens D1");
+constexpr int DRAMC_M1B = DRAMP_LITS, DRAMC_LITS = DRAMP_LITS + 4, DRAVC_V1B = DRAV_LITS, DRAVC_LITS = DRAV_LITS + 4;
+constexpr int MAX_FRAG_DRA_MDEV_PCIE = MAX_FRAG_DRA_MDEV_PF + PCIE_BLOCK_MAX;
+constexpr int MAX_FRAG_DRA_VF_VGPU_PCIE = MAX_FRAG_DRA_VF_VGPU + PCIE_BLOCK_MAX;
+constexpr int DRAMC_PARTS = DRAMC_LITS + 2, DRAVC_PARTS = DRAVC_LITS + 2;
+// the three layouts with the block; its literals follow the split literal's second half: R0 = that index + 1
+__host__ __device__ constexpr bool dra_pcie(int layout) {
+    return layout == LAYOUT_PCI_PCIE || layout == LAYOUT_MDEV_PCIE || layout == LAYOUT_VF_VGPU_PCIE;
+}
+__host__ __device__ constexpr int dra_pcie_r0(int layout) {
+    return layout == LAYOUT_PCI_PCIE ? DRAC_R0 : layout == LAYOUT_MDEV_PCIE ? DRAMC_M1B + 1 : DRAVC_V1B + 1;
+}
 
 // Taints (kxpu_dra_slices[_mdev]_taint[s]).  A device that carries some taint ends with its last literal less that
 // literal's final '}' (the one that closes the device), then KX_TAINTS_OPEN, for each carried taint in table order its
@@ -669,6 +707,8 @@ constexpr int DRAP_F_PHYSFN = DRA_F_COUNT, DRAP_F_PHYSFN_DEVICE = DRA_F_COUNT + 
 constexpr int DRAC_F_KEY = DRAP_F_COUNT, DRAC_F_ORPHAN = DRAP_F_COUNT + 1, DRAC_F_COUNT = DRAP_F_COUNT + 2;
 constexpr int DRAV_F_PRODUCT = 0, DRAV_F_KEY = 1, DRAV_F_BDF = 2, DRAV_F_PARENT = 3, DRAV_F_ROOT = 4, DRAV_F_VENDOR = 5,
               DRAV_F_DEVICE = 6, DRAV_F_GROUP = 7, DRAV_F_TYPE_ID = 8, DRAV_F_PLEN = 9, DRAV_F_COUNT = 10;
+// kxpu_dramdevpcie and kxpu_dravfvgpupcie: the flags of their first member's layout, then the PCIe layout's two
+constexpr int DRAMC_F_COUNT = DRAMP_F_COUNT + 2, DRAVC_F_COUNT = DRAV_F_COUNT + 2;
 
 // T devices per slice, FRAG bytes per fragment, a POOL-byte pool
 template <int T, int FRAG, int POOL>
@@ -718,6 +758,14 @@ template <int T, int FRAG, int POOL>
 struct DraPcieSmem : DraPfSmem<T, FRAG, POOL> {
     uint8_t klen[T];     // root port | switch << 3, each address length less 11 (12..16 -> 1..5), 0 = absent
 };
+template <int T, int FRAG, int POOL>
+struct DraMdevPcieSmem : DraMdevPfSmem<T, FRAG, POOL> {
+    uint8_t klen[T];     // as DraPcieSmem's
+};
+template <int T, int FRAG, int POOL>
+struct DraVfVgpuPcieSmem : DraVfVgpuSmem<T, FRAG, POOL> {
+    uint8_t klen[T];     // as DraPcieSmem's
+};
 template <typename Base, int NT>
 struct DraTaintsSmem : Base {
     uint8_t ts[TAINT_TILE][NT][20];  // timeAdded of taint t of device d
@@ -753,15 +801,31 @@ template <> struct DraLayout<LAYOUT_PCI_PCIE> {
     template <int T, int FRAG, int POOL> using Smem = DraPcieSmem<T, FRAG, POOL>;
     static constexpr int PARTS = DRAC_PARTS, LAST = 8, F_COUNT = DRAC_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_PCIE;
 };
-// the mdev record of either mdev layout, the PCI record of each PCI layout, the PF fields of the PCI-PF and PCIe ones
+template <> struct DraLayout<LAYOUT_MDEV_PCIE> {
+    using Rec = kxpu_dramdevpcie;
+    template <int T, int FRAG, int POOL> using Smem = DraMdevPcieSmem<T, FRAG, POOL>;
+    static constexpr int PARTS = DRAMC_PARTS, LAST = DRAM_E, F_COUNT = DRAMC_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_MDEV_PCIE;
+};
+template <> struct DraLayout<LAYOUT_VF_VGPU_PCIE> {
+    using Rec = kxpu_dravfvgpupcie;
+    template <int T, int FRAG, int POOL> using Smem = DraVfVgpuPcieSmem<T, FRAG, POOL>;
+    static constexpr int PARTS = DRAVC_PARTS, LAST = DRAV_E, F_COUNT = DRAVC_F_COUNT, MAX_FRAG = MAX_FRAG_DRA_VF_VGPU_PCIE;
+};
+// the mdev record of each mdev layout, the PCI record of each PCI layout, the PF fields of the PF and PCIe ones, the
+// VF-vGPU record of either VF-vGPU layout
 __device__ __forceinline__ const kxpu_dramdev *dram_of(const kxpu_dramdev *r) { return r; }
 __device__ __forceinline__ const kxpu_dramdev *dram_of(const kxpu_dramdevpf *r) { return &r->dev; }
+__device__ __forceinline__ const kxpu_dramdev *dram_of(const kxpu_dramdevpcie *r) { return &r->pf.dev; }
+__device__ __forceinline__ const kxpu_dramdevpf *drampf_of(const kxpu_dramdevpf *r) { return r; }
+__device__ __forceinline__ const kxpu_dramdevpf *drampf_of(const kxpu_dramdevpcie *r) { return &r->pf; }
+__device__ __forceinline__ const kxpu_dravfvgpu *drav_of(const kxpu_dravfvgpu *r) { return r; }
+__device__ __forceinline__ const kxpu_dravfvgpu *drav_of(const kxpu_dravfvgpupcie *r) { return &r->dev; }
 __device__ __forceinline__ const kxpu_dradev *dra_of(const kxpu_dradev *r) { return r; }
 __device__ __forceinline__ const kxpu_dradev *dra_of(const kxpu_dradevpf *r) { return &r->dev; }
 __device__ __forceinline__ const kxpu_dradev *dra_of(const kxpu_dradevpcie *r) { return &r->pf.dev; }
 __device__ __forceinline__ const kxpu_dradevpf *drapf_of(const kxpu_dradevpf *r) { return r; }
 __device__ __forceinline__ const kxpu_dradevpf *drapf_of(const kxpu_dradevpcie *r) { return &r->pf; }
-// the PCIe layout's kernel parameters: the other layouts' and the names' position among the nine keys
+// the PCIe layouts' kernel parameters: the other layouts' and the names' position among the layout's keys
 template <typename Base>
 struct DraPcieParams : Base {
     uint32_t pos;
@@ -775,15 +839,17 @@ template <int LAYOUT, int NT> struct DraKernel {
     static constexpr int PARTS = L::PARTS + (TAINT ? NT + 3 : 0);
     static constexpr int T_OPEN = L::PARTS - 2, T_ENTRY = T_OPEN + 1, T_ECLOSE = T_ENTRY + NT, T_CLOSE = T_ECLOSE + 1;
     static constexpr int F_SINCE = L::F_COUNT, F_DUP = F_SINCE + 1, F_COUNT = L::F_COUNT + (TAINT ? 2 : 0);
-    static constexpr int POOL = dra_pool_max(NT) + (LAYOUT == LAYOUT_PCI_PCIE ? DRAC_POOL_EXTRA : 0);
+    static constexpr int POOL = dra_pool_max(NT) + (dra_pcie(LAYOUT) ? DRAC_POOL_EXTRA : 0);
     static_assert(!TAINT || taints_pool_need(NT) <= dra_pool_max(NT) - DRA_POOL_MAX, "taint pool bound");
     static constexpr int MAXF = L::MAX_FRAG + (TAINT ? taints_part_max(NT) : 0);
     // CTAs per SM asked of ptxas, 0 for none.  Left to itself ptxas gives NT = 1 96 registers (PCI) or 101 (vGPU), so
     // two CTAs per SM, where its 47 / 56 KB of shared memory allow four; asked for three it takes 48, without spills
-    static constexpr int MIN_CTAS = NT == 1 ? 3 : 0;
+    // The four-entry VF-vGPU PCIe kernel, left to itself, takes 40 registers and spills; asked for one CTA per SM it
+    // keeps its values in registers
+    static constexpr int MIN_CTAS = NT == 1 ? 3 : LAYOUT == LAYOUT_VF_VGPU_PCIE && NT > 1 ? 1 : 0;
     using Base = typename L::template Smem<T, MAXF, POOL>;
     using BaseParams = std::conditional_t<TAINT, DraTaintsParams<PARTS, NT, POOL>, DraParams<PARTS, POOL>>;
-    using Params = std::conditional_t<LAYOUT == LAYOUT_PCI_PCIE, DraPcieParams<BaseParams>, BaseParams>;
+    using Params = std::conditional_t<dra_pcie(LAYOUT), DraPcieParams<BaseParams>, BaseParams>;
     using Smem = std::conditional_t<TAINT, DraTaintsSmem<Base, NT>, Base>;
 };
 // the VF-vGPU fragment bound: its widest instantiation still stages a whole slice in one CTA's shared memory, and its
@@ -800,6 +866,12 @@ static_assert(sizeof(DraKernel<LAYOUT_PCI_PF, KXPU_DRA_MAX_TAINTS>::Smem) <= 227
 static_assert(sizeof(DraKernel<LAYOUT_PCI_PCIE, KXPU_DRA_MAX_TAINTS>::Smem) <= 227 * 1024 &&
                   2 * (sizeof(DraKernel<LAYOUT_PCI_PCIE, 0>::Smem) + 1024) <= 228 * 1024,
               "MAX_FRAG_DRA_PCIE: the PCIe staging outgrew the shared memory");
+static_assert(sizeof(DraKernel<LAYOUT_MDEV_PCIE, KXPU_DRA_MAX_TAINTS>::Smem) <= 227 * 1024 &&
+                  2 * (sizeof(DraKernel<LAYOUT_MDEV_PCIE, 0>::Smem) + 1024) <= 228 * 1024,
+              "MAX_FRAG_DRA_MDEV_PCIE: the mdev PCIe staging outgrew the shared memory");
+static_assert(sizeof(DraKernel<LAYOUT_VF_VGPU_PCIE, KXPU_DRA_MAX_TAINTS>::Smem) <= 227 * 1024 &&
+                  2 * (sizeof(DraKernel<LAYOUT_VF_VGPU_PCIE, 0>::Smem) + 1024) <= 228 * 1024,
+              "MAX_FRAG_DRA_VF_VGPU_PCIE: the VF-vGPU PCIe staging outgrew the shared memory");
 
 // a function key's sysfs address (include/kxpu.h, kxpu_dra_slices_pcie): the domain's digit count (4, or 5..8 without a
 // leading zero above ffff) and byte l of "<domain>:<bus>:<dev>.<fn>"; the domain is bounded to 32 bits, so a key outside
@@ -820,6 +892,22 @@ __device__ __forceinline__ uint8_t key_addr_byte(unsigned long long k, uint32_t 
     case 6: return (uint8_t)'.';
     default: return hx((uint32_t)k & 7u);
     }
+}
+
+// the vGPU PCIe layouts: a device's two keys (q: the root port in .xy, the switch in .zw) checked into the layout's last
+// two flags, their address lengths into *klen (DraPcieSmem's form) and what the block adds to the device's fragment: the
+// PCI layout's statements, which that layout keeps inline so that its kernels stay as they were compiled (the copy in
+// k_dra_slices' LAYOUT_PCI_PCIE length step: change both together)
+template <int LAYOUT, typename P>
+__device__ __forceinline__ uint32_t ports_len(const P &E, const uint4 q, uint8_t *klen) {
+    constexpr int F_KEY = DraLayout<LAYOUT>::F_COUNT - 2, R0 = dra_pcie_r0(LAYOUT);
+    const unsigned long long rp = ((unsigned long long)q.y << 32) | q.x, sw = ((unsigned long long)q.w << 32) | q.z;
+    const bool hr = rp != KXPU_PCIE_NO_KEY, hs = sw != KXPU_PCIE_NO_KEY;
+    if ((hr && (rp >> 48)) || (hs && (sw >> 48))) E.flags[F_KEY] = 1u;
+    if (hs && !hr) E.flags[F_KEY + 1] = 1u;
+    const uint32_t kl = hr ? key_dom_digits(rp) + 8u : 0u, sl = hs ? key_dom_digits(sw) + 8u : 0u;
+    *klen = (uint8_t)((kl ? kl - 11u : 0u) | (sl ? sl - 11u : 0u) << 3);
+    return (kl ? E.len[R0] + kl + E.len[R0 + 2] : 0u) + (sl ? E.len[R0 + 1] + sl : 0u);
 }
 
 template <int W>
@@ -927,7 +1015,9 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             S.xlen[tid] = (uint8_t)(xl | yl << 5);
             flen += (xl ? E.len[DRAP_Q0] + xl : 0u) + (yl ? E.len[DRAP_Q1] + yl : 0u);
         }
-        if constexpr (LAYOUT == LAYOUT_PCI_PCIE) {  // root_port and pcie_switch: bytes 160..176 (q10)
+        // root_port and pcie_switch: bytes 160..176 (q10).  The same statements as ports_len, which the vGPU PCIe layouts
+        // call; kept inline here so that this layout's kernels compile as before.  Change both together.
+        if constexpr (LAYOUT == LAYOUT_PCI_PCIE) {
             const uint4 q10 = p[10];
             const unsigned long long rp = ((unsigned long long)q10.y << 32) | q10.x, sw = ((unsigned long long)q10.w << 32) | q10.z;
             const bool hr = rp != KXPU_PCIE_NO_KEY, hs = sw != KXPU_PCIE_NO_KEY;
@@ -938,9 +1028,9 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             flen += (kl ? E.len[DRAC_R0] + kl + E.len[DRAC_R2] : 0u) + (sl ? E.len[DRAC_R1] + sl : 0u);
         }
     }
-    if constexpr (LAYOUT == LAYOUT_MDEV || LAYOUT == LAYOUT_MDEV_PF) {
+    if constexpr (LAYOUT == LAYOUT_MDEV || LAYOUT == LAYOUT_MDEV_PF || LAYOUT == LAYOUT_MDEV_PCIE) {
         if (tid < in_slice) {
-            // 208 bytes = 13 uint4 (kxpu_dramdevpf: its dev); read field by field so that no more than a few of them are
+            // 208 bytes = 13 uint4 (kxpu_dramdevpf, kxpu_dramdevpcie: its dev); read field by field so that no more than a few of them are
             // live at once
             const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const Rec *>(E.devs) + i0 + tid);
             uint32_t pl, tl, bl, rl, vl, dl;
@@ -1002,7 +1092,7 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             flen = E.len[0] + E.len[1] + 2u * gl + li + E.len[2] + tl + ls + E.len[4] + bl + ls + E.len[6] + vl + ls +
                    E.len[9] + 36u + ls + E.len[DRAM_E] + (nl ? E.len[3] + nl + li : 0u) + (dl ? E.len[5] + dl + ls : 0u) +
                    (pl ? E.len[7] + pl + ls : 0u) + (rl ? E.len[8] + rl + ls : 0u) + (tid + 1u < in_slice ? 1u : 0u);
-            if constexpr (LAYOUT == LAYOUT_MDEV_PF) {  // physfn and physfn_device: bytes 208..232 (q13, q14.xy)
+            if constexpr (LAYOUT == LAYOUT_MDEV_PF || LAYOUT == LAYOUT_MDEV_PCIE) {  // physfn and physfn_device: bytes 208..232 (q13, q14.xy)
                 const uint4 q13 = p[13];
                 const uint2 q14 = reinterpret_cast<const uint2 *>(p + 14)[0];
                 const uint32_t pf[4] = {q13.x, q13.y, q13.z, q13.w}, pd[2] = {q14.x, q14.y};
@@ -1014,11 +1104,13 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
                 S.xlen[tid] = (uint8_t)(xl | yl << 5);
                 flen += (xl ? E.len[DRAMP_P0] + xl + ls : 0u) + (yl ? E.len[DRAMP_P1] + yl + ls : 0u);
             }
+            if constexpr (LAYOUT == LAYOUT_MDEV_PCIE)  // M1's second half, then the keys: bytes 240..256 (q15)
+                flen += E.len[DRAMC_M1B] + ports_len<LAYOUT>(E, p[15], &S.klen[tid]);
         }
     }
-    if constexpr (LAYOUT == LAYOUT_VF_VGPU) {
+    if constexpr (LAYOUT == LAYOUT_VF_VGPU || LAYOUT == LAYOUT_VF_VGPU_PCIE) {
         if (tid < in_slice) {
-            // 192 bytes = 12 uint4; read field by field, as the mdev layout does, so that few of them are live at once
+            // 192 bytes = 12 uint4 (kxpu_dravfvgpupcie: its dev); read field by field, as the mdev layout does, so that few of them are live at once
             const uint4 *p = reinterpret_cast<const uint4 *>(static_cast<const Rec *>(E.devs) + i0 + tid);
             uint32_t pl, tl, xl, bl, rl, vl, dl;
             {  // product_len and product (q11, q0..q3)
@@ -1083,6 +1175,8 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
                    E.len[9] + tl + ls + E.len[10] + il + li + E.len[DRAV_E] + (nl ? E.len[2] + nl + li : 0u) +
                    (dl ? E.len[4] + dl + ls : 0u) + (pl ? E.len[7] + pl + ls : 0u) + (rl ? E.len[8] + rl + ls : 0u) +
                    (tid + 1u < in_slice ? 1u : 0u);
+            if constexpr (LAYOUT == LAYOUT_VF_VGPU_PCIE)  // V1's second half, then the keys: bytes 192..208 (q12)
+                flen += E.len[DRAVC_V1B] + ports_len<LAYOUT>(E, p[12], &S.klen[tid]);
         }
     }
     if constexpr (K::TAINT) {  // the device's row of the table: which taints it carries, and their times
@@ -1165,6 +1259,28 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             lit(k);
         };
         const auto bytes = [](const char *s) { return reinterpret_cast<const uint8_t *>(s); };
+        // the vGPU PCIe layouts: the block of the two attributes when the names sit at position at: R0, the root port's
+        // address, [R1, the switch's address,] R2, as the LAYOUT_PCI_PCIE branch below writes it with its own copy of
+        // these lambdas (change both together); nothing in the other layouts
+        uint32_t kl = 0, sl = 0;  // the two address lengths, 0 = absent: set by each vGPU PCIe branch from S.klen[d]
+        const auto port_lens = [&](uint32_t kk) {
+            kl = kk & 7u ? (kk & 7u) + 11u : 0u;
+            sl = kk >> 3 ? (kk >> 3) + 11u : 0u;
+        };
+        const auto ports = [&](uint32_t at) {
+            if constexpr (LAYOUT == LAYOUT_MDEV_PCIE || LAYOUT == LAYOUT_VF_VGPU_PCIE) {
+                constexpr int R0 = dra_pcie_r0(LAYOUT);
+                const auto addr = [&](unsigned long long key, uint32_t L) {
+                    const uint32_t dd = L - 8u;
+                    for (uint32_t l = lane; l < L; l += 32u) dst[o + l] = key_addr_byte(key, dd, l);
+                    o += L;
+                };
+                if (E.pos != at || !kl) return;
+                lit(R0); addr(r->root_port, kl);
+                if (sl) { lit(R0 + 1); addr(r->pcie_switch, sl); }
+                lit(R0 + 2);
+            }
+        };
         if constexpr (LAYOUT == LAYOUT_PCI || LAYOUT == LAYOUT_PCI_PF) {
             const kxpu_dradev *q = dra_of(r);
             lit(0); put(S.dec[d], gl); lit(1); put(bytes(q->device), dl);
@@ -1189,7 +1305,8 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
                 for (uint32_t l = lane; l < L; l += 32u) dst[o + l] = key_addr_byte(key, dd, l);
                 o += L;
             };
-            // the two attributes when the names sit at position at
+            // the two attributes when the names sit at position at.  The same lambdas as the vGPU PCIe layouts' `ports`
+            // above the branches; kept here so that this layout's kernels compile as before.  Change both together.
             const auto ports = [&](uint32_t at) {
                 if (E.pos != at || !kl) return;
                 lit(DRAC_R0); addr(r->root_port, kl);
@@ -1210,35 +1327,53 @@ __global__ void __launch_bounds__(EMIT_THREADS, DraKernel<LAYOUT, NT>::MIN_CTAS)
             if (rl) { lit(6); put(bytes(q->pcie_root), rl); }
             ports(8u);
             lit(7); put(bytes(q->vendor), vl); ports(9u); close(DraLayout<LAYOUT>::LAST);
-        } else if constexpr (LAYOUT == LAYOUT_VF_VGPU) {
+        } else if constexpr (LAYOUT == LAYOUT_VF_VGPU || LAYOUT == LAYOUT_VF_VGPU_PCIE) {
+            // ports(k): the block before key k of the ten (10: after the last); V1's second half follows position 0
+            const kxpu_dravfvgpu *v = drav_of(r);
             const uint32_t m2 = S.meta2[d], tl = m2 & 63u, xl = (m2 >> 6) & 31u, il = m2 >> 11;
-            lit(0); put(S.dec[d], gl); lit(1); put(S.dec[d], gl); lit(DRAV_I);
+            lit(0); put(S.dec[d], gl); lit(1);
+            if constexpr (LAYOUT == LAYOUT_VF_VGPU_PCIE) { port_lens(S.klen[d]); ports(0u); lit(DRAVC_V1B); }
+            put(S.dec[d], gl); lit(DRAV_I); ports(1u);
             if (nl) { lit(2); put(S.dec[d] + 10, nl); lit(DRAV_I); }
-            lit(3); put(bytes(r->parent), bl); lit(DRAV_S);
-            if (dl) { lit(4); put(bytes(r->device), dl); lit(DRAV_S); }
-            lit(5); put(bytes(r->vendor), vl); lit(DRAV_S);
-            lit(6); put(bytes(r->bdf), xl); lit(DRAV_S);
-            if (pl) { lit(7); put(r->product, pl); lit(DRAV_S); }
-            if (rl) { lit(8); put(bytes(r->pcie_root), rl); lit(DRAV_S); }
-            lit(9); put(bytes(r->type_key), tl); lit(DRAV_S);
-            lit(10); put(S.dec[d] + 12, il); lit(DRAV_I); close(DraLayout<LAYOUT>::LAST);
+            ports(2u);
+            lit(3); put(bytes(v->parent), bl); lit(DRAV_S); ports(3u);
+            if (dl) { lit(4); put(bytes(v->device), dl); lit(DRAV_S); }
+            ports(4u);
+            lit(5); put(bytes(v->vendor), vl); lit(DRAV_S); ports(5u);
+            lit(6); put(bytes(v->bdf), xl); lit(DRAV_S); ports(6u);
+            if (pl) { lit(7); put(v->product, pl); lit(DRAV_S); }
+            ports(7u);
+            if (rl) { lit(8); put(bytes(v->pcie_root), rl); lit(DRAV_S); }
+            ports(8u);
+            lit(9); put(bytes(v->type_key), tl); lit(DRAV_S); ports(9u);
+            lit(10); put(S.dec[d] + 12, il); lit(DRAV_I); ports(10u); close(DraLayout<LAYOUT>::LAST);
         } else {
+            // ports(k): the block before key k of the eleven (11: after the last); M1's second half follows position 0
             const kxpu_dramdev *m = dram_of(r);
             const uint32_t tl = S.tlen[d];
-            lit(0); put(S.dec[d], gl); lit(1); put(S.dec[d], gl); lit(DRAM_I);
-            lit(2); put(bytes(m->mdev_type), tl); lit(DRAM_S);
+            lit(0); put(S.dec[d], gl); lit(1);
+            if constexpr (LAYOUT == LAYOUT_MDEV_PCIE) { port_lens(S.klen[d]); ports(0u); lit(DRAMC_M1B); }
+            put(S.dec[d], gl); lit(DRAM_I); ports(1u);
+            lit(2); put(bytes(m->mdev_type), tl); lit(DRAM_S); ports(2u);
             if (nl) { lit(3); put(S.dec[d] + 10, nl); lit(DRAM_I); }
-            lit(4); put(bytes(m->parent), bl); lit(DRAM_S);
+            ports(3u);
+            lit(4); put(bytes(m->parent), bl); lit(DRAM_S); ports(4u);
             if (dl) { lit(5); put(bytes(m->device), dl); lit(DRAM_S); }
-            lit(6); put(bytes(m->vendor), vl); lit(DRAM_S);
-            if constexpr (LAYOUT == LAYOUT_MDEV_PF) {
+            ports(5u);
+            lit(6); put(bytes(m->vendor), vl); lit(DRAM_S); ports(6u);
+            if constexpr (LAYOUT == LAYOUT_MDEV_PF || LAYOUT == LAYOUT_MDEV_PCIE) {
+                const kxpu_dramdevpf *f = drampf_of(r);
                 const uint32_t x = S.xlen[d], xl = x & 31u, yl = x >> 5;
-                if (xl) { lit(DRAMP_P0); put(bytes(r->physfn), xl); lit(DRAM_S); }
-                if (yl) { lit(DRAMP_P1); put(bytes(r->physfn_device), yl); lit(DRAM_S); }
+                if (xl) { lit(DRAMP_P0); put(bytes(f->physfn), xl); lit(DRAM_S); }
+                ports(7u);
+                if (yl) { lit(DRAMP_P1); put(bytes(f->physfn_device), yl); lit(DRAM_S); }
             }
+            ports(8u);
             if (pl) { lit(7); put(m->product, pl); lit(DRAM_S); }
+            ports(9u);
             if (rl) { lit(8); put(bytes(m->pcie_root), rl); lit(DRAM_S); }
-            lit(9); put(bytes(m->uuid), 36u); lit(DRAM_S); close(DraLayout<LAYOUT>::LAST);
+            ports(10u);
+            lit(9); put(bytes(m->uuid), 36u); lit(DRAM_S); ports(11u); close(DraLayout<LAYOUT>::LAST);
         }
         if (d + 1u < in_slice && lane == 0) dst[o] = (uint8_t)',';
     }
@@ -1849,9 +1984,30 @@ struct DraTaint {
     const int64_t *since;  // [devices * n]
 };
 
+// The literals of a PCIe layout: the layout's own lits[0 .. n_lits) with literal 1 cut after KX_C1A (its second half
+// appended), then the block literals R0 / R1 / R2 for the names' position: the count of the layout's n_keys sorted keys
+// that sort before "<attr_domain>/pcieRootPort", returned.  closed: every value of the layout is closed by its own
+// bytes (the mdev and VF-vGPU layouts); else the literal after a value closes it (the PCI layouts), with an int before
+// the positions in int_before (bit pos).
+static uint32_t pcie_block_lits(const char *attr_domain, const char *const *keys, int n_keys, const char *const *lits,
+                                int n_lits, bool closed, uint32_t int_before, std::vector<std::string> &out) {
+    const std::string rk = std::string(attr_domain) + "/pcieRootPort", sk = std::string(attr_domain) + "/pcieSwitch";
+    uint32_t pos = 0;
+    while ((int)pos < n_keys && strcmp(keys[pos], rk.c_str()) < 0) pos++;
+    const bool after_int = (int_before >> pos) & 1u;
+    const std::string open = pos == 0 ? std::string() : closed ? "," : (after_int ? "}" : "\"}") + std::string(",");
+    out.assign(lits, lits + n_lits);
+    out[1] = KX_C1A;
+    out.push_back(std::string(lits[1]).substr(sizeof(KX_C1A) - 1));
+    out.push_back(open + "\"" + rk + "\":{\"string\":\"");
+    out.push_back("\"},\"" + sk + "\":{\"string\":\"");
+    out.push_back(pos == 0 ? "\"}," : closed ? "\"}" : after_int ? "\"" : "");
+    return pos;
+}
+
 // kxpu_dra_slices[_mdev][_taint[s]]: the argument checks, the pool (literals | taint parts | head | tail), one
 // k_dra_slices<LAYOUT, NT> launch, the domain flags and the copies
-// attr_domain: the PCIe layout's attribute domain (checked by its entry point), else unread
+// attr_domain: the PCIe layouts' attribute domain (checked by their entry points), else unread
 template <int LAYOUT, int NT = 0>
 static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, const char *pool, const char *node,
                           uint64_t generation, const typename DraLayout<LAYOUT>::Rec *devs, size_t n, uint8_t *out, size_t cap,
@@ -1862,11 +2018,12 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     constexpr bool TAINT = K::TAINT;
     constexpr int PARTS = K::PARTS, HEAD = PARTS - 2, TAIL = PARTS - 1;
     constexpr int LITS = LAYOUT == LAYOUT_PCI ? 9 : LAYOUT == LAYOUT_MDEV ? DRAM_LITS : LAYOUT == LAYOUT_MDEV_PF ? DRAMP_LITS
-                         : LAYOUT == LAYOUT_PCI_PF ? DRAP_LITS : LAYOUT == LAYOUT_PCI_PCIE ? DRAC_LITS : DRAV_LITS;
+                         : LAYOUT == LAYOUT_PCI_PF ? DRAP_LITS : LAYOUT == LAYOUT_PCI_PCIE ? DRAC_LITS
+                         : LAYOUT == LAYOUT_MDEV_PCIE ? DRAMC_LITS : LAYOUT == LAYOUT_VF_VGPU_PCIE ? DRAVC_LITS : DRAV_LITS;
     constexpr int MAXF = K::MAXF;
     constexpr int F_COUNT = K::F_COUNT;
     const char *const *lits = LAYOUT == LAYOUT_PCI ? h_dra_lits : LAYOUT == LAYOUT_MDEV ? h_dram_lits
-                              : LAYOUT == LAYOUT_MDEV_PF ? h_dramp_lits
+                              : LAYOUT == LAYOUT_MDEV_PF || LAYOUT == LAYOUT_MDEV_PCIE ? h_dramp_lits
                               : LAYOUT == LAYOUT_PCI_PF || LAYOUT == LAYOUT_PCI_PCIE ? h_drap_lits : h_drav_lits;
     if (!ctx || !len || !n_slices || (n && !devs)) return KXPU_E_INVALID;
     if (!dns_subdomain_ok(driver, 63) || !dns_subdomain_ok(pool, 253) || !dns_subdomain_ok(node, 253) ||
@@ -1911,28 +2068,27 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
     }
     typename K::Params E;
     memset(&E, 0, sizeof E);
-    // the PCIe layout: D1 split in C1A / C1B, and the block literals R0 / R1 / R2 for the names' position (the count of
-    // the nine keys that sort before "<attr_domain>/pcieRootPort")
+    // the PCIe layouts: literal 1 split before its first key, and the block literals for the names' position among the
+    // layout's keys (the PCI layout's numaNode and iommuGroup values are ints, closed by the literal after them)
     std::vector<std::string> pcie_lits;
     if constexpr (LAYOUT == LAYOUT_PCI_PCIE) {
         static const char *const nine[9] = {"deviceID", "iommuGroup", "numaNode", "pciAddress", "physfnAddress",
                                             "physfnDeviceID", "productName", "resource.kubernetes.io/pcieRoot", "vendorID"};
-        const std::string rk = std::string(attr_domain) + "/pcieRootPort", sk = std::string(attr_domain) + "/pcieSwitch";
-        uint32_t pos = 0;
-        while (pos < 9 && strcmp(nine[pos], rk.c_str()) < 0) pos++;
-        E.pos = pos;
-        const std::string after_int = "}", after_str = "\"}";
-        const std::string open = pos == 0 ? std::string() : (pos == 2 || pos == 3 ? after_int : after_str) + ",";
-        pcie_lits.assign(h_drap_lits, h_drap_lits + DRAP_LITS);
-        pcie_lits[1] = KX_C1A;
-        pcie_lits.push_back(KX_C1B);
-        pcie_lits.push_back(open + "\"" + rk + "\":{\"string\":\"");
-        pcie_lits.push_back("\"},\"" + sk + "\":{\"string\":\"");
-        pcie_lits.push_back(pos == 0 ? "\"}," : pos == 2 || pos == 3 ? "\"" : "");
+        E.pos = pcie_block_lits(attr_domain, nine, 9, h_drap_lits, DRAP_LITS, false, 1u << 2 | 1u << 3, pcie_lits);
+    } else if constexpr (LAYOUT == LAYOUT_MDEV_PCIE) {
+        static const char *const eleven[11] = {"iommuGroup", "mdevType", "numaNode", "parentAddress", "parentDeviceID",
+                                               "parentVendorID", "physfnAddress", "physfnDeviceID", "productName",
+                                               "resource.kubernetes.io/pcieRoot", "uuid"};
+        E.pos = pcie_block_lits(attr_domain, eleven, 11, h_dramp_lits, DRAMP_LITS, true, 0u, pcie_lits);
+    } else if constexpr (LAYOUT == LAYOUT_VF_VGPU_PCIE) {
+        static const char *const ten[10] = {"iommuGroup", "numaNode", "parentAddress", "parentDeviceID", "parentVendorID",
+                                            "pciAddress", "productName", "resource.kubernetes.io/pcieRoot", "vgpuType",
+                                            "vgpuTypeID"};
+        E.pos = pcie_block_lits(attr_domain, ten, 10, h_drav_lits, DRAV_LITS, true, 0u, pcie_lits);
     }
     uint32_t acc = 0;
     for (int k = 0; k < PARTS; k++) {
-        const std::string s = k < LITS ? (LAYOUT == LAYOUT_PCI_PCIE ? pcie_lits[k] : std::string(lits[k]))
+        const std::string s = k < LITS ? (dra_pcie(LAYOUT) ? pcie_lits[k] : std::string(lits[k]))
                               : k == HEAD ? head : k == TAIL ? std::string(KX_DRA_TAIL) : taint_parts[k - LITS];
         if (acc + s.size() > (size_t)K::POOL) return KXPU_E_INVALID;  // the literals grew: the pool bound must follow
         memcpy(E.pool + acc, s.data(), s.size());
@@ -2017,9 +2173,26 @@ static int32_t dra_slices(kxpu_ctx *ctx, const char *what, const char *driver, c
         "a physfn_device that is not 0..6 bytes of [0-9a-f], or is set without a physfn",
         "a root_port or pcie_switch that is a host-bridge key or has a bit of 48..62 set",
         "a pcie_switch without a root_port"};
+    static const char *const why_mdev_pcie[DRAMC_F_COUNT] = {
+        "a product byte outside [A-Za-z0-9_.-]", "an mdev_type that is empty or holds a byte outside [A-Za-z0-9_.-]",
+        "a uuid outside the canonical lowercase 8-4-4-4-12 form", "a parent that is empty or holds a byte outside [0-9a-f:.]",
+        "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
+        "a device id that is not 0..6 bytes of [0-9a-f]", "iommu_group 4294967295", "product_len above 64",
+        "a physfn that holds a byte outside [0-9a-f:.]",
+        "a physfn_device that is not 0..6 bytes of [0-9a-f], or is set without a physfn",
+        "a root_port or pcie_switch that is a host-bridge key or has a bit of 48..62 set",
+        "a pcie_switch without a root_port"};
+    static const char *const why_vf_vgpu_pcie[DRAVC_F_COUNT] = {
+        "a product byte outside [A-Za-z0-9_.-]", "a type_key that is empty or holds a byte outside [A-Za-z0-9_.-]",
+        "a bdf that is empty or holds a byte outside [0-9a-f:.]", "a parent that is empty or holds a byte outside [0-9a-f:.]",
+        "a pcie_root that is not \"pci\" followed by [0-9a-f:]", "a vendor id that is not 1..6 bytes of [0-9a-f]",
+        "a device id that is not 0..6 bytes of [0-9a-f]", "iommu_group 4294967295", "type_id 0", "product_len above 64",
+        "a root_port or pcie_switch that is a host-bridge key or has a bit of 48..62 set",
+        "a pcie_switch without a root_port"};
     const char *const *why = LAYOUT == LAYOUT_PCI ? why_pci : LAYOUT == LAYOUT_MDEV ? why_mdev
                              : LAYOUT == LAYOUT_MDEV_PF ? why_mdev_pf : LAYOUT == LAYOUT_PCI_PF ? why_pci_pf
-                             : LAYOUT == LAYOUT_PCI_PCIE ? why_pci_pcie : why_vf_vgpu;
+                             : LAYOUT == LAYOUT_PCI_PCIE ? why_pci_pcie : LAYOUT == LAYOUT_MDEV_PCIE ? why_mdev_pcie
+                             : LAYOUT == LAYOUT_VF_VGPU_PCIE ? why_vf_vgpu_pcie : why_vf_vgpu;
     const uint32_t *flags = reinterpret_cast<const uint32_t *>(h.data() + slices + 1);
     for (int f = 0; f < F_COUNT; f++)
         if (flags[f]) {
@@ -2169,7 +2342,23 @@ static bool attr_domain_ok(const char *d) {
     return true;
 }
 
-// the one entry point of the PCIe layout: the taint-list form, taint_since == NULL giving the untainted bytes
+// the entry point of each PCIe layout: the attribute domain's check, then the taint-list form, taint_since == NULL giving
+// the untainted bytes
+template <int LAYOUT>
+static int32_t dra_slices_ports(kxpu_ctx *ctx, const char *what, const char *driver, const char *pool, const char *node,
+                                uint64_t generation, const char *attr_domain, const typename DraLayout<LAYOUT>::Rec *devs,
+                                size_t n, const kxpu_dra_taint *taints, size_t n_taints, const int64_t *taint_since,
+                                uint8_t *out, size_t cap, size_t *len, uint64_t *slice_off, size_t *n_slices) {
+    if (!ctx) return KXPU_E_INVALID;
+    if (!attr_domain_ok(attr_domain)) {
+        KX_SET_ERR(ctx, "%s: attr_domain must be a lowercase DNS subdomain of at most 63 bytes outside kubernetes.io and "
+                        "k8s.io", what);
+        return KXPU_E_INVALID;
+    }
+    return dra_slices_tainted<LAYOUT>(ctx, what, driver, pool, node, generation, devs, n, taints, n_taints, taint_since,
+                                      out, cap, len, slice_off, n_slices, attr_domain);
+}
+
 extern "C" int32_t kxpu_dra_slices_pcie(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
                                         uint64_t generation, const char *attr_domain, const kxpu_dradevpcie *devs, size_t n,
                                         const kxpu_dra_taint *taints, size_t n_taints, const int64_t *taint_since,
@@ -2177,12 +2366,31 @@ extern "C" int32_t kxpu_dra_slices_pcie(kxpu_ctx *ctx, const char *driver, const
     static_assert(sizeof(kxpu_dradevpcie) == 176 && alignof(kxpu_dradevpcie) == 8 &&
                       offsetof(kxpu_dradevpcie, root_port) == 160 && offsetof(kxpu_dradevpcie, pcie_switch) == 168,
                   "kxpu_dradevpcie layout");
-    if (!ctx) return KXPU_E_INVALID;
-    if (!attr_domain_ok(attr_domain)) {
-        KX_SET_ERR(ctx, "dra_slices_pcie: attr_domain must be a lowercase DNS subdomain of at most 63 bytes outside "
-                        "kubernetes.io and k8s.io");
-        return KXPU_E_INVALID;
-    }
-    return dra_slices_tainted<LAYOUT_PCI_PCIE>(ctx, "dra_slices_pcie", driver, pool, node, generation, devs, n, taints,
-                                               n_taints, taint_since, out, cap, len, slice_off, n_slices, attr_domain);
+    return dra_slices_ports<LAYOUT_PCI_PCIE>(ctx, "dra_slices_pcie", driver, pool, node, generation, attr_domain, devs, n,
+                                             taints, n_taints, taint_since, out, cap, len, slice_off, n_slices);
+}
+
+extern "C" int32_t kxpu_dra_slices_mdev_pcie(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                             uint64_t generation, const char *attr_domain, const kxpu_dramdevpcie *devs,
+                                             size_t n, const kxpu_dra_taint *taints, size_t n_taints,
+                                             const int64_t *taint_since, uint8_t *out, size_t cap, size_t *len,
+                                             uint64_t *slice_off, size_t *n_slices) {
+    static_assert(sizeof(kxpu_dramdevpcie) == 256 && alignof(kxpu_dramdevpcie) == 8 &&
+                      offsetof(kxpu_dramdevpcie, root_port) == 240 && offsetof(kxpu_dramdevpcie, pcie_switch) == 248,
+                  "kxpu_dramdevpcie layout");
+    return dra_slices_ports<LAYOUT_MDEV_PCIE>(ctx, "dra_slices_mdev_pcie", driver, pool, node, generation, attr_domain, devs,
+                                              n, taints, n_taints, taint_since, out, cap, len, slice_off, n_slices);
+}
+
+extern "C" int32_t kxpu_dra_slices_vf_vgpu_pcie(kxpu_ctx *ctx, const char *driver, const char *pool, const char *node,
+                                                uint64_t generation, const char *attr_domain, const kxpu_dravfvgpupcie *devs,
+                                                size_t n, const kxpu_dra_taint *taints, size_t n_taints,
+                                                const int64_t *taint_since, uint8_t *out, size_t cap, size_t *len,
+                                                uint64_t *slice_off, size_t *n_slices) {
+    static_assert(sizeof(kxpu_dravfvgpupcie) == 208 && alignof(kxpu_dravfvgpupcie) == 8 &&
+                      offsetof(kxpu_dravfvgpupcie, root_port) == 192 && offsetof(kxpu_dravfvgpupcie, pcie_switch) == 200,
+                  "kxpu_dravfvgpupcie layout");
+    return dra_slices_ports<LAYOUT_VF_VGPU_PCIE>(ctx, "dra_slices_vf_vgpu_pcie", driver, pool, node, generation,
+                                                 attr_domain, devs, n, taints, n_taints, taint_since, out, cap, len,
+                                                 slice_off, n_slices);
 }

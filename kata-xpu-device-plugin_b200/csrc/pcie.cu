@@ -18,7 +18,9 @@
 // kxpu_pcie_tree's kernels.  kxpu_pcie_tree_mdev runs k_parse<kxpu_mdevrec, false>, whose leaf is the record's UUID
 // below its parent function (lanes 8..11 stage the record's UUID and parent next to the path), and kxpu_pcie_tree's
 // other kernels.  kxpu_pcie_ports runs kxpu_pcie_tree's parse, then k_ports: the LCP pass (group_lcp<false>, shared
-// with k_lcp) writing each group's root port and switch instead of its prefix.
+// with k_lcp) writing each group's root port and switch instead of its prefix.  kxpu_pcie_ports_mdev runs
+// k_parse<kxpu_mdevrec, false>, then k_ports_mdev: the same pass over each member's chain one key short (its parent
+// chain).
 #include <algorithm>
 #include <type_traits>
 
@@ -179,14 +181,17 @@ struct Tree {
 };
 
 // the longest common prefix of group g's member chains into k[0 .. return value); *bad: a member index >= n.  SR: a
-// member whose PF has a known chain shorter than MAXD reads the PF's chain followed by the PF's own key
-template <bool SR>
+// member whose PF has a known chain shorter than MAXD reads the PF's chain followed by the PF's own key.  PARENT
+// (kxpu_pcie_ports_mdev): a member reads its known chain less its last key, the parent function
+template <bool SR, bool PARENT = false>
 __device__ __forceinline__ int group_lcp(const Tree &T, uint32_t g, unsigned long long (&k)[MAXD], bool &bad) {
+    static_assert(!(SR && PARENT), "the parent chain is read from mdev chains");
     int L = -1;
     for (uint32_t m = T.goff[g]; m < T.goff[g + 1]; m++) {
         const uint32_t i = T.gmem[m];
         if (i >= T.n) { bad = true; continue; }
         int l = T.clen[i];
+        if constexpr (PARENT) l = max(l - 1, 0);  // a known mdev chain has 2..MAXD keys
         const unsigned long long *c = T.chain + (size_t)i * MAXD;
         unsigned long long tail = 0;  // SR, through the PF (via): the key at position l - 1
         bool via = false;
@@ -228,15 +233,17 @@ __global__ void __launch_bounds__(256) k_lcp(const Tree T) {
     T.glen[g] = (uint8_t)L;
 }
 
-// kxpu_pcie_ports: the LCP pass of kxpu_pcie_tree (plain chains), then the rule of include/kxpu.h on the prefix: the
-// functions after its last host bridge are f0, f1, ...; the root port is f0, the switch f_j for the greatest odd j
-__global__ void __launch_bounds__(256) k_ports(const Tree T, unsigned long long *__restrict__ root_port,
-                                               unsigned long long *__restrict__ pcie_switch) {
+// the LCP pass of kxpu_pcie_tree (plain chains; PARENT: the mdevs' parent chains), then the rule of include/kxpu.h on
+// the prefix: the functions after its last host bridge are f0, f1, ...; the root port is f0, the switch f_j for the
+// greatest odd j
+template <bool PARENT>
+__device__ __forceinline__ void group_ports(const Tree &T, unsigned long long *__restrict__ root_port,
+                                            unsigned long long *__restrict__ pcie_switch) {
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= T.G) return;
     unsigned long long k[MAXD];
     bool bad = false;
-    const int L = group_lcp<false>(T, g, k, bad);
+    const int L = group_lcp<false, PARENT>(T, g, k, bad);
     if (bad) atomicOr(T.err, 1u);
     // one pass root to leaf: a host bridge starts the function list again, f0 is the root port, each odd f_j the switch
     unsigned long long rp = KXPU_PCIE_NO_KEY, sw = KXPU_PCIE_NO_KEY;
@@ -255,6 +262,18 @@ __global__ void __launch_bounds__(256) k_ports(const Tree T, unsigned long long 
     }
     root_port[g] = rp;
     pcie_switch[g] = sw;
+}
+
+// kxpu_pcie_ports
+__global__ void __launch_bounds__(256) k_ports(const Tree T, unsigned long long *__restrict__ root_port,
+                                               unsigned long long *__restrict__ pcie_switch) {
+    group_ports<false>(T, root_port, pcie_switch);
+}
+
+// kxpu_pcie_ports_mdev
+__global__ void __launch_bounds__(256) k_ports_mdev(const Tree T, unsigned long long *__restrict__ root_port,
+                                                    unsigned long long *__restrict__ pcie_switch) {
+    group_ports<true>(T, root_port, pcie_switch);
 }
 
 __device__ __forceinline__ unsigned long long mix(unsigned long long h, unsigned long long x) {
@@ -460,14 +479,17 @@ extern "C" int32_t kxpu_pcie_tree_mdev(kxpu_ctx *ctx, const kxpu_mdevrec *recs, 
     return pcie_tree(ctx, recs, paths, n, group_off, group_members, n_groups, group_node, key, parent, depth, n_nodes, nullptr);
 }
 
-extern "C" int32_t kxpu_pcie_ports(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
-                                   const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
-                                   uint64_t *root_port, uint64_t *pcie_switch) {
+// Rec = kxpu_devrec: kxpu_pcie_ports; Rec = kxpu_mdevrec: kxpu_pcie_ports_mdev
+template <typename Rec>
+static int32_t pcie_ports(kxpu_ctx *ctx, const char *what, const Rec *recs, const kxpu_pcipath *paths, size_t n,
+                          const uint32_t *group_off, const uint32_t *group_members, size_t n_groups, uint64_t *root_port,
+                          uint64_t *pcie_switch) {
+    constexpr bool MD = std::is_same<Rec, kxpu_mdevrec>::value;
     static_assert(sizeof(unsigned long long) == sizeof(uint64_t), "keys");
     if (!ctx || (n && (!recs || !paths)) || !group_off) return KXPU_E_INVALID;
     if (n >= (1ull << 28) || n_groups >= (1ull << 28)) return KXPU_E_UNSUPPORTED;
     for (size_t g = 0; g < n_groups; g++)
-        if (group_off[g + 1] < group_off[g]) { KX_SET_ERR(ctx, "pcie_ports: group %zu: offsets decrease", g); return KXPU_E_INVALID; }
+        if (group_off[g + 1] < group_off[g]) { KX_SET_ERR(ctx, "%s: group %zu: offsets decrease", what, g); return KXPU_E_INVALID; }
     const size_t nm = group_off[n_groups];
     if ((nm && !group_members) || (n_groups && (!root_port || !pcie_switch))) return KXPU_E_INVALID;
     if (n_groups == 0) return KXPU_OK;
@@ -479,7 +501,7 @@ extern "C" int32_t kxpu_pcie_ports(kxpu_ctx *ctx, const kxpu_devrec *recs, const
     const size_t G = n_groups;
     size_t off = 0;
     auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
-    const size_t o_recs = take(n * sizeof(kxpu_devrec)), o_paths = take(n * sizeof(kxpu_pcipath));
+    const size_t o_recs = take(n * sizeof(Rec)), o_paths = take(n * sizeof(kxpu_pcipath));
     const size_t o_goff = take((G + 1) * 4), o_gmem = take(nm * 4), o_chain = take(n * MAXD * 8), o_clen = take(n);
     const size_t o_rp = take(G * 8), o_sw = take(G * 8), o_err = take(16);
     KxScratch sc(ctx);
@@ -487,7 +509,7 @@ extern "C" int32_t kxpu_pcie_ports(kxpu_ctx *ctx, const kxpu_devrec *recs, const
     KX_CUDA(ctx, sc.alloc((void **)&b, off));
     cudaStream_t st = ctx->stream;
     auto up = [&](size_t o, const void *h, size_t bytes) { if (bytes) cudaMemcpyAsync(b + o, h, bytes, cudaMemcpyHostToDevice, st); };
-    up(o_recs, recs, n * sizeof(kxpu_devrec)); up(o_paths, paths, n * sizeof(kxpu_pcipath));
+    up(o_recs, recs, n * sizeof(Rec)); up(o_paths, paths, n * sizeof(kxpu_pcipath));
     up(o_goff, group_off, (G + 1) * 4); up(o_gmem, group_members, nm * 4);
     cudaMemsetAsync(b + o_err, 0, 16, st);
     Tree T;
@@ -500,22 +522,34 @@ extern "C" int32_t kxpu_pcie_ports(kxpu_ctx *ctx, const kxpu_devrec *recs, const
     {
         KxTimer tm(ctx, KXPU_T_CLASSIFY);
         if (n) {
-            k_parse<kxpu_devrec, false><<<(unsigned)((n + PARSE_RECS - 1) / PARSE_RECS), PARSE_THREADS, 0, st>>>(
-                (const kxpu_devrec *)(b + o_recs), (const kxpu_pcipath *)(b + o_paths), (uint32_t)n,
+            k_parse<Rec, false><<<(unsigned)((n + PARSE_RECS - 1) / PARSE_RECS), PARSE_THREADS, 0, st>>>(
+                (const Rec *)(b + o_recs), (const kxpu_pcipath *)(b + o_paths), (uint32_t)n,
                 (unsigned long long *)(b + o_chain), b + o_clen, nullptr);
             ctx->launches++;
         }
-        k_ports<<<(unsigned)((G + 255) / 256), 256, 0, st>>>(T, d_rp, d_sw);
+        (MD ? k_ports_mdev : k_ports)<<<(unsigned)((G + 255) / 256), 256, 0, st>>>(T, d_rp, d_sw);
         ctx->launches++;
     }
     uint32_t *h = ctx->h_ctl;
     cudaMemcpyAsync(h, T.err, 4, cudaMemcpyDeviceToHost, st);
     cudaError_t e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { KX_SET_ERR(ctx, "pcie_ports failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
-    if (h[0]) { KX_SET_ERR(ctx, "pcie_ports: a group member index is >= n"); return KXPU_E_INVALID; }
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "%s failed: %s", what, cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    if (h[0]) { KX_SET_ERR(ctx, "%s: a group member index is >= n", what); return KXPU_E_INVALID; }
     cudaMemcpyAsync(root_port, d_rp, G * 8, cudaMemcpyDeviceToHost, st);
     cudaMemcpyAsync(pcie_switch, d_sw, G * 8, cudaMemcpyDeviceToHost, st);
     e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess) { KX_SET_ERR(ctx, "pcie_ports D2H failed: %s", cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "%s D2H failed: %s", what, cudaGetErrorString(e)); return KXPU_E_CUDA; }
     return KXPU_OK;
+}
+
+extern "C" int32_t kxpu_pcie_ports(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
+                                   const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
+                                   uint64_t *root_port, uint64_t *pcie_switch) {
+    return pcie_ports(ctx, "pcie_ports", recs, paths, n, group_off, group_members, n_groups, root_port, pcie_switch);
+}
+
+extern "C" int32_t kxpu_pcie_ports_mdev(kxpu_ctx *ctx, const kxpu_mdevrec *recs, const kxpu_pcipath *paths, size_t n,
+                                        const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
+                                        uint64_t *root_port, uint64_t *pcie_switch) {
+    return pcie_ports(ctx, "pcie_ports_mdev", recs, paths, n, group_off, group_members, n_groups, root_port, pcie_switch);
 }

@@ -763,6 +763,15 @@ Error Plugin::checkDraPcieDomain() const {
     return Error();
 }
 
+// draVgpuPcie: the vGPU pools' attributes take draPcieDomain's names, and only a vGPU class with DRA publishes them
+Error Plugin::checkDraVgpuPcie() const {
+    if (!draVgpuPcie) return Error();
+    if (draPcieDomain.empty()) return fail("draVgpuPcie is set but draPcieDomain is empty: it names the attributes");
+    if (!vgpuDraEnabled() && !vfVgpuDraEnabled())
+        return fail("draVgpuPcie is set but no vGPU class publishes DRA (no vGPU class has a draDriver, no class a vgpuDraDriver)");
+    return Error();
+}
+
 Error Plugin::checkResourceNames() const {
     size_t total = 0;
     std::map<std::string, size_t> classOf;  // name -> the class that configures it
@@ -1629,6 +1638,13 @@ Error Plugin::classify(MdevWalk &w) {
                                  w.nodeKey.data(), w.nodeParent.data(), w.nodeDepth.data(), &w.nNodes);
         if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_pcie_tree_mdev", rc);
     }
+    if (draVgpuPcie && vgpuDraEnabled()) {  // each group's root port and switch, from the links the DRA walk reads
+        w.rootPort.assign(c.nGroups + 1, KXPU_PCIE_NO_KEY);
+        w.pcieSwitch.assign(c.nGroups + 1, KXPU_PCIE_NO_KEY);
+        rc = kxpu_pcie_ports_mdev(ctx_, recs.data(), w.paths.data(), n, c.goff.data(), c.gmem.data(), c.nGroups,
+                                  w.rootPort.data(), w.pcieSwitch.data());
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_pcie_ports_mdev", rc);
+    }
     return Error();
 }
 
@@ -1653,6 +1669,7 @@ void Plugin::buildMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
         s.klass = groupClass[c.gids[g]];
         if (topologyAware) s.numa = c.gnuma[g];
         if (vgpuPcieTopologyAware) s.pcieNode = w.gnode[g];
+        if (!w.rootPort.empty()) { s.rootPort = w.rootPort[g]; s.pcieSwitch = w.pcieSwitch[g]; }
         if (vgpuSriovAware && w.pfOf[c.gmem[c.goff[g]]] != KXPU_NO_PF) {
             const kxpu_devrec &pf = pciRecs_[w.pfOf[c.gmem[c.goff[g]]]];
             s.pf.assign(pf.bdf, strnlen(pf.bdf, sizeof pf.bdf));
@@ -2320,6 +2337,7 @@ Error Plugin::InitiateDevicePlugin() {
     if (!e && vgpuSriovAware && vgpuClasses.empty()) e = fail("vgpuSriovAware is set but no vGPU class is configured");
     if (!e && sriovPfAware && !sriovAware) e = fail("sriovPfAware is set but sriovAware is off");
     if (!e) e = checkDraPcieDomain();
+    if (!e) e = checkDraVgpuPcie();
     if (e) return e;
     e = createIommuDeviceMap();  // :46
     if (e) return e;
@@ -2577,10 +2595,19 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
         auto qt = portsWas.find(iommuMap[g].first);  // a device moved under another root port or switch
         portsChanged |= qt != portsWas.end() && qt->second != std::make_pair(iommuState[g].rootPort, iommuState[g].pcieSwitch);
     }
+    std::map<std::string, std::pair<uint64_t, uint64_t>> mdevPortsWas;  // draVgpuPcie: mdev group id -> its ports
+    for (size_t g = 0; draVgpuPcie && g < mdevMap.size(); g++)
+        mdevPortsWas[mdevMap[g].first] = {mdevState[g].rootPort, mdevState[g].pcieSwitch};
+    bool mdevPortsChanged = false;
     if (!vgpuClasses.empty()) {
         MdevWalk mw;
         e = rewalk(mw, mdev_, report.mdev);
         if (e) return e;
+        for (size_t g = 0; g < mdevMap.size(); g++) {  // a vGPU moved under another root port or switch
+            auto qt = mdevPortsWas.find(mdevMap[g].first);
+            mdevPortsChanged |= qt != mdevPortsWas.end() &&
+                                qt->second != std::make_pair(mdevState[g].rootPort, mdevState[g].pcieSwitch);
+        }
     }
     e = computeAer();  // a re-enumerated function starts with zeroed counters
     if (e) return e;
@@ -2654,7 +2681,7 @@ Error Plugin::rediscover(RediscoverReport &report, const std::string &format) {
     const bool driftCleared = !driftTaint_.empty();  // the walk is the new truth: every drift reason is gone
     driftTaint_.clear();
     if (passthroughChanged || viabilityChanged || pfChanged || portsChanged || aerPt || driftCleared) pci_.draGeneration++;  // the next publication replaces these slices
-    if (vgpuChanged || aerVg) mdev_.draGeneration++;
+    if (vgpuChanged || mdevPortsChanged || aerVg) mdev_.draGeneration++;
     // 6. a fresh snapshot generation: Allocate answers from the snapshot again
     pci_.haveGen = haveGen;
     pci_.gen = gen;
@@ -3180,26 +3207,49 @@ Error Plugin::VgpuResourceSlices(size_t vgpuClass, std::vector<uint8_t> &out, st
         return fail("VgpuResourceSlices: vGPU class " + std::to_string(vgpuClass) + " has no DRA driver");
     std::vector<kxpu_dramdev> devs;
     std::vector<kxpu_dramdevpf> pfDevs;  // vgpuSriovAware: the same devices with their PFs
+    std::vector<kxpu_dramdevpcie> pcieDevs;  // draVgpuPcie: the same devices with their PFs (vgpuSriovAware) and ports
     std::vector<std::string> groups;
     forPublished(mdevMap, mdevState, vgpuClasses, [&](const std::string &g, const GroupState<kxpu_dramdev> &s) {
         if (s.klass != vgpuClass) return;
         groups.push_back(g);
-        if (!vgpuSriovAware) {
+        if (!vgpuSriovAware && !draVgpuPcie) {
             devs.push_back(*s.dra);
             return;
         }
         kxpu_dramdevpf d;
         memset(&d, 0, sizeof d);
         d.dev = *s.dra;
-        memcpy(d.physfn, s.pf.data(), std::min(s.pf.size(), sizeof d.physfn));
-        memcpy(d.physfn_device, s.pfDevice.data(), std::min(s.pfDevice.size(), sizeof d.physfn_device));
+        if (vgpuSriovAware) {
+            memcpy(d.physfn, s.pf.data(), std::min(s.pf.size(), sizeof d.physfn));
+            memcpy(d.physfn_device, s.pfDevice.data(), std::min(s.pfDevice.size(), sizeof d.physfn_device));
+        }
         if (!s.pfProduct.empty()) {  // the GPU's model, not the VF's
             memset(d.dev.product, 0, sizeof d.dev.product);
             d.dev.product_len = (uint8_t)std::min(s.pfProduct.size(), sizeof d.dev.product);
             memcpy(d.dev.product, s.pfProduct.data(), d.dev.product_len);
         }
-        pfDevs.push_back(d);
+        if (!draVgpuPcie) {
+            pfDevs.push_back(d);
+            return;
+        }
+        kxpu_dramdevpcie q;
+        memset(&q, 0, sizeof q);
+        q.pf = d;
+        q.root_port = s.rootPort;
+        q.pcie_switch = s.pcieSwitch;
+        pcieDevs.push_back(q);
     });
+    if (draVgpuPcie) {
+        const char *domain = draPcieDomain.c_str();
+        auto fn = [domain](kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                           const kxpu_dramdevpcie *v, size_t n, const kxpu_dra_taint *taints, size_t nt, const int64_t *since,
+                           uint8_t *o, size_t cap, size_t *len, uint64_t *off, size_t *ns) {
+            return kxpu_dra_slices_mdev_pcie(ctx, driver, pool, node, generation, domain, v, n, taints, nt, since, o, cap,
+                                             len, off, ns);
+        };
+        return draSlices(fn, "kxpu_dra_slices_mdev_pcie", vgpuClasses[vgpuClass].draDriver, mdev_.draGeneration, pcieDevs,
+                         groups, out, sliceOff);
+    }
     if (vgpuSriovAware)
         return draSlices(kxpu_dra_slices_mdev_pf, "kxpu_dra_slices_mdev_pf", vgpuClasses[vgpuClass].draDriver,
                          mdev_.draGeneration, pfDevs, groups, out, sliceOff);
@@ -3212,12 +3262,33 @@ Error Plugin::VfVgpuResourceSlices(size_t xpuClass, std::vector<uint8_t> &out, s
     if (xpuClass >= xpuClasses.size() || xpuClasses[xpuClass].vgpuDraDriver.empty())
         return fail("VfVgpuResourceSlices: class " + std::to_string(xpuClass) + " has no vGPU DRA driver");
     std::vector<kxpu_dravfvgpu> devs;
+    std::vector<kxpu_dravfvgpupcie> pcieDevs;  // draVgpuPcie: the same devices with the ports of their groups
     std::vector<std::string> groups;
     forPublishedVfVgpu(iommuMap, iommuState, xpuClasses, [&](const std::string &g, const GroupState<kxpu_dradev> &s) {
         if (s.klass != xpuClass) return;
-        devs.push_back(*s.vfVgpuDra);
         groups.push_back(g);
+        if (!draVgpuPcie) {
+            devs.push_back(*s.vfVgpuDra);
+            return;
+        }
+        kxpu_dravfvgpupcie q;
+        memset(&q, 0, sizeof q);
+        q.dev = *s.vfVgpuDra;
+        q.root_port = s.rootPort;
+        q.pcie_switch = s.pcieSwitch;
+        pcieDevs.push_back(q);
     });
+    if (draVgpuPcie) {
+        const char *domain = draPcieDomain.c_str();
+        auto fn = [domain](kxpu_ctx *ctx, const char *driver, const char *pool, const char *node, uint64_t generation,
+                           const kxpu_dravfvgpupcie *v, size_t n, const kxpu_dra_taint *taints, size_t nt,
+                           const int64_t *since, uint8_t *o, size_t cap, size_t *len, uint64_t *off, size_t *ns) {
+            return kxpu_dra_slices_vf_vgpu_pcie(ctx, driver, pool, node, generation, domain, v, n, taints, nt, since, o, cap,
+                                                len, off, ns);
+        };
+        return draSlices(fn, "kxpu_dra_slices_vf_vgpu_pcie", xpuClasses[xpuClass].vgpuDraDriver, pci_.draGeneration,
+                         pcieDevs, groups, out, sliceOff, vfVgpuHealth);
+    }
     return draSlices(kxpu_dra_slices_vf_vgpu, "kxpu_dra_slices_vf_vgpu", xpuClasses[xpuClass].vgpuDraDriver,
                      pci_.draGeneration, devs, groups, out, sliceOff, vfVgpuHealth);
 }
@@ -4632,6 +4703,7 @@ void kxh_set_vf_vgpu_health(void *h, int on) { ((Plugin *)h)->vfVgpuHealth = on 
 void kxh_set_vgpu_sriov(void *h, int on) { ((Plugin *)h)->vgpuSriovAware = on != 0; }
 void kxh_set_sriov_pf(void *h, int on) { ((Plugin *)h)->sriovPfAware = on != 0; }
 void kxh_set_dra_pcie_domain(void *h, const char *domain) { ((Plugin *)h)->draPcieDomain = domain ? domain : ""; }
+void kxh_set_dra_vgpu_pcie(void *h, int on) { ((Plugin *)h)->draVgpuPcie = on != 0; }
 uint64_t kxh_mdev_physfn_reads(void *h) { return ((Plugin *)h)->mdevPhysfnReads; }
 // refreshVfVgpuTypes: changed as kxh_refresh_aer_health's; *moved = bit 0 passthroughMoved, bit 1 typesMoved
 int kxh_refresh_vf_vgpu_types(void *h, size_t *changed, size_t cap, size_t *n_changed, int *moved, char *err, size_t errcap) {

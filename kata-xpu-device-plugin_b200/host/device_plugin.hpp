@@ -318,6 +318,9 @@ struct MdevWalk {
     std::vector<uint64_t> nodeKey;
     std::vector<uint8_t> nodeDepth;
     uint32_t nNodes = 0;
+    // draVgpuPcie (with a vGPU class that has a draDriver): per group ordinal its root port and switch
+    // (kxpu_pcie_ports_mdev), or KXPU_PCIE_NO_KEY
+    std::vector<uint64_t> rootPort, pcieSwitch;
     // mdevCdevEnabled only, one per record: N of its VFIO cdev, -1 = none or not read
     std::vector<int64_t> cdevs;
     // vgpuSriovAware only, one per record: its physfn read (kxpu_sriovrec, physfn only) and kxpu_mdev_pf's answer, the
@@ -365,8 +368,8 @@ struct GroupState {
     std::string drift{};
     // passthrough: the device id of the group's first member (readIDFromFile's text); names Device::model
     std::string firstDevice{};
-    // draPcieDomain, passthrough only: the group's root port and nearest switch upstream port (kxpu_pcie_ports' function
-    // keys), or KXPU_PCIE_NO_KEY
+    // draPcieDomain, PCI walk: the group's root port and nearest switch upstream port (kxpu_pcie_ports' function keys),
+    // or KXPU_PCIE_NO_KEY; draVgpuPcie, mdev walk: the same keys of the group's parent GPU (kxpu_pcie_ports_mdev)
     uint64_t rootPort = KXPU_PCIE_NO_KEY, pcieSwitch = KXPU_PCIE_NO_KEY;
 };
 
@@ -586,6 +589,23 @@ class Plugin {
     // Allocate, PrepareDraDevices, CDI specs, ListAndWatch, GetPreferredAllocation, metrics and the vGPU pools do not
     // change.
     std::string draPcieDomain;
+    // PCIe root ports and switches of vGPUs in DRA (include/kxpu.h, kxpu_pcie_ports_mdev, kxpu_dra_slices_mdev_pcie and
+    // kxpu_dra_slices_vf_vgpu_pcie): the vGPU pools publish <draPcieDomain>/pcieRootPort and <draPcieDomain>/pcieSwitch
+    // too, so a claim can keep a vGPU and a NIC VF of another DRA driver under one switch.  A switch of its own, not
+    // implied by draPcieDomain: with it off the vGPU pools' bytes are as above whatever draPcieDomain says.
+    // InitiateDevicePlugin refuses it while draPcieDomain is empty, and while no vGPU class publishes DRA (no vGPU class
+    // has a draDriver and no class a vgpuDraDriver).  false (default): no new call runs and every output, generation and
+    // counter is as above.  true:
+    //   - each mdev walk (with a vGPU class that has a draDriver) makes one kxpu_pcie_ports_mdev call over the classify
+    //     CSR, on the links the DRA walk already reads (no new file or link is read); each group keeps the keys of its
+    //     parent GPU (GroupState::rootPort / pcieSwitch);
+    //   - VgpuResourceSlices publishes through kxpu_dra_slices_mdev_pcie, the physfn fields filled only with
+    //     vgpuSriovAware and the PF's product as above; VfVgpuResourceSlices publishes through
+    //     kxpu_dra_slices_vf_vgpu_pcie with the keys the PCI walk keeps for each group (no new call);
+    //   - a rediscovery that moves a published mdev vGPU under another root port or switch moves draVgpuGeneration();
+    //     one that moves a VF-vGPU moves draGeneration(), as for any group of the PCI walk.
+    // Allocate, PrepareDraDevices, CDI specs, ListAndWatch, GetPreferredAllocation and the metrics do not change.
+    bool draVgpuPcie = false;
     // (type ID, type key) of every vGPU type a walk of this process named: the last name table of kxpu_vf_vgpu_types, so a
     // GPU that became full keeps its names across rediscover
     const std::map<uint32_t, std::string> &learnedVgpuTypes() const { return learnedVgpuTypes_; }
@@ -877,6 +897,7 @@ class Plugin {
                     bool typeTaint = false) const;
     Error checkDraClasses() const;
     Error checkDraPcieDomain() const;
+    Error checkDraVgpuPcie() const;
     void buildMdevDra(const MdevWalk &w);
     void buildVfVgpuDra(const PciWalk &w);
 };

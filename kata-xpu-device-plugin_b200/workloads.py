@@ -679,6 +679,49 @@ def pcie_ports_walk(n=1 << 20, vf_every=8):
     return recs, paths, np.arange(n + 1, dtype=np.uint32), np.arange(n, dtype=np.uint32)
 
 
+def pcie_ports_mdev_walk(n=1 << 20, vf_every=4, seed=23):
+    """kxpu_pcie_ports_mdev's and kxpu_pcie_tree_mdev's input: pcie_mdev_walk(n) (parent GPUs below root ports and
+    switches, one group per mdev), with the mdevs of one parent GPU in vf_every on a VF (function 4 beside the GPU, its
+    link beside the PF's).  Returns (recs, paths, group_off, group_members)."""
+    recs, paths, off, mem, _, _ = pcie_mdev_walk(n, seed)
+    par = recs["parent"]
+    vf = (np.char.str_len(par) > 0) & (np.frombuffer(par.tobytes(), np.uint8).reshape(n, 16)[:, 5] % vf_every == 0) \
+        if n else np.zeros(0, bool)
+    vfpar = np.char.replace(par, b":00.0", b":00.4")
+    text = paths["path"]
+    paths["path"] = np.where(vf, np.char.replace(text, np.char.add(par, b"/"), np.char.add(vfpar, b"/")), text)
+    recs["parent"] = np.where(vf, vfpar, par)
+    return recs, paths, off, mem
+
+
+def dra_mdev_pcie_devices(n=1 << 16, vf_every=8, seed=43):
+    """kxpu_dra_slices_mdev_pcie's input: dra_mdev_devices(n), one in vf_every on a VF with its PF's address and device
+    id, a root port on every device and a switch on three in four: 4-digit domains, 12-byte addresses"""
+    from .binding import DRAMDEVPCIE_DTYPE, PCIE_NO_KEY
+    d = np.zeros(n, DRAMDEVPCIE_DTYPE)
+    d["pf"]["dev"] = dra_mdev_devices(n, seed)
+    vf = np.arange(n) % vf_every == 0
+    d["pf"]["physfn"] = np.where(vf, b"0000:41:00.0", b"")
+    d["pf"]["physfn_device"] = np.where(vf, b"2330", b"")
+    _ports(d, n, PCIE_NO_KEY)
+    return d
+
+
+def dra_vf_vgpu_pcie_devices(n=1 << 16, seed=47):
+    """kxpu_dra_slices_vf_vgpu_pcie's input: dra_vf_vgpu_devices(n) with dra_mdev_pcie_devices' ports"""
+    from .binding import DRAVFVGPUPCIE_DTYPE, PCIE_NO_KEY
+    d = np.zeros(n, DRAVFVGPUPCIE_DTYPE)
+    d["dev"] = dra_vf_vgpu_devices(n, seed)
+    _ports(d, n, PCIE_NO_KEY)
+    return d
+
+
+def _ports(d, n, no_key):
+    k = np.arange(n, dtype=np.uint64)
+    d["root_port"] = (k >> np.uint64(6) & np.uint64(0xff)) << np.uint64(8) | np.uint64(8)
+    d["pcie_switch"] = np.where(k % 4 != 3, d["root_port"] + np.uint64(0x100), np.uint64(no_key))
+
+
 def dra_mdev_devices(n=1 << 16, seed=43):
     """n published vGPUs with every optional attribute present and the longest fields the host produces: a 64-byte
     product name, a 40-byte type key, a 12-byte parent address, a 10-byte PCIe root, 4-digit ids, one NUMA node, 9-digit

@@ -96,6 +96,17 @@ print("pcie_ports switches", int((pst != B.PCIE_NO_KEY).sum()), "dra_pcie slice 
       len(kx.dra_slices_pcie("d", "p", "n", 1, "pcie.example.com", pcdevs, [], None)[0]),
       len(kx.dra_slices_pcie("d", "p", "n", 1, "pcie.example.com", pcdevs, [("d/k", "", "NoSchedule")],
                              np.full((300, 1), 5, np.int64))[0]))
+# PCIe root ports and switches of vGPUs: the ports of an mdev walk, then both vGPU layouts untainted and with one taint
+vmr, vmp, vmo, vmm = W.pcie_ports_mdev_walk(3000)
+vrt, vst = kx.pcie_ports_mdev(vmr, vmp, vmo, vmm)
+vmdevs, vfdevs = W.dra_mdev_pcie_devices(300), W.dra_vf_vgpu_pcie_devices(300)
+print("pcie_ports_mdev switches", int((vst != B.PCIE_NO_KEY).sum()), "dra vgpu pcie slice bytes",
+      len(kx.dra_slices_mdev_pcie("d", "p", "n", 1, "pcie.example.com", vmdevs, [], None)[0]),
+      len(kx.dra_slices_mdev_pcie("d", "p", "n", 1, "pcie.example.com", vmdevs, [("d/k", "", "NoSchedule")],
+                                  np.full((300, 1), 5, np.int64))[0]),
+      len(kx.dra_slices_vf_vgpu_pcie("d", "p", "n", 1, "pcie.example.com", vfdevs, [], None)[0]),
+      len(kx.dra_slices_vf_vgpu_pcie("d", "p", "n", 1, "pcie.example.com", vfdevs, [("d/k", "", "NoSchedule")],
+                                     np.full((300, 1), 5, np.int64))[0]))
 # resets between tenants: every member's function reset or bus-reset set, on the classify CSR
 rrecs, rpaths, rrrs = W.reset_walk(20000)
 rres = kx.classify_rules([(b"10de", b"vfio-pci")], rrecs)
