@@ -71,7 +71,7 @@ uint64_t kxpu_launch_count(kxpu_ctx *ctx);
 #define KXPU_T_FINALIZE 1
 #define KXPU_T_LOOKUP   2  /* 0 after kxpu_pciids_join(_device): the join runs beside the names, under KXPU_T_FINALIZE */
 #define KXPU_T_NAMES    3
-#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s, kxpu_pcie_ports[_mdev]', kxpu_sriov's, kxpu_mdev_pf's and kxpu_reset_check's kernels: the slot holds the most recent call's */
+#define KXPU_T_CLASSIFY 4  /* also kxpu_reconcile's, kxpu_pcie_tree[_sriov / _mdev]'s, kxpu_pcie_ports[_mdev]', kxpu_aer_ports[_mdev]', kxpu_sriov's, kxpu_mdev_pf's and kxpu_reset_check's kernels: the slot holds the most recent call's */
 #define KXPU_T_EMIT     5  /* also kxpu_cdi_parse[_mdev|_cdev|_mdev_cdev|_vf_vgpu[_cdev]]: decode, re-emit and compare of the most recent call */
 #define KXPU_T_MERGE    6
 #define KXPU_T_RESOLVE  7  /* parse: second pass over the chunks whose governing line was not known */
@@ -1678,6 +1678,54 @@ int32_t kxpu_dra_slices_vf_vgpu_pcie(kxpu_ctx *ctx, const char *driver, const ch
                                      size_t n, const kxpu_dra_taint *taints, size_t n_taints,
                                      const int64_t *taint_since /* [n * n_taints] or NULL */, uint8_t *out, size_t cap,
                                      size_t *len, uint64_t *slice_off /* [n_slices+1] */, size_t *n_slices);
+
+/* ------------------------------------ the PCIe ports above every record (addition to ABI v14) */
+
+/* These calls were added to ABI v14 without a version bump: a caller detects them by symbol (dlsym), as for
+ * kxpu_pcie_ports.  They list the PCIe ports above each record, so that kxpu_aer_health can fold the ports' AER counts
+ * into the groups below them (Plugin::aerPortHealth).  Many uncorrectable errors are logged by a port, not by the device:
+ *   [assumed] the AER driver counts an error in the aer_dev_* files of the function that logged it: a Surprise Down in
+ *             the downstream port above the device that dropped off the link, a completion timeout in the requester (the
+ *             root port, for a CPU read), an error on the link between a root port and a switch in the root port or the
+ *             switch upstream port;
+ *   [assumed] ports have aer_dev_fatal and aer_dev_nonfatal when they have an AER capability, as any function does;
+ *   [assumed] whether errors that Downstream Port Containment (DPC) handles are counted depends on the kernel version;
+ *             this is unverified.
+ * A port without the files gives an unknown count, which never flags a group (kxpu_aer_health).  Which function logs
+ * which error is taken from the PCIe specification and the kernel's AER documentation; it has not been observed here.
+ *
+ * THE RULE.  The PORTS of record i are the function components of i's chain, exactly as kxpu_pcie_tree's parse reads it
+ * (kxpu_pcie_ports' chain, taken per record instead of per group), ordered NEAREST FIRST: from the last chain component
+ * toward the first.  Host-bridge components are skipped, VMD's pci10000:e0 included; the VMD endpoint function above
+ * it is a port like any other.  So:
+ *   - a record with an unknown path has no ports;
+ *   - a record directly below its host bridge has none;
+ *   - a VF needs no special case: its sysfs path sits beside its PF's, so it gets the PF's ports (physfn is not read);
+ *   - for kxpu_aer_ports_mdev the chain is the mdev's kxpu_pcie_tree_mdev chain WITHOUT its last key, the parent
+ *     function (the host reads the parent's files as the group's own): the parent GPU's ports, a VF parent's being its
+ *     PF's.
+ * Outputs:
+ *   - port_of[port_off[i] .. port_off[i+1]) holds the port numbers of record i, nearest first; port_off[0] = 0;
+ *   - port_key[p] is the function key of port p (kxpu_pcie_tree's key form: domain << 16 | bus << 8 | dev << 3 | fn);
+ *   - ports are numbered in the order of their first occurrence in port_of, so *n_ports is the number of distinct
+ *     ports of the walk and a switch port above 8 GPUs is one port.
+ * port_of and port_key hold (KXPU_PCIE_MAX_DEPTH - 1) * n entries at most (a known chain starts with a host bridge).
+ * KXPU_E_INVALID, nothing written: ctx NULL; recs or paths NULL with n > 0; port_off NULL; port_of, port_key or n_ports
+ * NULL with n > 0.  Limit (else KXPU_E_UNSUPPORTED, nothing written): n below 2^28.  With n == 0: port_off[0] = 0 and,
+ * when n_ports is not NULL, *n_ports = 0.
+ * GPU: kxpu_pcie_tree's parse (kxpu_pcie_tree_mdev's for the mdev call), then one thread per record in each pass: the
+ * count of its ports and the single-pass scan (port_off); an open-addressing table of the ports' keys in which an atomic
+ * min keeps each key's first position; per record the count of positions that are their key's first, and its scan (the
+ * ordinals); port_key and port_of.  Timed under KXPU_T_CLASSIFY. */
+int32_t kxpu_aer_ports(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
+                       uint32_t *port_off /* [n+1] */, uint32_t *port_of /* [KXPU_PCIE_MAX_DEPTH * n] */,
+                       uint64_t *port_key /* [KXPU_PCIE_MAX_DEPTH * n] */, uint32_t *n_ports);
+
+/* kxpu_aer_ports for the mdev walk's records (paths in kxpu_pcie_tree_mdev's grammar), by the rule above: the same
+ * outputs, errors and limits. */
+int32_t kxpu_aer_ports_mdev(kxpu_ctx *ctx, const kxpu_mdevrec *recs, const kxpu_pcipath *paths, size_t n,
+                            uint32_t *port_off /* [n+1] */, uint32_t *port_of /* [KXPU_PCIE_MAX_DEPTH * n] */,
+                            uint64_t *port_key /* [KXPU_PCIE_MAX_DEPTH * n] */, uint32_t *n_ports);
 
 /* ------------------------------------- resets between tenants (addition to ABI v14) */
 

@@ -561,6 +561,43 @@ func (k *kxpu) pciePortsMdev(recs []C.kxpu_mdevrec, paths []C.kxpu_pcipath, goff
 	return rootPort[:nGroups], pcieSwitch[:nGroups], err
 }
 
+// the PCIe ports above every record (an addition to ABI v14, detected by symbol): ports of record i are
+// portOf[portOff[i]:portOff[i+1]], nearest first, and portKey[p] is port p's function key.  Called once per PCI walk
+// when aerPortHealth is set; computeAer then reads each distinct port's aer_dev_* files after a group's own members.
+func (k *kxpu) aerPorts(recs []C.kxpu_devrec, paths []C.kxpu_pcipath) (portOff, portOf []uint32, portKey []uint64, err error) {
+	n := len(recs)
+	portOff = make([]uint32, n+1)
+	portOf, portKey = make([]uint32, C.KXPU_PCIE_MAX_DEPTH*n+1), make([]uint64, C.KXPU_PCIE_MAX_DEPTH*n+1)
+	var r unsafe.Pointer
+	var pp *C.kxpu_pcipath
+	if n > 0 {
+		r, pp = unsafe.Pointer(&recs[0]), &paths[0]
+	}
+	var nk C.uint32_t
+	err = kxCheck(k.ctx, "kxpu_aer_ports", C.kxpu_aer_ports(k.ctx, (*C.kxpu_devrec)(r), pp, C.size_t(n),
+		(*C.uint32_t)(unsafe.Pointer(&portOff[0])), (*C.uint32_t)(unsafe.Pointer(&portOf[0])),
+		(*C.uint64_t)(unsafe.Pointer(&portKey[0])), &nk))
+	return portOff, portOf[:portOff[n]], portKey[:nk], err
+}
+
+// aerPorts for the mdev walk: the ports above each mdev's parent GPU.  Called once per mdev walk when aerPortHealth is
+// set.
+func (k *kxpu) aerPortsMdev(recs []C.kxpu_mdevrec, paths []C.kxpu_pcipath) (portOff, portOf []uint32, portKey []uint64, err error) {
+	n := len(recs)
+	portOff = make([]uint32, n+1)
+	portOf, portKey = make([]uint32, C.KXPU_PCIE_MAX_DEPTH*n+1), make([]uint64, C.KXPU_PCIE_MAX_DEPTH*n+1)
+	var r unsafe.Pointer
+	var pp *C.kxpu_pcipath
+	if n > 0 {
+		r, pp = unsafe.Pointer(&recs[0]), &paths[0]
+	}
+	var nk C.uint32_t
+	err = kxCheck(k.ctx, "kxpu_aer_ports_mdev", C.kxpu_aer_ports_mdev(k.ctx, (*C.kxpu_mdevrec)(r), pp, C.size_t(n),
+		(*C.uint32_t)(unsafe.Pointer(&portOff[0])), (*C.uint32_t)(unsafe.Pointer(&portOf[0])),
+		(*C.uint64_t)(unsafe.Pointer(&portKey[0])), &nk))
+	return portOff, portOf[:portOff[n]], portKey[:nk], err
+}
+
 // pcieTree over records that carry only their address, one per link target (walk order): what pcieTree sees of a walk
 func (k *kxpu) pcieTreeOfLinks(bdfs, targets []string, goff, gmem []uint32) (gnode, parent []uint32, depth []uint8, err error) {
 	recs, paths := make([]C.kxpu_devrec, len(bdfs)), make([]C.kxpu_pcipath, len(bdfs))

@@ -183,6 +183,7 @@ ABI_SYMBOLS = [
     "kxpu_mdev_pf", "kxpu_dra_slices_mdev_pf", "kxpu_classify_named", "kxpu_dra_slices_pf",
     "kxpu_pcie_ports", "kxpu_dra_slices_pcie",
     "kxpu_pcie_ports_mdev", "kxpu_dra_slices_mdev_pcie", "kxpu_dra_slices_vf_vgpu_pcie",
+    "kxpu_aer_ports", "kxpu_aer_ports_mdev",
 ]
 
 
@@ -323,6 +324,8 @@ def load_library():
         "kxpu_dra_slices_pcie": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, C.c_char_p, vp, sz, vp, sz, vp, vp,
                                        sz, C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_pcie_ports_mdev": (i32, [vp, vp, vp, sz, vp, vp, sz, vp, vp]),
+        "kxpu_aer_ports": (i32, [vp, vp, vp, sz, vp, vp, vp, C.POINTER(C.c_uint32)]),
+        "kxpu_aer_ports_mdev": (i32, [vp, vp, vp, sz, vp, vp, vp, C.POINTER(C.c_uint32)]),
         "kxpu_dra_slices_mdev_pcie": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, C.c_char_p, vp, sz, vp, sz, vp,
                                             vp, sz, C.POINTER(sz), vp, C.POINTER(sz)]),
         "kxpu_dra_slices_vf_vgpu_pcie": (i32, [vp, C.c_char_p, C.c_char_p, C.c_char_p, u64, C.c_char_p, vp, sz, vp, sz,
@@ -972,6 +975,27 @@ class Kxpu:
         self._chk(self.L.kxpu_pcie_ports_mdev(self.ctx, _ptr(recs) if n else None, _ptr(paths) if n else None, n,
                                               _ptr(group_off), _ptr(group_members) if len(group_members) else None,
                                               len(group_off) - 1, _ptr(root_port), _ptr(pcie_switch)))
+
+    def aer_ports(self, recs, paths):
+        """kxpu_aer_ports (recs DEVREC_DTYPE) or kxpu_aer_ports_mdev (recs MDEVREC_DTYPE), paths PCIPATH_DTYPE at the same
+        indices.  Returns (port_off, port_of, port_key): the ports of record i are port_of[port_off[i]:port_off[i+1]],
+        nearest first, and port_key[p] is the function key of port p."""
+        recs, paths = np.ascontiguousarray(recs), np.ascontiguousarray(paths)
+        assert recs.dtype in (DEVREC_DTYPE, MDEVREC_DTYPE) and paths.dtype == PCIPATH_DTYPE and len(recs) == len(paths)
+        n = len(recs)
+        cap = max(PCIE_MAX_DEPTH * n, 1)
+        off, of, key = np.empty(n + 1, np.uint32), np.empty(cap, np.uint32), np.empty(cap, np.uint64)
+        nk = C.c_uint32(0)
+        self.aer_ports_raw(recs, paths, off, of, key, C.byref(nk))
+        return off, of[:off[n]], key[:nk.value]
+
+    def aer_ports_raw(self, recs, paths, port_off, port_of, port_key, n_ports, n=None, mdev=None):
+        """The bare call into caller buffers (timing loops, untouched-output checks); n defaults to len(recs), mdev to
+        whether recs are MDEVREC_DTYPE, and a None array is passed as NULL."""
+        n = len(recs) if n is None else n
+        mdev = recs is not None and recs.dtype == MDEVREC_DTYPE if mdev is None else mdev
+        f = self.L.kxpu_aer_ports_mdev if mdev else self.L.kxpu_aer_ports
+        self._chk(f(self.ctx, _ptr(recs), _ptr(paths), n, _ptr(port_off), _ptr(port_of), _ptr(port_key), n_ports))
 
     def pcie_tree_mdev(self, recs, paths, group_off, group_members):
         """kxpu_pcie_tree_mdev: recs (MDEVREC_DTYPE) and paths (PCIPATH_DTYPE, the entries' links) at the same indices,

@@ -20,7 +20,11 @@
 // other kernels.  kxpu_pcie_ports runs kxpu_pcie_tree's parse, then k_ports: the LCP pass (group_lcp<false>, shared
 // with k_lcp) writing each group's root port and switch instead of its prefix.  kxpu_pcie_ports_mdev runs
 // k_parse<kxpu_mdevrec, false>, then k_ports_mdev: the same pass over each member's chain one key short (its parent
-// chain).
+// chain).  kxpu_aer_ports[_mdev] run the same two parses, then one thread per record in each of: k_port_count (the
+// function keys of its chain, for the mdev variant less the parent), the single-pass scan (port_off), k_port_insert
+// (each port into an open-addressing table of u32 position codes, atomic min: a key's first position), k_port_first
+// (each position's slot and whether it is its key's first, counted per record), the scan of those counts (each
+// record's first ordinal; the total is n_ports), k_port_key (port_key, and the ordinal into the slot) and k_port_of.
 #include <algorithm>
 #include <type_traits>
 
@@ -349,6 +353,119 @@ __global__ void __launch_bounds__(256) k_emit(const Tree T) {
     T.group_node[g] = prev;
 }
 
+// kxpu_aer_ports[_mdev].  A record's ports are the function keys of its chain (MD: the chain less its last key, the
+// parent function), nearest first; position (i, t) of chain key t sorts as i << 3 | (MAXD - 1 - t).  One thread per
+// record in every pass.
+constexpr uint32_t EMPTY32 = ~0u;
+constexpr int PORTS_MAX = MAXD - 1;  // a known chain starts with a host bridge
+
+struct Ports {
+    uint32_t n;
+    const unsigned long long *chain;
+    const uint8_t *clen;
+    uint32_t *cnt, *off;     // [n] ports of record i, its first position
+    uint32_t *fcnt, *fbase;  // [n] positions of record i that are their key's first, their first ordinal
+    uint32_t *slots;         // [mask + 1]: the least position code of a key; after k_port_key, that key's ordinal
+    uint32_t mask;
+    uint32_t *pslot;         // [PORTS_MAX * n] slot of position p
+    uint8_t *pfirst;         // [PORTS_MAX * n] position p is its key's first
+    uint32_t *port_of;
+    unsigned long long *port_key;
+    uint32_t *err;           // [0] = 1: table overflow
+};
+
+template <bool MD>
+__device__ __forceinline__ int port_chain_len(const Ports &P, uint32_t i) {
+    const int l = P.clen[i];
+    return MD ? max(l - 1, 0) : l;
+}
+
+template <bool MD>
+__global__ void __launch_bounds__(256) k_port_count(const Ports P) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.n) return;
+    const unsigned long long *c = P.chain + (size_t)i * MAXD;
+    const int L = port_chain_len<MD>(P, i);
+    uint32_t k = 0;
+    for (int t = 0; t < L; t++) k += !(c[t] & HOST_BRIDGE);
+    P.cnt[i] = k;
+}
+
+// slot of a port key (insert: of position code me, the atomic min of the codes; else the key has been inserted).  A slot
+// holds a code whose key is read back from the chains, written by the parse, so the comparison stays valid while the
+// slot's code falls to another position of the same key.  At least two slots per position: the bound only guarantees
+// that a probe sequence ends (err[0] set, ~0u returned).
+__device__ __forceinline__ uint32_t port_slot(const Ports &P, unsigned long long key, uint32_t me, bool insert) {
+    uint32_t s = (uint32_t)mix(0x243F6A8885A308D3ull, key) & P.mask;
+    for (unsigned long long probes = 0; probes <= P.mask; probes++, s = (s + 1) & P.mask) {
+        uint32_t v = *reinterpret_cast<volatile uint32_t *>(P.slots + s);
+        if (v == EMPTY32) {
+            if (!insert) break;
+            v = atomicCAS(P.slots + s, EMPTY32, me);
+            if (v == EMPTY32) return s;
+        }
+        if (P.chain[(size_t)(v >> 3) * MAXD + (MAXD - 1 - (v & 7u))] != key) continue;
+        if (insert && me < v) atomicMin(P.slots + s, me);  // a shared port: most records see a smaller code already
+        return s;
+    }
+    atomicOr(P.err, 1u);
+    return ~0u;
+}
+
+template <bool MD>
+__global__ void __launch_bounds__(256) k_port_insert(const Ports P) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.n) return;
+    const unsigned long long *c = P.chain + (size_t)i * MAXD;
+    for (int t = port_chain_len<MD>(P, i) - 1; t >= 0; t--)
+        if (!(c[t] & HOST_BRIDGE)) port_slot(P, c[t], i << 3 | (uint32_t)(MAXD - 1 - t), true);
+}
+
+template <bool MD>
+__global__ void __launch_bounds__(256) k_port_first(const Ports P) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.n) return;
+    const unsigned long long *c = P.chain + (size_t)i * MAXD;
+    uint32_t p = P.off[i], f = 0;
+    for (int t = port_chain_len<MD>(P, i) - 1; t >= 0; t--) {
+        if (c[t] & HOST_BRIDGE) continue;
+        const uint32_t me = i << 3 | (uint32_t)(MAXD - 1 - t);
+        const uint32_t s = port_slot(P, c[t], me, false);
+        const bool first = s != ~0u && P.slots[s] == me;
+        P.pslot[p] = s;
+        P.pfirst[p] = first;
+        f += first;
+        p++;
+    }
+    P.fcnt[i] = f;
+}
+
+// a first position names its key: port_key[ordinal], and the ordinal replaces the code in its slot
+template <bool MD>
+__global__ void __launch_bounds__(256) k_port_key(const Ports P) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.n) return;
+    const unsigned long long *c = P.chain + (size_t)i * MAXD;
+    uint32_t p = P.off[i], o = P.fbase[i];
+    for (int t = port_chain_len<MD>(P, i) - 1; t >= 0; t--) {
+        if (c[t] & HOST_BRIDGE) continue;
+        if (P.pfirst[p]) {
+            P.port_key[o] = c[t];
+            P.slots[P.pslot[p]] = o++;
+        }
+        p++;
+    }
+}
+
+__global__ void __launch_bounds__(256) k_port_of(const Ports P) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.n) return;
+    for (uint32_t p = P.off[i], e = p + P.cnt[i]; p < e; p++) {
+        const uint32_t s = P.pslot[p];  // ~0u only after a table overflow, which the call reports
+        P.port_of[p] = s == ~0u ? ~0u : P.slots[s];
+    }
+}
+
 }  // namespace kxpcie
 
 using namespace kxpcie;
@@ -552,4 +669,93 @@ extern "C" int32_t kxpu_pcie_ports_mdev(kxpu_ctx *ctx, const kxpu_mdevrec *recs,
                                         const uint32_t *group_off, const uint32_t *group_members, size_t n_groups,
                                         uint64_t *root_port, uint64_t *pcie_switch) {
     return pcie_ports(ctx, "pcie_ports_mdev", recs, paths, n, group_off, group_members, n_groups, root_port, pcie_switch);
+}
+
+// Rec = kxpu_devrec: kxpu_aer_ports; Rec = kxpu_mdevrec: kxpu_aer_ports_mdev
+template <typename Rec>
+static int32_t aer_ports(kxpu_ctx *ctx, const char *what, const Rec *recs, const kxpu_pcipath *paths, size_t n,
+                         uint32_t *port_off, uint32_t *port_of, uint64_t *port_key, uint32_t *n_ports) {
+    constexpr bool MD = std::is_same<Rec, kxpu_mdevrec>::value;
+    if (!ctx || (n && (!recs || !paths)) || !port_off || (n && (!port_of || !port_key || !n_ports))) return KXPU_E_INVALID;
+    if (n >= (1ull << 28)) return KXPU_E_UNSUPPORTED;
+    if (n == 0) {
+        port_off[0] = 0;
+        if (n_ports) *n_ports = 0;
+        return KXPU_OK;
+    }
+
+    std::lock_guard<std::mutex> guard(ctx->mu);
+    cudaSetDevice(ctx->device);
+    kx_clear_timings(ctx);
+    const size_t NP = (size_t)PORTS_MAX * n;  // bounds the positions
+    uint32_t slots = 1;
+    while (slots < 2 * NP) slots <<= 1;
+    size_t off = 0;
+    auto take = [&](size_t bytes) { size_t o = off; off = (off + bytes + 255) / 256 * 256; return o; };
+    const size_t o_recs = take(n * sizeof(Rec)), o_paths = take(n * sizeof(kxpu_pcipath));
+    const size_t o_chain = take(n * MAXD * 8), o_clen = take(n);
+    const size_t o_cnt = take(n * 4), o_off = take(n * 4), o_fcnt = take(n * 4), o_fbase = take(n * 4);
+    const size_t o_slots = take((size_t)slots * 4), o_pslot = take(NP * 4), o_pfirst = take(NP);
+    const size_t o_of = take(NP * 4), o_key = take(NP * 8), o_err = take(32);
+    KxScratch sc(ctx);
+    uint8_t *b = nullptr;
+    KX_CUDA(ctx, sc.alloc((void **)&b, off));
+    cudaStream_t st = ctx->stream;
+    cudaMemcpyAsync(b + o_recs, recs, n * sizeof(Rec), cudaMemcpyHostToDevice, st);
+    cudaMemcpyAsync(b + o_paths, paths, n * sizeof(kxpu_pcipath), cudaMemcpyHostToDevice, st);
+    cudaMemsetAsync(b + o_slots, 0xFF, (size_t)slots * 4, st);
+    cudaMemsetAsync(b + o_err, 0, 32, st);
+    Ports P;
+    P.n = (uint32_t)n;
+    P.chain = (const unsigned long long *)(b + o_chain); P.clen = b + o_clen;
+    P.cnt = (uint32_t *)(b + o_cnt); P.off = (uint32_t *)(b + o_off);
+    P.fcnt = (uint32_t *)(b + o_fcnt); P.fbase = (uint32_t *)(b + o_fbase);
+    P.slots = (uint32_t *)(b + o_slots); P.mask = slots - 1;
+    P.pslot = (uint32_t *)(b + o_pslot); P.pfirst = b + o_pfirst;
+    P.port_of = (uint32_t *)(b + o_of); P.port_key = (unsigned long long *)(b + o_key);
+    P.err = (uint32_t *)(b + o_err);
+    unsigned long long *d_totals = (unsigned long long *)(b + o_err + 16);  // positions, distinct ports
+    {
+        KxTimer tm(ctx, KXPU_T_CLASSIFY);
+        k_parse<Rec, false><<<(unsigned)((n + PARSE_RECS - 1) / PARSE_RECS), PARSE_THREADS, 0, st>>>(
+            (const Rec *)(b + o_recs), (const kxpu_pcipath *)(b + o_paths), (uint32_t)n,
+            (unsigned long long *)(b + o_chain), b + o_clen, nullptr);
+        const unsigned nb = (unsigned)((n + 255) / 256);
+        k_port_count<MD><<<nb, 256, 0, st>>>(P);
+        ctx->launches += 2;
+        int32_t rc = kxscan::exclusive_scan(ctx, P.cnt, n, P.off, d_totals);
+        if (rc != KXPU_OK) return rc;
+        k_port_insert<MD><<<nb, 256, 0, st>>>(P);
+        k_port_first<MD><<<nb, 256, 0, st>>>(P);
+        ctx->launches += 2;
+        rc = kxscan::exclusive_scan(ctx, P.fcnt, n, P.fbase, d_totals + 1);
+        if (rc != KXPU_OK) return rc;
+        k_port_key<MD><<<nb, 256, 0, st>>>(P);
+        k_port_of<<<nb, 256, 0, st>>>(P);
+        ctx->launches += 2;
+    }
+    uint32_t *h = ctx->h_ctl;
+    cudaMemcpyAsync(h, P.err, 32, cudaMemcpyDeviceToHost, st);
+    cudaError_t e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "%s failed: %s", what, cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    if (h[0]) { KX_SET_ERR(ctx, "%s: port table overflow", what); return KXPU_E_CAPACITY; }
+    const uint32_t np = h[4], nk = h[6];  // the two totals' low words (each below 2^31)
+    cudaMemcpyAsync(port_off, P.off, n * 4, cudaMemcpyDeviceToHost, st);
+    if (np) cudaMemcpyAsync(port_of, P.port_of, (size_t)np * 4, cudaMemcpyDeviceToHost, st);
+    if (nk) cudaMemcpyAsync(port_key, P.port_key, (size_t)nk * 8, cudaMemcpyDeviceToHost, st);
+    e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { KX_SET_ERR(ctx, "%s D2H failed: %s", what, cudaGetErrorString(e)); return KXPU_E_CUDA; }
+    port_off[n] = np;
+    *n_ports = nk;
+    return KXPU_OK;
+}
+
+extern "C" int32_t kxpu_aer_ports(kxpu_ctx *ctx, const kxpu_devrec *recs, const kxpu_pcipath *paths, size_t n,
+                                  uint32_t *port_off, uint32_t *port_of, uint64_t *port_key, uint32_t *n_ports) {
+    return aer_ports(ctx, "aer_ports", recs, paths, n, port_off, port_of, port_key, n_ports);
+}
+
+extern "C" int32_t kxpu_aer_ports_mdev(kxpu_ctx *ctx, const kxpu_mdevrec *recs, const kxpu_pcipath *paths, size_t n,
+                                       uint32_t *port_off, uint32_t *port_of, uint64_t *port_key, uint32_t *n_ports) {
+    return aer_ports(ctx, "aer_ports_mdev", recs, paths, n, port_off, port_of, port_key, n_ports);
 }

@@ -1305,6 +1305,17 @@ Error Plugin::classify(PciWalk &w) {
                              w.rootPort.data(), w.pcieSwitch.data());
         if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_pcie_ports", rc);
     }
+    if (aerPortHealth) {  // the ports above every record, from the paths read above
+        w.aerPortOff.assign(n + 1, 0);
+        w.aerPortOf.assign((size_t)KXPU_PCIE_MAX_DEPTH * n + 1, 0);
+        w.aerPortKey.assign((size_t)KXPU_PCIE_MAX_DEPTH * n + 1, 0);
+        uint32_t nk = 0;
+        rc = kxpu_aer_ports(ctx_, recs.data(), w.paths.data(), n, w.aerPortOff.data(), w.aerPortOf.data(),
+                            w.aerPortKey.data(), &nk);
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_aer_ports", rc);
+        w.aerPortOf.resize(w.aerPortOff[n]);
+        w.aerPortKey.resize(nk);
+    }
     return Error();
 }
 
@@ -1325,6 +1336,36 @@ std::string Plugin::pfDeviceOf(const kxpu_devrec &pf, std::map<std::string, std:
     bool ok = id.size() <= 6;
     for (char ch : id) ok = ok && ((ch >= '0' && ch <= '9') || (ch >= 'a' && ch <= 'f'));
     return ok ? id : std::string();
+}
+
+// the sysfs address of a kxpu_pcie_tree function key: a 4-digit domain, or 5..8 digits above ffff (VMD)
+static std::string portAddress(uint64_t key) {
+    char b[24];
+    const unsigned long long dom = key >> 16;
+    snprintf(b, sizeof b, dom <= 0xffff ? "%04llx:%02x:%02x.%u" : "%llx:%02x:%02x.%u", dom, (unsigned)(key >> 8 & 0xff),
+             (unsigned)(key >> 3 & 0x1f), (unsigned)(key & 7));
+    return b;
+}
+
+// aerPortHealth: the ports above group g's members (kxpu_aer_ports' CSR of the walk), member by member, each nearest
+// first, each port once, with the function (fn of the member) it was first found above
+template <typename Dev>
+static std::vector<std::pair<std::string, std::string>> groupPorts(const std::vector<uint32_t> &off,
+                                                                   const std::vector<uint32_t> &of,
+                                                                   const std::vector<uint64_t> &key, const ClassifyResult &c,
+                                                                   uint32_t g, const std::vector<Dev> &devs,
+                                                                   std::string Dev::*fn) {
+    std::vector<std::pair<std::string, std::string>> out;
+    std::vector<uint32_t> seen;
+    for (uint32_t k = c.goff[g]; k < c.goff[g + 1]; k++) {
+        const uint32_t i = c.gmem[k];
+        for (uint32_t p = off[i]; p < off[i + 1]; p++) {
+            if (std::find(seen.begin(), seen.end(), of[p]) != seen.end()) continue;
+            seen.push_back(of[p]);
+            out.emplace_back(portAddress(key[of[p]]), devs[k - c.goff[g]].*fn);
+        }
+    }
+    return out;
 }
 
 void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
@@ -1380,6 +1421,7 @@ void Plugin::buildMaps(const PciWalk &w, const std::vector<uint64_t> *index) {
             s.pf.assign(pf.bdf, strnlen(pf.bdf, sizeof pf.bdf));
             if (draEnabled()) s.pfDevice = pfDeviceOf(pf, pfDeviceRead);
         }
+        if (aerPortHealth) s.aerPorts = groupPorts(w.aerPortOff, w.aerPortOf, w.aerPortKey, c, g, devs, &NvidiaGpuDevice::addr);
         if (!xpuClasses[s.klass].resourceNames.empty()) {
             const kxpu_devrec &r = w.recs[c.gmem[c.goff[g]]];
             s.firstDevice = trimID(std::string((const char *)r.device_txt, std::min<size_t>(r.device_len, sizeof r.device_txt)));
@@ -1645,6 +1687,17 @@ Error Plugin::classify(MdevWalk &w) {
                                   w.rootPort.data(), w.pcieSwitch.data());
         if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_pcie_ports_mdev", rc);
     }
+    if (aerPortHealth) {  // the ports above every mdev's parent, from the links read above
+        w.aerPortOff.assign(n + 1, 0);
+        w.aerPortOf.assign((size_t)KXPU_PCIE_MAX_DEPTH * n + 1, 0);
+        w.aerPortKey.assign((size_t)KXPU_PCIE_MAX_DEPTH * n + 1, 0);
+        uint32_t nk = 0;
+        rc = kxpu_aer_ports_mdev(ctx_, recs.data(), w.paths.data(), n, w.aerPortOff.data(), w.aerPortOf.data(),
+                                 w.aerPortKey.data(), &nk);
+        if (rc != KXPU_OK) return kxfail(ctx_, "kxpu_aer_ports_mdev", rc);
+        w.aerPortOf.resize(w.aerPortOff[n]);
+        w.aerPortKey.resize(nk);
+    }
     return Error();
 }
 
@@ -1674,6 +1727,7 @@ void Plugin::buildMaps(const MdevWalk &w, const std::vector<uint64_t> *index) {
             const kxpu_devrec &pf = pciRecs_[w.pfOf[c.gmem[c.goff[g]]]];
             s.pf.assign(pf.bdf, strnlen(pf.bdf, sizeof pf.bdf));
         }
+        if (aerPortHealth) s.aerPorts = groupPorts(w.aerPortOff, w.aerPortOf, w.aerPortKey, c, g, devs, &MdevDevice::parent);
         if (vgpuClasses[s.klass].mdevCdev)  // an mdev without a cdev: VFIO cannot open it
             for (const MdevDevice &m : devs)
                 if (m.cdev < 0) { s.blocker = m.uuid + " has no VFIO cdev"; s.blockerKind = KXPU_MR_VFIO_CDEV_MISSING; break; }
@@ -2336,6 +2390,7 @@ Error Plugin::InitiateDevicePlugin() {
     if (!e) e = checkResetMethods();
     if (!e && vgpuSriovAware && vgpuClasses.empty()) e = fail("vgpuSriovAware is set but no vGPU class is configured");
     if (!e && sriovPfAware && !sriovAware) e = fail("sriovPfAware is set but sriovAware is off");
+    if (!e && aerPortHealth && !aerHealth) e = fail("aerPortHealth is set but aerHealth is off");
     if (!e) e = checkDraPcieDomain();
     if (!e) e = checkDraVgpuPcie();
     if (e) return e;
@@ -2996,6 +3051,12 @@ Error Plugin::computeAer() {
     std::vector<uint32_t> len, goff{0}, members;
     std::vector<std::string> who;  // the function whose files record i read
     std::map<std::string, uint32_t> pfRecord;  // PF address -> its record
+    // aerPortHealth: after a group's members and PF, the ports above its members, one record per port address shared by
+    // every group of both walks.  label[m]: how a reason names member m; own[g]: the end of group g's own functions and
+    // PF, the files aerMax reports
+    std::map<std::string, uint32_t> portRecord;
+    std::vector<std::string> label;
+    std::vector<uint32_t> own;
     auto read = [&](const std::string &base, const std::string &entry, const std::string &fn) {  // the new record's index
         for (const char *name : {"aer_dev_fatal", "aer_dev_nonfatal"}) {
             std::string s;
@@ -3009,6 +3070,16 @@ Error Plugin::computeAer() {
         who.push_back(fn);
         return (uint32_t)(who.size() - 1);
     };
+    auto addPorts = [&](const std::vector<std::pair<std::string, std::string>> &ports) {  // empty without aerPortHealth
+        label.resize(members.size());
+        own.push_back((uint32_t)members.size());
+        for (const auto &pa : ports) {
+            auto it = portRecord.find(pa.first);
+            if (it == portRecord.end()) it = portRecord.emplace(pa.first, read(basePath, pa.first, pa.first)).first;
+            members.push_back(it->second);
+            label.push_back(pa.first + " (PCIe port above " + pa.second + ")");
+        }
+    };
     for (size_t g = 0; g < iommuMap.size(); g++) {
         for (const NvidiaGpuDevice &d : iommuMap[g].second) members.push_back(read(basePath, d.addr, d.addr));
         const std::string &pf = iommuState[g].pf;  // set only under vfVgpuHealth or sriovPfAware
@@ -3017,6 +3088,7 @@ Error Plugin::computeAer() {
             if (it == pfRecord.end()) it = pfRecord.emplace(pf, read(basePath, pf, pf)).first;
             members.push_back(it->second);
         }
+        addPorts(iommuState[g].aerPorts);
         goff.push_back((uint32_t)members.size());
     }
     for (size_t g = 0; g < mdevMap.size(); g++) {
@@ -3027,6 +3099,7 @@ Error Plugin::computeAer() {
             if (it == pfRecord.end()) it = pfRecord.emplace(pf, read(basePath, pf, pf)).first;
             members.push_back(it->second);
         }
+        addPorts(mdevState[g].aerPorts);
         goff.push_back((uint32_t)members.size());
     }
     const size_t n = who.size(), G = goff.size() - 1;
@@ -3042,12 +3115,12 @@ Error Plugin::computeAer() {
             for (uint32_t m = goff[g]; m < goff[g + 1] && why.empty(); m++) {
                 const uint64_t c = totals[2 * members[m] + k], limit = k ? aerNonFatalLimit : aerFatalLimit;
                 if (c != UINT64_MAX && c > limit)
-                    why = who[members[m]] + " reported " + std::to_string(c) + (k ? " non-fatal" : " fatal") +
+                    why = (label[m].empty() ? who[members[m]] : label[m]) + " reported " + std::to_string(c) + (k ? " non-fatal" : " fatal") +
                           " uncorrectable PCIe errors (limit " + std::to_string(limit) + ")";
             }
         uint64_t most[2] = {KXPU_METRICS_NO_VALUE, KXPU_METRICS_NO_VALUE};  // the highest known count of each severity
         for (int k = 0; k < 2; k++)
-            for (uint32_t m = goff[g]; m < goff[g + 1]; m++) {
+            for (uint32_t m = goff[g]; m < own[g]; m++) {  // the group's own functions and PF: not its ports
                 const uint64_t c = totals[2 * members[m] + k];
                 if (c != UINT64_MAX && (most[k] == KXPU_METRICS_NO_VALUE || c > most[k])) most[k] = c;
             }
@@ -4702,6 +4775,7 @@ int kxh_devs_aer(void *h, int plugin_index, char *out, size_t cap) {
 void kxh_set_vf_vgpu_health(void *h, int on) { ((Plugin *)h)->vfVgpuHealth = on != 0; }
 void kxh_set_vgpu_sriov(void *h, int on) { ((Plugin *)h)->vgpuSriovAware = on != 0; }
 void kxh_set_sriov_pf(void *h, int on) { ((Plugin *)h)->sriovPfAware = on != 0; }
+void kxh_set_aer_port_health(void *h, int on) { ((Plugin *)h)->aerPortHealth = on != 0; }
 void kxh_set_dra_pcie_domain(void *h, const char *domain) { ((Plugin *)h)->draPcieDomain = domain ? domain : ""; }
 void kxh_set_dra_vgpu_pcie(void *h, int on) { ((Plugin *)h)->draVgpuPcie = on != 0; }
 uint64_t kxh_mdev_physfn_reads(void *h) { return ((Plugin *)h)->mdevPhysfnReads; }

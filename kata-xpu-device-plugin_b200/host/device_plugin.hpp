@@ -287,6 +287,10 @@ struct PciWalk {
     std::vector<uint32_t> pfOf, numvfs, gsriov;
     // draPcieDomain: per group ordinal its root port and switch (kxpu_pcie_ports), or KXPU_PCIE_NO_KEY
     std::vector<uint64_t> rootPort, pcieSwitch;
+    // aerPortHealth: kxpu_aer_ports' CSR, the ports above every record (aerPortOf[aerPortOff[i] .. aerPortOff[i+1]),
+    // nearest first), and each port's function key
+    std::vector<uint32_t> aerPortOff, aerPortOf;
+    std::vector<uint64_t> aerPortKey;
     // resetCheck: per record its reset_method (or reset) read, and kxpu_reset_check's methods and set verdict; per group
     // ordinal the reset blocker or KXPU_VIABLE
     std::vector<kxpu_resetrec> rrs;
@@ -321,6 +325,9 @@ struct MdevWalk {
     // draVgpuPcie (with a vGPU class that has a draDriver): per group ordinal its root port and switch
     // (kxpu_pcie_ports_mdev), or KXPU_PCIE_NO_KEY
     std::vector<uint64_t> rootPort, pcieSwitch;
+    // aerPortHealth: kxpu_aer_ports_mdev's CSR and keys, the ports above every mdev's parent, as in PciWalk
+    std::vector<uint32_t> aerPortOff, aerPortOf;
+    std::vector<uint64_t> aerPortKey;
     // mdevCdevEnabled only, one per record: N of its VFIO cdev, -1 = none or not read
     std::vector<int64_t> cdevs;
     // vgpuSriovAware only, one per record: its physfn read (kxpu_sriovrec, physfn only) and kxpu_mdev_pf's answer, the
@@ -351,6 +358,9 @@ struct GroupState {
     // aerHealth: the highest known TOTAL_ERR_FATAL / _NONFATAL over the files computeAer folded for the group (members, an
     // mdev's parent, a VF's PF); KXPU_METRICS_NO_VALUE = none known.  Reported by MetricsText only
     uint64_t aerMax[2] = {KXPU_METRICS_NO_VALUE, KXPU_METRICS_NO_VALUE};
+    // aerPortHealth: the PCIe ports above the group's members (kxpu_aer_ports[_mdev]), member by member, each nearest
+    // first and each port once: (port address, the function it was found above: a member, or an mdev's parent)
+    std::vector<std::pair<std::string, std::string>> aerPorts{};
     std::optional<Dra> dra{};  // draEnabled (vgpuDraEnabled): the ResourceSlice record of its first member; none = unpublished
     // vfVgpuDraEnabled, a group of a class with a vgpuDraDriver whose first member is a VF that carries a named vGPU type:
     // its VF-vGPU ResourceSlice record; none = unpublished
@@ -443,9 +453,9 @@ class Plugin {
     std::string nodeName;
     bool draEnabled() const;  // some class has a draDriver
     // the PCI gathers read numa_node (topologyAware, draEnabled or vfVgpuDraEnabled) and the entry link
-    // (pcieTopologyAware, draEnabled, vfVgpuDraEnabled or resetCheck)
+    // (pcieTopologyAware, draEnabled, vfVgpuDraEnabled, resetCheck or aerPortHealth)
     bool readsNuma() const { return topologyAware || draEnabled() || vfVgpuDraEnabled(); }
-    bool readsPaths() const { return pcieTopologyAware || draEnabled() || vfVgpuDraEnabled() || resetCheck; }
+    bool readsPaths() const { return pcieTopologyAware || draEnabled() || vfVgpuDraEnabled() || resetCheck || aerPortHealth; }
     // DRA ResourceSlices of vGPUs on SR-IOV VFs (include/kxpu.h, kxpu_dra_slices_vf_vgpu): a vgpuDraDriver on a vfVgpu
     // class publishes its vGPUs (VfVgpuResourceSlices) in the pool nodeName.  With one set, the PCI gathers read
     // numa_node and the entry link as draEnabled does, and readVfVgpus keeps each VF's physfn basename; nothing else is
@@ -457,8 +467,9 @@ class Plugin {
     // read only leaves out its attribute.  The PCI walk and every device-plugin output stay as they are.
     bool vgpuDraEnabled() const;  // some vGPU class has a draDriver
     bool readsMdevNuma() const { return topologyAware || vgpuDraEnabled(); }
-    // the mdev walk reads each grouped entry's link (vgpuPcieTopologyAware or vgpuDraEnabled); one read serves both
-    bool readsMdevPaths() const { return vgpuPcieTopologyAware || vgpuDraEnabled(); }
+    // the mdev walk reads each grouped entry's link (vgpuPcieTopologyAware, vgpuDraEnabled or aerPortHealth); one read
+    // serves all
+    bool readsMdevPaths() const { return vgpuPcieTopologyAware || vgpuDraEnabled() || aerPortHealth; }
     // DRA device taints (ABI v11).  false (default): the slices never carry taints and every output and generation is as
     // above, even while a device is Unhealthy.  true: ResourceSlices, VfVgpuResourceSlices and VgpuResourceSlices pass taint times to the
     // slice call (64 devices per slice); a group that refreshDraHealth found unhealthy carries the taint
@@ -480,6 +491,21 @@ class Plugin {
     uint64_t aerFatalLimit = 0, aerNonFatalLimit = 0;
     // <base>/<entry>/<name>, at most KXPU_AER_FILE_MAX + 1 bytes; false or an empty out: a failed read (unknown count)
     std::function<bool(const std::string &base, const std::string &entry, const std::string &name, std::string &out)> readAerFile;
+    // AER errors of the PCIe ports above a device (include/kxpu.h, kxpu_aer_ports and kxpu_aer_ports_mdev).  A Surprise
+    // Down is logged by the downstream port above the device that dropped off the link, a completion timeout of a CPU read
+    // by the root port, an error on a root port - switch link by the root port or the switch upstream port: none of them
+    // in the device's own files [assumed, not observed here].  InitiateDevicePlugin refuses it while aerHealth is off.
+    // false (default): no new link or file is read and every output, generation and counter is as above.  true:
+    //   - the PCI walk reads every entry's link (as pcieTopologyAware does) and the mdev walk every grouped mdev's link
+    //     (as readsMdevPaths), one read serving every setting that wants it, and each walk makes one kxpu_aer_ports /
+    //     kxpu_aer_ports_mdev call after the gather, at start-up and on each rediscover (GroupState::aerPorts);
+    //   - computeAer folds, after a group's members and PF, the aer_dev_* files of the ports above each member
+    //     (<basePath>/<port>/aer_dev_fatal|nonfatal through readAerFile, counted in aerReads), one read per distinct port
+    //     per call, with the same limits; the reason reads "<port> (PCIe port above <bdf>) reported <n> fatal ...";
+    //   - a root port's count flags every group below it: errors are not traced further down.  The metrics' AER counts
+    //     stay the group's own functions' and PF's; Unhealthy, the pcie-aer taint and the reason sample follow as for any
+    //     AER flag, and refreshAerHealth re-reads the ports without a walk.
+    bool aerPortHealth = false;
     // Restart resume of CDI indices (include/kxpu.h, ABI v13).  false (default): nothing more is read or written and every
     // index is the walk order of the first walk.  true: InitiateDevicePlugin reads back the CDI specs a previous process
     // wrote (<cdiConfigPath><cdiFileStem>.yaml of every class, kxpu_cdi_parse / kxpu_cdi_parse_mdev) and the index state

@@ -694,6 +694,41 @@ def pcie_ports_mdev_walk(n=1 << 20, vf_every=4, seed=23):
     return recs, paths, off, mem
 
 
+def aer_port_walk(n=1 << 20, depth=2, fanout=8, seed=53, mixed=False):
+    """kxpu_aer_ports' input: n functions (DEVREC_DTYPE) below complete switch trees.  Each root port has a PCI domain of
+    its own (pci<dom>:00, then <dom>:00:01.0) and `depth` switch levels below it (0..3: a chain of at most 8 keys), each
+    switch an upstream port and `fanout` downstream ports (1..32), one function per downstream port of the last level,
+    so fanout**depth functions share a root port.  mixed: record i's chain stops after 1 + i % (2 * depth + 2) keys (a
+    function below the host bridge, the root port, a switch upstream or downstream port), at the same key counts for
+    every seed.  seed: the order of the records (a permutation of the leaves).  Returns (recs, paths)."""
+    from .binding import DEVREC_DTYPE, PCIPATH_DTYPE
+    assert 0 <= depth <= 3 and 1 <= fanout <= 32
+    rng = np.random.default_rng(seed)
+    leaves = fanout ** depth
+    first_bus = [1 + 2 * sum(fanout ** m for m in range(k)) for k in range(depth + 1)]  # level k's upstream buses
+    recs = np.zeros(n, DEVREC_DTYPE)
+    paths = np.zeros(n, PCIPATH_DTYPE)
+    bdfs, texts = [], []
+    for slot, i in enumerate(rng.permutation(n).tolist()):
+        dom, leaf = i // leaves, i % leaves
+        comps = ["pci%04x:00" % dom, "%04x:00:01.0" % dom]
+        j = 0  # the switch's index within its level
+        for k in range(depth):
+            d = leaf // fanout ** (depth - 1 - k) % fanout
+            up = first_bus[k] + 2 * j
+            comps += ["%04x:%02x:00.0" % (dom, up), "%04x:%02x:%02x.0" % (dom, up + 1, d)]
+            j = j * fanout + d
+        if mixed:
+            comps = comps[:1 + slot % (2 * depth + 2)]
+        bdf = "%04x:%02x:00.0" % (dom, 0x80 + leaf % 0x80)
+        bdfs.append(bdf.encode())
+        texts.append(("/".join(comps) + "/" + bdf).encode())
+    recs["bdf"] = bdfs
+    paths["path"] = texts
+    paths["len"] = [len(t) for t in texts]
+    return recs, paths
+
+
 def dra_mdev_pcie_devices(n=1 << 16, vf_every=8, seed=43):
     """kxpu_dra_slices_mdev_pcie's input: dra_mdev_devices(n), one in vf_every on a VF with its PF's address and device
     id, a root port on every device and a switch on three in four: 4-digit domains, 12-byte addresses"""

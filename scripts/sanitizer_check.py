@@ -96,6 +96,12 @@ print("pcie_ports switches", int((pst != B.PCIE_NO_KEY).sum()), "dra_pcie slice 
       len(kx.dra_slices_pcie("d", "p", "n", 1, "pcie.example.com", pcdevs, [], None)[0]),
       len(kx.dra_slices_pcie("d", "p", "n", 1, "pcie.example.com", pcdevs, [("d/k", "", "NoSchedule")],
                              np.full((300, 1), 5, np.int64))[0]))
+# the PCIe ports above every record (AER health): a PCI walk of switch trees with every chain end, then an mdev walk
+apr, app = W.aer_port_walk(3000, depth=3, fanout=4, mixed=True)
+apo, apf, apk = kx.aer_ports(apr, app)
+amr, amp, _, _ = W.pcie_ports_mdev_walk(3000)
+amo, amf, amk = kx.aer_ports(amr, amp)
+print("aer_ports positions", int(apo[-1]), "ports", len(apk), "aer_ports_mdev positions", int(amo[-1]), "ports", len(amk))
 # PCIe root ports and switches of vGPUs: the ports of an mdev walk, then both vGPU layouts untainted and with one taint
 vmr, vmp, vmo, vmm = W.pcie_ports_mdev_walk(3000)
 vrt, vst = kx.pcie_ports_mdev(vmr, vmp, vmo, vmm)
